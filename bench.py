@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py -- ResNet-50-DWT training-step throughput on B200 (BASELINE.json metric).
+"""bench.py -- ResNet-50-DWT training-step throughput on H100 (BASELINE.json metric).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
                     [--workload resnet|microbench] [--per-domain B] [--site-mode fused|modules]
+                    [--dump-outputs DIR]
 
 One "step" = one full training step of the ResNet-50-DWT harness model (harness/resnet50_dwt.py,
 the reference topology with this repo's CUDA layers dropped in) on one synthetic Office-Home-shaped
@@ -19,14 +20,16 @@ layers (oracle/torch_port.py, same harness model) timed on this box's host cores
 
 At N = 1 the line also carries
   `microbench`        BASELINE.json configs[1] (WTransform2d N=256 C=256 56x56 group_size=64, fwd+bwd: the TMA +
-                      tcgen05 kernels) with its own roofline, per-kernel table, CPU baseline and reference-on-GPU time;
+                      wgmma kernels) with its own roofline, per-kernel table, CPU baseline and reference-on-GPU time;
   `reference_on_gpu`  the reference's operator sequence (oracle/torch_port.py: stock ATen / cuBLAS / cuSOLVER / cuDNN
-                      ops, eager, torch's default math modes) on the SAME B200 for configs[2] -- what a user of the
+                      ops, eager, torch's default math modes) on the SAME GPU for configs[2] -- what a user of the
                       reference gets on this GPU today -- and the speed-up over it.
 
 --impl reference: the reference's own CPU path (no GPU): the same step with the reference's
 operator sequence on stock ATen CPU ops (oracle/torch_port.py), all host threads, a bounded sample.
 --workload microbench: only BASELINE.json configs[1] (WTransform2d N=256 C=256 56x56 gs=64 fwd+bwd).
+
+--dump-outputs DIR: write the last timed step's outputs as DIR/<name>.npy (float32; large ones as a fixed sample).
 """
 from __future__ import annotations
 
@@ -72,12 +75,12 @@ def measured_peaks():
             return float(d["hbm_gbs"]), "MEASURED_PEAKS.json"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (H100 SXM data sheet)"
 
 
 # ----------------------------------------------------------------------------------------- clocks
 class ClockSampler:
-    """nvidia-smi sampled every 200 ms during the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi sampled every 200 ms during the timed region: SM clock, power and throttle reasons."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -154,7 +157,7 @@ class FlatGradAllReduce:
     (94.6 MB for ResNet-50-DWT), averaged over the ranks by NCCL over NVLink (gloo in the CPU test).  Whitening / BN
     statistics are never exchanged: every rank normalises its own minibatch.
 
-    gather="copy" (the default of bench.py, measured on 2 B200s: 31.48 vs 31.75 ms per step): autograd produces its own
+    gather="copy" (the default of bench.py): autograd produces its own
     gradient tensors, ONE multi-tensor copy moves them into the flat buffer after backward, ONE all-reduce averages it, and
     .grad is re-pointed at the views for the optimizer -- instead of 161 small in-place accumulation kernels and a 94.6 MB
     memset per step.  gather="accumulate": .grad are the views themselves; then the buffer can also be cut into
@@ -166,9 +169,8 @@ class FlatGradAllReduce:
     layers are still back-propagating and only the small stem / layer1 / layer2 piece (6 MB) is exposed at the end.
     The collectives are issued asynchronously on NCCL's own stream (async_op) and joined in reduce(); no Python runs
     at replay time -- the whole step, collectives and cross-stream edges included, is captured into the CUDA graph.
-    Measured on 2 B200s the overlap buys nothing there (32.79 ms with 3 segments vs 32.71 ms with one collective: a
-    60 MB all-reduce between two GPUs takes ~0.2 ms and its kernel competes with backward for SMs and HBM); it stays
-    available (--grad-gather accumulate --grad-segments 3) for larger rank counts."""
+    Between two GPUs the overlap need not pay (the all-reduce kernel competes with backward for SMs and HBM); it
+    stays available (--grad-gather accumulate --grad-segments 3) for larger rank counts."""
 
     def __init__(self, model, world, segments=3, gather="accumulate"):
         import torch.distributed as dist
@@ -269,7 +271,7 @@ class FlatGradAllReduce:
 
 
 def train_step(model, mec, opt, images, labels, sync=None, head=None):
-    """head: dwt_b200.HeadLoss -- the same NLL + lambda*MEC as one fused launch (GPU arm)."""
+    """head: dwt_b200.HeadLoss -- the same NLL + lambda*MEC as one fused launch (GPU arm).  Returns (loss, logits)."""
     if sync is None:
         opt.zero_grad(set_to_none=True)
     else:
@@ -284,7 +286,7 @@ def train_step(model, mec, opt, images, labels, sync=None, head=None):
     if sync is not None:
         sync.reduce()
     opt.step()
-    return loss
+    return loss, logits
 
 
 # ----------------------------------------------------------------------------------------- arms
@@ -372,7 +374,7 @@ def workload_config(args, per_domain):
     return {"workload": "ResNet-50-DWT synthetic Office-Home 224x224, train step = fwd + NLL + 0.1*MEC + bwd + SGD",
             "per_domain_batch": per_domain, "images_per_gpu": 3 * per_domain, "global_images": 3 * per_domain * args.gpus,
             "group_size": 4, "parallelism": f"dp{args.gpus}",
-            "l2": "no explicit flush: per-step working set (activations) is tens of GB >> 126 MB L2"}
+            "l2": "no explicit flush: per-step working set (activations) is tens of GB >> 50 MB L2"}
 
 
 def implementation_note(args):
@@ -412,7 +414,7 @@ def reference_on_gpu_resnet(args, device):
     """configs[2] with the reference's operator sequence on this GPU (oracle/torch_port.py: x.mean / bmm /
     linalg.cholesky / inverse / grouped conv2d / F.batch_norm / split-cat-affine-relu composition, autograd backward),
     eager, NCHW, torch's default math modes (fp32 matmul, cuDNN TF32 convolutions -- the same convolutions as our
-    arm).  /root/reference itself cannot travel to the GPU box; the port restates utils/whitening.py:37-61,
+    arm).  The port restates the reference project's utils/whitening.py:37-61,
     utils/batch_norm.py:54-69, utils/consensus_loss.py:11-24 op for op (tests/test_oracle_vs_golden.py pins it)."""
     import oracle.torch_port as port
     from harness.synth import synth_batch
@@ -426,9 +428,9 @@ def reference_on_gpu_resnet(args, device):
     def step():
         train_step(model, mec, opt, images, labels)
 
-    for _ in range(3):
+    for _ in range(args.warmup):
         step()
-    k = max(3, min(args.steps, 10))
+    k = args.steps
     ms = timed_loop(step, k, device, False)
     del model, opt
     return {"value": 3 * B * k / (ms / 1e3), "unit": "images/s", "ms_per_step": ms / k, "steps": k,
@@ -449,9 +451,9 @@ def reference_on_gpu_micro(args, device):
     def step():
         torch.autograd.grad(m(x), x, dy)
 
-    for _ in range(3):
+    for _ in range(args.warmup):
         step()
-    k = max(3, min(args.steps, 10))
+    k = args.steps
     ms = timed_loop(step, k, device, False)
     return {"value": k / (ms / 1e3), "unit": "iterations/s", "ms_per_step": ms / k, "steps": k,
             "impl": "oracle/torch_port.py WTransform2d on cuda (mean, transposing copy, bmm, linalg.cholesky, inverse, "
@@ -512,7 +514,10 @@ def run_ours(args):
             os.dup2(saved, 1)
             os.close(saved)
     assert world == args.gpus, f"--gpus {args.gpus} but WORLD_SIZE={world}"
-    torch.backends.cudnn.benchmark = True
+    # --dump-outputs: the timed path computes the same outputs from the same arguments on every run, so cuDNN's heuristics
+    # (not timing runs, whose winner varies from run to run) choose the convolution algorithms, among deterministic ones
+    torch.backends.cudnn.benchmark = not args.dump_outputs
+    torch.backends.cudnn.deterministic = bool(args.dump_outputs)
     _native.lib()                                           # fail loudly if the extension is missing
 
     if args.workload == "microbench":
@@ -552,7 +557,7 @@ def run_ours(args):
     def step_e2e():
         im = host_images.to(device, non_blocking=True)
         lb = host_labels.to(device, non_blocking=True)
-        loss = train_step(net, mec, opt, im, lb, sync, head)
+        loss, _ = train_step(net, mec, opt, im, lb, sync, head)
         loss_host.copy_(loss.detach(), non_blocking=True)
         torch.cuda.current_stream(device).synchronize()     # the user reads the loss every step
 
@@ -569,7 +574,7 @@ def run_ours(args):
 
     # Pass 2: the same step captured once into a CUDA graph and replayed (the step is ~1400 launches, the
     # host launch path is as long as the GPU work).  This is the reported `value`; identical kernels and work.
-    graph, static_loss = None, None
+    graph, static_loss, static_logits = None, None, None
     if args.cuda_graph:
         try:
             side = torch.cuda.Stream(device)
@@ -581,7 +586,7 @@ def run_ours(args):
             torch.cuda.synchronize(device)
             graph = torch.cuda.CUDAGraph()
             with torch.cuda.graph(graph):
-                static_loss = train_step(net, mec, opt, images, labels, sync, head)
+                static_loss, static_logits = train_step(net, mec, opt, images, labels, sync, head)
             torch.cuda.synchronize(device)
         except Exception as e:                      # capture is an optimisation, never a requirement
             graph = None
@@ -613,11 +618,19 @@ def run_ours(args):
             loss_host.copy_(static_loss.detach(), non_blocking=True)
             cur.synchronize()                                # the user reads the loss every step
     else:
-        step_timed = step_resident
+        last = {}                                            # (loss, logits) of the latest timed step
+
+        def step_timed():
+            last["out"] = train_step(net, mec, opt, images, labels, sync, head)
     for _ in range(2):
         step_timed()
     with ClockSampler(local) as clocks:
         ms = timed_loop(step_timed, args.steps, device, distributed)
+    if args.dump_outputs and rank == 0:                     # before the e2e passes move the weights on
+        loss_t, logits_t = (static_loss, static_logits) if graph is not None else last["out"]
+        dump_outputs(args.dump_outputs, {"loss": loss_t, "logits": logits_t,
+                                         "params_sample": flat_sample([p.detach() for p in model.parameters()]),
+                                         "grads_sample": flat_sample([p.grad for p in model.parameters()])})
     for _ in range(2):
         step_e2e()
     ms_e2e = timed_loop(step_e2e, args.steps, device, distributed)
@@ -730,14 +743,15 @@ def run_ours(args):
         "gpu_launches": int(launches), "clocks": clocks.summary(), "roofline": roof, "kernels": fams,
         "e2e_uint8_input": e2e_u8,
         "cuda_graph": graph is not None, "eager_ms_per_step": ms_eager / args.steps,
-        "conv_math": "cuDNN, TF32 allowed (torch default) -- convolutions are not part of the hot path",
+        "conv_math": "cuDNN, TF32 allowed (torch default), " + ("deterministic algorithms chosen by heuristics" if args.dump_outputs else
+                                                          "algorithms chosen by timing (cudnn.benchmark)") + " -- not part of the hot path",
     }
     if args.cpu_baseline:
         out["cpu_baseline"] = cpu_baseline(args)
     out["status_word"] = _native.status_all(device)            # 0: no kernel reported a failure during the run
     if not distributed and args.extras:
         # free the step's graph, model and activations before the two side measurements
-        del graph, static_loss, model, net, opt
+        del graph, static_loss, static_logits, step_timed, model, net, opt
         import gc
         gc.collect()
         torch.cuda.empty_cache()
@@ -775,12 +789,14 @@ def run_microbench(args, device):
     x = (torch.einsum("dc,nchw->ndhw", mix, torch.randn(N, C, H, H, device=device)) + 2.0).contiguous().requires_grad_(True)
     dy = torch.randn(N, C, H, H, device=device)
     m = dwt_b200.WTransform2d(C, gs).to(device).train()
-    steps = max(args.steps, 20)                      # SURVEY §8d: >= 20 iterations after >= 5 warm-ups
-    warm = max(args.warmup, 5)
+    steps, warm = args.steps, args.warmup
+    out = {}                                         # y and dx of the last timed step (the graph's static outputs)
 
-    def step():
+    def step(keep=None):
         y = m(x)
-        torch.autograd.grad(y, x, dy)
+        (dx,) = torch.autograd.grad(y, x, dy)
+        if keep is not None:
+            keep["y"], keep["dx"] = y, dx
 
     for _ in range(warm):
         step()
@@ -793,13 +809,15 @@ def run_microbench(args, device):
         torch.cuda.current_stream(device).wait_stream(side)
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph):
-            step()
+            step(out)
         graph.replay()
     with ClockSampler(device.index) as clocks:
         _native.profile_begin()
-        eager_ms = timed_loop(step, steps, device, False)
+        eager_ms = timed_loop(step if graph is not None else lambda: step(out), steps, device, False)
         prof = _native.by_family(_native.profile_end())
         ms = timed_loop(graph.replay, steps, device, False) if graph is not None else eager_ms
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"y_sample": flat_sample([out["y"].detach()]), "dx_sample": flat_sample([out["dx"]])})
     peak, peak_src = measured_peaks()
     elems = N * C * H * H
     total_bytes = 32.0 * elems                       # 12 B/elem forward + 20 B/elem backward (SURVEY §8d)
@@ -825,7 +843,7 @@ def run_microbench(args, device):
         "dtype": "f32 (tf32 tensor-core contraction with hi/lo split operands, split-tf32 apply, fp32 accumulate)" if tc else "f32",
         "data": "synthetic",
         "config": {"workload": f"WTransform2d N={N} C={C} H=W={H} group_size={gs} fwd+bwd",
-                   "l2": f"tensor of {elems * 4 / 1e6:.0f} MB > 126 MB L2",
+                   "l2": f"tensor of {elems * 4 / 1e6:.0f} MB > 50 MB L2",
                    "launch": "cuda-graph replay" if graph is not None else "eager"},
         "roofline": {"bound": "hbm", "kernel": "fwd+bwd (all launches of the layer)", "achieved": gbs, "peak": peak, "unit": "GB/s",
                      "frac": gbs / peak, "traffic": ratio * total_bytes if ratio else None, "traffic_source": ratio_src,
@@ -835,10 +853,32 @@ def run_microbench(args, device):
     }
 
 
+DUMP_SAMPLE = 1 << 21                            # elements per sampled output: 8 MB of float32, 4 of them at most
+
+
+def flat_sample(tensors, k=DUMP_SAMPLE):
+    """A fixed seeded sample of k elements of the concatenation of `tensors` (all of it when it is smaller)."""
+    flat = torch.cat([t.reshape(-1).float() for t in tensors])
+    if flat.numel() <= k:
+        return flat
+    g = torch.Generator(device="cpu").manual_seed(0)
+    idx = torch.randperm(flat.numel(), generator=g)[:k].sort().values
+    return flat[idx.to(flat.device)]
+
+
+def dump_outputs(path, arrays):
+    """arrays: name -> tensor; written as path/<name>.npy in float32."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(path, name + ".npy"), t.detach().float().cpu().numpy())
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=10)
+    ap.add_argument("--steps", type=int, default=10,
+                    help="timed steps of every GPU measurement (the CPU reference arm times a bounded sample: 2-5 steps)")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", choices=["ours", "reference"], default="ours")
     ap.add_argument("--workload", choices=["resnet", "microbench"], default="resnet")
@@ -869,6 +909,9 @@ def main():
                     help="pieces the flat gradient buffer is all-reduced in (1 = one collective after backward)")
     ap.add_argument("--micro-n", type=int, default=256)
     ap.add_argument("--micro-gs", type=int, default=64)
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="after the timed steps, write the last timed step's outputs to DIR/<name>.npy; cuDNN then uses "
+                         "deterministic algorithms, so that runs with the same arguments write the same outputs")
     args = ap.parse_args()
     if args.warmup < 3 and args.impl == "ours":
         args.warmup = 3

@@ -1,4 +1,4 @@
-"""dwt_b200 -- B200-native Domain-Whitening-Transform layers and Min-Entropy-Consensus loss.
+"""dwt_b200 -- H100-native Domain-Whitening-Transform layers and Min-Entropy-Consensus loss.
 
 Put this package's parent directory (``dwt-domain-adaptation_b200/``) on ``sys.path`` ahead of
 the reference's ``utils/`` and the reference scripts' ``import whitening`` / ``import batch_norm``

@@ -1,10 +1,9 @@
-"""Build libdwt_b200.so in-tree with nvcc for sm_100a (no torch headers, no libtorch).
+"""Build libdwt_b200.so in-tree with nvcc for sm_90a (no torch headers, no libtorch).
 
     python dwt-domain-adaptation_b200/dwt_b200/build.py [--force] [--verbose]
 
 The library is a plain C-ABI shared object (include/dwt_b200.h) with a statically linked
-CUDA runtime; it cross-compiles on a box without a GPU.  The built file is git-ignored
-but travels to the GPU box with the gpurun snapshot.
+CUDA runtime; it cross-compiles on a machine without a GPU.  The built file is git-ignored.
 """
 from __future__ import annotations
 
@@ -17,7 +16,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "lib", "libdwt_b200.so")
 SOURCES = ["api.cu", "norm_small.cu", "norm_tiled.cu", "norm_tc.cu", "norm_tc_apply.cu", "norm_dense.cu", "norm_cl.cu", "mec.cu", "augment.cu", "pool.cu"]
-NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC,-fvisibility=hidden", "--expt-relaxed-constexpr"]
 NVCC_FLAGS += shlex.split(os.environ.get("DWT_NVCC_EXTRA", ""))     # development only, e.g. -DDWT_PROF_DENSE (phase clocks)
 
@@ -59,7 +58,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
             sys.stdout.write(out)
         if p.returncode:
             raise RuntimeError(f"nvcc failed on {src}")
-    link = [_nvcc(), "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-Xcompiler", "-fPIC", *objs, "-o", LIB]
+    link = [_nvcc(), "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler", "-fPIC", *objs, "-o", LIB]
     subprocess.check_call(link)
     return LIB
 

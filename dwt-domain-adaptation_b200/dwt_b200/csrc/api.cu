@@ -40,7 +40,7 @@ int sm_count() {
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess ||
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-      n = 148;   // B200
+      n = 132;   // H100 SXM
   }
   return n;
 }
@@ -123,7 +123,7 @@ int env_int(const char* name, int dflt) {
 // channels-last launch shaping.  Every kernel is ONE wave of persistent CTAs sweeping 32-row chunks (norm_cl.cu):
 // grid.x CTAs per (domain, column slab), grid.y slabs, grid.z = D domains side by side.  (grid.z = 1 -- all CTAs
 // sweeping the domains one after the other, so that the whole grid moves through the tensor as a single window --
-// was measured on the B200 step and is slower: 31.8 vs 31.5 ms, three times the partial rows for no extra L2 hits;
+// writes three times the partial rows for no extra L2 hits;
 // the kernels still accept it, DWT_CL_SEQ_MB=<tensor MB threshold> turns it on for experiments.)
 struct ClPlan { int nred, new_, S, gridy, gz_red, gz_ew; };
 ClPlan cl_plan(const dwt::Geom& g, int slots_red, int slots_ew, int unroll_red, int unroll_ew) {
@@ -384,7 +384,7 @@ int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, 
     Launch l(p.small ? "small_apply" : (tc ? "tc_apply" : "tiled_apply"), &p.gm, ((epi & DWT_EPI_RESIDUAL) ? 3 : 2) * E, st);
     if (p.small) dwt::small_apply(x, y, p.gm_ew, p.vec, p.chunks_ew, epi, save_mean, save_w, gamma, beta, residual, st);
     else if (tc) {
-      if (int cr = dwt::tc_apply(x, y, p.gm, tc_apply_ctas(p.gm, 1, 128), save_mean, save_w, st))
+      if (int cr = dwt::tc_apply(x, y, p.gm, tc_apply_ctas(p.gm, 1, 64), save_mean, save_w, st))
         return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d)", cr);
     } else dwt::tiled_apply(x, y, p.gm_ew, p.vec, p.chunks_ew, save_mean, save_w, st);
   }
@@ -483,7 +483,7 @@ int whiten_like_bwd(const float* x, const float* dout, const float* dout2, float
     Launch l(p.small ? "small_bwd_apply" : (tc ? "tc_bwd_apply" : "tiled_bwd_apply"), &p.gm, 3 * E, st);
     if (p.small) dwt::small_bwd_apply(x, dout, dx, p.gm_ew, p.vec, p.chunks_ew, epi, w.coef, save_mean, save_w, gamma, beta, st);
     else if (tc) {
-      if (int cr = dwt::tc_bwd_apply(x, dout, dx, p.gm, tc_apply_ctas(p.gm, 1, 128), w.coef, save_mean, w.shift, st))
+      if (int cr = dwt::tc_bwd_apply(x, dout, dx, p.gm, tc_apply_ctas(p.gm, 1, 64), w.coef, save_mean, w.shift, st))
         return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d)", cr);
     } else dwt::tiled_bwd_apply(x, dout, dx, p.gm_ew, p.vec, p.chunks_ew, w.coef, st);
   }

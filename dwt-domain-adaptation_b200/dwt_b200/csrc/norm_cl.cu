@@ -1,8 +1,7 @@
 // Channels-last (NHWC) register-resident path for group sizes 1, 2, 4.
 //
 // cuDNN's tensor-core convolutions are NHWC kernels: fed NCHW fp32 tensors they bracket every
-// convolution with nchwToNhwc / nhwcToNchw copies (12.8 % of the ResNet-50-DWT step,
-// profiles/launches_r01a_summary.md).  Running the whole model channels-last removes those copies,
+// convolution with nchwToNhwc / nhwcToNchw copies.  Running the whole model channels-last removes those copies,
 // provided the normalisation layers in between read and write NHWC natively -- this file.
 //
 // Layout: x[(n*HW + p)*C + c].  One float4 = 4 consecutive channels of one pixel = one whitening
@@ -18,10 +17,9 @@
 //   cl_bwd_reduce -> cl_bwd_finalize -> cl_bwd_apply (backward, 20 B/element)
 //
 // Sweep order (round 2).  The tensor a pass reads was touched a moment ago: x was just WRITTEN front to back
-// by the producing convolution, and the second pass of a site re-reads what the first pass just read.  126 MB
-// of it are still in L2 -- but only if the kernel gets to them before its own misses evict them (inside the
-// bench step cl_stats ran at 0.81 of the HBM peak although the same launch alone under ncu reads at 0.99: the
-// difference is the write-back of the producer's dirty lines).  So every kernel is a persistent grid of CTAs
+// by the producing convolution, and the second pass of a site re-reads what the first pass just read.  The newest
+// tens of MB of it are still in L2 (50 MB on H100) -- but only if the kernel gets to them before its own misses evict
+// them.  So every kernel is a persistent grid of CTAs
 // that together sweep the tensor as ONE moving window of consecutive 32-row chunks (chunk c -> CTA c mod grid):
 // the two reductions sweep from the END of the tensor to its start (newest bytes first, domains D-1..0 one
 // after the other), the two elementwise passes from the START to the end (where the reduction just finished).
@@ -181,9 +179,7 @@ __device__ __forceinline__ int acc_index(int g, int a) {
 // column in ascending order (independent 8-byte loads, several rows in flight), five xor-shuffles add the lanes in a
 // fixed tree, and lane 0 does the dense algebra of the column's 4/gs groups in registers.  This replaced a many-CTA
 // `vec_reduce` launch plus a finalize launch in which one thread per (group, domain) walked the reduced rows itself --
-// a chain of ~30 dependent L2 round trips: 4.7 + 7.1 us per pair in the step's launch list, 5.5 + 20 us with cold
-// caches (profiles/launches_r02_step.md, ncu_r02_cl_site.md), 212 launches per step; an 8-lane version of that pair
-// measured 4.4 + 9.3 us cold.  The running-statistic EMA follows
+// a chain of ~30 dependent L2 round trips, 212 launches per step.  The running-statistic EMA follows
 // the aliasing class found on the host: all domains on ONE buffer pair (the shipped models) -> one closed-form
 // read-modify-write r' = k^D r + m sum_d k^(D-1-d) s_d; all distinct -> every domain's warp updates its own buffers;
 // mixed -> the d == 0 warp applies the domains in order.  No atomics, fixed summation order.

@@ -2,8 +2,8 @@
 // behind the tensor-core contraction:
 //
 //   partial_reduce   sum the per-CTA partial Gram matrices of a 64-channel super-block in fixed
-//                    chunk order, spread over many CTAs (the single "last CTA" doing this alone was
-//                    ~70 % of the contraction kernel's elapsed time -- profiles/ncu_r01c_tc.txt)
+//                    chunk order, spread over many CTAs (a single "last CTA" doing this alone would idle
+//                    the rest of the grid)
 //   fwd_factor       per group: mean, covariance, S = a*cov + b*I, Cholesky S = L L^T, W = L^-1,
 //                    running-statistic EMA (domains in order: one CTA owns all domains of its group)
 //   bwd_coef         per (domain, group): A1 = W^T, Bm = (2a/M) sym(W^T Phi(-R W^T) W), cvec
@@ -120,9 +120,8 @@ __device__ __forceinline__ void store_block(float* M, const Blk& t, const float 
 // hands L11 and 1/diag to the other 15 by shuffle; every thread solves its 4 x 4 block of the panel L21 = A21 L11^-T and
 // of the finished row block W_k = L11^-1 B_k and publishes both to shared memory (double-buffered).  After the barrier
 // every thread applies the rank-4 updates  A -= L21 L21^T  (blocks at or below the diagonal of the trailing matrix)
-// and  B -= L21 W_k  (rows below the panel, columns up to it).  16 steps of ~1000 cycles replace 64 single-column steps
-// (770 cycles each: sqrt, reciprocal, broadcast and barrier per column) plus a separate recursive-doubling inverse
-// through shared memory -- 78 k cycles of the 84 k of this kernel at gs = 64 (phase clocks, profiles/dense_r02.md).
+// and  B -= L21 W_k  (rows below the panel, columns up to it).  16 steps replace 64 single-column steps (sqrt,
+// reciprocal, broadcast and barrier per column) plus a separate recursive-doubling inverse through shared memory.
 // Returns false on a non-positive pivot.
 struct PanelSmem {
   float L[2][kSB][4];      // L[i][4k + p] of the current panel, 0 for rows i < 4k + 4

@@ -42,7 +42,7 @@ void tiled_bwd_prep(const Geom& gm, const BwdFin& fin, cudaStream_t st);
 void tiled_bwd_apply(const float* x, const float* dout, float* dx, const Geom& gm, int vec, int chunks,
                      const float* coef, cudaStream_t st);
 
-// TMA + tcgen05 contraction path, group sizes 8..64 tiling a 64-channel super-block  (norm_tc.cu)
+// TMA + wgmma contraction path, group sizes 8..64 tiling a 64-channel super-block  (norm_tc.cu)
 int tc_init();      // driver entry point for cuTensorMapEncodeTiled + shared-memory opt-in; 0 on success
 bool tc_supports(const Geom& gm, int vec);
 int tc_superblocks(const Geom& gm);
@@ -56,7 +56,7 @@ void dense_partial_reduce(const float* partial, int nchunks, int problems, float
 void dense_fwd_factor(const float* gram, const float* shift, const Geom& gm, const FwdFin& fin, cudaStream_t st);
 void dense_bwd_coef(const float* rgram, const Geom& gm, const BwdFin& fin, float* dybar, cudaStream_t st);
 
-// TMA + tcgen05 apply path (norm_tc_apply.cu): split-TF32 GEMM of the block-diagonal group matrices
+// TMA + wgmma apply path (norm_tc_apply.cu): split-TF32 GEMM of the block-diagonal group matrices
 int tc_apply_init();
 int tc_apply(const float* x, float* y, const Geom& gm, int nctas, const float* save_mean, const float* save_w,
              cudaStream_t st);

@@ -4,43 +4,33 @@
 //   stats       G = sum_m (x-K)(x-K)^T        per 64-channel super-block (gs x gs diagonal blocks kept)
 //   bwd_reduce  R = sum_m dy (x-mean)^T
 //
-// 2*gs flop per 4 bytes read puts these above the FP32-core ridge but far below the TF32
-// tensor ridge: on tcgen05 they are HBM-bound (SURVEY.md §8d).  Both kernels are persistent CTAs (two per
-// SM) over a contiguous range of [64 channels x 32 pixels] tiles, warp-specialised:
+// 2*gs flop per 4 bytes read puts these far below the TF32 tensor ridge: they are HBM-bound.  Both kernels are
+// persistent CTAs (two per SM) over a contiguous range of [64 channels x 32 pixels] tiles, warp-specialised:
 //
-//   warp 0      TMA producer: cp.async.bulk.tensor.3d (box 32 px x 64 ch x 1 image, SWIZZLE_128B)
-//               into a shared-memory ring, mbarrier complete_tx.
-//   warps 2-9   transform the landed tile for the tensor core (below).
-//   warp 1      MMA issuer (the Gram kernel has a second one, warp 10): one elected lane, warp-uniform operands,
-//               tcgen05.mma.cta_group::1.kind::tf32, fp32 accumulator in TMEM; tcgen05.commit releases the stage back
-//               to the producer.  Operands are K-major straight from the swizzled tile (NCHW rows ARE K-major: the
-//               reference's transposing copy, whitening.py:46, disappears).
-//   epilogue    tcgen05.ld the accumulator -> per-CTA partial -> global.  The fixed-order reduction of the
-//               partials and the dense algebra (Cholesky / inverse / EMA, or the backward coefficients) run
-//               as the small follow-up launches of norm_dense.cu.
+//   warp 8      TMA producer: cp.async.bulk.tensor.3d (box 32 px x 64 ch x 1 image, SWIZZLE_128B) into a
+//               shared-memory ring, mbarrier complete_tx.
+//   warps 0-7   two consumer warpgroups taking alternate tiles: each transforms its landed tile in place for the
+//               tensor core, then issues wgmma.mma_async kind::tf32 (M = 64 channels, K = 8 pixels per instruction)
+//               into an fp32 accumulator held in its registers, and releases the stage.  Operands are K-major straight
+//               from the swizzled tile (NCHW rows ARE K-major: the reference's transposing copy, whitening.py:46,
+//               disappears).
+//   epilogue    the two warpgroups' accumulators are summed in shared memory -> per-CTA partial -> global.  The
+//               fixed-order reduction of the partials and the dense algebra (Cholesky / inverse / EMA, or the backward
+//               coefficients) run as the small follow-up launches of norm_dense.cu.
 //
 // stats (tc_gram_kernel) -- SPLIT precision.  The covariance feeds a Cholesky factor whose error is the Gram
 // error times the condition number (the eps = 1e-3 shrinkage is absolute and stops helping once activations are
-// large), so a single tf32 pass is not enough (ADVICE r1: y errors of 1e-3..5e-3 at cond >= 1e4).  Each centred
-// sample s = x - K is split hi = trunc_tf32(s) (what the tensor core reads of an fp32 word anyway: no instruction) and
-// lo = s - hi (exact in fp32; the core keeps its top 11 bits), and
+// large), so a single tf32 pass is not enough (y errors of 1e-3..5e-3 at cond >= 1e4).  Each centred sample
+// s = x - K is split hi = trunc_tf32(s) and lo = s - hi (exact in fp32; the core keeps its top 11 bits), and
 //       G = HH + LH + LH^T         HH = sum hi hi^T,  LH = sum lo hi^T        (lo lo^T ~ 3e-7 G is dropped)
-// comes out of ONE M=128 N=80 K=8 MMA per 8 pixels: the A operand (128 rows = TMEM lanes; quarter q carries channels
-// 16q..16q+15, s in lanes 0..15 and lo in lanes 16..31) is written to TENSOR MEMORY by the transform warps (tcgen05.st; a
-// warp may only touch its own 32-lane quarter), the B operand is the tile of s written back in place plus 16 constant rows
-// (a row of ones: accumulator column 64 = the row sums the mean needs).  Tiles alternate between two transform sets, two
-// MMA-issuing warps and two accumulators.  Measured on B200 (tests/test_gpu_parity_r2.py): running-covariance error 8e-8
-// (single tf32 pass: 4e-6), y error at cond 1e3 / 1e4 3.6e-6 / 2.3e-5 (single pass 1.2e-4 / 2.9e-4, the fp32 reference
-// itself 3.1e-5 / 2.0e-4).  What bounds it (0.73 of the HBM peak): profiles/ncu_r02_tc_gram.md.
+// comes out of two M=64 N=64 K=8 MMAs per 8 pixels: A = the hi tile (written back in place) or the lo tile (a
+// per-warpgroup buffer), B = the hi tile.  The row sums the mean needs are summed by the transform.
 //
 // bwd_reduce (tc_contract_kernel) -- single pass: R multiplies already-formed W's in the coefficient algebra and
 // its tf32 product errors are zero-mean over M >= 4096 samples (round-to-nearest operands).
 //
-// Reference: utils/whitening.py:46-47 (/root/reference) and its autograd transpose.
+// Reference: utils/whitening.py:46-47 of the reference project and its autograd transpose.
 #include <cuda.h>
-#ifdef DWT_PROF_GRAM
-#include <cstdio>
-#endif
 
 #include "dwt_common.cuh"
 #include "norm_launch.h"
@@ -51,31 +41,23 @@ namespace {
 
 using namespace tc;
 
-constexpr int kTW = 8;                                  // transform warps (4 left the kernel transform-latency-bound: 0.74 of the HBM peak, 0.87 without the transform)
-constexpr int kTT = 32 * kTW;                           // transform threads
-constexpr int kPer = 512 / kTT;                         // 16-byte chunks of a tile per transform thread
-constexpr int kTcThreads = 64 + kTT;
+constexpr int kConsumers = 2;                           // consumer warpgroups per CTA (warps 0-7)
+constexpr int kProducerWarp = 4 * kConsumers;           // warp 8
+constexpr int kTcThreads = 128 * kConsumers + 32;
+constexpr int kPer = 512 / 128;                         // 16-byte chunks of a tile per consumer thread
 constexpr int kTilePx = 32, kTileCh = 64;
 constexpr int kTileBytes = kTileCh * kTilePx * 4;       // 8192
-constexpr int kStagesStats = 12, kStagesBwd = 6;      // 97 KB per CTA, two CTAs per SM: ~190 KB of loads in flight per SM
-constexpr int kTmemCols = 64;
-// split-precision Gram kernel: accumulator (80 columns, padded to 96) + a ring of A-operand slots (32 columns =
-// 32 pixels each); two CTAs per SM share the 512 columns of tensor memory
-// kGramAcc independent accumulators (tiles alternate between them): consecutive tcgen05.mma into ONE accumulator form a
-// dependent chain -- the round-1 single-pass kernel and the first split kernels, very different otherwise, both ran at
-// ~270 cycles per MMA per CTA -- and two chains overlap their latency.  80 columns each, then the A slots.
-constexpr int kGramAcc = 2, kGramASlots = 3, kGramTmemCols = 256;
+constexpr int kStagesBwd = 6;                           // x + dy per stage: 96 KB per CTA, two CTAs per SM
+constexpr int kNacc = kTileCh * kTileCh + kTileCh;      // per-CTA partial: 64x64 moments + 64 row sums
+constexpr int kGramStages = 10;                         // 80 KB ring + 2 x 8 KB lo tiles per CTA, two CTAs per SM
+constexpr int kMaxStages = kGramStages > kStagesBwd ? kGramStages : kStagesBwd;
+// Consumer warpgroup w takes tiles w, w + 2, ...; both ring lengths are even, so every stage (and all phases of its
+// barriers) belongs to one warpgroup, and an mbarrier parity wait never meets a barrier two phases ahead.
+static_assert(kGramStages % kConsumers == 0 && kStagesBwd % kConsumers == 0, "stage ownership");
 
-// ------------------------------------------------------------------------------------------
-// shared memory carve-up
-// ------------------------------------------------------------------------------------------
 struct TcBarriers {
-  uint64_t full[kStagesStats];
-  uint64_t ready[kStagesStats];
-  uint64_t empty[kStagesStats];
-  uint64_t accum;
-  uint32_t tmem_slot;
-  int flag;
+  uint64_t full[kMaxStages];       // TMA landed the stage                  (1 arrival + tx bytes)
+  uint64_t empty[kMaxStages];      // the owning warpgroup's MMAs are done  (one arrival per consumer warp)
 };
 
 // Tile range of this CTA inside its (domain, super-block) problem.
@@ -89,21 +71,36 @@ struct TileRange {
   }
 };
 
-// In-place transform of one landed tile by the kTT transform threads:
+__device__ __forceinline__ float4 lds128(uint32_t addr) {
+  float4 v;
+  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
+  return v;
+}
+__device__ __forceinline__ void sts128(uint32_t addr, float a, float b, float c, float d) {
+  asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
+}
+
+// Pilot shift of channel ch0 + r: the mean of <= 32 mid-image pixels of image 0 of domain d.
+__device__ __forceinline__ float pilot_shift(const float* __restrict__ x, const Geom& gm, int d, int c) {
+  if (c >= gm.C) return 0.f;
+  const int np = gm.HW < 32 ? gm.HW : 32, p0 = ((gm.HW - np) / 2) & ~3;
+  const float* px = x + ((size_t)d * gm.N * gm.C + c) * gm.HW + p0;
+  float a = 0.f;
+  for (int k = 0; k < np; ++k) a += __ldg(px + k);
+  return a / (float)np;
+}
+
+// In-place transform of one landed tile by the 128 threads of a consumer warpgroup (thread t):
 //   v <- RN_tf32(v - shift[row]) inside the tensor, 0 outside; returns per-thread row sums of (v - shift).
-// Chunk q = tt + kTT*i (16-byte units): row = q >> 3, physical chunk jp = q & 7, logical chunk = jp ^ (row & 7).
-// Shared memory is addressed in its own state space (LDS/STS; a generic pointer costs an address-space check
-// and global-load latency class per access), all loads first.
-__device__ __forceinline__ void transform_tile(uint32_t tile, int tt, const float (&shift)[kPer], int px0, int HW, int ch0,
+// Chunk q = t + 128*i (16-byte units): row = q >> 3, physical chunk jp = q & 7, logical chunk = jp ^ (row & 7).
+__device__ __forceinline__ void transform_tile(uint32_t tile, int t, const float (&shift)[kPer], int px0, int HW, int ch0,
                                                int C, float (&rowsum)[kPer]) {
   float4 v[kPer];
 #pragma unroll
-  for (int i = 0; i < kPer; ++i)
-    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v[i].x), "=f"(v[i].y), "=f"(v[i].z), "=f"(v[i].w)
-                 : "r"(tile + 16u * (tt + kTT * i)));
+  for (int i = 0; i < kPer; ++i) v[i] = lds128(tile + 16u * (t + 128 * i));
 #pragma unroll
   for (int i = 0; i < kPer; ++i) {
-    const int q = tt + kTT * i, row = q >> 3, jp = q & 7, j = jp ^ (row & 7);
+    const int q = t + 128 * i, row = q >> 3, jp = q & 7, j = jp ^ (row & 7);
     const int px = px0 + 4 * j;
     const bool rowok = (ch0 + row) < C;
     float e[4] = {v[i].x, v[i].y, v[i].z, v[i].w};
@@ -114,21 +111,79 @@ __device__ __forceinline__ void transform_tile(uint32_t tile, int tt, const floa
       rowsum[i] += s;
       e[k] = round_tf32(s);
     }
-    asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(tile + 16u * (tt + kTT * i)), "f"(e[0]), "f"(e[1]),
-                 "f"(e[2]), "f"(e[3]) : "memory");
+    sts128(tile + 16u * (t + 128 * i), e[0], e[1], e[2], e[3]);
   }
 }
 
+// Split transform of one landed Gram tile: s = x - shift inside the tensor, 0 outside; hi = trunc_tf32(s) in place,
+// lo = s - hi (exact) to the warpgroup's lo tile at the same swizzled position; returns per-thread row sums of s.  hi is
+// written explicitly so that HH and LH see the same hi whatever rounding the tensor core applies to fp32 words.  Two
+// chunks at a time: the accumulators leave few registers at two CTAs per SM.
+__device__ __forceinline__ void gram_transform(uint32_t tile, uint32_t lo, int t, const float (&shift)[kPer], int px0, int HW,
+                                               int ch0, int C, float (&rowsum)[kPer]) {
+#pragma unroll
+  for (int h = 0; h < kPer; h += 2) {
+    float4 v[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) v[i] = lds128(tile + 16u * (t + 128 * (h + i)));
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int q = t + 128 * (h + i), row = q >> 3, j = (q & 7) ^ (row & 7);
+      const int px = px0 + 4 * j;
+      const bool rowok = (ch0 + row) < C;
+      float e[4] = {v[i].x, v[i].y, v[i].z, v[i].w}, l[4];
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        const float s = (rowok && (px + k) < HW) ? e[k] - shift[h + i] : 0.f;
+        rowsum[h + i] += s;
+        e[k] = __uint_as_float(__float_as_uint(s) & kTf32Mask);
+        l[k] = s - e[k];
+      }
+      sts128(tile + 16u * q, e[0], e[1], e[2], e[3]);
+      sts128(lo + 16u * q, l[0], l[1], l[2], l[3]);
+    }
+  }
+}
+
+// The 8 consecutive threads that share a tile row (chunk q = t + 128 i, row = q >> 3) add their row sums into s[row].
+__device__ __forceinline__ void add_rowsums(float* s, const float (&rowsum)[kPer], int t) {
+#pragma unroll
+  for (int i = 0; i < kPer; ++i) {
+    float v = rowsum[i];
+    v += __shfl_xor_sync(0xffffffffu, v, 1);
+    v += __shfl_xor_sync(0xffffffffu, v, 2);
+    v += __shfl_xor_sync(0xffffffffu, v, 4);
+    if ((t & 7) == 0) atomicAdd(s + ((t + 128 * i) >> 3), v);
+  }
+}
+
+// Adds a warpgroup's [64 x 8*NB] accumulator fragment into a shared [64][pitch] matrix.  wgmma layout: thread (warp w,
+// lane l) holds, for every 8-column block j, rows 16w + l/4 and 16w + l/4 + 8 at columns 8j + 2(l%4) and 8j + 2(l%4) + 1.
+// At most two warpgroups add into a zeroed entry, so the result does not depend on their order.
+template <int NB>
+__device__ __forceinline__ void add_fragment(float* s, int pitch, const float (&acc)[4 * NB], int warp, int lane) {
+  const int r0 = 16 * (warp & 3) + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+  for (int j = 0; j < NB; ++j) {
+    atomicAdd(s + r0 * pitch + 8 * j + c0, acc[4 * j]);
+    atomicAdd(s + r0 * pitch + 8 * j + c0 + 1, acc[4 * j + 1]);
+    atomicAdd(s + (r0 + 8) * pitch + 8 * j + c0, acc[4 * j + 2]);
+    atomicAdd(s + (r0 + 8) * pitch + 8 * j + c0 + 1, acc[4 * j + 3]);
+  }
+}
+
+__device__ __forceinline__ void init_ring(TcBarriers& bars, int stages) {
+  for (int s = 0; s < stages; ++s) { mbar_init(&bars.full[s], 1); mbar_init(&bars.empty[s], 4); }
+  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+}
+
 // ------------------------------------------------------------------------------------------
-// the contraction kernel.  TWO = false: G = sum xs xs^T (stats).  TWO = true: R = sum dy xc^T.
+// backward contraction: R = sum dy xc^T and the row sums of dy
 // ------------------------------------------------------------------------------------------
-template <bool TWO>
 __global__ void __launch_bounds__(kTcThreads, 2)
-tc_contract_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_g,
-                   const float* __restrict__ x, const Geom gm, const float* __restrict__ save_mean,
-                   float* __restrict__ shift_out, float* __restrict__ partial) {
-  constexpr int STAGES = TWO ? kStagesBwd : kStagesStats;
-  constexpr int NT = TWO ? 2 : 1;
+tc_contract_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_g, const Geom gm,
+                   const float* __restrict__ save_mean, float* __restrict__ partial) {
+  constexpr int STAGES = kStagesBwd;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   __shared__ TcBarriers bars;
@@ -138,421 +193,167 @@ tc_contract_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
   const TileRange tr(gm);
   const int ntiles = tr.end - tr.begin;
 
-  if (tid == 0) {
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&bars.full[s], 1); mbar_init(&bars.ready[s], kTW); mbar_init(&bars.empty[s], 1); }
-    mbar_init(&bars.accum, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) tmem_alloc<kTmemCols>(&bars.tmem_slot);
-  // shift per channel: pilot mean (stats) or the saved batch mean (backward)
-  if (tid >= 64 && tid < 128) {
-    const int r = tid - 64, c = ch0 + r;
-    float sh = 0.f;
-    if (c < gm.C) {
-      if (TWO) sh = save_mean[(size_t)d * gm.C + c];
-      else {
-        const int np = gm.HW < 32 ? gm.HW : 32, p0 = ((gm.HW - np) / 2) & ~3;
-        const float* px = x + ((size_t)d * gm.N * gm.C + c) * gm.HW + p0;
-        float a = 0.f;
-        for (int k = 0; k < np; ++k) a += __ldg(px + k);
-        sh = a / (float)np;
-      }
-    }
-    sShift[r] = sh;
-    if (!TWO && blockIdx.x == 0) shift_out[((size_t)d * gridDim.y + sb) * kTileCh + r] = sh;
-  }
-  tc_fence_before();
+  if (tid == 0) init_ring(bars, STAGES);
+  if (tid < kTileCh) sShift[tid] = ch0 + tid < gm.C ? save_mean[(size_t)d * gm.C + ch0 + tid] : 0.f;
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_d = bars.tmem_slot;
 
-  float rowsum[kPer];
+  float acc[32], rowsum[kPer];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) acc[i] = 0.f;
 #pragma unroll
   for (int i = 0; i < kPer; ++i) rowsum[i] = 0.f;
-  const int tt = tid - 64;                       // transform thread index (warps 2..9)
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     // ===== TMA producer =====
     if (lane == 0) {
       for (int it = 0; it < ntiles; ++it) {
-        const int s = it % STAGES, ph = (it / STAGES) & 1;
-        mbar_wait_relaxed(&bars.empty[s], ph ^ 1);
+        const int s = it % STAGES;
+        mbar_wait_relaxed(&bars.empty[s], ((it / STAGES) & 1) ^ 1);
         const int t = tr.begin + it, n = t / tr.PB, pb = t - n * tr.PB;
-        uint8_t* dst = smem + (size_t)s * NT * kTileBytes;
-        mbar_arrive_expect_tx(&bars.full[s], NT * kTileBytes);
+        uint8_t* dst = smem + (size_t)s * 2 * kTileBytes;
+        mbar_arrive_expect_tx(&bars.full[s], 2 * kTileBytes);
         tma_load_3d(dst, &map_x, pb * kTilePx, ch0, d * gm.N + n, &bars.full[s]);
-        if (TWO) tma_load_3d(dst + kTileBytes, &map_g, pb * kTilePx, ch0, d * gm.N + n, &bars.full[s]);
+        tma_load_3d(dst + kTileBytes, &map_g, pb * kTilePx, ch0, d * gm.N + n, &bars.full[s]);
       }
-    }
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    constexpr uint32_t idesc = make_idesc_tf32(64, 64);
-    for (int it = 0; it < ntiles; ++it) {
-      const int s = it % STAGES, ph = (it / STAGES) & 1;
-      mbar_wait(&bars.ready[s], ph);
-      tc_fence_after();
-      const uint32_t xaddr = smem_u32(smem + (size_t)s * NT * kTileBytes);      // warp-uniform; one elected lane issues
-      const uint64_t xdesc = make_kmajor_sw128_desc(xaddr);
-      const uint64_t adesc = TWO ? make_kmajor_sw128_desc(xaddr + kTileBytes) : xdesc;   // A = dy tile (rows i)
-      if (elect_one()) {
-#pragma unroll
-        for (int k = 0; k < kTilePx / 8; ++k)
-          umma_tf32(tmem_d, adesc + 2 * k, xdesc + 2 * k, idesc, (it > 0 || k > 0) ? 1u : 0u);
-        umma_commit(&bars.empty[s]);
-        if (it == ntiles - 1) umma_commit(&bars.accum);
-      }
-      __syncwarp();
     }
   } else {
-    // ===== transform warps =====
+    // ===== consumer warpgroups: transform, then D[64 x 64] += dy_tile (A) * xc_tile^T (B) =====
+    const int wg = warp >> 2, t = tid & 127;
     float shift[kPer], zero[kPer], dummy[kPer];
 #pragma unroll
-    for (int i = 0; i < kPer; ++i) { shift[i] = sShift[(tt + kTT * i) >> 3]; zero[i] = 0.f; dummy[i] = 0.f; }
-    for (int it = 0; it < ntiles; ++it) {
-      const int s = it % STAGES, ph = (it / STAGES) & 1;
-      mbar_wait(&bars.full[s], ph);
-      const int t = tr.begin + it, n = t / tr.PB, pb = t - n * tr.PB;
-      const uint32_t tile = smem_u32(smem + (size_t)s * NT * kTileBytes);
-      if (TWO) {
-        transform_tile(tile, tt, shift, pb * kTilePx, gm.HW, ch0, gm.C, dummy);                     // xc
-        transform_tile(tile + kTileBytes, tt, zero, pb * kTilePx, gm.HW, ch0, gm.C, rowsum);        // dy, sums
-      } else {
-        transform_tile(tile, tt, shift, pb * kTilePx, gm.HW, ch0, gm.C, rowsum);
-      }
+    for (int i = 0; i < kPer; ++i) { shift[i] = sShift[(t + 128 * i) >> 3]; zero[i] = 0.f; dummy[i] = 0.f; }
+    for (int it = wg; it < ntiles; it += kConsumers) {
+      const int s = it % STAGES;
+      mbar_wait(&bars.full[s], (it / STAGES) & 1);
+      const int tl = tr.begin + it, n = tl / tr.PB, pb = tl - n * tr.PB;
+      const uint32_t tile = smem_u32(smem + (size_t)s * 2 * kTileBytes);
+      transform_tile(tile, t, shift, pb * kTilePx, gm.HW, ch0, gm.C, dummy);                     // xc
+      transform_tile(tile + kTileBytes, t, zero, pb * kTilePx, gm.HW, ch0, gm.C, rowsum);        // dy, sums
       fence_proxy_async();
+      warpgroup_sync(wg);
+      wgmma_fence();
+      fence_operands(acc);
+      const uint64_t xdesc = make_kmajor_sw128_desc(tile), adesc = make_kmajor_sw128_desc(tile + kTileBytes);
+#pragma unroll
+      for (int k = 0; k < kTilePx / 8; ++k) wgmma_m64n64k8_ss(acc, adesc + 2 * k, xdesc + 2 * k);
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_operands(acc);
       __syncwarp();
-      if (lane == 0) mbar_arrive(&bars.ready[s]);
+      if (lane == 0) mbar_arrive(&bars.empty[s]);
     }
   }
 
-  // ===== epilogue: accumulator + row sums -> this CTA's partial row =====
-  const int nacc = kTileCh * kTileCh + kTileCh;
-  float* prow = partial + (((size_t)d * gridDim.y + sb) * gridDim.x + blockIdx.x) * nacc;
-  if (warp >= 2) {
-    if (ntiles > 0 && warp < 6) {                  // four warps cover the four TMEM lane quadrants
-      mbar_wait(&bars.accum, 0);
-      tc_fence_after();
-      const int quad = warp & 3;                   // TMEM lane quadrant this warp may access
-      float v[32];
-#pragma unroll
-      for (int half = 0; half < 2; ++half) {
-        tmem_ld32(tmem_d + ((uint32_t)(quad * 32) << 16) + half * 32, v);
-        if (lane < 16) {                           // M=64 accumulator: row = 16*quad + lane
-          float* dst = prow + (quad * 16 + lane) * kTileCh + half * 32;
-#pragma unroll
-          for (int c4 = 0; c4 < 8; ++c4)
-            *reinterpret_cast<float4*>(dst + 4 * c4) = make_float4(v[4 * c4], v[4 * c4 + 1], v[4 * c4 + 2], v[4 * c4 + 3]);
-        }
-      }
-      tc_fence_before();
-    } else if (ntiles == 0) {
-      for (int e = tt; e < kTileCh * kTileCh; e += kTT) prow[e] = 0.f;
-    }
-    // row sums: the 8 lanes that share a row are consecutive
-#pragma unroll
-    for (int i = 0; i < kPer; ++i) {
-      float s = rowsum[i];
-      s += __shfl_xor_sync(0xffffffffu, s, 1);
-      s += __shfl_xor_sync(0xffffffffu, s, 2);
-      s += __shfl_xor_sync(0xffffffffu, s, 4);
-      if ((tt & 7) == 0) prow[kTileCh * kTileCh + ((tt + kTT * i) >> 3)] = s;
-    }
+  // ===== epilogue: both warpgroups' accumulators + row sums -> this CTA's partial row =====
+  __syncthreads();                                 // every stage consumed: the ring is free
+  float* sAcc = reinterpret_cast<float*>(smem);    // [64][64] + [64]
+  for (int e = tid; e < kNacc; e += kTcThreads) sAcc[e] = 0.f;
+  __syncthreads();
+  if (warp < kProducerWarp) {
+    add_fragment<8>(sAcc, kTileCh, acc, warp, lane);
+    add_rowsums(sAcc + kTileCh * kTileCh, rowsum, tid & 127);
   }
   __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc<kTmemCols>(tmem_d); }
-
+  float* prow = partial + (((size_t)d * gridDim.y + sb) * gridDim.x + blockIdx.x) * kNacc;
+  for (int e = tid; e < kNacc; e += kTcThreads) prow[e] = sAcc[e];
 }
 
 // ------------------------------------------------------------------------------------------
 // split-precision Gram kernel (forward statistics): G = HH + LH + LH^T, see the file header
 // ------------------------------------------------------------------------------------------
-__device__ __forceinline__ float4 lds128(uint32_t addr) {
-  float4 v;
-  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
-  return v;
-}
-__device__ __forceinline__ void sts128(uint32_t addr, float a, float b, float c, float d) {
-  asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
-
-// Transform of one landed tile by one warp.  s = x - shift inside the tensor, 0 outside (the 32 lanes of a warp read 16
-// distinct 128-byte rows, 8 swizzled 16-byte chunks each).  A warp may only touch its own 32 TMEM lanes, and WHICH
-// A-operand row lives in which lane is free (D row r is just A row r times B): quarter q carries channels 16q..16q+15,
-// lanes 0..15 their hi rows and lanes 16..31 their lo rows.  The tensor core reads the top 19 bits of an fp32 word, so
-// hi = trunc_tf32(s) needs NO instruction: the hi lanes hand s itself to tensor memory and write s back in place as the
-// B operand (both truncated alike by the core: HH stays symmetric), the lo lanes hand over lo = s - trunc_tf32(s)
-// (exact in fp32, |lo| < 2^-10 |s|; the core keeps its top 11 bits).  One instruction stream serves both halves:
-// out = s - (s & mask), mask = 0 in the hi lanes (s - 0 = s) and 0xFFFFE000 in the lo lanes.  Per warp and tile:
-// 8 LDS.128 + 32 FADD (shift) + 8 predicated STS.128 + 32 LOP3 + 32 FADD + 1 tcgen05.st.  An earlier form with
-// homogeneous hi warps / lo warps and round-to-nearest (two integer instructions per element in both, the tile read
-// twice, the pairs meeting at a named barrier) needed 1040 warp instructions per tile against 720 here
-// (profiles/ncu_r02_tc_gram.md).  Truncation instead of rounding leaves lo one bit longer: the dropped lo lo^T term is
-// 3e-7 of the covariance (RN: 3e-8), a near-uniform scale of the diagonal that the whitened output does not see
-// (tools/tf32_gram_accuracy.py: y error unchanged).
-// (Waiting for the tensor-memory slot only before the final tcgen05.st, after the arithmetic, was slower -- 186 us against
-// 172: the two sets then compute concurrently and delay the OLDER tile, which is the one the MMA issuers wait for.)
-__device__ __forceinline__ void gram_transform_quarter(uint32_t tile, int ch, bool hi_lane, uint32_t lomask, float shift, int px0,
-                                                       int HW, bool rowok, uint32_t tmem_a) {
-  const uint32_t rbase = tile + 128u * (uint32_t)ch;
-  const int sw = ch & 7;
-  float2 v[16];                      // pairs: Blackwell's packed fp32 add halves the instruction count of both passes
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    const float4 t4 = lds128(rbase + 16u * (uint32_t)(j ^ sw));
-    v[2 * j] = make_float2(t4.x, t4.y); v[2 * j + 1] = make_float2(t4.z, t4.w);
-  }
-  if (rowok && px0 + kTilePx <= HW) {
-    const float2 ns = make_float2(-shift, -shift);               // x + (-K) == x - K
-#pragma unroll
-    for (int k = 0; k < 16; ++k) v[k] = __fadd2_rn(v[k], ns);
-  } else {
-#pragma unroll
-    for (int k = 0; k < 16; ++k) {
-      v[k].x = (rowok && px0 + 2 * k < HW) ? v[k].x - shift : 0.f;
-      v[k].y = (rowok && px0 + 2 * k + 1 < HW) ? v[k].y - shift : 0.f;
-    }
-  }
-  if (hi_lane) {                     // lanes l and l + 16 loaded the same row in the same instruction: no hazard
-#pragma unroll
-    for (int j = 0; j < 8; ++j) sts128(rbase + 16u * (uint32_t)(j ^ sw), v[2 * j].x, v[2 * j].y, v[2 * j + 1].x, v[2 * j + 1].y);
-  }
-  // out = s + (-(s & mask)): one LOP3 per element ((s & mask) ^ sign; -0 in the hi lanes, and s + -0 == s), one packed add per pair
-#pragma unroll
-  for (int k = 0; k < 16; ++k) {
-    const float2 t = make_float2(__uint_as_float((__float_as_uint(v[k].x) & lomask) ^ 0x80000000u),
-                                 __uint_as_float((__float_as_uint(v[k].y) & lomask) ^ 0x80000000u));
-    v[k] = __fadd2_rn(v[k], t);
-  }
-  tmem_st32(tmem_a, reinterpret_cast<const float(&)[32]>(v));
-}
-
-// Shared-memory stage of the Gram kernel: the landed [64 ch x 32 px] tile followed by 16 constant rows -- row 64 all
-// ones, rows 65..79 zero.  The MMA takes B = all 80 rows (N = 80), so accumulator column 64 collects sum_k A[:, k] * 1:
-// the per-channel sums of hi (hi rows) and lo (lo rows), i.e. the row sums the mean needs, for free on the tensor pipe.
-constexpr int kGramN = kTileCh + 16;
-constexpr int kGramStageBytes = kGramN * kTilePx * 4;            // 10240
-constexpr int kGramStages = 9;                                   // 90 KB + alignment: two CTAs per SM
-
-// Barriers of the Gram kernel.  Tiles alternate between two transform sets and two MMA issuers while the data rings
-// (9 stages, 3 A slots) have ODD lengths, so consecutive uses of one stage / slot belong to different waiters -- and an
-// mbarrier parity wait is only sound for a waiter that is at most one phase away from the barrier (two phases off it
-// falls through).  Every (ring index, tile parity) pair therefore has its own barrier: barrier rings of twice the
-// data-ring length, indexed by tile mod 2L with phase (tile / 2L) & 1.  All phases of one barrier then belong to one
-// waiter, which visits them in order, and nothing depends on how far the warps drift apart.
-struct GramBarriers {
-  uint64_t full[2 * kGramStages];      // TMA landed tile t                          waiter: transform set t & 1
-  uint64_t ready[2 * kGramStages];     // the 4 warps of set t & 1 transformed t      waiter: MMA issuer t & 1
-  uint64_t empty[kGramStages];         // MMAs of tile t complete, stage free         waiter: the producer, every phase
-  uint64_t a_empty[2 * kGramASlots];   // MMAs of tile t complete, A slot free        waiter: set (t + 3) & 1
-  uint64_t accum[kGramAcc];            // issuer m's accumulator is final
-  uint32_t tmem_slot;
-};
-
-// 11 warps: TMA producer, MMA issuer 0, 8 transform warps, MMA issuer 1 (tiles alternate between the two issuers, each
-// with its own accumulator).  One thread issuing the 4 tcgen05.mma + 2 tcgen05.commit of EVERY tile was the bottleneck of
-// the single-issuer versions (~1000 cycles per tile whatever the number of accumulators or A slots; the same 4 MMAs per
-// tile paced the round-1 single-pass kernel) -- profiles/ncu_r02_tc_gram.md.
-constexpr int kGramThreads = kTcThreads + 32;
-
-// development: -DDWT_PROF_GRAM records a clock64 timeline of tiles kProfT0.. of CTA (0, 0, 0) and prints it
-#ifdef DWT_PROF_GRAM
-constexpr int kProfT0 = 96, kProfN = 48;
-#define GPROF(ev, it) do { if (prof_on && (it) >= kProfT0 && (it) < kProfT0 + kProfN) sProf[ev][(it) - kProfT0] = clock64(); } while (0)
-#else
-#define GPROF(ev, it)
-#endif
-
-__global__ void __launch_bounds__(kGramThreads, 2)
+__global__ void __launch_bounds__(kTcThreads, 2)
 tc_gram_kernel(const __grid_constant__ CUtensorMap map_x, const float* __restrict__ x, const Geom gm,
                float* __restrict__ shift_out, float* __restrict__ partial) {
-  constexpr int STAGES = kGramStages, NA = kGramASlots, NACCUM = kGramAcc;    // 2 x 80 accumulator columns + 3 x 32 = 256
+  constexpr int STAGES = kGramStages;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  __shared__ GramBarriers bars;
+  __shared__ TcBarriers bars;
   __shared__ float sShift[kTileCh];
-  __shared__ float sRS[kTileCh];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, tid = threadIdx.x;
   const int sb = blockIdx.y, d = blockIdx.z, ch0 = sb * kTileCh;
-#ifdef DWT_PROF_GRAM
-  __shared__ long long sProf[6][kProfN];
-  const bool prof_on = blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && lane == 0;
-#endif
   const TileRange tr(gm);
   const int ntiles = tr.end - tr.begin;
 
-  if (tid == 0) {
-    for (int s = 0; s < 2 * STAGES; ++s) { mbar_init(&bars.full[s], 1); mbar_init(&bars.ready[s], 4); }
-    for (int s = 0; s < STAGES; ++s) mbar_init(&bars.empty[s], 1);
-    for (int a = 0; a < 2 * NA; ++a) mbar_init(&bars.a_empty[a], 1);
-    for (int m = 0; m < NACCUM; ++m) mbar_init(&bars.accum[m], 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  if (tid == 0) init_ring(bars, STAGES);
+  if (tid < kTileCh) {
+    const float sh = pilot_shift(x, gm, d, ch0 + tid);
+    sShift[tid] = sh;
+    if (blockIdx.x == 0) shift_out[((size_t)d * gridDim.y + sb) * kTileCh + tid] = sh;
   }
-  if (warp == 1) tmem_alloc<kGramTmemCols>(&bars.tmem_slot);
-  if (tid >= 64 && tid < 128) {                    // pilot shift per channel (mean of <= 32 mid-image pixels of image 0)
-    const int r = tid - 64, c = ch0 + r;
-    float sh = 0.f;
-    if (c < gm.C) {
-      const int np = gm.HW < 32 ? gm.HW : 32, p0 = ((gm.HW - np) / 2) & ~3;
-      const float* px = x + ((size_t)d * gm.N * gm.C + c) * gm.HW + p0;
-      float a = 0.f;
-      for (int k = 0; k < np; ++k) a += __ldg(px + k);
-      sh = a / (float)np;
-    }
-    sShift[r] = sh;
-    if (blockIdx.x == 0) shift_out[((size_t)d * gridDim.y + sb) * kTileCh + r] = sh;
-  }
-  // constant rows 64..79 of every stage (128 16-byte chunks each): row 64 (chunks 0..7, un-swizzled: 64 & 7 == 0) = 1.0
-  for (int e = tid; e < STAGES * 128; e += kGramThreads) {
-    const int s = e >> 7, q = e & 127;
-    const float val = q < 8 ? 1.f : 0.f;
-    sts128(smem_u32(smem + (size_t)s * kGramStageBytes + kTileBytes) + 16u * (uint32_t)q, val, val, val, val);
-  }
-  fence_proxy_async();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = bars.tmem_slot;
-  const uint32_t tmem_d = tmem, tmem_a0 = tmem + NACCUM * kGramN;   // accumulators: columns 0..159; A slots from column 160
 
-  // transform-warp geometry: two sets of four warps take alternate tiles; a warp may only touch the TMEM quarter
-  // warp & 3, which carries channels 16q..16q+15: hi rows in lanes 0..15, lo rows in lanes 16..31
-  const int quad = warp & 3, set = (warp - 2) >> 2;
-  const bool lo_lane = lane >= 16;                 // see gram_transform_quarter
-  const int row = 16 * quad + (lane & 15);         // channel row of the tile this lane handles
+  float hh[32], lh[32], rowsum[kPer];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) { hh[i] = 0.f; lh[i] = 0.f; }
+#pragma unroll
+  for (int i = 0; i < kPer; ++i) rowsum[i] = 0.f;
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     // ===== TMA producer =====
     if (lane == 0) {
       int n = tr.begin / tr.PB, pb = tr.begin - n * tr.PB;
       for (int it = 0; it < ntiles; ++it) {
         const int s = it % STAGES;
-        uint64_t* full = &bars.full[it % (2 * STAGES)];
         mbar_wait_relaxed(&bars.empty[s], ((it / STAGES) & 1) ^ 1);
-        GPROF(0, it);
-        mbar_arrive_expect_tx(full, kTileBytes);
-        tma_load_3d(smem + (size_t)s * kGramStageBytes, &map_x, pb * kTilePx, ch0, d * gm.N + n, full);
+        mbar_arrive_expect_tx(&bars.full[s], kTileBytes);
+        tma_load_3d(smem + (size_t)s * kTileBytes, &map_x, pb * kTilePx, ch0, d * gm.N + n, &bars.full[s]);
         if (++pb == tr.PB) { pb = 0; ++n; }
       }
     }
-  } else if (warp == 1 || warp == 10) {
-    // ===== MMA issuers: D_m[128 x 80] += [hi ; lo] (tensor memory) x [hi tile ; ones ; 0]^T (shared memory) =====
-    // issuer m takes tiles m, m + 2, ... into accumulator m (GramBarriers: its `ready` barriers are its own)
-    constexpr uint32_t idesc = make_idesc_tf32(128, kGramN);
-    const int m = warp == 1 ? 0 : 1;
-    const uint32_t dacc = tmem_d + (uint32_t)(m * kGramN);
-    for (int it = m; it < ntiles; it += 2) {
-      mbar_wait(&bars.ready[it % (2 * STAGES)], (it / (2 * STAGES)) & 1);
-      GPROF(4, it);
-      tc_fence_after();
-      const int s = it % STAGES, a = it % NA;                 // warp-uniform: computed by every lane, issued by one
-      const uint64_t bdesc = make_kmajor_sw128_desc(smem_u32(smem + (size_t)s * kGramStageBytes));
-      const uint32_t ta = tmem_a0 + (uint32_t)(a * kTilePx);
-      uint64_t* e_stage = &bars.empty[s];
-      uint64_t* e_slot = &bars.a_empty[it % (2 * NA)];
-      const bool last = it + 2 >= ntiles;
-      if (elect_one()) {
-#pragma unroll
-        for (int k = 0; k < kTilePx / 8; ++k)
-          umma_tf32_ts(dacc, ta + (uint32_t)(8 * k), bdesc + 2 * k, idesc, (it >= 2 || k > 0) ? 1u : 0u);
-        umma_commit(e_stage);
-        umma_commit(e_slot);
-        if (last) umma_commit(&bars.accum[m]);
-        GPROF(5, it);
-      }
-      __syncwarp();
-    }
   } else {
-    // ===== transform warps =====
-    const float shift = sShift[row];
-    const bool rowok = (ch0 + row) < gm.C;
-    const uint32_t smem0 = smem_u32(smem), ta0 = tmem_a0 + ((uint32_t)(quad * 32) << 16);
-    const int t0 = tr.begin + set;
-    int n = t0 / tr.PB, pb = t0 - n * tr.PB;
-    for (int it = set; it < ntiles; it += 2) {
-      const int s = it % STAGES, a = it % NA, u = it - NA;                // u: the tile that used A slot a before
-      mbar_wait(&bars.full[it % (2 * STAGES)], (it / (2 * STAGES)) & 1);
-      if (quad == 0) GPROF(1, it);
-      if (u >= 0) mbar_wait(&bars.a_empty[u % (2 * NA)], (u / (2 * NA)) & 1);
-      if (quad == 0) GPROF(2, it);
-      tc_fence_after();
-      const uint32_t tile = smem0 + (uint32_t)(s * kGramStageBytes), ta = ta0 + (uint32_t)(a * kTilePx);
-      gram_transform_quarter(tile, row, !lo_lane, lo_lane ? 0xFFFFE000u : 0u, shift, pb * kTilePx, gm.HW, rowok, ta);
-      tc_fence_before();
+    // ===== consumer warpgroups: HH[64 x 64] += hi * hi^T,  LH[64 x 64] += lo * hi^T =====
+    const int wg = warp >> 2, t = tid & 127;
+    const uint32_t lo = smem_u32(smem + (size_t)STAGES * kTileBytes + (size_t)wg * kTileBytes);
+    const uint64_t ldesc = make_kmajor_sw128_desc(lo);
+    float shift[kPer];
+#pragma unroll
+    for (int i = 0; i < kPer; ++i) shift[i] = sShift[(t + 128 * i) >> 3];
+    for (int it = wg; it < ntiles; it += kConsumers) {
+      const int s = it % STAGES;
+      mbar_wait(&bars.full[s], (it / STAGES) & 1);
+      const int tl = tr.begin + it, n = tl / tr.PB, pb = tl - n * tr.PB;
+      const uint32_t tile = smem_u32(smem + (size_t)s * kTileBytes);
+      gram_transform(tile, lo, t, shift, pb * kTilePx, gm.HW, ch0, gm.C, rowsum);
       fence_proxy_async();
+      warpgroup_sync(wg);
+      wgmma_fence();
+      fence_operands(hh);
+      fence_operands(lh);
+      const uint64_t bdesc = make_kmajor_sw128_desc(tile);
+#pragma unroll
+      for (int k = 0; k < kTilePx / 8; ++k) {
+        wgmma_m64n64k8_ss(hh, bdesc + 2 * k, bdesc + 2 * k);
+        wgmma_m64n64k8_ss(lh, ldesc + 2 * k, bdesc + 2 * k);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();                             // the lo tile is rewritten by this warpgroup's next transform
+      fence_operands(hh);
+      fence_operands(lh);
       __syncwarp();
-      if (lane == 0) mbar_arrive(&bars.ready[it % (2 * STAGES)]);
-      if (quad == 0) GPROF(3, it);
-      pb += 2;
-      while (pb >= tr.PB) { pb -= tr.PB; ++n; }
+      if (lane == 0) mbar_arrive(&bars.empty[s]);
     }
   }
 
   // ===== epilogue: G = HH + LH + LH^T and the row sums -> this CTA's partial row =====
-  const int nacc = kTileCh * kTileCh + kTileCh;
-  float* prow = partial + (((size_t)d * gridDim.y + sb) * gridDim.x + blockIdx.x) * nacc;
-  float* sT = reinterpret_cast<float*>(smem);      // LH, [64][65]; the tile ring is drained by now
-  float P[kTileCh], rs = 0.f;
-  const bool epi_warp = warp >= 2 && warp < 6;     // one warp per TMEM quarter
-  if (epi_warp && ntiles > 0) {
-    mbar_wait(&bars.accum[0], 0);
-    if (ntiles > 1) mbar_wait(&bars.accum[1], 0);
-    tc_fence_after();
-    float tail[16];
-    tmem_ld32(tmem_d + ((uint32_t)(quad * 32) << 16), reinterpret_cast<float(&)[32]>(P[0]));
-    tmem_ld32(tmem_d + ((uint32_t)(quad * 32) << 16) + 32, reinterpret_cast<float(&)[32]>(P[32]));
-    tmem_ld16(tmem_d + ((uint32_t)(quad * 32) << 16) + 64, tail);
-#pragma unroll
-    for (int acc = 1; acc < NACCUM; ++acc) {
-      if (acc < ntiles) {                           // accumulator `acc` received tiles acc, acc + NACCUM, ...
-        float t32[32], t16[16];
-#pragma unroll
-        for (int half = 0; half < 2; ++half) {
-          tmem_ld32(tmem_d + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * kGramN + half * 32), t32);
-#pragma unroll
-          for (int j = 0; j < 32; ++j) P[half * 32 + j] += t32[j];
-        }
-        tmem_ld16(tmem_d + ((uint32_t)(quad * 32) << 16) + (uint32_t)(acc * kGramN + 64), t16);
-        tail[0] += t16[0];
-      }
-    }
-    tc_fence_before();
-    rs = tail[0];                                  // sum over the CTA's samples of hi (hi rows) / lo (lo rows)
-    if (lo_lane) {
-#pragma unroll
-      for (int j = 0; j < kTileCh; ++j) sT[row * (kTileCh + 1) + j] = P[j];          // LH[row][j]
-      sRS[row] = rs;
-    }
+  constexpr int P = kTileCh + 1;                   // odd pitch: the transposed read of LH is conflict-free
+  __syncthreads();                                 // every stage consumed: the ring is free
+  float* sH = reinterpret_cast<float*>(smem);      // [64][P]
+  float* sL = sH + kTileCh * P;                    // [64][P]
+  float* sRS = sL + kTileCh * P;                   // [64]
+  for (int e = tid; e < 2 * kTileCh * P + kTileCh; e += kTcThreads) sH[e] = 0.f;
+  __syncthreads();
+  if (warp < kProducerWarp) {
+    add_fragment<8>(sH, P, hh, warp, lane);
+    add_fragment<8>(sL, P, lh, warp, lane);
+    add_rowsums(sRS, rowsum, tid & 127);
   }
   __syncthreads();
-  if (epi_warp && !lo_lane) {
-    if (ntiles > 0) {
-#pragma unroll
-      for (int j4 = 0; j4 < kTileCh / 4; ++j4) {
-        float o[4];
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          const int j = 4 * j4 + k;
-          o[k] = (P[j] + sT[row * (kTileCh + 1) + j]) + sT[j * (kTileCh + 1) + row];   // HH + LH + LH^T
-        }
-        *reinterpret_cast<float4*>(prow + row * kTileCh + 4 * j4) = make_float4(o[0], o[1], o[2], o[3]);
-      }
-      prow[kTileCh * kTileCh + row] = rs + sRS[row];
-    } else {
-      for (int j = 0; j < kTileCh; ++j) prow[row * kTileCh + j] = 0.f;
-      prow[kTileCh * kTileCh + row] = 0.f;
-    }
+  float* prow = partial + (((size_t)d * gridDim.y + sb) * gridDim.x + blockIdx.x) * kNacc;
+  for (int e = tid; e < kTileCh * kTileCh; e += kTcThreads) {
+    const int r = e >> 6, c = e & 63;
+    prow[e] = (sH[r * P + c] + sL[r * P + c]) + sL[c * P + r];
   }
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc<kGramTmemCols>(tmem); }
-#ifdef DWT_PROF_GRAM
-  if (tid == 0 && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && ntiles >= kProfT0 + kProfN) {
-    const long long t0 = sProf[0][0];
-    printf("tc_gram timeline (cycles from the TMA issue of tile %d): tile | tma full a_free arrive | ready issued\n", kProfT0);
-    for (int i = 0; i < kProfN; ++i)
-      printf("%3d %7lld %7lld %7lld %7lld %7lld %7lld\n", kProfT0 + i, sProf[0][i] - t0, sProf[1][i] - t0, sProf[2][i] - t0,
-             sProf[3][i] - t0, sProf[4][i] - t0, sProf[5][i] - t0);
-  }
-#endif
+  if (tid < kTileCh) prow[kTileCh * kTileCh + tid] = sRS[tid];
 }
 
 // ------------------------------------------------------------------------------------------
@@ -573,7 +374,10 @@ int make_map(CUtensorMap* map, const float* base, const Geom& gm) {
                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
 }
 
-size_t tc_smem_bytes(bool two) { return two ? (size_t)kStagesBwd * 2 * kTileBytes + 1024 : (size_t)kGramStages * kGramStageBytes + 1024; }
+size_t tc_smem_bytes(bool two) {
+  return two ? (size_t)kStagesBwd * 2 * kTileBytes + 1024
+             : (size_t)kGramStages * kTileBytes + (size_t)kConsumers * kTileBytes + 1024;
+}
 
 }  // namespace
 
@@ -585,16 +389,16 @@ int tc_init() {
   g_encode = reinterpret_cast<EncodeTiledFn>(fn);
   e = cudaFuncSetAttribute(tc_gram_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes(false));
   if (e == cudaSuccess)
-    e = cudaFuncSetAttribute(tc_contract_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes(true));
-  // two ~97 KB CTAs per SM need the full shared-memory carve-out
+    e = cudaFuncSetAttribute(tc_contract_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes(true));
+  // two ~90-97 KB CTAs per SM need the full shared-memory carve-out
   if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_gram_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_contract_kernel<true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_contract_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   if (e == cudaSuccess) e = (cudaError_t)dense_init();
   if (e == cudaSuccess) return tc_apply_init();
   return (int)e;
 }
 
-// The TMA/tcgen05 contraction takes group sizes that tile a 64-channel super-block, rows that TMA can
+// The TMA/wgmma contraction takes group sizes that tile a 64-channel super-block, rows that TMA can
 // address (16-byte strides and base) and at least one full 32-pixel box per row.
 // TF32 operands are rounded to nearest, so product errors are zero-mean and shrink as 1/sqrt(M); below a
 // few thousand samples per channel they do not, and the (exact fp32, FFMA) tiled kernels take the call.
@@ -610,7 +414,7 @@ int tc_stats(const float* x, const Geom& gm, int nchunks, float* shift, float* p
   bind_context();
   if (int rc = make_map(&mx, x, gm)) return rc;
   dim3 grid(nchunks, tc_superblocks(gm), gm.D);
-  tc_gram_kernel<<<grid, kGramThreads, tc_smem_bytes(false), st>>>(mx, x, gm, shift, partial);
+  tc_gram_kernel<<<grid, kTcThreads, tc_smem_bytes(false), st>>>(mx, x, gm, shift, partial);
   return 0;
 }
 
@@ -621,7 +425,7 @@ int tc_bwd_reduce(const float* x, const float* dout, const Geom& gm, int nchunks
   if (int rc = make_map(&mx, x, gm)) return rc;
   if (int rc = make_map(&mg, dout, gm)) return rc;
   dim3 grid(nchunks, tc_superblocks(gm), gm.D);
-  tc_contract_kernel<true><<<grid, kTcThreads, tc_smem_bytes(true), st>>>(mx, mg, x, gm, save_mean, nullptr, partial);
+  tc_contract_kernel<<<grid, kTcThreads, tc_smem_bytes(true), st>>>(mx, mg, gm, save_mean, partial);
   return 0;
 }
 

@@ -4,43 +4,26 @@
 //   bwd_apply   dx = A1 (dy - mean_M dy) + Bm (x - mean)        two input tensors
 //
 // Per 64-channel super-block the per-group matrices form one block-diagonal 64x64 matrix M, and a
-// [64 ch x 128 px] tile of the NCHW tensor is out = M * tile: a GEMM whose B operand is the tile exactly
-// as TMA lands it (rows = channels = K, pixels contiguous = MN-major), so nothing is transposed.
+// [64 ch x 64 px] tile of the NCHW tensor gives out = M * tile.  wgmma takes tf32 operands from shared memory only
+// K-major, and the landed tile is pixel-major, so the product is computed transposed, out^T = tile^T M^T:
+// A = tile^T (64 pixels x 64 channels) is loaded from the swizzled tile into the wgmma register fragment, and
+// B = M (rows = output channel, K = input channel) sits K-major in shared memory for the whole kernel.
 // A single-pass TF32 product is NOT accurate enough here -- each output is one length-64 dot product
 // whose terms can cancel by the condition number of the covariance -- so both operands are split
-// x = hi + lo and the four partial products are accumulated in fp32:
-//   matrix  hi = RN_tf32(m), lo = RN_tf32(m - hi), STACKED as a 128-row A operand [M_hi ; M_lo]: one M=128 MMA
-//           per B half yields M_hi*B and M_lo*B rows in TMEM and the epilogue adds the two row halves;
-//   tile    hi = the landed fp32 words themselves (the tensor core reads the top 19 bits: trunc_tf32), so the
-//           raw tile is an operand as it is; lo = RN_tf32(x - trunc_tf32(x)) is the only thing computed and
-//           written per element;
-//   centring is linear, M (x - shift) = M x - M shift, and is applied as one constant per row at the end.
+// v = hi + lo and all four partial products are accumulated in fp32 (lo*lo still moves the largest output errors,
+// ~1e-6 absolute, by a third -- enough to flip a ReLU mask downstream):
+//   matrix  hi = RN_tf32(m), lo = RN_tf32(m - hi)
+//   tile    v = x - shift (centred while it is loaded into registers), hi = trunc_tf32(v), lo = RN_tf32(v - hi)
+// Centring before the product keeps the fp32 accumulation error relative to |y| rather than to |M x|; centring after
+// it (M x - M shift) doubled the largest output errors on inputs with a large mean.
 //
-// CTA = 2 + 8 + 8 warps, one per SM, persistent over a contiguous range of 128-pixel tiles of one (domain,
-// super-block); every input tensor of a tile is one STEP through the rings:
-//   warp 0     TMA producer into a RAW ring (4 boxes of 32 px x 64 ch per slot,
-//              SWIZZLE_128B_ATOM_32B: the only layout the tensor core takes for an MN-major tf32 operand)
-//   warp 1     MMA issuer (tcgen05.mma kind::tf32, M=128 N=128 K=8; A resident in TMEM, B MN-major), TMEM owner
-//   TW warps   transform: raw slot -> lo slot
-//   EW warps   epilogue: tcgen05.ld of this warp's lane quadrant x 64 columns, hi/lo row halves folded by a
-//              half-warp exchange in which each half keeps 32 columns (one full 128-byte line per lane), 256-bit stores.
-//              (One merged worker group doing transform(it) then epilogue(it-1) serialised transform -> MMA ->
-//              epilogue into one chain: 1.5 us per two-input tile against 0.6 us of tensor time.)
-// The raw ring is deeper than the lo ring: a raw slot is busy from the TMA issue to the end of its MMAs (one HBM
-// latency + transform + MMA), a lo slot only from the transform to the end of the MMAs, and the bytes in flight
-// from HBM -- what bounds this kernel -- are the raw slots alone.  TMEM accumulators are double-buffered.
+// CTA = 2 consumer warpgroups + 1 TMA producer warp, one per SM, persistent over a contiguous range of 64-pixel
+// tiles of one (domain, super-block):
+//   warp 8      TMA producer into a ring (per input 2 boxes of 32 px x 64 ch, SWIZZLE_128B)
+//   warps 0-7   two consumer warpgroups taking alternate tiles: load the tile into registers (hi / lo split),
+//               release the stage, 4 x 8 wgmma m64n64k8 per input, then store the 64 x 64 output block.
 //
-// Round 2: a third accumulator changed nothing (292 / 443 us against 290-296 / 435-456 us).  A second MMA-issuing warp
-// (alternate tiles; the one thread issuing 16 / 32 tcgen05.mma + 3 / 5 tcgen05.commit per tile is ~4100 cycles per
-// two-input tile against 4150 at the HBM rate) needs per-issuer lo rings and accumulators: with the shared 2-slot lo
-// ring an issuer that skips the other's tiles meets mbarrier phases two steps away from its own count (parity waits are
-// only meaningful one phase away) -- it faulted on the full-size tensor and was backed out; the Gram kernel, whose
-// rings are deep, runs with two issuers (norm_tc.cu).
-//
-// Measured ceilings on B200 (N=256, C=256, 56x56, profiles/tc_apply_experiments_r01.md): TMA loads alone 0.96 of
-// the HBM peak; a pure TMA load->store copy in this tile order 0.88-0.91.
-//
-// Reference: the grouped 1x1 convolution at utils/whitening.py:55 (/root/reference) and its backward.
+// Reference: the grouped 1x1 convolution at utils/whitening.py:55 of the reference project and its backward.
 #include <cuda.h>
 #include <cstdlib>
 
@@ -55,33 +38,25 @@ using namespace tc;
 
 constexpr int kBoxPx = 32, kCh = 64;
 constexpr int kBoxBytes = kCh * kBoxPx * 4;          // 8192
-constexpr int kMatCols = 64;                         // TMEM columns per resident matrix
-constexpr int kMaxRaw = 6, kLo = 2;
+constexpr int kTilePx = 64, kNBox = kTilePx / kBoxPx;
+constexpr int kMatBytes = kCh * kCh * 4;             // one 64x64 matrix: two K halves of [64 rows x 128 B]
+constexpr int kConsumers = 2;
+constexpr int kProducerWarp = 4 * kConsumers;
+constexpr int kApThreads = 128 * kConsumers + 32;
+constexpr int kMaxStages = 6;
 
-// One STEP = one input tensor's [64 ch x 128 px] tile: a raw ring slot filled by TMA, a lo ring slot filled by the
-// transform warps, 16 MMAs (2 terms x 8 k-steps of N = 128) accumulating into the tile's TMEM accumulator.
-// N = 128 because a tcgen05.mma costs its issuing thread ~90 cycles whatever its N: with N = 64 the one warp
-// issuing 32 MMAs per two-input tile was 90 % busy while the tensor pipe was 35 % active and the kernel ran at 0.70 of
-// the HBM peak; N = 128 halves the instruction count per pixel (0.84).  The one-input kernel is bound by its memory
-// access pattern either way (same time at N = 64 with two CTAs per SM) and shares the configuration:
-//   5 raw + 2 lo slots of 32 KB = 225 KB, 2 + 8 + 8 warps, one CTA per SM, 512 TMEM columns
+//   one input:  6 stages of 16 KB + hi / lo matrix (32 KB) = 129 KB
+//   two inputs: 4 stages of 32 KB + 2 hi / lo matrices (64 KB) = 193 KB
 template <int NIN> struct ApCfg {
-  static constexpr int TPX = 128;
-  static constexpr int NBOX = TPX / kBoxPx;
-  static constexpr int TW = 8;                         // transform warps
-  static constexpr int EW = 8;                         // epilogue warps
-  static constexpr int THREADS = 64 + 32 * (TW + EW);
-  static constexpr int RAW = 5;
-  static constexpr int SLOT = NBOX * kBoxBytes;
-  static constexpr int TMEM = 512;                     // 2 accumulators of TPX columns + NIN matrices of 64
-  static constexpr size_t SMEM = (size_t)(RAW + kLo) * SLOT + 1024;
+  static constexpr int STAGES = NIN == 1 ? 6 : 4;
+  static constexpr int SLOT = NIN * kNBox * kBoxBytes;
+  static constexpr size_t SMEM = (size_t)STAGES * SLOT + (size_t)2 * NIN * kMatBytes + 1024;
+  static_assert(STAGES % kConsumers == 0 && STAGES <= kMaxStages, "stage ownership");
 };
 
 struct ApBarriers {
-  uint64_t full[kMaxRaw], raw_empty[kMaxRaw];       // TMA landed / MMAs done with the raw slot
-  uint64_t ready[kLo], lo_empty[kLo];               // lo slot written / MMAs done with it
-  uint64_t acc_full[2], acc_empty[2];
-  uint32_t tmem_slot;
+  uint64_t full[kMaxStages];       // TMA landed the stage
+  uint64_t empty[kMaxStages];      // the owning warpgroup holds the tile in registers (one arrival per warp)
 };
 
 // DWT_TC_INTERLEAVE=0/1 (development): tile order of the apply kernels
@@ -100,55 +75,37 @@ struct ApplyArgs {
   int interleave;         // 1: CTA b takes tiles b, b + grid, b + 2 grid, ... (neighbouring CTAs on neighbouring tiles)
 };
 
-// 128-bit shared-memory accesses with the state space spelled out: through a generic pointer these compile to
-// LD.E/ST.E (address-space check per access, global-load latency class); LDS/STS is what the transform wants.
-__device__ __forceinline__ float4 lds128(uint32_t addr) {
-  float4 v;
-  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
+__device__ __forceinline__ float lds32(uint32_t addr) {
+  float v;
+  asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr));
   return v;
 }
-__device__ __forceinline__ void sts128(uint32_t addr, float a, float b, float c, float d) {
-  asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
+
+// Byte offset of element (row, k) in a [64 rows x 64 K] K-major, 128-byte-swizzled operand: two K halves of
+// [64 rows x 32 tf32] (8 KB each), 16-byte chunk (k % 32) / 4 of a row XOR-ed with row % 8.
+__device__ __forceinline__ uint32_t kmajor_off(int row, int k) {
+  return (uint32_t)((k >> 5) * (kCh * 128) + row * 128 + ((((k & 31) >> 2) ^ (row & 7)) << 4) + (k & 3) * 4);
+}
+// Byte offset of (channel ch, pixel p) in the landed tile of one input: box p / 32 is [64 ch x 128 B], SWIZZLE_128B.
+__device__ __forceinline__ uint32_t tile_off(int ch, int p) {
+  const int pp = p & 31;
+  return (uint32_t)((p >> 5) * kBoxBytes + ch * 128 + (((pp >> 2) ^ (ch & 7)) << 4) + (pp & 3) * 4);
 }
 
-// lo = RN_tf32(v - trunc_tf32(v)) (the subtraction is exact) of one landed 32 px x 64 ch box by the 256 worker
-// threads (tt = 0..NT-1): chunk q = tt + NT i (16 bytes), same swizzled position in the lo slot.
-template <int NT>
-__device__ __forceinline__ void lo_box(uint32_t raw, uint32_t lo, int tt) {
-  constexpr int PER = 512 / NT;
-  float4 v[PER];
-#pragma unroll
-  for (int i = 0; i < PER; ++i) v[i] = lds128(raw + 16u * (tt + NT * i));
-#pragma unroll
-  for (int i = 0; i < PER; ++i) {
-    const float e[4] = {v[i].x, v[i].y, v[i].z, v[i].w};
-    float l[4];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) l[k] = round_tf32(e[k] - __uint_as_float(__float_as_uint(e[k]) & 0xFFFFE000u));
-    sts128(lo + 16u * (tt + NT * i), l[0], l[1], l[2], l[3]);
-  }
-}
-
-// The A operand lives in TENSOR MEMORY for the whole kernel (it is the same for every tile; reading
-// it from shared memory on every MMA was the largest shared-memory consumer of the first version).
-// Row order: TMEM lane 32q + l holds channel 16q + (l & 15), the hi part for l < 16 and the lo part
-// for l >= 16, so the two halves that must be added end up 16 lanes apart IN THE SAME WARP and the
-// epilogue folds them with one shuffle per value -- no shared-memory staging at all.
 template <int NIN>
-__global__ void __launch_bounds__(ApCfg<NIN>::THREADS, 1)
+__global__ void __launch_bounds__(kApThreads, 1)
 tc_apply_kernel(const __grid_constant__ CUtensorMap map0, const __grid_constant__ CUtensorMap map1, const Geom gm,
                 const ApplyArgs args) {
   using Cfg = ApCfg<NIN>;
-  constexpr int RAW = Cfg::RAW, SLOT = Cfg::SLOT, TW = Cfg::TW, EW = Cfg::EW, TPX = Cfg::TPX, NBOX = Cfg::NBOX;
+  constexpr int STAGES = Cfg::STAGES, SLOT = Cfg::SLOT;
   extern __shared__ __align__(1024) uint8_t smem_dyn[];
-  uint8_t* sRaw = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
-  uint8_t* sLo = sRaw + (size_t)RAW * SLOT;
+  uint8_t* sRing = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
+  uint8_t* sMat = sRing + (size_t)STAGES * SLOT;     // [NIN][hi, lo][kMatBytes]
   __shared__ ApBarriers bars;
   __shared__ float sShift[2][kCh];
-  __shared__ float sConst[kCh];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, tid = threadIdx.x;
   const int sb = blockIdx.y, d = blockIdx.z, ch0 = sb * kCh;
-  const int PB = (gm.HW + TPX - 1) / TPX;
+  const int PB = (gm.HW + kTilePx - 1) / kTilePx;
   const long long T = (long long)gm.N * PB;
   // tile of step `it`: a contiguous range per CTA, or (interleave) the CTAs of a super-block walk the tensor side by side
   const int t_step = args.interleave ? (int)gridDim.x : 1;
@@ -157,169 +114,109 @@ tc_apply_kernel(const __grid_constant__ CUtensorMap map0, const __grid_constant_
                                      : (int)(T * (blockIdx.x + 1) / gridDim.x) - t_begin;
 
   if (tid == 0) {
-    for (int r = 0; r < RAW; ++r) { mbar_init(&bars.full[r], 1); mbar_init(&bars.raw_empty[r], 1); }
-    for (int l = 0; l < kLo; ++l) { mbar_init(&bars.ready[l], TW); mbar_init(&bars.lo_empty[l], 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(&bars.acc_full[b], 1); mbar_init(&bars.acc_empty[b], EW); }
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&bars.full[s], 1); mbar_init(&bars.empty[s], 4); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) tmem_alloc<Cfg::TMEM>(&bars.tmem_slot);
   if (tid < NIN * kCh) {
     const int i = tid / kCh, r = tid - i * kCh, c = ch0 + r;
     sShift[i][r] = (c < gm.C && args.shift[i] != nullptr) ? __ldg(args.shift[i] + (size_t)d * args.shift_stride[i] + c) : 0.f;
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = bars.tmem_slot;
-  const uint32_t tmem_acc = tmem, tmem_mat = tmem + 2 * TPX;
 
-  if (warp >= 2 + TW && warp < 6 + TW) {
-    // four of the epilogue warps first park the split matrices in tensor memory and form the row constants
-    const int quad = warp & 3, i = 16 * quad + (lane & 15), GS = gm.GS, gi = i / GS, g = sb * (kCh / GS) + gi;
-    const bool lo_half = lane >= 16;
-    float rc = 0.f;                       // (sum_m M_m shift_m)[row i], full fp32 matrix entries
-    for (int m = 0; m < NIN; ++m) {
-      const float* rec = args.mats + ((size_t)d * gm.G + (g < gm.G ? g : 0)) * args.rec_stride + args.off[m] + (i - gi * GS) * GS;
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        float v[32];
-#pragma unroll
-        for (int c = 0; c < 32; ++c) {
-          const int k = h * 32 + c;
-          float w = 0.f;
-          if (g < gm.G && k / GS == gi) w = __ldg(rec + (k - gi * GS));
-          rc = fmaf(w, sShift[m][k], rc);
-          const float hi = round_tf32(w);
-          v[c] = lo_half ? round_tf32(w - hi) : hi;
-        }
-        tmem_st32(tmem_mat + m * kMatCols + ((uint32_t)(quad * 32) << 16) + h * 32, v);
-      }
-    }
-    if (!lo_half) sConst[i] = rc;
-    tc_fence_before();
+  // block-diagonal entry (row n, column k) of matrix m of this super-block, full fp32
+  auto entry = [&](int m, int n, int k) {
+    const int GS = gm.GS, gi = n / GS, g = sb * (kCh / GS) + gi;
+    if (g >= gm.G || k / GS != gi) return 0.f;
+    return __ldg(args.mats + ((size_t)d * gm.G + g) * args.rec_stride + args.off[m] + (n - gi * GS) * GS + (k - gi * GS));
+  };
+  // the split matrices as the B operand, resident for the whole kernel
+  for (int e = tid; e < NIN * kCh * kCh; e += kApThreads) {
+    const int m = e / (kCh * kCh), n = (e / kCh) % kCh, k = e % kCh;
+    const float w = entry(m, n, k), hi = round_tf32(w);
+    const uint32_t o = kmajor_off(n, k);
+    *reinterpret_cast<float*>(sMat + (size_t)(2 * m) * kMatBytes + o) = hi;
+    *reinterpret_cast<float*>(sMat + (size_t)(2 * m + 1) * kMatBytes + o) = round_tf32(w - hi);
   }
+  fence_proxy_async();
   __syncthreads();
-  tc_fence_after();
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     // ===== TMA producer =====
     if (lane == 0) {
       for (int it = 0; it < ntiles; ++it) {
-        const int t = t_begin + it * t_step, n = t / PB, pb = t - n * PB;
-        // 32-pixel boxes of the tile that lie entirely past the row end are not issued (their columns are never
-        // stored, whatever the stale shared memory holds)
-        int nbox = (gm.HW - pb * TPX + kBoxPx - 1) / kBoxPx;
-        nbox = nbox < NBOX ? nbox : NBOX;
+        const int t = t_begin + it * t_step, n = t / PB, pb = t - n * PB, s = it % STAGES;
+        // 32-pixel boxes of the tile that lie entirely past the row end are not issued (they only feed output
+        // pixels that are never stored, whatever the stale shared memory holds)
+        int nbox = (gm.HW - pb * kTilePx + kBoxPx - 1) / kBoxPx;
+        nbox = nbox < kNBox ? nbox : kNBox;
+        mbar_wait_relaxed(&bars.empty[s], ((it / STAGES) & 1) ^ 1);
+        mbar_arrive_expect_tx(&bars.full[s], NIN * nbox * kBoxBytes);
+        uint8_t* dst = sRing + (size_t)s * SLOT;
 #pragma unroll
-        for (int i = 0; i < NIN; ++i) {
-          const int st = it * NIN + i, r = st % RAW;
-          mbar_wait_relaxed(&bars.raw_empty[r], ((st / RAW) & 1) ^ 1);
-          uint8_t* dst = sRaw + (size_t)r * SLOT;
-          mbar_arrive_expect_tx(&bars.full[r], nbox * kBoxBytes);
+        for (int i = 0; i < NIN; ++i)
           for (int j = 0; j < nbox; ++j)
-            tma_load_3d(dst + j * kBoxBytes, i == 0 ? &map0 : &map1, pb * TPX + j * kBoxPx, ch0, d * gm.N + n, &bars.full[r]);
-        }
+            tma_load_3d(dst + (i * kNBox + j) * kBoxBytes, i == 0 ? &map0 : &map1, pb * kTilePx + j * kBoxPx, ch0,
+                        d * gm.N + n, &bars.full[s]);
       }
-    }
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    constexpr uint32_t idesc = make_idesc_tf32(128, TPX, true);
-    for (int it = 0; it < ntiles; ++it) {
-      const int b = it & 1, aph = (it >> 1) & 1;
-      mbar_wait(&bars.acc_empty[b], aph ^ 1);
-#pragma unroll
-      for (int i = 0; i < NIN; ++i) {
-        const int st = it * NIN + i, r = st % RAW, l = st % kLo;
-        mbar_wait(&bars.full[r], (st / RAW) & 1);             // already complete (the transform warps waited on it)
-        mbar_wait(&bars.ready[l], (st / kLo) & 1);
-        tc_fence_after();
-        // operands are warp-uniform and computed by every lane; ONE elected lane issues (tc_ptx.cuh elect_one: without it
-        // the compiler wrapped every tcgen05 instruction in its own election loop with four register-to-uniform moves)
-        const uint32_t raw = smem_u32(sRaw + (size_t)r * SLOT), lo = smem_u32(sLo + (size_t)l * SLOT);
-        if (elect_one()) {
-#pragma unroll
-          for (int term = 0; term < 2; ++term) {                 // B = raw tile (hi by truncation), then lo
-            const uint32_t bbase = term == 0 ? raw : lo;
-#pragma unroll
-            for (int ks = 0; ks < kCh / 8; ++ks) {
-              const uint64_t bdesc = make_mnmajor_sw128_32b_desc(bbase + ks * 1024, kBoxBytes, 512);
-              umma_tf32_ts(tmem_acc + b * TPX, tmem_mat + i * kMatCols + ks * 8, bdesc, idesc,
-                           (i == 0 && term == 0 && ks == 0) ? 0u : 1u);
-            }
-          }
-          umma_commit(&bars.raw_empty[r]);
-          umma_commit(&bars.lo_empty[l]);
-          if (i == NIN - 1) umma_commit(&bars.acc_full[b]);
-        }
-        __syncwarp();
-      }
-    }
-  } else if (warp < 2 + TW) {
-    // ===== transform warps: raw slot -> lo slot, one step at a time =====
-    const int tt = tid - 64;
-    const uint32_t raw0 = smem_u32(sRaw), lo0 = smem_u32(sLo);
-    for (int st = 0; st < ntiles * NIN; ++st) {
-      const int r = st % RAW, l = st % kLo;
-      mbar_wait(&bars.full[r], (st / RAW) & 1);
-      mbar_wait(&bars.lo_empty[l], ((st / kLo) & 1) ^ 1);
-      const uint32_t raw = raw0 + (uint32_t)(r * SLOT), lo = lo0 + (uint32_t)(l * SLOT);
-#pragma unroll
-      for (int j = 0; j < NBOX; ++j) lo_box<32 * TW>(raw + j * kBoxBytes, lo + j * kBoxBytes, tt);
-      fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bars.ready[l]);
     }
   } else {
-    // ===== epilogue warps =====
-    constexpr int WC = TPX / (EW / 4), KEEP = WC / 2;  // accumulator columns per warp / per lane after the fold
-    const int quad = warp & 3;                     // TMEM lane quadrant this warp may read
-    const int part = (warp - 2 - TW) >> 2;         // which WC accumulator columns this warp drains
-    const bool upper = lane >= 16;                 // lanes 16-31 hold the lo-matrix rows
-    const int ch = ch0 + 16 * quad + (lane & 15);
-    const float rconst = sConst[16 * quad + (lane & 15)];   // sum_i (M_i shift_i)[row]: the centring, applied at the end
-    for (int e = 0; e < ntiles; ++e) {
-      const int b = e & 1, aph = (e >> 1) & 1;
-      mbar_wait(&bars.acc_full[b], aph);
-      tc_fence_after();
-      float v[WC];
-      tmem_ld_cols<WC>(tmem_acc + ((uint32_t)(quad * 32) << 16) + b * TPX + part * WC, v);
-      tc_fence_before();
+    // ===== consumer warpgroups: D[64 px x 64 ch] = sum_i tile_i^T M_i^T =====
+    const int wg = warp >> 2;
+    // A fragment (tf32 m64k8): a[r] = element (pixel 16 w + l/4 + 8 (r & 1), channel k0 + l%4 + 4 (r >> 1)) of warp w
+    // D fragment: d[4 j + r] = (pixel 16 w + l/4 + 8 (r >> 1), channel 8 j + 2 (l%4) + (r & 1))
+    const int prow = 16 * (warp & 3) + (lane >> 2), kq = lane & 3;
+    const uint32_t mat0 = smem_u32(sMat);
+    for (int it = wg; it < ntiles; it += kConsumers) {
+      const int s = it % STAGES;
+      mbar_wait(&bars.full[s], (it / STAGES) & 1);
+      const uint32_t slot = smem_u32(sRing + (size_t)s * SLOT);
+      uint32_t ahi[NIN][kCh / 8][4], alo[NIN][kCh / 8][4];
+#pragma unroll
+      for (int i = 0; i < NIN; ++i)
+#pragma unroll
+        for (int ks = 0; ks < kCh / 8; ++ks)
+#pragma unroll
+          for (int r = 0; r < 4; ++r) {
+            const int k = 8 * ks + kq + 4 * (r >> 1);
+            const float v = lds32(slot + i * kNBox * kBoxBytes + tile_off(k, prow + 8 * (r & 1))) - sShift[i][k];
+            const uint32_t h = __float_as_uint(v) & kTf32Mask;
+            ahi[i][ks][r] = h;
+            alo[i][ks][r] = __float_as_uint(round_tf32(v - __uint_as_float(h)));
+          }
       __syncwarp();
-      if (lane == 0) mbar_arrive(&bars.acc_empty[b]);          // this warp's share is drained
-      // lanes l and l+16 hold the hi- and lo-matrix rows of one channel: the lower lane keeps the first half of
-      // the summed columns, the upper lane the second half, each sending the other the values it does not keep
-      float o[KEEP];
+      if (lane == 0) mbar_arrive(&bars.empty[s]);   // the tile is in registers: the stage can be refilled
+      float acc[32];
 #pragma unroll
-      for (int c = 0; c < KEEP; ++c) {
-        const float keep = upper ? v[KEEP + c] : v[c];
-        const float send = upper ? v[c] : v[KEEP + c];
-        o[c] = (keep + __shfl_xor_sync(0xffffffffu, send, 16)) - rconst;
-      }
-      const int t = t_begin + e * t_step, n = t / PB, pb = t - n * PB;
-      const int px = pb * TPX + part * WC + (upper ? KEEP : 0);
-      if (ch < gm.C) {
-        float* orow = args.out + ((size_t)(d * gm.N + n) * gm.C + ch) * gm.HW + px;
-        if ((gm.HW & 7) == 0) {
-          // 256-bit stores (sm_100 STG.256): every instruction writes whole 32-byte sectors of this lane's row;
-          // 128-bit stores left half-written sectors behind (2x the L2 write traffic)
+      for (int j = 0; j < 32; ++j) acc[j] = 0.f;
+      wgmma_fence();
+      fence_operands(acc);
 #pragma unroll
-          for (int c8 = 0; c8 < KEEP / 8; ++c8)
-            if (px + 8 * c8 < gm.HW)
-              asm volatile("st.global.v8.f32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(orow + 8 * c8),
-                           "f"(o[8 * c8]), "f"(o[8 * c8 + 1]), "f"(o[8 * c8 + 2]), "f"(o[8 * c8 + 3]),
-                           "f"(o[8 * c8 + 4]), "f"(o[8 * c8 + 5]), "f"(o[8 * c8 + 6]), "f"(o[8 * c8 + 7]) : "memory");
-        } else {
+      for (int i = 0; i < NIN; ++i)
 #pragma unroll
-          for (int c4 = 0; c4 < KEEP / 4; ++c4)
-            if (px + 4 * c4 < gm.HW)
-              *reinterpret_cast<float4*>(orow + 4 * c4) = make_float4(o[4 * c4], o[4 * c4 + 1], o[4 * c4 + 2], o[4 * c4 + 3]);
+        for (int ks = 0; ks < kCh / 8; ++ks) {
+          // k-step ks: K half ks / 4, 32 bytes further per step inside the 128-byte row
+          const uint32_t koff = (uint32_t)((ks >> 2) * (kCh * 128) + (ks & 3) * 32);
+          const uint64_t bhi = make_kmajor_sw128_desc(mat0 + (uint32_t)(2 * i) * kMatBytes + koff);
+          const uint64_t blo = make_kmajor_sw128_desc(mat0 + (uint32_t)(2 * i + 1) * kMatBytes + koff);
+          wgmma_m64n64k8_rs(acc, ahi[i][ks], bhi);
+          wgmma_m64n64k8_rs(acc, ahi[i][ks], blo);
+          wgmma_m64n64k8_rs(acc, alo[i][ks], bhi);
+          wgmma_m64n64k8_rs(acc, alo[i][ks], blo);
         }
-      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_operands(acc);
+      const int t = t_begin + it * t_step, n = t / PB, pb = t - n * PB;
+      float* obase = args.out + (size_t)(d * gm.N + n) * gm.C * gm.HW;
+#pragma unroll
+      for (int j = 0; j < kCh / 8; ++j)
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+          const int c = 8 * j + 2 * kq + (r & 1), px = pb * kTilePx + prow + 8 * (r >> 1);
+          if (ch0 + c < gm.C && px < gm.HW) obase[(size_t)(ch0 + c) * gm.HW + px] = acc[4 * j + r];
+        }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc<ApCfg<NIN>::TMEM>(tmem); }
 }
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -333,7 +230,7 @@ int make_map_ap(CUtensorMap* map, const float* base, const Geom& gm) {
   const cuuint32_t box[3] = {kBoxPx, kCh, 1};
   const cuuint32_t estr[3] = {1, 1, 1};
   return (int)g_encode_ap(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(base), dims, strides, box, estr,
-                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
 }
 
@@ -349,7 +246,7 @@ int tc_apply_init() {
   g_encode_ap = reinterpret_cast<EncodeTiledFn>(fn);
   e = cudaFuncSetAttribute(tc_apply_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ap_smem<1>());
   if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_apply_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ap_smem<2>());
-  // a 225 KB CTA needs the full shared-memory carve-out
+  // a 129 / 193 KB CTA needs the full shared-memory carve-out
   if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_apply_kernel<1>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_apply_kernel<2>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   return (int)e;
@@ -367,7 +264,7 @@ int tc_apply(const float* x, float* y, const Geom& gm, int nctas, const float* s
   a.shift[0] = save_mean; a.shift_stride[0] = gm.C; a.shift[1] = nullptr; a.shift_stride[1] = 0;
   a.out = y;
   dim3 grid(nctas, (gm.C + kCh - 1) / kCh, gm.D);
-  tc_apply_kernel<1><<<grid, ApCfg<1>::THREADS, ap_smem<1>(), st>>>(mx, mx, gm, a);
+  tc_apply_kernel<1><<<grid, kApThreads, ap_smem<1>(), st>>>(mx, mx, gm, a);
   return 0;
 }
 
@@ -385,7 +282,7 @@ int tc_bwd_apply(const float* x, const float* dout, float* dx, const Geom& gm, i
   a.shift[1] = save_mean; a.shift_stride[1] = gm.C;
   a.out = dx;
   dim3 grid(nctas, (gm.C + kCh - 1) / kCh, gm.D);
-  tc_apply_kernel<2><<<grid, ApCfg<2>::THREADS, ap_smem<2>(), st>>>(mg, mx, gm, a);
+  tc_apply_kernel<2><<<grid, kApThreads, ap_smem<2>(), st>>>(mg, mx, gm, a);
   return 0;
 }
 

@@ -1,5 +1,5 @@
 // Shared-memory tiled path for any group size up to 64 (the general-shape path: group
-// sizes the register-resident kernels do not cover, and shapes the TMA/tcgen05 kernels
+// sizes the register-resident kernels do not cover, and shapes the TMA/wgmma kernels
 // cannot take, e.g. H*W not a multiple of 4).
 //
 // The flattened sample axis m = n*HW + p is cut into tiles of TP samples; a CTA stages a

@@ -1,9 +1,8 @@
 // Channels-last max-pool, forward + backward: the op that sits between the stem whitening site and layer1
 // (`x = self.maxpool(self.relu(...))`, resnet50_dwt_mec_officehome.py:337-338; nn.MaxPool2d(3, 2, 1) at :295).
 //
-// Why it is here: on B200 the stock ATen kernels for this op in NHWC fp32 (max_pool_forward_nhwc 0.65 ms,
-// max_pool_backward_nhwc 1.31 ms, int64 argmax map of 308 MB) cost 5 % of the whole ResNet-50-DWT step
-// (profiles/launches_r02_step.md) for 1.1 GB of algorithmic traffic = 0.17 ms at the HBM peak.  Both passes here
+// Why it is here: the stock ATen kernels for this op in NHWC fp32 (max_pool_forward_nhwc, max_pool_backward_nhwc
+// with an int64 argmax map of 308 MB) take many times what 1.1 GB of algorithmic traffic needs.  Both passes here
 // are pure gathers -- no atomics, deterministic:
 //   forward   one CTA per output row, one thread per output float4 (4 channels of one output pixel): k*k coalesced
 //             float4 loads (a warp covers whole pixels: C/4 consecutive float4), max with ATen's rule (strict >, NaN wins, first maximum

@@ -1,6 +1,5 @@
-// Inline-PTX wrappers for the Blackwell async machinery used by the tensor-core kernels:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld / fences) and the
-// shared-memory / instruction descriptors of cute::UMMA (layouts restated from the CUTLASS headers).
+// Inline-PTX wrappers for the Hopper async machinery used by the tensor-core kernels: mbarrier, TMA
+// (cp.async.bulk.tensor), warpgroup MMA (wgmma.mma_async kind tf32) and its shared-memory matrix descriptor.
 #pragma once
 #include <cuda.h>
 #include <stdint.h>
@@ -23,7 +22,7 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t by
 }
 // Waits fail instead of hanging the GPU: a protocol bug traps after kWaitTimeoutNs of wall time (%globaltimer, read
 // every 256 polls), however long a single poll lasts.
-constexpr uint32_t kSuspendHintNs = 20000u;    // measured: no effect on B200 (168.4 us with and without), kept as a hint
+constexpr uint32_t kSuspendHintNs = 20000u;    // upper bound on one hardware-suspended poll
 constexpr unsigned long long kWaitTimeoutNs = 4000000000ull;
 __device__ __forceinline__ unsigned long long global_ns() {
   unsigned long long t;
@@ -84,118 +83,50 @@ __device__ __forceinline__ uint64_t l2_policy_evict_first() {
   return p;
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-template <int COLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* slot) {     // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot)), "n"(COLS) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int COLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {   // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(COLS) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]^T, tf32 inputs, fp32 accumulate
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-               "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-               ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// same with the A operand resident in tensor memory (lane = row, one 32-bit column per K element)
-// one lane of a fully active, converged warp (elect.sync): the compiler keeps warp-uniform operands of the tcgen05
-// instructions inside such a region in uniform registers instead of broadcasting them per instruction
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void umma_tf32_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  const uint32_t z = 0;
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-               "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, {%5, %6, %7, %8}, p;\n\t}"
-               ::"r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(z), "r"(z), "r"(z), "r"(z) : "memory");
-}
-// registers -> 32 lanes x 32 consecutive columns of tensor memory (thread L writes TMEM lane base+L)
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const float (&v)[32]) {
-  uint32_t r[32];
+// ---- warpgroup MMA (wgmma, sm_90a): issued by all 128 threads of an aligned warpgroup, fp32 accumulator in registers
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMA
+template <int N>
+__device__ __forceinline__ void fence_operands(float (&d)[N]) {
 #pragma unroll
-  for (int i = 0; i < 32; ++i) r[i] = __float_as_uint(v[i]);
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-        "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]),
-        "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]),
-        "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31]) : "memory");
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// 32 lanes x 32 consecutive columns -> 32 registers per thread (thread L gets TMEM lane base+L)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-  uint32_t r[32];
+// named barrier over the 128 threads of one warpgroup (id 1 + warpgroup index; id 0 is __syncthreads)
+__device__ __forceinline__ void warpgroup_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
+
+// D[64 x 64] += A[64 x 8] * B[64 x 8]^T, both operands K-major in shared memory (descriptors)
+__device__ __forceinline__ void wgmma_m64n64k8_ss(float (&d)[32], uint64_t da, uint64_t db) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db));
 }
 
-// 32 lanes x 16 consecutive columns
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
+// D[64 x 64] += A[64 x 8] * B[64 x 8]^T, A from registers (tf32 fragment), B K-major in shared memory
+__device__ __forceinline__ void wgmma_m64n64k8_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t db) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db));
 }
-template <int COLS> __device__ __forceinline__ void tmem_ld_cols(uint32_t taddr, float (&v)[COLS]);
-template <> __device__ __forceinline__ void tmem_ld_cols<32>(uint32_t taddr, float (&v)[32]) { tmem_ld32(taddr, v); }
-template <> __device__ __forceinline__ void tmem_ld_cols<64>(uint32_t taddr, float (&v)[64]) {
-  tmem_ld32(taddr, reinterpret_cast<float(&)[32]>(v[0]));
-  tmem_ld32(taddr + 32, reinterpret_cast<float(&)[32]>(v[32]));
-}
-template <> __device__ __forceinline__ void tmem_ld_cols<16>(uint32_t taddr, float (&v)[16]) { tmem_ld16(taddr, v); }
 
-// K-major SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): start address
-// >> 4, LBO = 1 (unused with swizzle), SBO = 1024 B between 8-row groups, version 1, layout type 2.
+// K-major SWIZZLE_128B shared-memory matrix descriptor (wgmma): start address >> 4, LBO = 1 (unused with swizzle),
+// SBO = 1024 B between 8-row groups, layout type 1 (128-byte swizzle) in bits 62-63.  A row is 128 B = 32 tf32 along K;
+// the k-th group of 8 tf32 starts 32 B further (descriptor + 2 * k).  The atom base must be 1024-byte aligned.
 __device__ __forceinline__ uint64_t make_kmajor_sw128_desc(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) |
-         ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
-}
-// MN-major descriptor for 32-bit (tf32) operands.  The ONLY shared-memory layout the tensor core accepts
-// for MN-major tf32 is SWIZZLE_128B_BASE32B (cute::UMMA::Layout_MN_SW128_32B_Atom, layout type 1):
-// rows of 128 B (32 elements along M/N), 32-byte chunks XOR-swizzled by (row & 3), K atoms of 4 rows.
-// TMA writes exactly this with CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B.  LBO = stride between 32-element
-// blocks along M/N, SBO = stride between 4-row groups along K.
-__device__ __forceinline__ uint64_t make_mnmajor_sw128_32b_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) |
-         ((uint64_t)1 << 46) | ((uint64_t)1 << 61);
-}
-// Instruction descriptor (cute::UMMA::InstrDescriptor): D = F32, A = B = TF32, A K-major, M x N;
-// b_mn_major selects an MN-major (transposed) B operand.
-__host__ __device__ constexpr uint32_t make_idesc_tf32(int M, int N, bool b_mn_major = false) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((b_mn_major ? 1u : 0u) << 16) | ((uint32_t)(N >> 3) << 17) |
-         ((uint32_t)(M >> 4) << 24);
+  return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 62);
 }
 // Round to the nearest tf32 (10 explicit mantissa bits), ties away from zero, on the integer ALU:
-// cvt.rna.tf32.f32 is a conversion-pipe instruction (a quarter of the FP32 issue rate) and the
-// transform warps round every element of every tile.
+// cvt.rna.tf32.f32 is a conversion-pipe instruction and the transform rounds every element of every tile.
+constexpr uint32_t kTf32Mask = 0xFFFFE000u;     // sign, exponent and the 10 mantissa bits a tf32 operand keeps
 __device__ __forceinline__ float round_tf32(float v) {
   return __uint_as_float((__float_as_uint(v) + 0x1000u) & 0xFFFFE000u);
 }

@@ -3,7 +3,7 @@
 ``MaxPool2d(kernel_size, stride, padding)`` stands where the reference model has ``nn.MaxPool2d(kernel_size=3,
 stride=2, padding=1)`` (resnet50_dwt_mec_officehome.py:295, applied right behind the stem whitening site at :337-338).
 Same results as the stock op bit for bit (ties, NaN, gradient routing); one byte of argmax per output element instead of
-an int64.  It takes dense ``torch.channels_last`` CUDA tensors with C % 4 == 0 only -- the layout the B200 step runs
+an int64.  It takes dense ``torch.channels_last`` CUDA tensors with C % 4 == 0 only -- the layout the benchmark step runs
 in; anything else raises (build the model with ``nn.MaxPool2d`` for NCHW).
 """
 from __future__ import annotations

@@ -1,5 +1,5 @@
 """Drop-in for the reference's ``utils/whitening.py`` (same class names, constructor and
-forward signatures, attributes, buffers and error texts), computing on hand-written sm_100a
+forward signatures, attributes, buffers and error texts), computing on hand-written sm_90a
 kernels through libdwt_b200.so.
 
 Reference: /root/reference/utils/whitening.py:5-71.

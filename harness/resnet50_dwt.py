@@ -153,16 +153,16 @@ class ResNet50DWT(_SiteOwner):
         # stem_s2d: evaluate the 7x7 / stride-2 / pad-3 stem convolution as the 4x4 / stride-1 convolution of the 2x2
         # space-to-depth rearrangement of the image (12 channels) -- see _stem_s2d.  Same sums of the same products; the
         # 12-channel operand gives cuDNN a tensor-core implicit-GEMM kernel where the 3-channel one only has legacy
-        # engines (2.0 ms forward + 2.2 ms weight gradient per step on B200, profiles/launches_r02_step.md).
+        # engines.
         self.stem_s2d = stem_s2d
         # stem_nchw: run ONLY the 3-channel 7x7 stem convolution in NCHW (its weight stays NCHW-contiguous, the image is
         # viewed / copied to NCHW, the 64-channel result is copied to channels-last once) -- cuDNN's NHWC engines for a
-        # 3-channel input are legacy kernels (profiles/launches_r02_step.md); same arithmetic, different cuDNN kernel
+        # 3-channel input are legacy kernels; same arithmetic, different cuDNN kernel
         self.stem_nchw = stem_nchw
         # stem_pad = 4 / 8: feed the 7x7 stem convolution a zero-padded 4- / 8-channel image and the equally padded
         # weight -- identical arithmetic (the extra products are exact zeros), but cuDNN has no tensor-core kernel for
-        # a 3-channel NHWC tensor and falls back to a legacy engine (2.0 ms forward + 2.2 ms weight gradient per
-        # step on B200, profiles/launches_r02_step.md).  The parameter keeps the reference's [64, 3, 7, 7] shape.
+        # a 3-channel NHWC tensor and falls back to a legacy engine.  The parameter keeps the reference's [64, 3, 7, 7]
+        # shape.
         self.stem_pad = stem_pad
         if site_mode not in ("modules", "fused"):
             raise ValueError("site_mode must be 'modules' or 'fused'")

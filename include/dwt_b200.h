@@ -1,11 +1,11 @@
 /*
- * dwt_b200.h -- C ABI of the B200-native DWT hot path (libdwt_b200.so).
+ * dwt_b200.h -- C ABI of the H100-native DWT hot path (libdwt_b200.so).
  *
  * Plain C, no torch types: raw device pointers, sizes, scalars, a caller-owned
  * workspace and a CUDA stream.  Every entry point is stream-ordered, never
  * synchronises the host, never allocates, and returns 0 on success or a negative
  * DWT_E_* code (text through dwt_last_error()).  There is NO CPU path: the library
- * only launches sm_100a kernels.
+ * only launches sm_90a kernels.
  *
  * What each entry point replaces in the reference (paths relative to
  * /root/reference; the reference has no FFI -- its "plugin boundary" is Python

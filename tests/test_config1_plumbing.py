@@ -1,59 +1,44 @@
 """BASELINE.json configs[0]: usps_mnist.py USPS->MNIST, group_size=4, 1 epoch -- plumbing.
 
-CPU side (build container, needs /root/reference): the UNMODIFIED reference script is driven end to end
-on synthetic dataset files, its `from whitening import WTransform2d` resolved by sys.path order to a
-stand-in directory (tests/support/port_utils) -- the same zero-edit mechanism that puts the CUDA layers
-under it on a B200 (INTEGRATION.md §1).  The LeNet restatement used on the GPU box is checked against
-the script's own LeNet.  GPU side: one epoch of the restated LeNet on the CUDA layers.
+CPU side: the LeNet restatement used on the GPU (harness/lenet_dwt.py) against the reference script's own LeNet,
+through the outputs that model gave on the same weights and batch (tests/golden/ref_lenet.npz, written by
+tests/golden/make_golden_models.py from the unmodified reference).  GPU side: one epoch of the restated LeNet on the
+CUDA layers.
 """
+import importlib.util
 import os
-import subprocess
-import sys
 
+import numpy as np
 import pytest
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = "/root/reference"
-SUPPORT = os.path.join(ROOT, "tests", "support")
-needs_ref = pytest.mark.skipif(not os.path.exists(os.path.join(REF, "usps_mnist.py")), reason="reference not mounted")
+GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
-@needs_ref
-@pytest.mark.timeout(900)
-def test_reference_script_runs_unmodified_on_synthetic_files(tmp_path):
-    from harness.synth_digits import write_digit_files
-    write_digit_files(str(tmp_path / "data"), seed=0)
-    work = tmp_path / "work"
-    work.mkdir()
-    env = dict(os.environ, CUDA_VISIBLE_DEVICES="", OMP_NUM_THREADS="4",
-               PYTHONPATH=os.pathsep.join([os.path.join(SUPPORT, "stubs"), os.path.join(SUPPORT, "port_utils"), ROOT]))
-    cmd = [sys.executable, os.path.join(REF, "usps_mnist.py"), "--group_size", "4", "--source", "usps", "--target",
-           "mnist", "--epochs", "1", "--num_workers", "0", "--log_interval", "4", "--seed", "1"]
-    res = subprocess.run(cmd, cwd=str(work), env=env, capture_output=True, text=True, timeout=800)
-    assert res.returncode == 0, res.stderr[-2000:]
-    assert "Train Epoch: 0" in res.stdout and "Test set: Classification loss" in res.stdout, res.stdout[-1000:]
+def golden_module():
+    spec = importlib.util.spec_from_file_location("make_golden_models", os.path.join(GOLDEN, "make_golden_models.py"))
+    mod = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(mod)
+    return mod
 
 
-@needs_ref
-def test_lenet_restatement_matches_reference_lenet(monkeypatch):
-    import importlib
+def test_lenet_restatement_matches_reference_lenet():
     import oracle.torch_port as port
     from harness.lenet_dwt import LeNetDWT
-    monkeypatch.syspath_prepend(os.path.join(SUPPORT, "port_utils"))
-    monkeypatch.syspath_prepend(os.path.join(SUPPORT, "stubs"))
-    monkeypatch.syspath_prepend(REF)
-    monkeypatch.chdir(REF)
-    script = importlib.import_module("usps_mnist")
-    torch.manual_seed(0)
-    ref = script.LeNet(group_size=4)
+    ref = np.load(os.path.join(GOLDEN, "ref_lenet.npz"))
     mine = LeNetDWT(port, group_size=4)
-    missing, unexpected = mine.load_state_dict(ref.state_dict(), strict=True)
-    x = torch.randn(16, 1, 28, 28)
-    ref.train(); mine.train()
-    assert torch.allclose(ref(x), mine(x), atol=1e-5)
-    ref.eval(); mine.eval()
-    assert torch.allclose(ref(x), mine(x), atol=1e-5)
+    assert [k for k, _ in mine.named_parameters()] == list(ref["param_names"])
+    golden_module().seeded_params(mine)
+    bufs = {k[len("buf/"):]: torch.from_numpy(ref[k]) for k in ref.files if k.startswith("buf/")}
+    assert set(bufs) == {k for k, _ in mine.named_buffers()}
+    mine.load_state_dict({**dict(mine.named_parameters()), **bufs}, strict=True)
+    x = torch.from_numpy(ref["x"])
+    mine.train()
+    assert torch.allclose(mine(x), torch.from_numpy(ref["train_out"]), atol=1e-5)
+    mine.eval()
+    with torch.no_grad():
+        assert torch.allclose(mine(x), torch.from_numpy(ref["eval_out"]), atol=1e-5)
 
 
 @pytest.mark.gpu

@@ -1,6 +1,6 @@
 """Summarise an `ncu --metrics gpu__time_duration.sum --csv` launch list: the LAST complete iteration (between the
 last two launches whose name matches --mark) grouped by kernel family.
-    python tools/launch_summary.py gpurun_out/b/launches.csv --mark head_loss"""
+    python tools/launch_summary.py launches.csv --mark head_loss"""
 import csv, re, sys, collections
 
 def family(name):

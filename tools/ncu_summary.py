@@ -1,5 +1,5 @@
-"""Condense an `ncu --set full` report into the few lines profiles/ keeps per kernel.
-    ncu -i gpurun_out/x/prof.ncu-rep --page raw --csv > raw.csv ; python tools/ncu_summary.py raw.csv [algorithmic-bytes-per-kernel ...]
+"""Condense an `ncu --set full` report into a few lines per kernel.
+    ncu -i prof.ncu-rep --page raw --csv > raw.csv ; python tools/ncu_summary.py raw.csv [algorithmic-bytes-per-kernel ...]
 Algorithmic bytes (optional, one per captured launch in order, e.g. 822083584 or 2E with E=...) add the traffic ratio."""
 import csv, sys
 

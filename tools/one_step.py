@@ -1,5 +1,5 @@
 """Scratch: build the bench model (NHWC, fused sites), run 2 warm-up steps and ONE training step eagerly --
-the command profiled for the ncu launch list (profiles/launches_r0*_step.md).  python tools/one_step.py [--stem direct|s2d]"""
+the command to profile for a launch list.  python tools/one_step.py [--stem direct|s2d]"""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path[:0] = [os.path.join(ROOT, "dwt-domain-adaptation_b200"), ROOT]

@@ -1,5 +1,5 @@
 """Scratch: the reference's operator sequence (oracle/torch_port.py, stock ATen ops) on the GPU -- the command profiled
-for the "where the time goes today" launch list (profiles/launches_r02_reference_*.md).
+for a "where the time goes today" launch list.
     python tools/ref_once.py micro     one WTransform2d fwd+bwd at BASELINE configs[1] after 2 warm-ups
     python tools/ref_once.py resnet    one ResNet-50-DWT training step (3x64 images) after 2 warm-ups"""
 import os, sys

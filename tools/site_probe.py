@@ -53,7 +53,7 @@ def main():
         for k, v in prof.items():
             res[k] = dict(us=1e3 * v["ms"] / v["launches"], gbs=v["bytes"] / v["ms"] / 1e6)
     for k, v in sorted(res.items()):
-        print(f"{k:40s} {v['us']:8.1f} us {v['gbs']:7.0f} GB/s  {v['gbs']/6576.1:5.2f}")
+        print(f"{k:40s} {v['us']:8.1f} us {v['gbs']:7.0f} GB/s  {v['gbs']/3350.0:5.2f}")
 
 if __name__ == "__main__":
     main()
