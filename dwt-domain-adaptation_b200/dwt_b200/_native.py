@@ -14,16 +14,26 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # DWT_B200_LIB: another build of the same library (development: A/B timing of a kernel variant on one box)
 LIB_PATH = os.environ.get("DWT_B200_LIB") or os.path.join(_HERE, "lib", "libdwt_b200.so")
 
-ABI_VERSION = 5
+ABI_VERSION = 6
 MAX_DOMAINS = 4
 MAX_GROUP_SIZE = 64
 MODE_TRAIN, MODE_EVAL = 0, 1
 EPI_NONE, EPI_AFFINE, EPI_RELU, EPI_RESIDUAL = 0, 1, 2, 4
 LAYOUT_NHWC = 0x100
 STATUS_NOT_PD, STATUS_BAD_LABEL = 1, 2
+KIND_WHITEN, KIND_BN = 0, 1
 
 _c_float_p = ctypes.c_void_p
 _PtrArray = ctypes.c_void_p * MAX_DOMAINS
+
+
+class TailSite(ctypes.Structure):
+    """dwt_tail_site: one of the two norm sites of dwt_tail2_fwd / dwt_tail2_bwd."""
+    _fields_ = [("x", ctypes.c_void_p), ("eps", ctypes.c_float), ("momentum", ctypes.c_float),
+                ("update_running", ctypes.c_int), ("running_mean", ctypes.POINTER(ctypes.c_void_p)),
+                ("running_cov", ctypes.POINTER(ctypes.c_void_p)), ("gamma", ctypes.c_void_p), ("beta", ctypes.c_void_p),
+                ("save_mean", ctypes.c_void_p), ("save_w", ctypes.c_void_p), ("dx", ctypes.c_void_p),
+                ("dgamma", ctypes.c_void_p), ("dbeta", ctypes.c_void_p)]
 
 _SIGNATURES = {
     "dwt_abi_version": (ctypes.c_int, []),
@@ -48,6 +58,12 @@ _SIGNATURES = {
                                   ctypes.c_int, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
                                   ctypes.c_void_p, _c_float_p, ctypes.c_int, _c_float_p, _c_float_p, ctypes.c_void_p,
                                   ctypes.c_size_t, ctypes.c_void_p]),
+    "dwt_tail2_fwd": (ctypes.c_int, [ctypes.c_int, ctypes.POINTER(TailSite), _c_float_p, ctypes.c_void_p, ctypes.c_int64,
+                                     ctypes.c_int64, ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_void_p,
+                                     ctypes.c_size_t, ctypes.c_void_p]),
+    "dwt_tail2_bwd": (ctypes.c_int, [ctypes.c_int, ctypes.POINTER(TailSite), _c_float_p, _c_float_p, ctypes.c_void_p,
+                                     _c_float_p, ctypes.c_int64, ctypes.c_int64, ctypes.c_int64, ctypes.c_int, ctypes.c_int,
+                                     ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]),
     "dwt_mec_fwd_bwd": (ctypes.c_int, [_c_float_p, _c_float_p, ctypes.c_int64, ctypes.c_int64, _c_float_p,
                                        _c_float_p, _c_float_p, ctypes.c_void_p]),
     "dwt_head_loss_fwd_bwd": (ctypes.c_int, [_c_float_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_int64, ctypes.c_float,

@@ -189,17 +189,18 @@ struct Workspace {
 
 // The head of the workspace holds ONLY the status word and the arrival counters, at offsets
 // that do not depend on the geometry: every call leaves its counters at zero, so calls with
-// different shapes can share one zero-initialised buffer.  Scratch (any content) follows.
+// different shapes can share one zero-initialised buffer.  Scratch (any content) follows; the two-site tail carves
+// a second site's scratch behind the first (carve(..., start = first.bytes)), sharing the head.
 constexpr size_t kMaxGroups = 65536;
 constexpr size_t kOffCounters = 256;
 constexpr size_t kOffDom1 = kOffCounters + sizeof(int) * DWT_MAX_DOMAINS * kMaxGroups;
 constexpr size_t kOffDom2 = kOffDom1 + sizeof(int) * kMaxGroups;
 constexpr size_t kOffScratch = kOffDom2 + sizeof(int) * kMaxGroups;
 
-Workspace carve(void* base, int64_t C, int GS, int D) {
+Workspace carve(void* base, int64_t C, int GS, int D, size_t start = kOffScratch) {
   const int G = (int)(C / GS);
   const int cap = chunk_cap(GS, G, D);
-  size_t off = kOffScratch;
+  size_t off = start;
   auto take = [&](size_t nbytes) { size_t o = off; off = align_up(off + nbytes, 256); return o; };
   char* b = static_cast<char*>(base);
   Workspace w;
@@ -288,6 +289,46 @@ int make_plan(Plan& p, KernelKind reduce_kind, KernelKind ew_kind, const void* a
   return DWT_OK;
 }
 
+int check_running(bool need_running, float* const* rmean, float* const* rcov, int D) {
+  if (!need_running) return DWT_OK;
+  if (!rmean || !rcov) return fail(DWT_E_INVALID, "running buffers required");
+  for (int d = 0; d < D; ++d)
+    if (!rmean[d] || !rcov[d]) return fail(DWT_E_INVALID, "running buffer of domain %d is null", d);
+  return DWT_OK;
+}
+
+dwt::FwdFin make_fwd_fin(float a, float b, float momentum, float unbias, int update_running, bool need_running,
+                         float* const* rmean, float* const* rcov, float* save_mean, float* save_w, const Workspace& w, int D) {
+  dwt::FwdFin fin{};
+  fin.a = a; fin.b = b; fin.momentum = momentum; fin.unbias = unbias;
+  fin.update_running = update_running;
+  fin.save_mean = save_mean; fin.save_w = save_w; fin.save_cov = w.save_cov;
+  for (int d = 0; d < D; ++d) { fin.rmean[d] = need_running ? rmean[d] : nullptr; fin.rcov[d] = need_running ? rcov[d] : nullptr; }
+  fin.dom_counter = w.dom_counter; fin.status = w.status; fin.bad = w.bad;
+  if (need_running && D > 1) {
+    bool all_same = true, all_distinct = true;
+    for (int d = 1; d < D; ++d) {
+      if (rmean[d] != rmean[0] || rcov[d] != rcov[0]) all_same = false;
+      for (int e = 0; e < d; ++e)
+        if (rmean[d] == rmean[e] || rcov[d] == rcov[e]) all_distinct = false;
+    }
+    fin.aliased = all_same ? 1 : (all_distinct ? 0 : -1);
+  }
+  return fin;
+}
+
+dwt::BwdFin make_bwd_fin(float a, int mode, int epi, const float* save_mean, const float* save_w, const float* gamma,
+                         float* dgamma, float* dbeta, const Workspace& w) {
+  dwt::BwdFin fin{};
+  fin.a = a; fin.mode = mode; fin.epi = epi;
+  fin.save_mean = save_mean; fin.save_w = save_w; fin.gamma = gamma;
+  fin.coef = w.coef; fin.dgb_part = w.dgb_part;
+  fin.dgamma = (epi & DWT_EPI_AFFINE) ? dgamma : nullptr;
+  fin.dbeta = (epi & DWT_EPI_AFFINE) ? dbeta : nullptr;
+  fin.dom_counter = w.dom_counter2;
+  return fin;
+}
+
 int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, int GS, int D, int mode, float a,
                     float b, float momentum, float unbias, int update_running, float* const* rmean,
                     float* const* rcov, const float* gamma, const float* beta, const float* residual,
@@ -311,31 +352,14 @@ int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, 
   if (epi != 0 && !p.small)
     return fail(DWT_E_UNSUPPORTED, "fused gamma/beta/ReLU epilogue is built for group_size 1, 2, 4 (got %d)", GS);
   const bool need_running = (mode == DWT_MODE_EVAL) || update_running;
-  if (need_running) {
-    if (!rmean || !rcov) return fail(DWT_E_INVALID, "running buffers required");
-    for (int d = 0; d < D; ++d)
-      if (!rmean[d] || !rcov[d]) return fail(DWT_E_INVALID, "running buffer of domain %d is null", d);
-  }
+  if (int rc = check_running(need_running, rmean, rcov, D)) return rc;
   Workspace w = carve(ws, C, GS, D);
   if (w.bytes > ws_bytes) return fail(DWT_E_WORKSPACE, "workspace too small: need %zu bytes, got %zu", w.bytes, ws_bytes);
   if ((uintptr_t)ws % 256 != 0) return fail(DWT_E_WORKSPACE, "workspace must be 256-byte aligned");
   if (!p.small && ensure_tiled() != 0) return fail(DWT_E_LAUNCH, "cudaFuncSetAttribute failed (%d)", g_tiled_rc);
 
-  dwt::FwdFin fin{};
-  fin.a = a; fin.b = b; fin.momentum = momentum; fin.unbias = unbias;
-  fin.update_running = (mode == DWT_MODE_TRAIN) ? update_running : 0;
-  fin.save_mean = save_mean; fin.save_w = save_w; fin.save_cov = w.save_cov;
-  for (int d = 0; d < D; ++d) { fin.rmean[d] = need_running ? rmean[d] : nullptr; fin.rcov[d] = need_running ? rcov[d] : nullptr; }
-  fin.dom_counter = w.dom_counter; fin.status = w.status; fin.bad = w.bad;
-  if (need_running && D > 1) {
-    bool all_same = true, all_distinct = true;
-    for (int d = 1; d < D; ++d) {
-      if (rmean[d] != rmean[0] || rcov[d] != rcov[0]) all_same = false;
-      for (int e = 0; e < d; ++e)
-        if (rmean[d] == rmean[e] || rcov[d] == rcov[e]) all_distinct = false;
-    }
-    fin.aliased = all_same ? 1 : (all_distinct ? 0 : -1);
-  }
+  const dwt::FwdFin fin = make_fwd_fin(a, b, momentum, unbias, mode == DWT_MODE_TRAIN ? update_running : 0, need_running,
+                                       rmean, rcov, save_mean, save_w, w, D);
 
   const double E = 4.0 * (double)D * (double)N * (double)C * (double)HW;   // bytes of one activation tensor
   if (nhwc) {
@@ -410,11 +434,12 @@ int whiten_like_bwd(const float* x, const float* dout, const float* dout2, float
   if ((epi & DWT_EPI_RELU) && !(epi & DWT_EPI_AFFINE)) return fail(DWT_E_INVALID, "RELU epilogue needs AFFINE");
   if ((epi & DWT_EPI_AFFINE) && (!gamma || !beta)) return fail(DWT_E_INVALID, "AFFINE epilogue needs gamma and beta");
   if (epi & DWT_EPI_RESIDUAL) {
-    // backward of out = relu(z + residual): the ReLU mask comes from the byte map the forward wrote
-    if (!nhwc || !relu_mask || (epi & 3) != 3)
-      return fail(DWT_E_INVALID, "backward of a RESIDUAL forward needs the channels-last layout, AFFINE|RELU and the forward's "
-                                 "ReLU byte map (or pass dout already masked by (out > 0) with epilogue AFFINE)");
-    if (dresidual && (uintptr_t)dresidual % 16 != 0) return fail(DWT_E_INVALID, "dresidual must be 16-byte aligned");
+    // backward of out = relu(z + residual): the ReLU mask comes from the byte map the forward wrote, the masked
+    // gradient goes to dresidual and is what the apply pass reads
+    if (!nhwc || !relu_mask || (epi & 3) != 3 || !dresidual)
+      return fail(DWT_E_INVALID, "backward of a RESIDUAL forward needs the channels-last layout, AFFINE|RELU, the forward's "
+                                 "ReLU byte map and dresidual (or pass dout already masked by (out > 0) with epilogue AFFINE)");
+    if ((uintptr_t)dresidual % 16 != 0) return fail(DWT_E_INVALID, "dresidual must be 16-byte aligned");
   } else if (relu_mask || dresidual) {
     return fail(DWT_E_INVALID, "relu_mask / dresidual belong to the RESIDUAL epilogue");
   }
@@ -426,23 +451,17 @@ int whiten_like_bwd(const float* x, const float* dout, const float* dout2, float
   if ((uintptr_t)ws % 256 != 0) return fail(DWT_E_WORKSPACE, "workspace must be 256-byte aligned");
   if (!p.small && ensure_tiled() != 0) return fail(DWT_E_LAUNCH, "cudaFuncSetAttribute failed (%d)", g_tiled_rc);
 
-  dwt::BwdFin fin{};
-  fin.a = a; fin.mode = mode; fin.epi = epi;
-  fin.save_mean = save_mean; fin.save_w = save_w; fin.gamma = gamma;
-  fin.coef = w.coef; fin.dgb_part = w.dgb_part;
-  fin.dgamma = (epi & DWT_EPI_AFFINE) ? dgamma : nullptr;
-  fin.dbeta = (epi & DWT_EPI_AFFINE) ? dbeta : nullptr;
-  fin.dom_counter = w.dom_counter2;
+  const dwt::BwdFin fin = make_bwd_fin(a, mode, epi, save_mean, save_w, gamma, dgamma, dbeta, w);
+  const bool masked = nhwc && (epi & DWT_EPI_RESIDUAL) != 0;   // the reduction also writes the masked gradient
 
-  const bool need_reduce = (mode == DWT_MODE_TRAIN) || (fin.dgamma != nullptr);
+  const bool need_reduce = (mode == DWT_MODE_TRAIN) || (fin.dgamma != nullptr) || masked;
   const double E = 4.0 * (double)D * (double)N * (double)C * (double)HW;
   if (nhwc) {
     const ClPlan cp = cl_plan(p.gm, 2, 2, 4, 4);
-    const bool masked = (epi & DWT_EPI_RESIDUAL) != 0;
     if (need_reduce) {
       {
-        Launch l("cl_bwd_reduce", &p.gm, ((masked ? 2.0625 : 2.0) + (dout2 ? 1.0 : 0.0)) * E, st);
-        dwt::cl_bwd_reduce(x, dout, dout2, p.gm, cp.nred, cp.gz_red, epi, save_mean, save_w, gamma, beta, relu_mask, w.partial, st);
+        Launch l("cl_bwd_reduce", &p.gm, ((masked ? 3.0625 : 2.0) + (dout2 ? 1.0 : 0.0)) * E, st);
+        dwt::cl_bwd_reduce(x, dout, dout2, p.gm, cp.nred, cp.gz_red, epi, save_mean, save_w, gamma, beta, relu_mask, dresidual, w.partial, st);
       }
       if (int rc = check_launch("channels-last backward reduction kernel")) return rc;
       Launch l("cl_bwd_finalize", &p.gm, 0.0, st);
@@ -453,8 +472,9 @@ int whiten_like_bwd(const float* x, const float* dout, const float* dout2, float
     }
     if (int rc = check_launch("channels-last backward finalize kernel")) return rc;
     {
-      Launch l("cl_bwd_apply", &p.gm, ((masked ? (dresidual ? 4.0625 : 3.0625) : 3.0) + (dout2 ? 1.0 : 0.0)) * E, st);
-      dwt::cl_bwd_apply(x, dout, dout2, dx, p.gm, cp.new_, cp.gz_ew, epi, w.coef, save_mean, save_w, gamma, beta, relu_mask, dresidual, st);
+      Launch l("cl_bwd_apply", &p.gm, (3.0 + (dout2 && !masked ? 1.0 : 0.0)) * E, st);
+      if (masked) dwt::cl_bwd_apply(x, dresidual, nullptr, dx, p.gm, cp.new_, cp.gz_ew, DWT_EPI_AFFINE, w.coef, save_mean, save_w, gamma, beta, st);
+      else dwt::cl_bwd_apply(x, dout, dout2, dx, p.gm, cp.new_, cp.gz_ew, epi, w.coef, save_mean, save_w, gamma, beta, st);
     }
     return check_launch("channels-last backward apply kernel");
   }
@@ -490,6 +510,112 @@ int whiten_like_bwd(const float* x, const float* dout, const float* dout2, float
   return check_launch("whitening backward apply kernel");
 }
 
+// ---- two-site residual tail (dwt_tail2_fwd / dwt_tail2_bwd) ----------------------------------------------
+struct SiteConst { float a, b, unbias; };
+SiteConst site_const(int kind, float eps, int64_t N, int64_t HW) {
+  if (kind == DWT_KIND_BN) {                       // as dwt_bn_fwd: S = var + eps, unbiased variance into the EMA
+    const double M = (double)N * (double)HW;
+    return {1.f, eps, M > 1.0 ? (float)(M / (M - 1.0)) : 1.f};
+  }
+  return {1.f - eps, eps, 1.f};                    // as dwt_whiten_fwd
+}
+
+// checks shared by both directions; out is the tensor-sized output of the call (y, or dz)
+int tail2_plan(Plan& p, int kind, const dwt_tail_site* s, const void* out, int64_t N, int64_t C, int64_t HW, int GS, int D) {
+  if (kind != DWT_KIND_WHITEN && kind != DWT_KIND_BN) return fail(DWT_E_INVALID, "bad kind %d", kind);
+  if (kind == DWT_KIND_BN && GS != 1) return fail(DWT_E_INVALID, "batch norm has group_size 1 (got %d)", GS);
+  if (!s) return fail(DWT_E_INVALID, "null pointer argument");
+  if (int rc = make_plan(p, K_STATS, K_APPLY, s[0].x, s[1].x, out, N, C, HW, GS, D)) return rc;
+  if (!dwt::cl_supports((int)C, GS))
+    return fail(DWT_E_UNSUPPORTED, "the two-site tail runs on the channels-last kernels: group_size 1, 2, 4 with C/4 a power of two (C=%lld gs=%d)",
+                (long long)C, GS);
+  for (int k = 0; k < 2; ++k)
+    if (!s[k].x || !s[k].gamma || !s[k].beta || !s[k].save_mean || !s[k].save_w || !out) return fail(DWT_E_INVALID, "null pointer argument");
+  if ((((uintptr_t)s[0].x | (uintptr_t)s[1].x | (uintptr_t)out) % 16) != 0) return fail(DWT_E_INVALID, "channels-last tensors must be 16-byte aligned");
+  return DWT_OK;
+}
+
+// the two sites' scratch: site 1 behind site 0, sharing the head (status word, counters)
+int tail2_workspace(Workspace (&w)[2], void* ws, size_t ws_bytes, int64_t C, int GS, int D) {
+  if (!ws) return fail(DWT_E_INVALID, "null pointer argument");
+  w[0] = carve(ws, C, GS, D);
+  w[1] = carve(ws, C, GS, D, w[0].bytes);
+  if (w[1].bytes > ws_bytes) return fail(DWT_E_WORKSPACE, "workspace too small: need %zu bytes, got %zu", w[1].bytes, ws_bytes);
+  if ((uintptr_t)ws % 256 != 0) return fail(DWT_E_WORKSPACE, "workspace must be 256-byte aligned");
+  return DWT_OK;
+}
+
+int tail2_fwd(int kind, const dwt_tail_site* s, float* y, uint8_t* relu_mask, int64_t N, int64_t C, int64_t HW, int GS, int D,
+              void* ws, size_t ws_bytes, cudaStream_t st) {
+  Plan p;
+  if (int rc = tail2_plan(p, kind, s, y, N, C, HW, GS, D)) return rc;
+  if (!relu_mask) return fail(DWT_E_INVALID, "the two-site tail writes the ReLU byte map its backward reads");
+  for (int k = 0; k < 2; ++k)
+    if (int rc = check_running(s[k].update_running != 0, s[k].running_mean, s[k].running_cov, D)) return rc;
+  Workspace w[2];
+  if (int rc = tail2_workspace(w, ws, ws_bytes, C, GS, D)) return rc;
+  dwt::FwdFin fin[2];
+  for (int k = 0; k < 2; ++k) {
+    const SiteConst sc = site_const(kind, s[k].eps, N, HW);
+    fin[k] = make_fwd_fin(sc.a, sc.b, s[k].momentum, sc.unbias, s[k].update_running, s[k].update_running != 0, s[k].running_mean,
+                          s[k].running_cov, s[k].save_mean, s[k].save_w, w[k], D);
+  }
+  const double E = 4.0 * (double)D * (double)N * (double)C * (double)HW;
+  const ClPlan cp = cl_plan(p.gm, 3, 3, 8, 4);
+  for (int k = 0; k < 2; ++k) {            // the tail's input first: conv3 wrote it last, its end is still in L2
+    Launch l("cl_stats", &p.gm, E, st);
+    dwt::cl_stats(s[k].x, p.gm, cp.nred, cp.gz_red, w[k].partial, w[k].shift, st);
+  }
+  if (int rc = check_launch("channels-last statistics kernel")) return rc;
+  {
+    Launch l("cl_tail2_fwd_finalize", &p.gm, 0.0, st);
+    dwt::cl_fwd_finalize(w[0].partial, cp.nred, w[0].shift, p.gm, fin[0], st, &fin[1], (size_t)(w[1].partial - w[0].partial),
+                         (size_t)(w[1].shift - w[0].shift));
+  }
+  if (int rc = check_launch("channels-last finalize kernel")) return rc;
+  {
+    Launch l("cl_tail2_apply", &p.gm, 3.0625 * E, st);       // x, xd -> out + byte map
+    dwt::cl_tail2_apply(s[0].x, s[1].x, y, p.gm, cp.new_, cp.gz_ew, s[0].save_mean, s[0].save_w, s[0].gamma, s[0].beta,
+                        s[1].save_mean, s[1].save_w, s[1].gamma, s[1].beta, relu_mask, st);
+  }
+  return check_launch("channels-last two-site apply kernel");
+}
+
+int tail2_bwd(int kind, const dwt_tail_site* s, const float* dout, const float* dout2, const uint8_t* relu_mask, float* dz,
+              int64_t N, int64_t C, int64_t HW, int GS, int D, void* ws, size_t ws_bytes, cudaStream_t st) {
+  Plan p;
+  if (int rc = tail2_plan(p, kind, s, dz, N, C, HW, GS, D)) return rc;
+  if (!dout || !relu_mask || !s[0].dx || !s[1].dx) return fail(DWT_E_INVALID, "null pointer argument");
+  if ((((uintptr_t)dout | (uintptr_t)dout2 | (uintptr_t)s[0].dx | (uintptr_t)s[1].dx) % 16) != 0)
+    return fail(DWT_E_INVALID, "channels-last tensors must be 16-byte aligned");
+  for (int k = 0; k < 2; ++k)
+    if ((s[k].dgamma == nullptr) != (s[k].dbeta == nullptr)) return fail(DWT_E_INVALID, "dgamma and dbeta go together");
+  Workspace w[2];
+  if (int rc = tail2_workspace(w, ws, ws_bytes, C, GS, D)) return rc;
+  dwt::BwdFin fin[2];
+  for (int k = 0; k < 2; ++k)
+    fin[k] = make_bwd_fin(site_const(kind, s[k].eps, N, HW).a, DWT_MODE_TRAIN, k ? DWT_EPI_AFFINE : (DWT_EPI_AFFINE | DWT_EPI_RELU | DWT_EPI_RESIDUAL),
+                          s[k].save_mean, s[k].save_w, s[k].gamma, s[k].dgamma, s[k].dbeta, w[k]);
+  const double E = 4.0 * (double)D * (double)N * (double)C * (double)HW;
+  const ClPlan cp = cl_plan(p.gm, 2, 2, 4, 4);
+  {
+    Launch l("cl_tail2_bwd_reduce", &p.gm, (4.0625 + (dout2 ? 1.0 : 0.0)) * E, st);   // x, xd, dout (+ dout2), byte map -> dz
+    dwt::cl_tail2_bwd_reduce(s[0].x, s[1].x, dout, dout2, p.gm, cp.nred, cp.gz_red, s[0].save_mean, s[1].save_mean, relu_mask, dz,
+                             w[0].partial, (size_t)(w[1].partial - w[0].partial), st);
+  }
+  if (int rc = check_launch("channels-last two-site backward reduction kernel")) return rc;
+  {
+    Launch l("cl_tail2_bwd_finalize", &p.gm, 0.0, st);
+    dwt::cl_bwd_finalize(w[0].partial, cp.nred, p.gm, fin[0], st, &fin[1], (size_t)(w[1].partial - w[0].partial));
+  }
+  if (int rc = check_launch("channels-last backward finalize kernel")) return rc;
+  {
+    Launch l("cl_tail2_bwd_apply", &p.gm, 5.0 * E, st);       // x, xd, dz -> dx, dxd
+    dwt::cl_tail2_bwd_apply(s[0].x, s[1].x, dz, s[0].dx, s[1].dx, p.gm, cp.new_, cp.gz_ew, w[0].coef, w[1].coef, st);
+  }
+  return check_launch("channels-last two-site backward apply kernel");
+}
+
 }  // namespace
 
 extern "C" {
@@ -503,7 +629,7 @@ size_t dwt_workspace_bytes(int64_t N, int64_t C, int64_t HW, int group_size, int
   if (C <= 0 || group_size < 1 || group_size > DWT_MAX_GROUP_SIZE || C % group_size != 0 || n_domains < 1 ||
       n_domains > DWT_MAX_DOMAINS)
     return 0;
-  return carve(nullptr, C, group_size, n_domains).bytes;
+  return carve(nullptr, C, group_size, n_domains, carve(nullptr, C, group_size, n_domains).bytes).bytes;   // two sites
 }
 
 int dwt_whiten_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, int group_size, int n_domains,
@@ -545,6 +671,18 @@ int dwt_bn_bwd(const float* x, const float* dout, const float* dout2, float* dx,
   return whiten_like_bwd(x, dout, dout2, dx, N, C, HW, 1, n_domains, mode, 1.f, save_mean, save_invstd, weight, bias,
                          relu_mask, dresidual, epilogue, dweight, dbias, workspace, workspace_bytes,
                          (cudaStream_t)stream);
+}
+
+int dwt_tail2_fwd(int kind, const dwt_tail_site* sites, float* y, uint8_t* relu_mask, int64_t N, int64_t C, int64_t HW,
+                  int group_size, int n_domains, void* workspace, size_t workspace_bytes, dwt_stream_t stream) {
+  return tail2_fwd(kind, sites, y, relu_mask, N, C, HW, group_size, n_domains, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int dwt_tail2_bwd(int kind, const dwt_tail_site* sites, const float* dout, const float* dout2, const uint8_t* relu_mask, float* dz,
+                  int64_t N, int64_t C, int64_t HW, int group_size, int n_domains, void* workspace, size_t workspace_bytes,
+                  dwt_stream_t stream) {
+  return tail2_bwd(kind, sites, dout, dout2, relu_mask, dz, N, C, HW, group_size, n_domains, workspace, workspace_bytes,
+                   (cudaStream_t)stream);
 }
 
 int dwt_mec_fwd_bwd(const float* x, const float* y, int64_t N, int64_t K, float* loss, float* gx, float* gy,

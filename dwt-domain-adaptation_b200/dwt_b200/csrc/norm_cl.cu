@@ -16,6 +16,12 @@
 //   cl_stats -> cl_fwd_finalize -> cl_apply          (forward, 12 B/element)
 //   cl_bwd_reduce -> cl_bwd_finalize -> cl_bwd_apply (backward, 20 B/element)
 //
+// Two-site tail (template flag DS): the residual tail of a downsampling Bottleneck,
+// relu(site3(x3) + site_d(xd)) with site_d = gamma_d W_d (xd - mu_d) + beta_d.  Both sites share N, C, HW, gs and D;
+// the statistics run per site, the finalize launches serve both sites (grid.y = site) and the elementwise and
+// backward-reduction kernels sweep x3 and xd together, so the identity tensor is never written and the backward
+// gradient of the downsample site's output (the masked dz) is read from the same pass as the tail's.
+//
 // Sweep order (round 2).  The tensor a pass reads was touched a moment ago: x was just WRITTEN front to back
 // by the producing convolution, and the second pass of a site re-reads what the first pass just read.  The newest
 // tens of MB of it are still in L2 (50 MB on H100) -- but only if the kernel gets to them before its own misses evict
@@ -26,8 +32,9 @@
 // A CTA's partial sums are still a fixed set added in a fixed order: results stay deterministic.
 //
 // The residual tail relu(z + identity) (resnet50_dwt_mec_officehome.py:239-240): the forward apply leaves one
-// byte per float4 with the four (out > 0) bits; the backward passes mask dout with it (the pre-activation cannot
-// be recomputed without the residual) and bwd_apply also writes the masked gradient for the identity branch.
+// byte per float4 with the four (out > 0) bits; the backward reduction masks dout with it (the pre-activation cannot
+// be recomputed without the residual) and writes the masked gradient dz, which is also the gradient of the identity
+// branch; bwd_apply then reads x and dz only (the plain AFFINE apply with dout = dz).
 // Such a site's output is used twice by the next block (first convolution and identity branch): the two gradients
 // arrive as dout and dout2 and are summed where they are read (template flag D2; dwt_b200.h, functional.fork_for_sum)
 // instead of by an elementwise kernel in between.
@@ -220,8 +227,8 @@ __device__ __forceinline__ void take_group(const float (&a)[NSUB * PER], int s, 
 }
 
 template <int GS>
-__global__ void __launch_bounds__(32 * kFinQ * DWT_MAX_DOMAINS) cl_fwd_finalize_kernel(const float* __restrict__ partial, int nrows, const float* __restrict__ shift,
-                                                                                      const Geom gm, const FwdFin fin) {
+__device__ __forceinline__ void cl_fwd_finalize_site(const float* __restrict__ partial, int nrows, const float* __restrict__ shift,
+                                                     const Geom& gm, const FwdFin& fin) {
   using SH = ClShape<GS>;
   constexpr int NST = GS + GS * GS;
   __shared__ float sStat[DWT_MAX_DOMAINS][kFinQ][SH::NSUB][NST + 1];
@@ -308,27 +315,45 @@ __global__ void __launch_bounds__(32 * kFinQ * DWT_MAX_DOMAINS) cl_fwd_finalize_
   }
 }
 
+// grid.y = sites: site 1 (two-site tail) reads its partial rows at partial + pstride and its shifts at shift + sstride
+template <int GS>
+__global__ void __launch_bounds__(32 * kFinQ * DWT_MAX_DOMAINS) cl_fwd_finalize_kernel(const float* __restrict__ partial, size_t pstride, int nrows,
+                                                                                      const float* __restrict__ shift, size_t sstride, const Geom gm,
+                                                                                      const __grid_constant__ FwdFin fin, const __grid_constant__ FwdFin fin2) {
+  const bool second = blockIdx.y != 0;
+  cl_fwd_finalize_site<GS>(partial + (second ? pstride : 0), nrows, shift + (second ? sstride : 0), gm, second ? fin2 : fin);
+}
+
 // ------------------------------------------------------------------------------------------
 // apply
 // ------------------------------------------------------------------------------------------
-template <int GS, int EPI>
+// DS (two-site tail, EPI = AFFINE|RELU|RESIDUAL): `res` is the downsample site's INPUT xd and the residual is its
+// output gamma_d W_d (xd - mu_d) + beta_d, formed in registers exactly as the downsample site's own apply would.
+template <int GS, int EPI, bool DS>
 __global__ void __launch_bounds__(kT, 3) cl_apply_kernel(const float* __restrict__ x, float* __restrict__ y, const Geom gm,
                                                          const float* __restrict__ save_mean, const float* __restrict__ save_w,
                                                          const float* __restrict__ gamma, const float* __restrict__ beta,
-                                                         const float* __restrict__ res, uint8_t* __restrict__ mask) {
+                                                         const float* __restrict__ res, uint8_t* __restrict__ mask,
+                                                         const float* __restrict__ save_mean_d, const float* __restrict__ save_w_d,
+                                                         const float* __restrict__ gamma_d, const float* __restrict__ beta_d) {
   using S = ClShape<GS>;
   constexpr bool RES = (EPI & DWT_EPI_RESIDUAL) != 0;
-  constexpr int UNROLL = RES ? 4 : 8;
+  static_assert(!DS || RES, "the two-site tail is a residual epilogue");
+  // rows per thread and step (the grid shape comes from cl_plan either way): two sites' maps need the registers
+  constexpr int UNROLL = DS ? 2 : (RES ? 4 : 8);
   const ClThread t(gm);
   const unsigned rows = (unsigned)gm.N * gm.HW;
   pdl_wait();                                       // save_mean / save_w of the finalize launch are complete
   CL_FOR_DOMAINS(d, gm, false) {
-    float Wp[S::NSUB][S::NM], bp[S::NSUB][GS];
+    float Wp[S::NSUB][S::NM], bp[S::NSUB][GS], Wd[DS ? S::NSUB : 1][S::NM], bd[DS ? S::NSUB : 1][GS];
 #pragma unroll
     for (int s = 0; s < S::NSUB; ++s) {
       const int g = t.q * S::NSUB + s;
       load_forward_map<GS, EPI>(save_w + ((size_t)d * gm.G + g) * GS * GS, save_mean + (size_t)d * gm.C + g * GS,
                                 gamma + g * GS, beta + g * GS, Wp[s], bp[s]);
+      if constexpr (DS)
+        load_forward_map<GS, DWT_EPI_AFFINE>(save_w_d + ((size_t)d * gm.G + g) * GS * GS, save_mean_d + (size_t)d * gm.C + g * GS,
+                                             gamma_d + g * GS, beta_d + g * GS, Wd[s], bd[s]);
     }
     const size_t base = (size_t)d * rows * gm.C + 4 * t.q;
     const float* xd = x + base;
@@ -356,6 +381,14 @@ __global__ void __launch_bounds__(kT, 3) cl_apply_kernel(const float* __restrict
 #pragma unroll
           for (int s = 0; s < S::NSUB; ++s) {
             float xi[GS], oi[GS];
+            if constexpr (DS) {
+              float xdi[GS], odi[GS];
+#pragma unroll
+              for (int c = 0; c < GS; ++c) xdi[c] = ra[s * GS + c];
+              apply_group<GS>(Wd[s], bd[s], xdi, odi);
+#pragma unroll
+              for (int c = 0; c < GS; ++c) ra[s * GS + c] = odi[c];
+            }
 #pragma unroll
             for (int c = 0; c < GS; ++c) xi[c] = e[s * GS + c];
             apply_group<GS>(Wp[s], bp[s], xi, oi);
@@ -377,22 +410,40 @@ __global__ void __launch_bounds__(kT, 3) cl_apply_kernel(const float* __restrict
 // ------------------------------------------------------------------------------------------
 // backward reduce: partial[d][cta][q][BWD]  (per problem: R row-major, then sdz)
 // ------------------------------------------------------------------------------------------
-template <int GS, int EPI, bool D2>
+// one row's contribution to a problem's backward accumulators: R += dz (x - mu)^T, sdz += dz
+template <int GS>
+__device__ __forceinline__ void bwd_accumulate(float* acc, const float (&dz)[GS], const float (&xi)[GS], const float* mu) {
+#pragma unroll
+  for (int i = 0; i < GS; ++i) {
+    acc[GS * GS + i] += dz[i];
+#pragma unroll
+    for (int j = 0; j < GS; ++j) acc[i * GS + j] = fmaf(dz[i], xi[j] - mu[j], acc[i * GS + j]);
+  }
+}
+
+// MASK (residual tail): the masked gradient dz -- also the gradient of the identity branch -- is written to dzout.
+// DS (two-site tail): the downsample site's input xd is swept alongside x; its gradient is the same dz, so its
+// accumulators (R_d, sdz) go to a second set of partial rows at partial + pstride.
+template <int GS, int EPI, bool D2, bool DS>
 __global__ void __launch_bounds__(kT, 2) cl_bwd_reduce_kernel(const float* __restrict__ x, const float* __restrict__ dout, const float* __restrict__ dout2,
                                                               const Geom gm, const float* __restrict__ save_mean,
                                                               const float* __restrict__ save_w, const float* __restrict__ gamma,
                                                               const float* __restrict__ beta, const uint8_t* __restrict__ mask,
-                                                              float* __restrict__ partial) {
+                                                              float* __restrict__ dzout, float* __restrict__ partial,
+                                                              const float* __restrict__ xds, const float* __restrict__ save_mean_d,
+                                                              size_t pstride) {
   using S = ClShape<GS>;
   constexpr int UNROLL = 4;
   constexpr bool MASK = (EPI & DWT_EPI_RESIDUAL) != 0;          // ReLU mask saved by the forward (residual tail)
   constexpr bool RELU = (EPI & DWT_EPI_RELU) != 0 && !MASK;     // ReLU mask recomputed from x
+  static_assert(!DS || MASK, "the two-site tail is a residual epilogue");
+  constexpr int NS = DS ? 2 : 1;
   __shared__ float sRed[kT * S::BWD];
   const ClThread t(gm);
   const unsigned rows = (unsigned)gm.N * gm.HW;
   pdl_launch_dependents();
   CL_FOR_DOMAINS(d, gm, true) {
-    float Wp[S::NSUB][S::NM], bp[S::NSUB][GS], mu[4];
+    float Wp[S::NSUB][S::NM], bp[S::NSUB][GS], mu[NS][4];
 #pragma unroll
     for (int s = 0; s < S::NSUB; ++s) {
       const int g = t.q * S::NSUB + s;
@@ -400,41 +451,60 @@ __global__ void __launch_bounds__(kT, 2) cl_bwd_reduce_kernel(const float* __res
         load_forward_map<GS, EPI>(save_w + ((size_t)d * gm.G + g) * GS * GS, save_mean + (size_t)d * gm.C + g * GS,
                                   gamma + g * GS, beta + g * GS, Wp[s], bp[s]);
     }
-    {
-      const float4 m4 = ldg4(save_mean + (size_t)d * gm.C + 4 * t.q);
-      mu[0] = m4.x; mu[1] = m4.y; mu[2] = m4.z; mu[3] = m4.w;
-    }
-    float acc[S::BWD];
 #pragma unroll
-    for (int i = 0; i < S::BWD; ++i) acc[i] = 0.f;
+    for (int k = 0; k < NS; ++k) {
+      const float4 m4 = ldg4((k ? save_mean_d : save_mean) + (size_t)d * gm.C + 4 * t.q);
+      mu[k][0] = m4.x; mu[k][1] = m4.y; mu[k][2] = m4.z; mu[k][3] = m4.w;
+    }
+    float acc[NS][S::BWD];
+#pragma unroll
+    for (int k = 0; k < NS; ++k)
+#pragma unroll
+      for (int i = 0; i < S::BWD; ++i) acc[k][i] = 0.f;
     const size_t base = (size_t)d * rows * gm.C + 4 * t.q;
-    const float* xd = x + base;
+    const float* xp[NS];
+    xp[0] = x + base;
+    if constexpr (DS) xp[NS - 1] = xds + base;
     const float* gd = dout + base;
     const float* gd2 = D2 ? dout2 + base : nullptr;        // second addend of the incoming gradient (see dwt_b200.h)
+    float* zd = MASK ? dzout + base : nullptr;
     const uint8_t* md = mask + (size_t)d * rows * t.C4 + t.q;
-    sweep_rows<UNROLL, true>(t, rows, [&](unsigned r) {
-      float4 v[UNROLL], q[UNROLL], q2[D2 ? UNROLL : 1];
-      unsigned mb[UNROLL];
+    // rows per load batch: all of the chunk's rows, or (two sites) half of them, so that both sites' accumulators stay
+    // in registers.  The rows are accumulated in the same order either way.
+    constexpr int H = DS ? UNROLL / 2 : UNROLL;
+    sweep_rows<UNROLL, true>(t, rows, [&](unsigned r0) {
 #pragma unroll
-      for (int u = 0; u < UNROLL; ++u) {                       // every load of the step first: nothing waits on another
+     for (int h = 0; h < UNROLL; h += H) {
+      const unsigned r = r0 + h * t.rpi;
+      float4 v[NS][H], q[H], q2[D2 ? H : 1];
+      unsigned mb[H];
+#pragma unroll
+      for (int u = 0; u < H; ++u) {                            // every load of the batch first: nothing waits on another
         const unsigned rr = r + u * t.rpi;
         if (rr < rows) {
-          v[u] = ldg4(xd + (size_t)rr * gm.C); q[u] = ldg4(gd + (size_t)rr * gm.C);
+#pragma unroll
+          for (int k = 0; k < NS; ++k) v[k][u] = ldg4(xp[k] + (size_t)rr * gm.C);
+          q[u] = ldg4(gd + (size_t)rr * gm.C);
           if constexpr (MASK) mb[u] = __ldg(md + (size_t)rr * t.C4);
           if constexpr (D2) q2[u] = ldg4(gd2 + (size_t)rr * gm.C);
         } else {
-          v[u] = make_float4(mu[0], mu[1], mu[2], mu[3]); q[u] = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+          for (int k = 0; k < NS; ++k) v[k][u] = make_float4(mu[k][0], mu[k][1], mu[k][2], mu[k][3]);
+          q[u] = make_float4(0.f, 0.f, 0.f, 0.f);
           if constexpr (MASK) mb[u] = 0u;
           if constexpr (D2) q2[u] = make_float4(0.f, 0.f, 0.f, 0.f);
         }
       }
       if constexpr (D2) {
 #pragma unroll
-        for (int u = 0; u < UNROLL; ++u) { q[u].x += q2[u].x; q[u].y += q2[u].y; q[u].z += q2[u].z; q[u].w += q2[u].w; }
+        for (int u = 0; u < H; ++u) { q[u].x += q2[u].x; q[u].y += q2[u].y; q[u].z += q2[u].z; q[u].w += q2[u].w; }
       }
 #pragma unroll
-      for (int u = 0; u < UNROLL; ++u) {
-        const float e[4] = {v[u].x, v[u].y, v[u].z, v[u].w}, ge[4] = {q[u].x, q[u].y, q[u].z, q[u].w};
+      for (int u = 0; u < H; ++u) {
+        const float ge[4] = {q[u].x, q[u].y, q[u].z, q[u].w};
+        const float e[4] = {v[0][u].x, v[0][u].y, v[0][u].z, v[0][u].w};
+        const float ed[4] = {v[NS - 1][u].x, v[NS - 1][u].y, v[NS - 1][u].z, v[NS - 1][u].w};
+        float zm[4];
 #pragma unroll
         for (int s = 0; s < S::NSUB; ++s) {
           float xi[GS], dz[GS];
@@ -448,22 +518,31 @@ __global__ void __launch_bounds__(kT, 2) cl_bwd_reduce_kernel(const float* __res
           }
           if constexpr (MASK) {
 #pragma unroll
-            for (int c = 0; c < GS; ++c) dz[c] = ((mb[u] >> (s * GS + c)) & 1u) ? dz[c] : 0.f;
+            for (int c = 0; c < GS; ++c) { dz[c] = ((mb[u] >> (s * GS + c)) & 1u) ? dz[c] : 0.f; zm[s * GS + c] = dz[c]; }
           }
+          bwd_accumulate<GS>(acc[0] + s * S::BWD1, dz, xi, &mu[0][s * GS]);
+          if constexpr (DS) {
 #pragma unroll
-          for (int i = 0; i < GS; ++i) {
-            acc[s * S::BWD1 + GS * GS + i] += dz[i];
-#pragma unroll
-            for (int j = 0; j < GS; ++j) acc[s * S::BWD1 + i * GS + j] = fmaf(dz[i], xi[j] - mu[s * GS + j], acc[s * S::BWD1 + i * GS + j]);
+            for (int c = 0; c < GS; ++c) xi[c] = ed[s * GS + c];
+            bwd_accumulate<GS>(acc[NS - 1] + s * S::BWD1, dz, xi, &mu[NS - 1][s * GS]);
           }
         }
+        if constexpr (MASK) {
+          const unsigned rr = r + u * t.rpi;
+          if (rr < rows) *reinterpret_cast<float4*>(zd + (size_t)rr * gm.C) = make_float4(zm[0], zm[1], zm[2], zm[3]);
+        }
       }
+     }
     });
-    column_reduce<S::BWD>(t, acc, sRed);
-    if (t.rsub == 0) {
-      float* dst = partial + (((size_t)d * gridDim.x + blockIdx.x) * t.C4 + t.q) * S::BWD;
 #pragma unroll
-      for (int i = 0; i < S::BWD; ++i) dst[i] = acc[i];
+    for (int k = 0; k < NS; ++k) {
+      if (k) __syncthreads();                          // sRed is reused by the second site
+      column_reduce<S::BWD>(t, acc[k], sRed);
+      if (t.rsub == 0) {
+        float* dst = partial + k * pstride + (((size_t)d * gridDim.x + blockIdx.x) * t.C4 + t.q) * S::BWD;
+#pragma unroll
+        for (int i = 0; i < S::BWD; ++i) dst[i] = acc[k][i];
+      }
     }
     if (gridDim.z == 1) __syncthreads();             // sRed is reused by the next domain
   }
@@ -472,7 +551,7 @@ __global__ void __launch_bounds__(kT, 2) cl_bwd_reduce_kernel(const float* __res
 // Same arrangement as the forward finalize (one warp per (float4 column, domain)); dgamma / dbeta are summed over the
 // domains by the d == 0 warp after the barrier.
 template <int GS>
-__global__ void __launch_bounds__(32 * kFinQ * DWT_MAX_DOMAINS) cl_bwd_finalize_kernel(const float* __restrict__ partial, int nrows, const Geom gm, const BwdFin fin) {
+__device__ __forceinline__ void cl_bwd_finalize_site(const float* __restrict__ partial, int nrows, const Geom& gm, const BwdFin& fin) {
   using SH = ClShape<GS>;
   const int s = threadIdx.x, d = threadIdx.z, q = blockIdx.x * blockDim.y + threadIdx.y;
   const int W = (gm.C >> 2) * SH::BWD;
@@ -503,57 +582,97 @@ __global__ void __launch_bounds__(32 * kFinQ * DWT_MAX_DOMAINS) cl_bwd_finalize_
   }
 }
 
+// grid.y = sites, as for the forward finalize
+template <int GS>
+__global__ void __launch_bounds__(32 * kFinQ * DWT_MAX_DOMAINS) cl_bwd_finalize_kernel(const float* __restrict__ partial, size_t pstride, int nrows,
+                                                                                      const Geom gm, const __grid_constant__ BwdFin fin,
+                                                                                      const __grid_constant__ BwdFin fin2) {
+  const bool second = blockIdx.y != 0;
+  cl_bwd_finalize_site<GS>(partial + (second ? pstride : 0), nrows, gm, second ? fin2 : fin);
+}
+
 // ------------------------------------------------------------------------------------------
 // backward apply
 // ------------------------------------------------------------------------------------------
-template <int GS, int EPI, bool D2>
+// Per-thread copy of a problem's backward coefficients (dx = A1 dz + Bm x + cvec; A1 upper-, Bm full symmetric,
+// both kept as packed lower triangles)
+template <int GS>
+struct BwdCoef {
+  float A1[GS * (GS + 1) / 2], Bm[GS * (GS + 1) / 2], cv[GS];
+  __device__ __forceinline__ void load(const float* cf) {
+#pragma unroll
+    for (int i = 0; i < GS; ++i) {
+      cv[i] = __ldg(cf + 2 * GS * GS + i);
+#pragma unroll
+      for (int j = 0; j <= i; ++j) {
+        A1[i * (i + 1) / 2 + j] = __ldg(cf + j * GS + i);
+        Bm[i * (i + 1) / 2 + j] = __ldg(cf + GS * GS + i * GS + j);
+      }
+    }
+  }
+  __device__ __forceinline__ void apply(const float (&dz)[GS], const float (&xi)[GS], float* o) const {
+#pragma unroll
+    for (int i = 0; i < GS; ++i) {
+      float a = cv[i];
+#pragma unroll
+      for (int j = i; j < GS; ++j) a = fmaf(A1[j * (j + 1) / 2 + i], dz[j], a);
+#pragma unroll
+      for (int j = 0; j < GS; ++j) {
+        const int hi = i > j ? i : j, lo = i > j ? j : i;
+        a = fmaf(Bm[hi * (hi + 1) / 2 + lo], xi[j], a);
+      }
+      o[i] = a;
+    }
+  }
+};
+
+// The residual tail's apply is the AFFINE one with dout = the masked dz its reduction wrote.  DS (two-site tail):
+// the same dz is the downsample site's output gradient, so the pass also reads xd and writes dxd with the downsample
+// site's coefficients (coef_d).
+template <int GS, int EPI, bool D2, bool DS>
 __global__ void __launch_bounds__(kT, 2) cl_bwd_apply_kernel(const float* __restrict__ x, const float* __restrict__ dout, const float* __restrict__ dout2,
                                                              float* __restrict__ dx, const Geom gm, const float* __restrict__ coef,
                                                              const float* __restrict__ save_mean, const float* __restrict__ save_w,
                                                              const float* __restrict__ gamma, const float* __restrict__ beta,
-                                                             const uint8_t* __restrict__ mask, float* __restrict__ dres) {
+                                                             const float* __restrict__ xds, float* __restrict__ dxds,
+                                                             const float* __restrict__ coef_d) {
   using S = ClShape<GS>;
   constexpr int UNROLL = 4;
-  constexpr bool MASK = (EPI & DWT_EPI_RESIDUAL) != 0;
-  constexpr bool RELU = (EPI & DWT_EPI_RELU) != 0 && !MASK;
+  constexpr bool RELU = (EPI & DWT_EPI_RELU) != 0;
+  static_assert((EPI & DWT_EPI_RESIDUAL) == 0, "the residual tail's apply runs with EPI = AFFINE on dz");
+  static_assert(!DS || (!D2 && !RELU), "the two-site tail's apply reads dz");
+  constexpr int NS = DS ? 2 : 1;
   const ClThread t(gm);
   const unsigned rows = (unsigned)gm.N * gm.HW;
   pdl_wait();                                       // the coefficients of the backward finalize launch are complete
   CL_FOR_DOMAINS(d, gm, false) {
-    float Wp[S::NSUB][S::NM], bp[S::NSUB][GS], A1[S::NSUB][S::NM], Bm[S::NSUB][S::NM], cv[S::NSUB][GS];
+    float Wp[S::NSUB][S::NM], bp[S::NSUB][GS];
+    BwdCoef<GS> cf[NS][S::NSUB];
 #pragma unroll
     for (int s = 0; s < S::NSUB; ++s) {
       const int g = t.q * S::NSUB + s;
       if constexpr (RELU)
         load_forward_map<GS, EPI>(save_w + ((size_t)d * gm.G + g) * GS * GS, save_mean + (size_t)d * gm.C + g * GS,
                                   gamma + g * GS, beta + g * GS, Wp[s], bp[s]);
-      const float* cf = coef + ((size_t)d * gm.G + g) * coef_stride(GS);
 #pragma unroll
-      for (int i = 0; i < GS; ++i) {
-        cv[s][i] = __ldg(cf + 2 * GS * GS + i);
-#pragma unroll
-        for (int j = 0; j <= i; ++j) {
-          A1[s][i * (i + 1) / 2 + j] = __ldg(cf + j * GS + i);
-          Bm[s][i * (i + 1) / 2 + j] = __ldg(cf + GS * GS + i * GS + j);
-        }
-      }
+      for (int k = 0; k < NS; ++k) cf[k][s].load((k ? coef_d : coef) + ((size_t)d * gm.G + g) * coef_stride(GS));
     }
     const size_t base = (size_t)d * rows * gm.C + 4 * t.q;
-    const float* xd = x + base;
+    const float* xp[NS];
+    float* op[NS];
+    xp[0] = x + base; op[0] = dx + base;
+    if constexpr (DS) { xp[NS - 1] = xds + base; op[NS - 1] = dxds + base; }
     const float* gd = dout + base;
     const float* gd2 = D2 ? dout2 + base : nullptr;        // second addend of the incoming gradient (see dwt_b200.h)
-    float* od = dx + base;
-    float* rd = dres + base;
-    const uint8_t* md = mask + (size_t)d * rows * t.C4 + t.q;
     sweep_rows<UNROLL, false>(t, rows, [&](unsigned r) {
-      float4 v[UNROLL], q[UNROLL], q2[D2 ? UNROLL : 1];
-      unsigned mb[UNROLL];
+      float4 v[NS][UNROLL], q[UNROLL], q2[D2 ? UNROLL : 1];
 #pragma unroll
       for (int u = 0; u < UNROLL; ++u) {
         const unsigned rr = r + u * t.rpi;
         if (rr < rows) {
-          v[u] = ldg4(xd + (size_t)rr * gm.C); q[u] = ldg4(gd + (size_t)rr * gm.C);
-          if constexpr (MASK) mb[u] = __ldg(md + (size_t)rr * t.C4);
+#pragma unroll
+          for (int k = 0; k < NS; ++k) v[k][u] = ldg4(xp[k] + (size_t)rr * gm.C);
+          q[u] = ldg4(gd + (size_t)rr * gm.C);
           if constexpr (D2) q2[u] = ldg4(gd2 + (size_t)rr * gm.C);
         }
       }
@@ -566,39 +685,26 @@ __global__ void __launch_bounds__(kT, 2) cl_bwd_apply_kernel(const float* __rest
       for (int u = 0; u < UNROLL; ++u) {
         const unsigned rr = r + u * t.rpi;
         if (rr < rows) {
-          const float e[4] = {v[u].x, v[u].y, v[u].z, v[u].w}, ge[4] = {q[u].x, q[u].y, q[u].z, q[u].w};
-          float o[4], zm[4];
+          const float ge[4] = {q[u].x, q[u].y, q[u].z, q[u].w};
 #pragma unroll
-          for (int s = 0; s < S::NSUB; ++s) {
-            float xi[GS], dz[GS];
+          for (int k = 0; k < NS; ++k) {
+            const float e[4] = {v[k][u].x, v[k][u].y, v[k][u].z, v[k][u].w};
+            float o[4];
 #pragma unroll
-            for (int c = 0; c < GS; ++c) { xi[c] = e[s * GS + c]; dz[c] = ge[s * GS + c]; }
-            if constexpr (RELU) {
-              float oi[GS];
-              apply_group<GS>(Wp[s], bp[s], xi, oi);
+            for (int s = 0; s < S::NSUB; ++s) {
+              float xi[GS], dz[GS];
 #pragma unroll
-              for (int c = 0; c < GS; ++c) dz[c] = oi[c] > 0.f ? dz[c] : 0.f;
-            }
-            if constexpr (MASK) {
+              for (int c = 0; c < GS; ++c) { xi[c] = e[s * GS + c]; dz[c] = ge[s * GS + c]; }
+              if constexpr (RELU) {
+                float oi[GS];
+                apply_group<GS>(Wp[s], bp[s], xi, oi);
 #pragma unroll
-              for (int c = 0; c < GS; ++c) { dz[c] = ((mb[u] >> (s * GS + c)) & 1u) ? dz[c] : 0.f; zm[s * GS + c] = dz[c]; }
-            }
-#pragma unroll
-            for (int i = 0; i < GS; ++i) {
-              float a = cv[s][i];
-#pragma unroll
-              for (int j = i; j < GS; ++j) a = fmaf(A1[s][j * (j + 1) / 2 + i], dz[j], a);
-#pragma unroll
-              for (int j = 0; j < GS; ++j) {
-                const int hi = i > j ? i : j, lo = i > j ? j : i;
-                a = fmaf(Bm[s][hi * (hi + 1) / 2 + lo], xi[j], a);
+                for (int c = 0; c < GS; ++c) dz[c] = oi[c] > 0.f ? dz[c] : 0.f;
               }
-              o[s * GS + i] = a;
+              cf[k][s].apply(dz, xi, o + s * GS);
             }
+            *reinterpret_cast<float4*>(op[k] + (size_t)rr * gm.C) = make_float4(o[0], o[1], o[2], o[3]);
           }
-          *reinterpret_cast<float4*>(od + (size_t)rr * gm.C) = make_float4(o[0], o[1], o[2], o[3]);
-          // gradient of the identity branch of relu(z + identity): the masked dout itself
-          if constexpr (MASK) { if (dres != nullptr) *reinterpret_cast<float4*>(rd + (size_t)rr * gm.C) = make_float4(zm[0], zm[1], zm[2], zm[3]); }
         }
       }
     });
@@ -616,10 +722,13 @@ __global__ void __launch_bounds__(kT, 2) cl_bwd_apply_kernel(const float* __rest
   if ((E_) == 3) { constexpr int kEPI = 3; __VA_ARGS__; }                 \
   else if ((E_) == 1) { constexpr int kEPI = 1; __VA_ARGS__; }            \
   else { constexpr int kEPI = 0; __VA_ARGS__; }
-// backward: 7 = AFFINE with the ReLU mask of the residual tail read from the forward's byte map
+// backward reduction: 7 = AFFINE with the ReLU mask of the residual tail read from the forward's byte map
 #define CL_EPI_BWD(E_, ...)                                               \
   if ((E_) == 7) { constexpr int kEPI = 7; __VA_ARGS__; }                 \
   else CL_EPI(E_, __VA_ARGS__)
+#define CL_D2(P_, ...)                                                    \
+  if (P_) { constexpr bool kD2 = true; __VA_ARGS__; }                     \
+  else { constexpr bool kD2 = false; __VA_ARGS__; }
 
 inline bool use_pdl() {
   static const bool on = [] { const char* v = getenv("DWT_PDL"); return v != nullptr && v[0] == '1'; }();
@@ -655,42 +764,61 @@ bool cl_supports(int C, int GS) {
 int cl_fwd_width(int C, int GS) { return (C / 4) * (4 / GS) * (GS + GS * (GS + 1) / 2); }
 int cl_bwd_width(int C, int GS) { return (C / 4) * (4 / GS) * (GS * GS + GS); }
 
+
 void cl_stats(const float* x, const Geom& gm, int nctas, int gz, float* partial, float* shift, cudaStream_t st) {
   CL_GS(gm.GS, (cl_stats_kernel<kGS><<<cl_grid(gm, nctas, gz), kT, 0, st>>>(x, gm, partial, shift)));
 }
 inline dim3 fin_block(const Geom& gm) { const int c4 = gm.C / 4; return dim3(32, c4 < kFinQ ? c4 : kFinQ, gm.D); }
-void cl_fwd_finalize(const float* partial, int nrows, const float* shift, const Geom& gm, const FwdFin& fin, cudaStream_t st) {
-  const dim3 b = fin_block(gm);
-  CL_GS(gm.GS, (launch_k(cl_fwd_finalize_kernel<kGS>, dim3((gm.C / 4) / b.y), b, st, use_pdl(), partial, nrows, shift, gm, fin)));
+void cl_fwd_finalize(const float* partial, int nrows, const float* shift, const Geom& gm, const FwdFin& fin, cudaStream_t st,
+                     const FwdFin* fin2, size_t pstride, size_t sstride) {
+  const dim3 b = fin_block(gm), g((gm.C / 4) / b.y, fin2 ? 2 : 1);
+  CL_GS(gm.GS, (launch_k(cl_fwd_finalize_kernel<kGS>, g, b, st, use_pdl(), partial, pstride, nrows, shift, sstride, gm, fin, fin2 ? *fin2 : fin)));
 }
 void cl_apply(const float* x, float* y, const Geom& gm, int nctas, int gz, int epi, const float* mean, const float* w,
               const float* gamma, const float* beta, const float* residual, uint8_t* mask, cudaStream_t st) {
+  const float* nul = nullptr;
   if (epi == 7) {
-    CL_GS(gm.GS, (launch_k(cl_apply_kernel<kGS, 7>, cl_grid(gm, nctas, gz), dim3(kT), st, use_pdl(), x, y, gm, mean, w, gamma, beta, residual, mask)));
+    CL_GS(gm.GS, (launch_k(cl_apply_kernel<kGS, 7, false>, cl_grid(gm, nctas, gz), dim3(kT), st, use_pdl(), x, y, gm, mean, w, gamma, beta, residual, mask,
+                           nul, nul, nul, nul)));
     return;
   }
-  CL_GS(gm.GS, CL_EPI(epi, (launch_k(cl_apply_kernel<kGS, kEPI>, cl_grid(gm, nctas, gz), dim3(kT), st, use_pdl(), x, y, gm, mean, w, gamma, beta,
-                                     (const float*)nullptr, (uint8_t*)nullptr))));
+  CL_GS(gm.GS, CL_EPI(epi, (launch_k(cl_apply_kernel<kGS, kEPI, false>, cl_grid(gm, nctas, gz), dim3(kT), st, use_pdl(), x, y, gm, mean, w, gamma, beta,
+                                     nul, (uint8_t*)nullptr, nul, nul, nul, nul))));
+}
+void cl_tail2_apply(const float* x, const float* xd, float* y, const Geom& gm, int nctas, int gz, const float* mean, const float* w,
+                    const float* gamma, const float* beta, const float* mean_d, const float* w_d, const float* gamma_d,
+                    const float* beta_d, uint8_t* mask, cudaStream_t st) {
+  CL_GS(gm.GS, (launch_k(cl_apply_kernel<kGS, 7, true>, cl_grid(gm, nctas, gz), dim3(kT), st, use_pdl(), x, y, gm, mean, w, gamma, beta, xd, mask,
+                         mean_d, w_d, gamma_d, beta_d)));
 }
 void cl_bwd_reduce(const float* x, const float* dout, const float* dout2, const Geom& gm, int nctas, int gz, int epi, const float* mean, const float* w,
-                   const float* gamma, const float* beta, const uint8_t* mask, float* partial, cudaStream_t st) {
-  if (dout2) { CL_GS(gm.GS, CL_EPI_BWD(epi, (cl_bwd_reduce_kernel<kGS, kEPI, true><<<cl_grid(gm, nctas, gz), kT, 0, st>>>(x, dout, dout2, gm, mean, w, gamma, beta, mask, partial)))); }
-  else { CL_GS(gm.GS, CL_EPI_BWD(epi, (cl_bwd_reduce_kernel<kGS, kEPI, false><<<cl_grid(gm, nctas, gz), kT, 0, st>>>(x, dout, dout2, gm, mean, w, gamma, beta, mask, partial)))); }
+                   const float* gamma, const float* beta, const uint8_t* mask, float* dz, float* partial, cudaStream_t st) {
+  const float* nul = nullptr;
+  CL_GS(gm.GS, CL_D2(dout2, CL_EPI_BWD(epi, (cl_bwd_reduce_kernel<kGS, kEPI, kD2, false><<<cl_grid(gm, nctas, gz), kT, 0, st>>>(
+                                                x, dout, dout2, gm, mean, w, gamma, beta, mask, dz, partial, nul, nul, 0)))));
 }
-void cl_bwd_finalize(const float* partial, int nrows, const Geom& gm, const BwdFin& fin, cudaStream_t st) {
-  const dim3 b = fin_block(gm);
-  CL_GS(gm.GS, (launch_k(cl_bwd_finalize_kernel<kGS>, dim3((gm.C / 4) / b.y), b, st, use_pdl(), partial, nrows, gm, fin)));
+void cl_tail2_bwd_reduce(const float* x, const float* xd, const float* dout, const float* dout2, const Geom& gm, int nctas, int gz,
+                         const float* mean, const float* mean_d, const uint8_t* mask, float* dz, float* partial, size_t pstride,
+                         cudaStream_t st) {
+  const float* nul = nullptr;
+  CL_GS(gm.GS, CL_D2(dout2, (cl_bwd_reduce_kernel<kGS, 7, kD2, true><<<cl_grid(gm, nctas, gz), kT, 0, st>>>(
+                                x, dout, dout2, gm, mean, nul, nul, nul, mask, dz, partial, xd, mean_d, pstride))));
+}
+void cl_bwd_finalize(const float* partial, int nrows, const Geom& gm, const BwdFin& fin, cudaStream_t st, const BwdFin* fin2, size_t pstride) {
+  const dim3 b = fin_block(gm), g((gm.C / 4) / b.y, fin2 ? 2 : 1);
+  CL_GS(gm.GS, (launch_k(cl_bwd_finalize_kernel<kGS>, g, b, st, use_pdl(), partial, pstride, nrows, gm, fin, fin2 ? *fin2 : fin)));
 }
 void cl_bwd_apply(const float* x, const float* dout, const float* dout2, float* dx, const Geom& gm, int nctas, int gz, int epi, const float* coef,
-                  const float* mean, const float* w, const float* gamma, const float* beta, const uint8_t* mask, float* dres,
-                  cudaStream_t st) {
-  if (dout2) {
-    CL_GS(gm.GS, CL_EPI_BWD(epi, (launch_k(cl_bwd_apply_kernel<kGS, kEPI, true>, cl_grid(gm, nctas, gz), dim3(kT), st, use_pdl(), x, dout, dout2, dx, gm, coef, mean, w, gamma,
-                                         beta, mask, dres))));
-  } else {
-    CL_GS(gm.GS, CL_EPI_BWD(epi, (launch_k(cl_bwd_apply_kernel<kGS, kEPI, false>, cl_grid(gm, nctas, gz), dim3(kT), st, use_pdl(), x, dout, dout2, dx, gm, coef, mean, w, gamma,
-                                         beta, mask, dres))));
-  }
+                  const float* mean, const float* w, const float* gamma, const float* beta, cudaStream_t st) {
+  const float* nul = nullptr;
+  CL_GS(gm.GS, CL_D2(dout2, CL_EPI(epi, (launch_k(cl_bwd_apply_kernel<kGS, kEPI, kD2, false>, cl_grid(gm, nctas, gz), dim3(kT), st, use_pdl(), x, dout,
+                                                  dout2, dx, gm, coef, mean, w, gamma, beta, nul, (float*)nullptr, nul)))));
+}
+void cl_tail2_bwd_apply(const float* x, const float* xd, const float* dz, float* dx, float* dxd, const Geom& gm, int nctas, int gz,
+                        const float* coef, const float* coef_d, cudaStream_t st) {
+  const float* nul = nullptr;
+  CL_GS(gm.GS, (launch_k(cl_bwd_apply_kernel<kGS, 1, false, true>, cl_grid(gm, nctas, gz), dim3(kT), st, use_pdl(), x, dz, nul, dx, gm, coef,
+                         nul, nul, nul, nul, xd, dxd, coef_d)));
 }
 
 }  // namespace dwt

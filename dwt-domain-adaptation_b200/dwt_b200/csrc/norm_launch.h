@@ -67,16 +67,30 @@ int tc_bwd_apply(const float* x, const float* dout, float* dx, const Geom& gm, i
 bool cl_supports(int C, int GS);
 int cl_fwd_width(int C, int GS);
 int cl_bwd_width(int C, int GS);
+// The finalize launches serve a second site (the two-site tail) when fin2 is given: its partial rows start at
+// partial + pstride, its pilot shifts at shift + sstride.
 void cl_stats(const float* x, const Geom& gm, int nctas, int gz, float* partial, float* shift, cudaStream_t st);
-void cl_fwd_finalize(const float* partial, int nrows, const float* shift, const Geom& gm, const FwdFin& fin, cudaStream_t st);
+void cl_fwd_finalize(const float* partial, int nrows, const float* shift, const Geom& gm, const FwdFin& fin, cudaStream_t st,
+                     const FwdFin* fin2 = nullptr, size_t pstride = 0, size_t sstride = 0);
 void cl_apply(const float* x, float* y, const Geom& gm, int nctas, int gz, int epi, const float* mean, const float* w,
               const float* gamma, const float* beta, const float* residual, uint8_t* mask, cudaStream_t st);
+// epi 7 (residual tail): masks dout (+ dout2) with the byte map and writes the masked gradient to dz
 void cl_bwd_reduce(const float* x, const float* dout, const float* dout2, const Geom& gm, int nctas, int gz, int epi, const float* mean, const float* w,
-                   const float* gamma, const float* beta, const uint8_t* mask, float* partial, cudaStream_t st);
-void cl_bwd_finalize(const float* partial, int nrows, const Geom& gm, const BwdFin& fin, cudaStream_t st);
+                   const float* gamma, const float* beta, const uint8_t* mask, float* dz, float* partial, cudaStream_t st);
+void cl_bwd_finalize(const float* partial, int nrows, const Geom& gm, const BwdFin& fin, cudaStream_t st,
+                     const BwdFin* fin2 = nullptr, size_t pstride = 0);
+// epi 0, 1 or 3; the residual tail runs it with epi 1 on the dz of its reduction
 void cl_bwd_apply(const float* x, const float* dout, const float* dout2, float* dx, const Geom& gm, int nctas, int gz, int epi, const float* coef,
-                  const float* mean, const float* w, const float* gamma, const float* beta, const uint8_t* mask, float* dres,
-                  cudaStream_t st);
+                  const float* mean, const float* w, const float* gamma, const float* beta, cudaStream_t st);
+// two-site tail relu(site(x) + site_d(xd)): site's epilogue AFFINE|RELU|RESIDUAL, site_d's AFFINE
+void cl_tail2_apply(const float* x, const float* xd, float* y, const Geom& gm, int nctas, int gz, const float* mean, const float* w,
+                    const float* gamma, const float* beta, const float* mean_d, const float* w_d, const float* gamma_d,
+                    const float* beta_d, uint8_t* mask, cudaStream_t st);
+void cl_tail2_bwd_reduce(const float* x, const float* xd, const float* dout, const float* dout2, const Geom& gm, int nctas, int gz,
+                         const float* mean, const float* mean_d, const uint8_t* mask, float* dz, float* partial, size_t pstride,
+                         cudaStream_t st);
+void cl_tail2_bwd_apply(const float* x, const float* xd, const float* dz, float* dx, float* dxd, const Geom& gm, int nctas, int gz,
+                        const float* coef, const float* coef_d, cudaStream_t st);
 
 // channels-last max-pool (pool.cu)
 void maxpool_fwd_launch(const float* x, float* y, uint8_t* idx, int N, int H, int W, int C, int OH, int OW, int k, int s, int p,

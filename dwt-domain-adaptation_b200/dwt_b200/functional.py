@@ -106,7 +106,7 @@ class _NormFunction(torch.autograd.Function):
         # backward of relu(z + residual): dz = dout * (out > 0) is also the residual's gradient
         ctx.residual_mode = None
         if mask is not None:
-            # channels-last: both backward kernels mask dout with the saved bits, bwd_apply also writes dz
+            # channels-last: the backward reduction masks dout with the saved bits and writes dz, bwd_apply reads it
             ctx.save_for_backward(x, save_mean, save_w, gamma_c, beta_c, mask)
             ctx.residual_mode = "mask"
         elif residual is not None:
@@ -145,11 +145,10 @@ class _NormFunction(torch.autograd.Function):
         dx = torch.empty_like(x)
         want_affine = gamma_c is not None and (ctx.needs_input_grad[1] or ctx.needs_input_grad[2])
         d_res = None
-        if ctx.needs_input_grad[3]:
-            if ctx.residual_mode == "mask":
-                d_res = torch.empty_like(x)
-            elif ctx.residual_mode == "aten":
-                d_res = dout
+        if ctx.residual_mode == "mask":
+            d_res = torch.empty_like(x)              # dz, written even when the residual needs no gradient
+        elif ctx.residual_mode == "aten" and ctx.needs_input_grad[3]:
+            d_res = dout
         dgamma = torch.empty(c, dtype=torch.float32, device=dev) if want_affine else None
         dbeta = torch.empty(c, dtype=torch.float32, device=dev) if want_affine else None
         ws = nv.workspace(dev, n, c, hw, gs, n_domains)
@@ -167,12 +166,102 @@ class _NormFunction(torch.autograd.Function):
         nv.check(rc)
         if want_affine:
             dgamma, dbeta = dgamma.view(gshape), dbeta.view(gshape)
-        return (dx, dgamma, dbeta, d_res) + (None,) * 9
+        return (dx, dgamma, dbeta, d_res if ctx.needs_input_grad[3] else None) + (None,) * 9
+
+
+class _TailPairFunction(torch.autograd.Function):
+    """out = relu(site(x) + site_d(xd)): the residual tail of a downsampling Bottleneck, both norm sites (domain-triple,
+    gamma/beta each) and the ReLU in the kernels of dwt_tail2_fwd / dwt_tail2_bwd.  Channels-last, training statistics.
+    `sites` holds per site (running pairs, eps, momentum, update_running); the running buffers get the same EMA updates
+    as from the two-call composition."""
+
+    @staticmethod
+    def forward(ctx, x, xd, gamma, beta, gamma_d, beta_d, kind, group_size, n_domains, sites):
+        lib = nv.lib()
+        gs = group_size if kind == "whiten" else 1
+        if not (x.dim() == 4 and x.shape == xd.shape and _dense(x, gs)[4] and _dense(xd, gs)[4]):
+            raise ValueError("the two-site tail takes two channels-last tensors of one shape with a channels-last build")
+        if x.shape[0] % n_domains != 0:
+            raise ValueError(f"batch of {x.shape[0]} does not split into {n_domains} domains")
+        n_all, c = x.shape[0], x.shape[1]
+        hw = x.shape[2] * x.shape[3]
+        n = n_all // n_domains
+        dev = nv.require_cuda(x, xd, gamma, beta, gamma_d, beta_d, *[t for run, *_ in sites for pair in run for t in pair])
+        params = [(gamma, beta), (gamma_d, beta_d)]
+        c_sites = (nv.TailSite * 2)()
+        keep = []                                    # save tensors and pointer arrays alive across the call
+        saved = []
+        for k, (inp, (g, b), (running, eps, momentum, update)) in enumerate(zip((x, xd), params, sites)):
+            for d, (rm_t, rv_t) in enumerate(running):
+                _check_param(f"running mean of domain {d}", rm_t, c)
+                _check_param(f"running second moment of domain {d}", rv_t, c * gs)
+            _check_param("gamma / weight", g, c)
+            _check_param("beta / bias", b, c)
+            g_c, b_c = g.detach().reshape(-1).contiguous(), b.detach().reshape(-1).contiguous()
+            save_mean = torch.empty(n_domains, c, dtype=torch.float32, device=dev)
+            save_w = torch.empty(n_domains, c // gs, gs, gs, dtype=torch.float32, device=dev)
+            rm = nv.ptr_array([pr[0] for pr in running]) if update else None
+            rv = nv.ptr_array([pr[1] for pr in running]) if update else None
+            c_sites[k] = nv.TailSite(inp.data_ptr(), eps, momentum, int(update), rm, rv, g_c.data_ptr(), b_c.data_ptr(),
+                                     save_mean.data_ptr(), save_w.data_ptr(), None, None, None)
+            keep += [g_c, b_c, rm, rv]
+            saved += [save_mean, save_w, g_c]
+        y = torch.empty_like(x)
+        mask = torch.empty(x.numel() // 4, dtype=torch.uint8, device=dev)
+        ws = nv.workspace(dev, n, c, hw, gs, n_domains)
+        nv_kind = nv.KIND_WHITEN if kind == "whiten" else nv.KIND_BN
+        with torch.cuda.device(dev):
+            rc = lib.dwt_tail2_fwd(nv_kind, c_sites, nv.ptr(y), nv.ptr(mask), n, c, hw, gs, n_domains, nv.ptr(ws), ws.numel(),
+                                   nv.stream_ptr(dev))
+        nv.check(rc)
+        nv.poll_status(dev)
+        seen = set()
+        for running, _, _, update in sites:
+            for buf in (t for pair in running for t in pair) if update else ():
+                if id(buf) not in seen:              # see _NormFunction.forward
+                    seen.add(id(buf))
+                    torch.autograd.graph.increment_version(buf)
+        ctx.save_for_backward(x, xd, mask, *saved)
+        ctx.cfg = (nv_kind, gs, n_domains, n, c, hw, [s[1] for s in sites], gamma.shape, gamma_d.shape)
+        return y
+
+    @staticmethod
+    def backward(ctx, dout):
+        lib = nv.lib()
+        x, xd, mask, mean0, w0, g0, mean1, w1, g1 = ctx.saved_tensors
+        nv_kind, gs, n_domains, n, c, hw, eps, gshape, gshape_d = ctx.cfg
+        dout2 = ctx.__dict__.pop("_dwt_extra_grad", None)      # parked by fork_for_sum, as for _NormFunction
+        if dout2 is not None and not (dout2.shape == dout.shape and dout2.dtype == torch.float32
+                                      and dout2.is_contiguous(memory_format=torch.channels_last)):
+            dout, dout2 = dout + dout2, None
+        dout = dout.contiguous(memory_format=torch.channels_last)
+        dev = nv.require_cuda(dout)
+        dz = torch.empty_like(x)
+        dx, dxd = torch.empty_like(x), torch.empty_like(xd)
+        grads = [torch.empty(2, c, dtype=torch.float32, device=dev) for _ in range(2)]   # (dgamma, dbeta) per site
+        c_sites = (nv.TailSite * 2)()
+        for k, (inp, mean, w, g, d_in, gr) in enumerate(zip((x, xd), (mean0, mean1), (w0, w1), (g0, g1), (dx, dxd), grads)):
+            c_sites[k] = nv.TailSite(inp.data_ptr(), eps[k], 0.0, 0, None, None, g.data_ptr(), g.data_ptr(), mean.data_ptr(),
+                                     w.data_ptr(), d_in.data_ptr(), gr[0].data_ptr(), gr[1].data_ptr())
+        ws = nv.workspace(dev, n, c, hw, gs, n_domains)
+        with torch.cuda.device(dev):
+            rc = lib.dwt_tail2_bwd(nv_kind, c_sites, nv.ptr(dout), nv.ptr(dout2), nv.ptr(mask), nv.ptr(dz), n, c, hw, gs, n_domains,
+                                   nv.ptr(ws), ws.numel(), nv.stream_ptr(dev))
+        nv.check(rc)
+        return (dx, dxd, grads[0][0].view(gshape), grads[0][1].view(gshape), grads[1][0].view(gshape_d),
+                grads[1][1].view(gshape_d)) + (None,) * 4
+
+
+def tail_pair(x, xd, gamma, beta, gamma_d, beta_d, *, kind, group_size, n_domains, sites):
+    """relu(site(x) + site_d(xd)) in training mode on channels-last tensors of one shape (see _TailPairFunction);
+    sites = ((running, eps, momentum, update_running) of site, the same of site_d)."""
+    return _TailPairFunction.apply(x, xd, gamma, beta, gamma_d, beta_d, kind, group_size, n_domains,
+                                   [(r, float(e), float(m), bool(u)) for r, e, m, u in sites])
 
 
 class _ForkForSum(torch.autograd.Function):
     """a, b = fork(y): two aliases of y whose gradients are NOT summed by autograd.  y must be the output of a
-    _NormFunction node (the producer): backward hands the first gradient on as y's gradient and parks the second on the
+    _NormFunction or _TailPairFunction node (the producer): backward hands the first gradient on as y's gradient and parks the second on the
     producer's node, whose backward passes it to the kernels as the second addend (dwt_whiten_bwd's dout2).  If y gets
     other gradients as well, autograd adds them to the first one as usual -- the parked addend is independent of that."""
 
@@ -198,7 +287,7 @@ def fork_for_sum(y):
     (a, b), two aliases of y.  Falls back to (y, y) when y was not produced by one of this package's norm sites or no
     gradient is being recorded; results are identical either way."""
     fn = getattr(y, "grad_fn", None)
-    if not torch.is_grad_enabled() or fn is None or not isinstance(fn, _NormFunction._backward_cls):
+    if not torch.is_grad_enabled() or fn is None or not isinstance(fn, (_NormFunction._backward_cls, _TailPairFunction._backward_cls)):
         return y, y
     return _ForkForSum.apply(y)
 

@@ -27,6 +27,7 @@ from __future__ import annotations
 import torch
 import torch.nn as nn
 
+from . import _native as nv
 from . import functional as F
 
 
@@ -58,6 +59,17 @@ class DomainTripleNorm(nn.Module):
             raise ValueError('expected 4D input (got {}D input)'.format(x.dim()))
         if replicated:
             return self._forward_replicated(x, mods, gamma, beta, relu, residual, count_batches)
+        running, eps, momentum, update = self._running_args(mods, count_batches)
+        if not self.kernel_epilogue:
+            y = F.norm(x, None, None, kind=self.kind, group_size=self.group_size, n_domains=self.n_domains,
+                       training_stats=True, eps=eps, momentum=momentum, update_running=update, running=running)
+            return self._tensor_epilogue(y, gamma, beta, relu, residual)
+        return F.norm(x, gamma, beta, kind=self.kind, group_size=self.group_size, n_domains=self.n_domains,
+                      training_stats=True, eps=eps, momentum=momentum, update_running=update,
+                      running=running, relu=relu, residual=residual)
+
+    def _running_args(self, mods, count_batches):
+        """-> (running buffer pairs, eps, momentum, update_running) of a training-statistics call on mods."""
         m0 = mods[0]
         if self.kind == "whiten":
             running = [(m.running_mean, m.running_variance) for m in mods]
@@ -70,14 +82,28 @@ class DomainTripleNorm(nn.Module):
             running = [(m.running_mean, m.running_var) for m in mods]
             eps = m0.eps
             momentum = m0.momentum if m0.momentum is not None else 1.0 / m0.num_batches_tracked.item()
-        update = m0.training and m0.track_running_stats
-        if not self.kernel_epilogue:
-            y = F.norm(x, None, None, kind=self.kind, group_size=self.group_size, n_domains=self.n_domains,
-                       training_stats=True, eps=eps, momentum=momentum, update_running=update, running=running)
-            return self._tensor_epilogue(y, gamma, beta, relu, residual)
-        return F.norm(x, gamma, beta, kind=self.kind, group_size=self.group_size, n_domains=self.n_domains,
-                      training_stats=True, eps=eps, momentum=momentum, update_running=update,
-                      running=running, relu=relu, residual=residual)
+        return running, eps, momentum, m0.training and m0.track_running_stats
+
+    def forward_with_downsample(self, x, domain_modules, gamma, beta, xd, down, down_modules, down_gamma, down_beta,
+                                count_batches=True):
+        """relu(self(x) + down(xd)): the residual tail of a downsampling Bottleneck (resnet50_dwt_mec_officehome.py:
+        236-240), `down` being the downsample branch's DomainTripleNorm.  Channels-last tensors of one shape with
+        both sites on the fused-epilogue kernels run as ONE two-site call (functional.tail_pair: the identity tensor is
+        never written); anything else runs the two-call composition down(xd) -> self(x, residual=identity).  Results,
+        gradients and running buffers are the same either way."""
+        mods, down_mods = list(domain_modules), list(down_modules)
+        pair = (self.kernel_epilogue and down.kernel_epilogue and self.kind == down.kind
+                and self.group_size == down.group_size and self.n_domains == down.n_domains
+                and len(mods) == len(down_mods) == self.n_domains and x.dim() == 4 and x.shape == xd.shape
+                and all(t.is_contiguous(memory_format=torch.channels_last) and not t.is_contiguous() for t in (x, xd))
+                and nv.channels_last_supported(x.shape[1], self.group_size))
+        if not pair:
+            identity = down(xd, down_mods, down_gamma, down_beta, relu=False, count_batches=count_batches)
+            return self(x, mods, gamma, beta, True, residual=identity, count_batches=count_batches)
+        down_args = down._running_args(down_mods, count_batches)
+        site_args = self._running_args(mods, count_batches)
+        return F.tail_pair(x, xd, gamma, beta, down_gamma, down_beta, kind=self.kind, group_size=self.group_size,
+                           n_domains=self.n_domains, sites=(site_args, down_args))
 
     @staticmethod
     def _tensor_epilogue(y, gamma, beta, relu, residual):

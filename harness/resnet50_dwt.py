@@ -142,8 +142,22 @@ class Bottleneck(_SiteOwner):
         xa, xb = self._fork(x) if (self._fork is not None and self.training) else (x, x)
         out = self._site("1", self.conv1(xa), relu=True)
         out = self._site("2", self.conv2(out), relu=True)
-        identity = xb if self.downsample is None else self._site("downsample", self.downsample(xb), relu=False)
-        return self._site("3", self.conv3(out), relu=True, residual=identity)
+        if self.downsample is None:
+            return self._site("3", self.conv3(out), relu=True, residual=xb)
+        tail = getattr(self, "_fused_3", None) if (self.training and not _REPLICATED[0]) else None
+        if tail is None:
+            identity = self._site("downsample", self.downsample(xb), relu=False)
+            return self._site("3", self.conv3(out), relu=True, residual=identity)
+        # fused training sites: relu(bn3(conv3) + downsample_bn(downsample)) as one two-site call, the identity tensor
+        # never written (DomainTripleNorm.forward_with_downsample)
+        xd = self.downsample(xb)
+        names, gname, bname, whiten = self._sites["3"]
+        dnames, dgname, dbname, _ = self._sites["downsample"]
+        unwrap = (lambda m: m.wh) if whiten else (lambda m: m)
+        return tail.forward_with_downsample(
+            self.conv3(out), [unwrap(getattr(self, n)) for n in names], getattr(self, gname), getattr(self, bname),
+            xd, self._fused_downsample, [unwrap(getattr(self, n)) for n in dnames], getattr(self, dgname),
+            getattr(self, dbname), count_batches=not _BATCHED_COUNTERS[0])
 
 
 class ResNet50DWT(_SiteOwner):

@@ -18,6 +18,8 @@
  *                     resnet50_dwt_mec_officehome.py:59-63,220-222, when asked)
  *   dwt_whiten_bwd   autograd through the above     utils/whitening.py:41-55
  *   dwt_bn_fwd/bwd   _BatchNorm.forward             utils/batch_norm.py:54-69
+ *   dwt_tail2_fwd/bwd  the residual tail of a downsampling Bottleneck: two norm sites and the ReLU in one pass
+ *                    resnet50_dwt_mec_officehome.py:236-240
  *   dwt_mec_fwd_bwd  MinEntropyConsensusLoss.forward utils/consensus_loss.py:11-24
  *   dwt_head_loss_fwd_bwd  the training loop's NLL + lambda*MEC   resnet50_dwt_mec_officehome.py:421-428
  *   dwt_augment_pair the loader's two target views  resnet50_dwt_mec_officehome.py:481-492,526-542;
@@ -44,7 +46,7 @@
 extern "C" {
 #endif
 
-#define DWT_B200_ABI_VERSION 5
+#define DWT_B200_ABI_VERSION 6
 #define DWT_MAX_DOMAINS 4
 #define DWT_MAX_GROUP_SIZE 64
 
@@ -125,9 +127,9 @@ DWT_API int dwt_whiten_fwd(const float *x, float *y, int64_t N, int64_t C, int64
  * forward's output (after the epilogue, if any).  dgamma/dbeta [C] are written
  * (summed over domains) when the epilogue has AFFINE; pass NULL otherwise.
  * Epilogue AFFINE|RELU|RESIDUAL (channels-last only): dout is the gradient of relu(z + residual); the ReLU mask is
- * read from the forward's relu_mask and, when dresidual is not NULL, the masked gradient dout * (out > 0) -- the
- * gradient of the identity branch -- is written there in the same pass (resnet50_dwt_mec_officehome.py:239-240).
- * Without RESIDUAL pass relu_mask = dresidual = NULL.
+ * read from the forward's relu_mask and the masked gradient dout * (out > 0) -- the gradient of the identity branch
+ * -- is written to dresidual (required, tensor-sized) by the reduction pass; the apply pass reads it back instead of
+ * dout and the mask (resnet50_dwt_mec_officehome.py:239-240).  Without RESIDUAL pass relu_mask = dresidual = NULL.
  */
 DWT_API int dwt_whiten_bwd(const float *x, const float *dout, const float *dout2, float *dx, int64_t N, int64_t C, int64_t HW,
                    int group_size, int n_domains, int mode, float eps, const float *save_mean,
@@ -151,6 +153,43 @@ DWT_API int dwt_bn_bwd(const float *x, const float *dout, const float *dout2, fl
                int n_domains, int mode, const float *save_mean, const float *save_invstd,
                const float *weight, const float *bias, const uint8_t *relu_mask, float *dresidual, int epilogue,
                float *dweight, float *dbias, void *workspace, size_t workspace_bytes, dwt_stream_t stream);
+
+/*
+ * Two-site residual tail of a downsampling Bottleneck (block 0 of a stage, resnet50_dwt_mec_officehome.py:236-240),
+ * training mode, channels-last only:
+ *   out = relu(site(x) + site_d(xd)),   site(x)    = gamma   W   (x  - mu)   + beta     (the norm site after conv3)
+ *                                       site_d(xd) = gamma_d W_d (xd - mu_d) + beta_d   (the downsample branch's site)
+ * sites[0] describes site, sites[1] site_d; both have the same N, C, HW, group_size and n_domains.  The identity
+ * tensor site_d(xd) is never written.  Bit for bit the same as the two-call composition
+ *   dwt_*_fwd(xd -> identity, AFFINE);  dwt_*_fwd(x -> out, AFFINE|RELU|RESIDUAL, residual = identity)
+ * and its backward (dwt_*_bwd of both sites, the second fed the first's dresidual), including running-statistic
+ * updates and, per site, the non-positive-definite handling of DWT_STATUS_NOT_PD.
+ *   kind        DWT_KIND_WHITEN (as dwt_whiten_*, group_size 1, 2, 4) or DWT_KIND_BN (as dwt_bn_*, group_size 1)
+ *   relu_mask   the byte map of dwt_whiten_fwd's RESIDUAL epilogue: written by fwd, read by bwd
+ *   dz          bwd: tensor-sized scratch, receives dout * (out > 0) (the gradient of both sites' outputs)
+ *   dout2       NULL, or a second addend of the incoming gradient, as for dwt_whiten_bwd
+ * The workspace is sized by dwt_workspace_bytes for the same geometry.
+ */
+#define DWT_KIND_WHITEN 0
+#define DWT_KIND_BN 1
+typedef struct {
+  const float *x;              /* the site's input [n_domains*N, HW, C], 16-byte aligned                         */
+  float eps, momentum;         /* as in dwt_whiten_fwd / dwt_bn_fwd (momentum = batch norm's factor)             */
+  int update_running;          /* fwd: apply the EMA to running_mean / running_cov (batch norm: running_var)     */
+  float *const *running_mean;  /* [n_domains], may alias across domains; read only when update_running         */
+  float *const *running_cov;
+  const float *gamma, *beta;   /* [C], required                                                                  */
+  float *save_mean, *save_w;   /* [n_domains, C], [n_domains, C/gs, gs, gs]: written by fwd, read by bwd        */
+  float *dx;                   /* bwd: gradient of x                                                             */
+  float *dgamma, *dbeta;       /* bwd: [C] (summed over domains), or both NULL                                    */
+} dwt_tail_site;
+
+DWT_API int dwt_tail2_fwd(int kind, const dwt_tail_site *sites, float *y, uint8_t *relu_mask, int64_t N, int64_t C,
+                  int64_t HW, int group_size, int n_domains, void *workspace, size_t workspace_bytes,
+                  dwt_stream_t stream);
+DWT_API int dwt_tail2_bwd(int kind, const dwt_tail_site *sites, const float *dout, const float *dout2,
+                  const uint8_t *relu_mask, float *dz, int64_t N, int64_t C, int64_t HW, int group_size,
+                  int n_domains, void *workspace, size_t workspace_bytes, dwt_stream_t stream);
 
 /*
  * Min-Entropy-Consensus loss, forward and both gradients in one launch.
