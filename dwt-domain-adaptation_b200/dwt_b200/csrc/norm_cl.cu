@@ -127,7 +127,14 @@ __global__ void __launch_bounds__(kT, 3) cl_stats_kernel(const float* __restrict
   pdl_launch_dependents();
   CL_FOR_DOMAINS(d, gm, true) {
     const float* xd = x + (size_t)d * rows * gm.C + 4 * t.q;
-    // pilot shift: mean of the first <= 8 rows of the domain, per channel (every thread of a column agrees)
+    // pilot shift K, per channel (every thread of a column agrees): the mean of the first <= 8 rows of the domain,
+    // unless they sit far from the rest of it.  The one-pass moments lose digits in proportion to (K - mean)^2 / var:
+    // a first image whose top row sat 30 sigma off cost 1.1e-4 of the stem site's covariance at the benchmark's size
+    // (test_channels_last_fp64.py).  So 8 rows spread over the domain are read as well (the middle pixel, for square
+    // images, of the image at row (2k+1) * rows / 16: never the same border pixel of 8 images), and where their mean
+    // lies more than 20 of their standard deviations from K, K moves to it.  The threshold sits above what real
+    // activations show (at most 14 over the sites of 20 training steps), so they keep the first rows' K and their
+    // statistics bit for bit.
     float K[4] = {0.f, 0.f, 0.f, 0.f};
     {
       const unsigned np = rows < 8 ? rows : 8;
@@ -137,6 +144,21 @@ __global__ void __launch_bounds__(kT, 3) cl_stats_kernel(const float* __restrict
       }
 #pragma unroll
       for (int c = 0; c < 4; ++c) K[c] /= (float)np;
+      if (rows > 8) {
+        float s1[4] = {0.f, 0.f, 0.f, 0.f}, s2[4] = {0.f, 0.f, 0.f, 0.f};   // moments of the spread rows around K
+        const size_t mid = (size_t)gm.HW / 2 + (size_t)sqrtf((float)gm.HW) / 2;
+        for (unsigned k = 0; k < 8; ++k) {
+          const float4 v = ldg4(xd + ((2 * (size_t)k + 1) * rows / 16 + mid) % rows * gm.C);
+          const float e[4] = {v.x - K[0], v.y - K[1], v.z - K[2], v.w - K[3]};
+#pragma unroll
+          for (int c = 0; c < 4; ++c) { s1[c] += e[c]; s2[c] = fmaf(e[c], e[c], s2[c]); }
+        }
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+          const float dk = s1[c] * 0.125f;                      // spread mean - K; spread variance = s2 / 8 - dk^2
+          if (401.f * dk * dk > 400.f * (s2[c] * 0.125f)) K[c] += dk;   // dk^2 > 400 * spread variance
+        }
+      }
       if (blockIdx.x == 0 && t.rsub == 0) *reinterpret_cast<float4*>(shift + (size_t)d * gm.C + 4 * t.q) = make_float4(K[0], K[1], K[2], K[3]);
     }
     float acc[S::FWD];

@@ -411,7 +411,11 @@ def test_fused_triple_buffer_aliasing_classes(layout, dev):
 
 # --------------------------------------------------------------------------- channels-last (NHWC) kernels
 @pytest.mark.parametrize("kind,c,hw,gs", [("whiten", 64, 28, 4), ("whiten", 256, 14, 4), ("whiten", 16, 10, 4),
-                                           ("whiten", 32, 9, 2), ("bn", 128, 14, 1), ("bn", 2048, 7, 1), ("bn", 8, 5, 1)])
+                                           ("whiten", 32, 9, 2), ("bn", 128, 14, 1), ("bn", 2048, 7, 1), ("bn", 8, 5, 1),
+                                           # launch edges: C = 4, 8 (every float4 column shared by 256 / 128 threads),
+                                           # C = 1024 / 2048 / 4096 (one thread per column, grid.y = 1 / 2 / 4)
+                                           ("whiten", 4, 3, 4), ("whiten", 8, 4, 2), ("whiten", 1024, 3, 4),
+                                           ("whiten", 2048, 2, 2), ("bn", 4096, 2, 1)])
 @pytest.mark.parametrize("relu", [True, False])
 def test_channels_last_site_matches_oracle(kind, c, hw, gs, relu, dev):
     """The NHWC kernels (torch.channels_last tensors) against the same oracle as the NCHW ones: fused domain
@@ -465,12 +469,12 @@ def test_channels_last_site_matches_oracle(kind, c, hw, gs, relu, dev):
 
 
 def test_channels_last_module_paths(dev):
-    """Single-domain modules on channels-last input: train, no-grad train, eval (+ backward), and a channel count
-    without a channels-last build (C/4 not a power of two) silently takes the NCHW kernels."""
+    """Single-domain modules on channels-last input: train, no-grad train, eval (+ backward), and channel counts
+    without a channels-last build (C/4 not a power of two, C/4 > 16384) silently take the NCHW kernels."""
     import whitening
     rng = np.random.default_rng(41)
-    for c, gs in [(64, 4), (48, 4)]:
-        x = _correlated(rng, 5, c, 12, 12)
+    for (nimg, c, h, w), gs in [((5, 64, 12, 12), 4), ((5, 48, 12, 12), 4), ((3, 131072, 2, 2), 4)]:
+        x = _correlated(rng, nimg, c, h, w) if c <= 64 else rng.standard_normal((nimg, c, h, w)) + 2.0
         dy = rng.standard_normal(x.shape)
         y_o, mean_o, w_o, rm1, rv1, _ = O.whiten_forward(x, gs, running_mean=np.zeros(c), running_cov=np.ones((c // gs, gs, gs)))
         m = whitening.WTransform2d(c, gs).to(dev).train()
