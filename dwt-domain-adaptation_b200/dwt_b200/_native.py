@@ -14,12 +14,13 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # DWT_B200_LIB: another build of the same library (development: A/B timing of a kernel variant on one box)
 LIB_PATH = os.environ.get("DWT_B200_LIB") or os.path.join(_HERE, "lib", "libdwt_b200.so")
 
-ABI_VERSION = 6
+ABI_VERSION = 7
 MAX_DOMAINS = 4
 MAX_GROUP_SIZE = 64
 MODE_TRAIN, MODE_EVAL = 0, 1
 EPI_NONE, EPI_AFFINE, EPI_RELU, EPI_RESIDUAL = 0, 1, 2, 4
 LAYOUT_NHWC = 0x100
+DTYPE_BF16 = 0x200                 # bf16 activations (channels-last kernels only; include/dwt_b200.h)
 STATUS_NOT_PD, STATUS_BAD_LABEL = 1, 2
 KIND_WHITEN, KIND_BN = 0, 1
 
@@ -73,9 +74,9 @@ _SIGNATURES = {
                                         ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_float), _c_float_p,
                                         _c_float_p, ctypes.c_int, ctypes.c_void_p]),
     "dwt_maxpool_fwd": (ctypes.c_int, [_c_float_p, _c_float_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_int64, ctypes.c_int64,
-                                       ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]),
+                                       ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]),
     "dwt_maxpool_bwd": (ctypes.c_int, [_c_float_p, ctypes.c_void_p, _c_float_p, ctypes.c_int64, ctypes.c_int64, ctypes.c_int64,
-                                       ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]),
+                                       ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]),
     "dwt_launch_count": (ctypes.c_int64, []),
     "dwt_profile_begin": (None, []),
     "dwt_profile_end": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int]),
@@ -165,15 +166,17 @@ def ptr_array(tensors):
     return ctypes.cast(arr, ctypes.POINTER(ctypes.c_void_p))
 
 
-def require_cuda(*tensors, any_dtype=False) -> torch.device:
+def require_cuda(*tensors, any_dtype=False, bf16=False) -> torch.device:
+    """Device of the tensors (all CUDA, all on one device).  They must be float32 unless any_dtype; bf16=True also
+    admits bfloat16 (activations: statistics, parameters and running buffers are always float32)."""
     dev = None
     for t in tensors:
         if t is None:
             continue
         if not t.is_cuda:
             raise NativeError("dwt_b200 runs on CUDA tensors only (no CPU fallback); got a tensor on " + str(t.device))
-        if t.dtype != torch.float32 and not any_dtype:
-            raise NativeError("dwt_b200 computes in float32; got " + str(t.dtype))
+        if t.dtype != torch.float32 and not any_dtype and not (bf16 and t.dtype == torch.bfloat16):
+            raise NativeError("dwt_b200 computes in float32 (activations may also be bfloat16); got " + str(t.dtype))
         if dev is None:
             dev = t.device
         elif t.device != dev:

@@ -120,6 +120,21 @@ int env_int(const char* name, int dflt) {
   return (v && *v) ? atoi(v) : dflt;
 }
 
+// DWT_DTYPE_BF16 (dwt_b200.h): bf16 activations run the channels-last kernels only; a thread's four channels are then
+// 8 bytes, so that is the alignment the tensors need (16 for fp32)
+int check_bf16_geometry(bool bf16, bool nhwc, int64_t C, int GS) {
+  if (bf16 && !(nhwc && dwt::cl_supports((int)C, GS)))
+    return fail(DWT_E_UNSUPPORTED, "bf16 activations are built for the channels-last kernels: DWT_LAYOUT_NHWC, group_size 1, 2, 4 with C/4 a "
+                                   "power of two (C=%lld gs=%d%s)", (long long)C, GS, nhwc ? "" : ", NCHW layout");
+  return DWT_OK;
+}
+int check_align(bool bf16, uintptr_t bits, const char* what) {
+  if (bits % (bf16 ? 8 : 16) == 0) return DWT_OK;
+  return bf16 ? fail(DWT_E_INVALID, "%s must be 8-byte aligned (bf16)", what) : fail(DWT_E_INVALID, "%s must be 16-byte aligned", what);
+}
+// family name of a launch in the profile: bf16 calls report under their own names (algorithmic bytes at 2 B/element)
+inline const char* fam(bool bf16, const char* f32, const char* b16) { return bf16 ? b16 : f32; }
+
 // channels-last launch shaping.  Every kernel is ONE wave of persistent CTAs sweeping 32-row chunks (norm_cl.cu):
 // grid.x CTAs per (domain, column slab), grid.y slabs, grid.z = D domains side by side.  (grid.z = 1 -- all CTAs
 // sweeping the domains one after the other, so that the whole grid moves through the tensor as a single window --
@@ -334,19 +349,20 @@ int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, 
                     float* const* rcov, const float* gamma, const float* beta, const float* residual,
                     uint8_t* relu_mask, int epi, float* save_mean, float* save_w, void* ws, size_t ws_bytes,
                     cudaStream_t st) {
-  const bool nhwc = (mode & DWT_LAYOUT_NHWC) != 0;
+  const bool nhwc = (mode & DWT_LAYOUT_NHWC) != 0, bf16 = (mode & DWT_DTYPE_BF16) != 0;
   mode &= 0xFF;
   Plan p;
   if (int rc = make_plan(p, K_STATS, K_APPLY, x, y, nullptr, N, C, HW, GS, D)) return rc;
   if (!x || !y || !save_mean || !save_w || !ws) return fail(DWT_E_INVALID, "null pointer argument");
+  if (int rc = check_bf16_geometry(bf16, nhwc, C, GS)) return rc;
   if (nhwc && !dwt::cl_supports((int)C, GS))
     return fail(DWT_E_UNSUPPORTED, "channels-last layout is built for group_size 1, 2, 4 with C/4 a power of two (C=%lld gs=%d)", (long long)C, GS);
-  if (nhwc && (((uintptr_t)x | (uintptr_t)y) % 16 != 0)) return fail(DWT_E_INVALID, "channels-last tensors must be 16-byte aligned");
+  if (nhwc) if (int rc = check_align(bf16, (uintptr_t)x | (uintptr_t)y, "channels-last tensors")) return rc;
   if (mode != DWT_MODE_TRAIN && mode != DWT_MODE_EVAL) return fail(DWT_E_INVALID, "bad mode %d", mode);
   if ((epi & DWT_EPI_RELU) && !(epi & DWT_EPI_AFFINE)) return fail(DWT_E_INVALID, "RELU epilogue needs AFFINE");
   if ((epi & DWT_EPI_AFFINE) && (!gamma || !beta)) return fail(DWT_E_INVALID, "AFFINE epilogue needs gamma and beta");
   if ((epi & DWT_EPI_RESIDUAL) && ((epi & 3) != 3 || !residual)) return fail(DWT_E_INVALID, "RESIDUAL epilogue needs AFFINE|RELU and a residual tensor");
-  if ((epi & DWT_EPI_RESIDUAL) && (uintptr_t)residual % 16 != 0) return fail(DWT_E_INVALID, "residual must be 16-byte aligned");
+  if (epi & DWT_EPI_RESIDUAL) if (int rc = check_align(bf16, (uintptr_t)residual, "residual")) return rc;
   if (relu_mask && !((epi & DWT_EPI_RESIDUAL) && nhwc))
     return fail(DWT_E_UNSUPPORTED, "the ReLU byte map is written by the channels-last RESIDUAL epilogue only");
   if (epi != 0 && !p.small)
@@ -361,25 +377,26 @@ int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, 
   const dwt::FwdFin fin = make_fwd_fin(a, b, momentum, unbias, mode == DWT_MODE_TRAIN ? update_running : 0, need_running,
                                        rmean, rcov, save_mean, save_w, w, D);
 
-  const double E = 4.0 * (double)D * (double)N * (double)C * (double)HW;   // bytes of one activation tensor
+  const double n_el = (double)D * (double)N * (double)C * (double)HW;
+  const double E = (bf16 ? 2.0 : 4.0) * n_el, Mb = 0.25 * n_el;   // bytes of one activation tensor, of the ReLU byte map
   if (nhwc) {
     const ClPlan cp = cl_plan(p.gm, 3, 3, 8, (epi & DWT_EPI_RESIDUAL) ? 4 : 8);
     if (mode == DWT_MODE_TRAIN) {
       {
-        Launch l("cl_stats", &p.gm, E, st);
-        dwt::cl_stats(x, p.gm, cp.nred, cp.gz_red, w.partial, w.shift, st);
+        Launch l(fam(bf16, "cl_stats", "cl_stats_bf16"), &p.gm, E, st);
+        dwt::cl_stats(x, bf16, p.gm, cp.nred, cp.gz_red, w.partial, w.shift, st);
       }
       if (int rc = check_launch("channels-last statistics kernel")) return rc;
-      Launch l("cl_fwd_finalize", &p.gm, 0.0, st);
+      Launch l(fam(bf16, "cl_fwd_finalize", "cl_fwd_finalize_bf16"), &p.gm, 0.0, st);
       dwt::cl_fwd_finalize(w.partial, cp.nred, w.shift, p.gm, fin, st);
     } else {
-      Launch l("eval_prep", &p.gm, 0.0, st);
+      Launch l(fam(bf16, "eval_prep", "cl_eval_prep_bf16"), &p.gm, 0.0, st);
       dwt::small_eval_prep(p.gm, fin, st);
     }
     if (int rc = check_launch("channels-last finalize kernel")) return rc;
     {
-      Launch l("cl_apply", &p.gm, ((epi & DWT_EPI_RESIDUAL) ? (relu_mask ? 3.0625 : 3.0) : 2.0) * E, st);
-      dwt::cl_apply(x, y, p.gm, cp.new_, cp.gz_ew, epi, save_mean, save_w, gamma, beta, residual, relu_mask, st);
+      Launch l(fam(bf16, "cl_apply", "cl_apply_bf16"), &p.gm, (epi & DWT_EPI_RESIDUAL) ? 3.0 * E + (relu_mask ? Mb : 0.0) : 2.0 * E, st);
+      dwt::cl_apply(x, y, bf16, p.gm, cp.new_, cp.gz_ew, epi, save_mean, save_w, gamma, beta, residual, relu_mask, st);
     }
     return check_launch("channels-last apply kernel");
   }
@@ -419,17 +436,18 @@ int whiten_like_bwd(const float* x, const float* dout, const float* dout2, float
                     int mode, float a, const float* save_mean, const float* save_w, const float* gamma,
                     const float* beta, const uint8_t* relu_mask, float* dresidual, int epi, float* dgamma,
                     float* dbeta, void* ws, size_t ws_bytes, cudaStream_t st) {
-  const bool nhwc = (mode & DWT_LAYOUT_NHWC) != 0;
+  const bool nhwc = (mode & DWT_LAYOUT_NHWC) != 0, bf16 = (mode & DWT_DTYPE_BF16) != 0;
   mode &= 0xFF;
   Plan p;
   if (int rc = make_plan(p, K_BWD_REDUCE, K_BWD_APPLY, x, dout, dx, N, C, HW, GS, D)) return rc;
   if (!x || !dout || !dx || !save_mean || !save_w || !ws) return fail(DWT_E_INVALID, "null pointer argument");
-  if (dout2 && (!nhwc || (uintptr_t)dout2 % 16 != 0))
+  if (int rc = check_bf16_geometry(bf16, nhwc, C, GS)) return rc;
+  if (dout2 && (!nhwc || (uintptr_t)dout2 % (bf16 ? 8 : 16) != 0))
     return fail(nhwc ? DWT_E_INVALID : DWT_E_UNSUPPORTED, "a second gradient addend (dout2) is built for the channels-last "
-                "kernels (16-byte aligned tensor); add it to dout otherwise");
+                "kernels (16-byte aligned tensor, 8 for bf16); add it to dout otherwise");
   if (nhwc && !dwt::cl_supports((int)C, GS))
     return fail(DWT_E_UNSUPPORTED, "channels-last layout is built for group_size 1, 2, 4 with C/4 a power of two (C=%lld gs=%d)", (long long)C, GS);
-  if (nhwc && (((uintptr_t)x | (uintptr_t)dout | (uintptr_t)dx) % 16 != 0)) return fail(DWT_E_INVALID, "channels-last tensors must be 16-byte aligned");
+  if (nhwc) if (int rc = check_align(bf16, (uintptr_t)x | (uintptr_t)dout | (uintptr_t)dx, "channels-last tensors")) return rc;
   if (mode != DWT_MODE_TRAIN && mode != DWT_MODE_EVAL) return fail(DWT_E_INVALID, "bad mode %d", mode);
   if ((epi & DWT_EPI_RELU) && !(epi & DWT_EPI_AFFINE)) return fail(DWT_E_INVALID, "RELU epilogue needs AFFINE");
   if ((epi & DWT_EPI_AFFINE) && (!gamma || !beta)) return fail(DWT_E_INVALID, "AFFINE epilogue needs gamma and beta");
@@ -439,7 +457,7 @@ int whiten_like_bwd(const float* x, const float* dout, const float* dout2, float
     if (!nhwc || !relu_mask || (epi & 3) != 3 || !dresidual)
       return fail(DWT_E_INVALID, "backward of a RESIDUAL forward needs the channels-last layout, AFFINE|RELU, the forward's "
                                  "ReLU byte map and dresidual (or pass dout already masked by (out > 0) with epilogue AFFINE)");
-    if ((uintptr_t)dresidual % 16 != 0) return fail(DWT_E_INVALID, "dresidual must be 16-byte aligned");
+    if (int rc = check_align(bf16, (uintptr_t)dresidual, "dresidual")) return rc;
   } else if (relu_mask || dresidual) {
     return fail(DWT_E_INVALID, "relu_mask / dresidual belong to the RESIDUAL epilogue");
   }
@@ -455,26 +473,27 @@ int whiten_like_bwd(const float* x, const float* dout, const float* dout2, float
   const bool masked = nhwc && (epi & DWT_EPI_RESIDUAL) != 0;   // the reduction also writes the masked gradient
 
   const bool need_reduce = (mode == DWT_MODE_TRAIN) || (fin.dgamma != nullptr) || masked;
-  const double E = 4.0 * (double)D * (double)N * (double)C * (double)HW;
+  const double n_el = (double)D * (double)N * (double)C * (double)HW;
+  const double E = (bf16 ? 2.0 : 4.0) * n_el, Mb = 0.25 * n_el;
   if (nhwc) {
     const ClPlan cp = cl_plan(p.gm, 2, 2, 4, 4);
     if (need_reduce) {
       {
-        Launch l("cl_bwd_reduce", &p.gm, ((masked ? 3.0625 : 2.0) + (dout2 ? 1.0 : 0.0)) * E, st);
-        dwt::cl_bwd_reduce(x, dout, dout2, p.gm, cp.nred, cp.gz_red, epi, save_mean, save_w, gamma, beta, relu_mask, dresidual, w.partial, st);
+        Launch l(fam(bf16, "cl_bwd_reduce", "cl_bwd_reduce_bf16"), &p.gm, (masked ? 3.0 * E + Mb : 2.0 * E) + (dout2 ? E : 0.0), st);
+        dwt::cl_bwd_reduce(x, dout, dout2, bf16, p.gm, cp.nred, cp.gz_red, epi, save_mean, save_w, gamma, beta, relu_mask, dresidual, w.partial, st);
       }
       if (int rc = check_launch("channels-last backward reduction kernel")) return rc;
-      Launch l("cl_bwd_finalize", &p.gm, 0.0, st);
+      Launch l(fam(bf16, "cl_bwd_finalize", "cl_bwd_finalize_bf16"), &p.gm, 0.0, st);
       dwt::cl_bwd_finalize(w.partial, cp.nred, p.gm, fin, st);
     } else {
-      Launch l("bwd_prep", &p.gm, 0.0, st);
+      Launch l(fam(bf16, "bwd_prep", "cl_bwd_prep_bf16"), &p.gm, 0.0, st);
       dwt::small_bwd_prep(p.gm, fin, st);
     }
     if (int rc = check_launch("channels-last backward finalize kernel")) return rc;
     {
-      Launch l("cl_bwd_apply", &p.gm, (3.0 + (dout2 && !masked ? 1.0 : 0.0)) * E, st);
-      if (masked) dwt::cl_bwd_apply(x, dresidual, nullptr, dx, p.gm, cp.new_, cp.gz_ew, DWT_EPI_AFFINE, w.coef, save_mean, save_w, gamma, beta, st);
-      else dwt::cl_bwd_apply(x, dout, dout2, dx, p.gm, cp.new_, cp.gz_ew, epi, w.coef, save_mean, save_w, gamma, beta, st);
+      Launch l(fam(bf16, "cl_bwd_apply", "cl_bwd_apply_bf16"), &p.gm, (3.0 + (dout2 && !masked ? 1.0 : 0.0)) * E, st);
+      if (masked) dwt::cl_bwd_apply(x, dresidual, nullptr, dx, bf16, p.gm, cp.new_, cp.gz_ew, DWT_EPI_AFFINE, w.coef, save_mean, save_w, gamma, beta, st);
+      else dwt::cl_bwd_apply(x, dout, dout2, dx, bf16, p.gm, cp.new_, cp.gz_ew, epi, w.coef, save_mean, save_w, gamma, beta, st);
     }
     return check_launch("channels-last backward apply kernel");
   }
@@ -521,7 +540,7 @@ SiteConst site_const(int kind, float eps, int64_t N, int64_t HW) {
 }
 
 // checks shared by both directions; out is the tensor-sized output of the call (y, or dz)
-int tail2_plan(Plan& p, int kind, const dwt_tail_site* s, const void* out, int64_t N, int64_t C, int64_t HW, int GS, int D) {
+int tail2_plan(Plan& p, int kind, bool bf16, const dwt_tail_site* s, const void* out, int64_t N, int64_t C, int64_t HW, int GS, int D) {
   if (kind != DWT_KIND_WHITEN && kind != DWT_KIND_BN) return fail(DWT_E_INVALID, "bad kind %d", kind);
   if (kind == DWT_KIND_BN && GS != 1) return fail(DWT_E_INVALID, "batch norm has group_size 1 (got %d)", GS);
   if (!s) return fail(DWT_E_INVALID, "null pointer argument");
@@ -531,8 +550,7 @@ int tail2_plan(Plan& p, int kind, const dwt_tail_site* s, const void* out, int64
                 (long long)C, GS);
   for (int k = 0; k < 2; ++k)
     if (!s[k].x || !s[k].gamma || !s[k].beta || !s[k].save_mean || !s[k].save_w || !out) return fail(DWT_E_INVALID, "null pointer argument");
-  if ((((uintptr_t)s[0].x | (uintptr_t)s[1].x | (uintptr_t)out) % 16) != 0) return fail(DWT_E_INVALID, "channels-last tensors must be 16-byte aligned");
-  return DWT_OK;
+  return check_align(bf16, (uintptr_t)s[0].x | (uintptr_t)s[1].x | (uintptr_t)out, "channels-last tensors");
 }
 
 // the two sites' scratch: site 1 behind site 0, sharing the head (status word, counters)
@@ -547,8 +565,10 @@ int tail2_workspace(Workspace (&w)[2], void* ws, size_t ws_bytes, int64_t C, int
 
 int tail2_fwd(int kind, const dwt_tail_site* s, float* y, uint8_t* relu_mask, int64_t N, int64_t C, int64_t HW, int GS, int D,
               void* ws, size_t ws_bytes, cudaStream_t st) {
+  const bool bf16 = (kind & DWT_DTYPE_BF16) != 0;
+  kind &= ~DWT_DTYPE_BF16;
   Plan p;
-  if (int rc = tail2_plan(p, kind, s, y, N, C, HW, GS, D)) return rc;
+  if (int rc = tail2_plan(p, kind, bf16, s, y, N, C, HW, GS, D)) return rc;
   if (!relu_mask) return fail(DWT_E_INVALID, "the two-site tail writes the ReLU byte map its backward reads");
   for (int k = 0; k < 2; ++k)
     if (int rc = check_running(s[k].update_running != 0, s[k].running_mean, s[k].running_cov, D)) return rc;
@@ -560,22 +580,23 @@ int tail2_fwd(int kind, const dwt_tail_site* s, float* y, uint8_t* relu_mask, in
     fin[k] = make_fwd_fin(sc.a, sc.b, s[k].momentum, sc.unbias, s[k].update_running, s[k].update_running != 0, s[k].running_mean,
                           s[k].running_cov, s[k].save_mean, s[k].save_w, w[k], D);
   }
-  const double E = 4.0 * (double)D * (double)N * (double)C * (double)HW;
+  const double n_el = (double)D * (double)N * (double)C * (double)HW;
+  const double E = (bf16 ? 2.0 : 4.0) * n_el, Mb = 0.25 * n_el;
   const ClPlan cp = cl_plan(p.gm, 3, 3, 8, 4);
   for (int k = 0; k < 2; ++k) {            // the tail's input first: conv3 wrote it last, its end is still in L2
-    Launch l("cl_stats", &p.gm, E, st);
-    dwt::cl_stats(s[k].x, p.gm, cp.nred, cp.gz_red, w[k].partial, w[k].shift, st);
+    Launch l(fam(bf16, "cl_stats", "cl_stats_bf16"), &p.gm, E, st);
+    dwt::cl_stats(s[k].x, bf16, p.gm, cp.nred, cp.gz_red, w[k].partial, w[k].shift, st);
   }
   if (int rc = check_launch("channels-last statistics kernel")) return rc;
   {
-    Launch l("cl_tail2_fwd_finalize", &p.gm, 0.0, st);
+    Launch l(fam(bf16, "cl_tail2_fwd_finalize", "cl_tail2_fwd_finalize_bf16"), &p.gm, 0.0, st);
     dwt::cl_fwd_finalize(w[0].partial, cp.nred, w[0].shift, p.gm, fin[0], st, &fin[1], (size_t)(w[1].partial - w[0].partial),
                          (size_t)(w[1].shift - w[0].shift));
   }
   if (int rc = check_launch("channels-last finalize kernel")) return rc;
   {
-    Launch l("cl_tail2_apply", &p.gm, 3.0625 * E, st);       // x, xd -> out + byte map
-    dwt::cl_tail2_apply(s[0].x, s[1].x, y, p.gm, cp.new_, cp.gz_ew, s[0].save_mean, s[0].save_w, s[0].gamma, s[0].beta,
+    Launch l(fam(bf16, "cl_tail2_apply", "cl_tail2_apply_bf16"), &p.gm, 3.0 * E + Mb, st);       // x, xd -> out + byte map
+    dwt::cl_tail2_apply(s[0].x, s[1].x, y, bf16, p.gm, cp.new_, cp.gz_ew, s[0].save_mean, s[0].save_w, s[0].gamma, s[0].beta,
                         s[1].save_mean, s[1].save_w, s[1].gamma, s[1].beta, relu_mask, st);
   }
   return check_launch("channels-last two-site apply kernel");
@@ -583,11 +604,12 @@ int tail2_fwd(int kind, const dwt_tail_site* s, float* y, uint8_t* relu_mask, in
 
 int tail2_bwd(int kind, const dwt_tail_site* s, const float* dout, const float* dout2, const uint8_t* relu_mask, float* dz,
               int64_t N, int64_t C, int64_t HW, int GS, int D, void* ws, size_t ws_bytes, cudaStream_t st) {
+  const bool bf16 = (kind & DWT_DTYPE_BF16) != 0;
+  kind &= ~DWT_DTYPE_BF16;
   Plan p;
-  if (int rc = tail2_plan(p, kind, s, dz, N, C, HW, GS, D)) return rc;
+  if (int rc = tail2_plan(p, kind, bf16, s, dz, N, C, HW, GS, D)) return rc;
   if (!dout || !relu_mask || !s[0].dx || !s[1].dx) return fail(DWT_E_INVALID, "null pointer argument");
-  if ((((uintptr_t)dout | (uintptr_t)dout2 | (uintptr_t)s[0].dx | (uintptr_t)s[1].dx) % 16) != 0)
-    return fail(DWT_E_INVALID, "channels-last tensors must be 16-byte aligned");
+  if (int rc = check_align(bf16, (uintptr_t)dout | (uintptr_t)dout2 | (uintptr_t)s[0].dx | (uintptr_t)s[1].dx, "channels-last tensors")) return rc;
   for (int k = 0; k < 2; ++k)
     if ((s[k].dgamma == nullptr) != (s[k].dbeta == nullptr)) return fail(DWT_E_INVALID, "dgamma and dbeta go together");
   Workspace w[2];
@@ -596,22 +618,23 @@ int tail2_bwd(int kind, const dwt_tail_site* s, const float* dout, const float* 
   for (int k = 0; k < 2; ++k)
     fin[k] = make_bwd_fin(site_const(kind, s[k].eps, N, HW).a, DWT_MODE_TRAIN, k ? DWT_EPI_AFFINE : (DWT_EPI_AFFINE | DWT_EPI_RELU | DWT_EPI_RESIDUAL),
                           s[k].save_mean, s[k].save_w, s[k].gamma, s[k].dgamma, s[k].dbeta, w[k]);
-  const double E = 4.0 * (double)D * (double)N * (double)C * (double)HW;
+  const double n_el = (double)D * (double)N * (double)C * (double)HW;
+  const double E = (bf16 ? 2.0 : 4.0) * n_el, Mb = 0.25 * n_el;
   const ClPlan cp = cl_plan(p.gm, 2, 2, 4, 4);
   {
-    Launch l("cl_tail2_bwd_reduce", &p.gm, (4.0625 + (dout2 ? 1.0 : 0.0)) * E, st);   // x, xd, dout (+ dout2), byte map -> dz
-    dwt::cl_tail2_bwd_reduce(s[0].x, s[1].x, dout, dout2, p.gm, cp.nred, cp.gz_red, s[0].save_mean, s[1].save_mean, relu_mask, dz,
+    Launch l(fam(bf16, "cl_tail2_bwd_reduce", "cl_tail2_bwd_reduce_bf16"), &p.gm, (4.0 + (dout2 ? 1.0 : 0.0)) * E + Mb, st);   // x, xd, dout (+ dout2), byte map -> dz
+    dwt::cl_tail2_bwd_reduce(s[0].x, s[1].x, dout, dout2, bf16, p.gm, cp.nred, cp.gz_red, s[0].save_mean, s[1].save_mean, relu_mask, dz,
                              w[0].partial, (size_t)(w[1].partial - w[0].partial), st);
   }
   if (int rc = check_launch("channels-last two-site backward reduction kernel")) return rc;
   {
-    Launch l("cl_tail2_bwd_finalize", &p.gm, 0.0, st);
+    Launch l(fam(bf16, "cl_tail2_bwd_finalize", "cl_tail2_bwd_finalize_bf16"), &p.gm, 0.0, st);
     dwt::cl_bwd_finalize(w[0].partial, cp.nred, p.gm, fin[0], st, &fin[1], (size_t)(w[1].partial - w[0].partial));
   }
   if (int rc = check_launch("channels-last backward finalize kernel")) return rc;
   {
-    Launch l("cl_tail2_bwd_apply", &p.gm, 5.0 * E, st);       // x, xd, dz -> dx, dxd
-    dwt::cl_tail2_bwd_apply(s[0].x, s[1].x, dz, s[0].dx, s[1].dx, p.gm, cp.new_, cp.gz_ew, w[0].coef, w[1].coef, st);
+    Launch l(fam(bf16, "cl_tail2_bwd_apply", "cl_tail2_bwd_apply_bf16"), &p.gm, 5.0 * E, st);       // x, xd, dz -> dx, dxd
+    dwt::cl_tail2_bwd_apply(s[0].x, s[1].x, dz, s[0].dx, s[1].dx, bf16, p.gm, cp.new_, cp.gz_ew, w[0].coef, w[1].coef, st);
   }
   return check_launch("channels-last two-site backward apply kernel");
 }
@@ -743,29 +766,35 @@ int pool_check(int64_t N, int64_t H, int64_t W, int64_t C, int k, int s, int p, 
 }  // namespace
 
 int dwt_maxpool_fwd(const float* x, float* y, uint8_t* argmax, int64_t N, int64_t H, int64_t W, int64_t C, int kernel,
-                    int stride, int padding, dwt_stream_t stream) {
+                    int stride, int padding, int flags, dwt_stream_t stream) {
   int OH = 0, OW = 0;
   if (int rc = pool_check(N, H, W, C, kernel, stride, padding, &OH, &OW)) return rc;
+  if (flags != 0 && flags != DWT_DTYPE_BF16) return fail(DWT_E_INVALID, "bad flags %#x (0 or DWT_DTYPE_BF16)", flags);
+  const bool bf16 = flags == DWT_DTYPE_BF16;
   if (!x || !y || !argmax) return fail(DWT_E_INVALID, "null pointer argument");
-  if ((((uintptr_t)x | (uintptr_t)y) % 16) != 0 || (uintptr_t)argmax % 4 != 0) return fail(DWT_E_INVALID, "pooling tensors must be 16-byte aligned");
+  if ((uintptr_t)argmax % 4 != 0) return fail(DWT_E_INVALID, "pooling tensors must be 16-byte aligned");
+  if (int rc = check_align(bf16, (uintptr_t)x | (uintptr_t)y, "pooling tensors")) return rc;
   {
     const double in = (double)N * H * W * C, out = (double)N * OH * OW * C;
-    Launch l("maxpool_fwd", nullptr, 4.0 * (in + out) + out, (cudaStream_t)stream);
-    dwt::maxpool_fwd_launch(x, y, argmax, (int)N, (int)H, (int)W, (int)C, OH, OW, kernel, stride, padding, (cudaStream_t)stream);
+    Launch l(fam(bf16, "maxpool_fwd", "maxpool_fwd_bf16"), nullptr, (bf16 ? 2.0 : 4.0) * (in + out) + out, (cudaStream_t)stream);
+    dwt::maxpool_fwd_launch(x, y, bf16, argmax, (int)N, (int)H, (int)W, (int)C, OH, OW, kernel, stride, padding, (cudaStream_t)stream);
   }
   return check_launch("max-pool forward kernel");
 }
 
 int dwt_maxpool_bwd(const float* dy, const uint8_t* argmax, float* dx, int64_t N, int64_t H, int64_t W, int64_t C, int kernel,
-                    int stride, int padding, dwt_stream_t stream) {
+                    int stride, int padding, int flags, dwt_stream_t stream) {
   int OH = 0, OW = 0;
   if (int rc = pool_check(N, H, W, C, kernel, stride, padding, &OH, &OW)) return rc;
+  if (flags != 0 && flags != DWT_DTYPE_BF16) return fail(DWT_E_INVALID, "bad flags %#x (0 or DWT_DTYPE_BF16)", flags);
+  const bool bf16 = flags == DWT_DTYPE_BF16;
   if (!dy || !dx || !argmax) return fail(DWT_E_INVALID, "null pointer argument");
-  if ((((uintptr_t)dy | (uintptr_t)dx) % 16) != 0 || (uintptr_t)argmax % 4 != 0) return fail(DWT_E_INVALID, "pooling tensors must be 16-byte aligned");
+  if ((uintptr_t)argmax % 4 != 0) return fail(DWT_E_INVALID, "pooling tensors must be 16-byte aligned");
+  if (int rc = check_align(bf16, (uintptr_t)dy | (uintptr_t)dx, "pooling tensors")) return rc;
   {
     const double in = (double)N * H * W * C, out = (double)N * OH * OW * C;
-    Launch l("maxpool_bwd", nullptr, 4.0 * (in + out) + out, (cudaStream_t)stream);
-    dwt::maxpool_bwd_launch(dy, argmax, dx, (int)N, (int)H, (int)W, (int)C, OH, OW, kernel, stride, padding, (cudaStream_t)stream);
+    Launch l(fam(bf16, "maxpool_bwd", "maxpool_bwd_bf16"), nullptr, (bf16 ? 2.0 : 4.0) * (in + out) + out, (cudaStream_t)stream);
+    dwt::maxpool_bwd_launch(dy, argmax, dx, bf16, (int)N, (int)H, (int)W, (int)C, OH, OW, kernel, stride, padding, (cudaStream_t)stream);
   }
   return check_launch("max-pool backward kernel");
 }

@@ -42,6 +42,10 @@
 // Reference semantics: utils/whitening.py:37-61, utils/batch_norm.py:54-69 (/root/reference).
 #include <stdlib.h>
 
+#include <type_traits>
+
+#include <cuda_bf16.h>
+
 #include "dwt_common.cuh"
 #include "norm_launch.h"
 #include "small_algebra.cuh"
@@ -95,6 +99,28 @@ __device__ __forceinline__ void sweep_rows(const ClThread& t, unsigned rows, F&&
 
 __device__ __forceinline__ float4 ldg4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
 
+// Activation storage T: float, or __nv_bfloat16 (DWT_DTYPE_BF16).  A thread's four channels are one float4 or 8 bytes of
+// bf16: they widen to fp32 as they load and round to nearest-even as they store; everything in between is the fp32 code,
+// on the same schedule, so a bf16 call's sums, statistics and coefficients are those of the fp32 kernels on x.float().
+template <class T> constexpr bool kBf16 = !std::is_same<T, float>::value;
+__device__ __forceinline__ float4 ld4(const float* p) { return ldg4(p); }
+__device__ __forceinline__ float4 ld4(const __nv_bfloat16* p) {
+  const uint2 u = __ldg(reinterpret_cast<const uint2*>(p));          // bf16 -> fp32 is exact: the high half of the word
+  return make_float4(__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xFFFF0000u), __uint_as_float(u.y << 16),
+                     __uint_as_float(u.y & 0xFFFF0000u));
+}
+__device__ __forceinline__ void st4(float* p, const float4& v) { *reinterpret_cast<float4*>(p) = v; }
+__device__ __forceinline__ void st4(__nv_bfloat16* p, const float4& v) {
+  const __nv_bfloat162 a = __floats2bfloat162_rn(v.x, v.y), b = __floats2bfloat162_rn(v.z, v.w);
+  *reinterpret_cast<uint2*>(p) = make_uint2(*reinterpret_cast<const unsigned*>(&a), *reinterpret_cast<const unsigned*>(&b));
+}
+// the value as T stores it: v itself in fp32, RN_bf16(v) in bf16
+template <class T>
+__device__ __forceinline__ float as_stored(float v) {
+  if constexpr (kBf16<T>) return __bfloat162float(__float2bfloat16_rn(v));
+  else return v;
+}
+
 // Sum the per-thread accumulators of the rpi threads that share a column; thread rsub == 0 of every column
 // then holds the CTA total.  sRed must hold kT * NACC floats.
 template <int NACC>
@@ -116,8 +142,8 @@ __device__ __forceinline__ void column_reduce(const ClThread& t, float (&acc)[NA
 // ------------------------------------------------------------------------------------------
 // forward statistics: partial[d][cta][q][FWD] ; CTA (0, y, d) also publishes the pilot shift
 // ------------------------------------------------------------------------------------------
-template <int GS>
-__global__ void __launch_bounds__(kT, 3) cl_stats_kernel(const float* __restrict__ x, const Geom gm,
+template <class T, int GS>
+__global__ void __launch_bounds__(kT, 3) cl_stats_kernel(const T* __restrict__ x, const Geom gm,
                                                          float* __restrict__ partial, float* __restrict__ shift) {
   using S = ClShape<GS>;
   constexpr int UNROLL = 8;
@@ -126,7 +152,7 @@ __global__ void __launch_bounds__(kT, 3) cl_stats_kernel(const float* __restrict
   const unsigned rows = (unsigned)gm.N * gm.HW;
   pdl_launch_dependents();
   CL_FOR_DOMAINS(d, gm, true) {
-    const float* xd = x + (size_t)d * rows * gm.C + 4 * t.q;
+    const T* xd = x + (size_t)d * rows * gm.C + 4 * t.q;
     // pilot shift K, per channel (every thread of a column agrees): the mean of the first <= 8 rows of the domain,
     // unless they sit far from the rest of it.  The one-pass moments lose digits in proportion to (K - mean)^2 / var:
     // a first image whose top row sat 30 sigma off cost 1.1e-4 of the stem site's covariance at the benchmark's size
@@ -139,7 +165,7 @@ __global__ void __launch_bounds__(kT, 3) cl_stats_kernel(const float* __restrict
     {
       const unsigned np = rows < 8 ? rows : 8;
       for (unsigned r = 0; r < np; ++r) {
-        const float4 v = ldg4(xd + (size_t)r * gm.C);
+        const float4 v = ld4(xd + (size_t)r * gm.C);
         K[0] += v.x; K[1] += v.y; K[2] += v.z; K[3] += v.w;
       }
 #pragma unroll
@@ -148,7 +174,7 @@ __global__ void __launch_bounds__(kT, 3) cl_stats_kernel(const float* __restrict
         float s1[4] = {0.f, 0.f, 0.f, 0.f}, s2[4] = {0.f, 0.f, 0.f, 0.f};   // moments of the spread rows around K
         const size_t mid = (size_t)gm.HW / 2 + (size_t)sqrtf((float)gm.HW) / 2;
         for (unsigned k = 0; k < 8; ++k) {
-          const float4 v = ldg4(xd + ((2 * (size_t)k + 1) * rows / 16 + mid) % rows * gm.C);
+          const float4 v = ld4(xd + ((2 * (size_t)k + 1) * rows / 16 + mid) % rows * gm.C);
           const float e[4] = {v.x - K[0], v.y - K[1], v.z - K[2], v.w - K[3]};
 #pragma unroll
           for (int c = 0; c < 4; ++c) { s1[c] += e[c]; s2[c] = fmaf(e[c], e[c], s2[c]); }
@@ -169,7 +195,7 @@ __global__ void __launch_bounds__(kT, 3) cl_stats_kernel(const float* __restrict
 #pragma unroll
       for (int u = 0; u < UNROLL; ++u) {
         const unsigned rr = r + u * t.rpi;
-        v[u] = rr < rows ? ldg4(xd + (size_t)rr * gm.C) : make_float4(K[0], K[1], K[2], K[3]);
+        v[u] = rr < rows ? ld4(xd + (size_t)rr * gm.C) : make_float4(K[0], K[1], K[2], K[3]);
       }
 #pragma unroll
       for (int u = 0; u < UNROLL; ++u) {
@@ -350,12 +376,13 @@ __global__ void __launch_bounds__(32 * kFinQ * DWT_MAX_DOMAINS) cl_fwd_finalize_
 // apply
 // ------------------------------------------------------------------------------------------
 // DS (two-site tail, EPI = AFFINE|RELU|RESIDUAL): `res` is the downsample site's INPUT xd and the residual is its
-// output gamma_d W_d (xd - mu_d) + beta_d, formed in registers exactly as the downsample site's own apply would.
-template <int GS, int EPI, bool DS>
-__global__ void __launch_bounds__(kT, 3) cl_apply_kernel(const float* __restrict__ x, float* __restrict__ y, const Geom gm,
+// output gamma_d W_d (xd - mu_d) + beta_d, formed in registers exactly as the downsample site's own apply would -- and
+// rounded as that apply would store it (bf16), so the pass stays bit for bit its two-call composition.
+template <class T, int GS, int EPI, bool DS>
+__global__ void __launch_bounds__(kT, 3) cl_apply_kernel(const T* __restrict__ x, T* __restrict__ y, const Geom gm,
                                                          const float* __restrict__ save_mean, const float* __restrict__ save_w,
                                                          const float* __restrict__ gamma, const float* __restrict__ beta,
-                                                         const float* __restrict__ res, uint8_t* __restrict__ mask,
+                                                         const T* __restrict__ res, uint8_t* __restrict__ mask,
                                                          const float* __restrict__ save_mean_d, const float* __restrict__ save_w_d,
                                                          const float* __restrict__ gamma_d, const float* __restrict__ beta_d) {
   using S = ClShape<GS>;
@@ -378,9 +405,9 @@ __global__ void __launch_bounds__(kT, 3) cl_apply_kernel(const float* __restrict
                                              gamma_d + g * GS, beta_d + g * GS, Wd[s], bd[s]);
     }
     const size_t base = (size_t)d * rows * gm.C + 4 * t.q;
-    const float* xd = x + base;
-    const float* rd = res + base;
-    float* yd = y + base;
+    const T* xd = x + base;
+    const T* rd = res + base;
+    T* yd = y + base;
     uint8_t* md = mask + (size_t)d * rows * t.C4 + t.q;          // one byte per float4: the four (out > 0) bits
     sweep_rows<UNROLL, false>(t, rows, [&](unsigned r) {
       float4 v[UNROLL], rs[UNROLL];
@@ -388,8 +415,8 @@ __global__ void __launch_bounds__(kT, 3) cl_apply_kernel(const float* __restrict
       for (int u = 0; u < UNROLL; ++u) {
         const unsigned rr = r + u * t.rpi;
         if (rr < rows) {
-          v[u] = ldg4(xd + (size_t)rr * gm.C);
-          if constexpr (RES) rs[u] = ldg4(rd + (size_t)rr * gm.C);
+          v[u] = ld4(xd + (size_t)rr * gm.C);
+          if constexpr (RES) rs[u] = ld4(rd + (size_t)rr * gm.C);
         }
       }
 #pragma unroll
@@ -409,7 +436,7 @@ __global__ void __launch_bounds__(kT, 3) cl_apply_kernel(const float* __restrict
               for (int c = 0; c < GS; ++c) xdi[c] = ra[s * GS + c];
               apply_group<GS>(Wd[s], bd[s], xdi, odi);
 #pragma unroll
-              for (int c = 0; c < GS; ++c) ra[s * GS + c] = odi[c];
+              for (int c = 0; c < GS; ++c) ra[s * GS + c] = as_stored<T>(odi[c]);
             }
 #pragma unroll
             for (int c = 0; c < GS; ++c) xi[c] = e[s * GS + c];
@@ -421,7 +448,7 @@ __global__ void __launch_bounds__(kT, 3) cl_apply_kernel(const float* __restrict
               o[s * GS + c] = (EPI & DWT_EPI_RELU) ? fmaxf(z, 0.f) : z;
             }
           }
-          *reinterpret_cast<float4*>(yd + (size_t)rr * gm.C) = make_float4(o[0], o[1], o[2], o[3]);
+          st4(yd + (size_t)rr * gm.C, make_float4(o[0], o[1], o[2], o[3]));
           if constexpr (RES) { if (mask != nullptr) md[(size_t)rr * t.C4] = (uint8_t)bits; }
         }
       }
@@ -446,13 +473,13 @@ __device__ __forceinline__ void bwd_accumulate(float* acc, const float (&dz)[GS]
 // MASK (residual tail): the masked gradient dz -- also the gradient of the identity branch -- is written to dzout.
 // DS (two-site tail): the downsample site's input xd is swept alongside x; its gradient is the same dz, so its
 // accumulators (R_d, sdz) go to a second set of partial rows at partial + pstride.
-template <int GS, int EPI, bool D2, bool DS>
-__global__ void __launch_bounds__(kT, 2) cl_bwd_reduce_kernel(const float* __restrict__ x, const float* __restrict__ dout, const float* __restrict__ dout2,
+template <class T, int GS, int EPI, bool D2, bool DS>
+__global__ void __launch_bounds__(kT, 2) cl_bwd_reduce_kernel(const T* __restrict__ x, const T* __restrict__ dout, const T* __restrict__ dout2,
                                                               const Geom gm, const float* __restrict__ save_mean,
                                                               const float* __restrict__ save_w, const float* __restrict__ gamma,
                                                               const float* __restrict__ beta, const uint8_t* __restrict__ mask,
-                                                              float* __restrict__ dzout, float* __restrict__ partial,
-                                                              const float* __restrict__ xds, const float* __restrict__ save_mean_d,
+                                                              T* __restrict__ dzout, float* __restrict__ partial,
+                                                              const T* __restrict__ xds, const float* __restrict__ save_mean_d,
                                                               size_t pstride) {
   using S = ClShape<GS>;
   constexpr int UNROLL = 4;
@@ -484,12 +511,12 @@ __global__ void __launch_bounds__(kT, 2) cl_bwd_reduce_kernel(const float* __res
 #pragma unroll
       for (int i = 0; i < S::BWD; ++i) acc[k][i] = 0.f;
     const size_t base = (size_t)d * rows * gm.C + 4 * t.q;
-    const float* xp[NS];
+    const T* xp[NS];
     xp[0] = x + base;
     if constexpr (DS) xp[NS - 1] = xds + base;
-    const float* gd = dout + base;
-    const float* gd2 = D2 ? dout2 + base : nullptr;        // second addend of the incoming gradient (see dwt_b200.h)
-    float* zd = MASK ? dzout + base : nullptr;
+    const T* gd = dout + base;
+    const T* gd2 = D2 ? dout2 + base : nullptr;            // second addend of the incoming gradient (see dwt_b200.h)
+    T* zd = MASK ? dzout + base : nullptr;
     const uint8_t* md = mask + (size_t)d * rows * t.C4 + t.q;
     // rows per load batch: all of the chunk's rows, or (two sites) half of them, so that both sites' accumulators stay
     // in registers.  The rows are accumulated in the same order either way.
@@ -505,10 +532,10 @@ __global__ void __launch_bounds__(kT, 2) cl_bwd_reduce_kernel(const float* __res
         const unsigned rr = r + u * t.rpi;
         if (rr < rows) {
 #pragma unroll
-          for (int k = 0; k < NS; ++k) v[k][u] = ldg4(xp[k] + (size_t)rr * gm.C);
-          q[u] = ldg4(gd + (size_t)rr * gm.C);
+          for (int k = 0; k < NS; ++k) v[k][u] = ld4(xp[k] + (size_t)rr * gm.C);
+          q[u] = ld4(gd + (size_t)rr * gm.C);
           if constexpr (MASK) mb[u] = __ldg(md + (size_t)rr * t.C4);
-          if constexpr (D2) q2[u] = ldg4(gd2 + (size_t)rr * gm.C);
+          if constexpr (D2) q2[u] = ld4(gd2 + (size_t)rr * gm.C);
         } else {
 #pragma unroll
           for (int k = 0; k < NS; ++k) v[k][u] = make_float4(mu[k][0], mu[k][1], mu[k][2], mu[k][3]);
@@ -517,9 +544,12 @@ __global__ void __launch_bounds__(kT, 2) cl_bwd_reduce_kernel(const float* __res
           if constexpr (D2) q2[u] = make_float4(0.f, 0.f, 0.f, 0.f);
         }
       }
-      if constexpr (D2) {
+      if constexpr (D2) {                                      // bf16: RN(dout + dout2), autograd's own bf16 sum
 #pragma unroll
-        for (int u = 0; u < H; ++u) { q[u].x += q2[u].x; q[u].y += q2[u].y; q[u].z += q2[u].z; q[u].w += q2[u].w; }
+        for (int u = 0; u < H; ++u) {
+          q[u].x = as_stored<T>(q[u].x + q2[u].x); q[u].y = as_stored<T>(q[u].y + q2[u].y);
+          q[u].z = as_stored<T>(q[u].z + q2[u].z); q[u].w = as_stored<T>(q[u].w + q2[u].w);
+        }
       }
 #pragma unroll
       for (int u = 0; u < H; ++u) {
@@ -551,7 +581,7 @@ __global__ void __launch_bounds__(kT, 2) cl_bwd_reduce_kernel(const float* __res
         }
         if constexpr (MASK) {
           const unsigned rr = r + u * t.rpi;
-          if (rr < rows) *reinterpret_cast<float4*>(zd + (size_t)rr * gm.C) = make_float4(zm[0], zm[1], zm[2], zm[3]);
+          if (rr < rows) st4(zd + (size_t)rr * gm.C, make_float4(zm[0], zm[1], zm[2], zm[3]));   // exact: zm is a stored value or 0
         }
       }
      }
@@ -651,12 +681,12 @@ struct BwdCoef {
 // The residual tail's apply is the AFFINE one with dout = the masked dz its reduction wrote.  DS (two-site tail):
 // the same dz is the downsample site's output gradient, so the pass also reads xd and writes dxd with the downsample
 // site's coefficients (coef_d).
-template <int GS, int EPI, bool D2, bool DS>
-__global__ void __launch_bounds__(kT, 2) cl_bwd_apply_kernel(const float* __restrict__ x, const float* __restrict__ dout, const float* __restrict__ dout2,
-                                                             float* __restrict__ dx, const Geom gm, const float* __restrict__ coef,
+template <class T, int GS, int EPI, bool D2, bool DS>
+__global__ void __launch_bounds__(kT, 2) cl_bwd_apply_kernel(const T* __restrict__ x, const T* __restrict__ dout, const T* __restrict__ dout2,
+                                                             T* __restrict__ dx, const Geom gm, const float* __restrict__ coef,
                                                              const float* __restrict__ save_mean, const float* __restrict__ save_w,
                                                              const float* __restrict__ gamma, const float* __restrict__ beta,
-                                                             const float* __restrict__ xds, float* __restrict__ dxds,
+                                                             const T* __restrict__ xds, T* __restrict__ dxds,
                                                              const float* __restrict__ coef_d) {
   using S = ClShape<GS>;
   constexpr int UNROLL = 4;
@@ -680,12 +710,12 @@ __global__ void __launch_bounds__(kT, 2) cl_bwd_apply_kernel(const float* __rest
       for (int k = 0; k < NS; ++k) cf[k][s].load((k ? coef_d : coef) + ((size_t)d * gm.G + g) * coef_stride(GS));
     }
     const size_t base = (size_t)d * rows * gm.C + 4 * t.q;
-    const float* xp[NS];
-    float* op[NS];
+    const T* xp[NS];
+    T* op[NS];
     xp[0] = x + base; op[0] = dx + base;
     if constexpr (DS) { xp[NS - 1] = xds + base; op[NS - 1] = dxds + base; }
-    const float* gd = dout + base;
-    const float* gd2 = D2 ? dout2 + base : nullptr;        // second addend of the incoming gradient (see dwt_b200.h)
+    const T* gd = dout + base;
+    const T* gd2 = D2 ? dout2 + base : nullptr;            // second addend of the incoming gradient (see dwt_b200.h)
     sweep_rows<UNROLL, false>(t, rows, [&](unsigned r) {
       float4 v[NS][UNROLL], q[UNROLL], q2[D2 ? UNROLL : 1];
 #pragma unroll
@@ -693,15 +723,18 @@ __global__ void __launch_bounds__(kT, 2) cl_bwd_apply_kernel(const float* __rest
         const unsigned rr = r + u * t.rpi;
         if (rr < rows) {
 #pragma unroll
-          for (int k = 0; k < NS; ++k) v[k][u] = ldg4(xp[k] + (size_t)rr * gm.C);
-          q[u] = ldg4(gd + (size_t)rr * gm.C);
-          if constexpr (D2) q2[u] = ldg4(gd2 + (size_t)rr * gm.C);
+          for (int k = 0; k < NS; ++k) v[k][u] = ld4(xp[k] + (size_t)rr * gm.C);
+          q[u] = ld4(gd + (size_t)rr * gm.C);
+          if constexpr (D2) q2[u] = ld4(gd2 + (size_t)rr * gm.C);
         }
       }
       if constexpr (D2) {
 #pragma unroll
         for (int u = 0; u < UNROLL; ++u)
-          if (r + u * t.rpi < rows) { q[u].x += q2[u].x; q[u].y += q2[u].y; q[u].z += q2[u].z; q[u].w += q2[u].w; }
+          if (r + u * t.rpi < rows) {                            // the reduction's sum, as there
+            q[u].x = as_stored<T>(q[u].x + q2[u].x); q[u].y = as_stored<T>(q[u].y + q2[u].y);
+            q[u].z = as_stored<T>(q[u].z + q2[u].z); q[u].w = as_stored<T>(q[u].w + q2[u].w);
+          }
       }
 #pragma unroll
       for (int u = 0; u < UNROLL; ++u) {
@@ -725,7 +758,7 @@ __global__ void __launch_bounds__(kT, 2) cl_bwd_apply_kernel(const float* __rest
               }
               cf[k][s].apply(dz, xi, o + s * GS);
             }
-            *reinterpret_cast<float4*>(op[k] + (size_t)rr * gm.C) = make_float4(o[0], o[1], o[2], o[3]);
+            st4(op[k] + (size_t)rr * gm.C, make_float4(o[0], o[1], o[2], o[3]));
           }
         }
       }
@@ -787,8 +820,15 @@ int cl_fwd_width(int C, int GS) { return (C / 4) * (4 / GS) * (GS + GS * (GS + 1
 int cl_bwd_width(int C, int GS) { return (C / 4) * (4 / GS) * (GS * GS + GS); }
 
 
-void cl_stats(const float* x, const Geom& gm, int nctas, int gz, float* partial, float* shift, cudaStream_t st) {
-  CL_GS(gm.GS, (cl_stats_kernel<kGS><<<cl_grid(gm, nctas, gz), kT, 0, st>>>(x, gm, partial, shift)));
+// Activation storage of a launch: TT = float, or __nv_bfloat16 when bf16
+#define CL_T(BF16_, ...)                                                  \
+  if (BF16_) { using TT = __nv_bfloat16; __VA_ARGS__; }                   \
+  else { using TT = float; __VA_ARGS__; }
+#define CL_IN(P_) static_cast<const TT*>(P_)
+#define CL_OUT(P_) static_cast<TT*>(P_)
+
+void cl_stats(const void* x, bool bf16, const Geom& gm, int nctas, int gz, float* partial, float* shift, cudaStream_t st) {
+  CL_T(bf16, CL_GS(gm.GS, (cl_stats_kernel<TT, kGS><<<cl_grid(gm, nctas, gz), kT, 0, st>>>(CL_IN(x), gm, partial, shift))));
 }
 inline dim3 fin_block(const Geom& gm) { const int c4 = gm.C / 4; return dim3(32, c4 < kFinQ ? c4 : kFinQ, gm.D); }
 void cl_fwd_finalize(const float* partial, int nrows, const float* shift, const Geom& gm, const FwdFin& fin, cudaStream_t st,
@@ -796,51 +836,66 @@ void cl_fwd_finalize(const float* partial, int nrows, const float* shift, const 
   const dim3 b = fin_block(gm), g((gm.C / 4) / b.y, fin2 ? 2 : 1);
   CL_GS(gm.GS, (launch_k(cl_fwd_finalize_kernel<kGS>, g, b, st, use_pdl(), partial, pstride, nrows, shift, sstride, gm, fin, fin2 ? *fin2 : fin)));
 }
-void cl_apply(const float* x, float* y, const Geom& gm, int nctas, int gz, int epi, const float* mean, const float* w,
-              const float* gamma, const float* beta, const float* residual, uint8_t* mask, cudaStream_t st) {
+void cl_apply(const void* x, void* y, bool bf16, const Geom& gm, int nctas, int gz, int epi, const float* mean, const float* w,
+              const float* gamma, const float* beta, const void* residual, uint8_t* mask, cudaStream_t st) {
   const float* nul = nullptr;
-  if (epi == 7) {
-    CL_GS(gm.GS, (launch_k(cl_apply_kernel<kGS, 7, false>, cl_grid(gm, nctas, gz), dim3(kT), st, use_pdl(), x, y, gm, mean, w, gamma, beta, residual, mask,
-                           nul, nul, nul, nul)));
-    return;
-  }
-  CL_GS(gm.GS, CL_EPI(epi, (launch_k(cl_apply_kernel<kGS, kEPI, false>, cl_grid(gm, nctas, gz), dim3(kT), st, use_pdl(), x, y, gm, mean, w, gamma, beta,
-                                     nul, (uint8_t*)nullptr, nul, nul, nul, nul))));
+  CL_T(bf16, {
+    const TT* tnul = nullptr;
+    if (epi == 7) {
+      CL_GS(gm.GS, (launch_k(cl_apply_kernel<TT, kGS, 7, false>, cl_grid(gm, nctas, gz), dim3(kT), st, use_pdl(), CL_IN(x), CL_OUT(y), gm, mean, w,
+                             gamma, beta, CL_IN(residual), mask, nul, nul, nul, nul)));
+    } else {
+      CL_GS(gm.GS, CL_EPI(epi, (launch_k(cl_apply_kernel<TT, kGS, kEPI, false>, cl_grid(gm, nctas, gz), dim3(kT), st, use_pdl(), CL_IN(x), CL_OUT(y),
+                                         gm, mean, w, gamma, beta, tnul, (uint8_t*)nullptr, nul, nul, nul, nul))));
+    }
+  });
 }
-void cl_tail2_apply(const float* x, const float* xd, float* y, const Geom& gm, int nctas, int gz, const float* mean, const float* w,
+void cl_tail2_apply(const void* x, const void* xd, void* y, bool bf16, const Geom& gm, int nctas, int gz, const float* mean, const float* w,
                     const float* gamma, const float* beta, const float* mean_d, const float* w_d, const float* gamma_d,
                     const float* beta_d, uint8_t* mask, cudaStream_t st) {
-  CL_GS(gm.GS, (launch_k(cl_apply_kernel<kGS, 7, true>, cl_grid(gm, nctas, gz), dim3(kT), st, use_pdl(), x, y, gm, mean, w, gamma, beta, xd, mask,
-                         mean_d, w_d, gamma_d, beta_d)));
+  CL_T(bf16, CL_GS(gm.GS, (launch_k(cl_apply_kernel<TT, kGS, 7, true>, cl_grid(gm, nctas, gz), dim3(kT), st, use_pdl(), CL_IN(x), CL_OUT(y), gm, mean,
+                                    w, gamma, beta, CL_IN(xd), mask, mean_d, w_d, gamma_d, beta_d))));
 }
-void cl_bwd_reduce(const float* x, const float* dout, const float* dout2, const Geom& gm, int nctas, int gz, int epi, const float* mean, const float* w,
-                   const float* gamma, const float* beta, const uint8_t* mask, float* dz, float* partial, cudaStream_t st) {
+void cl_bwd_reduce(const void* x, const void* dout, const void* dout2, bool bf16, const Geom& gm, int nctas, int gz, int epi, const float* mean,
+                   const float* w, const float* gamma, const float* beta, const uint8_t* mask, void* dz, float* partial, cudaStream_t st) {
   const float* nul = nullptr;
-  CL_GS(gm.GS, CL_D2(dout2, CL_EPI_BWD(epi, (cl_bwd_reduce_kernel<kGS, kEPI, kD2, false><<<cl_grid(gm, nctas, gz), kT, 0, st>>>(
-                                                x, dout, dout2, gm, mean, w, gamma, beta, mask, dz, partial, nul, nul, 0)))));
+  CL_T(bf16, {
+    const TT* tnul = nullptr;
+    CL_GS(gm.GS, CL_D2(dout2, CL_EPI_BWD(epi, (cl_bwd_reduce_kernel<TT, kGS, kEPI, kD2, false><<<cl_grid(gm, nctas, gz), kT, 0, st>>>(
+                                                  CL_IN(x), CL_IN(dout), CL_IN(dout2), gm, mean, w, gamma, beta, mask, CL_OUT(dz), partial, tnul,
+                                                  nul, 0)))));
+  });
 }
-void cl_tail2_bwd_reduce(const float* x, const float* xd, const float* dout, const float* dout2, const Geom& gm, int nctas, int gz,
-                         const float* mean, const float* mean_d, const uint8_t* mask, float* dz, float* partial, size_t pstride,
+void cl_tail2_bwd_reduce(const void* x, const void* xd, const void* dout, const void* dout2, bool bf16, const Geom& gm, int nctas, int gz,
+                         const float* mean, const float* mean_d, const uint8_t* mask, void* dz, float* partial, size_t pstride,
                          cudaStream_t st) {
   const float* nul = nullptr;
-  CL_GS(gm.GS, CL_D2(dout2, (cl_bwd_reduce_kernel<kGS, 7, kD2, true><<<cl_grid(gm, nctas, gz), kT, 0, st>>>(
-                                x, dout, dout2, gm, mean, nul, nul, nul, mask, dz, partial, xd, mean_d, pstride))));
+  CL_T(bf16, CL_GS(gm.GS, CL_D2(dout2, (cl_bwd_reduce_kernel<TT, kGS, 7, kD2, true><<<cl_grid(gm, nctas, gz), kT, 0, st>>>(
+                                           CL_IN(x), CL_IN(dout), CL_IN(dout2), gm, mean, nul, nul, nul, mask, CL_OUT(dz), partial, CL_IN(xd),
+                                           mean_d, pstride)))));
 }
 void cl_bwd_finalize(const float* partial, int nrows, const Geom& gm, const BwdFin& fin, cudaStream_t st, const BwdFin* fin2, size_t pstride) {
   const dim3 b = fin_block(gm), g((gm.C / 4) / b.y, fin2 ? 2 : 1);
   CL_GS(gm.GS, (launch_k(cl_bwd_finalize_kernel<kGS>, g, b, st, use_pdl(), partial, pstride, nrows, gm, fin, fin2 ? *fin2 : fin)));
 }
-void cl_bwd_apply(const float* x, const float* dout, const float* dout2, float* dx, const Geom& gm, int nctas, int gz, int epi, const float* coef,
-                  const float* mean, const float* w, const float* gamma, const float* beta, cudaStream_t st) {
+void cl_bwd_apply(const void* x, const void* dout, const void* dout2, void* dx, bool bf16, const Geom& gm, int nctas, int gz, int epi,
+                  const float* coef, const float* mean, const float* w, const float* gamma, const float* beta, cudaStream_t st) {
   const float* nul = nullptr;
-  CL_GS(gm.GS, CL_D2(dout2, CL_EPI(epi, (launch_k(cl_bwd_apply_kernel<kGS, kEPI, kD2, false>, cl_grid(gm, nctas, gz), dim3(kT), st, use_pdl(), x, dout,
-                                                  dout2, dx, gm, coef, mean, w, gamma, beta, nul, (float*)nullptr, nul)))));
+  CL_T(bf16, {
+    const TT* tnul = nullptr;
+    CL_GS(gm.GS, CL_D2(dout2, CL_EPI(epi, (launch_k(cl_bwd_apply_kernel<TT, kGS, kEPI, kD2, false>, cl_grid(gm, nctas, gz), dim3(kT), st, use_pdl(),
+                                                    CL_IN(x), CL_IN(dout), CL_IN(dout2), CL_OUT(dx), gm, coef, mean, w, gamma, beta, tnul,
+                                                    (TT*)nullptr, nul)))));
+  });
 }
-void cl_tail2_bwd_apply(const float* x, const float* xd, const float* dz, float* dx, float* dxd, const Geom& gm, int nctas, int gz,
+void cl_tail2_bwd_apply(const void* x, const void* xd, const void* dz, void* dx, void* dxd, bool bf16, const Geom& gm, int nctas, int gz,
                         const float* coef, const float* coef_d, cudaStream_t st) {
   const float* nul = nullptr;
-  CL_GS(gm.GS, (launch_k(cl_bwd_apply_kernel<kGS, 1, false, true>, cl_grid(gm, nctas, gz), dim3(kT), st, use_pdl(), x, dz, nul, dx, gm, coef,
-                         nul, nul, nul, nul, xd, dxd, coef_d)));
+  CL_T(bf16, {
+    const TT* tnul = nullptr;
+    CL_GS(gm.GS, (launch_k(cl_bwd_apply_kernel<TT, kGS, 1, false, true>, cl_grid(gm, nctas, gz), dim3(kT), st, use_pdl(), CL_IN(x), CL_IN(dz), tnul,
+                           CL_OUT(dx), gm, coef, nul, nul, nul, nul, CL_IN(xd), CL_OUT(dxd), coef_d)));
+  });
 }
 
 }  // namespace dwt

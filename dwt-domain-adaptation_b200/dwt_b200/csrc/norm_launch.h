@@ -67,35 +67,37 @@ int tc_bwd_apply(const float* x, const float* dout, float* dx, const Geom& gm, i
 bool cl_supports(int C, int GS);
 int cl_fwd_width(int C, int GS);
 int cl_bwd_width(int C, int GS);
+// Activation pointers are void: fp32, or bf16 when `bf16` (DWT_DTYPE_BF16; the same kernels, loads widened to fp32 and
+// stores rounded to nearest-even).  Statistics, partial rows, coefficients and running buffers are fp32 either way.
 // The finalize launches serve a second site (the two-site tail) when fin2 is given: its partial rows start at
 // partial + pstride, its pilot shifts at shift + sstride.
-void cl_stats(const float* x, const Geom& gm, int nctas, int gz, float* partial, float* shift, cudaStream_t st);
+void cl_stats(const void* x, bool bf16, const Geom& gm, int nctas, int gz, float* partial, float* shift, cudaStream_t st);
 void cl_fwd_finalize(const float* partial, int nrows, const float* shift, const Geom& gm, const FwdFin& fin, cudaStream_t st,
                      const FwdFin* fin2 = nullptr, size_t pstride = 0, size_t sstride = 0);
-void cl_apply(const float* x, float* y, const Geom& gm, int nctas, int gz, int epi, const float* mean, const float* w,
-              const float* gamma, const float* beta, const float* residual, uint8_t* mask, cudaStream_t st);
+void cl_apply(const void* x, void* y, bool bf16, const Geom& gm, int nctas, int gz, int epi, const float* mean, const float* w,
+              const float* gamma, const float* beta, const void* residual, uint8_t* mask, cudaStream_t st);
 // epi 7 (residual tail): masks dout (+ dout2) with the byte map and writes the masked gradient to dz
-void cl_bwd_reduce(const float* x, const float* dout, const float* dout2, const Geom& gm, int nctas, int gz, int epi, const float* mean, const float* w,
-                   const float* gamma, const float* beta, const uint8_t* mask, float* dz, float* partial, cudaStream_t st);
+void cl_bwd_reduce(const void* x, const void* dout, const void* dout2, bool bf16, const Geom& gm, int nctas, int gz, int epi, const float* mean,
+                   const float* w, const float* gamma, const float* beta, const uint8_t* mask, void* dz, float* partial, cudaStream_t st);
 void cl_bwd_finalize(const float* partial, int nrows, const Geom& gm, const BwdFin& fin, cudaStream_t st,
                      const BwdFin* fin2 = nullptr, size_t pstride = 0);
 // epi 0, 1 or 3; the residual tail runs it with epi 1 on the dz of its reduction
-void cl_bwd_apply(const float* x, const float* dout, const float* dout2, float* dx, const Geom& gm, int nctas, int gz, int epi, const float* coef,
-                  const float* mean, const float* w, const float* gamma, const float* beta, cudaStream_t st);
+void cl_bwd_apply(const void* x, const void* dout, const void* dout2, void* dx, bool bf16, const Geom& gm, int nctas, int gz, int epi,
+                  const float* coef, const float* mean, const float* w, const float* gamma, const float* beta, cudaStream_t st);
 // two-site tail relu(site(x) + site_d(xd)): site's epilogue AFFINE|RELU|RESIDUAL, site_d's AFFINE
-void cl_tail2_apply(const float* x, const float* xd, float* y, const Geom& gm, int nctas, int gz, const float* mean, const float* w,
+void cl_tail2_apply(const void* x, const void* xd, void* y, bool bf16, const Geom& gm, int nctas, int gz, const float* mean, const float* w,
                     const float* gamma, const float* beta, const float* mean_d, const float* w_d, const float* gamma_d,
                     const float* beta_d, uint8_t* mask, cudaStream_t st);
-void cl_tail2_bwd_reduce(const float* x, const float* xd, const float* dout, const float* dout2, const Geom& gm, int nctas, int gz,
-                         const float* mean, const float* mean_d, const uint8_t* mask, float* dz, float* partial, size_t pstride,
+void cl_tail2_bwd_reduce(const void* x, const void* xd, const void* dout, const void* dout2, bool bf16, const Geom& gm, int nctas, int gz,
+                         const float* mean, const float* mean_d, const uint8_t* mask, void* dz, float* partial, size_t pstride,
                          cudaStream_t st);
-void cl_tail2_bwd_apply(const float* x, const float* xd, const float* dz, float* dx, float* dxd, const Geom& gm, int nctas, int gz,
+void cl_tail2_bwd_apply(const void* x, const void* xd, const void* dz, void* dx, void* dxd, bool bf16, const Geom& gm, int nctas, int gz,
                         const float* coef, const float* coef_d, cudaStream_t st);
 
-// channels-last max-pool (pool.cu)
-void maxpool_fwd_launch(const float* x, float* y, uint8_t* idx, int N, int H, int W, int C, int OH, int OW, int k, int s, int p,
+// channels-last max-pool (pool.cu); bf16: x, y, dy, dx are bf16 (compared and summed in fp32, stored rounded)
+void maxpool_fwd_launch(const void* x, void* y, bool bf16, uint8_t* idx, int N, int H, int W, int C, int OH, int OW, int k, int s, int p,
                         cudaStream_t st);
-void maxpool_bwd_launch(const float* dy, const uint8_t* idx, float* dx, int N, int H, int W, int C, int OH, int OW, int k, int s,
+void maxpool_bwd_launch(const void* dy, const uint8_t* idx, void* dx, bool bf16, int N, int H, int W, int C, int OH, int OW, int k, int s,
                         int p, cudaStream_t st);
 
 // MEC loss (mec.cu)

@@ -10,10 +10,15 @@
 //   backward  one CTA per input row, one thread per INPUT float4: the <= ceil(k/s)^2 windows that contain the pixel
 //             are visited, and a window's gradient is taken iff its saved index names this pixel; the stem geometry
 //             (3 x 3 / 2 / 1, even H and W) has its own kernel: one thread per 2 x 2 input patch, all loads up front.
-// Algorithmic bytes: forward 4*(in + out) + out, backward 4*(in + out) + out  (in, out = element counts).
+// Algorithmic bytes: forward 4*(in + out) + out, backward 4*(in + out) + out  (in, out = element counts); bf16 activations
+// (DWT_DTYPE_BF16) 2*(in + out) + out: the same kernels on 8-byte channel quads, widened to fp32 as they load and rounded
+// to nearest-even as they store -- exact for the forward (a maximum is one of its inputs), and for the backward's sums
+// of at most ceil(k/s)^2 gradients it is the fp32 sum rounded once.
 //
 // Semantics = torch.nn.functional.max_pool2d(x, k, s, p) (dilation 1, ceil_mode False) and its autograd, bit for bit
 // including the tie rule (post-ReLU windows of all zeros are common: the gradient goes to the first element).
+#include <cuda_bf16.h>
+
 #include "dwt_common.cuh"
 #include "norm_launch.h"
 
@@ -34,15 +39,36 @@ __device__ __forceinline__ PoolGeom fixed(PoolGeom g) {
 
 __device__ __forceinline__ bool takes(float v, float best) { return (v > best) || (v != v); }
 
+// Storage of one channel quad: a float4, or four bf16 in a uint2
+template <class T> struct Quad;
+template <> struct Quad<float> {
+  using V = float4;
+  static __device__ __forceinline__ float4 widen(const float4& v) { return v; }
+  static __device__ __forceinline__ float4 narrow(const float4& v) { return v; }
+};
+template <> struct Quad<__nv_bfloat16> {
+  using V = uint2;
+  static __device__ __forceinline__ float4 widen(const uint2& u) {
+    return make_float4(__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xFFFF0000u), __uint_as_float(u.y << 16),
+                       __uint_as_float(u.y & 0xFFFF0000u));
+  }
+  static __device__ __forceinline__ uint2 narrow(const float4& v) {
+    const __nv_bfloat162 a = __floats2bfloat162_rn(v.x, v.y), b = __floats2bfloat162_rn(v.z, v.w);
+    return make_uint2(*reinterpret_cast<const unsigned*>(&a), *reinterpret_cast<const unsigned*>(&b));
+  }
+};
+
 // One CTA per output row (n, oh): the W*C4 float4 of up to k input rows are re-read from L1/L2 by neighbouring
 // windows; threads run over (ow, c4) with 32-bit index arithmetic only.
-template <int K, int S, int P, bool POW2>
-__global__ void __launch_bounds__(256) maxpool_fwd_kernel(const float* __restrict__ x, float* __restrict__ y,
+template <class T, int K, int S, int P, bool POW2>
+__global__ void __launch_bounds__(256) maxpool_fwd_kernel(const T* __restrict__ x, T* __restrict__ y,
                                                           uint8_t* __restrict__ idx, const PoolGeom g0) {
+  using Q = Quad<T>;
+  using V = typename Q::V;
   const PoolGeom g = fixed<K, S, P>(g0);
   const int n = blockIdx.x / g.OH, oh = blockIdx.x - n * g.OH;
   const int h0 = oh * g.s - g.p;
-  const float4* xn = reinterpret_cast<const float4*>(x) + (size_t)n * g.H * g.W * g.C4;
+  const V* xn = reinterpret_cast<const V*>(x) + (size_t)n * g.H * g.W * g.C4;
   const size_t obase = ((size_t)n * g.OH + oh) * g.OW * g.C4;
   for (int t = threadIdx.x; t < g.OW * g.C4; t += blockDim.x) {
     const int ow = POW2 ? (t >> g.c4shift) : t / g.C4, c4 = t - ow * g.C4;
@@ -53,12 +79,12 @@ __global__ void __launch_bounds__(256) maxpool_fwd_kernel(const float* __restric
     for (int kh = 0; kh < g.k; ++kh) {
       const int h = h0 + kh;
       if (h < 0 || h >= g.H) continue;
-      const float4* xr = xn + (size_t)h * g.W * g.C4 + c4;
+      const V* xr = xn + (size_t)h * g.W * g.C4 + c4;
 #pragma unroll
       for (int kw = 0; kw < g.k; ++kw) {
         const int w = w0 + kw;
         if (w < 0 || w >= g.W) continue;
-        const float4 v = __ldg(xr + (size_t)w * g.C4);
+        const float4 v = Q::widen(__ldg(xr + (size_t)w * g.C4));
         const float e[4] = {v.x, v.y, v.z, v.w};
         const unsigned code = (unsigned)(kh * g.k + kw);
 #pragma unroll
@@ -66,15 +92,17 @@ __global__ void __launch_bounds__(256) maxpool_fwd_kernel(const float* __restric
           if (takes(e[c], best[c])) { best[c] = e[c]; bi[c] = code; }
       }
     }
-    reinterpret_cast<float4*>(y)[obase + t] = make_float4(best[0], best[1], best[2], best[3]);
+    reinterpret_cast<V*>(y)[obase + t] = Q::narrow(make_float4(best[0], best[1], best[2], best[3]));
     reinterpret_cast<uint32_t*>(idx)[obase + t] = bi[0] | (bi[1] << 8) | (bi[2] << 16) | (bi[3] << 24);
   }
 }
 
 // One CTA per input row (n, h): every input float4 gathers from the <= ceil(k/s)^2 windows that contain it.
-template <int K, int S, int P, bool POW2>
-__global__ void __launch_bounds__(256) maxpool_bwd_kernel(const float* __restrict__ dy, const uint8_t* __restrict__ idx,
-                                                          float* __restrict__ dx, const PoolGeom g0) {
+template <class T, int K, int S, int P, bool POW2>
+__global__ void __launch_bounds__(256) maxpool_bwd_kernel(const T* __restrict__ dy, const uint8_t* __restrict__ idx,
+                                                          T* __restrict__ dx, const PoolGeom g0) {
+  using Q = Quad<T>;
+  using V = typename Q::V;
   const PoolGeom g = fixed<K, S, P>(g0);
   const int n = blockIdx.x / g.H, h = blockIdx.x - n * g.H;
   // windows (oh, ow) with oh*s - p <= h <= oh*s - p + k - 1
@@ -82,9 +110,9 @@ __global__ void __launch_bounds__(256) maxpool_bwd_kernel(const float* __restric
   oh0 = oh0 <= 0 ? 0 : (oh0 + g.s - 1) / g.s;
   int oh1 = (h + g.p) / g.s;
   if (oh1 > g.OH - 1) oh1 = g.OH - 1;
-  const float4* dyn = reinterpret_cast<const float4*>(dy) + (size_t)n * g.OH * g.OW * g.C4;
+  const V* dyn = reinterpret_cast<const V*>(dy) + (size_t)n * g.OH * g.OW * g.C4;
   const uint32_t* ixn = reinterpret_cast<const uint32_t*>(idx) + (size_t)n * g.OH * g.OW * g.C4;
-  float4* dxr = reinterpret_cast<float4*>(dx) + ((size_t)n * g.H + h) * g.W * g.C4;
+  V* dxr = reinterpret_cast<V*>(dx) + ((size_t)n * g.H + h) * g.W * g.C4;
   for (int t = threadIdx.x; t < g.W * g.C4; t += blockDim.x) {
     const int w = POW2 ? (t >> g.c4shift) : t / g.C4, c4 = t - w * g.C4;
     int ow0 = w + g.p - g.k + 1;
@@ -100,7 +128,7 @@ __global__ void __launch_bounds__(256) maxpool_bwd_kernel(const float* __restric
         const uint32_t m = __ldg(ixn + o);
         const bool h0 = (m & 0xFFu) == code, h1 = ((m >> 8) & 0xFFu) == code, h2 = ((m >> 16) & 0xFFu) == code, h3 = (m >> 24) == code;
         if (h0 || h1 || h2 || h3) {
-          const float4 gq = __ldg(dyn + o);
+          const float4 gq = Q::widen(__ldg(dyn + o));
           if (h0) acc[0] += gq.x;
           if (h1) acc[1] += gq.y;
           if (h2) acc[2] += gq.z;
@@ -108,7 +136,7 @@ __global__ void __launch_bounds__(256) maxpool_bwd_kernel(const float* __restric
         }
       }
     }
-    dxr[t] = make_float4(acc[0], acc[1], acc[2], acc[3]);
+    dxr[t] = Q::narrow(make_float4(acc[0], acc[1], acc[2], acc[3]));
   }
 }
 
@@ -118,14 +146,17 @@ __global__ void __launch_bounds__(256) maxpool_bwd_kernel(const float* __restric
 // traffic, 0.69 of the HBM peak).  The patch is streamed row by row; every output sees its window in row-major order
 // (rows ascending, columns ascending inside a row), so the tie rule (first maximum keeps the index, NaN wins) is the
 // generic kernel's.
-__global__ void __launch_bounds__(256) maxpool_fwd_3s2_kernel(const float* __restrict__ x, float* __restrict__ y,
+template <class T>
+__global__ void __launch_bounds__(256) maxpool_fwd_3s2_kernel(const T* __restrict__ x, T* __restrict__ y,
                                                               uint8_t* __restrict__ idx, const PoolGeom g) {
+  using Q = Quad<T>;
+  using V = typename Q::V;
   const int OH2 = g.OH >> 1, OW2 = g.OW >> 1;
   const int n = blockIdx.y / OH2, a = blockIdx.y - n * OH2;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= OW2 * g.C4) return;
   const int b = i >> g.c4shift, c4 = i & (g.C4 - 1);
-  const float4* xn = reinterpret_cast<const float4*>(x) + (size_t)n * g.H * g.W * g.C4 + c4;
+  const V* xn = reinterpret_cast<const V*>(x) + (size_t)n * g.H * g.W * g.C4 + c4;
   float best[2][2][4];
   unsigned bi[2][2][4];
 #pragma unroll
@@ -145,7 +176,7 @@ __global__ void __launch_bounds__(256) maxpool_fwd_3s2_kernel(const float* __res
     for (int cc = 0; cc < 5; ++cc) {
       const int w = w0 + cc;
       in[cc] = w >= 0 && w < g.W;
-      row[cc] = in[cc] ? __ldg(xn + ((size_t)h * g.W + w) * g.C4) : make_float4(0.f, 0.f, 0.f, 0.f);
+      row[cc] = in[cc] ? Q::widen(__ldg(xn + ((size_t)h * g.W + w) * g.C4)) : make_float4(0.f, 0.f, 0.f, 0.f);
     }
 #pragma unroll
     for (int oa = 0; oa < 2; ++oa) {
@@ -170,7 +201,7 @@ __global__ void __launch_bounds__(256) maxpool_fwd_3s2_kernel(const float* __res
 #pragma unroll
     for (int ob = 0; ob < 2; ++ob) {
       const size_t o = (((size_t)n * g.OH + 2 * a + oa) * g.OW + 2 * b + ob) * g.C4 + c4;
-      reinterpret_cast<float4*>(y)[o] = make_float4(best[oa][ob][0], best[oa][ob][1], best[oa][ob][2], best[oa][ob][3]);
+      reinterpret_cast<V*>(y)[o] = Q::narrow(make_float4(best[oa][ob][0], best[oa][ob][1], best[oa][ob][2], best[oa][ob][3]));
       reinterpret_cast<uint32_t*>(idx)[o] = bi[oa][ob][0] | (bi[oa][ob][1] << 8) | (bi[oa][ob][2] << 16) | (bi[oa][ob][3] << 24);
     }
 }
@@ -190,14 +221,17 @@ __device__ __forceinline__ void take(float4& acc, const float4& gq, uint32_t m, 
   if ((m >> 24) == code) acc.w += gq.w;
 }
 
-__global__ void __launch_bounds__(256) maxpool_bwd_3s2_kernel(const float* __restrict__ dy, const uint8_t* __restrict__ idx,
-                                                              float* __restrict__ dx, const PoolGeom g) {
+template <class T>
+__global__ void __launch_bounds__(256) maxpool_bwd_3s2_kernel(const T* __restrict__ dy, const uint8_t* __restrict__ idx,
+                                                              T* __restrict__ dx, const PoolGeom g) {
+  using Q = Quad<T>;
+  using V = typename Q::V;
   const int H2 = g.H >> 1, W2 = g.W >> 1;
   const int n = blockIdx.y / H2, k = blockIdx.y - n * H2;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= W2 * g.C4) return;
   const int j = i >> g.c4shift, c4 = i & (g.C4 - 1);
-  const float4* dyn = reinterpret_cast<const float4*>(dy) + (size_t)n * g.OH * g.OW * g.C4;
+  const V* dyn = reinterpret_cast<const V*>(dy) + (size_t)n * g.OH * g.OW * g.C4;
   const uint32_t* ixn = reinterpret_cast<const uint32_t*>(idx) + (size_t)n * g.OH * g.OW * g.C4;
   uint32_t m[2][2];
   float4 gq[2][2];
@@ -208,17 +242,17 @@ __global__ void __launch_bounds__(256) maxpool_bwd_3s2_kernel(const float* __res
       const bool ok = (k + a < g.OH) && (j + b < g.OW);
       const size_t o = ((size_t)(k + a) * g.OW + (j + b)) * g.C4 + c4;
       m[a][b] = ok ? __ldg(ixn + o) : 0xFFFFFFFFu;          // 0xFF matches no code
-      gq[a][b] = ok ? __ldg(dyn + o) : make_float4(0.f, 0.f, 0.f, 0.f);
+      gq[a][b] = ok ? Q::widen(__ldg(dyn + o)) : make_float4(0.f, 0.f, 0.f, 0.f);
     }
   float4 o00 = make_float4(0.f, 0.f, 0.f, 0.f), o01 = o00, o10 = o00, o11 = o00;
   take(o00, gq[0][0], m[0][0], 4u);
   take(o01, gq[0][0], m[0][0], 5u); take(o01, gq[0][1], m[0][1], 3u);
   take(o10, gq[0][0], m[0][0], 7u); take(o10, gq[1][0], m[1][0], 1u);
   take(o11, gq[0][0], m[0][0], 8u); take(o11, gq[0][1], m[0][1], 6u); take(o11, gq[1][0], m[1][0], 2u); take(o11, gq[1][1], m[1][1], 0u);
-  float4* r0 = reinterpret_cast<float4*>(dx) + (((size_t)n * g.H + 2 * k) * g.W + 2 * j) * g.C4 + c4;
-  float4* r1 = r0 + (size_t)g.W * g.C4;
-  r0[0] = o00; r0[g.C4] = o01;
-  r1[0] = o10; r1[g.C4] = o11;
+  V* r0 = reinterpret_cast<V*>(dx) + (((size_t)n * g.H + 2 * k) * g.W + 2 * j) * g.C4 + c4;
+  V* r1 = r0 + (size_t)g.W * g.C4;
+  r0[0] = Q::narrow(o00); r0[g.C4] = Q::narrow(o01);
+  r1[0] = Q::narrow(o10); r1[g.C4] = Q::narrow(o11);
 }
 
 }  // namespace
@@ -229,28 +263,40 @@ int pow2_shift(int v) {
   while ((1 << sh) < v) ++sh;
   return (1 << sh) == v ? sh : -1;
 }
-}  // namespace
 
-void maxpool_fwd_launch(const float* x, float* y, uint8_t* idx, int N, int H, int W, int C, int OH, int OW, int k, int s, int p,
-                        cudaStream_t st) {
+template <class T>
+void maxpool_fwd(const T* x, T* y, uint8_t* idx, int N, int H, int W, int C, int OH, int OW, int k, int s, int p, cudaStream_t st) {
   const int sh = pow2_shift(C / 4);
   const PoolGeom g{N, H, W, C / 4, OH, OW, k, s, p, sh < 0 ? 0 : sh};
   if (k == 3 && s == 2 && p == 1 && sh >= 0 && H % 4 == 0 && W % 4 == 0 && (long long)N * (OH / 2) <= 65535) {
     const int items = (OW / 2) * (C / 4), threads = items >= 256 ? 256 : ((items + 31) / 32) * 32;
-    maxpool_fwd_3s2_kernel<<<dim3((items + threads - 1) / threads, N * (OH / 2)), threads, 0, st>>>(x, y, idx, g);
-  } else if (k == 3 && s == 2 && p == 1 && sh >= 0) maxpool_fwd_kernel<3, 2, 1, true><<<N * OH, 256, 0, st>>>(x, y, idx, g);
-  else maxpool_fwd_kernel<0, 0, 0, false><<<N * OH, 256, 0, st>>>(x, y, idx, g);
+    maxpool_fwd_3s2_kernel<T><<<dim3((items + threads - 1) / threads, N * (OH / 2)), threads, 0, st>>>(x, y, idx, g);
+  } else if (k == 3 && s == 2 && p == 1 && sh >= 0) maxpool_fwd_kernel<T, 3, 2, 1, true><<<N * OH, 256, 0, st>>>(x, y, idx, g);
+  else maxpool_fwd_kernel<T, 0, 0, 0, false><<<N * OH, 256, 0, st>>>(x, y, idx, g);
 }
 
-void maxpool_bwd_launch(const float* dy, const uint8_t* idx, float* dx, int N, int H, int W, int C, int OH, int OW, int k, int s,
-                        int p, cudaStream_t st) {
+template <class T>
+void maxpool_bwd(const T* dy, const uint8_t* idx, T* dx, int N, int H, int W, int C, int OH, int OW, int k, int s, int p, cudaStream_t st) {
   const int sh = pow2_shift(C / 4);
   const PoolGeom g{N, H, W, C / 4, OH, OW, k, s, p, sh < 0 ? 0 : sh};
   if (k == 3 && s == 2 && p == 1 && sh >= 0 && H % 2 == 0 && W % 2 == 0 && (long long)N * (H / 2) <= 65535) {
     const int items = (W / 2) * (C / 4), threads = items >= 256 ? 256 : ((items + 31) / 32) * 32;
-    maxpool_bwd_3s2_kernel<<<dim3((items + threads - 1) / threads, N * (H / 2)), threads, 0, st>>>(dy, idx, dx, g);
-  } else if (k == 3 && s == 2 && p == 1 && sh >= 0) maxpool_bwd_kernel<3, 2, 1, true><<<N * H, 256, 0, st>>>(dy, idx, dx, g);
-  else maxpool_bwd_kernel<0, 0, 0, false><<<N * H, 256, 0, st>>>(dy, idx, dx, g);
+    maxpool_bwd_3s2_kernel<T><<<dim3((items + threads - 1) / threads, N * (H / 2)), threads, 0, st>>>(dy, idx, dx, g);
+  } else if (k == 3 && s == 2 && p == 1 && sh >= 0) maxpool_bwd_kernel<T, 3, 2, 1, true><<<N * H, 256, 0, st>>>(dy, idx, dx, g);
+  else maxpool_bwd_kernel<T, 0, 0, 0, false><<<N * H, 256, 0, st>>>(dy, idx, dx, g);
+}
+}  // namespace
+
+void maxpool_fwd_launch(const void* x, void* y, bool bf16, uint8_t* idx, int N, int H, int W, int C, int OH, int OW, int k, int s, int p,
+                        cudaStream_t st) {
+  if (bf16) maxpool_fwd(static_cast<const __nv_bfloat16*>(x), static_cast<__nv_bfloat16*>(y), idx, N, H, W, C, OH, OW, k, s, p, st);
+  else maxpool_fwd(static_cast<const float*>(x), static_cast<float*>(y), idx, N, H, W, C, OH, OW, k, s, p, st);
+}
+
+void maxpool_bwd_launch(const void* dy, const uint8_t* idx, void* dx, bool bf16, int N, int H, int W, int C, int OH, int OW, int k, int s,
+                        int p, cudaStream_t st) {
+  if (bf16) maxpool_bwd(static_cast<const __nv_bfloat16*>(dy), idx, static_cast<__nv_bfloat16*>(dx), N, H, W, C, OH, OW, k, s, p, st);
+  else maxpool_bwd(static_cast<const float*>(dy), idx, static_cast<float*>(dx), N, H, W, C, OH, OW, k, s, p, st);
 }
 
 }  // namespace dwt

@@ -3,6 +3,11 @@
 Saved for backward: the layer input x plus the tiny per-group statistics (mean, W) -- never a
 centred copy, a transposed copy or the covariance graph the reference's autograd keeps
 (utils/whitening.py:44-55).
+
+Activations are float32 or bfloat16 (what torch.autocast(dtype=torch.bfloat16) hands over from a convolution): a bf16
+call whose activations are all bf16 and channels-last on a channels-last geometry runs the bf16 kernels
+(DWT_DTYPE_BF16); any other bf16 call runs the float32 kernels on upcast copies and casts the result back.  Statistics,
+parameters, their gradients and the running buffers are float32 either way, like nn.BatchNorm2d under autocast.
 """
 from __future__ import annotations
 
@@ -51,11 +56,17 @@ class _NormFunction(torch.autograd.Function):
         lib = nv.lib()
         gs = group_size if kind == "whiten" else 1
         x, n_all, c, hw, nhwc = _dense(x, gs)
-        layout = nv.LAYOUT_NHWC if nhwc else 0
+        bf16 = x.dtype == torch.bfloat16
+        if bf16 and not (nhwc and (residual is None or residual.dtype == x.dtype)):
+            raise nv.NativeError("bfloat16 runs on the channels-last kernels with every activation in bfloat16 (norm() "
+                                 "upcasts anything else)")
+        layout = (nv.LAYOUT_NHWC if nhwc else 0) | (nv.DTYPE_BF16 if bf16 else 0)
         if n_all % n_domains != 0:
             raise ValueError(f"batch of {n_all} does not split into {n_domains} domains")
         n = n_all // n_domains
-        dev = nv.require_cuda(x, gamma, beta, residual, *[t for pair in running for t in pair])
+        stats = [gamma, beta, *[t for pair in running for t in pair]]
+        dev = nv.require_cuda(x, residual, *stats, bf16=True)
+        nv.require_cuda(*stats)                      # parameters and running buffers are float32 whatever x is
         for d, (rm_t, rv_t) in enumerate(running):
             _check_param(f"running mean of domain {d}", rm_t, c)
             _check_param(f"running second moment of domain {d}", rv_t, c * gs)
@@ -137,11 +148,13 @@ class _NormFunction(torch.autograd.Function):
         # second addend of the incoming gradient, left here by fork_for_sum's backward (see there): the channels-last
         # kernels add it where they read dout; any other path adds it now
         dout2 = ctx.__dict__.pop("_dwt_extra_grad", None)
-        if dout2 is not None and not ((mode & nv.LAYOUT_NHWC) and dout2.shape == dout.shape and dout2.dtype == torch.float32
+        if dout.dtype != x.dtype:
+            dout = dout.to(x.dtype)
+        if dout2 is not None and not ((mode & nv.LAYOUT_NHWC) and dout2.shape == dout.shape and dout2.dtype == dout.dtype
                                       and dout2.is_contiguous(memory_format=torch.channels_last)):
             dout, dout2 = dout + dout2, None
         dout = dout.contiguous(memory_format=torch.channels_last) if (mode & nv.LAYOUT_NHWC) else dout.contiguous()
-        dev = nv.require_cuda(dout)
+        dev = nv.require_cuda(dout, bf16=True)
         dx = torch.empty_like(x)
         want_affine = gamma_c is not None and (ctx.needs_input_grad[1] or ctx.needs_input_grad[2])
         d_res = None
@@ -186,7 +199,12 @@ class _TailPairFunction(torch.autograd.Function):
         n_all, c = x.shape[0], x.shape[1]
         hw = x.shape[2] * x.shape[3]
         n = n_all // n_domains
-        dev = nv.require_cuda(x, xd, gamma, beta, gamma_d, beta_d, *[t for run, *_ in sites for pair in run for t in pair])
+        if xd.dtype != x.dtype:
+            raise ValueError("the two-site tail takes two tensors of one dtype")
+        bf16 = x.dtype == torch.bfloat16
+        stats = [gamma, beta, gamma_d, beta_d, *[t for run, *_ in sites for pair in run for t in pair]]
+        dev = nv.require_cuda(x, xd, *stats, bf16=True)
+        nv.require_cuda(*stats)
         params = [(gamma, beta), (gamma_d, beta_d)]
         c_sites = (nv.TailSite * 2)()
         keep = []                                    # save tensors and pointer arrays alive across the call
@@ -209,7 +227,7 @@ class _TailPairFunction(torch.autograd.Function):
         y = torch.empty_like(x)
         mask = torch.empty(x.numel() // 4, dtype=torch.uint8, device=dev)
         ws = nv.workspace(dev, n, c, hw, gs, n_domains)
-        nv_kind = nv.KIND_WHITEN if kind == "whiten" else nv.KIND_BN
+        nv_kind = (nv.KIND_WHITEN if kind == "whiten" else nv.KIND_BN) | (nv.DTYPE_BF16 if bf16 else 0)
         with torch.cuda.device(dev):
             rc = lib.dwt_tail2_fwd(nv_kind, c_sites, nv.ptr(y), nv.ptr(mask), n, c, hw, gs, n_domains, nv.ptr(ws), ws.numel(),
                                    nv.stream_ptr(dev))
@@ -231,11 +249,13 @@ class _TailPairFunction(torch.autograd.Function):
         x, xd, mask, mean0, w0, g0, mean1, w1, g1 = ctx.saved_tensors
         nv_kind, gs, n_domains, n, c, hw, eps, gshape, gshape_d = ctx.cfg
         dout2 = ctx.__dict__.pop("_dwt_extra_grad", None)      # parked by fork_for_sum, as for _NormFunction
-        if dout2 is not None and not (dout2.shape == dout.shape and dout2.dtype == torch.float32
+        if dout.dtype != x.dtype:
+            dout = dout.to(x.dtype)
+        if dout2 is not None and not (dout2.shape == dout.shape and dout2.dtype == dout.dtype
                                       and dout2.is_contiguous(memory_format=torch.channels_last)):
             dout, dout2 = dout + dout2, None
         dout = dout.contiguous(memory_format=torch.channels_last)
-        dev = nv.require_cuda(dout)
+        dev = nv.require_cuda(dout, bf16=True)
         dz = torch.empty_like(x)
         dx, dxd = torch.empty_like(x), torch.empty_like(xd)
         grads = [torch.empty(2, c, dtype=torch.float32, device=dev) for _ in range(2)]   # (dgamma, dbeta) per site
@@ -292,11 +312,22 @@ def fork_for_sum(y):
     return _ForkForSum.apply(y)
 
 
+_ACT_DTYPES = (torch.float32, torch.bfloat16)
+
+
 def norm(x, gamma, beta, *, kind, group_size, n_domains, training_stats, eps, momentum, update_running,
          running, relu=False, residual=None):
     mode = nv.MODE_TRAIN if training_stats else nv.MODE_EVAL
-    return _NormFunction.apply(x, gamma, beta, residual, kind, group_size, n_domains, mode, float(eps),
-                               float(momentum), bool(update_running), running, bool(relu))
+    args = (kind, group_size, n_domains, mode, float(eps), float(momentum), bool(update_running), running, bool(relu))
+    dtypes = {x.dtype} | ({residual.dtype} if residual is not None else set())
+    if torch.bfloat16 in dtypes and dtypes <= set(_ACT_DTYPES):
+        bf16_kernels = dtypes == {torch.bfloat16} and _dense(x, group_size if kind == "whiten" else 1)[4]
+        if not bf16_kernels:
+            # NCHW, group sizes the bf16 kernels lack, or mixed dtypes: the float32 kernels on upcast copies, the result
+            # (and through autograd every gradient of x and the residual) back in x's dtype
+            y = _NormFunction.apply(x.float(), gamma, beta, None if residual is None else residual.float(), *args)
+            return y.to(x.dtype)
+    return _NormFunction.apply(x, gamma, beta, residual, *args)
 
 
 class _MecFunction(torch.autograd.Function):
@@ -322,8 +353,13 @@ class _MecFunction(torch.autograd.Function):
         return g * gx, g * gy
 
 
+def _upcast_logits(t):
+    """bf16 logits (a Linear head under autocast) are [3B, K]: the losses upcast them, their gradient flows back as bf16."""
+    return t.float() if t.dtype == torch.bfloat16 else t
+
+
 def mec_loss(x, y):
-    return _MecFunction.apply(x, y)
+    return _MecFunction.apply(_upcast_logits(x), _upcast_logits(y))
 
 
 class _HeadLossFunction(torch.autograd.Function):
@@ -356,4 +392,4 @@ class _HeadLossFunction(torch.autograd.Function):
 
 def head_loss(logits, labels, lambda_mec):
     """-> (total loss (differentiable), tensor [total, classification, lambda*MEC])."""
-    return _HeadLossFunction.apply(logits, labels, lambda_mec)
+    return _HeadLossFunction.apply(_upcast_logits(logits), labels, lambda_mec)

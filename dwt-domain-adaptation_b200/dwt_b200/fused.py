@@ -57,6 +57,11 @@ class DomainTripleNorm(nn.Module):
             raise ValueError(f"expected {self.n_domains} domain modules")
         if x.dim() != 4:
             raise ValueError('expected 4D input (got {}D input)'.format(x.dim()))
+        if not self.kernel_epilogue and torch.bfloat16 in (x.dtype, getattr(residual, "dtype", None)):
+            # the tensor epilogue would promote to float32 and round twice: the whole site in float32, rounded once
+            out = self.forward(x.float(), mods, gamma, beta, relu, None if residual is None else residual.float(), replicated,
+                               count_batches)
+            return out.to(x.dtype)
         if replicated:
             return self._forward_replicated(x, mods, gamma, beta, relu, residual, count_batches)
         running, eps, momentum, update = self._running_args(mods, count_batches)
@@ -90,11 +95,13 @@ class DomainTripleNorm(nn.Module):
         236-240), `down` being the downsample branch's DomainTripleNorm.  Channels-last tensors of one shape with
         both sites on the fused-epilogue kernels run as ONE two-site call (functional.tail_pair: the identity tensor is
         never written); anything else runs the two-call composition down(xd) -> self(x, residual=identity).  Results,
-        gradients and running buffers are the same either way."""
+        gradients and running buffers are the same either way -- in bfloat16 too: the two-site kernels round the
+        identity to bf16 before they add it, as the composition stores it."""
         mods, down_mods = list(domain_modules), list(down_modules)
         pair = (self.kernel_epilogue and down.kernel_epilogue and self.kind == down.kind
                 and self.group_size == down.group_size and self.n_domains == down.n_domains
                 and len(mods) == len(down_mods) == self.n_domains and x.dim() == 4 and x.shape == xd.shape
+                and x.dtype == xd.dtype
                 and all(t.is_contiguous(memory_format=torch.channels_last) and not t.is_contiguous() for t in (x, xd))
                 and nv.channels_last_supported(x.shape[1], self.group_size))
         if not pair:

@@ -31,7 +31,7 @@
  * (shared-memory opt-in, carve-out) and the TMA encoder are set up once per process, on the device that is
  * current at the first call.  Every entry point may be captured into a CUDA graph.
  *
- * Tensor layout: activations are fp32, contiguous [n_domains * N, C, HW]
+ * Tensor layout: activations are fp32 (or bf16, DWT_DTYPE_BF16), contiguous [n_domains * N, C, HW]
  * ("NCHW" with H*W flattened); domain d owns images [d*N, (d+1)*N).  The
  * reference calls one module per domain (n_domains = 1); the fused domain-triple
  * site passes n_domains = 3 in the order source | target | target-aug.
@@ -46,7 +46,7 @@
 extern "C" {
 #endif
 
-#define DWT_B200_ABI_VERSION 6
+#define DWT_B200_ABI_VERSION 7
 #define DWT_MAX_DOMAINS 4
 #define DWT_MAX_GROUP_SIZE 64
 
@@ -66,6 +66,18 @@ extern "C" {
  * group sizes 1, 2, 4 with C/4 a power of two (the layout cuDNN's tensor-core convolutions want: a
  * channels-last model needs no NCHW<->NHWC copies around its convolutions). */
 #define DWT_LAYOUT_NHWC 0x100
+
+/* activation storage, OR-ed into `mode` (dwt_whiten_*, dwt_bn_*), `kind` (dwt_tail2_*) or `flags` (dwt_maxpool_*):
+ * default = fp32; DWT_DTYPE_BF16 = every ACTIVATION pointer of the call points at bfloat16 -- x, y, residual, dout,
+ * dout2, dx, dresidual / dz, dwt_tail_site.x / .dx, and the max-pool's x, y, dy, dx.  Running buffers, gamma / beta and
+ * their gradients, save_mean / save_w and the workspace stay fp32.  Built for the channels-last kernels only: it needs
+ * DWT_LAYOUT_NHWC (the tail and the max-pool are channels-last anyway) and a group size 1, 2, 4 with C/4 a power of two
+ * (DWT_E_UNSUPPORTED otherwise); bf16 tensors must be 8-byte aligned (DWT_E_INVALID otherwise).
+ * The kernels run the fp32 schedule of the same shape: loads widen to fp32, stores round to nearest-even, so statistics,
+ * running-buffer updates, dgamma / dbeta and status bits are bit for bit those of the fp32 call on the widened inputs,
+ * and every bf16 output is that call's fp32 output rounded.  Two things are rounded where a bf16 caller would round
+ * them: the two-site tail's identity site_d(xd) before it is added, and dout + dout2 (once; both passes use that sum). */
+#define DWT_DTYPE_BF16 0x200
 
 /* epilogue flags */
 #define DWT_EPI_NONE 0
@@ -164,7 +176,8 @@ DWT_API int dwt_bn_bwd(const float *x, const float *dout, const float *dout2, fl
  *   dwt_*_fwd(xd -> identity, AFFINE);  dwt_*_fwd(x -> out, AFFINE|RELU|RESIDUAL, residual = identity)
  * and its backward (dwt_*_bwd of both sites, the second fed the first's dresidual), including running-statistic
  * updates and, per site, the non-positive-definite handling of DWT_STATUS_NOT_PD.
- *   kind        DWT_KIND_WHITEN (as dwt_whiten_*, group_size 1, 2, 4) or DWT_KIND_BN (as dwt_bn_*, group_size 1)
+ *   kind        DWT_KIND_WHITEN (as dwt_whiten_*, group_size 1, 2, 4) or DWT_KIND_BN (as dwt_bn_*, group_size 1),
+ *               optionally | DWT_DTYPE_BF16
  *   relu_mask   the byte map of dwt_whiten_fwd's RESIDUAL epilogue: written by fwd, read by bwd
  *   dz          bwd: tensor-sized scratch, receives dout * (out > 0) (the gradient of both sites' outputs)
  *   dout2       NULL, or a second addend of the incoming gradient, as for dwt_whiten_bwd
@@ -232,14 +245,15 @@ DWT_API int dwt_augment_pair(const uint8_t *images, int64_t B, int src_h, int sr
  * Channels-last max-pool and its backward: the op between the stem whitening site and layer1
  * (nn.MaxPool2d(3, 2, 1), resnet50_dwt_mec_officehome.py:295,337-338).  Semantics = torch max_pool2d (dilation 1,
  * ceil_mode False) and its autograd, bit for bit including ties (first maximum in row-major window order) and NaN.
+ *   flags  0 (fp32) or DWT_DTYPE_BF16 (x, y, dy, dx in bf16, 8-byte aligned; gradients summed in fp32, rounded once)
  *   x  [N, H, W, C] fp32 (torch.channels_last), C % 4 == 0;  y [N, OH, OW, C], OH = (H + 2*padding - kernel)/stride + 1
  *   argmax [N, OH, OW, C] uint8: window-local index kh*kernel + kw of the maximum (written by fwd, read by bwd)
  *   dy [N, OH, OW, C] -> dx [N, H, W, C] (every element written; no atomics, deterministic)
  */
 DWT_API int dwt_maxpool_fwd(const float *x, float *y, uint8_t *argmax, int64_t N, int64_t H, int64_t W, int64_t C,
-                    int kernel, int stride, int padding, dwt_stream_t stream);
+                    int kernel, int stride, int padding, int flags, dwt_stream_t stream);
 DWT_API int dwt_maxpool_bwd(const float *dy, const uint8_t *argmax, float *dx, int64_t N, int64_t H, int64_t W, int64_t C,
-                    int kernel, int stride, int padding, dwt_stream_t stream);
+                    int kernel, int stride, int padding, int flags, dwt_stream_t stream);
 
 /*
  * Measurement hooks (used by bench.py; not part of the reference's surface).
