@@ -94,19 +94,51 @@ __device__ __forceinline__ bool arrive_is_last(int* counter, int n, int* s_flag)
   return last;
 }
 
-// Pilot shift for the one-pass moments: mean of up to 32 pixels from the middle of the
-// first image of each channel of the group.  Every CTA of a (domain, group) computes the
-// same value, so partial sums are directly addable.  (Centres the data well enough that
-// E[(x-K)^2] - (mean-K)^2 does not cancel; the reference is two-pass, whitening.py:41-47.)
+// Pilot shift K of the NCHW one-pass moments, per channel: the mean of up to 32 pixels from the middle of image 0,
+// unless they sit far from the rest of the domain.  E[(x-K)^2] - (mean-K)^2 loses digits in proportion to
+// (K - mean)^2 / var: an image 0 whose pilot window sat 30 sigma off cost 0.28 of the covariance on the tensor-core
+// path at the microbench size (test_nchw_fp64.py).  So 32 samples spread over the domain are read as well (flattened
+// sample (2k+1) M / 64 + the middle pixel: for N a multiple of 64, the middle pixel of images spread across N), and
+// where their mean lies more than 20 of their standard deviations from K, K moves to it -- the rule of the
+// channels-last cl_stats_kernel, whose threshold real activations stay below, so ordinary inputs keep K bit for bit.
+// 32 samples rather than cl_stats' 8: with 8, about 1 % of channels estimate their spread 1.5x too wide and keep a K
+// 30 sigma off, which still cost 4.3e-3 of the microbench covariance on the tensor-core path.  Every CTA of a
+// (domain, group) computes the same K from the same loads, so partial sums stay directly addable.  The reference is
+// two-pass (whitening.py:41-47).
+constexpr int kPilotSpread = 32;
+
+// element offset, from image 0's channel, of spread sample k (0..31) of a domain of N images.  M = N * HW < 2^31
+// (make_plan checks N * C * HW), and the sample index below stays under 2M: 32-bit division, no modulo.
+__device__ __forceinline__ size_t pilot_spread_offset(int k, int N, int HW, size_t img_stride) {
+  const unsigned M = (unsigned)N * (unsigned)HW;
+  unsigned m = (unsigned)((2ull * k + 1) * M / (2 * kPilotSpread)) + (unsigned)HW / 2 + (unsigned)sqrtf((float)HW) / 2;
+  if (m >= M) m -= M;
+  const unsigned n = m / (unsigned)HW;
+  return (size_t)n * img_stride + (m - n * (unsigned)HW);
+}
+
+// s1, s2: sum and sum of squares of (spread sample - K) over the spread samples
+__device__ __forceinline__ float pilot_refine(float K, float s1, float s2) {
+  constexpr float inv = 1.f / kPilotSpread;            // exact
+  const float dk = s1 * inv;                           // spread mean - K; spread variance = s2 / 32 - dk^2
+  return 401.f * dk * dk > 400.f * (s2 * inv) ? K + dk : K;      // dk^2 > 400 * spread variance
+}
+
 __device__ __forceinline__ void pilot_shift(const float* xg /* image 0, first channel of group */,
-                                            int GS, int HW, float* sK) {
+                                            int GS, int N, int HW, size_t img_stride, float* sK) {
   const int np = HW < 32 ? HW : 32;
   const int p0 = ((HW - np) / 2) & ~3;
+  const bool spread = (long long)N * HW > kPilotSpread;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const size_t so = spread && lane < kPilotSpread ? pilot_spread_offset(lane, N, HW, img_stride) : 0;
   for (int c = warp; c < GS; c += kWarps) {
     float v = lane < np ? __ldg(xg + (size_t)c * HW + p0 + lane) : 0.f;
+    const float s = spread && lane < kPilotSpread ? __ldg(xg + (size_t)c * HW + so) : 0.f;
     v = warp_sum(v);
-    if (lane == 0) sK[c] = v / (float)np;
+    const float K = v / (float)np;
+    const float e = spread && lane < kPilotSpread ? s - K : 0.f;
+    const float s1 = warp_sum(e), s2 = warp_sum(e * e);
+    if (lane == 0) sK[c] = spread ? pilot_refine(K, s1, s2) : K;
   }
 }
 

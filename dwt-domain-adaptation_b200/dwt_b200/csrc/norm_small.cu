@@ -114,13 +114,20 @@ __global__ void __launch_bounds__(kThreads, (GS * VEC >= 16) ? 3 : 4) small_stat
   const unsigned items = (unsigned)gm.N * map.PV, stride = gridDim.x * tm.tthreads;
   unsigned i0 = blockIdx.x * tm.tthreads + tm.ttid;
 
-  // Pilot shift (mean of <=32 mid-image pixels of image 0, per channel) overlapped with the
-  // first batch of loads: the loads do not depend on K, only the arithmetic does.
-  float pv[GS];
+  // Pilot shift (mean of <=32 mid-image pixels of image 0, per channel, checked against 32 samples spread over the
+  // domain: pilot_shift in dwt_common.cuh) overlapped with the first batch of loads: the loads do not depend on K,
+  // only the arithmetic does.
+  const bool spread = (long long)gm.N * gm.HW > kPilotSpread;
+  const bool spread_lane = spread && tm.ttid < kPilotSpread;
+  float pv[GS], ps[GS];
   {
     const int np = gm.HW < 32 ? gm.HW : 32, p0 = ((gm.HW - np) / 2) & ~3, lane = threadIdx.x & 31;
+    const size_t so = spread_lane ? pilot_spread_offset(tm.ttid, gm.N, gm.HW, (size_t)gm.C * gm.HW) : 0;
 #pragma unroll
-    for (int c = 0; c < GS; ++c) pv[c] = (tm.ttid < 32 && lane < np) ? __ldg(xg + (size_t)c * gm.HW + p0 + lane) : 0.f;
+    for (int c = 0; c < GS; ++c) {
+      pv[c] = (tm.ttid < 32 && lane < np) ? __ldg(xg + (size_t)c * gm.HW + p0 + lane) : 0.f;
+      ps[c] = spread_lane ? __ldg(xg + (size_t)c * gm.HW + so) : 0.f;
+    }
   }
   float v[UNROLL][GS][VEC];
   bool have[UNROLL];
@@ -141,8 +148,10 @@ __global__ void __launch_bounds__(kThreads, (GS * VEC >= 16) ? 3 : 4) small_stat
     const int np = gm.HW < 32 ? gm.HW : 32;
 #pragma unroll
     for (int c = 0; c < GS; ++c) {
-      const float t = warp_sum(pv[c]);
-      if (tm.ttid == 0) sK[tm.team][c] = t / (float)np;
+      const float K0 = warp_sum(pv[c]) / (float)np;
+      const float e = spread_lane ? ps[c] - K0 : 0.f;
+      const float s1 = warp_sum(e), s2 = warp_sum(e * e);
+      if (tm.ttid == 0) sK[tm.team][c] = spread ? pilot_refine(K0, s1, s2) : K0;
     }
   }
   __syncthreads();

@@ -80,14 +80,23 @@ __device__ __forceinline__ void sts128(uint32_t addr, float a, float b, float c,
   asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
 }
 
-// Pilot shift of channel ch0 + r: the mean of <= 32 mid-image pixels of image 0 of domain d.
+// Pilot shift of channel c: the mean of <= 32 mid-image pixels of image 0 of domain d, moved to the mean of 32 samples
+// spread over the domain where that lies more than 20 of their standard deviations away (pilot_shift in dwt_common.cuh).
 __device__ __forceinline__ float pilot_shift(const float* __restrict__ x, const Geom& gm, int d, int c) {
   if (c >= gm.C) return 0.f;
   const int np = gm.HW < 32 ? gm.HW : 32, p0 = ((gm.HW - np) / 2) & ~3;
-  const float* px = x + ((size_t)d * gm.N * gm.C + c) * gm.HW + p0;
+  const float* xc = x + ((size_t)d * gm.N * gm.C + c) * gm.HW;
   float a = 0.f;
-  for (int k = 0; k < np; ++k) a += __ldg(px + k);
-  return a / (float)np;
+  for (int k = 0; k < np; ++k) a += __ldg(xc + p0 + k);
+  const float K = a / (float)np;
+  if ((long long)gm.N * gm.HW <= kPilotSpread) return K;
+  float s1 = 0.f, s2 = 0.f;
+  for (int k = 0; k < kPilotSpread; ++k) {
+    const float e = __ldg(xc + pilot_spread_offset(k, gm.N, gm.HW, (size_t)gm.C * gm.HW)) - K;
+    s1 += e;
+    s2 = fmaf(e, e, s2);
+  }
+  return pilot_refine(K, s1, s2);
 }
 
 // In-place transform of one landed tile by the 128 threads of a consumer warpgroup (thread t):

@@ -167,7 +167,7 @@ __global__ void __launch_bounds__(kThreads) tiled_stats_kernel(const float* __re
   const int GS = gm.GS, g = blockIdx.y, d = blockIdx.z, tid = threadIdx.x;
   const ReduceSmem L(GS);
   const TileSrc src{x + ((size_t)d * gm.N * gm.C + (size_t)g * GS) * gm.HW, gm.HW, (size_t)gm.C * gm.HW};
-  pilot_shift(src.base, GS, gm.HW, sK);
+  pilot_shift(src.base, GS, gm.N, gm.HW, src.img_stride, sK);
   __syncthreads();
   const unsigned Mtot = (unsigned)gm.N * gm.HW, ntiles = (Mtot + TP - 1) / TP;
   const int blk = tid % L.nblk, slice = tid / L.nblk;

@@ -46,7 +46,8 @@ class DomainTripleNorm(nn.Module):
 
     def forward(self, x, domain_modules, gamma, beta, relu=False, residual=None, replicated=False, count_batches=True):
         """x: [n_domains*N, C, H, W]; domain_modules: the per-domain WTransform2d / BatchNorm2d
-        modules (training mode), whose buffers receive the EMA updates; gamma/beta: [C,1,1];
+        modules, whose buffers receive the EMA updates in training mode and normalise the batch in eval mode (as the
+        modules themselves would); gamma/beta: [C,1,1];
         residual (needs relu=True): out = relu(norm(x)*gamma + beta + residual), the Bottleneck tail
         (resnet50_dwt_mec_officehome.py:239-240) folded into the apply pass.
         count_batches=False: the caller has already done the `num_batches_tracked += 1` of the three BatchNorm
@@ -65,17 +66,21 @@ class DomainTripleNorm(nn.Module):
         if replicated:
             return self._forward_replicated(x, mods, gamma, beta, relu, residual, count_batches)
         running, eps, momentum, update = self._running_args(mods, count_batches)
+        # modules in eval mode normalise with their running statistics, as each module called on its domain would
+        batch_stats = mods[0].training or not mods[0].track_running_stats
         if not self.kernel_epilogue:
             y = F.norm(x, None, None, kind=self.kind, group_size=self.group_size, n_domains=self.n_domains,
-                       training_stats=True, eps=eps, momentum=momentum, update_running=update, running=running)
+                       training_stats=batch_stats, eps=eps, momentum=momentum, update_running=update, running=running)
             return self._tensor_epilogue(y, gamma, beta, relu, residual)
         return F.norm(x, gamma, beta, kind=self.kind, group_size=self.group_size, n_domains=self.n_domains,
-                      training_stats=True, eps=eps, momentum=momentum, update_running=update,
+                      training_stats=batch_stats, eps=eps, momentum=momentum, update_running=update,
                       running=running, relu=relu, residual=residual)
 
     def _running_args(self, mods, count_batches):
-        """-> (running buffer pairs, eps, momentum, update_running) of a training-statistics call on mods."""
+        """-> (running buffer pairs, eps, momentum, update_running) of a call on mods (statistics of the batch when
+        they train, of the running buffers in eval)."""
         m0 = mods[0]
+        update = m0.training and m0.track_running_stats
         if self.kind == "whiten":
             running = [(m.running_mean, m.running_variance) for m in mods]
             eps, momentum = m0.eps, m0.momentum
@@ -86,8 +91,8 @@ class DomainTripleNorm(nn.Module):
                     torch._foreach_add_(counters, 1)
             running = [(m.running_mean, m.running_var) for m in mods]
             eps = m0.eps
-            momentum = m0.momentum if m0.momentum is not None else 1.0 / m0.num_batches_tracked.item()
-        return running, eps, momentum, m0.training and m0.track_running_stats
+            momentum = m0.momentum if m0.momentum is not None or not update else 1.0 / m0.num_batches_tracked.item()
+        return running, eps, momentum or 0.0, update
 
     def forward_with_downsample(self, x, domain_modules, gamma, beta, xd, down, down_modules, down_gamma, down_beta,
                                 count_batches=True):
@@ -101,6 +106,7 @@ class DomainTripleNorm(nn.Module):
         pair = (self.kernel_epilogue and down.kernel_epilogue and self.kind == down.kind
                 and self.group_size == down.group_size and self.n_domains == down.n_domains
                 and len(mods) == len(down_mods) == self.n_domains and x.dim() == 4 and x.shape == xd.shape
+                and mods[0].training and down_mods[0].training
                 and x.dtype == xd.dtype
                 and all(t.is_contiguous(memory_format=torch.channels_last) and not t.is_contiguous() for t in (x, xd))
                 and nv.channels_last_supported(x.shape[1], self.group_size))
