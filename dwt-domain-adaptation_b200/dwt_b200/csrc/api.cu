@@ -120,14 +120,6 @@ int env_int(const char* name, int dflt) {
   return (v && *v) ? atoi(v) : dflt;
 }
 
-// DWT_DTYPE_BF16 (dwt_b200.h): bf16 activations run the channels-last kernels only; a thread's four channels are then
-// 8 bytes, so that is the alignment the tensors need (16 for fp32)
-int check_bf16_geometry(bool bf16, bool nhwc, int64_t C, int GS) {
-  if (bf16 && !(nhwc && dwt::cl_supports((int)C, GS)))
-    return fail(DWT_E_UNSUPPORTED, "bf16 activations are built for the channels-last kernels: DWT_LAYOUT_NHWC, group_size 1, 2, 4 with C/4 a "
-                                   "power of two (C=%lld gs=%d%s)", (long long)C, GS, nhwc ? "" : ", NCHW layout");
-  return DWT_OK;
-}
 int check_align(bool bf16, uintptr_t bits, const char* what) {
   if (bits % (bf16 ? 8 : 16) == 0) return DWT_OK;
   return bf16 ? fail(DWT_E_INVALID, "%s must be 8-byte aligned (bf16)", what) : fail(DWT_E_INVALID, "%s must be 16-byte aligned", what);
@@ -304,6 +296,33 @@ int make_plan(Plan& p, KernelKind reduce_kind, KernelKind ew_kind, const void* a
   return DWT_OK;
 }
 
+// DWT_DTYPE_BF16 (dwt_b200.h): bf16 activations run the channels-last kernels (group sizes 1, 2, 4), where a thread's
+// four channels are 8 bytes, so that is the alignment the tensors need (16 for fp32); and, on NCHW, the tensor-core
+// family (group sizes 8..64, tc_supports), whose TMA loads need 16-byte rows (HW % 8 == 0) and a 16-byte-aligned x / dout
+bool tc_bf16_supports(const dwt::Geom& g) { return dwt::tc_supports(g, 4) && g.HW % 8 == 0; }
+int check_bf16_geometry(bool bf16, bool nhwc, const dwt::Geom& g) {
+  if (!bf16 || (nhwc ? dwt::cl_supports(g.C, g.GS) : tc_bf16_supports(g))) return DWT_OK;
+  if (nhwc)
+    return fail(DWT_E_UNSUPPORTED, "channels-last bf16 activations are built for group_size 1, 2, 4 with C/4 a power of two "
+                                   "(C=%d gs=%d)", g.C, g.GS);
+  return fail(DWT_E_UNSUPPORTED, "NCHW bf16 activations are built for the tensor-core kernels: group_size 8, 16, 32, 64, "
+                                 "HW >= 32 and a multiple of 8, N*HW >= 4096 per domain (C=%d HW=%d N=%d gs=%d)", g.C, g.HW, g.N, g.GS);
+}
+int check_tc_bf16_align(bool bf16, bool nhwc, uintptr_t bits, const char* what) {
+  if (!bf16 || nhwc || bits % 16 == 0) return DWT_OK;
+  return fail(DWT_E_INVALID, "%s must be 16-byte aligned (bf16 NCHW: TMA)", what);
+}
+// the tensor-core family runs every fp32 call whose geometry and alignment it takes (else the tiled kernels), and every
+// bf16 NCHW call (validated above: there is no other bf16 NCHW kernel to fall back to)
+int tc_route(bool bf16, const Plan& p, bool* tc) {
+  if (bf16) {
+    if (ensure_tc() != 0) return fail(DWT_E_LAUNCH, "tensor-core kernel set-up failed (%d)", g_tc_rc);
+    *tc = true;
+  } else {
+    *tc = !p.small && dwt::tc_supports(p.gm, p.vec) && ensure_tc() == 0;
+  }
+  return DWT_OK;
+}
 int check_running(bool need_running, float* const* rmean, float* const* rcov, int D) {
   if (!need_running) return DWT_OK;
   if (!rmean || !rcov) return fail(DWT_E_INVALID, "running buffers required");
@@ -354,10 +373,11 @@ int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, 
   Plan p;
   if (int rc = make_plan(p, K_STATS, K_APPLY, x, y, nullptr, N, C, HW, GS, D)) return rc;
   if (!x || !y || !save_mean || !save_w || !ws) return fail(DWT_E_INVALID, "null pointer argument");
-  if (int rc = check_bf16_geometry(bf16, nhwc, C, GS)) return rc;
+  if (int rc = check_bf16_geometry(bf16, nhwc, p.gm)) return rc;
   if (nhwc && !dwt::cl_supports((int)C, GS))
     return fail(DWT_E_UNSUPPORTED, "channels-last layout is built for group_size 1, 2, 4 with C/4 a power of two (C=%lld gs=%d)", (long long)C, GS);
   if (nhwc) if (int rc = check_align(bf16, (uintptr_t)x | (uintptr_t)y, "channels-last tensors")) return rc;
+  if (int rc = check_tc_bf16_align(bf16, nhwc, (uintptr_t)x, "x")) return rc;
   if (mode != DWT_MODE_TRAIN && mode != DWT_MODE_EVAL) return fail(DWT_E_INVALID, "bad mode %d", mode);
   if ((epi & DWT_EPI_RELU) && !(epi & DWT_EPI_AFFINE)) return fail(DWT_E_INVALID, "RELU epilogue needs AFFINE");
   if ((epi & DWT_EPI_AFFINE) && (!gamma || !beta)) return fail(DWT_E_INVALID, "AFFINE epilogue needs gamma and beta");
@@ -400,32 +420,34 @@ int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, 
     }
     return check_launch("channels-last apply kernel");
   }
-  const bool tc = !p.small && dwt::tc_supports(p.gm, p.vec) && ensure_tc() == 0;
+  bool tc = false;
+  if (int rc = tc_route(bf16, p, &tc)) return rc;
   if (mode == DWT_MODE_TRAIN) {
-    Launch l(p.small ? "small_stats" : (tc ? "tc_stats" : "tiled_stats"), &p.gm, E, st);
+    Launch l(p.small ? "small_stats" : (tc ? fam(bf16, "tc_stats", "tc_stats_bf16") : "tiled_stats"), &p.gm, E, st);
     if (p.small) dwt::small_stats(x, p.gm, p.vec, fin, w.partial, w.counters, st);
     else if (tc) {
-      if (int cr = dwt::tc_stats(x, p.gm, tc_chunks(p.gm), w.shift, w.partial, st))
+      if (int cr = dwt::tc_stats(x, bf16, p.gm, tc_chunks(p.gm), w.shift, w.partial, st))
         return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d) x=%p N=%d C=%d HW=%d D=%d", cr, (const void*)x, p.gm.N, p.gm.C, p.gm.HW, p.gm.D);
     } else dwt::tiled_stats(x, p.gm, p.vec, fin, w.partial, w.counters, st);
   } else {
-    Launch l("eval_prep", &p.gm, 0.0, st);
+    Launch l(fam(bf16, "eval_prep", "eval_prep_bf16"), &p.gm, 0.0, st);
     if (p.small) dwt::small_eval_prep(p.gm, fin, st);
     else if (tc) dwt::dense_fwd_factor(nullptr, nullptr, p.gm, fin, st);
     else dwt::tiled_eval_prep(p.gm, fin, st);
   }
   if (tc && mode == DWT_MODE_TRAIN) {
     if (int rc = check_launch("tensor-core statistics kernel")) return rc;
-    Launch l("dense_fwd_finalize", &p.gm, 0.0, st);
+    Launch l(fam(bf16, "dense_fwd_finalize", "dense_fwd_finalize_bf16"), &p.gm, 0.0, st);
     dwt::dense_partial_reduce(w.partial, tc_chunks(p.gm), dwt::tc_superblocks(p.gm) * D, w.gram, st);
     dwt::dense_fwd_factor(w.gram, w.shift, p.gm, fin, st);
   }
   if (int rc = check_launch("whitening statistics kernel")) return rc;
   {
-    Launch l(p.small ? "small_apply" : (tc ? "tc_apply" : "tiled_apply"), &p.gm, ((epi & DWT_EPI_RESIDUAL) ? 3 : 2) * E, st);
+    Launch l(p.small ? "small_apply" : (tc ? fam(bf16, "tc_apply", "tc_apply_bf16") : "tiled_apply"), &p.gm,
+             ((epi & DWT_EPI_RESIDUAL) ? 3 : 2) * E, st);
     if (p.small) dwt::small_apply(x, y, p.gm_ew, p.vec, p.chunks_ew, epi, save_mean, save_w, gamma, beta, residual, st);
     else if (tc) {
-      if (int cr = dwt::tc_apply(x, y, p.gm, tc_apply_ctas(p.gm, 1, 64), save_mean, save_w, st))
+      if (int cr = dwt::tc_apply(x, y, bf16, p.gm, tc_apply_ctas(p.gm, 1, 64), save_mean, save_w, st))
         return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d)", cr);
     } else dwt::tiled_apply(x, y, p.gm_ew, p.vec, p.chunks_ew, save_mean, save_w, st);
   }
@@ -441,13 +463,14 @@ int whiten_like_bwd(const float* x, const float* dout, const float* dout2, float
   Plan p;
   if (int rc = make_plan(p, K_BWD_REDUCE, K_BWD_APPLY, x, dout, dx, N, C, HW, GS, D)) return rc;
   if (!x || !dout || !dx || !save_mean || !save_w || !ws) return fail(DWT_E_INVALID, "null pointer argument");
-  if (int rc = check_bf16_geometry(bf16, nhwc, C, GS)) return rc;
+  if (int rc = check_bf16_geometry(bf16, nhwc, p.gm)) return rc;
   if (dout2 && (!nhwc || (uintptr_t)dout2 % (bf16 ? 8 : 16) != 0))
     return fail(nhwc ? DWT_E_INVALID : DWT_E_UNSUPPORTED, "a second gradient addend (dout2) is built for the channels-last "
                 "kernels (16-byte aligned tensor, 8 for bf16); add it to dout otherwise");
   if (nhwc && !dwt::cl_supports((int)C, GS))
     return fail(DWT_E_UNSUPPORTED, "channels-last layout is built for group_size 1, 2, 4 with C/4 a power of two (C=%lld gs=%d)", (long long)C, GS);
   if (nhwc) if (int rc = check_align(bf16, (uintptr_t)x | (uintptr_t)dout | (uintptr_t)dx, "channels-last tensors")) return rc;
+  if (int rc = check_tc_bf16_align(bf16, nhwc, (uintptr_t)x | (uintptr_t)dout, "x and dout")) return rc;
   if (mode != DWT_MODE_TRAIN && mode != DWT_MODE_EVAL) return fail(DWT_E_INVALID, "bad mode %d", mode);
   if ((epi & DWT_EPI_RELU) && !(epi & DWT_EPI_AFFINE)) return fail(DWT_E_INVALID, "RELU epilogue needs AFFINE");
   if ((epi & DWT_EPI_AFFINE) && (!gamma || !beta)) return fail(DWT_E_INVALID, "AFFINE epilogue needs gamma and beta");
@@ -497,32 +520,33 @@ int whiten_like_bwd(const float* x, const float* dout, const float* dout2, float
     }
     return check_launch("channels-last backward apply kernel");
   }
-  const bool tc = !p.small && dwt::tc_supports(p.gm, p.vec) && ensure_tc() == 0;
+  bool tc = false;
+  if (int rc = tc_route(bf16, p, &tc)) return rc;
   if (need_reduce) {
-    Launch l(p.small ? "small_bwd_reduce" : (tc ? "tc_bwd_reduce" : "tiled_bwd_reduce"), &p.gm, 2 * E, st);
+    Launch l(p.small ? "small_bwd_reduce" : (tc ? fam(bf16, "tc_bwd_reduce", "tc_bwd_reduce_bf16") : "tiled_bwd_reduce"), &p.gm, 2 * E, st);
     if (p.small) dwt::small_bwd_reduce(x, dout, p.gm, p.vec, fin, beta, w.partial, w.counters, st);
     else if (tc) {
-      if (int cr = dwt::tc_bwd_reduce(x, dout, p.gm, tc_chunks(p.gm), save_mean, w.partial, st))
+      if (int cr = dwt::tc_bwd_reduce(x, dout, bf16, p.gm, tc_chunks(p.gm), save_mean, w.partial, st))
         return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d) x=%p dout=%p N=%d C=%d HW=%d D=%d", cr, (const void*)x, (const void*)dout, p.gm.N, p.gm.C, p.gm.HW, p.gm.D);
     } else dwt::tiled_bwd_reduce(x, dout, p.gm, p.vec, fin, w.partial, w.counters, st);
   } else {
-    Launch l("bwd_prep", &p.gm, 0.0, st);
+    Launch l(fam(bf16, "bwd_prep", "bwd_prep_bf16"), &p.gm, 0.0, st);
     if (p.small) dwt::small_bwd_prep(p.gm, fin, st);
     else if (tc) dwt::dense_bwd_coef(nullptr, p.gm, fin, w.shift, st);
     else dwt::tiled_bwd_prep(p.gm, fin, st);
   }
   if (tc && need_reduce) {
     if (int rc = check_launch("tensor-core backward reduction kernel")) return rc;
-    Launch l("dense_bwd_finalize", &p.gm, 0.0, st);
+    Launch l(fam(bf16, "dense_bwd_finalize", "dense_bwd_finalize_bf16"), &p.gm, 0.0, st);
     dwt::dense_partial_reduce(w.partial, tc_chunks(p.gm), dwt::tc_superblocks(p.gm) * D, w.gram, st);
     dwt::dense_bwd_coef(w.gram, p.gm, fin, w.shift, st);
   }
   if (int rc = check_launch("whitening backward reduction kernel")) return rc;
   {
-    Launch l(p.small ? "small_bwd_apply" : (tc ? "tc_bwd_apply" : "tiled_bwd_apply"), &p.gm, 3 * E, st);
+    Launch l(p.small ? "small_bwd_apply" : (tc ? fam(bf16, "tc_bwd_apply", "tc_bwd_apply_bf16") : "tiled_bwd_apply"), &p.gm, 3 * E, st);
     if (p.small) dwt::small_bwd_apply(x, dout, dx, p.gm_ew, p.vec, p.chunks_ew, epi, w.coef, save_mean, save_w, gamma, beta, st);
     else if (tc) {
-      if (int cr = dwt::tc_bwd_apply(x, dout, dx, p.gm, tc_apply_ctas(p.gm, 1, 64), w.coef, save_mean, w.shift, st))
+      if (int cr = dwt::tc_bwd_apply(x, dout, dx, bf16, p.gm, tc_apply_ctas(p.gm, 1, 64), w.coef, save_mean, w.shift, st))
         return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d)", cr);
     } else dwt::tiled_bwd_apply(x, dout, dx, p.gm_ew, p.vec, p.chunks_ew, w.coef, st);
   }

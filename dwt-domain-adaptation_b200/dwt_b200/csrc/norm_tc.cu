@@ -29,8 +29,19 @@
 // bwd_reduce (tc_contract_kernel) -- single pass: R multiplies already-formed W's in the coefficient algebra and
 // its tf32 product errors are zero-mean over M >= 4096 samples (round-to-nearest operands).
 //
+// bf16 activations (DWT_DTYPE_BF16): both kernels are templated on the storage type T.  A bf16 box is 32 px x 64 ch of
+// 2-byte values, 64-byte rows landed without swizzle (only ld.shared reads it: a warp's 8-byte loads cover whole rows,
+// conflict-free).  The transform widens each value to fp32 and writes exactly what it writes in place for an fp32 tile
+// -- same values, same SWIZZLE_128B positions -- into a per-warpgroup fp32 staging tile (the Gram kernel: hi there, lo to
+// its lo tile; the contraction: xc and dy each to their own), releases the ring stage and issues the unchanged wgmma
+// sequence from the staging tiles.  Grid, tile ranges, warpgroup alternation and epilogue are those of the fp32 kernels,
+// so every partial is bit for bit the fp32 kernel's on x.float().
+//
 // Reference: utils/whitening.py:46-47 of the reference project and its autograd transpose.
 #include <cuda.h>
+#include <cuda_bf16.h>
+
+#include <type_traits>
 
 #include "dwt_common.cuh"
 #include "norm_launch.h"
@@ -46,10 +57,13 @@ constexpr int kProducerWarp = 4 * kConsumers;           // warp 8
 constexpr int kTcThreads = 128 * kConsumers + 32;
 constexpr int kPer = 512 / 128;                         // 16-byte chunks of a tile per consumer thread
 constexpr int kTilePx = 32, kTileCh = 64;
-constexpr int kTileBytes = kTileCh * kTilePx * 4;       // 8192
-constexpr int kStagesBwd = 6;                           // x + dy per stage: 96 KB per CTA, two CTAs per SM
+constexpr int kTileBytes = kTileCh * kTilePx * 4;       // 8192: one fp32 tile (also a staging tile of the bf16 kernels)
+constexpr int kStagesBwd = 6;                           // x + dy per stage: 96 KB per CTA (bf16: 48 KB + 32 KB staging)
 constexpr int kNacc = kTileCh * kTileCh + kTileCh;      // per-CTA partial: 64x64 moments + 64 row sums
-constexpr int kGramStages = 10;                         // 80 KB ring + 2 x 8 KB lo tiles per CTA, two CTAs per SM
+constexpr int kGramStages = 10;                         // 80 KB ring + 2 x 8 KB lo tiles per CTA (bf16: 40 KB + 32 KB)
+// Activation storage T: float, or __nv_bfloat16 (DWT_DTYPE_BF16); a landed box is kTileCh x kTilePx values of T
+template <class T> constexpr bool kBf16 = !std::is_same<T, float>::value;
+template <class T> constexpr int kBoxBytes = kTileCh * kTilePx * (int)sizeof(T);
 constexpr int kMaxStages = kGramStages > kStagesBwd ? kGramStages : kStagesBwd;
 // Consumer warpgroup w takes tiles w, w + 2, ...; both ring lengths are even, so every stage (and all phases of its
 // barriers) belongs to one warpgroup, and an mbarrier parity wait never meets a barrier two phases ahead.
@@ -80,33 +94,57 @@ __device__ __forceinline__ void sts128(uint32_t addr, float a, float b, float c,
   asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
 }
 
+// Pixels 4j .. 4j+3 of tile row `row` as fp32.  fp32: the 16-byte chunk q = 8 row + (j ^ (row & 7)) of the SWIZZLE_128B
+// tile.  bf16: 8 bytes at row * 64 + 8 j of the unswizzled box, widened (bf16 -> fp32 is exact: the high half of the word).
+template <class T>
+__device__ __forceinline__ float4 ld_px4(uint32_t tile, int q, int row, int j) {
+  if constexpr (kBf16<T>) {
+    uint32_t a, b;
+    asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(a), "=r"(b) : "r"(tile + 64u * row + 8u * j));
+    return make_float4(__uint_as_float(a << 16), __uint_as_float(a & 0xFFFF0000u), __uint_as_float(b << 16),
+                       __uint_as_float(b & 0xFFFF0000u));
+  } else {
+    return lds128(tile + 16u * q);
+  }
+}
+template <class T> __device__ __forceinline__ float ldg_f(const T* p) {
+  if constexpr (kBf16<T>) return __bfloat162float(__ldg(p));
+  else return __ldg(p);
+}
+
 // Pilot shift of channel c: the mean of <= 32 mid-image pixels of image 0 of domain d, moved to the mean of 32 samples
 // spread over the domain where that lies more than 20 of their standard deviations away (pilot_shift in dwt_common.cuh).
-__device__ __forceinline__ float pilot_shift(const float* __restrict__ x, const Geom& gm, int d, int c) {
+template <class T>
+__device__ __forceinline__ float pilot_shift(const T* __restrict__ x, const Geom& gm, int d, int c) {
   if (c >= gm.C) return 0.f;
   const int np = gm.HW < 32 ? gm.HW : 32, p0 = ((gm.HW - np) / 2) & ~3;
-  const float* xc = x + ((size_t)d * gm.N * gm.C + c) * gm.HW;
+  const T* xc = x + ((size_t)d * gm.N * gm.C + c) * gm.HW;
   float a = 0.f;
-  for (int k = 0; k < np; ++k) a += __ldg(xc + p0 + k);
+  for (int k = 0; k < np; ++k) a += ldg_f(xc + p0 + k);
   const float K = a / (float)np;
   if ((long long)gm.N * gm.HW <= kPilotSpread) return K;
   float s1 = 0.f, s2 = 0.f;
   for (int k = 0; k < kPilotSpread; ++k) {
-    const float e = __ldg(xc + pilot_spread_offset(k, gm.N, gm.HW, (size_t)gm.C * gm.HW)) - K;
+    const float e = ldg_f(xc + pilot_spread_offset(k, gm.N, gm.HW, (size_t)gm.C * gm.HW)) - K;
     s1 += e;
     s2 = fmaf(e, e, s2);
   }
   return pilot_refine(K, s1, s2);
 }
 
-// In-place transform of one landed tile by the 128 threads of a consumer warpgroup (thread t):
+// Transform of one landed tile by the 128 threads of a consumer warpgroup (thread t), into the fp32 SWIZZLE_128B tile dst
+// (fp32: dst == tile, in place):
 //   v <- RN_tf32(v - shift[row]) inside the tensor, 0 outside; returns per-thread row sums of (v - shift).
 // Chunk q = t + 128*i (16-byte units): row = q >> 3, physical chunk jp = q & 7, logical chunk = jp ^ (row & 7).
-__device__ __forceinline__ void transform_tile(uint32_t tile, int t, const float (&shift)[kPer], int px0, int HW, int ch0,
-                                               int C, float (&rowsum)[kPer]) {
+template <class T>
+__device__ __forceinline__ void transform_tile(uint32_t tile, uint32_t dst, int t, const float (&shift)[kPer], int px0, int HW,
+                                               int ch0, int C, float (&rowsum)[kPer]) {
   float4 v[kPer];
 #pragma unroll
-  for (int i = 0; i < kPer; ++i) v[i] = lds128(tile + 16u * (t + 128 * i));
+  for (int i = 0; i < kPer; ++i) {
+    const int q = t + 128 * i, row = q >> 3;
+    v[i] = ld_px4<T>(tile, q, row, (q & 7) ^ (row & 7));
+  }
 #pragma unroll
   for (int i = 0; i < kPer; ++i) {
     const int q = t + 128 * i, row = q >> 3, jp = q & 7, j = jp ^ (row & 7);
@@ -120,21 +158,25 @@ __device__ __forceinline__ void transform_tile(uint32_t tile, int t, const float
       rowsum[i] += s;
       e[k] = round_tf32(s);
     }
-    sts128(tile + 16u * (t + 128 * i), e[0], e[1], e[2], e[3]);
+    sts128(dst + 16u * (t + 128 * i), e[0], e[1], e[2], e[3]);
   }
 }
 
-// Split transform of one landed Gram tile: s = x - shift inside the tensor, 0 outside; hi = trunc_tf32(s) in place,
-// lo = s - hi (exact) to the warpgroup's lo tile at the same swizzled position; returns per-thread row sums of s.  hi is
-// written explicitly so that HH and LH see the same hi whatever rounding the tensor core applies to fp32 words.  Two
-// chunks at a time: the accumulators leave few registers at two CTAs per SM.
-__device__ __forceinline__ void gram_transform(uint32_t tile, uint32_t lo, int t, const float (&shift)[kPer], int px0, int HW,
-                                               int ch0, int C, float (&rowsum)[kPer]) {
+// Split transform of one landed Gram tile: s = x - shift inside the tensor, 0 outside; hi = trunc_tf32(s) to hi (fp32:
+// the tile itself, in place), lo = s - hi (exact) to the warpgroup's lo tile at the same swizzled position; returns
+// per-thread row sums of s.  hi is written explicitly so that HH and LH see the same hi whatever rounding the tensor core
+// applies to fp32 words.  Two chunks at a time: the accumulators leave few registers at two CTAs per SM.
+template <class T>
+__device__ __forceinline__ void gram_transform(uint32_t tile, uint32_t hi, uint32_t lo, int t, const float (&shift)[kPer], int px0,
+                                               int HW, int ch0, int C, float (&rowsum)[kPer]) {
 #pragma unroll
   for (int h = 0; h < kPer; h += 2) {
     float4 v[2];
 #pragma unroll
-    for (int i = 0; i < 2; ++i) v[i] = lds128(tile + 16u * (t + 128 * (h + i)));
+    for (int i = 0; i < 2; ++i) {
+      const int q = t + 128 * (h + i), row = q >> 3;
+      v[i] = ld_px4<T>(tile, q, row, (q & 7) ^ (row & 7));
+    }
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
       const int q = t + 128 * (h + i), row = q >> 3, j = (q & 7) ^ (row & 7);
@@ -148,7 +190,7 @@ __device__ __forceinline__ void gram_transform(uint32_t tile, uint32_t lo, int t
         e[k] = __uint_as_float(__float_as_uint(s) & kTf32Mask);
         l[k] = s - e[k];
       }
-      sts128(tile + 16u * q, e[0], e[1], e[2], e[3]);
+      sts128(hi + 16u * q, e[0], e[1], e[2], e[3]);
       sts128(lo + 16u * q, l[0], l[1], l[2], l[3]);
     }
   }
@@ -189,10 +231,11 @@ __device__ __forceinline__ void init_ring(TcBarriers& bars, int stages) {
 // ------------------------------------------------------------------------------------------
 // backward contraction: R = sum dy xc^T and the row sums of dy
 // ------------------------------------------------------------------------------------------
+template <class T>
 __global__ void __launch_bounds__(kTcThreads, 2)
 tc_contract_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_g, const Geom gm,
                    const float* __restrict__ save_mean, float* __restrict__ partial) {
-  constexpr int STAGES = kStagesBwd;
+  constexpr int STAGES = kStagesBwd, BOX = kBoxBytes<T>;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   __shared__ TcBarriers bars;
@@ -219,10 +262,10 @@ tc_contract_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
         const int s = it % STAGES;
         mbar_wait_relaxed(&bars.empty[s], ((it / STAGES) & 1) ^ 1);
         const int t = tr.begin + it, n = t / tr.PB, pb = t - n * tr.PB;
-        uint8_t* dst = smem + (size_t)s * 2 * kTileBytes;
-        mbar_arrive_expect_tx(&bars.full[s], 2 * kTileBytes);
+        uint8_t* dst = smem + (size_t)s * 2 * BOX;
+        mbar_arrive_expect_tx(&bars.full[s], 2 * BOX);
         tma_load_3d(dst, &map_x, pb * kTilePx, ch0, d * gm.N + n, &bars.full[s]);
-        tma_load_3d(dst + kTileBytes, &map_g, pb * kTilePx, ch0, d * gm.N + n, &bars.full[s]);
+        tma_load_3d(dst + BOX, &map_g, pb * kTilePx, ch0, d * gm.N + n, &bars.full[s]);
       }
     }
   } else {
@@ -231,25 +274,34 @@ tc_contract_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
     float shift[kPer], zero[kPer], dummy[kPer];
 #pragma unroll
     for (int i = 0; i < kPer; ++i) { shift[i] = sShift[(t + 128 * i) >> 3]; zero[i] = 0.f; dummy[i] = 0.f; }
+    // bf16: the warpgroup's fp32 staging tiles (xc, dy) behind the ring; fp32: the landed tiles themselves
+    const uint32_t stage_f32 = smem_u32(smem + (size_t)STAGES * 2 * BOX + (size_t)wg * 2 * kTileBytes);
     for (int it = wg; it < ntiles; it += kConsumers) {
       const int s = it % STAGES;
       mbar_wait(&bars.full[s], (it / STAGES) & 1);
       const int tl = tr.begin + it, n = tl / tr.PB, pb = tl - n * tr.PB;
-      const uint32_t tile = smem_u32(smem + (size_t)s * 2 * kTileBytes);
-      transform_tile(tile, t, shift, pb * kTilePx, gm.HW, ch0, gm.C, dummy);                     // xc
-      transform_tile(tile + kTileBytes, t, zero, pb * kTilePx, gm.HW, ch0, gm.C, rowsum);        // dy, sums
+      const uint32_t tile = smem_u32(smem + (size_t)s * 2 * BOX);
+      const uint32_t xs = kBf16<T> ? stage_f32 : tile, ys = kBf16<T> ? stage_f32 + kTileBytes : tile + kTileBytes;
+      transform_tile<T>(tile, xs, t, shift, pb * kTilePx, gm.HW, ch0, gm.C, dummy);               // xc
+      transform_tile<T>(tile + BOX, ys, t, zero, pb * kTilePx, gm.HW, ch0, gm.C, rowsum);         // dy, sums
+      if constexpr (kBf16<T>) {                    // the stage is read: it can be refilled while the MMAs run
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&bars.empty[s]);
+      }
       fence_proxy_async();
       warpgroup_sync(wg);
       wgmma_fence();
       fence_operands(acc);
-      const uint64_t xdesc = make_kmajor_sw128_desc(tile), adesc = make_kmajor_sw128_desc(tile + kTileBytes);
+      const uint64_t xdesc = make_kmajor_sw128_desc(xs), adesc = make_kmajor_sw128_desc(ys);
 #pragma unroll
       for (int k = 0; k < kTilePx / 8; ++k) wgmma_m64n64k8_ss(acc, adesc + 2 * k, xdesc + 2 * k);
       wgmma_commit();
-      wgmma_wait<0>();
+      wgmma_wait<0>();                             // bf16: the staging tiles are rewritten by the next transform
       fence_operands(acc);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bars.empty[s]);
+      if constexpr (!kBf16<T>) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&bars.empty[s]);
+      }
     }
   }
 
@@ -270,10 +322,11 @@ tc_contract_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
 // ------------------------------------------------------------------------------------------
 // split-precision Gram kernel (forward statistics): G = HH + LH + LH^T, see the file header
 // ------------------------------------------------------------------------------------------
+template <class T>
 __global__ void __launch_bounds__(kTcThreads, 2)
-tc_gram_kernel(const __grid_constant__ CUtensorMap map_x, const float* __restrict__ x, const Geom gm,
+tc_gram_kernel(const __grid_constant__ CUtensorMap map_x, const T* __restrict__ x, const Geom gm,
                float* __restrict__ shift_out, float* __restrict__ partial) {
-  constexpr int STAGES = kGramStages;
+  constexpr int STAGES = kGramStages, BOX = kBoxBytes<T>;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   __shared__ TcBarriers bars;
@@ -304,15 +357,17 @@ tc_gram_kernel(const __grid_constant__ CUtensorMap map_x, const float* __restric
       for (int it = 0; it < ntiles; ++it) {
         const int s = it % STAGES;
         mbar_wait_relaxed(&bars.empty[s], ((it / STAGES) & 1) ^ 1);
-        mbar_arrive_expect_tx(&bars.full[s], kTileBytes);
-        tma_load_3d(smem + (size_t)s * kTileBytes, &map_x, pb * kTilePx, ch0, d * gm.N + n, &bars.full[s]);
+        mbar_arrive_expect_tx(&bars.full[s], BOX);
+        tma_load_3d(smem + (size_t)s * BOX, &map_x, pb * kTilePx, ch0, d * gm.N + n, &bars.full[s]);
         if (++pb == tr.PB) { pb = 0; ++n; }
       }
     }
   } else {
     // ===== consumer warpgroups: HH[64 x 64] += hi * hi^T,  LH[64 x 64] += lo * hi^T =====
     const int wg = warp >> 2, t = tid & 127;
-    const uint32_t lo = smem_u32(smem + (size_t)STAGES * kTileBytes + (size_t)wg * kTileBytes);
+    // per warpgroup behind the ring: the lo tile (fp32), or the hi staging tile and the lo tile (bf16)
+    const uint32_t wgbuf = smem_u32(smem + (size_t)STAGES * BOX + (size_t)wg * (kBf16<T> ? 2 : 1) * kTileBytes);
+    const uint32_t lo = kBf16<T> ? wgbuf + kTileBytes : wgbuf;
     const uint64_t ldesc = make_kmajor_sw128_desc(lo);
     float shift[kPer];
 #pragma unroll
@@ -321,25 +376,32 @@ tc_gram_kernel(const __grid_constant__ CUtensorMap map_x, const float* __restric
       const int s = it % STAGES;
       mbar_wait(&bars.full[s], (it / STAGES) & 1);
       const int tl = tr.begin + it, n = tl / tr.PB, pb = tl - n * tr.PB;
-      const uint32_t tile = smem_u32(smem + (size_t)s * kTileBytes);
-      gram_transform(tile, lo, t, shift, pb * kTilePx, gm.HW, ch0, gm.C, rowsum);
+      const uint32_t tile = smem_u32(smem + (size_t)s * BOX);
+      const uint32_t hi = kBf16<T> ? wgbuf : tile;
+      gram_transform<T>(tile, hi, lo, t, shift, pb * kTilePx, gm.HW, ch0, gm.C, rowsum);
+      if constexpr (kBf16<T>) {                    // the stage is read: it can be refilled while the MMAs run
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&bars.empty[s]);
+      }
       fence_proxy_async();
       warpgroup_sync(wg);
       wgmma_fence();
       fence_operands(hh);
       fence_operands(lh);
-      const uint64_t bdesc = make_kmajor_sw128_desc(tile);
+      const uint64_t bdesc = make_kmajor_sw128_desc(hi);
 #pragma unroll
       for (int k = 0; k < kTilePx / 8; ++k) {
         wgmma_m64n64k8_ss(hh, bdesc + 2 * k, bdesc + 2 * k);
         wgmma_m64n64k8_ss(lh, ldesc + 2 * k, bdesc + 2 * k);
       }
       wgmma_commit();
-      wgmma_wait<0>();                             // the lo tile is rewritten by this warpgroup's next transform
+      wgmma_wait<0>();                             // the lo (bf16: and hi) tile is rewritten by this warpgroup's next transform
       fence_operands(hh);
       fence_operands(lh);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bars.empty[s]);
+      if constexpr (!kBf16<T>) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&bars.empty[s]);
+      }
     }
   }
 
@@ -373,19 +435,37 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 EncodeTiledFn g_encode = nullptr;
 
-int make_map(CUtensorMap* map, const float* base, const Geom& gm) {
+// fp32: 32 px x 64 ch boxes of 128-byte rows, SWIZZLE_128B (the wgmma operand layout).  bf16: 64-byte rows, no swizzle
+// (read by ld.shared only); TMA then needs HW % 8 == 0 for 16-byte strides.
+int make_map(CUtensorMap* map, const void* base, const Geom& gm, bool bf16) {
+  const cuuint64_t es = bf16 ? 2 : 4;
   const cuuint64_t dims[3] = {(cuuint64_t)gm.HW, (cuuint64_t)gm.C, (cuuint64_t)gm.N * gm.D};
-  const cuuint64_t strides[2] = {(cuuint64_t)gm.HW * 4, (cuuint64_t)gm.C * gm.HW * 4};
+  const cuuint64_t strides[2] = {(cuuint64_t)gm.HW * es, (cuuint64_t)gm.C * gm.HW * es};
   const cuuint32_t box[3] = {kTilePx, kTileCh, 1};
   const cuuint32_t estr[3] = {1, 1, 1};
-  return (int)g_encode(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(base), dims, strides, box, estr,
-                       CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+  return (int)g_encode(map, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<void*>(base),
+                       dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                       bf16 ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
 }
 
+// fp32: the ring (+ the lo tiles); bf16: the ring of half-size boxes + fp32 staging tiles (two per warpgroup)
+template <class T>
 size_t tc_smem_bytes(bool two) {
-  return two ? (size_t)kStagesBwd * 2 * kTileBytes + 1024
-             : (size_t)kGramStages * kTileBytes + (size_t)kConsumers * kTileBytes + 1024;
+  const size_t wgbuf = (size_t)kConsumers * (kBf16<T> ? 2 : 1) * kTileBytes;
+  return two ? (size_t)kStagesBwd * 2 * kBoxBytes<T> + (kBf16<T> ? wgbuf : 0) + 1024
+             : (size_t)kGramStages * kBoxBytes<T> + wgbuf + 1024;
+}
+
+template <class T>
+cudaError_t tc_kernel_attrs() {
+  cudaError_t e = cudaFuncSetAttribute(tc_gram_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes<T>(false));
+  if (e == cudaSuccess)
+    e = cudaFuncSetAttribute(tc_contract_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes<T>(true));
+  // two ~73-97 KB CTAs per SM need the full shared-memory carve-out
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_gram_kernel<T>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_contract_kernel<T>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  return e;
 }
 
 }  // namespace
@@ -396,12 +476,8 @@ int tc_init() {
   cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q);
   if (e != cudaSuccess || fn == nullptr || q != cudaDriverEntryPointSuccess) return e == cudaSuccess ? -1 : (int)e;
   g_encode = reinterpret_cast<EncodeTiledFn>(fn);
-  e = cudaFuncSetAttribute(tc_gram_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes(false));
-  if (e == cudaSuccess)
-    e = cudaFuncSetAttribute(tc_contract_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes(true));
-  // two ~90-97 KB CTAs per SM need the full shared-memory carve-out
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_gram_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_contract_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  e = tc_kernel_attrs<float>();
+  if (e == cudaSuccess) e = tc_kernel_attrs<__nv_bfloat16>();
   if (e == cudaSuccess) e = (cudaError_t)dense_init();
   if (e == cudaSuccess) return tc_apply_init();
   return (int)e;
@@ -418,23 +494,30 @@ bool tc_supports(const Geom& gm, int vec) {
 int tc_superblocks(const Geom& gm) { return (gm.C + kTileCh - 1) / kTileCh; }
 
 // partial: [D][SB][nchunks][64*64+64] per-CTA moments;  shift: [D][SB][64] pilot shift of every channel
-int tc_stats(const float* x, const Geom& gm, int nchunks, float* shift, float* partial, cudaStream_t st) {
+int tc_stats(const void* x, bool bf16, const Geom& gm, int nchunks, float* shift, float* partial, cudaStream_t st) {
   CUtensorMap mx;
   bind_context();
-  if (int rc = make_map(&mx, x, gm)) return rc;
+  if (int rc = make_map(&mx, x, gm, bf16)) return rc;
   dim3 grid(nchunks, tc_superblocks(gm), gm.D);
-  tc_gram_kernel<<<grid, kTcThreads, tc_smem_bytes(false), st>>>(mx, x, gm, shift, partial);
+  if (bf16)
+    tc_gram_kernel<__nv_bfloat16><<<grid, kTcThreads, tc_smem_bytes<__nv_bfloat16>(false), st>>>(
+        mx, static_cast<const __nv_bfloat16*>(x), gm, shift, partial);
+  else
+    tc_gram_kernel<float><<<grid, kTcThreads, tc_smem_bytes<float>(false), st>>>(mx, static_cast<const float*>(x), gm, shift, partial);
   return 0;
 }
 
-int tc_bwd_reduce(const float* x, const float* dout, const Geom& gm, int nchunks, const float* save_mean,
+int tc_bwd_reduce(const void* x, const void* dout, bool bf16, const Geom& gm, int nchunks, const float* save_mean,
                   float* partial, cudaStream_t st) {
   CUtensorMap mx, mg;
   bind_context();
-  if (int rc = make_map(&mx, x, gm)) return rc;
-  if (int rc = make_map(&mg, dout, gm)) return rc;
+  if (int rc = make_map(&mx, x, gm, bf16)) return rc;
+  if (int rc = make_map(&mg, dout, gm, bf16)) return rc;
   dim3 grid(nchunks, tc_superblocks(gm), gm.D);
-  tc_contract_kernel<<<grid, kTcThreads, tc_smem_bytes(true), st>>>(mx, mg, gm, save_mean, partial);
+  if (bf16)
+    tc_contract_kernel<__nv_bfloat16><<<grid, kTcThreads, tc_smem_bytes<__nv_bfloat16>(true), st>>>(mx, mg, gm, save_mean, partial);
+  else
+    tc_contract_kernel<float><<<grid, kTcThreads, tc_smem_bytes<float>(true), st>>>(mx, mg, gm, save_mean, partial);
   return 0;
 }
 

@@ -23,9 +23,16 @@
 //   warps 0-7   two consumer warpgroups taking alternate tiles: load the tile into registers (hi / lo split),
 //               release the stage, 4 x 8 wgmma m64n64k8 per input, then store the 64 x 64 output block.
 //
+// bf16 activations (DWT_DTYPE_BF16): the kernel is templated on the storage type T.  A bf16 input lands as ONE box of
+// 64 px x 64 ch (128-byte rows, SWIZZLE_128B: the A-fragment reads of a warp -- 8 consecutive pixels of 4 channels -- hit
+// four distinct 16-byte chunks); each value is widened to fp32 as it is loaded into the fragment and the output is stored
+// rounded to nearest-even, 2 bytes per element.  Everything between is the fp32 kernel on the same tiles in the same order.
+//
 // Reference: the grouped 1x1 convolution at utils/whitening.py:55 of the reference project and its backward.
 #include <cuda.h>
+#include <cuda_bf16.h>
 #include <cstdlib>
+#include <type_traits>
 
 #include "dwt_common.cuh"
 #include "norm_launch.h"
@@ -45,11 +52,13 @@ constexpr int kProducerWarp = 4 * kConsumers;
 constexpr int kApThreads = 128 * kConsumers + 32;
 constexpr int kMaxStages = 6;
 
-//   one input:  6 stages of 16 KB + hi / lo matrix (32 KB) = 129 KB
-//   two inputs: 4 stages of 32 KB + 2 hi / lo matrices (64 KB) = 193 KB
-template <int NIN> struct ApCfg {
+template <class T> constexpr bool kBf16 = !std::is_same<T, float>::value;
+
+//   one input:  6 stages of 16 KB + hi / lo matrix (32 KB) = 129 KB        bf16: 6 x 8 KB + 32 KB = 81 KB
+//   two inputs: 4 stages of 32 KB + 2 hi / lo matrices (64 KB) = 193 KB    bf16: 4 x 16 KB + 64 KB = 129 KB
+template <class T, int NIN> struct ApCfg {
   static constexpr int STAGES = NIN == 1 ? 6 : 4;
-  static constexpr int SLOT = NIN * kNBox * kBoxBytes;
+  static constexpr int SLOT = NIN * kCh * kTilePx * (int)sizeof(T);
   static constexpr size_t SMEM = (size_t)STAGES * SLOT + (size_t)2 * NIN * kMatBytes + 1024;
   static_assert(STAGES % kConsumers == 0 && STAGES <= kMaxStages, "stage ownership");
 };
@@ -71,7 +80,7 @@ struct ApplyArgs {
   int off[2];             // offset of the matrix applied to input i inside a record
   const float* shift[2];  // per-channel shift of input i
   int shift_stride[2];    // floats per domain in shift[i]
-  float* out;
+  void* out;              // T
   int interleave;         // 1: CTA b takes tiles b, b + grid, b + 2 grid, ... (neighbouring CTAs on neighbouring tiles)
 };
 
@@ -86,17 +95,31 @@ __device__ __forceinline__ float lds32(uint32_t addr) {
 __device__ __forceinline__ uint32_t kmajor_off(int row, int k) {
   return (uint32_t)((k >> 5) * (kCh * 128) + row * 128 + ((((k & 31) >> 2) ^ (row & 7)) << 4) + (k & 3) * 4);
 }
-// Byte offset of (channel ch, pixel p) in the landed tile of one input: box p / 32 is [64 ch x 128 B], SWIZZLE_128B.
+// Byte offset of (channel ch, pixel p) in the landed tile of one input, SWIZZLE_128B.  fp32: box p / 32 is
+// [64 ch x 128 B].  bf16: one box [64 ch x 128 B] of 64 pixels.
+template <class T>
 __device__ __forceinline__ uint32_t tile_off(int ch, int p) {
+  if constexpr (kBf16<T>) return (uint32_t)(ch * 128 + (((p >> 3) ^ (ch & 7)) << 4) + (p & 7) * 2);
   const int pp = p & 31;
   return (uint32_t)((p >> 5) * kBoxBytes + ch * 128 + (((pp >> 2) ^ (ch & 7)) << 4) + (pp & 3) * 4);
 }
+// the landed value at addr, as fp32 (bf16 -> fp32 is exact: the high half of the word)
+template <class T>
+__device__ __forceinline__ float lds_f(uint32_t addr) {
+  if constexpr (kBf16<T>) {
+    unsigned short u;
+    asm volatile("ld.shared.u16 %0, [%1];" : "=h"(u) : "r"(addr));
+    return __uint_as_float((uint32_t)u << 16);
+  } else {
+    return lds32(addr);
+  }
+}
 
-template <int NIN>
+template <class T, int NIN>
 __global__ void __launch_bounds__(kApThreads, 1)
 tc_apply_kernel(const __grid_constant__ CUtensorMap map0, const __grid_constant__ CUtensorMap map1, const Geom gm,
                 const ApplyArgs args) {
-  using Cfg = ApCfg<NIN>;
+  using Cfg = ApCfg<T, NIN>;
   constexpr int STAGES = Cfg::STAGES, SLOT = Cfg::SLOT;
   extern __shared__ __align__(1024) uint8_t smem_dyn[];
   uint8_t* sRing = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
@@ -106,12 +129,12 @@ tc_apply_kernel(const __grid_constant__ CUtensorMap map0, const __grid_constant_
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, tid = threadIdx.x;
   const int sb = blockIdx.y, d = blockIdx.z, ch0 = sb * kCh;
   const int PB = (gm.HW + kTilePx - 1) / kTilePx;
-  const long long T = (long long)gm.N * PB;
+  const long long NT = (long long)gm.N * PB;
   // tile of step `it`: a contiguous range per CTA, or (interleave) the CTAs of a super-block walk the tensor side by side
   const int t_step = args.interleave ? (int)gridDim.x : 1;
-  const int t_begin = args.interleave ? (int)blockIdx.x : (int)(T * blockIdx.x / gridDim.x);
-  const int ntiles = args.interleave ? (int)((T - blockIdx.x + gridDim.x - 1) / gridDim.x)
-                                     : (int)(T * (blockIdx.x + 1) / gridDim.x) - t_begin;
+  const int t_begin = args.interleave ? (int)blockIdx.x : (int)(NT * blockIdx.x / gridDim.x);
+  const int ntiles = args.interleave ? (int)((NT - blockIdx.x + gridDim.x - 1) / gridDim.x)
+                                     : (int)(NT * (blockIdx.x + 1) / gridDim.x) - t_begin;
 
   if (tid == 0) {
     for (int s = 0; s < STAGES; ++s) { mbar_init(&bars.full[s], 1); mbar_init(&bars.empty[s], 4); }
@@ -145,18 +168,25 @@ tc_apply_kernel(const __grid_constant__ CUtensorMap map0, const __grid_constant_
     if (lane == 0) {
       for (int it = 0; it < ntiles; ++it) {
         const int t = t_begin + it * t_step, n = t / PB, pb = t - n * PB, s = it % STAGES;
-        // 32-pixel boxes of the tile that lie entirely past the row end are not issued (they only feed output
-        // pixels that are never stored, whatever the stale shared memory holds)
-        int nbox = (gm.HW - pb * kTilePx + kBoxPx - 1) / kBoxPx;
-        nbox = nbox < kNBox ? nbox : kNBox;
         mbar_wait_relaxed(&bars.empty[s], ((it / STAGES) & 1) ^ 1);
-        mbar_arrive_expect_tx(&bars.full[s], NIN * nbox * kBoxBytes);
         uint8_t* dst = sRing + (size_t)s * SLOT;
+        if constexpr (kBf16<T>) {                  // one 64-pixel box per input
+          mbar_arrive_expect_tx(&bars.full[s], SLOT);
 #pragma unroll
-        for (int i = 0; i < NIN; ++i)
-          for (int j = 0; j < nbox; ++j)
-            tma_load_3d(dst + (i * kNBox + j) * kBoxBytes, i == 0 ? &map0 : &map1, pb * kTilePx + j * kBoxPx, ch0,
-                        d * gm.N + n, &bars.full[s]);
+          for (int i = 0; i < NIN; ++i)
+            tma_load_3d(dst + i * (SLOT / NIN), i == 0 ? &map0 : &map1, pb * kTilePx, ch0, d * gm.N + n, &bars.full[s]);
+        } else {
+          // 32-pixel boxes of the tile that lie entirely past the row end are not issued (they only feed output
+          // pixels that are never stored, whatever the stale shared memory holds)
+          int nbox = (gm.HW - pb * kTilePx + kBoxPx - 1) / kBoxPx;
+          nbox = nbox < kNBox ? nbox : kNBox;
+          mbar_arrive_expect_tx(&bars.full[s], NIN * nbox * kBoxBytes);
+#pragma unroll
+          for (int i = 0; i < NIN; ++i)
+            for (int j = 0; j < nbox; ++j)
+              tma_load_3d(dst + (i * kNBox + j) * kBoxBytes, i == 0 ? &map0 : &map1, pb * kTilePx + j * kBoxPx, ch0,
+                          d * gm.N + n, &bars.full[s]);
+        }
       }
     }
   } else {
@@ -178,7 +208,7 @@ tc_apply_kernel(const __grid_constant__ CUtensorMap map0, const __grid_constant_
 #pragma unroll
           for (int r = 0; r < 4; ++r) {
             const int k = 8 * ks + kq + 4 * (r >> 1);
-            const float v = lds32(slot + i * kNBox * kBoxBytes + tile_off(k, prow + 8 * (r & 1))) - sShift[i][k];
+            const float v = lds_f<T>(slot + i * (SLOT / NIN) + tile_off<T>(k, prow + 8 * (r & 1))) - sShift[i][k];
             const uint32_t h = __float_as_uint(v) & kTf32Mask;
             ahi[i][ks][r] = h;
             alo[i][ks][r] = __float_as_uint(round_tf32(v - __uint_as_float(h)));
@@ -207,13 +237,16 @@ tc_apply_kernel(const __grid_constant__ CUtensorMap map0, const __grid_constant_
       wgmma_wait<0>();
       fence_operands(acc);
       const int t = t_begin + it * t_step, n = t / PB, pb = t - n * PB;
-      float* obase = args.out + (size_t)(d * gm.N + n) * gm.C * gm.HW;
+      T* obase = static_cast<T*>(args.out) + (size_t)(d * gm.N + n) * gm.C * gm.HW;
 #pragma unroll
       for (int j = 0; j < kCh / 8; ++j)
 #pragma unroll
         for (int r = 0; r < 4; ++r) {
           const int c = 8 * j + 2 * kq + (r & 1), px = pb * kTilePx + prow + 8 * (r >> 1);
-          if (ch0 + c < gm.C && px < gm.HW) obase[(size_t)(ch0 + c) * gm.HW + px] = acc[4 * j + r];
+          if (ch0 + c < gm.C && px < gm.HW) {
+            if constexpr (kBf16<T>) obase[(size_t)(ch0 + c) * gm.HW + px] = __float2bfloat16_rn(acc[4 * j + r]);
+            else obase[(size_t)(ch0 + c) * gm.HW + px] = acc[4 * j + r];
+          }
         }
     }
   }
@@ -224,17 +257,27 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 EncodeTiledFn g_encode_ap = nullptr;
 
-int make_map_ap(CUtensorMap* map, const float* base, const Geom& gm) {
+// a box is 128 bytes wide either way: 32 fp32 or 64 bf16 pixels of 64 channels (bf16 needs HW % 8 == 0: 16-byte strides)
+int make_map_ap(CUtensorMap* map, const void* base, const Geom& gm, bool bf16) {
+  const cuuint64_t es = bf16 ? 2 : 4;
   const cuuint64_t dims[3] = {(cuuint64_t)gm.HW, (cuuint64_t)gm.C, (cuuint64_t)gm.N * gm.D};
-  const cuuint64_t strides[2] = {(cuuint64_t)gm.HW * 4, (cuuint64_t)gm.C * gm.HW * 4};
-  const cuuint32_t box[3] = {kBoxPx, kCh, 1};
+  const cuuint64_t strides[2] = {(cuuint64_t)gm.HW * es, (cuuint64_t)gm.C * gm.HW * es};
+  const cuuint32_t box[3] = {bf16 ? (cuuint32_t)kTilePx : (cuuint32_t)kBoxPx, kCh, 1};
   const cuuint32_t estr[3] = {1, 1, 1};
-  return (int)g_encode_ap(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(base), dims, strides, box, estr,
-                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return (int)g_encode_ap(map, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<void*>(base),
+                          dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                          CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
 }
 
-template <int NIN> constexpr size_t ap_smem() { return ApCfg<NIN>::SMEM; }
+template <class T, int NIN> constexpr size_t ap_smem() { return ApCfg<T, NIN>::SMEM; }
+
+template <class T, int NIN>
+cudaError_t ap_attrs() {
+  cudaError_t e = cudaFuncSetAttribute(tc_apply_kernel<T, NIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ap_smem<T, NIN>());
+  // a 129 / 193 KB CTA needs the full shared-memory carve-out
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_apply_kernel<T, NIN>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  return e;
+}
 
 }  // namespace
 
@@ -244,37 +287,37 @@ int tc_apply_init() {
   cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q);
   if (e != cudaSuccess || fn == nullptr || q != cudaDriverEntryPointSuccess) return e == cudaSuccess ? -1 : (int)e;
   g_encode_ap = reinterpret_cast<EncodeTiledFn>(fn);
-  e = cudaFuncSetAttribute(tc_apply_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ap_smem<1>());
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_apply_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ap_smem<2>());
-  // a 129 / 193 KB CTA needs the full shared-memory carve-out
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_apply_kernel<1>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_apply_kernel<2>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  e = ap_attrs<float, 1>();
+  if (e == cudaSuccess) e = ap_attrs<float, 2>();
+  if (e == cudaSuccess) e = ap_attrs<__nv_bfloat16, 1>();
+  if (e == cudaSuccess) e = ap_attrs<__nv_bfloat16, 2>();
   return (int)e;
 }
 
 // y = W (x - mean): W from save_w [D][G][gs*gs], mean from save_mean [D][C]
-int tc_apply(const float* x, float* y, const Geom& gm, int nctas, const float* save_mean, const float* save_w,
+int tc_apply(const void* x, void* y, bool bf16, const Geom& gm, int nctas, const float* save_mean, const float* save_w,
              cudaStream_t st) {
   CUtensorMap mx;
   bind_context();
-  if (int rc = make_map_ap(&mx, x, gm)) return rc;
+  if (int rc = make_map_ap(&mx, x, gm, bf16)) return rc;
   ApplyArgs a{};
   a.interleave = tile_interleave();
   a.mats = save_w; a.rec_stride = gm.GS * gm.GS; a.off[0] = 0; a.off[1] = 0;
   a.shift[0] = save_mean; a.shift_stride[0] = gm.C; a.shift[1] = nullptr; a.shift_stride[1] = 0;
   a.out = y;
   dim3 grid(nctas, (gm.C + kCh - 1) / kCh, gm.D);
-  tc_apply_kernel<1><<<grid, kApThreads, ap_smem<1>(), st>>>(mx, mx, gm, a);
+  if (bf16) tc_apply_kernel<__nv_bfloat16, 1><<<grid, kApThreads, ap_smem<__nv_bfloat16, 1>(), st>>>(mx, mx, gm, a);
+  else tc_apply_kernel<float, 1><<<grid, kApThreads, ap_smem<float, 1>(), st>>>(mx, mx, gm, a);
   return 0;
 }
 
 // dx = A1 (dy - dybar) + Bm (x - mean): coef [D][G][2 gs^2 + gs] = A1 | Bm | cvec, dybar [D][SB*64]
-int tc_bwd_apply(const float* x, const float* dout, float* dx, const Geom& gm, int nctas, const float* coef,
+int tc_bwd_apply(const void* x, const void* dout, void* dx, bool bf16, const Geom& gm, int nctas, const float* coef,
                  const float* save_mean, const float* dybar, cudaStream_t st) {
   CUtensorMap mx, mg;
   bind_context();
-  if (int rc = make_map_ap(&mg, dout, gm)) return rc;
-  if (int rc = make_map_ap(&mx, x, gm)) return rc;
+  if (int rc = make_map_ap(&mg, dout, gm, bf16)) return rc;
+  if (int rc = make_map_ap(&mx, x, gm, bf16)) return rc;
   ApplyArgs a{};
   a.interleave = tile_interleave();
   a.mats = coef; a.rec_stride = coef_stride(gm.GS); a.off[0] = 0; a.off[1] = gm.GS * gm.GS;
@@ -282,7 +325,8 @@ int tc_bwd_apply(const float* x, const float* dout, float* dx, const Geom& gm, i
   a.shift[1] = save_mean; a.shift_stride[1] = gm.C;
   a.out = dx;
   dim3 grid(nctas, (gm.C + kCh - 1) / kCh, gm.D);
-  tc_apply_kernel<2><<<grid, kApThreads, ap_smem<2>(), st>>>(mg, mx, gm, a);
+  if (bf16) tc_apply_kernel<__nv_bfloat16, 2><<<grid, kApThreads, ap_smem<__nv_bfloat16, 2>(), st>>>(mg, mx, gm, a);
+  else tc_apply_kernel<float, 2><<<grid, kApThreads, ap_smem<float, 2>(), st>>>(mg, mx, gm, a);
   return 0;
 }
 

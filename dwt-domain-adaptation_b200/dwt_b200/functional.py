@@ -5,9 +5,10 @@ centred copy, a transposed copy or the covariance graph the reference's autograd
 (utils/whitening.py:44-55).
 
 Activations are float32 or bfloat16 (what torch.autocast(dtype=torch.bfloat16) hands over from a convolution): a bf16
-call whose activations are all bf16 and channels-last on a channels-last geometry runs the bf16 kernels
-(DWT_DTYPE_BF16); any other bf16 call runs the float32 kernels on upcast copies and casts the result back.  Statistics,
-parameters, their gradients and the running buffers are float32 either way, like nn.BatchNorm2d under autocast.
+call whose activations are all bf16 runs the bf16 kernels (DWT_DTYPE_BF16) when it is channels-last on a channels-last
+geometry (group sizes 1, 2, 4), or NCHW whitening on a tensor-core geometry (_bf16_tensor_core); any other bf16 call runs
+the float32 kernels on upcast copies and casts the result back.  Statistics, parameters, their gradients and the running
+buffers are float32 either way, like nn.BatchNorm2d under autocast.
 """
 from __future__ import annotations
 
@@ -30,6 +31,18 @@ def _dense(x: torch.Tensor, group_size: int):
     if not nhwc and not x.is_contiguous():
         x = x.contiguous()
     return x, n, c, hw, nhwc
+
+
+def _bf16_tensor_core(x, kind, group_size, n_domains, residual):
+    """A bf16 NCHW whitening call the tensor-core kernels take in bf16 (nv.tensor_core_bf16_supported, 16-byte-aligned
+    x; a non-contiguous x is copied into a fresh, aligned tensor by _dense)."""
+    if kind != "whiten" or residual is not None or x.dim() < 3 or x.shape[0] % n_domains:
+        return False
+    n, c = x.shape[0] // n_domains, x.shape[1]
+    hw = 1
+    for s in x.shape[2:]:
+        hw *= s
+    return nv.tensor_core_bf16_supported(n, c, hw, group_size) and (not x.is_contiguous() or x.data_ptr() % 16 == 0)
 
 
 def _check_param(name, t, numel):
@@ -57,9 +70,10 @@ class _NormFunction(torch.autograd.Function):
         gs = group_size if kind == "whiten" else 1
         x, n_all, c, hw, nhwc = _dense(x, gs)
         bf16 = x.dtype == torch.bfloat16
-        if bf16 and not (nhwc and (residual is None or residual.dtype == x.dtype)):
-            raise nv.NativeError("bfloat16 runs on the channels-last kernels with every activation in bfloat16 (norm() "
-                                 "upcasts anything else)")
+        if bf16 and not ((nhwc and (residual is None or residual.dtype == x.dtype))
+                         or (not nhwc and _bf16_tensor_core(x, kind, gs, n_domains, residual))):
+            raise nv.NativeError("bfloat16 runs on the channels-last kernels with every activation in bfloat16, or on the "
+                                 "NCHW tensor-core whitening kernels (norm() upcasts anything else)")
         layout = (nv.LAYOUT_NHWC if nhwc else 0) | (nv.DTYPE_BF16 if bf16 else 0)
         if n_all % n_domains != 0:
             raise ValueError(f"batch of {n_all} does not split into {n_domains} domains")
@@ -154,6 +168,8 @@ class _NormFunction(torch.autograd.Function):
                                       and dout2.is_contiguous(memory_format=torch.channels_last)):
             dout, dout2 = dout + dout2, None
         dout = dout.contiguous(memory_format=torch.channels_last) if (mode & nv.LAYOUT_NHWC) else dout.contiguous()
+        if (mode & nv.DTYPE_BF16) and not (mode & nv.LAYOUT_NHWC) and dout.data_ptr() % 16:
+            dout = dout.clone()                      # the forward ran the tensor-core kernels: their TMA loads need 16 bytes
         dev = nv.require_cuda(dout, bf16=True)
         dx = torch.empty_like(x)
         want_affine = gamma_c is not None and (ctx.needs_input_grad[1] or ctx.needs_input_grad[2])
@@ -321,10 +337,14 @@ def norm(x, gamma, beta, *, kind, group_size, n_domains, training_stats, eps, mo
     args = (kind, group_size, n_domains, mode, float(eps), float(momentum), bool(update_running), running, bool(relu))
     dtypes = {x.dtype} | ({residual.dtype} if residual is not None else set())
     if torch.bfloat16 in dtypes and dtypes <= set(_ACT_DTYPES):
-        bf16_kernels = dtypes == {torch.bfloat16} and _dense(x, group_size if kind == "whiten" else 1)[4]
+        gs = group_size if kind == "whiten" else 1
+        cl = x.dim() == 4 and not x.is_contiguous() and x.is_contiguous(memory_format=torch.channels_last)
+        bf16_kernels = dtypes == {torch.bfloat16} and (
+            nv.channels_last_supported(x.shape[1], gs) if cl else _bf16_tensor_core(x, kind, gs, n_domains, residual))
         if not bf16_kernels:
-            # NCHW, group sizes the bf16 kernels lack, or mixed dtypes: the float32 kernels on upcast copies, the result
-            # (and through autograd every gradient of x and the residual) back in x's dtype
+            # NCHW group sizes 1, 2, 4, geometries and alignments the bf16 kernels lack, or mixed dtypes: the float32
+            # kernels on upcast copies, the result (and through autograd every gradient of x and the residual) back in
+            # x's dtype
             y = _NormFunction.apply(x.float(), gamma, beta, None if residual is None else residual.float(), *args)
             return y.to(x.dtype)
     return _NormFunction.apply(x, gamma, beta, residual, *args)
