@@ -14,13 +14,13 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # DWT_B200_LIB: another build of the same library (development: A/B timing of a kernel variant on one box)
 LIB_PATH = os.environ.get("DWT_B200_LIB") or os.path.join(_HERE, "lib", "libdwt_b200.so")
 
-ABI_VERSION = 8
+ABI_VERSION = 9
 MAX_DOMAINS = 4
 MAX_GROUP_SIZE = 64
 MODE_TRAIN, MODE_EVAL = 0, 1
 EPI_NONE, EPI_AFFINE, EPI_RELU, EPI_RESIDUAL = 0, 1, 2, 4
 LAYOUT_NHWC = 0x100
-DTYPE_BF16 = 0x200                 # bf16 activations (channels-last gs 1/2/4, NCHW tensor-core gs 8..64; include/dwt_b200.h)
+DTYPE_BF16 = 0x200                 # bf16 activations (channels-last gs 1/2/4, tensor-core gs 8..64; include/dwt_b200.h)
 STATUS_NOT_PD, STATUS_BAD_LABEL = 1, 2
 KIND_WHITEN, KIND_BN = 0, 1
 
@@ -156,6 +156,15 @@ def tensor_core_bf16_supported(n: int, channels: int, hw: int, group_size: int) 
     (16-byte TMA rows), and at least 4096 samples per domain (n = images per domain).  The tensors also need a
     16-byte-aligned data_ptr()."""
     return (group_size in (8, 16, 32, 64) and channels % group_size == 0 and hw >= 32 and hw % 8 == 0
+            and n * hw >= 4096)
+
+
+def tensor_core_nhwc_supported(n: int, channels: int, hw: int, group_size: int) -> bool:
+    """Mirror of the C ABI's channels-last tensor-core rule (csrc/api.cu, tc_nhwc_supports): whitening at group sizes
+    8..64 dividing 64 runs on channels-last tensors when HW >= 32 and a multiple of 4 and there are at least 4096
+    samples per domain (n = images per domain), fp32 and bf16 alike.  The tensors also need a 16-byte-aligned
+    data_ptr()."""
+    return (group_size in (8, 16, 32, 64) and channels % group_size == 0 and hw >= 32 and hw % 4 == 0
             and n * hw >= 4096)
 
 

@@ -296,15 +296,21 @@ int make_plan(Plan& p, KernelKind reduce_kind, KernelKind ew_kind, const void* a
   return DWT_OK;
 }
 
+// DWT_LAYOUT_NHWC runs the channels-last kernels (group sizes 1, 2, 4, cl_supports) or, at group sizes 8..64, the
+// tensor-core family on channels-last tensors: tc_supports with HW % 4 == 0 (the NCHW rule, whose vec == 4 needs it too),
+// in fp32 and bf16 alike (the TMA rows are C channels: 16-byte strides for every group size that tiles 64), with x, y,
+// dout and dx 16-byte aligned.
+bool tc_nhwc_supports(const dwt::Geom& g) { return dwt::tc_supports(g, 4) && g.HW % 4 == 0; }
 // DWT_DTYPE_BF16 (dwt_b200.h): bf16 activations run the channels-last kernels (group sizes 1, 2, 4), where a thread's
-// four channels are 8 bytes, so that is the alignment the tensors need (16 for fp32); and, on NCHW, the tensor-core
-// family (group sizes 8..64, tc_supports), whose TMA loads need 16-byte rows (HW % 8 == 0) and a 16-byte-aligned x / dout
+// four channels are 8 bytes, so that is the alignment the tensors need (16 for fp32); and the tensor-core family
+// (group sizes 8..64, tc_supports), whose TMA loads need 16-byte rows (NCHW: HW % 8 == 0) and a 16-byte-aligned x / dout
 bool tc_bf16_supports(const dwt::Geom& g) { return dwt::tc_supports(g, 4) && g.HW % 8 == 0; }
 int check_bf16_geometry(bool bf16, bool nhwc, const dwt::Geom& g) {
-  if (!bf16 || (nhwc ? dwt::cl_supports(g.C, g.GS) : tc_bf16_supports(g))) return DWT_OK;
+  if (!bf16 || (nhwc ? dwt::cl_supports(g.C, g.GS) || tc_nhwc_supports(g) : tc_bf16_supports(g))) return DWT_OK;
   if (nhwc)
-    return fail(DWT_E_UNSUPPORTED, "channels-last bf16 activations are built for group_size 1, 2, 4 with C/4 a power of two "
-                                   "(C=%d gs=%d)", g.C, g.GS);
+    return fail(DWT_E_UNSUPPORTED, "channels-last bf16 activations are built for group_size 1, 2, 4 with C/4 a power of two, "
+                                   "and for the tensor-core kernels: group_size 8, 16, 32, 64, HW >= 32 and a multiple of 4, "
+                                   "N*HW >= 4096 per domain (C=%d HW=%d N=%d gs=%d)", g.C, g.HW, g.N, g.GS);
   return fail(DWT_E_UNSUPPORTED, "NCHW bf16 activations are built for the tensor-core kernels: group_size 8, 16, 32, 64, "
                                  "HW >= 32 and a multiple of 8, N*HW >= 4096 per domain (C=%d HW=%d N=%d gs=%d)", g.C, g.HW, g.N, g.GS);
 }
@@ -312,16 +318,29 @@ int check_tc_bf16_align(bool bf16, bool nhwc, uintptr_t bits, const char* what) 
   if (!bf16 || nhwc || bits % 16 == 0) return DWT_OK;
   return fail(DWT_E_INVALID, "%s must be 16-byte aligned (bf16 NCHW: TMA)", what);
 }
-// the tensor-core family runs every fp32 call whose geometry and alignment it takes (else the tiled kernels), and every
-// bf16 NCHW call (validated above: there is no other bf16 NCHW kernel to fall back to)
-int tc_route(bool bf16, const Plan& p, bool* tc) {
-  if (bf16) {
+// the tensor-core family runs every fp32 NCHW call whose geometry and alignment it takes (else the tiled kernels), and
+// every bf16 NCHW call and channels-last call routed to it (validated above: there is no other kernel to fall back to)
+int tc_route(bool bf16, bool nhwc, const Plan& p, bool* tc) {
+  if (bf16 || nhwc) {
     if (ensure_tc() != 0) return fail(DWT_E_LAUNCH, "tensor-core kernel set-up failed (%d)", g_tc_rc);
     *tc = true;
   } else {
     *tc = !p.small && dwt::tc_supports(p.gm, p.vec) && ensure_tc() == 0;
   }
   return DWT_OK;
+}
+int check_tc_nhwc_align(uintptr_t bits, const char* what) {
+  if (bits % 16 == 0) return DWT_OK;
+  return fail(DWT_E_INVALID, "%s must be 16-byte aligned (channels-last tensor-core kernels: TMA)", what);
+}
+int fail_nhwc_geometry(const dwt::Geom& g) {
+  return fail(DWT_E_UNSUPPORTED, "channels-last layout is built for group_size 1, 2, 4 with C/4 a power of two, and for the "
+              "tensor-core kernels: group_size 8, 16, 32, 64, HW >= 32 and a multiple of 4, N*HW >= 4096 per domain "
+              "(C=%d HW=%d N=%d gs=%d)", g.C, g.HW, g.N, g.GS);
+}
+// profile family of a tensor-core launch by layout and dtype
+inline const char* tc_fam(bool bf16, bool nhwc, const char* f32, const char* b16, const char* nhwc_f32, const char* nhwc_b16) {
+  return nhwc ? fam(bf16, nhwc_f32, nhwc_b16) : fam(bf16, f32, b16);
 }
 int check_running(bool need_running, float* const* rmean, float* const* rcov, int D) {
   if (!need_running) return DWT_OK;
@@ -374,9 +393,10 @@ int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, 
   if (int rc = make_plan(p, K_STATS, K_APPLY, x, y, nullptr, N, C, HW, GS, D)) return rc;
   if (!x || !y || !save_mean || !save_w || !ws) return fail(DWT_E_INVALID, "null pointer argument");
   if (int rc = check_bf16_geometry(bf16, nhwc, p.gm)) return rc;
-  if (nhwc && !dwt::cl_supports((int)C, GS))
-    return fail(DWT_E_UNSUPPORTED, "channels-last layout is built for group_size 1, 2, 4 with C/4 a power of two (C=%lld gs=%d)", (long long)C, GS);
-  if (nhwc) if (int rc = check_align(bf16, (uintptr_t)x | (uintptr_t)y, "channels-last tensors")) return rc;
+  const bool nhwc_tc = nhwc && tc_nhwc_supports(p.gm);
+  if (nhwc && !nhwc_tc && !dwt::cl_supports((int)C, GS)) return fail_nhwc_geometry(p.gm);
+  if (nhwc_tc) if (int rc = check_tc_nhwc_align((uintptr_t)x | (uintptr_t)y, "x and y")) return rc;
+  if (nhwc && !nhwc_tc) if (int rc = check_align(bf16, (uintptr_t)x | (uintptr_t)y, "channels-last tensors")) return rc;
   if (int rc = check_tc_bf16_align(bf16, nhwc, (uintptr_t)x, "x")) return rc;
   if (mode != DWT_MODE_TRAIN && mode != DWT_MODE_EVAL) return fail(DWT_E_INVALID, "bad mode %d", mode);
   if ((epi & DWT_EPI_RELU) && !(epi & DWT_EPI_AFFINE)) return fail(DWT_E_INVALID, "RELU epilogue needs AFFINE");
@@ -399,7 +419,7 @@ int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, 
 
   const double n_el = (double)D * (double)N * (double)C * (double)HW;
   const double E = (bf16 ? 2.0 : 4.0) * n_el, Mb = 0.25 * n_el;   // bytes of one activation tensor, of the ReLU byte map
-  if (nhwc) {
+  if (nhwc && !nhwc_tc) {
     const ClPlan cp = cl_plan(p.gm, 3, 3, 8, (epi & DWT_EPI_RESIDUAL) ? 4 : 8);
     if (mode == DWT_MODE_TRAIN) {
       {
@@ -421,12 +441,12 @@ int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, 
     return check_launch("channels-last apply kernel");
   }
   bool tc = false;
-  if (int rc = tc_route(bf16, p, &tc)) return rc;
+  if (int rc = tc_route(bf16, nhwc, p, &tc)) return rc;
   if (mode == DWT_MODE_TRAIN) {
-    Launch l(p.small ? "small_stats" : (tc ? fam(bf16, "tc_stats", "tc_stats_bf16") : "tiled_stats"), &p.gm, E, st);
+    Launch l(p.small ? "small_stats" : (tc ? tc_fam(bf16, nhwc, "tc_stats", "tc_stats_bf16", "tc_stats_nhwc", "tc_stats_nhwc_bf16") : "tiled_stats"), &p.gm, E, st);
     if (p.small) dwt::small_stats(x, p.gm, p.vec, fin, w.partial, w.counters, st);
     else if (tc) {
-      if (int cr = dwt::tc_stats(x, bf16, p.gm, tc_chunks(p.gm), w.shift, w.partial, st))
+      if (int cr = dwt::tc_stats(x, bf16, nhwc, p.gm, tc_chunks(p.gm), w.shift, w.partial, st))
         return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d) x=%p N=%d C=%d HW=%d D=%d", cr, (const void*)x, p.gm.N, p.gm.C, p.gm.HW, p.gm.D);
     } else dwt::tiled_stats(x, p.gm, p.vec, fin, w.partial, w.counters, st);
   } else {
@@ -443,11 +463,11 @@ int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, 
   }
   if (int rc = check_launch("whitening statistics kernel")) return rc;
   {
-    Launch l(p.small ? "small_apply" : (tc ? fam(bf16, "tc_apply", "tc_apply_bf16") : "tiled_apply"), &p.gm,
+    Launch l(p.small ? "small_apply" : (tc ? tc_fam(bf16, nhwc, "tc_apply", "tc_apply_bf16", "tc_apply_nhwc", "tc_apply_nhwc_bf16") : "tiled_apply"), &p.gm,
              ((epi & DWT_EPI_RESIDUAL) ? 3 : 2) * E, st);
     if (p.small) dwt::small_apply(x, y, p.gm_ew, p.vec, p.chunks_ew, epi, save_mean, save_w, gamma, beta, residual, st);
     else if (tc) {
-      if (int cr = dwt::tc_apply(x, y, bf16, p.gm, tc_apply_ctas(p.gm, 1, 64), save_mean, save_w, st))
+      if (int cr = dwt::tc_apply(x, y, bf16, nhwc, p.gm, tc_apply_ctas(p.gm, 1, 64), save_mean, save_w, st))
         return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d)", cr);
     } else dwt::tiled_apply(x, y, p.gm_ew, p.vec, p.chunks_ew, save_mean, save_w, st);
   }
@@ -464,12 +484,13 @@ int whiten_like_bwd(const float* x, const float* dout, const float* dout2, float
   if (int rc = make_plan(p, K_BWD_REDUCE, K_BWD_APPLY, x, dout, dx, N, C, HW, GS, D)) return rc;
   if (!x || !dout || !dx || !save_mean || !save_w || !ws) return fail(DWT_E_INVALID, "null pointer argument");
   if (int rc = check_bf16_geometry(bf16, nhwc, p.gm)) return rc;
-  if (dout2 && (!nhwc || (uintptr_t)dout2 % (bf16 ? 8 : 16) != 0))
-    return fail(nhwc ? DWT_E_INVALID : DWT_E_UNSUPPORTED, "a second gradient addend (dout2) is built for the channels-last "
-                "kernels (16-byte aligned tensor, 8 for bf16); add it to dout otherwise");
-  if (nhwc && !dwt::cl_supports((int)C, GS))
-    return fail(DWT_E_UNSUPPORTED, "channels-last layout is built for group_size 1, 2, 4 with C/4 a power of two (C=%lld gs=%d)", (long long)C, GS);
-  if (nhwc) if (int rc = check_align(bf16, (uintptr_t)x | (uintptr_t)dout | (uintptr_t)dx, "channels-last tensors")) return rc;
+  const bool nhwc_tc = nhwc && tc_nhwc_supports(p.gm);
+  if (dout2 && (!nhwc || nhwc_tc || (uintptr_t)dout2 % (bf16 ? 8 : 16) != 0))
+    return fail(nhwc && !nhwc_tc ? DWT_E_INVALID : DWT_E_UNSUPPORTED, "a second gradient addend (dout2) is built for the "
+                "channels-last kernels of group sizes 1, 2, 4 (16-byte aligned tensor, 8 for bf16); add it to dout otherwise");
+  if (nhwc && !nhwc_tc && !dwt::cl_supports((int)C, GS)) return fail_nhwc_geometry(p.gm);
+  if (nhwc_tc) if (int rc = check_tc_nhwc_align((uintptr_t)x | (uintptr_t)dout | (uintptr_t)dx, "x, dout and dx")) return rc;
+  if (nhwc && !nhwc_tc) if (int rc = check_align(bf16, (uintptr_t)x | (uintptr_t)dout | (uintptr_t)dx, "channels-last tensors")) return rc;
   if (int rc = check_tc_bf16_align(bf16, nhwc, (uintptr_t)x | (uintptr_t)dout, "x and dout")) return rc;
   if (mode != DWT_MODE_TRAIN && mode != DWT_MODE_EVAL) return fail(DWT_E_INVALID, "bad mode %d", mode);
   if ((epi & DWT_EPI_RELU) && !(epi & DWT_EPI_AFFINE)) return fail(DWT_E_INVALID, "RELU epilogue needs AFFINE");
@@ -498,7 +519,7 @@ int whiten_like_bwd(const float* x, const float* dout, const float* dout2, float
   const bool need_reduce = (mode == DWT_MODE_TRAIN) || (fin.dgamma != nullptr) || masked;
   const double n_el = (double)D * (double)N * (double)C * (double)HW;
   const double E = (bf16 ? 2.0 : 4.0) * n_el, Mb = 0.25 * n_el;
-  if (nhwc) {
+  if (nhwc && !nhwc_tc) {
     const ClPlan cp = cl_plan(p.gm, 2, 2, 4, 4);
     if (need_reduce) {
       {
@@ -521,12 +542,12 @@ int whiten_like_bwd(const float* x, const float* dout, const float* dout2, float
     return check_launch("channels-last backward apply kernel");
   }
   bool tc = false;
-  if (int rc = tc_route(bf16, p, &tc)) return rc;
+  if (int rc = tc_route(bf16, nhwc, p, &tc)) return rc;
   if (need_reduce) {
-    Launch l(p.small ? "small_bwd_reduce" : (tc ? fam(bf16, "tc_bwd_reduce", "tc_bwd_reduce_bf16") : "tiled_bwd_reduce"), &p.gm, 2 * E, st);
+    Launch l(p.small ? "small_bwd_reduce" : (tc ? tc_fam(bf16, nhwc, "tc_bwd_reduce", "tc_bwd_reduce_bf16", "tc_bwd_reduce_nhwc", "tc_bwd_reduce_nhwc_bf16") : "tiled_bwd_reduce"), &p.gm, 2 * E, st);
     if (p.small) dwt::small_bwd_reduce(x, dout, p.gm, p.vec, fin, beta, w.partial, w.counters, st);
     else if (tc) {
-      if (int cr = dwt::tc_bwd_reduce(x, dout, bf16, p.gm, tc_chunks(p.gm), save_mean, w.partial, st))
+      if (int cr = dwt::tc_bwd_reduce(x, dout, bf16, nhwc, p.gm, tc_chunks(p.gm), save_mean, w.partial, st))
         return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d) x=%p dout=%p N=%d C=%d HW=%d D=%d", cr, (const void*)x, (const void*)dout, p.gm.N, p.gm.C, p.gm.HW, p.gm.D);
     } else dwt::tiled_bwd_reduce(x, dout, p.gm, p.vec, fin, w.partial, w.counters, st);
   } else {
@@ -543,10 +564,10 @@ int whiten_like_bwd(const float* x, const float* dout, const float* dout2, float
   }
   if (int rc = check_launch("whitening backward reduction kernel")) return rc;
   {
-    Launch l(p.small ? "small_bwd_apply" : (tc ? fam(bf16, "tc_bwd_apply", "tc_bwd_apply_bf16") : "tiled_bwd_apply"), &p.gm, 3 * E, st);
+    Launch l(p.small ? "small_bwd_apply" : (tc ? tc_fam(bf16, nhwc, "tc_bwd_apply", "tc_bwd_apply_bf16", "tc_bwd_apply_nhwc", "tc_bwd_apply_nhwc_bf16") : "tiled_bwd_apply"), &p.gm, 3 * E, st);
     if (p.small) dwt::small_bwd_apply(x, dout, dx, p.gm_ew, p.vec, p.chunks_ew, epi, w.coef, save_mean, save_w, gamma, beta, st);
     else if (tc) {
-      if (int cr = dwt::tc_bwd_apply(x, dout, dx, bf16, p.gm, tc_apply_ctas(p.gm, 1, 64), w.coef, save_mean, w.shift, st))
+      if (int cr = dwt::tc_bwd_apply(x, dout, dx, bf16, nhwc, p.gm, tc_apply_ctas(p.gm, 1, 64), w.coef, save_mean, w.shift, st))
         return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d)", cr);
     } else dwt::tiled_bwd_apply(x, dout, dx, p.gm_ew, p.vec, p.chunks_ew, w.coef, st);
   }

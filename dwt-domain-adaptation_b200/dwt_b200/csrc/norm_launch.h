@@ -46,10 +46,11 @@ void tiled_bwd_apply(const float* x, const float* dout, float* dx, const Geom& g
 int tc_init();      // driver entry point for cuTensorMapEncodeTiled + shared-memory opt-in; 0 on success
 bool tc_supports(const Geom& gm, int vec);
 int tc_superblocks(const Geom& gm);
-// Activation pointers are void: fp32, or bf16 when `bf16` (HW % 8 == 0, 16-byte aligned; the same schedule, loads
-// widened to fp32, stores rounded to nearest-even).  Partials, shifts, statistics and coefficients are fp32 either way.
-int tc_stats(const void* x, bool bf16, const Geom& gm, int nchunks, float* shift, float* partial, cudaStream_t st);
-int tc_bwd_reduce(const void* x, const void* dout, bool bf16, const Geom& gm, int nchunks, const float* save_mean,
+// Activation pointers are void: fp32, or bf16 when `bf16` (NCHW: HW % 8 == 0; 16-byte aligned; the same schedule, loads
+// widened to fp32, stores rounded to nearest-even).  `nhwc`: dense channels-last tensors (HW % 4 == 0, 16-byte aligned;
+// the same schedule and arithmetic as NCHW).  Partials, shifts, statistics and coefficients are fp32 either way.
+int tc_stats(const void* x, bool bf16, bool nhwc, const Geom& gm, int nchunks, float* shift, float* partial, cudaStream_t st);
+int tc_bwd_reduce(const void* x, const void* dout, bool bf16, bool nhwc, const Geom& gm, int nchunks, const float* save_mean,
                   float* partial, cudaStream_t st);
 
 // dense per-group algebra behind the contraction (norm_dense.cu)
@@ -60,9 +61,9 @@ void dense_bwd_coef(const float* rgram, const Geom& gm, const BwdFin& fin, float
 
 // TMA + wgmma apply path (norm_tc_apply.cu): split-TF32 GEMM of the block-diagonal group matrices
 int tc_apply_init();
-int tc_apply(const void* x, void* y, bool bf16, const Geom& gm, int nctas, const float* save_mean, const float* save_w,
+int tc_apply(const void* x, void* y, bool bf16, bool nhwc, const Geom& gm, int nctas, const float* save_mean, const float* save_w,
              cudaStream_t st);
-int tc_bwd_apply(const void* x, const void* dout, void* dx, bool bf16, const Geom& gm, int nctas, const float* coef,
+int tc_bwd_apply(const void* x, const void* dout, void* dx, bool bf16, bool nhwc, const Geom& gm, int nctas, const float* coef,
                  const float* save_mean, const float* dybar, cudaStream_t st);
 
 // channels-last (NHWC) register-resident path, GS in {1,2,4}, C/4 a power of two  (norm_cl.cu)

@@ -37,6 +37,15 @@
 // sequence from the staging tiles.  Grid, tile ranges, warpgroup alternation and epilogue are those of the fp32 kernels,
 // so every partial is bit for bit the fp32 kernel's on x.float().
 //
+// channels-last activations (DWT_LAYOUT_NHWC): both kernels are also templated on the layout.  The tensor map is 3-D
+// {C, HW, N*D} with channels innermost; a tile is the same [64 ch x 32 px] block of one image, landed as rows of pixels:
+// fp32 two boxes of 32 ch x 32 px (128-byte rows, SWIZZLE_128B), bf16 one box of 64 ch x 32 px (likewise).  TMA zero
+// fill past C and past HW keeps the NCHW tile schedule, partial tiles and partial super-blocks included.  wgmma wants K
+// (the pixels) contiguous, so the transform reads each thread's (channel, 4-pixel chunk) from the landed [px][ch] tile
+// and writes exactly what the NCHW transform writes, at the same swizzled positions, into the per-warpgroup fp32
+// staging tiles of the bf16 kernels; the rest is the NCHW kernel, so every partial is bit for bit the NCHW kernel's on
+// x.contiguous().  fp32 rings are shallower (Gram 8, contraction 4 stages) to keep two CTAs per SM with the staging.
+//
 // Reference: utils/whitening.py:46-47 of the reference project and its autograd transpose.
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -64,10 +73,16 @@ constexpr int kGramStages = 10;                         // 80 KB ring + 2 x 8 KB
 // Activation storage T: float, or __nv_bfloat16 (DWT_DTYPE_BF16); a landed box is kTileCh x kTilePx values of T
 template <class T> constexpr bool kBf16 = !std::is_same<T, float>::value;
 template <class T> constexpr int kBoxBytes = kTileCh * kTilePx * (int)sizeof(T);
+// Layout NHWC: the transform writes to staging tiles (the bf16 kernels always do).  fp32 NHWC: the staging tiles cost
+// 32 KB per CTA, so the rings are shallower to keep two CTAs per SM (Gram 64 + 32 KB, contraction 64 + 32 KB).
+template <class T, bool NHWC> constexpr bool kStaged = kBf16<T> || NHWC;
+template <class T, bool NHWC> constexpr int kGramStagesOf = (NHWC && !kBf16<T>) ? 8 : kGramStages;
+template <class T, bool NHWC> constexpr int kStagesBwdOf = (NHWC && !kBf16<T>) ? 4 : kStagesBwd;
 constexpr int kMaxStages = kGramStages > kStagesBwd ? kGramStages : kStagesBwd;
-// Consumer warpgroup w takes tiles w, w + 2, ...; both ring lengths are even, so every stage (and all phases of its
+// Consumer warpgroup w takes tiles w, w + 2, ...; all ring lengths are even, so every stage (and all phases of its
 // barriers) belongs to one warpgroup, and an mbarrier parity wait never meets a barrier two phases ahead.
 static_assert(kGramStages % kConsumers == 0 && kStagesBwd % kConsumers == 0, "stage ownership");
+static_assert(kGramStagesOf<float, true> % kConsumers == 0 && kStagesBwdOf<float, true> % kConsumers == 0, "stage ownership");
 
 struct TcBarriers {
   uint64_t full[kMaxStages];       // TMA landed the stage                  (1 arrival + tx bytes)
@@ -94,11 +109,31 @@ __device__ __forceinline__ void sts128(uint32_t addr, float a, float b, float c,
   asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
 }
 
+template <class T>
+__device__ __forceinline__ float lds_nhwc(uint32_t addr) {
+  if constexpr (kBf16<T>) {
+    unsigned short u;
+    asm volatile("ld.shared.u16 %0, [%1];" : "=h"(u) : "r"(addr));
+    return __uint_as_float((uint32_t)u << 16);
+  } else {
+    float v;
+    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr));
+    return v;
+  }
+}
 // Pixels 4j .. 4j+3 of tile row `row` as fp32.  fp32: the 16-byte chunk q = 8 row + (j ^ (row & 7)) of the SWIZZLE_128B
 // tile.  bf16: 8 bytes at row * 64 + 8 j of the unswizzled box, widened (bf16 -> fp32 is exact: the high half of the word).
-template <class T>
+// NHWC: channel `row` of pixels 4j .. 4j+3 of the landed [px][ch] tile, one load per pixel.
+template <class T, bool NHWC>
 __device__ __forceinline__ float4 ld_px4(uint32_t tile, int q, int row, int j) {
-  if constexpr (kBf16<T>) {
+  if constexpr (NHWC) {
+    // landed [px][ch] tile, 128-byte pixel rows, SWIZZLE_128B (fp32: two boxes of 32 channels, 4 KB apart; bf16: one of
+    // 64).  Pixel 4j + k is row 4j + k; its 16-byte chunk holding channel `row` is c4 ^ (4 (j & 1) + k) = a ^ k.
+    const int c4 = kBf16<T> ? row >> 3 : (row & 31) >> 2, a = c4 ^ ((j & 1) << 2);
+    const uint32_t base = tile + 512u * j + (kBf16<T> ? 2u * (row & 7) : 4096u * (row >> 5) + 4u * (row & 3));
+    return make_float4(lds_nhwc<T>(base + (a << 4)), lds_nhwc<T>(base + 128u + ((a ^ 1) << 4)),
+                       lds_nhwc<T>(base + 256u + ((a ^ 2) << 4)), lds_nhwc<T>(base + 384u + ((a ^ 3) << 4)));
+  } else if constexpr (kBf16<T>) {
     uint32_t a, b;
     asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(a), "=r"(b) : "r"(tile + 64u * row + 8u * j));
     return make_float4(__uint_as_float(a << 16), __uint_as_float(a & 0xFFFF0000u), __uint_as_float(b << 16),
@@ -114,18 +149,22 @@ template <class T> __device__ __forceinline__ float ldg_f(const T* p) {
 
 // Pilot shift of channel c: the mean of <= 32 mid-image pixels of image 0 of domain d, moved to the mean of 32 samples
 // spread over the domain where that lies more than 20 of their standard deviations away (pilot_shift in dwt_common.cuh).
-template <class T>
+// NHWC reads the same samples: pixel p of image n at (n * HW + p) * C from the channel.
+template <class T, bool NHWC>
 __device__ __forceinline__ float pilot_shift(const T* __restrict__ x, const Geom& gm, int d, int c) {
   if (c >= gm.C) return 0.f;
   const int np = gm.HW < 32 ? gm.HW : 32, p0 = ((gm.HW - np) / 2) & ~3;
-  const T* xc = x + ((size_t)d * gm.N * gm.C + c) * gm.HW;
+  const T* xc = NHWC ? x + (size_t)d * gm.N * gm.C * gm.HW + c : x + ((size_t)d * gm.N * gm.C + c) * gm.HW;
   float a = 0.f;
-  for (int k = 0; k < np; ++k) a += ldg_f(xc + p0 + k);
+  if constexpr (NHWC) for (int k = 0; k < np; ++k) a += ldg_f(xc + (size_t)(p0 + k) * gm.C);
+  else for (int k = 0; k < np; ++k) a += ldg_f(xc + p0 + k);
   const float K = a / (float)np;
   if ((long long)gm.N * gm.HW <= kPilotSpread) return K;
   float s1 = 0.f, s2 = 0.f;
   for (int k = 0; k < kPilotSpread; ++k) {
-    const float e = ldg_f(xc + pilot_spread_offset(k, gm.N, gm.HW, (size_t)gm.C * gm.HW)) - K;
+    const size_t o = NHWC ? pilot_spread_offset(k, gm.N, gm.HW, (size_t)gm.HW) * gm.C
+                          : pilot_spread_offset(k, gm.N, gm.HW, (size_t)gm.C * gm.HW);
+    const float e = ldg_f(xc + o) - K;
     s1 += e;
     s2 = fmaf(e, e, s2);
   }
@@ -136,18 +175,19 @@ __device__ __forceinline__ float pilot_shift(const T* __restrict__ x, const Geom
 // (fp32: dst == tile, in place):
 //   v <- RN_tf32(v - shift[row]) inside the tensor, 0 outside; returns per-thread row sums of (v - shift).
 // Chunk q = t + 128*i (16-byte units): row = q >> 3, physical chunk jp = q & 7, logical chunk = jp ^ (row & 7).
-template <class T>
+template <class T, bool NHWC>
 __device__ __forceinline__ void transform_tile(uint32_t tile, uint32_t dst, int t, const float (&shift)[kPer], int px0, int HW,
                                                int ch0, int C, float (&rowsum)[kPer]) {
   float4 v[kPer];
 #pragma unroll
   for (int i = 0; i < kPer; ++i) {
     const int q = t + 128 * i, row = q >> 3;
-    v[i] = ld_px4<T>(tile, q, row, (q & 7) ^ (row & 7));
+    if constexpr (!NHWC) v[i] = ld_px4<T, NHWC>(tile, q, row, (q & 7) ^ (row & 7));
   }
 #pragma unroll
   for (int i = 0; i < kPer; ++i) {
     const int q = t + 128 * i, row = q >> 3, jp = q & 7, j = jp ^ (row & 7);
+    if constexpr (NHWC) v[i] = ld_px4<T, NHWC>(tile, q, row, j);        // four scalar loads: one chunk at a time
     const int px = px0 + 4 * j;
     const bool rowok = (ch0 + row) < C;
     float e[4] = {v[i].x, v[i].y, v[i].z, v[i].w};
@@ -166,7 +206,7 @@ __device__ __forceinline__ void transform_tile(uint32_t tile, uint32_t dst, int 
 // the tile itself, in place), lo = s - hi (exact) to the warpgroup's lo tile at the same swizzled position; returns
 // per-thread row sums of s.  hi is written explicitly so that HH and LH see the same hi whatever rounding the tensor core
 // applies to fp32 words.  Two chunks at a time: the accumulators leave few registers at two CTAs per SM.
-template <class T>
+template <class T, bool NHWC>
 __device__ __forceinline__ void gram_transform(uint32_t tile, uint32_t hi, uint32_t lo, int t, const float (&shift)[kPer], int px0,
                                                int HW, int ch0, int C, float (&rowsum)[kPer]) {
 #pragma unroll
@@ -175,11 +215,12 @@ __device__ __forceinline__ void gram_transform(uint32_t tile, uint32_t hi, uint3
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
       const int q = t + 128 * (h + i), row = q >> 3;
-      v[i] = ld_px4<T>(tile, q, row, (q & 7) ^ (row & 7));
+      if constexpr (!NHWC) v[i] = ld_px4<T, NHWC>(tile, q, row, (q & 7) ^ (row & 7));
     }
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
       const int q = t + 128 * (h + i), row = q >> 3, j = (q & 7) ^ (row & 7);
+      if constexpr (NHWC) v[i] = ld_px4<T, NHWC>(tile, q, row, j);
       const int px = px0 + 4 * j;
       const bool rowok = (ch0 + row) < C;
       float e[4] = {v[i].x, v[i].y, v[i].z, v[i].w}, l[4];
@@ -223,6 +264,18 @@ __device__ __forceinline__ void add_fragment(float* s, int pitch, const float (&
   }
 }
 
+// TMA of one input's tile (channels ch0.., pixels px0.. of image img) into dst: NCHW one box {32 px, 64 ch}; NHWC fp32 two
+// boxes {32 ch, 32 px} (channel halves, 4 KB apart), NHWC bf16 one box {64 ch, 32 px}.  Always kBoxBytes<T> bytes.
+template <class T, bool NHWC>
+__device__ __forceinline__ void tma_tile(uint8_t* dst, const CUtensorMap* map, int ch0, int px0, int img, uint64_t* bar) {
+  if constexpr (!NHWC) {
+    tma_load_3d(dst, map, px0, ch0, img, bar);
+  } else {
+    tma_load_3d(dst, map, ch0, px0, img, bar);
+    if constexpr (!kBf16<T>) tma_load_3d(dst + 4096, map, ch0 + 32, px0, img, bar);
+  }
+}
+
 __device__ __forceinline__ void init_ring(TcBarriers& bars, int stages) {
   for (int s = 0; s < stages; ++s) { mbar_init(&bars.full[s], 1); mbar_init(&bars.empty[s], 4); }
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -231,11 +284,12 @@ __device__ __forceinline__ void init_ring(TcBarriers& bars, int stages) {
 // ------------------------------------------------------------------------------------------
 // backward contraction: R = sum dy xc^T and the row sums of dy
 // ------------------------------------------------------------------------------------------
-template <class T>
+template <class T, bool NHWC>
 __global__ void __launch_bounds__(kTcThreads, 2)
 tc_contract_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_g, const Geom gm,
                    const float* __restrict__ save_mean, float* __restrict__ partial) {
-  constexpr int STAGES = kStagesBwd, BOX = kBoxBytes<T>;
+  constexpr int STAGES = kStagesBwdOf<T, NHWC>, BOX = kBoxBytes<T>;
+  constexpr bool STAGED = kStaged<T, NHWC>;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   __shared__ TcBarriers bars;
@@ -264,8 +318,8 @@ tc_contract_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
         const int t = tr.begin + it, n = t / tr.PB, pb = t - n * tr.PB;
         uint8_t* dst = smem + (size_t)s * 2 * BOX;
         mbar_arrive_expect_tx(&bars.full[s], 2 * BOX);
-        tma_load_3d(dst, &map_x, pb * kTilePx, ch0, d * gm.N + n, &bars.full[s]);
-        tma_load_3d(dst + BOX, &map_g, pb * kTilePx, ch0, d * gm.N + n, &bars.full[s]);
+        tma_tile<T, NHWC>(dst, &map_x, ch0, pb * kTilePx, d * gm.N + n, &bars.full[s]);
+        tma_tile<T, NHWC>(dst + BOX, &map_g, ch0, pb * kTilePx, d * gm.N + n, &bars.full[s]);
       }
     }
   } else {
@@ -274,17 +328,17 @@ tc_contract_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
     float shift[kPer], zero[kPer], dummy[kPer];
 #pragma unroll
     for (int i = 0; i < kPer; ++i) { shift[i] = sShift[(t + 128 * i) >> 3]; zero[i] = 0.f; dummy[i] = 0.f; }
-    // bf16: the warpgroup's fp32 staging tiles (xc, dy) behind the ring; fp32: the landed tiles themselves
+    // bf16 / NHWC: the warpgroup's fp32 staging tiles (xc, dy) behind the ring; fp32 NCHW: the landed tiles themselves
     const uint32_t stage_f32 = smem_u32(smem + (size_t)STAGES * 2 * BOX + (size_t)wg * 2 * kTileBytes);
     for (int it = wg; it < ntiles; it += kConsumers) {
       const int s = it % STAGES;
       mbar_wait(&bars.full[s], (it / STAGES) & 1);
       const int tl = tr.begin + it, n = tl / tr.PB, pb = tl - n * tr.PB;
       const uint32_t tile = smem_u32(smem + (size_t)s * 2 * BOX);
-      const uint32_t xs = kBf16<T> ? stage_f32 : tile, ys = kBf16<T> ? stage_f32 + kTileBytes : tile + kTileBytes;
-      transform_tile<T>(tile, xs, t, shift, pb * kTilePx, gm.HW, ch0, gm.C, dummy);               // xc
-      transform_tile<T>(tile + BOX, ys, t, zero, pb * kTilePx, gm.HW, ch0, gm.C, rowsum);         // dy, sums
-      if constexpr (kBf16<T>) {                    // the stage is read: it can be refilled while the MMAs run
+      const uint32_t xs = STAGED ? stage_f32 : tile, ys = STAGED ? stage_f32 + kTileBytes : tile + kTileBytes;
+      transform_tile<T, NHWC>(tile, xs, t, shift, pb * kTilePx, gm.HW, ch0, gm.C, dummy);               // xc
+      transform_tile<T, NHWC>(tile + BOX, ys, t, zero, pb * kTilePx, gm.HW, ch0, gm.C, rowsum);         // dy, sums
+      if constexpr (STAGED) {                      // the stage is read: it can be refilled while the MMAs run
         __syncwarp();
         if (lane == 0) mbar_arrive(&bars.empty[s]);
       }
@@ -296,9 +350,9 @@ tc_contract_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
 #pragma unroll
       for (int k = 0; k < kTilePx / 8; ++k) wgmma_m64n64k8_ss(acc, adesc + 2 * k, xdesc + 2 * k);
       wgmma_commit();
-      wgmma_wait<0>();                             // bf16: the staging tiles are rewritten by the next transform
+      wgmma_wait<0>();                             // staged: the staging tiles are rewritten by the next transform
       fence_operands(acc);
-      if constexpr (!kBf16<T>) {
+      if constexpr (!STAGED) {
         __syncwarp();
         if (lane == 0) mbar_arrive(&bars.empty[s]);
       }
@@ -322,11 +376,12 @@ tc_contract_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
 // ------------------------------------------------------------------------------------------
 // split-precision Gram kernel (forward statistics): G = HH + LH + LH^T, see the file header
 // ------------------------------------------------------------------------------------------
-template <class T>
+template <class T, bool NHWC>
 __global__ void __launch_bounds__(kTcThreads, 2)
 tc_gram_kernel(const __grid_constant__ CUtensorMap map_x, const T* __restrict__ x, const Geom gm,
                float* __restrict__ shift_out, float* __restrict__ partial) {
-  constexpr int STAGES = kGramStages, BOX = kBoxBytes<T>;
+  constexpr int STAGES = kGramStagesOf<T, NHWC>, BOX = kBoxBytes<T>;
+  constexpr bool STAGED = kStaged<T, NHWC>;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   __shared__ TcBarriers bars;
@@ -338,7 +393,7 @@ tc_gram_kernel(const __grid_constant__ CUtensorMap map_x, const T* __restrict__ 
 
   if (tid == 0) init_ring(bars, STAGES);
   if (tid < kTileCh) {
-    const float sh = pilot_shift(x, gm, d, ch0 + tid);
+    const float sh = pilot_shift<T, NHWC>(x, gm, d, ch0 + tid);
     sShift[tid] = sh;
     if (blockIdx.x == 0) shift_out[((size_t)d * gridDim.y + sb) * kTileCh + tid] = sh;
   }
@@ -358,16 +413,16 @@ tc_gram_kernel(const __grid_constant__ CUtensorMap map_x, const T* __restrict__ 
         const int s = it % STAGES;
         mbar_wait_relaxed(&bars.empty[s], ((it / STAGES) & 1) ^ 1);
         mbar_arrive_expect_tx(&bars.full[s], BOX);
-        tma_load_3d(smem + (size_t)s * BOX, &map_x, pb * kTilePx, ch0, d * gm.N + n, &bars.full[s]);
+        tma_tile<T, NHWC>(smem + (size_t)s * BOX, &map_x, ch0, pb * kTilePx, d * gm.N + n, &bars.full[s]);
         if (++pb == tr.PB) { pb = 0; ++n; }
       }
     }
   } else {
     // ===== consumer warpgroups: HH[64 x 64] += hi * hi^T,  LH[64 x 64] += lo * hi^T =====
     const int wg = warp >> 2, t = tid & 127;
-    // per warpgroup behind the ring: the lo tile (fp32), or the hi staging tile and the lo tile (bf16)
-    const uint32_t wgbuf = smem_u32(smem + (size_t)STAGES * BOX + (size_t)wg * (kBf16<T> ? 2 : 1) * kTileBytes);
-    const uint32_t lo = kBf16<T> ? wgbuf + kTileBytes : wgbuf;
+    // per warpgroup behind the ring: the lo tile (fp32 NCHW), or the hi staging tile and the lo tile (bf16 / NHWC)
+    const uint32_t wgbuf = smem_u32(smem + (size_t)STAGES * BOX + (size_t)wg * (STAGED ? 2 : 1) * kTileBytes);
+    const uint32_t lo = STAGED ? wgbuf + kTileBytes : wgbuf;
     const uint64_t ldesc = make_kmajor_sw128_desc(lo);
     float shift[kPer];
 #pragma unroll
@@ -377,9 +432,9 @@ tc_gram_kernel(const __grid_constant__ CUtensorMap map_x, const T* __restrict__ 
       mbar_wait(&bars.full[s], (it / STAGES) & 1);
       const int tl = tr.begin + it, n = tl / tr.PB, pb = tl - n * tr.PB;
       const uint32_t tile = smem_u32(smem + (size_t)s * BOX);
-      const uint32_t hi = kBf16<T> ? wgbuf : tile;
-      gram_transform<T>(tile, hi, lo, t, shift, pb * kTilePx, gm.HW, ch0, gm.C, rowsum);
-      if constexpr (kBf16<T>) {                    // the stage is read: it can be refilled while the MMAs run
+      const uint32_t hi = STAGED ? wgbuf : tile;
+      gram_transform<T, NHWC>(tile, hi, lo, t, shift, pb * kTilePx, gm.HW, ch0, gm.C, rowsum);
+      if constexpr (STAGED) {                    // the stage is read: it can be refilled while the MMAs run
         __syncwarp();
         if (lane == 0) mbar_arrive(&bars.empty[s]);
       }
@@ -395,10 +450,10 @@ tc_gram_kernel(const __grid_constant__ CUtensorMap map_x, const T* __restrict__ 
         wgmma_m64n64k8_ss(lh, ldesc + 2 * k, bdesc + 2 * k);
       }
       wgmma_commit();
-      wgmma_wait<0>();                             // the lo (bf16: and hi) tile is rewritten by this warpgroup's next transform
+      wgmma_wait<0>();                             // the lo (staged: and hi) tile is rewritten by this warpgroup's next transform
       fence_operands(hh);
       fence_operands(lh);
-      if constexpr (!kBf16<T>) {
+      if constexpr (!STAGED) {
         __syncwarp();
         if (lane == 0) mbar_arrive(&bars.empty[s]);
       }
@@ -437,35 +492,59 @@ EncodeTiledFn g_encode = nullptr;
 
 // fp32: 32 px x 64 ch boxes of 128-byte rows, SWIZZLE_128B (the wgmma operand layout).  bf16: 64-byte rows, no swizzle
 // (read by ld.shared only); TMA then needs HW % 8 == 0 for 16-byte strides.
-int make_map(CUtensorMap* map, const void* base, const Geom& gm, bool bf16) {
+// nhwc: dims {C, HW, N*D}, boxes of 32 (fp32) or 64 (bf16) channels x 32 px, 128-byte rows, SWIZZLE_128B; the strides are
+// C and HW * C elements (16-byte multiples: C % 8 == 0 for every group size the tensor-core path takes).
+int make_map(CUtensorMap* map, const void* base, const Geom& gm, bool bf16, bool nhwc) {
   const cuuint64_t es = bf16 ? 2 : 4;
+  const cuuint32_t estr[3] = {1, 1, 1};
+  const CUtensorMapDataType dt = bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+  if (nhwc) {
+    const cuuint64_t dims[3] = {(cuuint64_t)gm.C, (cuuint64_t)gm.HW, (cuuint64_t)gm.N * gm.D};
+    const cuuint64_t strides[2] = {(cuuint64_t)gm.C * es, (cuuint64_t)gm.HW * gm.C * es};
+    const cuuint32_t box[3] = {bf16 ? 64u : 32u, kTilePx, 1};
+    return (int)g_encode(map, dt, 3, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  }
   const cuuint64_t dims[3] = {(cuuint64_t)gm.HW, (cuuint64_t)gm.C, (cuuint64_t)gm.N * gm.D};
   const cuuint64_t strides[2] = {(cuuint64_t)gm.HW * es, (cuuint64_t)gm.C * gm.HW * es};
   const cuuint32_t box[3] = {kTilePx, kTileCh, 1};
-  const cuuint32_t estr[3] = {1, 1, 1};
-  return (int)g_encode(map, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<void*>(base),
+  return (int)g_encode(map, dt, 3, const_cast<void*>(base),
                        dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                        bf16 ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
 }
 
-// fp32: the ring (+ the lo tiles); bf16: the ring of half-size boxes + fp32 staging tiles (two per warpgroup)
-template <class T>
+// fp32 NCHW: the ring (+ the lo tiles); bf16 / NHWC: the ring + fp32 staging tiles (two per warpgroup)
+template <class T, bool NHWC>
 size_t tc_smem_bytes(bool two) {
-  const size_t wgbuf = (size_t)kConsumers * (kBf16<T> ? 2 : 1) * kTileBytes;
-  return two ? (size_t)kStagesBwd * 2 * kBoxBytes<T> + (kBf16<T> ? wgbuf : 0) + 1024
-             : (size_t)kGramStages * kBoxBytes<T> + wgbuf + 1024;
+  constexpr bool staged = kStaged<T, NHWC>;
+  const size_t wgbuf = (size_t)kConsumers * (staged ? 2 : 1) * kTileBytes;
+  return two ? (size_t)kStagesBwdOf<T, NHWC> * 2 * kBoxBytes<T> + (staged ? wgbuf : 0) + 1024
+             : (size_t)kGramStagesOf<T, NHWC> * kBoxBytes<T> + wgbuf + 1024;
 }
 
-template <class T>
+template <class T, bool NHWC>
 cudaError_t tc_kernel_attrs() {
-  cudaError_t e = cudaFuncSetAttribute(tc_gram_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes<T>(false));
+  cudaError_t e = cudaFuncSetAttribute(tc_gram_kernel<T, NHWC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes<T, NHWC>(false));
   if (e == cudaSuccess)
-    e = cudaFuncSetAttribute(tc_contract_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes<T>(true));
+    e = cudaFuncSetAttribute(tc_contract_kernel<T, NHWC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes<T, NHWC>(true));
   // two ~73-97 KB CTAs per SM need the full shared-memory carve-out
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_gram_kernel<T>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_contract_kernel<T>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_gram_kernel<T, NHWC>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_contract_kernel<T, NHWC>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   return e;
+}
+
+template <class T, bool NHWC>
+void launch_gram(const CUtensorMap& mx, const void* x, const Geom& gm, int nchunks, float* shift, float* partial, cudaStream_t st) {
+  dim3 grid(nchunks, tc_superblocks(gm), gm.D);
+  tc_gram_kernel<T, NHWC><<<grid, kTcThreads, tc_smem_bytes<T, NHWC>(false), st>>>(mx, static_cast<const T*>(x), gm, shift, partial);
+}
+
+template <class T, bool NHWC>
+void launch_contract(const CUtensorMap& mx, const CUtensorMap& mg, const Geom& gm, int nchunks, const float* save_mean,
+                     float* partial, cudaStream_t st) {
+  dim3 grid(nchunks, tc_superblocks(gm), gm.D);
+  tc_contract_kernel<T, NHWC><<<grid, kTcThreads, tc_smem_bytes<T, NHWC>(true), st>>>(mx, mg, gm, save_mean, partial);
 }
 
 }  // namespace
@@ -476,8 +555,10 @@ int tc_init() {
   cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q);
   if (e != cudaSuccess || fn == nullptr || q != cudaDriverEntryPointSuccess) return e == cudaSuccess ? -1 : (int)e;
   g_encode = reinterpret_cast<EncodeTiledFn>(fn);
-  e = tc_kernel_attrs<float>();
-  if (e == cudaSuccess) e = tc_kernel_attrs<__nv_bfloat16>();
+  e = tc_kernel_attrs<float, false>();
+  if (e == cudaSuccess) e = tc_kernel_attrs<__nv_bfloat16, false>();
+  if (e == cudaSuccess) e = tc_kernel_attrs<float, true>();
+  if (e == cudaSuccess) e = tc_kernel_attrs<__nv_bfloat16, true>();
   if (e == cudaSuccess) e = (cudaError_t)dense_init();
   if (e == cudaSuccess) return tc_apply_init();
   return (int)e;
@@ -494,30 +575,33 @@ bool tc_supports(const Geom& gm, int vec) {
 int tc_superblocks(const Geom& gm) { return (gm.C + kTileCh - 1) / kTileCh; }
 
 // partial: [D][SB][nchunks][64*64+64] per-CTA moments;  shift: [D][SB][64] pilot shift of every channel
-int tc_stats(const void* x, bool bf16, const Geom& gm, int nchunks, float* shift, float* partial, cudaStream_t st) {
+int tc_stats(const void* x, bool bf16, bool nhwc, const Geom& gm, int nchunks, float* shift, float* partial, cudaStream_t st) {
   CUtensorMap mx;
   bind_context();
-  if (int rc = make_map(&mx, x, gm, bf16)) return rc;
-  dim3 grid(nchunks, tc_superblocks(gm), gm.D);
-  if (bf16)
-    tc_gram_kernel<__nv_bfloat16><<<grid, kTcThreads, tc_smem_bytes<__nv_bfloat16>(false), st>>>(
-        mx, static_cast<const __nv_bfloat16*>(x), gm, shift, partial);
-  else
-    tc_gram_kernel<float><<<grid, kTcThreads, tc_smem_bytes<float>(false), st>>>(mx, static_cast<const float*>(x), gm, shift, partial);
+  if (int rc = make_map(&mx, x, gm, bf16, nhwc)) return rc;
+  if (nhwc) {
+    if (bf16) launch_gram<__nv_bfloat16, true>(mx, x, gm, nchunks, shift, partial, st);
+    else launch_gram<float, true>(mx, x, gm, nchunks, shift, partial, st);
+  } else {
+    if (bf16) launch_gram<__nv_bfloat16, false>(mx, x, gm, nchunks, shift, partial, st);
+    else launch_gram<float, false>(mx, x, gm, nchunks, shift, partial, st);
+  }
   return 0;
 }
 
-int tc_bwd_reduce(const void* x, const void* dout, bool bf16, const Geom& gm, int nchunks, const float* save_mean,
+int tc_bwd_reduce(const void* x, const void* dout, bool bf16, bool nhwc, const Geom& gm, int nchunks, const float* save_mean,
                   float* partial, cudaStream_t st) {
   CUtensorMap mx, mg;
   bind_context();
-  if (int rc = make_map(&mx, x, gm, bf16)) return rc;
-  if (int rc = make_map(&mg, dout, gm, bf16)) return rc;
-  dim3 grid(nchunks, tc_superblocks(gm), gm.D);
-  if (bf16)
-    tc_contract_kernel<__nv_bfloat16><<<grid, kTcThreads, tc_smem_bytes<__nv_bfloat16>(true), st>>>(mx, mg, gm, save_mean, partial);
-  else
-    tc_contract_kernel<float><<<grid, kTcThreads, tc_smem_bytes<float>(true), st>>>(mx, mg, gm, save_mean, partial);
+  if (int rc = make_map(&mx, x, gm, bf16, nhwc)) return rc;
+  if (int rc = make_map(&mg, dout, gm, bf16, nhwc)) return rc;
+  if (nhwc) {
+    if (bf16) launch_contract<__nv_bfloat16, true>(mx, mg, gm, nchunks, save_mean, partial, st);
+    else launch_contract<float, true>(mx, mg, gm, nchunks, save_mean, partial, st);
+  } else {
+    if (bf16) launch_contract<__nv_bfloat16, false>(mx, mg, gm, nchunks, save_mean, partial, st);
+    else launch_contract<float, false>(mx, mg, gm, nchunks, save_mean, partial, st);
+  }
   return 0;
 }
 

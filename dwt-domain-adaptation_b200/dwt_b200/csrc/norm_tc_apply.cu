@@ -28,6 +28,12 @@
 // four distinct 16-byte chunks); each value is widened to fp32 as it is loaded into the fragment and the output is stored
 // rounded to nearest-even, 2 bytes per element.  Everything between is the fp32 kernel on the same tiles in the same order.
 //
+// channels-last activations (DWT_LAYOUT_NHWC): the kernel is also templated on the layout.  A tile is the same 64 px x 64 ch
+// block, landed as pixel rows of 128 bytes (SWIZZLE_128B) from a {C, HW, N*D} tensor map: per 32-pixel half, fp32 two
+// boxes of 32 ch x 32 px, bf16 one box of 64 ch x 32 px.  The A fragment -- 8 pixels x 4 channels per warp -- reads 32
+// distinct banks.  The output fragment is stored at NHWC addresses, two adjacent channels per store (8 bytes fp32, 4 bytes
+// bf16).  Same fragments, same products, same order: y and dx are bit for bit the NCHW kernel's on x.contiguous().
+//
 // Reference: the grouped 1x1 convolution at utils/whitening.py:55 of the reference project and its backward.
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -96,9 +102,14 @@ __device__ __forceinline__ uint32_t kmajor_off(int row, int k) {
   return (uint32_t)((k >> 5) * (kCh * 128) + row * 128 + ((((k & 31) >> 2) ^ (row & 7)) << 4) + (k & 3) * 4);
 }
 // Byte offset of (channel ch, pixel p) in the landed tile of one input, SWIZZLE_128B.  fp32: box p / 32 is
-// [64 ch x 128 B].  bf16: one box [64 ch x 128 B] of 64 pixels.
-template <class T>
+// [64 ch x 128 B].  bf16: one box [64 ch x 128 B] of 64 pixels.  NHWC: pixel rows of 128 B; fp32 channel half ch / 32 is
+// [64 px x 128 B] (two boxes of 32 px), bf16 one [64 px x 128 B] (two boxes of 32 px).
+template <class T, bool NHWC>
 __device__ __forceinline__ uint32_t tile_off(int ch, int p) {
+  if constexpr (NHWC) {
+    if constexpr (kBf16<T>) return (uint32_t)(p * 128 + (((ch >> 3) ^ (p & 7)) << 4) + (ch & 7) * 2);
+    return (uint32_t)((ch >> 5) * (kTilePx * 128) + p * 128 + ((((ch & 31) >> 2) ^ (p & 7)) << 4) + (ch & 3) * 4);
+  }
   if constexpr (kBf16<T>) return (uint32_t)(ch * 128 + (((p >> 3) ^ (ch & 7)) << 4) + (p & 7) * 2);
   const int pp = p & 31;
   return (uint32_t)((p >> 5) * kBoxBytes + ch * 128 + (((pp >> 2) ^ (ch & 7)) << 4) + (pp & 3) * 4);
@@ -115,7 +126,7 @@ __device__ __forceinline__ float lds_f(uint32_t addr) {
   }
 }
 
-template <class T, int NIN>
+template <class T, int NIN, bool NHWC>
 __global__ void __launch_bounds__(kApThreads, 1)
 tc_apply_kernel(const __grid_constant__ CUtensorMap map0, const __grid_constant__ CUtensorMap map1, const Geom gm,
                 const ApplyArgs args) {
@@ -170,7 +181,22 @@ tc_apply_kernel(const __grid_constant__ CUtensorMap map0, const __grid_constant_
         const int t = t_begin + it * t_step, n = t / PB, pb = t - n * PB, s = it % STAGES;
         mbar_wait_relaxed(&bars.empty[s], ((it / STAGES) & 1) ^ 1);
         uint8_t* dst = sRing + (size_t)s * SLOT;
-        if constexpr (kBf16<T>) {                  // one 64-pixel box per input
+        if constexpr (NHWC) {
+          // per 32-pixel half (halves entirely past the row end are not issued, as below): fp32 two boxes of 32 channels,
+          // bf16 one of 64; an input's half lands at + h * 4 KB, a 32-channel half of fp32 at + 8 KB
+          constexpr int HALF = SLOT / NIN / 2;
+          int nh = (gm.HW - pb * kTilePx + kBoxPx - 1) / kBoxPx;
+          nh = nh < kNBox ? nh : kNBox;
+          mbar_arrive_expect_tx(&bars.full[s], NIN * nh * HALF);
+#pragma unroll
+          for (int i = 0; i < NIN; ++i)
+            for (int h = 0; h < nh; ++h) {
+              uint8_t* b = dst + i * (SLOT / NIN) + h * (kBoxPx * 128);
+              const CUtensorMap* m = i == 0 ? &map0 : &map1;
+              tma_load_3d(b, m, ch0, pb * kTilePx + h * kBoxPx, d * gm.N + n, &bars.full[s]);
+              if constexpr (!kBf16<T>) tma_load_3d(b + kTilePx * 128, m, ch0 + 32, pb * kTilePx + h * kBoxPx, d * gm.N + n, &bars.full[s]);
+            }
+        } else if constexpr (kBf16<T>) {                  // one 64-pixel box per input
           mbar_arrive_expect_tx(&bars.full[s], SLOT);
 #pragma unroll
           for (int i = 0; i < NIN; ++i)
@@ -208,7 +234,7 @@ tc_apply_kernel(const __grid_constant__ CUtensorMap map0, const __grid_constant_
 #pragma unroll
           for (int r = 0; r < 4; ++r) {
             const int k = 8 * ks + kq + 4 * (r >> 1);
-            const float v = lds_f<T>(slot + i * (SLOT / NIN) + tile_off<T>(k, prow + 8 * (r & 1))) - sShift[i][k];
+            const float v = lds_f<T>(slot + i * (SLOT / NIN) + tile_off<T, NHWC>(k, prow + 8 * (r & 1))) - sShift[i][k];
             const uint32_t h = __float_as_uint(v) & kTf32Mask;
             ahi[i][ks][r] = h;
             alo[i][ks][r] = __float_as_uint(round_tf32(v - __uint_as_float(h)));
@@ -238,16 +264,33 @@ tc_apply_kernel(const __grid_constant__ CUtensorMap map0, const __grid_constant_
       fence_operands(acc);
       const int t = t_begin + it * t_step, n = t / PB, pb = t - n * PB;
       T* obase = static_cast<T*>(args.out) + (size_t)(d * gm.N + n) * gm.C * gm.HW;
+      if constexpr (NHWC) {
+        // channels c, c + 1 of pixel px: adjacent, one store (C % 8 == 0: both or neither inside the tensor)
+        const int px = pb * kTilePx + prow;
+        T* o = obase + (size_t)px * gm.C + ch0 + 2 * kq;
 #pragma unroll
-      for (int j = 0; j < kCh / 8; ++j)
+        for (int j = 0; j < kCh / 8; ++j)
 #pragma unroll
-        for (int r = 0; r < 4; ++r) {
-          const int c = 8 * j + 2 * kq + (r & 1), px = pb * kTilePx + prow + 8 * (r >> 1);
-          if (ch0 + c < gm.C && px < gm.HW) {
-            if constexpr (kBf16<T>) obase[(size_t)(ch0 + c) * gm.HW + px] = __float2bfloat16_rn(acc[4 * j + r]);
-            else obase[(size_t)(ch0 + c) * gm.HW + px] = acc[4 * j + r];
+          for (int h = 0; h < 2; ++h) {
+            if (ch0 + 8 * j + 2 * kq < gm.C && px + 8 * h < gm.HW) {
+              T* oj = o + (size_t)h * 8 * gm.C + 8 * j;
+              const float a0 = acc[4 * j + 2 * h], a1 = acc[4 * j + 2 * h + 1];
+              if constexpr (kBf16<T>) *reinterpret_cast<__nv_bfloat162*>(oj) = __floats2bfloat162_rn(a0, a1);
+              else *reinterpret_cast<float2*>(oj) = make_float2(a0, a1);
+            }
           }
-        }
+      } else {
+#pragma unroll
+        for (int j = 0; j < kCh / 8; ++j)
+#pragma unroll
+          for (int r = 0; r < 4; ++r) {
+            const int c = 8 * j + 2 * kq + (r & 1), px = pb * kTilePx + prow + 8 * (r >> 1);
+            if (ch0 + c < gm.C && px < gm.HW) {
+              if constexpr (kBf16<T>) obase[(size_t)(ch0 + c) * gm.HW + px] = __float2bfloat16_rn(acc[4 * j + r]);
+              else obase[(size_t)(ch0 + c) * gm.HW + px] = acc[4 * j + r];
+            }
+          }
+      }
     }
   }
 }
@@ -257,13 +300,22 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 EncodeTiledFn g_encode_ap = nullptr;
 
-// a box is 128 bytes wide either way: 32 fp32 or 64 bf16 pixels of 64 channels (bf16 needs HW % 8 == 0: 16-byte strides)
-int make_map_ap(CUtensorMap* map, const void* base, const Geom& gm, bool bf16) {
+// a box is 128 bytes wide either way: 32 fp32 or 64 bf16 pixels of 64 channels (bf16 needs HW % 8 == 0: 16-byte strides).
+// nhwc: dims {C, HW, N*D}, boxes of 32 fp32 or 64 bf16 channels x 32 pixels (C % 8 == 0: 16-byte strides).
+int make_map_ap(CUtensorMap* map, const void* base, const Geom& gm, bool bf16, bool nhwc) {
   const cuuint64_t es = bf16 ? 2 : 4;
+  const cuuint32_t estr[3] = {1, 1, 1};
+  if (nhwc) {
+    const cuuint64_t dims[3] = {(cuuint64_t)gm.C, (cuuint64_t)gm.HW, (cuuint64_t)gm.N * gm.D};
+    const cuuint64_t strides[2] = {(cuuint64_t)gm.C * es, (cuuint64_t)gm.HW * gm.C * es};
+    const cuuint32_t box[3] = {bf16 ? 64u : 32u, (cuuint32_t)kBoxPx, 1};
+    return (int)g_encode_ap(map, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<void*>(base),
+                            dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                            CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  }
   const cuuint64_t dims[3] = {(cuuint64_t)gm.HW, (cuuint64_t)gm.C, (cuuint64_t)gm.N * gm.D};
   const cuuint64_t strides[2] = {(cuuint64_t)gm.HW * es, (cuuint64_t)gm.C * gm.HW * es};
   const cuuint32_t box[3] = {bf16 ? (cuuint32_t)kTilePx : (cuuint32_t)kBoxPx, kCh, 1};
-  const cuuint32_t estr[3] = {1, 1, 1};
   return (int)g_encode_ap(map, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<void*>(base),
                           dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                           CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
@@ -271,12 +323,24 @@ int make_map_ap(CUtensorMap* map, const void* base, const Geom& gm, bool bf16) {
 
 template <class T, int NIN> constexpr size_t ap_smem() { return ApCfg<T, NIN>::SMEM; }
 
-template <class T, int NIN>
+template <class T, int NIN, bool NHWC>
 cudaError_t ap_attrs() {
-  cudaError_t e = cudaFuncSetAttribute(tc_apply_kernel<T, NIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ap_smem<T, NIN>());
+  cudaError_t e = cudaFuncSetAttribute(tc_apply_kernel<T, NIN, NHWC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ap_smem<T, NIN>());
   // a 129 / 193 KB CTA needs the full shared-memory carve-out
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_apply_kernel<T, NIN>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_apply_kernel<T, NIN, NHWC>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   return e;
+}
+
+template <int NIN>
+void launch_apply(bool bf16, bool nhwc, dim3 grid, const CUtensorMap& m0, const CUtensorMap& m1, const Geom& gm, const ApplyArgs& a,
+                  cudaStream_t st) {
+  if (nhwc) {
+    if (bf16) tc_apply_kernel<__nv_bfloat16, NIN, true><<<grid, kApThreads, ap_smem<__nv_bfloat16, NIN>(), st>>>(m0, m1, gm, a);
+    else tc_apply_kernel<float, NIN, true><<<grid, kApThreads, ap_smem<float, NIN>(), st>>>(m0, m1, gm, a);
+  } else {
+    if (bf16) tc_apply_kernel<__nv_bfloat16, NIN, false><<<grid, kApThreads, ap_smem<__nv_bfloat16, NIN>(), st>>>(m0, m1, gm, a);
+    else tc_apply_kernel<float, NIN, false><<<grid, kApThreads, ap_smem<float, NIN>(), st>>>(m0, m1, gm, a);
+  }
 }
 
 }  // namespace
@@ -287,46 +351,46 @@ int tc_apply_init() {
   cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q);
   if (e != cudaSuccess || fn == nullptr || q != cudaDriverEntryPointSuccess) return e == cudaSuccess ? -1 : (int)e;
   g_encode_ap = reinterpret_cast<EncodeTiledFn>(fn);
-  e = ap_attrs<float, 1>();
-  if (e == cudaSuccess) e = ap_attrs<float, 2>();
-  if (e == cudaSuccess) e = ap_attrs<__nv_bfloat16, 1>();
-  if (e == cudaSuccess) e = ap_attrs<__nv_bfloat16, 2>();
+  e = ap_attrs<float, 1, false>();
+  if (e == cudaSuccess) e = ap_attrs<float, 2, false>();
+  if (e == cudaSuccess) e = ap_attrs<__nv_bfloat16, 1, false>();
+  if (e == cudaSuccess) e = ap_attrs<__nv_bfloat16, 2, false>();
+  if (e == cudaSuccess) e = ap_attrs<float, 1, true>();
+  if (e == cudaSuccess) e = ap_attrs<float, 2, true>();
+  if (e == cudaSuccess) e = ap_attrs<__nv_bfloat16, 1, true>();
+  if (e == cudaSuccess) e = ap_attrs<__nv_bfloat16, 2, true>();
   return (int)e;
 }
 
 // y = W (x - mean): W from save_w [D][G][gs*gs], mean from save_mean [D][C]
-int tc_apply(const void* x, void* y, bool bf16, const Geom& gm, int nctas, const float* save_mean, const float* save_w,
+int tc_apply(const void* x, void* y, bool bf16, bool nhwc, const Geom& gm, int nctas, const float* save_mean, const float* save_w,
              cudaStream_t st) {
   CUtensorMap mx;
   bind_context();
-  if (int rc = make_map_ap(&mx, x, gm, bf16)) return rc;
+  if (int rc = make_map_ap(&mx, x, gm, bf16, nhwc)) return rc;
   ApplyArgs a{};
   a.interleave = tile_interleave();
   a.mats = save_w; a.rec_stride = gm.GS * gm.GS; a.off[0] = 0; a.off[1] = 0;
   a.shift[0] = save_mean; a.shift_stride[0] = gm.C; a.shift[1] = nullptr; a.shift_stride[1] = 0;
   a.out = y;
-  dim3 grid(nctas, (gm.C + kCh - 1) / kCh, gm.D);
-  if (bf16) tc_apply_kernel<__nv_bfloat16, 1><<<grid, kApThreads, ap_smem<__nv_bfloat16, 1>(), st>>>(mx, mx, gm, a);
-  else tc_apply_kernel<float, 1><<<grid, kApThreads, ap_smem<float, 1>(), st>>>(mx, mx, gm, a);
+  launch_apply<1>(bf16, nhwc, dim3(nctas, (gm.C + kCh - 1) / kCh, gm.D), mx, mx, gm, a, st);
   return 0;
 }
 
 // dx = A1 (dy - dybar) + Bm (x - mean): coef [D][G][2 gs^2 + gs] = A1 | Bm | cvec, dybar [D][SB*64]
-int tc_bwd_apply(const void* x, const void* dout, void* dx, bool bf16, const Geom& gm, int nctas, const float* coef,
+int tc_bwd_apply(const void* x, const void* dout, void* dx, bool bf16, bool nhwc, const Geom& gm, int nctas, const float* coef,
                  const float* save_mean, const float* dybar, cudaStream_t st) {
   CUtensorMap mx, mg;
   bind_context();
-  if (int rc = make_map_ap(&mg, dout, gm, bf16)) return rc;
-  if (int rc = make_map_ap(&mx, x, gm, bf16)) return rc;
+  if (int rc = make_map_ap(&mg, dout, gm, bf16, nhwc)) return rc;
+  if (int rc = make_map_ap(&mx, x, gm, bf16, nhwc)) return rc;
   ApplyArgs a{};
   a.interleave = tile_interleave();
   a.mats = coef; a.rec_stride = coef_stride(gm.GS); a.off[0] = 0; a.off[1] = gm.GS * gm.GS;
   a.shift[0] = dybar; a.shift_stride[0] = ((gm.C + kCh - 1) / kCh) * kCh;
   a.shift[1] = save_mean; a.shift_stride[1] = gm.C;
   a.out = dx;
-  dim3 grid(nctas, (gm.C + kCh - 1) / kCh, gm.D);
-  if (bf16) tc_apply_kernel<__nv_bfloat16, 2><<<grid, kApThreads, ap_smem<__nv_bfloat16, 2>(), st>>>(mg, mx, gm, a);
-  else tc_apply_kernel<float, 2><<<grid, kApThreads, ap_smem<float, 2>(), st>>>(mg, mx, gm, a);
+  launch_apply<2>(bf16, nhwc, dim3(nctas, (gm.C + kCh - 1) / kCh, gm.D), mg, mx, gm, a, st);
   return 0;
 }
 

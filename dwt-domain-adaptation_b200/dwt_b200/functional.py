@@ -6,7 +6,8 @@ centred copy, a transposed copy or the covariance graph the reference's autograd
 
 Activations are float32 or bfloat16 (what torch.autocast(dtype=torch.bfloat16) hands over from a convolution): a bf16
 call whose activations are all bf16 runs the bf16 kernels (DWT_DTYPE_BF16) when it is channels-last on a channels-last
-geometry (group sizes 1, 2, 4), or NCHW whitening on a tensor-core geometry (_bf16_tensor_core); any other bf16 call runs
+geometry (group sizes 1, 2, 4) or on a channels-last tensor-core geometry (_nhwc_tensor_core), or NCHW whitening on a
+tensor-core geometry (_bf16_tensor_core); any other bf16 call runs
 the float32 kernels on upcast copies and casts the result back.  Statistics, parameters, their gradients and the running
 buffers are float32 either way, like nn.BatchNorm2d under autocast.
 """
@@ -17,17 +18,27 @@ import torch
 from . import _native as nv
 
 
-def _dense(x: torch.Tensor, group_size: int):
+def _nhwc_tensor_core(x, group_size, n_domains):
+    """The channels-last tensor-core rule for x (nv.tensor_core_nhwc_supported on its per-domain geometry) with a
+    16-byte-aligned data_ptr(); a misaligned view is not taken (it is copied to NCHW by _dense)."""
+    if n_domains is None or x.dim() != 4 or x.shape[0] % n_domains:
+        return False
+    return (nv.tensor_core_nhwc_supported(x.shape[0] // n_domains, x.shape[1], x.shape[2] * x.shape[3], group_size)
+            and x.data_ptr() % 16 == 0)
+
+
+def _dense(x: torch.Tensor, group_size: int, n_domains=None):
     """[N, C, *spatial] -> (dense tensor, N, C, HW, channels_last?).
 
-    A 4-D tensor that is already dense in torch.channels_last order is used as it is (NHWC kernels) when
-    the geometry has a channels-last build; anything else is made NCHW-contiguous."""
+    A 4-D tensor that is already dense in torch.channels_last order is used as it is (NHWC kernels) when the geometry
+    has a channels-last build: the channels-last kernels (group sizes 1, 2, 4), or -- given n_domains -- the tensor-core
+    kernels (_nhwc_tensor_core); anything else is made NCHW-contiguous."""
     n, c = x.shape[0], x.shape[1]
     hw = 1
     for s in x.shape[2:]:
         hw *= s
     nhwc = (x.dim() == 4 and not x.is_contiguous() and x.is_contiguous(memory_format=torch.channels_last)
-            and nv.channels_last_supported(c, group_size))
+            and (nv.channels_last_supported(c, group_size) or _nhwc_tensor_core(x, group_size, n_domains)))
     if not nhwc and not x.is_contiguous():
         x = x.contiguous()
     return x, n, c, hw, nhwc
@@ -68,7 +79,7 @@ class _NormFunction(torch.autograd.Function):
                 running, relu):
         lib = nv.lib()
         gs = group_size if kind == "whiten" else 1
-        x, n_all, c, hw, nhwc = _dense(x, gs)
+        x, n_all, c, hw, nhwc = _dense(x, gs, n_domains)
         bf16 = x.dtype == torch.bfloat16
         if bf16 and not ((nhwc and (residual is None or residual.dtype == x.dtype))
                          or (not nhwc and _bf16_tensor_core(x, kind, gs, n_domains, residual))):
@@ -160,18 +171,21 @@ class _NormFunction(torch.autograd.Function):
             x, save_mean, save_w, gamma_c, beta_c = ctx.saved_tensors
         kind, gs, n_domains, mode, eps, epi, n, c, hw, gshape = ctx.cfg
         # second addend of the incoming gradient, left here by fork_for_sum's backward (see there): the channels-last
-        # kernels add it where they read dout; any other path adds it now
+        # kernels of group sizes 1, 2, 4 add it where they read dout; any other path adds it now
         dout2 = ctx.__dict__.pop("_dwt_extra_grad", None)
         if dout.dtype != x.dtype:
             dout = dout.to(x.dtype)
-        if dout2 is not None and not ((mode & nv.LAYOUT_NHWC) and dout2.shape == dout.shape and dout2.dtype == dout.dtype
+        nhwc = bool(mode & nv.LAYOUT_NHWC)
+        cl_kernels = nhwc and nv.channels_last_supported(c, gs)
+        if dout2 is not None and not (cl_kernels and dout2.shape == dout.shape and dout2.dtype == dout.dtype
                                       and dout2.is_contiguous(memory_format=torch.channels_last)):
             dout, dout2 = dout + dout2, None
-        dout = dout.contiguous(memory_format=torch.channels_last) if (mode & nv.LAYOUT_NHWC) else dout.contiguous()
-        if (mode & nv.DTYPE_BF16) and not (mode & nv.LAYOUT_NHWC) and dout.data_ptr() % 16:
-            dout = dout.clone()                      # the forward ran the tensor-core kernels: their TMA loads need 16 bytes
+        dout = dout.contiguous(memory_format=torch.channels_last) if nhwc else dout.contiguous()
+        if ((mode & nv.DTYPE_BF16) or nhwc) and not cl_kernels and dout.data_ptr() % 16:
+            # the forward ran the tensor-core kernels: their TMA loads need 16 bytes (a fresh tensor keeps the layout)
+            dout = dout.clone(memory_format=torch.channels_last if nhwc else torch.contiguous_format)
         dev = nv.require_cuda(dout, bf16=True)
-        dx = torch.empty_like(x)
+        dx = torch.empty_like(x)                     # x's layout: channels-last when the forward ran NHWC
         want_affine = gamma_c is not None and (ctx.needs_input_grad[1] or ctx.needs_input_grad[2])
         d_res = None
         if ctx.residual_mode == "mask":
@@ -339,8 +353,9 @@ def norm(x, gamma, beta, *, kind, group_size, n_domains, training_stats, eps, mo
     if torch.bfloat16 in dtypes and dtypes <= set(_ACT_DTYPES):
         gs = group_size if kind == "whiten" else 1
         cl = x.dim() == 4 and not x.is_contiguous() and x.is_contiguous(memory_format=torch.channels_last)
+        cl_tc = kind == "whiten" and residual is None and _nhwc_tensor_core(x, gs, n_domains)
         bf16_kernels = dtypes == {torch.bfloat16} and (
-            nv.channels_last_supported(x.shape[1], gs) if cl else _bf16_tensor_core(x, kind, gs, n_domains, residual))
+            (nv.channels_last_supported(x.shape[1], gs) or cl_tc) if cl else _bf16_tensor_core(x, kind, gs, n_domains, residual))
         if not bf16_kernels:
             # NCHW group sizes 1, 2, 4, geometries and alignments the bf16 kernels lack, or mixed dtypes: the float32
             # kernels on upcast copies, the result (and through autograd every gradient of x and the residual) back in

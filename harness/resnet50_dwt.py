@@ -268,13 +268,15 @@ class ResNet50DWT(_SiteOwner):
 
 
 def build_resnet50_dwt(state_dict, layers, site_mode="modules", num_classes=65, channels_last=False, stem_pad=0,
-                       stem_nchw=False, stem_s2d=False):
+                       stem_nchw=False, stem_s2d=False, group_size=4):
     """state_dict uses the reference checkpoint's key names *without* the 7-char
     ``module.`` prefix (resnet50_dwt_mec_officehome.py:370-376).  channels_last=True converts the
     convolution weights to torch.channels_last so that, fed channels-last images, every activation
-    stays NHWC (no cuDNN NCHW<->NHWC copies); results are identical, only strides change."""
-    model = ResNet50DWT(layers, state_dict, num_classes=num_classes, site_mode=site_mode, stem_pad=stem_pad,
-                        stem_nchw=stem_nchw and channels_last, stem_s2d=stem_s2d)
+    stays NHWC (no cuDNN NCHW<->NHWC copies); results are identical, only strides change.
+    group_size is the reference ResNet's option (resnet50_dwt_mec_officehome.py:266): the stem site's whitening group
+    size (the layers keep 4, as the reference's _make_layer does)."""
+    model = ResNet50DWT(layers, state_dict, num_classes=num_classes, group_size=group_size, site_mode=site_mode,
+                        stem_pad=stem_pad, stem_nchw=stem_nchw and channels_last, stem_s2d=stem_s2d)
     model.load_state_dict(state_dict, strict=False)
     if channels_last and hasattr(layers, "MaxPool2d"):
         model.maxpool = layers.MaxPool2d(3, stride=2, padding=1)    # the library's channels-last kernel pair (no state)

@@ -46,7 +46,7 @@
 extern "C" {
 #endif
 
-#define DWT_B200_ABI_VERSION 8
+#define DWT_B200_ABI_VERSION 9
 #define DWT_MAX_DOMAINS 4
 #define DWT_MAX_GROUP_SIZE 64
 
@@ -62,9 +62,15 @@ extern "C" {
 #define DWT_MODE_EVAL 1  /* running statistics                                        */
 
 /* memory layout of the activation tensors, OR-ed into `mode`:
- * default = [n_domains*N, C, HW] (NCHW); DWT_LAYOUT_NHWC = [n_domains*N, HW, C] (torch.channels_last), built for
- * group sizes 1, 2, 4 with C/4 a power of two (the layout cuDNN's tensor-core convolutions want: a
- * channels-last model needs no NCHW<->NHWC copies around its convolutions). */
+ * default = [n_domains*N, C, HW] (NCHW); DWT_LAYOUT_NHWC = [n_domains*N, HW, C] (torch.channels_last: the layout
+ * cuDNN's tensor-core convolutions want, so a channels-last model needs no NCHW<->NHWC copies around its convolutions).
+ * Built for two kernel families:
+ *   - group sizes 1, 2, 4 with C/4 a power of two (the channels-last kernels, every epilogue, dout2);
+ *   - whitening at group sizes 8, 16, 32, 64 on the tensor-core kernels: HW >= 32 and HW % 4 == 0, N*HW >= 4096 per
+ *     domain, x / y / dout / dx 16-byte aligned (else DWT_E_INVALID), epilogue 0 and no dout2 (else DWT_E_UNSUPPORTED),
+ *     fp32 or bf16.  Same schedule and arithmetic as the NCHW call: every output, statistic, running-buffer update and
+ *     status bit is bit for bit that of the NCHW call on the same values.  Profile families tc_*_nhwc[_bf16].
+ * Any other channels-last geometry is DWT_E_UNSUPPORTED. */
 #define DWT_LAYOUT_NHWC 0x100
 
 /* activation storage, OR-ed into `mode` (dwt_whiten_*, dwt_bn_*), `kind` (dwt_tail2_*) or `flags` (dwt_maxpool_*):
@@ -73,8 +79,9 @@ extern "C" {
  * their gradients, save_mean / save_w and the workspace stay fp32.  Built for two kernel families:
  *   - channels-last (DWT_LAYOUT_NHWC; the tail and the max-pool are channels-last anyway), group size 1, 2, 4 with C/4
  *     a power of two; bf16 tensors 8-byte aligned;
- *   - NCHW whitening on the tensor-core kernels: group size 8, 16, 32, 64, HW >= 32 and HW % 8 == 0, N*HW >= 4096 per
- *     domain; x and dout 16-byte aligned (TMA).
+ *   - whitening on the tensor-core kernels: group size 8, 16, 32, 64, HW >= 32, N*HW >= 4096 per domain; NCHW with
+ *     HW % 8 == 0 and x and dout 16-byte aligned (TMA), or channels-last with HW % 4 == 0 and x, y, dout, dx 16-byte
+ *     aligned (see DWT_LAYOUT_NHWC).
  * Any other geometry is DWT_E_UNSUPPORTED (NCHW group sizes 1, 2, 4 and batch norm included); a misaligned tensor is
  * DWT_E_INVALID.  bf16 launches report in the profile as <family>_bf16 and count 2 bytes per activation element.
  * The kernels run the fp32 schedule of the same shape: loads widen to fp32, stores round to nearest-even, so statistics,
