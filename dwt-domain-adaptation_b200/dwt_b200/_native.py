@@ -14,13 +14,13 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # DWT_B200_LIB: another build of the same library (development: A/B timing of a kernel variant on one box)
 LIB_PATH = os.environ.get("DWT_B200_LIB") or os.path.join(_HERE, "lib", "libdwt_b200.so")
 
-ABI_VERSION = 9
+ABI_VERSION = 10
 MAX_DOMAINS = 4
 MAX_GROUP_SIZE = 64
 MODE_TRAIN, MODE_EVAL = 0, 1
 EPI_NONE, EPI_AFFINE, EPI_RELU, EPI_RESIDUAL = 0, 1, 2, 4
 LAYOUT_NHWC = 0x100
-DTYPE_BF16 = 0x200                 # bf16 activations (channels-last gs 1/2/4, tensor-core gs 8..64; include/dwt_b200.h)
+DTYPE_BF16 = 0x200                 # bf16 activations (gs 1/2/4 and BN channels-last or NCHW, tensor-core gs 8..64; dwt_b200.h)
 STATUS_NOT_PD, STATUS_BAD_LABEL = 1, 2
 KIND_WHITEN, KIND_BN = 0, 1
 
@@ -148,6 +148,13 @@ def channels_last_supported(channels: int, group_size: int) -> bool:
         return False
     c4 = channels // 4
     return c4 & (c4 - 1) == 0 and c4 <= 16384
+
+
+def small_bf16_supported(hw: int, group_size: int) -> bool:
+    """Mirror of the C ABI's bf16 rule for the NCHW register-resident kernels (csrc/api.cu, small_bf16_supports):
+    whitening at group sizes 1, 2, 4 and batch norm (group_size 1) take bf16 activations when HW is a multiple of 4 (a
+    thread reads four pixels of a channel row as 8 bytes).  The tensors also need an 8-byte-aligned data_ptr()."""
+    return group_size in (1, 2, 4) and hw % 4 == 0
 
 
 def tensor_core_bf16_supported(n: int, channels: int, hw: int, group_size: int) -> bool:

@@ -269,8 +269,10 @@ void shape(dwt::Geom& g, int64_t work_units, KernelKind kind, bool small, int* c
   *chunks = n;
 }
 
+// vec = 4 when rows can be read as 4-element vectors: HW % 4 == 0 and a0..a2 aligned to 4 elements of elem_bytes each
+// (16 bytes in fp32, 8 in bf16), so an aligned bf16 call gets the plan of the fp32 call of its shape
 int make_plan(Plan& p, KernelKind reduce_kind, KernelKind ew_kind, const void* a0, const void* a1, const void* a2,
-              int64_t N, int64_t C, int64_t HW, int GS, int D) {
+              int64_t N, int64_t C, int64_t HW, int GS, int D, int elem_bytes) {
   if (N <= 0 || C <= 0 || HW <= 0) return fail(DWT_E_INVALID, "empty tensor (N=%lld C=%lld HW=%lld)", (long long)N,
                                                (long long)C, (long long)HW);
   if (GS < 1 || GS > DWT_MAX_GROUP_SIZE) return fail(DWT_E_UNSUPPORTED, "group_size %d outside [1,%d]", GS,
@@ -283,7 +285,7 @@ int make_plan(Plan& p, KernelKind reduce_kind, KernelKind ew_kind, const void* a
   g.N = (int)N; g.C = (int)C; g.HW = (int)HW; g.GS = GS; g.G = (int)(C / GS); g.D = D;
   g.M = (float)((double)N * (double)HW);
   const uintptr_t bits = (uintptr_t)a0 | (uintptr_t)a1 | (uintptr_t)a2;
-  p.vec = (HW % 4 == 0 && bits % 16 == 0) ? 4 : 1;
+  p.vec = (HW % 4 == 0 && bits % (4 * elem_bytes) == 0) ? 4 : 1;
   p.small = dwt::small_supports(GS);
   int64_t work_units;   // CTA-sized pieces of work available per (domain, group)
   if (p.small) work_units = (N * (HW / p.vec) + dwt::kThreads * 2 - 1) / (dwt::kThreads * 2);
@@ -302,26 +304,32 @@ int make_plan(Plan& p, KernelKind reduce_kind, KernelKind ew_kind, const void* a
 // dout and dx 16-byte aligned.
 bool tc_nhwc_supports(const dwt::Geom& g) { return dwt::tc_supports(g, 4) && g.HW % 4 == 0; }
 // DWT_DTYPE_BF16 (dwt_b200.h): bf16 activations run the channels-last kernels (group sizes 1, 2, 4), where a thread's
-// four channels are 8 bytes, so that is the alignment the tensors need (16 for fp32); and the tensor-core family
-// (group sizes 8..64, tc_supports), whose TMA loads need 16-byte rows (NCHW: HW % 8 == 0) and a 16-byte-aligned x / dout
+// four channels are 8 bytes, so that is the alignment the tensors need (16 for fp32); the NCHW register-resident kernels
+// (group sizes 1, 2, 4 and batch norm), where a thread's four pixels of a channel row are 8 bytes: HW % 4 == 0 and
+// 8-byte-aligned tensors, the fp32 plan with vec == 4; and the tensor-core family (group sizes 8..64, tc_supports),
+// whose TMA loads need 16-byte rows (NCHW: HW % 8 == 0) and a 16-byte-aligned x / dout
 bool tc_bf16_supports(const dwt::Geom& g) { return dwt::tc_supports(g, 4) && g.HW % 8 == 0; }
+bool small_bf16_supports(const dwt::Geom& g) { return dwt::small_supports(g.GS) && g.HW % 4 == 0; }
 int check_bf16_geometry(bool bf16, bool nhwc, const dwt::Geom& g) {
-  if (!bf16 || (nhwc ? dwt::cl_supports(g.C, g.GS) || tc_nhwc_supports(g) : tc_bf16_supports(g))) return DWT_OK;
+  if (!bf16 || (nhwc ? dwt::cl_supports(g.C, g.GS) || tc_nhwc_supports(g) : small_bf16_supports(g) || tc_bf16_supports(g)))
+    return DWT_OK;
   if (nhwc)
     return fail(DWT_E_UNSUPPORTED, "channels-last bf16 activations are built for group_size 1, 2, 4 with C/4 a power of two, "
                                    "and for the tensor-core kernels: group_size 8, 16, 32, 64, HW >= 32 and a multiple of 4, "
                                    "N*HW >= 4096 per domain (C=%d HW=%d N=%d gs=%d)", g.C, g.HW, g.N, g.GS);
-  return fail(DWT_E_UNSUPPORTED, "NCHW bf16 activations are built for the tensor-core kernels: group_size 8, 16, 32, 64, "
-                                 "HW >= 32 and a multiple of 8, N*HW >= 4096 per domain (C=%d HW=%d N=%d gs=%d)", g.C, g.HW, g.N, g.GS);
+  return fail(DWT_E_UNSUPPORTED, "NCHW bf16 activations are built for group_size 1, 2, 4 and batch norm with HW a multiple "
+                                 "of 4, and for the tensor-core kernels: group_size 8, 16, 32, 64, HW >= 32 and a multiple "
+                                 "of 8, N*HW >= 4096 per domain (C=%d HW=%d N=%d gs=%d)", g.C, g.HW, g.N, g.GS);
 }
 int check_tc_bf16_align(bool bf16, bool nhwc, uintptr_t bits, const char* what) {
   if (!bf16 || nhwc || bits % 16 == 0) return DWT_OK;
   return fail(DWT_E_INVALID, "%s must be 16-byte aligned (bf16 NCHW: TMA)", what);
 }
 // the tensor-core family runs every fp32 NCHW call whose geometry and alignment it takes (else the tiled kernels), and
-// every bf16 NCHW call and channels-last call routed to it (validated above: there is no other kernel to fall back to)
+// every bf16 NCHW call of group size 8..64 and channels-last call routed to it (validated above: there is no other
+// kernel to fall back to)
 int tc_route(bool bf16, bool nhwc, const Plan& p, bool* tc) {
-  if (bf16 || nhwc) {
+  if (!p.small && (bf16 || nhwc)) {
     if (ensure_tc() != 0) return fail(DWT_E_LAUNCH, "tensor-core kernel set-up failed (%d)", g_tc_rc);
     *tc = true;
   } else {
@@ -390,14 +398,18 @@ int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, 
   const bool nhwc = (mode & DWT_LAYOUT_NHWC) != 0, bf16 = (mode & DWT_DTYPE_BF16) != 0;
   mode &= 0xFF;
   Plan p;
-  if (int rc = make_plan(p, K_STATS, K_APPLY, x, y, nullptr, N, C, HW, GS, D)) return rc;
+  if (int rc = make_plan(p, K_STATS, K_APPLY, x, y, nullptr, N, C, HW, GS, D, bf16 && !nhwc ? 2 : 4)) return rc;
   if (!x || !y || !save_mean || !save_w || !ws) return fail(DWT_E_INVALID, "null pointer argument");
   if (int rc = check_bf16_geometry(bf16, nhwc, p.gm)) return rc;
   const bool nhwc_tc = nhwc && tc_nhwc_supports(p.gm);
   if (nhwc && !nhwc_tc && !dwt::cl_supports((int)C, GS)) return fail_nhwc_geometry(p.gm);
   if (nhwc_tc) if (int rc = check_tc_nhwc_align((uintptr_t)x | (uintptr_t)y, "x and y")) return rc;
   if (nhwc && !nhwc_tc) if (int rc = check_align(bf16, (uintptr_t)x | (uintptr_t)y, "channels-last tensors")) return rc;
-  if (int rc = check_tc_bf16_align(bf16, nhwc, (uintptr_t)x, "x")) return rc;
+  if (bf16 && !nhwc && p.small) {
+    if (int rc = check_align(bf16, (uintptr_t)x | (uintptr_t)y, "x and y")) return rc;
+  } else if (int rc = check_tc_bf16_align(bf16, nhwc, (uintptr_t)x, "x")) {
+    return rc;
+  }
   if (mode != DWT_MODE_TRAIN && mode != DWT_MODE_EVAL) return fail(DWT_E_INVALID, "bad mode %d", mode);
   if ((epi & DWT_EPI_RELU) && !(epi & DWT_EPI_AFFINE)) return fail(DWT_E_INVALID, "RELU epilogue needs AFFINE");
   if ((epi & DWT_EPI_AFFINE) && (!gamma || !beta)) return fail(DWT_E_INVALID, "AFFINE epilogue needs gamma and beta");
@@ -443,8 +455,8 @@ int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, 
   bool tc = false;
   if (int rc = tc_route(bf16, nhwc, p, &tc)) return rc;
   if (mode == DWT_MODE_TRAIN) {
-    Launch l(p.small ? "small_stats" : (tc ? tc_fam(bf16, nhwc, "tc_stats", "tc_stats_bf16", "tc_stats_nhwc", "tc_stats_nhwc_bf16") : "tiled_stats"), &p.gm, E, st);
-    if (p.small) dwt::small_stats(x, p.gm, p.vec, fin, w.partial, w.counters, st);
+    Launch l(p.small ? fam(bf16, "small_stats", "small_stats_bf16") : (tc ? tc_fam(bf16, nhwc, "tc_stats", "tc_stats_bf16", "tc_stats_nhwc", "tc_stats_nhwc_bf16") : "tiled_stats"), &p.gm, E, st);
+    if (p.small) dwt::small_stats(x, bf16, p.gm, p.vec, fin, w.partial, w.counters, st);
     else if (tc) {
       if (int cr = dwt::tc_stats(x, bf16, nhwc, p.gm, tc_chunks(p.gm), w.shift, w.partial, st))
         return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d) x=%p N=%d C=%d HW=%d D=%d", cr, (const void*)x, p.gm.N, p.gm.C, p.gm.HW, p.gm.D);
@@ -463,9 +475,9 @@ int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, 
   }
   if (int rc = check_launch("whitening statistics kernel")) return rc;
   {
-    Launch l(p.small ? "small_apply" : (tc ? tc_fam(bf16, nhwc, "tc_apply", "tc_apply_bf16", "tc_apply_nhwc", "tc_apply_nhwc_bf16") : "tiled_apply"), &p.gm,
+    Launch l(p.small ? fam(bf16, "small_apply", "small_apply_bf16") : (tc ? tc_fam(bf16, nhwc, "tc_apply", "tc_apply_bf16", "tc_apply_nhwc", "tc_apply_nhwc_bf16") : "tiled_apply"), &p.gm,
              ((epi & DWT_EPI_RESIDUAL) ? 3 : 2) * E, st);
-    if (p.small) dwt::small_apply(x, y, p.gm_ew, p.vec, p.chunks_ew, epi, save_mean, save_w, gamma, beta, residual, st);
+    if (p.small) dwt::small_apply(x, y, bf16, p.gm_ew, p.vec, p.chunks_ew, epi, save_mean, save_w, gamma, beta, residual, st);
     else if (tc) {
       if (int cr = dwt::tc_apply(x, y, bf16, nhwc, p.gm, tc_apply_ctas(p.gm, 1, 64), save_mean, save_w, st))
         return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d)", cr);
@@ -481,7 +493,7 @@ int whiten_like_bwd(const float* x, const float* dout, const float* dout2, float
   const bool nhwc = (mode & DWT_LAYOUT_NHWC) != 0, bf16 = (mode & DWT_DTYPE_BF16) != 0;
   mode &= 0xFF;
   Plan p;
-  if (int rc = make_plan(p, K_BWD_REDUCE, K_BWD_APPLY, x, dout, dx, N, C, HW, GS, D)) return rc;
+  if (int rc = make_plan(p, K_BWD_REDUCE, K_BWD_APPLY, x, dout, dx, N, C, HW, GS, D, bf16 && !nhwc ? 2 : 4)) return rc;
   if (!x || !dout || !dx || !save_mean || !save_w || !ws) return fail(DWT_E_INVALID, "null pointer argument");
   if (int rc = check_bf16_geometry(bf16, nhwc, p.gm)) return rc;
   const bool nhwc_tc = nhwc && tc_nhwc_supports(p.gm);
@@ -491,7 +503,11 @@ int whiten_like_bwd(const float* x, const float* dout, const float* dout2, float
   if (nhwc && !nhwc_tc && !dwt::cl_supports((int)C, GS)) return fail_nhwc_geometry(p.gm);
   if (nhwc_tc) if (int rc = check_tc_nhwc_align((uintptr_t)x | (uintptr_t)dout | (uintptr_t)dx, "x, dout and dx")) return rc;
   if (nhwc && !nhwc_tc) if (int rc = check_align(bf16, (uintptr_t)x | (uintptr_t)dout | (uintptr_t)dx, "channels-last tensors")) return rc;
-  if (int rc = check_tc_bf16_align(bf16, nhwc, (uintptr_t)x | (uintptr_t)dout, "x and dout")) return rc;
+  if (bf16 && !nhwc && p.small) {
+    if (int rc = check_align(bf16, (uintptr_t)x | (uintptr_t)dout | (uintptr_t)dx, "x, dout and dx")) return rc;
+  } else if (int rc = check_tc_bf16_align(bf16, nhwc, (uintptr_t)x | (uintptr_t)dout, "x and dout")) {
+    return rc;
+  }
   if (mode != DWT_MODE_TRAIN && mode != DWT_MODE_EVAL) return fail(DWT_E_INVALID, "bad mode %d", mode);
   if ((epi & DWT_EPI_RELU) && !(epi & DWT_EPI_AFFINE)) return fail(DWT_E_INVALID, "RELU epilogue needs AFFINE");
   if ((epi & DWT_EPI_AFFINE) && (!gamma || !beta)) return fail(DWT_E_INVALID, "AFFINE epilogue needs gamma and beta");
@@ -544,8 +560,8 @@ int whiten_like_bwd(const float* x, const float* dout, const float* dout2, float
   bool tc = false;
   if (int rc = tc_route(bf16, nhwc, p, &tc)) return rc;
   if (need_reduce) {
-    Launch l(p.small ? "small_bwd_reduce" : (tc ? tc_fam(bf16, nhwc, "tc_bwd_reduce", "tc_bwd_reduce_bf16", "tc_bwd_reduce_nhwc", "tc_bwd_reduce_nhwc_bf16") : "tiled_bwd_reduce"), &p.gm, 2 * E, st);
-    if (p.small) dwt::small_bwd_reduce(x, dout, p.gm, p.vec, fin, beta, w.partial, w.counters, st);
+    Launch l(p.small ? fam(bf16, "small_bwd_reduce", "small_bwd_reduce_bf16") : (tc ? tc_fam(bf16, nhwc, "tc_bwd_reduce", "tc_bwd_reduce_bf16", "tc_bwd_reduce_nhwc", "tc_bwd_reduce_nhwc_bf16") : "tiled_bwd_reduce"), &p.gm, 2 * E, st);
+    if (p.small) dwt::small_bwd_reduce(x, dout, bf16, p.gm, p.vec, fin, beta, w.partial, w.counters, st);
     else if (tc) {
       if (int cr = dwt::tc_bwd_reduce(x, dout, bf16, nhwc, p.gm, tc_chunks(p.gm), save_mean, w.partial, st))
         return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d) x=%p dout=%p N=%d C=%d HW=%d D=%d", cr, (const void*)x, (const void*)dout, p.gm.N, p.gm.C, p.gm.HW, p.gm.D);
@@ -564,8 +580,8 @@ int whiten_like_bwd(const float* x, const float* dout, const float* dout2, float
   }
   if (int rc = check_launch("whitening backward reduction kernel")) return rc;
   {
-    Launch l(p.small ? "small_bwd_apply" : (tc ? tc_fam(bf16, nhwc, "tc_bwd_apply", "tc_bwd_apply_bf16", "tc_bwd_apply_nhwc", "tc_bwd_apply_nhwc_bf16") : "tiled_bwd_apply"), &p.gm, 3 * E, st);
-    if (p.small) dwt::small_bwd_apply(x, dout, dx, p.gm_ew, p.vec, p.chunks_ew, epi, w.coef, save_mean, save_w, gamma, beta, st);
+    Launch l(p.small ? fam(bf16, "small_bwd_apply", "small_bwd_apply_bf16") : (tc ? tc_fam(bf16, nhwc, "tc_bwd_apply", "tc_bwd_apply_bf16", "tc_bwd_apply_nhwc", "tc_bwd_apply_nhwc_bf16") : "tiled_bwd_apply"), &p.gm, 3 * E, st);
+    if (p.small) dwt::small_bwd_apply(x, dout, dx, bf16, p.gm_ew, p.vec, p.chunks_ew, epi, w.coef, save_mean, save_w, gamma, beta, st);
     else if (tc) {
       if (int cr = dwt::tc_bwd_apply(x, dout, dx, bf16, nhwc, p.gm, tc_apply_ctas(p.gm, 1, 64), w.coef, save_mean, w.shift, st))
         return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d)", cr);
@@ -589,7 +605,7 @@ int tail2_plan(Plan& p, int kind, bool bf16, const dwt_tail_site* s, const void*
   if (kind != DWT_KIND_WHITEN && kind != DWT_KIND_BN) return fail(DWT_E_INVALID, "bad kind %d", kind);
   if (kind == DWT_KIND_BN && GS != 1) return fail(DWT_E_INVALID, "batch norm has group_size 1 (got %d)", GS);
   if (!s) return fail(DWT_E_INVALID, "null pointer argument");
-  if (int rc = make_plan(p, K_STATS, K_APPLY, s[0].x, s[1].x, out, N, C, HW, GS, D)) return rc;
+  if (int rc = make_plan(p, K_STATS, K_APPLY, s[0].x, s[1].x, out, N, C, HW, GS, D, 4)) return rc;
   if (!dwt::cl_supports((int)C, GS))
     return fail(DWT_E_UNSUPPORTED, "the two-site tail runs on the channels-last kernels: group_size 1, 2, 4 with C/4 a power of two (C=%lld gs=%d)",
                 (long long)C, GS);

@@ -7,6 +7,7 @@
 //   utils/batch_norm.py:66-69        F.batch_norm: biased var normalises, unbiased var -> EMA
 //   backward: closed form of SURVEY.md §8a (autograd through whitening.py:41-55)
 #pragma once
+#include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -74,6 +75,27 @@ __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
+}
+
+// Activation storage of the register-resident kernels (norm_small.cu, norm_cl.cu): float, or __nv_bfloat16
+// (DWT_DTYPE_BF16).  Four consecutive elements are one float4 or 8 bytes of bf16: bf16 widens to fp32 exactly as it
+// loads and rounds to nearest-even as it stores, so everything between a load and a store is the fp32 code.
+__device__ __forceinline__ float4 ldg4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
+__device__ __forceinline__ float4 ld4(const float* p) { return ldg4(p); }
+__device__ __forceinline__ float4 ld4(const __nv_bfloat16* p) {
+  const uint2 u = __ldg(reinterpret_cast<const uint2*>(p));          // bf16 -> fp32 is exact: the high half of the word
+  return make_float4(__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xFFFF0000u), __uint_as_float(u.y << 16),
+                     __uint_as_float(u.y & 0xFFFF0000u));
+}
+__device__ __forceinline__ void st4(float* p, const float4& v) { *reinterpret_cast<float4*>(p) = v; }
+__device__ __forceinline__ void st4(__nv_bfloat16* p, const float4& v) {
+  const __nv_bfloat162 a = __floats2bfloat162_rn(v.x, v.y), b = __floats2bfloat162_rn(v.z, v.w);
+  *reinterpret_cast<uint2*>(p) = make_uint2(*reinterpret_cast<const unsigned*>(&a), *reinterpret_cast<const unsigned*>(&b));
+}
+// one element, widened
+__device__ __forceinline__ float ld1(const float* p) { return __ldg(p); }
+__device__ __forceinline__ float ld1(const __nv_bfloat16* p) {
+  return __uint_as_float((unsigned)__ldg(reinterpret_cast<const unsigned short*>(p)) << 16);
 }
 
 // All threads call. Returns true in every thread of the CTA that arrived last on `counter`

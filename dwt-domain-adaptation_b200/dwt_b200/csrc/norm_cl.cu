@@ -97,23 +97,10 @@ __device__ __forceinline__ void sweep_rows(const ClThread& t, unsigned rows, F&&
 #define CL_FOR_DOMAINS(d, gm, DESC) \
   for (int di_ = blockIdx.z, d = (DESC) ? (gm).D - 1 - di_ : di_; di_ < (gm).D; di_ += gridDim.z, d = (DESC) ? (gm).D - 1 - di_ : di_)
 
-__device__ __forceinline__ float4 ldg4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
-
 // Activation storage T: float, or __nv_bfloat16 (DWT_DTYPE_BF16).  A thread's four channels are one float4 or 8 bytes of
-// bf16: they widen to fp32 as they load and round to nearest-even as they store; everything in between is the fp32 code,
-// on the same schedule, so a bf16 call's sums, statistics and coefficients are those of the fp32 kernels on x.float().
+// bf16 (ld4 / st4, dwt_common.cuh); everything in between is the fp32 code, on the same schedule, so a bf16 call's sums,
+// statistics and coefficients are those of the fp32 kernels on x.float().
 template <class T> constexpr bool kBf16 = !std::is_same<T, float>::value;
-__device__ __forceinline__ float4 ld4(const float* p) { return ldg4(p); }
-__device__ __forceinline__ float4 ld4(const __nv_bfloat16* p) {
-  const uint2 u = __ldg(reinterpret_cast<const uint2*>(p));          // bf16 -> fp32 is exact: the high half of the word
-  return make_float4(__uint_as_float(u.x << 16), __uint_as_float(u.x & 0xFFFF0000u), __uint_as_float(u.y << 16),
-                     __uint_as_float(u.y & 0xFFFF0000u));
-}
-__device__ __forceinline__ void st4(float* p, const float4& v) { *reinterpret_cast<float4*>(p) = v; }
-__device__ __forceinline__ void st4(__nv_bfloat16* p, const float4& v) {
-  const __nv_bfloat162 a = __floats2bfloat162_rn(v.x, v.y), b = __floats2bfloat162_rn(v.z, v.w);
-  *reinterpret_cast<uint2*>(p) = make_uint2(*reinterpret_cast<const unsigned*>(&a), *reinterpret_cast<const unsigned*>(&b));
-}
 // the value as T stores it: v itself in fp32, RN_bf16(v) in bf16
 template <class T>
 __device__ __forceinline__ float as_stored(float v) {

@@ -16,15 +16,17 @@ inline void bind_context() {
 
 // register-resident path, GS in {1,2,4}  (norm_small.cu)
 bool small_supports(int GS);
-void small_stats(const float* x, const Geom& gm, int vec, const FwdFin& fin, float* partial, int* counters,
+// Activation pointers are void: fp32, or bf16 when `bf16` (vec must be 4: HW % 4 == 0, 8-byte-aligned tensors; the fp32
+// plan of the shape, loads widened to fp32, stores rounded to nearest-even).  Statistics and coefficients are fp32.
+void small_stats(const void* x, bool bf16, const Geom& gm, int vec, const FwdFin& fin, float* partial, int* counters,
                  cudaStream_t st);
 void small_eval_prep(const Geom& gm, const FwdFin& fin, cudaStream_t st);
-void small_apply(const float* x, float* y, const Geom& gm, int vec, int chunks, int epi, const float* mean,
-                 const float* w, const float* gamma, const float* beta, const float* residual, cudaStream_t st);
-void small_bwd_reduce(const float* x, const float* dout, const Geom& gm, int vec, const BwdFin& fin,
+void small_apply(const void* x, void* y, bool bf16, const Geom& gm, int vec, int chunks, int epi, const float* mean,
+                 const float* w, const float* gamma, const float* beta, const void* residual, cudaStream_t st);
+void small_bwd_reduce(const void* x, const void* dout, bool bf16, const Geom& gm, int vec, const BwdFin& fin,
                       const float* beta, float* partial, int* counters, cudaStream_t st);
 void small_bwd_prep(const Geom& gm, const BwdFin& fin, cudaStream_t st);
-void small_bwd_apply(const float* x, const float* dout, float* dx, const Geom& gm, int vec, int chunks, int epi,
+void small_bwd_apply(const void* x, const void* dout, void* dx, bool bf16, const Geom& gm, int vec, int chunks, int epi,
                      const float* coef, const float* mean, const float* w, const float* gamma, const float* beta,
                      cudaStream_t st);
 

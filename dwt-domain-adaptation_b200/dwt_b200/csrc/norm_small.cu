@@ -9,6 +9,12 @@
 //   bwd_apply   read x, dout, write dx    dx = A1 dz + Bm x + cvec
 // i.e. 12 B/element forward + 20 B/element backward, the algorithmic minimum of SURVEY.md §8d.
 //
+// Activation storage T: float, or __nv_bfloat16 (DWT_DTYPE_BF16; half the bytes).  A thread's VEC = 4 pixels of one
+// channel row are one float4 or 8 bytes of bf16 (ld4 / st4, dwt_common.cuh); the pilot shift's scalar loads and the
+// residual widen the same way.  Everything between load and store is the fp32 code on the fp32 plan of the shape, so a
+// bf16 call's sums, statistics, W, coefficients, dgamma / dbeta, running buffers and status bits are those of the fp32
+// kernels on x.float(), and y / dx are their outputs rounded to nearest-even.
+//
 // Work decomposition.  A "problem" is one (domain, group).  A CTA of 8 warps serves `ppc`
 // consecutive groups of one domain, 8/ppc warps ("team") per problem, so that sites with
 // thousands of tiny problems (domain BN at 7x7: 6144 problems of 12.5 KB) still run a few
@@ -97,8 +103,8 @@ __device__ __forceinline__ bool team_reduce(const Geom& gm, const Team& tm, int 
 // ------------------------------------------------------------------------------------------
 // stats
 // ------------------------------------------------------------------------------------------
-template <int GS, int VEC>
-__global__ void __launch_bounds__(kThreads, (GS * VEC >= 16) ? 3 : 4) small_stats_kernel(const float* __restrict__ x, const Geom gm,
+template <class T, int GS, int VEC>
+__global__ void __launch_bounds__(kThreads, (GS * VEC >= 16) ? 3 : 4) small_stats_kernel(const T* __restrict__ x, const Geom gm,
                                                                 const FwdFin fin, float* __restrict__ partial,
                                                                 int* counters) {
   constexpr int NM = GS * (GS + 1) / 2, NACC = GS + NM, UNROLL = Unroll<GS, VEC>::stats;
@@ -109,7 +115,7 @@ __global__ void __launch_bounds__(kThreads, (GS * VEC >= 16) ? 3 : 4) small_stat
   const Team tm(gm);
   const int d = blockIdx.z;
   const int g = tm.valid ? tm.g : gm.G - 1;          // out-of-range teams shadow the last group, results dropped
-  const float* xg = x + ((size_t)d * gm.N * gm.C + (size_t)g * GS) * gm.HW;
+  const T* xg = x + ((size_t)d * gm.N * gm.C + (size_t)g * GS) * gm.HW;
   const ItemMap map{(unsigned)(gm.HW / VEC), (unsigned)(gm.C * gm.HW)};
   const unsigned items = (unsigned)gm.N * map.PV, stride = gridDim.x * tm.tthreads;
   unsigned i0 = blockIdx.x * tm.tthreads + tm.ttid;
@@ -125,11 +131,11 @@ __global__ void __launch_bounds__(kThreads, (GS * VEC >= 16) ? 3 : 4) small_stat
     const size_t so = spread_lane ? pilot_spread_offset(tm.ttid, gm.N, gm.HW, (size_t)gm.C * gm.HW) : 0;
 #pragma unroll
     for (int c = 0; c < GS; ++c) {
-      pv[c] = (tm.ttid < 32 && lane < np) ? __ldg(xg + (size_t)c * gm.HW + p0 + lane) : 0.f;
-      ps[c] = spread_lane ? __ldg(xg + (size_t)c * gm.HW + so) : 0.f;
+      pv[c] = (tm.ttid < 32 && lane < np) ? ld1(xg + (size_t)c * gm.HW + p0 + lane) : 0.f;
+      ps[c] = spread_lane ? ld1(xg + (size_t)c * gm.HW + so) : 0.f;
     }
   }
-  float v[UNROLL][GS][VEC];
+  HeldVec<T, VEC> v[UNROLL][GS];        // the next batch stays in flight across the accumulation of this one
   bool have[UNROLL];
   auto load_batch = [&](unsigned base) {
 #pragma unroll
@@ -137,9 +143,9 @@ __global__ void __launch_bounds__(kThreads, (GS * VEC >= 16) ? 3 : 4) small_stat
       const unsigned it = base + u * stride;
       have[u] = it < items;
       if (have[u]) {
-        const float* p = xg + map.offset(it, VEC);
+        const T* p = xg + map.offset(it, VEC);
 #pragma unroll
-        for (int c = 0; c < GS; ++c) load_vec<VEC>(p + (size_t)c * gm.HW, v[u][c]);
+        for (int c = 0; c < GS; ++c) v[u][c].load(p + (size_t)c * gm.HW);
       }
     }
   };
@@ -215,13 +221,13 @@ __global__ void __launch_bounds__(kThreads) small_eval_prep_kernel(const Geom gm
 // ------------------------------------------------------------------------------------------
 // apply
 // ------------------------------------------------------------------------------------------
-template <int GS, int VEC, int EPI>
-__global__ void __launch_bounds__(kThreads, (GS * VEC >= 16) ? 3 : 4) small_apply_kernel(const float* __restrict__ x, float* __restrict__ y,
+template <class T, int GS, int VEC, int EPI>
+__global__ void __launch_bounds__(kThreads, (GS * VEC >= 16) ? 3 : 4) small_apply_kernel(const T* __restrict__ x, T* __restrict__ y,
                                                                 const Geom gm, const float* __restrict__ save_mean,
                                                                 const float* __restrict__ save_w,
                                                                 const float* __restrict__ gamma,
                                                                 const float* __restrict__ beta,
-                                                                const float* __restrict__ res) {
+                                                                const T* __restrict__ res) {
   constexpr bool RES = (EPI & DWT_EPI_RESIDUAL) != 0;
   constexpr int NM = GS * (GS + 1) / 2, UNROLL = RES ? Unroll<GS, VEC>::one : Unroll<GS, VEC>::stats;
   const Team tm(gm);
@@ -231,11 +237,11 @@ __global__ void __launch_bounds__(kThreads, (GS * VEC >= 16) ? 3 : 4) small_appl
   load_forward_map<GS, EPI>(save_w + ((size_t)d * gm.G + g) * GS * GS, save_mean + (size_t)d * gm.C + g * GS,
                             gamma + g * GS, beta + g * GS, Wp, bp);
   const size_t base = ((size_t)d * gm.N * gm.C + (size_t)g * GS) * gm.HW;
-  const float* xg = x + base;
-  float* yg = y + base;
+  const T* xg = x + base;
+  T* yg = y + base;
   const ItemMap map{(unsigned)(gm.HW / VEC), (unsigned)(gm.C * gm.HW)};
   const unsigned items = (unsigned)gm.N * map.PV, stride = gridDim.x * tm.tthreads;
-  const float* rg = res + base;
+  const T* rg = res + base;
   for (unsigned i0 = blockIdx.x * tm.tthreads + tm.ttid; i0 < items; i0 += stride * UNROLL) {
     float v[UNROLL][GS][VEC], rs[RES ? UNROLL : 1][GS][VEC];
     unsigned off[UNROLL];
@@ -279,9 +285,9 @@ __global__ void __launch_bounds__(kThreads, (GS * VEC >= 16) ? 3 : 4) small_appl
 // ------------------------------------------------------------------------------------------
 // backward reduce
 // ------------------------------------------------------------------------------------------
-template <int GS, int VEC, int EPI>
-__global__ void __launch_bounds__(kThreads, 3) small_bwd_reduce_kernel(const float* __restrict__ x,
-                                                                     const float* __restrict__ dout, const Geom gm,
+template <class T, int GS, int VEC, int EPI>
+__global__ void __launch_bounds__(kThreads, 3) small_bwd_reduce_kernel(const T* __restrict__ x,
+                                                                     const T* __restrict__ dout, const Geom gm,
                                                                      const BwdFin fin, const float* __restrict__ beta,
                                                                      float* __restrict__ partial, int* counters) {
   constexpr int NM = GS * (GS + 1) / 2, NACC = GS * GS + GS, UNROLL = Unroll<GS, VEC>::one;
@@ -303,8 +309,8 @@ __global__ void __launch_bounds__(kThreads, 3) small_bwd_reduce_kernel(const flo
 #pragma unroll
   for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
   const size_t base = ((size_t)d * gm.N * gm.C + (size_t)g * GS) * gm.HW;
-  const float* xg = x + base;
-  const float* gg = dout + base;
+  const T* xg = x + base;
+  const T* gg = dout + base;
   const ItemMap map{(unsigned)(gm.HW / VEC), (unsigned)(gm.C * gm.HW)};
   const unsigned items = (unsigned)gm.N * map.PV, stride = gridDim.x * tm.tthreads;
   for (unsigned i0 = blockIdx.x * tm.tthreads + tm.ttid; i0 < items; i0 += stride * UNROLL) {
@@ -377,10 +383,10 @@ __global__ void __launch_bounds__(kThreads) small_bwd_prep_kernel(const Geom gm,
 // ------------------------------------------------------------------------------------------
 // backward apply
 // ------------------------------------------------------------------------------------------
-template <int GS, int VEC, int EPI>
-__global__ void __launch_bounds__(kThreads, 3) small_bwd_apply_kernel(const float* __restrict__ x,
-                                                                    const float* __restrict__ dout,
-                                                                    float* __restrict__ dx, const Geom gm,
+template <class T, int GS, int VEC, int EPI>
+__global__ void __launch_bounds__(kThreads, 3) small_bwd_apply_kernel(const T* __restrict__ x,
+                                                                    const T* __restrict__ dout,
+                                                                    T* __restrict__ dx, const Geom gm,
                                                                     const float* __restrict__ coef,
                                                                     const float* __restrict__ save_mean,
                                                                     const float* __restrict__ save_w,
@@ -408,9 +414,9 @@ __global__ void __launch_bounds__(kThreads, 3) small_bwd_apply_kernel(const floa
     }
   }
   const size_t base = ((size_t)d * gm.N * gm.C + (size_t)g * GS) * gm.HW;
-  const float* xg = x + base;
-  const float* gg = dout + base;
-  float* dg = dx + base;
+  const T* xg = x + base;
+  const T* gg = dout + base;
+  T* dg = dx + base;
   const ItemMap map{(unsigned)(gm.HW / VEC), (unsigned)(gm.C * gm.HW)};
   const unsigned items = (unsigned)gm.N * map.PV, stride = gridDim.x * tm.tthreads;
   for (unsigned i0 = blockIdx.x * tm.tthreads + tm.ttid; i0 < items; i0 += stride * UNROLL) {
@@ -483,47 +489,54 @@ inline dim3 grid_prep(const Geom& gm) { return dim3((gm.G + kThreads - 1) / kThr
   if ((E_) == 3) { constexpr int kEPI = 3; __VA_ARGS__; }                 \
   else if ((E_) == 1) { constexpr int kEPI = 1; __VA_ARGS__; }            \
   else { constexpr int kEPI = 0; __VA_ARGS__; }
+// Activation storage and row vector of a launch: TT = float with VEC 4 or 1, or __nv_bfloat16 with VEC 4 (the C ABI
+// takes bf16 only where the float32 call of the shape has vec == 4, and runs that call's plan)
+#define DWT_DISPATCH_T_VEC(BF16_, V_, ...)                                                \
+  if (BF16_) { using TT = __nv_bfloat16; constexpr int kVEC = 4; __VA_ARGS__; }           \
+  else { using TT = float; DWT_DISPATCH_VEC(V_, __VA_ARGS__); }
+#define DWT_IN(P_) static_cast<const TT*>(P_)
+#define DWT_OUT(P_) static_cast<TT*>(P_)
 
 }  // namespace
 
 bool small_supports(int GS) { return GS == 1 || GS == 2 || GS == 4; }
 
-void small_stats(const float* x, const Geom& gm, int vec, const FwdFin& fin, float* partial, int* counters,
+void small_stats(const void* x, bool bf16, const Geom& gm, int vec, const FwdFin& fin, float* partial, int* counters,
                  cudaStream_t st) {
-  DWT_DISPATCH_GS(gm.GS, DWT_DISPATCH_VEC(vec, (small_stats_kernel<kGS, kVEC><<<grid_of(gm, gm.nchunks), kThreads, 0, st>>>(
-                                                   x, gm, fin, partial, counters))));
+  DWT_DISPATCH_GS(gm.GS, DWT_DISPATCH_T_VEC(bf16, vec, (small_stats_kernel<TT, kGS, kVEC><<<grid_of(gm, gm.nchunks), kThreads, 0, st>>>(
+                                                            DWT_IN(x), gm, fin, partial, counters))));
 }
 
 void small_eval_prep(const Geom& gm, const FwdFin& fin, cudaStream_t st) {
   DWT_DISPATCH_GS(gm.GS, (small_eval_prep_kernel<kGS><<<grid_prep(gm), kThreads, 0, st>>>(gm, fin)));
 }
 
-void small_apply(const float* x, float* y, const Geom& gm, int vec, int chunks, int epi, const float* mean,
-                 const float* w, const float* gamma, const float* beta, const float* residual, cudaStream_t st) {
+void small_apply(const void* x, void* y, bool bf16, const Geom& gm, int vec, int chunks, int epi, const float* mean,
+                 const float* w, const float* gamma, const float* beta, const void* residual, cudaStream_t st) {
   if (epi == 7) {
-    DWT_DISPATCH_GS(gm.GS, DWT_DISPATCH_VEC(vec, (small_apply_kernel<kGS, kVEC, 7><<<grid_of(gm, chunks), kThreads, 0, st>>>(
-                                                     x, y, gm, mean, w, gamma, beta, residual))));
+    DWT_DISPATCH_GS(gm.GS, DWT_DISPATCH_T_VEC(bf16, vec, (small_apply_kernel<TT, kGS, kVEC, 7><<<grid_of(gm, chunks), kThreads, 0, st>>>(
+                                                              DWT_IN(x), DWT_OUT(y), gm, mean, w, gamma, beta, DWT_IN(residual)))));
     return;
   }
-  DWT_DISPATCH_GS(gm.GS, DWT_DISPATCH_VEC(vec, DWT_DISPATCH_EPI(epi, (small_apply_kernel<kGS, kVEC, kEPI><<<grid_of(gm, chunks), kThreads, 0, st>>>(
-                                                                         x, y, gm, mean, w, gamma, beta, nullptr)))));
+  DWT_DISPATCH_GS(gm.GS, DWT_DISPATCH_T_VEC(bf16, vec, DWT_DISPATCH_EPI(epi, (small_apply_kernel<TT, kGS, kVEC, kEPI><<<grid_of(gm, chunks), kThreads, 0, st>>>(
+                                                                                  DWT_IN(x), DWT_OUT(y), gm, mean, w, gamma, beta, nullptr)))));
 }
 
-void small_bwd_reduce(const float* x, const float* dout, const Geom& gm, int vec, const BwdFin& fin,
+void small_bwd_reduce(const void* x, const void* dout, bool bf16, const Geom& gm, int vec, const BwdFin& fin,
                       const float* beta, float* partial, int* counters, cudaStream_t st) {
-  DWT_DISPATCH_GS(gm.GS, DWT_DISPATCH_VEC(vec, DWT_DISPATCH_EPI(fin.epi, (small_bwd_reduce_kernel<kGS, kVEC, kEPI><<<grid_of(gm, gm.nchunks), kThreads, 0, st>>>(
-                                                                             x, dout, gm, fin, beta, partial, counters)))));
+  DWT_DISPATCH_GS(gm.GS, DWT_DISPATCH_T_VEC(bf16, vec, DWT_DISPATCH_EPI(fin.epi, (small_bwd_reduce_kernel<TT, kGS, kVEC, kEPI><<<grid_of(gm, gm.nchunks), kThreads, 0, st>>>(
+                                                                                      DWT_IN(x), DWT_IN(dout), gm, fin, beta, partial, counters)))));
 }
 
 void small_bwd_prep(const Geom& gm, const BwdFin& fin, cudaStream_t st) {
   DWT_DISPATCH_GS(gm.GS, (small_bwd_prep_kernel<kGS><<<grid_prep(gm), kThreads, 0, st>>>(gm, fin)));
 }
 
-void small_bwd_apply(const float* x, const float* dout, float* dx, const Geom& gm, int vec, int chunks, int epi,
+void small_bwd_apply(const void* x, const void* dout, void* dx, bool bf16, const Geom& gm, int vec, int chunks, int epi,
                      const float* coef, const float* mean, const float* w, const float* gamma, const float* beta,
                      cudaStream_t st) {
-  DWT_DISPATCH_GS(gm.GS, DWT_DISPATCH_VEC(vec, DWT_DISPATCH_EPI(epi, (small_bwd_apply_kernel<kGS, kVEC, kEPI><<<grid_of(gm, chunks), kThreads, 0, st>>>(
-                                                                         x, dout, dx, gm, coef, mean, w, gamma, beta)))));
+  DWT_DISPATCH_GS(gm.GS, DWT_DISPATCH_T_VEC(bf16, vec, DWT_DISPATCH_EPI(epi, (small_bwd_apply_kernel<TT, kGS, kVEC, kEPI><<<grid_of(gm, chunks), kThreads, 0, st>>>(
+                                                                                  DWT_IN(x), DWT_IN(dout), DWT_OUT(dx), gm, coef, mean, w, gamma, beta)))));
 }
 
 }  // namespace dwt

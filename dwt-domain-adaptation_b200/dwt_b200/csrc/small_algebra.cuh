@@ -1,5 +1,5 @@
 // Thread-level building blocks shared by the register-resident kernels of both memory layouts
-// (norm_small.cu: NCHW, norm_cl.cu: channels-last): vector loads, the group's forward map, and the
+// (norm_small.cu: NCHW, norm_cl.cu: channels-last): vector loads (fp32, or bf16 widened), the group's forward map, and the
 // single-thread dense algebra for group sizes <= 4 (Cholesky, triangular inverse, EMA, backward
 // coefficients), everything in registers.
 #pragma once
@@ -25,6 +25,35 @@ __device__ __forceinline__ void store_vec(float* p, const float (&v)[VEC]) {
     *p = v[0];
   }
 }
+// bf16 activations: 8-byte vectors only (the C ABI takes NCHW bf16 at HW % 4 == 0 with 8-byte-aligned tensors)
+template <int VEC>
+__device__ __forceinline__ void load_vec(const __nv_bfloat16* p, float (&v)[VEC]) {
+  static_assert(VEC == 4, "bf16 rows are read as 8-byte vectors");
+  const float4 t = ld4(p);
+  v[0] = t.x; v[1] = t.y; v[2] = t.z; v[3] = t.w;
+}
+template <int VEC>
+__device__ __forceinline__ void store_vec(__nv_bfloat16* p, const float (&v)[VEC]) {
+  static_assert(VEC == 4, "bf16 rows are written as 8-byte vectors");
+  st4(p, make_float4(v[0], v[1], v[2], v[3]));
+}
+
+// VEC elements of one row held in registers from their load to their use: fp32 values, or the 8 loaded bytes of bf16,
+// widened (exactly) where each value is read -- a prefetched bf16 batch then takes the registers of its bytes
+template <class T, int VEC> struct HeldVec {
+  float v[VEC];
+  __device__ __forceinline__ void load(const float* p) { load_vec<VEC>(p, v); }
+  __device__ __forceinline__ float operator[](int e) const { return v[e]; }
+};
+template <int VEC> struct HeldVec<__nv_bfloat16, VEC> {
+  static_assert(VEC == 4, "bf16 rows are read as 8-byte vectors");
+  uint2 u;
+  __device__ __forceinline__ void load(const __nv_bfloat16* p) { u = __ldg(reinterpret_cast<const uint2*>(p)); }
+  __device__ __forceinline__ float operator[](int e) const {
+    const unsigned w = e < 2 ? u.x : u.y;
+    return __uint_as_float((e & 1) ? (w & 0xFFFF0000u) : (w << 16));
+  }
+};
 
 // out_c = bp_c + sum_{j<=c} Wp[c][j] x_j : W is lower-triangular (Cholesky basis, SURVEY H1).
 // One fixed FMA order, shared by forward apply and the backward's ReLU-mask recompute so

@@ -6,9 +6,9 @@ centred copy, a transposed copy or the covariance graph the reference's autograd
 
 Activations are float32 or bfloat16 (what torch.autocast(dtype=torch.bfloat16) hands over from a convolution): a bf16
 call whose activations are all bf16 runs the bf16 kernels (DWT_DTYPE_BF16) when it is channels-last on a channels-last
-geometry (group sizes 1, 2, 4) or on a channels-last tensor-core geometry (_nhwc_tensor_core), or NCHW whitening on a
-tensor-core geometry (_bf16_tensor_core); any other bf16 call runs
-the float32 kernels on upcast copies and casts the result back.  Statistics, parameters, their gradients and the running
+geometry (group sizes 1, 2, 4) or on a channels-last tensor-core geometry (_nhwc_tensor_core), NCHW whitening at group
+sizes 1, 2, 4 or NCHW batch norm with HW % 4 == 0 (_bf16_small), or NCHW whitening on a tensor-core geometry
+(_bf16_tensor_core); any other bf16 call runs the float32 kernels on upcast copies and casts the result back.  Statistics, parameters, their gradients and the running
 buffers are float32 either way, like nn.BatchNorm2d under autocast.
 """
 from __future__ import annotations
@@ -56,6 +56,17 @@ def _bf16_tensor_core(x, kind, group_size, n_domains, residual):
     return nv.tensor_core_bf16_supported(n, c, hw, group_size) and (not x.is_contiguous() or x.data_ptr() % 16 == 0)
 
 
+def _bf16_small(x, group_size, residual):
+    """A bf16 NCHW call the register-resident kernels take in bf16 (nv.small_bf16_supported: whitening at group sizes
+    1, 2, 4 or batch norm, HW % 4 == 0): x and the residual bf16 and 8-byte aligned, or non-contiguous (then copied
+    into a fresh, aligned tensor by _dense / _NormFunction.forward)."""
+    hw = 1
+    for s in x.shape[2:]:
+        hw *= s
+    return nv.small_bf16_supported(hw, group_size) and all(
+        t.dtype == torch.bfloat16 and (not t.is_contiguous() or t.data_ptr() % 8 == 0) for t in (x, residual) if t is not None)
+
+
 def _check_param(name, t, numel):
     """The C ABI takes raw pointers: a strided or mis-sized statistics / affine tensor would be read or written out
     of bounds on the device, where the reference raises a shape error.  Validate before taking data_ptr()."""
@@ -82,9 +93,10 @@ class _NormFunction(torch.autograd.Function):
         x, n_all, c, hw, nhwc = _dense(x, gs, n_domains)
         bf16 = x.dtype == torch.bfloat16
         if bf16 and not ((nhwc and (residual is None or residual.dtype == x.dtype))
-                         or (not nhwc and _bf16_tensor_core(x, kind, gs, n_domains, residual))):
-            raise nv.NativeError("bfloat16 runs on the channels-last kernels with every activation in bfloat16, or on the "
-                                 "NCHW tensor-core whitening kernels (norm() upcasts anything else)")
+                         or (not nhwc and (_bf16_small(x, gs, residual) or _bf16_tensor_core(x, kind, gs, n_domains, residual)))):
+            raise nv.NativeError("bfloat16 runs on the channels-last kernels and the NCHW kernels of group sizes 1, 2, 4 "
+                                 "(HW % 4 == 0) with every activation in bfloat16, or on the NCHW tensor-core whitening "
+                                 "kernels (norm() upcasts anything else)")
         layout = (nv.LAYOUT_NHWC if nhwc else 0) | (nv.DTYPE_BF16 if bf16 else 0)
         if n_all % n_domains != 0:
             raise ValueError(f"batch of {n_all} does not split into {n_domains} domains")
@@ -181,8 +193,10 @@ class _NormFunction(torch.autograd.Function):
                                       and dout2.is_contiguous(memory_format=torch.channels_last)):
             dout, dout2 = dout + dout2, None
         dout = dout.contiguous(memory_format=torch.channels_last) if nhwc else dout.contiguous()
-        if ((mode & nv.DTYPE_BF16) or nhwc) and not cl_kernels and dout.data_ptr() % 16:
-            # the forward ran the tensor-core kernels: their TMA loads need 16 bytes (a fresh tensor keeps the layout)
+        # the forward ran the tensor-core kernels, whose TMA loads need 16 bytes, or (bf16 NCHW, group sizes 1, 2, 4) the
+        # register-resident kernels, whose bf16 loads need 8: copy a misaligned dout (a fresh tensor keeps the layout)
+        align = 8 if not nhwc and gs in (1, 2, 4) else 16
+        if ((mode & nv.DTYPE_BF16) or nhwc) and not cl_kernels and dout.data_ptr() % align:
             dout = dout.clone(memory_format=torch.channels_last if nhwc else torch.contiguous_format)
         dev = nv.require_cuda(dout, bf16=True)
         dx = torch.empty_like(x)                     # x's layout: channels-last when the forward ran NHWC
@@ -355,11 +369,12 @@ def norm(x, gamma, beta, *, kind, group_size, n_domains, training_stats, eps, mo
         cl = x.dim() == 4 and not x.is_contiguous() and x.is_contiguous(memory_format=torch.channels_last)
         cl_tc = kind == "whiten" and residual is None and _nhwc_tensor_core(x, gs, n_domains)
         bf16_kernels = dtypes == {torch.bfloat16} and (
-            (nv.channels_last_supported(x.shape[1], gs) or cl_tc) if cl else _bf16_tensor_core(x, kind, gs, n_domains, residual))
+            (nv.channels_last_supported(x.shape[1], gs) or cl_tc) if cl
+            else _bf16_small(x, gs, residual) or _bf16_tensor_core(x, kind, gs, n_domains, residual))
         if not bf16_kernels:
-            # NCHW group sizes 1, 2, 4, geometries and alignments the bf16 kernels lack, or mixed dtypes: the float32
-            # kernels on upcast copies, the result (and through autograd every gradient of x and the residual) back in
-            # x's dtype
+            # geometries and alignments the bf16 kernels lack (NCHW HW % 4 != 0, BatchNorm1d on [N, C], a misaligned
+            # view, ...) or mixed dtypes: the float32 kernels on upcast copies, the result (and through autograd every
+            # gradient of x and the residual) back in x's dtype
             y = _NormFunction.apply(x.float(), gamma, beta, None if residual is None else residual.float(), *args)
             return y.to(x.dtype)
     return _NormFunction.apply(x, gamma, beta, residual, *args)

@@ -46,7 +46,7 @@
 extern "C" {
 #endif
 
-#define DWT_B200_ABI_VERSION 9
+#define DWT_B200_ABI_VERSION 10
 #define DWT_MAX_DOMAINS 4
 #define DWT_MAX_GROUP_SIZE 64
 
@@ -76,14 +76,17 @@ extern "C" {
 /* activation storage, OR-ed into `mode` (dwt_whiten_*, dwt_bn_*), `kind` (dwt_tail2_*) or `flags` (dwt_maxpool_*):
  * default = fp32; DWT_DTYPE_BF16 = every ACTIVATION pointer of the call points at bfloat16 -- x, y, residual, dout,
  * dout2, dx, dresidual / dz, dwt_tail_site.x / .dx, and the max-pool's x, y, dy, dx.  Running buffers, gamma / beta and
- * their gradients, save_mean / save_w and the workspace stay fp32.  Built for two kernel families:
+ * their gradients, save_mean / save_w and the workspace stay fp32.  Built for three kernel families:
  *   - channels-last (DWT_LAYOUT_NHWC; the tail and the max-pool are channels-last anyway), group size 1, 2, 4 with C/4
  *     a power of two; bf16 tensors 8-byte aligned;
+ *   - NCHW whitening at group size 1, 2, 4 and NCHW batch norm (dwt_whiten_*, dwt_bn_*; every mode and epilogue) with
+ *     HW % 4 == 0; x, y, residual, dout and dx 8-byte aligned; no dout2 (DWT_E_UNSUPPORTED, as in fp32 NCHW);
  *   - whitening on the tensor-core kernels: group size 8, 16, 32, 64, HW >= 32, N*HW >= 4096 per domain; NCHW with
  *     HW % 8 == 0 and x and dout 16-byte aligned (TMA), or channels-last with HW % 4 == 0 and x, y, dout, dx 16-byte
  *     aligned (see DWT_LAYOUT_NHWC).
- * Any other geometry is DWT_E_UNSUPPORTED (NCHW group sizes 1, 2, 4 and batch norm included); a misaligned tensor is
- * DWT_E_INVALID.  bf16 launches report in the profile as <family>_bf16 and count 2 bytes per activation element.
+ * Any other geometry is DWT_E_UNSUPPORTED (NCHW group sizes 1, 2, 4 and batch norm at HW % 4 != 0 included); a
+ * misaligned tensor is DWT_E_INVALID.  bf16 launches report in the profile as <family>_bf16 and count 2 bytes per
+ * activation element.
  * The kernels run the fp32 schedule of the same shape: loads widen to fp32, stores round to nearest-even, so statistics,
  * running-buffer updates, dgamma / dbeta and status bits are bit for bit those of the fp32 call on the widened inputs,
  * and every bf16 output is that call's fp32 output rounded.  Two things are rounded where a bf16 caller would round
