@@ -17,6 +17,7 @@ LIB_PATH = os.environ.get("DWT_B200_LIB") or os.path.join(_HERE, "lib", "libdwt_
 ABI_VERSION = 10
 MAX_DOMAINS = 4
 MAX_GROUP_SIZE = 64
+TC_MAX_GROUP_SIZE = 128            # the one wider group size: fp32 whitening on the tensor-core kernels only
 MODE_TRAIN, MODE_EVAL = 0, 1
 EPI_NONE, EPI_AFFINE, EPI_RELU, EPI_RESIDUAL = 0, 1, 2, 4
 LAYOUT_NHWC = 0x100
@@ -168,10 +169,10 @@ def tensor_core_bf16_supported(n: int, channels: int, hw: int, group_size: int) 
 
 def tensor_core_nhwc_supported(n: int, channels: int, hw: int, group_size: int) -> bool:
     """Mirror of the C ABI's channels-last tensor-core rule (csrc/api.cu, tc_nhwc_supports): whitening at group sizes
-    8..64 dividing 64 runs on channels-last tensors when HW >= 32 and a multiple of 4 and there are at least 4096
-    samples per domain (n = images per domain), fp32 and bf16 alike.  The tensors also need a 16-byte-aligned
-    data_ptr()."""
-    return (group_size in (8, 16, 32, 64) and channels % group_size == 0 and hw >= 32 and hw % 4 == 0
+    8..64 dividing 64, and 128, runs on channels-last tensors when HW >= 32 and a multiple of 4 and there are at least
+    4096 samples per domain (n = images per domain); fp32 and bf16 alike up to 64, fp32 only at 128 (bf16 upcasts).
+    The tensors also need a 16-byte-aligned data_ptr()."""
+    return (group_size in (8, 16, 32, 64, TC_MAX_GROUP_SIZE) and channels % group_size == 0 and hw >= 32 and hw % 4 == 0
             and n * hw >= 4096)
 
 
@@ -219,6 +220,8 @@ _workspaces: dict = {}
 
 
 def workspace(device, n, c, hw, gs, nd):
+    if gs == TC_MAX_GROUP_SIZE and c % gs == 0:
+        c, gs = 2 * c, MAX_GROUP_SIZE                # dwt_b200.h: the group-size-64 query on 2C channels covers it
     need = lib().dwt_workspace_bytes(n, c, hw, gs, nd)
     if need == 0:
         raise NativeError(f"invalid geometry for workspace: C={c} group_size={gs} domains={nd}")

@@ -97,13 +97,19 @@ int ensure_tc() {
   return g_tc_rc;
 }
 
-// CTAs per (domain, super-block) of the tensor-core contraction: one full wave of 2 CTAs per SM
-int tc_chunks(const dwt::Geom& g) {
-  const int problems = dwt::tc_superblocks(g) * g.D;
+// CTAs per problem of a tensor-core contraction: one full wave of 2 CTAs per SM.  Problems: (domain, super-block);
+// at group size 128 also (domain, group) of the off-diagonal Gram block and (domain, block of R), see tc_pair_chunks
+int tc_chunks(const dwt::Geom& g, int problems = 0) {
+  if (problems == 0) problems = dwt::tc_superblocks(g) * g.D;
   int n = 2 * sm_count() / problems;
   const int64_t tiles = (int64_t)g.N * ((g.HW + 31) / 32);
   if (n > tiles) n = (int)tiles;
   return n < 1 ? 1 : n;
+}
+// group size 128: the forward's off-diagonal Gram blocks (SB/2 per domain) and the backward's four blocks of R per group
+int tc_pair_chunks(const dwt::Geom& g, bool bwd) {
+  const int SB = dwt::tc_superblocks(g);
+  return tc_chunks(g, (bwd ? 2 * SB : SB / 2) * g.D);
 }
 
 // persistent CTAs per (domain, super-block) of the tensor-core apply kernels: per_sm CTAs per SM
@@ -215,10 +221,20 @@ Workspace carve(void* base, int64_t C, int GS, int D, size_t start = kOffScratch
   w.counters = reinterpret_cast<int*>(b + kOffCounters);
   w.dom_counter = reinterpret_cast<int*>(b + kOffDom1);
   w.dom_counter2 = reinterpret_cast<int*>(b + kOffDom2);
-  size_t partial_floats = (size_t)D * G * cap * (GS * GS + GS);
+  const bool gs128 = GS == DWT_TC_MAX_GROUP_SIZE;         // tensor-core kernels only: no tiled partials
+  size_t partial_floats = gs128 ? 0 : (size_t)D * G * cap * (GS * GS + GS);
   if (GS >= 8 && 64 % GS == 0) {                           // tensor-core contraction: per super-block partials
     const size_t tc = ((size_t)2 * sm_count() + (size_t)((C + 63) / 64) * D) * (64 * 64 + 64);
     if (tc > partial_floats) partial_floats = tc;
+  }
+  if (gs128) {
+    // tc_chunks(g, problems) * problems <= max(2 SMs, problems).  Forward: SB diagonal blocks, then SB/2 off-diagonal
+    // blocks behind them; backward: 2 SB blocks of R -- per domain.  This stays within the partials of the group-size-64
+    // call on 2C channels, whose workspace therefore covers this one (dwt_workspace_bytes, dwt_b200.h).
+    const size_t S2 = (size_t)2 * sm_count(), P = (size_t)(C / 64) * D;
+    auto wave = [&](size_t problems) { return problems > S2 ? problems : S2; };
+    const size_t fwd = wave(P) + wave(P / 2), bwd = wave(2 * P);
+    partial_floats = (fwd > bwd ? fwd : bwd) * (64 * 64 + 64);
   }
   size_t red_floats = 1;
   if (dwt::cl_supports((int)C, GS)) {                      // channels-last path: per-CTA rows of C/4-column vectors
@@ -234,7 +250,8 @@ Workspace carve(void* base, int64_t C, int GS, int D, size_t start = kOffScratch
   w.coef = reinterpret_cast<float*>(b + take(sizeof(float) * (size_t)D * G * dwt::coef_stride(GS)));
   w.dgb_part = reinterpret_cast<float*>(b + take(sizeof(float) * (size_t)D * 2 * C));
   const size_t SBn = (size_t)((C + 63) / 64);
-  w.gram = reinterpret_cast<float*>(b + take(sizeof(float) * (size_t)D * SBn * (64 * 64 + 64)));
+  // group size 128: forward SB diagonal + SB/2 off-diagonal blocks, backward 2 SB blocks of R, per domain
+  w.gram = reinterpret_cast<float*>(b + take(sizeof(float) * (size_t)D * (gs128 ? 2 : 1) * SBn * (64 * 64 + 64)));
   w.shift = reinterpret_cast<float*>(b + take(sizeof(float) * (size_t)D * SBn * 64));
   w.bad = reinterpret_cast<int*>(b + take(sizeof(int) * (size_t)D * G));
   w.bytes = off;
@@ -275,8 +292,8 @@ int make_plan(Plan& p, KernelKind reduce_kind, KernelKind ew_kind, const void* a
               int64_t N, int64_t C, int64_t HW, int GS, int D, int elem_bytes) {
   if (N <= 0 || C <= 0 || HW <= 0) return fail(DWT_E_INVALID, "empty tensor (N=%lld C=%lld HW=%lld)", (long long)N,
                                                (long long)C, (long long)HW);
-  if (GS < 1 || GS > DWT_MAX_GROUP_SIZE) return fail(DWT_E_UNSUPPORTED, "group_size %d outside [1,%d]", GS,
-                                                     DWT_MAX_GROUP_SIZE);
+  if (GS < 1 || (GS > DWT_MAX_GROUP_SIZE && GS != DWT_TC_MAX_GROUP_SIZE))
+    return fail(DWT_E_UNSUPPORTED, "group_size %d outside [1,%d] and not %d", GS, DWT_MAX_GROUP_SIZE, DWT_TC_MAX_GROUP_SIZE);
   if (C % GS != 0) return fail(DWT_E_INVALID, "channels %lld not divisible by group_size %d", (long long)C, GS);
   if (D < 1 || D > DWT_MAX_DOMAINS) return fail(DWT_E_INVALID, "n_domains %d outside [1,%d]", D, DWT_MAX_DOMAINS);
   if (N * C * HW >= (int64_t)1 << 31 || C / GS > 65535)
@@ -329,13 +346,23 @@ int check_tc_bf16_align(bool bf16, bool nhwc, uintptr_t bits, const char* what) 
 // every bf16 NCHW call of group size 8..64 and channels-last call routed to it (validated above: there is no other
 // kernel to fall back to)
 int tc_route(bool bf16, bool nhwc, const Plan& p, bool* tc) {
-  if (!p.small && (bf16 || nhwc)) {
+  if (!p.small && (bf16 || nhwc || p.gm.GS > DWT_MAX_GROUP_SIZE)) {
     if (ensure_tc() != 0) return fail(DWT_E_LAUNCH, "tensor-core kernel set-up failed (%d)", g_tc_rc);
     *tc = true;
   } else {
     *tc = !p.small && dwt::tc_supports(p.gm, p.vec) && ensure_tc() == 0;
   }
   return DWT_OK;
+}
+// group size 128 runs on the tensor-core kernels only (no tiled kernel is that wide), in fp32: below their geometry,
+// or in bf16, the call is refused rather than sent elsewhere
+int check_gs128(bool bf16, bool nhwc, const Plan& p) {
+  const dwt::Geom& g = p.gm;
+  if (g.GS != DWT_TC_MAX_GROUP_SIZE) return DWT_OK;
+  if (bf16) return fail(DWT_E_UNSUPPORTED, "group_size 128 is built for fp32 activations (C=%d HW=%d N=%d)", g.C, g.HW, g.N);
+  if (nhwc ? tc_nhwc_supports(g) : dwt::tc_supports(g, p.vec)) return DWT_OK;
+  return fail(DWT_E_UNSUPPORTED, "group_size 128 runs on the tensor-core kernels only: HW >= 32 and a multiple of 4, "
+              "N*HW >= 4096 per domain, NCHW tensors 16-byte aligned (C=%d HW=%d N=%d)", g.C, g.HW, g.N);
 }
 int check_tc_nhwc_align(uintptr_t bits, const char* what) {
   if (bits % 16 == 0) return DWT_OK;
@@ -400,6 +427,7 @@ int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, 
   Plan p;
   if (int rc = make_plan(p, K_STATS, K_APPLY, x, y, nullptr, N, C, HW, GS, D, bf16 && !nhwc ? 2 : 4)) return rc;
   if (!x || !y || !save_mean || !save_w || !ws) return fail(DWT_E_INVALID, "null pointer argument");
+  if (int rc = check_gs128(bf16, nhwc, p)) return rc;
   if (int rc = check_bf16_geometry(bf16, nhwc, p.gm)) return rc;
   const bool nhwc_tc = nhwc && tc_nhwc_supports(p.gm);
   if (nhwc && !nhwc_tc && !dwt::cl_supports((int)C, GS)) return fail_nhwc_geometry(p.gm);
@@ -454,12 +482,17 @@ int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, 
   }
   bool tc = false;
   if (int rc = tc_route(bf16, nhwc, p, &tc)) return rc;
+  const bool gs128 = GS == DWT_TC_MAX_GROUP_SIZE;
+  const size_t pair_part = (size_t)tc_chunks(p.gm) * dwt::tc_superblocks(p.gm) * D * (64 * 64 + 64);   // behind the diagonal partials
   if (mode == DWT_MODE_TRAIN) {
     Launch l(p.small ? fam(bf16, "small_stats", "small_stats_bf16") : (tc ? tc_fam(bf16, nhwc, "tc_stats", "tc_stats_bf16", "tc_stats_nhwc", "tc_stats_nhwc_bf16") : "tiled_stats"), &p.gm, E, st);
     if (p.small) dwt::small_stats(x, bf16, p.gm, p.vec, fin, w.partial, w.counters, st);
     else if (tc) {
-      if (int cr = dwt::tc_stats(x, bf16, nhwc, p.gm, tc_chunks(p.gm), w.shift, w.partial, st))
-        return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d) x=%p N=%d C=%d HW=%d D=%d", cr, (const void*)x, p.gm.N, p.gm.C, p.gm.HW, p.gm.D);
+      int cr = dwt::tc_stats(x, bf16, nhwc, p.gm, tc_chunks(p.gm), w.shift, w.partial, st);
+      // group size 128: the off-diagonal blocks behind the diagonal ones (a second read of x, counted once above)
+      if (cr == 0 && gs128)
+        cr = dwt::tc_gram_pair(x, nhwc, p.gm, tc_pair_chunks(p.gm, false), w.shift, w.partial + pair_part, st);
+      if (cr) return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d) x=%p N=%d C=%d HW=%d D=%d", cr, (const void*)x, p.gm.N, p.gm.C, p.gm.HW, p.gm.D);
     } else dwt::tiled_stats(x, p.gm, p.vec, fin, w.partial, w.counters, st);
   } else {
     Launch l(fam(bf16, "eval_prep", "eval_prep_bf16"), &p.gm, 0.0, st);
@@ -471,6 +504,9 @@ int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, 
     if (int rc = check_launch("tensor-core statistics kernel")) return rc;
     Launch l(fam(bf16, "dense_fwd_finalize", "dense_fwd_finalize_bf16"), &p.gm, 0.0, st);
     dwt::dense_partial_reduce(w.partial, tc_chunks(p.gm), dwt::tc_superblocks(p.gm) * D, w.gram, st);
+    if (gs128)
+      dwt::dense_partial_reduce(w.partial + pair_part, tc_pair_chunks(p.gm, false), dwt::tc_superblocks(p.gm) / 2 * D,
+                                w.gram + (size_t)dwt::tc_superblocks(p.gm) * D * (64 * 64 + 64), st);
     dwt::dense_fwd_factor(w.gram, w.shift, p.gm, fin, st);
   }
   if (int rc = check_launch("whitening statistics kernel")) return rc;
@@ -495,6 +531,7 @@ int whiten_like_bwd(const float* x, const float* dout, const float* dout2, float
   Plan p;
   if (int rc = make_plan(p, K_BWD_REDUCE, K_BWD_APPLY, x, dout, dx, N, C, HW, GS, D, bf16 && !nhwc ? 2 : 4)) return rc;
   if (!x || !dout || !dx || !save_mean || !save_w || !ws) return fail(DWT_E_INVALID, "null pointer argument");
+  if (int rc = check_gs128(bf16, nhwc, p)) return rc;
   if (int rc = check_bf16_geometry(bf16, nhwc, p.gm)) return rc;
   const bool nhwc_tc = nhwc && tc_nhwc_supports(p.gm);
   if (dout2 && (!nhwc || nhwc_tc || (uintptr_t)dout2 % (bf16 ? 8 : 16) != 0))
@@ -559,11 +596,15 @@ int whiten_like_bwd(const float* x, const float* dout, const float* dout2, float
   }
   bool tc = false;
   if (int rc = tc_route(bf16, nhwc, p, &tc)) return rc;
+  // group size 128: four blocks of R per group, 2 SB problems per domain
+  const bool gs128 = GS == DWT_TC_MAX_GROUP_SIZE;
+  const int rchunks = gs128 ? tc_pair_chunks(p.gm, true) : tc_chunks(p.gm);
+  const int rproblems = (gs128 ? 2 : 1) * dwt::tc_superblocks(p.gm) * D;
   if (need_reduce) {
     Launch l(p.small ? fam(bf16, "small_bwd_reduce", "small_bwd_reduce_bf16") : (tc ? tc_fam(bf16, nhwc, "tc_bwd_reduce", "tc_bwd_reduce_bf16", "tc_bwd_reduce_nhwc", "tc_bwd_reduce_nhwc_bf16") : "tiled_bwd_reduce"), &p.gm, 2 * E, st);
     if (p.small) dwt::small_bwd_reduce(x, dout, bf16, p.gm, p.vec, fin, beta, w.partial, w.counters, st);
     else if (tc) {
-      if (int cr = dwt::tc_bwd_reduce(x, dout, bf16, nhwc, p.gm, tc_chunks(p.gm), save_mean, w.partial, st))
+      if (int cr = dwt::tc_bwd_reduce(x, dout, bf16, nhwc, p.gm, rchunks, save_mean, w.partial, st))
         return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d) x=%p dout=%p N=%d C=%d HW=%d D=%d", cr, (const void*)x, (const void*)dout, p.gm.N, p.gm.C, p.gm.HW, p.gm.D);
     } else dwt::tiled_bwd_reduce(x, dout, p.gm, p.vec, fin, w.partial, w.counters, st);
   } else {
@@ -575,7 +616,7 @@ int whiten_like_bwd(const float* x, const float* dout, const float* dout2, float
   if (tc && need_reduce) {
     if (int rc = check_launch("tensor-core backward reduction kernel")) return rc;
     Launch l(fam(bf16, "dense_bwd_finalize", "dense_bwd_finalize_bf16"), &p.gm, 0.0, st);
-    dwt::dense_partial_reduce(w.partial, tc_chunks(p.gm), dwt::tc_superblocks(p.gm) * D, w.gram, st);
+    dwt::dense_partial_reduce(w.partial, rchunks, rproblems, w.gram, st);
     dwt::dense_bwd_coef(w.gram, p.gm, fin, w.shift, st);
   }
   if (int rc = check_launch("whitening backward reduction kernel")) return rc;
@@ -710,6 +751,7 @@ const char* dwt_last_error(void) { return g_err; }
 
 size_t dwt_workspace_bytes(int64_t N, int64_t C, int64_t HW, int group_size, int n_domains) {
   (void)N; (void)HW;
+  // group size 128 is sized by the group-size-64 query on 2C channels (dwt_b200.h): this query keeps its range
   if (C <= 0 || group_size < 1 || group_size > DWT_MAX_GROUP_SIZE || C % group_size != 0 || n_domains < 1 ||
       n_domains > DWT_MAX_DOMAINS)
     return 0;

@@ -13,6 +13,9 @@
 // right-looking sweep of 16 panel steps (one block barrier each): the matrices live in registers, shared
 // memory only carries the 4-column panel of L and the 4-row panel of W of the current step.
 //
+// Group size 128 runs fwd_factor128 / bwd_coef128 (one 1024-thread CTA per group on the generic shared-memory routines
+// of dwt_common.cuh); partial_reduce serves it unchanged (its problems are 64 x 64 blocks).
+//
 // Reference: utils/whitening.py:47-53,57-59 (/root/reference); backward: SURVEY.md §8a.
 #ifdef DWT_PROF_DENSE
 #include <cstdio>
@@ -438,6 +441,100 @@ __global__ void __launch_bounds__(256) bwd_coef_kernel(const float* __restrict__
   PROF_DUMP("bwd_coef load|mm1|mm2|mm3|tail");
 }
 
+// ------------------------------------------------------------------------------------------
+// group size 128: one 1024-thread CTA per group runs the shared-memory routines of dwt_common.cuh (fwd_factor_block:
+// right-looking Cholesky + forward-substitution inverse; bwd_finalize_block: P, T = W^T P, S' = T W, A1, Bm) on the
+// whole 128 x 128 matrix, assembled from the 64 x 64 blocks the tensor-core contractions reduced.  Three matrices of
+// 128 x 129 floats: 194 KB of shared memory.
+// ------------------------------------------------------------------------------------------
+constexpr int kGS2 = 2 * kSB, kLD2 = kGS2 + 1, kMat2 = kGS2 * kLD2;
+constexpr int kThreads2 = 1024;
+constexpr size_t kFactor2Smem = sizeof(float) * (3 * kMat2 + kGS2);
+constexpr size_t kCoef2Smem = sizeof(float) * (3 * kMat2 + 3 * kGS2);
+
+// fwd_factor at 128: grid (G), domains in order (EMA sequence).  gram [D][SB][kNacc] holds the diagonal blocks and the
+// row sums (super-blocks 2g, 2g + 1), goff [D][SB/2][kNacc] the off-diagonal block G10 of group g; null: eval.
+__global__ void __launch_bounds__(kThreads2) fwd_factor128_kernel(const float* __restrict__ gram, const float* __restrict__ goff,
+                                                                  const float* __restrict__ shift, const Geom gm, const FwdFin f) {
+  extern __shared__ __align__(16) float dsm2[];
+  float* sCov = dsm2;
+  float* sL = sCov + kMat2;
+  float* sW = sL + kMat2;
+  float* sMean = sW + kMat2;
+  __shared__ float sRow[kGS2];
+  const int g = blockIdx.x, tid = threadIdx.x, SB = gm.C / kSB;
+  const float invM = 1.f / gm.M;
+  for (int d = 0; d < gm.D; ++d) {
+    const float* Gd = gram ? gram + ((size_t)d * SB + 2 * g) * kNacc : nullptr;
+    const float* Go = gram ? goff + ((size_t)d * (SB / 2) + g) * kNacc : nullptr;
+    if (tid < kGS2) {
+      float mu;
+      if (Gd) {
+        const float rs = __ldcg(Gd + (tid >> 6) * kNacc + kSB * kSB + (tid & 63));
+        mu = shift[((size_t)d * SB + 2 * g) * kSB + tid] + rs * invM;
+        sRow[tid] = rs * invM;                        // mean of the shifted samples
+      } else {
+        mu = f.rmean[d][g * kGS2 + tid];
+      }
+      sMean[tid] = mu;
+    }
+    __syncthreads();
+    // lower triangle (i >= j) of the Gram from its block, mirrored: the covariance is exactly symmetric
+    for (int e = tid; e < kGS2 * kGS2; e += kThreads2) {
+      const int i = e >> 7, j = e & 127, hi = i > j ? i : j, lo = i > j ? j : i;
+      float c;
+      if (Gd) {
+        const float raw = (hi >> 6) == (lo >> 6) ? __ldcg(Gd + (hi >> 6) * kNacc + (hi & 63) * kSB + (lo & 63))
+                                                 : __ldcg(Go + (hi & 63) * kSB + lo);
+        c = raw * invM - sRow[i] * sRow[j];
+      } else {
+        c = f.rcov[d][(size_t)g * kGS2 * kGS2 + e];
+      }
+      sCov[i * kLD2 + j] = c;
+    }
+    __syncthreads();
+    fwd_factor_block(gm, f, d, g, sMean, sCov, sL, sW, Gd != nullptr);   // save_mean, save_w, status; train: bad[d][g]
+    __syncthreads();
+    if (Gd && f.update_running && !__ldcg(f.bad + d * gm.G + g)) {     // a non-PD batch covariance never reaches the EMA
+      const float m = f.momentum, k = 1.f - f.momentum;
+      for (int e = tid; e < kGS2 * kGS2; e += kThreads2) {
+        float* rc = f.rcov[d] + (size_t)g * kGS2 * kGS2 + e;
+        *rc = m * (sCov[(e >> 7) * kLD2 + (e & 127)] * f.unbias) + k * *rc;
+      }
+      if (tid < kGS2) f.rmean[d][g * kGS2 + tid] = m * sMean[tid] + k * f.rmean[d][g * kGS2 + tid];
+    }
+    __syncthreads();      // this domain's buffer writes before the next domain's reads (aliasing)
+  }
+}
+
+// bwd_coef at 128: grid (G, 1, D).  rgram [D][2 SB][kNacc]: block (r, c) of group g's R = sum dy xc^T at 4 g + 2 r + c,
+// the dy row sums of rows r in block (r, r).
+__global__ void __launch_bounds__(kThreads2) bwd_coef128_kernel(const float* __restrict__ rgram, const Geom gm, const BwdFin f,
+                                                                float* __restrict__ dybar) {
+  extern __shared__ __align__(16) float dsm2[];
+  float* sW = dsm2;
+  float* sR = sW + kMat2;
+  float* sT1 = sR + kMat2;
+  float* sVec = sT1 + kMat2;                         // gamma | mean (bwd_finalize_block)
+  float* sSdz = sVec + 2 * kGS2;
+  __shared__ int s_flag;
+  const int g = blockIdx.x, d = blockIdx.z, tid = threadIdx.x, SB = gm.C / kSB;
+  const bool train = f.mode == DWT_MODE_TRAIN;
+  const float* G = (rgram && train) ? rgram + ((size_t)d * 2 * SB + 4 * g) * kNacc : nullptr;
+  for (int e = tid; e < kGS2 * kGS2; e += kThreads2) {
+    const int i = e >> 7, j = e & 127;
+    sR[i * kLD2 + j] = G ? __ldcg(G + (2 * (i >> 6) + (j >> 6)) * kNacc + (i & 63) * kSB + (j & 63)) : 0.f;
+  }
+  if (tid < kGS2) {
+    const float sdz = G ? __ldcg(G + 3 * (tid >> 6) * kNacc + kSB * kSB + (tid & 63)) : 0.f;
+    sSdz[tid] = sdz;
+    if (dybar) dybar[((size_t)d * SB + 2 * g) * kSB + tid] = sdz * (1.f / gm.M);   // mean_M dy (0 in eval mode)
+  }
+  // bwd_finalize_block's barrier after loading W publishes sR and sSdz; R is dead once P is formed, so its buffer
+  // doubles as the T scratch
+  bwd_finalize_block(gm, f, d, g, sR, sSdz, sW, sT1, sR, sVec, &s_flag);
+}
+
 constexpr size_t kFactorSmem = 0;   // fwd_factor: static shared memory only (panel buffers + covariance)
 constexpr size_t kCoefSmem = sizeof(float) * 4 * kMat;
 
@@ -446,6 +543,8 @@ constexpr size_t kCoefSmem = sizeof(float) * 4 * kMat;
 int dense_init() {
   cudaError_t e = cudaFuncSetAttribute(fwd_factor_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFactorSmem);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(bwd_coef_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kCoefSmem);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(fwd_factor128_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFactor2Smem);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(bwd_coef128_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kCoef2Smem);
   return (int)e;
 }
 
@@ -454,13 +553,23 @@ void dense_partial_reduce(const float* partial, int nchunks, int problems, float
   partial_reduce_kernel<<<dim3((kNacc + 63) / 64, problems), 256, 0, st>>>(partial, nchunks, gram);
 }
 
-// gram == nullptr: eval mode (running buffers -> W)
+// gram == nullptr: eval mode (running buffers -> W).  Group size 128: gram holds [D][SB] diagonal blocks followed by
+// [D][SB/2] off-diagonal blocks.
 void dense_fwd_factor(const float* gram, const float* shift, const Geom& gm, const FwdFin& fin, cudaStream_t st) {
+  if (gm.GS == kGS2) {
+    const float* goff = gram ? gram + (size_t)gm.D * (gm.C / kSB) * kNacc : nullptr;
+    fwd_factor128_kernel<<<gm.G, kThreads2, kFactor2Smem, st>>>(gram, goff, shift, gm, fin);
+    return;
+  }
   fwd_factor_kernel<<<gm.G, 256, kFactorSmem, st>>>(gram, shift, gm, fin);
 }
 
-// rgram == nullptr: eval mode without affine (A1 = W^T only)
+// rgram == nullptr: eval mode without affine (A1 = W^T only).  Group size 128: rgram [D][2 SB] blocks.
 void dense_bwd_coef(const float* rgram, const Geom& gm, const BwdFin& fin, float* dybar, cudaStream_t st) {
+  if (gm.GS == kGS2) {
+    bwd_coef128_kernel<<<dim3(gm.G, 1, gm.D), kThreads2, kCoef2Smem, st>>>(rgram, gm, fin, dybar);
+    return;
+  }
   bwd_coef_kernel<<<dim3(gm.G, 1, gm.D), 256, kCoefSmem, st>>>(rgram, gm, fin, dybar);
 }
 

@@ -44,7 +44,7 @@ void tiled_bwd_prep(const Geom& gm, const BwdFin& fin, cudaStream_t st);
 void tiled_bwd_apply(const float* x, const float* dout, float* dx, const Geom& gm, int vec, int chunks,
                      const float* coef, cudaStream_t st);
 
-// TMA + wgmma contraction path, group sizes 8..64 tiling a 64-channel super-block  (norm_tc.cu)
+// TMA + wgmma contraction path, group sizes 8..64 tiling a 64-channel super-block, and 128 spanning two  (norm_tc.cu)
 int tc_init();      // driver entry point for cuTensorMapEncodeTiled + shared-memory opt-in; 0 on success
 bool tc_supports(const Geom& gm, int vec);
 int tc_superblocks(const Geom& gm);
@@ -52,6 +52,9 @@ int tc_superblocks(const Geom& gm);
 // widened to fp32, stores rounded to nearest-even).  `nhwc`: dense channels-last tensors (HW % 4 == 0, 16-byte aligned;
 // the same schedule and arithmetic as NCHW).  Partials, shifts, statistics and coefficients are fp32 either way.
 int tc_stats(const void* x, bool bf16, bool nhwc, const Geom& gm, int nchunks, float* shift, float* partial, cudaStream_t st);
+// group size 128 (fp32): the off-diagonal 64 x 64 Gram block of every 128-channel group, around tc_stats' shifts.
+// tc_bwd_reduce at group size 128 forms all four blocks of every group's R.
+int tc_gram_pair(const void* x, bool nhwc, const Geom& gm, int nchunks, const float* shift, float* partial, cudaStream_t st);
 int tc_bwd_reduce(const void* x, const void* dout, bool bf16, bool nhwc, const Geom& gm, int nchunks, const float* save_mean,
                   float* partial, cudaStream_t st);
 

@@ -1,5 +1,5 @@
 // Tensor-core path for the two CONTRACTIONS over the flattened N*H*W axis when groups are large
-// (group size 8..64, i.e. BASELINE.json config 2: C=256, group_size=64):
+// (group size 8..64, i.e. BASELINE.json config 2: C=256, group_size=64; and 128, see below):
 //
 //   stats       G = sum_m (x-K)(x-K)^T        per 64-channel super-block (gs x gs diagonal blocks kept)
 //   bwd_reduce  R = sum_m dy (x-mean)^T
@@ -45,6 +45,23 @@
 // and writes exactly what the NCHW transform writes, at the same swizzled positions, into the per-warpgroup fp32
 // staging tiles of the bf16 kernels; the rest is the NCHW kernel, so every partial is bit for bit the NCHW kernel's on
 // x.contiguous().  fp32 rings are shallower (Gram 8, contraction 4 stages) to keep two CTAs per SM with the staging.
+//
+// group size 128 (fp32, both layouts): a group spans the super-blocks 2p and 2p + 1, so its 128 x 128 statistics are
+// three 64 x 64 blocks plus the 128 row sums.
+//   Gram: the diagonal blocks and row sums are tc_gram_kernel's, unchanged (it never reads the group size); the
+//   off-diagonal block G10 = sum s1 s0^T comes from tc_gram_pair_kernel, one launch later: a stage carries the tiles of
+//   both super-blocks, each is split hi / lo by gram_transform around the same pilot shifts (read back from the diagonal
+//   launch), and H1 H0^T + L1 H0^T + H1 L0^T go into one accumulator -- the hi/lo model of the diagonal kernel over the
+//   whole 128-vector (lo lo^T dropped, lo hi^T kept on both sides).  Chosen over one CTA holding both super-blocks'
+//   tiles and all seven 64 x 64 accumulators (224 registers per thread for one warpgroup, or an uneven split of block
+//   rows across warpgroups) because it reuses the diagonal kernel as it is and keeps two CTAs per SM.  Cost: x is read
+//   from HBM twice per call (the second pass is a separate launch over an 822 MB tensor at BASELINE config 2, far
+//   beyond L2) -- 2x by design, not measured directly; the profile counts the algorithmic bytes once.
+//   Contraction: tc_contract_kernel<.., PAIR = true> forms all four blocks of R (it is not symmetric), blockIdx.y =
+//   4 p + 2 r + c: dy rows from super-block 2p + r, x columns from 2p + c; x and dy are each read twice (concurrently
+//   by the blocks of one wave, so partly from L2; not measured).
+//   ptxas (sm_90a): tc_gram_pair_kernel NCHW 91 / NHWC 87 registers; tc_contract_kernel<float, NCHW / NHWC, PAIR> 89 /
+//   85 registers; no spills; dynamic shared memory 97 KB (gram pair) and the contraction's 97 / 129 KB as above.
 //
 // Reference: utils/whitening.py:46-47 of the reference project and its autograd transpose.
 #include <cuda.h>
@@ -284,7 +301,9 @@ __device__ __forceinline__ void init_ring(TcBarriers& bars, int stages) {
 // ------------------------------------------------------------------------------------------
 // backward contraction: R = sum dy xc^T and the row sums of dy
 // ------------------------------------------------------------------------------------------
-template <class T, bool NHWC>
+// PAIR (group size 128): blockIdx.y = 4 p + 2 r + c is block (r, c) of the 128 x 128 R of pair p: dy rows from
+// super-block 2p + r, x columns from super-block 2p + c (R is not symmetric: all four blocks are formed).
+template <class T, bool NHWC, bool PAIR = false>
 __global__ void __launch_bounds__(kTcThreads, 2)
 tc_contract_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_g, const Geom gm,
                    const float* __restrict__ save_mean, float* __restrict__ partial) {
@@ -295,12 +314,14 @@ tc_contract_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
   __shared__ TcBarriers bars;
   __shared__ float sShift[kTileCh];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, tid = threadIdx.x;
-  const int sb = blockIdx.y, d = blockIdx.z, ch0 = sb * kTileCh;
+  const int sb = blockIdx.y, d = blockIdx.z;
+  const int ch0 = PAIR ? (2 * (sb >> 2) + ((sb >> 1) & 1)) * kTileCh : sb * kTileCh;     // dy channels
+  const int chx = PAIR ? (2 * (sb >> 2) + (sb & 1)) * kTileCh : ch0;                    // x channels
   const TileRange tr(gm);
   const int ntiles = tr.end - tr.begin;
 
   if (tid == 0) init_ring(bars, STAGES);
-  if (tid < kTileCh) sShift[tid] = ch0 + tid < gm.C ? save_mean[(size_t)d * gm.C + ch0 + tid] : 0.f;
+  if (tid < kTileCh) sShift[tid] = chx + tid < gm.C ? save_mean[(size_t)d * gm.C + chx + tid] : 0.f;
   __syncthreads();
 
   float acc[32], rowsum[kPer];
@@ -318,7 +339,7 @@ tc_contract_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
         const int t = tr.begin + it, n = t / tr.PB, pb = t - n * tr.PB;
         uint8_t* dst = smem + (size_t)s * 2 * BOX;
         mbar_arrive_expect_tx(&bars.full[s], 2 * BOX);
-        tma_tile<T, NHWC>(dst, &map_x, ch0, pb * kTilePx, d * gm.N + n, &bars.full[s]);
+        tma_tile<T, NHWC>(dst, &map_x, chx, pb * kTilePx, d * gm.N + n, &bars.full[s]);
         tma_tile<T, NHWC>(dst + BOX, &map_g, ch0, pb * kTilePx, d * gm.N + n, &bars.full[s]);
       }
     }
@@ -336,7 +357,7 @@ tc_contract_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
       const int tl = tr.begin + it, n = tl / tr.PB, pb = tl - n * tr.PB;
       const uint32_t tile = smem_u32(smem + (size_t)s * 2 * BOX);
       const uint32_t xs = STAGED ? stage_f32 : tile, ys = STAGED ? stage_f32 + kTileBytes : tile + kTileBytes;
-      transform_tile<T, NHWC>(tile, xs, t, shift, pb * kTilePx, gm.HW, ch0, gm.C, dummy);               // xc
+      transform_tile<T, NHWC>(tile, xs, t, shift, pb * kTilePx, gm.HW, chx, gm.C, dummy);               // xc
       transform_tile<T, NHWC>(tile + BOX, ys, t, zero, pb * kTilePx, gm.HW, ch0, gm.C, rowsum);         // dy, sums
       if constexpr (STAGED) {                      // the stage is read: it can be refilled while the MMAs run
         __syncwarp();
@@ -483,6 +504,112 @@ tc_gram_kernel(const __grid_constant__ CUtensorMap map_x, const T* __restrict__ 
 }
 
 // ------------------------------------------------------------------------------------------
+// group size 128, off-diagonal Gram block: G10 = sum_m s1 s0^T of pair p (s1: super-block 2p + 1, s0: super-block 2p),
+// split precision over the whole 128-vector:  G10 = H1 H0^T + L1 H0^T + H1 L0^T  (L1 L0^T dropped, as lo lo^T above)
+// ------------------------------------------------------------------------------------------
+// fp32 only.  Stage = the two [64 ch x 32 px] tiles of one image block.  The three products share ONE accumulator (no
+// transpose is needed off the diagonal), so registers stay below the diagonal kernel's.  Shared memory per CTA: NCHW
+// 4 stages x 16 KB + two lo tiles per warpgroup (hi in place) = 96 KB; NHWC 2 stages x 16 KB + hi and lo staging of
+// both tiles per warpgroup = 96 KB; two CTAs per SM either way.  The pilot shifts are the diagonal kernel's (shift).
+template <bool NHWC> constexpr int kPairStagesOf = NHWC ? 2 : 4;
+static_assert(kPairStagesOf<false> % kConsumers == 0 && kPairStagesOf<true> % kConsumers == 0, "stage ownership");
+
+template <bool NHWC>
+__global__ void __launch_bounds__(kTcThreads, 2)
+tc_gram_pair_kernel(const __grid_constant__ CUtensorMap map_x, const Geom gm, const float* __restrict__ shift,
+                    float* __restrict__ partial) {
+  constexpr int STAGES = kPairStagesOf<NHWC>, BOX = kTileBytes;
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+  __shared__ TcBarriers bars;
+  __shared__ float sShift[2][kTileCh];             // [0] rows (super-block 2p + 1), [1] columns (super-block 2p)
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, tid = threadIdx.x;
+  const int p = blockIdx.y, d = blockIdx.z, SB = gm.C / kTileCh;
+  const int chr = (2 * p + 1) * kTileCh, chc = 2 * p * kTileCh;
+  const TileRange tr(gm);
+  const int ntiles = tr.end - tr.begin;
+
+  if (tid == 0) init_ring(bars, STAGES);
+  if (tid < 2 * kTileCh) sShift[tid >> 6][tid & 63] = shift[((size_t)d * SB + 2 * p + 1 - (tid >> 6)) * kTileCh + (tid & 63)];
+  __syncthreads();
+
+  float acc[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+
+  if (warp == kProducerWarp) {
+    // ===== TMA producer =====
+    if (lane == 0) {
+      int n = tr.begin / tr.PB, pb = tr.begin - n * tr.PB;
+      for (int it = 0; it < ntiles; ++it) {
+        const int s = it % STAGES;
+        mbar_wait_relaxed(&bars.empty[s], ((it / STAGES) & 1) ^ 1);
+        uint8_t* dst = smem + (size_t)s * 2 * BOX;
+        mbar_arrive_expect_tx(&bars.full[s], 2 * BOX);
+        tma_tile<float, NHWC>(dst, &map_x, chr, pb * kTilePx, d * gm.N + n, &bars.full[s]);
+        tma_tile<float, NHWC>(dst + BOX, &map_x, chc, pb * kTilePx, d * gm.N + n, &bars.full[s]);
+        if (++pb == tr.PB) { pb = 0; ++n; }
+      }
+    }
+  } else {
+    // ===== consumer warpgroups: G10[64 x 64] += h1 h0^T + l1 h0^T + h1 l0^T =====
+    const int wg = warp >> 2, t = tid & 127;
+    // per warpgroup behind the ring: NCHW the lo tiles of rows and columns (hi in place); NHWC hi, lo of rows, hi, lo of columns
+    const uint32_t wgbuf = smem_u32(smem + (size_t)STAGES * 2 * BOX + (size_t)wg * (NHWC ? 4 : 2) * kTileBytes);
+    const uint32_t lo_r = NHWC ? wgbuf + kTileBytes : wgbuf, lo_c = NHWC ? wgbuf + 3 * kTileBytes : wgbuf + kTileBytes;
+    float shr[kPer], shc[kPer], dummy[kPer];
+#pragma unroll
+    for (int i = 0; i < kPer; ++i) {
+      shr[i] = sShift[0][(t + 128 * i) >> 3];
+      shc[i] = sShift[1][(t + 128 * i) >> 3];
+      dummy[i] = 0.f;
+    }
+    for (int it = wg; it < ntiles; it += kConsumers) {
+      const int s = it % STAGES;
+      mbar_wait(&bars.full[s], (it / STAGES) & 1);
+      const int tl = tr.begin + it, n = tl / tr.PB, pb = tl - n * tr.PB;
+      const uint32_t tile = smem_u32(smem + (size_t)s * 2 * BOX);
+      const uint32_t hi_r = NHWC ? wgbuf : tile, hi_c = NHWC ? wgbuf + 2 * kTileBytes : tile + BOX;
+      gram_transform<float, NHWC>(tile, hi_r, lo_r, t, shr, pb * kTilePx, gm.HW, chr, gm.C, dummy);
+      gram_transform<float, NHWC>(tile + BOX, hi_c, lo_c, t, shc, pb * kTilePx, gm.HW, chc, gm.C, dummy);
+      if constexpr (NHWC) {                        // the stage is read: it can be refilled while the MMAs run
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&bars.empty[s]);
+      }
+      fence_proxy_async();
+      warpgroup_sync(wg);
+      wgmma_fence();
+      fence_operands(acc);
+      const uint64_t hr = make_kmajor_sw128_desc(hi_r), lr = make_kmajor_sw128_desc(lo_r);
+      const uint64_t hc = make_kmajor_sw128_desc(hi_c), lc = make_kmajor_sw128_desc(lo_c);
+#pragma unroll
+      for (int k = 0; k < kTilePx / 8; ++k) {
+        wgmma_m64n64k8_ss(acc, hr + 2 * k, hc + 2 * k);
+        wgmma_m64n64k8_ss(acc, lr + 2 * k, hc + 2 * k);
+        wgmma_m64n64k8_ss(acc, hr + 2 * k, lc + 2 * k);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();                             // the lo (NHWC: and hi) tiles are rewritten by the next transform
+      fence_operands(acc);
+      if constexpr (!NHWC) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&bars.empty[s]);
+      }
+    }
+  }
+
+  // ===== epilogue: both warpgroups' accumulators -> this CTA's partial row (row-sum slots 0: the diagonal kernel has them) =====
+  __syncthreads();
+  float* sAcc = reinterpret_cast<float*>(smem);    // [64][64]
+  for (int e = tid; e < kTileCh * kTileCh; e += kTcThreads) sAcc[e] = 0.f;
+  __syncthreads();
+  if (warp < kProducerWarp) add_fragment<8>(sAcc, kTileCh, acc, warp, lane);
+  __syncthreads();
+  float* prow = partial + (((size_t)d * gridDim.y + p) * gridDim.x + blockIdx.x) * kNacc;
+  for (int e = tid; e < kNacc; e += kTcThreads) prow[e] = e < kTileCh * kTileCh ? sAcc[e] : 0.f;
+}
+
+// ------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -534,6 +661,21 @@ cudaError_t tc_kernel_attrs() {
   return e;
 }
 
+// group size 128 (fp32): the off-diagonal Gram kernel and the four-block contraction
+template <bool NHWC> size_t tc_pair_smem_bytes() {
+  return (size_t)kPairStagesOf<NHWC> * 2 * kTileBytes + (size_t)kConsumers * (NHWC ? 4 : 2) * kTileBytes + 1024;
+}
+
+template <bool NHWC>
+cudaError_t tc_pair_attrs() {
+  cudaError_t e = cudaFuncSetAttribute(tc_gram_pair_kernel<NHWC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_pair_smem_bytes<NHWC>());
+  if (e == cudaSuccess)
+    e = cudaFuncSetAttribute(tc_contract_kernel<float, NHWC, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes<float, NHWC>(true));
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_gram_pair_kernel<NHWC>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_contract_kernel<float, NHWC, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  return e;
+}
+
 template <class T, bool NHWC>
 void launch_gram(const CUtensorMap& mx, const void* x, const Geom& gm, int nchunks, float* shift, float* partial, cudaStream_t st) {
   dim3 grid(nchunks, tc_superblocks(gm), gm.D);
@@ -543,6 +685,13 @@ void launch_gram(const CUtensorMap& mx, const void* x, const Geom& gm, int nchun
 template <class T, bool NHWC>
 void launch_contract(const CUtensorMap& mx, const CUtensorMap& mg, const Geom& gm, int nchunks, const float* save_mean,
                      float* partial, cudaStream_t st) {
+  if constexpr (!kBf16<T>) {
+    if (gm.GS == 2 * kTileCh) {                  // group size 128: the four 64 x 64 blocks of every group's R
+      dim3 grid(nchunks, 2 * tc_superblocks(gm), gm.D);
+      tc_contract_kernel<T, NHWC, true><<<grid, kTcThreads, tc_smem_bytes<T, NHWC>(true), st>>>(mx, mg, gm, save_mean, partial);
+      return;
+    }
+  }
   dim3 grid(nchunks, tc_superblocks(gm), gm.D);
   tc_contract_kernel<T, NHWC><<<grid, kTcThreads, tc_smem_bytes<T, NHWC>(true), st>>>(mx, mg, gm, save_mean, partial);
 }
@@ -559,17 +708,21 @@ int tc_init() {
   if (e == cudaSuccess) e = tc_kernel_attrs<__nv_bfloat16, false>();
   if (e == cudaSuccess) e = tc_kernel_attrs<float, true>();
   if (e == cudaSuccess) e = tc_kernel_attrs<__nv_bfloat16, true>();
+  if (e == cudaSuccess) e = tc_pair_attrs<false>();
+  if (e == cudaSuccess) e = tc_pair_attrs<true>();
   if (e == cudaSuccess) e = (cudaError_t)dense_init();
   if (e == cudaSuccess) return tc_apply_init();
   return (int)e;
 }
 
-// The TMA/wgmma contraction takes group sizes that tile a 64-channel super-block, rows that TMA can
-// address (16-byte strides and base) and at least one full 32-pixel box per row.
+// The TMA/wgmma contraction takes group sizes that tile a 64-channel super-block or span two of them (128), rows
+// that TMA can address (16-byte strides and base) and at least one full 32-pixel box per row.
 // TF32 operands are rounded to nearest, so product errors are zero-mean and shrink as 1/sqrt(M); below a
-// few thousand samples per channel they do not, and the (exact fp32, FFMA) tiled kernels take the call.
+// few thousand samples per channel they do not, and the (exact fp32, FFMA) tiled kernels take the call (group sizes
+// up to 64; group size 128 has no tiled kernel and is refused there).
 bool tc_supports(const Geom& gm, int vec) {
-  return gm.GS >= 8 && kTileCh % gm.GS == 0 && vec == 4 && gm.HW >= kTilePx && (long long)gm.N * gm.HW >= 4096;
+  return gm.GS >= 8 && (kTileCh % gm.GS == 0 || gm.GS == 2 * kTileCh) && vec == 4 && gm.HW >= kTilePx &&
+         (long long)gm.N * gm.HW >= 4096;
 }
 
 int tc_superblocks(const Geom& gm) { return (gm.C + kTileCh - 1) / kTileCh; }
@@ -589,6 +742,18 @@ int tc_stats(const void* x, bool bf16, bool nhwc, const Geom& gm, int nchunks, f
   return 0;
 }
 
+// partial: [D][SB/2][nchunks][64*64+64] off-diagonal blocks of the 128-channel groups; shift: tc_stats' pilot shifts
+int tc_gram_pair(const void* x, bool nhwc, const Geom& gm, int nchunks, const float* shift, float* partial, cudaStream_t st) {
+  CUtensorMap mx;
+  bind_context();
+  if (int rc = make_map(&mx, x, gm, false, nhwc)) return rc;
+  const dim3 grid(nchunks, tc_superblocks(gm) / 2, gm.D);
+  if (nhwc) tc_gram_pair_kernel<true><<<grid, kTcThreads, tc_pair_smem_bytes<true>(), st>>>(mx, gm, shift, partial);
+  else tc_gram_pair_kernel<false><<<grid, kTcThreads, tc_pair_smem_bytes<false>(), st>>>(mx, gm, shift, partial);
+  return 0;
+}
+
+// group size 128: partial [D][2 SB][nchunks][64*64+64], block (r, c) of group p at 4 p + 2 r + c
 int tc_bwd_reduce(const void* x, const void* dout, bool bf16, bool nhwc, const Geom& gm, int nchunks, const float* save_mean,
                   float* partial, cudaStream_t st) {
   CUtensorMap mx, mg;

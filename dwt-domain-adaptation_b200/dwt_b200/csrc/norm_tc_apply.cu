@@ -34,6 +34,11 @@
 // distinct banks.  The output fragment is stored at NHWC addresses, two adjacent channels per store (8 bytes fp32, 4 bytes
 // bf16).  Same fragments, same products, same order: y and dx are bit for bit the NCHW kernel's on x.contiguous().
 //
+// group size 128 (fp32, both layouts): tc_apply128_kernel, below -- the K = 128 product in two K = 64 halves into one
+// accumulator.  ptxas (sm_90a): forward NCHW 152 / NHWC 144 registers, no spills; backward NCHW 168 registers with 40
+// bytes of spill stores / loads, NHWC 168 with 44 (the per-input argument arrays, indexed at run time by the rolled
+// half loop); dynamic shared memory 129 KB forward, 193 KB backward.
+//
 // Reference: the grouped 1x1 convolution at utils/whitening.py:55 of the reference project and its backward.
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -295,6 +300,163 @@ tc_apply_kernel(const __grid_constant__ CUtensorMap map0, const __grid_constant_
   }
 }
 
+// ------------------------------------------------------------------------------------------
+// group size 128 (fp32): output block r = blockIdx.y & 1 of pair p = blockIdx.y >> 1 (channels (2p + r) * 64 ..) is
+//   out_r = sum_i sum_h M_i[r][h] (in_i[h] - shift_i[h])           in_i[h] = input i at super-block 2p + h
+// -- the K = 128 product in two K = 64 halves accumulated into ONE fp32 accumulator: a warpgroup takes a tile's h = 0
+// stage, then its h = 1 stage.  Same split-tf32 operands, same centring on load, same fragments and store as above.
+// The 2 x NIN blocks [64 x 64] of M (hi and lo) stay resident: 64 KB forward, 128 KB backward.  Each warpgroup owns
+// SPW ring stages of one 64-channel half of every input (16 KB per input): forward 4 x 16 KB = 64 KB (128 KB in all),
+// backward 2 x 32 KB = 64 KB (192 KB in all); one CTA per SM.  Zero blocks (W is lower-, A1 = W^T upper-triangular)
+// are multiplied like any other: their products are exact zeros.
+// ------------------------------------------------------------------------------------------
+template <int NIN> struct Ap128Cfg {
+  static constexpr int SPW = NIN == 1 ? 2 : 1;                 // ring stages per consumer warpgroup
+  static constexpr int STAGES = kConsumers * SPW;
+  static constexpr int SLOT = NIN * kCh * kTilePx * 4;
+  static constexpr size_t SMEM = (size_t)STAGES * SLOT + (size_t)2 * 2 * NIN * kMatBytes + 1024;
+  static_assert(STAGES <= kMaxStages, "stages");
+};
+
+template <int NIN, bool NHWC>
+__global__ void __launch_bounds__(kApThreads, 1)
+tc_apply128_kernel(const __grid_constant__ CUtensorMap map0, const __grid_constant__ CUtensorMap map1, const Geom gm,
+                   const ApplyArgs args) {
+  using Cfg = Ap128Cfg<NIN>;
+  constexpr int SPW = Cfg::SPW, SLOT = Cfg::SLOT;
+  extern __shared__ __align__(1024) uint8_t smem_dyn[];
+  uint8_t* sRing = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 1023) & ~(uintptr_t)1023);
+  uint8_t* sMat = sRing + (size_t)Cfg::STAGES * SLOT;     // [NIN][h][hi, lo][kMatBytes]
+  __shared__ ApBarriers bars;
+  __shared__ float sShift[NIN][2][kCh];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, tid = threadIdx.x;
+  const int p = blockIdx.y >> 1, r = blockIdx.y & 1, d = blockIdx.z, ch0 = (2 * p + r) * kCh;
+  const int PB = (gm.HW + kTilePx - 1) / kTilePx;
+  const long long NT = (long long)gm.N * PB;
+  const int t_begin = (int)(NT * blockIdx.x / gridDim.x);
+  const int ntiles = (int)(NT * (blockIdx.x + 1) / gridDim.x) - t_begin;
+  // j-th load of warpgroup w (tile it = 2 (j / 2) + w, half h = j % 2): stage w + 2 (j % SPW), parity (j / SPW) & 1
+  auto stage_of = [](int w, int j) { return w + kConsumers * (j % SPW); };
+
+  if (tid == 0) {
+    for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&bars.full[s], 1); mbar_init(&bars.empty[s], 4); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  if (tid < NIN * 2 * kCh) {
+    const int i = tid / (2 * kCh), h = (tid / kCh) & 1, k = tid % kCh;
+    sShift[i][h][k] = __ldg(args.shift[i] + (size_t)d * args.shift_stride[i] + (2 * p + h) * kCh + k);
+  }
+  // the split matrices: block (r, h) of input i's 128 x 128 group matrix, K-major as the B operand
+  for (int e = tid; e < NIN * 2 * kCh * kCh; e += kApThreads) {
+    const int m = e / (2 * kCh * kCh), h = (e / (kCh * kCh)) & 1, n = (e / kCh) % kCh, k = e % kCh;
+    const float w = __ldg(args.mats + ((size_t)d * gm.G + p) * args.rec_stride + args.off[m] + (size_t)(r * kCh + n) * (2 * kCh) +
+                          h * kCh + k);
+    const float hi = round_tf32(w);
+    const uint32_t o = kmajor_off(n, k);
+    *reinterpret_cast<float*>(sMat + (size_t)(4 * m + 2 * h) * kMatBytes + o) = hi;
+    *reinterpret_cast<float*>(sMat + (size_t)(4 * m + 2 * h + 1) * kMatBytes + o) = round_tf32(w - hi);
+  }
+  fence_proxy_async();
+  __syncthreads();
+
+  if (warp == kProducerWarp) {
+    // ===== TMA producer: per pair of tiles (one per warpgroup) the h = 0 halves, then the h = 1 halves =====
+    if (lane == 0) {
+      for (int it0 = 0; it0 < ntiles; it0 += kConsumers)
+        for (int h = 0; h < 2; ++h)
+          for (int w = 0; w < kConsumers && it0 + w < ntiles; ++w) {
+            const int t = t_begin + it0 + w, n = t / PB, pb = t - n * PB, j = it0 + h, s = stage_of(w, j);
+            const int chh = (2 * p + h) * kCh;
+            mbar_wait_relaxed(&bars.empty[s], ((j / SPW) & 1) ^ 1);
+            uint8_t* dst = sRing + (size_t)s * SLOT;
+            int nb = (gm.HW - pb * kTilePx + kBoxPx - 1) / kBoxPx;      // 32-pixel boxes not entirely past the row end
+            nb = nb < kNBox ? nb : kNBox;
+            mbar_arrive_expect_tx(&bars.full[s], NIN * nb * kBoxBytes);
+#pragma unroll
+            for (int i = 0; i < NIN; ++i)
+              for (int b = 0; b < nb; ++b) {
+                const CUtensorMap* m = i == 0 ? &map0 : &map1;
+                if constexpr (NHWC) {
+                  uint8_t* bb = dst + i * (SLOT / NIN) + b * (kBoxPx * 128);
+                  tma_load_3d(bb, m, chh, pb * kTilePx + b * kBoxPx, d * gm.N + n, &bars.full[s]);
+                  tma_load_3d(bb + kTilePx * 128, m, chh + 32, pb * kTilePx + b * kBoxPx, d * gm.N + n, &bars.full[s]);
+                } else {
+                  tma_load_3d(dst + (i * kNBox + b) * kBoxBytes, m, pb * kTilePx + b * kBoxPx, chh, d * gm.N + n, &bars.full[s]);
+                }
+              }
+          }
+    }
+  } else {
+    // ===== consumer warpgroups: D[64 px x 64 ch] = sum_h sum_i tile_i[h]^T M_i[r][h]^T =====
+    const int wg = warp >> 2;
+    const int prow = 16 * (warp & 3) + (lane >> 2), kq = lane & 3;
+    const uint32_t mat0 = smem_u32(sMat);
+    for (int it = wg; it < ntiles; it += kConsumers) {
+      float acc[32];
+#pragma unroll
+      for (int q = 0; q < 32; ++q) acc[q] = 0.f;
+#pragma unroll 1
+      for (int h = 0; h < 2; ++h) {
+        const int j = it - wg + h, s = stage_of(wg, j);
+        mbar_wait(&bars.full[s], (j / SPW) & 1);
+        const uint32_t slot = smem_u32(sRing + (size_t)s * SLOT);
+        uint32_t ahi[NIN][kCh / 8][4], alo[NIN][kCh / 8][4];
+#pragma unroll
+        for (int i = 0; i < NIN; ++i)
+#pragma unroll
+          for (int ks = 0; ks < kCh / 8; ++ks)
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+              const int k = 8 * ks + kq + 4 * (q >> 1);
+              const float v = lds32(slot + i * (SLOT / NIN) + tile_off<float, NHWC>(k, prow + 8 * (q & 1))) - sShift[i][h][k];
+              const uint32_t hb = __float_as_uint(v) & kTf32Mask;
+              ahi[i][ks][q] = hb;
+              alo[i][ks][q] = __float_as_uint(round_tf32(v - __uint_as_float(hb)));
+            }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&bars.empty[s]);   // the half is in registers: the stage can be refilled
+        wgmma_fence();
+        fence_operands(acc);
+#pragma unroll
+        for (int i = 0; i < NIN; ++i)
+#pragma unroll
+          for (int ks = 0; ks < kCh / 8; ++ks) {
+            const uint32_t koff = (uint32_t)((ks >> 2) * (kCh * 128) + (ks & 3) * 32);
+            const uint64_t bhi = make_kmajor_sw128_desc(mat0 + (uint32_t)(4 * i + 2 * h) * kMatBytes + koff);
+            const uint64_t blo = make_kmajor_sw128_desc(mat0 + (uint32_t)(4 * i + 2 * h + 1) * kMatBytes + koff);
+            wgmma_m64n64k8_rs(acc, ahi[i][ks], bhi);
+            wgmma_m64n64k8_rs(acc, ahi[i][ks], blo);
+            wgmma_m64n64k8_rs(acc, alo[i][ks], bhi);
+            wgmma_m64n64k8_rs(acc, alo[i][ks], blo);
+          }
+        wgmma_commit();
+        wgmma_wait<0>();                               // the fragments are reloaded for the next half
+        fence_operands(acc);
+      }
+      const int t = t_begin + it, n = t / PB, pb = t - n * PB;
+      float* obase = static_cast<float*>(args.out) + (size_t)(d * gm.N + n) * gm.C * gm.HW;
+      if constexpr (NHWC) {
+        const int px = pb * kTilePx + prow;
+        float* o = obase + (size_t)px * gm.C + ch0 + 2 * kq;
+#pragma unroll
+        for (int jj = 0; jj < kCh / 8; ++jj)
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh)
+            if (px + 8 * hh < gm.HW)
+              *reinterpret_cast<float2*>(o + (size_t)hh * 8 * gm.C + 8 * jj) = make_float2(acc[4 * jj + 2 * hh], acc[4 * jj + 2 * hh + 1]);
+      } else {
+#pragma unroll
+        for (int jj = 0; jj < kCh / 8; ++jj)
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            const int c = 8 * jj + 2 * kq + (q & 1), px = pb * kTilePx + prow + 8 * (q >> 1);
+            if (px < gm.HW) obase[(size_t)(ch0 + c) * gm.HW + px] = acc[4 * jj + q];
+          }
+      }
+    }
+  }
+}
+
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -331,9 +493,21 @@ cudaError_t ap_attrs() {
   return e;
 }
 
+template <int NIN, bool NHWC>
+cudaError_t ap128_attrs() {
+  cudaError_t e = cudaFuncSetAttribute(tc_apply128_kernel<NIN, NHWC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Ap128Cfg<NIN>::SMEM);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_apply128_kernel<NIN, NHWC>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  return e;
+}
+
 template <int NIN>
 void launch_apply(bool bf16, bool nhwc, dim3 grid, const CUtensorMap& m0, const CUtensorMap& m1, const Geom& gm, const ApplyArgs& a,
                   cudaStream_t st) {
+  if (gm.GS == 2 * kCh) {                          // group size 128 (fp32 only: the C ABI refuses bf16 there)
+    if (nhwc) tc_apply128_kernel<NIN, true><<<grid, kApThreads, Ap128Cfg<NIN>::SMEM, st>>>(m0, m1, gm, a);
+    else tc_apply128_kernel<NIN, false><<<grid, kApThreads, Ap128Cfg<NIN>::SMEM, st>>>(m0, m1, gm, a);
+    return;
+  }
   if (nhwc) {
     if (bf16) tc_apply_kernel<__nv_bfloat16, NIN, true><<<grid, kApThreads, ap_smem<__nv_bfloat16, NIN>(), st>>>(m0, m1, gm, a);
     else tc_apply_kernel<float, NIN, true><<<grid, kApThreads, ap_smem<float, NIN>(), st>>>(m0, m1, gm, a);
@@ -359,6 +533,10 @@ int tc_apply_init() {
   if (e == cudaSuccess) e = ap_attrs<float, 2, true>();
   if (e == cudaSuccess) e = ap_attrs<__nv_bfloat16, 1, true>();
   if (e == cudaSuccess) e = ap_attrs<__nv_bfloat16, 2, true>();
+  if (e == cudaSuccess) e = ap128_attrs<1, false>();
+  if (e == cudaSuccess) e = ap128_attrs<2, false>();
+  if (e == cudaSuccess) e = ap128_attrs<1, true>();
+  if (e == cudaSuccess) e = ap128_attrs<2, true>();
   return (int)e;
 }
 

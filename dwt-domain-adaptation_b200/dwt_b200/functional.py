@@ -193,10 +193,11 @@ class _NormFunction(torch.autograd.Function):
                                       and dout2.is_contiguous(memory_format=torch.channels_last)):
             dout, dout2 = dout + dout2, None
         dout = dout.contiguous(memory_format=torch.channels_last) if nhwc else dout.contiguous()
-        # the forward ran the tensor-core kernels, whose TMA loads need 16 bytes, or (bf16 NCHW, group sizes 1, 2, 4) the
+        # the forward ran the tensor-core kernels, whose TMA loads need 16 bytes (group size 128 in NCHW fp32 as well: it
+        # has no other kernel), or (bf16 NCHW, group sizes 1, 2, 4) the
         # register-resident kernels, whose bf16 loads need 8: copy a misaligned dout (a fresh tensor keeps the layout)
         align = 8 if not nhwc and gs in (1, 2, 4) else 16
-        if ((mode & nv.DTYPE_BF16) or nhwc) and not cl_kernels and dout.data_ptr() % align:
+        if ((mode & nv.DTYPE_BF16) or nhwc or gs > nv.MAX_GROUP_SIZE) and not cl_kernels and dout.data_ptr() % align:
             dout = dout.clone(memory_format=torch.channels_last if nhwc else torch.contiguous_format)
         dev = nv.require_cuda(dout, bf16=True)
         dx = torch.empty_like(x)                     # x's layout: channels-last when the forward ran NHWC
@@ -367,7 +368,9 @@ def norm(x, gamma, beta, *, kind, group_size, n_domains, training_stats, eps, mo
     if torch.bfloat16 in dtypes and dtypes <= set(_ACT_DTYPES):
         gs = group_size if kind == "whiten" else 1
         cl = x.dim() == 4 and not x.is_contiguous() and x.is_contiguous(memory_format=torch.channels_last)
-        cl_tc = kind == "whiten" and residual is None and _nhwc_tensor_core(x, gs, n_domains)
+        # the bf16 tensor-core kernels stop at group size 64: a channels-last bf16 call at 128 upcasts (x.float() keeps
+        # the channels-last strides, so the fp32 channels-last kernels run)
+        cl_tc = kind == "whiten" and residual is None and gs <= nv.MAX_GROUP_SIZE and _nhwc_tensor_core(x, gs, n_domains)
         bf16_kernels = dtypes == {torch.bfloat16} and (
             (nv.channels_last_supported(x.shape[1], gs) or cl_tc) if cl
             else _bf16_small(x, gs, residual) or _bf16_tensor_core(x, kind, gs, n_domains, residual))

@@ -49,6 +49,8 @@ extern "C" {
 #define DWT_B200_ABI_VERSION 10
 #define DWT_MAX_DOMAINS 4
 #define DWT_MAX_GROUP_SIZE 64
+/* the one group size above DWT_MAX_GROUP_SIZE: whitening on the tensor-core kernels only, fp32 (dwt_whiten_fwd) */
+#define DWT_TC_MAX_GROUP_SIZE 128
 
 /* error codes */
 #define DWT_OK 0
@@ -66,9 +68,9 @@ extern "C" {
  * cuDNN's tensor-core convolutions want, so a channels-last model needs no NCHW<->NHWC copies around its convolutions).
  * Built for two kernel families:
  *   - group sizes 1, 2, 4 with C/4 a power of two (the channels-last kernels, every epilogue, dout2);
- *   - whitening at group sizes 8, 16, 32, 64 on the tensor-core kernels: HW >= 32 and HW % 4 == 0, N*HW >= 4096 per
- *     domain, x / y / dout / dx 16-byte aligned (else DWT_E_INVALID), epilogue 0 and no dout2 (else DWT_E_UNSUPPORTED),
- *     fp32 or bf16.  Same schedule and arithmetic as the NCHW call: every output, statistic, running-buffer update and
+ *   - whitening at group sizes 8, 16, 32, 64 (fp32 or bf16) and 128 (fp32) on the tensor-core kernels: HW >= 32 and
+ *     HW % 4 == 0, N*HW >= 4096 per domain, x / y / dout / dx 16-byte aligned (else DWT_E_INVALID), epilogue 0 and no
+ *     dout2 (else DWT_E_UNSUPPORTED).  Same schedule and arithmetic as the NCHW call: every output, statistic, running-buffer update and
  *     status bit is bit for bit that of the NCHW call on the same values.  Profile families tc_*_nhwc[_bf16].
  * Any other channels-last geometry is DWT_E_UNSUPPORTED. */
 #define DWT_LAYOUT_NHWC 0x100
@@ -113,7 +115,10 @@ DWT_API const char *dwt_last_error(void);
 
 /* Workspace: one caller-owned device buffer, ZERO-FILLED once when allocated (the
  * kernels keep their arrival counters self-resetting), reusable by any sequence of
- * calls issued on ONE stream.  Size for the largest call the caller will make. */
+ * calls issued on ONE stream.  Size for the largest call the caller will make.
+ * Group sizes 1..64 (returns 0 for any other, DWT_TC_MAX_GROUP_SIZE included).  A group-size-128 call on C channels
+ * needs no more than the group-size-64 call on 2C channels: size it with dwt_workspace_bytes(N, 2*C, HW, 64, n_domains)
+ * (a smaller workspace is refused with DWT_E_WORKSPACE, never overrun). */
 DWT_API size_t dwt_workspace_bytes(int64_t N, int64_t C, int64_t HW, int group_size, int n_domains);
 
 /* Device status word (first int of the workspace): 0 = ok; bits below are OR-ed in by the kernels and stay
@@ -141,6 +146,11 @@ DWT_API size_t dwt_workspace_bytes(int64_t N, int64_t C, int64_t HW, int group_s
  * domain by domain in order (so aliased buffers see s, then t, then t_aug --
  * SURVEY.md H5), on the UN-shrunk covariance (whitening.py:57-59).
  * EVAL: mean/cov come from the running buffers, nothing is written to them.
+ * group_size: 1..64 dividing C, or 128 (DWT_TC_MAX_GROUP_SIZE, C a multiple of 128) on the tensor-core kernels only:
+ * fp32, HW >= 32 and HW % 4 == 0, N*HW >= 4096 per domain, NCHW x / y 16-byte aligned (channels-last: x, y, dout,
+ * dx 16-byte aligned, else DWT_E_INVALID), epilogue 0 and no dout2.  Group size 128 below that geometry, in bf16, with
+ * an epilogue or a dout2, and every other group size above 64, is DWT_E_UNSUPPORTED.  Same modes, status and EMA
+ * semantics as below 64; dwt_whiten_bwd takes the same group sizes.
  */
 DWT_API int dwt_whiten_fwd(const float *x, float *y, int64_t N, int64_t C, int64_t HW, int group_size,
                    int n_domains, int mode, float eps, float momentum, int update_running,
