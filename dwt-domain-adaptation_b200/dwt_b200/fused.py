@@ -20,7 +20,9 @@ into its running buffers.  The three thirds are identical, so are their statisti
 outputs: here x is the single copy [N, C, H, W], the statistics are computed once, the output is
 written once, and a buffer shared by k branches receives the k-fold EMA in one update,
 r <- (1-m)^k r + (1 - (1-m)^k) s -- a third of the traffic at every site and a third of the
-convolution work between them.
+convolution work between them.  The output is the first third of the reference's: with the first
+domain module in eval mode (tracking running statistics) it is x normalised with that module's
+running buffers, as ``cat((data, data, data))`` through eval-mode modules gives, and no buffer moves.
 """
 from __future__ import annotations
 
@@ -129,7 +131,10 @@ class DomainTripleNorm(nn.Module):
         return torch.relu(y) if relu else y
 
     def _forward_replicated(self, x, mods, gamma, beta, relu, residual, count_batches=True):
-        """One copy of the batch stands for all n_domains branches (see the module docstring)."""
+        """One copy of the batch stands for all n_domains branches (see the module docstring).  The output is what
+        mods[0] gives on x: batch statistics when it trains (or tracks no running statistics), its running buffers in
+        eval -- normalised before any training branch that shares those buffers updates them, as in the reference's
+        order of calls."""
         second = "running_variance" if self.kind == "whiten" else "running_var"
         keep = {}                                  # distinct buffer pair -> product of (1 - factor) over its branches
         for m in mods:
@@ -156,12 +161,14 @@ class DomainTripleNorm(nn.Module):
             g_arg, b_arg = gamma, beta
         else:
             g_arg = b_arg = None
-        if not keep:
+        out = None
+        if not m0.training and m0.track_running_stats:
+            out = F.norm(x, g_arg, b_arg, momentum=0.0, update_running=False,
+                         running=[(m0.running_mean, getattr(m0, second))], **dict(common, training_stats=False))
+        for prod, pair in keep.values():           # one launch per distinct buffer set (one, in a loaded model)
+            y = F.norm(x, g_arg, b_arg, momentum=1.0 - prod, update_running=True, running=[pair], **common)
+            out = y if out is None else out
+        if out is None:
             out = F.norm(x, g_arg, b_arg, momentum=0.0, update_running=False,
                          running=[(m0.running_mean, getattr(m0, second))], **common)
-        else:
-            out = None
-            for prod, pair in keep.values():       # one launch per distinct buffer set (one, in a loaded model)
-                y = F.norm(x, g_arg, b_arg, momentum=1.0 - prod, update_running=True, running=[pair], **common)
-                out = y if out is None else out
         return out if self.kernel_epilogue else self._tensor_epilogue(out, gamma, beta, relu, residual)
