@@ -144,11 +144,10 @@ def lib() -> ctypes.CDLL:
 
 
 def channels_last_supported(channels: int, group_size: int) -> bool:
-    """Mirror of cl_supports() in csrc/norm_cl.cu: group sizes 1/2/4 with C/4 a power of two, at most 16384."""
+    """Mirror of cl_supports() in csrc/norm_cl.cu: group sizes 1/2/4 with C a multiple of 4 and C/4 at most 16384."""
     if group_size not in (1, 2, 4) or channels % 4:
         return False
-    c4 = channels // 4
-    return c4 & (c4 - 1) == 0 and c4 <= 16384
+    return 0 < channels // 4 <= 16384
 
 
 def small_bf16_supported(hw: int, group_size: int) -> bool:

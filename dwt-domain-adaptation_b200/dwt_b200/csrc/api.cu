@@ -141,7 +141,8 @@ inline const char* fam(bool bf16, const char* f32, const char* b16) { return bf1
 struct ClPlan { int nred, new_, S, gridy, gz_red, gz_ew; };
 ClPlan cl_plan(const dwt::Geom& g, int slots_red, int slots_ew, int unroll_red, int unroll_ew) {
   static const int seq_mb = env_int("DWT_CL_SEQ_MB", 1 << 30);  // experiment switch, off by default
-  const int C4 = g.C / 4, CW = C4 < 256 ? C4 : 256, rpi = 256 / CW, gridy = C4 / CW;
+  const int C4 = g.C / 4, gridy = dwt::cl_slabs(g.C), CW = (C4 + gridy - 1) / gridy,
+            rpi = 256 / dwt::cl_lane(g.C, CW);
   const long long rows = (long long)g.N * g.HW;
   const double mbytes = 4.0 * (double)g.D * (double)rows * (double)g.C / 1048576.0;
   const bool seq = g.D > 1 && mbytes >= (double)seq_mb;
@@ -239,7 +240,7 @@ Workspace carve(void* base, int64_t C, int GS, int D, size_t start = kOffScratch
   size_t red_floats = 1;
   if (dwt::cl_supports((int)C, GS)) {                      // channels-last path: per-CTA rows of C/4-column vectors
     const size_t W = (size_t)dwt::cl_bwd_width((int)C, GS);
-    const int C4 = (int)C / 4, gridy = C4 <= 256 ? 1 : C4 / 256;
+    const int gridy = dwt::cl_slabs((int)C);                // cl_plan's grid.x <= 3 SMs / grid.y
     const size_t cl = (size_t)D * (3 * sm_count() / gridy + 1) * W;     // one row per (domain, CTA of grid.x)
     if (cl > partial_floats) partial_floats = cl;
     red_floats = (size_t)D * 8 * W;
@@ -331,7 +332,7 @@ int check_bf16_geometry(bool bf16, bool nhwc, const dwt::Geom& g) {
   if (!bf16 || (nhwc ? dwt::cl_supports(g.C, g.GS) || tc_nhwc_supports(g) : small_bf16_supports(g) || tc_bf16_supports(g)))
     return DWT_OK;
   if (nhwc)
-    return fail(DWT_E_UNSUPPORTED, "channels-last bf16 activations are built for group_size 1, 2, 4 with C/4 a power of two, "
+    return fail(DWT_E_UNSUPPORTED, "channels-last bf16 activations are built for group_size 1, 2, 4 with C a multiple of 4, C/4 <= 16384, "
                                    "and for the tensor-core kernels: group_size 8, 16, 32, 64, HW >= 32 and a multiple of 4, "
                                    "N*HW >= 4096 per domain (C=%d HW=%d N=%d gs=%d)", g.C, g.HW, g.N, g.GS);
   return fail(DWT_E_UNSUPPORTED, "NCHW bf16 activations are built for group_size 1, 2, 4 and batch norm with HW a multiple "
@@ -369,7 +370,7 @@ int check_tc_nhwc_align(uintptr_t bits, const char* what) {
   return fail(DWT_E_INVALID, "%s must be 16-byte aligned (channels-last tensor-core kernels: TMA)", what);
 }
 int fail_nhwc_geometry(const dwt::Geom& g) {
-  return fail(DWT_E_UNSUPPORTED, "channels-last layout is built for group_size 1, 2, 4 with C/4 a power of two, and for the "
+  return fail(DWT_E_UNSUPPORTED, "channels-last layout is built for group_size 1, 2, 4 with C a multiple of 4, C/4 <= 16384, and for the "
               "tensor-core kernels: group_size 8, 16, 32, 64, HW >= 32 and a multiple of 4, N*HW >= 4096 per domain "
               "(C=%d HW=%d N=%d gs=%d)", g.C, g.HW, g.N, g.GS);
 }
@@ -648,7 +649,7 @@ int tail2_plan(Plan& p, int kind, bool bf16, const dwt_tail_site* s, const void*
   if (!s) return fail(DWT_E_INVALID, "null pointer argument");
   if (int rc = make_plan(p, K_STATS, K_APPLY, s[0].x, s[1].x, out, N, C, HW, GS, D, 4)) return rc;
   if (!dwt::cl_supports((int)C, GS))
-    return fail(DWT_E_UNSUPPORTED, "the two-site tail runs on the channels-last kernels: group_size 1, 2, 4 with C/4 a power of two (C=%lld gs=%d)",
+    return fail(DWT_E_UNSUPPORTED, "the two-site tail runs on the channels-last kernels: group_size 1, 2, 4 with C a multiple of 4, C/4 <= 16384 (C=%lld gs=%d)",
                 (long long)C, GS);
   for (int k = 0; k < 2; ++k)
     if (!s[k].x || !s[k].gamma || !s[k].beta || !s[k].save_mean || !s[k].save_w || !out) return fail(DWT_E_INVALID, "null pointer argument");

@@ -31,6 +31,8 @@ struct Geom {
   int nchunks;  // CTAs cooperating on one (domain, group)
   int ppc;      // (domain, group) problems served by one CTA (register-resident path; 1, 2, 4 or 8)
   float M;      // N * HW as float
+  int cw = 0;   // channels-last kernels: float4 columns per CTA slab (set by their launchers, norm_cl.cu)
+  int ls = 0;   // channels-last kernels: threads per row lane, >= cw (set by their launchers, norm_cl.cu)
 };
 
 struct FwdFin {

@@ -6,10 +6,13 @@
 //
 // Layout: x[(n*HW + p)*C + c].  One float4 = 4 consecutive channels of one pixel = one whitening
 // group (gs = 4), two groups (gs = 2) or four batch-norm channels (gs = 1).  A thread owns one float4
-// COLUMN q (channels 4q..4q+3) and walks down the rows (pixels); a warp therefore reads 512
-// contiguous bytes per step, and a thread's accumulators always belong to the same channels.
-// A CTA covers CW = min(C/4, 256) columns x a contiguous range of rows; 256/CW threads share a column
-// and are summed in shared memory.  Per-CTA partial moments go to global memory; one small finalize launch
+// COLUMN q (channels 4q..4q+3) and walks down the rows (pixels), and a thread's accumulators always belong to the
+// same channels.  A CTA covers a slab of CW columns x a contiguous range of rows: the 256 threads form rpi = 256/LS row
+// lanes of LS >= CW threads, the rpi threads of a column are summed in shared memory.  CW = LS = min(C/4, 256) when C/4
+// is a power of two: a warp reads 512 contiguous bytes (fp32) per step.  At any other C (a multiple of 4, C/4 <= 16384)
+// cl_slabs() picks the slabs and cl_lane() pads a lane to 8, 16 or 32 threads or to whole warps, so that every warp's
+// piece of a row is a contiguous run of >= 8 columns (128 bytes in fp32) starting on a 128-byte boundary of the slab;
+// the threads left over (lane padding, 256 mod LS, columns past the end of a ragged last slab) sit the sweep out.  Per-CTA partial moments go to global memory; one small finalize launch
 // (a warp per float4 column and domain) adds them in fixed order and does the dense algebra
 // (small_algebra.cuh) and the ordered running-statistic EMA -- no atomics.
 //
@@ -72,22 +75,30 @@ template <int GS> struct ClShape {
   static constexpr int BWD = NSUB * BWD1;
 };
 
-// Thread placement inside the CTA.
+// Thread placement inside the CTA.  grid.y = the column slabs chosen by cl_slabs(); a slab is CW = gm.cw =
+// ceil(C4 / grid.y) columns wide (the last one may be narrower).  Row lane k is threads [k*LS, k*LS + LS), LS = gm.ls
+// (cl_lane), and rpi = 256 / LS lanes share a column.  The threads with col >= CW (lane padding) or rsub >= rpi own no
+// row lane, and in a ragged last slab the threads with q >= C4 own no column: such a thread is not `active`.  It reads and writes no row, adds nothing to the shared sums and writes no
+// partial row, but reaches every __syncthreads() of its kernel.
 struct ClThread {
-  int C4, CW, rpi, col, rsub, q;
+  int C4, CW, LS, rpi, col, rsub, q;
+  bool active;
   __device__ __forceinline__ ClThread(const Geom& gm) {
     C4 = gm.C >> 2;
-    CW = C4 < kT ? C4 : kT;
-    rpi = kT / CW;
-    col = threadIdx.x % CW;
-    rsub = threadIdx.x / CW;
+    CW = gm.cw;
+    LS = gm.ls;
+    rpi = kT / LS;
+    col = threadIdx.x % LS;
+    rsub = threadIdx.x / LS;
     q = blockIdx.y * CW + col;
+    active = col < CW && rsub < rpi && q < C4;
   }
 };
 
 // The CTAs of grid.x sweep the rows of one domain as a moving window of chunks of rpi*UNROLL consecutive rows:
 // chunk c belongs to CTA c mod gridDim.x; DESC walks from the last chunk to the first.  body(r) gets the first
 // row of the calling thread inside the chunk (its rows are r + u*rpi, u < UNROLL, to be guarded by r < rows).
+// Only active threads may call it.
 template <int UNROLL, bool DESC, class F>
 __device__ __forceinline__ void sweep_rows(const ClThread& t, unsigned rows, F&& body) {
   const unsigned krows = (unsigned)t.rpi * UNROLL, nch = (rows + krows - 1) / krows;
@@ -109,18 +120,21 @@ __device__ __forceinline__ float as_stored(float v) {
 }
 
 // Sum the per-thread accumulators of the rpi threads that share a column; thread rsub == 0 of every column
-// then holds the CTA total.  sRed must hold kT * NACC floats.
+// then holds the CTA total.  sRed must hold kT * NACC floats.  Threads without a row lane (rsub >= rpi) store nothing;
+// the sums read lanes r < rpi only.
 template <int NACC>
 __device__ __forceinline__ void column_reduce(const ClThread& t, float (&acc)[NACC], float* sRed) {
   if (t.rpi == 1) return;
+  if (t.rsub < t.rpi) {
 #pragma unroll
-  for (int i = 0; i < NACC; ++i) sRed[i * kT + threadIdx.x] = acc[i];
+    for (int i = 0; i < NACC; ++i) sRed[i * kT + threadIdx.x] = acc[i];
+  }
   __syncthreads();
   if (t.rsub == 0) {
 #pragma unroll
     for (int i = 0; i < NACC; ++i) {
       float s = acc[i];
-      for (int r = 1; r < t.rpi; ++r) s += sRed[i * kT + r * t.CW + t.col];
+      for (int r = 1; r < t.rpi; ++r) s += sRed[i * kT + r * t.LS + t.col];
       acc[i] = s;
     }
   }
@@ -149,7 +163,7 @@ __global__ void __launch_bounds__(kT, 3) cl_stats_kernel(const T* __restrict__ x
     // activations show (at most 14 over the sites of 20 training steps), so they keep the first rows' K and their
     // statistics bit for bit.
     float K[4] = {0.f, 0.f, 0.f, 0.f};
-    {
+    if (t.active) {
       const unsigned np = rows < 8 ? rows : 8;
       for (unsigned r = 0; r < np; ++r) {
         const float4 v = ld4(xd + (size_t)r * gm.C);
@@ -177,7 +191,7 @@ __global__ void __launch_bounds__(kT, 3) cl_stats_kernel(const T* __restrict__ x
     float acc[S::FWD];
 #pragma unroll
     for (int i = 0; i < S::FWD; ++i) acc[i] = 0.f;
-    sweep_rows<UNROLL, true>(t, rows, [&](unsigned r) {
+    if (t.active) sweep_rows<UNROLL, true>(t, rows, [&](unsigned r) {
       float4 v[UNROLL];
 #pragma unroll
       for (int u = 0; u < UNROLL; ++u) {
@@ -200,7 +214,7 @@ __global__ void __launch_bounds__(kT, 3) cl_stats_kernel(const T* __restrict__ x
       }
     });
     column_reduce<S::FWD>(t, acc, sRed);
-    if (t.rsub == 0) {
+    if (t.rsub == 0 && t.active) {
       float* dst = partial + (((size_t)d * gridDim.x + blockIdx.x) * t.C4 + t.q) * S::FWD;
 #pragma unroll
       for (int i = 0; i < S::FWD; ++i) dst[i] = acc[i];
@@ -271,7 +285,8 @@ __device__ __forceinline__ void cl_fwd_finalize_site(const float* __restrict__ p
   const int s = threadIdx.x, ql = threadIdx.y, d = threadIdx.z, q = blockIdx.x * blockDim.y + ql;
   const int W = (gm.C >> 2) * SH::FWD;
   const float invM = 1.f / gm.M;
-  const bool lead = s < SH::NSUB;                          // lane s finalizes group q * NSUB + s
+  const bool colok = q < (gm.C >> 2);                      // the grid's last block may reach past the last column
+  const bool lead = colok && s < SH::NSUB;                 // lane s finalizes group q * NSUB + s
   const int g = q * SH::NSUB + (lead ? s : 0);
   const bool direct = gm.D == 1 || fin.aliased == 0;       // this domain owns its buffers
   // the running buffers this lane will update are fetched first: their (DRAM) latency hides behind the row sums
@@ -287,7 +302,7 @@ __device__ __forceinline__ void cl_fwd_finalize_site(const float* __restrict__ p
   pdl_launch_dependents();
   pdl_wait();                                       // the reduction's partial rows and pilot shifts are complete
   float a[SH::FWD];
-  column_row_sum<SH::FWD>(partial + (size_t)d * nrows * W + (size_t)q * SH::FWD, nrows, W, a);
+  if (colok) column_row_sum<SH::FWD>(partial + (size_t)d * nrows * W + (size_t)q * SH::FWD, nrows, W, a);   // warp-uniform
   if (lead) {
     float v[SH::FWD1];
     take_group<SH::NSUB, SH::FWD1>(a, s, v);
@@ -378,7 +393,8 @@ __global__ void __launch_bounds__(kT, 3) cl_apply_kernel(const T* __restrict__ x
   // rows per thread and step (the grid shape comes from cl_plan either way): two sites' maps need the registers
   constexpr int UNROLL = DS ? 2 : (RES ? 4 : 8);
   const ClThread t(gm);
-  const unsigned rows = (unsigned)gm.N * gm.HW;
+  if (!t.active) return;                            // no barrier below: a thread without rows can leave
+  const unsigned rows = (unsigned)gm.N * gm.HW;   // rows * C < 2^31 (make_plan): 32-bit offsets inside a domain
   pdl_wait();                                       // save_mean / save_w of the finalize launch are complete
   CL_FOR_DOMAINS(d, gm, false) {
     float Wp[S::NSUB][S::NM], bp[S::NSUB][GS], Wd[DS ? S::NSUB : 1][S::NM], bd[DS ? S::NSUB : 1][GS];
@@ -402,8 +418,8 @@ __global__ void __launch_bounds__(kT, 3) cl_apply_kernel(const T* __restrict__ x
       for (int u = 0; u < UNROLL; ++u) {
         const unsigned rr = r + u * t.rpi;
         if (rr < rows) {
-          v[u] = ld4(xd + (size_t)rr * gm.C);
-          if constexpr (RES) rs[u] = ld4(rd + (size_t)rr * gm.C);
+          v[u] = ld4(xd + rr * (unsigned)gm.C);
+          if constexpr (RES) rs[u] = ld4(rd + rr * (unsigned)gm.C);
         }
       }
 #pragma unroll
@@ -435,8 +451,8 @@ __global__ void __launch_bounds__(kT, 3) cl_apply_kernel(const T* __restrict__ x
               o[s * GS + c] = (EPI & DWT_EPI_RELU) ? fmaxf(z, 0.f) : z;
             }
           }
-          st4(yd + (size_t)rr * gm.C, make_float4(o[0], o[1], o[2], o[3]));
-          if constexpr (RES) { if (mask != nullptr) md[(size_t)rr * t.C4] = (uint8_t)bits; }
+          st4(yd + rr * (unsigned)gm.C, make_float4(o[0], o[1], o[2], o[3]));
+          if constexpr (RES) { if (mask != nullptr) md[rr * (unsigned)t.C4] = (uint8_t)bits; }
         }
       }
     });
@@ -480,17 +496,19 @@ __global__ void __launch_bounds__(kT, 2) cl_bwd_reduce_kernel(const T* __restric
   pdl_launch_dependents();
   CL_FOR_DOMAINS(d, gm, true) {
     float Wp[S::NSUB][S::NM], bp[S::NSUB][GS], mu[NS][4];
+    if (t.active) {                                 // a thread without a column has no parameters to read
 #pragma unroll
-    for (int s = 0; s < S::NSUB; ++s) {
-      const int g = t.q * S::NSUB + s;
-      if constexpr (RELU)
-        load_forward_map<GS, EPI>(save_w + ((size_t)d * gm.G + g) * GS * GS, save_mean + (size_t)d * gm.C + g * GS,
-                                  gamma + g * GS, beta + g * GS, Wp[s], bp[s]);
-    }
+      for (int s = 0; s < S::NSUB; ++s) {
+        const int g = t.q * S::NSUB + s;
+        if constexpr (RELU)
+          load_forward_map<GS, EPI>(save_w + ((size_t)d * gm.G + g) * GS * GS, save_mean + (size_t)d * gm.C + g * GS,
+                                    gamma + g * GS, beta + g * GS, Wp[s], bp[s]);
+      }
 #pragma unroll
-    for (int k = 0; k < NS; ++k) {
-      const float4 m4 = ldg4((k ? save_mean_d : save_mean) + (size_t)d * gm.C + 4 * t.q);
-      mu[k][0] = m4.x; mu[k][1] = m4.y; mu[k][2] = m4.z; mu[k][3] = m4.w;
+      for (int k = 0; k < NS; ++k) {
+        const float4 m4 = ldg4((k ? save_mean_d : save_mean) + (size_t)d * gm.C + 4 * t.q);
+        mu[k][0] = m4.x; mu[k][1] = m4.y; mu[k][2] = m4.z; mu[k][3] = m4.w;
+      }
     }
     float acc[NS][S::BWD];
 #pragma unroll
@@ -508,7 +526,7 @@ __global__ void __launch_bounds__(kT, 2) cl_bwd_reduce_kernel(const T* __restric
     // rows per load batch: all of the chunk's rows, or (two sites) half of them, so that both sites' accumulators stay
     // in registers.  The rows are accumulated in the same order either way.
     constexpr int H = DS ? UNROLL / 2 : UNROLL;
-    sweep_rows<UNROLL, true>(t, rows, [&](unsigned r0) {
+    if (t.active) sweep_rows<UNROLL, true>(t, rows, [&](unsigned r0) {
 #pragma unroll
      for (int h = 0; h < UNROLL; h += H) {
       const unsigned r = r0 + h * t.rpi;
@@ -577,7 +595,7 @@ __global__ void __launch_bounds__(kT, 2) cl_bwd_reduce_kernel(const T* __restric
     for (int k = 0; k < NS; ++k) {
       if (k) __syncthreads();                          // sRed is reused by the second site
       column_reduce<S::BWD>(t, acc[k], sRed);
-      if (t.rsub == 0) {
+      if (t.rsub == 0 && t.active) {
         float* dst = partial + k * pstride + (((size_t)d * gridDim.x + blockIdx.x) * t.C4 + t.q) * S::BWD;
 #pragma unroll
         for (int i = 0; i < S::BWD; ++i) dst[i] = acc[k][i];
@@ -594,11 +612,12 @@ __device__ __forceinline__ void cl_bwd_finalize_site(const float* __restrict__ p
   using SH = ClShape<GS>;
   const int s = threadIdx.x, d = threadIdx.z, q = blockIdx.x * blockDim.y + threadIdx.y;
   const int W = (gm.C >> 2) * SH::BWD;
+  const bool colok = q < (gm.C >> 2);               // the grid's last block may reach past the last column
   pdl_launch_dependents();
   pdl_wait();                                       // the backward reduction's partial rows are complete
   float a[SH::BWD];
-  column_row_sum<SH::BWD>(partial + (size_t)d * nrows * W + (size_t)q * SH::BWD, nrows, W, a);
-  if (s < SH::NSUB) {                               // lane s finalizes group q * NSUB + s
+  if (colok) column_row_sum<SH::BWD>(partial + (size_t)d * nrows * W + (size_t)q * SH::BWD, nrows, W, a);   // warp-uniform
+  if (colok && s < SH::NSUB) {                      // lane s finalizes group q * NSUB + s
     float v[SH::BWD1], R[GS][GS], sdz[GS];
     take_group<SH::NSUB, SH::BWD1>(a, s, v);
 #pragma unroll
@@ -609,7 +628,7 @@ __device__ __forceinline__ void cl_bwd_finalize_site(const float* __restrict__ p
   }
   if (!((fin.epi & DWT_EPI_AFFINE) && fin.dgamma != nullptr)) return;
   __syncthreads();                                  // the block's dgb_part writes (global) are visible block-wide
-  if (d == 0 && s < 4) {                            // lane i sums channel 4q + i over the domains
+  if (colok && d == 0 && s < 4) {                   // lane i sums channel 4q + i over the domains
     const int ch = 4 * q + s;
     float sg = 0.f, sb = 0.f;
     for (int dd = 0; dd < gm.D; ++dd) {
@@ -682,6 +701,7 @@ __global__ void __launch_bounds__(kT, 2) cl_bwd_apply_kernel(const T* __restrict
   static_assert(!DS || (!D2 && !RELU), "the two-site tail's apply reads dz");
   constexpr int NS = DS ? 2 : 1;
   const ClThread t(gm);
+  if (!t.active) return;                            // no barrier below: a thread without rows can leave
   const unsigned rows = (unsigned)gm.N * gm.HW;
   pdl_wait();                                       // the coefficients of the backward finalize launch are complete
   CL_FOR_DOMAINS(d, gm, false) {
@@ -789,20 +809,75 @@ inline void launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, cudaStream
   cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
 }
 
-// grid.x = CTAs sweeping one domain, grid.y = column slabs, grid.z = 1 (domains one after the other) or D
-inline dim3 cl_grid(const Geom& gm, int nctas, int gz) {
-  const int C4 = gm.C / 4, CW = C4 < kT ? C4 : kT;
-  return dim3(nctas, C4 / CW, gz);
-}
-
 }  // namespace
 
-// C/4 must be a power of two (every thread keeps one float4 column for the whole kernel)
+// Every thread keeps one float4 column for the whole kernel; C/4 <= 16384 bounds the groups the workspace head counts.
 bool cl_supports(int C, int GS) {
   if (!(GS == 1 || GS == 2 || GS == 4) || C % 4 != 0) return false;
   const int c4 = C / 4;
-  return (c4 & (c4 - 1)) == 0 && c4 <= 16384;
+  return c4 >= 1 && c4 <= 16384;
 }
+
+// Threads per row lane of a slab CW columns wide.  C/4 < 8 (C < 32): CW itself.  Otherwise 8, 16 or 32 (lanes pack
+// whole into warps) or whole warps: a warp's piece of one row then starts on a multiple of 8 columns of the slab.
+// A power-of-two C/4 keeps LS = CW.
+int cl_lane(int C, int CW) {
+  if (C / 4 < 8) return CW;
+  if (CW <= 32) {
+    int l = 8;
+    while (l < CW) l <<= 1;
+    return l;
+  }
+  return (CW + 31) / 32 * 32;
+}
+
+namespace {
+// Share of a CTA's threads that own a row lane and a column with `n` slabs, or -1 when n is not allowed: slabs of
+// at least 8 columns, none empty, and every warp's piece of a row (in the last, ragged slab too) at least 8 columns --
+// a lane of LS <= 32 threads is one warp's piece; a wider lane is cut into 32-column pieces and a remainder.
+double cl_busy(int C4, int n) {
+  const int cw = (C4 + n - 1) / n, last = C4 - (n - 1) * cw;
+  if (cw < 8 || last <= 0) return -1.0;
+  const int ls = cl_lane(4 * C4, cw);
+  for (int v : {cw, last})
+    if (ls <= 32 ? v < 8 : (v % 32 != 0 && v % 32 < 8)) return -1.0;
+  return (double)C4 * (kT / ls) / ((double)n * kT);
+}
+}  // namespace
+
+// Column slabs (grid.y) of the sweeping kernels; their slab width is CW = ceil(C4 / slabs) (cl_geom).
+// C4 a power of two: slabs of min(C4, 256) columns, every thread busy.  C4 < 8: one slab.  Otherwise, among the slab
+// counts cl_busy() allows, the fewest whose share of busy threads is within 1/64 of the best.  C4 = 144, for example:
+// one 144-column slab (lanes of 160 threads) keeps 144 of 256 threads busy, nine 16-column slabs all of them.
+int cl_slabs(int C) {
+  const int C4 = C / 4;
+  if ((C4 & (C4 - 1)) == 0) return C4 <= kT ? 1 : C4 / kT;
+  if (C4 < 8) return 1;
+  thread_local int memo_c = 0, memo_s = 0;       // the search is a few thousand steps at most; calls repeat a width
+  if (memo_c == C) return memo_s;
+  const int lo = (C4 + kT - 1) / kT, hi = C4 / 8;
+  double top = 0.0;
+  for (int n = lo; n <= hi; ++n) top = fmax(top, cl_busy(C4, n));
+  int best = lo;
+  for (int n = lo; n <= hi; ++n)
+    if (cl_busy(C4, n) >= 0.0 && 64.0 * cl_busy(C4, n) >= 64.0 * top - 1.0) { best = n; break; }
+  memo_c = C;
+  memo_s = best;
+  return best;
+}
+
+namespace {
+// grid.x = CTAs sweeping one domain, grid.y = column slabs, grid.z = 1 (domains one after the other) or D
+inline dim3 cl_grid(const Geom& gm, int nctas, int gz) { return dim3(nctas, cl_slabs(gm.C), gz); }
+// the geometry a sweeping kernel gets: gm with the slab width and lane stride of cl_grid's grid.y
+inline Geom cl_geom(const Geom& gm) {
+  Geom g = gm;
+  const int C4 = gm.C / 4, slabs = cl_slabs(gm.C);
+  g.cw = (C4 + slabs - 1) / slabs;
+  g.ls = cl_lane(gm.C, g.cw);
+  return g;
+}
+}  // namespace
 int cl_fwd_width(int C, int GS) { return (C / 4) * (4 / GS) * (GS + GS * (GS + 1) / 2); }
 int cl_bwd_width(int C, int GS) { return (C / 4) * (4 / GS) * (GS * GS + GS); }
 
@@ -815,12 +890,14 @@ int cl_bwd_width(int C, int GS) { return (C / 4) * (4 / GS) * (GS * GS + GS); }
 #define CL_OUT(P_) static_cast<TT*>(P_)
 
 void cl_stats(const void* x, bool bf16, const Geom& gm, int nctas, int gz, float* partial, float* shift, cudaStream_t st) {
-  CL_T(bf16, CL_GS(gm.GS, (cl_stats_kernel<TT, kGS><<<cl_grid(gm, nctas, gz), kT, 0, st>>>(CL_IN(x), gm, partial, shift))));
+  CL_T(bf16, CL_GS(gm.GS, (cl_stats_kernel<TT, kGS><<<cl_grid(gm, nctas, gz), kT, 0, st>>>(CL_IN(x), cl_geom(gm), partial, shift))));
 }
+// finalize launches: ceil(C4 / kFinQ) blocks of kFinQ columns (the last block's extra columns idle)
 inline dim3 fin_block(const Geom& gm) { const int c4 = gm.C / 4; return dim3(32, c4 < kFinQ ? c4 : kFinQ, gm.D); }
+inline unsigned fin_blocks(const Geom& gm, const dim3& b) { return (unsigned)((gm.C / 4 + b.y - 1) / b.y); }
 void cl_fwd_finalize(const float* partial, int nrows, const float* shift, const Geom& gm, const FwdFin& fin, cudaStream_t st,
                      const FwdFin* fin2, size_t pstride, size_t sstride) {
-  const dim3 b = fin_block(gm), g((gm.C / 4) / b.y, fin2 ? 2 : 1);
+  const dim3 b = fin_block(gm), g(fin_blocks(gm, b), fin2 ? 2 : 1);
   CL_GS(gm.GS, (launch_k(cl_fwd_finalize_kernel<kGS>, g, b, st, use_pdl(), partial, pstride, nrows, shift, sstride, gm, fin, fin2 ? *fin2 : fin)));
 }
 void cl_apply(const void* x, void* y, bool bf16, const Geom& gm, int nctas, int gz, int epi, const float* mean, const float* w,
@@ -829,18 +906,18 @@ void cl_apply(const void* x, void* y, bool bf16, const Geom& gm, int nctas, int 
   CL_T(bf16, {
     const TT* tnul = nullptr;
     if (epi == 7) {
-      CL_GS(gm.GS, (launch_k(cl_apply_kernel<TT, kGS, 7, false>, cl_grid(gm, nctas, gz), dim3(kT), st, use_pdl(), CL_IN(x), CL_OUT(y), gm, mean, w,
+      CL_GS(gm.GS, (launch_k(cl_apply_kernel<TT, kGS, 7, false>, cl_grid(gm, nctas, gz), dim3(kT), st, use_pdl(), CL_IN(x), CL_OUT(y), cl_geom(gm), mean, w,
                              gamma, beta, CL_IN(residual), mask, nul, nul, nul, nul)));
     } else {
       CL_GS(gm.GS, CL_EPI(epi, (launch_k(cl_apply_kernel<TT, kGS, kEPI, false>, cl_grid(gm, nctas, gz), dim3(kT), st, use_pdl(), CL_IN(x), CL_OUT(y),
-                                         gm, mean, w, gamma, beta, tnul, (uint8_t*)nullptr, nul, nul, nul, nul))));
+                                         cl_geom(gm), mean, w, gamma, beta, tnul, (uint8_t*)nullptr, nul, nul, nul, nul))));
     }
   });
 }
 void cl_tail2_apply(const void* x, const void* xd, void* y, bool bf16, const Geom& gm, int nctas, int gz, const float* mean, const float* w,
                     const float* gamma, const float* beta, const float* mean_d, const float* w_d, const float* gamma_d,
                     const float* beta_d, uint8_t* mask, cudaStream_t st) {
-  CL_T(bf16, CL_GS(gm.GS, (launch_k(cl_apply_kernel<TT, kGS, 7, true>, cl_grid(gm, nctas, gz), dim3(kT), st, use_pdl(), CL_IN(x), CL_OUT(y), gm, mean,
+  CL_T(bf16, CL_GS(gm.GS, (launch_k(cl_apply_kernel<TT, kGS, 7, true>, cl_grid(gm, nctas, gz), dim3(kT), st, use_pdl(), CL_IN(x), CL_OUT(y), cl_geom(gm), mean,
                                     w, gamma, beta, CL_IN(xd), mask, mean_d, w_d, gamma_d, beta_d))));
 }
 void cl_bwd_reduce(const void* x, const void* dout, const void* dout2, bool bf16, const Geom& gm, int nctas, int gz, int epi, const float* mean,
@@ -849,7 +926,7 @@ void cl_bwd_reduce(const void* x, const void* dout, const void* dout2, bool bf16
   CL_T(bf16, {
     const TT* tnul = nullptr;
     CL_GS(gm.GS, CL_D2(dout2, CL_EPI_BWD(epi, (cl_bwd_reduce_kernel<TT, kGS, kEPI, kD2, false><<<cl_grid(gm, nctas, gz), kT, 0, st>>>(
-                                                  CL_IN(x), CL_IN(dout), CL_IN(dout2), gm, mean, w, gamma, beta, mask, CL_OUT(dz), partial, tnul,
+                                                  CL_IN(x), CL_IN(dout), CL_IN(dout2), cl_geom(gm), mean, w, gamma, beta, mask, CL_OUT(dz), partial, tnul,
                                                   nul, 0)))));
   });
 }
@@ -858,11 +935,11 @@ void cl_tail2_bwd_reduce(const void* x, const void* xd, const void* dout, const 
                          cudaStream_t st) {
   const float* nul = nullptr;
   CL_T(bf16, CL_GS(gm.GS, CL_D2(dout2, (cl_bwd_reduce_kernel<TT, kGS, 7, kD2, true><<<cl_grid(gm, nctas, gz), kT, 0, st>>>(
-                                           CL_IN(x), CL_IN(dout), CL_IN(dout2), gm, mean, nul, nul, nul, mask, CL_OUT(dz), partial, CL_IN(xd),
+                                           CL_IN(x), CL_IN(dout), CL_IN(dout2), cl_geom(gm), mean, nul, nul, nul, mask, CL_OUT(dz), partial, CL_IN(xd),
                                            mean_d, pstride)))));
 }
 void cl_bwd_finalize(const float* partial, int nrows, const Geom& gm, const BwdFin& fin, cudaStream_t st, const BwdFin* fin2, size_t pstride) {
-  const dim3 b = fin_block(gm), g((gm.C / 4) / b.y, fin2 ? 2 : 1);
+  const dim3 b = fin_block(gm), g(fin_blocks(gm, b), fin2 ? 2 : 1);
   CL_GS(gm.GS, (launch_k(cl_bwd_finalize_kernel<kGS>, g, b, st, use_pdl(), partial, pstride, nrows, gm, fin, fin2 ? *fin2 : fin)));
 }
 void cl_bwd_apply(const void* x, const void* dout, const void* dout2, void* dx, bool bf16, const Geom& gm, int nctas, int gz, int epi,
@@ -871,7 +948,7 @@ void cl_bwd_apply(const void* x, const void* dout, const void* dout2, void* dx, 
   CL_T(bf16, {
     const TT* tnul = nullptr;
     CL_GS(gm.GS, CL_D2(dout2, CL_EPI(epi, (launch_k(cl_bwd_apply_kernel<TT, kGS, kEPI, kD2, false>, cl_grid(gm, nctas, gz), dim3(kT), st, use_pdl(),
-                                                    CL_IN(x), CL_IN(dout), CL_IN(dout2), CL_OUT(dx), gm, coef, mean, w, gamma, beta, tnul,
+                                                    CL_IN(x), CL_IN(dout), CL_IN(dout2), CL_OUT(dx), cl_geom(gm), coef, mean, w, gamma, beta, tnul,
                                                     (TT*)nullptr, nul)))));
   });
 }
@@ -881,7 +958,7 @@ void cl_tail2_bwd_apply(const void* x, const void* xd, const void* dz, void* dx,
   CL_T(bf16, {
     const TT* tnul = nullptr;
     CL_GS(gm.GS, (launch_k(cl_bwd_apply_kernel<TT, kGS, 1, false, true>, cl_grid(gm, nctas, gz), dim3(kT), st, use_pdl(), CL_IN(x), CL_IN(dz), tnul,
-                           CL_OUT(dx), gm, coef, nul, nul, nul, nul, CL_IN(xd), CL_OUT(dxd), coef_d)));
+                           CL_OUT(dx), cl_geom(gm), coef, nul, nul, nul, nul, CL_IN(xd), CL_OUT(dxd), coef_d)));
   });
 }
 

@@ -71,8 +71,12 @@ int tc_apply(const void* x, void* y, bool bf16, bool nhwc, const Geom& gm, int n
 int tc_bwd_apply(const void* x, const void* dout, void* dx, bool bf16, bool nhwc, const Geom& gm, int nctas, const float* coef,
                  const float* save_mean, const float* dybar, cudaStream_t st);
 
-// channels-last (NHWC) register-resident path, GS in {1,2,4}, C/4 a power of two  (norm_cl.cu)
+// channels-last (NHWC) register-resident path, GS in {1,2,4}, C a multiple of 4, C/4 <= 16384  (norm_cl.cu)
 bool cl_supports(int C, int GS);
+// column slabs (grid.y) of the sweeping kernels; every launch plan and workspace size of a call uses this count
+int cl_slabs(int C);
+// threads per row lane of a slab CW columns wide
+int cl_lane(int C, int CW);
 int cl_fwd_width(int C, int GS);
 int cl_bwd_width(int C, int GS);
 // Activation pointers are void: fp32, or bf16 when `bf16` (DWT_DTYPE_BF16; the same kernels, loads widened to fp32 and

@@ -67,7 +67,7 @@ extern "C" {
  * default = [n_domains*N, C, HW] (NCHW); DWT_LAYOUT_NHWC = [n_domains*N, HW, C] (torch.channels_last: the layout
  * cuDNN's tensor-core convolutions want, so a channels-last model needs no NCHW<->NHWC copies around its convolutions).
  * Built for two kernel families:
- *   - group sizes 1, 2, 4 with C/4 a power of two (the channels-last kernels, every epilogue, dout2);
+ *   - group sizes 1, 2, 4 with C a multiple of 4, C/4 <= 16384 (the channels-last kernels, every epilogue, dout2);
  *   - whitening at group sizes 8, 16, 32, 64 (fp32 or bf16) and 128 (fp32) on the tensor-core kernels: HW >= 32 and
  *     HW % 4 == 0, N*HW >= 4096 per domain, x / y / dout / dx 16-byte aligned (else DWT_E_INVALID), epilogue 0 and no
  *     dout2 (else DWT_E_UNSUPPORTED).  Same schedule and arithmetic as the NCHW call: every output, statistic, running-buffer update and
@@ -79,8 +79,8 @@ extern "C" {
  * default = fp32; DWT_DTYPE_BF16 = every ACTIVATION pointer of the call points at bfloat16 -- x, y, residual, dout,
  * dout2, dx, dresidual / dz, dwt_tail_site.x / .dx, and the max-pool's x, y, dy, dx.  Running buffers, gamma / beta and
  * their gradients, save_mean / save_w and the workspace stay fp32.  Built for three kernel families:
- *   - channels-last (DWT_LAYOUT_NHWC; the tail and the max-pool are channels-last anyway), group size 1, 2, 4 with C/4
- *     a power of two; bf16 tensors 8-byte aligned;
+ *   - channels-last (DWT_LAYOUT_NHWC; the tail and the max-pool are channels-last anyway), group size 1, 2, 4 with C
+ *     a multiple of 4, C/4 <= 16384; bf16 tensors 8-byte aligned;
  *   - NCHW whitening at group size 1, 2, 4 and NCHW batch norm (dwt_whiten_*, dwt_bn_*; every mode and epilogue) with
  *     HW % 4 == 0; x, y, residual, dout and dx 8-byte aligned; no dout2 (DWT_E_UNSUPPORTED, as in fp32 NCHW);
  *   - whitening on the tensor-core kernels: group size 8, 16, 32, 64, HW >= 32, N*HW >= 4096 per domain; NCHW with
@@ -192,7 +192,7 @@ DWT_API int dwt_bn_bwd(const float *x, const float *dout, const float *dout2, fl
 
 /*
  * Two-site residual tail of a downsampling Bottleneck (block 0 of a stage, resnet50_dwt_mec_officehome.py:236-240),
- * training mode, channels-last only:
+ * training mode, channels-last only (the channels-last kernels: C a multiple of 4, C/4 <= 16384, else DWT_E_UNSUPPORTED):
  *   out = relu(site(x) + site_d(xd)),   site(x)    = gamma   W   (x  - mu)   + beta     (the norm site after conv3)
  *                                       site_d(xd) = gamma_d W_d (xd - mu_d) + beta_d   (the downsample branch's site)
  * sites[0] describes site, sites[1] site_d; both have the same N, C, HW, group_size and n_domains.  The identity
