@@ -151,14 +151,15 @@ def channels_last_supported(channels: int, group_size: int) -> bool:
 
 
 def small_bf16_supported(hw: int, group_size: int) -> bool:
-    """Mirror of the C ABI's bf16 rule for the NCHW register-resident kernels (csrc/api.cu, small_bf16_supports):
+    """Mirror of the C ABI's bf16 rule for the NCHW register-resident kernels (csrc/api.cu, route(): the SMALL family):
     whitening at group sizes 1, 2, 4 and batch norm (group_size 1) take bf16 activations when HW is a multiple of 4 (a
     thread reads four pixels of a channel row as 8 bytes).  The tensors also need an 8-byte-aligned data_ptr()."""
     return group_size in (1, 2, 4) and hw % 4 == 0
 
 
 def tensor_core_bf16_supported(n: int, channels: int, hw: int, group_size: int) -> bool:
-    """Mirror of the C ABI's bf16 NCHW rule (csrc/api.cu, tc_bf16_supports over tc_supports in csrc/norm_tc.cu): the
+    """Mirror of the C ABI's bf16 NCHW rule (csrc/api.cu, route(): the TC family, over tc_supports in
+    csrc/norm_tc.cu): the
     tensor-core whitening kernels take bf16 activations for group sizes 8..64 dividing 64, HW >= 32 and a multiple of 8
     (16-byte TMA rows), and at least 4096 samples per domain (n = images per domain).  The tensors also need a
     16-byte-aligned data_ptr()."""
@@ -167,7 +168,7 @@ def tensor_core_bf16_supported(n: int, channels: int, hw: int, group_size: int) 
 
 
 def tensor_core_nhwc_supported(n: int, channels: int, hw: int, group_size: int) -> bool:
-    """Mirror of the C ABI's channels-last tensor-core rule (csrc/api.cu, tc_nhwc_supports): whitening at group sizes
+    """Mirror of the C ABI's channels-last tensor-core rule (csrc/api.cu, route(): the TC family): whitening at group sizes
     8..64 dividing 64, and 128, runs on channels-last tensors when HW >= 32 and a multiple of 4 and there are at least
     4096 samples per domain (n = images per domain); fp32 and bf16 alike up to 64, fp32 only at 128 (bf16 upcasts).
     The tensors also need a 16-byte-aligned data_ptr()."""

@@ -264,7 +264,6 @@ struct Plan {
   dwt::Geom gm_ew;    // same geometry shaped for the elementwise kernel of this call
   int vec;            // 4 when rows can be read as float4
   int chunks_ew;      // grid.x of the elementwise (apply) kernel
-  bool small;
 };
 
 void shape(dwt::Geom& g, int64_t work_units, KernelKind kind, bool small, int* chunks) {
@@ -304,80 +303,95 @@ int make_plan(Plan& p, KernelKind reduce_kind, KernelKind ew_kind, const void* a
   g.M = (float)((double)N * (double)HW);
   const uintptr_t bits = (uintptr_t)a0 | (uintptr_t)a1 | (uintptr_t)a2;
   p.vec = (HW % 4 == 0 && bits % (4 * elem_bytes) == 0) ? 4 : 1;
-  p.small = dwt::small_supports(GS);
+  const bool small = dwt::small_supports(GS);
   int64_t work_units;   // CTA-sized pieces of work available per (domain, group)
-  if (p.small) work_units = (N * (HW / p.vec) + dwt::kThreads * 2 - 1) / (dwt::kThreads * 2);
+  if (small) work_units = (N * (HW / p.vec) + dwt::kThreads * 2 - 1) / (dwt::kThreads * 2);
   else work_units = (N * HW + 127) / 128;
   if (work_units < 1) work_units = 1;
-  shape(g, work_units, reduce_kind, p.small, &g.nchunks);
+  shape(g, work_units, reduce_kind, small, &g.nchunks);
   p.gm_ew = g;
-  shape(p.gm_ew, work_units, ew_kind, p.small, &p.chunks_ew);
+  shape(p.gm_ew, work_units, ew_kind, small, &p.chunks_ew);
   p.gm_ew.nchunks = g.nchunks;
   return DWT_OK;
 }
 
-// DWT_LAYOUT_NHWC runs the channels-last kernels (group sizes 1, 2, 4, cl_supports) or, at group sizes 8..64, the
-// tensor-core family on channels-last tensors: tc_supports with HW % 4 == 0 (the NCHW rule, whose vec == 4 needs it too),
-// in fp32 and bf16 alike (the TMA rows are C channels: 16-byte strides for every group size that tiles 64), with x, y,
-// dout and dx 16-byte aligned.
-bool tc_nhwc_supports(const dwt::Geom& g) { return dwt::tc_supports(g, 4) && g.HW % 4 == 0; }
-// DWT_DTYPE_BF16 (dwt_b200.h): bf16 activations run the channels-last kernels (group sizes 1, 2, 4), where a thread's
-// four channels are 8 bytes, so that is the alignment the tensors need (16 for fp32); the NCHW register-resident kernels
-// (group sizes 1, 2, 4 and batch norm), where a thread's four pixels of a channel row are 8 bytes: HW % 4 == 0 and
-// 8-byte-aligned tensors, the fp32 plan with vec == 4; and the tensor-core family (group sizes 8..64, tc_supports),
-// whose TMA loads need 16-byte rows (NCHW: HW % 8 == 0) and a 16-byte-aligned x / dout
-bool tc_bf16_supports(const dwt::Geom& g) { return dwt::tc_supports(g, 4) && g.HW % 8 == 0; }
-bool small_bf16_supports(const dwt::Geom& g) { return dwt::small_supports(g.GS) && g.HW % 4 == 0; }
-int check_bf16_geometry(bool bf16, bool nhwc, const dwt::Geom& g) {
-  if (!bf16 || (nhwc ? dwt::cl_supports(g.C, g.GS) || tc_nhwc_supports(g) : small_bf16_supports(g) || tc_bf16_supports(g)))
-    return DWT_OK;
-  if (nhwc)
-    return fail(DWT_E_UNSUPPORTED, "channels-last bf16 activations are built for group_size 1, 2, 4 with C a multiple of 4, C/4 <= 16384, "
-                                   "and for the tensor-core kernels: group_size 8, 16, 32, 64, HW >= 32 and a multiple of 4, "
-                                   "N*HW >= 4096 per domain (C=%d HW=%d N=%d gs=%d)", g.C, g.HW, g.N, g.GS);
-  return fail(DWT_E_UNSUPPORTED, "NCHW bf16 activations are built for group_size 1, 2, 4 and batch norm with HW a multiple "
-                                 "of 4, and for the tensor-core kernels: group_size 8, 16, 32, 64, HW >= 32 and a multiple "
-                                 "of 8, N*HW >= 4096 per domain (C=%d HW=%d N=%d gs=%d)", g.C, g.HW, g.N, g.GS);
-}
-int check_tc_bf16_align(bool bf16, bool nhwc, uintptr_t bits, const char* what) {
-  if (!bf16 || nhwc || bits % 16 == 0) return DWT_OK;
-  return fail(DWT_E_INVALID, "%s must be 16-byte aligned (bf16 NCHW: TMA)", what);
-}
-// the tensor-core family runs every fp32 NCHW call whose geometry and alignment it takes (else the tiled kernels), and
-// every bf16 NCHW call of group size 8..64 and channels-last call routed to it (validated above: there is no other
-// kernel to fall back to)
-int tc_route(bool bf16, bool nhwc, const Plan& p, bool* tc) {
-  if (!p.small && (bf16 || nhwc || p.gm.GS > DWT_MAX_GROUP_SIZE)) {
-    if (ensure_tc() != 0) return fail(DWT_E_LAUNCH, "tensor-core kernel set-up failed (%d)", g_tc_rc);
-    *tc = true;
-  } else {
-    *tc = !p.small && dwt::tc_supports(p.gm, p.vec) && ensure_tc() == 0;
+// ---- which kernel family runs a norm call ------------------------------------------------------------------
+// CL: channels-last (DWT_LAYOUT_NHWC) register-resident kernels, group sizes 1, 2, 4.  SMALL: their NCHW counterparts
+// (bf16: a thread's four pixels of a channel row are 8 bytes, the fp32 plan with vec == 4).  TC: TMA + wgmma kernels,
+// group sizes 8..64 and 128 (fp32 only, no other kernel is that wide); NCHW fp32 when geometry and alignment allow and
+// the kernels could be set up.  TILED: NCHW fp32 shared-memory kernels, any group size up to 64, any alignment.
+enum Family { CL, SMALL, TC, TILED };
+enum Pass { REDUCE, FINALIZE, PREP, APPLY };
+
+struct Route {
+  Family fam;
+  int align;            // bytes the activation tensors' addresses must be a multiple of; 0: any (the plan's vec adapts)
+  bool inputs_only;     // the rule covers the tensors the kernels read through TMA (x, dout), not the one they write
+  const char* what;     // how a refusal names the tensors (nullptr: by name)
+  const char* why;      // what it says after "N-byte aligned"
+};
+
+#define DWT_CL_RULE "group_size 1, 2, 4 with C a multiple of 4, C/4 <= 16384"
+
+// Family and alignment rule of a call with plan p, or the refusal of its geometry or of its second gradient addend
+// (dout2, backward only: the channels-last kernels read it).  No device or driver call: the tensor-core kernels are
+// set up (ensure_tc) only once the call has passed every check.
+int route(const Plan& p, bool nhwc, bool bf16, const void* dout2, Route* r) {
+  const dwt::Geom& g = p.gm;
+  const bool cl = dwt::cl_supports(g.C, g.GS), tc_nhwc = dwt::tc_supports(g, 4) && g.HW % 4 == 0, small = dwt::small_supports(g.GS);
+  if (g.GS == DWT_TC_MAX_GROUP_SIZE) {
+    if (bf16) return fail(DWT_E_UNSUPPORTED, "group_size 128 is built for fp32 activations (C=%d HW=%d N=%d)", g.C, g.HW, g.N);
+    if (!(nhwc ? tc_nhwc : dwt::tc_supports(g, p.vec)))
+      return fail(DWT_E_UNSUPPORTED, "group_size 128 runs on the tensor-core kernels only: HW >= 32 and a multiple of 4, "
+                  "N*HW >= 4096 per domain, NCHW tensors 16-byte aligned (C=%d HW=%d N=%d)", g.C, g.HW, g.N);
   }
+  auto fail_nhwc = [&] {
+    return fail(DWT_E_UNSUPPORTED, "channels-last %s built for " DWT_CL_RULE ", and for the tensor-core kernels: group_size "
+                "8, 16, 32, 64, HW >= 32 and a multiple of 4, N*HW >= 4096 per domain (C=%d HW=%d N=%d gs=%d)",
+                bf16 ? "bf16 activations are" : "layout is", g.C, g.HW, g.N, g.GS);
+  };
+  if (bf16 && nhwc && !cl && !tc_nhwc) return fail_nhwc();
+  if (bf16 && !nhwc && !(small ? g.HW % 4 == 0 : dwt::tc_supports(g, 4) && g.HW % 8 == 0))
+    return fail(DWT_E_UNSUPPORTED, "NCHW bf16 activations are built for group_size 1, 2, 4 and batch norm with HW a multiple "
+                "of 4, and for the tensor-core kernels: group_size 8, 16, 32, 64, HW >= 32 and a multiple of 8, N*HW >= 4096 "
+                "per domain (C=%d HW=%d N=%d gs=%d)", g.C, g.HW, g.N, g.GS);
+  if (dout2 && (!nhwc || tc_nhwc || (uintptr_t)dout2 % (bf16 ? 8 : 16) != 0))
+    return fail(nhwc && !tc_nhwc ? DWT_E_INVALID : DWT_E_UNSUPPORTED, "a second gradient addend (dout2) is built for the "
+                "channels-last kernels of group sizes 1, 2, 4 (16-byte aligned tensor, 8 for bf16); add it to dout otherwise");
+  if (nhwc) {
+    if (!cl && !tc_nhwc) return fail_nhwc();
+    *r = cl ? Route{CL, bf16 ? 8 : 16, false, "channels-last tensors", bf16 ? " (bf16)" : ""}
+            : Route{TC, 16, false, nullptr, " (channels-last tensor-core kernels: TMA)"};
+    return DWT_OK;
+  }
+  if (small) *r = Route{SMALL, bf16 ? 8 : 0, false, nullptr, " (bf16)"};
+  else if (bf16) *r = Route{TC, 16, true, nullptr, " (bf16 NCHW: TMA)"};
+  else *r = Route{g.GS > DWT_MAX_GROUP_SIZE || dwt::tc_supports(g, p.vec) ? TC : TILED, 0, false, nullptr, ""};
   return DWT_OK;
 }
-// group size 128 runs on the tensor-core kernels only (no tiled kernel is that wide), in fp32: below their geometry,
-// or in bf16, the call is refused rather than sent elsewhere
-int check_gs128(bool bf16, bool nhwc, const Plan& p) {
-  const dwt::Geom& g = p.gm;
-  if (g.GS != DWT_TC_MAX_GROUP_SIZE) return DWT_OK;
-  if (bf16) return fail(DWT_E_UNSUPPORTED, "group_size 128 is built for fp32 activations (C=%d HW=%d N=%d)", g.C, g.HW, g.N);
-  if (nhwc ? tc_nhwc_supports(g) : dwt::tc_supports(g, p.vec)) return DWT_OK;
-  return fail(DWT_E_UNSUPPORTED, "group_size 128 runs on the tensor-core kernels only: HW >= 32 and a multiple of 4, "
-              "N*HW >= 4096 per domain, NCHW tensors 16-byte aligned (C=%d HW=%d N=%d)", g.C, g.HW, g.N);
-}
-int check_tc_nhwc_align(uintptr_t bits, const char* what) {
-  if (bits % 16 == 0) return DWT_OK;
-  return fail(DWT_E_INVALID, "%s must be 16-byte aligned (channels-last tensor-core kernels: TMA)", what);
-}
-int fail_nhwc_geometry(const dwt::Geom& g) {
-  return fail(DWT_E_UNSUPPORTED, "channels-last layout is built for group_size 1, 2, 4 with C a multiple of 4, C/4 <= 16384, and for the "
-              "tensor-core kernels: group_size 8, 16, 32, 64, HW >= 32 and a multiple of 4, N*HW >= 4096 per domain "
-              "(C=%d HW=%d N=%d gs=%d)", g.C, g.HW, g.N, g.GS);
-}
-// profile family of a tensor-core launch by layout and dtype
-inline const char* tc_fam(bool bf16, bool nhwc, const char* f32, const char* b16, const char* nhwc_f32, const char* nhwc_b16) {
-  return nhwc ? fam(bf16, nhwc_f32, nhwc_b16) : fam(bf16, f32, b16);
-}
+
+// Profile family name of a launch: [backward][family][pass][channels-last * 2 + bf16].  bf16 launches report under
+// their own names (algorithmic bytes at 2 B/element); fp32 channels-last prep runs, and is named as, the NCHW one.
+const char* const kProfName[2][4][4][4] = {
+    {{{"", "", "cl_stats", "cl_stats_bf16"}, {"", "", "cl_fwd_finalize", "cl_fwd_finalize_bf16"},
+      {"", "", "eval_prep", "cl_eval_prep_bf16"}, {"", "", "cl_apply", "cl_apply_bf16"}},
+     {{"small_stats", "small_stats_bf16", "", ""}, {"", "", "", ""}, {"eval_prep", "eval_prep_bf16", "", ""},
+      {"small_apply", "small_apply_bf16", "", ""}},
+     {{"tc_stats", "tc_stats_bf16", "tc_stats_nhwc", "tc_stats_nhwc_bf16"},
+      {"dense_fwd_finalize", "dense_fwd_finalize_bf16", "dense_fwd_finalize", "dense_fwd_finalize_bf16"},
+      {"eval_prep", "eval_prep_bf16", "eval_prep", "eval_prep_bf16"},
+      {"tc_apply", "tc_apply_bf16", "tc_apply_nhwc", "tc_apply_nhwc_bf16"}},
+     {{"tiled_stats", "", "", ""}, {"", "", "", ""}, {"eval_prep", "", "", ""}, {"tiled_apply", "", "", ""}}},
+    {{{"", "", "cl_bwd_reduce", "cl_bwd_reduce_bf16"}, {"", "", "cl_bwd_finalize", "cl_bwd_finalize_bf16"},
+      {"", "", "bwd_prep", "cl_bwd_prep_bf16"}, {"", "", "cl_bwd_apply", "cl_bwd_apply_bf16"}},
+     {{"small_bwd_reduce", "small_bwd_reduce_bf16", "", ""}, {"", "", "", ""}, {"bwd_prep", "bwd_prep_bf16", "", ""},
+      {"small_bwd_apply", "small_bwd_apply_bf16", "", ""}},
+     {{"tc_bwd_reduce", "tc_bwd_reduce_bf16", "tc_bwd_reduce_nhwc", "tc_bwd_reduce_nhwc_bf16"},
+      {"dense_bwd_finalize", "dense_bwd_finalize_bf16", "dense_bwd_finalize", "dense_bwd_finalize_bf16"},
+      {"bwd_prep", "bwd_prep_bf16", "bwd_prep", "bwd_prep_bf16"},
+      {"tc_bwd_apply", "tc_bwd_apply_bf16", "tc_bwd_apply_nhwc", "tc_bwd_apply_nhwc_bf16"}},
+     {{"tiled_bwd_reduce", "", "", ""}, {"", "", "", ""}, {"bwd_prep", "", "", ""}, {"tiled_bwd_apply", "", "", ""}}}};
+
 int check_running(bool need_running, float* const* rmean, float* const* rcov, int D) {
   if (!need_running) return DWT_OK;
   if (!rmean || !rcov) return fail(DWT_E_INVALID, "running buffers required");
@@ -418,218 +432,202 @@ dwt::BwdFin make_bwd_fin(float a, int mode, int epi, const float* save_mean, con
   return fin;
 }
 
+// A norm call past its checks: plan, route, workspace, and its mode with the layout and dtype bits stripped
+struct Call {
+  Plan p;
+  Route r;
+  Workspace w;
+  bool nhwc, bf16;
+  int mode;
+  const char* name(bool bwd, Pass ps) const { return kProfName[bwd][r.fam][ps][2 * nhwc + bf16]; }
+};
+
+// The checks both directions make, in order; `own` holds the direction's own (residual, running buffers, gradient
+// outputs), checked before the epilogue's family rule.  in0, in1: the tensors the kernels read (x, x or x, dout);
+// out: the one they write (y or dx); dout2: the backward's second gradient addend.
+template <class Own>
+int validate(Call& c, bool bwd, const void* in0, const void* in1, const void* out, const void* dout2, int64_t N, int64_t C, int64_t HW, int GS,
+             int D, int mode, int epi, const float* gamma, const float* beta, const float* save_mean, const float* save_w,
+             void* ws, size_t ws_bytes, Own own) {
+  c.nhwc = (mode & DWT_LAYOUT_NHWC) != 0, c.bf16 = (mode & DWT_DTYPE_BF16) != 0, c.mode = mode & 0xFF;
+  const int elem_bytes = c.bf16 && !c.nhwc ? 2 : 4;
+  if (int rc = make_plan(c.p, bwd ? K_BWD_REDUCE : K_STATS, bwd ? K_BWD_APPLY : K_APPLY, in0, in1, out, N, C, HW, GS, D, elem_bytes)) return rc;
+  if (!in0 || !in1 || !out || !save_mean || !save_w || !ws) return fail(DWT_E_INVALID, "null pointer argument");
+  if (int rc = route(c.p, c.nhwc, c.bf16, dout2, &c.r)) return rc;
+  const uintptr_t bits = (uintptr_t)in0 | (uintptr_t)in1 | (c.r.inputs_only ? 0 : (uintptr_t)out);
+  if (c.r.align && bits % c.r.align != 0)
+    return fail(DWT_E_INVALID, "%s must be %d-byte aligned%s", c.r.what ? c.r.what : bwd ? (c.r.inputs_only ? "x and dout" : "x, dout and dx")
+                : (c.r.inputs_only ? "x" : "x and y"), c.r.align, c.r.why);
+  if (c.mode != DWT_MODE_TRAIN && c.mode != DWT_MODE_EVAL) return fail(DWT_E_INVALID, "bad mode %d", c.mode);
+  if ((epi & DWT_EPI_RELU) && !(epi & DWT_EPI_AFFINE)) return fail(DWT_E_INVALID, "RELU epilogue needs AFFINE");
+  if ((epi & DWT_EPI_AFFINE) && (!gamma || !beta)) return fail(DWT_E_INVALID, "AFFINE epilogue needs gamma and beta");
+  if (int rc = own()) return rc;
+  if (epi != 0 && c.r.fam != CL && c.r.fam != SMALL)
+    return fail(DWT_E_UNSUPPORTED, "fused gamma/beta/ReLU epilogue is built for group_size 1, 2, 4 (got %d)", GS);
+  c.w = carve(ws, C, GS, D);
+  if (c.w.bytes > ws_bytes) return fail(DWT_E_WORKSPACE, "workspace too small: need %zu bytes, got %zu", c.w.bytes, ws_bytes);
+  if ((uintptr_t)ws % 256 != 0) return fail(DWT_E_WORKSPACE, "workspace must be 256-byte aligned");
+  if ((c.r.fam == TC || c.r.fam == TILED) && ensure_tiled() != 0)
+    return fail(DWT_E_LAUNCH, "cudaFuncSetAttribute failed (%d)", g_tiled_rc);
+  if (c.r.fam == TC && ensure_tc() != 0) {
+    if (c.bf16 || c.nhwc || GS > DWT_MAX_GROUP_SIZE) return fail(DWT_E_LAUNCH, "tensor-core kernel set-up failed (%d)", g_tc_rc);
+    c.r.fam = TILED;      // fp32 NCHW up to group size 64: the tiled kernels take every geometry
+  }
+  return DWT_OK;
+}
+
 int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, int GS, int D, int mode, float a,
                     float b, float momentum, float unbias, int update_running, float* const* rmean,
                     float* const* rcov, const float* gamma, const float* beta, const float* residual,
                     uint8_t* relu_mask, int epi, float* save_mean, float* save_w, void* ws, size_t ws_bytes,
                     cudaStream_t st) {
-  const bool nhwc = (mode & DWT_LAYOUT_NHWC) != 0, bf16 = (mode & DWT_DTYPE_BF16) != 0;
-  mode &= 0xFF;
-  Plan p;
-  if (int rc = make_plan(p, K_STATS, K_APPLY, x, y, nullptr, N, C, HW, GS, D, bf16 && !nhwc ? 2 : 4)) return rc;
-  if (!x || !y || !save_mean || !save_w || !ws) return fail(DWT_E_INVALID, "null pointer argument");
-  if (int rc = check_gs128(bf16, nhwc, p)) return rc;
-  if (int rc = check_bf16_geometry(bf16, nhwc, p.gm)) return rc;
-  const bool nhwc_tc = nhwc && tc_nhwc_supports(p.gm);
-  if (nhwc && !nhwc_tc && !dwt::cl_supports((int)C, GS)) return fail_nhwc_geometry(p.gm);
-  if (nhwc_tc) if (int rc = check_tc_nhwc_align((uintptr_t)x | (uintptr_t)y, "x and y")) return rc;
-  if (nhwc && !nhwc_tc) if (int rc = check_align(bf16, (uintptr_t)x | (uintptr_t)y, "channels-last tensors")) return rc;
-  if (bf16 && !nhwc && p.small) {
-    if (int rc = check_align(bf16, (uintptr_t)x | (uintptr_t)y, "x and y")) return rc;
-  } else if (int rc = check_tc_bf16_align(bf16, nhwc, (uintptr_t)x, "x")) {
-    return rc;
-  }
-  if (mode != DWT_MODE_TRAIN && mode != DWT_MODE_EVAL) return fail(DWT_E_INVALID, "bad mode %d", mode);
-  if ((epi & DWT_EPI_RELU) && !(epi & DWT_EPI_AFFINE)) return fail(DWT_E_INVALID, "RELU epilogue needs AFFINE");
-  if ((epi & DWT_EPI_AFFINE) && (!gamma || !beta)) return fail(DWT_E_INVALID, "AFFINE epilogue needs gamma and beta");
-  if ((epi & DWT_EPI_RESIDUAL) && ((epi & 3) != 3 || !residual)) return fail(DWT_E_INVALID, "RESIDUAL epilogue needs AFFINE|RELU and a residual tensor");
-  if (epi & DWT_EPI_RESIDUAL) if (int rc = check_align(bf16, (uintptr_t)residual, "residual")) return rc;
-  if (relu_mask && !((epi & DWT_EPI_RESIDUAL) && nhwc))
-    return fail(DWT_E_UNSUPPORTED, "the ReLU byte map is written by the channels-last RESIDUAL epilogue only");
-  if (epi != 0 && !p.small)
-    return fail(DWT_E_UNSUPPORTED, "fused gamma/beta/ReLU epilogue is built for group_size 1, 2, 4 (got %d)", GS);
-  const bool need_running = (mode == DWT_MODE_EVAL) || update_running;
-  if (int rc = check_running(need_running, rmean, rcov, D)) return rc;
-  Workspace w = carve(ws, C, GS, D);
-  if (w.bytes > ws_bytes) return fail(DWT_E_WORKSPACE, "workspace too small: need %zu bytes, got %zu", w.bytes, ws_bytes);
-  if ((uintptr_t)ws % 256 != 0) return fail(DWT_E_WORKSPACE, "workspace must be 256-byte aligned");
-  if (!p.small && ensure_tiled() != 0) return fail(DWT_E_LAUNCH, "cudaFuncSetAttribute failed (%d)", g_tiled_rc);
-
-  const dwt::FwdFin fin = make_fwd_fin(a, b, momentum, unbias, mode == DWT_MODE_TRAIN ? update_running : 0, need_running,
-                                       rmean, rcov, save_mean, save_w, w, D);
-
+  Call c;
+  const bool need_running = ((mode & 0xFF) == DWT_MODE_EVAL) || update_running;
+  const int rc = validate(c, false, x, x, y, nullptr, N, C, HW, GS, D, mode, epi, gamma, beta, save_mean, save_w, ws, ws_bytes, [&] {
+    if ((epi & DWT_EPI_RESIDUAL) && ((epi & 3) != 3 || !residual)) return fail(DWT_E_INVALID, "RESIDUAL epilogue needs AFFINE|RELU and a residual tensor");
+    if (epi & DWT_EPI_RESIDUAL) if (int rc = check_align(c.bf16, (uintptr_t)residual, "residual")) return rc;
+    if (relu_mask && !((epi & DWT_EPI_RESIDUAL) && c.nhwc))
+      return fail(DWT_E_UNSUPPORTED, "the ReLU byte map is written by the channels-last RESIDUAL epilogue only");
+    return check_running(need_running, rmean, rcov, D);
+  });
+  if (rc) return rc;
+  const Plan& p = c.p; const Workspace& w = c.w;
+  const bool bf16 = c.bf16, nhwc = c.nhwc, train = c.mode == DWT_MODE_TRAIN;
+  const dwt::FwdFin fin = make_fwd_fin(a, b, momentum, unbias, train ? update_running : 0, need_running, rmean, rcov,
+                                       save_mean, save_w, w, D);
   const double n_el = (double)D * (double)N * (double)C * (double)HW;
   const double E = (bf16 ? 2.0 : 4.0) * n_el, Mb = 0.25 * n_el;   // bytes of one activation tensor, of the ReLU byte map
-  if (nhwc && !nhwc_tc) {
-    const ClPlan cp = cl_plan(p.gm, 3, 3, 8, (epi & DWT_EPI_RESIDUAL) ? 4 : 8);
-    if (mode == DWT_MODE_TRAIN) {
-      {
-        Launch l(fam(bf16, "cl_stats", "cl_stats_bf16"), &p.gm, E, st);
-        dwt::cl_stats(x, bf16, p.gm, cp.nred, cp.gz_red, w.partial, w.shift, st);
-      }
-      if (int rc = check_launch("channels-last statistics kernel")) return rc;
-      Launch l(fam(bf16, "cl_fwd_finalize", "cl_fwd_finalize_bf16"), &p.gm, 0.0, st);
-      dwt::cl_fwd_finalize(w.partial, cp.nred, w.shift, p.gm, fin, st);
-    } else {
-      Launch l(fam(bf16, "eval_prep", "cl_eval_prep_bf16"), &p.gm, 0.0, st);
-      dwt::small_eval_prep(p.gm, fin, st);
-    }
-    if (int rc = check_launch("channels-last finalize kernel")) return rc;
-    {
-      Launch l(fam(bf16, "cl_apply", "cl_apply_bf16"), &p.gm, (epi & DWT_EPI_RESIDUAL) ? 3.0 * E + (relu_mask ? Mb : 0.0) : 2.0 * E, st);
-      dwt::cl_apply(x, y, bf16, p.gm, cp.new_, cp.gz_ew, epi, save_mean, save_w, gamma, beta, residual, relu_mask, st);
-    }
-    return check_launch("channels-last apply kernel");
-  }
-  bool tc = false;
-  if (int rc = tc_route(bf16, nhwc, p, &tc)) return rc;
+  const ClPlan cp = c.r.fam == CL ? cl_plan(p.gm, 3, 3, 8, (epi & DWT_EPI_RESIDUAL) ? 4 : 8) : ClPlan{};
   const bool gs128 = GS == DWT_TC_MAX_GROUP_SIZE;
   const size_t pair_part = (size_t)tc_chunks(p.gm) * dwt::tc_superblocks(p.gm) * D * (64 * 64 + 64);   // behind the diagonal partials
-  if (mode == DWT_MODE_TRAIN) {
-    Launch l(p.small ? fam(bf16, "small_stats", "small_stats_bf16") : (tc ? tc_fam(bf16, nhwc, "tc_stats", "tc_stats_bf16", "tc_stats_nhwc", "tc_stats_nhwc_bf16") : "tiled_stats"), &p.gm, E, st);
-    if (p.small) dwt::small_stats(x, bf16, p.gm, p.vec, fin, w.partial, w.counters, st);
-    else if (tc) {
-      int cr = dwt::tc_stats(x, bf16, nhwc, p.gm, tc_chunks(p.gm), w.shift, w.partial, st);
-      // group size 128: the off-diagonal blocks behind the diagonal ones (a second read of x, counted once above)
-      if (cr == 0 && gs128)
-        cr = dwt::tc_gram_pair(x, nhwc, p.gm, tc_pair_chunks(p.gm, false), w.shift, w.partial + pair_part, st);
-      if (cr) return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d) x=%p N=%d C=%d HW=%d D=%d", cr, (const void*)x, p.gm.N, p.gm.C, p.gm.HW, p.gm.D);
-    } else dwt::tiled_stats(x, p.gm, p.vec, fin, w.partial, w.counters, st);
+  // reduce: batch statistics (train) or the eval coefficients from the running buffers
+  if (train) {
+    {
+      Launch l(c.name(false, REDUCE), &p.gm, E, st);
+      switch (c.r.fam) {
+        case CL: dwt::cl_stats(x, bf16, p.gm, cp.nred, cp.gz_red, w.partial, w.shift, st); break;
+        case SMALL: dwt::small_stats(x, bf16, p.gm, p.vec, fin, w.partial, w.counters, st); break;
+        case TILED: dwt::tiled_stats(x, p.gm, p.vec, fin, w.partial, w.counters, st); break;
+        case TC: {
+          int cr = dwt::tc_stats(x, bf16, nhwc, p.gm, tc_chunks(p.gm), w.shift, w.partial, st);
+          // group size 128: the off-diagonal blocks behind the diagonal ones (a second read of x, counted once above)
+          if (cr == 0 && gs128)
+            cr = dwt::tc_gram_pair(x, nhwc, p.gm, tc_pair_chunks(p.gm, false), w.shift, w.partial + pair_part, st);
+          if (cr) return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d) x=%p N=%d C=%d HW=%d D=%d", cr, (const void*)x, p.gm.N, p.gm.C, p.gm.HW, p.gm.D);
+        }
+      }
+    }
+    if (c.r.fam == CL || c.r.fam == TC) {   // the small and tiled kernels finalize in their last CTA
+      if (int rc = check_launch(c.r.fam == CL ? "channels-last statistics kernel" : "tensor-core statistics kernel")) return rc;
+      Launch l(c.name(false, FINALIZE), &p.gm, 0.0, st);
+      if (c.r.fam == CL) {
+        dwt::cl_fwd_finalize(w.partial, cp.nred, w.shift, p.gm, fin, st);
+      } else {
+        dwt::dense_partial_reduce(w.partial, tc_chunks(p.gm), dwt::tc_superblocks(p.gm) * D, w.gram, st);
+        if (gs128)
+          dwt::dense_partial_reduce(w.partial + pair_part, tc_pair_chunks(p.gm, false), dwt::tc_superblocks(p.gm) / 2 * D,
+                                    w.gram + (size_t)dwt::tc_superblocks(p.gm) * D * (64 * 64 + 64), st);
+        dwt::dense_fwd_factor(w.gram, w.shift, p.gm, fin, st);
+      }
+    }
   } else {
-    Launch l(fam(bf16, "eval_prep", "eval_prep_bf16"), &p.gm, 0.0, st);
-    if (p.small) dwt::small_eval_prep(p.gm, fin, st);
-    else if (tc) dwt::dense_fwd_factor(nullptr, nullptr, p.gm, fin, st);
-    else dwt::tiled_eval_prep(p.gm, fin, st);
+    Launch l(c.name(false, PREP), &p.gm, 0.0, st);
+    if (c.r.fam == TC) dwt::dense_fwd_factor(nullptr, nullptr, p.gm, fin, st);
+    else if (c.r.fam == TILED) dwt::tiled_eval_prep(p.gm, fin, st);
+    else dwt::small_eval_prep(p.gm, fin, st);
   }
-  if (tc && mode == DWT_MODE_TRAIN) {
-    if (int rc = check_launch("tensor-core statistics kernel")) return rc;
-    Launch l(fam(bf16, "dense_fwd_finalize", "dense_fwd_finalize_bf16"), &p.gm, 0.0, st);
-    dwt::dense_partial_reduce(w.partial, tc_chunks(p.gm), dwt::tc_superblocks(p.gm) * D, w.gram, st);
-    if (gs128)
-      dwt::dense_partial_reduce(w.partial + pair_part, tc_pair_chunks(p.gm, false), dwt::tc_superblocks(p.gm) / 2 * D,
-                                w.gram + (size_t)dwt::tc_superblocks(p.gm) * D * (64 * 64 + 64), st);
-    dwt::dense_fwd_factor(w.gram, w.shift, p.gm, fin, st);
-  }
-  if (int rc = check_launch("whitening statistics kernel")) return rc;
+  if (int rc = check_launch(c.r.fam == CL ? "channels-last finalize kernel" : "whitening statistics kernel")) return rc;
   {
-    Launch l(p.small ? fam(bf16, "small_apply", "small_apply_bf16") : (tc ? tc_fam(bf16, nhwc, "tc_apply", "tc_apply_bf16", "tc_apply_nhwc", "tc_apply_nhwc_bf16") : "tiled_apply"), &p.gm,
-             ((epi & DWT_EPI_RESIDUAL) ? 3 : 2) * E, st);
-    if (p.small) dwt::small_apply(x, y, bf16, p.gm_ew, p.vec, p.chunks_ew, epi, save_mean, save_w, gamma, beta, residual, st);
-    else if (tc) {
-      if (int cr = dwt::tc_apply(x, y, bf16, nhwc, p.gm, tc_apply_ctas(p.gm, 1, 64), save_mean, save_w, st))
-        return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d)", cr);
-    } else dwt::tiled_apply(x, y, p.gm_ew, p.vec, p.chunks_ew, save_mean, save_w, st);
+    Launch l(c.name(false, APPLY), &p.gm, (epi & DWT_EPI_RESIDUAL) ? 3.0 * E + (relu_mask ? Mb : 0.0) : 2.0 * E, st);
+    switch (c.r.fam) {
+      case CL: dwt::cl_apply(x, y, bf16, p.gm, cp.new_, cp.gz_ew, epi, save_mean, save_w, gamma, beta, residual, relu_mask, st); break;
+      case SMALL: dwt::small_apply(x, y, bf16, p.gm_ew, p.vec, p.chunks_ew, epi, save_mean, save_w, gamma, beta, residual, st); break;
+      case TILED: dwt::tiled_apply(x, y, p.gm_ew, p.vec, p.chunks_ew, save_mean, save_w, st); break;
+      case TC:
+        if (int cr = dwt::tc_apply(x, y, bf16, nhwc, p.gm, tc_apply_ctas(p.gm, 1, 64), save_mean, save_w, st))
+          return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d)", cr);
+    }
   }
-  return check_launch("whitening apply kernel");
+  return check_launch(c.r.fam == CL ? "channels-last apply kernel" : "whitening apply kernel");
 }
 
 int whiten_like_bwd(const float* x, const float* dout, const float* dout2, float* dx, int64_t N, int64_t C, int64_t HW, int GS, int D,
                     int mode, float a, const float* save_mean, const float* save_w, const float* gamma,
                     const float* beta, const uint8_t* relu_mask, float* dresidual, int epi, float* dgamma,
                     float* dbeta, void* ws, size_t ws_bytes, cudaStream_t st) {
-  const bool nhwc = (mode & DWT_LAYOUT_NHWC) != 0, bf16 = (mode & DWT_DTYPE_BF16) != 0;
-  mode &= 0xFF;
-  Plan p;
-  if (int rc = make_plan(p, K_BWD_REDUCE, K_BWD_APPLY, x, dout, dx, N, C, HW, GS, D, bf16 && !nhwc ? 2 : 4)) return rc;
-  if (!x || !dout || !dx || !save_mean || !save_w || !ws) return fail(DWT_E_INVALID, "null pointer argument");
-  if (int rc = check_gs128(bf16, nhwc, p)) return rc;
-  if (int rc = check_bf16_geometry(bf16, nhwc, p.gm)) return rc;
-  const bool nhwc_tc = nhwc && tc_nhwc_supports(p.gm);
-  if (dout2 && (!nhwc || nhwc_tc || (uintptr_t)dout2 % (bf16 ? 8 : 16) != 0))
-    return fail(nhwc && !nhwc_tc ? DWT_E_INVALID : DWT_E_UNSUPPORTED, "a second gradient addend (dout2) is built for the "
-                "channels-last kernels of group sizes 1, 2, 4 (16-byte aligned tensor, 8 for bf16); add it to dout otherwise");
-  if (nhwc && !nhwc_tc && !dwt::cl_supports((int)C, GS)) return fail_nhwc_geometry(p.gm);
-  if (nhwc_tc) if (int rc = check_tc_nhwc_align((uintptr_t)x | (uintptr_t)dout | (uintptr_t)dx, "x, dout and dx")) return rc;
-  if (nhwc && !nhwc_tc) if (int rc = check_align(bf16, (uintptr_t)x | (uintptr_t)dout | (uintptr_t)dx, "channels-last tensors")) return rc;
-  if (bf16 && !nhwc && p.small) {
-    if (int rc = check_align(bf16, (uintptr_t)x | (uintptr_t)dout | (uintptr_t)dx, "x, dout and dx")) return rc;
-  } else if (int rc = check_tc_bf16_align(bf16, nhwc, (uintptr_t)x | (uintptr_t)dout, "x and dout")) {
-    return rc;
-  }
-  if (mode != DWT_MODE_TRAIN && mode != DWT_MODE_EVAL) return fail(DWT_E_INVALID, "bad mode %d", mode);
-  if ((epi & DWT_EPI_RELU) && !(epi & DWT_EPI_AFFINE)) return fail(DWT_E_INVALID, "RELU epilogue needs AFFINE");
-  if ((epi & DWT_EPI_AFFINE) && (!gamma || !beta)) return fail(DWT_E_INVALID, "AFFINE epilogue needs gamma and beta");
-  if (epi & DWT_EPI_RESIDUAL) {
-    // backward of out = relu(z + residual): the ReLU mask comes from the byte map the forward wrote, the masked
-    // gradient goes to dresidual and is what the apply pass reads
-    if (!nhwc || !relu_mask || (epi & 3) != 3 || !dresidual)
-      return fail(DWT_E_INVALID, "backward of a RESIDUAL forward needs the channels-last layout, AFFINE|RELU, the forward's "
-                                 "ReLU byte map and dresidual (or pass dout already masked by (out > 0) with epilogue AFFINE)");
-    if (int rc = check_align(bf16, (uintptr_t)dresidual, "dresidual")) return rc;
-  } else if (relu_mask || dresidual) {
-    return fail(DWT_E_INVALID, "relu_mask / dresidual belong to the RESIDUAL epilogue");
-  }
-  if ((dgamma == nullptr) != (dbeta == nullptr)) return fail(DWT_E_INVALID, "dgamma and dbeta go together");
-  if (epi != 0 && !p.small)
-    return fail(DWT_E_UNSUPPORTED, "fused gamma/beta/ReLU epilogue is built for group_size 1, 2, 4 (got %d)", GS);
-  Workspace w = carve(ws, C, GS, D);
-  if (w.bytes > ws_bytes) return fail(DWT_E_WORKSPACE, "workspace too small: need %zu bytes, got %zu", w.bytes, ws_bytes);
-  if ((uintptr_t)ws % 256 != 0) return fail(DWT_E_WORKSPACE, "workspace must be 256-byte aligned");
-  if (!p.small && ensure_tiled() != 0) return fail(DWT_E_LAUNCH, "cudaFuncSetAttribute failed (%d)", g_tiled_rc);
-
-  const dwt::BwdFin fin = make_bwd_fin(a, mode, epi, save_mean, save_w, gamma, dgamma, dbeta, w);
+  Call c;
+  const int rc = validate(c, true, x, dout, dx, dout2, N, C, HW, GS, D, mode, epi, gamma, beta, save_mean, save_w, ws, ws_bytes, [&] {
+    if (epi & DWT_EPI_RESIDUAL) {
+      // backward of out = relu(z + residual): the ReLU mask comes from the byte map the forward wrote, the masked
+      // gradient goes to dresidual and is what the apply pass reads
+      if (!c.nhwc || !relu_mask || (epi & 3) != 3 || !dresidual)
+        return fail(DWT_E_INVALID, "backward of a RESIDUAL forward needs the channels-last layout, AFFINE|RELU, the forward's "
+                                   "ReLU byte map and dresidual (or pass dout already masked by (out > 0) with epilogue AFFINE)");
+      if (int rc = check_align(c.bf16, (uintptr_t)dresidual, "dresidual")) return rc;
+    } else if (relu_mask || dresidual) {
+      return fail(DWT_E_INVALID, "relu_mask / dresidual belong to the RESIDUAL epilogue");
+    }
+    if ((dgamma == nullptr) != (dbeta == nullptr)) return fail(DWT_E_INVALID, "dgamma and dbeta go together");
+    return DWT_OK;
+  });
+  if (rc) return rc;
+  const Plan& p = c.p; const Workspace& w = c.w;
+  const bool bf16 = c.bf16, nhwc = c.nhwc;
+  const dwt::BwdFin fin = make_bwd_fin(a, c.mode, epi, save_mean, save_w, gamma, dgamma, dbeta, w);
   const bool masked = nhwc && (epi & DWT_EPI_RESIDUAL) != 0;   // the reduction also writes the masked gradient
-
-  const bool need_reduce = (mode == DWT_MODE_TRAIN) || (fin.dgamma != nullptr) || masked;
+  const bool need_reduce = (c.mode == DWT_MODE_TRAIN) || (fin.dgamma != nullptr) || masked;
   const double n_el = (double)D * (double)N * (double)C * (double)HW;
   const double E = (bf16 ? 2.0 : 4.0) * n_el, Mb = 0.25 * n_el;
-  if (nhwc && !nhwc_tc) {
-    const ClPlan cp = cl_plan(p.gm, 2, 2, 4, 4);
-    if (need_reduce) {
-      {
-        Launch l(fam(bf16, "cl_bwd_reduce", "cl_bwd_reduce_bf16"), &p.gm, (masked ? 3.0 * E + Mb : 2.0 * E) + (dout2 ? E : 0.0), st);
-        dwt::cl_bwd_reduce(x, dout, dout2, bf16, p.gm, cp.nred, cp.gz_red, epi, save_mean, save_w, gamma, beta, relu_mask, dresidual, w.partial, st);
-      }
-      if (int rc = check_launch("channels-last backward reduction kernel")) return rc;
-      Launch l(fam(bf16, "cl_bwd_finalize", "cl_bwd_finalize_bf16"), &p.gm, 0.0, st);
-      dwt::cl_bwd_finalize(w.partial, cp.nred, p.gm, fin, st);
-    } else {
-      Launch l(fam(bf16, "bwd_prep", "cl_bwd_prep_bf16"), &p.gm, 0.0, st);
-      dwt::small_bwd_prep(p.gm, fin, st);
-    }
-    if (int rc = check_launch("channels-last backward finalize kernel")) return rc;
-    {
-      Launch l(fam(bf16, "cl_bwd_apply", "cl_bwd_apply_bf16"), &p.gm, (3.0 + (dout2 && !masked ? 1.0 : 0.0)) * E, st);
-      if (masked) dwt::cl_bwd_apply(x, dresidual, nullptr, dx, bf16, p.gm, cp.new_, cp.gz_ew, DWT_EPI_AFFINE, w.coef, save_mean, save_w, gamma, beta, st);
-      else dwt::cl_bwd_apply(x, dout, dout2, dx, bf16, p.gm, cp.new_, cp.gz_ew, epi, w.coef, save_mean, save_w, gamma, beta, st);
-    }
-    return check_launch("channels-last backward apply kernel");
-  }
-  bool tc = false;
-  if (int rc = tc_route(bf16, nhwc, p, &tc)) return rc;
+  const ClPlan cp = c.r.fam == CL ? cl_plan(p.gm, 2, 2, 4, 4) : ClPlan{};
   // group size 128: four blocks of R per group, 2 SB problems per domain
   const bool gs128 = GS == DWT_TC_MAX_GROUP_SIZE;
   const int rchunks = gs128 ? tc_pair_chunks(p.gm, true) : tc_chunks(p.gm);
   const int rproblems = (gs128 ? 2 : 1) * dwt::tc_superblocks(p.gm) * D;
+  // reduce: the gradient moments (train, dgamma/dbeta or the masked gradient), or the eval coefficients
   if (need_reduce) {
-    Launch l(p.small ? fam(bf16, "small_bwd_reduce", "small_bwd_reduce_bf16") : (tc ? tc_fam(bf16, nhwc, "tc_bwd_reduce", "tc_bwd_reduce_bf16", "tc_bwd_reduce_nhwc", "tc_bwd_reduce_nhwc_bf16") : "tiled_bwd_reduce"), &p.gm, 2 * E, st);
-    if (p.small) dwt::small_bwd_reduce(x, dout, bf16, p.gm, p.vec, fin, beta, w.partial, w.counters, st);
-    else if (tc) {
-      if (int cr = dwt::tc_bwd_reduce(x, dout, bf16, nhwc, p.gm, rchunks, save_mean, w.partial, st))
-        return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d) x=%p dout=%p N=%d C=%d HW=%d D=%d", cr, (const void*)x, (const void*)dout, p.gm.N, p.gm.C, p.gm.HW, p.gm.D);
-    } else dwt::tiled_bwd_reduce(x, dout, p.gm, p.vec, fin, w.partial, w.counters, st);
+    {
+      Launch l(c.name(true, REDUCE), &p.gm, (masked ? 3.0 * E + Mb : 2.0 * E) + (dout2 ? E : 0.0), st);
+      switch (c.r.fam) {
+        case CL: dwt::cl_bwd_reduce(x, dout, dout2, bf16, p.gm, cp.nred, cp.gz_red, epi, save_mean, save_w, gamma, beta, relu_mask, dresidual, w.partial, st); break;
+        case SMALL: dwt::small_bwd_reduce(x, dout, bf16, p.gm, p.vec, fin, beta, w.partial, w.counters, st); break;
+        case TILED: dwt::tiled_bwd_reduce(x, dout, p.gm, p.vec, fin, w.partial, w.counters, st); break;
+        case TC:
+          if (int cr = dwt::tc_bwd_reduce(x, dout, bf16, nhwc, p.gm, rchunks, save_mean, w.partial, st))
+            return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d) x=%p dout=%p N=%d C=%d HW=%d D=%d", cr, (const void*)x, (const void*)dout, p.gm.N, p.gm.C, p.gm.HW, p.gm.D);
+      }
+    }
+    if (c.r.fam == CL || c.r.fam == TC) {   // the small and tiled kernels finalize in their last CTA
+      if (int rc = check_launch(c.r.fam == CL ? "channels-last backward reduction kernel" : "tensor-core backward reduction kernel")) return rc;
+      Launch l(c.name(true, FINALIZE), &p.gm, 0.0, st);
+      if (c.r.fam == CL) {
+        dwt::cl_bwd_finalize(w.partial, cp.nred, p.gm, fin, st);
+      } else {
+        dwt::dense_partial_reduce(w.partial, rchunks, rproblems, w.gram, st);
+        dwt::dense_bwd_coef(w.gram, p.gm, fin, w.shift, st);
+      }
+    }
   } else {
-    Launch l(fam(bf16, "bwd_prep", "bwd_prep_bf16"), &p.gm, 0.0, st);
-    if (p.small) dwt::small_bwd_prep(p.gm, fin, st);
-    else if (tc) dwt::dense_bwd_coef(nullptr, p.gm, fin, w.shift, st);
-    else dwt::tiled_bwd_prep(p.gm, fin, st);
+    Launch l(c.name(true, PREP), &p.gm, 0.0, st);
+    if (c.r.fam == TC) dwt::dense_bwd_coef(nullptr, p.gm, fin, w.shift, st);
+    else if (c.r.fam == TILED) dwt::tiled_bwd_prep(p.gm, fin, st);
+    else dwt::small_bwd_prep(p.gm, fin, st);
   }
-  if (tc && need_reduce) {
-    if (int rc = check_launch("tensor-core backward reduction kernel")) return rc;
-    Launch l(fam(bf16, "dense_bwd_finalize", "dense_bwd_finalize_bf16"), &p.gm, 0.0, st);
-    dwt::dense_partial_reduce(w.partial, rchunks, rproblems, w.gram, st);
-    dwt::dense_bwd_coef(w.gram, p.gm, fin, w.shift, st);
-  }
-  if (int rc = check_launch("whitening backward reduction kernel")) return rc;
+  if (int rc = check_launch(c.r.fam == CL ? "channels-last backward finalize kernel" : "whitening backward reduction kernel")) return rc;
   {
-    Launch l(p.small ? fam(bf16, "small_bwd_apply", "small_bwd_apply_bf16") : (tc ? tc_fam(bf16, nhwc, "tc_bwd_apply", "tc_bwd_apply_bf16", "tc_bwd_apply_nhwc", "tc_bwd_apply_nhwc_bf16") : "tiled_bwd_apply"), &p.gm, 3 * E, st);
-    if (p.small) dwt::small_bwd_apply(x, dout, dx, bf16, p.gm_ew, p.vec, p.chunks_ew, epi, w.coef, save_mean, save_w, gamma, beta, st);
-    else if (tc) {
-      if (int cr = dwt::tc_bwd_apply(x, dout, dx, bf16, nhwc, p.gm, tc_apply_ctas(p.gm, 1, 64), w.coef, save_mean, w.shift, st))
-        return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d)", cr);
-    } else dwt::tiled_bwd_apply(x, dout, dx, p.gm_ew, p.vec, p.chunks_ew, w.coef, st);
+    Launch l(c.name(true, APPLY), &p.gm, (3.0 + (dout2 && !masked ? 1.0 : 0.0)) * E, st);
+    switch (c.r.fam) {
+      case CL:
+        if (masked) dwt::cl_bwd_apply(x, dresidual, nullptr, dx, bf16, p.gm, cp.new_, cp.gz_ew, DWT_EPI_AFFINE, w.coef, save_mean, save_w, gamma, beta, st);
+        else dwt::cl_bwd_apply(x, dout, dout2, dx, bf16, p.gm, cp.new_, cp.gz_ew, epi, w.coef, save_mean, save_w, gamma, beta, st);
+        break;
+      case SMALL: dwt::small_bwd_apply(x, dout, dx, bf16, p.gm_ew, p.vec, p.chunks_ew, epi, w.coef, save_mean, save_w, gamma, beta, st); break;
+      case TILED: dwt::tiled_bwd_apply(x, dout, dx, p.gm_ew, p.vec, p.chunks_ew, w.coef, st); break;
+      case TC:
+        if (int cr = dwt::tc_bwd_apply(x, dout, dx, bf16, nhwc, p.gm, tc_apply_ctas(p.gm, 1, 64), w.coef, save_mean, w.shift, st))
+          return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d)", cr);
+    }
   }
-  return check_launch("whitening backward apply kernel");
+  return check_launch(c.r.fam == CL ? "channels-last backward apply kernel" : "whitening backward apply kernel");
 }
 
 // ---- two-site residual tail (dwt_tail2_fwd / dwt_tail2_bwd) ----------------------------------------------
@@ -648,8 +646,9 @@ int tail2_plan(Plan& p, int kind, bool bf16, const dwt_tail_site* s, const void*
   if (kind == DWT_KIND_BN && GS != 1) return fail(DWT_E_INVALID, "batch norm has group_size 1 (got %d)", GS);
   if (!s) return fail(DWT_E_INVALID, "null pointer argument");
   if (int rc = make_plan(p, K_STATS, K_APPLY, s[0].x, s[1].x, out, N, C, HW, GS, D, 4)) return rc;
-  if (!dwt::cl_supports((int)C, GS))
-    return fail(DWT_E_UNSUPPORTED, "the two-site tail runs on the channels-last kernels: group_size 1, 2, 4 with C a multiple of 4, C/4 <= 16384 (C=%lld gs=%d)",
+  Route r;
+  if (route(p, true, bf16, nullptr, &r) != DWT_OK || r.fam != CL)
+    return fail(DWT_E_UNSUPPORTED, "the two-site tail runs on the channels-last kernels: " DWT_CL_RULE " (C=%lld gs=%d)",
                 (long long)C, GS);
   for (int k = 0; k < 2; ++k)
     if (!s[k].x || !s[k].gamma || !s[k].beta || !s[k].save_mean || !s[k].save_w || !out) return fail(DWT_E_INVALID, "null pointer argument");

@@ -4,66 +4,80 @@ Saved for backward: the layer input x plus the tiny per-group statistics (mean, 
 centred copy, a transposed copy or the covariance graph the reference's autograd keeps
 (utils/whitening.py:44-55).
 
-Activations are float32 or bfloat16 (what torch.autocast(dtype=torch.bfloat16) hands over from a convolution): a bf16
-call whose activations are all bf16 runs the bf16 kernels (DWT_DTYPE_BF16) when it is channels-last on a channels-last
-geometry (group sizes 1, 2, 4) or on a channels-last tensor-core geometry (_nhwc_tensor_core), NCHW whitening at group
-sizes 1, 2, 4 or NCHW batch norm with HW % 4 == 0 (_bf16_small), or NCHW whitening on a tensor-core geometry
-(_bf16_tensor_core); any other bf16 call runs the float32 kernels on upcast copies and casts the result back.  Statistics, parameters, their gradients and the running
-buffers are float32 either way, like nn.BatchNorm2d under autocast.
+Activations are float32 or bfloat16 (what torch.autocast(dtype=torch.bfloat16) hands over from a convolution): route()
+decides whether the bf16 kernels (DWT_DTYPE_BF16) take a bf16 call or the float32 kernels run on upcast copies.
+Statistics, parameters, their gradients and the running buffers are float32 either way, like nn.BatchNorm2d under autocast.
 """
 from __future__ import annotations
+
+import math
+from typing import NamedTuple
 
 import torch
 
 from . import _native as nv
 
 
+def _channels_last(x):
+    """x is a 4-D tensor dense in torch.channels_last order (and not also NCHW-contiguous)."""
+    return x.dim() == 4 and not x.is_contiguous() and x.is_contiguous(memory_format=torch.channels_last)
+
+
+def _channels_last_family(x, group_size):
+    """x runs on the channels-last kernels of group sizes 1, 2, 4 (nv.channels_last_supported) as it is."""
+    return _channels_last(x) and nv.channels_last_supported(x.shape[1], group_size)
+
+
 def _nhwc_tensor_core(x, group_size, n_domains):
     """The channels-last tensor-core rule for x (nv.tensor_core_nhwc_supported on its per-domain geometry) with a
-    16-byte-aligned data_ptr(); a misaligned view is not taken (it is copied to NCHW by _dense)."""
-    if n_domains is None or x.dim() != 4 or x.shape[0] % n_domains:
-        return False
-    return (nv.tensor_core_nhwc_supported(x.shape[0] // n_domains, x.shape[1], x.shape[2] * x.shape[3], group_size)
-            and x.data_ptr() % 16 == 0)
+    16-byte-aligned data_ptr(); a misaligned view is not taken (the forward copies it to NCHW)."""
+    return (x.dim() == 4 and x.shape[0] % n_domains == 0 and x.data_ptr() % 16 == 0
+            and nv.tensor_core_nhwc_supported(x.shape[0] // n_domains, x.shape[1], x.shape[2] * x.shape[3], group_size))
 
 
-def _dense(x: torch.Tensor, group_size: int, n_domains=None):
-    """[N, C, *spatial] -> (dense tensor, N, C, HW, channels_last?).
+class Route(NamedTuple):
+    """How a norm call reaches the kernels (the Python side of route() in csrc/api.cu)."""
+    nhwc: bool        # x goes as it is, channels-last (DWT_LAYOUT_NHWC); else NCHW-contiguous
+    bf16: bool        # the kernels take the bf16 activations (DWT_DTYPE_BF16)
+    cl: bool          # the channels-last kernels of group sizes 1, 2, 4: they also take a second gradient addend
+    align: int        # bytes of alignment the kernels need of dout (a misaligned one is copied); 0: any, or refused
 
-    A 4-D tensor that is already dense in torch.channels_last order is used as it is (NHWC kernels) when the geometry
-    has a channels-last build: the channels-last kernels (group sizes 1, 2, 4), or -- given n_domains -- the tensor-core
-    kernels (_nhwc_tensor_core); anything else is made NCHW-contiguous."""
-    n, c = x.shape[0], x.shape[1]
-    hw = 1
-    for s in x.shape[2:]:
-        hw *= s
-    nhwc = (x.dim() == 4 and not x.is_contiguous() and x.is_contiguous(memory_format=torch.channels_last)
-            and (nv.channels_last_supported(c, group_size) or _nhwc_tensor_core(x, group_size, n_domains)))
-    if not nhwc and not x.is_contiguous():
-        x = x.contiguous()
-    return x, n, c, hw, nhwc
+
+def route(x, residual, kind, group_size, n_domains):
+    """The Route of a norm call on x (and the residual), or None when the call runs the float32 kernels on upcast copies:
+    bf16 activations the bf16 kernels lack (a geometry or alignment they are not built for, mixed dtypes).  Ask again
+    for the float32 copies: their rules differ (a channels-last call at group size 128 stays channels-last)."""
+    gs = group_size if kind == "whiten" else 1
+    dtypes = {x.dtype} | ({residual.dtype} if residual is not None else set())
+    cl = _channels_last_family(x, gs)
+    if torch.bfloat16 in dtypes and dtypes <= set(_ACT_DTYPES):
+        if dtypes != {torch.bfloat16}:
+            return None
+        if _channels_last(x):   # the bf16 tensor-core kernels stop at group size 64
+            tc = kind == "whiten" and residual is None and gs <= nv.MAX_GROUP_SIZE and _nhwc_tensor_core(x, gs, n_domains)
+            return Route(True, True, cl, 0 if cl else 16) if cl or tc else None
+        if _bf16_small(x, gs, residual) or _bf16_tensor_core(x, kind, gs, n_domains, residual):
+            return Route(False, True, False, 8 if gs in (1, 2, 4) else 16)     # register-resident or tensor-core kernels
+        return None
+    nhwc = cl or (_channels_last(x) and _nhwc_tensor_core(x, gs, n_domains))
+    # tensor-core kernels: 16 bytes for their TMA loads (group size 128 in NCHW fp32 as well: it has no other kernel)
+    return Route(nhwc, False, cl, 16 if not cl and (nhwc or gs > nv.MAX_GROUP_SIZE) else 0)
 
 
 def _bf16_tensor_core(x, kind, group_size, n_domains, residual):
     """A bf16 NCHW whitening call the tensor-core kernels take in bf16 (nv.tensor_core_bf16_supported, 16-byte-aligned
-    x; a non-contiguous x is copied into a fresh, aligned tensor by _dense)."""
+    x; a non-contiguous x is copied into a fresh, aligned tensor by the forward)."""
     if kind != "whiten" or residual is not None or x.dim() < 3 or x.shape[0] % n_domains:
         return False
-    n, c = x.shape[0] // n_domains, x.shape[1]
-    hw = 1
-    for s in x.shape[2:]:
-        hw *= s
+    n, c, hw = x.shape[0] // n_domains, x.shape[1], math.prod(x.shape[2:])
     return nv.tensor_core_bf16_supported(n, c, hw, group_size) and (not x.is_contiguous() or x.data_ptr() % 16 == 0)
 
 
 def _bf16_small(x, group_size, residual):
     """A bf16 NCHW call the register-resident kernels take in bf16 (nv.small_bf16_supported: whitening at group sizes
     1, 2, 4 or batch norm, HW % 4 == 0): x and the residual bf16 and 8-byte aligned, or non-contiguous (then copied
-    into a fresh, aligned tensor by _dense / _NormFunction.forward)."""
-    hw = 1
-    for s in x.shape[2:]:
-        hw *= s
-    return nv.small_bf16_supported(hw, group_size) and all(
+    into a fresh, aligned tensor by _NormFunction.forward)."""
+    return nv.small_bf16_supported(math.prod(x.shape[2:]), group_size) and all(
         t.dtype == torch.bfloat16 and (not t.is_contiguous() or t.data_ptr() % 8 == 0) for t in (x, residual) if t is not None)
 
 
@@ -82,22 +96,18 @@ class _NormFunction(torch.autograd.Function):
     """Shared by whitening (kind='whiten') and domain batch norm (kind='bn').
 
     x is [n_domains*N, C, *]; `running` is a list of n_domains (mean, second-moment) buffer pairs
-    (entries may alias); gamma/beta are [C]-sized or None; relu fuses max(.,0) behind the affine.
+    (entries may alias); gamma/beta are [C]-sized or None; relu fuses max(.,0) behind the affine; r: route() of the call.
     """
 
     @staticmethod
     def forward(ctx, x, gamma, beta, residual, kind, group_size, n_domains, mode, eps, momentum, update_running,
-                running, relu):
+                running, relu, r):
         lib = nv.lib()
         gs = group_size if kind == "whiten" else 1
-        x, n_all, c, hw, nhwc = _dense(x, gs, n_domains)
-        bf16 = x.dtype == torch.bfloat16
-        if bf16 and not ((nhwc and (residual is None or residual.dtype == x.dtype))
-                         or (not nhwc and (_bf16_small(x, gs, residual) or _bf16_tensor_core(x, kind, gs, n_domains, residual)))):
-            raise nv.NativeError("bfloat16 runs on the channels-last kernels and the NCHW kernels of group sizes 1, 2, 4 "
-                                 "(HW % 4 == 0) with every activation in bfloat16, or on the NCHW tensor-core whitening "
-                                 "kernels (norm() upcasts anything else)")
-        layout = (nv.LAYOUT_NHWC if nhwc else 0) | (nv.DTYPE_BF16 if bf16 else 0)
+        if not r.nhwc and not x.is_contiguous():
+            x = x.contiguous()
+        n_all, c, hw = x.shape[0], x.shape[1], math.prod(x.shape[2:])
+        layout = (nv.LAYOUT_NHWC if r.nhwc else 0) | (nv.DTYPE_BF16 if r.bf16 else 0)
         if n_all % n_domains != 0:
             raise ValueError(f"batch of {n_all} does not split into {n_domains} domains")
         n = n_all // n_domains
@@ -113,7 +123,7 @@ class _NormFunction(torch.autograd.Function):
         if residual is not None:
             if gamma is None or not relu or residual.shape != x.shape:
                 raise ValueError("a fused residual needs gamma/beta, relu=True and a tensor shaped like x")
-            residual = residual.contiguous(memory_format=torch.channels_last) if nhwc else residual.contiguous()
+            residual = residual.contiguous(memory_format=torch.channels_last) if r.nhwc else residual.contiguous()
         if gamma is not None:
             epi = nv.EPI_AFFINE | (nv.EPI_RELU if relu else 0) | (nv.EPI_RESIDUAL if residual is not None else 0)
             gamma_c, beta_c = gamma.detach().reshape(-1).contiguous(), beta.detach().reshape(-1).contiguous()
@@ -122,7 +132,7 @@ class _NormFunction(torch.autograd.Function):
         y = torch.empty_like(x)                      # keeps x's memory format
         # residual tail on the channels-last kernels: the apply pass leaves one byte per float4 with the four
         # (out > 0) bits, which is all the backward needs of the output
-        mask = torch.empty(x.numel() // 4, dtype=torch.uint8, device=dev) if (residual is not None and nhwc) else None
+        mask = torch.empty(x.numel() // 4, dtype=torch.uint8, device=dev) if (residual is not None and r.nhwc) else None
         save_mean = torch.empty(n_domains, c, dtype=torch.float32, device=dev)
         save_w = torch.empty(n_domains, c // gs, gs, gs, dtype=torch.float32, device=dev)
         ws = nv.workspace(dev, n, c, hw, gs, n_domains)
@@ -165,6 +175,7 @@ class _NormFunction(torch.autograd.Function):
         else:
             ctx.save_for_backward(x, save_mean, save_w, gamma_c, beta_c)
         ctx.cfg = (kind, gs, n_domains, mode | layout, eps, epi, n, c, hw, None if gamma is None else gamma.shape)
+        ctx.route = r
         return y
 
     @staticmethod
@@ -182,23 +193,18 @@ class _NormFunction(torch.autograd.Function):
         else:
             x, save_mean, save_w, gamma_c, beta_c = ctx.saved_tensors
         kind, gs, n_domains, mode, eps, epi, n, c, hw, gshape = ctx.cfg
+        r = ctx.route
         # second addend of the incoming gradient, left here by fork_for_sum's backward (see there): the channels-last
         # kernels of group sizes 1, 2, 4 add it where they read dout; any other path adds it now
         dout2 = ctx.__dict__.pop("_dwt_extra_grad", None)
         if dout.dtype != x.dtype:
             dout = dout.to(x.dtype)
-        nhwc = bool(mode & nv.LAYOUT_NHWC)
-        cl_kernels = nhwc and nv.channels_last_supported(c, gs)
-        if dout2 is not None and not (cl_kernels and dout2.shape == dout.shape and dout2.dtype == dout.dtype
+        if dout2 is not None and not (r.cl and dout2.shape == dout.shape and dout2.dtype == dout.dtype
                                       and dout2.is_contiguous(memory_format=torch.channels_last)):
             dout, dout2 = dout + dout2, None
-        dout = dout.contiguous(memory_format=torch.channels_last) if nhwc else dout.contiguous()
-        # the forward ran the tensor-core kernels, whose TMA loads need 16 bytes (group size 128 in NCHW fp32 as well: it
-        # has no other kernel), or (bf16 NCHW, group sizes 1, 2, 4) the
-        # register-resident kernels, whose bf16 loads need 8: copy a misaligned dout (a fresh tensor keeps the layout)
-        align = 8 if not nhwc and gs in (1, 2, 4) else 16
-        if ((mode & nv.DTYPE_BF16) or nhwc or gs > nv.MAX_GROUP_SIZE) and not cl_kernels and dout.data_ptr() % align:
-            dout = dout.clone(memory_format=torch.channels_last if nhwc else torch.contiguous_format)
+        dout = dout.contiguous(memory_format=torch.channels_last) if r.nhwc else dout.contiguous()
+        if r.align and dout.data_ptr() % r.align:    # a fresh tensor keeps the layout
+            dout = dout.clone(memory_format=torch.channels_last if r.nhwc else torch.contiguous_format)
         dev = nv.require_cuda(dout, bf16=True)
         dx = torch.empty_like(x)                     # x's layout: channels-last when the forward ran NHWC
         want_affine = gamma_c is not None and (ctx.needs_input_grad[1] or ctx.needs_input_grad[2])
@@ -224,7 +230,7 @@ class _NormFunction(torch.autograd.Function):
         nv.check(rc)
         if want_affine:
             dgamma, dbeta = dgamma.view(gshape), dbeta.view(gshape)
-        return (dx, dgamma, dbeta, d_res if ctx.needs_input_grad[3] else None) + (None,) * 9
+        return (dx, dgamma, dbeta, d_res if ctx.needs_input_grad[3] else None) + (None,) * 10
 
 
 class _TailPairFunction(torch.autograd.Function):
@@ -237,7 +243,7 @@ class _TailPairFunction(torch.autograd.Function):
     def forward(ctx, x, xd, gamma, beta, gamma_d, beta_d, kind, group_size, n_domains, sites):
         lib = nv.lib()
         gs = group_size if kind == "whiten" else 1
-        if not (x.dim() == 4 and x.shape == xd.shape and _dense(x, gs)[4] and _dense(xd, gs)[4]):
+        if not (x.shape == xd.shape and _channels_last_family(x, gs) and _channels_last_family(xd, gs)):
             raise ValueError("the two-site tail takes two channels-last tensors of one shape with a channels-last build")
         if x.shape[0] % n_domains != 0:
             raise ValueError(f"batch of {x.shape[0]} does not split into {n_domains} domains")
@@ -364,23 +370,15 @@ def norm(x, gamma, beta, *, kind, group_size, n_domains, training_stats, eps, mo
          running, relu=False, residual=None):
     mode = nv.MODE_TRAIN if training_stats else nv.MODE_EVAL
     args = (kind, group_size, n_domains, mode, float(eps), float(momentum), bool(update_running), running, bool(relu))
-    dtypes = {x.dtype} | ({residual.dtype} if residual is not None else set())
-    if torch.bfloat16 in dtypes and dtypes <= set(_ACT_DTYPES):
-        gs = group_size if kind == "whiten" else 1
-        cl = x.dim() == 4 and not x.is_contiguous() and x.is_contiguous(memory_format=torch.channels_last)
-        # the bf16 tensor-core kernels stop at group size 64: a channels-last bf16 call at 128 upcasts (x.float() keeps
-        # the channels-last strides, so the fp32 channels-last kernels run)
-        cl_tc = kind == "whiten" and residual is None and gs <= nv.MAX_GROUP_SIZE and _nhwc_tensor_core(x, gs, n_domains)
-        bf16_kernels = dtypes == {torch.bfloat16} and (
-            (nv.channels_last_supported(x.shape[1], gs) or cl_tc) if cl
-            else _bf16_small(x, gs, residual) or _bf16_tensor_core(x, kind, gs, n_domains, residual))
-        if not bf16_kernels:
-            # geometries and alignments the bf16 kernels lack (NCHW HW % 4 != 0, BatchNorm1d on [N, C], a misaligned
-            # view, ...) or mixed dtypes: the float32 kernels on upcast copies, the result (and through autograd every
-            # gradient of x and the residual) back in x's dtype
-            y = _NormFunction.apply(x.float(), gamma, beta, None if residual is None else residual.float(), *args)
-            return y.to(x.dtype)
-    return _NormFunction.apply(x, gamma, beta, residual, *args)
+    r = route(x, residual, kind, group_size, n_domains)
+    if r is None:
+        # geometries and alignments the bf16 kernels lack (NCHW HW % 4 != 0, BatchNorm1d on [N, C], a misaligned
+        # view, ...) or mixed dtypes: the float32 kernels on upcast copies (x.float() keeps channels-last strides), the
+        # result (and through autograd every gradient of x and the residual) back in x's dtype
+        xf, rf = x.float(), None if residual is None else residual.float()
+        y = _NormFunction.apply(xf, gamma, beta, rf, *args, route(xf, rf, kind, group_size, n_domains))
+        return y.to(x.dtype)
+    return _NormFunction.apply(x, gamma, beta, residual, *args, r)
 
 
 class _MecFunction(torch.autograd.Function):

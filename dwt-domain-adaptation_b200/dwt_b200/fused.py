@@ -29,7 +29,6 @@ from __future__ import annotations
 import torch
 import torch.nn as nn
 
-from . import _native as nv
 from . import functional as F
 
 
@@ -110,8 +109,7 @@ class DomainTripleNorm(nn.Module):
                 and len(mods) == len(down_mods) == self.n_domains and x.dim() == 4 and x.shape == xd.shape
                 and mods[0].training and down_mods[0].training
                 and x.dtype == xd.dtype
-                and all(t.is_contiguous(memory_format=torch.channels_last) and not t.is_contiguous() for t in (x, xd))
-                and nv.channels_last_supported(x.shape[1], self.group_size))
+                and all(F._channels_last_family(t, self.group_size) for t in (x, xd)))
         if not pair:
             identity = down(xd, down_mods, down_gamma, down_beta, relu=False, count_batches=count_batches)
             return self(x, mods, gamma, beta, True, residual=identity, count_batches=count_batches)
