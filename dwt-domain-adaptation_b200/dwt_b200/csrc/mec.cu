@@ -22,6 +22,58 @@ __device__ __forceinline__ float warp_max(float v) {
   return v;
 }
 
+// log_softmax(x)[k] = (x[k] - a) - b for one row of max mx and log partition sum ls = log(sum_k exp(x[k] - mx)).
+// Once |mx| is large, (a, b) = (mx, ls): subtracting the max first keeps ls's absolute precision, which rounding
+// mx + ls to fp32 would cost (gradient error 2e-5 at logits ~1e3, 2e-4 at ~1e4).  Below kShiftedFrom the row keeps
+// (a, b) = (mx + ls, 0), the earlier form, bit for bit: there that rounding costs at most 2^-18 absolute, and a
+// training step carries a one-ulp change of this gradient to a ~1e-2 change of the logits after one update, so
+// results (and the benchmark's outputs) stay reproducible across builds.
+constexpr float kShiftedFrom = 64.f;
+
+struct Lsm {
+  float a, b;
+};
+
+__device__ __forceinline__ Lsm lsm_of(float mx, float ls) {
+  return fabsf(mx) < kShiftedFrom ? Lsm{mx + ls, 0.f} : Lsm{mx, ls};
+}
+
+__device__ __forceinline__ float lsm(float x, Lsm l) { return (x - l.a) - l.b; }
+
+// One warp's work on row pair (x, y) of the MEC term.  The row minimum of s_k = -(lsm(x)[k] + lsm(y)[k]) / 2 follows
+// torch.min: the first minimum, and a NaN wins (the first NaN), so a non-finite row reaches the loss as NaN instead of
+// leaving best at FLT_MAX.
+struct MecRow {
+  Lsm lx, ly;
+  float best;               // min_k s_k (NaN if any s_k is NaN)
+  int bk;                   // its class k*
+};
+
+__device__ __forceinline__ MecRow mec_row(const float* __restrict__ xr, const float* __restrict__ yr, int K, int lane) {
+  MecRow r;
+  float mx = -FLT_MAX, my = -FLT_MAX;
+  for (int k = lane; k < K; k += 32) { mx = fmaxf(mx, xr[k]); my = fmaxf(my, yr[k]); }
+  mx = warp_max(mx); my = warp_max(my);
+  float sx = 0.f, sy = 0.f;
+  for (int k = lane; k < K; k += 32) { sx += expf(xr[k] - mx); sy += expf(yr[k] - my); }
+  r.lx = lsm_of(mx, logf(warp_sum(sx)));
+  r.ly = lsm_of(my, logf(warp_sum(sy)));
+  float best = FLT_MAX; int bk = 0x7fffffff;
+  for (int k = lane; k < K; k += 32) {
+    const float s = -0.5f * (lsm(xr[k], r.lx) + lsm(yr[k], r.ly));
+    if (s < best || (s != s && best == best)) { best = s; bk = k; }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float ob = __shfl_xor_sync(0xffffffffu, best, o);
+    const int ok = __shfl_xor_sync(0xffffffffu, bk, o);
+    const bool onan = ob != ob, bnan = best != best;
+    if (ob < best || (onan && !bnan) || ((ob == best || (onan && bnan)) && ok < bk)) { best = ob; bk = ok; }
+  }
+  r.best = best; r.bk = bk;
+  return r;
+}
+
 __global__ void __launch_bounds__(kMecThreads) mec_kernel(const float* __restrict__ x, const float* __restrict__ y,
                                                            int N, int K, float* __restrict__ loss,
                                                            float* __restrict__ gx, float* __restrict__ gy) {
@@ -32,30 +84,12 @@ __global__ void __launch_bounds__(kMecThreads) mec_kernel(const float* __restric
   for (int n = warp; n < N; n += nwarps) {
     const float* xr = x + (size_t)n * K;
     const float* yr = y + (size_t)n * K;
-    float mx = -FLT_MAX, my = -FLT_MAX;
-    for (int k = lane; k < K; k += 32) { mx = fmaxf(mx, xr[k]); my = fmaxf(my, yr[k]); }
-    mx = warp_max(mx); my = warp_max(my);
-    float sx = 0.f, sy = 0.f;
-    for (int k = lane; k < K; k += 32) { sx += expf(xr[k] - mx); sy += expf(yr[k] - my); }
-    sx = warp_sum(sx); sy = warp_sum(sy);
-    const float lzx = mx + logf(sx), lzy = my + logf(sy);     // log partition functions
-    // s_k = -(lx_k + ly_k)/2 ; first minimum over k
-    float best = FLT_MAX; int bk = 0x7fffffff;
+    const MecRow r = mec_row(xr, yr, K, lane);
+    wsum += r.best;
     for (int k = lane; k < K; k += 32) {
-      float s = -0.5f * ((xr[k] - lzx) + (yr[k] - lzy));
-      if (s < best) { best = s; bk = k; }
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      float ob = __shfl_xor_sync(0xffffffffu, best, o);
-      int ok = __shfl_xor_sync(0xffffffffu, bk, o);
-      if (ob < best || (ob == best && ok < bk)) { best = ob; bk = ok; }
-    }
-    wsum += best;
-    for (int k = lane; k < K; k += 32) {
-      const float hot = (k == bk) ? 1.f : 0.f;
-      gx[(size_t)n * K + k] = scale * (expf(xr[k] - lzx) - hot);
-      gy[(size_t)n * K + k] = scale * (expf(yr[k] - lzy) - hot);
+      const float hot = (k == r.bk) ? 1.f : 0.f;
+      gx[(size_t)n * K + k] = scale * (expf(lsm(xr[k], r.lx)) - hot);
+      gy[(size_t)n * K + k] = scale * (expf(lsm(yr[k], r.ly)) - hot);
     }
   }
   if (lane == 0) sRow[warp] = wsum;
@@ -107,38 +141,20 @@ __global__ void __launch_bounds__(kMecThreads) head_loss_kernel(const float* __r
       mx = warp_max(mx);
       float sx = 0.f;
       for (int k = lane; k < K; k += 32) sx += expf(xr[k] - mx);
-      sx = warp_sum(sx);
-      const float lz = mx + logf(sx);
-      cls += (lane == 0 && use) ? (lz - xr[y]) : 0.f;
+      const Lsm l = lsm_of(mx, logf(warp_sum(sx)));
+      cls += (lane == 0 && use) ? ((l.a - xr[y]) + l.b) : 0.f;     // -lsm(x)[y]
       const float sc = use ? 1.f / (float)valid : 0.f;
-      for (int k = lane; k < K; k += 32) grad[(size_t)n * K + k] = sc * (expf(xr[k] - lz) - (k == y ? 1.f : 0.f));
+      for (int k = lane; k < K; k += 32) grad[(size_t)n * K + k] = sc * (expf(lsm(xr[k], l)) - (k == y ? 1.f : 0.f));
     } else {                                       // target row n and its augmented twin n + B: MEC
       const float* xr = logits + (size_t)n * K;
       const float* yr = logits + (size_t)(n + B) * K;
-      float mx = -FLT_MAX, my = -FLT_MAX;
-      for (int k = lane; k < K; k += 32) { mx = fmaxf(mx, xr[k]); my = fmaxf(my, yr[k]); }
-      mx = warp_max(mx); my = warp_max(my);
-      float sx = 0.f, sy = 0.f;
-      for (int k = lane; k < K; k += 32) { sx += expf(xr[k] - mx); sy += expf(yr[k] - my); }
-      sx = warp_sum(sx); sy = warp_sum(sy);
-      const float lzx = mx + logf(sx), lzy = my + logf(sy);
-      float best = FLT_MAX; int bk = 0x7fffffff;
-      for (int k = lane; k < K; k += 32) {
-        const float s = -0.5f * ((xr[k] - lzx) + (yr[k] - lzy));
-        if (s < best) { best = s; bk = k; }
-      }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        const float ob = __shfl_xor_sync(0xffffffffu, best, o);
-        const int ok = __shfl_xor_sync(0xffffffffu, bk, o);
-        if (ob < best || (ob == best && ok < bk)) { best = ob; bk = ok; }
-      }
-      mec += (lane == 0) ? best : 0.f;
+      const MecRow r = mec_row(xr, yr, K, lane);
+      mec += (lane == 0) ? r.best : 0.f;
       const float sc = lambda * 0.5f / (float)B;
       for (int k = lane; k < K; k += 32) {
-        const float hot = (k == bk) ? 1.f : 0.f;
-        grad[(size_t)n * K + k] = sc * (expf(xr[k] - lzx) - hot);
-        grad[(size_t)(n + B) * K + k] = sc * (expf(yr[k] - lzy) - hot);
+        const float hot = (k == r.bk) ? 1.f : 0.f;
+        grad[(size_t)n * K + k] = sc * (expf(lsm(xr[k], r.lx)) - hot);
+        grad[(size_t)(n + B) * K + k] = sc * (expf(lsm(yr[k], r.ly)) - hot);
       }
     }
   }
