@@ -442,6 +442,31 @@ struct Call {
   const char* name(bool bwd, Pass ps) const { return kProfName[bwd][r.fam][ps][2 * nhwc + bf16]; }
 };
 
+// The ZCA basis (dwt_whiten_zca_*): Newton-Schulz iterations, and the matrices they save for the backward.
+// on == false: the Cholesky basis (dwt_whiten_*, dwt_bn_*).
+struct Zca {
+  bool on = false;
+  int iters = 0;
+  const float* save_p = nullptr;   // [D][C/gs][iters][gs][gs]: written by the forward, read by the backward
+};
+
+int zca_refuse(const Call& c) {
+  const dwt::Geom& g = c.p.gm;
+  return fail(DWT_E_UNSUPPORTED, "the ZCA basis is built for the tensor-core kernels only: group_size 8, 16, 32, 64, HW >= 32 "
+              "and a multiple of 4 (NCHW bf16: of 8), N*HW >= 4096 per domain, tensors 16-byte aligned (C=%d HW=%d N=%d gs=%d)",
+              g.C, g.HW, g.N, g.GS);
+}
+
+// a ZCA call's own arguments, and its family: validate()'s route, which must be the tensor-core one
+int zca_check(const Call& c, const Zca& z) {
+  if (z.iters < 1 || z.iters > DWT_ZCA_MAX_ITERATIONS)
+    return fail(DWT_E_INVALID, "iterations %d outside [1,%d]", z.iters, DWT_ZCA_MAX_ITERATIONS);
+  if (!z.save_p) return fail(DWT_E_INVALID, "null pointer argument (save_p)");
+  if ((uintptr_t)z.save_p % 16 != 0) return fail(DWT_E_INVALID, "save_p must be 16-byte aligned");
+  if (c.p.gm.GS > DWT_MAX_GROUP_SIZE || c.r.fam != TC) return zca_refuse(c);
+  return DWT_OK;
+}
+
 // The checks both directions make, in order; `own` holds the direction's own (residual, running buffers, gradient
 // outputs), checked before the epilogue's family rule.  in0, in1: the tensors the kernels read (x, x or x, dout);
 // out: the one they write (y or dx); dout2: the backward's second gradient addend.
@@ -480,7 +505,7 @@ int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, 
                     float b, float momentum, float unbias, int update_running, float* const* rmean,
                     float* const* rcov, const float* gamma, const float* beta, const float* residual,
                     uint8_t* relu_mask, int epi, float* save_mean, float* save_w, void* ws, size_t ws_bytes,
-                    cudaStream_t st) {
+                    cudaStream_t st, const Zca& zca = Zca{}) {
   Call c;
   const bool need_running = ((mode & 0xFF) == DWT_MODE_EVAL) || update_running;
   const int rc = validate(c, false, x, x, y, nullptr, N, C, HW, GS, D, mode, epi, gamma, beta, save_mean, save_w, ws, ws_bytes, [&] {
@@ -488,9 +513,11 @@ int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, 
     if (epi & DWT_EPI_RESIDUAL) if (int rc = check_align(c.bf16, (uintptr_t)residual, "residual")) return rc;
     if (relu_mask && !((epi & DWT_EPI_RESIDUAL) && c.nhwc))
       return fail(DWT_E_UNSUPPORTED, "the ReLU byte map is written by the channels-last RESIDUAL epilogue only");
+    if (zca.on) if (int rc = zca_check(c, zca)) return rc;
     return check_running(need_running, rmean, rcov, D);
   });
   if (rc) return rc;
+  if (zca.on && c.r.fam != TC) return zca_refuse(c);   // the tensor-core kernels could not be set up: no tiled ZCA
   const Plan& p = c.p; const Workspace& w = c.w;
   const bool bf16 = c.bf16, nhwc = c.nhwc, train = c.mode == DWT_MODE_TRAIN;
   const dwt::FwdFin fin = make_fwd_fin(a, b, momentum, unbias, train ? update_running : 0, need_running, rmean, rcov,
@@ -519,7 +546,7 @@ int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, 
     }
     if (c.r.fam == CL || c.r.fam == TC) {   // the small and tiled kernels finalize in their last CTA
       if (int rc = check_launch(c.r.fam == CL ? "channels-last statistics kernel" : "tensor-core statistics kernel")) return rc;
-      Launch l(c.name(false, FINALIZE), &p.gm, 0.0, st);
+      Launch l(zca.on ? fam(bf16, "dense_fwd_zca", "dense_fwd_zca_bf16") : c.name(false, FINALIZE), &p.gm, 0.0, st);
       if (c.r.fam == CL) {
         dwt::cl_fwd_finalize(w.partial, cp.nred, w.shift, p.gm, fin, st);
       } else {
@@ -527,9 +554,13 @@ int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, 
         if (gs128)
           dwt::dense_partial_reduce(w.partial + pair_part, tc_pair_chunks(p.gm, false), dwt::tc_superblocks(p.gm) / 2 * D,
                                     w.gram + (size_t)dwt::tc_superblocks(p.gm) * D * (64 * 64 + 64), st);
-        dwt::dense_fwd_factor(w.gram, w.shift, p.gm, fin, st);
+        if (zca.on) dwt::dense_fwd_zca(w.gram, w.shift, p.gm, fin, zca.iters, const_cast<float*>(zca.save_p), st);
+        else dwt::dense_fwd_factor(w.gram, w.shift, p.gm, fin, st);
       }
     }
+  } else if (zca.on) {
+    Launch l(fam(bf16, "dense_fwd_zca", "dense_fwd_zca_bf16"), &p.gm, 0.0, st);
+    dwt::dense_fwd_zca(nullptr, nullptr, p.gm, fin, zca.iters, const_cast<float*>(zca.save_p), st);
   } else {
     Launch l(c.name(false, PREP), &p.gm, 0.0, st);
     if (c.r.fam == TC) dwt::dense_fwd_factor(nullptr, nullptr, p.gm, fin, st);
@@ -554,7 +585,7 @@ int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, 
 int whiten_like_bwd(const float* x, const float* dout, const float* dout2, float* dx, int64_t N, int64_t C, int64_t HW, int GS, int D,
                     int mode, float a, const float* save_mean, const float* save_w, const float* gamma,
                     const float* beta, const uint8_t* relu_mask, float* dresidual, int epi, float* dgamma,
-                    float* dbeta, void* ws, size_t ws_bytes, cudaStream_t st) {
+                    float* dbeta, void* ws, size_t ws_bytes, cudaStream_t st, const Zca& zca = Zca{}) {
   Call c;
   const int rc = validate(c, true, x, dout, dx, dout2, N, C, HW, GS, D, mode, epi, gamma, beta, save_mean, save_w, ws, ws_bytes, [&] {
     if (epi & DWT_EPI_RESIDUAL) {
@@ -568,9 +599,11 @@ int whiten_like_bwd(const float* x, const float* dout, const float* dout2, float
       return fail(DWT_E_INVALID, "relu_mask / dresidual belong to the RESIDUAL epilogue");
     }
     if ((dgamma == nullptr) != (dbeta == nullptr)) return fail(DWT_E_INVALID, "dgamma and dbeta go together");
+    if (zca.on) return zca_check(c, zca);
     return DWT_OK;
   });
   if (rc) return rc;
+  if (zca.on && c.r.fam != TC) return zca_refuse(c);   // the tensor-core kernels could not be set up: no tiled ZCA
   const Plan& p = c.p; const Workspace& w = c.w;
   const bool bf16 = c.bf16, nhwc = c.nhwc;
   const dwt::BwdFin fin = make_bwd_fin(a, c.mode, epi, save_mean, save_w, gamma, dgamma, dbeta, w);
@@ -598,14 +631,18 @@ int whiten_like_bwd(const float* x, const float* dout, const float* dout2, float
     }
     if (c.r.fam == CL || c.r.fam == TC) {   // the small and tiled kernels finalize in their last CTA
       if (int rc = check_launch(c.r.fam == CL ? "channels-last backward reduction kernel" : "tensor-core backward reduction kernel")) return rc;
-      Launch l(c.name(true, FINALIZE), &p.gm, 0.0, st);
+      Launch l(zca.on ? fam(bf16, "dense_bwd_zca", "dense_bwd_zca_bf16") : c.name(true, FINALIZE), &p.gm, 0.0, st);
       if (c.r.fam == CL) {
         dwt::cl_bwd_finalize(w.partial, cp.nred, p.gm, fin, st);
       } else {
         dwt::dense_partial_reduce(w.partial, rchunks, rproblems, w.gram, st);
-        dwt::dense_bwd_coef(w.gram, p.gm, fin, w.shift, st);
+        if (zca.on) dwt::dense_bwd_zca(w.gram, p.gm, fin, zca.iters, zca.save_p, w.shift, st);
+        else dwt::dense_bwd_coef(w.gram, p.gm, fin, w.shift, st);
       }
     }
+  } else if (zca.on) {
+    Launch l(fam(bf16, "dense_bwd_zca", "dense_bwd_zca_bf16"), &p.gm, 0.0, st);
+    dwt::dense_bwd_zca(nullptr, p.gm, fin, zca.iters, zca.save_p, w.shift, st);
   } else {
     Launch l(c.name(true, PREP), &p.gm, 0.0, st);
     if (c.r.fam == TC) dwt::dense_bwd_coef(nullptr, p.gm, fin, w.shift, st);
@@ -775,6 +812,23 @@ int dwt_whiten_bwd(const float* x, const float* dout, const float* dout2, float*
   return whiten_like_bwd(x, dout, dout2, dx, N, C, HW, group_size, n_domains, mode, 1.f - eps, save_mean, save_w, gamma,
                          beta, relu_mask, dresidual, epilogue, dgamma, dbeta, workspace, workspace_bytes,
                          (cudaStream_t)stream);
+}
+
+int dwt_whiten_zca_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, int group_size, int n_domains, int mode,
+                       float eps, float momentum, int update_running, float* const* running_mean, float* const* running_cov,
+                       int iterations, float* save_mean, float* save_w, float* save_p, void* workspace,
+                       size_t workspace_bytes, dwt_stream_t stream) {
+  return whiten_like_fwd(x, y, N, C, HW, group_size, n_domains, mode, 1.f - eps, eps, momentum, 1.f, update_running,
+                         running_mean, running_cov, nullptr, nullptr, nullptr, nullptr, 0, save_mean, save_w, workspace,
+                         workspace_bytes, (cudaStream_t)stream, Zca{true, iterations, save_p});
+}
+
+int dwt_whiten_zca_bwd(const float* x, const float* dout, float* dx, int64_t N, int64_t C, int64_t HW, int group_size,
+                       int n_domains, int mode, float eps, int iterations, const float* save_mean, const float* save_w,
+                       const float* save_p, void* workspace, size_t workspace_bytes, dwt_stream_t stream) {
+  return whiten_like_bwd(x, dout, nullptr, dx, N, C, HW, group_size, n_domains, mode, 1.f - eps, save_mean, save_w, nullptr,
+                         nullptr, nullptr, nullptr, 0, nullptr, nullptr, workspace, workspace_bytes, (cudaStream_t)stream,
+                         Zca{true, iterations, save_p});
 }
 
 // Batch norm is the group-size-1 member of the same family: "covariance" = biased variance,

@@ -7,6 +7,9 @@
 //   fwd_factor       per group: mean, covariance, S = a*cov + b*I, Cholesky S = L L^T, W = L^-1,
 //                    running-statistic EMA (domains in order: one CTA owns all domains of its group)
 //   bwd_coef         per (domain, group): A1 = W^T, Bm = (2a/M) sym(W^T Phi(-R W^T) W), cvec
+//   fwd_zca/bwd_zca  the same two steps in the ZCA basis (dwt_whiten_zca_*): W = P_T / sqrt(tr S) by T Newton-Schulz
+//                    iterations on shared-memory operands, and the reverse of that recursion; fwd_zca shares fwd_factor's
+//                    statistics prologue and EMA tail
 //
 // All three keep a 64x64 problem in ONE 256-thread CTA arranged 16x16, each thread owning a 4x4
 // register block.  fwd_factor runs the Cholesky factorisation AND the triangular inverse as one blocked
@@ -238,9 +241,97 @@ __device__ __forceinline__ bool factor_and_invert(float (&a)[4][4], float (&b)[4
 }
 
 // ------------------------------------------------------------------------------------------
-// fwd_factor: grid (G), 256 threads; loops over the domains in order (EMA sequence, SURVEY H5)
+// Statistics prologue and EMA tail of one domain, shared by fwd_factor and fwd_zca: both bases see the same S, write the
+// same save_mean and apply the same running-buffer update, bit for bit.
 //   gram  [D][SB][kNacc]  reduced moments around the pilot shift (null: take the running buffers = eval)
 //   shift [D][SB*64]
+// ------------------------------------------------------------------------------------------
+constexpr int kEmaPer = kSB * kSB / 256;
+
+struct EmaOld {            // the running buffers as the domain's EMA finds them (loaded with the moments)
+  float rc[kEmaPer], rm;
+  bool on;                 // train with update_running
+};
+
+// Loads domain d's moments G (null: eval, the running buffers), writes save_mean, and leaves this thread's block of
+// S = a cov + b I in a[r][s] = S(4bi + r, 4bj + s); train: the un-shrunk covariance in sC.  Contains one block barrier.
+__device__ __forceinline__ void domain_stats(const float* G, const float* __restrict__ shift, int d, int g, int sb, int o,
+                                             int SB, float invM, const Geom& gm, const FwdFin& f, const Blk& t, float* sC,
+                                             float* sMean, float* sRow, int& sBadDom, float (&a)[4][4], EmaOld& old) {
+  const int GS = gm.GS;
+  // every global load of this domain is issued before the first dependent instruction: the Gram block, the row
+  // sums, and the running buffers the EMA needs at the very end (their latency hides behind the factorisation;
+  // the previous domain's stores precede this point by a block barrier, so aliased buffers still see the ordered
+  // sequence)
+  float graw[4][4];
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+#pragma unroll
+    for (int s = 0; s < 4; ++s) {
+      float v = 0.f;
+      if (t.act) {
+        const int i = 4 * t.bi + r, j = 4 * t.bj + s, hi = i > j ? i : j, lo = i > j ? j : i;
+        v = G ? __ldcg(G + (o + hi) * kSB + o + lo) : f.rcov[d][(size_t)g * GS * GS + i * GS + j];
+      }
+      graw[r][s] = v;
+    }
+  float rowsum = 0.f, shf = 0.f;
+  if ((int)threadIdx.x < GS) {
+    if (G) { rowsum = __ldcg(G + kSB * kSB + o + threadIdx.x); shf = shift[((size_t)d * SB + sb) * kSB + o + threadIdx.x]; }
+    else shf = f.rmean[d][g * GS + threadIdx.x];
+  }
+  old.rm = 0.f;
+  old.on = G != nullptr && f.update_running;
+  if (old.on) {
+#pragma unroll
+    for (int n = 0; n < kEmaPer; ++n) {
+      const int e = threadIdx.x + 256 * n;
+      old.rc[n] = e < GS * GS ? f.rcov[d][(size_t)g * GS * GS + e] : 0.f;
+    }
+    if ((int)threadIdx.x < GS) old.rm = f.rmean[d][g * GS + threadIdx.x];
+  }
+  if ((int)threadIdx.x < GS) {
+    const float mu = G ? shf + rowsum * invM : shf;
+    sMean[threadIdx.x] = mu;
+    sRow[threadIdx.x] = rowsum * invM;              // mean of the shifted samples
+    f.save_mean[(size_t)d * gm.C + g * GS + threadIdx.x] = mu;
+  }
+  if (threadIdx.x == 0) sBadDom = 0;
+  __syncthreads();
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+#pragma unroll
+    for (int s = 0; s < 4; ++s) {
+      float v = 0.f;
+      if (t.act) {
+        const int i = 4 * t.bi + r, j = 4 * t.bj + s;
+        float cov = graw[r][s];
+        if (G) {
+          cov = cov * invM - sRow[i] * sRow[j];
+          sC[i * LDS + j] = cov;
+        }
+        v = f.a * cov + (i == j ? f.b : 0.f);
+      }
+      a[r][s] = v;
+    }
+}
+
+// The EMA of domain d (train, update_running, batch covariance accepted): sC and sMean complete behind a block barrier.
+__device__ __forceinline__ void domain_ema(int d, int g, const Geom& gm, const FwdFin& f, const float* sC, const float* sMean,
+                                           const EmaOld& old) {
+  const int GS = gm.GS;
+  const float m = f.momentum, k = 1.f - f.momentum;
+#pragma unroll
+  for (int n = 0; n < kEmaPer; ++n) {
+    const int e = threadIdx.x + 256 * n;
+    if (e < GS * GS) f.rcov[d][(size_t)g * GS * GS + e] = m * (sC[(e / GS) * LDS + e % GS] * f.unbias) + k * old.rc[n];
+  }
+  // the contraction fwd_factor has always used: fma(1 - m, old, m * mean)
+  if ((int)threadIdx.x < GS) f.rmean[d][g * GS + threadIdx.x] = fmaf(k, old.rm, __fmul_rn(m, sMean[threadIdx.x]));
+}
+
+// ------------------------------------------------------------------------------------------
+// fwd_factor: grid (G), 256 threads; loops over the domains in order (EMA sequence, SURVEY H5)
 // ------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) fwd_factor_kernel(const float* __restrict__ gram, const float* __restrict__ shift,
                                                          const Geom gm, const FwdFin f) {
@@ -258,63 +349,9 @@ __global__ void __launch_bounds__(256) fwd_factor_kernel(const float* __restrict
   for (int d = 0; d < gm.D; ++d) {
     const float* G = gram ? gram + ((size_t)d * SB + sb) * kNacc : nullptr;
     const size_t gbase = ((size_t)d * gm.G + g) * GS * GS;
-    // every global load of this domain is issued before the first dependent instruction: the Gram block, the row
-    // sums, and the running buffers the EMA needs at the very end (their latency hides behind the factorisation;
-    // the previous domain's stores precede this point by a block barrier, so aliased buffers still see the ordered
-    // sequence)
-    float graw[4][4];
-#pragma unroll
-    for (int r = 0; r < 4; ++r)
-#pragma unroll
-      for (int s = 0; s < 4; ++s) {
-        float v = 0.f;
-        if (t.act) {
-          const int i = 4 * t.bi + r, j = 4 * t.bj + s, hi = i > j ? i : j, lo = i > j ? j : i;
-          v = G ? __ldcg(G + (o + hi) * kSB + o + lo) : f.rcov[d][(size_t)g * GS * GS + i * GS + j];
-        }
-        graw[r][s] = v;
-      }
-    float rowsum = 0.f, shf = 0.f;
-    if ((int)threadIdx.x < GS) {
-      if (G) { rowsum = __ldcg(G + kSB * kSB + o + threadIdx.x); shf = shift[((size_t)d * SB + sb) * kSB + o + threadIdx.x]; }
-      else shf = f.rmean[d][g * GS + threadIdx.x];
-    }
-    constexpr int kEmaPer = kSB * kSB / 256;
-    float rc_old[kEmaPer], rm_old = 0.f;
-    const bool ema = G != nullptr && f.update_running;
-    if (ema) {
-#pragma unroll
-      for (int n = 0; n < kEmaPer; ++n) {
-        const int e = threadIdx.x + 256 * n;
-        rc_old[n] = e < GS * GS ? f.rcov[d][(size_t)g * GS * GS + e] : 0.f;
-      }
-      if ((int)threadIdx.x < GS) rm_old = f.rmean[d][g * GS + threadIdx.x];
-    }
-    if ((int)threadIdx.x < GS) {
-      const float mu = G ? shf + rowsum * invM : shf;
-      sMean[threadIdx.x] = mu;
-      sRow[threadIdx.x] = rowsum * invM;              // mean of the shifted samples
-      f.save_mean[(size_t)d * gm.C + g * GS + threadIdx.x] = mu;
-    }
-    if (threadIdx.x == 0) sBadDom = 0;
-    __syncthreads();
     float a[4][4], w[4][4];
-#pragma unroll
-    for (int r = 0; r < 4; ++r)
-#pragma unroll
-      for (int s = 0; s < 4; ++s) {
-        float v = 0.f;
-        if (t.act) {
-          const int i = 4 * t.bi + r, j = 4 * t.bj + s;
-          float cov = graw[r][s];
-          if (G) {
-            cov = cov * invM - sRow[i] * sRow[j];
-            sC[i * LDS + j] = cov;
-          }
-          v = f.a * cov + (i == j ? f.b : 0.f);
-        }
-        a[r][s] = v;
-      }
+    EmaOld old;
+    domain_stats(G, shift, d, g, sb, o, SB, invM, gm, f, t, sC, sMean, sRow, sBadDom, a, old);
     PROF_MARK();
     if (!factor_and_invert(a, w, GS, t, sp)) { sBad = 1; sBadDom = 1; }
     PROF_MARK();
@@ -325,15 +362,7 @@ __global__ void __launch_bounds__(256) fwd_factor_kernel(const float* __restrict
             make_float4(w[r][0], w[r][1], w[r][2], w[r][3]);
     }
     __syncthreads();                                  // sC complete, sBadDom final
-    if (ema && !sBadDom) {                            // a non-PD batch covariance never reaches the running buffers
-      const float m = f.momentum, k = 1.f - f.momentum;
-#pragma unroll
-      for (int n = 0; n < kEmaPer; ++n) {
-        const int e = threadIdx.x + 256 * n;
-        if (e < GS * GS) f.rcov[d][(size_t)g * GS * GS + e] = m * (sC[(e / GS) * LDS + e % GS] * f.unbias) + k * rc_old[n];
-      }
-      if ((int)threadIdx.x < GS) f.rmean[d][g * GS + threadIdx.x] = m * sMean[threadIdx.x] + k * rm_old;
-    }
+    if (old.on && !sBadDom) domain_ema(d, g, gm, f, sC, sMean, old);   // a non-PD batch covariance never reaches the running buffers
     __syncthreads();      // also orders this domain's buffer writes before the next domain's reads (aliasing)
     PROF_MARK();
   }
@@ -442,6 +471,293 @@ __global__ void __launch_bounds__(256) bwd_coef_kernel(const float* __restrict__
 }
 
 // ------------------------------------------------------------------------------------------
+// ZCA basis (dwt_whiten_zca_*): W = S^-1/2 by T steps of the Newton-Schulz iteration instead of W = L^-1
+//   t = tr S,  N = S / t,  P_0 = I,  P_k = (3 P_{k-1} - P_{k-1}^3 N) / 2  (k = 1..T),  W = P_T / sqrt(t)
+// W is NOT symmetrised: it is P_T / sqrt(t) as computed, symmetric in exact arithmetic only, and both apply kernels use
+// exactly the saved W (A1 = W^T in full).  save_p [D][G][T][GS*GS]: slot 0 holds S, slot k holds P_k (k = 1..T-1).
+// ------------------------------------------------------------------------------------------
+// this thread's 4 x 4 block to a dense GS x GS matrix in global memory
+__device__ __forceinline__ void store_block_global(float* M, int GS, const Blk& t, const float (&c)[4][4]) {
+  if (!t.act) return;
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+    *reinterpret_cast<float4*>(M + (size_t)(4 * t.bi + r) * GS + 4 * t.bj) = make_float4(c[r][0], c[r][1], c[r][2], c[r][3]);
+}
+
+__device__ __forceinline__ void load_block(const float* M, const Blk& t, float (&c)[4][4]) {
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+#pragma unroll
+    for (int s = 0; s < 4; ++s) c[r][s] = t.act ? M[(4 * t.bi + r) * LDS + 4 * t.bj + s] : 0.f;
+}
+
+// tr M of a shared matrix, in one fixed order (fwd_zca and bwd_zca form the same t from the same S); ends with a barrier
+__device__ __forceinline__ float trace_of(const float* M, int GS, float* sRed) {
+  if (threadIdx.x < 32) {
+    const int l = threadIdx.x;
+    float v = (l < GS ? M[l * LDS + l] : 0.f) + (l + 32 < GS ? M[(l + 32) * LDS + l + 32] : 0.f);
+    v = warp_sum(v);
+    if (l == 0) sRed[0] = v;
+  }
+  __syncthreads();
+  return sRed[0];
+}
+
+// sum of v over the CTA in one fixed order (warps, then the 8 warp totals); every thread gets it.  Two barriers.
+__device__ __forceinline__ float block_sum(float v, float* sRed) {
+  v = warp_sum(v);
+  if ((threadIdx.x & 31) == 0) sRed[threadIdx.x >> 5] = v;
+  __syncthreads();
+  float s = 0.f;
+#pragma unroll
+  for (int w = 0; w < 8; ++w) s += sRed[w];
+  __syncthreads();
+  return s;
+}
+
+// fwd_zca: grid (G), 256 threads, domains in order with fwd_factor's statistics prologue and EMA tail.  Three products
+// per iteration (P P, (P P) P, (P P P) N) on shared-memory operands; each thread keeps its block of P in registers.
+// A non-finite or non-positive t, or a non-finite W, flags the domain as a non-positive pivot does in fwd_factor
+// (DWT_STATUS_NOT_PD, no EMA).  An indefinite S whose iteration stays finite is not detected: batch statistics are
+// positive semi-definite and shrunk, so only running buffers a user supplied (eval) can be indefinite.
+__global__ void __launch_bounds__(256) fwd_zca_kernel(const float* __restrict__ gram, const float* __restrict__ shift,
+                                                      const Geom gm, const FwdFin f, int T, float* __restrict__ save_p) {
+  extern __shared__ __align__(16) float dsm[];
+  float* sN = dsm;                 // S, then N = S / t
+  float* sP = sN + kMat;
+  float* sT1 = sP + kMat;          // P P
+  float* sT2 = sT1 + kMat;         // P P P
+  __shared__ float sC[kMat];       // un-shrunk covariance (for the EMA)
+  __shared__ float sMean[kSB], sRow[kSB], sRed[1];
+  __shared__ int sBad, sBadDom;
+  const int g = blockIdx.x, GS = gm.GS, nb = kSB / GS, sb = g / nb, o = (g % nb) * GS;
+  const Blk t(GS);
+  const int SB = (gm.C + kSB - 1) / kSB;
+  const float invM = 1.f / gm.M;
+  if (threadIdx.x == 0) sBad = 0;
+  PROF_DECL;
+  PROF_MARK();
+  for (int d = 0; d < gm.D; ++d) {
+    const float* G = gram ? gram + ((size_t)d * SB + sb) * kNacc : nullptr;
+    const size_t gbase = ((size_t)d * gm.G + g) * GS * GS;
+    float* pd = save_p + gbase * T;
+    float a[4][4], p[4][4], c[4][4];
+    EmaOld old;
+    domain_stats(G, shift, d, g, sb, o, SB, invM, gm, f, t, sC, sMean, sRow, sBadDom, a, old);
+    store_block(sN, t, a);
+    store_block_global(pd, GS, t, a);                 // slot 0: S
+    __syncthreads();
+    const float tr = trace_of(sN, GS, sRed);
+    if (threadIdx.x == 0 && !(tr > 0.f && tr < INFINITY)) { sBad = 1; sBadDom = 1; }
+#pragma unroll
+    for (int r = 0; r < 4; ++r)
+#pragma unroll
+      for (int s = 0; s < 4; ++s) {
+        a[r][s] = a[r][s] / tr;
+        p[r][s] = (t.act && t.bi == t.bj && r == s) ? 1.f : 0.f;
+      }
+    store_block(sN, t, a);                            // own block: every read of S was before trace_of's barrier
+    store_block(sP, t, p);
+    __syncthreads();
+    PROF_MARK();
+    for (int k = 1; k <= T; ++k) {
+      mm_block<false, false>(sP, sP, GS, t, c);
+      store_block(sT1, t, c);
+      __syncthreads();
+      mm_block<false, false>(sT1, sP, GS, t, c);
+      store_block(sT2, t, c);
+      __syncthreads();
+      mm_block<false, false>(sT2, sN, GS, t, c);      // nothing reads sP in this phase: P_k replaces P_{k-1} in place
+#pragma unroll
+      for (int r = 0; r < 4; ++r)
+#pragma unroll
+        for (int s = 0; s < 4; ++s) p[r][s] = 0.5f * (3.f * p[r][s] - c[r][s]);
+      if (k < T) {
+        store_block(sP, t, p);
+        store_block_global(pd + (size_t)k * GS * GS, GS, t, p);
+      }
+      __syncthreads();
+    }
+    PROF_MARK();
+    const float rs = 1.f / sqrtf(tr);
+    bool finite = true;
+#pragma unroll
+    for (int r = 0; r < 4; ++r)
+#pragma unroll
+      for (int s = 0; s < 4; ++s) {
+        p[r][s] *= rs;
+        finite = finite && isfinite(p[r][s]);
+      }
+    store_block_global(f.save_w + gbase, GS, t, p);
+    if (!finite) { sBad = 1; sBadDom = 1; }
+    __syncthreads();                                  // sC complete, sBadDom final
+    if (old.on && !sBadDom) domain_ema(d, g, gm, f, sC, sMean, old);
+    __syncthreads();      // also orders this domain's buffer writes before the next domain's reads (aliasing)
+    PROF_MARK();
+  }
+  PROF_DUMP("fwd_zca load|iterate|save+ema");
+  if (threadIdx.x == 0 && sBad) atomicOr(f.status, DWT_STATUS_NOT_PD);
+}
+
+// bwd_zca: grid (G, 1, D), 256 threads.  The reverse of fwd_zca's recursion from dL/dW = R = sum dy xc^T:
+//   Q_T = R / sqrt(t),  tbar = -<R, P_T> t^-3/2 / 2 = -<R, W> / (2 t),  Nbar = 0
+//   k = T..1, P = P_{k-1}:  Nbar -= P^3 Q_k / 2,  Q_{k-1} = 3 Q_k / 2 - (Q_k N P^2 + P Q_k N P + P^2 Q_k N) / 2
+//   G = dL/dS = Nbar / t + (tbar - <Nbar, N> / t) I,   Bm = (a/M)(G + G^T),   A1 = W^T (full),   cvec
+// Step k = 1 has P_0 = I: Nbar -= Q_1 / 2, and Q_0 is not needed.  Steps k >= 2 run eight products in three phases.
+// coef[d][g] = A1 | Bm | cvec where tc_bwd_apply reads them; eval (rgram null): A1 = W^T, Bm = 0.
+__global__ void __launch_bounds__(256) bwd_zca_kernel(const float* __restrict__ rgram, const Geom gm, const BwdFin f, int T,
+                                                      const float* __restrict__ save_p, float* __restrict__ dybar) {
+  extern __shared__ __align__(16) float dsm[];
+  float* sW = dsm;
+  float* sN = sW + kMat;           // S, then N = S / t
+  float* sQ = sN + kMat;           // R, then Q_k
+  float* sP = sQ + kMat;           // P_{k-1}
+  float* sPP = sP + kMat;          // P^2; at the end Bm
+  float* sQN = sPP + kMat;         // Q N
+  float* sP3 = sQN + kMat;         // P^3
+  float* sT = sP3 + kMat;          // P Q N; at the end G
+  __shared__ float sSdz[kSB], sMu[kSB], sRed[8];
+  const int g = blockIdx.x, d = blockIdx.z, GS = gm.GS, nb = kSB / GS, sb = g / nb, o = (g % nb) * GS;
+  const Blk t(GS);
+  const int SB = (gm.C + kSB - 1) / kSB;
+  const bool train = f.mode == DWT_MODE_TRAIN && rgram != nullptr;
+  const float* G = train ? rgram + ((size_t)d * SB + sb) * kNacc : nullptr;
+  const size_t gbase = ((size_t)d * gm.G + g) * GS * GS;
+  const float* pd = save_p + gbase * T;
+  float* coef = f.coef + ((size_t)d * gm.G + g) * coef_stride(GS);
+  const int gsh = __ffs(GS) - 1;
+  const float invM = 1.f / gm.M;
+  constexpr int kPer = kSB * kSB / 256;
+  PROF_DECL;
+  PROF_MARK();
+  float wv[kPer], rv[kPer], sv[kPer];
+#pragma unroll
+  for (int n = 0; n < kPer; ++n) {
+    const int e = threadIdx.x + 256 * n, i = e >> gsh, j = e & (GS - 1);
+    const bool in = e < GS * GS;
+    wv[n] = in ? f.save_w[gbase + e] : 0.f;
+    rv[n] = (in && train) ? __ldcg(G + (o + i) * kSB + o + j) : 0.f;
+    sv[n] = (in && train) ? pd[e] : 0.f;
+  }
+  float sdz = 0.f, mu = 0.f;
+  if ((int)threadIdx.x < GS) {
+    sdz = train ? __ldcg(G + kSB * kSB + o + threadIdx.x) : 0.f;
+    mu = f.save_mean[(size_t)d * gm.C + g * GS + threadIdx.x];
+  }
+  float rw = 0.f;                                     // this thread's share of <R, W>
+#pragma unroll
+  for (int n = 0; n < kPer; ++n) {
+    const int e = threadIdx.x + 256 * n, i = e >> gsh, j = e & (GS - 1);
+    if (e < GS * GS) { sW[i * LDS + j] = wv[n]; sQ[i * LDS + j] = rv[n]; sN[i * LDS + j] = sv[n]; }
+    rw = fmaf(rv[n], wv[n], rw);
+  }
+  if ((int)threadIdx.x < GS) {
+    sSdz[threadIdx.x] = sdz * invM;                   // mean_M dy (0 in eval mode)
+    sMu[threadIdx.x] = mu;
+    if (dybar) dybar[((size_t)d * SB + sb) * kSB + o + threadIdx.x] = sdz * invM;
+  }
+  __syncthreads();
+  PROF_MARK();
+  if (train) {
+    const float tr = trace_of(sN, GS, sRed);          // fwd_zca's t, bit for bit
+    const float rs = 1.f / sqrtf(tr);
+    const float tbar = -0.5f * block_sum(rw, sRed) / tr;
+    float q[4][4], nbar[4][4], c[4][4], acc[4][4];
+    load_block(sN, t, c);
+    load_block(sQ, t, q);
+#pragma unroll
+    for (int r = 0; r < 4; ++r)
+#pragma unroll
+      for (int s = 0; s < 4; ++s) {
+        c[r][s] = c[r][s] / tr;
+        q[r][s] *= rs;
+        nbar[r][s] = 0.f;
+      }
+    store_block(sN, t, c);                            // own blocks only
+    store_block(sQ, t, q);
+    for (int k = T; k >= 2; --k) {
+      const float* pk = pd + (size_t)(k - 1) * GS * GS;
+#pragma unroll
+      for (int n = 0; n < kPer; ++n) {
+        const int e = threadIdx.x + 256 * n;
+        if (e < GS * GS) sP[(e >> gsh) * LDS + (e & (GS - 1))] = pk[e];
+      }
+      __syncthreads();
+      mm_block<false, false>(sP, sP, GS, t, c);       // P^2
+      store_block(sPP, t, c);
+      mm_block<false, false>(sQ, sN, GS, t, c);       // Q N
+      store_block(sQN, t, c);
+      __syncthreads();
+      mm_block<false, false>(sPP, sP, GS, t, c);      // P^3
+      store_block(sP3, t, c);
+      mm_block<false, false>(sP, sQN, GS, t, c);      // P Q N
+      store_block(sT, t, c);
+      mm_block<false, false>(sQN, sPP, GS, t, acc);   // Q N P^2
+      mm_block<false, false>(sPP, sQN, GS, t, c);     // P^2 Q N
+#pragma unroll
+      for (int r = 0; r < 4; ++r)
+#pragma unroll
+        for (int s = 0; s < 4; ++s) acc[r][s] += c[r][s];
+      __syncthreads();
+      mm_block<false, false>(sP3, sQ, GS, t, c);      // P^3 Q
+#pragma unroll
+      for (int r = 0; r < 4; ++r)
+#pragma unroll
+        for (int s = 0; s < 4; ++s) nbar[r][s] = fmaf(-0.5f, c[r][s], nbar[r][s]);
+      mm_block<false, false>(sT, sP, GS, t, c);       // P Q N P
+#pragma unroll
+      for (int r = 0; r < 4; ++r)
+#pragma unroll
+        for (int s = 0; s < 4; ++s) q[r][s] = 1.5f * q[r][s] - 0.5f * (acc[r][s] + c[r][s]);
+      __syncthreads();                                // every read of sQ and sP of this step is done
+      store_block(sQ, t, q);
+    }
+    // k = 1 (P_0 = I), then G = Nbar / t + (tbar - <Nbar, N> / t) I
+    float nn = 0.f;
+#pragma unroll
+    for (int r = 0; r < 4; ++r)
+#pragma unroll
+      for (int s = 0; s < 4; ++s) {
+        nbar[r][s] = fmaf(-0.5f, q[r][s], nbar[r][s]);
+        if (t.act) nn = fmaf(nbar[r][s], sN[(4 * t.bi + r) * LDS + 4 * t.bj + s], nn);
+      }
+    const float diag = tbar - block_sum(nn, sRed) / tr;
+#pragma unroll
+    for (int r = 0; r < 4; ++r)
+#pragma unroll
+      for (int s = 0; s < 4; ++s) c[r][s] = nbar[r][s] / tr + ((t.bi == t.bj && r == s) ? diag : 0.f);
+    store_block(sT, t, c);
+    __syncthreads();
+  }
+  PROF_MARK();
+  const float sc = f.a * invM;
+#pragma unroll
+  for (int n = 0; n < kPer; ++n) {
+    const int e = threadIdx.x + 256 * n, i = e >> gsh, j = e & (GS - 1);
+    if (e < GS * GS) {
+      const float bm = train ? sc * (sT[i * LDS + j] + sT[j * LDS + i]) : 0.f;
+      coef[e] = sW[j * LDS + i];                      // A1 = W^T, every element
+      coef[GS * GS + e] = bm;
+      sPP[i * LDS + j] = bm;
+    }
+  }
+  __syncthreads();
+  // cvec_i = -(sum_j W_ji mean(dy)_j + sum_j Bm_ij mu_j): 4 threads per row, partial sums met by shuffle
+  {
+    const int i = threadIdx.x >> 2, q = threadIdx.x & 3;
+    float cv = 0.f;
+    if (train && i < GS) {
+      for (int j = q; j < GS; j += 4) cv = fmaf(sW[j * LDS + i], sSdz[j], fmaf(sPP[i * LDS + j], sMu[j], cv));
+    }
+    cv += __shfl_xor_sync(0xffffffffu, cv, 1);
+    cv += __shfl_xor_sync(0xffffffffu, cv, 2);
+    if (q == 0 && i < GS) coef[2 * GS * GS + i] = -cv;
+  }
+  PROF_MARK();
+  PROF_DUMP("bwd_zca load|iterate|tail");
+}
+
+// ------------------------------------------------------------------------------------------
 // group size 128: one 1024-thread CTA per group runs the shared-memory routines of dwt_common.cuh (fwd_factor_block:
 // right-looking Cholesky + forward-substitution inverse; bwd_finalize_block: P, T = W^T P, S' = T W, A1, Bm) on the
 // whole 128 x 128 matrix, assembled from the 64 x 64 blocks the tensor-core contractions reduced.  Three matrices of
@@ -537,6 +853,8 @@ __global__ void __launch_bounds__(kThreads2) bwd_coef128_kernel(const float* __r
 
 constexpr size_t kFactorSmem = 0;   // fwd_factor: static shared memory only (panel buffers + covariance)
 constexpr size_t kCoefSmem = sizeof(float) * 4 * kMat;
+constexpr size_t kZcaFwdSmem = sizeof(float) * 4 * kMat;   // N, P, P^2, P^3 (66.6 KB; + 16.9 KB static)
+constexpr size_t kZcaBwdSmem = sizeof(float) * 8 * kMat;   // W, N, Q, P, P^2, Q N, P^3, P Q N (133 KB)
 
 }  // namespace
 
@@ -545,6 +863,8 @@ int dense_init() {
   if (e == cudaSuccess) e = cudaFuncSetAttribute(bwd_coef_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kCoefSmem);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(fwd_factor128_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFactor2Smem);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(bwd_coef128_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kCoef2Smem);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(fwd_zca_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kZcaFwdSmem);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(bwd_zca_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kZcaBwdSmem);
   return (int)e;
 }
 
@@ -571,6 +891,16 @@ void dense_bwd_coef(const float* rgram, const Geom& gm, const BwdFin& fin, float
     return;
   }
   bwd_coef_kernel<<<dim3(gm.G, 1, gm.D), 256, kCoefSmem, st>>>(rgram, gm, fin, dybar);
+}
+
+void dense_fwd_zca(const float* gram, const float* shift, const Geom& gm, const FwdFin& fin, int iters, float* save_p,
+                   cudaStream_t st) {
+  fwd_zca_kernel<<<gm.G, 256, kZcaFwdSmem, st>>>(gram, shift, gm, fin, iters, save_p);
+}
+
+void dense_bwd_zca(const float* rgram, const Geom& gm, const BwdFin& fin, int iters, const float* save_p, float* dybar,
+                   cudaStream_t st) {
+  bwd_zca_kernel<<<dim3(gm.G, 1, gm.D), 256, kZcaBwdSmem, st>>>(rgram, gm, fin, iters, save_p, dybar);
 }
 
 }  // namespace dwt

@@ -63,6 +63,12 @@ int dense_init();
 void dense_partial_reduce(const float* partial, int nchunks, int problems, float* gram, cudaStream_t st);
 void dense_fwd_factor(const float* gram, const float* shift, const Geom& gm, const FwdFin& fin, cudaStream_t st);
 void dense_bwd_coef(const float* rgram, const Geom& gm, const BwdFin& fin, float* dybar, cudaStream_t st);
+// ZCA basis, group sizes 8..64: W = S^-1/2 by `iters` Newton-Schulz steps.  save_p [D][G][iters][GS*GS] (S, P_1..P_{iters-1})
+// is written by the forward and read by the backward; both leave what dense_fwd_factor / dense_bwd_coef leave.
+void dense_fwd_zca(const float* gram, const float* shift, const Geom& gm, const FwdFin& fin, int iters, float* save_p,
+                   cudaStream_t st);
+void dense_bwd_zca(const float* rgram, const Geom& gm, const BwdFin& fin, int iters, const float* save_p, float* dybar,
+                   cudaStream_t st);
 
 // TMA + wgmma apply path (norm_tc_apply.cu): split-TF32 GEMM of the block-diagonal group matrices
 int tc_apply_init();

@@ -96,12 +96,14 @@ class _NormFunction(torch.autograd.Function):
     """Shared by whitening (kind='whiten') and domain batch norm (kind='bn').
 
     x is [n_domains*N, C, *]; `running` is a list of n_domains (mean, second-moment) buffer pairs
-    (entries may alias); gamma/beta are [C]-sized or None; relu fuses max(.,0) behind the affine; r: route() of the call.
+    (entries may alias); gamma/beta are [C]-sized or None; relu fuses max(.,0) behind the affine; r: route() of the call;
+    iterations: 0 for the Cholesky basis, else the Newton-Schulz iterations of the ZCA basis (dwt_whiten_zca_*, whitening
+    without gamma/beta or residual; the per-group matrices of the iteration are saved for backward).
     """
 
     @staticmethod
     def forward(ctx, x, gamma, beta, residual, kind, group_size, n_domains, mode, eps, momentum, update_running,
-                running, relu, r):
+                running, relu, r, iterations):
         lib = nv.lib()
         gs = group_size if kind == "whiten" else 1
         if not r.nhwc and not x.is_contiguous():
@@ -119,6 +121,8 @@ class _NormFunction(torch.autograd.Function):
             _check_param(f"running second moment of domain {d}", rv_t, c * gs)
         _check_param("gamma / weight", gamma, c)
         _check_param("beta / bias", beta, c)
+        if iterations and (kind != "whiten" or gamma is not None or residual is not None):
+            raise nv.NativeError("the ZCA basis whitens without a fused gamma/beta/ReLU epilogue or residual")
         epi = nv.EPI_NONE
         if residual is not None:
             if gamma is None or not relu or residual.shape != x.shape:
@@ -135,12 +139,17 @@ class _NormFunction(torch.autograd.Function):
         mask = torch.empty(x.numel() // 4, dtype=torch.uint8, device=dev) if (residual is not None and r.nhwc) else None
         save_mean = torch.empty(n_domains, c, dtype=torch.float32, device=dev)
         save_w = torch.empty(n_domains, c // gs, gs, gs, dtype=torch.float32, device=dev)
+        save_p = torch.empty(n_domains, c // gs, iterations, gs, gs, dtype=torch.float32, device=dev) if iterations else None
         ws = nv.workspace(dev, n, c, hw, gs, n_domains)
         need_running = (mode == nv.MODE_EVAL) or update_running
         rm = nv.ptr_array([p[0] for p in running]) if need_running else None
         rv = nv.ptr_array([p[1] for p in running]) if need_running else None
         with torch.cuda.device(dev):
-            if kind == "whiten":
+            if iterations:
+                rc = lib.dwt_whiten_zca_fwd(nv.ptr(x), nv.ptr(y), n, c, hw, gs, n_domains, mode | layout, eps, momentum,
+                                            int(update_running), rm, rv, int(iterations), nv.ptr(save_mean), nv.ptr(save_w),
+                                            nv.ptr(save_p), nv.ptr(ws), ws.numel(), nv.stream_ptr(dev))
+            elif kind == "whiten":
                 rc = lib.dwt_whiten_fwd(nv.ptr(x), nv.ptr(y), n, c, hw, gs, n_domains, mode | layout, eps, momentum,
                                         int(update_running), rm, rv, nv.ptr(gamma_c), nv.ptr(beta_c), nv.ptr(residual),
                                         nv.ptr(mask), epi, nv.ptr(save_mean), nv.ptr(save_w), nv.ptr(ws), ws.numel(),
@@ -172,8 +181,11 @@ class _NormFunction(torch.autograd.Function):
             ctx.save_for_backward(x, save_mean, save_w, gamma_c, beta_c, y)
             epi = nv.EPI_AFFINE
             ctx.residual_mode = "aten"
+        elif iterations:
+            ctx.save_for_backward(x, save_mean, save_w, gamma_c, beta_c, save_p)
         else:
             ctx.save_for_backward(x, save_mean, save_w, gamma_c, beta_c)
+        ctx.iterations = iterations
         ctx.cfg = (kind, gs, n_domains, mode | layout, eps, epi, n, c, hw, None if gamma is None else gamma.shape)
         ctx.route = r
         return y
@@ -181,8 +193,10 @@ class _NormFunction(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dout):
         lib = nv.lib()
-        mask = None
-        if ctx.residual_mode == "mask":
+        mask = save_p = None
+        if ctx.iterations:
+            x, save_mean, save_w, gamma_c, beta_c, save_p = ctx.saved_tensors
+        elif ctx.residual_mode == "mask":
             x, save_mean, save_w, gamma_c, beta_c, mask = ctx.saved_tensors
         elif ctx.residual_mode == "aten":
             x, save_mean, save_w, gamma_c, beta_c, out = ctx.saved_tensors
@@ -217,7 +231,11 @@ class _NormFunction(torch.autograd.Function):
         dbeta = torch.empty(c, dtype=torch.float32, device=dev) if want_affine else None
         ws = nv.workspace(dev, n, c, hw, gs, n_domains)
         with torch.cuda.device(dev):
-            if kind == "whiten":
+            if ctx.iterations:
+                rc = lib.dwt_whiten_zca_bwd(nv.ptr(x), nv.ptr(dout), nv.ptr(dx), n, c, hw, gs, n_domains, mode, eps,
+                                            int(ctx.iterations), nv.ptr(save_mean), nv.ptr(save_w), nv.ptr(save_p),
+                                            nv.ptr(ws), ws.numel(), nv.stream_ptr(dev))
+            elif kind == "whiten":
                 rc = lib.dwt_whiten_bwd(nv.ptr(x), nv.ptr(dout), nv.ptr(dout2), nv.ptr(dx), n, c, hw, gs, n_domains, mode, eps,
                                         nv.ptr(save_mean), nv.ptr(save_w), nv.ptr(gamma_c), nv.ptr(beta_c), nv.ptr(mask),
                                         nv.ptr(d_res) if mask is not None else None, epi,
@@ -230,7 +248,7 @@ class _NormFunction(torch.autograd.Function):
         nv.check(rc)
         if want_affine:
             dgamma, dbeta = dgamma.view(gshape), dbeta.view(gshape)
-        return (dx, dgamma, dbeta, d_res if ctx.needs_input_grad[3] else None) + (None,) * 10
+        return (dx, dgamma, dbeta, d_res if ctx.needs_input_grad[3] else None) + (None,) * 11
 
 
 class _TailPairFunction(torch.autograd.Function):
@@ -367,7 +385,11 @@ _ACT_DTYPES = (torch.float32, torch.bfloat16)
 
 
 def norm(x, gamma, beta, *, kind, group_size, n_domains, training_stats, eps, momentum, update_running,
-         running, relu=False, residual=None):
+         running, relu=False, residual=None, iterations=0):
+    """iterations: 0 whitens in the Cholesky basis; 1..16 in the ZCA basis by that many Newton-Schulz iterations (the
+    tensor-core kernels only: a call they cannot take raises NativeError, it is never sent to another family)."""
+    if iterations and not 1 <= iterations <= nv.ZCA_MAX_ITERATIONS:
+        raise ValueError(f"iterations must be in [1, {nv.ZCA_MAX_ITERATIONS}] (got {iterations})")
     mode = nv.MODE_TRAIN if training_stats else nv.MODE_EVAL
     args = (kind, group_size, n_domains, mode, float(eps), float(momentum), bool(update_running), running, bool(relu))
     r = route(x, residual, kind, group_size, n_domains)
@@ -376,9 +398,9 @@ def norm(x, gamma, beta, *, kind, group_size, n_domains, training_stats, eps, mo
         # view, ...) or mixed dtypes: the float32 kernels on upcast copies (x.float() keeps channels-last strides), the
         # result (and through autograd every gradient of x and the residual) back in x's dtype
         xf, rf = x.float(), None if residual is None else residual.float()
-        y = _NormFunction.apply(xf, gamma, beta, rf, *args, route(xf, rf, kind, group_size, n_domains))
+        y = _NormFunction.apply(xf, gamma, beta, rf, *args, route(xf, rf, kind, group_size, n_domains), iterations)
         return y.to(x.dtype)
-    return _NormFunction.apply(x, gamma, beta, residual, *args, r)
+    return _NormFunction.apply(x, gamma, beta, residual, *args, r, iterations)
 
 
 class _MecFunction(torch.autograd.Function):

@@ -11,7 +11,9 @@ target-aug in order so aliased buffers end exactly as after three sequential mod
 (SURVEY.md H5).  Backward is likewise two tensor-sized launches and also yields dgamma/dbeta and,
 for the residual tail, the gradient of the identity branch.
 
-It owns no state: it borrows the running buffers of the three domain modules at call time.
+It owns no state: it borrows the running buffers of the three domain modules at call time, and with them their
+hyper-parameters -- eps, momentum and, for whitening, the basis: three ``ZCAWTransform2d`` modules make a ZCA site
+(the tensor-core kernels, no fused epilogue), and modules that disagree on the basis are refused.
 
 ``replicated=True`` is the statistics-collection pass (SURVEY.md §8f-3;
 resnet50_dwt_mec_officehome.py:380-389): the reference feeds ``cat((data, data, data))`` through
@@ -29,7 +31,9 @@ from __future__ import annotations
 import torch
 import torch.nn as nn
 
+from . import _native as nv
 from . import functional as F
+from .whitening import _Whitening
 
 
 class DomainTripleNorm(nn.Module):
@@ -66,16 +70,32 @@ class DomainTripleNorm(nn.Module):
             return out.to(x.dtype)
         if replicated:
             return self._forward_replicated(x, mods, gamma, beta, relu, residual, count_batches)
+        iterations = self._iterations(mods)
         running, eps, momentum, update = self._running_args(mods, count_batches)
         # modules in eval mode normalise with their running statistics, as each module called on its domain would
         batch_stats = mods[0].training or not mods[0].track_running_stats
         if not self.kernel_epilogue:
             y = F.norm(x, None, None, kind=self.kind, group_size=self.group_size, n_domains=self.n_domains,
-                       training_stats=batch_stats, eps=eps, momentum=momentum, update_running=update, running=running)
+                       training_stats=batch_stats, eps=eps, momentum=momentum, update_running=update, running=running,
+                       iterations=iterations)
             return self._tensor_epilogue(y, gamma, beta, relu, residual)
         return F.norm(x, gamma, beta, kind=self.kind, group_size=self.group_size, n_domains=self.n_domains,
                       training_stats=batch_stats, eps=eps, momentum=momentum, update_running=update,
                       running=running, relu=relu, residual=residual)
+
+    def _iterations(self, mods):
+        """The whitening basis the domain modules share (functional.norm's iterations: 0 = Cholesky)."""
+        if self.kind != "whiten":
+            return 0
+        basis = {m._iterations() if isinstance(m, _Whitening) else 0 for m in mods}
+        if len(basis) != 1:
+            raise ValueError("the domain modules of a whitening site must share one basis (WTransform2d, or "
+                             f"ZCAWTransform2d with one number of iterations); got iterations {sorted(basis)}")
+        iterations = basis.pop()
+        if iterations and self.kernel_epilogue:
+            raise nv.NativeError("the ZCA basis runs on the tensor-core kernels: group_size 8, 16, 32, 64 "
+                                 f"(got {self.group_size})")
+        return iterations
 
     def _running_args(self, mods, count_batches):
         """-> (running buffer pairs, eps, momentum, update_running) of a call on mods (statistics of the batch when
@@ -104,7 +124,9 @@ class DomainTripleNorm(nn.Module):
         gradients and running buffers are the same either way -- in bfloat16 too: the two-site kernels round the
         identity to bf16 before they add it, as the composition stores it."""
         mods, down_mods = list(domain_modules), list(down_modules)
-        pair = (self.kernel_epilogue and down.kernel_epilogue and self.kind == down.kind
+        self._iterations(mods)              # a ZCA basis the fused-epilogue kernels lack is refused, never run as Cholesky
+        down._iterations(down_mods)
+        pair =(self.kernel_epilogue and down.kernel_epilogue and self.kind == down.kind
                 and self.group_size == down.group_size and self.n_domains == down.n_domains
                 and len(mods) == len(down_mods) == self.n_domains and x.dim() == 4 and x.shape == xd.shape
                 and mods[0].training and down_mods[0].training
@@ -153,7 +175,9 @@ class DomainTripleNorm(nn.Module):
         if len(means) != len(keep) or len(seconds) != len(keep):
             raise ValueError("replicated statistics need each running_mean paired with one second-moment buffer")
         m0 = mods[0]
-        common = dict(kind=self.kind, group_size=self.group_size, n_domains=1, training_stats=True, eps=m0.eps)
+        iterations = self._iterations(mods)
+        common = dict(kind=self.kind, group_size=self.group_size, n_domains=1, training_stats=True, eps=m0.eps,
+                      iterations=iterations)
         if self.kernel_epilogue:
             common.update(relu=relu, residual=residual)
             g_arg, b_arg = gamma, beta

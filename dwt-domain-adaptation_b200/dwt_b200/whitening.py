@@ -46,6 +46,11 @@ class _Whitening(nn.Module):
     def _check_group_size(self):
         raise NotImplementedError
 
+    def _iterations(self):
+        """Newton-Schulz iterations of the whitening basis: 0 is the inverse Cholesky factor (the ZCA layer, zca.py,
+        returns its own)."""
+        return 0
+
     def forward(self, x):
         self._check_input_dim(x)
         self._check_group_size()
@@ -55,7 +60,7 @@ class _Whitening(nn.Module):
         return F.norm(x, None, None, kind="whiten", group_size=self.group_size, n_domains=1,
                       training_stats=self.training or not tracking, eps=self.eps, momentum=self.momentum,
                       update_running=self.training and tracking,
-                      running=[(self.running_mean, self.running_variance)])
+                      running=[(self.running_mean, self.running_variance)], iterations=self._iterations())
 
 
 class WTransform2d(_Whitening):

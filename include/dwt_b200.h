@@ -17,6 +17,7 @@
  *                    (+ the caller's shared gamma/beta/ReLU epilogue,
  *                     resnet50_dwt_mec_officehome.py:59-63,220-222, when asked)
  *   dwt_whiten_bwd   autograd through the above     utils/whitening.py:41-55
+ *   dwt_whiten_zca_fwd/bwd  the same layer in the ZCA basis (Newton-Schulz iteration; not in the reference)
  *   dwt_bn_fwd/bwd   _BatchNorm.forward             utils/batch_norm.py:54-69
  *   dwt_tail2_fwd/bwd  the residual tail of a downsampling Bottleneck: two norm sites and the ReLU in one pass
  *                    resnet50_dwt_mec_officehome.py:236-240
@@ -172,6 +173,39 @@ DWT_API int dwt_whiten_bwd(const float *x, const float *dout, const float *dout2
                    const float *save_w, const float *gamma, const float *beta, const uint8_t *relu_mask,
                    float *dresidual, int epilogue, float *dgamma, float *dbeta, void *workspace,
                    size_t workspace_bytes, dwt_stream_t stream);
+
+/*
+ * Whitening in the ZCA basis (decorrelated batch norm / IterNorm): W = S^-1/2 by Newton-Schulz iteration instead of
+ * the inverse Cholesky factor of dwt_whiten_fwd.  Per domain and group, with S = (1-eps) cov + eps I (the statistics,
+ * pilot shift and shrinkage of dwt_whiten_fwd):
+ *   t = tr S,  N = S / t,  P_0 = I,  P_k = (3 P_{k-1} - P_{k-1}^3 N) / 2  (k = 1..iterations),  W = P_T / sqrt(t),
+ *   y = W (x - mean).
+ * At a finite T this is IterNorm's partial whitening (W -> S^-1/2 as T grows), and dwt_whiten_zca_bwd differentiates
+ * that function, not the limit.  W is not symmetrised: save_w holds P_T / sqrt(t) as computed.
+ *   iterations  T, 1..DWT_ZCA_MAX_ITERATIONS (else DWT_E_INVALID)
+ *   save_p      [n_domains, C/gs, iterations, gs, gs], 16-byte aligned (else DWT_E_INVALID): slot 0 holds S, slot k
+ *               holds P_k (k = 1..T-1); written by fwd, read by bwd
+ *   everything else as dwt_whiten_fwd / dwt_whiten_bwd with epilogue 0 and no dout2.
+ * Running buffers get the EMA of the un-shrunk covariance, in domain order: after a training call they and save_mean
+ * equal dwt_whiten_fwd's bit for bit, so running buffers are interchangeable between the two bases.  mode takes
+ * DWT_MODE_*, DWT_LAYOUT_NHWC and DWT_DTYPE_BF16.
+ * Built for the tensor-core kernels only: group size 8, 16, 32, 64, HW >= 32 and HW % 4 == 0, N*HW >= 4096 per domain,
+ * NCHW bf16 also HW % 8 == 0, tensors aligned as for dwt_whiten_fwd.  Every other group size (1, 2, 4, 128), every
+ * other geometry, and a call whose tensor-core kernels could not be set up is DWT_E_UNSUPPORTED.
+ * Status: a non-finite or non-positive tr S, or a non-finite W, sets DWT_STATUS_NOT_PD and skips that domain's EMA.  An
+ * indefinite S whose iteration stays finite is NOT detected (batch statistics cannot be indefinite; running buffers a
+ * caller supplies for eval can).
+ * Profile families dense_fwd_zca / dense_bwd_zca (_bf16) for the per-group algebra; the other passes keep tc_*.  The
+ * workspace is sized by dwt_workspace_bytes as for dwt_whiten_fwd.
+ */
+#define DWT_ZCA_MAX_ITERATIONS 16
+DWT_API int dwt_whiten_zca_fwd(const float *x, float *y, int64_t N, int64_t C, int64_t HW, int group_size, int n_domains,
+                       int mode, float eps, float momentum, int update_running, float *const *running_mean,
+                       float *const *running_cov, int iterations, float *save_mean, float *save_w, float *save_p,
+                       void *workspace, size_t workspace_bytes, dwt_stream_t stream);
+DWT_API int dwt_whiten_zca_bwd(const float *x, const float *dout, float *dx, int64_t N, int64_t C, int64_t HW, int group_size,
+                       int n_domains, int mode, float eps, int iterations, const float *save_mean, const float *save_w,
+                       const float *save_p, void *workspace, size_t workspace_bytes, dwt_stream_t stream);
 
 /*
  * Domain batch norm (F.batch_norm semantics): biased batch variance normalises,
