@@ -16,7 +16,10 @@
 // of at most ceil(k/s)^2 gradients it is the fp32 sum rounded once.
 //
 // Semantics = torch.nn.functional.max_pool2d(x, k, s, p) (dilation 1, ceil_mode False) and its autograd, bit for bit
-// including the tie rule (post-ReLU windows of all zeros are common: the gradient goes to the first element).
+// including the tie rule (post-ReLU windows of all zeros are common: the gradient goes to the first element).  The index
+// starts at the window's first IN-IMAGE position, (max(0, -h0), max(0, -w0)) for a window whose top-left corner is
+// (h0, w0): a window whose in-image elements are all -inf keeps it, and its gradient goes to that element as in ATen
+// (a start at the top-left corner would name padding there, and the backward would drop the window's gradient).
 #include <cuda_bf16.h>
 
 #include "dwt_common.cuh"
@@ -74,7 +77,8 @@ __global__ void __launch_bounds__(256) maxpool_fwd_kernel(const T* __restrict__ 
     const int ow = POW2 ? (t >> g.c4shift) : t / g.C4, c4 = t - ow * g.C4;
     const int w0 = ow * g.s - g.p;
     float best[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-    unsigned bi[4] = {0u, 0u, 0u, 0u};
+    const unsigned first = (unsigned)(max(0, -h0) * g.k + max(0, -w0));   // the first in-image position
+    unsigned bi[4] = {first, first, first, first};
 #pragma unroll
     for (int kh = 0; kh < g.k; ++kh) {
       const int h = h0 + kh;
@@ -159,13 +163,16 @@ __global__ void __launch_bounds__(256) maxpool_fwd_3s2_kernel(const T* __restric
   const V* xn = reinterpret_cast<const V*>(x) + (size_t)n * g.H * g.W * g.C4 + c4;
   float best[2][2][4];
   unsigned bi[2][2][4];
+  const int h0 = 4 * a - 1, w0 = 4 * b - 1;
 #pragma unroll
   for (int oa = 0; oa < 2; ++oa)
 #pragma unroll
-    for (int ob = 0; ob < 2; ++ob)
+    for (int ob = 0; ob < 2; ++ob) {
+      // window (oa, ob) starts at (h0 + 2 oa, w0 + 2 ob): its first in-image position, as in the generic kernel
+      const unsigned first = (unsigned)(max(0, -(h0 + 2 * oa)) * 3 + max(0, -(w0 + 2 * ob)));
 #pragma unroll
-      for (int c = 0; c < 4; ++c) { best[oa][ob][c] = -INFINITY; bi[oa][ob][c] = 0u; }
-  const int h0 = 4 * a - 1, w0 = 4 * b - 1;
+      for (int c = 0; c < 4; ++c) { best[oa][ob][c] = -INFINITY; bi[oa][ob][c] = first; }
+    }
 #pragma unroll
   for (int r = 0; r < 5; ++r) {
     const int h = h0 + r;

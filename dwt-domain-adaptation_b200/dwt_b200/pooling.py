@@ -4,8 +4,9 @@
 stride=2, padding=1)`` (resnet50_dwt_mec_officehome.py:295, applied right behind the stem whitening site at :337-338).
 Same results as the stock op bit for bit (ties, NaN, gradient routing); one byte of argmax per output element instead of
 an int64.  It takes dense ``torch.channels_last`` CUDA tensors with C % 4 == 0 only -- the layout the benchmark step runs
-in; anything else raises (build the model with ``nn.MaxPool2d`` for NCHW).  float32 or bfloat16 (autocast); the output
-and the gradient keep the input's dtype.
+in; anything else raises (build the model with ``nn.MaxPool2d`` for NCHW), and so does an input whose data_ptr() is not
+16-byte aligned (8 for bfloat16).  An incoming gradient at such an offset is copied instead: the caller of backward()
+cannot choose it.  float32 or bfloat16 (autocast); the output and the gradient keep the input's dtype.
 """
 from __future__ import annotations
 
@@ -40,6 +41,8 @@ class _MaxPoolFunction(torch.autograd.Function):
         (idx,) = ctx.saved_tensors
         n, c, h, w, k, s, p, dtype, flags = ctx.cfg
         dy = dy.to(dtype).contiguous(memory_format=torch.channels_last)
+        if dy.data_ptr() % (8 if flags else 16):     # a dense view at an odd offset: the kernels read whole channel quads
+            dy = dy.clone(memory_format=torch.channels_last)
         dev = nv.require_cuda(dy, bf16=True)
         dx = torch.empty((n, c, h, w), dtype=dtype, device=dev, memory_format=torch.channels_last)
         with torch.cuda.device(dev):

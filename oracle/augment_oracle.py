@@ -23,7 +23,10 @@ Third-party arithmetic restated (not under /root/reference; versions probed in t
     `hflip`, `crop`.
 
 Parity pin: tests/golden/augment.npz holds outputs of the unmodified reference functions + torchvision
-(tests/golden/make_golden_augment.py); tests/test_oracle_vs_golden.py requires BIT-EXACT agreement.
+(tests/golden/make_golden_augment.py); tests/test_oracle_vs_golden.py requires BIT-EXACT agreement.  The same holds
+for tests/golden/augment_edges.npz (translations, reflections, singular and zoom matrices, non-square sources, crops
+of 1 and of the whole source; tests/test_pool_augment_exact.py).  Crop corners must lie in [0, src - crop]: numpy
+slicing would shorten the crop, the GPU kernel clamps the corner, torchvision pads.
 """
 from __future__ import annotations
 
