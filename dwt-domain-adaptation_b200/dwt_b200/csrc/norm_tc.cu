@@ -26,16 +26,26 @@
 // comes out of two M=64 N=64 K=8 MMAs per 8 pixels: A = the hi tile (written back in place) or the lo tile (a
 // per-warpgroup buffer), B = the hi tile.  The row sums the mean needs are summed by the transform.
 //
-// bwd_reduce (tc_contract_kernel) -- single pass: R multiplies already-formed W's in the coefficient algebra and
-// its tf32 product errors are zero-mean over M >= 4096 samples (round-to-nearest operands).
+// bwd_reduce (tc_contract_kernel) -- SPLIT precision, dy CENTRED.  A single tf32 pass (RN_tf32(dy) RN_tf32(xc)^T) is
+// accurate only for gradients like iid randn.  A per-channel mean c in dy adds about 2^-11 c sigma_x sqrt(M) of error to
+// R, although the true R does not depend on c (sum xc = 0); and a dy mostly along y largely cancels in dx, so R's 2^-11
+// relative error comes back amplified.  Both are what real networks send back (a following bias, an affine layer's
+// dgamma direction): at N*HW = 4096 dx was off by up to 1.1e-2 of fp64.  So dy is centred around a per-(domain, channel)
+// pilot shift K of dy (pilot_shift on dout: every CTA of a problem computes the same K), e = dy - K and xc = x - mean are
+// both split hi / lo as in the Gram kernel, and  R = Eh Xh^T + El Xh^T + Eh Xl^T  (sum e xc^T is R: sum_m xc = 0 up to the
+// rounding of save_mean), each tile into a fresh accumulator added into an fp32 register sum; the row sums are
+// sum e + n_valid K, in the CTA epilogue, so the partial layout and everything downstream are unchanged.  dx then lands
+// within a small factor of the float32 operator sequence (tools/tf32_contract_accuracy.py,
+// tests/test_tc_backward_fp64.py).  Cost at config 2 (DESIGN.md section 8): fp32 +3.4 % on this kernel, fp32 NHWC +13 %,
+// bf16 +57 % (NCHW) / +53 % (NHWC): with half the bytes, the split transform rather than HBM bounds the bf16 kernels.
 //
 // bf16 activations (DWT_DTYPE_BF16): both kernels are templated on the storage type T.  A bf16 box is 32 px x 64 ch of
 // 2-byte values, 64-byte rows landed without swizzle (only ld.shared reads it: a warp's 8-byte loads cover whole rows,
 // conflict-free).  The transform widens each value to fp32 and writes exactly what it writes in place for an fp32 tile
 // -- same values, same SWIZZLE_128B positions -- into a per-warpgroup fp32 staging tile (the Gram kernel: hi there, lo to
-// its lo tile; the contraction: xc and dy each to their own), releases the ring stage and issues the unchanged wgmma
-// sequence from the staging tiles.  Grid, tile ranges, warpgroup alternation and epilogue are those of the fp32 kernels,
-// so every partial is bit for bit the fp32 kernel's on x.float().
+// its lo tile; the contraction: the hi parts of xc and dy each to their own, the lo parts to the lo tiles), releases the
+// ring stage and issues the unchanged wgmma sequence from the staging tiles.  Grid, tile ranges, warpgroup alternation
+// and epilogue are those of the fp32 kernels, so every partial is bit for bit the fp32 kernel's on x.float().
 //
 // channels-last activations (DWT_LAYOUT_NHWC): both kernels are also templated on the layout.  The tensor map is 3-D
 // {C, HW, N*D} with channels innermost; a tile is the same [64 ch x 32 px] block of one image, landed as rows of pixels:
@@ -44,13 +54,13 @@
 // (the pixels) contiguous, so the transform reads each thread's (channel, 4-pixel chunk) from the landed [px][ch] tile
 // and writes exactly what the NCHW transform writes, at the same swizzled positions, into the per-warpgroup fp32
 // staging tiles of the bf16 kernels; the rest is the NCHW kernel, so every partial is bit for bit the NCHW kernel's on
-// x.contiguous().  fp32 rings are shallower (Gram 8, contraction 4 stages) to keep two CTAs per SM with the staging.
+// x.contiguous().  fp32 rings are shallower (Gram 8, contraction 2 stages) to keep two CTAs per SM with the staging.
 //
 // group size 128 (fp32, both layouts): a group spans the super-blocks 2p and 2p + 1, so its 128 x 128 statistics are
 // three 64 x 64 blocks plus the 128 row sums.
 //   Gram: the diagonal blocks and row sums are tc_gram_kernel's, unchanged (it never reads the group size); the
 //   off-diagonal block G10 = sum s1 s0^T comes from tc_gram_pair_kernel, one launch later: a stage carries the tiles of
-//   both super-blocks, each is split hi / lo by gram_transform around the same pilot shifts (read back from the diagonal
+//   both super-blocks, each is split hi / lo by split_transform around the same pilot shifts (read back from the diagonal
 //   launch), and H1 H0^T + L1 H0^T + H1 L0^T go into one accumulator -- the hi/lo model of the diagonal kernel over the
 //   whole 128-vector (lo lo^T dropped, lo hi^T kept on both sides).  Chosen over one CTA holding both super-blocks'
 //   tiles and all seven 64 x 64 accumulators (224 registers per thread for one warpgroup, or an uneven split of block
@@ -58,10 +68,10 @@
 //   from HBM twice per call (the second pass is a separate launch over an 822 MB tensor at BASELINE config 2, far
 //   beyond L2) -- 2x by design, not measured directly; the profile counts the algorithmic bytes once.
 //   Contraction: tc_contract_kernel<.., PAIR = true> forms all four blocks of R (it is not symmetric), blockIdx.y =
-//   4 p + 2 r + c: dy rows from super-block 2p + r, x columns from 2p + c; x and dy are each read twice (concurrently
+//   4 p + 2 r + c: dy rows from super-block 2p + r (and their shift K), x columns from 2p + c; x and dy are each read twice (concurrently
 //   by the blocks of one wave, so partly from L2; not measured).
-//   ptxas (sm_90a): tc_gram_pair_kernel NCHW 91 / NHWC 87 registers; tc_contract_kernel<float, NCHW / NHWC, PAIR> 89 /
-//   85 registers; no spills; dynamic shared memory 97 KB (gram pair) and the contraction's 97 / 129 KB as above.
+//   ptxas (sm_90a): tc_gram_pair_kernel NCHW 85 / NHWC 87 registers; tc_contract_kernel<float, NCHW / NHWC, PAIR> 96 /
+//   96 registers; no spills; dynamic shared memory 97 KB (gram pair) and the contraction's 97 KB as above.
 //
 // Reference: utils/whitening.py:46-47 of the reference project and its autograd transpose.
 #include <cuda.h>
@@ -84,17 +94,18 @@ constexpr int kTcThreads = 128 * kConsumers + 32;
 constexpr int kPer = 512 / 128;                         // 16-byte chunks of a tile per consumer thread
 constexpr int kTilePx = 32, kTileCh = 64;
 constexpr int kTileBytes = kTileCh * kTilePx * 4;       // 8192: one fp32 tile (also a staging tile of the bf16 kernels)
-constexpr int kStagesBwd = 6;                           // x + dy per stage: 96 KB per CTA (bf16: 48 KB + 32 KB staging)
+constexpr int kStagesBwd = 4;                           // x + dy per stage: 64 KB + 32 KB lo tiles per CTA (bf16: 32 KB + 64 KB)
 constexpr int kNacc = kTileCh * kTileCh + kTileCh;      // per-CTA partial: 64x64 moments + 64 row sums
 constexpr int kGramStages = 10;                         // 80 KB ring + 2 x 8 KB lo tiles per CTA (bf16: 40 KB + 32 KB)
 // Activation storage T: float, or __nv_bfloat16 (DWT_DTYPE_BF16); a landed box is kTileCh x kTilePx values of T
 template <class T> constexpr bool kBf16 = !std::is_same<T, float>::value;
 template <class T> constexpr int kBoxBytes = kTileCh * kTilePx * (int)sizeof(T);
 // Layout NHWC: the transform writes to staging tiles (the bf16 kernels always do).  fp32 NHWC: the staging tiles cost
-// 32 KB per CTA, so the rings are shallower to keep two CTAs per SM (Gram 64 + 32 KB, contraction 64 + 32 KB).
+// 32 KB (Gram) or 64 KB (contraction: hi and lo of xc and dy) per CTA, so the rings are shallower to keep two CTAs per SM
+// (Gram 64 + 32 KB, contraction 32 + 64 KB).
 template <class T, bool NHWC> constexpr bool kStaged = kBf16<T> || NHWC;
 template <class T, bool NHWC> constexpr int kGramStagesOf = (NHWC && !kBf16<T>) ? 8 : kGramStages;
-template <class T, bool NHWC> constexpr int kStagesBwdOf = (NHWC && !kBf16<T>) ? 4 : kStagesBwd;
+template <class T, bool NHWC> constexpr int kStagesBwdOf = (NHWC && !kBf16<T>) ? 2 : kStagesBwd;
 constexpr int kMaxStages = kGramStages > kStagesBwd ? kGramStages : kStagesBwd;
 // Consumer warpgroup w takes tiles w, w + 2, ...; all ring lengths are even, so every stage (and all phases of its
 // barriers) belongs to one warpgroup, and an mbarrier parity wait never meets a barrier two phases ahead.
@@ -188,44 +199,16 @@ __device__ __forceinline__ float pilot_shift(const T* __restrict__ x, const Geom
   return pilot_refine(K, s1, s2);
 }
 
-// Transform of one landed tile by the 128 threads of a consumer warpgroup (thread t), into the fp32 SWIZZLE_128B tile dst
-// (fp32: dst == tile, in place):
-//   v <- RN_tf32(v - shift[row]) inside the tensor, 0 outside; returns per-thread row sums of (v - shift).
-// Chunk q = t + 128*i (16-byte units): row = q >> 3, physical chunk jp = q & 7, logical chunk = jp ^ (row & 7).
+// Split transform of one landed tile by the 128 threads of a consumer warpgroup (thread t): s = v - shift[row] (shared
+// memory) inside the
+// tensor, 0 outside; hi = trunc_tf32(s) to hi (fp32 NCHW: the tile itself, in place), lo = s - hi (exact) to the
+// warpgroup's lo tile at the same swizzled position; returns per-thread row sums of s.  hi is written explicitly so that
+// every product sees the same hi whatever rounding the tensor core applies to fp32 words.  Chunk q = t + 128 i (16-byte
+// units): row = q >> 3, physical chunk q & 7, logical chunk (q & 7) ^ (row & 7).  Two chunks at a time: the accumulators
+// leave few registers at two CTAs per SM.
 template <class T, bool NHWC>
-__device__ __forceinline__ void transform_tile(uint32_t tile, uint32_t dst, int t, const float (&shift)[kPer], int px0, int HW,
-                                               int ch0, int C, float (&rowsum)[kPer]) {
-  float4 v[kPer];
-#pragma unroll
-  for (int i = 0; i < kPer; ++i) {
-    const int q = t + 128 * i, row = q >> 3;
-    if constexpr (!NHWC) v[i] = ld_px4<T, NHWC>(tile, q, row, (q & 7) ^ (row & 7));
-  }
-#pragma unroll
-  for (int i = 0; i < kPer; ++i) {
-    const int q = t + 128 * i, row = q >> 3, jp = q & 7, j = jp ^ (row & 7);
-    if constexpr (NHWC) v[i] = ld_px4<T, NHWC>(tile, q, row, j);        // four scalar loads: one chunk at a time
-    const int px = px0 + 4 * j;
-    const bool rowok = (ch0 + row) < C;
-    float e[4] = {v[i].x, v[i].y, v[i].z, v[i].w};
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const bool ok = rowok && (px + k) < HW;
-      const float s = ok ? e[k] - shift[i] : 0.f;
-      rowsum[i] += s;
-      e[k] = round_tf32(s);
-    }
-    sts128(dst + 16u * (t + 128 * i), e[0], e[1], e[2], e[3]);
-  }
-}
-
-// Split transform of one landed Gram tile: s = x - shift inside the tensor, 0 outside; hi = trunc_tf32(s) to hi (fp32:
-// the tile itself, in place), lo = s - hi (exact) to the warpgroup's lo tile at the same swizzled position; returns
-// per-thread row sums of s.  hi is written explicitly so that HH and LH see the same hi whatever rounding the tensor core
-// applies to fp32 words.  Two chunks at a time: the accumulators leave few registers at two CTAs per SM.
-template <class T, bool NHWC>
-__device__ __forceinline__ void gram_transform(uint32_t tile, uint32_t hi, uint32_t lo, int t, const float (&shift)[kPer], int px0,
-                                               int HW, int ch0, int C, float (&rowsum)[kPer]) {
+__device__ __forceinline__ void split_transform(uint32_t tile, uint32_t hi, uint32_t lo, int t, const float* shift, int px0,
+                                                int HW, int ch0, int C, float (&rowsum)[kPer]) {
 #pragma unroll
   for (int h = 0; h < kPer; h += 2) {
     float4 v[2];
@@ -240,10 +223,11 @@ __device__ __forceinline__ void gram_transform(uint32_t tile, uint32_t hi, uint3
       if constexpr (NHWC) v[i] = ld_px4<T, NHWC>(tile, q, row, j);
       const int px = px0 + 4 * j;
       const bool rowok = (ch0 + row) < C;
+      const float sh = shift[row];
       float e[4] = {v[i].x, v[i].y, v[i].z, v[i].w}, l[4];
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
-        const float s = (rowok && (px + k) < HW) ? e[k] - shift[h + i] : 0.f;
+        const float s = (rowok && (px + k) < HW) ? e[k] - sh : 0.f;
         rowsum[h + i] += s;
         e[k] = __uint_as_float(__float_as_uint(s) & kTf32Mask);
         l[k] = s - e[k];
@@ -299,20 +283,27 @@ __device__ __forceinline__ void init_ring(TcBarriers& bars, int stages) {
 }
 
 // ------------------------------------------------------------------------------------------
-// backward contraction: R = sum dy xc^T and the row sums of dy
+// backward contraction: R = sum dy xc^T and the row sums of dy, split and centred (see the file header)
 // ------------------------------------------------------------------------------------------
+// Per tile: xc = x - save_mean and e = dy - K (K: the pilot shift of dy's channel, the same in every CTA of a problem)
+// are split hi / lo by split_transform, and  Eh Xh^T + El Xh^T + Eh Xl^T  go into a fresh accumulator (El Xl^T dropped, as
+// in the Gram kernel) that is added into the warpgroup's fp32 sum after the tile.  The tensor core's own accumulation
+// loses about one low bit per instruction; over the ~1,100 instructions per warpgroup of a config-2 CTA that built up
+// to 6e-3 of the dx of a y-aligned gradient (measured), per tile it stays at 12.  sum_m e xc^T is R itself: sum_m xc is
+// M (mean - save_mean), zero up to the rounding of save_mean, so K (sum xc)^T is not formed (it would add back the
+// M K (mean - save_mean)^T that rounding costs).  The row sums need K back:  rowsum_cta = sum_cta e + n_valid K.
 // PAIR (group size 128): blockIdx.y = 4 p + 2 r + c is block (r, c) of the 128 x 128 R of pair p: dy rows from
 // super-block 2p + r, x columns from super-block 2p + c (R is not symmetric: all four blocks are formed).
 template <class T, bool NHWC, bool PAIR = false>
 __global__ void __launch_bounds__(kTcThreads, 2)
-tc_contract_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_g, const Geom gm,
-                   const float* __restrict__ save_mean, float* __restrict__ partial) {
+tc_contract_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_g, const T* __restrict__ dout,
+                   const Geom gm, const float* __restrict__ save_mean, float* __restrict__ partial) {
   constexpr int STAGES = kStagesBwdOf<T, NHWC>, BOX = kBoxBytes<T>;
   constexpr bool STAGED = kStaged<T, NHWC>;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   __shared__ TcBarriers bars;
-  __shared__ float sShift[kTileCh];
+  __shared__ float sShift[kTileCh], sK[kTileCh];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, tid = threadIdx.x;
   const int sb = blockIdx.y, d = blockIdx.z;
   const int ch0 = PAIR ? (2 * (sb >> 2) + ((sb >> 1) & 1)) * kTileCh : sb * kTileCh;     // dy channels
@@ -324,11 +315,11 @@ tc_contract_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
   if (tid < kTileCh) sShift[tid] = chx + tid < gm.C ? save_mean[(size_t)d * gm.C + chx + tid] : 0.f;
   __syncthreads();
 
-  float acc[32], rowsum[kPer];
+  float acc[32], tot[32], rowsum[kPer], dummy[kPer];
 #pragma unroll
-  for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+  for (int i = 0; i < 32; ++i) { acc[i] = 0.f; tot[i] = 0.f; }
 #pragma unroll
-  for (int i = 0; i < kPer; ++i) rowsum[i] = 0.f;
+  for (int i = 0; i < kPer; ++i) { rowsum[i] = 0.f; dummy[i] = 0.f; }
 
   if (warp == kProducerWarp) {
     // ===== TMA producer =====
@@ -344,21 +335,22 @@ tc_contract_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
       }
     }
   } else {
-    // ===== consumer warpgroups: transform, then D[64 x 64] += dy_tile (A) * xc_tile^T (B) =====
+    // ===== consumer warpgroups: split transforms, then D[64 x 64] = Eh Xh^T + El Xh^T + Eh Xl^T, sum += D =====
     const int wg = warp >> 2, t = tid & 127;
-    float shift[kPer], zero[kPer], dummy[kPer];
-#pragma unroll
-    for (int i = 0; i < kPer; ++i) { shift[i] = sShift[(t + 128 * i) >> 3]; zero[i] = 0.f; dummy[i] = 0.f; }
-    // bf16 / NHWC: the warpgroup's fp32 staging tiles (xc, dy) behind the ring; fp32 NCHW: the landed tiles themselves
-    const uint32_t stage_f32 = smem_u32(smem + (size_t)STAGES * 2 * BOX + (size_t)wg * 2 * kTileBytes);
+    // dy's shift: its dependent loads overlap the producer's first TMA loads (named barrier 3: the consumers only)
+    if (tid < kTileCh) sK[tid] = pilot_shift<T, NHWC>(dout, gm, d, ch0 + tid);          // 0 past C
+    asm volatile("bar.sync 3, %0;" ::"n"(128 * kConsumers) : "memory");
+    // per warpgroup behind the ring: the lo tiles of xc and dy (fp32 NCHW: hi in place), or hi and lo of both (bf16 / NHWC)
+    const uint32_t wgbuf = smem_u32(smem + (size_t)STAGES * 2 * BOX + (size_t)wg * (STAGED ? 4 : 2) * kTileBytes);
+    const uint32_t xlo = STAGED ? wgbuf + 2 * kTileBytes : wgbuf, dlo = xlo + kTileBytes;
     for (int it = wg; it < ntiles; it += kConsumers) {
       const int s = it % STAGES;
       mbar_wait(&bars.full[s], (it / STAGES) & 1);
       const int tl = tr.begin + it, n = tl / tr.PB, pb = tl - n * tr.PB;
       const uint32_t tile = smem_u32(smem + (size_t)s * 2 * BOX);
-      const uint32_t xs = STAGED ? stage_f32 : tile, ys = STAGED ? stage_f32 + kTileBytes : tile + kTileBytes;
-      transform_tile<T, NHWC>(tile, xs, t, shift, pb * kTilePx, gm.HW, chx, gm.C, dummy);               // xc
-      transform_tile<T, NHWC>(tile + BOX, ys, t, zero, pb * kTilePx, gm.HW, ch0, gm.C, rowsum);         // dy, sums
+      const uint32_t xhi = STAGED ? wgbuf : tile, dhi = STAGED ? wgbuf + kTileBytes : tile + kTileBytes;
+      split_transform<T, NHWC>(tile, xhi, xlo, t, sShift, pb * kTilePx, gm.HW, chx, gm.C, dummy);          // xc
+      split_transform<T, NHWC>(tile + BOX, dhi, dlo, t, sK, pb * kTilePx, gm.HW, ch0, gm.C, rowsum);    // dy - K
       if constexpr (STAGED) {                      // the stage is read: it can be refilled while the MMAs run
         __syncwarp();
         if (lane == 0) mbar_arrive(&bars.empty[s]);
@@ -367,31 +359,42 @@ tc_contract_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
       warpgroup_sync(wg);
       wgmma_fence();
       fence_operands(acc);
-      const uint64_t xdesc = make_kmajor_sw128_desc(xs), adesc = make_kmajor_sw128_desc(ys);
+      const uint64_t xhdesc = make_kmajor_sw128_desc(xhi), dhdesc = make_kmajor_sw128_desc(dhi);
+      const uint64_t xldesc = make_kmajor_sw128_desc(xlo), dldesc = make_kmajor_sw128_desc(dlo);
 #pragma unroll
-      for (int k = 0; k < kTilePx / 8; ++k) wgmma_m64n64k8_ss(acc, adesc + 2 * k, xdesc + 2 * k);
+      for (int k = 0; k < kTilePx / 8; ++k) {
+        if (k == 0) wgmma_m64n64k8_ss<false>(acc, dhdesc, xhdesc);           // D = product: a fresh sum per tile
+        else wgmma_m64n64k8_ss(acc, dhdesc + 2 * k, xhdesc + 2 * k);
+        wgmma_m64n64k8_ss(acc, dldesc + 2 * k, xhdesc + 2 * k);
+        wgmma_m64n64k8_ss(acc, dhdesc + 2 * k, xldesc + 2 * k);
+      }
       wgmma_commit();
-      wgmma_wait<0>();                             // staged: the staging tiles are rewritten by the next transform
+      wgmma_wait<0>();                             // the lo (staged: and hi) tiles are rewritten by the next transform
       fence_operands(acc);
       if constexpr (!STAGED) {
         __syncwarp();
         if (lane == 0) mbar_arrive(&bars.empty[s]);
       }
+#pragma unroll
+      for (int i = 0; i < 32; ++i) tot[i] += acc[i];
     }
   }
 
-  // ===== epilogue: both warpgroups' accumulators + row sums -> this CTA's partial row =====
+  // ===== epilogue: both warpgroups' sums + row sums (K folded back in) -> this CTA's partial row =====
   __syncthreads();                                 // every stage consumed: the ring is free
   float* sAcc = reinterpret_cast<float*>(smem);    // [64][64] + [64]
   for (int e = tid; e < kNacc; e += kTcThreads) sAcc[e] = 0.f;
   __syncthreads();
   if (warp < kProducerWarp) {
-    add_fragment<8>(sAcc, kTileCh, acc, warp, lane);
+    add_fragment<8>(sAcc, kTileCh, tot, warp, lane);
     add_rowsums(sAcc + kTileCh * kTileCh, rowsum, tid & 127);
   }
   __syncthreads();
+  // in-tensor pixels of the range: 32 per tile, less (PB * 32 - HW) for every last tile of an image in it
+  const int n_valid = ntiles * kTilePx - (tr.end / tr.PB - tr.begin / tr.PB) * (tr.PB * kTilePx - gm.HW);
   float* prow = partial + (((size_t)d * gridDim.y + sb) * gridDim.x + blockIdx.x) * kNacc;
-  for (int e = tid; e < kNacc; e += kTcThreads) prow[e] = sAcc[e];
+  for (int e = tid; e < kTileCh * kTileCh; e += kTcThreads) prow[e] = sAcc[e];
+  if (tid < kTileCh) prow[kTileCh * kTileCh + tid] = fmaf((float)n_valid, sK[tid], sAcc[kTileCh * kTileCh + tid]);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -445,16 +448,13 @@ tc_gram_kernel(const __grid_constant__ CUtensorMap map_x, const T* __restrict__ 
     const uint32_t wgbuf = smem_u32(smem + (size_t)STAGES * BOX + (size_t)wg * (STAGED ? 2 : 1) * kTileBytes);
     const uint32_t lo = STAGED ? wgbuf + kTileBytes : wgbuf;
     const uint64_t ldesc = make_kmajor_sw128_desc(lo);
-    float shift[kPer];
-#pragma unroll
-    for (int i = 0; i < kPer; ++i) shift[i] = sShift[(t + 128 * i) >> 3];
     for (int it = wg; it < ntiles; it += kConsumers) {
       const int s = it % STAGES;
       mbar_wait(&bars.full[s], (it / STAGES) & 1);
       const int tl = tr.begin + it, n = tl / tr.PB, pb = tl - n * tr.PB;
       const uint32_t tile = smem_u32(smem + (size_t)s * BOX);
       const uint32_t hi = STAGED ? wgbuf : tile;
-      gram_transform<T, NHWC>(tile, hi, lo, t, shift, pb * kTilePx, gm.HW, ch0, gm.C, rowsum);
+      split_transform<T, NHWC>(tile, hi, lo, t, sShift, pb * kTilePx, gm.HW, ch0, gm.C, rowsum);
       if constexpr (STAGED) {                    // the stage is read: it can be refilled while the MMAs run
         __syncwarp();
         if (lane == 0) mbar_arrive(&bars.empty[s]);
@@ -557,21 +557,17 @@ tc_gram_pair_kernel(const __grid_constant__ CUtensorMap map_x, const Geom gm, co
     // per warpgroup behind the ring: NCHW the lo tiles of rows and columns (hi in place); NHWC hi, lo of rows, hi, lo of columns
     const uint32_t wgbuf = smem_u32(smem + (size_t)STAGES * 2 * BOX + (size_t)wg * (NHWC ? 4 : 2) * kTileBytes);
     const uint32_t lo_r = NHWC ? wgbuf + kTileBytes : wgbuf, lo_c = NHWC ? wgbuf + 3 * kTileBytes : wgbuf + kTileBytes;
-    float shr[kPer], shc[kPer], dummy[kPer];
+    float dummy[kPer];
 #pragma unroll
-    for (int i = 0; i < kPer; ++i) {
-      shr[i] = sShift[0][(t + 128 * i) >> 3];
-      shc[i] = sShift[1][(t + 128 * i) >> 3];
-      dummy[i] = 0.f;
-    }
+    for (int i = 0; i < kPer; ++i) dummy[i] = 0.f;
     for (int it = wg; it < ntiles; it += kConsumers) {
       const int s = it % STAGES;
       mbar_wait(&bars.full[s], (it / STAGES) & 1);
       const int tl = tr.begin + it, n = tl / tr.PB, pb = tl - n * tr.PB;
       const uint32_t tile = smem_u32(smem + (size_t)s * 2 * BOX);
       const uint32_t hi_r = NHWC ? wgbuf : tile, hi_c = NHWC ? wgbuf + 2 * kTileBytes : tile + BOX;
-      gram_transform<float, NHWC>(tile, hi_r, lo_r, t, shr, pb * kTilePx, gm.HW, chr, gm.C, dummy);
-      gram_transform<float, NHWC>(tile + BOX, hi_c, lo_c, t, shc, pb * kTilePx, gm.HW, chc, gm.C, dummy);
+      split_transform<float, NHWC>(tile, hi_r, lo_r, t, sShift[0], pb * kTilePx, gm.HW, chr, gm.C, dummy);
+      split_transform<float, NHWC>(tile + BOX, hi_c, lo_c, t, sShift[1], pb * kTilePx, gm.HW, chc, gm.C, dummy);
       if constexpr (NHWC) {                        // the stage is read: it can be refilled while the MMAs run
         __syncwarp();
         if (lane == 0) mbar_arrive(&bars.empty[s]);
@@ -641,13 +637,13 @@ int make_map(CUtensorMap* map, const void* base, const Geom& gm, bool bf16, bool
                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
 }
 
-// fp32 NCHW: the ring (+ the lo tiles); bf16 / NHWC: the ring + fp32 staging tiles (two per warpgroup)
+// The ring + per-warpgroup fp32 tiles: Gram lo (bf16 / NHWC: + hi staging); contraction lo of xc and dy (bf16 / NHWC: +
+// hi staging of both).  97 KB per contraction CTA in every instantiation.
 template <class T, bool NHWC>
 size_t tc_smem_bytes(bool two) {
   constexpr bool staged = kStaged<T, NHWC>;
-  const size_t wgbuf = (size_t)kConsumers * (staged ? 2 : 1) * kTileBytes;
-  return two ? (size_t)kStagesBwdOf<T, NHWC> * 2 * kBoxBytes<T> + (staged ? wgbuf : 0) + 1024
-             : (size_t)kGramStagesOf<T, NHWC> * kBoxBytes<T> + wgbuf + 1024;
+  return two ? (size_t)kStagesBwdOf<T, NHWC> * 2 * kBoxBytes<T> + (size_t)kConsumers * (staged ? 4 : 2) * kTileBytes + 1024
+             : (size_t)kGramStagesOf<T, NHWC> * kBoxBytes<T> + (size_t)kConsumers * (staged ? 2 : 1) * kTileBytes + 1024;
 }
 
 template <class T, bool NHWC>
@@ -683,17 +679,18 @@ void launch_gram(const CUtensorMap& mx, const void* x, const Geom& gm, int nchun
 }
 
 template <class T, bool NHWC>
-void launch_contract(const CUtensorMap& mx, const CUtensorMap& mg, const Geom& gm, int nchunks, const float* save_mean,
-                     float* partial, cudaStream_t st) {
+void launch_contract(const CUtensorMap& mx, const CUtensorMap& mg, const void* dout, const Geom& gm, int nchunks,
+                     const float* save_mean, float* partial, cudaStream_t st) {
+  const T* g = static_cast<const T*>(dout);
   if constexpr (!kBf16<T>) {
     if (gm.GS == 2 * kTileCh) {                  // group size 128: the four 64 x 64 blocks of every group's R
       dim3 grid(nchunks, 2 * tc_superblocks(gm), gm.D);
-      tc_contract_kernel<T, NHWC, true><<<grid, kTcThreads, tc_smem_bytes<T, NHWC>(true), st>>>(mx, mg, gm, save_mean, partial);
+      tc_contract_kernel<T, NHWC, true><<<grid, kTcThreads, tc_smem_bytes<T, NHWC>(true), st>>>(mx, mg, g, gm, save_mean, partial);
       return;
     }
   }
   dim3 grid(nchunks, tc_superblocks(gm), gm.D);
-  tc_contract_kernel<T, NHWC><<<grid, kTcThreads, tc_smem_bytes<T, NHWC>(true), st>>>(mx, mg, gm, save_mean, partial);
+  tc_contract_kernel<T, NHWC><<<grid, kTcThreads, tc_smem_bytes<T, NHWC>(true), st>>>(mx, mg, g, gm, save_mean, partial);
 }
 
 }  // namespace
@@ -761,11 +758,11 @@ int tc_bwd_reduce(const void* x, const void* dout, bool bf16, bool nhwc, const G
   if (int rc = make_map(&mx, x, gm, bf16, nhwc)) return rc;
   if (int rc = make_map(&mg, dout, gm, bf16, nhwc)) return rc;
   if (nhwc) {
-    if (bf16) launch_contract<__nv_bfloat16, true>(mx, mg, gm, nchunks, save_mean, partial, st);
-    else launch_contract<float, true>(mx, mg, gm, nchunks, save_mean, partial, st);
+    if (bf16) launch_contract<__nv_bfloat16, true>(mx, mg, dout, gm, nchunks, save_mean, partial, st);
+    else launch_contract<float, true>(mx, mg, dout, gm, nchunks, save_mean, partial, st);
   } else {
-    if (bf16) launch_contract<__nv_bfloat16, false>(mx, mg, gm, nchunks, save_mean, partial, st);
-    else launch_contract<float, false>(mx, mg, gm, nchunks, save_mean, partial, st);
+    if (bf16) launch_contract<__nv_bfloat16, false>(mx, mg, dout, gm, nchunks, save_mean, partial, st);
+    else launch_contract<float, false>(mx, mg, dout, gm, nchunks, save_mean, partial, st);
   }
   return 0;
 }

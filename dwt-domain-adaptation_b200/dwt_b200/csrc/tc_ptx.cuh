@@ -98,14 +98,15 @@ __device__ __forceinline__ void fence_operands(float (&d)[N]) {
 // named barrier over the 128 threads of one warpgroup (id 1 + warpgroup index; id 0 is __syncthreads)
 __device__ __forceinline__ void warpgroup_sync(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory"); }
 
-// D[64 x 64] += A[64 x 8] * B[64 x 8]^T, both operands K-major in shared memory (descriptors)
+// D[64 x 64] += A[64 x 8] * B[64 x 8]^T, both operands K-major in shared memory (descriptors); ACC = false: D = A B^T
+template <bool ACC = true>
 __device__ __forceinline__ void wgmma_m64n64k8_ss(float (&d)[32], uint64_t da, uint64_t db) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
       "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 "
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-      : "l"(da), "l"(db));
+      : "l"(da), "l"(db), "n"(ACC ? 1 : 0));
 }
 
 // D[64 x 64] += A[64 x 8] * B[64 x 8]^T, A from registers (tf32 fragment), B K-major in shared memory
