@@ -22,9 +22,14 @@
 // error times the condition number (the eps = 1e-3 shrinkage is absolute and stops helping once activations are
 // large), so a single tf32 pass is not enough (y errors of 1e-3..5e-3 at cond >= 1e4).  Each centred sample
 // s = x - K is split hi = trunc_tf32(s) and lo = s - hi (exact in fp32; the core keeps its top 11 bits), and
-//       G = HH + LH + LH^T         HH = sum hi hi^T,  LH = sum lo hi^T        (lo lo^T ~ 3e-7 G is dropped)
-// comes out of two M=64 N=64 K=8 MMAs per 8 pixels: A = the hi tile (written back in place) or the lo tile (a
-// per-warpgroup buffer), B = the hi tile.  The row sums the mean needs are summed by the transform.
+//       G = (S + S^T) / 2,  S = HH + 2 LH      HH = sum hi hi^T,  LH = sum lo hi^T     (lo lo^T ~ 3e-7 G is dropped)
+// comes out of two M=64 N=64 K=8 MMAs per 8 pixels: A = the hi tile (written back in place) or the 2 lo tile (a
+// per-warpgroup buffer; doubling is exact), B = the hi tile.  ACCUMULATION: each 32-pixel tile's eight MMAs go into a
+// fresh accumulator (the first one overwrites it) that is added into an fp32 register sum after the tile.  The tensor
+// core's own fp32 accumulation loses about one low bit per instruction, and not at random: with one accumulator per CTA
+// (~760 instructions per warpgroup at config 2, ~380 tiles per CTA) the covariance drifted 3.9e-5 from float64, growing
+// with the tiles per CTA (8.1e-5 at 760); per tile it stays at 7.5e-7 at every length
+// (tests/test_tc_forward_stats_fp64.py).  The row sums the mean needs are summed by the transform.
 //
 // bwd_reduce (tc_contract_kernel) -- SPLIT precision, dy CENTRED.  A single tf32 pass (RN_tf32(dy) RN_tf32(xc)^T) is
 // accurate only for gradients like iid randn.  A per-channel mean c in dy adds about 2^-11 c sigma_x sqrt(M) of error to
@@ -61,17 +66,17 @@
 //   Gram: the diagonal blocks and row sums are tc_gram_kernel's, unchanged (it never reads the group size); the
 //   off-diagonal block G10 = sum s1 s0^T comes from tc_gram_pair_kernel, one launch later: a stage carries the tiles of
 //   both super-blocks, each is split hi / lo by split_transform around the same pilot shifts (read back from the diagonal
-//   launch), and H1 H0^T + L1 H0^T + H1 L0^T go into one accumulator -- the hi/lo model of the diagonal kernel over the
-//   whole 128-vector (lo lo^T dropped, lo hi^T kept on both sides).  Chosen over one CTA holding both super-blocks'
-//   tiles and all seven 64 x 64 accumulators (224 registers per thread for one warpgroup, or an uneven split of block
-//   rows across warpgroups) because it reuses the diagonal kernel as it is and keeps two CTAs per SM.  Cost: x is read
+//   launch), and H1 H0^T + L1 H0^T + H1 L0^T go into a fresh accumulator per tile, added into an fp32 register sum --
+//   the hi/lo model of the diagonal kernel over the whole 128-vector (lo lo^T dropped, lo hi^T kept on both sides).
+//   Chosen over one CTA holding both super-blocks' tiles and all seven 64 x 64 accumulators (224 registers per thread
+//   for one warpgroup, or an uneven split of block rows across warpgroups) because it reuses the diagonal kernel as it is and keeps two CTAs per SM.  Cost: x is read
 //   from HBM twice per call (the second pass is a separate launch over an 822 MB tensor at BASELINE config 2, far
 //   beyond L2) -- 2x by design, not measured directly; the profile counts the algorithmic bytes once.
 //   Contraction: tc_contract_kernel<.., PAIR = true> forms all four blocks of R (it is not symmetric), blockIdx.y =
 //   4 p + 2 r + c: dy rows from super-block 2p + r (and their shift K), x columns from 2p + c; x and dy are each read twice (concurrently
 //   by the blocks of one wave, so partly from L2; not measured).
-//   ptxas (sm_90a): tc_gram_pair_kernel NCHW 85 / NHWC 87 registers; tc_contract_kernel<float, NCHW / NHWC, PAIR> 96 /
-//   96 registers; no spills; dynamic shared memory 97 KB (gram pair) and the contraction's 97 KB as above.
+//   ptxas (sm_90a): tc_gram_kernel 96 registers in all four instantiations; tc_gram_pair_kernel NCHW 93 / NHWC 88
+//   registers; tc_contract_kernel<float, NCHW / NHWC, PAIR> 96 / 96 registers; no spills; dynamic shared memory 97 KB (gram pair) and the contraction's 97 KB as above.
 //
 // Reference: utils/whitening.py:46-47 of the reference project and its autograd transpose.
 #include <cuda.h>
@@ -205,8 +210,8 @@ __device__ __forceinline__ float pilot_shift(const T* __restrict__ x, const Geom
 // warpgroup's lo tile at the same swizzled position; returns per-thread row sums of s.  hi is written explicitly so that
 // every product sees the same hi whatever rounding the tensor core applies to fp32 words.  Chunk q = t + 128 i (16-byte
 // units): row = q >> 3, physical chunk q & 7, logical chunk (q & 7) ^ (row & 7).  Two chunks at a time: the accumulators
-// leave few registers at two CTAs per SM.
-template <class T, bool NHWC>
+// leave few registers at two CTAs per SM.  LO2: the lo tile holds 2 lo (exact), for the Gram kernel's symmetric form.
+template <class T, bool NHWC, bool LO2 = false>
 __device__ __forceinline__ void split_transform(uint32_t tile, uint32_t hi, uint32_t lo, int t, const float* shift, int px0,
                                                 int HW, int ch0, int C, float (&rowsum)[kPer]) {
 #pragma unroll
@@ -230,7 +235,7 @@ __device__ __forceinline__ void split_transform(uint32_t tile, uint32_t hi, uint
         const float s = (rowok && (px + k) < HW) ? e[k] - sh : 0.f;
         rowsum[h + i] += s;
         e[k] = __uint_as_float(__float_as_uint(s) & kTf32Mask);
-        l[k] = s - e[k];
+        l[k] = LO2 ? 2.f * (s - e[k]) : s - e[k];
       }
       sts128(hi + 16u * q, e[0], e[1], e[2], e[3]);
       sts128(lo + 16u * q, l[0], l[1], l[2], l[3]);
@@ -423,9 +428,9 @@ tc_gram_kernel(const __grid_constant__ CUtensorMap map_x, const T* __restrict__ 
   }
   __syncthreads();
 
-  float hh[32], lh[32], rowsum[kPer];
+  float acc[32], tot[32], rowsum[kPer];
 #pragma unroll
-  for (int i = 0; i < 32; ++i) { hh[i] = 0.f; lh[i] = 0.f; }
+  for (int i = 0; i < 32; ++i) { acc[i] = 0.f; tot[i] = 0.f; }
 #pragma unroll
   for (int i = 0; i < kPer; ++i) rowsum[i] = 0.f;
 
@@ -442,7 +447,7 @@ tc_gram_kernel(const __grid_constant__ CUtensorMap map_x, const T* __restrict__ 
       }
     }
   } else {
-    // ===== consumer warpgroups: HH[64 x 64] += hi * hi^T,  LH[64 x 64] += lo * hi^T =====
+    // ===== consumer warpgroups: D[64 x 64] = hi hi^T + (2 lo) hi^T per tile, sum += D =====
     const int wg = warp >> 2, t = tid & 127;
     // per warpgroup behind the ring: the lo tile (fp32 NCHW), or the hi staging tile and the lo tile (bf16 / NHWC)
     const uint32_t wgbuf = smem_u32(smem + (size_t)STAGES * BOX + (size_t)wg * (STAGED ? 2 : 1) * kTileBytes);
@@ -454,7 +459,7 @@ tc_gram_kernel(const __grid_constant__ CUtensorMap map_x, const T* __restrict__ 
       const int tl = tr.begin + it, n = tl / tr.PB, pb = tl - n * tr.PB;
       const uint32_t tile = smem_u32(smem + (size_t)s * BOX);
       const uint32_t hi = STAGED ? wgbuf : tile;
-      split_transform<T, NHWC>(tile, hi, lo, t, sShift, pb * kTilePx, gm.HW, ch0, gm.C, rowsum);
+      split_transform<T, NHWC, true>(tile, hi, lo, t, sShift, pb * kTilePx, gm.HW, ch0, gm.C, rowsum);
       if constexpr (STAGED) {                    // the stage is read: it can be refilled while the MMAs run
         __syncwarp();
         if (lane == 0) mbar_arrive(&bars.empty[s]);
@@ -462,43 +467,42 @@ tc_gram_kernel(const __grid_constant__ CUtensorMap map_x, const T* __restrict__ 
       fence_proxy_async();
       warpgroup_sync(wg);
       wgmma_fence();
-      fence_operands(hh);
-      fence_operands(lh);
+      fence_operands(acc);
       const uint64_t bdesc = make_kmajor_sw128_desc(hi);
 #pragma unroll
       for (int k = 0; k < kTilePx / 8; ++k) {
-        wgmma_m64n64k8_ss(hh, bdesc + 2 * k, bdesc + 2 * k);
-        wgmma_m64n64k8_ss(lh, ldesc + 2 * k, bdesc + 2 * k);
+        if (k == 0) wgmma_m64n64k8_ss<false>(acc, bdesc, bdesc);             // D = product: a fresh sum per tile
+        else wgmma_m64n64k8_ss(acc, bdesc + 2 * k, bdesc + 2 * k);
+        wgmma_m64n64k8_ss(acc, ldesc + 2 * k, bdesc + 2 * k);
       }
       wgmma_commit();
       wgmma_wait<0>();                             // the lo (staged: and hi) tile is rewritten by this warpgroup's next transform
-      fence_operands(hh);
-      fence_operands(lh);
+      fence_operands(acc);
       if constexpr (!STAGED) {
         __syncwarp();
         if (lane == 0) mbar_arrive(&bars.empty[s]);
       }
+#pragma unroll
+      for (int i = 0; i < 32; ++i) tot[i] += acc[i];
     }
   }
 
-  // ===== epilogue: G = HH + LH + LH^T and the row sums -> this CTA's partial row =====
-  constexpr int P = kTileCh + 1;                   // odd pitch: the transposed read of LH is conflict-free
+  // ===== epilogue: both warpgroups' sums S = HH + 2 LH, G = (S + S^T) / 2 and the row sums -> this CTA's partial row =====
+  constexpr int P = kTileCh + 1;                   // odd pitch: the transposed read is conflict-free
   __syncthreads();                                 // every stage consumed: the ring is free
-  float* sH = reinterpret_cast<float*>(smem);      // [64][P]
-  float* sL = sH + kTileCh * P;                    // [64][P]
-  float* sRS = sL + kTileCh * P;                   // [64]
-  for (int e = tid; e < 2 * kTileCh * P + kTileCh; e += kTcThreads) sH[e] = 0.f;
+  float* sS = reinterpret_cast<float*>(smem);      // [64][P]
+  float* sRS = sS + kTileCh * P;                   // [64]
+  for (int e = tid; e < kTileCh * P + kTileCh; e += kTcThreads) sS[e] = 0.f;
   __syncthreads();
   if (warp < kProducerWarp) {
-    add_fragment<8>(sH, P, hh, warp, lane);
-    add_fragment<8>(sL, P, lh, warp, lane);
+    add_fragment<8>(sS, P, tot, warp, lane);
     add_rowsums(sRS, rowsum, tid & 127);
   }
   __syncthreads();
   float* prow = partial + (((size_t)d * gridDim.y + sb) * gridDim.x + blockIdx.x) * kNacc;
   for (int e = tid; e < kTileCh * kTileCh; e += kTcThreads) {
     const int r = e >> 6, c = e & 63;
-    prow[e] = (sH[r * P + c] + sL[r * P + c]) + sL[c * P + r];
+    prow[e] = 0.5f * (sS[r * P + c] + sS[c * P + r]);
   }
   if (tid < kTileCh) prow[kTileCh * kTileCh + tid] = sRS[tid];
 }
@@ -533,9 +537,9 @@ tc_gram_pair_kernel(const __grid_constant__ CUtensorMap map_x, const Geom gm, co
   if (tid < 2 * kTileCh) sShift[tid >> 6][tid & 63] = shift[((size_t)d * SB + 2 * p + 1 - (tid >> 6)) * kTileCh + (tid & 63)];
   __syncthreads();
 
-  float acc[32];
+  float acc[32], tot[32];
 #pragma unroll
-  for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+  for (int i = 0; i < 32; ++i) { acc[i] = 0.f; tot[i] = 0.f; }
 
   if (warp == kProducerWarp) {
     // ===== TMA producer =====
@@ -552,7 +556,7 @@ tc_gram_pair_kernel(const __grid_constant__ CUtensorMap map_x, const Geom gm, co
       }
     }
   } else {
-    // ===== consumer warpgroups: G10[64 x 64] += h1 h0^T + l1 h0^T + h1 l0^T =====
+    // ===== consumer warpgroups: D[64 x 64] = h1 h0^T + l1 h0^T + h1 l0^T per tile, sum += D =====
     const int wg = warp >> 2, t = tid & 127;
     // per warpgroup behind the ring: NCHW the lo tiles of rows and columns (hi in place); NHWC hi, lo of rows, hi, lo of columns
     const uint32_t wgbuf = smem_u32(smem + (size_t)STAGES * 2 * BOX + (size_t)wg * (NHWC ? 4 : 2) * kTileBytes);
@@ -580,7 +584,8 @@ tc_gram_pair_kernel(const __grid_constant__ CUtensorMap map_x, const Geom gm, co
       const uint64_t hc = make_kmajor_sw128_desc(hi_c), lc = make_kmajor_sw128_desc(lo_c);
 #pragma unroll
       for (int k = 0; k < kTilePx / 8; ++k) {
-        wgmma_m64n64k8_ss(acc, hr + 2 * k, hc + 2 * k);
+        if (k == 0) wgmma_m64n64k8_ss<false>(acc, hr, hc);                   // D = product: a fresh sum per tile
+        else wgmma_m64n64k8_ss(acc, hr + 2 * k, hc + 2 * k);
         wgmma_m64n64k8_ss(acc, lr + 2 * k, hc + 2 * k);
         wgmma_m64n64k8_ss(acc, hr + 2 * k, lc + 2 * k);
       }
@@ -591,15 +596,17 @@ tc_gram_pair_kernel(const __grid_constant__ CUtensorMap map_x, const Geom gm, co
         __syncwarp();
         if (lane == 0) mbar_arrive(&bars.empty[s]);
       }
+#pragma unroll
+      for (int i = 0; i < 32; ++i) tot[i] += acc[i];
     }
   }
 
-  // ===== epilogue: both warpgroups' accumulators -> this CTA's partial row (row-sum slots 0: the diagonal kernel has them) =====
+  // ===== epilogue: both warpgroups' sums -> this CTA's partial row (row-sum slots 0: the diagonal kernel has them) =====
   __syncthreads();
   float* sAcc = reinterpret_cast<float*>(smem);    // [64][64]
   for (int e = tid; e < kTileCh * kTileCh; e += kTcThreads) sAcc[e] = 0.f;
   __syncthreads();
-  if (warp < kProducerWarp) add_fragment<8>(sAcc, kTileCh, acc, warp, lane);
+  if (warp < kProducerWarp) add_fragment<8>(sAcc, kTileCh, tot, warp, lane);
   __syncthreads();
   float* prow = partial + (((size_t)d * gridDim.y + p) * gridDim.x + blockIdx.x) * kNacc;
   for (int e = tid; e < kNacc; e += kTcThreads) prow[e] = e < kTileCh * kTileCh ? sAcc[e] : 0.f;

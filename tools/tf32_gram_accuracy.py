@@ -1,15 +1,18 @@
 """CPU emulation of the tf32 Gram contraction of the forward statistics (csrc/norm_tc.cu): covariance and y error of
 
   single   G = sum RN_tf32(s) RN_tf32(s)^T                        (round-1 kernel: one tf32 pass)
-  split    G = HH + LH + LH^T,  hi = trunc_tf32(s), lo = trunc_tf32(s - hi): the shipped tc_gram_kernel -- the tensor
-           core reads the top 19 bits of the fp32 words it is handed (s itself for hi, s - trunc(s) for lo)
+  split    G = HH + LH + LH^T,  hi = trunc_tf32(s), lo = trunc_tf32(s - hi): the products of tc_gram_kernel -- the
+           tensor core reads the top 19 bits of the fp32 words it is handed (s itself for hi, s - trunc(s) for lo)
   split-rn the same with hi = RN_tf32(s) (the first round-2 kernel: two more instructions per element)
   fp32     the same sums with fp32 operands                        (what the reference's torch.bmm computes)
 
 against the fp64 covariance, over condition number, activation scale and |mean|/sigma.  s = x - K with the pilot
-shift K; products are exact in fp32 and the accumulation is emulated in fp64 (the kernel keeps per-CTA partials of a
-few thousand samples and reduces them in fixed order); optionally with a truncating fp32 accumulator per 8-sample
-MMA step (--rz) as a pessimistic model of the tensor core's accumulate.  Pure numpy.
+shift K; products are exact in fp32 and the accumulation is emulated in fp64; optionally with a truncating fp32
+accumulator per 8-sample MMA step (--rz) as a pessimistic model of the tensor core's accumulate.  The kernel's per-CTA
+partials are not a few thousand samples: a Gram CTA covers N*HW*SB / (2 SMs) samples of its super-block, about 12,000
+(380 tiles of 32 pixels) at BASELINE config 2 on 132 SMs.  So it sums each 32-pixel tile in a fresh tensor-core
+accumulator and the tiles in fp32 registers; one accumulator per CTA drifted 3.9e-5 from the fp64 covariance there
+(tests/test_tc_forward_stats_fp64.py), which the fp64 accumulation here does not model.  Pure numpy.
       python tools/tf32_gram_accuracy.py [--rz]
 """
 import sys
