@@ -24,6 +24,7 @@ LAYOUT_NHWC = 0x100
 DTYPE_BF16 = 0x200                 # bf16 activations (gs 1/2/4 and BN channels-last or NCHW, tensor-core gs 8..64; dwt_b200.h)
 STATUS_NOT_PD, STATUS_BAD_LABEL = 1, 2
 ZCA_MAX_ITERATIONS = 16            # Newton-Schulz iterations of the ZCA basis (dwt_whiten_zca_*): 1..16
+EIGH = "eigh"                      # the exact ZCA basis (dwt_whiten_eigh_*) where a number of iterations goes
 KIND_WHITEN, KIND_BN = 0, 1
 
 _c_float_p = ctypes.c_void_p
@@ -61,6 +62,15 @@ _SIGNATURES = {
                                           ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float,
                                           ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, ctypes.c_void_p,
                                           ctypes.c_size_t, ctypes.c_void_p]),
+    "dwt_whiten_eigh_fwd": (ctypes.c_int, [_c_float_p, _c_float_p, ctypes.c_int64, ctypes.c_int64, ctypes.c_int64,
+                                           ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float,
+                                           ctypes.c_int, ctypes.POINTER(ctypes.c_void_p), ctypes.POINTER(ctypes.c_void_p),
+                                           _c_float_p, _c_float_p, _c_float_p, ctypes.c_void_p, ctypes.c_size_t,
+                                           ctypes.c_void_p]),
+    "dwt_whiten_eigh_bwd": (ctypes.c_int, [_c_float_p, _c_float_p, _c_float_p, ctypes.c_int64, ctypes.c_int64,
+                                           ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float,
+                                           _c_float_p, _c_float_p, _c_float_p, ctypes.c_void_p, ctypes.c_size_t,
+                                           ctypes.c_void_p]),
     "dwt_bn_fwd": (ctypes.c_int, [_c_float_p, _c_float_p, ctypes.c_int64, ctypes.c_int64, ctypes.c_int64,
                                   ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_int,
                                   ctypes.POINTER(ctypes.c_void_p), ctypes.POINTER(ctypes.c_void_p), _c_float_p,

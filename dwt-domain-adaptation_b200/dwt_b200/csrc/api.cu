@@ -442,29 +442,49 @@ struct Call {
   const char* name(bool bwd, Pass ps) const { return kProfName[bwd][r.fam][ps][2 * nhwc + bf16]; }
 };
 
-// The ZCA basis (dwt_whiten_zca_*): Newton-Schulz iterations, and the matrices they save for the backward.
-// on == false: the Cholesky basis (dwt_whiten_*, dwt_bn_*).
-struct Zca {
-  bool on = false;
+// The whitening basis of a call, and the per-group matrices its forward saves for the backward:
+//   CHOLESKY       dwt_whiten_*, dwt_bn_* (nothing saved beyond save_w)
+//   NEWTON_SCHULZ  dwt_whiten_zca_*: `iters` iterations, save = save_p [D][C/gs][iters][gs][gs]
+//   EIGH           dwt_whiten_eigh_*: the exact ZCA basis, save = save_e [D][C/gs][gs+1][gs] (U, then lambda)
+// Both ZCA bases run their own dense pair in place of fwd_factor / bwd_coef; every other pass is the Cholesky basis's.
+struct Basis {
+  enum Kind { CHOLESKY, NEWTON_SCHULZ, EIGH } kind = CHOLESKY;
   int iters = 0;
-  const float* save_p = nullptr;   // [D][C/gs][iters][gs][gs]: written by the forward, read by the backward
+  const float* save = nullptr;     // written by the forward, read by the backward
+  bool zca() const { return kind != CHOLESKY; }
 };
 
-int zca_refuse(const Call& c) {
+int zca_refuse(const Call& c, const Basis& z) {
   const dwt::Geom& g = c.p.gm;
-  return fail(DWT_E_UNSUPPORTED, "the ZCA basis is built for the tensor-core kernels only: group_size 8, 16, 32, 64, HW >= 32 "
+  return fail(DWT_E_UNSUPPORTED, "the %s is built for the tensor-core kernels only: group_size 8, 16, 32, 64, HW >= 32 "
               "and a multiple of 4 (NCHW bf16: of 8), N*HW >= 4096 per domain, tensors 16-byte aligned (C=%d HW=%d N=%d gs=%d)",
-              g.C, g.HW, g.N, g.GS);
+              z.kind == Basis::EIGH ? "exact ZCA basis (eigendecomposition)" : "ZCA basis", g.C, g.HW, g.N, g.GS);
 }
 
 // a ZCA call's own arguments, and its family: validate()'s route, which must be the tensor-core one
-int zca_check(const Call& c, const Zca& z) {
-  if (z.iters < 1 || z.iters > DWT_ZCA_MAX_ITERATIONS)
+int zca_check(const Call& c, const Basis& z) {
+  const char* name = z.kind == Basis::EIGH ? "save_e" : "save_p";
+  if (z.kind == Basis::NEWTON_SCHULZ && (z.iters < 1 || z.iters > DWT_ZCA_MAX_ITERATIONS))
     return fail(DWT_E_INVALID, "iterations %d outside [1,%d]", z.iters, DWT_ZCA_MAX_ITERATIONS);
-  if (!z.save_p) return fail(DWT_E_INVALID, "null pointer argument (save_p)");
-  if ((uintptr_t)z.save_p % 16 != 0) return fail(DWT_E_INVALID, "save_p must be 16-byte aligned");
-  if (c.p.gm.GS > DWT_MAX_GROUP_SIZE || c.r.fam != TC) return zca_refuse(c);
+  if (!z.save) return fail(DWT_E_INVALID, "null pointer argument (%s)", name);
+  if ((uintptr_t)z.save % 16 != 0) return fail(DWT_E_INVALID, "%s must be 16-byte aligned", name);
+  if (c.p.gm.GS > DWT_MAX_GROUP_SIZE || c.r.fam != TC) return zca_refuse(c, z);
   return DWT_OK;
+}
+
+const char* zca_family(const Basis& z, bool bwd, bool bf16) {
+  if (z.kind == Basis::EIGH) return bwd ? fam(bf16, "dense_bwd_eigh", "dense_bwd_eigh_bf16") : fam(bf16, "dense_fwd_eigh", "dense_fwd_eigh_bf16");
+  return bwd ? fam(bf16, "dense_bwd_zca", "dense_bwd_zca_bf16") : fam(bf16, "dense_fwd_zca", "dense_fwd_zca_bf16");
+}
+
+void zca_fwd(const float* gram, const float* shift, const dwt::Geom& gm, const dwt::FwdFin& fin, const Basis& z, cudaStream_t st) {
+  if (z.kind == Basis::EIGH) dwt::dense_fwd_eigh(gram, shift, gm, fin, const_cast<float*>(z.save), st);
+  else dwt::dense_fwd_zca(gram, shift, gm, fin, z.iters, const_cast<float*>(z.save), st);
+}
+
+void zca_bwd(const float* rgram, const dwt::Geom& gm, const dwt::BwdFin& fin, const Basis& z, float* dybar, cudaStream_t st) {
+  if (z.kind == Basis::EIGH) dwt::dense_bwd_eigh(rgram, gm, fin, z.save, dybar, st);
+  else dwt::dense_bwd_zca(rgram, gm, fin, z.iters, z.save, dybar, st);
 }
 
 // The checks both directions make, in order; `own` holds the direction's own (residual, running buffers, gradient
@@ -505,7 +525,7 @@ int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, 
                     float b, float momentum, float unbias, int update_running, float* const* rmean,
                     float* const* rcov, const float* gamma, const float* beta, const float* residual,
                     uint8_t* relu_mask, int epi, float* save_mean, float* save_w, void* ws, size_t ws_bytes,
-                    cudaStream_t st, const Zca& zca = Zca{}) {
+                    cudaStream_t st, const Basis& zca = Basis{}) {
   Call c;
   const bool need_running = ((mode & 0xFF) == DWT_MODE_EVAL) || update_running;
   const int rc = validate(c, false, x, x, y, nullptr, N, C, HW, GS, D, mode, epi, gamma, beta, save_mean, save_w, ws, ws_bytes, [&] {
@@ -513,11 +533,11 @@ int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, 
     if (epi & DWT_EPI_RESIDUAL) if (int rc = check_align(c.bf16, (uintptr_t)residual, "residual")) return rc;
     if (relu_mask && !((epi & DWT_EPI_RESIDUAL) && c.nhwc))
       return fail(DWT_E_UNSUPPORTED, "the ReLU byte map is written by the channels-last RESIDUAL epilogue only");
-    if (zca.on) if (int rc = zca_check(c, zca)) return rc;
+    if (zca.zca()) if (int rc = zca_check(c, zca)) return rc;
     return check_running(need_running, rmean, rcov, D);
   });
   if (rc) return rc;
-  if (zca.on && c.r.fam != TC) return zca_refuse(c);   // the tensor-core kernels could not be set up: no tiled ZCA
+  if (zca.zca() && c.r.fam != TC) return zca_refuse(c, zca);   // the tensor-core kernels could not be set up: no tiled ZCA
   const Plan& p = c.p; const Workspace& w = c.w;
   const bool bf16 = c.bf16, nhwc = c.nhwc, train = c.mode == DWT_MODE_TRAIN;
   const dwt::FwdFin fin = make_fwd_fin(a, b, momentum, unbias, train ? update_running : 0, need_running, rmean, rcov,
@@ -546,7 +566,7 @@ int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, 
     }
     if (c.r.fam == CL || c.r.fam == TC) {   // the small and tiled kernels finalize in their last CTA
       if (int rc = check_launch(c.r.fam == CL ? "channels-last statistics kernel" : "tensor-core statistics kernel")) return rc;
-      Launch l(zca.on ? fam(bf16, "dense_fwd_zca", "dense_fwd_zca_bf16") : c.name(false, FINALIZE), &p.gm, 0.0, st);
+      Launch l(zca.zca() ? zca_family(zca, false, bf16) : c.name(false, FINALIZE), &p.gm, 0.0, st);
       if (c.r.fam == CL) {
         dwt::cl_fwd_finalize(w.partial, cp.nred, w.shift, p.gm, fin, st);
       } else {
@@ -554,13 +574,13 @@ int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, 
         if (gs128)
           dwt::dense_partial_reduce(w.partial + pair_part, tc_pair_chunks(p.gm, false), dwt::tc_superblocks(p.gm) / 2 * D,
                                     w.gram + (size_t)dwt::tc_superblocks(p.gm) * D * (64 * 64 + 64), st);
-        if (zca.on) dwt::dense_fwd_zca(w.gram, w.shift, p.gm, fin, zca.iters, const_cast<float*>(zca.save_p), st);
+        if (zca.zca()) zca_fwd(w.gram, w.shift, p.gm, fin, zca, st);
         else dwt::dense_fwd_factor(w.gram, w.shift, p.gm, fin, st);
       }
     }
-  } else if (zca.on) {
-    Launch l(fam(bf16, "dense_fwd_zca", "dense_fwd_zca_bf16"), &p.gm, 0.0, st);
-    dwt::dense_fwd_zca(nullptr, nullptr, p.gm, fin, zca.iters, const_cast<float*>(zca.save_p), st);
+  } else if (zca.zca()) {
+    Launch l(zca_family(zca, false, bf16), &p.gm, 0.0, st);
+    zca_fwd(nullptr, nullptr, p.gm, fin, zca, st);
   } else {
     Launch l(c.name(false, PREP), &p.gm, 0.0, st);
     if (c.r.fam == TC) dwt::dense_fwd_factor(nullptr, nullptr, p.gm, fin, st);
@@ -585,7 +605,7 @@ int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, 
 int whiten_like_bwd(const float* x, const float* dout, const float* dout2, float* dx, int64_t N, int64_t C, int64_t HW, int GS, int D,
                     int mode, float a, const float* save_mean, const float* save_w, const float* gamma,
                     const float* beta, const uint8_t* relu_mask, float* dresidual, int epi, float* dgamma,
-                    float* dbeta, void* ws, size_t ws_bytes, cudaStream_t st, const Zca& zca = Zca{}) {
+                    float* dbeta, void* ws, size_t ws_bytes, cudaStream_t st, const Basis& zca = Basis{}) {
   Call c;
   const int rc = validate(c, true, x, dout, dx, dout2, N, C, HW, GS, D, mode, epi, gamma, beta, save_mean, save_w, ws, ws_bytes, [&] {
     if (epi & DWT_EPI_RESIDUAL) {
@@ -599,11 +619,11 @@ int whiten_like_bwd(const float* x, const float* dout, const float* dout2, float
       return fail(DWT_E_INVALID, "relu_mask / dresidual belong to the RESIDUAL epilogue");
     }
     if ((dgamma == nullptr) != (dbeta == nullptr)) return fail(DWT_E_INVALID, "dgamma and dbeta go together");
-    if (zca.on) return zca_check(c, zca);
+    if (zca.zca()) return zca_check(c, zca);
     return DWT_OK;
   });
   if (rc) return rc;
-  if (zca.on && c.r.fam != TC) return zca_refuse(c);   // the tensor-core kernels could not be set up: no tiled ZCA
+  if (zca.zca() && c.r.fam != TC) return zca_refuse(c, zca);   // the tensor-core kernels could not be set up: no tiled ZCA
   const Plan& p = c.p; const Workspace& w = c.w;
   const bool bf16 = c.bf16, nhwc = c.nhwc;
   const dwt::BwdFin fin = make_bwd_fin(a, c.mode, epi, save_mean, save_w, gamma, dgamma, dbeta, w);
@@ -631,18 +651,18 @@ int whiten_like_bwd(const float* x, const float* dout, const float* dout2, float
     }
     if (c.r.fam == CL || c.r.fam == TC) {   // the small and tiled kernels finalize in their last CTA
       if (int rc = check_launch(c.r.fam == CL ? "channels-last backward reduction kernel" : "tensor-core backward reduction kernel")) return rc;
-      Launch l(zca.on ? fam(bf16, "dense_bwd_zca", "dense_bwd_zca_bf16") : c.name(true, FINALIZE), &p.gm, 0.0, st);
+      Launch l(zca.zca() ? zca_family(zca, true, bf16) : c.name(true, FINALIZE), &p.gm, 0.0, st);
       if (c.r.fam == CL) {
         dwt::cl_bwd_finalize(w.partial, cp.nred, p.gm, fin, st);
       } else {
         dwt::dense_partial_reduce(w.partial, rchunks, rproblems, w.gram, st);
-        if (zca.on) dwt::dense_bwd_zca(w.gram, p.gm, fin, zca.iters, zca.save_p, w.shift, st);
+        if (zca.zca()) zca_bwd(w.gram, p.gm, fin, zca, w.shift, st);
         else dwt::dense_bwd_coef(w.gram, p.gm, fin, w.shift, st);
       }
     }
-  } else if (zca.on) {
-    Launch l(fam(bf16, "dense_bwd_zca", "dense_bwd_zca_bf16"), &p.gm, 0.0, st);
-    dwt::dense_bwd_zca(nullptr, p.gm, fin, zca.iters, zca.save_p, w.shift, st);
+  } else if (zca.zca()) {
+    Launch l(zca_family(zca, true, bf16), &p.gm, 0.0, st);
+    zca_bwd(nullptr, p.gm, fin, zca, w.shift, st);
   } else {
     Launch l(c.name(true, PREP), &p.gm, 0.0, st);
     if (c.r.fam == TC) dwt::dense_bwd_coef(nullptr, p.gm, fin, w.shift, st);
@@ -820,7 +840,7 @@ int dwt_whiten_zca_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t H
                        size_t workspace_bytes, dwt_stream_t stream) {
   return whiten_like_fwd(x, y, N, C, HW, group_size, n_domains, mode, 1.f - eps, eps, momentum, 1.f, update_running,
                          running_mean, running_cov, nullptr, nullptr, nullptr, nullptr, 0, save_mean, save_w, workspace,
-                         workspace_bytes, (cudaStream_t)stream, Zca{true, iterations, save_p});
+                         workspace_bytes, (cudaStream_t)stream, Basis{Basis::NEWTON_SCHULZ, iterations, save_p});
 }
 
 int dwt_whiten_zca_bwd(const float* x, const float* dout, float* dx, int64_t N, int64_t C, int64_t HW, int group_size,
@@ -828,7 +848,24 @@ int dwt_whiten_zca_bwd(const float* x, const float* dout, float* dx, int64_t N, 
                        const float* save_p, void* workspace, size_t workspace_bytes, dwt_stream_t stream) {
   return whiten_like_bwd(x, dout, nullptr, dx, N, C, HW, group_size, n_domains, mode, 1.f - eps, save_mean, save_w, nullptr,
                          nullptr, nullptr, nullptr, 0, nullptr, nullptr, workspace, workspace_bytes, (cudaStream_t)stream,
-                         Zca{true, iterations, save_p});
+                         Basis{Basis::NEWTON_SCHULZ, iterations, save_p});
+}
+
+int dwt_whiten_eigh_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, int group_size, int n_domains, int mode,
+                        float eps, float momentum, int update_running, float* const* running_mean, float* const* running_cov,
+                        float* save_mean, float* save_w, float* save_e, void* workspace, size_t workspace_bytes,
+                        dwt_stream_t stream) {
+  return whiten_like_fwd(x, y, N, C, HW, group_size, n_domains, mode, 1.f - eps, eps, momentum, 1.f, update_running,
+                         running_mean, running_cov, nullptr, nullptr, nullptr, nullptr, 0, save_mean, save_w, workspace,
+                         workspace_bytes, (cudaStream_t)stream, Basis{Basis::EIGH, 0, save_e});
+}
+
+int dwt_whiten_eigh_bwd(const float* x, const float* dout, float* dx, int64_t N, int64_t C, int64_t HW, int group_size,
+                        int n_domains, int mode, float eps, const float* save_mean, const float* save_w, const float* save_e,
+                        void* workspace, size_t workspace_bytes, dwt_stream_t stream) {
+  return whiten_like_bwd(x, dout, nullptr, dx, N, C, HW, group_size, n_domains, mode, 1.f - eps, save_mean, save_w, nullptr,
+                         nullptr, nullptr, nullptr, 0, nullptr, nullptr, workspace, workspace_bytes, (cudaStream_t)stream,
+                         Basis{Basis::EIGH, 0, save_e});
 }
 
 // Batch norm is the group-size-1 member of the same family: "covariance" = biased variance,

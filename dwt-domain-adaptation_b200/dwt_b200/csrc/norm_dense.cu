@@ -10,6 +10,8 @@
 //   fwd_zca/bwd_zca  the same two steps in the ZCA basis (dwt_whiten_zca_*): W = P_T / sqrt(tr S) by T Newton-Schulz
 //                    iterations on shared-memory operands, and the reverse of that recursion; fwd_zca shares fwd_factor's
 //                    statistics prologue and EMA tail
+//   fwd_eigh/bwd_eigh  the exact ZCA basis (dwt_whiten_eigh_*): W = U diag(lambda^-1/2) U^T by a cyclic Jacobi
+//                    eigensolver in shared memory, and the Daleckii-Krein backward; the same prologue and EMA tail
 //
 // All three keep a 64x64 problem in ONE 256-thread CTA arranged 16x16, each thread owning a 4x4
 // register block.  fwd_factor runs the Cholesky factorisation AND the triangular inverse as one blocked
@@ -758,6 +760,266 @@ __global__ void __launch_bounds__(256) bwd_zca_kernel(const float* __restrict__ 
 }
 
 // ------------------------------------------------------------------------------------------
+// Exact ZCA basis (dwt_whiten_eigh_*): W = U diag(lambda^-1/2) U^T from S = U diag(lambda) U^T
+// Cyclic two-sided Jacobi in shared memory: one sweep is GS - 1 steps of the round-robin (circle) ordering, each step
+// GS/2 disjoint rotations at once with Rutishauser's formulas, U accumulates the rotations.  A rotation is skipped when
+// |a_pq| <= kJacobiTol sqrt(|a_pp a_qq|) (the relative criterion of positive definite Jacobi); the solver stops after
+// the first sweep that skips every rotation, or after kJacobiSweeps.  Every decision is a fixed function of the data:
+// reruns are bit-identical.  save_e [D][G][GS + 1][GS]: rows 0..GS-1 hold U (column j the eigenvector of lambda_j),
+// row GS holds lambda, in the order the sweeps leave them.
+// ------------------------------------------------------------------------------------------
+constexpr float kJacobiTol = 1.2e-7f;   // about FLT_EPSILON
+constexpr int kJacobiSweeps = 16;
+
+// pair k of step r of the circle method on n = GS indices: index n - 1 stays, the other n - 1 rotate; p < q
+__device__ __forceinline__ void jacobi_pair(int n, int r, int k, int& p, int& q) {
+  const int m = n - 1;
+  const int a = k == 0 ? r : (r + k) % m, b = k == 0 ? m : (r - k + m) % m;
+  p = a < b ? a : b;
+  q = a < b ? b : a;
+}
+
+struct JacobiSmem {
+  int p[kSB / 2], q[kSB / 2];
+  float c[kSB / 2], s[kSB / 2], t[kSB / 2];
+  int rot[2];                      // a rotation happened in the sweep of this parity
+};
+
+// Diagonalises the symmetric GS x GS matrix in sA in place (its diagonal ends as lambda) and leaves U in sU.  The
+// caller has published sA behind a block barrier; ends with one.
+__device__ void jacobi_eigh(float* sA, float* sU, int GS, JacobiSmem& js) {
+  const int np = GS >> 1, lnp = __ffs(np) - 1, lgs = __ffs(GS) - 1;
+  for (int e = threadIdx.x; e < GS * GS; e += blockDim.x) sU[(e >> lgs) * LDS + (e & (GS - 1))] = (e >> lgs) == (e & (GS - 1)) ? 1.f : 0.f;
+  if (threadIdx.x < 2) js.rot[threadIdx.x] = 0;
+  __syncthreads();
+  for (int sweep = 0; sweep < kJacobiSweeps; ++sweep) {
+    const int par = sweep & 1;
+    for (int r = 0; r < GS - 1; ++r) {
+      if ((int)threadIdx.x < np) {                    // the rotations of this step
+        int p, q;
+        jacobi_pair(GS, r, threadIdx.x, p, q);
+        const float app = sA[p * LDS + p], aqq = sA[q * LDS + q], apq = sA[p * LDS + q];
+        float c = 1.f, s = 0.f, tt = 0.f;
+        if (!(fabsf(apq) <= kJacobiTol * sqrtf(fabsf(app * aqq)))) {
+          const float theta = 0.5f * (aqq - app) / apq;
+          tt = copysignf(1.f, theta) / (fabsf(theta) + sqrtf(fmaf(theta, theta, 1.f)));   // the smaller root: |angle| <= pi/4
+          c = 1.f / sqrtf(fmaf(tt, tt, 1.f));
+          s = tt * c;
+          js.rot[par] = 1;
+        }
+        js.p[threadIdx.x] = p; js.q[threadIdx.x] = q;
+        js.c[threadIdx.x] = c; js.s[threadIdx.x] = s; js.t[threadIdx.x] = tt;
+      }
+      __syncthreads();
+      if (r == 0 && threadIdx.x == 0) js.rot[par ^ 1] = 0;   // every thread read it before the barrier above
+      // A <- J^T A J on the 2 x 2 blocks (pair k rows, pair l columns): disjoint, so in place
+      for (int b = threadIdx.x; b < np * np; b += blockDim.x) {
+        const int k = b >> lnp, l = b & (np - 1);
+        const int pk = js.p[k], qk = js.q[k], pl = js.p[l], ql = js.q[l];
+        const float ck = js.c[k], sk = js.s[k];
+        if (k == l) {                                 // Rutishauser: a_pp -= t a_pq, a_qq += t a_pq, a_pq = 0
+          if (sk == 0.f) continue;
+          const float apq = sA[pk * LDS + qk], tk = js.t[k];
+          sA[pk * LDS + pk] = fmaf(-tk, apq, sA[pk * LDS + pk]);
+          sA[qk * LDS + qk] = fmaf(tk, apq, sA[qk * LDS + qk]);
+          sA[pk * LDS + qk] = 0.f;
+          sA[qk * LDS + pk] = 0.f;
+          continue;
+        }
+        const float cl = js.c[l], sl = js.s[l];
+        const float a00 = sA[pk * LDS + pl], a01 = sA[pk * LDS + ql], a10 = sA[qk * LDS + pl], a11 = sA[qk * LDS + ql];
+        const float x00 = ck * a00 - sk * a10, x01 = ck * a01 - sk * a11;        // rows
+        const float x10 = sk * a00 + ck * a10, x11 = sk * a01 + ck * a11;
+        sA[pk * LDS + pl] = cl * x00 - sl * x01;                                 // columns
+        sA[pk * LDS + ql] = sl * x00 + cl * x01;
+        sA[qk * LDS + pl] = cl * x10 - sl * x11;
+        sA[qk * LDS + ql] = sl * x10 + cl * x11;
+      }
+      // U <- U J
+      for (int e = threadIdx.x; e < GS * np; e += blockDim.x) {
+        const int i = e & (GS - 1), k = e >> lgs;
+        const float sk = js.s[k];
+        if (sk == 0.f) continue;
+        const int pk = js.p[k], qk = js.q[k];
+        const float ck = js.c[k], up = sU[i * LDS + pk], uq = sU[i * LDS + qk];
+        sU[i * LDS + pk] = ck * up - sk * uq;
+        sU[i * LDS + qk] = sk * up + ck * uq;
+      }
+      __syncthreads();
+    }
+    if (!js.rot[par]) break;                          // final since the last barrier: every thread leaves together
+  }
+}
+
+// fwd_eigh: grid (G), 256 threads, domains in order with fwd_factor's statistics prologue and EMA tail.  A
+// non-finite S skips the solver; a non-finite or non-positive eigenvalue (an indefinite running buffer in eval, too)
+// flags the domain as a non-positive pivot does in fwd_factor (DWT_STATUS_NOT_PD, no EMA).  W = V V^T with
+// V = U diag(lambda^-1/4): symmetric bit for bit.
+__global__ void __launch_bounds__(256) fwd_eigh_kernel(const float* __restrict__ gram, const float* __restrict__ shift,
+                                                       const Geom gm, const FwdFin f, float* __restrict__ save_e) {
+  extern __shared__ __align__(16) float dsm[];
+  float* sA = dsm;                 // S, then diag(lambda) + rounding, then V
+  float* sU = sA + kMat;
+  __shared__ float sC[kMat];       // un-shrunk covariance (for the EMA)
+  __shared__ float sMean[kSB], sRow[kSB], sLam[kSB];
+  __shared__ JacobiSmem js;
+  __shared__ int sBad, sBadDom;
+  const int g = blockIdx.x, GS = gm.GS, nb = kSB / GS, sb = g / nb, o = (g % nb) * GS;
+  const Blk t(GS);
+  const int SB = (gm.C + kSB - 1) / kSB;
+  const float invM = 1.f / gm.M;
+  const int lgs = __ffs(GS) - 1;
+  if (threadIdx.x == 0) sBad = 0;
+  PROF_DECL;
+  PROF_MARK();
+  for (int d = 0; d < gm.D; ++d) {
+    const float* G = gram ? gram + ((size_t)d * SB + sb) * kNacc : nullptr;
+    const size_t gbase = ((size_t)d * gm.G + g) * GS * GS;
+    float* ed = save_e + ((size_t)d * gm.G + g) * (GS + 1) * GS;
+    float a[4][4], c[4][4];
+    EmaOld old;
+    domain_stats(G, shift, d, g, sb, o, SB, invM, gm, f, t, sC, sMean, sRow, sBadDom, a, old);
+    bool finite = true;
+#pragma unroll
+    for (int r = 0; r < 4; ++r)
+#pragma unroll
+      for (int s = 0; s < 4; ++s) finite = finite && isfinite(a[r][s]);
+    store_block(sA, t, a);
+    if (!finite) { sBad = 1; sBadDom = 1; }
+    __syncthreads();
+    PROF_MARK();
+    if (!sBadDom) jacobi_eigh(sA, sU, GS, js);        // block-uniform
+    PROF_MARK();
+    if ((int)threadIdx.x < GS) {
+      const float lam = sA[threadIdx.x * LDS + threadIdx.x];
+      sLam[threadIdx.x] = lam;
+      ed[GS * GS + threadIdx.x] = lam;
+      if (!(lam > 0.f && lam < INFINITY)) { sBad = 1; sBadDom = 1; }
+    }
+    __syncthreads();
+    for (int e = threadIdx.x; e < GS * GS; e += blockDim.x) {
+      const int i = e >> lgs, j = e & (GS - 1);
+      const float u = sBadDom ? NAN : sU[i * LDS + j];   // a skipped solver left no U
+      ed[e] = u;
+      sA[i * LDS + j] = u / sqrtf(sqrtf(sLam[j]));    // V = U lambda^-1/4
+    }
+    __syncthreads();
+    mm_block<false, true>(sA, sA, GS, t, c);          // W = V V^T
+    store_block_global(f.save_w + gbase, GS, t, c);
+    __syncthreads();                                  // sC complete, sBadDom final
+    if (old.on && !sBadDom) domain_ema(d, g, gm, f, sC, sMean, old);
+    __syncthreads();      // also orders this domain's buffer writes before the next domain's reads (aliasing)
+    PROF_MARK();
+  }
+  PROF_DUMP("fwd_eigh load|solve|save+ema");
+  if (threadIdx.x == 0 && sBad) atomicOr(f.status, DWT_STATUS_NOT_PD);
+}
+
+// bwd_eigh: grid (G, 1, D), 256 threads.  From dL/dW = R = sum dy xc^T by the Daleckii-Krein formula:
+//   G = dL/dS = U [(U^T R U) o F] U^T,  F_ij = -1 / (sqrt(l_i) sqrt(l_j) (sqrt(l_i) + sqrt(l_j)))
+// F is the divided difference of l^-1/2 without its cancellation: finite at equal eigenvalues (-l^-3/2 / 2).  Then as
+// bwd_zca: Bm = (a/M)(G + G^T), A1 = W^T (full), cvec; eval (rgram null): A1 = W^T, Bm = 0.  Four products.
+__global__ void __launch_bounds__(256) bwd_eigh_kernel(const float* __restrict__ rgram, const Geom gm, const BwdFin f,
+                                                       const float* __restrict__ save_e, float* __restrict__ dybar) {
+  extern __shared__ __align__(16) float dsm[];
+  float* sW = dsm;
+  float* sU = sW + kMat;
+  float* sR = sU + kMat;           // R; at the end G
+  float* sT1 = sR + kMat;          // R U, then U H
+  float* sH = sT1 + kMat;          // H = (U^T R U) o F; at the end Bm
+  __shared__ float sSdz[kSB], sMu[kSB], sRl[kSB];
+  const int g = blockIdx.x, d = blockIdx.z, GS = gm.GS, nb = kSB / GS, sb = g / nb, o = (g % nb) * GS;
+  const Blk t(GS);
+  const int SB = (gm.C + kSB - 1) / kSB;
+  const bool train = f.mode == DWT_MODE_TRAIN && rgram != nullptr;
+  const float* G = train ? rgram + ((size_t)d * SB + sb) * kNacc : nullptr;
+  const size_t gbase = ((size_t)d * gm.G + g) * GS * GS;
+  const float* ed = save_e + ((size_t)d * gm.G + g) * (GS + 1) * GS;
+  float* coef = f.coef + ((size_t)d * gm.G + g) * coef_stride(GS);
+  const int gsh = __ffs(GS) - 1;
+  const float invM = 1.f / gm.M;
+  constexpr int kPer = kSB * kSB / 256;
+  PROF_DECL;
+  PROF_MARK();
+  float wv[kPer], rv[kPer], uv[kPer];
+#pragma unroll
+  for (int n = 0; n < kPer; ++n) {
+    const int e = threadIdx.x + 256 * n, i = e >> gsh, j = e & (GS - 1);
+    const bool in = e < GS * GS;
+    wv[n] = in ? f.save_w[gbase + e] : 0.f;
+    rv[n] = (in && train) ? __ldcg(G + (o + i) * kSB + o + j) : 0.f;
+    uv[n] = (in && train) ? ed[e] : 0.f;
+  }
+  float sdz = 0.f, mu = 0.f, lam = 1.f;
+  if ((int)threadIdx.x < GS) {
+    sdz = train ? __ldcg(G + kSB * kSB + o + threadIdx.x) : 0.f;
+    mu = f.save_mean[(size_t)d * gm.C + g * GS + threadIdx.x];
+    if (train) lam = ed[GS * GS + threadIdx.x];
+  }
+#pragma unroll
+  for (int n = 0; n < kPer; ++n) {
+    const int e = threadIdx.x + 256 * n, i = e >> gsh, j = e & (GS - 1);
+    if (e < GS * GS) { sW[i * LDS + j] = wv[n]; sR[i * LDS + j] = rv[n]; sU[i * LDS + j] = uv[n]; }
+  }
+  if ((int)threadIdx.x < GS) {
+    sSdz[threadIdx.x] = sdz * invM;                   // mean_M dy (0 in eval mode)
+    sMu[threadIdx.x] = mu;
+    sRl[threadIdx.x] = sqrtf(lam);
+    if (dybar) dybar[((size_t)d * SB + sb) * kSB + o + threadIdx.x] = sdz * invM;
+  }
+  __syncthreads();
+  PROF_MARK();
+  if (train) {
+    float c[4][4];
+    mm_block<false, false>(sR, sU, GS, t, c);         // R U
+    store_block(sT1, t, c);
+    __syncthreads();
+    mm_block<true, false>(sU, sT1, GS, t, c);         // U^T R U, times F
+#pragma unroll
+    for (int r = 0; r < 4; ++r)
+#pragma unroll
+      for (int s = 0; s < 4; ++s) {
+        const float ri = sRl[4 * t.bi + r], rj = sRl[4 * t.bj + s];
+        c[r][s] = -c[r][s] / (ri * rj * (ri + rj));
+      }
+    store_block(sH, t, c);
+    __syncthreads();
+    mm_block<false, false>(sU, sH, GS, t, c);         // U H (every read of sT1 was before the barrier above)
+    store_block(sT1, t, c);
+    __syncthreads();
+    mm_block<false, true>(sT1, sU, GS, t, c);         // G = U H U^T (R is dead)
+    store_block(sR, t, c);
+    __syncthreads();
+  }
+  PROF_MARK();
+  const float sc = f.a * invM;
+#pragma unroll
+  for (int n = 0; n < kPer; ++n) {
+    const int e = threadIdx.x + 256 * n, i = e >> gsh, j = e & (GS - 1);
+    if (e < GS * GS) {
+      const float bm = train ? sc * (sR[i * LDS + j] + sR[j * LDS + i]) : 0.f;
+      coef[e] = sW[j * LDS + i];                      // A1 = W^T, every element
+      coef[GS * GS + e] = bm;
+      sH[i * LDS + j] = bm;
+    }
+  }
+  __syncthreads();
+  // cvec_i = -(sum_j W_ji mean(dy)_j + sum_j Bm_ij mu_j): 4 threads per row, partial sums met by shuffle
+  {
+    const int i = threadIdx.x >> 2, q = threadIdx.x & 3;
+    float cv = 0.f;
+    if (train && i < GS) {
+      for (int j = q; j < GS; j += 4) cv = fmaf(sW[j * LDS + i], sSdz[j], fmaf(sH[i * LDS + j], sMu[j], cv));
+    }
+    cv += __shfl_xor_sync(0xffffffffu, cv, 1);
+    cv += __shfl_xor_sync(0xffffffffu, cv, 2);
+    if (q == 0 && i < GS) coef[2 * GS * GS + i] = -cv;
+  }
+  PROF_MARK();
+  PROF_DUMP("bwd_eigh load|solve|tail");
+}
+
+// ------------------------------------------------------------------------------------------
 // group size 128: one 1024-thread CTA per group runs the shared-memory routines of dwt_common.cuh (fwd_factor_block:
 // right-looking Cholesky + forward-substitution inverse; bwd_finalize_block: P, T = W^T P, S' = T W, A1, Bm) on the
 // whole 128 x 128 matrix, assembled from the 64 x 64 blocks the tensor-core contractions reduced.  Three matrices of
@@ -855,6 +1117,8 @@ constexpr size_t kFactorSmem = 0;   // fwd_factor: static shared memory only (pa
 constexpr size_t kCoefSmem = sizeof(float) * 4 * kMat;
 constexpr size_t kZcaFwdSmem = sizeof(float) * 4 * kMat;   // N, P, P^2, P^3 (66.6 KB; + 16.9 KB static)
 constexpr size_t kZcaBwdSmem = sizeof(float) * 8 * kMat;   // W, N, Q, P, P^2, Q N, P^3, P Q N (133 KB)
+constexpr size_t kEighFwdSmem = sizeof(float) * 2 * kMat;  // S / V, U (33.3 KB; + 17.6 KB static)
+constexpr size_t kEighBwdSmem = sizeof(float) * 5 * kMat;  // W, U, R / G, R U / U H, H / Bm (83.2 KB)
 
 }  // namespace
 
@@ -865,6 +1129,8 @@ int dense_init() {
   if (e == cudaSuccess) e = cudaFuncSetAttribute(bwd_coef128_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kCoef2Smem);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(fwd_zca_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kZcaFwdSmem);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(bwd_zca_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kZcaBwdSmem);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(fwd_eigh_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kEighFwdSmem);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(bwd_eigh_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kEighBwdSmem);
   return (int)e;
 }
 
@@ -901,6 +1167,14 @@ void dense_fwd_zca(const float* gram, const float* shift, const Geom& gm, const 
 void dense_bwd_zca(const float* rgram, const Geom& gm, const BwdFin& fin, int iters, const float* save_p, float* dybar,
                    cudaStream_t st) {
   bwd_zca_kernel<<<dim3(gm.G, 1, gm.D), 256, kZcaBwdSmem, st>>>(rgram, gm, fin, iters, save_p, dybar);
+}
+
+void dense_fwd_eigh(const float* gram, const float* shift, const Geom& gm, const FwdFin& fin, float* save_e, cudaStream_t st) {
+  fwd_eigh_kernel<<<gm.G, 256, kEighFwdSmem, st>>>(gram, shift, gm, fin, save_e);
+}
+
+void dense_bwd_eigh(const float* rgram, const Geom& gm, const BwdFin& fin, const float* save_e, float* dybar, cudaStream_t st) {
+  bwd_eigh_kernel<<<dim3(gm.G, 1, gm.D), 256, kEighBwdSmem, st>>>(rgram, gm, fin, save_e, dybar);
 }
 
 }  // namespace dwt

@@ -69,6 +69,10 @@ void dense_fwd_zca(const float* gram, const float* shift, const Geom& gm, const 
                    cudaStream_t st);
 void dense_bwd_zca(const float* rgram, const Geom& gm, const BwdFin& fin, int iters, const float* save_p, float* dybar,
                    cudaStream_t st);
+// exact ZCA basis, group sizes 8..64: W = U diag(lambda^-1/2) U^T by a Jacobi eigensolver.  save_e [D][G][GS+1][GS]
+// (U, then lambda) is written by the forward and read by the backward; both leave what dense_fwd_factor / dense_bwd_coef leave.
+void dense_fwd_eigh(const float* gram, const float* shift, const Geom& gm, const FwdFin& fin, float* save_e, cudaStream_t st);
+void dense_bwd_eigh(const float* rgram, const Geom& gm, const BwdFin& fin, const float* save_e, float* dybar, cudaStream_t st);
 
 // TMA + wgmma apply path (norm_tc_apply.cu): split-TF32 GEMM of the block-diagonal group matrices
 int tc_apply_init();

@@ -98,7 +98,8 @@ class _NormFunction(torch.autograd.Function):
     x is [n_domains*N, C, *]; `running` is a list of n_domains (mean, second-moment) buffer pairs
     (entries may alias); gamma/beta are [C]-sized or None; relu fuses max(.,0) behind the affine; r: route() of the call;
     iterations: 0 for the Cholesky basis, else the Newton-Schulz iterations of the ZCA basis (dwt_whiten_zca_*, whitening
-    without gamma/beta or residual; the per-group matrices of the iteration are saved for backward).
+    without gamma/beta or residual; the per-group matrices of the iteration are saved for backward), or nv.EIGH for the
+    exact ZCA basis (dwt_whiten_eigh_*; the per-group eigenvectors and eigenvalues are saved for backward).
     """
 
     @staticmethod
@@ -139,13 +140,21 @@ class _NormFunction(torch.autograd.Function):
         mask = torch.empty(x.numel() // 4, dtype=torch.uint8, device=dev) if (residual is not None and r.nhwc) else None
         save_mean = torch.empty(n_domains, c, dtype=torch.float32, device=dev)
         save_w = torch.empty(n_domains, c // gs, gs, gs, dtype=torch.float32, device=dev)
-        save_p = torch.empty(n_domains, c // gs, iterations, gs, gs, dtype=torch.float32, device=dev) if iterations else None
+        exact = iterations == nv.EIGH
+        if exact:                                    # save_e: U, then the eigenvalues
+            save_p = torch.empty(n_domains, c // gs, gs + 1, gs, dtype=torch.float32, device=dev)
+        else:
+            save_p = torch.empty(n_domains, c // gs, iterations, gs, gs, dtype=torch.float32, device=dev) if iterations else None
         ws = nv.workspace(dev, n, c, hw, gs, n_domains)
         need_running = (mode == nv.MODE_EVAL) or update_running
         rm = nv.ptr_array([p[0] for p in running]) if need_running else None
         rv = nv.ptr_array([p[1] for p in running]) if need_running else None
         with torch.cuda.device(dev):
-            if iterations:
+            if exact:
+                rc = lib.dwt_whiten_eigh_fwd(nv.ptr(x), nv.ptr(y), n, c, hw, gs, n_domains, mode | layout, eps, momentum,
+                                             int(update_running), rm, rv, nv.ptr(save_mean), nv.ptr(save_w), nv.ptr(save_p),
+                                             nv.ptr(ws), ws.numel(), nv.stream_ptr(dev))
+            elif iterations:
                 rc = lib.dwt_whiten_zca_fwd(nv.ptr(x), nv.ptr(y), n, c, hw, gs, n_domains, mode | layout, eps, momentum,
                                             int(update_running), rm, rv, int(iterations), nv.ptr(save_mean), nv.ptr(save_w),
                                             nv.ptr(save_p), nv.ptr(ws), ws.numel(), nv.stream_ptr(dev))
@@ -231,7 +240,11 @@ class _NormFunction(torch.autograd.Function):
         dbeta = torch.empty(c, dtype=torch.float32, device=dev) if want_affine else None
         ws = nv.workspace(dev, n, c, hw, gs, n_domains)
         with torch.cuda.device(dev):
-            if ctx.iterations:
+            if ctx.iterations == nv.EIGH:
+                rc = lib.dwt_whiten_eigh_bwd(nv.ptr(x), nv.ptr(dout), nv.ptr(dx), n, c, hw, gs, n_domains, mode, eps,
+                                             nv.ptr(save_mean), nv.ptr(save_w), nv.ptr(save_p), nv.ptr(ws), ws.numel(),
+                                             nv.stream_ptr(dev))
+            elif ctx.iterations:
                 rc = lib.dwt_whiten_zca_bwd(nv.ptr(x), nv.ptr(dout), nv.ptr(dx), n, c, hw, gs, n_domains, mode, eps,
                                             int(ctx.iterations), nv.ptr(save_mean), nv.ptr(save_w), nv.ptr(save_p),
                                             nv.ptr(ws), ws.numel(), nv.stream_ptr(dev))
@@ -386,9 +399,10 @@ _ACT_DTYPES = (torch.float32, torch.bfloat16)
 
 def norm(x, gamma, beta, *, kind, group_size, n_domains, training_stats, eps, momentum, update_running,
          running, relu=False, residual=None, iterations=0):
-    """iterations: 0 whitens in the Cholesky basis; 1..16 in the ZCA basis by that many Newton-Schulz iterations (the
-    tensor-core kernels only: a call they cannot take raises NativeError, it is never sent to another family)."""
-    if iterations and not 1 <= iterations <= nv.ZCA_MAX_ITERATIONS:
+    """iterations: 0 whitens in the Cholesky basis; 1..16 in the ZCA basis by that many Newton-Schulz iterations;
+    nv.EIGH ("eigh") in the exact ZCA basis by eigendecomposition (both ZCA bases: the tensor-core kernels only, a call
+    they cannot take raises NativeError, it is never sent to another family or basis)."""
+    if iterations != nv.EIGH and iterations and not 1 <= iterations <= nv.ZCA_MAX_ITERATIONS:
         raise ValueError(f"iterations must be in [1, {nv.ZCA_MAX_ITERATIONS}] (got {iterations})")
     mode = nv.MODE_TRAIN if training_stats else nv.MODE_EVAL
     args = (kind, group_size, n_domains, mode, float(eps), float(momentum), bool(update_running), running, bool(relu))

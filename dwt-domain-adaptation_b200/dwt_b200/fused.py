@@ -12,8 +12,9 @@ target-aug in order so aliased buffers end exactly as after three sequential mod
 for the residual tail, the gradient of the identity branch.
 
 It owns no state: it borrows the running buffers of the three domain modules at call time, and with them their
-hyper-parameters -- eps, momentum and, for whitening, the basis: three ``ZCAWTransform2d`` modules make a ZCA site
-(the tensor-core kernels, no fused epilogue), and modules that disagree on the basis are refused.
+hyper-parameters -- eps, momentum and, for whitening, the basis: three ``ZCAWTransform2d`` modules make a ZCA site,
+three ``ExactZCAWTransform2d`` modules an exact-ZCA site (both on the tensor-core kernels, no fused epilogue), and
+modules that disagree on the basis are refused.
 
 ``replicated=True`` is the statistics-collection pass (SURVEY.md §8f-3;
 resnet50_dwt_mec_officehome.py:380-389): the reference feeds ``cat((data, data, data))`` through
@@ -84,13 +85,14 @@ class DomainTripleNorm(nn.Module):
                       running=running, relu=relu, residual=residual)
 
     def _iterations(self, mods):
-        """The whitening basis the domain modules share (functional.norm's iterations: 0 = Cholesky)."""
+        """The whitening basis the domain modules share (functional.norm's iterations: 0 = Cholesky, "eigh" = exact ZCA)."""
         if self.kind != "whiten":
             return 0
         basis = {m._iterations() if isinstance(m, _Whitening) else 0 for m in mods}
         if len(basis) != 1:
-            raise ValueError("the domain modules of a whitening site must share one basis (WTransform2d, or "
-                             f"ZCAWTransform2d with one number of iterations); got iterations {sorted(basis)}")
+            raise ValueError("the domain modules of a whitening site must share one basis (WTransform2d, "
+                             "ExactZCAWTransform2d, or ZCAWTransform2d with one number of iterations); got iterations "
+                             f"{sorted(basis, key=str)}")
         iterations = basis.pop()
         if iterations and self.kernel_epilogue:
             raise nv.NativeError("the ZCA basis runs on the tensor-core kernels: group_size 8, 16, 32, 64 "

@@ -47,8 +47,8 @@ class _Whitening(nn.Module):
         raise NotImplementedError
 
     def _iterations(self):
-        """Newton-Schulz iterations of the whitening basis: 0 is the inverse Cholesky factor (the ZCA layer, zca.py,
-        returns its own)."""
+        """The whitening basis as functional.norm's `iterations`: 0 is the inverse Cholesky factor (the ZCA layers,
+        zca.py, return their Newton-Schulz iterations or "eigh")."""
         return 0
 
     def forward(self, x):

@@ -10,9 +10,11 @@ and y = W (x - mean).  At a finite T this is IterNorm's partial whitening (W -> 
 the exact gradient of that function.  The running buffers receive the same EMA of the un-shrunk covariance as
 ``WTransform2d``'s, bit for bit, so state dicts load into either class.
 
-The layer runs on the tensor-core kernels only (dwt_whiten_zca_fwd / _bwd): group sizes 8, 16, 32, 64, H*W >= 32 and a
+``ExactZCAWTransform2d`` computes the same basis exactly, W = S^-1/2 by an eigendecomposition of S.
+
+Both layers run on the tensor-core kernels only (dwt_whiten_zca_* / dwt_whiten_eigh_*): group sizes 8, 16, 32, 64, H*W >= 32 and a
 multiple of 4, at least 4096 samples per domain.  Anything else raises ``NativeError``; nothing falls back to another
-basis or family.  It lives outside whitening.py because the reference-facing ``whitening`` shim star-imports that file.
+basis or family.  They live outside whitening.py because the reference-facing ``whitening`` shim star-imports that file.
 """
 from __future__ import annotations
 
@@ -36,3 +38,23 @@ class ZCAWTransform2d(_Whitening):
 
     def extra_repr(self):
         return f"{self.num_features}, group_size={self.group_size}, iterations={self.iterations}"
+
+
+class ExactZCAWTransform2d(_Whitening):
+    """Whitening in the exact ZCA basis: W = S^-1/2 = U diag(lambda^-1/2) U^T from the eigendecomposition
+    S = U diag(lambda) U^T of S = (1 - eps) cov + eps I, and y = W (x - mean) (decorrelated batch norm's whitening).
+
+    ``WTransform2d``'s constructor, buffers, attributes, error texts and running-statistic updates (bit for bit, so state
+    dicts load into any of the three classes).  Unlike ``ZCAWTransform2d``'s finite Newton-Schulz iteration, the output
+    is white at every condition number; the price is an iterative eigensolver per group (dwt_whiten_eigh_fwd, a cyclic
+    Jacobi method) in place of a fixed number of matrix products.  The backward is the exact gradient of S^-1/2
+    (Daleckii-Krein), finite for repeated eigenvalues.  A group whose S is not positive definite -- in eval mode, an
+    indefinite running buffer -- sets the not-positive-definite status, as in ``WTransform2d``.  Same tensor-core-only
+    geometry as ``ZCAWTransform2d``.
+    """
+
+    _check_input_dim = WTransform2d._check_input_dim
+    _check_group_size = WTransform2d._check_group_size
+
+    def _iterations(self):
+        return nv.EIGH

@@ -18,6 +18,7 @@
  *                     resnet50_dwt_mec_officehome.py:59-63,220-222, when asked)
  *   dwt_whiten_bwd   autograd through the above     utils/whitening.py:41-55
  *   dwt_whiten_zca_fwd/bwd  the same layer in the ZCA basis (Newton-Schulz iteration; not in the reference)
+ *   dwt_whiten_eigh_fwd/bwd the same layer in the exact ZCA basis (Jacobi eigendecomposition; not in the reference)
  *   dwt_bn_fwd/bwd   _BatchNorm.forward             utils/batch_norm.py:54-69
  *   dwt_tail2_fwd/bwd  the residual tail of a downsampling Bottleneck: two norm sites and the ReLU in one pass
  *                    resnet50_dwt_mec_officehome.py:236-240
@@ -206,6 +207,32 @@ DWT_API int dwt_whiten_zca_fwd(const float *x, float *y, int64_t N, int64_t C, i
 DWT_API int dwt_whiten_zca_bwd(const float *x, const float *dout, float *dx, int64_t N, int64_t C, int64_t HW, int group_size,
                        int n_domains, int mode, float eps, int iterations, const float *save_mean, const float *save_w,
                        const float *save_p, void *workspace, size_t workspace_bytes, dwt_stream_t stream);
+
+/*
+ * Whitening in the exact ZCA basis (decorrelated batch norm): W = S^-1/2 = U diag(lambda^-1/2) U^T from the
+ * eigendecomposition S = U diag(lambda) U^T, with S = (1-eps) cov + eps I as in dwt_whiten_fwd, and y = W (x - mean).
+ * Unlike dwt_whiten_zca_fwd's finite Newton-Schulz iteration this whitens fully at every condition number: the output
+ * covariance is S^-1/2 cov S^-1/2, which tends to I as eps -> 0.  A cyclic Jacobi eigensolver diagonalises S in float32 per group; it stops after the
+ * first sweep that rotates nothing, at most 16 sweeps, and reruns are bit-identical.  W = V V^T with
+ * V = U diag(lambda^-1/4) is symmetric bit for bit.  dwt_whiten_eigh_bwd differentiates W(S) by the Daleckii-Krein
+ * formula  dL/dS = U [(U^T R U) o F] U^T,  F_ij = -1 / (sqrt(l_i) sqrt(l_j) (sqrt(l_i) + sqrt(l_j))),  R = dL/dW, which
+ * is finite for repeated eigenvalues.
+ *   save_e      [n_domains, C/gs, gs + 1, gs], 16-byte aligned (else DWT_E_INVALID): rows 0..gs-1 hold U (column j the
+ *               eigenvector of lambda_j), row gs holds lambda; written by fwd, read by bwd
+ *   everything else as dwt_whiten_zca_fwd / dwt_whiten_zca_bwd without iterations: the same statistics, running-buffer
+ *   EMA (bit for bit dwt_whiten_fwd's), geometry, layouts, dtypes and workspace.  Every other group size (1, 2, 4, 128)
+ *   or geometry is DWT_E_UNSUPPORTED with a text naming the exact ZCA basis.
+ * Status: a non-finite S, or an eigenvalue that is not finite and positive, sets DWT_STATUS_NOT_PD and skips that
+ * domain's EMA; in eval mode this also catches an indefinite running buffer.
+ * Profile families dense_fwd_eigh / dense_bwd_eigh (_bf16) for the per-group algebra; the other passes keep tc_*.
+ */
+DWT_API int dwt_whiten_eigh_fwd(const float *x, float *y, int64_t N, int64_t C, int64_t HW, int group_size, int n_domains,
+                       int mode, float eps, float momentum, int update_running, float *const *running_mean,
+                       float *const *running_cov, float *save_mean, float *save_w, float *save_e,
+                       void *workspace, size_t workspace_bytes, dwt_stream_t stream);
+DWT_API int dwt_whiten_eigh_bwd(const float *x, const float *dout, float *dx, int64_t N, int64_t C, int64_t HW, int group_size,
+                       int n_domains, int mode, float eps, const float *save_mean, const float *save_w,
+                       const float *save_e, void *workspace, size_t workspace_bytes, dwt_stream_t stream);
 
 /*
  * Domain batch norm (F.batch_norm semantics): biased batch variance normalises,

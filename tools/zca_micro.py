@@ -7,10 +7,13 @@ microbench builds it.  Arms, alternated round by round in one process:
   chol        WTransform2d (the inverse Cholesky factor), CUDA-graph replay;
   zca_t5      ZCAWTransform2d, 5 Newton-Schulz iterations (the default), CUDA-graph replay;
   zca_t16     ZCAWTransform2d, 16 iterations, CUDA-graph replay;
+  exact       ExactZCAWTransform2d (Jacobi eigendecomposition), CUDA-graph replay;
+  exact_bf16  ExactZCAWTransform2d on bfloat16 x and dy, CUDA-graph replay;
   aten_t5     the same ZCA function as an ATen op sequence (tests/support/zca_reference.py: mean, bmm, the iterations,
               a grouped 1x1 convolution; autograd backward) in float32 on the same GPU, CUDA-graph replay.
-Per library arm: the kernel families from one eager profiled pass (ms per iteration), dense_*_zca among them.  The
-card's name and power limit are read in the same process.
+Per library arm: the kernel families from one eager profiled pass (ms per iteration), dense_*_zca / dense_*_eigh among
+them, and the share of the basis's dense kernels (partial reduction + per-group algebra) in that pass.  The card's name
+and power limit are read in the same process.
 """
 from __future__ import annotations
 
@@ -89,15 +92,20 @@ def main():
     x = (torch.einsum("dc,nchw->ndhw", mix, torch.randn(N, C, H, H, device=dev)) + 2.0).contiguous()
     dy = torch.randn(N, C, H, H, device=dev)
     mods = {"chol": dwt_b200.WTransform2d(C, GS), "zca_t5": dwt_b200.ZCAWTransform2d(C, GS, iterations=5),
-            "zca_t16": dwt_b200.ZCAWTransform2d(C, GS, iterations=16)}
+            "zca_t16": dwt_b200.ZCAWTransform2d(C, GS, iterations=16), "exact": dwt_b200.ExactZCAWTransform2d(C, GS),
+            "exact_bf16": dwt_b200.ExactZCAWTransform2d(C, GS)}
     arms, recs = {}, {}
     for name, m in mods.items():
-        step = _step_fn(m.to(dev).train(), x, dy)
+        bf16 = name.endswith("_bf16")
+        step = _step_fn(m.to(dev).train(), x.bfloat16() if bf16 else x, dy.bfloat16() if bf16 else dy)
         for _ in range(args.warmup):
             step()
         fams = _families(step, args.steps)
         arms[name] = _graphed(step, dev)
-        recs[name] = {"kernels_ms": fams, "kernel_ms_per_iter": round(sum(fams.values()), 4), "ms_per_iter": []}
+        total = sum(fams.values())
+        dense = sum(v for f, v in fams.items() if f.startswith("dense_"))
+        recs[name] = {"kernels_ms": fams, "kernel_ms_per_iter": round(total, 4), "dense_share": round(dense / total, 3),
+                      "ms_per_iter": []}
     aten = _step_fn(lambda xi: zca_reference.zca_torch(xi, GS, 5)[0], x, dy)
     for _ in range(args.warmup):
         aten()
@@ -117,6 +125,7 @@ def main():
         "steps": args.steps, "rounds": args.rounds, "arms": recs,
         "zca_t5_over_chol_ms": round(med["zca_t5"] - med["chol"], 4),
         "zca_t16_over_chol_ms": round(med["zca_t16"] - med["chol"], 4),
+        "exact_over_chol_ms": round(med["exact"] - med["chol"], 4),
         "speedup_over_aten_t5": round(med["aten_t5"] / med["zca_t5"], 2),
     }))
 
