@@ -8,6 +8,7 @@ from . import _native
 from ._native import NotPositiveDefiniteError, check_status, raise_on_status
 from .augment import PairedAugment, draw_params
 from .batch_norm import BatchNorm1d, BatchNorm2d, BatchNorm3d
+from .coloring import WCTransform2d
 from .consensus_loss import HeadLoss, MinEntropyConsensusLoss
 from .functional import fork_for_sum
 from .fused import DomainTripleNorm
@@ -15,6 +16,6 @@ from .pooling import MaxPool2d
 from .whitening import WTransform2d
 from .zca import ExactZCAWTransform2d, ZCAWTransform2d
 
-__all__ = ["WTransform2d", "ZCAWTransform2d", "ExactZCAWTransform2d", "BatchNorm1d", "BatchNorm2d", "BatchNorm3d", "MinEntropyConsensusLoss",
+__all__ = ["WTransform2d", "ZCAWTransform2d", "ExactZCAWTransform2d", "WCTransform2d", "BatchNorm1d", "BatchNorm2d", "BatchNorm3d", "MinEntropyConsensusLoss",
            "DomainTripleNorm", "fork_for_sum", "HeadLoss", "MaxPool2d", "PairedAugment", "draw_params", "raise_on_status", "check_status",
            "NotPositiveDefiniteError", "_native"]

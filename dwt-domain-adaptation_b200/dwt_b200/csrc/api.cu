@@ -446,44 +446,70 @@ struct Call {
 //   CHOLESKY       dwt_whiten_*, dwt_bn_* (nothing saved beyond save_w)
 //   NEWTON_SCHULZ  dwt_whiten_zca_*: `iters` iterations, save = save_p [D][C/gs][iters][gs][gs]
 //   EIGH           dwt_whiten_eigh_*: the exact ZCA basis, save = save_e [D][C/gs][gs+1][gs] (U, then lambda)
-// Both ZCA bases run their own dense pair in place of fwd_factor / bwd_coef; every other pass is the Cholesky basis's.
+//   COLOR          dwt_whiten_color_*: the Cholesky basis coloured, y = color W (x - mean) + bias; color W goes to the
+//                  workspace's coefficient area (w.coef, unused by a forward), bias into the apply's accumulator
+// All but CHOLESKY run their own dense pair in place of fwd_factor / bwd_coef; every other pass is the Cholesky basis's.
 struct Basis {
-  enum Kind { CHOLESKY, NEWTON_SCHULZ, EIGH } kind = CHOLESKY;
+  enum Kind { CHOLESKY, NEWTON_SCHULZ, EIGH, COLOR } kind = CHOLESKY;
   int iters = 0;
   const float* save = nullptr;     // written by the forward, read by the backward
-  bool zca() const { return kind != CHOLESKY; }
+  const float* color = nullptr;    // COLOR: [C/gs][gs][gs] and [C]
+  const float* bias = nullptr;
+  float* dcolor = nullptr;         // COLOR backward: both or neither
+  float* dbias = nullptr;
+  bool own() const { return kind != CHOLESKY; }
 };
 
-int zca_refuse(const Call& c, const Basis& z) {
-  const dwt::Geom& g = c.p.gm;
+int basis_refuse(const Basis& z, int64_t N, int64_t C, int64_t HW, int GS) {
   return fail(DWT_E_UNSUPPORTED, "the %s is built for the tensor-core kernels only: group_size 8, 16, 32, 64, HW >= 32 "
-              "and a multiple of 4 (NCHW bf16: of 8), N*HW >= 4096 per domain, tensors 16-byte aligned (C=%d HW=%d N=%d gs=%d)",
-              z.kind == Basis::EIGH ? "exact ZCA basis (eigendecomposition)" : "ZCA basis", g.C, g.HW, g.N, g.GS);
+              "and a multiple of 4 (NCHW bf16: of 8), N*HW >= 4096 per domain, tensors 16-byte aligned (C=%lld HW=%lld N=%lld gs=%d)",
+              z.kind == Basis::EIGH ? "exact ZCA basis (eigendecomposition)" : z.kind == Basis::COLOR ? "colouring transform" : "ZCA basis",
+              (long long)C, (long long)HW, (long long)N, GS);
 }
 
-// a ZCA call's own arguments, and its family: validate()'s route, which must be the tensor-core one
-int zca_check(const Call& c, const Basis& z) {
-  const char* name = z.kind == Basis::EIGH ? "save_e" : "save_p";
-  if (z.kind == Basis::NEWTON_SCHULZ && (z.iters < 1 || z.iters > DWT_ZCA_MAX_ITERATIONS))
-    return fail(DWT_E_INVALID, "iterations %d outside [1,%d]", z.iters, DWT_ZCA_MAX_ITERATIONS);
-  if (!z.save) return fail(DWT_E_INVALID, "null pointer argument (%s)", name);
-  if ((uintptr_t)z.save % 16 != 0) return fail(DWT_E_INVALID, "%s must be 16-byte aligned", name);
-  if (c.p.gm.GS > DWT_MAX_GROUP_SIZE || c.r.fam != TC) return zca_refuse(c, z);
+int check_param(const float* p, const char* name) {
+  if (!p) return fail(DWT_E_INVALID, "null pointer argument (%s)", name);
+  if ((uintptr_t)p % 16 != 0) return fail(DWT_E_INVALID, "%s must be 16-byte aligned", name);
   return DWT_OK;
 }
 
-const char* zca_family(const Basis& z, bool bwd, bool bf16) {
+// a call's own basis arguments, and its family: validate()'s route, which must be the tensor-core one
+int basis_check(const Call& c, const Basis& z, bool bwd) {
+  if (z.kind == Basis::COLOR) {
+    if (int rc = check_param(z.color, "color")) return rc;
+    if (!bwd) { if (int rc = check_param(z.bias, "bias")) return rc; }
+    if ((z.dcolor == nullptr) != (z.dbias == nullptr)) return fail(DWT_E_INVALID, "dcolor and dbias go together");
+    if (z.dcolor) {
+      if (int rc = check_param(z.dcolor, "dcolor")) return rc;
+      if (int rc = check_param(z.dbias, "dbias")) return rc;
+    }
+  } else {
+    const char* name = z.kind == Basis::EIGH ? "save_e" : "save_p";
+    if (z.kind == Basis::NEWTON_SCHULZ && (z.iters < 1 || z.iters > DWT_ZCA_MAX_ITERATIONS))
+      return fail(DWT_E_INVALID, "iterations %d outside [1,%d]", z.iters, DWT_ZCA_MAX_ITERATIONS);
+    if (int rc = check_param(z.save, name)) return rc;
+  }
+  const dwt::Geom& g = c.p.gm;
+  if (g.GS > DWT_MAX_GROUP_SIZE || c.r.fam != TC) return basis_refuse(z, g.N, g.C, g.HW, g.GS);
+  return DWT_OK;
+}
+
+const char* basis_family(const Basis& z, bool bwd, bool bf16) {
   if (z.kind == Basis::EIGH) return bwd ? fam(bf16, "dense_bwd_eigh", "dense_bwd_eigh_bf16") : fam(bf16, "dense_fwd_eigh", "dense_fwd_eigh_bf16");
+  if (z.kind == Basis::COLOR) return bwd ? fam(bf16, "dense_bwd_color", "dense_bwd_color_bf16") : fam(bf16, "dense_fwd_color", "dense_fwd_color_bf16");
   return bwd ? fam(bf16, "dense_bwd_zca", "dense_bwd_zca_bf16") : fam(bf16, "dense_fwd_zca", "dense_fwd_zca_bf16");
 }
 
-void zca_fwd(const float* gram, const float* shift, const dwt::Geom& gm, const dwt::FwdFin& fin, const Basis& z, cudaStream_t st) {
+void basis_fwd(const float* gram, const float* shift, const dwt::Geom& gm, const dwt::FwdFin& fin, const Basis& z, const Workspace& w,
+               cudaStream_t st) {
   if (z.kind == Basis::EIGH) dwt::dense_fwd_eigh(gram, shift, gm, fin, const_cast<float*>(z.save), st);
+  else if (z.kind == Basis::COLOR) dwt::dense_fwd_color(gram, shift, gm, fin, z.color, w.coef, st);
   else dwt::dense_fwd_zca(gram, shift, gm, fin, z.iters, const_cast<float*>(z.save), st);
 }
 
-void zca_bwd(const float* rgram, const dwt::Geom& gm, const dwt::BwdFin& fin, const Basis& z, float* dybar, cudaStream_t st) {
+void basis_bwd(const float* rgram, const dwt::Geom& gm, const dwt::BwdFin& fin, const Basis& z, float* dybar, cudaStream_t st) {
   if (z.kind == Basis::EIGH) dwt::dense_bwd_eigh(rgram, gm, fin, z.save, dybar, st);
+  else if (z.kind == Basis::COLOR) dwt::dense_bwd_color(rgram, gm, fin, z.color, z.dcolor, z.dbias, dybar, st);
   else dwt::dense_bwd_zca(rgram, gm, fin, z.iters, z.save, dybar, st);
 }
 
@@ -525,7 +551,7 @@ int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, 
                     float b, float momentum, float unbias, int update_running, float* const* rmean,
                     float* const* rcov, const float* gamma, const float* beta, const float* residual,
                     uint8_t* relu_mask, int epi, float* save_mean, float* save_w, void* ws, size_t ws_bytes,
-                    cudaStream_t st, const Basis& zca = Basis{}) {
+                    cudaStream_t st, const Basis& basis = Basis{}) {
   Call c;
   const bool need_running = ((mode & 0xFF) == DWT_MODE_EVAL) || update_running;
   const int rc = validate(c, false, x, x, y, nullptr, N, C, HW, GS, D, mode, epi, gamma, beta, save_mean, save_w, ws, ws_bytes, [&] {
@@ -533,11 +559,13 @@ int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, 
     if (epi & DWT_EPI_RESIDUAL) if (int rc = check_align(c.bf16, (uintptr_t)residual, "residual")) return rc;
     if (relu_mask && !((epi & DWT_EPI_RESIDUAL) && c.nhwc))
       return fail(DWT_E_UNSUPPORTED, "the ReLU byte map is written by the channels-last RESIDUAL epilogue only");
-    if (zca.zca()) if (int rc = zca_check(c, zca)) return rc;
+    if (basis.own()) if (int rc = basis_check(c, basis, false)) return rc;
     return check_running(need_running, rmean, rcov, D);
   });
+  // colouring names itself in every refusal of its geometry (route()'s and make_plan()'s included)
+  if (rc == DWT_E_UNSUPPORTED && basis.kind == Basis::COLOR) return basis_refuse(basis, N, C, HW, GS);
   if (rc) return rc;
-  if (zca.zca() && c.r.fam != TC) return zca_refuse(c, zca);   // the tensor-core kernels could not be set up: no tiled ZCA
+  if (basis.own() && c.r.fam != TC) return basis_refuse(basis, N, C, HW, GS);   // the tensor-core kernels could not be set up
   const Plan& p = c.p; const Workspace& w = c.w;
   const bool bf16 = c.bf16, nhwc = c.nhwc, train = c.mode == DWT_MODE_TRAIN;
   const dwt::FwdFin fin = make_fwd_fin(a, b, momentum, unbias, train ? update_running : 0, need_running, rmean, rcov,
@@ -566,7 +594,7 @@ int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, 
     }
     if (c.r.fam == CL || c.r.fam == TC) {   // the small and tiled kernels finalize in their last CTA
       if (int rc = check_launch(c.r.fam == CL ? "channels-last statistics kernel" : "tensor-core statistics kernel")) return rc;
-      Launch l(zca.zca() ? zca_family(zca, false, bf16) : c.name(false, FINALIZE), &p.gm, 0.0, st);
+      Launch l(basis.own() ? basis_family(basis, false, bf16) : c.name(false, FINALIZE), &p.gm, 0.0, st);
       if (c.r.fam == CL) {
         dwt::cl_fwd_finalize(w.partial, cp.nred, w.shift, p.gm, fin, st);
       } else {
@@ -574,13 +602,13 @@ int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, 
         if (gs128)
           dwt::dense_partial_reduce(w.partial + pair_part, tc_pair_chunks(p.gm, false), dwt::tc_superblocks(p.gm) / 2 * D,
                                     w.gram + (size_t)dwt::tc_superblocks(p.gm) * D * (64 * 64 + 64), st);
-        if (zca.zca()) zca_fwd(w.gram, w.shift, p.gm, fin, zca, st);
+        if (basis.own()) basis_fwd(w.gram, w.shift, p.gm, fin, basis, w, st);
         else dwt::dense_fwd_factor(w.gram, w.shift, p.gm, fin, st);
       }
     }
-  } else if (zca.zca()) {
-    Launch l(zca_family(zca, false, bf16), &p.gm, 0.0, st);
-    zca_fwd(nullptr, nullptr, p.gm, fin, zca, st);
+  } else if (basis.own()) {
+    Launch l(basis_family(basis, false, bf16), &p.gm, 0.0, st);
+    basis_fwd(nullptr, nullptr, p.gm, fin, basis, w, st);
   } else {
     Launch l(c.name(false, PREP), &p.gm, 0.0, st);
     if (c.r.fam == TC) dwt::dense_fwd_factor(nullptr, nullptr, p.gm, fin, st);
@@ -594,8 +622,10 @@ int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, 
       case CL: dwt::cl_apply(x, y, bf16, p.gm, cp.new_, cp.gz_ew, epi, save_mean, save_w, gamma, beta, residual, relu_mask, st); break;
       case SMALL: dwt::small_apply(x, y, bf16, p.gm_ew, p.vec, p.chunks_ew, epi, save_mean, save_w, gamma, beta, residual, st); break;
       case TILED: dwt::tiled_apply(x, y, p.gm_ew, p.vec, p.chunks_ew, save_mean, save_w, st); break;
-      case TC:
-        if (int cr = dwt::tc_apply(x, y, bf16, nhwc, p.gm, tc_apply_ctas(p.gm, 1, 64), save_mean, save_w, st))
+      case TC:   // colouring: color W from the workspace, and the bias
+        if (int cr = basis.kind == Basis::COLOR
+                         ? dwt::tc_apply(x, y, bf16, nhwc, p.gm, tc_apply_ctas(p.gm, 1, 64), save_mean, w.coef, st, basis.bias)
+                         : dwt::tc_apply(x, y, bf16, nhwc, p.gm, tc_apply_ctas(p.gm, 1, 64), save_mean, save_w, st))
           return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d)", cr);
     }
   }
@@ -605,7 +635,7 @@ int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, 
 int whiten_like_bwd(const float* x, const float* dout, const float* dout2, float* dx, int64_t N, int64_t C, int64_t HW, int GS, int D,
                     int mode, float a, const float* save_mean, const float* save_w, const float* gamma,
                     const float* beta, const uint8_t* relu_mask, float* dresidual, int epi, float* dgamma,
-                    float* dbeta, void* ws, size_t ws_bytes, cudaStream_t st, const Basis& zca = Basis{}) {
+                    float* dbeta, void* ws, size_t ws_bytes, cudaStream_t st, const Basis& basis = Basis{}) {
   Call c;
   const int rc = validate(c, true, x, dout, dx, dout2, N, C, HW, GS, D, mode, epi, gamma, beta, save_mean, save_w, ws, ws_bytes, [&] {
     if (epi & DWT_EPI_RESIDUAL) {
@@ -619,16 +649,17 @@ int whiten_like_bwd(const float* x, const float* dout, const float* dout2, float
       return fail(DWT_E_INVALID, "relu_mask / dresidual belong to the RESIDUAL epilogue");
     }
     if ((dgamma == nullptr) != (dbeta == nullptr)) return fail(DWT_E_INVALID, "dgamma and dbeta go together");
-    if (zca.zca()) return zca_check(c, zca);
+    if (basis.own()) return basis_check(c, basis, true);
     return DWT_OK;
   });
+  if (rc == DWT_E_UNSUPPORTED && basis.kind == Basis::COLOR) return basis_refuse(basis, N, C, HW, GS);
   if (rc) return rc;
-  if (zca.zca() && c.r.fam != TC) return zca_refuse(c, zca);   // the tensor-core kernels could not be set up: no tiled ZCA
+  if (basis.own() && c.r.fam != TC) return basis_refuse(basis, N, C, HW, GS);   // the tensor-core kernels could not be set up
   const Plan& p = c.p; const Workspace& w = c.w;
   const bool bf16 = c.bf16, nhwc = c.nhwc;
   const dwt::BwdFin fin = make_bwd_fin(a, c.mode, epi, save_mean, save_w, gamma, dgamma, dbeta, w);
   const bool masked = nhwc && (epi & DWT_EPI_RESIDUAL) != 0;   // the reduction also writes the masked gradient
-  const bool need_reduce = (c.mode == DWT_MODE_TRAIN) || (fin.dgamma != nullptr) || masked;
+  const bool need_reduce = (c.mode == DWT_MODE_TRAIN) || (fin.dgamma != nullptr) || masked || (basis.dcolor != nullptr);
   const double n_el = (double)D * (double)N * (double)C * (double)HW;
   const double E = (bf16 ? 2.0 : 4.0) * n_el, Mb = 0.25 * n_el;
   const ClPlan cp = c.r.fam == CL ? cl_plan(p.gm, 2, 2, 4, 4) : ClPlan{};
@@ -645,24 +676,25 @@ int whiten_like_bwd(const float* x, const float* dout, const float* dout2, float
         case SMALL: dwt::small_bwd_reduce(x, dout, bf16, p.gm, p.vec, fin, beta, w.partial, w.counters, st); break;
         case TILED: dwt::tiled_bwd_reduce(x, dout, p.gm, p.vec, fin, w.partial, w.counters, st); break;
         case TC:
-          if (int cr = dwt::tc_bwd_reduce(x, dout, bf16, nhwc, p.gm, rchunks, save_mean, w.partial, st))
+          // the pilot shift of dy needs save_mean to be the batch mean: not in eval (colouring's dcolor)
+          if (int cr = dwt::tc_bwd_reduce(x, dout, bf16, nhwc, p.gm, rchunks, save_mean, w.partial, st, c.mode == DWT_MODE_TRAIN))
             return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d) x=%p dout=%p N=%d C=%d HW=%d D=%d", cr, (const void*)x, (const void*)dout, p.gm.N, p.gm.C, p.gm.HW, p.gm.D);
       }
     }
     if (c.r.fam == CL || c.r.fam == TC) {   // the small and tiled kernels finalize in their last CTA
       if (int rc = check_launch(c.r.fam == CL ? "channels-last backward reduction kernel" : "tensor-core backward reduction kernel")) return rc;
-      Launch l(zca.zca() ? zca_family(zca, true, bf16) : c.name(true, FINALIZE), &p.gm, 0.0, st);
+      Launch l(basis.own() ? basis_family(basis, true, bf16) : c.name(true, FINALIZE), &p.gm, 0.0, st);
       if (c.r.fam == CL) {
         dwt::cl_bwd_finalize(w.partial, cp.nred, p.gm, fin, st);
       } else {
         dwt::dense_partial_reduce(w.partial, rchunks, rproblems, w.gram, st);
-        if (zca.zca()) zca_bwd(w.gram, p.gm, fin, zca, w.shift, st);
+        if (basis.own()) basis_bwd(w.gram, p.gm, fin, basis, w.shift, st);
         else dwt::dense_bwd_coef(w.gram, p.gm, fin, w.shift, st);
       }
     }
-  } else if (zca.zca()) {
-    Launch l(zca_family(zca, true, bf16), &p.gm, 0.0, st);
-    zca_bwd(nullptr, p.gm, fin, zca, w.shift, st);
+  } else if (basis.own()) {
+    Launch l(basis_family(basis, true, bf16), &p.gm, 0.0, st);
+    basis_bwd(nullptr, p.gm, fin, basis, w.shift, st);
   } else {
     Launch l(c.name(true, PREP), &p.gm, 0.0, st);
     if (c.r.fam == TC) dwt::dense_bwd_coef(nullptr, p.gm, fin, w.shift, st);
@@ -866,6 +898,26 @@ int dwt_whiten_eigh_bwd(const float* x, const float* dout, float* dx, int64_t N,
   return whiten_like_bwd(x, dout, nullptr, dx, N, C, HW, group_size, n_domains, mode, 1.f - eps, save_mean, save_w, nullptr,
                          nullptr, nullptr, nullptr, 0, nullptr, nullptr, workspace, workspace_bytes, (cudaStream_t)stream,
                          Basis{Basis::EIGH, 0, save_e});
+}
+
+int dwt_whiten_color_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, int group_size, int n_domains, int mode,
+                         float eps, float momentum, int update_running, float* const* running_mean, float* const* running_cov,
+                         const float* color, const float* bias, float* save_mean, float* save_w, void* workspace,
+                         size_t workspace_bytes, dwt_stream_t stream) {
+  Basis b;
+  b.kind = Basis::COLOR; b.color = color; b.bias = bias;
+  return whiten_like_fwd(x, y, N, C, HW, group_size, n_domains, mode, 1.f - eps, eps, momentum, 1.f, update_running,
+                         running_mean, running_cov, nullptr, nullptr, nullptr, nullptr, 0, save_mean, save_w, workspace,
+                         workspace_bytes, (cudaStream_t)stream, b);
+}
+
+int dwt_whiten_color_bwd(const float* x, const float* dout, float* dx, int64_t N, int64_t C, int64_t HW, int group_size,
+                         int n_domains, int mode, float eps, const float* save_mean, const float* save_w, const float* color,
+                         float* dcolor, float* dbias, void* workspace, size_t workspace_bytes, dwt_stream_t stream) {
+  Basis b;
+  b.kind = Basis::COLOR; b.color = color; b.dcolor = dcolor; b.dbias = dbias;
+  return whiten_like_bwd(x, dout, nullptr, dx, N, C, HW, group_size, n_domains, mode, 1.f - eps, save_mean, save_w, nullptr,
+                         nullptr, nullptr, nullptr, 0, nullptr, nullptr, workspace, workspace_bytes, (cudaStream_t)stream, b);
 }
 
 // Batch norm is the group-size-1 member of the same family: "covariance" = biased variance,

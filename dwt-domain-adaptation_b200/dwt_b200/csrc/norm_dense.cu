@@ -12,6 +12,8 @@
 //                    statistics prologue and EMA tail
 //   fwd_eigh/bwd_eigh  the exact ZCA basis (dwt_whiten_eigh_*): W = U diag(lambda^-1/2) U^T by a cyclic Jacobi
 //                    eigensolver in shared memory, and the Daleckii-Krein backward; the same prologue and EMA tail
+//   fwd_factor<COLOR>, bwd_color  colouring (dwt_whiten_color_*): fwd_factor also writes color W; bwd_color runs bwd_coef's
+//                    algebra on color^T R, domains in order in one CTA per group, and sums dcolor and dbias over them
 //
 // All three keep a 64x64 problem in ONE 256-thread CTA arranged 16x16, each thread owning a 4x4
 // register block.  fwd_factor runs the Cholesky factorisation AND the triangular inverse as one blocked
@@ -114,6 +116,14 @@ __device__ __forceinline__ void store_block(float* M, const Blk& t, const float 
   for (int r = 0; r < 4; ++r)
 #pragma unroll
     for (int s = 0; s < 4; ++s) M[(4 * t.bi + r) * LDS + 4 * t.bj + s] = c[r][s];
+}
+
+// this thread's 4 x 4 block to a dense GS x GS matrix in global memory
+__device__ __forceinline__ void store_block_global(float* M, int GS, const Blk& t, const float (&c)[4][4]) {
+  if (!t.act) return;
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+    *reinterpret_cast<float4*>(M + (size_t)(4 * t.bi + r) * GS + 4 * t.bj) = make_float4(c[r][0], c[r][1], c[r][2], c[r][3]);
 }
 
 // Blocked right-looking sweep: S = L L^T and W = L^-1 together, 4 columns per step, ONE block barrier per step.
@@ -334,9 +344,13 @@ __device__ __forceinline__ void domain_ema(int d, int g, const Geom& gm, const F
 
 // ------------------------------------------------------------------------------------------
 // fwd_factor: grid (G), 256 threads; loops over the domains in order (EMA sequence, SURVEY H5)
+// COLOR: also gw [D][G][gs*gs] = color[g] W (color [G][gs*gs]), for the apply in place of W; dynamic shared memory holds
+// color and W (kColorFwdSmem)
 // ------------------------------------------------------------------------------------------
+template <bool COLOR>
 __global__ void __launch_bounds__(256) fwd_factor_kernel(const float* __restrict__ gram, const float* __restrict__ shift,
-                                                         const Geom gm, const FwdFin f) {
+                                                         const Geom gm, const FwdFin f, const float* __restrict__ color,
+                                                         float* __restrict__ gw) {
   __shared__ __align__(16) PanelSmem sp;
   __shared__ float sC[kMat];       // un-shrunk covariance (for the EMA)
   __shared__ float sMean[kSB], sRow[kSB];
@@ -346,6 +360,12 @@ __global__ void __launch_bounds__(256) fwd_factor_kernel(const float* __restrict
   const int SB = (gm.C + kSB - 1) / kSB;
   const float invM = 1.f / gm.M;
   if (threadIdx.x == 0) sBad = 0;
+  extern __shared__ __align__(16) float dsm[];
+  float* sGam = dsm;                                  // COLOR: color[g], then W of the domain
+  float* sWd = dsm + kMat;
+  if constexpr (COLOR) {                              // published by domain_stats' barrier
+    for (int e = threadIdx.x; e < GS * GS; e += 256) sGam[(e / GS) * LDS + e % GS] = color[(size_t)g * GS * GS + e];
+  }
   PROF_DECL;
   PROF_MARK();
   for (int d = 0; d < gm.D; ++d) {
@@ -363,13 +383,45 @@ __global__ void __launch_bounds__(256) fwd_factor_kernel(const float* __restrict
         *reinterpret_cast<float4*>(f.save_w + gbase + (size_t)(4 * t.bi + r) * GS + 4 * t.bj) =
             make_float4(w[r][0], w[r][1], w[r][2], w[r][3]);
     }
+    if constexpr (COLOR) store_block(sWd, t, w);
     __syncthreads();                                  // sC complete, sBadDom final
+    if constexpr (COLOR) {
+      float c[4][4];
+      mm_block<false, false>(sGam, sWd, GS, t, c);
+      store_block_global(gw + gbase, GS, t, c);
+    }
     if (old.on && !sBadDom) domain_ema(d, g, gm, f, sC, sMean, old);   // a non-PD batch covariance never reaches the running buffers
     __syncthreads();      // also orders this domain's buffer writes before the next domain's reads (aliasing)
     PROF_MARK();
   }
   PROF_DUMP("fwd_factor load|factor+invert|save+ema");
   if (threadIdx.x == 0 && sBad) atomicOr(f.status, DWT_STATUS_NOT_PD);
+}
+
+// bwd_color's copy of bwd_coef's three products (bwd_coef keeps them inline: factoring them out changes its code):
+// from R = sum dL/dy xc^T (sR) and W (sW), S' = W^T Phi(-R W^T) W into sT1 (sT2: scratch), Bm = (a/M)(S' + S'^T).
+// Ends with a block barrier.
+__device__ __forceinline__ void chol_bwd_core(const float* sR, const float* sW, float* sT1, float* sT2, int GS, const Blk& t PROF_ARGS) {
+  float c[4][4];
+  mm_block<false, true>(sR, sW, GS, t, c);               // R W^T ; P = Phi(-R W^T)
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+#pragma unroll
+    for (int s = 0; s < 4; ++s) {
+      const int i = 4 * t.bi + r, j = 4 * t.bj + s;
+      c[r][s] = (i > j) ? -c[r][s] : ((i == j) ? -0.5f * c[r][s] : 0.f);
+    }
+  store_block(sT1, t, c);
+  __syncthreads();
+  PROF_MARK();
+  mm_block<true, false>(sW, sT1, GS, t, c);              // T = W^T P
+  store_block(sT2, t, c);
+  __syncthreads();
+  PROF_MARK();
+  mm_block<false, false>(sT2, sW, GS, t, c);             // S' = T W
+  store_block(sT1, t, c);
+  __syncthreads();
+  PROF_MARK();
 }
 
 // ------------------------------------------------------------------------------------------
@@ -473,19 +525,109 @@ __global__ void __launch_bounds__(256) bwd_coef_kernel(const float* __restrict__
 }
 
 // ------------------------------------------------------------------------------------------
+// bwd_color: grid (G), 256 threads, the domains of a group in order.  y = color W xc + bias: with dy_hat = color^T dy, per domain
+//   train: bwd_coef's algebra on R_hat = color^T R, A1 = W^T color^T (full), dybar = mean_M dy (tc_bwd_apply: A1 (dy - dybar))
+//   eval:  A1 = W^T color^T, Bm = 0, dybar = 0
+// and, when dcolor is given (rgram given), dcolor[g] = sum_d R_d W_d^T, dbias[g] = sum_d sum_m dy, summed in domain order in
+// registers: deterministic.  In eval R comes from the contraction without pilot shift (tc_bwd_reduce, pilot = false).
+// ------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) bwd_color_kernel(const float* __restrict__ rgram, const Geom gm, const BwdFin f,
+                                                        const float* __restrict__ color, float* __restrict__ dcolor,
+                                                        float* __restrict__ dbias, float* __restrict__ dybar) {
+  extern __shared__ __align__(16) float dsm[];
+  float* sW = dsm;
+  float* sR = sW + kMat;           // R, then R_hat
+  float* sT1 = sR + kMat;
+  float* sT2 = sT1 + kMat;
+  float* sGam = sT2 + kMat;        // color[g]
+  float* sGW = sGam + kMat;        // color W = A1^T
+  __shared__ float sSdz[kSB], sMu[kSB];
+  const int g = blockIdx.x, GS = gm.GS, nb = kSB / GS, sb = g / nb, o = (g % nb) * GS;
+  const Blk t(GS);
+  const int SB = (gm.C + kSB - 1) / kSB;
+  const bool train = f.mode == DWT_MODE_TRAIN;
+  const int gsh = __ffs(GS) - 1;
+  const float invM = 1.f / gm.M;
+  constexpr int kPer = kSB * kSB / 256;
+  for (int e = threadIdx.x; e < GS * GS; e += 256) sGam[(e >> gsh) * LDS + (e & (GS - 1))] = color[(size_t)g * GS * GS + e];
+  PROF_DECL;
+  float dg[4][4], db = 0.f;
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+#pragma unroll
+    for (int s = 0; s < 4; ++s) dg[r][s] = 0.f;
+  for (int d = 0; d < gm.D; ++d) {
+    const float* G = rgram ? rgram + ((size_t)d * SB + sb) * kNacc : nullptr;
+    const size_t gbase = ((size_t)d * gm.G + g) * GS * GS;
+    float* coef = f.coef + ((size_t)d * gm.G + g) * coef_stride(GS);
+#pragma unroll
+    for (int n = 0; n < kPer; ++n) {
+      const int e = threadIdx.x + 256 * n, i = e >> gsh, j = e & (GS - 1);
+      if (e < GS * GS) {
+        sW[i * LDS + j] = f.save_w[gbase + e];
+        sR[i * LDS + j] = G ? __ldcg(G + (o + i) * kSB + o + j) : 0.f;
+      }
+    }
+    if ((int)threadIdx.x < GS) {
+      const float sdz = G ? __ldcg(G + kSB * kSB + o + threadIdx.x) : 0.f;
+      db += sdz;
+      sSdz[threadIdx.x] = train ? sdz * invM : 0.f;   // mean_M dy
+      sMu[threadIdx.x] = f.save_mean[(size_t)d * gm.C + g * GS + threadIdx.x];
+      if (dybar) dybar[((size_t)d * SB + sb) * kSB + o + threadIdx.x] = train ? sdz * invM : 0.f;
+    }
+    __syncthreads();
+    float c[4][4], gw[4][4];
+    if (dcolor) {
+      mm_block<false, true>(sR, sW, GS, t, c);        // R W^T
+#pragma unroll
+      for (int r = 0; r < 4; ++r)
+#pragma unroll
+        for (int s = 0; s < 4; ++s) dg[r][s] += c[r][s];
+    }
+    mm_block<false, false>(sGam, sW, GS, t, gw);      // color W
+    if (train) mm_block<true, false>(sGam, sR, GS, t, c);   // R_hat = color^T R
+    __syncthreads();                                  // every read of sR is done
+    if (train) store_block(sR, t, c);
+    store_block(sGW, t, gw);
+    __syncthreads();
+    if (train) chol_bwd_core(sR, sW, sT1, sT2, GS, t PROF_PASS);
+    const float sc = f.a * invM;
+#pragma unroll
+    for (int n = 0; n < kPer; ++n) {
+      const int e = threadIdx.x + 256 * n, i = e >> gsh, j = e & (GS - 1);
+      if (e < GS * GS) {
+        const float bm = train ? sc * (sT1[i * LDS + j] + sT1[j * LDS + i]) : 0.f;
+        coef[e] = sGW[j * LDS + i];                   // A1 = (color W)^T, every element
+        coef[GS * GS + e] = bm;
+        sT2[i * LDS + j] = bm;
+      }
+    }
+    __syncthreads();
+    // cvec_i = -(sum_j A1_ij mean(dy)_j + sum_j Bm_ij mu_j), as in bwd_coef
+    {
+      const int i = threadIdx.x >> 2, q = threadIdx.x & 3;
+      float cv = 0.f;
+      if (train && i < GS) {
+        for (int j = q; j < GS; j += 4) cv = fmaf(sGW[j * LDS + i], sSdz[j], fmaf(sT2[i * LDS + j], sMu[j], cv));
+      }
+      cv += __shfl_xor_sync(0xffffffffu, cv, 1);
+      cv += __shfl_xor_sync(0xffffffffu, cv, 2);
+      if (q == 0 && i < GS) coef[2 * GS * GS + i] = -cv;
+    }
+    __syncthreads();                                  // the next domain overwrites every shared matrix
+  }
+  if (dcolor) {
+    store_block_global(dcolor + (size_t)g * GS * GS, GS, t, dg);
+    if ((int)threadIdx.x < GS) dbias[g * GS + threadIdx.x] = db;
+  }
+}
+
+// ------------------------------------------------------------------------------------------
 // ZCA basis (dwt_whiten_zca_*): W = S^-1/2 by T steps of the Newton-Schulz iteration instead of W = L^-1
 //   t = tr S,  N = S / t,  P_0 = I,  P_k = (3 P_{k-1} - P_{k-1}^3 N) / 2  (k = 1..T),  W = P_T / sqrt(t)
 // W is NOT symmetrised: it is P_T / sqrt(t) as computed, symmetric in exact arithmetic only, and both apply kernels use
 // exactly the saved W (A1 = W^T in full).  save_p [D][G][T][GS*GS]: slot 0 holds S, slot k holds P_k (k = 1..T-1).
 // ------------------------------------------------------------------------------------------
-// this thread's 4 x 4 block to a dense GS x GS matrix in global memory
-__device__ __forceinline__ void store_block_global(float* M, int GS, const Blk& t, const float (&c)[4][4]) {
-  if (!t.act) return;
-#pragma unroll
-  for (int r = 0; r < 4; ++r)
-    *reinterpret_cast<float4*>(M + (size_t)(4 * t.bi + r) * GS + 4 * t.bj) = make_float4(c[r][0], c[r][1], c[r][2], c[r][3]);
-}
-
 __device__ __forceinline__ void load_block(const float* M, const Blk& t, float (&c)[4][4]) {
 #pragma unroll
   for (int r = 0; r < 4; ++r)
@@ -1119,11 +1261,13 @@ constexpr size_t kZcaFwdSmem = sizeof(float) * 4 * kMat;   // N, P, P^2, P^3 (66
 constexpr size_t kZcaBwdSmem = sizeof(float) * 8 * kMat;   // W, N, Q, P, P^2, Q N, P^3, P Q N (133 KB)
 constexpr size_t kEighFwdSmem = sizeof(float) * 2 * kMat;  // S / V, U (33.3 KB; + 17.6 KB static)
 constexpr size_t kEighBwdSmem = sizeof(float) * 5 * kMat;  // W, U, R / G, R U / U H, H / Bm (83.2 KB)
+constexpr size_t kColorFwdSmem = sizeof(float) * 2 * kMat; // color, W (33.3 KB; + 21.3 KB static)
+constexpr size_t kColorBwdSmem = sizeof(float) * 6 * kMat; // W, R / R_hat, T1, T2, color, color W (99.8 KB)
 
 }  // namespace
 
 int dense_init() {
-  cudaError_t e = cudaFuncSetAttribute(fwd_factor_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFactorSmem);
+  cudaError_t e = cudaFuncSetAttribute(fwd_factor_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFactorSmem);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(bwd_coef_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kCoefSmem);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(fwd_factor128_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFactor2Smem);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(bwd_coef128_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kCoef2Smem);
@@ -1131,6 +1275,8 @@ int dense_init() {
   if (e == cudaSuccess) e = cudaFuncSetAttribute(bwd_zca_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kZcaBwdSmem);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(fwd_eigh_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kEighFwdSmem);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(bwd_eigh_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kEighBwdSmem);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(fwd_factor_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kColorFwdSmem);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(bwd_color_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kColorBwdSmem);
   return (int)e;
 }
 
@@ -1147,7 +1293,7 @@ void dense_fwd_factor(const float* gram, const float* shift, const Geom& gm, con
     fwd_factor128_kernel<<<gm.G, kThreads2, kFactor2Smem, st>>>(gram, goff, shift, gm, fin);
     return;
   }
-  fwd_factor_kernel<<<gm.G, 256, kFactorSmem, st>>>(gram, shift, gm, fin);
+  fwd_factor_kernel<false><<<gm.G, 256, kFactorSmem, st>>>(gram, shift, gm, fin, nullptr, nullptr);
 }
 
 // rgram == nullptr: eval mode without affine (A1 = W^T only).  Group size 128: rgram [D][2 SB] blocks.
@@ -1175,6 +1321,16 @@ void dense_fwd_eigh(const float* gram, const float* shift, const Geom& gm, const
 
 void dense_bwd_eigh(const float* rgram, const Geom& gm, const BwdFin& fin, const float* save_e, float* dybar, cudaStream_t st) {
   bwd_eigh_kernel<<<dim3(gm.G, 1, gm.D), 256, kEighBwdSmem, st>>>(rgram, gm, fin, save_e, dybar);
+}
+
+void dense_fwd_color(const float* gram, const float* shift, const Geom& gm, const FwdFin& fin, const float* color, float* gw,
+                     cudaStream_t st) {
+  fwd_factor_kernel<true><<<gm.G, 256, kColorFwdSmem, st>>>(gram, shift, gm, fin, color, gw);
+}
+
+void dense_bwd_color(const float* rgram, const Geom& gm, const BwdFin& fin, const float* color, float* dcolor, float* dbias,
+                     float* dybar, cudaStream_t st) {
+  bwd_color_kernel<<<gm.G, 256, kColorBwdSmem, st>>>(rgram, gm, fin, color, dcolor, dbias, dybar);
 }
 
 }  // namespace dwt

@@ -55,8 +55,10 @@ int tc_stats(const void* x, bool bf16, bool nhwc, const Geom& gm, int nchunks, f
 // group size 128 (fp32): the off-diagonal 64 x 64 Gram block of every 128-channel group, around tc_stats' shifts.
 // tc_bwd_reduce at group size 128 forms all four blocks of every group's R.
 int tc_gram_pair(const void* x, bool nhwc, const Geom& gm, int nchunks, const float* shift, float* partial, cudaStream_t st);
+// pilot = false (group sizes 8..64): dy is not centred.  The centring drops K (sum xc)^T, which is zero only when save_mean
+// is the batch mean (training); with running statistics R must be formed without it.
 int tc_bwd_reduce(const void* x, const void* dout, bool bf16, bool nhwc, const Geom& gm, int nchunks, const float* save_mean,
-                  float* partial, cudaStream_t st);
+                  float* partial, cudaStream_t st, bool pilot = true);
 
 // dense per-group algebra behind the contraction (norm_dense.cu)
 int dense_init();
@@ -73,11 +75,19 @@ void dense_bwd_zca(const float* rgram, const Geom& gm, const BwdFin& fin, int it
 // (U, then lambda) is written by the forward and read by the backward; both leave what dense_fwd_factor / dense_bwd_coef leave.
 void dense_fwd_eigh(const float* gram, const float* shift, const Geom& gm, const FwdFin& fin, float* save_e, cudaStream_t st);
 void dense_bwd_eigh(const float* rgram, const Geom& gm, const BwdFin& fin, const float* save_e, float* dybar, cudaStream_t st);
+// colouring, group sizes 8..64 (dwt_whiten_color_*): fwd_factor that also writes gw [D][G][gs*gs] = color W; and the Cholesky
+// backward on Gamma^T R with A1 = W^T color^T, plus dcolor [G][gs*gs] = sum_d R W^T and dbias [C] = sum_d sum dy over the
+// domains in order (both or neither; rgram null: eval without them)
+void dense_fwd_color(const float* gram, const float* shift, const Geom& gm, const FwdFin& fin, const float* color, float* gw,
+                     cudaStream_t st);
+void dense_bwd_color(const float* rgram, const Geom& gm, const BwdFin& fin, const float* color, float* dcolor, float* dbias,
+                     float* dybar, cudaStream_t st);
 
 // TMA + wgmma apply path (norm_tc_apply.cu): split-TF32 GEMM of the block-diagonal group matrices
 int tc_apply_init();
+// bias [C] (group sizes 8..64): y = W (x - mean) + bias, the accumulator starting at bias
 int tc_apply(const void* x, void* y, bool bf16, bool nhwc, const Geom& gm, int nctas, const float* save_mean, const float* save_w,
-             cudaStream_t st);
+             cudaStream_t st, const float* bias = nullptr);
 int tc_bwd_apply(const void* x, const void* dout, void* dx, bool bf16, bool nhwc, const Geom& gm, int nctas, const float* coef,
                  const float* save_mean, const float* dybar, cudaStream_t st);
 

@@ -299,7 +299,8 @@ __device__ __forceinline__ void init_ring(TcBarriers& bars, int stages) {
 // M K (mean - save_mean)^T that rounding costs).  The row sums need K back:  rowsum_cta = sum_cta e + n_valid K.
 // PAIR (group size 128): blockIdx.y = 4 p + 2 r + c is block (r, c) of the 128 x 128 R of pair p: dy rows from
 // super-block 2p + r, x columns from super-block 2p + c (R is not symmetric: all four blocks are formed).
-template <class T, bool NHWC, bool PAIR = false>
+// PILOT = false: K = 0.  With save_mean a running mean, sum xc is not zero and the centred sum is not R.
+template <class T, bool NHWC, bool PAIR = false, bool PILOT = true>
 __global__ void __launch_bounds__(kTcThreads, 2)
 tc_contract_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_g, const T* __restrict__ dout,
                    const Geom gm, const float* __restrict__ save_mean, float* __restrict__ partial) {
@@ -343,7 +344,7 @@ tc_contract_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
     // ===== consumer warpgroups: split transforms, then D[64 x 64] = Eh Xh^T + El Xh^T + Eh Xl^T, sum += D =====
     const int wg = warp >> 2, t = tid & 127;
     // dy's shift: its dependent loads overlap the producer's first TMA loads (named barrier 3: the consumers only)
-    if (tid < kTileCh) sK[tid] = pilot_shift<T, NHWC>(dout, gm, d, ch0 + tid);          // 0 past C
+    if (tid < kTileCh) sK[tid] = PILOT ? pilot_shift<T, NHWC>(dout, gm, d, ch0 + tid) : 0.f;          // 0 past C
     asm volatile("bar.sync 3, %0;" ::"n"(128 * kConsumers) : "memory");
     // per warpgroup behind the ring: the lo tiles of xc and dy (fp32 NCHW: hi in place), or hi and lo of both (bf16 / NHWC)
     const uint32_t wgbuf = smem_u32(smem + (size_t)STAGES * 2 * BOX + (size_t)wg * (STAGED ? 4 : 2) * kTileBytes);
@@ -661,6 +662,9 @@ cudaError_t tc_kernel_attrs() {
   // two ~73-97 KB CTAs per SM need the full shared-memory carve-out
   if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_gram_kernel<T, NHWC>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_contract_kernel<T, NHWC>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  if (e == cudaSuccess)
+    e = cudaFuncSetAttribute(tc_contract_kernel<T, NHWC, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes<T, NHWC>(true));
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_contract_kernel<T, NHWC, false, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   return e;
 }
 
@@ -687,7 +691,7 @@ void launch_gram(const CUtensorMap& mx, const void* x, const Geom& gm, int nchun
 
 template <class T, bool NHWC>
 void launch_contract(const CUtensorMap& mx, const CUtensorMap& mg, const void* dout, const Geom& gm, int nchunks,
-                     const float* save_mean, float* partial, cudaStream_t st) {
+                     const float* save_mean, float* partial, cudaStream_t st, bool pilot) {
   const T* g = static_cast<const T*>(dout);
   if constexpr (!kBf16<T>) {
     if (gm.GS == 2 * kTileCh) {                  // group size 128: the four 64 x 64 blocks of every group's R
@@ -697,7 +701,8 @@ void launch_contract(const CUtensorMap& mx, const CUtensorMap& mg, const void* d
     }
   }
   dim3 grid(nchunks, tc_superblocks(gm), gm.D);
-  tc_contract_kernel<T, NHWC><<<grid, kTcThreads, tc_smem_bytes<T, NHWC>(true), st>>>(mx, mg, g, gm, save_mean, partial);
+  if (pilot) tc_contract_kernel<T, NHWC><<<grid, kTcThreads, tc_smem_bytes<T, NHWC>(true), st>>>(mx, mg, g, gm, save_mean, partial);
+  else tc_contract_kernel<T, NHWC, false, false><<<grid, kTcThreads, tc_smem_bytes<T, NHWC>(true), st>>>(mx, mg, g, gm, save_mean, partial);
 }
 
 }  // namespace
@@ -759,17 +764,17 @@ int tc_gram_pair(const void* x, bool nhwc, const Geom& gm, int nchunks, const fl
 
 // group size 128: partial [D][2 SB][nchunks][64*64+64], block (r, c) of group p at 4 p + 2 r + c
 int tc_bwd_reduce(const void* x, const void* dout, bool bf16, bool nhwc, const Geom& gm, int nchunks, const float* save_mean,
-                  float* partial, cudaStream_t st) {
+                  float* partial, cudaStream_t st, bool pilot) {
   CUtensorMap mx, mg;
   bind_context();
   if (int rc = make_map(&mx, x, gm, bf16, nhwc)) return rc;
   if (int rc = make_map(&mg, dout, gm, bf16, nhwc)) return rc;
   if (nhwc) {
-    if (bf16) launch_contract<__nv_bfloat16, true>(mx, mg, dout, gm, nchunks, save_mean, partial, st);
-    else launch_contract<float, true>(mx, mg, dout, gm, nchunks, save_mean, partial, st);
+    if (bf16) launch_contract<__nv_bfloat16, true>(mx, mg, dout, gm, nchunks, save_mean, partial, st, pilot);
+    else launch_contract<float, true>(mx, mg, dout, gm, nchunks, save_mean, partial, st, pilot);
   } else {
-    if (bf16) launch_contract<__nv_bfloat16, false>(mx, mg, dout, gm, nchunks, save_mean, partial, st);
-    else launch_contract<float, false>(mx, mg, dout, gm, nchunks, save_mean, partial, st);
+    if (bf16) launch_contract<__nv_bfloat16, false>(mx, mg, dout, gm, nchunks, save_mean, partial, st, pilot);
+    else launch_contract<float, false>(mx, mg, dout, gm, nchunks, save_mean, partial, st, pilot);
   }
   return 0;
 }

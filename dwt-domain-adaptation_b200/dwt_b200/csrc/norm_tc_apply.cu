@@ -131,7 +131,9 @@ __device__ __forceinline__ float lds_f(uint32_t addr) {
   }
 }
 
-template <class T, int NIN, bool NHWC>
+// BIAS (one input): out = M (x - shift) + bias, bias [C] in the second input's slot (args.shift[1]); the accumulator starts
+// at the bias of its channel (the colouring transform's beta)
+template <class T, int NIN, bool NHWC, bool BIAS = false>
 __global__ void __launch_bounds__(kApThreads, 1)
 tc_apply_kernel(const __grid_constant__ CUtensorMap map0, const __grid_constant__ CUtensorMap map1, const Geom gm,
                 const ApplyArgs args) {
@@ -159,6 +161,10 @@ tc_apply_kernel(const __grid_constant__ CUtensorMap map0, const __grid_constant_
   if (tid < NIN * kCh) {
     const int i = tid / kCh, r = tid - i * kCh, c = ch0 + r;
     sShift[i][r] = (c < gm.C && args.shift[i] != nullptr) ? __ldg(args.shift[i] + (size_t)d * args.shift_stride[i] + c) : 0.f;
+  }
+  if constexpr (BIAS) {
+    static_assert(NIN == 1, "the bias takes the second input's slot");
+    if (tid >= kCh && tid < 2 * kCh) sShift[1][tid - kCh] = ch0 + tid - kCh < gm.C ? __ldg(args.shift[1] + ch0 + tid - kCh) : 0.f;
   }
   __syncthreads();
 
@@ -247,8 +253,17 @@ tc_apply_kernel(const __grid_constant__ CUtensorMap map0, const __grid_constant_
       __syncwarp();
       if (lane == 0) mbar_arrive(&bars.empty[s]);   // the tile is in registers: the stage can be refilled
       float acc[32];
+      if constexpr (BIAS) {
+        // acc[4 j + r] belongs to channel 8 j + 2 (l%4) + (r & 1) (the D fragment above)
 #pragma unroll
-      for (int j = 0; j < 32; ++j) acc[j] = 0.f;
+        for (int j = 0; j < kCh / 8; ++j) {
+          const float b0 = sShift[1][8 * j + 2 * kq], b1 = sShift[1][8 * j + 2 * kq + 1];
+          acc[4 * j] = b0; acc[4 * j + 1] = b1; acc[4 * j + 2] = b0; acc[4 * j + 3] = b1;
+        }
+      } else {
+#pragma unroll
+        for (int j = 0; j < 32; ++j) acc[j] = 0.f;
+      }
       wgmma_fence();
       fence_operands(acc);
 #pragma unroll
@@ -485,11 +500,11 @@ int make_map_ap(CUtensorMap* map, const void* base, const Geom& gm, bool bf16, b
 
 template <class T, int NIN> constexpr size_t ap_smem() { return ApCfg<T, NIN>::SMEM; }
 
-template <class T, int NIN, bool NHWC>
+template <class T, int NIN, bool NHWC, bool BIAS = false>
 cudaError_t ap_attrs() {
-  cudaError_t e = cudaFuncSetAttribute(tc_apply_kernel<T, NIN, NHWC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ap_smem<T, NIN>());
+  cudaError_t e = cudaFuncSetAttribute(tc_apply_kernel<T, NIN, NHWC, BIAS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ap_smem<T, NIN>());
   // a 129 / 193 KB CTA needs the full shared-memory carve-out
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_apply_kernel<T, NIN, NHWC>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_apply_kernel<T, NIN, NHWC, BIAS>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   return e;
 }
 
@@ -500,7 +515,7 @@ cudaError_t ap128_attrs() {
   return e;
 }
 
-template <int NIN>
+template <int NIN, bool BIAS = false>
 void launch_apply(bool bf16, bool nhwc, dim3 grid, const CUtensorMap& m0, const CUtensorMap& m1, const Geom& gm, const ApplyArgs& a,
                   cudaStream_t st) {
   if (gm.GS == 2 * kCh) {                          // group size 128 (fp32 only: the C ABI refuses bf16 there)
@@ -509,11 +524,11 @@ void launch_apply(bool bf16, bool nhwc, dim3 grid, const CUtensorMap& m0, const 
     return;
   }
   if (nhwc) {
-    if (bf16) tc_apply_kernel<__nv_bfloat16, NIN, true><<<grid, kApThreads, ap_smem<__nv_bfloat16, NIN>(), st>>>(m0, m1, gm, a);
-    else tc_apply_kernel<float, NIN, true><<<grid, kApThreads, ap_smem<float, NIN>(), st>>>(m0, m1, gm, a);
+    if (bf16) tc_apply_kernel<__nv_bfloat16, NIN, true, BIAS><<<grid, kApThreads, ap_smem<__nv_bfloat16, NIN>(), st>>>(m0, m1, gm, a);
+    else tc_apply_kernel<float, NIN, true, BIAS><<<grid, kApThreads, ap_smem<float, NIN>(), st>>>(m0, m1, gm, a);
   } else {
-    if (bf16) tc_apply_kernel<__nv_bfloat16, NIN, false><<<grid, kApThreads, ap_smem<__nv_bfloat16, NIN>(), st>>>(m0, m1, gm, a);
-    else tc_apply_kernel<float, NIN, false><<<grid, kApThreads, ap_smem<float, NIN>(), st>>>(m0, m1, gm, a);
+    if (bf16) tc_apply_kernel<__nv_bfloat16, NIN, false, BIAS><<<grid, kApThreads, ap_smem<__nv_bfloat16, NIN>(), st>>>(m0, m1, gm, a);
+    else tc_apply_kernel<float, NIN, false, BIAS><<<grid, kApThreads, ap_smem<float, NIN>(), st>>>(m0, m1, gm, a);
   }
 }
 
@@ -533,6 +548,10 @@ int tc_apply_init() {
   if (e == cudaSuccess) e = ap_attrs<float, 2, true>();
   if (e == cudaSuccess) e = ap_attrs<__nv_bfloat16, 1, true>();
   if (e == cudaSuccess) e = ap_attrs<__nv_bfloat16, 2, true>();
+  if (e == cudaSuccess) e = ap_attrs<float, 1, false, true>();
+  if (e == cudaSuccess) e = ap_attrs<__nv_bfloat16, 1, false, true>();
+  if (e == cudaSuccess) e = ap_attrs<float, 1, true, true>();
+  if (e == cudaSuccess) e = ap_attrs<__nv_bfloat16, 1, true, true>();
   if (e == cudaSuccess) e = ap128_attrs<1, false>();
   if (e == cudaSuccess) e = ap128_attrs<2, false>();
   if (e == cudaSuccess) e = ap128_attrs<1, true>();
@@ -540,9 +559,9 @@ int tc_apply_init() {
   return (int)e;
 }
 
-// y = W (x - mean): W from save_w [D][G][gs*gs], mean from save_mean [D][C]
+// y = W (x - mean) (+ bias): W from save_w [D][G][gs*gs], mean from save_mean [D][C], bias [C] or null (group sizes 8..64)
 int tc_apply(const void* x, void* y, bool bf16, bool nhwc, const Geom& gm, int nctas, const float* save_mean, const float* save_w,
-             cudaStream_t st) {
+             cudaStream_t st, const float* bias) {
   CUtensorMap mx;
   bind_context();
   if (int rc = make_map_ap(&mx, x, gm, bf16, nhwc)) return rc;
@@ -551,7 +570,10 @@ int tc_apply(const void* x, void* y, bool bf16, bool nhwc, const Geom& gm, int n
   a.mats = save_w; a.rec_stride = gm.GS * gm.GS; a.off[0] = 0; a.off[1] = 0;
   a.shift[0] = save_mean; a.shift_stride[0] = gm.C; a.shift[1] = nullptr; a.shift_stride[1] = 0;
   a.out = y;
-  launch_apply<1>(bf16, nhwc, dim3(nctas, (gm.C + kCh - 1) / kCh, gm.D), mx, mx, gm, a, st);
+  a.shift[1] = bias;                               // null: no bias
+  const dim3 grid(nctas, (gm.C + kCh - 1) / kCh, gm.D);
+  if (bias) launch_apply<1, true>(bf16, nhwc, grid, mx, mx, gm, a, st);
+  else launch_apply<1>(bf16, nhwc, grid, mx, mx, gm, a, st);
   return 0;
 }
 

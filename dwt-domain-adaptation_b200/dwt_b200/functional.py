@@ -417,6 +417,104 @@ def norm(x, gamma, beta, *, kind, group_size, n_domains, training_stats, eps, mo
     return _NormFunction.apply(x, gamma, beta, residual, *args, r, iterations)
 
 
+def _aligned(t):
+    """t as a contiguous float32 tensor whose data_ptr() is 16-byte aligned (the colouring entry points' rule)."""
+    t = t.detach().contiguous()
+    return t if t.data_ptr() % 16 == 0 else t.clone()
+
+
+class _ColorFunction(torch.autograd.Function):
+    """y = color_g W (x - mean) + bias (dwt_whiten_color_fwd / _bwd): whitening in the Cholesky basis followed by a
+    learnable per-group colouring matrix color [C/gs, gs, gs] and bias [C], both float32 and shared by the n_domains
+    domains of x.  Statistics, running buffers and the route r as in _NormFunction."""
+
+    @staticmethod
+    def forward(ctx, x, color, bias, group_size, n_domains, mode, eps, momentum, update_running, running, r):
+        lib = nv.lib()
+        gs = group_size
+        if not r.nhwc and not x.is_contiguous():
+            x = x.contiguous()
+        n_all, c, hw = x.shape[0], x.shape[1], math.prod(x.shape[2:])
+        layout = (nv.LAYOUT_NHWC if r.nhwc else 0) | (nv.DTYPE_BF16 if r.bf16 else 0)
+        if n_all % n_domains != 0:
+            raise ValueError(f"batch of {n_all} does not split into {n_domains} domains")
+        n = n_all // n_domains
+        stats = [color, bias, *[t for pair in running for t in pair]]
+        dev = nv.require_cuda(x, *stats, bf16=True)
+        nv.require_cuda(*stats)
+        for d, (rm_t, rv_t) in enumerate(running):
+            _check_param(f"running mean of domain {d}", rm_t, c)
+            _check_param(f"running second moment of domain {d}", rv_t, c * gs)
+        color_c, bias_c = _aligned(color), _aligned(bias)
+        _check_param("color / weight", color_c, c * gs)
+        _check_param("bias", bias_c, c)
+        y = torch.empty_like(x)
+        save_mean = torch.empty(n_domains, c, dtype=torch.float32, device=dev)
+        save_w = torch.empty(n_domains, c // gs, gs, gs, dtype=torch.float32, device=dev)
+        ws = nv.workspace(dev, n, c, hw, gs, n_domains)
+        need_running = (mode == nv.MODE_EVAL) or update_running
+        rm = nv.ptr_array([p[0] for p in running]) if need_running else None
+        rv = nv.ptr_array([p[1] for p in running]) if need_running else None
+        with torch.cuda.device(dev):
+            rc = lib.dwt_whiten_color_fwd(nv.ptr(x), nv.ptr(y), n, c, hw, gs, n_domains, mode | layout, eps, momentum,
+                                          int(update_running), rm, rv, nv.ptr(color_c), nv.ptr(bias_c), nv.ptr(save_mean),
+                                          nv.ptr(save_w), nv.ptr(ws), ws.numel(), nv.stream_ptr(dev))
+        nv.check(rc)
+        nv.poll_status(dev)
+        if update_running and mode == nv.MODE_TRAIN:
+            seen = set()                             # see _NormFunction.forward
+            for pair in running:
+                for buf in pair:
+                    if buf is not None and id(buf) not in seen:
+                        seen.add(id(buf))
+                        torch.autograd.graph.increment_version(buf)
+        ctx.save_for_backward(x, save_mean, save_w, color_c)
+        ctx.cfg = (gs, n_domains, mode | layout, eps, n, c, hw, color.shape, bias.shape)
+        ctx.route = r
+        return y
+
+    @staticmethod
+    def backward(ctx, dout):
+        lib = nv.lib()
+        x, save_mean, save_w, color_c = ctx.saved_tensors
+        gs, n_domains, mode, eps, n, c, hw, cshape, bshape = ctx.cfg
+        r = ctx.route
+        if dout.dtype != x.dtype:
+            dout = dout.to(x.dtype)
+        dout = dout.contiguous(memory_format=torch.channels_last) if r.nhwc else dout.contiguous()
+        if r.align and dout.data_ptr() % r.align:
+            dout = dout.clone(memory_format=torch.channels_last if r.nhwc else torch.contiguous_format)
+        dev = nv.require_cuda(dout, bf16=True)
+        dx = torch.empty_like(x)
+        want = ctx.needs_input_grad[1] or ctx.needs_input_grad[2]
+        dcolor = torch.empty(c // gs, gs, gs, dtype=torch.float32, device=dev) if want else None
+        dbias = torch.empty(c, dtype=torch.float32, device=dev) if want else None
+        ws = nv.workspace(dev, n, c, hw, gs, n_domains)
+        with torch.cuda.device(dev):
+            rc = lib.dwt_whiten_color_bwd(nv.ptr(x), nv.ptr(dout), nv.ptr(dx), n, c, hw, gs, n_domains, mode, eps,
+                                          nv.ptr(save_mean), nv.ptr(save_w), nv.ptr(color_c), nv.ptr(dcolor), nv.ptr(dbias),
+                                          nv.ptr(ws), ws.numel(), nv.stream_ptr(dev))
+        nv.check(rc)
+        if want:
+            dcolor, dbias = dcolor.view(cshape), dbias.view(bshape)
+        return (dx, dcolor, dbias) + (None,) * 8
+
+
+def color(x, weight, bias, *, group_size, n_domains, training_stats, eps, momentum, update_running, running):
+    """y = weight_g W (x - mean) + bias: whitening in the Cholesky basis, then the learnable colouring of each group of
+    group_size channels (weight [C/gs, gs, gs], bias with C elements, float32; see _ColorFunction).  The tensor-core
+    kernels only: a call they cannot take raises NativeError.  bf16 activations run the bf16 kernels where they are
+    built, else the float32 kernels on upcast copies (functional.norm's rule)."""
+    mode = nv.MODE_TRAIN if training_stats else nv.MODE_EVAL
+    args = (group_size, n_domains, mode, float(eps), float(momentum), bool(update_running), running)
+    r = route(x, None, "whiten", group_size, n_domains)
+    if r is None:
+        xf = x.float()
+        y = _ColorFunction.apply(xf, weight, bias, *args, route(xf, None, "whiten", group_size, n_domains))
+        return y.to(x.dtype)
+    return _ColorFunction.apply(x, weight, bias, *args, r)
+
+
 class _MecFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, y):

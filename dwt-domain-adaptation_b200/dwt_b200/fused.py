@@ -14,7 +14,9 @@ for the residual tail, the gradient of the identity branch.
 It owns no state: it borrows the running buffers of the three domain modules at call time, and with them their
 hyper-parameters -- eps, momentum and, for whitening, the basis: three ``ZCAWTransform2d`` modules make a ZCA site,
 three ``ExactZCAWTransform2d`` modules an exact-ZCA site (both on the tensor-core kernels, no fused epilogue), and
-modules that disagree on the basis are refused.
+modules that disagree on the basis are refused.  A matrix ``gamma`` [C/gs, gs, gs] with ``WTransform2d`` modules at group
+sizes 8..64 colours the site instead (the whitening-and-colouring transform, functional.color: y = gamma_g W (x - mean) +
+beta, one call for all domains).
 
 ``replicated=True`` is the statistics-collection pass (SURVEY.md §8f-3;
 resnet50_dwt_mec_officehome.py:380-389): the reference feeds ``cat((data, data, data))`` through
@@ -64,6 +66,8 @@ class DomainTripleNorm(nn.Module):
             raise ValueError(f"expected {self.n_domains} domain modules")
         if x.dim() != 4:
             raise ValueError('expected 4D input (got {}D input)'.format(x.dim()))
+        if gamma is not None and gamma.dim() == 3 and tuple(gamma.shape[1:]) != (1, 1):    # [C,1,1]: per channel
+            return self._forward_color(x, mods, gamma, beta, relu, residual, replicated, count_batches)
         if not self.kernel_epilogue and torch.bfloat16 in (x.dtype, getattr(residual, "dtype", None)):
             # the tensor epilogue would promote to float32 and round twice: the whole site in float32, rounded once
             out = self.forward(x.float(), mods, gamma, beta, relu, None if residual is None else residual.float(), replicated,
@@ -83,6 +87,31 @@ class DomainTripleNorm(nn.Module):
         return F.norm(x, gamma, beta, kind=self.kind, group_size=self.group_size, n_domains=self.n_domains,
                       training_stats=batch_stats, eps=eps, momentum=momentum, update_running=update,
                       running=running, relu=relu, residual=residual)
+
+    def _forward_color(self, x, mods, gamma, beta, relu, residual, replicated, count_batches):
+        """gamma [C/gs, gs, gs], beta [C] or [C,1,1]: the colouring transform in the whitening kernels (one call for all
+        domains, or the replicated pass); ReLU and the residual follow as tensor ops."""
+        gs = self.group_size
+        if self.kind != "whiten" or self.kernel_epilogue:
+            raise nv.NativeError("a matrix gamma (colouring) is built for whitening at group_size 8, 16, 32, 64 on the "
+                                 f"tensor-core kernels (got {self.kind}, group_size {gs})")
+        if self._iterations(mods):
+            raise nv.NativeError("a matrix gamma (colouring) whitens in the Cholesky basis: the domain modules must be "
+                                 "WTransform2d")
+        if tuple(gamma.shape) != (self.num_features // gs, gs, gs):
+            raise ValueError(f"a matrix gamma has shape [C/gs, gs, gs] = {[self.num_features // gs, gs, gs]}, "
+                             f"got {list(gamma.shape)}")
+        if residual is not None and not relu:
+            raise ValueError("a fused residual needs relu=True")
+        bias = beta.reshape(-1)
+        if replicated:
+            y = self._forward_replicated(x, mods, gamma, bias, False, None, count_batches, color=True)
+        else:
+            running, eps, momentum, update = self._running_args(mods, count_batches)
+            y = F.color(x, gamma, bias, group_size=gs, n_domains=self.n_domains,
+                        training_stats=mods[0].training or not mods[0].track_running_stats, eps=eps, momentum=momentum,
+                        update_running=update, running=running)
+        return self._tensor_epilogue(y, None, None, relu, residual)
 
     def _iterations(self, mods):
         """The whitening basis the domain modules share (functional.norm's iterations: 0 = Cholesky, "eigh" = exact ZCA)."""
@@ -152,11 +181,11 @@ class DomainTripleNorm(nn.Module):
             y = y + residual
         return torch.relu(y) if relu else y
 
-    def _forward_replicated(self, x, mods, gamma, beta, relu, residual, count_batches=True):
+    def _forward_replicated(self, x, mods, gamma, beta, relu, residual, count_batches=True, color=False):
         """One copy of the batch stands for all n_domains branches (see the module docstring).  The output is what
         mods[0] gives on x: batch statistics when it trains (or tracks no running statistics), its running buffers in
         eval -- normalised before any training branch that shares those buffers updates them, as in the reference's
-        order of calls."""
+        order of calls.  color: gamma is a colouring matrix (_forward_color); the output is returned without epilogue."""
         second = "running_variance" if self.kind == "whiten" else "running_var"
         keep = {}                                  # distinct buffer pair -> product of (1 - factor) over its branches
         for m in mods:
@@ -185,14 +214,19 @@ class DomainTripleNorm(nn.Module):
             g_arg, b_arg = gamma, beta
         else:
             g_arg = b_arg = None
+
+        def site(training_stats, momentum, update_running, running):
+            if color:
+                return F.color(x, gamma, beta, group_size=self.group_size, n_domains=1, training_stats=training_stats,
+                               eps=m0.eps, momentum=momentum, update_running=update_running, running=running)
+            return F.norm(x, g_arg, b_arg, momentum=momentum, update_running=update_running, running=running,
+                          **dict(common, training_stats=training_stats))
         out = None
         if not m0.training and m0.track_running_stats:
-            out = F.norm(x, g_arg, b_arg, momentum=0.0, update_running=False,
-                         running=[(m0.running_mean, getattr(m0, second))], **dict(common, training_stats=False))
+            out = site(False, 0.0, False, [(m0.running_mean, getattr(m0, second))])
         for prod, pair in keep.values():           # one launch per distinct buffer set (one, in a loaded model)
-            y = F.norm(x, g_arg, b_arg, momentum=1.0 - prod, update_running=True, running=[pair], **common)
+            y = site(True, 1.0 - prod, True, [pair])
             out = y if out is None else out
         if out is None:
-            out = F.norm(x, g_arg, b_arg, momentum=0.0, update_running=False,
-                         running=[(m0.running_mean, getattr(m0, second))], **common)
-        return out if self.kernel_epilogue else self._tensor_epilogue(out, gamma, beta, relu, residual)
+            out = site(True, 0.0, False, [(m0.running_mean, getattr(m0, second))])
+        return out if self.kernel_epilogue or color else self._tensor_epilogue(out, gamma, beta, relu, residual)

@@ -19,6 +19,7 @@
  *   dwt_whiten_bwd   autograd through the above     utils/whitening.py:41-55
  *   dwt_whiten_zca_fwd/bwd  the same layer in the ZCA basis (Newton-Schulz iteration; not in the reference)
  *   dwt_whiten_eigh_fwd/bwd the same layer in the exact ZCA basis (Jacobi eigendecomposition; not in the reference)
+ *   dwt_whiten_color_fwd/bwd whitening followed by a learnable per-group colouring matrix and bias (not in the reference)
  *   dwt_bn_fwd/bwd   _BatchNorm.forward             utils/batch_norm.py:54-69
  *   dwt_tail2_fwd/bwd  the residual tail of a downsampling Bottleneck: two norm sites and the ReLU in one pass
  *                    resnet50_dwt_mec_officehome.py:236-240
@@ -233,6 +234,34 @@ DWT_API int dwt_whiten_eigh_fwd(const float *x, float *y, int64_t N, int64_t C, 
 DWT_API int dwt_whiten_eigh_bwd(const float *x, const float *dout, float *dx, int64_t N, int64_t C, int64_t HW, int group_size,
                        int n_domains, int mode, float eps, const float *save_mean, const float *save_w,
                        const float *save_e, void *workspace, size_t workspace_bytes, dwt_stream_t stream);
+
+/*
+ * Whitening followed by a learnable colouring (the whitening-and-colouring transform of Siarohin, Sangineto and Sebe,
+ * "Whitening and Coloring Batch Transform", ICLR 2019), in the Cholesky basis of dwt_whiten_fwd:
+ *     y = color_g W (x - mean) + bias
+ *   color       [C/gs, gs, gs] (color_g: a full gs x gs matrix per group), bias [C]; shared by every domain of the call;
+ *               float32, 16-byte aligned (a null or misaligned pointer is DWT_E_INVALID)
+ *   save_w      W = L^-1 exactly as dwt_whiten_fwd writes it, bit for bit; color W lives in the workspace only
+ *   everything else as dwt_whiten_fwd without epilogue: statistics, shrinkage, running-buffer EMA, eval mode from the
+ *   running buffers, DWT_STATUS_NOT_PD (a not positive definite group skips its domain's EMA).
+ * dwt_whiten_color_bwd, with R_d = sum_m dout (x - mean)^T per domain and group, M = N*HW:
+ *   dcolor = sum_d R_d W_d^T,  dbias = sum_d sum_m dout   [C/gs, gs, gs] and [C], both or neither (NULL: not formed),
+ *               summed over the domains in a fixed order (reruns are bit-identical)
+ *   train: dx = W^T color^T (dout - mean_M dout) + Bm (x - mean), Bm the Cholesky backward of dwt_whiten_bwd on color^T R
+ *   eval:  dx = W^T color^T dout (no reduction pass unless dcolor / dbias are asked for)
+ * mode takes DWT_MODE_*, DWT_LAYOUT_NHWC and DWT_DTYPE_BF16, with dwt_whiten_zca_fwd's layout, dtype and alignment rules.
+ * Built for the tensor-core kernels only: group size 8, 16, 32, 64.  Every other group size (1, 2, 4, 128), every other
+ * geometry, and a call whose tensor-core kernels could not be set up is DWT_E_UNSUPPORTED with a text naming the
+ * colouring transform.  Workspace: dwt_workspace_bytes as for dwt_whiten_fwd.
+ * Profile families dense_fwd_color / dense_bwd_color (_bf16) for the per-group algebra; the other passes keep tc_*.
+ */
+DWT_API int dwt_whiten_color_fwd(const float *x, float *y, int64_t N, int64_t C, int64_t HW, int group_size, int n_domains,
+                       int mode, float eps, float momentum, int update_running, float *const *running_mean,
+                       float *const *running_cov, const float *color, const float *bias, float *save_mean, float *save_w,
+                       void *workspace, size_t workspace_bytes, dwt_stream_t stream);
+DWT_API int dwt_whiten_color_bwd(const float *x, const float *dout, float *dx, int64_t N, int64_t C, int64_t HW, int group_size,
+                       int n_domains, int mode, float eps, const float *save_mean, const float *save_w, const float *color,
+                       float *dcolor, float *dbias, void *workspace, size_t workspace_bytes, dwt_stream_t stream);
 
 /*
  * Domain batch norm (F.batch_norm semantics): biased batch variance normalises,
