@@ -830,11 +830,168 @@ int tail2_bwd(int kind, const dwt_tail_site* s, const float* dout, const float* 
   return check_launch("channels-last two-site backward apply kernel");
 }
 
+// ---- instance whitening (dwt_whiten_instance_fwd / dwt_whiten_instance_bwd) ------------------------------------------
+// Every image is its own problem.  The tensor-core kernels index their problems by (domain, super-block) and the dense
+// ones by (domain, group); instance whitening runs them with the images as the domains: Geom D = N images of N = 1 each,
+// M = HW.  Statistics and the backward contraction are tc_stats / tc_bwd_reduce unchanged (tc_chunks splits an image over
+// CTAs when there are fewer problems than two per SM, and gives a CTA a whole image otherwise -- then the partials are the
+// reduced moments and the fixed-order reduction is skipped); apply and backward apply are tc_apply / tc_bwd_apply
+// unchanged; the backward coefficients are bwd_coef unchanged (one CTA per (domain, group) already); the forward factor is
+// fwd_instance (fwd_factor serialises the domains of a group in one CTA for its ordered EMA).
+int inst_refuse(int64_t N, int64_t C, int64_t HW, int GS, int flags) {
+  return fail(DWT_E_UNSUPPORTED, "instance whitening is built for the tensor-core kernels only: group_size 8, 16, 32, 64 "
+              "dividing C, HW >= 256 and a multiple of 4 (NCHW bf16: of 8), N <= 65535 images, N*C*HW < 2^31 "
+              "(C=%lld HW=%lld N=%lld gs=%d flags=%#x)", (long long)C, (long long)HW, (long long)N, GS, flags);
+}
+
+// flags and geometry; fills gm (no device call)
+int inst_geom(dwt::Geom& gm, int64_t N, int64_t C, int64_t HW, int GS, int flags) {
+  if (flags & ~(DWT_LAYOUT_NHWC | DWT_DTYPE_BF16)) return fail(DWT_E_INVALID, "bad flags %#x (DWT_LAYOUT_NHWC | DWT_DTYPE_BF16)", flags);
+  if (N <= 0 || C <= 0 || HW <= 0) return fail(DWT_E_INVALID, "empty tensor (N=%lld C=%lld HW=%lld)", (long long)N,
+                                               (long long)C, (long long)HW);
+  const bool nchw_bf16 = (flags & DWT_DTYPE_BF16) && !(flags & DWT_LAYOUT_NHWC);
+  if ((GS != 8 && GS != 16 && GS != 32 && GS != 64) || C % GS != 0 || HW < 256 || HW % (nchw_bf16 ? 8 : 4) != 0 ||
+      N > 65535 || N * C * HW >= (int64_t)1 << 31)
+    return inst_refuse(N, C, HW, GS, flags);
+  gm = dwt::Geom{};
+  gm.N = 1; gm.C = (int)C; gm.HW = (int)HW; gm.GS = GS; gm.G = (int)(C / GS); gm.D = (int)N; gm.ppc = 1;
+  gm.M = (float)HW;
+  gm.nchunks = tc_chunks(gm);
+  return DWT_OK;
+}
+
+// Scratch behind the common head (the status word is shared with every other call on the stream's workspace):
+// partials [N][SB][nchunks][64*64+64], reduced moments (only when nchunks > 1), pilot shifts / mean of dy [N][SB][64],
+// backward coefficients [N][G][2 gs^2 + gs]
+Workspace carve_instance(void* base, const dwt::Geom& gm) {
+  const size_t P = (size_t)dwt::tc_superblocks(gm) * gm.D, nacc = 64 * 64 + 64;
+  size_t off = kOffScratch;
+  auto take = [&](size_t nbytes) { size_t o = off; off = align_up(off + nbytes, 256); return o; };
+  char* b = static_cast<char*>(base);
+  Workspace w{};
+  w.status = reinterpret_cast<int*>(b);
+  w.counters = reinterpret_cast<int*>(b + kOffCounters);
+  w.dom_counter = reinterpret_cast<int*>(b + kOffDom1);
+  w.dom_counter2 = reinterpret_cast<int*>(b + kOffDom2);
+  w.partial = reinterpret_cast<float*>(b + take(sizeof(float) * P * gm.nchunks * nacc));
+  w.gram = gm.nchunks > 1 ? reinterpret_cast<float*>(b + take(sizeof(float) * P * nacc)) : w.partial;
+  w.shift = reinterpret_cast<float*>(b + take(sizeof(float) * P * 64));
+  w.coef = reinterpret_cast<float*>(b + take(sizeof(float) * (size_t)gm.D * gm.G * dwt::coef_stride(gm.GS)));
+  w.bytes = off;
+  return w;
+}
+
+// Profile family of a launch: [pass][channels-last * 2 + bf16]
+const char* const kIwName[6][4] = {
+    {"iw_stats", "iw_stats_bf16", "iw_stats_nhwc", "iw_stats_nhwc_bf16"},
+    {"iw_fwd_finalize", "iw_fwd_finalize_bf16", "iw_fwd_finalize", "iw_fwd_finalize_bf16"},
+    {"iw_apply", "iw_apply_bf16", "iw_apply_nhwc", "iw_apply_nhwc_bf16"},
+    {"iw_bwd_reduce", "iw_bwd_reduce_bf16", "iw_bwd_reduce_nhwc", "iw_bwd_reduce_nhwc_bf16"},
+    {"iw_bwd_finalize", "iw_bwd_finalize_bf16", "iw_bwd_finalize", "iw_bwd_finalize_bf16"},
+    {"iw_bwd_apply", "iw_bwd_apply_bf16", "iw_bwd_apply_nhwc", "iw_bwd_apply_nhwc_bf16"}};
+
+// The checks both directions make, in order: flags and geometry, pointers, alignment, workspace, kernel set-up.
+// in0, in1: what the kernels read (x; x and dout); out: what they write (y; dx).
+int inst_validate(dwt::Geom& gm, Workspace& w, const void* in0, const void* in1, const void* out, int64_t N, int64_t C, int64_t HW,
+                  int GS, int flags, const float* save_mean, const float* save_w, void* ws, size_t ws_bytes) {
+  if (int rc = inst_geom(gm, N, C, HW, GS, flags)) return rc;
+  if (!in0 || !in1 || !out || !save_mean || !save_w || !ws) return fail(DWT_E_INVALID, "null pointer argument");
+  if (((uintptr_t)in0 | (uintptr_t)in1 | (uintptr_t)out | (uintptr_t)save_w) % 16 != 0)
+    return fail(DWT_E_INVALID, "activation tensors and save_w must be 16-byte aligned (instance whitening: TMA and vector stores)");
+  w = carve_instance(ws, gm);
+  if (w.bytes > ws_bytes) return fail(DWT_E_WORKSPACE, "workspace too small: need %zu bytes, got %zu", w.bytes, ws_bytes);
+  if ((uintptr_t)ws % 256 != 0) return fail(DWT_E_WORKSPACE, "workspace must be 256-byte aligned");
+  if (ensure_tc() != 0) return inst_refuse(N, C, HW, GS, flags);      // the tensor-core kernels could not be set up
+  return DWT_OK;
+}
+
+int instance_fwd(const void* x, void* y, int64_t N, int64_t C, int64_t HW, int GS, int flags, float eps, float* save_mean,
+                 float* save_w, void* ws, size_t ws_bytes, cudaStream_t st) {
+  dwt::Geom gm;
+  Workspace w;
+  if (int rc = inst_validate(gm, w, x, x, y, N, C, HW, GS, flags, save_mean, save_w, ws, ws_bytes)) return rc;
+  const bool nhwc = (flags & DWT_LAYOUT_NHWC) != 0, bf16 = (flags & DWT_DTYPE_BF16) != 0;
+  const int k = 2 * nhwc + bf16;
+  const double E = (bf16 ? 2.0 : 4.0) * (double)N * (double)C * (double)HW;
+  dwt::FwdFin fin{};
+  fin.a = 1.f - eps; fin.b = eps; fin.save_mean = save_mean; fin.save_w = save_w; fin.status = w.status;
+  {
+    Launch l(kIwName[0][k], &gm, E, st);
+    if (int cr = dwt::tc_stats(x, bf16, nhwc, gm, gm.nchunks, w.shift, w.partial, st))
+      return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d) x=%p N=%lld C=%d HW=%d", cr, x, (long long)N, gm.C, gm.HW);
+  }
+  if (int rc = check_launch("instance whitening statistics kernel")) return rc;
+  {
+    Launch l(kIwName[1][k], &gm, 0.0, st);
+    if (gm.nchunks > 1) dwt::dense_partial_reduce(w.partial, gm.nchunks, dwt::tc_superblocks(gm) * gm.D, w.gram, st);
+    dwt::dense_fwd_instance(w.gram, w.shift, gm, fin, st);
+  }
+  if (int rc = check_launch("instance whitening finalize kernel")) return rc;
+  {
+    Launch l(kIwName[2][k], &gm, 2.0 * E, st);
+    if (int cr = dwt::tc_apply(x, y, bf16, nhwc, gm, tc_apply_ctas(gm, 1, 64), save_mean, save_w, st))
+      return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d)", cr);
+  }
+  return check_launch("instance whitening apply kernel");
+}
+
+int instance_bwd(const void* x, const void* dout, void* dx, int64_t N, int64_t C, int64_t HW, int GS, int flags, float eps,
+                 const float* save_mean, const float* save_w, void* ws, size_t ws_bytes, cudaStream_t st) {
+  dwt::Geom gm;
+  Workspace w;
+  if (int rc = inst_validate(gm, w, x, dout, dx, N, C, HW, GS, flags, save_mean, save_w, ws, ws_bytes)) return rc;
+  const bool nhwc = (flags & DWT_LAYOUT_NHWC) != 0, bf16 = (flags & DWT_DTYPE_BF16) != 0;
+  const int k = 2 * nhwc + bf16;
+  const double E = (bf16 ? 2.0 : 4.0) * (double)N * (double)C * (double)HW;
+  dwt::BwdFin fin{};
+  fin.a = 1.f - eps; fin.mode = DWT_MODE_TRAIN; fin.save_mean = save_mean; fin.save_w = save_w; fin.coef = w.coef;
+  {
+    Launch l(kIwName[3][k], &gm, 2.0 * E, st);
+    if (int cr = dwt::tc_bwd_reduce(x, dout, bf16, nhwc, gm, gm.nchunks, save_mean, w.partial, st))
+      return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d) x=%p dout=%p N=%lld C=%d HW=%d", cr, x, dout,
+                  (long long)N, gm.C, gm.HW);
+  }
+  if (int rc = check_launch("instance whitening backward reduction kernel")) return rc;
+  {
+    Launch l(kIwName[4][k], &gm, 0.0, st);
+    if (gm.nchunks > 1) dwt::dense_partial_reduce(w.partial, gm.nchunks, dwt::tc_superblocks(gm) * gm.D, w.gram, st);
+    dwt::dense_bwd_coef(w.gram, gm, fin, w.shift, st);                 // w.shift: mean_M dy per (image, channel)
+  }
+  if (int rc = check_launch("instance whitening backward finalize kernel")) return rc;
+  {
+    Launch l(kIwName[5][k], &gm, 3.0 * E, st);
+    if (int cr = dwt::tc_bwd_apply(x, dout, dx, bf16, nhwc, gm, tc_apply_ctas(gm, 1, 64), w.coef, save_mean, w.shift, st))
+      return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d)", cr);
+  }
+  return check_launch("instance whitening backward apply kernel");
+}
+
 }  // namespace
 
 extern "C" {
 
 int dwt_abi_version(void) { return DWT_B200_ABI_VERSION; }
+
+size_t dwt_instance_workspace_bytes(int64_t N, int64_t C, int64_t HW, int group_size) {
+  dwt::Geom gm;
+  char saved[sizeof(g_err)];
+  memcpy(saved, g_err, sizeof(g_err));            // a size query leaves the last error text alone
+  const int rc = inst_geom(gm, N, C, HW, group_size, 0);
+  memcpy(g_err, saved, sizeof(g_err));
+  return rc ? 0 : carve_instance(nullptr, gm).bytes;
+}
+
+int dwt_whiten_instance_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, int group_size, int flags, float eps,
+                            float* save_mean, float* save_w, void* workspace, size_t workspace_bytes, dwt_stream_t stream) {
+  return instance_fwd(x, y, N, C, HW, group_size, flags, eps, save_mean, save_w, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int dwt_whiten_instance_bwd(const float* x, const float* dout, float* dx, int64_t N, int64_t C, int64_t HW, int group_size,
+                            int flags, float eps, const float* save_mean, const float* save_w, void* workspace,
+                            size_t workspace_bytes, dwt_stream_t stream) {
+  return instance_bwd(x, dout, dx, N, C, HW, group_size, flags, eps, save_mean, save_w, workspace, workspace_bytes,
+                      (cudaStream_t)stream);
+}
 
 const char* dwt_last_error(void) { return g_err; }
 

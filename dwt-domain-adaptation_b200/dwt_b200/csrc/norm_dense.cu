@@ -14,6 +14,8 @@
 //                    eigensolver in shared memory, and the Daleckii-Krein backward; the same prologue and EMA tail
 //   fwd_factor<COLOR>, bwd_color  colouring (dwt_whiten_color_*): fwd_factor also writes color W; bwd_color runs bwd_coef's
 //                    algebra on color^T R, domains in order in one CTA per group, and sums dcolor and dbias over them
+//   fwd_instance     instance whitening (dwt_whiten_instance_*): fwd_factor's prologue and factorisation, one CTA per
+//                    (image, group), no EMA; its backward is bwd_coef as it is, with the images as the domains
 //
 // All three keep a 64x64 problem in ONE 256-thread CTA arranged 16x16, each thread owning a 4x4
 // register block.  fwd_factor runs the Cholesky factorisation AND the triangular inverse as one blocked
@@ -1255,6 +1257,40 @@ __global__ void __launch_bounds__(kThreads2) bwd_coef128_kernel(const float* __r
   bwd_finalize_block(gm, f, d, g, sR, sSdz, sW, sT1, sR, sVec, &s_flag);
 }
 
+// ------------------------------------------------------------------------------------------
+// fwd_instance: instance whitening (dwt_whiten_instance_fwd), grid (G, 1, D), 256 threads, one CTA per (image, group):
+// the Geom's domains are the images (N = 1, M = HW).  fwd_factor's statistics prologue and blocked Cholesky + inverse,
+// without the EMA and without its loop over the domains: fwd_factor serialises them in one CTA per group, which at
+// hundreds of images would leave all but G CTAs of the H100 idle.  A group whose S is not positive definite (or not
+// finite) gets W = NaN in full, so that image's whole group reads NaN, and sets DWT_STATUS_NOT_PD.
+// ------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) fwd_instance_kernel(const float* __restrict__ gram, const float* __restrict__ shift,
+                                                           const Geom gm, const FwdFin f) {
+  __shared__ __align__(16) PanelSmem sp;
+  __shared__ float sC[kMat];       // written by domain_stats, not read (no EMA)
+  __shared__ float sMean[kSB], sRow[kSB];
+  __shared__ int sBadDom;
+  const int g = blockIdx.x, d = blockIdx.z, GS = gm.GS, nb = kSB / GS, sb = g / nb, o = (g % nb) * GS;
+  const Blk t(GS);
+  const int SB = (gm.C + kSB - 1) / kSB;
+  const float* G = gram + ((size_t)d * SB + sb) * kNacc;
+  float a[4][4], w[4][4];
+  EmaOld old;                      // f.update_running is 0: domain_stats reads no running buffer
+  domain_stats(G, shift, d, g, sb, o, SB, 1.f / gm.M, gm, f, t, sC, sMean, sRow, sBadDom, a, old);
+  if (!factor_and_invert(a, w, GS, t, sp)) sBadDom = 1;
+  __syncthreads();                 // sBadDom final
+  const bool bad = sBadDom != 0;
+  if (t.act) {
+    float* wout = f.save_w + ((size_t)d * gm.G + g) * GS * GS;
+    const float q = __int_as_float(0x7fc00000);   // a NaN the apply's TF32 split keeps (0x7fffffff would round to -0)
+#pragma unroll
+    for (int r = 0; r < 4; ++r)
+      *reinterpret_cast<float4*>(wout + (size_t)(4 * t.bi + r) * GS + 4 * t.bj) =
+          bad ? make_float4(q, q, q, q) : make_float4(w[r][0], w[r][1], w[r][2], w[r][3]);
+  }
+  if (threadIdx.x == 0 && bad) atomicOr(f.status, DWT_STATUS_NOT_PD);
+}
+
 constexpr size_t kFactorSmem = 0;   // fwd_factor: static shared memory only (panel buffers + covariance)
 constexpr size_t kCoefSmem = sizeof(float) * 4 * kMat;
 constexpr size_t kZcaFwdSmem = sizeof(float) * 4 * kMat;   // N, P, P^2, P^3 (66.6 KB; + 16.9 KB static)
@@ -1331,6 +1367,10 @@ void dense_fwd_color(const float* gram, const float* shift, const Geom& gm, cons
 void dense_bwd_color(const float* rgram, const Geom& gm, const BwdFin& fin, const float* color, float* dcolor, float* dbias,
                      float* dybar, cudaStream_t st) {
   bwd_color_kernel<<<gm.G, 256, kColorBwdSmem, st>>>(rgram, gm, fin, color, dcolor, dbias, dybar);
+}
+
+void dense_fwd_instance(const float* gram, const float* shift, const Geom& gm, const FwdFin& fin, cudaStream_t st) {
+  fwd_instance_kernel<<<dim3(gm.G, 1, gm.D), 256, 0, st>>>(gram, shift, gm, fin);
 }
 
 }  // namespace dwt

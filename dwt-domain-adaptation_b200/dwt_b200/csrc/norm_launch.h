@@ -82,6 +82,9 @@ void dense_fwd_color(const float* gram, const float* shift, const Geom& gm, cons
                      cudaStream_t st);
 void dense_bwd_color(const float* rgram, const Geom& gm, const BwdFin& fin, const float* color, float* dcolor, float* dbias,
                      float* dybar, cudaStream_t st);
+// instance whitening, group sizes 8..64 (dwt_whiten_instance_*; gm.D = images, gm.N = 1): fwd_factor's work with one CTA
+// per (image, group) and no EMA, W = NaN for a group that is not positive definite.  The backward is dense_bwd_coef.
+void dense_fwd_instance(const float* gram, const float* shift, const Geom& gm, const FwdFin& fin, cudaStream_t st);
 
 // TMA + wgmma apply path (norm_tc_apply.cu): split-TF32 GEMM of the block-diagonal group matrices
 int tc_apply_init();

@@ -515,6 +515,70 @@ def color(x, weight, bias, *, group_size, n_domains, training_stats, eps, moment
     return _ColorFunction.apply(x, weight, bias, *args, r)
 
 
+class _InstanceFunction(torch.autograd.Function):
+    """Instance whitening (dwt_whiten_instance_fwd / _bwd): every image of x [N, C, *] whitened by the mean and covariance
+    of its own pixels, per group of group_size channels, in the Cholesky basis.  No running statistics; the gradient
+    always flows through the per-image mean and covariance.  x is float32 or bfloat16, NCHW-contiguous or (4-D)
+    channels-last; it goes to the kernels in its own layout and dtype."""
+
+    @staticmethod
+    def forward(ctx, x, group_size, eps):
+        dev = nv.require_cuda(x, bf16=True)
+        lib = nv.lib()
+        gs = group_size
+        nhwc = _channels_last(x)
+        fmt = torch.channels_last if nhwc else torch.contiguous_format
+        x = x.contiguous(memory_format=fmt)
+        if x.data_ptr() % 16:                        # the kernels read x through TMA
+            x = x.clone(memory_format=fmt)
+        n, c, hw = x.shape[0], x.shape[1], math.prod(x.shape[2:])
+        flags = (nv.LAYOUT_NHWC if nhwc else 0) | (nv.DTYPE_BF16 if x.dtype == torch.bfloat16 else 0)
+        y = torch.empty_like(x)
+        save_mean = torch.empty(n, c, dtype=torch.float32, device=dev)
+        save_w = torch.empty(n, max(c // gs, 1), gs, gs, dtype=torch.float32, device=dev)
+        ws = nv.instance_workspace(dev, n, c, hw, gs)
+        with torch.cuda.device(dev):
+            rc = lib.dwt_whiten_instance_fwd(nv.ptr(x), nv.ptr(y), n, c, hw, gs, flags, eps, nv.ptr(save_mean),
+                                             nv.ptr(save_w), nv.ptr(ws), ws.numel(), nv.stream_ptr(dev))
+        nv.check(rc)
+        nv.poll_status(dev)
+        ctx.save_for_backward(x, save_mean, save_w)
+        ctx.cfg = (gs, flags, eps, n, c, hw, fmt)
+        return y
+
+    @staticmethod
+    def backward(ctx, dout):
+        lib = nv.lib()
+        x, save_mean, save_w = ctx.saved_tensors
+        gs, flags, eps, n, c, hw, fmt = ctx.cfg
+        dout = dout.to(x.dtype).contiguous(memory_format=fmt)
+        if dout.data_ptr() % 16:
+            dout = dout.clone(memory_format=fmt)
+        dev = nv.require_cuda(dout, bf16=True)
+        dx = torch.empty_like(x)
+        ws = nv.instance_workspace(dev, n, c, hw, gs)
+        with torch.cuda.device(dev):
+            rc = lib.dwt_whiten_instance_bwd(nv.ptr(x), nv.ptr(dout), nv.ptr(dx), n, c, hw, gs, flags, eps, nv.ptr(save_mean),
+                                             nv.ptr(save_w), nv.ptr(ws), ws.numel(), nv.stream_ptr(dev))
+        nv.check(rc)
+        return dx, None, None
+
+
+def instance_whiten(x, *, group_size, eps):
+    """Instance whitening of x [N, C, *]: per image n and group g of group_size channels, with M pixels,
+    S = (1 - eps) cov + eps I of the image's own (biased) covariance, W = inverse(cholesky(S)), y = W (x - mean).
+    The tensor-core kernels only (group sizes 8, 16, 32, 64, H*W >= 256; dwt_b200.h): a call they cannot take raises
+    NativeError with the library's reason and is never sent to another kernel family.  A bfloat16 NCHW x whose H*W is not
+    a multiple of 8 (the bf16 kernels' TMA rows) runs the same kernels in float32 on an upcast copy, the result in
+    bfloat16."""
+    if x.dim() < 3:
+        raise ValueError(f"instance whitening expects [N, C, *] input (got {x.dim()}D input)")
+    nv.require_cuda(x, bf16=True)
+    if x.dtype == torch.bfloat16 and not _channels_last(x) and math.prod(x.shape[2:]) % 8:
+        return _InstanceFunction.apply(x.float(), int(group_size), float(eps)).to(x.dtype)
+    return _InstanceFunction.apply(x, int(group_size), float(eps))
+
+
 class _MecFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, y):

@@ -20,6 +20,7 @@
  *   dwt_whiten_zca_fwd/bwd  the same layer in the ZCA basis (Newton-Schulz iteration; not in the reference)
  *   dwt_whiten_eigh_fwd/bwd the same layer in the exact ZCA basis (Jacobi eigendecomposition; not in the reference)
  *   dwt_whiten_color_fwd/bwd whitening followed by a learnable per-group colouring matrix and bias (not in the reference)
+ *   dwt_whiten_instance_fwd/bwd  instance whitening: each image by its own statistics (not in the reference)
  *   dwt_bn_fwd/bwd   _BatchNorm.forward             utils/batch_norm.py:54-69
  *   dwt_tail2_fwd/bwd  the residual tail of a downsampling Bottleneck: two norm sites and the ReLU in one pass
  *                    resnet50_dwt_mec_officehome.py:236-240
@@ -262,6 +263,44 @@ DWT_API int dwt_whiten_color_fwd(const float *x, float *y, int64_t N, int64_t C,
 DWT_API int dwt_whiten_color_bwd(const float *x, const float *dout, float *dx, int64_t N, int64_t C, int64_t HW, int group_size,
                        int n_domains, int mode, float eps, const float *save_mean, const float *save_w, const float *color,
                        float *dcolor, float *dbias, void *workspace, size_t workspace_bytes, dwt_stream_t stream);
+
+/*
+ * Instance whitening: every image whitened by its own statistics (the per-sample whitening of Switchable Whitening,
+ * Pan et al., ICCV 2019; the instance-whitening statistic of RobustNet, Choi et al., CVPR 2021; the whitening step of
+ * WCT style transfer, Li et al., NeurIPS 2017).  It is to dwt_whiten_fwd what InstanceNorm is to BatchNorm.  Per image n
+ * and group g, with M = HW:
+ *     mean = sum_pixels x / M,  cov = (x - mean)(x - mean)^T / M (biased),  S = (1-eps) cov + eps I = L L^T,
+ *     W = L^-1,  y = W (x - mean).
+ * No running buffers and no modes: training and inference compute the same thing, and dwt_whiten_instance_bwd always
+ * differentiates through mean and cov (the closed form of dwt_whiten_bwd per image, with R = sum_pixels dout (x-mean)^T):
+ *     dx = W^T (dout - mean_M dout) + Bm (x - mean),  Bm = (2 (1-eps) / M) sym(W^T Phi(-R W^T) W).
+ *   x, y, dout, dx  [N, C, HW] (or channels-last [N, HW, C] with DWT_LAYOUT_NHWC), fp32 or bf16 (DWT_DTYPE_BF16)
+ *   flags           DWT_LAYOUT_NHWC | DWT_DTYPE_BF16 (any other bit: DWT_E_INVALID)
+ *   save_mean       [N, C] per-image mean;  save_w [N, C/gs, gs, gs] per-image W (16-byte aligned); written by fwd,
+ *                   read by bwd
+ * The statistics, factorisation, apply and backward are the tensor-core whitening kernels with the images as the domains
+ * (same split-TF32 arithmetic, pilot shift and fixed-order reductions: reruns are bit-identical).  bf16 loads widen to
+ * fp32 and stores round to nearest-even: every bf16 output is the fp32 call's output on the widened input, rounded.
+ * Channels-last outputs are bit for bit those of the NCHW call on the same values.
+ * Built for group size 8, 16, 32, 64 dividing C, HW >= 256 and HW % 4 == 0 (NCHW bf16: HW % 8 == 0), N <= 65535 and
+ * N*C*HW < 2^31; there is no floor on N or N*HW.  Anything else -- and a call whose tensor-core kernels could not be set
+ * up -- is DWT_E_UNSUPPORTED with a text naming instance whitening.  x, y, dout, dx and save_w must be 16-byte aligned
+ * (else DWT_E_INVALID).  Every n_domains rule of the other entry points (DWT_MAX_DOMAINS) is unchanged: this family has
+ * no domain count.
+ * Status: an (image, group) whose S is not positive definite or not finite sets DWT_STATUS_NOT_PD, and its W, and so its
+ * output and its dx, are NaN; other images and groups are not affected.
+ * Workspace: dwt_instance_workspace_bytes(N, C, HW, group_size) bytes, 256-byte aligned, zero-filled once (it may be the
+ * same buffer as the other entry points'; the status word is shared).  It returns 0 for a geometry the entry points refuse.
+ * Profile families iw_stats, iw_fwd_finalize, iw_apply, iw_bwd_reduce, iw_bwd_finalize, iw_bwd_apply (_nhwc, _bf16);
+ * the geometry in the profile name reports the images as domains of one image each.
+ */
+DWT_API size_t dwt_instance_workspace_bytes(int64_t N, int64_t C, int64_t HW, int group_size);
+DWT_API int dwt_whiten_instance_fwd(const float *x, float *y, int64_t N, int64_t C, int64_t HW, int group_size, int flags,
+                       float eps, float *save_mean, float *save_w, void *workspace, size_t workspace_bytes,
+                       dwt_stream_t stream);
+DWT_API int dwt_whiten_instance_bwd(const float *x, const float *dout, float *dx, int64_t N, int64_t C, int64_t HW,
+                       int group_size, int flags, float eps, const float *save_mean, const float *save_w, void *workspace,
+                       size_t workspace_bytes, dwt_stream_t stream);
 
 /*
  * Domain batch norm (F.batch_norm semantics): biased batch variance normalises,
