@@ -87,6 +87,15 @@ _SIGNATURES = {
     "dwt_whiten_instance_bwd": (ctypes.c_int, [_c_float_p, _c_float_p, _c_float_p, ctypes.c_int64, ctypes.c_int64,
                                                ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_float, _c_float_p,
                                                _c_float_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]),
+    "dwt_switch_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int64, ctypes.c_int64, ctypes.c_int64, ctypes.c_int]),
+    "dwt_whiten_switch_fwd": (ctypes.c_int, [_c_float_p, _c_float_p, ctypes.c_int64, ctypes.c_int64, ctypes.c_int64,
+                                             ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_int,
+                                             _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
+                                             ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]),
+    "dwt_whiten_switch_bwd": (ctypes.c_int, [_c_float_p, _c_float_p, _c_float_p, ctypes.c_int64, ctypes.c_int64,
+                                             ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_float, _c_float_p,
+                                             _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_void_p,
+                                             ctypes.c_size_t, ctypes.c_void_p]),
     "dwt_bn_fwd": (ctypes.c_int, [_c_float_p, _c_float_p, ctypes.c_int64, ctypes.c_int64, ctypes.c_int64,
                                   ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_int,
                                   ctypes.POINTER(ctypes.c_void_p), ctypes.POINTER(ctypes.c_void_p), _c_float_p,
@@ -273,6 +282,17 @@ def instance_workspace(device, n, c, hw, gs):
     """The current stream's workspace (see workspace()), grown to what instance whitening of [n, c, hw] at group size gs
     needs (dwt_instance_workspace_bytes; 0 for a geometry the entry points refuse, which then report why)."""
     need = lib().dwt_instance_workspace_bytes(n, c, hw, gs)
+    buf = workspace(device, 1, 4, 1, 1, 1)
+    if buf.numel() < need:
+        buf = torch.zeros(need, dtype=torch.uint8, device=device)
+        _workspaces[(device.index, torch.cuda.current_stream(device).cuda_stream)] = buf
+    return buf
+
+
+def switch_workspace(device, n, c, hw, gs):
+    """The current stream's workspace (see workspace()), grown to what switchable whitening of [n, c, hw] at group size gs
+    needs (dwt_switch_workspace_bytes; 0 for a geometry the entry points refuse, which then report why)."""
+    need = lib().dwt_switch_workspace_bytes(n, c, hw, gs)
     buf = workspace(device, 1, 4, 1, 1, 1)
     if buf.numel() < need:
         buf = torch.zeros(need, dtype=torch.uint8, device=device)

@@ -838,21 +838,22 @@ int tail2_bwd(int kind, const dwt_tail_site* s, const float* dout, const float* 
 // reduced moments and the fixed-order reduction is skipped); apply and backward apply are tc_apply / tc_bwd_apply
 // unchanged; the backward coefficients are bwd_coef unchanged (one CTA per (domain, group) already); the forward factor is
 // fwd_instance (fwd_factor serialises the domains of a group in one CTA for its ordered EMA).
-int inst_refuse(int64_t N, int64_t C, int64_t HW, int GS, int flags) {
-  return fail(DWT_E_UNSUPPORTED, "instance whitening is built for the tensor-core kernels only: group_size 8, 16, 32, 64 "
+// what: the family the refusal text names (switchable whitening shares the geometry)
+int inst_refuse(int64_t N, int64_t C, int64_t HW, int GS, int flags, const char* what = "instance whitening") {
+  return fail(DWT_E_UNSUPPORTED, "%s is built for the tensor-core kernels only: group_size 8, 16, 32, 64 "
               "dividing C, HW >= 256 and a multiple of 4 (NCHW bf16: of 8), N <= 65535 images, N*C*HW < 2^31 "
-              "(C=%lld HW=%lld N=%lld gs=%d flags=%#x)", (long long)C, (long long)HW, (long long)N, GS, flags);
+              "(C=%lld HW=%lld N=%lld gs=%d flags=%#x)", what, (long long)C, (long long)HW, (long long)N, GS, flags);
 }
 
 // flags and geometry; fills gm (no device call)
-int inst_geom(dwt::Geom& gm, int64_t N, int64_t C, int64_t HW, int GS, int flags) {
+int inst_geom(dwt::Geom& gm, int64_t N, int64_t C, int64_t HW, int GS, int flags, const char* what = "instance whitening") {
   if (flags & ~(DWT_LAYOUT_NHWC | DWT_DTYPE_BF16)) return fail(DWT_E_INVALID, "bad flags %#x (DWT_LAYOUT_NHWC | DWT_DTYPE_BF16)", flags);
   if (N <= 0 || C <= 0 || HW <= 0) return fail(DWT_E_INVALID, "empty tensor (N=%lld C=%lld HW=%lld)", (long long)N,
                                                (long long)C, (long long)HW);
   const bool nchw_bf16 = (flags & DWT_DTYPE_BF16) && !(flags & DWT_LAYOUT_NHWC);
   if ((GS != 8 && GS != 16 && GS != 32 && GS != 64) || C % GS != 0 || HW < 256 || HW % (nchw_bf16 ? 8 : 4) != 0 ||
       N > 65535 || N * C * HW >= (int64_t)1 << 31)
-    return inst_refuse(N, C, HW, GS, flags);
+    return inst_refuse(N, C, HW, GS, flags, what);
   gm = dwt::Geom{};
   gm.N = 1; gm.C = (int)C; gm.HW = (int)HW; gm.GS = GS; gm.G = (int)(C / GS); gm.D = (int)N; gm.ppc = 1;
   gm.M = (float)HW;
@@ -966,6 +967,148 @@ int instance_bwd(const void* x, const void* dout, void* dx, int64_t N, int64_t C
   return check_launch("instance whitening backward apply kernel");
 }
 
+// ---- switchable whitening (dwt_whiten_switch_fwd / dwt_whiten_switch_bwd) --------------------------------------------
+// Instance whitening's passes with the images as the domains (inst_geom), plus the batch moments and the mixture.
+// Forward: tc_stats (per-image moments) -> [partial_reduce] sw_stats (save_stats: per-image rows and the batch row by the
+// law of total covariance, no second pass over x) -> sw_fwd_factor (mix, Cholesky + inverse, EMA) -> tc_apply with the
+// per-image W and mixed mean.  Backward: tc_bwd_reduce about the mixed mean without the pilot centring (sum (x - m) is not
+// zero) -> [partial_reduce] sw_bwd_coef / sw_bwd_sum / sw_dmix / sw_bwd_apply_coef -> tc_bwd_apply, centred on the images'
+// own means, with the per-image constant of dx carried by dybar.
+constexpr const char* kSw = "switchable whitening";
+
+struct SwWork {
+  Workspace w;
+  float* pd;       // [N][G][gs*gs + gs]  P_n | dm_n
+  float* part;     // [N][G][8]           dmix terms per (image, group)
+  float* sums;     // [G][gs*gs + gs]     sum_n P_n | sum_n dm_n
+  float* mu;       // [N][C]              the images' own means (the backward apply's centre)
+};
+
+// Scratch behind the common head: instance whitening's (partials, reduced moments, shifts / dybar, coefficients), then
+// pd, part, sums and mu
+SwWork carve_switch(void* base, const dwt::Geom& gm) {
+  SwWork s{};
+  s.w = carve_instance(base, gm);
+  const size_t rec = (size_t)gm.GS * gm.GS + gm.GS, P = (size_t)gm.D * gm.G;
+  size_t off = s.w.bytes;
+  auto take = [&](size_t nbytes) { size_t o = off; off = align_up(off + nbytes, 256); return o; };
+  char* b = static_cast<char*>(base);
+  s.pd = reinterpret_cast<float*>(b + take(sizeof(float) * P * rec));
+  s.part = reinterpret_cast<float*>(b + take(sizeof(float) * P * 8));
+  s.sums = reinterpret_cast<float*>(b + take(sizeof(float) * gm.G * rec));
+  s.mu = reinterpret_cast<float*>(b + take(sizeof(float) * (size_t)gm.D * gm.C));
+  s.w.bytes = off;
+  return s;
+}
+
+int sw_geom(dwt::Geom& gm, int64_t N, int64_t C, int64_t HW, int GS, int mode) {
+  if (mode & ~(DWT_MODE_EVAL | DWT_LAYOUT_NHWC | DWT_DTYPE_BF16))
+    return fail(DWT_E_INVALID, "bad mode %#x (DWT_MODE_TRAIN or DWT_MODE_EVAL | DWT_LAYOUT_NHWC | DWT_DTYPE_BF16)", mode);
+  return inst_geom(gm, N, C, HW, GS, mode & ~DWT_MODE_EVAL, kSw);
+}
+
+// Profile family of a launch: [pass][channels-last * 2 + bf16]
+const char* const kSwName[6][4] = {
+    {"sw_stats", "sw_stats_bf16", "sw_stats_nhwc", "sw_stats_nhwc_bf16"},
+    {"sw_fwd_finalize", "sw_fwd_finalize_bf16", "sw_fwd_finalize", "sw_fwd_finalize_bf16"},
+    {"sw_apply", "sw_apply_bf16", "sw_apply_nhwc", "sw_apply_nhwc_bf16"},
+    {"sw_bwd_reduce", "sw_bwd_reduce_bf16", "sw_bwd_reduce_nhwc", "sw_bwd_reduce_nhwc_bf16"},
+    {"sw_bwd_finalize", "sw_bwd_finalize_bf16", "sw_bwd_finalize", "sw_bwd_finalize_bf16"},
+    {"sw_bwd_apply", "sw_bwd_apply_bf16", "sw_bwd_apply_nhwc", "sw_bwd_apply_nhwc_bf16"}};
+
+// The checks both directions make, in order: mode and geometry, pointers, alignment, workspace, kernel set-up.
+// in0, in1: what the kernels read (x; x and dout); out: what they write (y; dx).
+int sw_validate(dwt::Geom& gm, SwWork& s, const void* in0, const void* in1, const void* out, int64_t N, int64_t C, int64_t HW,
+                int GS, int mode, const float* mix, const float* save_mean, const float* save_w, const float* save_stats,
+                void* ws, size_t ws_bytes, bool running_missing = false) {
+  if (int rc = sw_geom(gm, N, C, HW, GS, mode)) return rc;
+  if (!in0 || !in1 || !out || !mix || !save_mean || !save_w || !save_stats || !ws) return fail(DWT_E_INVALID, "null pointer argument");
+  if (running_missing) return fail(DWT_E_INVALID, "running buffer is null (eval, or train with update_running)");
+  if (((uintptr_t)in0 | (uintptr_t)in1 | (uintptr_t)out | (uintptr_t)save_w | (uintptr_t)save_stats | (uintptr_t)mix) % 16 != 0)
+    return fail(DWT_E_INVALID, "activation tensors, mix, save_w and save_stats must be 16-byte aligned (switchable whitening)");
+  s = carve_switch(ws, gm);
+  if (s.w.bytes > ws_bytes) return fail(DWT_E_WORKSPACE, "workspace too small: need %zu bytes, got %zu", s.w.bytes, ws_bytes);
+  if ((uintptr_t)ws % 256 != 0) return fail(DWT_E_WORKSPACE, "workspace must be 256-byte aligned");
+  if (ensure_tc() != 0) return inst_refuse(N, C, HW, GS, mode & ~DWT_MODE_EVAL, kSw);   // the tensor-core kernels could not be set up
+  return DWT_OK;
+}
+
+dwt::SwFin make_sw_fin(int mode, float eps, const float* mix, float* save_mean, float* save_w, float* save_stats, int* status) {
+  dwt::SwFin f{};
+  f.a = 1.f - eps; f.b = eps; f.train = (mode & DWT_MODE_EVAL) == 0; f.mix = mix;
+  f.save_mean = save_mean; f.save_w = save_w; f.save_stats = save_stats; f.status = status;
+  return f;
+}
+
+int switch_fwd(const void* x, void* y, int64_t N, int64_t C, int64_t HW, int GS, int mode, float eps, float momentum,
+               int update_running, float* running_mean, float* running_cov, const float* mix, float* save_mean, float* save_w,
+               float* save_stats, void* ws, size_t ws_bytes, cudaStream_t st) {
+  dwt::Geom gm;
+  SwWork s;
+  const bool train = (mode & DWT_MODE_EVAL) == 0;
+  const bool running_missing = (!train || update_running) && (!running_mean || !running_cov);
+  if (int rc = sw_validate(gm, s, x, x, y, N, C, HW, GS, mode, mix, save_mean, save_w, save_stats, ws, ws_bytes, running_missing))
+    return rc;
+  const bool nhwc = (mode & DWT_LAYOUT_NHWC) != 0, bf16 = (mode & DWT_DTYPE_BF16) != 0;
+  const int k = 2 * nhwc + bf16;
+  const double E = (bf16 ? 2.0 : 4.0) * (double)N * (double)C * (double)HW;
+  dwt::SwFin fin = make_sw_fin(mode, eps, mix, save_mean, save_w, save_stats, s.w.status);
+  fin.momentum = momentum; fin.update_running = train && update_running;
+  fin.rmean = running_mean; fin.rcov = running_cov;
+  {
+    Launch l(kSwName[0][k], &gm, E, st);
+    if (int cr = dwt::tc_stats(x, bf16, nhwc, gm, gm.nchunks, s.w.shift, s.w.partial, st))
+      return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d) x=%p N=%lld C=%d HW=%d", cr, x, (long long)N, gm.C, gm.HW);
+  }
+  if (int rc = check_launch("switchable whitening statistics kernel")) return rc;
+  {
+    Launch l(kSwName[1][k], &gm, 0.0, st);
+    if (gm.nchunks > 1) dwt::dense_partial_reduce(s.w.partial, gm.nchunks, dwt::tc_superblocks(gm) * gm.D, s.w.gram, st);
+    dwt::dense_sw_stats(s.w.gram, s.w.shift, gm, fin, st);
+    dwt::dense_sw_fwd_factor(gm, fin, st);
+  }
+  if (int rc = check_launch("switchable whitening finalize kernel")) return rc;
+  {
+    Launch l(kSwName[2][k], &gm, 2.0 * E, st);
+    if (int cr = dwt::tc_apply(x, y, bf16, nhwc, gm, tc_apply_ctas(gm, 1, 64), save_mean, save_w, st))
+      return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d)", cr);
+  }
+  return check_launch("switchable whitening apply kernel");
+}
+
+int switch_bwd(const void* x, const void* dout, void* dx, int64_t N, int64_t C, int64_t HW, int GS, int mode, float eps,
+               const float* mix, const float* save_mean, const float* save_w, const float* save_stats, float* dmix, void* ws,
+               size_t ws_bytes, cudaStream_t st) {
+  dwt::Geom gm;
+  SwWork s;
+  if (int rc = sw_validate(gm, s, x, dout, dx, N, C, HW, GS, mode, mix, save_mean, save_w, save_stats, ws, ws_bytes)) return rc;
+  const bool nhwc = (mode & DWT_LAYOUT_NHWC) != 0, bf16 = (mode & DWT_DTYPE_BF16) != 0;
+  const int k = 2 * nhwc + bf16;
+  const double E = (bf16 ? 2.0 : 4.0) * (double)N * (double)C * (double)HW;
+  // the kernels only read save_mean, save_w and save_stats
+  const dwt::SwFin fin = make_sw_fin(mode, eps, mix, const_cast<float*>(save_mean), const_cast<float*>(save_w),
+                                     const_cast<float*>(save_stats), s.w.status);
+  {
+    Launch l(kSwName[3][k], &gm, 2.0 * E, st);
+    if (int cr = dwt::tc_bwd_reduce(x, dout, bf16, nhwc, gm, gm.nchunks, save_mean, s.w.partial, st, /*pilot=*/false))
+      return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d) x=%p dout=%p N=%lld C=%d HW=%d", cr, x, dout,
+                  (long long)N, gm.C, gm.HW);
+  }
+  if (int rc = check_launch("switchable whitening backward reduction kernel")) return rc;
+  {
+    Launch l(kSwName[4][k], &gm, 0.0, st);
+    if (gm.nchunks > 1) dwt::dense_partial_reduce(s.w.partial, gm.nchunks, dwt::tc_superblocks(gm) * gm.D, s.w.gram, st);
+    dwt::dense_sw_bwd(s.w.gram, gm, fin, s.pd, s.part, s.sums, dmix, s.w.coef, s.w.shift, s.mu, st);
+  }
+  if (int rc = check_launch("switchable whitening backward finalize kernel")) return rc;
+  {
+    Launch l(kSwName[5][k], &gm, 3.0 * E, st);
+    if (int cr = dwt::tc_bwd_apply(x, dout, dx, bf16, nhwc, gm, tc_apply_ctas(gm, 1, 64), s.w.coef, s.mu, s.w.shift, st))
+      return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d)", cr);
+  }
+  return check_launch("switchable whitening backward apply kernel");
+}
+
 }  // namespace
 
 extern "C" {
@@ -984,6 +1127,30 @@ size_t dwt_instance_workspace_bytes(int64_t N, int64_t C, int64_t HW, int group_
 int dwt_whiten_instance_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, int group_size, int flags, float eps,
                             float* save_mean, float* save_w, void* workspace, size_t workspace_bytes, dwt_stream_t stream) {
   return instance_fwd(x, y, N, C, HW, group_size, flags, eps, save_mean, save_w, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+size_t dwt_switch_workspace_bytes(int64_t N, int64_t C, int64_t HW, int group_size) {
+  dwt::Geom gm;
+  char saved[sizeof(g_err)];
+  memcpy(saved, g_err, sizeof(g_err));            // a size query leaves the last error text alone
+  const int rc = sw_geom(gm, N, C, HW, group_size, 0);
+  memcpy(g_err, saved, sizeof(g_err));
+  return rc ? 0 : carve_switch(nullptr, gm).w.bytes;
+}
+
+int dwt_whiten_switch_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, int group_size, int mode, float eps,
+                          float momentum, int update_running, float* running_mean, float* running_cov, const float* mix,
+                          float* save_mean, float* save_w, float* save_stats, void* workspace, size_t workspace_bytes,
+                          dwt_stream_t stream) {
+  return switch_fwd(x, y, N, C, HW, group_size, mode, eps, momentum, update_running, running_mean, running_cov, mix, save_mean,
+                    save_w, save_stats, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int dwt_whiten_switch_bwd(const float* x, const float* dout, float* dx, int64_t N, int64_t C, int64_t HW, int group_size,
+                          int mode, float eps, const float* mix, const float* save_mean, const float* save_w,
+                          const float* save_stats, float* dmix, void* workspace, size_t workspace_bytes, dwt_stream_t stream) {
+  return switch_bwd(x, dout, dx, N, C, HW, group_size, mode, eps, mix, save_mean, save_w, save_stats, dmix, workspace,
+                    workspace_bytes, (cudaStream_t)stream);
 }
 
 int dwt_whiten_instance_bwd(const float* x, const float* dout, float* dx, int64_t N, int64_t C, int64_t HW, int group_size,

@@ -16,6 +16,10 @@
 //                    algebra on color^T R, domains in order in one CTA per group, and sums dcolor and dbias over them
 //   fwd_instance     instance whitening (dwt_whiten_instance_*): fwd_factor's prologue and factorisation, one CTA per
 //                    (image, group), no EMA; its backward is bwd_coef as it is, with the images as the domains
+//   sw_*             switchable whitening (dwt_whiten_switch_*): per-image and batch moments (sw_stats), the mixture and
+//                    fwd_instance's factorisation (sw_fwd_factor); backward: dL/dcov_hat and dL/dm per (image, group)
+//                    (sw_bwd_coef), their fixed-order sums over the images (sw_bwd_sum, sw_dmix) and tc_bwd_apply's
+//                    coefficients (sw_bwd_apply_coef)
 //
 // All three keep a 64x64 problem in ONE 256-thread CTA arranged 16x16, each thread owning a 4x4
 // register block.  fwd_factor runs the Cholesky factorisation AND the triangular inverse as one blocked
@@ -1291,6 +1295,342 @@ __global__ void __launch_bounds__(256) fwd_instance_kernel(const float* __restri
   if (threadIdx.x == 0 && bad) atomicOr(f.status, DWT_STATUS_NOT_PD);
 }
 
+// ------------------------------------------------------------------------------------------
+// Switchable whitening (dwt_whiten_switch_*): the Geom's domains are the images (N = 1, M = HW), as for fwd_instance.
+// A group's statistics record is rec = gs*gs + gs floats (covariance, then mean); save_stats holds [D + 1][G] of them, the
+// images' own and then the batch's.  mix = (a_b, a_i, w_bw, w_iw, w_bn, w_in).
+// ------------------------------------------------------------------------------------------
+__device__ __forceinline__ int sw_rec(int GS) { return GS * GS + GS; }
+
+// sw_stats: grid (ceil(rec / 256), G), 256 threads, one record element per thread.  Each image's own covariance and mean
+// into save_stats rows 0..D-1 (fp32, fwd_instance's arithmetic).  Train: the batch moments into row D by the law of total
+// covariance, cov_b = mean_n cov_n + cov_n(mu_n), accumulated in fp64 over the images in order about image 0's mean (no
+// second pass over x; bit-identical reruns).  Eval: row D is a copy of the running buffers.
+__global__ void __launch_bounds__(256) sw_stats_kernel(const float* __restrict__ gram, const float* __restrict__ shift,
+                                                       const Geom gm, const SwFin f) {
+  const int GS = gm.GS, g = blockIdx.y, nb = kSB / GS, sb = g / nb, o = (g % nb) * GS, rec = sw_rec(GS);
+  const int e = blockIdx.x * 256 + threadIdx.x;
+  if (e >= rec) return;
+  const int SB = (gm.C + kSB - 1) / kSB, D = gm.D;
+  const float invM = 1.f / gm.M;
+  const double invMd = 1.0 / (double)gm.M;
+  const bool cov = e < GS * GS;
+  const int i = cov ? e / GS : e - GS * GS, j = cov ? e % GS : i, hi = i > j ? i : j, lo = i > j ? j : i;
+  float* out = f.save_stats + (size_t)g * rec + e;
+  const size_t ostride = (size_t)gm.G * rec;
+  const float* G0 = gram + (size_t)sb * kNacc;
+  const float* S0 = shift + (size_t)sb * kSB + o;
+  const double ci = (double)S0[i] + (double)__ldcg(G0 + kSB * kSB + o + i) * invMd;   // image 0's mean: the common shift
+  const double cj = (double)S0[j] + (double)__ldcg(G0 + kSB * kSB + o + j) * invMd;
+  double acc = 0.0, accm = 0.0, acci = 0.0, accj = 0.0;
+#pragma unroll 4
+  for (int d = 0; d < D; ++d) {
+    const float* Gd = G0 + (size_t)d * SB * kNacc;
+    const float* Sd = S0 + (size_t)d * SB * kSB;
+    const float ri = __ldcg(Gd + kSB * kSB + o + i), si = Sd[i];
+    if (cov) {
+      const float graw = __ldcg(Gd + (o + hi) * kSB + o + lo), rj = __ldcg(Gd + kSB * kSB + o + j), sj = Sd[j];
+      const float ri_m = ri * invM, rj_m = rj * invM;
+      out[(size_t)d * ostride] = graw * invM - ri_m * rj_m;
+      if (f.train) {
+        const double dri = (double)ri * invMd, drj = (double)rj * invMd;
+        const double mi = ((double)si + dri) - ci, mj = ((double)sj + drj) - cj;
+        acc += (double)graw * invMd - dri * drj;
+        accm = fma(mi, mj, accm);
+        acci += mi;
+        accj += mj;
+      }
+    } else {
+      out[(size_t)d * ostride] = si + ri * invM;
+      if (f.train) acci += ((double)si + (double)ri * invMd) - ci;
+    }
+  }
+  float b;
+  if (f.train) {
+    const double invD = 1.0 / (double)D, mi = acci * invD, mj = accj * invD;
+    b = cov ? (float)(acc * invD + (accm * invD - mi * mj)) : (float)(ci + mi);
+  } else {
+    b = cov ? f.rcov[(size_t)g * GS * GS + e] : f.rmean[g * GS + i];
+  }
+  out[(size_t)D * ostride] = b;
+}
+
+// sw_fwd_factor: grid (G, 1, D), 256 threads, one CTA per (image, group): the mixed mean m = a_b mu_b + a_i mu_n into
+// save_mean, the mixed covariance, S = a cov_hat + b I and fwd_instance's blocked Cholesky + inverse.  An (image, group)
+// whose S is not positive definite, or whose S or m is not finite, gets W = NaN in full and sets DWT_STATUS_NOT_PD.
+// The CTAs of image 0 also run the EMA of their group's batch moments (train, update_running), skipped with
+// DWT_STATUS_NOT_PD when those are not finite.
+__global__ void __launch_bounds__(256) sw_fwd_factor_kernel(const Geom gm, const SwFin f) {
+  __shared__ __align__(16) PanelSmem sp;
+  const int g = blockIdx.x, d = blockIdx.z, GS = gm.GS, rec = sw_rec(GS);
+  const Blk t(GS);
+  const float* sn = f.save_stats + ((size_t)d * gm.G + g) * rec;
+  const float* sbt = f.save_stats + ((size_t)gm.D * gm.G + g) * rec;
+  const float a_b = f.mix[0], a_i = f.mix[1], w_bw = f.mix[2], w_iw = f.mix[3], w_bn = f.mix[4], w_in = f.mix[5];
+  bool bad = false;
+  float a[4][4], w[4][4];
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+#pragma unroll
+    for (int s = 0; s < 4; ++s) {
+      float v = 0.f;
+      if (t.act) {
+        const int i = 4 * t.bi + r, j = 4 * t.bj + s;
+        const float cn = sn[i * GS + j], cb = sbt[i * GS + j];
+        float c = fmaf(w_iw, cn, w_bw * cb);
+        if (i == j) c = fmaf(w_in, cn, fmaf(w_bn, cb, c));
+        v = f.a * c + (i == j ? f.b : 0.f);
+        bad = bad || !isfinite(v);
+      }
+      a[r][s] = v;
+    }
+  if ((int)threadIdx.x < GS) {
+    const float m = fmaf(a_i, sn[GS * GS + threadIdx.x], a_b * sbt[GS * GS + threadIdx.x]);
+    f.save_mean[(size_t)d * gm.C + g * GS + threadIdx.x] = m;
+    bad = bad || !isfinite(m);
+  }
+  const bool ok = factor_and_invert(a, w, GS, t, sp);
+  bad = __syncthreads_or(bad || !ok) != 0;
+  if (t.act) {
+    float* wout = f.save_w + ((size_t)d * gm.G + g) * GS * GS;
+    const float q = __int_as_float(0x7fc00000);   // a NaN the apply's TF32 split keeps
+#pragma unroll
+    for (int r = 0; r < 4; ++r)
+      *reinterpret_cast<float4*>(wout + (size_t)(4 * t.bi + r) * GS + 4 * t.bj) =
+          bad ? make_float4(q, q, q, q) : make_float4(w[r][0], w[r][1], w[r][2], w[r][3]);
+  }
+  if (threadIdx.x == 0 && bad) atomicOr(f.status, DWT_STATUS_NOT_PD);
+  if (d != 0 || !f.train || !f.update_running) return;
+  constexpr int kPer = (kSB * kSB + kSB + 255) / 256;
+  float old[kPer], stat[kPer];
+  bool fin = true;
+#pragma unroll
+  for (int n = 0; n < kPer; ++n) {
+    const int e = threadIdx.x + 256 * n;
+    stat[n] = e < rec ? sbt[e] : 0.f;
+    old[n] = e < GS * GS ? f.rcov[(size_t)g * GS * GS + e] : (e < rec ? f.rmean[g * GS + e - GS * GS] : 0.f);
+    fin = fin && isfinite(stat[n]);
+  }
+  if (!__syncthreads_or(!fin)) {        // dwt_whiten_fwd's EMA: (1 - m) old + m stat on the unshrunk batch moments
+    const float m = f.momentum, k = 1.f - f.momentum;
+#pragma unroll
+    for (int n = 0; n < kPer; ++n) {
+      const int e = threadIdx.x + 256 * n;
+      if (e < GS * GS) f.rcov[(size_t)g * GS * GS + e] = m * stat[n] + k * old[n];
+      else if (e < rec) f.rmean[g * GS + e - GS * GS] = fmaf(k, old[n], __fmul_rn(m, stat[n]));
+    }
+  } else if (threadIdx.x == 0) {
+    atomicOr(f.status, DWT_STATUS_NOT_PD);
+  }
+}
+
+// Deterministic sum of v over the CTA (256 threads): warp trees, then the 8 warps in order; the total in every thread.
+__device__ __forceinline__ float cta_sum(float v, float* sRed) {
+  v = warp_sum(v);
+  __syncthreads();                     // sRed free
+  if ((threadIdx.x & 31) == 0) sRed[threadIdx.x >> 5] = v;
+  __syncthreads();
+  float s = 0.f;
+#pragma unroll
+  for (int w = 0; w < 8; ++w) s += sRed[w];
+  return s;
+}
+
+// sw_bwd_coef: grid (G, 1, D), 256 threads, one CTA per (image, group).  rgram [D][SB][kNacc] = (R = sum dy (x - m)^T |
+// sum dy).  P = a sym(W^T Phi(-R W^T) W) (dL/dcov_hat) and dm = -W^T sum dy (dL/dm) into pd [D][G][rec], and the image's
+// six dmix terms (<dm, mu_b>, <dm, mu_n>, <P, cov_b>, <P, cov_n>, <diag P, cov_b>, <diag P, cov_n>) into part [D][G][8].
+__global__ void __launch_bounds__(256) sw_bwd_coef_kernel(const float* __restrict__ rgram, const Geom gm, const SwFin f,
+                                                          float* __restrict__ pd, float* __restrict__ part) {
+  extern __shared__ __align__(16) float dsm[];
+  float* sW = dsm;
+  float* sR = sW + kMat;
+  float* sT = sR + kMat;
+  __shared__ float sSdz[kSB], sRed[8];
+  const int g = blockIdx.x, d = blockIdx.z, GS = gm.GS, nb = kSB / GS, sb = g / nb, o = (g % nb) * GS, rec = sw_rec(GS);
+  const Blk t(GS);
+  const int SB = (gm.C + kSB - 1) / kSB, gsh = __ffs(GS) - 1;
+  const float* G = rgram + ((size_t)d * SB + sb) * kNacc;
+  const float* sn = f.save_stats + ((size_t)d * gm.G + g) * rec;
+  const float* sbt = f.save_stats + ((size_t)gm.D * gm.G + g) * rec;
+  float* out = pd + ((size_t)d * gm.G + g) * rec;
+  constexpr int kPer = kSB * kSB / 256;
+  float wv[kPer], rv[kPer];
+#pragma unroll
+  for (int n = 0; n < kPer; ++n) {
+    const int e = threadIdx.x + 256 * n, i = e >> gsh, j = e & (GS - 1);
+    const bool in = e < GS * GS;
+    wv[n] = in ? f.save_w[((size_t)d * gm.G + g) * GS * GS + e] : 0.f;
+    rv[n] = in ? __ldcg(G + (o + i) * kSB + o + j) : 0.f;
+  }
+  if ((int)threadIdx.x < GS) sSdz[threadIdx.x] = __ldcg(G + kSB * kSB + o + threadIdx.x);
+#pragma unroll
+  for (int n = 0; n < kPer; ++n) {
+    const int e = threadIdx.x + 256 * n, i = e >> gsh, j = e & (GS - 1);
+    if (e < GS * GS) { sW[i * LDS + j] = wv[n]; sR[i * LDS + j] = rv[n]; }
+  }
+  __syncthreads();
+  float c[4][4];
+  mm_block<false, true>(sR, sW, GS, t, c);               // R W^T ; Phi(-R W^T)
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+#pragma unroll
+    for (int s = 0; s < 4; ++s) {
+      const int i = 4 * t.bi + r, j = 4 * t.bj + s;
+      c[r][s] = (i > j) ? -c[r][s] : ((i == j) ? -0.5f * c[r][s] : 0.f);
+    }
+  store_block(sT, t, c);
+  __syncthreads();
+  mm_block<true, false>(sW, sT, GS, t, c);               // W^T Phi (sR is free: the barrier above follows its reads)
+  store_block(sR, t, c);
+  __syncthreads();
+  mm_block<false, false>(sR, sW, GS, t, c);              // T' = W^T Phi W
+  store_block(sT, t, c);
+  __syncthreads();
+  const float h = 0.5f * f.a;
+  float p_bw = 0.f, p_iw = 0.f, p_bn = 0.f, p_in = 0.f;
+#pragma unroll
+  for (int n = 0; n < kPer; ++n) {
+    const int e = threadIdx.x + 256 * n, i = e >> gsh, j = e & (GS - 1);
+    if (e < GS * GS) {
+      const float p = h * (sT[i * LDS + j] + sT[j * LDS + i]);
+      out[e] = p;
+      const float cb = sbt[e], cn = sn[e];
+      p_bw = fmaf(p, cb, p_bw);
+      p_iw = fmaf(p, cn, p_iw);
+      if (i == j) { p_bn = fmaf(p, cb, p_bn); p_in = fmaf(p, cn, p_in); }
+    }
+  }
+  // dm_i = -sum_j W_ji sdz_j: 4 threads per row, partial sums met by shuffle
+  float t_b = 0.f, t_i = 0.f;
+  {
+    const int i = threadIdx.x >> 2, q = threadIdx.x & 3;
+    float v = 0.f;
+    if (i < GS)
+      for (int j = q; j < GS; j += 4) v = fmaf(sW[j * LDS + i], sSdz[j], v);   // W_ji = 0 for j < i
+    v += __shfl_xor_sync(0xffffffffu, v, 1);
+    v += __shfl_xor_sync(0xffffffffu, v, 2);
+    if (q == 0 && i < GS) {
+      out[GS * GS + i] = -v;
+      t_b = -v * sbt[GS * GS + i];
+      t_i = -v * sn[GS * GS + i];
+    }
+  }
+  const float terms[6] = {t_b, t_i, p_bw, p_iw, p_bn, p_in};
+#pragma unroll
+  for (int k = 0; k < 6; ++k) {
+    const float s = cta_sum(terms[k], sRed);
+    if (threadIdx.x == 0) part[((size_t)d * gm.G + g) * 8 + k] = s;
+  }
+}
+
+// sw_bwd_sum: grid (ceil(rec / 256), G), 256 threads: sums [G][rec] = sum over the images, in order and in fp64, of pd
+// (sum_n P_n | sum_n dm_n).
+__global__ void __launch_bounds__(256) sw_bwd_sum_kernel(const float* __restrict__ pd, const Geom gm, float* __restrict__ sums) {
+  const int g = blockIdx.y, rec = sw_rec(gm.GS), e = blockIdx.x * 256 + threadIdx.x;
+  if (e >= rec) return;
+  const float* p = pd + (size_t)g * rec + e;
+  const size_t stride = (size_t)gm.G * rec;
+  double acc = 0.0;
+#pragma unroll 8
+  for (int d = 0; d < gm.D; ++d) acc += (double)__ldcg(p + (size_t)d * stride);
+  sums[(size_t)g * rec + e] = (float)acc;
+}
+
+// sw_dmix: one CTA of 256 threads: dmix[k] = the sum over every (image, group) of part[.][.][k], in a fixed order in fp64.
+__global__ void __launch_bounds__(256) sw_dmix_kernel(const float* __restrict__ part, int problems, float* __restrict__ dmix) {
+  __shared__ double sRed[256];
+  for (int k = 0; k < 6; ++k) {
+    double v = 0.0;
+    for (int p = threadIdx.x; p < problems; p += 256) v += (double)__ldcg(part + (size_t)p * 8 + k);
+    sRed[threadIdx.x] = v;
+    __syncthreads();
+    for (int h = 128; h > 0; h >>= 1) {
+      if ((int)threadIdx.x < h) sRed[threadIdx.x] += sRed[threadIdx.x + h];
+      __syncthreads();
+    }
+    if (threadIdx.x == 0) dmix[k] = (float)sRed[0];
+    __syncthreads();
+  }
+}
+
+// sw_bwd_apply_coef: grid (G, 1, D), 256 threads, one CTA per (image, group): the coefficients of tc_bwd_apply's
+// dx = A1 (dy - dybar) + Bm (x - mu) with mu = mu_n (written to mu [D][C]):
+//   A1 = W^T,  Bm = (2/M) Q_n + train (2/NM) Q_b,  Q_n = w_iw P_n + w_in diag P_n,  Q_b = w_bw sum P + w_bn diag sum P
+//   k = (a_i/M) dm_n + train ((a_b/NM) sum dm + (2/NM) Q_b (mu_n - mu_b)),   dybar = -W^-T k (back substitution; 0 when
+//   A1 or Bm is not finite)
+__global__ void __launch_bounds__(256) sw_bwd_apply_coef_kernel(const float* __restrict__ pd, const float* __restrict__ sums,
+                                                                const Geom gm, const SwFin f, float* __restrict__ coef,
+                                                                float* __restrict__ dybar, float* __restrict__ mu) {
+  extern __shared__ __align__(16) float dsm[];
+  float* sW = dsm;
+  float* sQ = sW + kMat;
+  __shared__ float sDmu[kSB], sK[kSB];
+  const int g = blockIdx.x, d = blockIdx.z, GS = gm.GS, nb = kSB / GS, sb = g / nb, o = (g % nb) * GS, rec = sw_rec(GS);
+  const int SB = (gm.C + kSB - 1) / kSB, gsh = __ffs(GS) - 1;
+  const float* p = pd + ((size_t)d * gm.G + g) * rec;
+  const float* ps = sums + (size_t)g * rec;
+  const float* sn = f.save_stats + ((size_t)d * gm.G + g) * rec;
+  const float* sbt = f.save_stats + ((size_t)gm.D * gm.G + g) * rec;
+  float* cf = coef + ((size_t)d * gm.G + g) * coef_stride(GS);
+  const float a_b = f.mix[0], a_i = f.mix[1], w_bw = f.mix[2], w_iw = f.mix[3], w_bn = f.mix[4], w_in = f.mix[5];
+  const float invM = 1.f / gm.M, invNM = invM / (float)gm.D;
+  const bool train = f.train != 0;                       // eval: the batch terms are constants (sums is not read)
+  bool nanc = false;
+  for (int e = threadIdx.x; e < GS * GS; e += 256) {
+    const int i = e >> gsh, j = e & (GS - 1);
+    sW[i * LDS + j] = f.save_w[((size_t)d * gm.G + g) * GS * GS + e];
+    const float pb = train ? ps[e] : 0.f, pn = p[e], qb = train ? (i == j ? fmaf(w_bn, pb, w_bw * pb) : w_bw * pb) : 0.f;
+    const float qn = i == j ? fmaf(w_in, pn, w_iw * pn) : w_iw * pn;
+    sQ[i * LDS + j] = qb;
+    const float bm = 2.f * fmaf(invM, qn, invNM * qb);
+    cf[GS * GS + e] = bm;
+    nanc = nanc || !isfinite(bm) || !isfinite(sW[i * LDS + j]);
+  }
+  if ((int)threadIdx.x < GS) {
+    const float mn = sn[GS * GS + threadIdx.x];
+    sDmu[threadIdx.x] = mn - sbt[GS * GS + threadIdx.x];
+    mu[(size_t)d * gm.C + g * GS + threadIdx.x] = mn;
+  }
+  nanc = __syncthreads_or(nanc) != 0;
+  // a group whose A1 or Bm is not finite gets both as the quiet NaN the apply's TF32 split keeps (an arithmetic NaN,
+  // 0x7fffffff, would round to -0 there and leave a finite, wrong dx)
+  const float q = __int_as_float(0x7fc00000);
+  for (int e = threadIdx.x; e < GS * GS; e += 256) {
+    const int i = e >> gsh, j = e & (GS - 1);
+    cf[e] = nanc ? q : ((j >= i) ? sW[j * LDS + i] : 0.f);   // A1 = W^T
+    if (nanc) cf[GS * GS + e] = q;
+  }
+  {
+    const int i = threadIdx.x >> 2, q = threadIdx.x & 3;
+    float v = 0.f;
+    if (i < GS)
+      for (int j = q; j < GS; j += 4) v = fmaf(sQ[i * LDS + j], sDmu[j], v);
+    v += __shfl_xor_sync(0xffffffffu, v, 1);
+    v += __shfl_xor_sync(0xffffffffu, v, 2);
+    if (q == 0 && i < GS) {
+      const float kb = train ? fmaf(a_b * invNM, ps[GS * GS + i], 2.f * invNM * v) : 0.f;
+      sK[i] = fmaf(a_i * invM, p[GS * GS + i], kb);
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x < 32) {                                 // W^T z = -k, W^T upper triangular: rows i from the bottom
+    const int l = threadIdx.x;
+    float r0 = l < GS ? -sK[l] : 0.f, r1 = l + 32 < GS ? -sK[l + 32] : 0.f;
+    for (int i = GS - 1; i >= 0; --i) {
+      const float own = i >= 32 ? r1 : r0;
+      const float zi = __shfl_sync(0xffffffffu, own, i & 31) / sW[i * LDS + i];
+      if (l == (i & 31)) { if (i >= 32) r1 = zi; else r0 = zi; }
+      if (l < i) r0 = fmaf(-sW[i * LDS + l], zi, r0);     // (W^T)_{l i} = W_il
+      if (l + 32 < i) r1 = fmaf(-sW[i * LDS + l + 32], zi, r1);
+    }
+    // a group whose A1 or Bm is not finite (W = NaN from the forward; in training, Q_b of a group with such an image) has
+    // a NaN dx through them (above); dybar = 0 keeps that NaN out of the other groups of its super-block
+    float* db = dybar + ((size_t)d * SB + sb) * kSB + o;
+    if (l < GS) db[l] = nanc ? 0.f : r0;
+    if (l + 32 < GS) db[l + 32] = nanc ? 0.f : r1;
+  }
+}
+
 constexpr size_t kFactorSmem = 0;   // fwd_factor: static shared memory only (panel buffers + covariance)
 constexpr size_t kCoefSmem = sizeof(float) * 4 * kMat;
 constexpr size_t kZcaFwdSmem = sizeof(float) * 4 * kMat;   // N, P, P^2, P^3 (66.6 KB; + 16.9 KB static)
@@ -1299,6 +1639,8 @@ constexpr size_t kEighFwdSmem = sizeof(float) * 2 * kMat;  // S / V, U (33.3 KB;
 constexpr size_t kEighBwdSmem = sizeof(float) * 5 * kMat;  // W, U, R / G, R U / U H, H / Bm (83.2 KB)
 constexpr size_t kColorFwdSmem = sizeof(float) * 2 * kMat; // color, W (33.3 KB; + 21.3 KB static)
 constexpr size_t kColorBwdSmem = sizeof(float) * 6 * kMat; // W, R / R_hat, T1, T2, color, color W (99.8 KB)
+constexpr size_t kSwCoefSmem = sizeof(float) * 3 * kMat;   // switchable backward: W, R / W^T Phi, Phi / T' (49.9 KB)
+constexpr size_t kSwApplySmem = sizeof(float) * 2 * kMat;  // switchable backward coefficients: W, Q_b (33.3 KB)
 
 }  // namespace
 
@@ -1313,6 +1655,7 @@ int dense_init() {
   if (e == cudaSuccess) e = cudaFuncSetAttribute(bwd_eigh_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kEighBwdSmem);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(fwd_factor_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kColorFwdSmem);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(bwd_color_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kColorBwdSmem);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(sw_bwd_coef_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSwCoefSmem);
   return (int)e;
 }
 
@@ -1371,6 +1714,22 @@ void dense_bwd_color(const float* rgram, const Geom& gm, const BwdFin& fin, cons
 
 void dense_fwd_instance(const float* gram, const float* shift, const Geom& gm, const FwdFin& fin, cudaStream_t st) {
   fwd_instance_kernel<<<dim3(gm.G, 1, gm.D), 256, 0, st>>>(gram, shift, gm, fin);
+}
+
+void dense_sw_stats(const float* gram, const float* shift, const Geom& gm, const SwFin& fin, cudaStream_t st) {
+  sw_stats_kernel<<<dim3((gm.GS * gm.GS + gm.GS + 255) / 256, gm.G), 256, 0, st>>>(gram, shift, gm, fin);
+}
+
+void dense_sw_fwd_factor(const Geom& gm, const SwFin& fin, cudaStream_t st) {
+  sw_fwd_factor_kernel<<<dim3(gm.G, 1, gm.D), 256, 0, st>>>(gm, fin);
+}
+
+void dense_sw_bwd(const float* rgram, const Geom& gm, const SwFin& fin, float* pd, float* part, float* sums, float* dmix,
+                  float* coef, float* dybar, float* mu, cudaStream_t st) {
+  sw_bwd_coef_kernel<<<dim3(gm.G, 1, gm.D), 256, kSwCoefSmem, st>>>(rgram, gm, fin, pd, part);
+  if (fin.train) sw_bwd_sum_kernel<<<dim3((gm.GS * gm.GS + gm.GS + 255) / 256, gm.G), 256, 0, st>>>(pd, gm, sums);
+  if (dmix) sw_dmix_kernel<<<1, 256, 0, st>>>(part, gm.D * gm.G, dmix);
+  sw_bwd_apply_coef_kernel<<<dim3(gm.G, 1, gm.D), 256, kSwApplySmem, st>>>(pd, sums, gm, fin, coef, dybar, mu);
 }
 
 }  // namespace dwt

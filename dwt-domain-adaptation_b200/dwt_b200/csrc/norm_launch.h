@@ -85,6 +85,28 @@ void dense_bwd_color(const float* rgram, const Geom& gm, const BwdFin& fin, cons
 // instance whitening, group sizes 8..64 (dwt_whiten_instance_*; gm.D = images, gm.N = 1): fwd_factor's work with one CTA
 // per (image, group) and no EMA, W = NaN for a group that is not positive definite.  The backward is dense_bwd_coef.
 void dense_fwd_instance(const float* gram, const float* shift, const Geom& gm, const FwdFin& fin, cudaStream_t st);
+// switchable whitening, group sizes 8..64 (dwt_whiten_switch_*; gm.D = images, gm.N = 1).  save_stats [D + 1][G][gs*gs + gs]:
+// each image's (cov, mean), then the batch's.  dense_sw_stats fills it from tc_stats' per-image moments (train: the batch
+// row by the law of total covariance; eval: the running buffers); dense_sw_fwd_factor mixes, factors, writes save_mean /
+// save_w and runs the EMA.  dense_sw_bwd turns tc_bwd_reduce's R (about save_mean, no pilot) into tc_bwd_apply's coef,
+// dybar and mean (mu = the images' own means), and dmix when it is given.  Scratch: pd [D][G][rec], part [D][G][8],
+// sums [G][rec].
+struct SwFin {
+  float a, b;                 // S = a cov_hat + b I (1 - eps, eps)
+  float momentum;
+  int train, update_running;
+  const float* mix;           // [6] a_b, a_i, w_bw, w_iw, w_bn, w_in
+  float* rmean;               // [C]
+  float* rcov;                // [G][gs*gs]
+  float* save_mean;           // [D][C]
+  float* save_w;              // [D][G][gs*gs]
+  float* save_stats;          // [D + 1][G][gs*gs + gs]
+  int* status;
+};
+void dense_sw_stats(const float* gram, const float* shift, const Geom& gm, const SwFin& fin, cudaStream_t st);
+void dense_sw_fwd_factor(const Geom& gm, const SwFin& fin, cudaStream_t st);
+void dense_sw_bwd(const float* rgram, const Geom& gm, const SwFin& fin, float* pd, float* part, float* sums, float* dmix,
+                  float* coef, float* dybar, float* mu, cudaStream_t st);
 
 // TMA + wgmma apply path (norm_tc_apply.cu): split-TF32 GEMM of the block-diagonal group matrices
 int tc_apply_init();

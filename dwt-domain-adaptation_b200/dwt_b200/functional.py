@@ -579,6 +579,96 @@ def instance_whiten(x, *, group_size, eps):
     return _InstanceFunction.apply(x, int(group_size), float(eps))
 
 
+class _SwitchFunction(torch.autograd.Function):
+    """Switchable whitening (dwt_whiten_switch_fwd / _bwd): every image of x [N, C, *] whitened by a mixture, with the six
+    weights of mix (a_b, a_i, w_bw, w_iw, w_bn, w_in; float32, on the device), of the batch's and its own mean and
+    covariance, per group of group_size channels, in the Cholesky basis.  The gradient of mix is returned.  Running buffers
+    as _NormFunction's (one domain).  x is float32 or bfloat16, NCHW-contiguous or (4-D) channels-last; it goes to the
+    kernels in its own layout and dtype."""
+
+    @staticmethod
+    def forward(ctx, x, mix, group_size, mode, eps, momentum, update_running, running):
+        dev = nv.require_cuda(x, bf16=True)
+        rm_t, rv_t = running
+        nv.require_cuda(mix, rm_t, rv_t)
+        lib = nv.lib()
+        gs = group_size
+        nhwc = _channels_last(x)
+        fmt = torch.channels_last if nhwc else torch.contiguous_format
+        x = x.contiguous(memory_format=fmt)
+        if x.data_ptr() % 16:                        # the kernels read x through TMA
+            x = x.clone(memory_format=fmt)
+        n, c, hw = x.shape[0], x.shape[1], math.prod(x.shape[2:])
+        mix_c = _aligned(mix)
+        _check_param("mix", mix_c, 6)
+        need_running = (mode == nv.MODE_EVAL) or update_running
+        if need_running:
+            _check_param("running mean", rm_t, c)
+            _check_param("running second moment", rv_t, c * gs)
+        flags = mode | (nv.LAYOUT_NHWC if nhwc else 0) | (nv.DTYPE_BF16 if x.dtype == torch.bfloat16 else 0)
+        y = torch.empty_like(x)
+        g = max(c // gs, 1)
+        save_mean = torch.empty(n, c, dtype=torch.float32, device=dev)
+        save_w = torch.empty(n, g, gs, gs, dtype=torch.float32, device=dev)
+        save_stats = torch.empty(n + 1, g, gs * gs + gs, dtype=torch.float32, device=dev)
+        ws = nv.switch_workspace(dev, n, c, hw, gs)
+        rm, rv = (nv.ptr(rm_t), nv.ptr(rv_t)) if need_running else (None, None)
+        with torch.cuda.device(dev):
+            rc = lib.dwt_whiten_switch_fwd(nv.ptr(x), nv.ptr(y), n, c, hw, gs, flags, eps, momentum, int(update_running), rm,
+                                           rv, nv.ptr(mix_c), nv.ptr(save_mean), nv.ptr(save_w), nv.ptr(save_stats),
+                                           nv.ptr(ws), ws.numel(), nv.stream_ptr(dev))
+        nv.check(rc)
+        nv.poll_status(dev)
+        if update_running and mode == nv.MODE_TRAIN:
+            for buf in {id(b): b for b in (rm_t, rv_t)}.values():    # see _NormFunction.forward
+                torch.autograd.graph.increment_version(buf)
+        ctx.save_for_backward(x, mix_c, save_mean, save_w, save_stats)
+        ctx.cfg = (gs, flags, eps, n, c, hw, fmt)
+        return y
+
+    @staticmethod
+    def backward(ctx, dout):
+        lib = nv.lib()
+        x, mix_c, save_mean, save_w, save_stats = ctx.saved_tensors
+        gs, flags, eps, n, c, hw, fmt = ctx.cfg
+        dout = dout.to(x.dtype).contiguous(memory_format=fmt)
+        if dout.data_ptr() % 16:
+            dout = dout.clone(memory_format=fmt)
+        dev = nv.require_cuda(dout, bf16=True)
+        dx = torch.empty_like(x)
+        dmix = torch.empty(6, dtype=torch.float32, device=dev) if ctx.needs_input_grad[1] else None
+        ws = nv.switch_workspace(dev, n, c, hw, gs)
+        with torch.cuda.device(dev):
+            rc = lib.dwt_whiten_switch_bwd(nv.ptr(x), nv.ptr(dout), nv.ptr(dx), n, c, hw, gs, flags, eps, nv.ptr(mix_c),
+                                           nv.ptr(save_mean), nv.ptr(save_w), nv.ptr(save_stats), nv.ptr(dmix), nv.ptr(ws),
+                                           ws.numel(), nv.stream_ptr(dev))
+        nv.check(rc)
+        return dx, dmix, None, None, None, None, None, None
+
+
+def switchable_whiten(x, mix, *, group_size, training_stats, eps, momentum, update_running, running):
+    """Switchable whitening of x [N, C, *]: per image n and group g of group_size channels, with the image's own mean and
+    (biased) covariance mu_n, cov_n and the batch's mu_b, cov_b (training_stats=False: the running buffers), and
+    mix = (a_b, a_i, w_bw, w_iw, w_bn, w_in), a float32 tensor of 6 used as given (no softmax):
+        m = a_b mu_b + a_i mu_n,  cov_hat = w_bw cov_b + w_iw cov_n + w_bn diag(cov_b) + w_in diag(cov_n),
+        S = (1 - eps) cov_hat + eps I,  W = inverse(cholesky(S)),  y = W (x - m).
+    running = (mean with C elements, second moment [C/gs, gs, gs]): read when training_stats is False; updated with
+    (mu_b, cov_b) by momentum when training_stats and update_running.  mix gets its gradient.
+    The tensor-core kernels only (group sizes 8, 16, 32, 64, H*W >= 256; dwt_b200.h): a call they cannot take raises
+    NativeError with the library's reason and is never sent to another kernel family.  A bfloat16 NCHW x whose H*W is not
+    a multiple of 8 (the bf16 kernels' TMA rows) runs the same kernels in float32 on an upcast copy, the result in
+    bfloat16."""
+    if x.dim() < 3:
+        raise ValueError(f"switchable whitening expects [N, C, *] input (got {x.dim()}D input)")
+    nv.require_cuda(x, bf16=True)
+    mode = nv.MODE_TRAIN if training_stats else nv.MODE_EVAL
+    args = (int(group_size), mode, float(eps), float(momentum), bool(update_running), tuple(running))
+    mix = mix.float()
+    if x.dtype == torch.bfloat16 and not _channels_last(x) and math.prod(x.shape[2:]) % 8:
+        return _SwitchFunction.apply(x.float(), mix, *args).to(x.dtype)
+    return _SwitchFunction.apply(x, mix, *args)
+
+
 class _MecFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, y):

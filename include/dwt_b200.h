@@ -21,6 +21,7 @@
  *   dwt_whiten_eigh_fwd/bwd the same layer in the exact ZCA basis (Jacobi eigendecomposition; not in the reference)
  *   dwt_whiten_color_fwd/bwd whitening followed by a learnable per-group colouring matrix and bias (not in the reference)
  *   dwt_whiten_instance_fwd/bwd  instance whitening: each image by its own statistics (not in the reference)
+ *   dwt_whiten_switch_fwd/bwd  switchable whitening: a learned mix of batch and per-image statistics (not in the reference)
  *   dwt_bn_fwd/bwd   _BatchNorm.forward             utils/batch_norm.py:54-69
  *   dwt_tail2_fwd/bwd  the residual tail of a downsampling Bottleneck: two norm sites and the ReLU in one pass
  *                    resnet50_dwt_mec_officehome.py:236-240
@@ -301,6 +302,55 @@ DWT_API int dwt_whiten_instance_fwd(const float *x, float *y, int64_t N, int64_t
 DWT_API int dwt_whiten_instance_bwd(const float *x, const float *dout, float *dx, int64_t N, int64_t C, int64_t HW,
                        int group_size, int flags, float eps, const float *save_mean, const float *save_w, void *workspace,
                        size_t workspace_bytes, dwt_stream_t stream);
+
+/*
+ * Switchable whitening (Pan et al., ICCV 2019): every image whitened by a learned mixture of the batch's and its own
+ * statistics.  Per image n and group g, with M = HW, the image's own mean and biased covariance mu_n, cov_n (as
+ * dwt_whiten_instance_fwd), the batch's mu_b, cov_b over all N*M pixels (DWT_MODE_EVAL: the running buffers instead) and
+ * mix = (a_b, a_i, w_bw, w_iw, w_bn, w_in), six device floats:
+ *     m_n = a_b mu_b + a_i mu_n,   cov_hat = w_bw cov_b + w_iw cov_n + w_bn diag(cov_b) + w_in diag(cov_n),
+ *     S = (1-eps) cov_hat + eps I = L L^T,   W = L^-1,   y = W (x - m_n).
+ * Each covariance is about its own mean.  mix is used as given: no softmax, normalisation or sign check (the softmax
+ * belongs to the caller, SwitchableWTransform2d).
+ * DWT_MODE_TRAIN with update_running: running = (1-momentum) running + momentum stat on the unshrunk (mu_b, cov_b), the
+ * convention of dwt_whiten_fwd (the buffers are interchangeable with its running_mean[0] / running_cov[0]); skipped, with
+ * DWT_STATUS_NOT_PD, for a group whose mu_b or cov_b is not finite.  DWT_MODE_EVAL reads the buffers and writes nothing.
+ * dwt_whiten_switch_bwd is the exact gradient of the forward (in eval the batch statistics are constants):
+ *     P_n = dL/dcov_hat = (1-eps) sym(W^T Phi(-R W^T) W), R = sum_pixels dout (x - m_n)^T;  dm_n = -W^T sum_pixels dout
+ *     Q_n = w_iw P_n + w_in diag(P_n),  Q_b = sum_n (w_bw P_n + w_bn diag(P_n))
+ *     dx = W^T dout + (a_i/M) dm_n + (2/M) Q_n (x - mu_n)  [train: + (a_b/NM) sum_k dm_k + (2/NM) Q_b (x - mu_b)]
+ *     dmix = sum over images and groups of (<dm_n, mu_b>, <dm_n, mu_n>, <P_n, cov_b>, <P_n, cov_n>, <P_n, diag cov_b>,
+ *            <P_n, diag cov_n>)
+ *   x, y, dout, dx  [N, C, HW] (or channels-last [N, HW, C] with DWT_LAYOUT_NHWC), fp32 or bf16 (DWT_DTYPE_BF16)
+ *   mode            DWT_MODE_TRAIN / DWT_MODE_EVAL | DWT_LAYOUT_NHWC | DWT_DTYPE_BF16 (any other bit: DWT_E_INVALID)
+ *   running_mean [C], running_cov [C/gs, gs, gs]: read in eval, updated in train with update_running (else unused, may be
+ *                   NULL)
+ *   save_mean [N, C] the mixed mean m_n;  save_w [N, C/gs, gs, gs] W;  save_stats [N + 1, C/gs, gs*gs + gs]: rows 0..N-1
+ *                   each image's (cov_n, mu_n), row N the (cov_b, mu_b) the call used.  Written by fwd, read by bwd.
+ *   dmix [6]        written (never accumulated) by bwd; NULL skips it
+ * mix, save_w and save_stats must be 16-byte aligned, as must x, y, dout and dx (else DWT_E_INVALID).
+ * The batch moments come from the per-image ones by the law of total covariance (cov_b = mean cov_n + cov(mu_n)),
+ * summed in fp64 over the images in order about image 0's mean: no second pass over x.  Every reduction is in a fixed
+ * order: reruns are bit-identical, dmix included.  bf16 loads widen to fp32 and stores round to nearest-even: every bf16
+ * output is the fp32 call's output on the widened input, rounded.  Channels-last outputs are bit for bit those of NCHW.
+ * Geometry as dwt_whiten_instance_*: group size 8, 16, 32, 64 dividing C, HW >= 256 and HW % 4 == 0 (NCHW bf16:
+ * HW % 8 == 0), N <= 65535 and N*C*HW < 2^31.  Anything else -- and a call whose tensor-core kernels could not be set
+ * up -- is DWT_E_UNSUPPORTED with a text naming switchable whitening.
+ * Status: an (image, group) whose S is not positive definite, or whose S or m_n is not finite (a non-finite mix, say),
+ * gets a NaN W, so NaN output and dx, and sets DWT_STATUS_NOT_PD; other images and groups are not affected, except that in
+ * training the batch terms of the backward carry the NaN to that group's dx in every image, and dmix is NaN.
+ * Workspace: dwt_switch_workspace_bytes(N, C, HW, group_size) bytes, 256-byte aligned, zero-filled once (it may be the
+ * same buffer as the other entry points'; the status word is shared).  It returns 0 for a geometry the entry points refuse.
+ * Profile families sw_stats, sw_fwd_finalize, sw_apply, sw_bwd_reduce, sw_bwd_finalize, sw_bwd_apply (_nhwc, _bf16).
+ */
+DWT_API size_t dwt_switch_workspace_bytes(int64_t N, int64_t C, int64_t HW, int group_size);
+DWT_API int dwt_whiten_switch_fwd(const float *x, float *y, int64_t N, int64_t C, int64_t HW, int group_size, int mode,
+                   float eps, float momentum, int update_running, float *running_mean, float *running_cov,
+                   const float *mix, float *save_mean, float *save_w, float *save_stats,
+                   void *workspace, size_t workspace_bytes, dwt_stream_t stream);
+DWT_API int dwt_whiten_switch_bwd(const float *x, const float *dout, float *dx, int64_t N, int64_t C, int64_t HW,
+                   int group_size, int mode, float eps, const float *mix, const float *save_mean, const float *save_w,
+                   const float *save_stats, float *dmix, void *workspace, size_t workspace_bytes, dwt_stream_t stream);
 
 /*
  * Domain batch norm (F.batch_norm semantics): biased batch variance normalises,
