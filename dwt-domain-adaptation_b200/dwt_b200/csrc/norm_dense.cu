@@ -26,6 +26,11 @@
 // right-looking sweep of 16 panel steps (one block barrier each): the matrices live in registers, shared
 // memory only carries the 4-column panel of L and the 4-row panel of W of the current step.
 //
+// The backward kernels are built from shared pieces: load_operands / store_operands (W, R = sum dy xc^T, sum dy and a
+// basis' third matrix; bwd_coef, bwd_zca, bwd_eigh, sw_bwd_coef), chol_bwd_core (the Cholesky basis' three products;
+// bwd_coef, bwd_color, sw_bwd_coef) and coef_tail (A1 | Bm | cvec from dL/dS; bwd_coef, bwd_color, bwd_zca, bwd_eigh).
+// A basis' backward kernel adds only its own dL/dS between them.
+//
 // Group size 128 runs fwd_factor128 / bwd_coef128 (one 1024-thread CTA per group on the generic shared-memory routines
 // of dwt_common.cuh); partial_reduce serves it unchanged (its problems are 64 x 64 blocks).
 //
@@ -130,6 +135,45 @@ __device__ __forceinline__ void store_block_global(float* M, int GS, const Blk& 
 #pragma unroll
   for (int r = 0; r < 4; ++r)
     *reinterpret_cast<float4*>(M + (size_t)(4 * t.bi + r) * GS + 4 * t.bj) = make_float4(c[r][0], c[r][1], c[r][2], c[r][3]);
+}
+
+// The NaN a problem that cannot be whitened writes into W or A1 | Bm: the quiet NaN the apply's TF32 split keeps (an
+// arithmetic NaN, 0x7fffffff, would round to -0 there and leave a finite, wrong result)
+constexpr int kApplyNaN = 0x7fc00000;
+
+// this thread's block of W to save_w (dense GS x GS), or NaN in full when the problem is bad
+__device__ __forceinline__ void store_w_or_nan(float* save_w, size_t problem, int GS, const Blk& t, const float (&w)[4][4], bool bad) {
+  if (!t.act) return;
+  float* M = save_w + problem * GS * GS;
+  const float q = __int_as_float(kApplyNaN);
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+    *reinterpret_cast<float4*>(M + (size_t)(4 * t.bi + r) * GS + 4 * t.bj) =
+        bad ? make_float4(q, q, q, q) : make_float4(w[r][0], w[r][1], w[r][2], w[r][3]);
+}
+
+// Where group g sits in the 64-channel super-blocks the tensor-core passes reduce: super-block sb of SB, first
+// channel o inside it
+struct GroupPos {
+  int GS, sb, o, SB;
+};
+
+__device__ __forceinline__ GroupPos group_pos(const Geom& gm, int g) {
+  const int nb = kSB / gm.GS;
+  return {gm.GS, g / nb, (g % nb) * gm.GS, (gm.C + kSB - 1) / kSB};
+}
+
+// sum of v over the CTA (256 threads) in one fixed order: warp trees, then the 8 warp totals in order; every thread
+// gets it.  Two block barriers, the first so that sRed is free however the caller used it last.
+__device__ __forceinline__ float block_sum(float v, float* sRed) {
+  v = warp_sum(v);
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) sRed[threadIdx.x >> 5] = v;
+  __syncthreads();
+  float s = 0.f;
+#pragma unroll
+  for (int w = 0; w < 8; ++w) s += sRed[w];
+  return s;
 }
 
 // Blocked right-looking sweep: S = L L^T and W = L^-1 together, 4 columns per step, ONE block barrier per step.
@@ -361,9 +405,9 @@ __global__ void __launch_bounds__(256) fwd_factor_kernel(const float* __restrict
   __shared__ float sC[kMat];       // un-shrunk covariance (for the EMA)
   __shared__ float sMean[kSB], sRow[kSB];
   __shared__ int sBad, sBadDom;
-  const int g = blockIdx.x, GS = gm.GS, nb = kSB / GS, sb = g / nb, o = (g % nb) * GS;
+  const int g = blockIdx.x;
+  const auto [GS, sb, o, SB] = group_pos(gm, g);
   const Blk t(GS);
-  const int SB = (gm.C + kSB - 1) / kSB;
   const float invM = 1.f / gm.M;
   if (threadIdx.x == 0) sBad = 0;
   extern __shared__ __align__(16) float dsm[];
@@ -404,9 +448,53 @@ __global__ void __launch_bounds__(256) fwd_factor_kernel(const float* __restrict
   if (threadIdx.x == 0 && sBad) atomicOr(f.status, DWT_STATUS_NOT_PD);
 }
 
-// bwd_color's copy of bwd_coef's three products (bwd_coef keeps them inline: factoring them out changes its code):
-// from R = sum dL/dy xc^T (sR) and W (sW), S' = W^T Phi(-R W^T) W into sT1 (sT2: scratch), Bm = (a/M)(S' + S'^T).
-// Ends with a block barrier.
+// ------------------------------------------------------------------------------------------
+// Backward pieces shared by the per-group backward kernels (gs 8..64)
+// ------------------------------------------------------------------------------------------
+constexpr int kPer = kSB * kSB / 256;   // elements of a 64 x 64 matrix per thread: e = threadIdx.x + 256 n
+
+// One (domain, group) problem's backward operands in registers: this thread's elements of W, of R = sum dy xc^T and,
+// with HAS_X, of a third GS x GS matrix X; and sum dy of channel threadIdx.x.
+struct Operands {
+  float w[kPer], r[kPer], x[kPer];
+  float sdz;
+};
+
+// Issues the loads of W (w: the problem's save_w), of R and sum dy (G: the problem's reduced block [kNacc], channel o of
+// the super-block) and of X (x).  on false (eval): R, X and sdz are zeros, and G and x are not read.  Every global load
+// goes out before the first shared-memory store: interleaved with their stores, the compiler kept the loads in order (16
+// dependent round trips, 17.7 k of bwd_coef's 44 k cycles at gs = 64).  So a caller issues its own per-channel loads
+// between load_operands and store_operands.  GS is a power of two: shifts, not divisions.
+template <bool HAS_X>
+__device__ __forceinline__ void load_operands(Operands& op, const float* w, const float* G, const float* x, bool on, int GS,
+                                              int gsh, int o) {
+#pragma unroll
+  for (int n = 0; n < kPer; ++n) {
+    const int e = threadIdx.x + 256 * n, i = e >> gsh, j = e & (GS - 1);
+    const bool in = e < GS * GS;
+    op.w[n] = in ? w[e] : 0.f;
+    op.r[n] = (in && on) ? __ldcg(G + (o + i) * kSB + o + j) : 0.f;
+    if constexpr (HAS_X) op.x[n] = (in && on) ? x[e] : 0.f;
+  }
+  op.sdz = 0.f;
+  if ((int)threadIdx.x < GS) op.sdz = on ? __ldcg(G + kSB * kSB + o + threadIdx.x) : 0.f;
+}
+
+template <bool HAS_X>
+__device__ __forceinline__ void store_operands(const Operands& op, float* sW, float* sR, float* sX, int GS, int gsh) {
+#pragma unroll
+  for (int n = 0; n < kPer; ++n) {
+    const int e = threadIdx.x + 256 * n, i = e >> gsh, j = e & (GS - 1);
+    if (e < GS * GS) {
+      sW[i * LDS + j] = op.w[n];
+      sR[i * LDS + j] = op.r[n];
+      if constexpr (HAS_X) sX[i * LDS + j] = op.x[n];
+    }
+  }
+}
+
+// The Cholesky basis' backward: from R = sum dL/dy xc^T (sR) and W (sW), S' = W^T Phi(-R W^T) W into sT1 (sT2: scratch;
+// it may be sR, which is read only before the first barrier), Bm = (a/M)(S' + S'^T).  Ends with a block barrier.
 __device__ __forceinline__ void chol_bwd_core(const float* sR, const float* sW, float* sT1, float* sT2, int GS, const Blk& t PROF_ARGS) {
   float c[4][4];
   mm_block<false, true>(sR, sW, GS, t, c);               // R W^T ; P = Phi(-R W^T)
@@ -430,9 +518,40 @@ __device__ __forceinline__ void chol_bwd_core(const float* sR, const float* sW, 
   PROF_MARK();
 }
 
+// The coefficients tc_bwd_apply reads, coef = A1 | Bm | cvec with dx = A1 dy + Bm x + cvec, from the matrix sA whose
+// transpose is A1 and, in training, G = dL/dS (sG):
+//   A1 = sA^T, in full, or TRI: its upper triangle and zeros below (a Cholesky W of a group that is not positive
+//        definite can hold NaN above its diagonal, 0 x NaN from a NaN 1/diag)
+//   Bm = (a/M)(G + G^T) = sc (G + G^T), also into the scratch sBm; 0 in eval
+//   cvec_i = -(sum_j A1_ij mean(dy)_j + sum_j Bm_ij mu_j): 4 threads per row, partial sums met by shuffle; 0 in eval
+// One block barrier.
+template <bool TRI>
+__device__ __forceinline__ void coef_tail(const float* sA, const float* sG, float* sBm, const float* sSdz, const float* sMu,
+                                          bool train, float sc, int GS, int gsh, float* coef) {
+#pragma unroll
+  for (int n = 0; n < kPer; ++n) {
+    const int e = threadIdx.x + 256 * n, i = e >> gsh, j = e & (GS - 1);
+    if (e < GS * GS) {
+      const float bm = train ? sc * (sG[i * LDS + j] + sG[j * LDS + i]) : 0.f;
+      coef[e] = (!TRI || j >= i) ? sA[j * LDS + i] : 0.f;
+      coef[GS * GS + e] = bm;
+      sBm[i * LDS + j] = bm;
+    }
+  }
+  __syncthreads();
+  const int i = threadIdx.x >> 2, q = threadIdx.x & 3;
+  float cv = 0.f;
+  if (train && i < GS) {
+    for (int j = q; j < GS; j += 4) cv = fmaf(sA[j * LDS + i], sSdz[j], fmaf(sBm[i * LDS + j], sMu[j], cv));
+  }
+  cv += __shfl_xor_sync(0xffffffffu, cv, 1);
+  cv += __shfl_xor_sync(0xffffffffu, cv, 2);
+  if (q == 0 && i < GS) coef[2 * GS * GS + i] = -cv;
+}
+
 // ------------------------------------------------------------------------------------------
 // bwd_coef: grid (G, 1, D), 256 threads.  rgram [D][SB][kNacc] = (R = sum dy xc^T | sdz = sum dy).
-// coef[d][g] = A1 | Bm | cvec  with  dx = A1 dy + Bm x + cvec   (no affine epilogue on this path)
+// coef[d][g] = A1 | Bm | cvec  with  dx = A1 dy + Bm x + cvec   (no affine epilogue on this path), A1 = W^T
 // ------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) bwd_coef_kernel(const float* __restrict__ rgram, const Geom gm, const BwdFin f,
                                                        float* __restrict__ dybar) {
@@ -442,90 +561,30 @@ __global__ void __launch_bounds__(256) bwd_coef_kernel(const float* __restrict__
   float* sT1 = sR + kMat;
   float* sT2 = sT1 + kMat;
   __shared__ float sSdz[kSB], sMu[kSB];
-  const int g = blockIdx.x, d = blockIdx.z, GS = gm.GS, nb = kSB / GS, sb = g / nb, o = (g % nb) * GS;
+  const int g = blockIdx.x, d = blockIdx.z;
+  const auto [GS, sb, o, SB] = group_pos(gm, g);
   const Blk t(GS);
-  const int SB = (gm.C + kSB - 1) / kSB;
   const bool train = f.mode == DWT_MODE_TRAIN;
   const float* G = rgram ? rgram + ((size_t)d * SB + sb) * kNacc : nullptr;
-  const size_t gbase = ((size_t)d * gm.G + g) * GS * GS;
   float* coef = f.coef + ((size_t)d * gm.G + g) * coef_stride(GS);
-  PROF_DECL;
-  PROF_MARK();
-  // all global loads first (interleaved with their shared-memory stores the compiler kept them in order: 16 dependent
-  // round trips, 17.7 k of this kernel's 44 k cycles at gs = 64); GS is a power of two: shifts, not divisions
   const int gsh = __ffs(GS) - 1;
   const float invM = 1.f / gm.M;
-  constexpr int kPer = kSB * kSB / 256;
-  float wv[kPer], rv[kPer];
-#pragma unroll
-  for (int n = 0; n < kPer; ++n) {
-    const int e = threadIdx.x + 256 * n, i = e >> gsh, j = e & (GS - 1);
-    const bool in = e < GS * GS;
-    wv[n] = in ? f.save_w[gbase + e] : 0.f;
-    rv[n] = (in && G && train) ? __ldcg(G + (o + i) * kSB + o + j) : 0.f;
-  }
-  float sdz = 0.f, mu = 0.f;
+  PROF_DECL;
+  PROF_MARK();
+  Operands op;
+  load_operands<false>(op, f.save_w + ((size_t)d * gm.G + g) * GS * GS, G, nullptr, G && train, GS, gsh, o);
+  float mu = 0.f;
+  if ((int)threadIdx.x < GS) mu = f.save_mean[(size_t)d * gm.C + g * GS + threadIdx.x];
+  store_operands<false>(op, sW, sR, nullptr, GS, gsh);
   if ((int)threadIdx.x < GS) {
-    sdz = (G && train) ? __ldcg(G + kSB * kSB + o + threadIdx.x) : 0.f;
-    mu = f.save_mean[(size_t)d * gm.C + g * GS + threadIdx.x];
-  }
-#pragma unroll
-  for (int n = 0; n < kPer; ++n) {
-    const int e = threadIdx.x + 256 * n, i = e >> gsh, j = e & (GS - 1);
-    if (e < GS * GS) { sW[i * LDS + j] = wv[n]; sR[i * LDS + j] = rv[n]; }
-  }
-  if ((int)threadIdx.x < GS) {
-    sSdz[threadIdx.x] = sdz * invM;                   // mean_M dy (0 in eval mode)
+    sSdz[threadIdx.x] = op.sdz * invM;                // mean_M dy (0 in eval mode)
     sMu[threadIdx.x] = mu;
-    if (dybar) dybar[((size_t)d * SB + sb) * kSB + o + threadIdx.x] = sdz * invM;
+    if (dybar) dybar[((size_t)d * SB + sb) * kSB + o + threadIdx.x] = op.sdz * invM;
   }
   __syncthreads();
   PROF_MARK();
-  float c[4][4];
-  if (train) {
-    mm_block<false, true>(sR, sW, GS, t, c);               // R W^T ; P = Phi(-R W^T)
-#pragma unroll
-    for (int r = 0; r < 4; ++r)
-#pragma unroll
-      for (int s = 0; s < 4; ++s) {
-        const int i = 4 * t.bi + r, j = 4 * t.bj + s;
-        c[r][s] = (i > j) ? -c[r][s] : ((i == j) ? -0.5f * c[r][s] : 0.f);
-      }
-    store_block(sT1, t, c);
-    __syncthreads();
-    PROF_MARK();
-    mm_block<true, false>(sW, sT1, GS, t, c);              // T = W^T P
-    store_block(sT2, t, c);
-    __syncthreads();
-    PROF_MARK();
-    mm_block<false, false>(sT2, sW, GS, t, c);             // S' = T W
-    store_block(sT1, t, c);
-    __syncthreads();
-    PROF_MARK();
-  }
-  const float sc = f.a * invM;
-#pragma unroll
-  for (int n = 0; n < kPer; ++n) {
-    const int e = threadIdx.x + 256 * n, i = e >> gsh, j = e & (GS - 1);
-    if (e < GS * GS) {
-      const float bm = train ? sc * (sT1[i * LDS + j] + sT1[j * LDS + i]) : 0.f;
-      coef[e] = (j >= i) ? sW[j * LDS + i] : 0.f;          // A1 = W^T
-      coef[GS * GS + e] = bm;
-      sT2[i * LDS + j] = bm;
-    }
-  }
-  __syncthreads();
-  // cvec_i = -(sum_j W_ji mean(dy)_j + sum_j Bm_ij mu_j): 4 threads per row, partial sums met by shuffle
-  {
-    const int i = threadIdx.x >> 2, q = threadIdx.x & 3;
-    float cv = 0.f;
-    if (train && i < GS) {
-      for (int j = q; j < GS; j += 4) cv = fmaf(sW[j * LDS + i], sSdz[j], fmaf(sT2[i * LDS + j], sMu[j], cv));   // W_ji = 0 for j < i
-    }
-    cv += __shfl_xor_sync(0xffffffffu, cv, 1);
-    cv += __shfl_xor_sync(0xffffffffu, cv, 2);
-    if (q == 0 && i < GS) coef[2 * GS * GS + i] = -cv;
-  }
+  if (train) chol_bwd_core(sR, sW, sT1, sT2, GS, t PROF_PASS);
+  coef_tail<true>(sW, sT1, sT2, sSdz, sMu, train, f.a * invM, GS, gsh, coef);
   PROF_MARK();
   PROF_DUMP("bwd_coef load|mm1|mm2|mm3|tail");
 }
@@ -548,13 +607,12 @@ __global__ void __launch_bounds__(256) bwd_color_kernel(const float* __restrict_
   float* sGam = sT2 + kMat;        // color[g]
   float* sGW = sGam + kMat;        // color W = A1^T
   __shared__ float sSdz[kSB], sMu[kSB];
-  const int g = blockIdx.x, GS = gm.GS, nb = kSB / GS, sb = g / nb, o = (g % nb) * GS;
+  const int g = blockIdx.x;
+  const auto [GS, sb, o, SB] = group_pos(gm, g);
   const Blk t(GS);
-  const int SB = (gm.C + kSB - 1) / kSB;
   const bool train = f.mode == DWT_MODE_TRAIN;
   const int gsh = __ffs(GS) - 1;
   const float invM = 1.f / gm.M;
-  constexpr int kPer = kSB * kSB / 256;
   for (int e = threadIdx.x; e < GS * GS; e += 256) sGam[(e >> gsh) * LDS + (e & (GS - 1))] = color[(size_t)g * GS * GS + e];
   PROF_DECL;
   float dg[4][4], db = 0.f;
@@ -597,29 +655,7 @@ __global__ void __launch_bounds__(256) bwd_color_kernel(const float* __restrict_
     store_block(sGW, t, gw);
     __syncthreads();
     if (train) chol_bwd_core(sR, sW, sT1, sT2, GS, t PROF_PASS);
-    const float sc = f.a * invM;
-#pragma unroll
-    for (int n = 0; n < kPer; ++n) {
-      const int e = threadIdx.x + 256 * n, i = e >> gsh, j = e & (GS - 1);
-      if (e < GS * GS) {
-        const float bm = train ? sc * (sT1[i * LDS + j] + sT1[j * LDS + i]) : 0.f;
-        coef[e] = sGW[j * LDS + i];                   // A1 = (color W)^T, every element
-        coef[GS * GS + e] = bm;
-        sT2[i * LDS + j] = bm;
-      }
-    }
-    __syncthreads();
-    // cvec_i = -(sum_j A1_ij mean(dy)_j + sum_j Bm_ij mu_j), as in bwd_coef
-    {
-      const int i = threadIdx.x >> 2, q = threadIdx.x & 3;
-      float cv = 0.f;
-      if (train && i < GS) {
-        for (int j = q; j < GS; j += 4) cv = fmaf(sGW[j * LDS + i], sSdz[j], fmaf(sT2[i * LDS + j], sMu[j], cv));
-      }
-      cv += __shfl_xor_sync(0xffffffffu, cv, 1);
-      cv += __shfl_xor_sync(0xffffffffu, cv, 2);
-      if (q == 0 && i < GS) coef[2 * GS * GS + i] = -cv;
-    }
+    coef_tail<false>(sGW, sT1, sT2, sSdz, sMu, train, f.a * invM, GS, gsh, coef);   // A1 = (color W)^T
     __syncthreads();                                  // the next domain overwrites every shared matrix
   }
   if (dcolor) {
@@ -653,18 +689,6 @@ __device__ __forceinline__ float trace_of(const float* M, int GS, float* sRed) {
   return sRed[0];
 }
 
-// sum of v over the CTA in one fixed order (warps, then the 8 warp totals); every thread gets it.  Two barriers.
-__device__ __forceinline__ float block_sum(float v, float* sRed) {
-  v = warp_sum(v);
-  if ((threadIdx.x & 31) == 0) sRed[threadIdx.x >> 5] = v;
-  __syncthreads();
-  float s = 0.f;
-#pragma unroll
-  for (int w = 0; w < 8; ++w) s += sRed[w];
-  __syncthreads();
-  return s;
-}
-
 // fwd_zca: grid (G), 256 threads, domains in order with fwd_factor's statistics prologue and EMA tail.  Three products
 // per iteration (P P, (P P) P, (P P P) N) on shared-memory operands; each thread keeps its block of P in registers.
 // A non-finite or non-positive t, or a non-finite W, flags the domain as a non-positive pivot does in fwd_factor
@@ -680,9 +704,9 @@ __global__ void __launch_bounds__(256) fwd_zca_kernel(const float* __restrict__ 
   __shared__ float sC[kMat];       // un-shrunk covariance (for the EMA)
   __shared__ float sMean[kSB], sRow[kSB], sRed[1];
   __shared__ int sBad, sBadDom;
-  const int g = blockIdx.x, GS = gm.GS, nb = kSB / GS, sb = g / nb, o = (g % nb) * GS;
+  const int g = blockIdx.x;
+  const auto [GS, sb, o, SB] = group_pos(gm, g);
   const Blk t(GS);
-  const int SB = (gm.C + kSB - 1) / kSB;
   const float invM = 1.f / gm.M;
   if (threadIdx.x == 0) sBad = 0;
   PROF_DECL;
@@ -767,9 +791,9 @@ __global__ void __launch_bounds__(256) bwd_zca_kernel(const float* __restrict__ 
   float* sP3 = sQN + kMat;         // P^3
   float* sT = sP3 + kMat;          // P Q N; at the end G
   __shared__ float sSdz[kSB], sMu[kSB], sRed[8];
-  const int g = blockIdx.x, d = blockIdx.z, GS = gm.GS, nb = kSB / GS, sb = g / nb, o = (g % nb) * GS;
+  const int g = blockIdx.x, d = blockIdx.z;
+  const auto [GS, sb, o, SB] = group_pos(gm, g);
   const Blk t(GS);
-  const int SB = (gm.C + kSB - 1) / kSB;
   const bool train = f.mode == DWT_MODE_TRAIN && rgram != nullptr;
   const float* G = train ? rgram + ((size_t)d * SB + sb) * kNacc : nullptr;
   const size_t gbase = ((size_t)d * gm.G + g) * GS * GS;
@@ -777,34 +801,20 @@ __global__ void __launch_bounds__(256) bwd_zca_kernel(const float* __restrict__ 
   float* coef = f.coef + ((size_t)d * gm.G + g) * coef_stride(GS);
   const int gsh = __ffs(GS) - 1;
   const float invM = 1.f / gm.M;
-  constexpr int kPer = kSB * kSB / 256;
   PROF_DECL;
   PROF_MARK();
-  float wv[kPer], rv[kPer], sv[kPer];
-#pragma unroll
-  for (int n = 0; n < kPer; ++n) {
-    const int e = threadIdx.x + 256 * n, i = e >> gsh, j = e & (GS - 1);
-    const bool in = e < GS * GS;
-    wv[n] = in ? f.save_w[gbase + e] : 0.f;
-    rv[n] = (in && train) ? __ldcg(G + (o + i) * kSB + o + j) : 0.f;
-    sv[n] = (in && train) ? pd[e] : 0.f;
-  }
-  float sdz = 0.f, mu = 0.f;
-  if ((int)threadIdx.x < GS) {
-    sdz = train ? __ldcg(G + kSB * kSB + o + threadIdx.x) : 0.f;
-    mu = f.save_mean[(size_t)d * gm.C + g * GS + threadIdx.x];
-  }
+  Operands op;
+  load_operands<true>(op, f.save_w + gbase, G, pd, train, GS, gsh, o);   // X = S (save_p slot 0)
+  float mu = 0.f;
+  if ((int)threadIdx.x < GS) mu = f.save_mean[(size_t)d * gm.C + g * GS + threadIdx.x];
+  store_operands<true>(op, sW, sQ, sN, GS, gsh);
   float rw = 0.f;                                     // this thread's share of <R, W>
 #pragma unroll
-  for (int n = 0; n < kPer; ++n) {
-    const int e = threadIdx.x + 256 * n, i = e >> gsh, j = e & (GS - 1);
-    if (e < GS * GS) { sW[i * LDS + j] = wv[n]; sQ[i * LDS + j] = rv[n]; sN[i * LDS + j] = sv[n]; }
-    rw = fmaf(rv[n], wv[n], rw);
-  }
+  for (int n = 0; n < kPer; ++n) rw = fmaf(op.r[n], op.w[n], rw);
   if ((int)threadIdx.x < GS) {
-    sSdz[threadIdx.x] = sdz * invM;                   // mean_M dy (0 in eval mode)
+    sSdz[threadIdx.x] = op.sdz * invM;                // mean_M dy (0 in eval mode)
     sMu[threadIdx.x] = mu;
-    if (dybar) dybar[((size_t)d * SB + sb) * kSB + o + threadIdx.x] = sdz * invM;
+    if (dybar) dybar[((size_t)d * SB + sb) * kSB + o + threadIdx.x] = op.sdz * invM;
   }
   __syncthreads();
   PROF_MARK();
@@ -880,29 +890,7 @@ __global__ void __launch_bounds__(256) bwd_zca_kernel(const float* __restrict__ 
     __syncthreads();
   }
   PROF_MARK();
-  const float sc = f.a * invM;
-#pragma unroll
-  for (int n = 0; n < kPer; ++n) {
-    const int e = threadIdx.x + 256 * n, i = e >> gsh, j = e & (GS - 1);
-    if (e < GS * GS) {
-      const float bm = train ? sc * (sT[i * LDS + j] + sT[j * LDS + i]) : 0.f;
-      coef[e] = sW[j * LDS + i];                      // A1 = W^T, every element
-      coef[GS * GS + e] = bm;
-      sPP[i * LDS + j] = bm;
-    }
-  }
-  __syncthreads();
-  // cvec_i = -(sum_j W_ji mean(dy)_j + sum_j Bm_ij mu_j): 4 threads per row, partial sums met by shuffle
-  {
-    const int i = threadIdx.x >> 2, q = threadIdx.x & 3;
-    float cv = 0.f;
-    if (train && i < GS) {
-      for (int j = q; j < GS; j += 4) cv = fmaf(sW[j * LDS + i], sSdz[j], fmaf(sPP[i * LDS + j], sMu[j], cv));
-    }
-    cv += __shfl_xor_sync(0xffffffffu, cv, 1);
-    cv += __shfl_xor_sync(0xffffffffu, cv, 2);
-    if (q == 0 && i < GS) coef[2 * GS * GS + i] = -cv;
-  }
+  coef_tail<false>(sW, sT, sPP, sSdz, sMu, train, f.a * invM, GS, gsh, coef);
   PROF_MARK();
   PROF_DUMP("bwd_zca load|iterate|tail");
 }
@@ -1012,9 +1000,9 @@ __global__ void __launch_bounds__(256) fwd_eigh_kernel(const float* __restrict__
   __shared__ float sMean[kSB], sRow[kSB], sLam[kSB];
   __shared__ JacobiSmem js;
   __shared__ int sBad, sBadDom;
-  const int g = blockIdx.x, GS = gm.GS, nb = kSB / GS, sb = g / nb, o = (g % nb) * GS;
+  const int g = blockIdx.x;
+  const auto [GS, sb, o, SB] = group_pos(gm, g);
   const Blk t(GS);
-  const int SB = (gm.C + kSB - 1) / kSB;
   const float invM = 1.f / gm.M;
   const int lgs = __ffs(GS) - 1;
   if (threadIdx.x == 0) sBad = 0;
@@ -1076,44 +1064,30 @@ __global__ void __launch_bounds__(256) bwd_eigh_kernel(const float* __restrict__
   float* sT1 = sR + kMat;          // R U, then U H
   float* sH = sT1 + kMat;          // H = (U^T R U) o F; at the end Bm
   __shared__ float sSdz[kSB], sMu[kSB], sRl[kSB];
-  const int g = blockIdx.x, d = blockIdx.z, GS = gm.GS, nb = kSB / GS, sb = g / nb, o = (g % nb) * GS;
+  const int g = blockIdx.x, d = blockIdx.z;
+  const auto [GS, sb, o, SB] = group_pos(gm, g);
   const Blk t(GS);
-  const int SB = (gm.C + kSB - 1) / kSB;
   const bool train = f.mode == DWT_MODE_TRAIN && rgram != nullptr;
   const float* G = train ? rgram + ((size_t)d * SB + sb) * kNacc : nullptr;
-  const size_t gbase = ((size_t)d * gm.G + g) * GS * GS;
   const float* ed = save_e + ((size_t)d * gm.G + g) * (GS + 1) * GS;
   float* coef = f.coef + ((size_t)d * gm.G + g) * coef_stride(GS);
   const int gsh = __ffs(GS) - 1;
   const float invM = 1.f / gm.M;
-  constexpr int kPer = kSB * kSB / 256;
   PROF_DECL;
   PROF_MARK();
-  float wv[kPer], rv[kPer], uv[kPer];
-#pragma unroll
-  for (int n = 0; n < kPer; ++n) {
-    const int e = threadIdx.x + 256 * n, i = e >> gsh, j = e & (GS - 1);
-    const bool in = e < GS * GS;
-    wv[n] = in ? f.save_w[gbase + e] : 0.f;
-    rv[n] = (in && train) ? __ldcg(G + (o + i) * kSB + o + j) : 0.f;
-    uv[n] = (in && train) ? ed[e] : 0.f;
-  }
-  float sdz = 0.f, mu = 0.f, lam = 1.f;
+  Operands op;
+  load_operands<true>(op, f.save_w + ((size_t)d * gm.G + g) * GS * GS, G, ed, train, GS, gsh, o);   // X = U
+  float mu = 0.f, lam = 1.f;
   if ((int)threadIdx.x < GS) {
-    sdz = train ? __ldcg(G + kSB * kSB + o + threadIdx.x) : 0.f;
     mu = f.save_mean[(size_t)d * gm.C + g * GS + threadIdx.x];
     if (train) lam = ed[GS * GS + threadIdx.x];
   }
-#pragma unroll
-  for (int n = 0; n < kPer; ++n) {
-    const int e = threadIdx.x + 256 * n, i = e >> gsh, j = e & (GS - 1);
-    if (e < GS * GS) { sW[i * LDS + j] = wv[n]; sR[i * LDS + j] = rv[n]; sU[i * LDS + j] = uv[n]; }
-  }
+  store_operands<true>(op, sW, sR, sU, GS, gsh);
   if ((int)threadIdx.x < GS) {
-    sSdz[threadIdx.x] = sdz * invM;                   // mean_M dy (0 in eval mode)
+    sSdz[threadIdx.x] = op.sdz * invM;                // mean_M dy (0 in eval mode)
     sMu[threadIdx.x] = mu;
     sRl[threadIdx.x] = sqrtf(lam);
-    if (dybar) dybar[((size_t)d * SB + sb) * kSB + o + threadIdx.x] = sdz * invM;
+    if (dybar) dybar[((size_t)d * SB + sb) * kSB + o + threadIdx.x] = op.sdz * invM;
   }
   __syncthreads();
   PROF_MARK();
@@ -1140,29 +1114,7 @@ __global__ void __launch_bounds__(256) bwd_eigh_kernel(const float* __restrict__
     __syncthreads();
   }
   PROF_MARK();
-  const float sc = f.a * invM;
-#pragma unroll
-  for (int n = 0; n < kPer; ++n) {
-    const int e = threadIdx.x + 256 * n, i = e >> gsh, j = e & (GS - 1);
-    if (e < GS * GS) {
-      const float bm = train ? sc * (sR[i * LDS + j] + sR[j * LDS + i]) : 0.f;
-      coef[e] = sW[j * LDS + i];                      // A1 = W^T, every element
-      coef[GS * GS + e] = bm;
-      sH[i * LDS + j] = bm;
-    }
-  }
-  __syncthreads();
-  // cvec_i = -(sum_j W_ji mean(dy)_j + sum_j Bm_ij mu_j): 4 threads per row, partial sums met by shuffle
-  {
-    const int i = threadIdx.x >> 2, q = threadIdx.x & 3;
-    float cv = 0.f;
-    if (train && i < GS) {
-      for (int j = q; j < GS; j += 4) cv = fmaf(sW[j * LDS + i], sSdz[j], fmaf(sH[i * LDS + j], sMu[j], cv));
-    }
-    cv += __shfl_xor_sync(0xffffffffu, cv, 1);
-    cv += __shfl_xor_sync(0xffffffffu, cv, 2);
-    if (q == 0 && i < GS) coef[2 * GS * GS + i] = -cv;
-  }
+  coef_tail<false>(sW, sR, sH, sSdz, sMu, train, f.a * invM, GS, gsh, coef);
   PROF_MARK();
   PROF_DUMP("bwd_eigh load|solve|tail");
 }
@@ -1274,9 +1226,9 @@ __global__ void __launch_bounds__(256) fwd_instance_kernel(const float* __restri
   __shared__ float sC[kMat];       // written by domain_stats, not read (no EMA)
   __shared__ float sMean[kSB], sRow[kSB];
   __shared__ int sBadDom;
-  const int g = blockIdx.x, d = blockIdx.z, GS = gm.GS, nb = kSB / GS, sb = g / nb, o = (g % nb) * GS;
+  const int g = blockIdx.x, d = blockIdx.z;
+  const auto [GS, sb, o, SB] = group_pos(gm, g);
   const Blk t(GS);
-  const int SB = (gm.C + kSB - 1) / kSB;
   const float* G = gram + ((size_t)d * SB + sb) * kNacc;
   float a[4][4], w[4][4];
   EmaOld old;                      // f.update_running is 0: domain_stats reads no running buffer
@@ -1284,14 +1236,7 @@ __global__ void __launch_bounds__(256) fwd_instance_kernel(const float* __restri
   if (!factor_and_invert(a, w, GS, t, sp)) sBadDom = 1;
   __syncthreads();                 // sBadDom final
   const bool bad = sBadDom != 0;
-  if (t.act) {
-    float* wout = f.save_w + ((size_t)d * gm.G + g) * GS * GS;
-    const float q = __int_as_float(0x7fc00000);   // a NaN the apply's TF32 split keeps (0x7fffffff would round to -0)
-#pragma unroll
-    for (int r = 0; r < 4; ++r)
-      *reinterpret_cast<float4*>(wout + (size_t)(4 * t.bi + r) * GS + 4 * t.bj) =
-          bad ? make_float4(q, q, q, q) : make_float4(w[r][0], w[r][1], w[r][2], w[r][3]);
-  }
+  store_w_or_nan(f.save_w, (size_t)d * gm.G + g, GS, t, w, bad);
   if (threadIdx.x == 0 && bad) atomicOr(f.status, DWT_STATUS_NOT_PD);
 }
 
@@ -1308,10 +1253,11 @@ __device__ __forceinline__ int sw_rec(int GS) { return GS * GS + GS; }
 // second pass over x; bit-identical reruns).  Eval: row D is a copy of the running buffers.
 __global__ void __launch_bounds__(256) sw_stats_kernel(const float* __restrict__ gram, const float* __restrict__ shift,
                                                        const Geom gm, const SwFin f) {
-  const int GS = gm.GS, g = blockIdx.y, nb = kSB / GS, sb = g / nb, o = (g % nb) * GS, rec = sw_rec(GS);
-  const int e = blockIdx.x * 256 + threadIdx.x;
+  const int g = blockIdx.y;
+  const auto [GS, sb, o, SB] = group_pos(gm, g);
+  const int rec = sw_rec(GS), e = blockIdx.x * 256 + threadIdx.x;
   if (e >= rec) return;
-  const int SB = (gm.C + kSB - 1) / kSB, D = gm.D;
+  const int D = gm.D;
   const float invM = 1.f / gm.M;
   const double invMd = 1.0 / (double)gm.M;
   const bool cov = e < GS * GS;
@@ -1391,21 +1337,14 @@ __global__ void __launch_bounds__(256) sw_fwd_factor_kernel(const Geom gm, const
   }
   const bool ok = factor_and_invert(a, w, GS, t, sp);
   bad = __syncthreads_or(bad || !ok) != 0;
-  if (t.act) {
-    float* wout = f.save_w + ((size_t)d * gm.G + g) * GS * GS;
-    const float q = __int_as_float(0x7fc00000);   // a NaN the apply's TF32 split keeps
-#pragma unroll
-    for (int r = 0; r < 4; ++r)
-      *reinterpret_cast<float4*>(wout + (size_t)(4 * t.bi + r) * GS + 4 * t.bj) =
-          bad ? make_float4(q, q, q, q) : make_float4(w[r][0], w[r][1], w[r][2], w[r][3]);
-  }
+  store_w_or_nan(f.save_w, (size_t)d * gm.G + g, GS, t, w, bad);
   if (threadIdx.x == 0 && bad) atomicOr(f.status, DWT_STATUS_NOT_PD);
   if (d != 0 || !f.train || !f.update_running) return;
-  constexpr int kPer = (kSB * kSB + kSB + 255) / 256;
-  float old[kPer], stat[kPer];
+  constexpr int kRecPer = (kSB * kSB + kSB + 255) / 256;
+  float old[kRecPer], stat[kRecPer];
   bool fin = true;
 #pragma unroll
-  for (int n = 0; n < kPer; ++n) {
+  for (int n = 0; n < kRecPer; ++n) {
     const int e = threadIdx.x + 256 * n;
     stat[n] = e < rec ? sbt[e] : 0.f;
     old[n] = e < GS * GS ? f.rcov[(size_t)g * GS * GS + e] : (e < rec ? f.rmean[g * GS + e - GS * GS] : 0.f);
@@ -1414,7 +1353,7 @@ __global__ void __launch_bounds__(256) sw_fwd_factor_kernel(const Geom gm, const
   if (!__syncthreads_or(!fin)) {        // dwt_whiten_fwd's EMA: (1 - m) old + m stat on the unshrunk batch moments
     const float m = f.momentum, k = 1.f - f.momentum;
 #pragma unroll
-    for (int n = 0; n < kPer; ++n) {
+    for (int n = 0; n < kRecPer; ++n) {
       const int e = threadIdx.x + 256 * n;
       if (e < GS * GS) f.rcov[(size_t)g * GS * GS + e] = m * stat[n] + k * old[n];
       else if (e < rec) f.rmean[g * GS + e - GS * GS] = fmaf(k, old[n], __fmul_rn(m, stat[n]));
@@ -1422,18 +1361,6 @@ __global__ void __launch_bounds__(256) sw_fwd_factor_kernel(const Geom gm, const
   } else if (threadIdx.x == 0) {
     atomicOr(f.status, DWT_STATUS_NOT_PD);
   }
-}
-
-// Deterministic sum of v over the CTA (256 threads): warp trees, then the 8 warps in order; the total in every thread.
-__device__ __forceinline__ float cta_sum(float v, float* sRed) {
-  v = warp_sum(v);
-  __syncthreads();                     // sRed free
-  if ((threadIdx.x & 31) == 0) sRed[threadIdx.x >> 5] = v;
-  __syncthreads();
-  float s = 0.f;
-#pragma unroll
-  for (int w = 0; w < 8; ++w) s += sRed[w];
-  return s;
 }
 
 // sw_bwd_coef: grid (G, 1, D), 256 threads, one CTA per (image, group).  rgram [D][SB][kNacc] = (R = sum dy (x - m)^T |
@@ -1446,46 +1373,21 @@ __global__ void __launch_bounds__(256) sw_bwd_coef_kernel(const float* __restric
   float* sR = sW + kMat;
   float* sT = sR + kMat;
   __shared__ float sSdz[kSB], sRed[8];
-  const int g = blockIdx.x, d = blockIdx.z, GS = gm.GS, nb = kSB / GS, sb = g / nb, o = (g % nb) * GS, rec = sw_rec(GS);
+  const int g = blockIdx.x, d = blockIdx.z, rec = sw_rec(gm.GS);
+  const auto [GS, sb, o, SB] = group_pos(gm, g);
   const Blk t(GS);
-  const int SB = (gm.C + kSB - 1) / kSB, gsh = __ffs(GS) - 1;
+  const int gsh = __ffs(GS) - 1;
   const float* G = rgram + ((size_t)d * SB + sb) * kNacc;
   const float* sn = f.save_stats + ((size_t)d * gm.G + g) * rec;
   const float* sbt = f.save_stats + ((size_t)gm.D * gm.G + g) * rec;
   float* out = pd + ((size_t)d * gm.G + g) * rec;
-  constexpr int kPer = kSB * kSB / 256;
-  float wv[kPer], rv[kPer];
-#pragma unroll
-  for (int n = 0; n < kPer; ++n) {
-    const int e = threadIdx.x + 256 * n, i = e >> gsh, j = e & (GS - 1);
-    const bool in = e < GS * GS;
-    wv[n] = in ? f.save_w[((size_t)d * gm.G + g) * GS * GS + e] : 0.f;
-    rv[n] = in ? __ldcg(G + (o + i) * kSB + o + j) : 0.f;
-  }
-  if ((int)threadIdx.x < GS) sSdz[threadIdx.x] = __ldcg(G + kSB * kSB + o + threadIdx.x);
-#pragma unroll
-  for (int n = 0; n < kPer; ++n) {
-    const int e = threadIdx.x + 256 * n, i = e >> gsh, j = e & (GS - 1);
-    if (e < GS * GS) { sW[i * LDS + j] = wv[n]; sR[i * LDS + j] = rv[n]; }
-  }
+  PROF_DECL;
+  Operands op;
+  load_operands<false>(op, f.save_w + ((size_t)d * gm.G + g) * GS * GS, G, nullptr, true, GS, gsh, o);
+  store_operands<false>(op, sW, sR, nullptr, GS, gsh);
+  if ((int)threadIdx.x < GS) sSdz[threadIdx.x] = op.sdz;
   __syncthreads();
-  float c[4][4];
-  mm_block<false, true>(sR, sW, GS, t, c);               // R W^T ; Phi(-R W^T)
-#pragma unroll
-  for (int r = 0; r < 4; ++r)
-#pragma unroll
-    for (int s = 0; s < 4; ++s) {
-      const int i = 4 * t.bi + r, j = 4 * t.bj + s;
-      c[r][s] = (i > j) ? -c[r][s] : ((i == j) ? -0.5f * c[r][s] : 0.f);
-    }
-  store_block(sT, t, c);
-  __syncthreads();
-  mm_block<true, false>(sW, sT, GS, t, c);               // W^T Phi (sR is free: the barrier above follows its reads)
-  store_block(sR, t, c);
-  __syncthreads();
-  mm_block<false, false>(sR, sW, GS, t, c);              // T' = W^T Phi W
-  store_block(sT, t, c);
-  __syncthreads();
+  chol_bwd_core(sR, sW, sT, sR, GS, t PROF_PASS);       // T' = W^T Phi(-R W^T) W into sT
   const float h = 0.5f * f.a;
   float p_bw = 0.f, p_iw = 0.f, p_bn = 0.f, p_in = 0.f;
 #pragma unroll
@@ -1518,7 +1420,7 @@ __global__ void __launch_bounds__(256) sw_bwd_coef_kernel(const float* __restric
   const float terms[6] = {t_b, t_i, p_bw, p_iw, p_bn, p_in};
 #pragma unroll
   for (int k = 0; k < 6; ++k) {
-    const float s = cta_sum(terms[k], sRed);
+    const float s = block_sum(terms[k], sRed);
     if (threadIdx.x == 0) part[((size_t)d * gm.G + g) * 8 + k] = s;
   }
 }
@@ -1565,8 +1467,9 @@ __global__ void __launch_bounds__(256) sw_bwd_apply_coef_kernel(const float* __r
   float* sW = dsm;
   float* sQ = sW + kMat;
   __shared__ float sDmu[kSB], sK[kSB];
-  const int g = blockIdx.x, d = blockIdx.z, GS = gm.GS, nb = kSB / GS, sb = g / nb, o = (g % nb) * GS, rec = sw_rec(GS);
-  const int SB = (gm.C + kSB - 1) / kSB, gsh = __ffs(GS) - 1;
+  const int g = blockIdx.x, d = blockIdx.z, rec = sw_rec(gm.GS);
+  const auto [GS, sb, o, SB] = group_pos(gm, g);
+  const int gsh = __ffs(GS) - 1;
   const float* p = pd + ((size_t)d * gm.G + g) * rec;
   const float* ps = sums + (size_t)g * rec;
   const float* sn = f.save_stats + ((size_t)d * gm.G + g) * rec;
@@ -1592,9 +1495,8 @@ __global__ void __launch_bounds__(256) sw_bwd_apply_coef_kernel(const float* __r
     mu[(size_t)d * gm.C + g * GS + threadIdx.x] = mn;
   }
   nanc = __syncthreads_or(nanc) != 0;
-  // a group whose A1 or Bm is not finite gets both as the quiet NaN the apply's TF32 split keeps (an arithmetic NaN,
-  // 0x7fffffff, would round to -0 there and leave a finite, wrong dx)
-  const float q = __int_as_float(0x7fc00000);
+  // a group whose A1 or Bm is not finite gets both as kApplyNaN
+  const float q = __int_as_float(kApplyNaN);
   for (int e = threadIdx.x; e < GS * GS; e += 256) {
     const int i = e >> gsh, j = e & (GS - 1);
     cf[e] = nanc ? q : ((j >= i) ? sW[j * LDS + i] : 0.f);   // A1 = W^T
