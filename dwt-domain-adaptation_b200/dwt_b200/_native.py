@@ -25,6 +25,7 @@ DTYPE_BF16 = 0x200                 # bf16 activations (gs 1/2/4 and BN channels-
 STATUS_NOT_PD, STATUS_BAD_LABEL = 1, 2
 ZCA_MAX_ITERATIONS = 16            # Newton-Schulz iterations of the ZCA basis (dwt_whiten_zca_*): 1..16
 EIGH = "eigh"                      # the exact ZCA basis (dwt_whiten_eigh_*) where a number of iterations goes
+COLOR = "color"                    # the Cholesky basis coloured (dwt_whiten_color_*): functional._NormFunction's basis
 KIND_WHITEN, KIND_BN = 0, 1
 
 _c_float_p = ctypes.c_void_p
@@ -270,33 +271,18 @@ def workspace(device, n, c, hw, gs, nd):
     need = lib().dwt_workspace_bytes(n, c, hw, gs, nd)
     if need == 0:
         raise NativeError(f"invalid geometry for workspace: C={c} group_size={gs} domains={nd}")
+    return grow_workspace(device, need)
+
+
+def grow_workspace(device, nbytes):
+    """The current stream's workspace, grown to at least nbytes (a new buffer has at least 8 MiB).  The per-image entry
+    points size theirs by dwt_instance_workspace_bytes / dwt_switch_workspace_bytes, which give 0 for a geometry they
+    refuse (the call then reports why)."""
     key = (device.index, torch.cuda.current_stream(device).cuda_stream)
     buf = _workspaces.get(key)
-    if buf is None or buf.numel() < need:
-        buf = torch.zeros(max(need, 8 << 20), dtype=torch.uint8, device=device)
+    if buf is None or buf.numel() < nbytes:
+        buf = torch.zeros(max(nbytes, 8 << 20), dtype=torch.uint8, device=device)
         _workspaces[key] = buf
-    return buf
-
-
-def instance_workspace(device, n, c, hw, gs):
-    """The current stream's workspace (see workspace()), grown to what instance whitening of [n, c, hw] at group size gs
-    needs (dwt_instance_workspace_bytes; 0 for a geometry the entry points refuse, which then report why)."""
-    need = lib().dwt_instance_workspace_bytes(n, c, hw, gs)
-    buf = workspace(device, 1, 4, 1, 1, 1)
-    if buf.numel() < need:
-        buf = torch.zeros(need, dtype=torch.uint8, device=device)
-        _workspaces[(device.index, torch.cuda.current_stream(device).cuda_stream)] = buf
-    return buf
-
-
-def switch_workspace(device, n, c, hw, gs):
-    """The current stream's workspace (see workspace()), grown to what switchable whitening of [n, c, hw] at group size gs
-    needs (dwt_switch_workspace_bytes; 0 for a geometry the entry points refuse, which then report why)."""
-    need = lib().dwt_switch_workspace_bytes(n, c, hw, gs)
-    buf = workspace(device, 1, 4, 1, 1, 1)
-    if buf.numel() < need:
-        buf = torch.zeros(need, dtype=torch.uint8, device=device)
-        _workspaces[(device.index, torch.cuda.current_stream(device).cuda_stream)] = buf
     return buf
 
 

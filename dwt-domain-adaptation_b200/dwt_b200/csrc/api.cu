@@ -25,11 +25,17 @@ int fail(int code, const char* fmt, ...) {
   return code;
 }
 
-int check_launch(const char* what) {
+// what: printf-style name of the kernel, formatted only when the launch failed
+int check_launch(const char* what, ...) {
   cudaError_t e = cudaPeekAtLastError();
   if (e != cudaSuccess) {
     cudaGetLastError();
-    return fail(DWT_E_LAUNCH, "%s: %s", what, cudaGetErrorString(e));
+    char name[128];
+    va_list ap;
+    va_start(ap, what);
+    vsnprintf(name, sizeof(name), what, ap);
+    va_end(ap);
+    return fail(DWT_E_LAUNCH, "%s: %s", name, cudaGetErrorString(e));
   }
   return DWT_OK;
 }
@@ -514,17 +520,22 @@ void basis_bwd(const float* rgram, const dwt::Geom& gm, const dwt::BwdFin& fin, 
 }
 
 // The checks both directions make, in order; `own` holds the direction's own (residual, running buffers, gradient
-// outputs), checked before the epilogue's family rule.  in0, in1: the tensors the kernels read (x, x or x, dout);
-// out: the one they write (y or dx); dout2: the backward's second gradient addend.
+// outputs, basis arguments), checked before the epilogue's family rule.  in0, in1: the tensors the kernels read (x, x or
+// x, dout); out: the one they write (y or dx); dout2: the backward's second gradient addend; z: the call's basis, which,
+// when it is not Cholesky, must end up on the tensor-core kernels.
 template <class Own>
-int validate(Call& c, bool bwd, const void* in0, const void* in1, const void* out, const void* dout2, int64_t N, int64_t C, int64_t HW, int GS,
-             int D, int mode, int epi, const float* gamma, const float* beta, const float* save_mean, const float* save_w,
-             void* ws, size_t ws_bytes, Own own) {
+int validate(Call& c, const Basis& z, bool bwd, const void* in0, const void* in1, const void* out, const void* dout2, int64_t N,
+             int64_t C, int64_t HW, int GS, int D, int mode, int epi, const float* gamma, const float* beta,
+             const float* save_mean, const float* save_w, void* ws, size_t ws_bytes, Own own) {
   c.nhwc = (mode & DWT_LAYOUT_NHWC) != 0, c.bf16 = (mode & DWT_DTYPE_BF16) != 0, c.mode = mode & 0xFF;
   const int elem_bytes = c.bf16 && !c.nhwc ? 2 : 4;
-  if (int rc = make_plan(c.p, bwd ? K_BWD_REDUCE : K_STATS, bwd ? K_BWD_APPLY : K_APPLY, in0, in1, out, N, C, HW, GS, D, elem_bytes)) return rc;
+  // colouring names itself in every refusal of its geometry, make_plan()'s and route()'s included
+  auto geometry = [&](int rc) { return rc == DWT_E_UNSUPPORTED && z.kind == Basis::COLOR ? basis_refuse(z, N, C, HW, GS) : rc; };
+  if (int rc = geometry(make_plan(c.p, bwd ? K_BWD_REDUCE : K_STATS, bwd ? K_BWD_APPLY : K_APPLY, in0, in1, out, N, C, HW,
+                                  GS, D, elem_bytes)))
+    return rc;
   if (!in0 || !in1 || !out || !save_mean || !save_w || !ws) return fail(DWT_E_INVALID, "null pointer argument");
-  if (int rc = route(c.p, c.nhwc, c.bf16, dout2, &c.r)) return rc;
+  if (int rc = geometry(route(c.p, c.nhwc, c.bf16, dout2, &c.r))) return rc;
   const uintptr_t bits = (uintptr_t)in0 | (uintptr_t)in1 | (c.r.inputs_only ? 0 : (uintptr_t)out);
   if (c.r.align && bits % c.r.align != 0)
     return fail(DWT_E_INVALID, "%s must be %d-byte aligned%s", c.r.what ? c.r.what : bwd ? (c.r.inputs_only ? "x and dout" : "x, dout and dx")
@@ -542,6 +553,7 @@ int validate(Call& c, bool bwd, const void* in0, const void* in1, const void* ou
     return fail(DWT_E_LAUNCH, "cudaFuncSetAttribute failed (%d)", g_tiled_rc);
   if (c.r.fam == TC && ensure_tc() != 0) {
     if (c.bf16 || c.nhwc || GS > DWT_MAX_GROUP_SIZE) return fail(DWT_E_LAUNCH, "tensor-core kernel set-up failed (%d)", g_tc_rc);
+    if (z.own()) return basis_refuse(z, N, C, HW, GS);                // no other kernels take it
     c.r.fam = TILED;      // fp32 NCHW up to group size 64: the tiled kernels take every geometry
   }
   return DWT_OK;
@@ -554,7 +566,7 @@ int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, 
                     cudaStream_t st, const Basis& basis = Basis{}) {
   Call c;
   const bool need_running = ((mode & 0xFF) == DWT_MODE_EVAL) || update_running;
-  const int rc = validate(c, false, x, x, y, nullptr, N, C, HW, GS, D, mode, epi, gamma, beta, save_mean, save_w, ws, ws_bytes, [&] {
+  const int rc = validate(c, basis, false, x, x, y, nullptr, N, C, HW, GS, D, mode, epi, gamma, beta, save_mean, save_w, ws, ws_bytes, [&] {
     if ((epi & DWT_EPI_RESIDUAL) && ((epi & 3) != 3 || !residual)) return fail(DWT_E_INVALID, "RESIDUAL epilogue needs AFFINE|RELU and a residual tensor");
     if (epi & DWT_EPI_RESIDUAL) if (int rc = check_align(c.bf16, (uintptr_t)residual, "residual")) return rc;
     if (relu_mask && !((epi & DWT_EPI_RESIDUAL) && c.nhwc))
@@ -562,10 +574,7 @@ int whiten_like_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, 
     if (basis.own()) if (int rc = basis_check(c, basis, false)) return rc;
     return check_running(need_running, rmean, rcov, D);
   });
-  // colouring names itself in every refusal of its geometry (route()'s and make_plan()'s included)
-  if (rc == DWT_E_UNSUPPORTED && basis.kind == Basis::COLOR) return basis_refuse(basis, N, C, HW, GS);
   if (rc) return rc;
-  if (basis.own() && c.r.fam != TC) return basis_refuse(basis, N, C, HW, GS);   // the tensor-core kernels could not be set up
   const Plan& p = c.p; const Workspace& w = c.w;
   const bool bf16 = c.bf16, nhwc = c.nhwc, train = c.mode == DWT_MODE_TRAIN;
   const dwt::FwdFin fin = make_fwd_fin(a, b, momentum, unbias, train ? update_running : 0, need_running, rmean, rcov,
@@ -637,7 +646,7 @@ int whiten_like_bwd(const float* x, const float* dout, const float* dout2, float
                     const float* beta, const uint8_t* relu_mask, float* dresidual, int epi, float* dgamma,
                     float* dbeta, void* ws, size_t ws_bytes, cudaStream_t st, const Basis& basis = Basis{}) {
   Call c;
-  const int rc = validate(c, true, x, dout, dx, dout2, N, C, HW, GS, D, mode, epi, gamma, beta, save_mean, save_w, ws, ws_bytes, [&] {
+  const int rc = validate(c, basis, true, x, dout, dx, dout2, N, C, HW, GS, D, mode, epi, gamma, beta, save_mean, save_w, ws, ws_bytes, [&] {
     if (epi & DWT_EPI_RESIDUAL) {
       // backward of out = relu(z + residual): the ReLU mask comes from the byte map the forward wrote, the masked
       // gradient goes to dresidual and is what the apply pass reads
@@ -652,9 +661,7 @@ int whiten_like_bwd(const float* x, const float* dout, const float* dout2, float
     if (basis.own()) return basis_check(c, basis, true);
     return DWT_OK;
   });
-  if (rc == DWT_E_UNSUPPORTED && basis.kind == Basis::COLOR) return basis_refuse(basis, N, C, HW, GS);
   if (rc) return rc;
-  if (basis.own() && c.r.fam != TC) return basis_refuse(basis, N, C, HW, GS);   // the tensor-core kernels could not be set up
   const Plan& p = c.p; const Workspace& w = c.w;
   const bool bf16 = c.bf16, nhwc = c.nhwc;
   const dwt::BwdFin fin = make_bwd_fin(a, c.mode, epi, save_mean, save_w, gamma, dgamma, dbeta, w);
@@ -830,30 +837,51 @@ int tail2_bwd(int kind, const dwt_tail_site* s, const float* dout, const float* 
   return check_launch("channels-last two-site backward apply kernel");
 }
 
-// ---- instance whitening (dwt_whiten_instance_fwd / dwt_whiten_instance_bwd) ------------------------------------------
+// ---- per-image whitening: instance (dwt_whiten_instance_*) and switchable (dwt_whiten_switch_*) -----------------------
 // Every image is its own problem.  The tensor-core kernels index their problems by (domain, super-block) and the dense
-// ones by (domain, group); instance whitening runs them with the images as the domains: Geom D = N images of N = 1 each,
+// ones by (domain, group); per-image whitening runs them with the images as the domains: Geom D = N images of N = 1 each,
 // M = HW.  Statistics and the backward contraction are tc_stats / tc_bwd_reduce unchanged (tc_chunks splits an image over
 // CTAs when there are fewer problems than two per SM, and gives a CTA a whole image otherwise -- then the partials are the
 // reduced moments and the fixed-order reduction is skipped); apply and backward apply are tc_apply / tc_bwd_apply
-// unchanged; the backward coefficients are bwd_coef unchanged (one CTA per (domain, group) already); the forward factor is
-// fwd_instance (fwd_factor serialises the domains of a group in one CTA for its ordered EMA).
-// what: the family the refusal text names (switchable whitening shares the geometry)
-int inst_refuse(int64_t N, int64_t C, int64_t HW, int GS, int flags, const char* what = "instance whitening") {
+// unchanged.  Between them each variant runs its own finalize:
+//   instance    forward fwd_instance (fwd_factor serialises the domains of a group in one CTA for its ordered EMA);
+//               backward bwd_coef unchanged (one CTA per (domain, group) already), tc_bwd_apply centred on save_mean.
+//   switchable  forward sw_stats (save_stats: per-image rows and the batch row by the law of total covariance, no second
+//               pass over x) -> sw_fwd_factor (mix, Cholesky + inverse, EMA); backward tc_bwd_reduce about the mixed mean
+//               without the pilot centring (sum (x - m) is not zero) -> sw_bwd_coef / sw_bwd_sum / sw_dmix /
+//               sw_bwd_apply_coef -> tc_bwd_apply centred on the images' own means, the per-image constant of dx in dybar.
+// What a switchable call adds to an instance call (Mix{} is instance whitening)
+struct Mix {
+  bool on = false;
+  const float* mix = nullptr;          // [6]
+  const float* save_stats = nullptr;   // [N + 1][G][gs*gs + gs], written by the forward
+  float momentum = 0.f;
+  int update_running = 0;
+  float* rmean = nullptr;              // [C], [G][gs][gs]
+  float* rcov = nullptr;
+  float* dmix = nullptr;               // backward: [6] or null
+  const char* what() const { return on ? "switchable whitening" : "instance whitening"; }
+};
+
+int image_refuse(int64_t N, int64_t C, int64_t HW, int GS, int flags, const char* what) {
   return fail(DWT_E_UNSUPPORTED, "%s is built for the tensor-core kernels only: group_size 8, 16, 32, 64 "
               "dividing C, HW >= 256 and a multiple of 4 (NCHW bf16: of 8), N <= 65535 images, N*C*HW < 2^31 "
               "(C=%lld HW=%lld N=%lld gs=%d flags=%#x)", what, (long long)C, (long long)HW, (long long)N, GS, flags);
 }
 
-// flags and geometry; fills gm (no device call)
-int inst_geom(dwt::Geom& gm, int64_t N, int64_t C, int64_t HW, int GS, int flags, const char* what = "instance whitening") {
-  if (flags & ~(DWT_LAYOUT_NHWC | DWT_DTYPE_BF16)) return fail(DWT_E_INVALID, "bad flags %#x (DWT_LAYOUT_NHWC | DWT_DTYPE_BF16)", flags);
+// flags (switchable: the mode word, which may also hold DWT_MODE_EVAL) and geometry; fills gm (no device call)
+int image_geom(dwt::Geom& gm, int64_t N, int64_t C, int64_t HW, int GS, int flags, const Mix& m) {
+  if (m.on && (flags & ~(DWT_MODE_EVAL | DWT_LAYOUT_NHWC | DWT_DTYPE_BF16)))
+    return fail(DWT_E_INVALID, "bad mode %#x (DWT_MODE_TRAIN or DWT_MODE_EVAL | DWT_LAYOUT_NHWC | DWT_DTYPE_BF16)", flags);
+  if (!m.on && (flags & ~(DWT_LAYOUT_NHWC | DWT_DTYPE_BF16)))
+    return fail(DWT_E_INVALID, "bad flags %#x (DWT_LAYOUT_NHWC | DWT_DTYPE_BF16)", flags);
+  flags &= ~DWT_MODE_EVAL;
   if (N <= 0 || C <= 0 || HW <= 0) return fail(DWT_E_INVALID, "empty tensor (N=%lld C=%lld HW=%lld)", (long long)N,
                                                (long long)C, (long long)HW);
   const bool nchw_bf16 = (flags & DWT_DTYPE_BF16) && !(flags & DWT_LAYOUT_NHWC);
   if ((GS != 8 && GS != 16 && GS != 32 && GS != 64) || C % GS != 0 || HW < 256 || HW % (nchw_bf16 ? 8 : 4) != 0 ||
       N > 65535 || N * C * HW >= (int64_t)1 << 31)
-    return inst_refuse(N, C, HW, GS, flags, what);
+    return image_refuse(N, C, HW, GS, flags, m.what());
   gm = dwt::Geom{};
   gm.N = 1; gm.C = (int)C; gm.HW = (int)HW; gm.GS = GS; gm.G = (int)(C / GS); gm.D = (int)N; gm.ppc = 1;
   gm.M = (float)HW;
@@ -861,15 +889,25 @@ int inst_geom(dwt::Geom& gm, int64_t N, int64_t C, int64_t HW, int GS, int flags
   return DWT_OK;
 }
 
+struct ImageWork {
+  Workspace w;
+  float* pd;       // switchable: [N][G][gs*gs + gs]  P_n | dm_n
+  float* part;     //             [N][G][8]           dmix terms per (image, group)
+  float* sums;     //             [G][gs*gs + gs]     sum_n P_n | sum_n dm_n
+  float* mu;       //             [N][C]              the images' own means (the backward apply's centre)
+};
+
 // Scratch behind the common head (the status word is shared with every other call on the stream's workspace):
-// partials [N][SB][nchunks][64*64+64], reduced moments (only when nchunks > 1), pilot shifts / mean of dy [N][SB][64],
-// backward coefficients [N][G][2 gs^2 + gs]
-Workspace carve_instance(void* base, const dwt::Geom& gm) {
+// partials [N][SB][nchunks][64*64+64], reduced moments (only when nchunks > 1), pilot shifts / mean of dy / dybar
+// [N][SB][64], backward coefficients [N][G][2 gs^2 + gs]; switchable whitening then pd, part, sums and mu
+ImageWork carve_image(void* base, const dwt::Geom& gm, const Mix& m) {
   const size_t P = (size_t)dwt::tc_superblocks(gm) * gm.D, nacc = 64 * 64 + 64;
+  const size_t rec = (size_t)gm.GS * gm.GS + gm.GS, PG = (size_t)gm.D * gm.G;
   size_t off = kOffScratch;
   auto take = [&](size_t nbytes) { size_t o = off; off = align_up(off + nbytes, 256); return o; };
   char* b = static_cast<char*>(base);
-  Workspace w{};
+  ImageWork s{};
+  Workspace& w = s.w;
   w.status = reinterpret_cast<int*>(b);
   w.counters = reinterpret_cast<int*>(b + kOffCounters);
   w.dom_counter = reinterpret_cast<int*>(b + kOffDom1);
@@ -877,236 +915,148 @@ Workspace carve_instance(void* base, const dwt::Geom& gm) {
   w.partial = reinterpret_cast<float*>(b + take(sizeof(float) * P * gm.nchunks * nacc));
   w.gram = gm.nchunks > 1 ? reinterpret_cast<float*>(b + take(sizeof(float) * P * nacc)) : w.partial;
   w.shift = reinterpret_cast<float*>(b + take(sizeof(float) * P * 64));
-  w.coef = reinterpret_cast<float*>(b + take(sizeof(float) * (size_t)gm.D * gm.G * dwt::coef_stride(gm.GS)));
+  w.coef = reinterpret_cast<float*>(b + take(sizeof(float) * PG * dwt::coef_stride(gm.GS)));
+  if (m.on) {
+    s.pd = reinterpret_cast<float*>(b + take(sizeof(float) * PG * rec));
+    s.part = reinterpret_cast<float*>(b + take(sizeof(float) * PG * 8));
+    s.sums = reinterpret_cast<float*>(b + take(sizeof(float) * gm.G * rec));
+    s.mu = reinterpret_cast<float*>(b + take(sizeof(float) * (size_t)gm.D * gm.C));
+  }
   w.bytes = off;
-  return w;
-}
-
-// Profile family of a launch: [pass][channels-last * 2 + bf16]
-const char* const kIwName[6][4] = {
-    {"iw_stats", "iw_stats_bf16", "iw_stats_nhwc", "iw_stats_nhwc_bf16"},
-    {"iw_fwd_finalize", "iw_fwd_finalize_bf16", "iw_fwd_finalize", "iw_fwd_finalize_bf16"},
-    {"iw_apply", "iw_apply_bf16", "iw_apply_nhwc", "iw_apply_nhwc_bf16"},
-    {"iw_bwd_reduce", "iw_bwd_reduce_bf16", "iw_bwd_reduce_nhwc", "iw_bwd_reduce_nhwc_bf16"},
-    {"iw_bwd_finalize", "iw_bwd_finalize_bf16", "iw_bwd_finalize", "iw_bwd_finalize_bf16"},
-    {"iw_bwd_apply", "iw_bwd_apply_bf16", "iw_bwd_apply_nhwc", "iw_bwd_apply_nhwc_bf16"}};
-
-// The checks both directions make, in order: flags and geometry, pointers, alignment, workspace, kernel set-up.
-// in0, in1: what the kernels read (x; x and dout); out: what they write (y; dx).
-int inst_validate(dwt::Geom& gm, Workspace& w, const void* in0, const void* in1, const void* out, int64_t N, int64_t C, int64_t HW,
-                  int GS, int flags, const float* save_mean, const float* save_w, void* ws, size_t ws_bytes) {
-  if (int rc = inst_geom(gm, N, C, HW, GS, flags)) return rc;
-  if (!in0 || !in1 || !out || !save_mean || !save_w || !ws) return fail(DWT_E_INVALID, "null pointer argument");
-  if (((uintptr_t)in0 | (uintptr_t)in1 | (uintptr_t)out | (uintptr_t)save_w) % 16 != 0)
-    return fail(DWT_E_INVALID, "activation tensors and save_w must be 16-byte aligned (instance whitening: TMA and vector stores)");
-  w = carve_instance(ws, gm);
-  if (w.bytes > ws_bytes) return fail(DWT_E_WORKSPACE, "workspace too small: need %zu bytes, got %zu", w.bytes, ws_bytes);
-  if ((uintptr_t)ws % 256 != 0) return fail(DWT_E_WORKSPACE, "workspace must be 256-byte aligned");
-  if (ensure_tc() != 0) return inst_refuse(N, C, HW, GS, flags);      // the tensor-core kernels could not be set up
-  return DWT_OK;
-}
-
-int instance_fwd(const void* x, void* y, int64_t N, int64_t C, int64_t HW, int GS, int flags, float eps, float* save_mean,
-                 float* save_w, void* ws, size_t ws_bytes, cudaStream_t st) {
-  dwt::Geom gm;
-  Workspace w;
-  if (int rc = inst_validate(gm, w, x, x, y, N, C, HW, GS, flags, save_mean, save_w, ws, ws_bytes)) return rc;
-  const bool nhwc = (flags & DWT_LAYOUT_NHWC) != 0, bf16 = (flags & DWT_DTYPE_BF16) != 0;
-  const int k = 2 * nhwc + bf16;
-  const double E = (bf16 ? 2.0 : 4.0) * (double)N * (double)C * (double)HW;
-  dwt::FwdFin fin{};
-  fin.a = 1.f - eps; fin.b = eps; fin.save_mean = save_mean; fin.save_w = save_w; fin.status = w.status;
-  {
-    Launch l(kIwName[0][k], &gm, E, st);
-    if (int cr = dwt::tc_stats(x, bf16, nhwc, gm, gm.nchunks, w.shift, w.partial, st))
-      return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d) x=%p N=%lld C=%d HW=%d", cr, x, (long long)N, gm.C, gm.HW);
-  }
-  if (int rc = check_launch("instance whitening statistics kernel")) return rc;
-  {
-    Launch l(kIwName[1][k], &gm, 0.0, st);
-    if (gm.nchunks > 1) dwt::dense_partial_reduce(w.partial, gm.nchunks, dwt::tc_superblocks(gm) * gm.D, w.gram, st);
-    dwt::dense_fwd_instance(w.gram, w.shift, gm, fin, st);
-  }
-  if (int rc = check_launch("instance whitening finalize kernel")) return rc;
-  {
-    Launch l(kIwName[2][k], &gm, 2.0 * E, st);
-    if (int cr = dwt::tc_apply(x, y, bf16, nhwc, gm, tc_apply_ctas(gm, 1, 64), save_mean, save_w, st))
-      return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d)", cr);
-  }
-  return check_launch("instance whitening apply kernel");
-}
-
-int instance_bwd(const void* x, const void* dout, void* dx, int64_t N, int64_t C, int64_t HW, int GS, int flags, float eps,
-                 const float* save_mean, const float* save_w, void* ws, size_t ws_bytes, cudaStream_t st) {
-  dwt::Geom gm;
-  Workspace w;
-  if (int rc = inst_validate(gm, w, x, dout, dx, N, C, HW, GS, flags, save_mean, save_w, ws, ws_bytes)) return rc;
-  const bool nhwc = (flags & DWT_LAYOUT_NHWC) != 0, bf16 = (flags & DWT_DTYPE_BF16) != 0;
-  const int k = 2 * nhwc + bf16;
-  const double E = (bf16 ? 2.0 : 4.0) * (double)N * (double)C * (double)HW;
-  dwt::BwdFin fin{};
-  fin.a = 1.f - eps; fin.mode = DWT_MODE_TRAIN; fin.save_mean = save_mean; fin.save_w = save_w; fin.coef = w.coef;
-  {
-    Launch l(kIwName[3][k], &gm, 2.0 * E, st);
-    if (int cr = dwt::tc_bwd_reduce(x, dout, bf16, nhwc, gm, gm.nchunks, save_mean, w.partial, st))
-      return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d) x=%p dout=%p N=%lld C=%d HW=%d", cr, x, dout,
-                  (long long)N, gm.C, gm.HW);
-  }
-  if (int rc = check_launch("instance whitening backward reduction kernel")) return rc;
-  {
-    Launch l(kIwName[4][k], &gm, 0.0, st);
-    if (gm.nchunks > 1) dwt::dense_partial_reduce(w.partial, gm.nchunks, dwt::tc_superblocks(gm) * gm.D, w.gram, st);
-    dwt::dense_bwd_coef(w.gram, gm, fin, w.shift, st);                 // w.shift: mean_M dy per (image, channel)
-  }
-  if (int rc = check_launch("instance whitening backward finalize kernel")) return rc;
-  {
-    Launch l(kIwName[5][k], &gm, 3.0 * E, st);
-    if (int cr = dwt::tc_bwd_apply(x, dout, dx, bf16, nhwc, gm, tc_apply_ctas(gm, 1, 64), w.coef, save_mean, w.shift, st))
-      return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d)", cr);
-  }
-  return check_launch("instance whitening backward apply kernel");
-}
-
-// ---- switchable whitening (dwt_whiten_switch_fwd / dwt_whiten_switch_bwd) --------------------------------------------
-// Instance whitening's passes with the images as the domains (inst_geom), plus the batch moments and the mixture.
-// Forward: tc_stats (per-image moments) -> [partial_reduce] sw_stats (save_stats: per-image rows and the batch row by the
-// law of total covariance, no second pass over x) -> sw_fwd_factor (mix, Cholesky + inverse, EMA) -> tc_apply with the
-// per-image W and mixed mean.  Backward: tc_bwd_reduce about the mixed mean without the pilot centring (sum (x - m) is not
-// zero) -> [partial_reduce] sw_bwd_coef / sw_bwd_sum / sw_dmix / sw_bwd_apply_coef -> tc_bwd_apply, centred on the images'
-// own means, with the per-image constant of dx carried by dybar.
-constexpr const char* kSw = "switchable whitening";
-
-struct SwWork {
-  Workspace w;
-  float* pd;       // [N][G][gs*gs + gs]  P_n | dm_n
-  float* part;     // [N][G][8]           dmix terms per (image, group)
-  float* sums;     // [G][gs*gs + gs]     sum_n P_n | sum_n dm_n
-  float* mu;       // [N][C]              the images' own means (the backward apply's centre)
-};
-
-// Scratch behind the common head: instance whitening's (partials, reduced moments, shifts / dybar, coefficients), then
-// pd, part, sums and mu
-SwWork carve_switch(void* base, const dwt::Geom& gm) {
-  SwWork s{};
-  s.w = carve_instance(base, gm);
-  const size_t rec = (size_t)gm.GS * gm.GS + gm.GS, P = (size_t)gm.D * gm.G;
-  size_t off = s.w.bytes;
-  auto take = [&](size_t nbytes) { size_t o = off; off = align_up(off + nbytes, 256); return o; };
-  char* b = static_cast<char*>(base);
-  s.pd = reinterpret_cast<float*>(b + take(sizeof(float) * P * rec));
-  s.part = reinterpret_cast<float*>(b + take(sizeof(float) * P * 8));
-  s.sums = reinterpret_cast<float*>(b + take(sizeof(float) * gm.G * rec));
-  s.mu = reinterpret_cast<float*>(b + take(sizeof(float) * (size_t)gm.D * gm.C));
-  s.w.bytes = off;
   return s;
 }
 
-int sw_geom(dwt::Geom& gm, int64_t N, int64_t C, int64_t HW, int GS, int mode) {
-  if (mode & ~(DWT_MODE_EVAL | DWT_LAYOUT_NHWC | DWT_DTYPE_BF16))
-    return fail(DWT_E_INVALID, "bad mode %#x (DWT_MODE_TRAIN or DWT_MODE_EVAL | DWT_LAYOUT_NHWC | DWT_DTYPE_BF16)", mode);
-  return inst_geom(gm, N, C, HW, GS, mode & ~DWT_MODE_EVAL, kSw);
+// A size query leaves the last error text alone
+size_t image_workspace_bytes(int64_t N, int64_t C, int64_t HW, int GS, const Mix& m) {
+  dwt::Geom gm;
+  char saved[sizeof(g_err)];
+  memcpy(saved, g_err, sizeof(g_err));
+  const int rc = image_geom(gm, N, C, HW, GS, 0, m);
+  memcpy(g_err, saved, sizeof(g_err));
+  return rc ? 0 : carve_image(nullptr, gm, m).w.bytes;
 }
 
-// Profile family of a launch: [pass][channels-last * 2 + bf16]
-const char* const kSwName[6][4] = {
-    {"sw_stats", "sw_stats_bf16", "sw_stats_nhwc", "sw_stats_nhwc_bf16"},
-    {"sw_fwd_finalize", "sw_fwd_finalize_bf16", "sw_fwd_finalize", "sw_fwd_finalize_bf16"},
-    {"sw_apply", "sw_apply_bf16", "sw_apply_nhwc", "sw_apply_nhwc_bf16"},
-    {"sw_bwd_reduce", "sw_bwd_reduce_bf16", "sw_bwd_reduce_nhwc", "sw_bwd_reduce_nhwc_bf16"},
-    {"sw_bwd_finalize", "sw_bwd_finalize_bf16", "sw_bwd_finalize", "sw_bwd_finalize_bf16"},
-    {"sw_bwd_apply", "sw_bwd_apply_bf16", "sw_bwd_apply_nhwc", "sw_bwd_apply_nhwc_bf16"}};
+// Profile family of a launch: [switchable][pass][channels-last * 2 + bf16]
+enum ImagePass { I_STATS, I_FWD_FINALIZE, I_APPLY, I_BWD_REDUCE, I_BWD_FINALIZE, I_BWD_APPLY };
+const char* const kImageName[2][6][4] = {
+    {{"iw_stats", "iw_stats_bf16", "iw_stats_nhwc", "iw_stats_nhwc_bf16"},
+     {"iw_fwd_finalize", "iw_fwd_finalize_bf16", "iw_fwd_finalize", "iw_fwd_finalize_bf16"},
+     {"iw_apply", "iw_apply_bf16", "iw_apply_nhwc", "iw_apply_nhwc_bf16"},
+     {"iw_bwd_reduce", "iw_bwd_reduce_bf16", "iw_bwd_reduce_nhwc", "iw_bwd_reduce_nhwc_bf16"},
+     {"iw_bwd_finalize", "iw_bwd_finalize_bf16", "iw_bwd_finalize", "iw_bwd_finalize_bf16"},
+     {"iw_bwd_apply", "iw_bwd_apply_bf16", "iw_bwd_apply_nhwc", "iw_bwd_apply_nhwc_bf16"}},
+    {{"sw_stats", "sw_stats_bf16", "sw_stats_nhwc", "sw_stats_nhwc_bf16"},
+     {"sw_fwd_finalize", "sw_fwd_finalize_bf16", "sw_fwd_finalize", "sw_fwd_finalize_bf16"},
+     {"sw_apply", "sw_apply_bf16", "sw_apply_nhwc", "sw_apply_nhwc_bf16"},
+     {"sw_bwd_reduce", "sw_bwd_reduce_bf16", "sw_bwd_reduce_nhwc", "sw_bwd_reduce_nhwc_bf16"},
+     {"sw_bwd_finalize", "sw_bwd_finalize_bf16", "sw_bwd_finalize", "sw_bwd_finalize_bf16"},
+     {"sw_bwd_apply", "sw_bwd_apply_bf16", "sw_bwd_apply_nhwc", "sw_bwd_apply_nhwc_bf16"}}};
 
-// The checks both directions make, in order: mode and geometry, pointers, alignment, workspace, kernel set-up.
-// in0, in1: what the kernels read (x; x and dout); out: what they write (y; dx).
-int sw_validate(dwt::Geom& gm, SwWork& s, const void* in0, const void* in1, const void* out, int64_t N, int64_t C, int64_t HW,
-                int GS, int mode, const float* mix, const float* save_mean, const float* save_w, const float* save_stats,
-                void* ws, size_t ws_bytes, bool running_missing = false) {
-  if (int rc = sw_geom(gm, N, C, HW, GS, mode)) return rc;
-  if (!in0 || !in1 || !out || !mix || !save_mean || !save_w || !save_stats || !ws) return fail(DWT_E_INVALID, "null pointer argument");
+// The checks both directions make, in order: flags and geometry, pointers, running buffers (switchable forward),
+// alignment, workspace, kernel set-up.  in0, in1: what the kernels read (x; x and dout); out: what they write (y; dx).
+int image_validate(dwt::Geom& gm, ImageWork& s, const Mix& m, const void* in0, const void* in1, const void* out, int64_t N,
+                   int64_t C, int64_t HW, int GS, int flags, const float* save_mean, const float* save_w, void* ws,
+                   size_t ws_bytes, bool running_missing = false) {
+  if (int rc = image_geom(gm, N, C, HW, GS, flags, m)) return rc;
+  if (!in0 || !in1 || !out || !save_mean || !save_w || !ws || (m.on && (!m.mix || !m.save_stats)))
+    return fail(DWT_E_INVALID, "null pointer argument");
   if (running_missing) return fail(DWT_E_INVALID, "running buffer is null (eval, or train with update_running)");
-  if (((uintptr_t)in0 | (uintptr_t)in1 | (uintptr_t)out | (uintptr_t)save_w | (uintptr_t)save_stats | (uintptr_t)mix) % 16 != 0)
-    return fail(DWT_E_INVALID, "activation tensors, mix, save_w and save_stats must be 16-byte aligned (switchable whitening)");
-  s = carve_switch(ws, gm);
+  // instance whitening: mix and save_stats are null
+  if (((uintptr_t)in0 | (uintptr_t)in1 | (uintptr_t)out | (uintptr_t)save_w | (uintptr_t)m.save_stats | (uintptr_t)m.mix) % 16 != 0)
+    return m.on ? fail(DWT_E_INVALID, "activation tensors, mix, save_w and save_stats must be 16-byte aligned (switchable whitening)")
+                : fail(DWT_E_INVALID, "activation tensors and save_w must be 16-byte aligned (instance whitening: TMA and vector stores)");
+  s = carve_image(ws, gm, m);
   if (s.w.bytes > ws_bytes) return fail(DWT_E_WORKSPACE, "workspace too small: need %zu bytes, got %zu", s.w.bytes, ws_bytes);
   if ((uintptr_t)ws % 256 != 0) return fail(DWT_E_WORKSPACE, "workspace must be 256-byte aligned");
-  if (ensure_tc() != 0) return inst_refuse(N, C, HW, GS, mode & ~DWT_MODE_EVAL, kSw);   // the tensor-core kernels could not be set up
+  if (ensure_tc() != 0) return image_refuse(N, C, HW, GS, flags & ~DWT_MODE_EVAL, m.what());   // the tensor-core kernels could not be set up
   return DWT_OK;
 }
 
-dwt::SwFin make_sw_fin(int mode, float eps, const float* mix, float* save_mean, float* save_w, float* save_stats, int* status) {
+// The kernels only read save_mean, save_w and save_stats in the backward
+dwt::SwFin make_sw_fin(int mode, float eps, const Mix& m, const float* save_mean, const float* save_w, int* status) {
   dwt::SwFin f{};
-  f.a = 1.f - eps; f.b = eps; f.train = (mode & DWT_MODE_EVAL) == 0; f.mix = mix;
-  f.save_mean = save_mean; f.save_w = save_w; f.save_stats = save_stats; f.status = status;
+  f.a = 1.f - eps; f.b = eps; f.train = (mode & DWT_MODE_EVAL) == 0; f.mix = m.mix;
+  f.save_mean = const_cast<float*>(save_mean); f.save_w = const_cast<float*>(save_w);
+  f.save_stats = const_cast<float*>(m.save_stats); f.status = status;
   return f;
 }
 
-int switch_fwd(const void* x, void* y, int64_t N, int64_t C, int64_t HW, int GS, int mode, float eps, float momentum,
-               int update_running, float* running_mean, float* running_cov, const float* mix, float* save_mean, float* save_w,
-               float* save_stats, void* ws, size_t ws_bytes, cudaStream_t st) {
+int image_fwd(const Mix& m, const void* x, void* y, int64_t N, int64_t C, int64_t HW, int GS, int flags, float eps,
+              float* save_mean, float* save_w, void* ws, size_t ws_bytes, cudaStream_t st) {
   dwt::Geom gm;
-  SwWork s;
-  const bool train = (mode & DWT_MODE_EVAL) == 0;
-  const bool running_missing = (!train || update_running) && (!running_mean || !running_cov);
-  if (int rc = sw_validate(gm, s, x, x, y, N, C, HW, GS, mode, mix, save_mean, save_w, save_stats, ws, ws_bytes, running_missing))
+  ImageWork s;
+  const bool train = (flags & DWT_MODE_EVAL) == 0;
+  const bool running_missing = m.on && (!train || m.update_running) && (!m.rmean || !m.rcov);
+  if (int rc = image_validate(gm, s, m, x, x, y, N, C, HW, GS, flags, save_mean, save_w, ws, ws_bytes, running_missing))
     return rc;
-  const bool nhwc = (mode & DWT_LAYOUT_NHWC) != 0, bf16 = (mode & DWT_DTYPE_BF16) != 0;
+  const bool nhwc = (flags & DWT_LAYOUT_NHWC) != 0, bf16 = (flags & DWT_DTYPE_BF16) != 0;
   const int k = 2 * nhwc + bf16;
   const double E = (bf16 ? 2.0 : 4.0) * (double)N * (double)C * (double)HW;
-  dwt::SwFin fin = make_sw_fin(mode, eps, mix, save_mean, save_w, save_stats, s.w.status);
-  fin.momentum = momentum; fin.update_running = train && update_running;
-  fin.rmean = running_mean; fin.rcov = running_cov;
   {
-    Launch l(kSwName[0][k], &gm, E, st);
+    Launch l(kImageName[m.on][I_STATS][k], &gm, E, st);
     if (int cr = dwt::tc_stats(x, bf16, nhwc, gm, gm.nchunks, s.w.shift, s.w.partial, st))
       return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d) x=%p N=%lld C=%d HW=%d", cr, x, (long long)N, gm.C, gm.HW);
   }
-  if (int rc = check_launch("switchable whitening statistics kernel")) return rc;
+  if (int rc = check_launch("%s statistics kernel", m.what())) return rc;
   {
-    Launch l(kSwName[1][k], &gm, 0.0, st);
+    Launch l(kImageName[m.on][I_FWD_FINALIZE][k], &gm, 0.0, st);
     if (gm.nchunks > 1) dwt::dense_partial_reduce(s.w.partial, gm.nchunks, dwt::tc_superblocks(gm) * gm.D, s.w.gram, st);
-    dwt::dense_sw_stats(s.w.gram, s.w.shift, gm, fin, st);
-    dwt::dense_sw_fwd_factor(gm, fin, st);
+    if (m.on) {
+      dwt::SwFin fin = make_sw_fin(flags, eps, m, save_mean, save_w, s.w.status);
+      fin.momentum = m.momentum; fin.update_running = train && m.update_running;
+      fin.rmean = m.rmean; fin.rcov = m.rcov;
+      dwt::dense_sw_stats(s.w.gram, s.w.shift, gm, fin, st);
+      dwt::dense_sw_fwd_factor(gm, fin, st);
+    } else {
+      dwt::FwdFin fin{};
+      fin.a = 1.f - eps; fin.b = eps; fin.save_mean = save_mean; fin.save_w = save_w; fin.status = s.w.status;
+      dwt::dense_fwd_instance(s.w.gram, s.w.shift, gm, fin, st);
+    }
   }
-  if (int rc = check_launch("switchable whitening finalize kernel")) return rc;
+  if (int rc = check_launch("%s finalize kernel", m.what())) return rc;
   {
-    Launch l(kSwName[2][k], &gm, 2.0 * E, st);
+    Launch l(kImageName[m.on][I_APPLY][k], &gm, 2.0 * E, st);
     if (int cr = dwt::tc_apply(x, y, bf16, nhwc, gm, tc_apply_ctas(gm, 1, 64), save_mean, save_w, st))
       return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d)", cr);
   }
-  return check_launch("switchable whitening apply kernel");
+  return check_launch("%s apply kernel", m.what());
 }
 
-int switch_bwd(const void* x, const void* dout, void* dx, int64_t N, int64_t C, int64_t HW, int GS, int mode, float eps,
-               const float* mix, const float* save_mean, const float* save_w, const float* save_stats, float* dmix, void* ws,
-               size_t ws_bytes, cudaStream_t st) {
+int image_bwd(const Mix& m, const void* x, const void* dout, void* dx, int64_t N, int64_t C, int64_t HW, int GS, int flags,
+              float eps, const float* save_mean, const float* save_w, void* ws, size_t ws_bytes, cudaStream_t st) {
   dwt::Geom gm;
-  SwWork s;
-  if (int rc = sw_validate(gm, s, x, dout, dx, N, C, HW, GS, mode, mix, save_mean, save_w, save_stats, ws, ws_bytes)) return rc;
-  const bool nhwc = (mode & DWT_LAYOUT_NHWC) != 0, bf16 = (mode & DWT_DTYPE_BF16) != 0;
+  ImageWork s;
+  if (int rc = image_validate(gm, s, m, x, dout, dx, N, C, HW, GS, flags, save_mean, save_w, ws, ws_bytes)) return rc;
+  const bool nhwc = (flags & DWT_LAYOUT_NHWC) != 0, bf16 = (flags & DWT_DTYPE_BF16) != 0;
   const int k = 2 * nhwc + bf16;
   const double E = (bf16 ? 2.0 : 4.0) * (double)N * (double)C * (double)HW;
-  // the kernels only read save_mean, save_w and save_stats
-  const dwt::SwFin fin = make_sw_fin(mode, eps, mix, const_cast<float*>(save_mean), const_cast<float*>(save_w),
-                                     const_cast<float*>(save_stats), s.w.status);
   {
-    Launch l(kSwName[3][k], &gm, 2.0 * E, st);
-    if (int cr = dwt::tc_bwd_reduce(x, dout, bf16, nhwc, gm, gm.nchunks, save_mean, s.w.partial, st, /*pilot=*/false))
+    Launch l(kImageName[m.on][I_BWD_REDUCE][k], &gm, 2.0 * E, st);
+    if (int cr = dwt::tc_bwd_reduce(x, dout, bf16, nhwc, gm, gm.nchunks, save_mean, s.w.partial, st, /*pilot=*/!m.on))
       return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d) x=%p dout=%p N=%lld C=%d HW=%d", cr, x, dout,
                   (long long)N, gm.C, gm.HW);
   }
-  if (int rc = check_launch("switchable whitening backward reduction kernel")) return rc;
+  if (int rc = check_launch("%s backward reduction kernel", m.what())) return rc;
   {
-    Launch l(kSwName[4][k], &gm, 0.0, st);
+    Launch l(kImageName[m.on][I_BWD_FINALIZE][k], &gm, 0.0, st);
     if (gm.nchunks > 1) dwt::dense_partial_reduce(s.w.partial, gm.nchunks, dwt::tc_superblocks(gm) * gm.D, s.w.gram, st);
-    dwt::dense_sw_bwd(s.w.gram, gm, fin, s.pd, s.part, s.sums, dmix, s.w.coef, s.w.shift, s.mu, st);
+    if (m.on) {
+      const dwt::SwFin fin = make_sw_fin(flags, eps, m, save_mean, save_w, s.w.status);
+      dwt::dense_sw_bwd(s.w.gram, gm, fin, s.pd, s.part, s.sums, m.dmix, s.w.coef, s.w.shift, s.mu, st);
+    } else {
+      dwt::BwdFin fin{};
+      fin.a = 1.f - eps; fin.mode = DWT_MODE_TRAIN; fin.save_mean = save_mean; fin.save_w = save_w; fin.coef = s.w.coef;
+      dwt::dense_bwd_coef(s.w.gram, gm, fin, s.w.shift, st);           // s.w.shift: mean_M dy per (image, channel)
+    }
   }
-  if (int rc = check_launch("switchable whitening backward finalize kernel")) return rc;
+  if (int rc = check_launch("%s backward finalize kernel", m.what())) return rc;
   {
-    Launch l(kSwName[5][k], &gm, 3.0 * E, st);
-    if (int cr = dwt::tc_bwd_apply(x, dout, dx, bf16, nhwc, gm, tc_apply_ctas(gm, 1, 64), s.w.coef, s.mu, s.w.shift, st))
+    Launch l(kImageName[m.on][I_BWD_APPLY][k], &gm, 3.0 * E, st);
+    if (int cr = dwt::tc_bwd_apply(x, dout, dx, bf16, nhwc, gm, tc_apply_ctas(gm, 1, 64), s.w.coef, m.on ? s.mu : save_mean,
+                                   s.w.shift, st))
       return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d)", cr);
   }
-  return check_launch("switchable whitening backward apply kernel");
+  return check_launch("%s backward apply kernel", m.what());
 }
 
 }  // namespace
@@ -1116,48 +1066,45 @@ extern "C" {
 int dwt_abi_version(void) { return DWT_B200_ABI_VERSION; }
 
 size_t dwt_instance_workspace_bytes(int64_t N, int64_t C, int64_t HW, int group_size) {
-  dwt::Geom gm;
-  char saved[sizeof(g_err)];
-  memcpy(saved, g_err, sizeof(g_err));            // a size query leaves the last error text alone
-  const int rc = inst_geom(gm, N, C, HW, group_size, 0);
-  memcpy(g_err, saved, sizeof(g_err));
-  return rc ? 0 : carve_instance(nullptr, gm).bytes;
+  return image_workspace_bytes(N, C, HW, group_size, Mix{});
 }
 
 int dwt_whiten_instance_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, int group_size, int flags, float eps,
                             float* save_mean, float* save_w, void* workspace, size_t workspace_bytes, dwt_stream_t stream) {
-  return instance_fwd(x, y, N, C, HW, group_size, flags, eps, save_mean, save_w, workspace, workspace_bytes, (cudaStream_t)stream);
+  return image_fwd(Mix{}, x, y, N, C, HW, group_size, flags, eps, save_mean, save_w, workspace, workspace_bytes,
+                   (cudaStream_t)stream);
+}
+
+int dwt_whiten_instance_bwd(const float* x, const float* dout, float* dx, int64_t N, int64_t C, int64_t HW, int group_size,
+                            int flags, float eps, const float* save_mean, const float* save_w, void* workspace,
+                            size_t workspace_bytes, dwt_stream_t stream) {
+  return image_bwd(Mix{}, x, dout, dx, N, C, HW, group_size, flags, eps, save_mean, save_w, workspace, workspace_bytes,
+                   (cudaStream_t)stream);
 }
 
 size_t dwt_switch_workspace_bytes(int64_t N, int64_t C, int64_t HW, int group_size) {
-  dwt::Geom gm;
-  char saved[sizeof(g_err)];
-  memcpy(saved, g_err, sizeof(g_err));            // a size query leaves the last error text alone
-  const int rc = sw_geom(gm, N, C, HW, group_size, 0);
-  memcpy(g_err, saved, sizeof(g_err));
-  return rc ? 0 : carve_switch(nullptr, gm).w.bytes;
+  Mix m;
+  m.on = true;
+  return image_workspace_bytes(N, C, HW, group_size, m);
 }
 
 int dwt_whiten_switch_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, int group_size, int mode, float eps,
                           float momentum, int update_running, float* running_mean, float* running_cov, const float* mix,
                           float* save_mean, float* save_w, float* save_stats, void* workspace, size_t workspace_bytes,
                           dwt_stream_t stream) {
-  return switch_fwd(x, y, N, C, HW, group_size, mode, eps, momentum, update_running, running_mean, running_cov, mix, save_mean,
-                    save_w, save_stats, workspace, workspace_bytes, (cudaStream_t)stream);
+  Mix m;
+  m.on = true; m.mix = mix; m.save_stats = save_stats;
+  m.momentum = momentum; m.update_running = update_running; m.rmean = running_mean; m.rcov = running_cov;
+  return image_fwd(m, x, y, N, C, HW, group_size, mode, eps, save_mean, save_w, workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 int dwt_whiten_switch_bwd(const float* x, const float* dout, float* dx, int64_t N, int64_t C, int64_t HW, int group_size,
                           int mode, float eps, const float* mix, const float* save_mean, const float* save_w,
                           const float* save_stats, float* dmix, void* workspace, size_t workspace_bytes, dwt_stream_t stream) {
-  return switch_bwd(x, dout, dx, N, C, HW, group_size, mode, eps, mix, save_mean, save_w, save_stats, dmix, workspace,
-                    workspace_bytes, (cudaStream_t)stream);
-}
-
-int dwt_whiten_instance_bwd(const float* x, const float* dout, float* dx, int64_t N, int64_t C, int64_t HW, int group_size,
-                            int flags, float eps, const float* save_mean, const float* save_w, void* workspace,
-                            size_t workspace_bytes, dwt_stream_t stream) {
-  return instance_bwd(x, dout, dx, N, C, HW, group_size, flags, eps, save_mean, save_w, workspace, workspace_bytes,
-                      (cudaStream_t)stream);
+  Mix m;
+  m.on = true; m.mix = mix; m.save_stats = save_stats; m.dmix = dmix;
+  return image_bwd(m, x, dout, dx, N, C, HW, group_size, mode, eps, save_mean, save_w, workspace, workspace_bytes,
+                   (cudaStream_t)stream);
 }
 
 const char* dwt_last_error(void) { return g_err; }

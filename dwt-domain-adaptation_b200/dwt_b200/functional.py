@@ -92,19 +92,89 @@ def _check_param(name, t, numel):
         raise ValueError(f"{name} must be contiguous (it is written / read through a raw pointer)")
 
 
+def _check_running(running, c, gs, domains=True):
+    """_check_param of (mean, second-moment) running buffer pairs: C and C*gs elements.  domains: name the domain."""
+    for d, (rm_t, rv_t) in enumerate(running):
+        at = f" of domain {d}" if domains else ""
+        _check_param(f"running mean{at}", rm_t, c)
+        _check_param(f"running second moment{at}", rv_t, c * gs)
+
+
+def _bump_versions(running):
+    """The kernels wrote the running buffers in place behind autograd's back: bump their version counters (each buffer
+    once) so a graph that saved one of them notices (the reference's in-place EMA, whitening.py:58-59, does the same)."""
+    seen = set()
+    for buf in (t for pair in running for t in pair):
+        if buf is not None and id(buf) not in seen:
+            seen.add(id(buf))
+            torch.autograd.graph.increment_version(buf)
+
+
+def _prepare_dout(ctx, dout, x, fmt, align=0, cl=False):
+    """The incoming gradient as the kernels read it -> (dout, dout2): dout in x's dtype, dense in memory format fmt, its
+    data_ptr() a multiple of align (0: any; a misaligned one is copied).  dout2 is the second addend fork_for_sum parked
+    on ctx's node (see there): the channels-last kernels of group sizes 1, 2, 4 (cl) add it where they read dout when it
+    matches dout; any other path adds it now."""
+    dout2 = ctx.__dict__.pop("_dwt_extra_grad", None)
+    if dout.dtype != x.dtype:
+        dout = dout.to(x.dtype)
+    if dout2 is not None and not (cl and dout2.shape == dout.shape and dout2.dtype == dout.dtype
+                                  and dout2.is_contiguous(memory_format=torch.channels_last)):
+        dout, dout2 = dout + dout2, None
+    dout = dout.contiguous(memory_format=fmt)
+    if align and dout.data_ptr() % align:        # a fresh tensor keeps the layout
+        dout = dout.clone(memory_format=fmt)
+    return dout, dout2
+
+
+def _fwd_entry(lib, kind, basis, head, epilogue, stats, save_p, tail):
+    """Call the forward entry point of a norm call in `basis`.  head: (x, y, N, C, HW, gs, n_domains, mode, eps, momentum,
+    update_running, running means, running second moments); epilogue: (gamma, beta, residual, ReLU byte map, epilogue
+    bits), the colouring matrix and bias in the colour basis; stats: (save_mean, save_w); tail: (workspace, bytes, stream)."""
+    if basis == nv.EIGH:
+        return lib.dwt_whiten_eigh_fwd(*head, *stats, save_p, *tail)
+    if basis == nv.COLOR:
+        return lib.dwt_whiten_color_fwd(*head, *epilogue[:2], *stats, *tail)
+    if basis:
+        return lib.dwt_whiten_zca_fwd(*head, int(basis), *stats, save_p, *tail)
+    if kind == "whiten":
+        return lib.dwt_whiten_fwd(*head, *epilogue, *stats, *tail)
+    return lib.dwt_bn_fwd(*head[:5], *head[6:], *epilogue, *stats, *tail)         # batch norm: no group_size argument
+
+
+def _bwd_entry(lib, kind, basis, io, dout2, geom, stats, epilogue, grads, save_p, tail):
+    """Call the backward entry point of a norm call in `basis`.  io: (x, dout, dx); dout2: the second gradient addend;
+    geom: (N, C, HW, gs, n_domains, mode, eps); stats: (save_mean, save_w); epilogue: (gamma, beta, ReLU byte map,
+    dresidual, epilogue bits), the colouring matrix in the colour basis; grads: (dgamma, dbeta), (dcolor, dbias) in the
+    colour basis; tail: (workspace, bytes, stream)."""
+    if basis == nv.EIGH:
+        return lib.dwt_whiten_eigh_bwd(*io, *geom, *stats, save_p, *tail)
+    if basis == nv.COLOR:
+        return lib.dwt_whiten_color_bwd(*io, *geom, *stats, epilogue[0], *grads, *tail)
+    if basis:
+        return lib.dwt_whiten_zca_bwd(*io, *geom, int(basis), *stats, save_p, *tail)
+    x, dout, dx = io
+    if kind == "whiten":
+        return lib.dwt_whiten_bwd(x, dout, dout2, dx, *geom, *stats, *epilogue, *grads, *tail)
+    n, c, hw, _, n_domains, mode, _ = geom                                        # batch norm: no group_size or eps
+    return lib.dwt_bn_bwd(x, dout, dout2, dx, n, c, hw, n_domains, mode, *stats, *epilogue, *grads, *tail)
+
+
 class _NormFunction(torch.autograd.Function):
     """Shared by whitening (kind='whiten') and domain batch norm (kind='bn').
 
     x is [n_domains*N, C, *]; `running` is a list of n_domains (mean, second-moment) buffer pairs
     (entries may alias); gamma/beta are [C]-sized or None; relu fuses max(.,0) behind the affine; r: route() of the call;
-    iterations: 0 for the Cholesky basis, else the Newton-Schulz iterations of the ZCA basis (dwt_whiten_zca_*, whitening
-    without gamma/beta or residual; the per-group matrices of the iteration are saved for backward), or nv.EIGH for the
-    exact ZCA basis (dwt_whiten_eigh_*; the per-group eigenvectors and eigenvalues are saved for backward).
+    basis: 0 for the Cholesky basis; 1..16, the Newton-Schulz iterations of the ZCA basis (dwt_whiten_zca_*, whitening
+    without gamma/beta or residual; the per-group matrices of the iteration are saved for backward); nv.EIGH for the exact
+    ZCA basis (dwt_whiten_eigh_*; the per-group eigenvectors and eigenvalues are saved for backward); or nv.COLOR for the
+    Cholesky basis coloured, y = gamma_g W (x - mean) + beta (dwt_whiten_color_*: gamma is the colouring matrix
+    [C/gs, gs, gs] and beta the bias with C elements, both float32 and shared by the n_domains domains of x).
     """
 
     @staticmethod
     def forward(ctx, x, gamma, beta, residual, kind, group_size, n_domains, mode, eps, momentum, update_running,
-                running, relu, r, iterations):
+                running, relu, r, basis):
         lib = nv.lib()
         gs = group_size if kind == "whiten" else 1
         if not r.nhwc and not x.is_contiguous():
@@ -117,68 +187,50 @@ class _NormFunction(torch.autograd.Function):
         stats = [gamma, beta, *[t for pair in running for t in pair]]
         dev = nv.require_cuda(x, residual, *stats, bf16=True)
         nv.require_cuda(*stats)                      # parameters and running buffers are float32 whatever x is
-        for d, (rm_t, rv_t) in enumerate(running):
-            _check_param(f"running mean of domain {d}", rm_t, c)
-            _check_param(f"running second moment of domain {d}", rv_t, c * gs)
-        _check_param("gamma / weight", gamma, c)
-        _check_param("beta / bias", beta, c)
-        if iterations and (kind != "whiten" or gamma is not None or residual is not None):
-            raise nv.NativeError("the ZCA basis whitens without a fused gamma/beta/ReLU epilogue or residual")
+        _check_running(running, c, gs)
         epi = nv.EPI_NONE
-        if residual is not None:
-            if gamma is None or not relu or residual.shape != x.shape:
-                raise ValueError("a fused residual needs gamma/beta, relu=True and a tensor shaped like x")
-            residual = residual.contiguous(memory_format=torch.channels_last) if r.nhwc else residual.contiguous()
-        if gamma is not None:
-            epi = nv.EPI_AFFINE | (nv.EPI_RELU if relu else 0) | (nv.EPI_RESIDUAL if residual is not None else 0)
-            gamma_c, beta_c = gamma.detach().reshape(-1).contiguous(), beta.detach().reshape(-1).contiguous()
+        if basis == nv.COLOR:
+            gamma_c, beta_c = _aligned(gamma), _aligned(beta)
+            _check_param("color / weight", gamma_c, c * gs)
+            _check_param("bias", beta_c, c)
         else:
-            gamma_c = beta_c = None
+            _check_param("gamma / weight", gamma, c)
+            _check_param("beta / bias", beta, c)
+            if basis and (kind != "whiten" or gamma is not None or residual is not None):
+                raise nv.NativeError("the ZCA basis whitens without a fused gamma/beta/ReLU epilogue or residual")
+            if residual is not None:
+                if gamma is None or not relu or residual.shape != x.shape:
+                    raise ValueError("a fused residual needs gamma/beta, relu=True and a tensor shaped like x")
+                residual = residual.contiguous(memory_format=torch.channels_last) if r.nhwc else residual.contiguous()
+            if gamma is not None:
+                epi = nv.EPI_AFFINE | (nv.EPI_RELU if relu else 0) | (nv.EPI_RESIDUAL if residual is not None else 0)
+                gamma_c, beta_c = gamma.detach().reshape(-1).contiguous(), beta.detach().reshape(-1).contiguous()
+            else:
+                gamma_c = beta_c = None
         y = torch.empty_like(x)                      # keeps x's memory format
         # residual tail on the channels-last kernels: the apply pass leaves one byte per float4 with the four
         # (out > 0) bits, which is all the backward needs of the output
         mask = torch.empty(x.numel() // 4, dtype=torch.uint8, device=dev) if (residual is not None and r.nhwc) else None
         save_mean = torch.empty(n_domains, c, dtype=torch.float32, device=dev)
         save_w = torch.empty(n_domains, c // gs, gs, gs, dtype=torch.float32, device=dev)
-        exact = iterations == nv.EIGH
-        if exact:                                    # save_e: U, then the eigenvalues
+        if basis == nv.EIGH:                         # save_e: U, then the eigenvalues
             save_p = torch.empty(n_domains, c // gs, gs + 1, gs, dtype=torch.float32, device=dev)
+        elif basis and basis != nv.COLOR:
+            save_p = torch.empty(n_domains, c // gs, basis, gs, gs, dtype=torch.float32, device=dev)
         else:
-            save_p = torch.empty(n_domains, c // gs, iterations, gs, gs, dtype=torch.float32, device=dev) if iterations else None
+            save_p = None
         ws = nv.workspace(dev, n, c, hw, gs, n_domains)
         need_running = (mode == nv.MODE_EVAL) or update_running
         rm = nv.ptr_array([p[0] for p in running]) if need_running else None
         rv = nv.ptr_array([p[1] for p in running]) if need_running else None
+        head = (nv.ptr(x), nv.ptr(y), n, c, hw, gs, n_domains, mode | layout, eps, momentum, int(update_running), rm, rv)
         with torch.cuda.device(dev):
-            if exact:
-                rc = lib.dwt_whiten_eigh_fwd(nv.ptr(x), nv.ptr(y), n, c, hw, gs, n_domains, mode | layout, eps, momentum,
-                                             int(update_running), rm, rv, nv.ptr(save_mean), nv.ptr(save_w), nv.ptr(save_p),
-                                             nv.ptr(ws), ws.numel(), nv.stream_ptr(dev))
-            elif iterations:
-                rc = lib.dwt_whiten_zca_fwd(nv.ptr(x), nv.ptr(y), n, c, hw, gs, n_domains, mode | layout, eps, momentum,
-                                            int(update_running), rm, rv, int(iterations), nv.ptr(save_mean), nv.ptr(save_w),
-                                            nv.ptr(save_p), nv.ptr(ws), ws.numel(), nv.stream_ptr(dev))
-            elif kind == "whiten":
-                rc = lib.dwt_whiten_fwd(nv.ptr(x), nv.ptr(y), n, c, hw, gs, n_domains, mode | layout, eps, momentum,
-                                        int(update_running), rm, rv, nv.ptr(gamma_c), nv.ptr(beta_c), nv.ptr(residual),
-                                        nv.ptr(mask), epi, nv.ptr(save_mean), nv.ptr(save_w), nv.ptr(ws), ws.numel(),
-                                        nv.stream_ptr(dev))
-            else:
-                rc = lib.dwt_bn_fwd(nv.ptr(x), nv.ptr(y), n, c, hw, n_domains, mode | layout, eps, momentum,
-                                    int(update_running), rm, rv, nv.ptr(gamma_c), nv.ptr(beta_c), nv.ptr(residual),
-                                    nv.ptr(mask), epi, nv.ptr(save_mean), nv.ptr(save_w), nv.ptr(ws), ws.numel(),
-                                    nv.stream_ptr(dev))
+            rc = _fwd_entry(lib, kind, basis, head, (nv.ptr(gamma_c), nv.ptr(beta_c), nv.ptr(residual), nv.ptr(mask), epi),
+                            (nv.ptr(save_mean), nv.ptr(save_w)), nv.ptr(save_p), (nv.ptr(ws), ws.numel(), nv.stream_ptr(dev)))
         nv.check(rc)
         nv.poll_status(dev)
         if update_running and mode == nv.MODE_TRAIN:
-            # the kernels wrote the running buffers in place behind autograd's back: bump their version counters so a
-            # graph that saved one of them notices (the reference's in-place EMA, whitening.py:58-59, does the same)
-            seen = set()
-            for pair in running:
-                for buf in pair:
-                    if buf is not None and id(buf) not in seen:
-                        seen.add(id(buf))
-                        torch.autograd.graph.increment_version(buf)
+            _bump_versions(running)
         # backward of relu(z + residual): dz = dout * (out > 0) is also the residual's gradient
         ctx.residual_mode = None
         if mask is not None:
@@ -190,44 +242,33 @@ class _NormFunction(torch.autograd.Function):
             ctx.save_for_backward(x, save_mean, save_w, gamma_c, beta_c, y)
             epi = nv.EPI_AFFINE
             ctx.residual_mode = "aten"
-        elif iterations:
+        elif save_p is not None:
             ctx.save_for_backward(x, save_mean, save_w, gamma_c, beta_c, save_p)
         else:
             ctx.save_for_backward(x, save_mean, save_w, gamma_c, beta_c)
-        ctx.iterations = iterations
-        ctx.cfg = (kind, gs, n_domains, mode | layout, eps, epi, n, c, hw, None if gamma is None else gamma.shape)
+        ctx.basis = basis
+        ctx.cfg = (kind, gs, n_domains, mode | layout, eps, epi, n, c, hw,
+                   None if gamma is None else (gamma.shape, beta.shape))
         ctx.route = r
         return y
 
     @staticmethod
     def backward(ctx, dout):
         lib = nv.lib()
+        x, save_mean, save_w, gamma_c, beta_c, *extra = ctx.saved_tensors
         mask = save_p = None
-        if ctx.iterations:
-            x, save_mean, save_w, gamma_c, beta_c, save_p = ctx.saved_tensors
-        elif ctx.residual_mode == "mask":
-            x, save_mean, save_w, gamma_c, beta_c, mask = ctx.saved_tensors
+        if ctx.residual_mode == "mask":
+            mask = extra[0]
         elif ctx.residual_mode == "aten":
-            x, save_mean, save_w, gamma_c, beta_c, out = ctx.saved_tensors
-            extra = ctx.__dict__.pop("_dwt_extra_grad", None)
-            if extra is not None:
-                dout = dout + extra
-            dout = torch.ops.aten.threshold_backward(dout, out, 0)
-        else:
-            x, save_mean, save_w, gamma_c, beta_c = ctx.saved_tensors
-        kind, gs, n_domains, mode, eps, epi, n, c, hw, gshape = ctx.cfg
+            dout2 = ctx.__dict__.pop("_dwt_extra_grad", None)
+            if dout2 is not None:
+                dout = dout + dout2
+            dout = torch.ops.aten.threshold_backward(dout, extra[0], 0)
+        elif extra:
+            save_p = extra[0]
+        kind, gs, n_domains, mode, eps, epi, n, c, hw, shapes = ctx.cfg
         r = ctx.route
-        # second addend of the incoming gradient, left here by fork_for_sum's backward (see there): the channels-last
-        # kernels of group sizes 1, 2, 4 add it where they read dout; any other path adds it now
-        dout2 = ctx.__dict__.pop("_dwt_extra_grad", None)
-        if dout.dtype != x.dtype:
-            dout = dout.to(x.dtype)
-        if dout2 is not None and not (r.cl and dout2.shape == dout.shape and dout2.dtype == dout.dtype
-                                      and dout2.is_contiguous(memory_format=torch.channels_last)):
-            dout, dout2 = dout + dout2, None
-        dout = dout.contiguous(memory_format=torch.channels_last) if r.nhwc else dout.contiguous()
-        if r.align and dout.data_ptr() % r.align:    # a fresh tensor keeps the layout
-            dout = dout.clone(memory_format=torch.channels_last if r.nhwc else torch.contiguous_format)
+        dout, dout2 = _prepare_dout(ctx, dout, x, torch.channels_last if r.nhwc else torch.contiguous_format, r.align, r.cl)
         dev = nv.require_cuda(dout, bf16=True)
         dx = torch.empty_like(x)                     # x's layout: channels-last when the forward ran NHWC
         want_affine = gamma_c is not None and (ctx.needs_input_grad[1] or ctx.needs_input_grad[2])
@@ -236,31 +277,17 @@ class _NormFunction(torch.autograd.Function):
             d_res = torch.empty_like(x)              # dz, written even when the residual needs no gradient
         elif ctx.residual_mode == "aten" and ctx.needs_input_grad[3]:
             d_res = dout
-        dgamma = torch.empty(c, dtype=torch.float32, device=dev) if want_affine else None
-        dbeta = torch.empty(c, dtype=torch.float32, device=dev) if want_affine else None
+        dgamma = torch.empty_like(gamma_c) if want_affine else None
+        dbeta = torch.empty_like(beta_c) if want_affine else None
         ws = nv.workspace(dev, n, c, hw, gs, n_domains)
         with torch.cuda.device(dev):
-            if ctx.iterations == nv.EIGH:
-                rc = lib.dwt_whiten_eigh_bwd(nv.ptr(x), nv.ptr(dout), nv.ptr(dx), n, c, hw, gs, n_domains, mode, eps,
-                                             nv.ptr(save_mean), nv.ptr(save_w), nv.ptr(save_p), nv.ptr(ws), ws.numel(),
-                                             nv.stream_ptr(dev))
-            elif ctx.iterations:
-                rc = lib.dwt_whiten_zca_bwd(nv.ptr(x), nv.ptr(dout), nv.ptr(dx), n, c, hw, gs, n_domains, mode, eps,
-                                            int(ctx.iterations), nv.ptr(save_mean), nv.ptr(save_w), nv.ptr(save_p),
-                                            nv.ptr(ws), ws.numel(), nv.stream_ptr(dev))
-            elif kind == "whiten":
-                rc = lib.dwt_whiten_bwd(nv.ptr(x), nv.ptr(dout), nv.ptr(dout2), nv.ptr(dx), n, c, hw, gs, n_domains, mode, eps,
-                                        nv.ptr(save_mean), nv.ptr(save_w), nv.ptr(gamma_c), nv.ptr(beta_c), nv.ptr(mask),
-                                        nv.ptr(d_res) if mask is not None else None, epi,
-                                        nv.ptr(dgamma), nv.ptr(dbeta), nv.ptr(ws), ws.numel(), nv.stream_ptr(dev))
-            else:
-                rc = lib.dwt_bn_bwd(nv.ptr(x), nv.ptr(dout), nv.ptr(dout2), nv.ptr(dx), n, c, hw, n_domains, mode,
-                                    nv.ptr(save_mean), nv.ptr(save_w), nv.ptr(gamma_c), nv.ptr(beta_c), nv.ptr(mask),
-                                    nv.ptr(d_res) if mask is not None else None, epi,
-                                    nv.ptr(dgamma), nv.ptr(dbeta), nv.ptr(ws), ws.numel(), nv.stream_ptr(dev))
+            rc = _bwd_entry(lib, kind, ctx.basis, (nv.ptr(x), nv.ptr(dout), nv.ptr(dx)), nv.ptr(dout2),
+                            (n, c, hw, gs, n_domains, mode, eps), (nv.ptr(save_mean), nv.ptr(save_w)),
+                            (nv.ptr(gamma_c), nv.ptr(beta_c), nv.ptr(mask), nv.ptr(d_res) if mask is not None else None, epi),
+                            (nv.ptr(dgamma), nv.ptr(dbeta)), nv.ptr(save_p), (nv.ptr(ws), ws.numel(), nv.stream_ptr(dev)))
         nv.check(rc)
         if want_affine:
-            dgamma, dbeta = dgamma.view(gshape), dbeta.view(gshape)
+            dgamma, dbeta = dgamma.view(shapes[0]), dbeta.view(shapes[1])
         return (dx, dgamma, dbeta, d_res if ctx.needs_input_grad[3] else None) + (None,) * 11
 
 
@@ -292,9 +319,7 @@ class _TailPairFunction(torch.autograd.Function):
         keep = []                                    # save tensors and pointer arrays alive across the call
         saved = []
         for k, (inp, (g, b), (running, eps, momentum, update)) in enumerate(zip((x, xd), params, sites)):
-            for d, (rm_t, rv_t) in enumerate(running):
-                _check_param(f"running mean of domain {d}", rm_t, c)
-                _check_param(f"running second moment of domain {d}", rv_t, c * gs)
+            _check_running(running, c, gs)
             _check_param("gamma / weight", g, c)
             _check_param("beta / bias", b, c)
             g_c, b_c = g.detach().reshape(-1).contiguous(), b.detach().reshape(-1).contiguous()
@@ -315,12 +340,7 @@ class _TailPairFunction(torch.autograd.Function):
                                    nv.stream_ptr(dev))
         nv.check(rc)
         nv.poll_status(dev)
-        seen = set()
-        for running, _, _, update in sites:
-            for buf in (t for pair in running for t in pair) if update else ():
-                if id(buf) not in seen:              # see _NormFunction.forward
-                    seen.add(id(buf))
-                    torch.autograd.graph.increment_version(buf)
+        _bump_versions([pair for running, _, _, update in sites if update for pair in running])
         ctx.save_for_backward(x, xd, mask, *saved)
         ctx.cfg = (nv_kind, gs, n_domains, n, c, hw, [s[1] for s in sites], gamma.shape, gamma_d.shape)
         return y
@@ -330,13 +350,7 @@ class _TailPairFunction(torch.autograd.Function):
         lib = nv.lib()
         x, xd, mask, mean0, w0, g0, mean1, w1, g1 = ctx.saved_tensors
         nv_kind, gs, n_domains, n, c, hw, eps, gshape, gshape_d = ctx.cfg
-        dout2 = ctx.__dict__.pop("_dwt_extra_grad", None)      # parked by fork_for_sum, as for _NormFunction
-        if dout.dtype != x.dtype:
-            dout = dout.to(x.dtype)
-        if dout2 is not None and not (dout2.shape == dout.shape and dout2.dtype == dout.dtype
-                                      and dout2.is_contiguous(memory_format=torch.channels_last)):
-            dout, dout2 = dout + dout2, None
-        dout = dout.contiguous(memory_format=torch.channels_last)
+        dout, dout2 = _prepare_dout(ctx, dout, x, torch.channels_last, cl=True)
         dev = nv.require_cuda(dout, bf16=True)
         dz = torch.empty_like(x)
         dx, dxd = torch.empty_like(x), torch.empty_like(xd)
@@ -404,6 +418,13 @@ def norm(x, gamma, beta, *, kind, group_size, n_domains, training_stats, eps, mo
     they cannot take raises NativeError, it is never sent to another family or basis)."""
     if iterations != nv.EIGH and iterations and not 1 <= iterations <= nv.ZCA_MAX_ITERATIONS:
         raise ValueError(f"iterations must be in [1, {nv.ZCA_MAX_ITERATIONS}] (got {iterations})")
+    return _norm(x, gamma, beta, residual, kind, group_size, n_domains, training_stats, eps, momentum, update_running,
+                 running, relu, iterations)
+
+
+def _norm(x, gamma, beta, residual, kind, group_size, n_domains, training_stats, eps, momentum, update_running, running,
+          relu, basis):
+    """A _NormFunction call in `basis` on x as route() takes it."""
     mode = nv.MODE_TRAIN if training_stats else nv.MODE_EVAL
     args = (kind, group_size, n_domains, mode, float(eps), float(momentum), bool(update_running), running, bool(relu))
     r = route(x, residual, kind, group_size, n_domains)
@@ -412,9 +433,9 @@ def norm(x, gamma, beta, *, kind, group_size, n_domains, training_stats, eps, mo
         # view, ...) or mixed dtypes: the float32 kernels on upcast copies (x.float() keeps channels-last strides), the
         # result (and through autograd every gradient of x and the residual) back in x's dtype
         xf, rf = x.float(), None if residual is None else residual.float()
-        y = _NormFunction.apply(xf, gamma, beta, rf, *args, route(xf, rf, kind, group_size, n_domains), iterations)
+        y = _NormFunction.apply(xf, gamma, beta, rf, *args, route(xf, rf, kind, group_size, n_domains), basis)
         return y.to(x.dtype)
-    return _NormFunction.apply(x, gamma, beta, residual, *args, r, iterations)
+    return _NormFunction.apply(x, gamma, beta, residual, *args, r, basis)
 
 
 def _aligned(t):
@@ -423,96 +444,29 @@ def _aligned(t):
     return t if t.data_ptr() % 16 == 0 else t.clone()
 
 
-class _ColorFunction(torch.autograd.Function):
-    """y = color_g W (x - mean) + bias (dwt_whiten_color_fwd / _bwd): whitening in the Cholesky basis followed by a
-    learnable per-group colouring matrix color [C/gs, gs, gs] and bias [C], both float32 and shared by the n_domains
-    domains of x.  Statistics, running buffers and the route r as in _NormFunction."""
-
-    @staticmethod
-    def forward(ctx, x, color, bias, group_size, n_domains, mode, eps, momentum, update_running, running, r):
-        lib = nv.lib()
-        gs = group_size
-        if not r.nhwc and not x.is_contiguous():
-            x = x.contiguous()
-        n_all, c, hw = x.shape[0], x.shape[1], math.prod(x.shape[2:])
-        layout = (nv.LAYOUT_NHWC if r.nhwc else 0) | (nv.DTYPE_BF16 if r.bf16 else 0)
-        if n_all % n_domains != 0:
-            raise ValueError(f"batch of {n_all} does not split into {n_domains} domains")
-        n = n_all // n_domains
-        stats = [color, bias, *[t for pair in running for t in pair]]
-        dev = nv.require_cuda(x, *stats, bf16=True)
-        nv.require_cuda(*stats)
-        for d, (rm_t, rv_t) in enumerate(running):
-            _check_param(f"running mean of domain {d}", rm_t, c)
-            _check_param(f"running second moment of domain {d}", rv_t, c * gs)
-        color_c, bias_c = _aligned(color), _aligned(bias)
-        _check_param("color / weight", color_c, c * gs)
-        _check_param("bias", bias_c, c)
-        y = torch.empty_like(x)
-        save_mean = torch.empty(n_domains, c, dtype=torch.float32, device=dev)
-        save_w = torch.empty(n_domains, c // gs, gs, gs, dtype=torch.float32, device=dev)
-        ws = nv.workspace(dev, n, c, hw, gs, n_domains)
-        need_running = (mode == nv.MODE_EVAL) or update_running
-        rm = nv.ptr_array([p[0] for p in running]) if need_running else None
-        rv = nv.ptr_array([p[1] for p in running]) if need_running else None
-        with torch.cuda.device(dev):
-            rc = lib.dwt_whiten_color_fwd(nv.ptr(x), nv.ptr(y), n, c, hw, gs, n_domains, mode | layout, eps, momentum,
-                                          int(update_running), rm, rv, nv.ptr(color_c), nv.ptr(bias_c), nv.ptr(save_mean),
-                                          nv.ptr(save_w), nv.ptr(ws), ws.numel(), nv.stream_ptr(dev))
-        nv.check(rc)
-        nv.poll_status(dev)
-        if update_running and mode == nv.MODE_TRAIN:
-            seen = set()                             # see _NormFunction.forward
-            for pair in running:
-                for buf in pair:
-                    if buf is not None and id(buf) not in seen:
-                        seen.add(id(buf))
-                        torch.autograd.graph.increment_version(buf)
-        ctx.save_for_backward(x, save_mean, save_w, color_c)
-        ctx.cfg = (gs, n_domains, mode | layout, eps, n, c, hw, color.shape, bias.shape)
-        ctx.route = r
-        return y
-
-    @staticmethod
-    def backward(ctx, dout):
-        lib = nv.lib()
-        x, save_mean, save_w, color_c = ctx.saved_tensors
-        gs, n_domains, mode, eps, n, c, hw, cshape, bshape = ctx.cfg
-        r = ctx.route
-        if dout.dtype != x.dtype:
-            dout = dout.to(x.dtype)
-        dout = dout.contiguous(memory_format=torch.channels_last) if r.nhwc else dout.contiguous()
-        if r.align and dout.data_ptr() % r.align:
-            dout = dout.clone(memory_format=torch.channels_last if r.nhwc else torch.contiguous_format)
-        dev = nv.require_cuda(dout, bf16=True)
-        dx = torch.empty_like(x)
-        want = ctx.needs_input_grad[1] or ctx.needs_input_grad[2]
-        dcolor = torch.empty(c // gs, gs, gs, dtype=torch.float32, device=dev) if want else None
-        dbias = torch.empty(c, dtype=torch.float32, device=dev) if want else None
-        ws = nv.workspace(dev, n, c, hw, gs, n_domains)
-        with torch.cuda.device(dev):
-            rc = lib.dwt_whiten_color_bwd(nv.ptr(x), nv.ptr(dout), nv.ptr(dx), n, c, hw, gs, n_domains, mode, eps,
-                                          nv.ptr(save_mean), nv.ptr(save_w), nv.ptr(color_c), nv.ptr(dcolor), nv.ptr(dbias),
-                                          nv.ptr(ws), ws.numel(), nv.stream_ptr(dev))
-        nv.check(rc)
-        if want:
-            dcolor, dbias = dcolor.view(cshape), dbias.view(bshape)
-        return (dx, dcolor, dbias) + (None,) * 8
-
-
 def color(x, weight, bias, *, group_size, n_domains, training_stats, eps, momentum, update_running, running):
     """y = weight_g W (x - mean) + bias: whitening in the Cholesky basis, then the learnable colouring of each group of
-    group_size channels (weight [C/gs, gs, gs], bias with C elements, float32; see _ColorFunction).  The tensor-core
-    kernels only: a call they cannot take raises NativeError.  bf16 activations run the bf16 kernels where they are
-    built, else the float32 kernels on upcast copies (functional.norm's rule)."""
-    mode = nv.MODE_TRAIN if training_stats else nv.MODE_EVAL
-    args = (group_size, n_domains, mode, float(eps), float(momentum), bool(update_running), running)
-    r = route(x, None, "whiten", group_size, n_domains)
-    if r is None:
-        xf = x.float()
-        y = _ColorFunction.apply(xf, weight, bias, *args, route(xf, None, "whiten", group_size, n_domains))
-        return y.to(x.dtype)
-    return _ColorFunction.apply(x, weight, bias, *args, r)
+    group_size channels (weight [C/gs, gs, gs], bias with C elements, float32; _NormFunction's colour basis).  The
+    tensor-core kernels only: a call they cannot take raises NativeError.  bf16 activations run the bf16 kernels where
+    they are built, else the float32 kernels on upcast copies (functional.norm's rule)."""
+    return _norm(x, weight, bias, None, "whiten", group_size, n_domains, training_stats, eps, momentum, update_running,
+                 running, False, nv.COLOR)
+
+
+def _tma_ready(x):
+    """-> (x dense in its own layout, channels-last or NCHW, with a 16-byte-aligned data_ptr() for the kernels' TMA reads;
+    that memory format)."""
+    fmt = torch.channels_last if _channels_last(x) else torch.contiguous_format
+    x = x.contiguous(memory_format=fmt)
+    return (x.clone(memory_format=fmt) if x.data_ptr() % 16 else x), fmt
+
+
+def _apply_per_image(fn, x, *args):
+    """fn.apply(x, *args) for the per-image kernels: a bfloat16 NCHW x whose H*W is not a multiple of 8 (the bf16 kernels'
+    TMA rows) runs the same kernels in float32 on an upcast copy, the result in bfloat16."""
+    if x.dtype == torch.bfloat16 and not _channels_last(x) and math.prod(x.shape[2:]) % 8:
+        return fn.apply(x.float(), *args).to(x.dtype)
+    return fn.apply(x, *args)
 
 
 class _InstanceFunction(torch.autograd.Function):
@@ -526,17 +480,13 @@ class _InstanceFunction(torch.autograd.Function):
         dev = nv.require_cuda(x, bf16=True)
         lib = nv.lib()
         gs = group_size
-        nhwc = _channels_last(x)
-        fmt = torch.channels_last if nhwc else torch.contiguous_format
-        x = x.contiguous(memory_format=fmt)
-        if x.data_ptr() % 16:                        # the kernels read x through TMA
-            x = x.clone(memory_format=fmt)
+        x, fmt = _tma_ready(x)
         n, c, hw = x.shape[0], x.shape[1], math.prod(x.shape[2:])
-        flags = (nv.LAYOUT_NHWC if nhwc else 0) | (nv.DTYPE_BF16 if x.dtype == torch.bfloat16 else 0)
+        flags = (nv.LAYOUT_NHWC if fmt == torch.channels_last else 0) | (nv.DTYPE_BF16 if x.dtype == torch.bfloat16 else 0)
         y = torch.empty_like(x)
         save_mean = torch.empty(n, c, dtype=torch.float32, device=dev)
         save_w = torch.empty(n, max(c // gs, 1), gs, gs, dtype=torch.float32, device=dev)
-        ws = nv.instance_workspace(dev, n, c, hw, gs)
+        ws = nv.grow_workspace(dev, lib.dwt_instance_workspace_bytes(n, c, hw, gs))
         with torch.cuda.device(dev):
             rc = lib.dwt_whiten_instance_fwd(nv.ptr(x), nv.ptr(y), n, c, hw, gs, flags, eps, nv.ptr(save_mean),
                                              nv.ptr(save_w), nv.ptr(ws), ws.numel(), nv.stream_ptr(dev))
@@ -551,12 +501,10 @@ class _InstanceFunction(torch.autograd.Function):
         lib = nv.lib()
         x, save_mean, save_w = ctx.saved_tensors
         gs, flags, eps, n, c, hw, fmt = ctx.cfg
-        dout = dout.to(x.dtype).contiguous(memory_format=fmt)
-        if dout.data_ptr() % 16:
-            dout = dout.clone(memory_format=fmt)
+        dout, _ = _prepare_dout(ctx, dout, x, fmt, 16)
         dev = nv.require_cuda(dout, bf16=True)
         dx = torch.empty_like(x)
-        ws = nv.instance_workspace(dev, n, c, hw, gs)
+        ws = nv.grow_workspace(dev, lib.dwt_instance_workspace_bytes(n, c, hw, gs))
         with torch.cuda.device(dev):
             rc = lib.dwt_whiten_instance_bwd(nv.ptr(x), nv.ptr(dout), nv.ptr(dx), n, c, hw, gs, flags, eps, nv.ptr(save_mean),
                                              nv.ptr(save_w), nv.ptr(ws), ws.numel(), nv.stream_ptr(dev))
@@ -574,9 +522,7 @@ def instance_whiten(x, *, group_size, eps):
     if x.dim() < 3:
         raise ValueError(f"instance whitening expects [N, C, *] input (got {x.dim()}D input)")
     nv.require_cuda(x, bf16=True)
-    if x.dtype == torch.bfloat16 and not _channels_last(x) and math.prod(x.shape[2:]) % 8:
-        return _InstanceFunction.apply(x.float(), int(group_size), float(eps)).to(x.dtype)
-    return _InstanceFunction.apply(x, int(group_size), float(eps))
+    return _apply_per_image(_InstanceFunction, x, int(group_size), float(eps))
 
 
 class _SwitchFunction(torch.autograd.Function):
@@ -593,25 +539,20 @@ class _SwitchFunction(torch.autograd.Function):
         nv.require_cuda(mix, rm_t, rv_t)
         lib = nv.lib()
         gs = group_size
-        nhwc = _channels_last(x)
-        fmt = torch.channels_last if nhwc else torch.contiguous_format
-        x = x.contiguous(memory_format=fmt)
-        if x.data_ptr() % 16:                        # the kernels read x through TMA
-            x = x.clone(memory_format=fmt)
+        x, fmt = _tma_ready(x)
         n, c, hw = x.shape[0], x.shape[1], math.prod(x.shape[2:])
         mix_c = _aligned(mix)
         _check_param("mix", mix_c, 6)
         need_running = (mode == nv.MODE_EVAL) or update_running
         if need_running:
-            _check_param("running mean", rm_t, c)
-            _check_param("running second moment", rv_t, c * gs)
-        flags = mode | (nv.LAYOUT_NHWC if nhwc else 0) | (nv.DTYPE_BF16 if x.dtype == torch.bfloat16 else 0)
+            _check_running([running], c, gs, domains=False)
+        flags = mode | (nv.LAYOUT_NHWC if fmt == torch.channels_last else 0) | (nv.DTYPE_BF16 if x.dtype == torch.bfloat16 else 0)
         y = torch.empty_like(x)
         g = max(c // gs, 1)
         save_mean = torch.empty(n, c, dtype=torch.float32, device=dev)
         save_w = torch.empty(n, g, gs, gs, dtype=torch.float32, device=dev)
         save_stats = torch.empty(n + 1, g, gs * gs + gs, dtype=torch.float32, device=dev)
-        ws = nv.switch_workspace(dev, n, c, hw, gs)
+        ws = nv.grow_workspace(dev, lib.dwt_switch_workspace_bytes(n, c, hw, gs))
         rm, rv = (nv.ptr(rm_t), nv.ptr(rv_t)) if need_running else (None, None)
         with torch.cuda.device(dev):
             rc = lib.dwt_whiten_switch_fwd(nv.ptr(x), nv.ptr(y), n, c, hw, gs, flags, eps, momentum, int(update_running), rm,
@@ -620,8 +561,7 @@ class _SwitchFunction(torch.autograd.Function):
         nv.check(rc)
         nv.poll_status(dev)
         if update_running and mode == nv.MODE_TRAIN:
-            for buf in {id(b): b for b in (rm_t, rv_t)}.values():    # see _NormFunction.forward
-                torch.autograd.graph.increment_version(buf)
+            _bump_versions([running])
         ctx.save_for_backward(x, mix_c, save_mean, save_w, save_stats)
         ctx.cfg = (gs, flags, eps, n, c, hw, fmt)
         return y
@@ -631,13 +571,11 @@ class _SwitchFunction(torch.autograd.Function):
         lib = nv.lib()
         x, mix_c, save_mean, save_w, save_stats = ctx.saved_tensors
         gs, flags, eps, n, c, hw, fmt = ctx.cfg
-        dout = dout.to(x.dtype).contiguous(memory_format=fmt)
-        if dout.data_ptr() % 16:
-            dout = dout.clone(memory_format=fmt)
+        dout, _ = _prepare_dout(ctx, dout, x, fmt, 16)
         dev = nv.require_cuda(dout, bf16=True)
         dx = torch.empty_like(x)
         dmix = torch.empty(6, dtype=torch.float32, device=dev) if ctx.needs_input_grad[1] else None
-        ws = nv.switch_workspace(dev, n, c, hw, gs)
+        ws = nv.grow_workspace(dev, lib.dwt_switch_workspace_bytes(n, c, hw, gs))
         with torch.cuda.device(dev):
             rc = lib.dwt_whiten_switch_bwd(nv.ptr(x), nv.ptr(dout), nv.ptr(dx), n, c, hw, gs, flags, eps, nv.ptr(mix_c),
                                            nv.ptr(save_mean), nv.ptr(save_w), nv.ptr(save_stats), nv.ptr(dmix), nv.ptr(ws),
@@ -663,10 +601,7 @@ def switchable_whiten(x, mix, *, group_size, training_stats, eps, momentum, upda
     nv.require_cuda(x, bf16=True)
     mode = nv.MODE_TRAIN if training_stats else nv.MODE_EVAL
     args = (int(group_size), mode, float(eps), float(momentum), bool(update_running), tuple(running))
-    mix = mix.float()
-    if x.dtype == torch.bfloat16 and not _channels_last(x) and math.prod(x.shape[2:]) % 8:
-        return _SwitchFunction.apply(x.float(), mix, *args).to(x.dtype)
-    return _SwitchFunction.apply(x, mix, *args)
+    return _apply_per_image(_SwitchFunction, x, mix.float(), *args)
 
 
 class _MecFunction(torch.autograd.Function):
