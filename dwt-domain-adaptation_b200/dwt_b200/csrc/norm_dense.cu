@@ -8,13 +8,12 @@
 //                    running-statistic EMA (domains in order: one CTA owns all domains of its group)
 //   bwd_coef         per (domain, group): A1 = W^T, Bm = (2a/M) sym(W^T Phi(-R W^T) W), cvec
 //   fwd_zca/bwd_zca  the same two steps in the ZCA basis (dwt_whiten_zca_*): W = P_T / sqrt(tr S) by T Newton-Schulz
-//                    iterations on shared-memory operands, and the reverse of that recursion; fwd_zca shares fwd_factor's
-//                    statistics prologue and EMA tail
+//                    iterations on shared-memory operands, and the reverse of that recursion
 //   fwd_eigh/bwd_eigh  the exact ZCA basis (dwt_whiten_eigh_*): W = U diag(lambda^-1/2) U^T by a cyclic Jacobi
-//                    eigensolver in shared memory, and the Daleckii-Krein backward; the same prologue and EMA tail
+//                    eigensolver in shared memory, and the Daleckii-Krein backward
 //   fwd_factor<COLOR>, bwd_color  colouring (dwt_whiten_color_*): fwd_factor also writes color W; bwd_color runs bwd_coef's
 //                    algebra on color^T R, domains in order in one CTA per group, and sums dcolor and dbias over them
-//   fwd_instance     instance whitening (dwt_whiten_instance_*): fwd_factor's prologue and factorisation, one CTA per
+//   fwd_instance     instance whitening (dwt_whiten_instance_*): fwd_factor's statistics and factorisation, one CTA per
 //                    (image, group), no EMA; its backward is bwd_coef as it is, with the images as the domains
 //   sw_*             switchable whitening (dwt_whiten_switch_*): per-image and batch moments (sw_stats), the mixture and
 //                    fwd_instance's factorisation (sw_fwd_factor); backward: dL/dcov_hat and dL/dm per (image, group)
@@ -25,6 +24,11 @@
 // register block.  fwd_factor runs the Cholesky factorisation AND the triangular inverse as one blocked
 // right-looking sweep of 16 panel steps (one block barrier each): the matrices live in registers, shared
 // memory only carries the 4-column panel of L and the 4-row panel of W of the current step.
+//
+// The forward kernels are built from shared pieces: fwd_domains (the domain loop of fwd_factor, fwd_zca and fwd_eigh:
+// domain_stats, the barriers, the EMA of an accepted domain (domain_ema) and DWT_STATUS_NOT_PD; a basis adds only its
+// step from S to W and its saved matrices) and image_factor_tail (factorisation, W or NaN and the status bit of
+// fwd_instance and sw_fwd_factor).  ema_cov / ema_mean are the one EMA formula of domain_ema and sw_fwd_factor.
 //
 // The backward kernels are built from shared pieces: load_operands / store_operands (W, R = sum dy xc^T, sum dy and a
 // basis' third matrix; bwd_coef, bwd_zca, bwd_eigh, sw_bwd_coef), chol_bwd_core (the Cholesky basis' three products;
@@ -303,15 +307,15 @@ __device__ __forceinline__ bool factor_and_invert(float (&a)[4][4], float (&b)[4
 }
 
 // ------------------------------------------------------------------------------------------
-// Statistics prologue and EMA tail of one domain, shared by fwd_factor and fwd_zca: both bases see the same S, write the
-// same save_mean and apply the same running-buffer update, bit for bit.
+// The domain loop of the per-group forward kernels (fwd_factor, fwd_zca, fwd_eigh): every basis sees the same S, writes
+// the same save_mean and applies the same running-buffer update, bit for bit.
 //   gram  [D][SB][kNacc]  reduced moments around the pilot shift (null: take the running buffers = eval)
 //   shift [D][SB*64]
 // ------------------------------------------------------------------------------------------
-constexpr int kEmaPer = kSB * kSB / 256;
+constexpr int kPer = kSB * kSB / 256;   // elements of a 64 x 64 matrix per thread: e = threadIdx.x + 256 n
 
 struct EmaOld {            // the running buffers as the domain's EMA finds them (loaded with the moments)
-  float rc[kEmaPer], rm;
+  float rc[kPer], rm;
   bool on;                 // train with update_running
 };
 
@@ -346,7 +350,7 @@ __device__ __forceinline__ void domain_stats(const float* G, const float* __rest
   old.on = G != nullptr && f.update_running;
   if (old.on) {
 #pragma unroll
-    for (int n = 0; n < kEmaPer; ++n) {
+    for (int n = 0; n < kPer; ++n) {
       const int e = threadIdx.x + 256 * n;
       old.rc[n] = e < GS * GS ? f.rcov[d][(size_t)g * GS * GS + e] : 0.f;
     }
@@ -378,22 +382,70 @@ __device__ __forceinline__ void domain_stats(const float* G, const float* __rest
     }
 }
 
+// One element of the running-statistic EMA (m = momentum, k = 1 - m), for every gs 8-64 forward, so that their running
+// buffers agree bit for bit: the covariance contracted by the compiler, the mean by the contraction fwd_factor has always
+// used, fma(1 - m, old, m * stat)
+__device__ __forceinline__ float ema_cov(float m, float k, float stat, float old) { return m * stat + k * old; }
+__device__ __forceinline__ float ema_mean(float m, float k, float stat, float old) { return fmaf(k, old, __fmul_rn(m, stat)); }
+
 // The EMA of domain d (train, update_running, batch covariance accepted): sC and sMean complete behind a block barrier.
 __device__ __forceinline__ void domain_ema(int d, int g, const Geom& gm, const FwdFin& f, const float* sC, const float* sMean,
                                            const EmaOld& old) {
   const int GS = gm.GS;
   const float m = f.momentum, k = 1.f - f.momentum;
 #pragma unroll
-  for (int n = 0; n < kEmaPer; ++n) {
+  for (int n = 0; n < kPer; ++n) {
     const int e = threadIdx.x + 256 * n;
-    if (e < GS * GS) f.rcov[d][(size_t)g * GS * GS + e] = m * (sC[(e / GS) * LDS + e % GS] * f.unbias) + k * old.rc[n];
+    if (e < GS * GS) f.rcov[d][(size_t)g * GS * GS + e] = ema_cov(m, k, sC[(e / GS) * LDS + e % GS] * f.unbias, old.rc[n]);
   }
-  // the contraction fwd_factor has always used: fma(1 - m, old, m * mean)
-  if ((int)threadIdx.x < GS) f.rmean[d][g * GS + threadIdx.x] = fmaf(k, old.rm, __fmul_rn(m, sMean[threadIdx.x]));
+  if ((int)threadIdx.x < GS) f.rmean[d][g * GS + threadIdx.x] = ema_mean(m, k, sMean[threadIdx.x], old.rm);
+}
+
+// fwd_domains' shared memory: domain_stats' outputs (sC [kMat], sMean, sRow [kSB]) and the bad flags of the group and of
+// the current domain.  Each kernel declares them as separate arrays: one __shared__ struct of them made ptxas schedule
+// fwd_factor's sweep differently and measurably slower.
+struct DomainSmem {
+  float *C, *mean, *row;
+  int &bad, &bad_dom;
+};
+
+// A basis' step flags the current domain: DWT_STATUS_NOT_PD at the end, and no EMA for the domain
+__device__ __forceinline__ void mark_bad(const DomainSmem& sd) { sd.bad = 1; sd.bad_dom = 1; }
+
+struct NoAfter { __device__ void operator()(size_t, const Blk&) const {} };
+
+// The domain loop of fwd_factor, fwd_zca and fwd_eigh: the CTA of group blockIdx.x runs the domains in order (EMA
+// sequence, SURVEY H5).  Per domain: domain_stats; the basis' step(d, gbase, a, t) with this thread's block of S in a,
+// which writes save_w + gbase and the basis' saved matrices and may call mark_bad; a block barrier; after(gbase, t),
+// which may read what the step left in shared memory; the EMA unless the domain was marked bad.
+template <class Step, class After = NoAfter>
+__device__ __forceinline__ void fwd_domains(const float* __restrict__ gram, const float* __restrict__ shift, const Geom& gm,
+                                            const FwdFin& f, const DomainSmem& sd PROF_ARGS, Step step, After after = {}) {
+  const int g = blockIdx.x;
+  const auto [GS, sb, o, SB] = group_pos(gm, g);
+  const Blk t(GS);
+  const float invM = 1.f / gm.M;
+  if (threadIdx.x == 0) sd.bad = 0;
+  PROF_MARK();
+  for (int d = 0; d < gm.D; ++d) {
+    const float* G = gram ? gram + ((size_t)d * SB + sb) * kNacc : nullptr;
+    const size_t gbase = ((size_t)d * gm.G + g) * GS * GS;
+    float a[4][4];
+    EmaOld old;
+    domain_stats(G, shift, d, g, sb, o, SB, invM, gm, f, t, sd.C, sd.mean, sd.row, sd.bad_dom, a, old);
+    step(d, gbase, a, t);
+    __syncthreads();                                  // sC complete, sBadDom final
+    after(gbase, t);
+    if (old.on && !sd.bad_dom) domain_ema(d, g, gm, f, sd.C, sd.mean, old);   // a non-PD batch covariance never reaches the running buffers
+    __syncthreads();      // also orders this domain's buffer writes before the next domain's reads (aliasing)
+    PROF_MARK();
+  }
+  if (threadIdx.x == 0 && sd.bad) atomicOr(f.status, DWT_STATUS_NOT_PD);
 }
 
 // ------------------------------------------------------------------------------------------
-// fwd_factor: grid (G), 256 threads; loops over the domains in order (EMA sequence, SURVEY H5)
+// fwd_factor: grid (G), 256 threads, fwd_domains with the blocked Cholesky + inverse as its step.  A domain that is not
+// positive definite keeps the W the sweep left (not NaN'd).
 // COLOR: also gw [D][G][gs*gs] = color[g] W (color [G][gs*gs]), for the apply in place of W; dynamic shared memory holds
 // color and W (kColorFwdSmem)
 // ------------------------------------------------------------------------------------------
@@ -402,57 +454,37 @@ __global__ void __launch_bounds__(256) fwd_factor_kernel(const float* __restrict
                                                          const Geom gm, const FwdFin f, const float* __restrict__ color,
                                                          float* __restrict__ gw) {
   __shared__ __align__(16) PanelSmem sp;
-  __shared__ float sC[kMat];       // un-shrunk covariance (for the EMA)
-  __shared__ float sMean[kSB], sRow[kSB];
+  __shared__ float sC[kMat], sMean[kSB], sRow[kSB];
   __shared__ int sBad, sBadDom;
-  const int g = blockIdx.x;
-  const auto [GS, sb, o, SB] = group_pos(gm, g);
-  const Blk t(GS);
-  const float invM = 1.f / gm.M;
-  if (threadIdx.x == 0) sBad = 0;
+  const DomainSmem sd{sC, sMean, sRow, sBad, sBadDom};
   extern __shared__ __align__(16) float dsm[];
   float* sGam = dsm;                                  // COLOR: color[g], then W of the domain
   float* sWd = dsm + kMat;
+  const int GS = gm.GS;
   if constexpr (COLOR) {                              // published by domain_stats' barrier
-    for (int e = threadIdx.x; e < GS * GS; e += 256) sGam[(e / GS) * LDS + e % GS] = color[(size_t)g * GS * GS + e];
+    for (int e = threadIdx.x; e < GS * GS; e += 256) sGam[(e / GS) * LDS + e % GS] = color[(size_t)blockIdx.x * GS * GS + e];
   }
   PROF_DECL;
-  PROF_MARK();
-  for (int d = 0; d < gm.D; ++d) {
-    const float* G = gram ? gram + ((size_t)d * SB + sb) * kNacc : nullptr;
-    const size_t gbase = ((size_t)d * gm.G + g) * GS * GS;
-    float a[4][4], w[4][4];
-    EmaOld old;
-    domain_stats(G, shift, d, g, sb, o, SB, invM, gm, f, t, sC, sMean, sRow, sBadDom, a, old);
+  fwd_domains(gram, shift, gm, f, sd PROF_PASS, [&](int, size_t gbase, float (&a)[4][4], const Blk& t) {
+    float w[4][4];
     PROF_MARK();
-    if (!factor_and_invert(a, w, GS, t, sp)) { sBad = 1; sBadDom = 1; }
+    if (!factor_and_invert(a, w, GS, t, sp)) mark_bad(sd);
     PROF_MARK();
-    if (t.act) {                                      // w[r][s] = W(4bi + r, 4bj + s): straight from the registers
-#pragma unroll
-      for (int r = 0; r < 4; ++r)
-        *reinterpret_cast<float4*>(f.save_w + gbase + (size_t)(4 * t.bi + r) * GS + 4 * t.bj) =
-            make_float4(w[r][0], w[r][1], w[r][2], w[r][3]);
-    }
+    store_block_global(f.save_w + gbase, GS, t, w);  // w[r][s] = W(4bi + r, 4bj + s): straight from the registers
     if constexpr (COLOR) store_block(sWd, t, w);
-    __syncthreads();                                  // sC complete, sBadDom final
+  }, [&](size_t gbase, const Blk& t) {
     if constexpr (COLOR) {
       float c[4][4];
       mm_block<false, false>(sGam, sWd, GS, t, c);
       store_block_global(gw + gbase, GS, t, c);
     }
-    if (old.on && !sBadDom) domain_ema(d, g, gm, f, sC, sMean, old);   // a non-PD batch covariance never reaches the running buffers
-    __syncthreads();      // also orders this domain's buffer writes before the next domain's reads (aliasing)
-    PROF_MARK();
-  }
+  });
   PROF_DUMP("fwd_factor load|factor+invert|save+ema");
-  if (threadIdx.x == 0 && sBad) atomicOr(f.status, DWT_STATUS_NOT_PD);
 }
 
 // ------------------------------------------------------------------------------------------
 // Backward pieces shared by the per-group backward kernels (gs 8..64)
 // ------------------------------------------------------------------------------------------
-constexpr int kPer = kSB * kSB / 256;   // elements of a 64 x 64 matrix per thread: e = threadIdx.x + 256 n
-
 // One (domain, group) problem's backward operands in registers: this thread's elements of W, of R = sum dy xc^T and,
 // with HAS_X, of a third GS x GS matrix X; and sum dy of channel threadIdx.x.
 struct Operands {
@@ -689,8 +721,8 @@ __device__ __forceinline__ float trace_of(const float* M, int GS, float* sRed) {
   return sRed[0];
 }
 
-// fwd_zca: grid (G), 256 threads, domains in order with fwd_factor's statistics prologue and EMA tail.  Three products
-// per iteration (P P, (P P) P, (P P P) N) on shared-memory operands; each thread keeps its block of P in registers.
+// fwd_zca: grid (G), 256 threads, fwd_domains with the Newton-Schulz iteration as its step.  Three products per
+// iteration (P P, (P P) P, (P P P) N) on shared-memory operands; each thread keeps its block of P in registers.
 // A non-finite or non-positive t, or a non-finite W, flags the domain as a non-positive pivot does in fwd_factor
 // (DWT_STATUS_NOT_PD, no EMA).  An indefinite S whose iteration stays finite is not detected: batch statistics are
 // positive semi-definite and shrunk, so only running buffers a user supplied (eval) can be indefinite.
@@ -701,28 +733,20 @@ __global__ void __launch_bounds__(256) fwd_zca_kernel(const float* __restrict__ 
   float* sP = sN + kMat;
   float* sT1 = sP + kMat;          // P P
   float* sT2 = sT1 + kMat;         // P P P
-  __shared__ float sC[kMat];       // un-shrunk covariance (for the EMA)
-  __shared__ float sMean[kSB], sRow[kSB], sRed[1];
+  __shared__ float sC[kMat], sMean[kSB], sRow[kSB];
   __shared__ int sBad, sBadDom;
-  const int g = blockIdx.x;
-  const auto [GS, sb, o, SB] = group_pos(gm, g);
-  const Blk t(GS);
-  const float invM = 1.f / gm.M;
-  if (threadIdx.x == 0) sBad = 0;
+  const DomainSmem sd{sC, sMean, sRow, sBad, sBadDom};
+  __shared__ float sRed[1];
+  const int GS = gm.GS;
   PROF_DECL;
-  PROF_MARK();
-  for (int d = 0; d < gm.D; ++d) {
-    const float* G = gram ? gram + ((size_t)d * SB + sb) * kNacc : nullptr;
-    const size_t gbase = ((size_t)d * gm.G + g) * GS * GS;
+  fwd_domains(gram, shift, gm, f, sd PROF_PASS, [&](int, size_t gbase, float (&a)[4][4], const Blk& t) {
     float* pd = save_p + gbase * T;
-    float a[4][4], p[4][4], c[4][4];
-    EmaOld old;
-    domain_stats(G, shift, d, g, sb, o, SB, invM, gm, f, t, sC, sMean, sRow, sBadDom, a, old);
+    float p[4][4], c[4][4];
     store_block(sN, t, a);
     store_block_global(pd, GS, t, a);                 // slot 0: S
     __syncthreads();
     const float tr = trace_of(sN, GS, sRed);
-    if (threadIdx.x == 0 && !(tr > 0.f && tr < INFINITY)) { sBad = 1; sBadDom = 1; }
+    if (threadIdx.x == 0 && !(tr > 0.f && tr < INFINITY)) mark_bad(sd);
 #pragma unroll
     for (int r = 0; r < 4; ++r)
 #pragma unroll
@@ -763,14 +787,9 @@ __global__ void __launch_bounds__(256) fwd_zca_kernel(const float* __restrict__ 
         finite = finite && isfinite(p[r][s]);
       }
     store_block_global(f.save_w + gbase, GS, t, p);
-    if (!finite) { sBad = 1; sBadDom = 1; }
-    __syncthreads();                                  // sC complete, sBadDom final
-    if (old.on && !sBadDom) domain_ema(d, g, gm, f, sC, sMean, old);
-    __syncthreads();      // also orders this domain's buffer writes before the next domain's reads (aliasing)
-    PROF_MARK();
-  }
+    if (!finite) mark_bad(sd);
+  });
   PROF_DUMP("fwd_zca load|iterate|save+ema");
-  if (threadIdx.x == 0 && sBad) atomicOr(f.status, DWT_STATUS_NOT_PD);
 }
 
 // bwd_zca: grid (G, 1, D), 256 threads.  The reverse of fwd_zca's recursion from dL/dW = R = sum dy xc^T:
@@ -987,68 +1006,54 @@ __device__ void jacobi_eigh(float* sA, float* sU, int GS, JacobiSmem& js) {
   }
 }
 
-// fwd_eigh: grid (G), 256 threads, domains in order with fwd_factor's statistics prologue and EMA tail.  A
-// non-finite S skips the solver; a non-finite or non-positive eigenvalue (an indefinite running buffer in eval, too)
-// flags the domain as a non-positive pivot does in fwd_factor (DWT_STATUS_NOT_PD, no EMA).  W = V V^T with
-// V = U diag(lambda^-1/4): symmetric bit for bit.
+// fwd_eigh: grid (G), 256 threads, fwd_domains with the Jacobi solve as its step.  A non-finite S skips the solver;
+// a non-finite or non-positive eigenvalue (an indefinite running buffer in eval, too) flags the domain as a
+// non-positive pivot does in fwd_factor (DWT_STATUS_NOT_PD, no EMA).  W = V V^T with V = U diag(lambda^-1/4):
+// symmetric bit for bit.
 __global__ void __launch_bounds__(256) fwd_eigh_kernel(const float* __restrict__ gram, const float* __restrict__ shift,
                                                        const Geom gm, const FwdFin f, float* __restrict__ save_e) {
   extern __shared__ __align__(16) float dsm[];
   float* sA = dsm;                 // S, then diag(lambda) + rounding, then V
   float* sU = sA + kMat;
-  __shared__ float sC[kMat];       // un-shrunk covariance (for the EMA)
-  __shared__ float sMean[kSB], sRow[kSB], sLam[kSB];
-  __shared__ JacobiSmem js;
+  __shared__ float sC[kMat], sMean[kSB], sRow[kSB];
   __shared__ int sBad, sBadDom;
-  const int g = blockIdx.x;
-  const auto [GS, sb, o, SB] = group_pos(gm, g);
-  const Blk t(GS);
-  const float invM = 1.f / gm.M;
-  const int lgs = __ffs(GS) - 1;
-  if (threadIdx.x == 0) sBad = 0;
+  const DomainSmem sd{sC, sMean, sRow, sBad, sBadDom};
+  __shared__ float sLam[kSB];
+  __shared__ JacobiSmem js;
+  const int GS = gm.GS, lgs = __ffs(GS) - 1;
   PROF_DECL;
-  PROF_MARK();
-  for (int d = 0; d < gm.D; ++d) {
-    const float* G = gram ? gram + ((size_t)d * SB + sb) * kNacc : nullptr;
-    const size_t gbase = ((size_t)d * gm.G + g) * GS * GS;
-    float* ed = save_e + ((size_t)d * gm.G + g) * (GS + 1) * GS;
-    float a[4][4], c[4][4];
-    EmaOld old;
-    domain_stats(G, shift, d, g, sb, o, SB, invM, gm, f, t, sC, sMean, sRow, sBadDom, a, old);
+  fwd_domains(gram, shift, gm, f, sd PROF_PASS, [&](int d, size_t gbase, float (&a)[4][4], const Blk& t) {
+    float* ed = save_e + ((size_t)d * gm.G + blockIdx.x) * (GS + 1) * GS;
+    float c[4][4];
     bool finite = true;
 #pragma unroll
     for (int r = 0; r < 4; ++r)
 #pragma unroll
       for (int s = 0; s < 4; ++s) finite = finite && isfinite(a[r][s]);
     store_block(sA, t, a);
-    if (!finite) { sBad = 1; sBadDom = 1; }
+    if (!finite) mark_bad(sd);
     __syncthreads();
     PROF_MARK();
-    if (!sBadDom) jacobi_eigh(sA, sU, GS, js);        // block-uniform
+    if (!sd.bad_dom) jacobi_eigh(sA, sU, GS, js);     // block-uniform
     PROF_MARK();
     if ((int)threadIdx.x < GS) {
       const float lam = sA[threadIdx.x * LDS + threadIdx.x];
       sLam[threadIdx.x] = lam;
       ed[GS * GS + threadIdx.x] = lam;
-      if (!(lam > 0.f && lam < INFINITY)) { sBad = 1; sBadDom = 1; }
+      if (!(lam > 0.f && lam < INFINITY)) mark_bad(sd);
     }
     __syncthreads();
     for (int e = threadIdx.x; e < GS * GS; e += blockDim.x) {
       const int i = e >> lgs, j = e & (GS - 1);
-      const float u = sBadDom ? NAN : sU[i * LDS + j];   // a skipped solver left no U
+      const float u = sd.bad_dom ? NAN : sU[i * LDS + j];   // a skipped solver left no U
       ed[e] = u;
       sA[i * LDS + j] = u / sqrtf(sqrtf(sLam[j]));    // V = U lambda^-1/4
     }
     __syncthreads();
     mm_block<false, true>(sA, sA, GS, t, c);          // W = V V^T
     store_block_global(f.save_w + gbase, GS, t, c);
-    __syncthreads();                                  // sC complete, sBadDom final
-    if (old.on && !sBadDom) domain_ema(d, g, gm, f, sC, sMean, old);
-    __syncthreads();      // also orders this domain's buffer writes before the next domain's reads (aliasing)
-    PROF_MARK();
-  }
+  });
   PROF_DUMP("fwd_eigh load|solve|save+ema");
-  if (threadIdx.x == 0 && sBad) atomicOr(f.status, DWT_STATUS_NOT_PD);
 }
 
 // bwd_eigh: grid (G, 1, D), 256 threads.  From dL/dW = R = sum dy xc^T by the Daleckii-Krein formula:
@@ -1214,30 +1219,37 @@ __global__ void __launch_bounds__(kThreads2) bwd_coef128_kernel(const float* __r
 }
 
 // ------------------------------------------------------------------------------------------
+// The end of the per-image forward kernels (fwd_instance, sw_fwd_factor): this thread's block of S (a) factored and
+// inverted, the CTA's OR of bad (S or the mean not finite) and of a non-positive pivot, W to save_w, or NaN in full for a
+// bad problem, and DWT_STATUS_NOT_PD
+__device__ __forceinline__ void image_factor_tail(float (&a)[4][4], bool bad, size_t problem, int GS, const Blk& t,
+                                                  PanelSmem& sp, float* save_w, int* status) {
+  float w[4][4];
+  const bool ok = factor_and_invert(a, w, GS, t, sp);
+  bad = __syncthreads_or(bad || !ok) != 0;
+  store_w_or_nan(save_w, problem, GS, t, w, bad);
+  if (threadIdx.x == 0 && bad) atomicOr(status, DWT_STATUS_NOT_PD);
+}
+
 // fwd_instance: instance whitening (dwt_whiten_instance_fwd), grid (G, 1, D), 256 threads, one CTA per (image, group):
 // the Geom's domains are the images (N = 1, M = HW).  fwd_factor's statistics prologue and blocked Cholesky + inverse,
 // without the EMA and without its loop over the domains: fwd_factor serialises them in one CTA per group, which at
 // hundreds of images would leave all but G CTAs of the H100 idle.  A group whose S is not positive definite (or not
 // finite) gets W = NaN in full, so that image's whole group reads NaN, and sets DWT_STATUS_NOT_PD.
-// ------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) fwd_instance_kernel(const float* __restrict__ gram, const float* __restrict__ shift,
                                                            const Geom gm, const FwdFin f) {
   __shared__ __align__(16) PanelSmem sp;
   __shared__ float sC[kMat];       // written by domain_stats, not read (no EMA)
   __shared__ float sMean[kSB], sRow[kSB];
-  __shared__ int sBadDom;
+  __shared__ int sBadDom;          // cleared by domain_stats, not read
   const int g = blockIdx.x, d = blockIdx.z;
   const auto [GS, sb, o, SB] = group_pos(gm, g);
   const Blk t(GS);
   const float* G = gram + ((size_t)d * SB + sb) * kNacc;
-  float a[4][4], w[4][4];
+  float a[4][4];
   EmaOld old;                      // f.update_running is 0: domain_stats reads no running buffer
   domain_stats(G, shift, d, g, sb, o, SB, 1.f / gm.M, gm, f, t, sC, sMean, sRow, sBadDom, a, old);
-  if (!factor_and_invert(a, w, GS, t, sp)) sBadDom = 1;
-  __syncthreads();                 // sBadDom final
-  const bool bad = sBadDom != 0;
-  store_w_or_nan(f.save_w, (size_t)d * gm.G + g, GS, t, w, bad);
-  if (threadIdx.x == 0 && bad) atomicOr(f.status, DWT_STATUS_NOT_PD);
+  image_factor_tail(a, false, (size_t)d * gm.G + g, GS, t, sp, f.save_w, f.status);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1314,7 +1326,7 @@ __global__ void __launch_bounds__(256) sw_fwd_factor_kernel(const Geom gm, const
   const float* sbt = f.save_stats + ((size_t)gm.D * gm.G + g) * rec;
   const float a_b = f.mix[0], a_i = f.mix[1], w_bw = f.mix[2], w_iw = f.mix[3], w_bn = f.mix[4], w_in = f.mix[5];
   bool bad = false;
-  float a[4][4], w[4][4];
+  float a[4][4];
 #pragma unroll
   for (int r = 0; r < 4; ++r)
 #pragma unroll
@@ -1335,10 +1347,7 @@ __global__ void __launch_bounds__(256) sw_fwd_factor_kernel(const Geom gm, const
     f.save_mean[(size_t)d * gm.C + g * GS + threadIdx.x] = m;
     bad = bad || !isfinite(m);
   }
-  const bool ok = factor_and_invert(a, w, GS, t, sp);
-  bad = __syncthreads_or(bad || !ok) != 0;
-  store_w_or_nan(f.save_w, (size_t)d * gm.G + g, GS, t, w, bad);
-  if (threadIdx.x == 0 && bad) atomicOr(f.status, DWT_STATUS_NOT_PD);
+  image_factor_tail(a, bad, (size_t)d * gm.G + g, GS, t, sp, f.save_w, f.status);
   if (d != 0 || !f.train || !f.update_running) return;
   constexpr int kRecPer = (kSB * kSB + kSB + 255) / 256;
   float old[kRecPer], stat[kRecPer];
@@ -1350,13 +1359,13 @@ __global__ void __launch_bounds__(256) sw_fwd_factor_kernel(const Geom gm, const
     old[n] = e < GS * GS ? f.rcov[(size_t)g * GS * GS + e] : (e < rec ? f.rmean[g * GS + e - GS * GS] : 0.f);
     fin = fin && isfinite(stat[n]);
   }
-  if (!__syncthreads_or(!fin)) {        // dwt_whiten_fwd's EMA: (1 - m) old + m stat on the unshrunk batch moments
+  if (!__syncthreads_or(!fin)) {        // dwt_whiten_fwd's EMA on the unshrunk batch moments
     const float m = f.momentum, k = 1.f - f.momentum;
 #pragma unroll
     for (int n = 0; n < kRecPer; ++n) {
       const int e = threadIdx.x + 256 * n;
-      if (e < GS * GS) f.rcov[(size_t)g * GS * GS + e] = m * stat[n] + k * old[n];
-      else if (e < rec) f.rmean[g * GS + e - GS * GS] = fmaf(k, old[n], __fmul_rn(m, stat[n]));
+      if (e < GS * GS) f.rcov[(size_t)g * GS * GS + e] = ema_cov(m, k, stat[n], old[n]);
+      else if (e < rec) f.rmean[g * GS + e - GS * GS] = ema_mean(m, k, stat[n], old[n]);
     }
   } else if (threadIdx.x == 0) {
     atomicOr(f.status, DWT_STATUS_NOT_PD);
@@ -1547,18 +1556,18 @@ constexpr size_t kSwApplySmem = sizeof(float) * 2 * kMat;  // switchable backwar
 }  // namespace
 
 int dense_init() {
-  cudaError_t e = cudaFuncSetAttribute(fwd_factor_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFactorSmem);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(bwd_coef_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kCoefSmem);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(fwd_factor128_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kFactor2Smem);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(bwd_coef128_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kCoef2Smem);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(fwd_zca_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kZcaFwdSmem);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(bwd_zca_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kZcaBwdSmem);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(fwd_eigh_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kEighFwdSmem);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(bwd_eigh_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kEighBwdSmem);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(fwd_factor_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kColorFwdSmem);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(bwd_color_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kColorBwdSmem);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(sw_bwd_coef_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSwCoefSmem);
-  return (int)e;
+  const struct { const void* kernel; size_t smem; } dynamic_smem[] = {
+      {(const void*)fwd_factor_kernel<false>, kFactorSmem},   {(const void*)bwd_coef_kernel, kCoefSmem},
+      {(const void*)fwd_factor128_kernel, kFactor2Smem},      {(const void*)bwd_coef128_kernel, kCoef2Smem},
+      {(const void*)fwd_zca_kernel, kZcaFwdSmem},             {(const void*)bwd_zca_kernel, kZcaBwdSmem},
+      {(const void*)fwd_eigh_kernel, kEighFwdSmem},           {(const void*)bwd_eigh_kernel, kEighBwdSmem},
+      {(const void*)fwd_factor_kernel<true>, kColorFwdSmem},  {(const void*)bwd_color_kernel, kColorBwdSmem},
+      {(const void*)sw_bwd_coef_kernel, kSwCoefSmem}};
+  for (const auto& k : dynamic_smem) {
+    const cudaError_t e = cudaFuncSetAttribute(k.kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k.smem);
+    if (e != cudaSuccess) return (int)e;
+  }
+  return (int)cudaSuccess;
 }
 
 // partial [problems][nchunks][kNacc] -> gram [problems][kNacc]
