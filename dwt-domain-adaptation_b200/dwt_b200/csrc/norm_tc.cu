@@ -4,18 +4,19 @@
 //   stats       G = sum_m (x-K)(x-K)^T        per 64-channel super-block (gs x gs diagonal blocks kept)
 //   bwd_reduce  R = sum_m dy (x-mean)^T
 //
-// 2*gs flop per 4 bytes read puts these far below the TF32 tensor ridge: they are HBM-bound.  Both kernels are
-// persistent CTAs (two per SM) over a contiguous range of [64 channels x 32 pixels] tiles, warp-specialised:
+// 2*gs flop per 4 bytes read puts these far below the TF32 tensor ridge: they are HBM-bound.  All three kernels are
+// persistent CTAs (two per SM) over a contiguous range of [64 channels x 32 pixels] tiles (TileRange), warp-specialised
+// (tc_ring.cuh), and differ only in what a stage holds, the transforms, the products and the last epilogue step:
 //
-//   warp 8      TMA producer: cp.async.bulk.tensor.3d (box 32 px x 64 ch x 1 image, SWIZZLE_128B) into a
-//               shared-memory ring, mbarrier complete_tx.
-//   warps 0-7   two consumer warpgroups taking alternate tiles: each transforms its landed tile in place for the
-//               tensor core, then issues wgmma.mma_async kind::tf32 (M = 64 channels, K = 8 pixels per instruction)
-//               into an fp32 accumulator held in its registers, and releases the stage.  Operands are K-major straight
-//               from the swizzled tile (NCHW rows ARE K-major: the reference's transposing copy, whitening.py:46,
-//               disappears).
-//   epilogue    the two warpgroups' accumulators are summed in shared memory -> per-CTA partial -> global.  The
-//               fixed-order reduction of the partials and the dense algebra (Cholesky / inverse / EMA, or the backward
+//   produce     warp 8: cp.async.bulk.tensor.3d (box 32 px x 64 ch x 1 image, SWIZZLE_128B) into the Ring of
+//               shared-memory stages, mbarrier complete_tx.
+//   consume     warps 0-7, two warpgroups taking alternate tiles: the kernel's transform splits the landed tile for the
+//               tensor core and names the tile's Products, issued as wgmma.mma_async kind::tf32 (M = 64 channels, K = 8
+//               pixels per instruction) into a fresh fp32 accumulator in registers, then the stage is released.  Operands
+//               are K-major straight from the swizzled tile (NCHW rows ARE K-major: the reference's transposing copy,
+//               whitening.py:46, disappears).
+//   cta_sums    the two warpgroups' sums are added in shared memory -> per-CTA partial -> global.  The fixed-order
+//               reduction of the partials and the dense algebra (Cholesky / inverse / EMA, or the backward
 //               coefficients) run as the small follow-up launches of norm_dense.cu.
 //
 // stats (tc_gram_kernel) -- SPLIT precision.  The covariance feeds a Cholesky factor whose error is the Gram
@@ -75,35 +76,29 @@
 //   Contraction: tc_contract_kernel<.., PAIR = true> forms all four blocks of R (it is not symmetric), blockIdx.y =
 //   4 p + 2 r + c: dy rows from super-block 2p + r (and their shift K), x columns from 2p + c; x and dy are each read twice (concurrently
 //   by the blocks of one wave, so partly from L2; not measured).
-//   ptxas (sm_90a): tc_gram_kernel 96 registers in all four instantiations; tc_gram_pair_kernel NCHW 93 / NHWC 88
-//   registers; tc_contract_kernel<float, NCHW / NHWC, PAIR> 96 / 96 registers; no spills; dynamic shared memory 97 KB (gram pair) and the contraction's 97 KB as above.
+//   ptxas (sm_90a): tc_gram_kernel 96 registers in all four instantiations; tc_gram_pair_kernel NCHW 90 / NHWC 88
+//   registers; tc_contract_kernel<float, NCHW / NHWC, PAIR> 96 / 94 registers; no spills; dynamic shared memory 97 KB (gram pair) and the contraction's 97 KB as above.
 //
 // Reference: utils/whitening.py:46-47 of the reference project and its autograd transpose.
 #include <cuda.h>
 #include <cuda_bf16.h>
 
-#include <type_traits>
-
 #include "dwt_common.cuh"
 #include "norm_launch.h"
-#include "tc_ptx.cuh"
+#include "tc_ring.cuh"
 
 namespace dwt {
 namespace {
 
 using namespace tc;
 
-constexpr int kConsumers = 2;                           // consumer warpgroups per CTA (warps 0-7)
-constexpr int kProducerWarp = 4 * kConsumers;           // warp 8
-constexpr int kTcThreads = 128 * kConsumers + 32;
 constexpr int kPer = 512 / 128;                         // 16-byte chunks of a tile per consumer thread
 constexpr int kTilePx = 32, kTileCh = 64;
 constexpr int kTileBytes = kTileCh * kTilePx * 4;       // 8192: one fp32 tile (also a staging tile of the bf16 kernels)
 constexpr int kStagesBwd = 4;                           // x + dy per stage: 64 KB + 32 KB lo tiles per CTA (bf16: 32 KB + 64 KB)
 constexpr int kNacc = kTileCh * kTileCh + kTileCh;      // per-CTA partial: 64x64 moments + 64 row sums
 constexpr int kGramStages = 10;                         // 80 KB ring + 2 x 8 KB lo tiles per CTA (bf16: 40 KB + 32 KB)
-// Activation storage T: float, or __nv_bfloat16 (DWT_DTYPE_BF16); a landed box is kTileCh x kTilePx values of T
-template <class T> constexpr bool kBf16 = !std::is_same<T, float>::value;
+// a landed box is kTileCh x kTilePx values of T
 template <class T> constexpr int kBoxBytes = kTileCh * kTilePx * (int)sizeof(T);
 // Layout NHWC: the transform writes to staging tiles (the bf16 kernels always do).  fp32 NHWC: the staging tiles cost
 // 32 KB (Gram) or 64 KB (contraction: hi and lo of xc and dy) per CTA, so the rings are shallower to keep two CTAs per SM
@@ -111,27 +106,7 @@ template <class T> constexpr int kBoxBytes = kTileCh * kTilePx * (int)sizeof(T);
 template <class T, bool NHWC> constexpr bool kStaged = kBf16<T> || NHWC;
 template <class T, bool NHWC> constexpr int kGramStagesOf = (NHWC && !kBf16<T>) ? 8 : kGramStages;
 template <class T, bool NHWC> constexpr int kStagesBwdOf = (NHWC && !kBf16<T>) ? 2 : kStagesBwd;
-constexpr int kMaxStages = kGramStages > kStagesBwd ? kGramStages : kStagesBwd;
-// Consumer warpgroup w takes tiles w, w + 2, ...; all ring lengths are even, so every stage (and all phases of its
-// barriers) belongs to one warpgroup, and an mbarrier parity wait never meets a barrier two phases ahead.
-static_assert(kGramStages % kConsumers == 0 && kStagesBwd % kConsumers == 0, "stage ownership");
-static_assert(kGramStagesOf<float, true> % kConsumers == 0 && kStagesBwdOf<float, true> % kConsumers == 0, "stage ownership");
-
-struct TcBarriers {
-  uint64_t full[kMaxStages];       // TMA landed the stage                  (1 arrival + tx bytes)
-  uint64_t empty[kMaxStages];      // the owning warpgroup's MMAs are done  (one arrival per consumer warp)
-};
-
-// Tile range of this CTA inside its (domain, super-block) problem.
-struct TileRange {
-  int begin, end, PB;     // tiles [begin, end), pixel blocks per image
-  __device__ TileRange(const Geom& gm) {
-    PB = (gm.HW + kTilePx - 1) / kTilePx;
-    const long long T = (long long)gm.N * PB;
-    begin = (int)(T * blockIdx.x / gridDim.x);
-    end = (int)(T * (blockIdx.x + 1) / gridDim.x);
-  }
-};
+template <bool NHWC> constexpr int kPairStagesOf = NHWC ? 2 : 4;
 
 __device__ __forceinline__ float4 lds128(uint32_t addr) {
   float4 v;
@@ -142,18 +117,6 @@ __device__ __forceinline__ void sts128(uint32_t addr, float a, float b, float c,
   asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
 }
 
-template <class T>
-__device__ __forceinline__ float lds_nhwc(uint32_t addr) {
-  if constexpr (kBf16<T>) {
-    unsigned short u;
-    asm volatile("ld.shared.u16 %0, [%1];" : "=h"(u) : "r"(addr));
-    return __uint_as_float((uint32_t)u << 16);
-  } else {
-    float v;
-    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr));
-    return v;
-  }
-}
 // Pixels 4j .. 4j+3 of tile row `row` as fp32.  fp32: the 16-byte chunk q = 8 row + (j ^ (row & 7)) of the SWIZZLE_128B
 // tile.  bf16: 8 bytes at row * 64 + 8 j of the unswizzled box, widened (bf16 -> fp32 is exact: the high half of the word).
 // NHWC: channel `row` of pixels 4j .. 4j+3 of the landed [px][ch] tile, one load per pixel.
@@ -164,8 +127,8 @@ __device__ __forceinline__ float4 ld_px4(uint32_t tile, int q, int row, int j) {
     // 64).  Pixel 4j + k is row 4j + k; its 16-byte chunk holding channel `row` is c4 ^ (4 (j & 1) + k) = a ^ k.
     const int c4 = kBf16<T> ? row >> 3 : (row & 31) >> 2, a = c4 ^ ((j & 1) << 2);
     const uint32_t base = tile + 512u * j + (kBf16<T> ? 2u * (row & 7) : 4096u * (row >> 5) + 4u * (row & 3));
-    return make_float4(lds_nhwc<T>(base + (a << 4)), lds_nhwc<T>(base + 128u + ((a ^ 1) << 4)),
-                       lds_nhwc<T>(base + 256u + ((a ^ 2) << 4)), lds_nhwc<T>(base + 384u + ((a ^ 3) << 4)));
+    return make_float4(lds_f<T>(base + (a << 4)), lds_f<T>(base + 128u + ((a ^ 1) << 4)),
+                       lds_f<T>(base + 256u + ((a ^ 2) << 4)), lds_f<T>(base + 384u + ((a ^ 3) << 4)));
   } else if constexpr (kBf16<T>) {
     uint32_t a, b;
     asm volatile("ld.shared.v2.u32 {%0, %1}, [%2];" : "=r"(a), "=r"(b) : "r"(tile + 64u * row + 8u * j));
@@ -282,9 +245,92 @@ __device__ __forceinline__ void tma_tile(uint8_t* dst, const CUtensorMap* map, i
   }
 }
 
-__device__ __forceinline__ void init_ring(TcBarriers& bars, int stages) {
-  for (int s = 0; s < stages; ++s) { mbar_init(&bars.full[s], 1); mbar_init(&bars.empty[s], 4); }
-  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+// ---- the pipeline shared by the three kernels
+
+// TMA producer (one thread): tile it of the range goes to stage it % STAGES once the stage's previous phase is released;
+// issue(stage, px0, image, full barrier) issues the tile's `bytes`.
+template <int STAGES, class Issue>
+__device__ __forceinline__ void produce(Ring<STAGES>& ring, const TileRange<kTilePx>& tr, int img0, uint32_t bytes, Issue issue) {
+  int n = tr.begin / tr.PB, pb = tr.begin - n * tr.PB;
+  for (int it = 0; it < tr.end - tr.begin; ++it) {
+    const int s = it % STAGES;
+    mbar_wait_relaxed(&ring.empty[s], ((it / STAGES) & 1) ^ 1);
+    mbar_arrive_expect_tx(&ring.full[s], bytes);
+    issue(s, pb * kTilePx, img0 + n, &ring.full[s]);
+    if (++pb == tr.PB) { pb = 0; ++n; }
+  }
+}
+
+// The MMA chain of one tile: per 8-pixel k-step, D += A_p B_p^T for p = 0 .. N-1 (K-major descriptors of 32-pixel rows)
+template <int N> struct Products {
+  static constexpr int kN = N;
+  uint64_t a[N], b[N];
+};
+
+// One consumer warpgroup's tiles.  transform(stage address, px0) splits the landed stage into the operand tiles and
+// returns the tile's products; they go into a fresh accumulator (the first MMA overwrites it, see the file header) that
+// is then added into tot.  A STAGED stage is released as soon as the transform has read it; an in-place one (fp32 NCHW:
+// hi is written over the landed tile) only after the wait on the MMAs.  The operand tiles of a warpgroup are rewritten
+// by its next transform, hence the wait before it.
+template <bool STAGED, int STAGES, class Transform>
+__device__ __forceinline__ void consume(Ring<STAGES>& ring, const TileRange<kTilePx>& tr, uint32_t ring0, uint32_t stage_bytes,
+                                        float (&tot)[32], Transform transform) {
+  const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
+  float acc[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) acc[i] = 0.f;
+  for (int it = wg; it < tr.end - tr.begin; it += kConsumers) {
+    const int s = it % STAGES;
+    mbar_wait(&ring.full[s], (it / STAGES) & 1);
+    const int tl = tr.begin + it, n = tl / tr.PB, pb = tl - n * tr.PB;
+    const auto p = transform(ring0 + s * stage_bytes, pb * kTilePx);
+    if constexpr (STAGED) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&ring.empty[s]);
+    }
+    fence_proxy_async();
+    warpgroup_sync(wg);
+    wgmma_fence();
+    fence_operands(acc);
+#pragma unroll
+    for (int k = 0; k < kTilePx / 8; ++k)
+#pragma unroll
+      for (int q = 0; q < p.kN; ++q) {
+        if (k == 0 && q == 0) wgmma_m64n64k8_ss<false>(acc, p.a[0], p.b[0]);     // D = product: a fresh sum per tile
+        else wgmma_m64n64k8_ss(acc, p.a[q] + 2 * k, p.b[q] + 2 * k);
+      }
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_operands(acc);
+    if constexpr (!STAGED) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&ring.empty[s]);
+    }
+#pragma unroll
+    for (int i = 0; i < 32; ++i) tot[i] += acc[i];
+  }
+}
+
+// Epilogue (all threads, once every stage is consumed and the ring is free): both warpgroups' tot and, unless null,
+// row sums are added into a zeroed [64][P] matrix + [64] row sums over the ring; returns it complete.
+template <int P>
+__device__ __forceinline__ const float* cta_sums(uint8_t* smem, const float (&tot)[32], const float (*rowsum)[kPer]) {
+  const int tid = threadIdx.x;
+  float* s = reinterpret_cast<float*>(smem);
+  __syncthreads();
+  for (int e = tid; e < kTileCh * P + kTileCh; e += kTcThreads) s[e] = 0.f;
+  __syncthreads();
+  if (tid < 32 * kProducerWarp) {
+    add_fragment<8>(s, P, tot, tid >> 5, tid & 31);
+    if (rowsum) add_rowsums(s + kTileCh * P, *rowsum, tid & 127);
+  }
+  __syncthreads();
+  return s;
+}
+
+// this CTA's row of partial: [D][gridDim.y][gridDim.x][kNacc]
+__device__ __forceinline__ float* partial_row(float* partial) {
+  return partial + (((size_t)blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x) * kNacc;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -307,100 +353,55 @@ tc_contract_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_const
   constexpr int STAGES = kStagesBwdOf<T, NHWC>, BOX = kBoxBytes<T>;
   constexpr bool STAGED = kStaged<T, NHWC>;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  __shared__ TcBarriers bars;
+  uint8_t* smem = ring_smem(smem_raw);
+  __shared__ Ring<STAGES> ring;
   __shared__ float sShift[kTileCh], sK[kTileCh];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, tid = threadIdx.x;
-  const int sb = blockIdx.y, d = blockIdx.z;
+  const int tid = threadIdx.x, sb = blockIdx.y, d = blockIdx.z;
   const int ch0 = PAIR ? (2 * (sb >> 2) + ((sb >> 1) & 1)) * kTileCh : sb * kTileCh;     // dy channels
   const int chx = PAIR ? (2 * (sb >> 2) + (sb & 1)) * kTileCh : ch0;                    // x channels
-  const TileRange tr(gm);
-  const int ntiles = tr.end - tr.begin;
+  const TileRange<kTilePx> tr(gm);
 
-  if (tid == 0) init_ring(bars, STAGES);
+  if (tid == 0) ring.init();
   if (tid < kTileCh) sShift[tid] = chx + tid < gm.C ? save_mean[(size_t)d * gm.C + chx + tid] : 0.f;
   __syncthreads();
 
-  float acc[32], tot[32], rowsum[kPer], dummy[kPer];
+  float tot[32], rowsum[kPer], dummy[kPer];
 #pragma unroll
-  for (int i = 0; i < 32; ++i) { acc[i] = 0.f; tot[i] = 0.f; }
+  for (int i = 0; i < 32; ++i) tot[i] = 0.f;
 #pragma unroll
   for (int i = 0; i < kPer; ++i) { rowsum[i] = 0.f; dummy[i] = 0.f; }
 
-  if (warp == kProducerWarp) {
-    // ===== TMA producer =====
-    if (lane == 0) {
-      for (int it = 0; it < ntiles; ++it) {
-        const int s = it % STAGES;
-        mbar_wait_relaxed(&bars.empty[s], ((it / STAGES) & 1) ^ 1);
-        const int t = tr.begin + it, n = t / tr.PB, pb = t - n * tr.PB;
-        uint8_t* dst = smem + (size_t)s * 2 * BOX;
-        mbar_arrive_expect_tx(&bars.full[s], 2 * BOX);
-        tma_tile<T, NHWC>(dst, &map_x, chx, pb * kTilePx, d * gm.N + n, &bars.full[s]);
-        tma_tile<T, NHWC>(dst + BOX, &map_g, ch0, pb * kTilePx, d * gm.N + n, &bars.full[s]);
-      }
-    }
+  if (tid >> 5 == kProducerWarp) {
+    if ((tid & 31) == 0)
+      produce(ring, tr, d * gm.N, 2 * BOX, [&](int s, int px0, int img, uint64_t* bar) {
+        tma_tile<T, NHWC>(smem + (size_t)s * 2 * BOX, &map_x, chx, px0, img, bar);
+        tma_tile<T, NHWC>(smem + (size_t)s * 2 * BOX + BOX, &map_g, ch0, px0, img, bar);
+      });
   } else {
-    // ===== consumer warpgroups: split transforms, then D[64 x 64] = Eh Xh^T + El Xh^T + Eh Xl^T, sum += D =====
-    const int wg = warp >> 2, t = tid & 127;
     // dy's shift: its dependent loads overlap the producer's first TMA loads (named barrier 3: the consumers only)
     if (tid < kTileCh) sK[tid] = PILOT ? pilot_shift<T, NHWC>(dout, gm, d, ch0 + tid) : 0.f;          // 0 past C
     asm volatile("bar.sync 3, %0;" ::"n"(128 * kConsumers) : "memory");
     // per warpgroup behind the ring: the lo tiles of xc and dy (fp32 NCHW: hi in place), or hi and lo of both (bf16 / NHWC)
-    const uint32_t wgbuf = smem_u32(smem + (size_t)STAGES * 2 * BOX + (size_t)wg * (STAGED ? 4 : 2) * kTileBytes);
+    const int t = tid & 127;
+    const uint32_t wgbuf = smem_u32(smem + (size_t)STAGES * 2 * BOX + (size_t)(tid >> 7) * (STAGED ? 4 : 2) * kTileBytes);
     const uint32_t xlo = STAGED ? wgbuf + 2 * kTileBytes : wgbuf, dlo = xlo + kTileBytes;
-    for (int it = wg; it < ntiles; it += kConsumers) {
-      const int s = it % STAGES;
-      mbar_wait(&bars.full[s], (it / STAGES) & 1);
-      const int tl = tr.begin + it, n = tl / tr.PB, pb = tl - n * tr.PB;
-      const uint32_t tile = smem_u32(smem + (size_t)s * 2 * BOX);
+    consume<STAGED>(ring, tr, smem_u32(smem), 2 * BOX, tot, [&](uint32_t tile, int px0) {
       const uint32_t xhi = STAGED ? wgbuf : tile, dhi = STAGED ? wgbuf + kTileBytes : tile + kTileBytes;
-      split_transform<T, NHWC>(tile, xhi, xlo, t, sShift, pb * kTilePx, gm.HW, chx, gm.C, dummy);          // xc
-      split_transform<T, NHWC>(tile + BOX, dhi, dlo, t, sK, pb * kTilePx, gm.HW, ch0, gm.C, rowsum);    // dy - K
-      if constexpr (STAGED) {                      // the stage is read: it can be refilled while the MMAs run
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&bars.empty[s]);
-      }
-      fence_proxy_async();
-      warpgroup_sync(wg);
-      wgmma_fence();
-      fence_operands(acc);
-      const uint64_t xhdesc = make_kmajor_sw128_desc(xhi), dhdesc = make_kmajor_sw128_desc(dhi);
-      const uint64_t xldesc = make_kmajor_sw128_desc(xlo), dldesc = make_kmajor_sw128_desc(dlo);
-#pragma unroll
-      for (int k = 0; k < kTilePx / 8; ++k) {
-        if (k == 0) wgmma_m64n64k8_ss<false>(acc, dhdesc, xhdesc);           // D = product: a fresh sum per tile
-        else wgmma_m64n64k8_ss(acc, dhdesc + 2 * k, xhdesc + 2 * k);
-        wgmma_m64n64k8_ss(acc, dldesc + 2 * k, xhdesc + 2 * k);
-        wgmma_m64n64k8_ss(acc, dhdesc + 2 * k, xldesc + 2 * k);
-      }
-      wgmma_commit();
-      wgmma_wait<0>();                             // the lo (staged: and hi) tiles are rewritten by the next transform
-      fence_operands(acc);
-      if constexpr (!STAGED) {
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&bars.empty[s]);
-      }
-#pragma unroll
-      for (int i = 0; i < 32; ++i) tot[i] += acc[i];
-    }
+      split_transform<T, NHWC>(tile, xhi, xlo, t, sShift, px0, gm.HW, chx, gm.C, dummy);          // xc
+      split_transform<T, NHWC>(tile + BOX, dhi, dlo, t, sK, px0, gm.HW, ch0, gm.C, rowsum);      // dy - K
+      const uint64_t xh = make_kmajor_sw128_desc(xhi), dh = make_kmajor_sw128_desc(dhi);
+      const uint64_t xl = make_kmajor_sw128_desc(xlo), dl = make_kmajor_sw128_desc(dlo);
+      return Products<3>{{dh, dl, dh}, {xh, xh, xl}};
+    });
   }
 
-  // ===== epilogue: both warpgroups' sums + row sums (K folded back in) -> this CTA's partial row =====
-  __syncthreads();                                 // every stage consumed: the ring is free
-  float* sAcc = reinterpret_cast<float*>(smem);    // [64][64] + [64]
-  for (int e = tid; e < kNacc; e += kTcThreads) sAcc[e] = 0.f;
-  __syncthreads();
-  if (warp < kProducerWarp) {
-    add_fragment<8>(sAcc, kTileCh, tot, warp, lane);
-    add_rowsums(sAcc + kTileCh * kTileCh, rowsum, tid & 127);
-  }
-  __syncthreads();
+  // both warpgroups' sums + row sums (K folded back in) -> this CTA's partial row
+  const float* s = cta_sums<kTileCh>(smem, tot, &rowsum);
   // in-tensor pixels of the range: 32 per tile, less (PB * 32 - HW) for every last tile of an image in it
-  const int n_valid = ntiles * kTilePx - (tr.end / tr.PB - tr.begin / tr.PB) * (tr.PB * kTilePx - gm.HW);
-  float* prow = partial + (((size_t)d * gridDim.y + sb) * gridDim.x + blockIdx.x) * kNacc;
-  for (int e = tid; e < kTileCh * kTileCh; e += kTcThreads) prow[e] = sAcc[e];
-  if (tid < kTileCh) prow[kTileCh * kTileCh + tid] = fmaf((float)n_valid, sK[tid], sAcc[kTileCh * kTileCh + tid]);
+  const int n_valid = (tr.end - tr.begin) * kTilePx - (tr.end / tr.PB - tr.begin / tr.PB) * (tr.PB * kTilePx - gm.HW);
+  float* prow = partial_row(partial);
+  for (int e = tid; e < kTileCh * kTileCh; e += kTcThreads) prow[e] = s[e];
+  if (tid < kTileCh) prow[kTileCh * kTileCh + tid] = fmaf((float)n_valid, sK[tid], s[kTileCh * kTileCh + tid]);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -413,15 +414,13 @@ tc_gram_kernel(const __grid_constant__ CUtensorMap map_x, const T* __restrict__ 
   constexpr int STAGES = kGramStagesOf<T, NHWC>, BOX = kBoxBytes<T>;
   constexpr bool STAGED = kStaged<T, NHWC>;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  __shared__ TcBarriers bars;
+  uint8_t* smem = ring_smem(smem_raw);
+  __shared__ Ring<STAGES> ring;
   __shared__ float sShift[kTileCh];
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, tid = threadIdx.x;
-  const int sb = blockIdx.y, d = blockIdx.z, ch0 = sb * kTileCh;
-  const TileRange tr(gm);
-  const int ntiles = tr.end - tr.begin;
+  const int tid = threadIdx.x, sb = blockIdx.y, d = blockIdx.z, ch0 = sb * kTileCh;
+  const TileRange<kTilePx> tr(gm);
 
-  if (tid == 0) init_ring(bars, STAGES);
+  if (tid == 0) ring.init();
   if (tid < kTileCh) {
     const float sh = pilot_shift<T, NHWC>(x, gm, d, ch0 + tid);
     sShift[tid] = sh;
@@ -429,83 +428,40 @@ tc_gram_kernel(const __grid_constant__ CUtensorMap map_x, const T* __restrict__ 
   }
   __syncthreads();
 
-  float acc[32], tot[32], rowsum[kPer];
+  float tot[32], rowsum[kPer];
 #pragma unroll
-  for (int i = 0; i < 32; ++i) { acc[i] = 0.f; tot[i] = 0.f; }
+  for (int i = 0; i < 32; ++i) tot[i] = 0.f;
 #pragma unroll
   for (int i = 0; i < kPer; ++i) rowsum[i] = 0.f;
 
-  if (warp == kProducerWarp) {
-    // ===== TMA producer =====
-    if (lane == 0) {
-      int n = tr.begin / tr.PB, pb = tr.begin - n * tr.PB;
-      for (int it = 0; it < ntiles; ++it) {
-        const int s = it % STAGES;
-        mbar_wait_relaxed(&bars.empty[s], ((it / STAGES) & 1) ^ 1);
-        mbar_arrive_expect_tx(&bars.full[s], BOX);
-        tma_tile<T, NHWC>(smem + (size_t)s * BOX, &map_x, ch0, pb * kTilePx, d * gm.N + n, &bars.full[s]);
-        if (++pb == tr.PB) { pb = 0; ++n; }
-      }
-    }
+  if (tid >> 5 == kProducerWarp) {
+    if ((tid & 31) == 0)
+      produce(ring, tr, d * gm.N, BOX, [&](int s, int px0, int img, uint64_t* bar) {
+        tma_tile<T, NHWC>(smem + (size_t)s * BOX, &map_x, ch0, px0, img, bar);
+      });
   } else {
-    // ===== consumer warpgroups: D[64 x 64] = hi hi^T + (2 lo) hi^T per tile, sum += D =====
-    const int wg = warp >> 2, t = tid & 127;
     // per warpgroup behind the ring: the lo tile (fp32 NCHW), or the hi staging tile and the lo tile (bf16 / NHWC)
-    const uint32_t wgbuf = smem_u32(smem + (size_t)STAGES * BOX + (size_t)wg * (STAGED ? 2 : 1) * kTileBytes);
+    const int t = tid & 127;
+    const uint32_t wgbuf = smem_u32(smem + (size_t)STAGES * BOX + (size_t)(tid >> 7) * (STAGED ? 2 : 1) * kTileBytes);
     const uint32_t lo = STAGED ? wgbuf + kTileBytes : wgbuf;
     const uint64_t ldesc = make_kmajor_sw128_desc(lo);
-    for (int it = wg; it < ntiles; it += kConsumers) {
-      const int s = it % STAGES;
-      mbar_wait(&bars.full[s], (it / STAGES) & 1);
-      const int tl = tr.begin + it, n = tl / tr.PB, pb = tl - n * tr.PB;
-      const uint32_t tile = smem_u32(smem + (size_t)s * BOX);
+    consume<STAGED>(ring, tr, smem_u32(smem), BOX, tot, [&](uint32_t tile, int px0) {       // hi hi^T + (2 lo) hi^T
       const uint32_t hi = STAGED ? wgbuf : tile;
-      split_transform<T, NHWC, true>(tile, hi, lo, t, sShift, pb * kTilePx, gm.HW, ch0, gm.C, rowsum);
-      if constexpr (STAGED) {                    // the stage is read: it can be refilled while the MMAs run
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&bars.empty[s]);
-      }
-      fence_proxy_async();
-      warpgroup_sync(wg);
-      wgmma_fence();
-      fence_operands(acc);
+      split_transform<T, NHWC, true>(tile, hi, lo, t, sShift, px0, gm.HW, ch0, gm.C, rowsum);
       const uint64_t bdesc = make_kmajor_sw128_desc(hi);
-#pragma unroll
-      for (int k = 0; k < kTilePx / 8; ++k) {
-        if (k == 0) wgmma_m64n64k8_ss<false>(acc, bdesc, bdesc);             // D = product: a fresh sum per tile
-        else wgmma_m64n64k8_ss(acc, bdesc + 2 * k, bdesc + 2 * k);
-        wgmma_m64n64k8_ss(acc, ldesc + 2 * k, bdesc + 2 * k);
-      }
-      wgmma_commit();
-      wgmma_wait<0>();                             // the lo (staged: and hi) tile is rewritten by this warpgroup's next transform
-      fence_operands(acc);
-      if constexpr (!STAGED) {
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&bars.empty[s]);
-      }
-#pragma unroll
-      for (int i = 0; i < 32; ++i) tot[i] += acc[i];
-    }
+      return Products<2>{{bdesc, ldesc}, {bdesc, bdesc}};
+    });
   }
 
-  // ===== epilogue: both warpgroups' sums S = HH + 2 LH, G = (S + S^T) / 2 and the row sums -> this CTA's partial row =====
+  // both warpgroups' sums S = HH + 2 LH, G = (S + S^T) / 2 and the row sums -> this CTA's partial row
   constexpr int P = kTileCh + 1;                   // odd pitch: the transposed read is conflict-free
-  __syncthreads();                                 // every stage consumed: the ring is free
-  float* sS = reinterpret_cast<float*>(smem);      // [64][P]
-  float* sRS = sS + kTileCh * P;                   // [64]
-  for (int e = tid; e < kTileCh * P + kTileCh; e += kTcThreads) sS[e] = 0.f;
-  __syncthreads();
-  if (warp < kProducerWarp) {
-    add_fragment<8>(sS, P, tot, warp, lane);
-    add_rowsums(sRS, rowsum, tid & 127);
-  }
-  __syncthreads();
-  float* prow = partial + (((size_t)d * gridDim.y + sb) * gridDim.x + blockIdx.x) * kNacc;
+  const float* s = cta_sums<P>(smem, tot, &rowsum);
+  float* prow = partial_row(partial);
   for (int e = tid; e < kTileCh * kTileCh; e += kTcThreads) {
     const int r = e >> 6, c = e & 63;
-    prow[e] = 0.5f * (sS[r * P + c] + sS[c * P + r]);
+    prow[e] = 0.5f * (s[r * P + c] + s[c * P + r]);
   }
-  if (tid < kTileCh) prow[kTileCh * kTileCh + tid] = sRS[tid];
+  if (tid < kTileCh) prow[kTileCh * kTileCh + tid] = s[kTileCh * P + tid];
 }
 
 // ------------------------------------------------------------------------------------------
@@ -516,101 +472,55 @@ tc_gram_kernel(const __grid_constant__ CUtensorMap map_x, const T* __restrict__ 
 // transpose is needed off the diagonal), so registers stay below the diagonal kernel's.  Shared memory per CTA: NCHW
 // 4 stages x 16 KB + two lo tiles per warpgroup (hi in place) = 96 KB; NHWC 2 stages x 16 KB + hi and lo staging of
 // both tiles per warpgroup = 96 KB; two CTAs per SM either way.  The pilot shifts are the diagonal kernel's (shift).
-template <bool NHWC> constexpr int kPairStagesOf = NHWC ? 2 : 4;
-static_assert(kPairStagesOf<false> % kConsumers == 0 && kPairStagesOf<true> % kConsumers == 0, "stage ownership");
-
 template <bool NHWC>
 __global__ void __launch_bounds__(kTcThreads, 2)
 tc_gram_pair_kernel(const __grid_constant__ CUtensorMap map_x, const Geom gm, const float* __restrict__ shift,
                     float* __restrict__ partial) {
   constexpr int STAGES = kPairStagesOf<NHWC>, BOX = kTileBytes;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  __shared__ TcBarriers bars;
+  uint8_t* smem = ring_smem(smem_raw);
+  __shared__ Ring<STAGES> ring;
   __shared__ float sShift[2][kTileCh];             // [0] rows (super-block 2p + 1), [1] columns (super-block 2p)
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, tid = threadIdx.x;
-  const int p = blockIdx.y, d = blockIdx.z, SB = gm.C / kTileCh;
+  const int tid = threadIdx.x, p = blockIdx.y, d = blockIdx.z, SB = gm.C / kTileCh;
   const int chr = (2 * p + 1) * kTileCh, chc = 2 * p * kTileCh;
-  const TileRange tr(gm);
-  const int ntiles = tr.end - tr.begin;
+  const TileRange<kTilePx> tr(gm);
 
-  if (tid == 0) init_ring(bars, STAGES);
+  if (tid == 0) ring.init();
   if (tid < 2 * kTileCh) sShift[tid >> 6][tid & 63] = shift[((size_t)d * SB + 2 * p + 1 - (tid >> 6)) * kTileCh + (tid & 63)];
   __syncthreads();
 
-  float acc[32], tot[32];
+  float tot[32];
 #pragma unroll
-  for (int i = 0; i < 32; ++i) { acc[i] = 0.f; tot[i] = 0.f; }
+  for (int i = 0; i < 32; ++i) tot[i] = 0.f;
 
-  if (warp == kProducerWarp) {
-    // ===== TMA producer =====
-    if (lane == 0) {
-      int n = tr.begin / tr.PB, pb = tr.begin - n * tr.PB;
-      for (int it = 0; it < ntiles; ++it) {
-        const int s = it % STAGES;
-        mbar_wait_relaxed(&bars.empty[s], ((it / STAGES) & 1) ^ 1);
-        uint8_t* dst = smem + (size_t)s * 2 * BOX;
-        mbar_arrive_expect_tx(&bars.full[s], 2 * BOX);
-        tma_tile<float, NHWC>(dst, &map_x, chr, pb * kTilePx, d * gm.N + n, &bars.full[s]);
-        tma_tile<float, NHWC>(dst + BOX, &map_x, chc, pb * kTilePx, d * gm.N + n, &bars.full[s]);
-        if (++pb == tr.PB) { pb = 0; ++n; }
-      }
-    }
+  if (tid >> 5 == kProducerWarp) {
+    if ((tid & 31) == 0)
+      produce(ring, tr, d * gm.N, 2 * BOX, [&](int s, int px0, int img, uint64_t* bar) {
+        tma_tile<float, NHWC>(smem + (size_t)s * 2 * BOX, &map_x, chr, px0, img, bar);
+        tma_tile<float, NHWC>(smem + (size_t)s * 2 * BOX + BOX, &map_x, chc, px0, img, bar);
+      });
   } else {
-    // ===== consumer warpgroups: D[64 x 64] = h1 h0^T + l1 h0^T + h1 l0^T per tile, sum += D =====
-    const int wg = warp >> 2, t = tid & 127;
     // per warpgroup behind the ring: NCHW the lo tiles of rows and columns (hi in place); NHWC hi, lo of rows, hi, lo of columns
-    const uint32_t wgbuf = smem_u32(smem + (size_t)STAGES * 2 * BOX + (size_t)wg * (NHWC ? 4 : 2) * kTileBytes);
+    const int t = tid & 127;
+    const uint32_t wgbuf = smem_u32(smem + (size_t)STAGES * 2 * BOX + (size_t)(tid >> 7) * (NHWC ? 4 : 2) * kTileBytes);
     const uint32_t lo_r = NHWC ? wgbuf + kTileBytes : wgbuf, lo_c = NHWC ? wgbuf + 3 * kTileBytes : wgbuf + kTileBytes;
     float dummy[kPer];
 #pragma unroll
     for (int i = 0; i < kPer; ++i) dummy[i] = 0.f;
-    for (int it = wg; it < ntiles; it += kConsumers) {
-      const int s = it % STAGES;
-      mbar_wait(&bars.full[s], (it / STAGES) & 1);
-      const int tl = tr.begin + it, n = tl / tr.PB, pb = tl - n * tr.PB;
-      const uint32_t tile = smem_u32(smem + (size_t)s * 2 * BOX);
+    consume<NHWC>(ring, tr, smem_u32(smem), 2 * BOX, tot, [&](uint32_t tile, int px0) {      // h1 h0^T + l1 h0^T + h1 l0^T
       const uint32_t hi_r = NHWC ? wgbuf : tile, hi_c = NHWC ? wgbuf + 2 * kTileBytes : tile + BOX;
-      split_transform<float, NHWC>(tile, hi_r, lo_r, t, sShift[0], pb * kTilePx, gm.HW, chr, gm.C, dummy);
-      split_transform<float, NHWC>(tile + BOX, hi_c, lo_c, t, sShift[1], pb * kTilePx, gm.HW, chc, gm.C, dummy);
-      if constexpr (NHWC) {                        // the stage is read: it can be refilled while the MMAs run
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&bars.empty[s]);
-      }
-      fence_proxy_async();
-      warpgroup_sync(wg);
-      wgmma_fence();
-      fence_operands(acc);
+      split_transform<float, NHWC>(tile, hi_r, lo_r, t, sShift[0], px0, gm.HW, chr, gm.C, dummy);
+      split_transform<float, NHWC>(tile + BOX, hi_c, lo_c, t, sShift[1], px0, gm.HW, chc, gm.C, dummy);
       const uint64_t hr = make_kmajor_sw128_desc(hi_r), lr = make_kmajor_sw128_desc(lo_r);
       const uint64_t hc = make_kmajor_sw128_desc(hi_c), lc = make_kmajor_sw128_desc(lo_c);
-#pragma unroll
-      for (int k = 0; k < kTilePx / 8; ++k) {
-        if (k == 0) wgmma_m64n64k8_ss<false>(acc, hr, hc);                   // D = product: a fresh sum per tile
-        else wgmma_m64n64k8_ss(acc, hr + 2 * k, hc + 2 * k);
-        wgmma_m64n64k8_ss(acc, lr + 2 * k, hc + 2 * k);
-        wgmma_m64n64k8_ss(acc, hr + 2 * k, lc + 2 * k);
-      }
-      wgmma_commit();
-      wgmma_wait<0>();                             // the lo (NHWC: and hi) tiles are rewritten by the next transform
-      fence_operands(acc);
-      if constexpr (!NHWC) {
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&bars.empty[s]);
-      }
-#pragma unroll
-      for (int i = 0; i < 32; ++i) tot[i] += acc[i];
-    }
+      return Products<3>{{hr, lr, hr}, {hc, hc, lc}};
+    });
   }
 
-  // ===== epilogue: both warpgroups' sums -> this CTA's partial row (row-sum slots 0: the diagonal kernel has them) =====
-  __syncthreads();
-  float* sAcc = reinterpret_cast<float*>(smem);    // [64][64]
-  for (int e = tid; e < kTileCh * kTileCh; e += kTcThreads) sAcc[e] = 0.f;
-  __syncthreads();
-  if (warp < kProducerWarp) add_fragment<8>(sAcc, kTileCh, tot, warp, lane);
-  __syncthreads();
-  float* prow = partial + (((size_t)d * gridDim.y + p) * gridDim.x + blockIdx.x) * kNacc;
-  for (int e = tid; e < kNacc; e += kTcThreads) prow[e] = e < kTileCh * kTileCh ? sAcc[e] : 0.f;
+  // both warpgroups' sums -> this CTA's partial row; its row-sum slots stay 0 (the diagonal kernel has them)
+  const float* s = cta_sums<kTileCh>(smem, tot, nullptr);
+  float* prow = partial_row(partial);
+  for (int e = tid; e < kNacc; e += kTcThreads) prow[e] = s[e];
 }
 
 // ------------------------------------------------------------------------------------------
@@ -621,91 +531,34 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 EncodeTiledFn g_encode = nullptr;
 
-// fp32: 32 px x 64 ch boxes of 128-byte rows, SWIZZLE_128B (the wgmma operand layout).  bf16: 64-byte rows, no swizzle
-// (read by ld.shared only); TMA then needs HW % 8 == 0 for 16-byte strides.
-// nhwc: dims {C, HW, N*D}, boxes of 32 (fp32) or 64 (bf16) channels x 32 px, 128-byte rows, SWIZZLE_128B; the strides are
-// C and HW * C elements (16-byte multiples: C % 8 == 0 for every group size the tensor-core path takes).
-int make_map(CUtensorMap* map, const void* base, const Geom& gm, bool bf16, bool nhwc) {
-  const cuuint64_t es = bf16 ? 2 : 4;
-  const cuuint32_t estr[3] = {1, 1, 1};
-  const CUtensorMapDataType dt = bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
-  if (nhwc) {
-    const cuuint64_t dims[3] = {(cuuint64_t)gm.C, (cuuint64_t)gm.HW, (cuuint64_t)gm.N * gm.D};
-    const cuuint64_t strides[2] = {(cuuint64_t)gm.C * es, (cuuint64_t)gm.HW * gm.C * es};
-    const cuuint32_t box[3] = {bf16 ? 64u : 32u, kTilePx, 1};
-    return (int)g_encode(map, dt, 3, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  }
-  const cuuint64_t dims[3] = {(cuuint64_t)gm.HW, (cuuint64_t)gm.C, (cuuint64_t)gm.N * gm.D};
-  const cuuint64_t strides[2] = {(cuuint64_t)gm.HW * es, (cuuint64_t)gm.C * gm.HW * es};
-  const cuuint32_t box[3] = {kTilePx, kTileCh, 1};
-  return (int)g_encode(map, dt, 3, const_cast<void*>(base),
-                       dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                       bf16 ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-}
-
 // The ring + per-warpgroup fp32 tiles: Gram lo (bf16 / NHWC: + hi staging); contraction lo of xc and dy (bf16 / NHWC: +
 // hi staging of both).  97 KB per contraction CTA in every instantiation.
 template <class T, bool NHWC>
-size_t tc_smem_bytes(bool two) {
+constexpr size_t tc_smem_bytes(bool two) {
   constexpr bool staged = kStaged<T, NHWC>;
   return two ? (size_t)kStagesBwdOf<T, NHWC> * 2 * kBoxBytes<T> + (size_t)kConsumers * (staged ? 4 : 2) * kTileBytes + 1024
              : (size_t)kGramStagesOf<T, NHWC> * kBoxBytes<T> + (size_t)kConsumers * (staged ? 2 : 1) * kTileBytes + 1024;
 }
-
-template <class T, bool NHWC>
-cudaError_t tc_kernel_attrs() {
-  cudaError_t e = cudaFuncSetAttribute(tc_gram_kernel<T, NHWC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes<T, NHWC>(false));
-  if (e == cudaSuccess)
-    e = cudaFuncSetAttribute(tc_contract_kernel<T, NHWC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes<T, NHWC>(true));
-  // two ~73-97 KB CTAs per SM need the full shared-memory carve-out
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_gram_kernel<T, NHWC>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_contract_kernel<T, NHWC>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  if (e == cudaSuccess)
-    e = cudaFuncSetAttribute(tc_contract_kernel<T, NHWC, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes<T, NHWC>(true));
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_contract_kernel<T, NHWC, false, false>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  return e;
-}
-
-// group size 128 (fp32): the off-diagonal Gram kernel and the four-block contraction
-template <bool NHWC> size_t tc_pair_smem_bytes() {
+// group size 128 (fp32): the off-diagonal Gram kernel
+template <bool NHWC> constexpr size_t tc_pair_smem_bytes() {
   return (size_t)kPairStagesOf<NHWC> * 2 * kTileBytes + (size_t)kConsumers * (NHWC ? 4 : 2) * kTileBytes + 1024;
 }
 
-template <bool NHWC>
-cudaError_t tc_pair_attrs() {
-  cudaError_t e = cudaFuncSetAttribute(tc_gram_pair_kernel<NHWC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_pair_smem_bytes<NHWC>());
-  if (e == cudaSuccess)
-    e = cudaFuncSetAttribute(tc_contract_kernel<float, NHWC, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc_smem_bytes<float, NHWC>(true));
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_gram_pair_kernel<NHWC>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(tc_contract_kernel<float, NHWC, true>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  return e;
-}
-
-template <class T, bool NHWC>
-void launch_gram(const CUtensorMap& mx, const void* x, const Geom& gm, int nchunks, float* shift, float* partial, cudaStream_t st) {
-  dim3 grid(nchunks, tc_superblocks(gm), gm.D);
-  tc_gram_kernel<T, NHWC><<<grid, kTcThreads, tc_smem_bytes<T, NHWC>(false), st>>>(mx, static_cast<const T*>(x), gm, shift, partial);
-}
-
-template <class T, bool NHWC>
-void launch_contract(const CUtensorMap& mx, const CUtensorMap& mg, const void* dout, const Geom& gm, int nchunks,
-                     const float* save_mean, float* partial, cudaStream_t st, bool pilot) {
-  const T* g = static_cast<const T*>(dout);
-  if constexpr (!kBf16<T>) {
-    if (gm.GS == 2 * kTileCh) {                  // group size 128: the four 64 x 64 blocks of every group's R
-      dim3 grid(nchunks, 2 * tc_superblocks(gm), gm.D);
-      tc_contract_kernel<T, NHWC, true><<<grid, kTcThreads, tc_smem_bytes<T, NHWC>(true), st>>>(mx, mg, g, gm, save_mean, partial);
-      return;
-    }
-  }
-  dim3 grid(nchunks, tc_superblocks(gm), gm.D);
-  if (pilot) tc_contract_kernel<T, NHWC><<<grid, kTcThreads, tc_smem_bytes<T, NHWC>(true), st>>>(mx, mg, g, gm, save_mean, partial);
-  else tc_contract_kernel<T, NHWC, false, false><<<grid, kTcThreads, tc_smem_bytes<T, NHWC>(true), st>>>(mx, mg, g, gm, save_mean, partial);
-}
-
 }  // namespace
+
+int tc::make_map(CUtensorMap* map, const void* base, const Geom& gm, bool bf16, bool nhwc, bool apply_box) {
+  const cuuint64_t es = bf16 ? 2 : 4;
+  const cuuint32_t estr[3] = {1, 1, 1};
+  const cuuint64_t dims[3] = {(cuuint64_t)(nhwc ? gm.C : gm.HW), (cuuint64_t)(nhwc ? gm.HW : gm.C), (cuuint64_t)gm.N * gm.D};
+  const cuuint64_t strides[2] = {(cuuint64_t)dims[0] * es, (cuuint64_t)gm.C * gm.HW * es};
+  const cuuint32_t box[3] = {nhwc ? (bf16 ? 64u : 32u) : (bf16 && apply_box ? 64u : (cuuint32_t)kTilePx),
+                             nhwc ? (cuuint32_t)kTilePx : (cuuint32_t)kTileCh, 1};
+  const bool swizzle = nhwc || !bf16 || apply_box;
+  return (int)g_encode(map, bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3,
+                       const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                       swizzle ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+}
 
 int tc_init() {
   void* fn = nullptr;
@@ -713,15 +566,27 @@ int tc_init() {
   cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q);
   if (e != cudaSuccess || fn == nullptr || q != cudaDriverEntryPointSuccess) return e == cudaSuccess ? -1 : (int)e;
   g_encode = reinterpret_cast<EncodeTiledFn>(fn);
-  e = tc_kernel_attrs<float, false>();
-  if (e == cudaSuccess) e = tc_kernel_attrs<__nv_bfloat16, false>();
-  if (e == cudaSuccess) e = tc_kernel_attrs<float, true>();
-  if (e == cudaSuccess) e = tc_kernel_attrs<__nv_bfloat16, true>();
-  if (e == cudaSuccess) e = tc_pair_attrs<false>();
-  if (e == cudaSuccess) e = tc_pair_attrs<true>();
-  if (e == cudaSuccess) e = (cudaError_t)dense_init();
-  if (e == cudaSuccess) return tc_apply_init();
-  return (int)e;
+  using bf16 = __nv_bfloat16;
+  const KernelSmem kernels[] = {
+      {(const void*)tc_gram_kernel<float, false>, tc_smem_bytes<float, false>(false)},
+      {(const void*)tc_gram_kernel<bf16, false>, tc_smem_bytes<bf16, false>(false)},
+      {(const void*)tc_gram_kernel<float, true>, tc_smem_bytes<float, true>(false)},
+      {(const void*)tc_gram_kernel<bf16, true>, tc_smem_bytes<bf16, true>(false)},
+      {(const void*)tc_contract_kernel<float, false>, tc_smem_bytes<float, false>(true)},
+      {(const void*)tc_contract_kernel<bf16, false>, tc_smem_bytes<bf16, false>(true)},
+      {(const void*)tc_contract_kernel<float, true>, tc_smem_bytes<float, true>(true)},
+      {(const void*)tc_contract_kernel<bf16, true>, tc_smem_bytes<bf16, true>(true)},
+      {(const void*)tc_contract_kernel<float, false, false, false>, tc_smem_bytes<float, false>(true)},
+      {(const void*)tc_contract_kernel<bf16, false, false, false>, tc_smem_bytes<bf16, false>(true)},
+      {(const void*)tc_contract_kernel<float, true, false, false>, tc_smem_bytes<float, true>(true)},
+      {(const void*)tc_contract_kernel<bf16, true, false, false>, tc_smem_bytes<bf16, true>(true)},
+      {(const void*)tc_contract_kernel<float, false, true>, tc_smem_bytes<float, false>(true)},
+      {(const void*)tc_contract_kernel<float, true, true>, tc_smem_bytes<float, true>(true)},
+      {(const void*)tc_gram_pair_kernel<false>, tc_pair_smem_bytes<false>()},
+      {(const void*)tc_gram_pair_kernel<true>, tc_pair_smem_bytes<true>()}};
+  if (int rc = opt_in(kernels)) return rc;
+  if (int rc = dense_init()) return rc;
+  return tc_apply_init();
 }
 
 // The TMA/wgmma contraction takes group sizes that tile a 64-channel super-block or span two of them (128), rows
@@ -741,13 +606,12 @@ int tc_stats(const void* x, bool bf16, bool nhwc, const Geom& gm, int nchunks, f
   CUtensorMap mx;
   bind_context();
   if (int rc = make_map(&mx, x, gm, bf16, nhwc)) return rc;
-  if (nhwc) {
-    if (bf16) launch_gram<__nv_bfloat16, true>(mx, x, gm, nchunks, shift, partial, st);
-    else launch_gram<float, true>(mx, x, gm, nchunks, shift, partial, st);
-  } else {
-    if (bf16) launch_gram<__nv_bfloat16, false>(mx, x, gm, nchunks, shift, partial, st);
-    else launch_gram<float, false>(mx, x, gm, nchunks, shift, partial, st);
-  }
+  const dim3 grid(nchunks, tc_superblocks(gm), gm.D);
+  dispatch(bf16, nhwc, [&](auto t, auto layout) {
+    using T = decltype(t);
+    constexpr bool NHWC = decltype(layout)::value;
+    tc_gram_kernel<T, NHWC><<<grid, kTcThreads, tc_smem_bytes<T, NHWC>(false), st>>>(mx, static_cast<const T*>(x), gm, shift, partial);
+  });
   return 0;
 }
 
@@ -769,13 +633,22 @@ int tc_bwd_reduce(const void* x, const void* dout, bool bf16, bool nhwc, const G
   bind_context();
   if (int rc = make_map(&mx, x, gm, bf16, nhwc)) return rc;
   if (int rc = make_map(&mg, dout, gm, bf16, nhwc)) return rc;
-  if (nhwc) {
-    if (bf16) launch_contract<__nv_bfloat16, true>(mx, mg, dout, gm, nchunks, save_mean, partial, st, pilot);
-    else launch_contract<float, true>(mx, mg, dout, gm, nchunks, save_mean, partial, st, pilot);
-  } else {
-    if (bf16) launch_contract<__nv_bfloat16, false>(mx, mg, dout, gm, nchunks, save_mean, partial, st, pilot);
-    else launch_contract<float, false>(mx, mg, dout, gm, nchunks, save_mean, partial, st, pilot);
-  }
+  dispatch(bf16, nhwc, [&](auto t, auto layout) {
+    using T = decltype(t);
+    constexpr bool NHWC = decltype(layout)::value;
+    constexpr size_t smem = tc_smem_bytes<T, NHWC>(true);
+    const T* g = static_cast<const T*>(dout);
+    dim3 grid(nchunks, tc_superblocks(gm), gm.D);
+    if constexpr (!kBf16<T>) {
+      if (gm.GS == 2 * kTileCh) {                // group size 128: the four 64 x 64 blocks of every group's R
+        grid.y *= 2;
+        tc_contract_kernel<T, NHWC, true><<<grid, kTcThreads, smem, st>>>(mx, mg, g, gm, save_mean, partial);
+        return;
+      }
+    }
+    if (pilot) tc_contract_kernel<T, NHWC><<<grid, kTcThreads, smem, st>>>(mx, mg, g, gm, save_mean, partial);
+    else tc_contract_kernel<T, NHWC, false, false><<<grid, kTcThreads, smem, st>>>(mx, mg, g, gm, save_mean, partial);
+  });
   return 0;
 }
 

@@ -63,25 +63,6 @@ __device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* map, i
   asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
                ::"r"(smem_u32(dst)), "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(smem_u32(bar)) : "memory");
 }
-// same, with an L2 eviction-priority hint (policy from l2_policy_evict_first(): the tile is read exactly once)
-__device__ __forceinline__ void tma_load_3d_hint(void* dst, const CUtensorMap* map, int c0, int c1, int c2, uint64_t* bar,
-                                                 uint64_t policy) {
-  asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%2, %3, %4}], [%5], %6;"
-               ::"r"(smem_u32(dst)), "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(smem_u32(bar)), "l"(policy) : "memory");
-}
-// shared -> global tile store (bulk async group of the issuing thread)
-__device__ __forceinline__ void tma_store_3d(const CUtensorMap* map, const void* src, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
-               ::"l"(map), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-__device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
-__device__ __forceinline__ uint64_t l2_policy_evict_first() {
-  uint64_t p;
-  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
-  return p;
-}
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ---- warpgroup MMA (wgmma, sm_90a): issued by all 128 threads of an aligned warpgroup, fp32 accumulator in registers
@@ -131,7 +112,6 @@ constexpr uint32_t kTf32Mask = 0xFFFFE000u;     // sign, exponent and the 10 man
 __device__ __forceinline__ float round_tf32(float v) {
   return __uint_as_float((__float_as_uint(v) + 0x1000u) & 0xFFFFE000u);
 }
-
 
 }  // namespace tc
 }  // namespace dwt
