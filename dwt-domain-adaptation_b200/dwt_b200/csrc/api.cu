@@ -837,7 +837,8 @@ int tail2_bwd(int kind, const dwt_tail_site* s, const float* dout, const float* 
   return check_launch("channels-last two-site backward apply kernel");
 }
 
-// ---- per-image whitening: instance (dwt_whiten_instance_*) and switchable (dwt_whiten_switch_*) -----------------------
+// ---- per-image whitening: instance (dwt_whiten_instance_*), switchable (dwt_whiten_switch_*) and latent-domain
+// (dwt_whiten_latent_*) ------------------------------------------------------------------------------------------------
 // Every image is its own problem.  The tensor-core kernels index their problems by (domain, super-block) and the dense
 // ones by (domain, group); per-image whitening runs them with the images as the domains: Geom D = N images of N = 1 each,
 // M = HW.  Statistics and the backward contraction are tc_stats / tc_bwd_reduce unchanged (tc_chunks splits an image over
@@ -850,17 +851,25 @@ int tail2_bwd(int kind, const dwt_tail_site* s, const float* dout, const float* 
 //               pass over x) -> sw_fwd_factor (mix, Cholesky + inverse, EMA); backward tc_bwd_reduce about the mixed mean
 //               without the pilot centring (sum (x - m) is not zero) -> sw_bwd_coef / sw_bwd_sum / sw_dmix /
 //               sw_bwd_apply_coef -> tc_bwd_apply centred on the images' own means, the per-image constant of dx in dybar.
-// What a switchable call adds to an instance call (Mix{} is instance whitening)
+//   latent      forward ld_stats (save_stats: per-image rows, each latent domain's weighted moments by the law of total
+//               covariance, s_k) -> ld_fwd_factor (W_k per (domain, group), EMA) -> ld_mix (A_n = sum_k w_nk W_k and m~_n);
+//               backward as switchable: tc_bwd_reduce about m~_n without the pilot -> ld_bwd_sum / ld_bwd_dom (per domain)
+//               / ld_bwd_coef (per image) / ld_dw -> tc_bwd_apply centred on the images' own means.
+// What a switchable or latent-domain call adds to an instance call (Mix{} is instance whitening)
+enum MixKind { MIX_INSTANCE = 0, MIX_SWITCH = 1, MIX_LATENT = 2 };
 struct Mix {
-  bool on = false;
-  const float* mix = nullptr;          // [6]
-  const float* save_stats = nullptr;   // [N + 1][G][gs*gs + gs], written by the forward
+  int kind = MIX_INSTANCE;
+  const float* mix = nullptr;          // switchable: [6];  latent: weights [N][K]
+  const float* save_stats = nullptr;   // switchable: [N + 1][G][gs*gs + gs];  latent: dwt_b200.h.  Written by the forward
+  int K = 0;                           // latent: domains
   float momentum = 0.f;
   int update_running = 0;
-  float* rmean = nullptr;              // [C], [G][gs][gs]
+  float* rmean = nullptr;              // switchable: [C], [G][gs][gs];  latent: [K][C], [K][G][gs][gs]
   float* rcov = nullptr;
-  float* dmix = nullptr;               // backward: [6] or null
-  const char* what() const { return on ? "switchable whitening" : "instance whitening"; }
+  float* dmix = nullptr;               // backward: switchable [6], latent dweights [N][K], or null
+  const char* what() const {
+    return kind == MIX_LATENT ? "latent-domain whitening" : kind == MIX_SWITCH ? "switchable whitening" : "instance whitening";
+  }
 };
 
 int image_refuse(int64_t N, int64_t C, int64_t HW, int GS, int flags, const char* what) {
@@ -869,11 +878,14 @@ int image_refuse(int64_t N, int64_t C, int64_t HW, int GS, int flags, const char
               "(C=%lld HW=%lld N=%lld gs=%d flags=%#x)", what, (long long)C, (long long)HW, (long long)N, GS, flags);
 }
 
-// flags (switchable: the mode word, which may also hold DWT_MODE_EVAL) and geometry; fills gm (no device call)
+// flags (switchable, latent: the mode word, which may also hold DWT_MODE_EVAL) and geometry; fills gm (no device call)
 int image_geom(dwt::Geom& gm, int64_t N, int64_t C, int64_t HW, int GS, int flags, const Mix& m) {
-  if (m.on && (flags & ~(DWT_MODE_EVAL | DWT_LAYOUT_NHWC | DWT_DTYPE_BF16)))
+  const bool on = m.kind != MIX_INSTANCE;
+  if (m.kind == MIX_LATENT && (m.K < 1 || m.K > DWT_MAX_LATENT_DOMAINS))
+    return fail(DWT_E_INVALID, "n_domains %d outside [1,%d] (latent-domain whitening)", m.K, DWT_MAX_LATENT_DOMAINS);
+  if (on && (flags & ~(DWT_MODE_EVAL | DWT_LAYOUT_NHWC | DWT_DTYPE_BF16)))
     return fail(DWT_E_INVALID, "bad mode %#x (DWT_MODE_TRAIN or DWT_MODE_EVAL | DWT_LAYOUT_NHWC | DWT_DTYPE_BF16)", flags);
-  if (!m.on && (flags & ~(DWT_LAYOUT_NHWC | DWT_DTYPE_BF16)))
+  if (!on && (flags & ~(DWT_LAYOUT_NHWC | DWT_DTYPE_BF16)))
     return fail(DWT_E_INVALID, "bad flags %#x (DWT_LAYOUT_NHWC | DWT_DTYPE_BF16)", flags);
   flags &= ~DWT_MODE_EVAL;
   if (N <= 0 || C <= 0 || HW <= 0) return fail(DWT_E_INVALID, "empty tensor (N=%lld C=%lld HW=%lld)", (long long)N,
@@ -891,15 +903,17 @@ int image_geom(dwt::Geom& gm, int64_t N, int64_t C, int64_t HW, int GS, int flag
 
 struct ImageWork {
   Workspace w;
-  float* pd;       // switchable: [N][G][gs*gs + gs]  P_n | dm_n
-  float* part;     //             [N][G][8]           dmix terms per (image, group)
-  float* sums;     //             [G][gs*gs + gs]     sum_n P_n | sum_n dm_n
+  float* pd;       // switchable: [N][G][gs*gs + gs]  P_n | dm_n;         latent: [K][G][gs*gs + gs]  P_k | mubar_k
+  float* part;     //             [N][G][8]           dmix terms per (image, group);  latent: [N][G][kLdMaxDomains] dweights terms
+  float* sums;     //             [G][gs*gs + gs]     sum_n P_n | sum_n dm_n;  latent: [K][G][gs*gs + gs]  Wbar_k | sum w g
   float* mu;       //             [N][C]              the images' own means (the backward apply's centre)
+  float* pc;       // latent:     [K][G]              <P_k, Sigma_k>
 };
 
 // Scratch behind the common head (the status word is shared with every other call on the stream's workspace):
 // partials [N][SB][nchunks][64*64+64], reduced moments (only when nchunks > 1), pilot shifts / mean of dy / dybar
-// [N][SB][64], backward coefficients [N][G][2 gs^2 + gs]; switchable whitening then pd, part, sums and mu
+// [N][SB][64], backward coefficients [N][G][2 gs^2 + gs]; switchable and latent-domain whitening then pd, part, sums
+// and mu (latent: and pc)
 ImageWork carve_image(void* base, const dwt::Geom& gm, const Mix& m) {
   const size_t P = (size_t)dwt::tc_superblocks(gm) * gm.D, nacc = 64 * 64 + 64;
   const size_t rec = (size_t)gm.GS * gm.GS + gm.GS, PG = (size_t)gm.D * gm.G;
@@ -916,11 +930,18 @@ ImageWork carve_image(void* base, const dwt::Geom& gm, const Mix& m) {
   w.gram = gm.nchunks > 1 ? reinterpret_cast<float*>(b + take(sizeof(float) * P * nacc)) : w.partial;
   w.shift = reinterpret_cast<float*>(b + take(sizeof(float) * P * 64));
   w.coef = reinterpret_cast<float*>(b + take(sizeof(float) * PG * dwt::coef_stride(gm.GS)));
-  if (m.on) {
+  if (m.kind == MIX_SWITCH) {
     s.pd = reinterpret_cast<float*>(b + take(sizeof(float) * PG * rec));
     s.part = reinterpret_cast<float*>(b + take(sizeof(float) * PG * 8));
     s.sums = reinterpret_cast<float*>(b + take(sizeof(float) * gm.G * rec));
     s.mu = reinterpret_cast<float*>(b + take(sizeof(float) * (size_t)gm.D * gm.C));
+  } else if (m.kind == MIX_LATENT) {
+    const size_t KG = (size_t)m.K * gm.G;
+    s.pd = reinterpret_cast<float*>(b + take(sizeof(float) * KG * rec));
+    s.part = reinterpret_cast<float*>(b + take(sizeof(float) * PG * dwt::kLdMaxDomains));
+    s.sums = reinterpret_cast<float*>(b + take(sizeof(float) * KG * rec));
+    s.mu = reinterpret_cast<float*>(b + take(sizeof(float) * (size_t)gm.D * gm.C));
+    s.pc = reinterpret_cast<float*>(b + take(sizeof(float) * KG));
   }
   w.bytes = off;
   return s;
@@ -936,9 +957,9 @@ size_t image_workspace_bytes(int64_t N, int64_t C, int64_t HW, int GS, const Mix
   return rc ? 0 : carve_image(nullptr, gm, m).w.bytes;
 }
 
-// Profile family of a launch: [switchable][pass][channels-last * 2 + bf16]
+// Profile family of a launch: [MixKind][pass][channels-last * 2 + bf16]
 enum ImagePass { I_STATS, I_FWD_FINALIZE, I_APPLY, I_BWD_REDUCE, I_BWD_FINALIZE, I_BWD_APPLY };
-const char* const kImageName[2][6][4] = {
+const char* const kImageName[3][6][4] = {
     {{"iw_stats", "iw_stats_bf16", "iw_stats_nhwc", "iw_stats_nhwc_bf16"},
      {"iw_fwd_finalize", "iw_fwd_finalize_bf16", "iw_fwd_finalize", "iw_fwd_finalize_bf16"},
      {"iw_apply", "iw_apply_bf16", "iw_apply_nhwc", "iw_apply_nhwc_bf16"},
@@ -950,21 +971,29 @@ const char* const kImageName[2][6][4] = {
      {"sw_apply", "sw_apply_bf16", "sw_apply_nhwc", "sw_apply_nhwc_bf16"},
      {"sw_bwd_reduce", "sw_bwd_reduce_bf16", "sw_bwd_reduce_nhwc", "sw_bwd_reduce_nhwc_bf16"},
      {"sw_bwd_finalize", "sw_bwd_finalize_bf16", "sw_bwd_finalize", "sw_bwd_finalize_bf16"},
-     {"sw_bwd_apply", "sw_bwd_apply_bf16", "sw_bwd_apply_nhwc", "sw_bwd_apply_nhwc_bf16"}}};
+     {"sw_bwd_apply", "sw_bwd_apply_bf16", "sw_bwd_apply_nhwc", "sw_bwd_apply_nhwc_bf16"}},
+    {{"ld_stats", "ld_stats_bf16", "ld_stats_nhwc", "ld_stats_nhwc_bf16"},
+     {"ld_fwd_finalize", "ld_fwd_finalize_bf16", "ld_fwd_finalize", "ld_fwd_finalize_bf16"},
+     {"ld_apply", "ld_apply_bf16", "ld_apply_nhwc", "ld_apply_nhwc_bf16"},
+     {"ld_bwd_reduce", "ld_bwd_reduce_bf16", "ld_bwd_reduce_nhwc", "ld_bwd_reduce_nhwc_bf16"},
+     {"ld_bwd_finalize", "ld_bwd_finalize_bf16", "ld_bwd_finalize", "ld_bwd_finalize_bf16"},
+     {"ld_bwd_apply", "ld_bwd_apply_bf16", "ld_bwd_apply_nhwc", "ld_bwd_apply_nhwc_bf16"}}};
 
-// The checks both directions make, in order: flags and geometry, pointers, running buffers (switchable forward),
+// The checks both directions make, in order: flags and geometry, pointers, running buffers (switchable, latent forward),
 // alignment, workspace, kernel set-up.  in0, in1: what the kernels read (x; x and dout); out: what they write (y; dx).
 int image_validate(dwt::Geom& gm, ImageWork& s, const Mix& m, const void* in0, const void* in1, const void* out, int64_t N,
                    int64_t C, int64_t HW, int GS, int flags, const float* save_mean, const float* save_w, void* ws,
                    size_t ws_bytes, bool running_missing = false) {
   if (int rc = image_geom(gm, N, C, HW, GS, flags, m)) return rc;
-  if (!in0 || !in1 || !out || !save_mean || !save_w || !ws || (m.on && (!m.mix || !m.save_stats)))
+  const bool on = m.kind != MIX_INSTANCE;
+  if (!in0 || !in1 || !out || !save_mean || !save_w || !ws || (on && (!m.mix || !m.save_stats)))
     return fail(DWT_E_INVALID, "null pointer argument");
   if (running_missing) return fail(DWT_E_INVALID, "running buffer is null (eval, or train with update_running)");
   // instance whitening: mix and save_stats are null
   if (((uintptr_t)in0 | (uintptr_t)in1 | (uintptr_t)out | (uintptr_t)save_w | (uintptr_t)m.save_stats | (uintptr_t)m.mix) % 16 != 0)
-    return m.on ? fail(DWT_E_INVALID, "activation tensors, mix, save_w and save_stats must be 16-byte aligned (switchable whitening)")
-                : fail(DWT_E_INVALID, "activation tensors and save_w must be 16-byte aligned (instance whitening: TMA and vector stores)");
+    return m.kind == MIX_LATENT ? fail(DWT_E_INVALID, "activation tensors, weights, save_w and save_stats must be 16-byte aligned (latent-domain whitening)")
+         : on ? fail(DWT_E_INVALID, "activation tensors, mix, save_w and save_stats must be 16-byte aligned (switchable whitening)")
+              : fail(DWT_E_INVALID, "activation tensors and save_w must be 16-byte aligned (instance whitening: TMA and vector stores)");
   s = carve_image(ws, gm, m);
   if (s.w.bytes > ws_bytes) return fail(DWT_E_WORKSPACE, "workspace too small: need %zu bytes, got %zu", s.w.bytes, ws_bytes);
   if ((uintptr_t)ws % 256 != 0) return fail(DWT_E_WORKSPACE, "workspace must be 256-byte aligned");
@@ -981,27 +1010,40 @@ dwt::SwFin make_sw_fin(int mode, float eps, const Mix& m, const float* save_mean
   return f;
 }
 
+dwt::LdFin make_ld_fin(int mode, float eps, const Mix& m, const float* save_mean, const float* save_w, int* status) {
+  dwt::LdFin f{};
+  f.a = 1.f - eps; f.b = eps; f.train = (mode & DWT_MODE_EVAL) == 0; f.K = m.K; f.weights = m.mix;
+  f.momentum = m.momentum; f.update_running = f.train && m.update_running; f.rmean = m.rmean; f.rcov = m.rcov;
+  f.save_mean = const_cast<float*>(save_mean); f.save_w = const_cast<float*>(save_w);
+  f.save_stats = const_cast<float*>(m.save_stats); f.status = status;
+  return f;
+}
+
 int image_fwd(const Mix& m, const void* x, void* y, int64_t N, int64_t C, int64_t HW, int GS, int flags, float eps,
               float* save_mean, float* save_w, void* ws, size_t ws_bytes, cudaStream_t st) {
   dwt::Geom gm;
   ImageWork s;
   const bool train = (flags & DWT_MODE_EVAL) == 0;
-  const bool running_missing = m.on && (!train || m.update_running) && (!m.rmean || !m.rcov);
+  const bool running_missing = m.kind != MIX_INSTANCE && (!train || m.update_running) && (!m.rmean || !m.rcov);
   if (int rc = image_validate(gm, s, m, x, x, y, N, C, HW, GS, flags, save_mean, save_w, ws, ws_bytes, running_missing))
     return rc;
   const bool nhwc = (flags & DWT_LAYOUT_NHWC) != 0, bf16 = (flags & DWT_DTYPE_BF16) != 0;
   const int k = 2 * nhwc + bf16;
   const double E = (bf16 ? 2.0 : 4.0) * (double)N * (double)C * (double)HW;
   {
-    Launch l(kImageName[m.on][I_STATS][k], &gm, E, st);
+    Launch l(kImageName[m.kind][I_STATS][k], &gm, E, st);
     if (int cr = dwt::tc_stats(x, bf16, nhwc, gm, gm.nchunks, s.w.shift, s.w.partial, st))
       return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d) x=%p N=%lld C=%d HW=%d", cr, x, (long long)N, gm.C, gm.HW);
   }
   if (int rc = check_launch("%s statistics kernel", m.what())) return rc;
   {
-    Launch l(kImageName[m.on][I_FWD_FINALIZE][k], &gm, 0.0, st);
+    Launch l(kImageName[m.kind][I_FWD_FINALIZE][k], &gm, 0.0, st);
     if (gm.nchunks > 1) dwt::dense_partial_reduce(s.w.partial, gm.nchunks, dwt::tc_superblocks(gm) * gm.D, s.w.gram, st);
-    if (m.on) {
+    if (m.kind == MIX_LATENT) {
+      const dwt::LdFin fin = make_ld_fin(flags, eps, m, save_mean, save_w, s.w.status);
+      dwt::dense_ld_stats(s.w.gram, s.w.shift, gm, fin, st);
+      dwt::dense_ld_fwd(gm, fin, st);
+    } else if (m.kind == MIX_SWITCH) {
       dwt::SwFin fin = make_sw_fin(flags, eps, m, save_mean, save_w, s.w.status);
       fin.momentum = m.momentum; fin.update_running = train && m.update_running;
       fin.rmean = m.rmean; fin.rcov = m.rcov;
@@ -1015,7 +1057,7 @@ int image_fwd(const Mix& m, const void* x, void* y, int64_t N, int64_t C, int64_
   }
   if (int rc = check_launch("%s finalize kernel", m.what())) return rc;
   {
-    Launch l(kImageName[m.on][I_APPLY][k], &gm, 2.0 * E, st);
+    Launch l(kImageName[m.kind][I_APPLY][k], &gm, 2.0 * E, st);
     if (int cr = dwt::tc_apply(x, y, bf16, nhwc, gm, tc_apply_ctas(gm, 1, 64), save_mean, save_w, st))
       return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d)", cr);
   }
@@ -1031,16 +1073,19 @@ int image_bwd(const Mix& m, const void* x, const void* dout, void* dx, int64_t N
   const int k = 2 * nhwc + bf16;
   const double E = (bf16 ? 2.0 : 4.0) * (double)N * (double)C * (double)HW;
   {
-    Launch l(kImageName[m.on][I_BWD_REDUCE][k], &gm, 2.0 * E, st);
-    if (int cr = dwt::tc_bwd_reduce(x, dout, bf16, nhwc, gm, gm.nchunks, save_mean, s.w.partial, st, /*pilot=*/!m.on))
+    Launch l(kImageName[m.kind][I_BWD_REDUCE][k], &gm, 2.0 * E, st);
+    if (int cr = dwt::tc_bwd_reduce(x, dout, bf16, nhwc, gm, gm.nchunks, save_mean, s.w.partial, st, /*pilot=*/m.kind == MIX_INSTANCE))
       return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d) x=%p dout=%p N=%lld C=%d HW=%d", cr, x, dout,
                   (long long)N, gm.C, gm.HW);
   }
   if (int rc = check_launch("%s backward reduction kernel", m.what())) return rc;
   {
-    Launch l(kImageName[m.on][I_BWD_FINALIZE][k], &gm, 0.0, st);
+    Launch l(kImageName[m.kind][I_BWD_FINALIZE][k], &gm, 0.0, st);
     if (gm.nchunks > 1) dwt::dense_partial_reduce(s.w.partial, gm.nchunks, dwt::tc_superblocks(gm) * gm.D, s.w.gram, st);
-    if (m.on) {
+    if (m.kind == MIX_LATENT) {
+      const dwt::LdFin fin = make_ld_fin(flags, eps, m, save_mean, save_w, s.w.status);
+      dwt::dense_ld_bwd(s.w.gram, gm, fin, s.sums, s.pd, s.pc, s.part, m.dmix, s.w.coef, s.w.shift, s.mu, st);
+    } else if (m.kind == MIX_SWITCH) {
       const dwt::SwFin fin = make_sw_fin(flags, eps, m, save_mean, save_w, s.w.status);
       dwt::dense_sw_bwd(s.w.gram, gm, fin, s.pd, s.part, s.sums, m.dmix, s.w.coef, s.w.shift, s.mu, st);
     } else {
@@ -1051,8 +1096,9 @@ int image_bwd(const Mix& m, const void* x, const void* dout, void* dx, int64_t N
   }
   if (int rc = check_launch("%s backward finalize kernel", m.what())) return rc;
   {
-    Launch l(kImageName[m.on][I_BWD_APPLY][k], &gm, 3.0 * E, st);
-    if (int cr = dwt::tc_bwd_apply(x, dout, dx, bf16, nhwc, gm, tc_apply_ctas(gm, 1, 64), s.w.coef, m.on ? s.mu : save_mean,
+    Launch l(kImageName[m.kind][I_BWD_APPLY][k], &gm, 3.0 * E, st);
+    if (int cr = dwt::tc_bwd_apply(x, dout, dx, bf16, nhwc, gm, tc_apply_ctas(gm, 1, 64), s.w.coef,
+                                   m.kind != MIX_INSTANCE ? s.mu : save_mean,
                                    s.w.shift, st))
       return fail(DWT_E_LAUNCH, "cuTensorMapEncodeTiled failed (CUresult %d)", cr);
   }
@@ -1084,7 +1130,7 @@ int dwt_whiten_instance_bwd(const float* x, const float* dout, float* dx, int64_
 
 size_t dwt_switch_workspace_bytes(int64_t N, int64_t C, int64_t HW, int group_size) {
   Mix m;
-  m.on = true;
+  m.kind = MIX_SWITCH;
   return image_workspace_bytes(N, C, HW, group_size, m);
 }
 
@@ -1093,7 +1139,7 @@ int dwt_whiten_switch_fwd(const float* x, float* y, int64_t N, int64_t C, int64_
                           float* save_mean, float* save_w, float* save_stats, void* workspace, size_t workspace_bytes,
                           dwt_stream_t stream) {
   Mix m;
-  m.on = true; m.mix = mix; m.save_stats = save_stats;
+  m.kind = MIX_SWITCH; m.mix = mix; m.save_stats = save_stats;
   m.momentum = momentum; m.update_running = update_running; m.rmean = running_mean; m.rcov = running_cov;
   return image_fwd(m, x, y, N, C, HW, group_size, mode, eps, save_mean, save_w, workspace, workspace_bytes, (cudaStream_t)stream);
 }
@@ -1102,7 +1148,32 @@ int dwt_whiten_switch_bwd(const float* x, const float* dout, float* dx, int64_t 
                           int mode, float eps, const float* mix, const float* save_mean, const float* save_w,
                           const float* save_stats, float* dmix, void* workspace, size_t workspace_bytes, dwt_stream_t stream) {
   Mix m;
-  m.on = true; m.mix = mix; m.save_stats = save_stats; m.dmix = dmix;
+  m.kind = MIX_SWITCH; m.mix = mix; m.save_stats = save_stats; m.dmix = dmix;
+  return image_bwd(m, x, dout, dx, N, C, HW, group_size, mode, eps, save_mean, save_w, workspace, workspace_bytes,
+                   (cudaStream_t)stream);
+}
+
+size_t dwt_latent_workspace_bytes(int64_t N, int64_t C, int64_t HW, int group_size, int n_domains) {
+  Mix m;
+  m.kind = MIX_LATENT; m.K = n_domains;
+  return image_workspace_bytes(N, C, HW, group_size, m);
+}
+
+int dwt_whiten_latent_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, int group_size, int n_domains, int mode,
+                          float eps, float momentum, int update_running, float* running_mean, float* running_cov,
+                          const float* weights, float* save_mean, float* save_w, float* save_stats, void* workspace,
+                          size_t workspace_bytes, dwt_stream_t stream) {
+  Mix m;
+  m.kind = MIX_LATENT; m.K = n_domains; m.mix = weights; m.save_stats = save_stats;
+  m.momentum = momentum; m.update_running = update_running; m.rmean = running_mean; m.rcov = running_cov;
+  return image_fwd(m, x, y, N, C, HW, group_size, mode, eps, save_mean, save_w, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
+int dwt_whiten_latent_bwd(const float* x, const float* dout, float* dx, int64_t N, int64_t C, int64_t HW, int group_size,
+                          int n_domains, int mode, float eps, const float* weights, const float* save_mean, const float* save_w,
+                          const float* save_stats, float* dweights, void* workspace, size_t workspace_bytes, dwt_stream_t stream) {
+  Mix m;
+  m.kind = MIX_LATENT; m.K = n_domains; m.mix = weights; m.save_stats = save_stats; m.dmix = dweights;
   return image_bwd(m, x, dout, dx, N, C, HW, group_size, mode, eps, save_mean, save_w, workspace, workspace_bytes,
                    (cudaStream_t)stream);
 }

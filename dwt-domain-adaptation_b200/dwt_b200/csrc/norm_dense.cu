@@ -19,6 +19,11 @@
 //                    fwd_instance's factorisation (sw_fwd_factor); backward: dL/dcov_hat and dL/dm per (image, group)
 //                    (sw_bwd_coef), their fixed-order sums over the images (sw_bwd_sum, sw_dmix) and tc_bwd_apply's
 //                    coefficients (sw_bwd_apply_coef)
+//   ld_*             latent-domain whitening (dwt_whiten_latent_*): each latent domain's weighted moments from the per-image
+//                    ones (ld_stats), fwd_instance's factorisation + EMA per (domain, group) (ld_fwd_factor), the per-image
+//                    mix A_n = sum_k w_nk W_k and its centre (ld_mix); backward: per-domain sums and the Cholesky backward
+//                    (ld_bwd_sum, ld_bwd_dom), tc_bwd_apply's coefficients and the dweights terms per (image, group)
+//                    (ld_bwd_coef) and their fixed-order sum over the groups (ld_dw)
 //
 // All three keep a 64x64 problem in ONE 256-thread CTA arranged 16x16, each thread owning a 4x4
 // register block.  fwd_factor runs the Cholesky factorisation AND the triangular inverse as one blocked
@@ -1219,16 +1224,17 @@ __global__ void __launch_bounds__(kThreads2) bwd_coef128_kernel(const float* __r
 }
 
 // ------------------------------------------------------------------------------------------
-// The end of the per-image forward kernels (fwd_instance, sw_fwd_factor): this thread's block of S (a) factored and
-// inverted, the CTA's OR of bad (S or the mean not finite) and of a non-positive pivot, W to save_w, or NaN in full for a
-// bad problem, and DWT_STATUS_NOT_PD
-__device__ __forceinline__ void image_factor_tail(float (&a)[4][4], bool bad, size_t problem, int GS, const Blk& t,
+// The end of the per-image forward kernels (fwd_instance, sw_fwd_factor) and of ld_fwd_factor: this thread's block of S
+// (a) factored and inverted, the CTA's OR of bad (S or the mean not finite) and of a non-positive pivot, W to save_w, or
+// NaN in full for a bad problem, and DWT_STATUS_NOT_PD.  Returns that OR (the same in every thread).
+__device__ __forceinline__ bool image_factor_tail(float (&a)[4][4], bool bad, size_t problem, int GS, const Blk& t,
                                                   PanelSmem& sp, float* save_w, int* status) {
   float w[4][4];
   const bool ok = factor_and_invert(a, w, GS, t, sp);
   bad = __syncthreads_or(bad || !ok) != 0;
   store_w_or_nan(save_w, problem, GS, t, w, bad);
   if (threadIdx.x == 0 && bad) atomicOr(status, DWT_STATUS_NOT_PD);
+  return bad;
 }
 
 // fwd_instance: instance whitening (dwt_whiten_instance_fwd), grid (G, 1, D), 256 threads, one CTA per (image, group):
@@ -1542,6 +1548,413 @@ __global__ void __launch_bounds__(256) sw_bwd_apply_coef_kernel(const float* __r
   }
 }
 
+// ------------------------------------------------------------------------------------------
+// Latent-domain whitening (dwt_whiten_latent_*): the Geom's domains are the images (N = 1, M = HW), as for fwd_instance;
+// K latent domains k weight image n by w_nk = weights[n][K].  save_stats (rec = gs*gs + gs floats per record):
+//   [D][G] records  each image's (C_n, m_n)          [K][G] records  each domain's (Sigma_k, mu_k)
+//   [K][G][gs*gs]   W_k = L_k^-1                     [K]             s_k = sum_n w_nk
+// A domain with s_k == 0 is skipped everywhere: no W_k, no EMA, no share in any output.  Every sum over the images skips
+// a weight that is exactly 0 instead of multiplying by it, so a non-finite domain or image stays out of the others.
+// ------------------------------------------------------------------------------------------
+struct LdLayout {
+  const int GS, rec, G, D, K;
+  float* base;
+  __device__ LdLayout(const Geom& gm, const LdFin& f)
+      : GS(gm.GS), rec(sw_rec(gm.GS)), G(gm.G), D(gm.D), K(f.K), base(f.save_stats) {}
+  __device__ float* img(int n, int g) const { return base + ((size_t)n * G + g) * rec; }
+  __device__ float* dom(int k, int g) const { return base + ((size_t)(D + k) * G + g) * rec; }
+  __device__ float* w_base() const { return base + (size_t)(D + K) * G * rec; }
+  __device__ float* mass() const { return w_base() + (size_t)K * G * GS * GS; }
+};
+
+// ld_stats: grid (ceil(rec / 256), G, K), 256 threads, one record element of one domain per thread.  The CTAs of domain 0
+// write each image's own covariance and mean (sw_stats' fp32 arithmetic).  s_k in fp64 over the images in order.  Train:
+// (Sigma_k, mu_k) = the w-weighted moments of the images' pixels by the law of total covariance,
+// Sigma_k = sum_n w_nk [C_n + (m_n - mu_k)(m_n - mu_k)^T] / s_k, accumulated in fp64 over the images in order about image
+// 0's mean; eval: a copy of domain k's running buffers.
+__global__ void __launch_bounds__(256) ld_stats_kernel(const float* __restrict__ gram, const float* __restrict__ shift,
+                                                       const Geom gm, const LdFin f) {
+  const int g = blockIdx.y, k = blockIdx.z;
+  const auto [GS, sb, o, SB] = group_pos(gm, g);
+  const LdLayout L(gm, f);
+  const int e = blockIdx.x * 256 + threadIdx.x;
+  if (e >= L.rec) return;
+  const int N = gm.D, K = f.K;
+  const float invM = 1.f / gm.M;
+  const double invMd = 1.0 / (double)gm.M;
+  const bool cov = e < GS * GS;
+  const int i = cov ? e / GS : e - GS * GS, j = cov ? e % GS : i, hi = i > j ? i : j, lo = i > j ? j : i;
+  const float* G0 = gram + (size_t)sb * kNacc;
+  const float* S0 = shift + (size_t)sb * kSB + o;
+  const double ci = (double)S0[i] + (double)__ldcg(G0 + kSB * kSB + o + i) * invMd;   // image 0's mean: the common shift
+  const double cj = (double)S0[j] + (double)__ldcg(G0 + kSB * kSB + o + j) * invMd;
+  double s = 0.0, acc = 0.0, accm = 0.0, acci = 0.0, accj = 0.0;
+  for (int n = 0; n < N; ++n) {
+    const float w = __ldg(f.weights + (size_t)n * K + k);
+    if (w != 0.f) s += (double)w;
+    const bool use = f.train && w != 0.f;
+    if (!use && k != 0) continue;
+    const float* Gd = G0 + (size_t)n * SB * kNacc;
+    const float* Sd = S0 + (size_t)n * SB * kSB;
+    const float ri = __ldcg(Gd + kSB * kSB + o + i), si = Sd[i];
+    const double dw = (double)w;
+    if (cov) {
+      const float graw = __ldcg(Gd + (o + hi) * kSB + o + lo), rj = __ldcg(Gd + kSB * kSB + o + j), sj = Sd[j];
+      if (k == 0) L.img(n, g)[e] = graw * invM - (ri * invM) * (rj * invM);
+      if (use) {
+        const double dri = (double)ri * invMd, drj = (double)rj * invMd;
+        const double mi = ((double)si + dri) - ci, mj = ((double)sj + drj) - cj;
+        acc += dw * ((double)graw * invMd - dri * drj);
+        accm += dw * (mi * mj);
+        acci += dw * mi;
+        accj += dw * mj;
+      }
+    } else {
+      if (k == 0) L.img(n, g)[e] = si + ri * invM;
+      if (use) acci += dw * (((double)si + (double)ri * invMd) - ci);
+    }
+  }
+  if (e == 0 && g == 0) L.mass()[k] = (float)s;
+  float v = 0.f;                                    // a zero-mass domain's row is never read
+  if (!f.train) {
+    v = cov ? f.rcov[((size_t)k * gm.G + g) * GS * GS + e] : f.rmean[(size_t)k * gm.C + g * GS + i];
+  } else if (s != 0.0) {
+    const double inv = 1.0 / s, mi = acci * inv, mj = accj * inv;
+    v = cov ? (float)(acc * inv + (accm * inv - mi * mj)) : (float)(ci + mi);
+  }
+  L.dom(k, g)[e] = v;
+}
+
+// ld_fwd_factor: grid (G, 1, K), 256 threads, one CTA per (domain, group): S_k = a Sigma_k + b I, fwd_instance's blocked
+// Cholesky + inverse into W_k, and the EMA of (Sigma_k, mu_k) (train, update_running).  A domain with s_k < 0 or NaN,
+// non-finite statistics or an S_k that is not positive definite gets W_k = NaN, sets DWT_STATUS_NOT_PD and skips its
+// EMA.  A domain with s_k == 0 is skipped (no W_k, no status, no EMA).
+__global__ void __launch_bounds__(256) ld_fwd_factor_kernel(const Geom gm, const LdFin f) {
+  __shared__ __align__(16) PanelSmem sp;
+  const int g = blockIdx.x, k = blockIdx.z, GS = gm.GS;
+  const LdLayout L(gm, f);
+  const Blk t(GS);
+  const float s = L.mass()[k];
+  if (s == 0.f) return;
+  const float* st = L.dom(k, g);
+  bool bad = !(s > 0.f);
+  float a[4][4];
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+      float v = 0.f;
+      if (t.act) {
+        const int i = 4 * t.bi + r, j = 4 * t.bj + c;
+        v = f.a * st[i * GS + j] + (i == j ? f.b : 0.f);
+        bad = bad || !isfinite(v);
+      }
+      a[r][c] = v;
+    }
+  if ((int)threadIdx.x < GS) bad = bad || !isfinite(st[GS * GS + threadIdx.x]);
+  bad = image_factor_tail(a, bad, (size_t)k * gm.G + g, GS, t, sp, L.w_base(), f.status);
+  if (bad || !f.train || !f.update_running) return;
+  const float m = f.momentum, km = 1.f - f.momentum;     // dwt_whiten_fwd's EMA on the unshrunk moments
+  float* rc = f.rcov + ((size_t)k * gm.G + g) * GS * GS;
+  float* rm = f.rmean + (size_t)k * gm.C + g * GS;
+  for (int e = threadIdx.x; e < GS * GS; e += 256) rc[e] = ema_cov(m, km, st[e], rc[e]);
+  if ((int)threadIdx.x < GS) rm[threadIdx.x] = ema_mean(m, km, st[GS * GS + threadIdx.x], rm[threadIdx.x]);
+}
+
+// ld_mix: grid (G, 1, D), 256 threads, one CTA per (image, group): A_n = sum_k w_nk W_k and b_n = sum_k w_nk W_k mu_k over
+// the domains in order (skipping w_nk == 0 and s_k == 0), then A_n m~_n = b_n by forward substitution (A_n is lower
+// triangular).  save_w = A_n, save_mean = m~_n; an (image, group) whose A_n has a diagonal entry that is not positive and
+// finite, or whose A_n or m~_n is not finite, gets A_n = NaN and m~_n = 0 and sets DWT_STATUS_NOT_PD (a NaN centre would
+// reach the other groups of its super-block through the apply's zero blocks).
+__global__ void __launch_bounds__(256) ld_mix_kernel(const Geom gm, const LdFin f) {
+  __shared__ float sA[kMat], sB[kSB];
+  const int g = blockIdx.x, n = blockIdx.z, GS = gm.GS, K = f.K;
+  const LdLayout L(gm, f);
+  const Blk t(GS);
+  const int ri = threadIdx.x >> 2, rq = threadIdx.x & 3;
+  float a[4][4], bq = 0.f;
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+#pragma unroll
+    for (int c = 0; c < 4; ++c) a[r][c] = 0.f;
+  for (int k = 0; k < K; ++k) {
+    const float w = __ldg(f.weights + (size_t)n * K + k);
+    if (w == 0.f || L.mass()[k] == 0.f) continue;       // CTA-uniform
+    const float* Wk = L.w_base() + ((size_t)k * gm.G + g) * GS * GS;
+    const float* mk = L.dom(k, g) + GS * GS;
+    if (t.act) {
+#pragma unroll
+      for (int r = 0; r < 4; ++r) {
+        const float4 v = *reinterpret_cast<const float4*>(Wk + (size_t)(4 * t.bi + r) * GS + 4 * t.bj);
+        a[r][0] = fmaf(w, v.x, a[r][0]); a[r][1] = fmaf(w, v.y, a[r][1]);
+        a[r][2] = fmaf(w, v.z, a[r][2]); a[r][3] = fmaf(w, v.w, a[r][3]);
+      }
+    }
+    if (ri < GS) {
+      float v = 0.f;
+      for (int j = rq; j <= ri; j += 4) v = fmaf(Wk[ri * GS + j], mk[j], v);   // W_k lower triangular
+      bq = fmaf(w, v, bq);
+    }
+  }
+  bq += __shfl_xor_sync(0xffffffffu, bq, 1);
+  bq += __shfl_xor_sync(0xffffffffu, bq, 2);
+  bool bad = false;
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+#pragma unroll
+    for (int c = 0; c < 4; ++c) bad = bad || (t.act && !isfinite(a[r][c]));
+  store_block(sA, t, a);
+  if (rq == 0 && ri < GS) sB[ri] = bq;
+  __syncthreads();
+  if (threadIdx.x < 32) {                                 // A z = b, rows i from the top
+    const int l = threadIdx.x;
+    float r0 = l < GS ? sB[l] : 0.f, r1 = l + 32 < GS ? sB[l + 32] : 0.f;
+    for (int i = 0; i < GS; ++i) {
+      const float d = sA[i * LDS + i];
+      bad = bad || !(d > 0.f && d < INFINITY);
+      const float own = i >= 32 ? r1 : r0;
+      const float zi = __shfl_sync(0xffffffffu, own, i & 31) / d;
+      if (l == (i & 31)) { if (i >= 32) r1 = zi; else r0 = zi; }
+      if (l > i && l < GS) r0 = fmaf(-sA[l * LDS + i], zi, r0);
+      if (l + 32 > i && l + 32 < GS) r1 = fmaf(-sA[(l + 32) * LDS + i], zi, r1);
+    }
+    bad = bad || (l < GS && !isfinite(r0)) || (l + 32 < GS && !isfinite(r1));
+    sB[l] = r0;                                           // each lane rewrites only its own rows
+    sB[l + 32] = r1;
+  }
+  bad = __syncthreads_or(bad) != 0;
+  store_w_or_nan(f.save_w, (size_t)n * gm.G + g, GS, t, a, bad);
+  if ((int)threadIdx.x < GS) f.save_mean[(size_t)n * gm.C + g * GS + threadIdx.x] = bad ? 0.f : sB[threadIdx.x];
+  if (threadIdx.x == 0 && bad) atomicOr(f.status, DWT_STATUS_NOT_PD);
+}
+
+// ld_bwd_sum: grid (ceil(rec / 256), G, K), 256 threads (train).  rgram [D][SB][kNacc] = (R~_n = sum dy (x - m~_n)^T |
+// g_n = sum dy).  sums[k][g] = (Wbar_k = sum_n w_nk [R~_n + g_n (m~_n - mu_k)^T] | sum_n w_nk g_n), over the images in
+// order in fp64.
+__global__ void __launch_bounds__(256) ld_bwd_sum_kernel(const float* __restrict__ rgram, const Geom gm, const LdFin f,
+                                                         float* __restrict__ sums) {
+  const int g = blockIdx.y, k = blockIdx.z;
+  const auto [GS, sb, o, SB] = group_pos(gm, g);
+  const LdLayout L(gm, f);
+  const int e = blockIdx.x * 256 + threadIdx.x;
+  if (e >= L.rec || L.mass()[k] == 0.f) return;
+  const bool cov = e < GS * GS;
+  const int i = cov ? e / GS : e - GS * GS, j = cov ? e % GS : 0;
+  const double muj = cov ? (double)L.dom(k, g)[GS * GS + j] : 0.0;
+  double acc = 0.0;
+  for (int n = 0; n < gm.D; ++n) {
+    const float w = __ldg(f.weights + (size_t)n * f.K + k);
+    if (w == 0.f) continue;
+    const float* Gn = rgram + ((size_t)n * SB + sb) * kNacc;
+    const double gi = (double)__ldcg(Gn + kSB * kSB + o + i);
+    double v = gi;
+    if (cov) v = (double)__ldcg(Gn + (o + i) * kSB + o + j) + gi * ((double)f.save_mean[(size_t)n * gm.C + g * GS + j] - muj);
+    acc += (double)w * v;
+  }
+  sums[((size_t)k * gm.G + g) * L.rec + e] = (float)acc;
+}
+
+// ld_bwd_dom: grid (G, 1, K), 256 threads (train), one CTA per (domain, group): from Wbar_k (sums) and W_k, the Cholesky
+// backward P_k = dL/dSigma_k = a sym(W^T Phi(-Wbar W^T) W) and mubar_k = -W_k^T sum_n w_nk g_n into pd[k][g], and
+// c_k = <P_k, Sigma_k> into pc[k][g].
+__global__ void __launch_bounds__(256) ld_bwd_dom_kernel(const Geom gm, const LdFin f, const float* __restrict__ sums,
+                                                         float* __restrict__ pd, float* __restrict__ pc) {
+  extern __shared__ __align__(16) float dsm[];
+  float* sW = dsm;
+  float* sR = sW + kMat;
+  float* sT = sR + kMat;
+  __shared__ float sSdz[kSB], sRed[8];
+  const int g = blockIdx.x, k = blockIdx.z, GS = gm.GS;
+  const LdLayout L(gm, f);
+  if (L.mass()[k] == 0.f) return;
+  const Blk t(GS);
+  const int gsh = __ffs(GS) - 1;
+  const float* Wk = L.w_base() + ((size_t)k * gm.G + g) * GS * GS;
+  const float* sm = sums + ((size_t)k * gm.G + g) * L.rec;
+  const float* st = L.dom(k, g);
+  float* out = pd + ((size_t)k * gm.G + g) * L.rec;
+  PROF_DECL;
+  for (int e = threadIdx.x; e < GS * GS; e += 256) {
+    const int i = e >> gsh, j = e & (GS - 1);
+    sW[i * LDS + j] = Wk[e];
+    sR[i * LDS + j] = sm[e];
+  }
+  if ((int)threadIdx.x < GS) sSdz[threadIdx.x] = sm[GS * GS + threadIdx.x];
+  __syncthreads();
+  chol_bwd_core(sR, sW, sT, sR, GS, t PROF_PASS);        // T' = W^T Phi(-Wbar W^T) W into sT
+  const float h = 0.5f * f.a;
+  float c = 0.f;
+  for (int e = threadIdx.x; e < GS * GS; e += 256) {
+    const int i = e >> gsh, j = e & (GS - 1);
+    const float p = h * (sT[i * LDS + j] + sT[j * LDS + i]);
+    out[e] = p;
+    c = fmaf(p, st[e], c);
+  }
+  {
+    const int i = threadIdx.x >> 2, q = threadIdx.x & 3;
+    float v = 0.f;
+    if (i < GS)
+      for (int j = q; j < GS; j += 4) v = fmaf(sW[j * LDS + i], sSdz[j], v);   // W_ji = 0 for j < i
+    v += __shfl_xor_sync(0xffffffffu, v, 1);
+    v += __shfl_xor_sync(0xffffffffu, v, 2);
+    if (q == 0 && i < GS) out[GS * GS + i] = -v;
+  }
+  c = block_sum(c, sRed);
+  if (threadIdx.x == 0) pc[(size_t)k * gm.G + g] = c;
+}
+
+// ld_bwd_coef: grid (G, 1, D), 256 threads, one CTA per (image, group), the domains in order (skipping s_k == 0; the
+// terms of dx also skip w_nk == 0, dweights does not: its derivative there is not 0).  With u_k = m_n - mu_k and
+// v_k = m~_n - mu_k:
+//   A1 = A_n^T,  Bm = train (2/M) sum_k (w_nk/s_k) P_k,
+//   k_n = train (1/M) sum_k (w_nk/s_k) [mubar_k + 2 P_k u_k],  dybar = -A_n^-T k_n (0 when A1 or Bm is not finite)
+//   part[n][g][k] = <W_k, R~_n + g_n v_k^T> + train [<mubar_k, u_k> + <P_k, C_n + u_k u_k^T> - c_k] / s_k
+// and mu [D][C] = m_n, the centre of tc_bwd_apply's Bm term.
+__global__ void __launch_bounds__(256) ld_bwd_coef_kernel(const float* __restrict__ rgram, const Geom gm, const LdFin f,
+                                                          const float* __restrict__ pd, const float* __restrict__ pc,
+                                                          float* __restrict__ part, float* __restrict__ coef,
+                                                          float* __restrict__ dybar, float* __restrict__ mu) {
+  extern __shared__ __align__(16) float dsm[];
+  float* sA = dsm;
+  float* sR = sA + kMat;
+  __shared__ float sU[kLdMaxDomains][kSB], sV[kLdMaxDomains][kSB], sG[kSB], sK[kSB], sRed[8][kLdMaxDomains];
+  const int g = blockIdx.x, n = blockIdx.z, K = f.K;
+  const auto [GS, sb, o, SB] = group_pos(gm, g);
+  const LdLayout L(gm, f);
+  const int gsh = __ffs(GS) - 1;
+  const bool train = f.train != 0;
+  const float invM = 1.f / gm.M;
+  const float* Gn = rgram + ((size_t)n * SB + sb) * kNacc;
+  const float* cn = L.img(n, g);
+  float* cf = coef + ((size_t)n * gm.G + g) * coef_stride(GS);
+  float wk[kLdMaxDomains], rs[kLdMaxDomains];                         // w_nk (0: no share in dx), 1/s_k (0: the domain is skipped)
+#pragma unroll
+  for (int k = 0; k < kLdMaxDomains; ++k) {
+    wk[k] = 0.f; rs[k] = 0.f;
+    if (k < K) {
+      const float s = L.mass()[k];
+      if (s != 0.f) { wk[k] = __ldg(f.weights + (size_t)n * K + k); rs[k] = 1.f / s; }
+    }
+  }
+  for (int e = threadIdx.x; e < GS * GS; e += 256) {
+    const int i = e >> gsh, j = e & (GS - 1);
+    sA[i * LDS + j] = f.save_w[((size_t)n * gm.G + g) * GS * GS + e];
+    sR[i * LDS + j] = __ldcg(Gn + (o + i) * kSB + o + j);
+  }
+  if ((int)threadIdx.x < GS) {
+    const int i = threadIdx.x;
+    const float mn = cn[GS * GS + i], mt = f.save_mean[(size_t)n * gm.C + g * GS + i];
+    sG[i] = __ldcg(Gn + kSB * kSB + o + i);
+    mu[(size_t)n * gm.C + g * GS + i] = mn;
+#pragma unroll
+    for (int k = 0; k < kLdMaxDomains; ++k) {
+      if (rs[k] == 0.f) continue;
+      const float muk = L.dom(k, g)[GS * GS + i];
+      sU[k][i] = mn - muk;
+      sV[k][i] = mt - muk;
+    }
+  }
+  __syncthreads();
+  float dwp[kLdMaxDomains];
+#pragma unroll
+  for (int k = 0; k < kLdMaxDomains; ++k) dwp[k] = 0.f;
+  bool nanc = false;
+  for (int e = threadIdx.x; e < GS * GS; e += 256) {
+    const int i = e >> gsh, j = e & (GS - 1);
+    const float r = sR[i * LDS + j], gi = sG[i], cij = train ? cn[e] : 0.f;
+    float q = 0.f;
+#pragma unroll
+    for (int k = 0; k < kLdMaxDomains; ++k) {
+      if (rs[k] == 0.f) continue;
+      const size_t kg = (size_t)k * gm.G + g;
+      dwp[k] = fmaf(L.w_base()[kg * GS * GS + e], fmaf(gi, sV[k][j], r), dwp[k]);
+      if (train) {
+        const float p = pd[kg * L.rec + e];
+        if (wk[k] != 0.f) q = fmaf(wk[k] * rs[k], p, q);
+        dwp[k] = fmaf(rs[k] * p, fmaf(sU[k][i], sU[k][j], cij), dwp[k]);
+      }
+    }
+    const float bm = 2.f * invM * q, av = sA[j * LDS + i];
+    cf[GS * GS + e] = bm;
+    cf[e] = j >= i ? av : 0.f;                            // A1 = A^T (A lower triangular)
+    nanc = nanc || !isfinite(bm) || !isfinite(av);
+  }
+  if (train && (int)threadIdx.x < GS) {                   // <mubar_k, u_k> and -c_k, over s_k
+    const int i = threadIdx.x;
+#pragma unroll
+    for (int k = 0; k < kLdMaxDomains; ++k) {
+      if (rs[k] == 0.f) continue;
+      const size_t kg = (size_t)k * gm.G + g;
+      float v = pd[kg * L.rec + GS * GS + i] * sU[k][i];
+      if (i == 0) v -= pc[kg];
+      dwp[k] = fmaf(rs[k], v, dwp[k]);
+    }
+  }
+  {                                                       // k_n: 4 threads per row, partial sums met by shuffle
+    const int i = threadIdx.x >> 2, qq = threadIdx.x & 3;
+    float v = 0.f;
+    if (train && i < GS) {
+#pragma unroll
+      for (int k = 0; k < kLdMaxDomains; ++k) {
+        if (wk[k] == 0.f) continue;
+        const float* pk = pd + ((size_t)k * gm.G + g) * L.rec;
+        float pu = 0.f;
+        for (int j = qq; j < GS; j += 4) pu = fmaf(pk[i * GS + j], sU[k][j], pu);
+        pu *= 2.f;
+        if (qq == 0) pu += pk[GS * GS + i];
+        v = fmaf(wk[k] * rs[k], pu, v);
+      }
+    }
+    v += __shfl_xor_sync(0xffffffffu, v, 1);
+    v += __shfl_xor_sync(0xffffffffu, v, 2);
+    if (qq == 0 && i < GS) sK[i] = v * invM;
+  }
+#pragma unroll
+  for (int k = 0; k < kLdMaxDomains; ++k) {
+    const float v = warp_sum(dwp[k]);
+    if ((threadIdx.x & 31) == 0) sRed[threadIdx.x >> 5][k] = v;
+  }
+  nanc = __syncthreads_or(nanc) != 0;
+  if ((int)threadIdx.x < K) {
+    float s = 0.f;
+#pragma unroll
+    for (int w = 0; w < 8; ++w) s += sRed[w][threadIdx.x];
+    part[((size_t)n * gm.G + g) * kLdMaxDomains + threadIdx.x] = s;
+  }
+  // a group whose A1 or Bm is not finite gets both as kApplyNaN
+  if (nanc) {
+    const float q = __int_as_float(kApplyNaN);
+    for (int e = threadIdx.x; e < GS * GS; e += 256) { cf[e] = q; cf[GS * GS + e] = q; }
+  }
+  if (threadIdx.x < 32) {                                 // A^T z = -k, A^T upper triangular: rows i from the bottom
+    const int l = threadIdx.x;
+    float r0 = l < GS ? -sK[l] : 0.f, r1 = l + 32 < GS ? -sK[l + 32] : 0.f;
+    for (int i = GS - 1; i >= 0; --i) {
+      const float own = i >= 32 ? r1 : r0;
+      const float zi = __shfl_sync(0xffffffffu, own, i & 31) / sA[i * LDS + i];
+      if (l == (i & 31)) { if (i >= 32) r1 = zi; else r0 = zi; }
+      if (l < i) r0 = fmaf(-sA[i * LDS + l], zi, r0);     // (A^T)_{l i} = A_il
+      if (l + 32 < i) r1 = fmaf(-sA[i * LDS + l + 32], zi, r1);
+    }
+    float* db = dybar + ((size_t)n * SB + sb) * kSB + o;
+    if (l < GS) db[l] = nanc ? 0.f : r0;
+    if (l + 32 < GS) db[l + 32] = nanc ? 0.f : r1;
+  }
+}
+
+// ld_dw: grid (ceil(D K / 256)), 256 threads: dweights[n][k] = the sum over the groups, in order and in fp64, of
+// part[n][g][k] (0 for a skipped domain).
+__global__ void __launch_bounds__(256) ld_dw_kernel(const float* __restrict__ part, const Geom gm, int K,
+                                                    float* __restrict__ dw) {
+  const int p = blockIdx.x * 256 + threadIdx.x;
+  if (p >= gm.D * K) return;
+  const int n = p / K, k = p % K;
+  const float* q = part + (size_t)n * gm.G * kLdMaxDomains + k;
+  double acc = 0.0;
+  for (int g = 0; g < gm.G; ++g) acc += (double)__ldcg(q + (size_t)g * kLdMaxDomains);
+  dw[p] = (float)acc;
+}
+
 constexpr size_t kFactorSmem = 0;   // fwd_factor: static shared memory only (panel buffers + covariance)
 constexpr size_t kCoefSmem = sizeof(float) * 4 * kMat;
 constexpr size_t kZcaFwdSmem = sizeof(float) * 4 * kMat;   // N, P, P^2, P^3 (66.6 KB; + 16.9 KB static)
@@ -1562,7 +1975,7 @@ int dense_init() {
       {(const void*)fwd_zca_kernel, kZcaFwdSmem},             {(const void*)bwd_zca_kernel, kZcaBwdSmem},
       {(const void*)fwd_eigh_kernel, kEighFwdSmem},           {(const void*)bwd_eigh_kernel, kEighBwdSmem},
       {(const void*)fwd_factor_kernel<true>, kColorFwdSmem},  {(const void*)bwd_color_kernel, kColorBwdSmem},
-      {(const void*)sw_bwd_coef_kernel, kSwCoefSmem}};
+      {(const void*)sw_bwd_coef_kernel, kSwCoefSmem},         {(const void*)ld_bwd_dom_kernel, kSwCoefSmem}};
   for (const auto& k : dynamic_smem) {
     const cudaError_t e = cudaFuncSetAttribute(k.kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k.smem);
     if (e != cudaSuccess) return (int)e;
@@ -1641,6 +2054,26 @@ void dense_sw_bwd(const float* rgram, const Geom& gm, const SwFin& fin, float* p
   if (fin.train) sw_bwd_sum_kernel<<<dim3((gm.GS * gm.GS + gm.GS + 255) / 256, gm.G), 256, 0, st>>>(pd, gm, sums);
   if (dmix) sw_dmix_kernel<<<1, 256, 0, st>>>(part, gm.D * gm.G, dmix);
   sw_bwd_apply_coef_kernel<<<dim3(gm.G, 1, gm.D), 256, kSwApplySmem, st>>>(pd, sums, gm, fin, coef, dybar, mu);
+}
+
+void dense_ld_stats(const float* gram, const float* shift, const Geom& gm, const LdFin& fin, cudaStream_t st) {
+  ld_stats_kernel<<<dim3((gm.GS * gm.GS + gm.GS + 255) / 256, gm.G, fin.K), 256, 0, st>>>(gram, shift, gm, fin);
+}
+
+void dense_ld_fwd(const Geom& gm, const LdFin& fin, cudaStream_t st) {
+  ld_fwd_factor_kernel<<<dim3(gm.G, 1, fin.K), 256, 0, st>>>(gm, fin);
+  ld_mix_kernel<<<dim3(gm.G, 1, gm.D), 256, 0, st>>>(gm, fin);
+}
+
+// eval: the coefficients and the direct term of dweights only (Sigma_k and mu_k are constants)
+void dense_ld_bwd(const float* rgram, const Geom& gm, const LdFin& fin, float* sums, float* pd, float* pc, float* part,
+                  float* dweights, float* coef, float* dybar, float* mu, cudaStream_t st) {
+  if (fin.train) {
+    ld_bwd_sum_kernel<<<dim3((gm.GS * gm.GS + gm.GS + 255) / 256, gm.G, fin.K), 256, 0, st>>>(rgram, gm, fin, sums);
+    ld_bwd_dom_kernel<<<dim3(gm.G, 1, fin.K), 256, kSwCoefSmem, st>>>(gm, fin, sums, pd, pc);
+  }
+  ld_bwd_coef_kernel<<<dim3(gm.G, 1, gm.D), 256, kSwApplySmem, st>>>(rgram, gm, fin, pd, pc, part, coef, dybar, mu);
+  if (dweights) ld_dw_kernel<<<(gm.D * fin.K + 255) / 256, 256, 0, st>>>(part, gm, fin.K, dweights);
 }
 
 }  // namespace dwt

@@ -107,6 +107,35 @@ void dense_sw_stats(const float* gram, const float* shift, const Geom& gm, const
 void dense_sw_fwd_factor(const Geom& gm, const SwFin& fin, cudaStream_t st);
 void dense_sw_bwd(const float* rgram, const Geom& gm, const SwFin& fin, float* pd, float* part, float* sums, float* dmix,
                   float* coef, float* dybar, float* mu, cudaStream_t st);
+// latent-domain whitening, group sizes 8..64 (dwt_whiten_latent_*; gm.D = images, gm.N = 1), K latent domains weighted
+// per image by weights [D][K].  save_stats (rec = gs*gs + gs): [D][G][rec] each image's (cov, mean), [K][G][rec] each
+// domain's (Sigma_k, mu_k), [K][G][gs*gs] W_k, [K] s_k (dwt_b200.h).  dense_ld_stats fills the statistics rows from tc_stats'
+// per-image moments (train: weighted by the law of total covariance; eval: the running buffers) and s_k; dense_ld_fwd
+// factors every (domain, group), runs its EMA and mixes every (image, group) into save_w = A_n and save_mean = m~_n.
+// dense_ld_bwd turns tc_bwd_reduce's R (about save_mean, no pilot) into tc_bwd_apply's coef, dybar and mean (mu = the
+// images' own means), and dweights when it is given.  Scratch: sums, pd [K][G][rec], pc [K][G],
+// part [D][G][kLdMaxDomains].
+// Domain slots per (image, group): ld_bwd_coef keeps one register accumulator per slot, and part and ld_dw use it as
+// their stride, so no domain count above it can be accepted.
+constexpr int kLdMaxDomains = 8;
+static_assert(DWT_MAX_LATENT_DOMAINS <= kLdMaxDomains, "latent-domain whitening: raise kLdMaxDomains with the header limit");
+struct LdFin {
+  float a, b;                 // S = a Sigma + b I (1 - eps, eps)
+  float momentum;
+  int train, update_running;
+  int K;                      // latent domains, 1..8
+  const float* weights;       // [D][K]
+  float* rmean;               // [K][C]
+  float* rcov;                // [K][G][gs*gs]
+  float* save_mean;           // [D][C]  m~_n
+  float* save_w;              // [D][G][gs*gs]  A_n
+  float* save_stats;
+  int* status;
+};
+void dense_ld_stats(const float* gram, const float* shift, const Geom& gm, const LdFin& fin, cudaStream_t st);
+void dense_ld_fwd(const Geom& gm, const LdFin& fin, cudaStream_t st);
+void dense_ld_bwd(const float* rgram, const Geom& gm, const LdFin& fin, float* sums, float* pd, float* pc, float* part,
+                  float* dweights, float* coef, float* dybar, float* mu, cudaStream_t st);
 
 // TMA + wgmma apply path (norm_tc_apply.cu): split-TF32 GEMM of the block-diagonal group matrices
 int tc_apply_init();

@@ -604,6 +604,96 @@ def switchable_whiten(x, mix, *, group_size, training_stats, eps, momentum, upda
     return _apply_per_image(_SwitchFunction, x, mix.float(), *args)
 
 
+class _LatentFunction(torch.autograd.Function):
+    """Latent-domain whitening (dwt_whiten_latent_fwd / _bwd): every image of x [N, C, *] whitened by the statistics of
+    n_domains latent domains under its row of weights [N, n_domains] (float32, on the device), per group of group_size
+    channels, in the Cholesky basis.  The gradient of weights is returned.  Running buffers: (mean [D, C], second moment
+    [D, C/gs, gs, gs]), one row per domain.  x is float32 or bfloat16, NCHW-contiguous or (4-D) channels-last; it goes to
+    the kernels in its own layout and dtype."""
+
+    @staticmethod
+    def forward(ctx, x, weights, group_size, mode, eps, momentum, update_running, running):
+        dev = nv.require_cuda(x, bf16=True)
+        rm_t, rv_t = running
+        nv.require_cuda(weights, rm_t, rv_t)
+        lib = nv.lib()
+        gs = group_size
+        x, fmt = _tma_ready(x)
+        n, c, hw = x.shape[0], x.shape[1], math.prod(x.shape[2:])
+        k = weights.shape[1]
+        w_c = _aligned(weights)
+        need_running = (mode == nv.MODE_EVAL) or update_running
+        if need_running:
+            _check_param("running mean", rm_t, k * c)
+            _check_param("running second moment", rv_t, k * c * gs)
+        flags = mode | (nv.LAYOUT_NHWC if fmt == torch.channels_last else 0) | (nv.DTYPE_BF16 if x.dtype == torch.bfloat16 else 0)
+        y = torch.empty_like(x)
+        g = max(c // gs, 1)
+        rec = gs * gs + gs
+        save_mean = torch.empty(n, c, dtype=torch.float32, device=dev)
+        save_w = torch.empty(n, g, gs, gs, dtype=torch.float32, device=dev)
+        save_stats = torch.empty((n + k) * g * rec + k * g * gs * gs + k, dtype=torch.float32, device=dev)
+        ws = nv.grow_workspace(dev, lib.dwt_latent_workspace_bytes(n, c, hw, gs, k))
+        rm, rv = (nv.ptr(rm_t), nv.ptr(rv_t)) if need_running else (None, None)
+        with torch.cuda.device(dev):
+            rc = lib.dwt_whiten_latent_fwd(nv.ptr(x), nv.ptr(y), n, c, hw, gs, k, flags, eps, momentum, int(update_running),
+                                           rm, rv, nv.ptr(w_c), nv.ptr(save_mean), nv.ptr(save_w), nv.ptr(save_stats),
+                                           nv.ptr(ws), ws.numel(), nv.stream_ptr(dev))
+        nv.check(rc)
+        nv.poll_status(dev)
+        if update_running and mode == nv.MODE_TRAIN:
+            _bump_versions([running])
+        ctx.save_for_backward(x, w_c, save_mean, save_w, save_stats)
+        ctx.cfg = (gs, flags, eps, n, c, hw, k, fmt)
+        return y
+
+    @staticmethod
+    def backward(ctx, dout):
+        lib = nv.lib()
+        x, w_c, save_mean, save_w, save_stats = ctx.saved_tensors
+        gs, flags, eps, n, c, hw, k, fmt = ctx.cfg
+        dout, _ = _prepare_dout(ctx, dout, x, fmt, 16)
+        dev = nv.require_cuda(dout, bf16=True)
+        dx = torch.empty_like(x)
+        dw = torch.empty(n, k, dtype=torch.float32, device=dev) if ctx.needs_input_grad[1] else None
+        ws = nv.grow_workspace(dev, lib.dwt_latent_workspace_bytes(n, c, hw, gs, k))
+        with torch.cuda.device(dev):
+            rc = lib.dwt_whiten_latent_bwd(nv.ptr(x), nv.ptr(dout), nv.ptr(dx), n, c, hw, gs, k, flags, eps, nv.ptr(w_c),
+                                           nv.ptr(save_mean), nv.ptr(save_w), nv.ptr(save_stats), nv.ptr(dw), nv.ptr(ws),
+                                           ws.numel(), nv.stream_ptr(dev))
+        nv.check(rc)
+        return dx, dw, None, None, None, None, None, None
+
+
+def latent_domain_whiten(x, weights, *, group_size, training_stats, eps, momentum, update_running, running):
+    """Latent-domain whitening of x [N, C, *] under per-image domain weights [N, D] (used as given: no softmax, no value
+    checks; cast to float32).  Per group of group_size channels, with each image's own mean and (biased) covariance
+    m_n, C_n and s_d = sum_n w_nd:
+        mu_d = sum_n w_nd m_n / s_d,  Sigma_d = sum_n w_nd [C_n + (m_n - mu_d)(m_n - mu_d)^T] / s_d
+        (training_stats=False: the running buffers),  W_d = inverse(cholesky((1 - eps) Sigma_d + eps I)),
+        y_n = sum_d w_nd W_d (x_n - mu_d).
+    A domain whose weights sum to exactly 0 is skipped (its weights get gradient 0).  running = (mean [D, C], second
+    moment [D, C/gs, gs, gs]): read when training_stats is False; updated with (mu_d, Sigma_d) by momentum when
+    training_stats and update_running.  weights gets its gradient.
+    The tensor-core kernels only (group sizes 8, 16, 32, 64, H*W >= 256, D <= 8; dwt_b200.h): a call they cannot take
+    raises NativeError with the library's reason and is never sent to another kernel family.  A bfloat16 NCHW x whose H*W
+    is not a multiple of 8 (the bf16 kernels' TMA rows) runs the same kernels in float32 on an upcast copy, the result in
+    bfloat16."""
+    if x.dim() < 3:
+        raise ValueError(f"latent-domain whitening expects [N, C, *] input (got {x.dim()}D input)")
+    if weights.dim() != 2 or weights.shape[0] != x.shape[0]:
+        raise ValueError(f"latent-domain whitening expects weights of shape [N, n_domains] with N = {x.shape[0]} "
+                         f"(got {list(weights.shape)})")
+    if not weights.is_floating_point():
+        raise TypeError(f"latent-domain whitening expects floating-point weights (got {weights.dtype})")
+    if weights.device != x.device:
+        raise ValueError(f"latent-domain whitening expects weights on x's device {x.device} (got {weights.device})")
+    nv.require_cuda(x, bf16=True)
+    mode = nv.MODE_TRAIN if training_stats else nv.MODE_EVAL
+    args = (int(group_size), mode, float(eps), float(momentum), bool(update_running), tuple(running))
+    return _apply_per_image(_LatentFunction, x, weights.float(), *args)
+
+
 class _MecFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, y):

@@ -22,6 +22,8 @@
  *   dwt_whiten_color_fwd/bwd whitening followed by a learnable per-group colouring matrix and bias (not in the reference)
  *   dwt_whiten_instance_fwd/bwd  instance whitening: each image by its own statistics (not in the reference)
  *   dwt_whiten_switch_fwd/bwd  switchable whitening: a learned mix of batch and per-image statistics (not in the reference)
+ *   dwt_whiten_latent_fwd/bwd  latent-domain whitening: statistics of up to 8 domains under per-image soft weights (not in
+ *                    the reference)
  *   dwt_bn_fwd/bwd   _BatchNorm.forward             utils/batch_norm.py:54-69
  *   dwt_tail2_fwd/bwd  the residual tail of a downsampling Bottleneck: two norm sites and the ReLU in one pass
  *                    resnet50_dwt_mec_officehome.py:236-240
@@ -53,6 +55,8 @@ extern "C" {
 
 #define DWT_B200_ABI_VERSION 10
 #define DWT_MAX_DOMAINS 4
+/* latent-domain whitening (dwt_whiten_latent_*): domains weighted per image, not contiguous slices of the batch */
+#define DWT_MAX_LATENT_DOMAINS 8
 #define DWT_MAX_GROUP_SIZE 64
 /* the one group size above DWT_MAX_GROUP_SIZE: whitening on the tensor-core kernels only, fp32 (dwt_whiten_fwd) */
 #define DWT_TC_MAX_GROUP_SIZE 128
@@ -351,6 +355,71 @@ DWT_API int dwt_whiten_switch_fwd(const float *x, float *y, int64_t N, int64_t C
 DWT_API int dwt_whiten_switch_bwd(const float *x, const float *dout, float *dx, int64_t N, int64_t C, int64_t HW,
                    int group_size, int mode, float eps, const float *mix, const float *save_mean, const float *save_w,
                    const float *save_stats, float *dmix, void *workspace, size_t workspace_bytes, dwt_stream_t stream);
+
+/*
+ * Latent-domain whitening (the whitening form of the mDA layer, Mancini et al., CVPR 2018): K = n_domains domains whose
+ * membership is a weight per image, weights [N, K] (soft assignments inferred by the network, or one-hot labels of uneven,
+ * interleaved domains).  Per group g, with M = HW, each image's own mean and biased covariance m_n, C_n (as
+ * dwt_whiten_instance_fwd) and s_k = sum_n w_nk:
+ *     mu_k = sum_n w_nk m_n / s_k,   Sigma_k = sum_n w_nk [C_n + (m_n - mu_k)(m_n - mu_k)^T] / s_k   (the w-weighted pixel
+ *     moments; DWT_MODE_EVAL: domain k's running buffers instead),   S_k = (1-eps) Sigma_k + eps I = L_k L_k^T,  W_k = L_k^-1,
+ *     y_n = sum_k w_nk W_k (x_n - mu_k) = A_n (x_n - m~_n),   A_n = sum_k w_nk W_k,   A_n m~_n = sum_k w_nk W_k mu_k.
+ * weights are used as given: no softmax, normalisation or sign check (the softmax belongs to the caller).
+ * Edge rules:
+ *   - a domain with s_k == 0 exactly is skipped: no W_k, no share in any output, running buffers untouched, no status,
+ *     dweights[:, k] = 0 (the function is not differentiable there);
+ *   - a domain with s_k < 0 or NaN, non-finite statistics, or an S_k that is not positive definite gets W_k = NaN, sets
+ *     DWT_STATUS_NOT_PD and skips its EMA;
+ *   - every sum over images or domains skips a weight that is exactly 0 instead of multiplying by it: an image whose weight
+ *     on a bad domain is 0 stays finite, and so does its dx;
+ *   - an (image, group) whose A_n has a diagonal entry that is not positive and finite (negative weights, no weight at all),
+ *     or whose A_n or m~_n is not finite, gets A_n = NaN (m~_n = 0), so NaN output and dx in that group, and sets
+ *     DWT_STATUS_NOT_PD.  A bad domain's NaN reaches, in training, that group's dx in every image with weight on it, and
+ *     dweights[:, k].
+ * DWT_MODE_TRAIN with update_running: running_k = (1-momentum) running_k + momentum (mu_k, Sigma_k), unshrunk and biased,
+ * the convention of dwt_whiten_fwd (with one-hot weights the buffers are those of a WTransform2d per domain).
+ * DWT_MODE_EVAL reads the buffers and writes nothing; s_k still comes from the weights (the zero-mass rule).
+ * dwt_whiten_latent_bwd is the exact gradient of the forward (in eval mu_k and Sigma_k are constants).  With
+ * g_n = sum_pixels dout, R_n = sum_pixels dout (x - m_n)^T:
+ *     Wbar_k = sum_n w_nk [R_n + g_n (m_n - mu_k)^T],  mubar_k = -W_k^T sum_n w_nk g_n,
+ *     P_k = dL/dSigma_k = (1-eps) sym(W_k^T Phi(-Wbar_k W_k^T) W_k)   (dwt_whiten_bwd's Cholesky backward)
+ *     dx = A_n^T dout + (1/M) sum_k (w_nk/s_k) [mubar_k + 2 P_k (x - mu_k)]         (eval: A_n^T dout)
+ *     dweights_nk = sum_g <W_k, R_n + g_n (m_n - mu_k)^T>
+ *                   + (1/s_k) [<mubar_k, m_n - mu_k> + <P_k, C_n + (m_n - mu_k)(m_n - mu_k)^T - Sigma_k>]   (eval: first term)
+ *   x, y, dout, dx  [N, C, HW] (or channels-last [N, HW, C] with DWT_LAYOUT_NHWC), fp32 or bf16 (DWT_DTYPE_BF16)
+ *   n_domains       K, 1..DWT_MAX_LATENT_DOMAINS (else DWT_E_INVALID)
+ *   mode            DWT_MODE_TRAIN / DWT_MODE_EVAL | DWT_LAYOUT_NHWC | DWT_DTYPE_BF16 (any other bit: DWT_E_INVALID)
+ *   running_mean [K, C], running_cov [K, C/gs, gs, gs] (contiguous): read in eval, updated in train with update_running
+ *                   (else unused, may be NULL)
+ *   weights [N, K]  fp32, device
+ *   save_mean [N, C] m~_n;  save_w [N, C/gs, gs, gs] A_n;  save_stats, with rec = gs*gs + gs and G = C/gs, floats:
+ *                   [N][G][rec] each image's (C_n, m_n), [K][G][rec] each domain's (Sigma_k, mu_k), [K][G][gs*gs] W_k,
+ *                   [K] s_k -- (N + K) G rec + K G gs^2 + K in all.  Written by fwd, read by bwd.
+ *   dweights [N, K] written (never accumulated) by bwd; NULL skips it
+ * weights, save_w and save_stats must be 16-byte aligned, as must x, y, dout and dx (else DWT_E_INVALID).
+ * The statistics, apply and backward contraction are dwt_whiten_instance_*'s tensor-core passes; the domain moments come
+ * from the per-image ones in fp64 over the images in order about image 0's mean (no second pass over x), and every other
+ * reduction is in a fixed order too: reruns are bit-identical, dweights included.  bf16 loads widen to fp32 and stores round
+ * to nearest-even: every bf16 output is the fp32 call's output on the widened input, rounded.  Channels-last outputs are
+ * bit for bit those of NCHW.
+ * Geometry as dwt_whiten_instance_*: group size 8, 16, 32, 64 dividing C, HW >= 256 and HW % 4 == 0 (NCHW bf16:
+ * HW % 8 == 0), N <= 65535 and N*C*HW < 2^31.  Anything else -- and a call whose tensor-core kernels could not be set
+ * up -- is DWT_E_UNSUPPORTED with a text naming latent-domain whitening.  DWT_MAX_DOMAINS and the other entry points'
+ * rules are unchanged.
+ * Workspace: dwt_latent_workspace_bytes(N, C, HW, group_size, n_domains) bytes, 256-byte aligned, zero-filled once (it may
+ * be the same buffer as the other entry points'; the status word is shared).  It returns 0 for a call the entry points
+ * refuse for its geometry or n_domains.
+ * Profile families ld_stats, ld_fwd_finalize, ld_apply, ld_bwd_reduce, ld_bwd_finalize, ld_bwd_apply (_nhwc, _bf16).
+ */
+DWT_API size_t dwt_latent_workspace_bytes(int64_t N, int64_t C, int64_t HW, int group_size, int n_domains);
+DWT_API int dwt_whiten_latent_fwd(const float *x, float *y, int64_t N, int64_t C, int64_t HW, int group_size, int n_domains,
+                   int mode, float eps, float momentum, int update_running, float *running_mean, float *running_cov,
+                   const float *weights, float *save_mean, float *save_w, float *save_stats,
+                   void *workspace, size_t workspace_bytes, dwt_stream_t stream);
+DWT_API int dwt_whiten_latent_bwd(const float *x, const float *dout, float *dx, int64_t N, int64_t C, int64_t HW,
+                   int group_size, int n_domains, int mode, float eps, const float *weights, const float *save_mean,
+                   const float *save_w, const float *save_stats, float *dweights, void *workspace, size_t workspace_bytes,
+                   dwt_stream_t stream);
 
 /*
  * Domain batch norm (F.batch_norm semantics): biased batch variance normalises,
