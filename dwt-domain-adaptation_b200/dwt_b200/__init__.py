@@ -14,11 +14,13 @@ from .functional import fork_for_sum
 from .fused import DomainTripleNorm
 from .instance import InstanceWTransform2d
 from .latent import LatentDomainWTransform2d
+from .latent_batch_norm import LatentDomainBatchNorm1d, LatentDomainBatchNorm2d
 from .pooling import MaxPool2d
 from .switchable import SwitchableWTransform2d
 from .whitening import WTransform2d
 from .zca import ExactZCAWTransform2d, ZCAWTransform2d
 
-__all__ = ["WTransform2d", "ZCAWTransform2d", "ExactZCAWTransform2d", "WCTransform2d", "InstanceWTransform2d", "SwitchableWTransform2d", "LatentDomainWTransform2d", "BatchNorm1d", "BatchNorm2d", "BatchNorm3d", "MinEntropyConsensusLoss",
+__all__ = ["WTransform2d", "ZCAWTransform2d", "ExactZCAWTransform2d", "WCTransform2d", "InstanceWTransform2d", "SwitchableWTransform2d", "LatentDomainWTransform2d", "LatentDomainBatchNorm1d",
+           "LatentDomainBatchNorm2d", "BatchNorm1d", "BatchNorm2d", "BatchNorm3d", "MinEntropyConsensusLoss",
            "DomainTripleNorm", "fork_for_sum", "HeadLoss", "MaxPool2d", "PairedAugment", "draw_params", "raise_on_status", "check_status",
            "NotPositiveDefiniteError", "_native"]

@@ -106,6 +106,15 @@ _SIGNATURES = {
                                              ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float,
                                              _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_void_p,
                                              ctypes.c_size_t, ctypes.c_void_p]),
+    "dwt_bn_latent_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int64, ctypes.c_int64, ctypes.c_int64, ctypes.c_int]),
+    "dwt_bn_latent_fwd": (ctypes.c_int, [_c_float_p, _c_float_p, ctypes.c_int64, ctypes.c_int64, ctypes.c_int64, ctypes.c_int,
+                                         ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_int, _c_float_p, _c_float_p,
+                                         _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_void_p, ctypes.c_size_t,
+                                         ctypes.c_void_p]),
+    "dwt_bn_latent_bwd": (ctypes.c_int, [_c_float_p, _c_float_p, _c_float_p, ctypes.c_int64, ctypes.c_int64, ctypes.c_int64,
+                                         ctypes.c_int, ctypes.c_int, ctypes.c_float, _c_float_p, _c_float_p, _c_float_p,
+                                         _c_float_p, _c_float_p, _c_float_p, ctypes.c_void_p, ctypes.c_size_t,
+                                         ctypes.c_void_p]),
     "dwt_bn_fwd": (ctypes.c_int, [_c_float_p, _c_float_p, ctypes.c_int64, ctypes.c_int64, ctypes.c_int64,
                                   ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_int,
                                   ctypes.POINTER(ctypes.c_void_p), ctypes.POINTER(ctypes.c_void_p), _c_float_p,
@@ -285,8 +294,9 @@ def workspace(device, n, c, hw, gs, nd):
 
 def grow_workspace(device, nbytes):
     """The current stream's workspace, grown to at least nbytes (a new buffer has at least 8 MiB).  The per-image entry
-    points size theirs by dwt_instance_workspace_bytes / dwt_switch_workspace_bytes / dwt_latent_workspace_bytes, which
-    give 0 for a geometry they refuse (the call then reports why)."""
+    points size theirs by dwt_instance_workspace_bytes / dwt_switch_workspace_bytes / dwt_latent_workspace_bytes, and
+    latent-domain batch norm by dwt_bn_latent_workspace_bytes, which give 0 for a geometry they refuse (the call then
+    reports why)."""
     key = (device.index, torch.cuda.current_stream(device).cuda_stream)
     buf = _workspaces.get(key)
     if buf is None or buf.numel() < nbytes:

@@ -15,7 +15,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "lib", "libdwt_b200.so")
-SOURCES = ["api.cu", "norm_small.cu", "norm_tiled.cu", "norm_tc.cu", "norm_tc_apply.cu", "norm_dense.cu", "norm_cl.cu", "mec.cu", "augment.cu", "pool.cu"]
+SOURCES = ["api.cu", "norm_small.cu", "norm_tiled.cu", "norm_tc.cu", "norm_tc_apply.cu", "norm_dense.cu", "norm_cl.cu", "norm_ldbn.cu", "mec.cu", "augment.cu", "pool.cu"]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC,-fvisibility=hidden", "--expt-relaxed-constexpr"]
 NVCC_FLAGS += shlex.split(os.environ.get("DWT_NVCC_EXTRA", ""))     # development only, e.g. -DDWT_PROF_DENSE (phase clocks)

@@ -1105,6 +1105,88 @@ int image_bwd(const Mix& m, const void* x, const void* dout, void* dx, int64_t N
   return check_launch("%s backward apply kernel", m.what());
 }
 
+// ---- latent-domain batch norm (dwt_bn_latent_*) -----------------------------------------------------------------------
+// Forward: ldbn_stats (train only) -> ldbn_fwd_finalize -> ldbn_apply; backward: ldbn_bwd_reduce -> ldbn_bwd_finalize
+// (+ ldbn_dw when dweights is given) -> ldbn_bwd_apply (norm_ldbn.cu).  Scratch behind the common head: the segment
+// partials (two arrays), the pilot shifts, three [N][C] coefficient arrays and the dweights shares.
+struct LdbnWork { float *pa, *pb, *pilot, *c0, *c1, *c2, *dw; size_t bytes; };
+
+LdbnWork carve_ldbn(void* base, const dwt::LdbnGeom& g) {
+  size_t part, nc, dw;
+  dwt::ldbn_scratch_floats(g, &part, &nc, &dw);
+  size_t off = kOffScratch;
+  char* b = static_cast<char*>(base);
+  auto take = [&](size_t floats) { size_t o = off; off = align_up(off + sizeof(float) * floats, 256); return reinterpret_cast<float*>(b + o); };
+  LdbnWork w;
+  w.pa = take(part); w.pb = take(part); w.pilot = take(nc);
+  w.c0 = take(nc); w.c1 = take(nc); w.c2 = take(nc); w.dw = take(dw);
+  w.bytes = off;
+  return w;
+}
+
+// n_domains, mode bits and geometry (no device call); fills the plan
+int ldbn_geom(dwt::LdbnGeom& g, int64_t N, int64_t C, int64_t HW, int D, int mode) {
+  if (D < 1 || D > DWT_MAX_LATENT_DOMAINS)
+    return fail(DWT_E_INVALID, "n_domains %d outside [1,%d] (latent-domain batch norm)", D, DWT_MAX_LATENT_DOMAINS);
+  if (mode & ~(DWT_MODE_EVAL | DWT_LAYOUT_NHWC | DWT_DTYPE_BF16))
+    return fail(DWT_E_INVALID, "bad mode %#x (DWT_MODE_TRAIN or DWT_MODE_EVAL | DWT_LAYOUT_NHWC | DWT_DTYPE_BF16)", mode);
+  if (N <= 0 || C <= 0 || HW <= 0) return fail(DWT_E_INVALID, "empty tensor (N=%lld C=%lld HW=%lld)", (long long)N,
+                                               (long long)C, (long long)HW);
+  const bool nhwc = (mode & DWT_LAYOUT_NHWC) != 0, bf16 = (mode & DWT_DTYPE_BF16) != 0;
+  if ((double)N * (double)C * (double)HW >= 2147483648.0)
+    return fail(DWT_E_UNSUPPORTED, "latent-domain batch norm needs N*C*HW < 2^31 (N=%lld C=%lld HW=%lld)", (long long)N,
+                (long long)C, (long long)HW);
+  if (nhwc && C % 4 != 0)
+    return fail(DWT_E_UNSUPPORTED, "latent-domain batch norm runs channels-last at C %% 4 == 0 only (C=%lld)", (long long)C);
+  if (bf16 && !nhwc && HW % 4 != 0)
+    return fail(DWT_E_UNSUPPORTED, "latent-domain batch norm runs NCHW bf16 at HW %% 4 == 0 only (HW=%lld)", (long long)HW);
+  g = dwt::ldbn_plan((int)N, (int)C, (int)HW, D, nhwc, bf16);
+  return DWT_OK;
+}
+
+// The checks both directions make, in order: geometry, pointers, alignment, workspace.  act: the activation tensors.
+int ldbn_validate(dwt::LdbnGeom& g, LdbnWork& w, int64_t N, int64_t C, int64_t HW, int D, int mode, const void* const (&act)[3],
+                  const float* weights, const float* save, const float* gamma, const float* beta, void* ws, size_t ws_bytes) {
+  if (int rc = ldbn_geom(g, N, C, HW, D, mode)) return rc;
+  if (!act[0] || !act[1] || !act[2] || !weights || !save || !ws) return fail(DWT_E_INVALID, "null pointer argument");
+  if (!gamma != !beta)
+    return fail(DWT_E_INVALID, "gamma and beta (dgamma and dbeta) must be both given or both NULL (latent-domain batch norm)");
+  const uintptr_t bits = (uintptr_t)act[0] | (uintptr_t)act[1] | (uintptr_t)act[2];
+  if (bits % (g.bf16 ? 8 : 16) != 0)
+    return fail(DWT_E_INVALID, "activation tensors must be %d-byte aligned (latent-domain batch norm)", g.bf16 ? 8 : 16);
+  if (((uintptr_t)weights | (uintptr_t)gamma | (uintptr_t)beta) % 4 != 0 || (uintptr_t)save % 16 != 0)
+    return fail(DWT_E_INVALID, "weights, gamma and beta must be 4-byte and save_stats 16-byte aligned (latent-domain batch norm)");
+  w = carve_ldbn(ws, g);
+  if (w.bytes > ws_bytes) return fail(DWT_E_WORKSPACE, "workspace too small: need %zu bytes, got %zu", w.bytes, ws_bytes);
+  if ((uintptr_t)ws % 256 != 0) return fail(DWT_E_WORKSPACE, "workspace must be 256-byte aligned");
+  return DWT_OK;
+}
+
+dwt::LdbnFin make_ldbn_fin(const dwt::LdbnGeom& g, int mode, float eps, const float* weights, const float* gamma,
+                           const float* beta, const float* save, void* ws) {
+  dwt::LdbnFin f{};
+  f.N = g.N; f.C = g.C; f.D = g.D; f.S = g.S; f.M = (double)g.HW;
+  f.eps = eps; f.train = (mode & DWT_MODE_EVAL) == 0;
+  f.weights = weights; f.gamma = gamma; f.beta = beta; f.save = const_cast<float*>(save);
+  f.status = static_cast<int*>(ws);
+  return f;
+}
+
+// Profile family of a launch: [pass][channels-last * 2 + bf16]
+const char* const kLdbnName[6][4] = {
+    {"ldbn_stats", "ldbn_stats_bf16", "ldbn_stats_nhwc", "ldbn_stats_nhwc_bf16"},
+    {"ldbn_fwd_finalize", "ldbn_fwd_finalize", "ldbn_fwd_finalize", "ldbn_fwd_finalize"},
+    {"ldbn_apply", "ldbn_apply_bf16", "ldbn_apply_nhwc", "ldbn_apply_nhwc_bf16"},
+    {"ldbn_bwd_reduce", "ldbn_bwd_reduce_bf16", "ldbn_bwd_reduce_nhwc", "ldbn_bwd_reduce_nhwc_bf16"},
+    {"ldbn_bwd_finalize", "ldbn_bwd_finalize", "ldbn_bwd_finalize", "ldbn_bwd_finalize"},
+    {"ldbn_bwd_apply", "ldbn_bwd_apply_bf16", "ldbn_bwd_apply_nhwc", "ldbn_bwd_apply_nhwc_bf16"}};
+
+dwt::Geom ldbn_prof_geom(const dwt::LdbnGeom& g) {
+  dwt::Geom gm{};
+  gm.N = g.N; gm.C = g.C; gm.HW = g.HW; gm.GS = 1; gm.G = g.C; gm.D = g.D;
+  return gm;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1176,6 +1258,92 @@ int dwt_whiten_latent_bwd(const float* x, const float* dout, float* dx, int64_t 
   m.kind = MIX_LATENT; m.K = n_domains; m.mix = weights; m.save_stats = save_stats; m.dmix = dweights;
   return image_bwd(m, x, dout, dx, N, C, HW, group_size, mode, eps, save_mean, save_w, workspace, workspace_bytes,
                    (cudaStream_t)stream);
+}
+
+size_t dwt_bn_latent_workspace_bytes(int64_t N, int64_t C, int64_t HW, int n_domains) {
+  char saved[sizeof(g_err)];
+  memcpy(saved, g_err, sizeof(g_err));
+  size_t bytes = 0;
+  dwt::LdbnGeom g;
+  // the larger of the two layouts' plans (channels-last only where it runs)
+  for (int mode : {0, DWT_LAYOUT_NHWC})
+    if (ldbn_geom(g, N, C, HW, n_domains, mode) == DWT_OK) {
+      const size_t b = carve_ldbn(nullptr, g).bytes;
+      if (b > bytes) bytes = b;
+    }
+  memcpy(g_err, saved, sizeof(g_err));
+  return bytes;
+}
+
+int dwt_bn_latent_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, int n_domains, int mode, float eps,
+                      float momentum, int update_running, float* running_mean, float* running_var, const float* weights,
+                      const float* gamma, const float* beta, float* save_stats, void* workspace, size_t workspace_bytes,
+                      dwt_stream_t stream) {
+  dwt::LdbnGeom g;
+  LdbnWork w;
+  const void* const act[3] = {x, x, y};
+  if (int rc = ldbn_validate(g, w, N, C, HW, n_domains, mode, act, weights, save_stats, gamma, beta, workspace,
+                             workspace_bytes))
+    return rc;
+  const bool train = (mode & DWT_MODE_EVAL) == 0;
+  if ((!train || update_running) && (!running_mean || !running_var))
+    return fail(DWT_E_INVALID, "running buffer is null (eval, or train with update_running)");
+  cudaStream_t st = (cudaStream_t)stream;
+  dwt::LdbnFin f = make_ldbn_fin(g, mode, eps, weights, gamma, beta, save_stats, workspace);
+  f.momentum = momentum; f.update_running = train && update_running; f.rmean = running_mean; f.rvar = running_var;
+  const dwt::Geom pg = ldbn_prof_geom(g);
+  const int k = 2 * g.nhwc + g.bf16;
+  const double E = (g.bf16 ? 2.0 : 4.0) * (double)N * (double)C * (double)HW;
+  if (train) {
+    Launch l(kLdbnName[0][k], &pg, E, st);
+    dwt::ldbn_stats(x, g, w.pa, w.pb, w.pilot, st);
+  }
+  if (int rc = check_launch("latent-domain batch norm statistics kernel")) return rc;
+  {
+    Launch l(kLdbnName[1][k], &pg, 0.0, st);
+    dwt::ldbn_fwd_finalize(f, w.pa, w.pb, w.pilot, w.c0, w.c1, st);
+  }
+  if (int rc = check_launch("latent-domain batch norm finalize kernel")) return rc;
+  {
+    Launch l(kLdbnName[2][k], &pg, 2.0 * E, st);
+    dwt::ldbn_apply(x, y, g, w.c0, w.c1, st);
+  }
+  return check_launch("latent-domain batch norm apply kernel");
+}
+
+int dwt_bn_latent_bwd(const float* x, const float* dout, float* dx, int64_t N, int64_t C, int64_t HW, int n_domains, int mode,
+                      float eps, const float* weights, const float* gamma, const float* save_stats, float* dweights,
+                      float* dgamma, float* dbeta, void* workspace, size_t workspace_bytes, dwt_stream_t stream) {
+  dwt::LdbnGeom g;
+  LdbnWork w;
+  const void* const act[3] = {x, dout, dx};
+  if (int rc = ldbn_validate(g, w, N, C, HW, n_domains, mode, act, weights, save_stats, dgamma, dbeta, workspace,
+                             workspace_bytes))
+    return rc;
+  if (dgamma && !gamma) return fail(DWT_E_INVALID, "dgamma / dbeta given without gamma (latent-domain batch norm)");
+  if ((uintptr_t)dweights % 4 != 0) return fail(DWT_E_INVALID, "dweights must be 4-byte aligned (latent-domain batch norm)");
+  cudaStream_t st = (cudaStream_t)stream;
+  dwt::LdbnFin f = make_ldbn_fin(g, mode, eps, weights, gamma, nullptr, save_stats, workspace);
+  f.dgamma = dgamma; f.dbeta = dbeta;
+  const dwt::Geom pg = ldbn_prof_geom(g);
+  const int k = 2 * g.nhwc + g.bf16;
+  const double E = (g.bf16 ? 2.0 : 4.0) * (double)N * (double)C * (double)HW;
+  const float* centre = save_stats;                           // [N][C] first in save_stats
+  {
+    Launch l(kLdbnName[3][k], &pg, 2.0 * E, st);
+    dwt::ldbn_bwd_reduce(x, dout, g, centre, w.pa, w.pb, st);
+  }
+  if (int rc = check_launch("latent-domain batch norm backward reduction kernel")) return rc;
+  {
+    Launch l(kLdbnName[4][k], &pg, 0.0, st);
+    dwt::ldbn_bwd_finalize(f, w.pa, w.pb, w.c0, w.c1, w.c2, w.dw, dweights, st);
+  }
+  if (int rc = check_launch("latent-domain batch norm backward finalize kernel")) return rc;
+  {
+    Launch l(kLdbnName[5][k], &pg, 3.0 * E, st);
+    dwt::ldbn_bwd_apply(x, dout, dx, g, w.c0, w.c1, w.c2, centre, st);
+  }
+  return check_launch("latent-domain batch norm backward apply kernel");
 }
 
 const char* dwt_last_error(void) { return g_err; }

@@ -180,6 +180,47 @@ void cl_tail2_bwd_reduce(const void* x, const void* xd, const void* dout, const 
 void cl_tail2_bwd_apply(const void* x, const void* xd, const void* dz, void* dx, void* dxd, bool bf16, const Geom& gm, int nctas, int gz,
                         const float* coef, const float* coef_d, cudaStream_t st);
 
+// latent-domain batch norm (norm_ldbn.cu; dwt_bn_latent_*).  Rows of one (image, channel) split into S segments of P
+// pixels; NCHW: any HW (bf16: HW % 4 == 0), channels-last: C % 4 == 0.  save (dwt_b200.h): [N][C] m_n (eval: the
+// centre), v_n, a_n, b_n, then [D][C] mu_d, sigma2_d, r_d.
+struct LdbnGeom {
+  int N, C, HW, D;
+  int nhwc, bf16;
+  int S, P;       // segments per row, pixels per segment
+  int qc, pr;     // channels-last: float4 columns x pixel rows of a CTA
+};
+struct LdbnFin {
+  int N, C, D, S;
+  double M;                   // HW
+  float eps, momentum;
+  int train, update_running;
+  const float* weights;       // [N][D]
+  float* rmean;               // [D][C]
+  float* rvar;                // [D][C]
+  const float* gamma;         // [C] or null (with beta)
+  const float* beta;
+  float* save;
+  float* dgamma;              // backward: [C] or null (with dbeta)
+  float* dbeta;
+  int* status;
+};
+LdbnGeom ldbn_plan(int N, int C, int HW, int D, bool nhwc, bool bf16);
+int ldbn_finalize_ctas(int C);
+// scratch floats of a call: two partial arrays of `part`, four [N][C] arrays of `nc` (pilot and the apply coefficients),
+// dweights shares `dw`
+size_t ldbn_scratch_floats(const LdbnGeom& g, size_t* part, size_t* nc, size_t* dw);
+void ldbn_stats(const void* x, const LdbnGeom& g, float* pa, float* pb, float* pilot, cudaStream_t st);
+void ldbn_fwd_finalize(const LdbnFin& f, const float* pa, const float* pb, const float* pilot, float* alpha, float* shift,
+                       cudaStream_t st);
+void ldbn_apply(const void* x, void* y, const LdbnGeom& g, const float* alpha, const float* shift, cudaStream_t st);
+void ldbn_bwd_reduce(const void* x, const void* dy, const LdbnGeom& g, const float* centre, float* pa, float* pb,
+                     cudaStream_t st);
+// dweights null: no dwpart, no ldbn_dw launch
+void ldbn_bwd_finalize(const LdbnFin& f, const float* pa, const float* pb, float* ca, float* cp, float* cq, float* dwpart,
+                       float* dweights, cudaStream_t st);
+void ldbn_bwd_apply(const void* x, const void* dy, void* dx, const LdbnGeom& g, const float* ca, const float* cp,
+                    const float* cq, const float* centre, cudaStream_t st);
+
 // channels-last max-pool (pool.cu); bf16: x, y, dy, dx are bf16 (compared and summed in fp32, stored rounded)
 void maxpool_fwd_launch(const void* x, void* y, bool bf16, uint8_t* idx, int N, int H, int W, int C, int OH, int OW, int k, int s, int p,
                         cudaStream_t st);

@@ -694,6 +694,105 @@ def latent_domain_whiten(x, weights, *, group_size, training_stats, eps, momentu
     return _apply_per_image(_LatentFunction, x, weights.float(), *args)
 
 
+class _LatentBatchNormFunction(torch.autograd.Function):
+    """Latent-domain batch norm (dwt_bn_latent_fwd / _bwd) of x [N, C, *] under weights [N, n_domains] (float32, on the
+    device).  x is float32 or bfloat16, NCHW-contiguous or channels-last as latent_domain_batch_norm routes it; gamma /
+    beta are [C]-sized or both None; running = (mean [D, C], var [D, C]).  Gradients of x, weights (when it needs one),
+    gamma and beta."""
+
+    @staticmethod
+    def forward(ctx, x, weights, gamma, beta, fmt, mode, eps, momentum, update_running, running):
+        dev = nv.require_cuda(x, bf16=True)
+        rm_t, rv_t = running
+        nv.require_cuda(weights, gamma, beta, rm_t, rv_t)
+        lib = nv.lib()
+        n, c, hw = x.shape[0], x.shape[1], math.prod(x.shape[2:])
+        k = weights.shape[1]
+        w_c = weights.detach().contiguous()
+        need_running = (mode == nv.MODE_EVAL) or update_running
+        if need_running:
+            _check_param("running mean", rm_t, k * c)
+            _check_param("running var", rv_t, k * c)
+        _check_param("gamma / weight", gamma, c)
+        _check_param("beta / bias", beta, c)
+        gamma_c = None if gamma is None else gamma.detach().reshape(-1).contiguous()
+        beta_c = None if beta is None else beta.detach().reshape(-1).contiguous()
+        flags = mode | (nv.LAYOUT_NHWC if fmt == torch.channels_last else 0) | (nv.DTYPE_BF16 if x.dtype == torch.bfloat16 else 0)
+        y = torch.empty_like(x)
+        save = torch.empty((4 * n + 3 * k) * c, dtype=torch.float32, device=dev)
+        ws = nv.grow_workspace(dev, lib.dwt_bn_latent_workspace_bytes(n, c, hw, k))
+        rm, rv = (nv.ptr(rm_t), nv.ptr(rv_t)) if need_running else (None, None)
+        with torch.cuda.device(dev):
+            rc = lib.dwt_bn_latent_fwd(nv.ptr(x), nv.ptr(y), n, c, hw, k, flags, eps, momentum, int(update_running), rm, rv,
+                                       nv.ptr(w_c), nv.ptr(gamma_c), nv.ptr(beta_c), nv.ptr(save), nv.ptr(ws), ws.numel(),
+                                       nv.stream_ptr(dev))
+        nv.check(rc)
+        nv.poll_status(dev)
+        if update_running and mode == nv.MODE_TRAIN:
+            _bump_versions([running])
+        ctx.save_for_backward(x, w_c, gamma_c, save)
+        ctx.cfg = (flags, eps, n, c, hw, k, fmt, None if gamma is None else (gamma.shape, beta.shape))
+        return y
+
+    @staticmethod
+    def backward(ctx, dout):
+        lib = nv.lib()
+        x, w_c, gamma_c, save = ctx.saved_tensors
+        flags, eps, n, c, hw, k, fmt, shapes = ctx.cfg
+        dout, _ = _prepare_dout(ctx, dout, x, fmt, 8 if x.dtype == torch.bfloat16 else 16)
+        dev = nv.require_cuda(dout, bf16=True)
+        dx = torch.empty_like(x)
+        dw = torch.empty(n, k, dtype=torch.float32, device=dev) if ctx.needs_input_grad[1] else None
+        want_affine = gamma_c is not None and (ctx.needs_input_grad[2] or ctx.needs_input_grad[3])
+        dgamma = torch.empty(c, dtype=torch.float32, device=dev) if want_affine else None
+        dbeta = torch.empty(c, dtype=torch.float32, device=dev) if want_affine else None
+        ws = nv.grow_workspace(dev, lib.dwt_bn_latent_workspace_bytes(n, c, hw, k))
+        with torch.cuda.device(dev):
+            rc = lib.dwt_bn_latent_bwd(nv.ptr(x), nv.ptr(dout), nv.ptr(dx), n, c, hw, k, flags, eps, nv.ptr(w_c),
+                                       nv.ptr(gamma_c), nv.ptr(save), nv.ptr(dw), nv.ptr(dgamma), nv.ptr(dbeta), nv.ptr(ws),
+                                       ws.numel(), nv.stream_ptr(dev))
+        nv.check(rc)
+        if want_affine:
+            dgamma, dbeta = dgamma.view(shapes[0]), dbeta.view(shapes[1])
+        return dx, dw, dgamma, dbeta, None, None, None, None, None, None
+
+
+def latent_domain_batch_norm(x, weights, weight, bias, *, training_stats, eps, momentum, update_running, running):
+    """Latent-domain batch norm of x [N, C, *] under per-image domain weights [N, D] (used as given: no softmax, no value
+    checks; cast to float32).  Per channel, with each image's own mean and (biased) variance m_n, v_n and s_d = sum_n w_nd:
+        mu_d = sum_n w_nd m_n / s_d,  sigma2_d = sum_n w_nd [v_n + (m_n - mu_d)^2] / s_d  (training_stats=False: the
+        running buffers),  y_n = weight * sum_d w_nd (x_n - mu_d) / sqrt(sigma2_d + eps) + bias.
+    weight / bias: [C]-sized or both None.  A domain whose weights sum to exactly 0 is skipped (its weights get gradient
+    0).  running = (mean [D, C], var [D, C]): read when training_stats is False; updated with (mu_d, the unbiased sigma2_d)
+    by momentum when training_stats and update_running.  x, weights, weight and bias get their gradients.
+    The latent-domain batch-norm kernels (dwt_bn_latent_*; dwt_b200.h) take every shape.  A channels-last x whose C is not
+    a multiple of 4 runs as an NCHW copy; a bfloat16 NCHW x whose H*W is not a multiple of 4 runs the float32 kernels on
+    an upcast copy, the result in bfloat16."""
+    if x.dim() < 2:
+        raise ValueError(f"latent-domain batch norm expects [N, C, *] input (got {x.dim()}D input)")
+    if weights.dim() != 2 or weights.shape[0] != x.shape[0]:
+        raise ValueError(f"latent-domain batch norm expects weights of shape [N, n_domains] with N = {x.shape[0]} "
+                         f"(got {list(weights.shape)})")
+    if not weights.is_floating_point():
+        raise TypeError(f"latent-domain batch norm expects floating-point weights (got {weights.dtype})")
+    if weights.device != x.device:
+        raise ValueError(f"latent-domain batch norm expects weights on x's device {x.device} (got {weights.device})")
+    if (weight is None) != (bias is None):
+        raise ValueError("latent-domain batch norm takes weight and bias together, or neither")
+    nv.require_cuda(x, bf16=True)
+    mode = nv.MODE_TRAIN if training_stats else nv.MODE_EVAL
+    args = (mode, float(eps), float(momentum), bool(update_running), tuple(running))
+    fmt = torch.channels_last if _channels_last(x) and x.shape[1] % 4 == 0 else torch.contiguous_format
+    xk = x
+    if x.dtype == torch.bfloat16 and fmt == torch.contiguous_format and math.prod(x.shape[2:]) % 4:
+        xk = x.float()
+    xk = xk.contiguous(memory_format=fmt)
+    if xk.data_ptr() % (8 if xk.dtype == torch.bfloat16 else 16):
+        xk = xk.clone(memory_format=fmt)
+    y = _LatentBatchNormFunction.apply(xk, weights.float(), weight, bias, fmt, *args)
+    return y.to(x.dtype)
+
+
 class _MecFunction(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, y):

@@ -24,6 +24,8 @@
  *   dwt_whiten_switch_fwd/bwd  switchable whitening: a learned mix of batch and per-image statistics (not in the reference)
  *   dwt_whiten_latent_fwd/bwd  latent-domain whitening: statistics of up to 8 domains under per-image soft weights (not in
  *                    the reference)
+ *   dwt_bn_latent_fwd/bwd  latent-domain batch norm: batch norm by the statistics of up to 8 domains under per-image soft
+ *                    weights (the mDA layer; not in the reference)
  *   dwt_bn_fwd/bwd   _BatchNorm.forward             utils/batch_norm.py:54-69
  *   dwt_tail2_fwd/bwd  the residual tail of a downsampling Bottleneck: two norm sites and the ReLU in one pass
  *                    resnet50_dwt_mec_officehome.py:236-240
@@ -420,6 +422,70 @@ DWT_API int dwt_whiten_latent_bwd(const float *x, const float *dout, float *dx, 
                    int group_size, int n_domains, int mode, float eps, const float *weights, const float *save_mean,
                    const float *save_w, const float *save_stats, float *dweights, void *workspace, size_t workspace_bytes,
                    dwt_stream_t stream);
+
+/*
+ * Latent-domain batch norm (the mDA layer of Mancini et al., CVPR 2018, in its batch-norm form): D = n_domains domains
+ * whose membership is a weight per image, weights [N, D], as dwt_whiten_latent_*.  Per channel c, with M = HW, each
+ * image's own mean and biased variance m_n, v_n and s_d = sum_n w_nd:
+ *     mu_d = sum_n w_nd m_n / s_d,   sigma2_d = sum_n w_nd [v_n + (m_n - mu_d)^2] / s_d   (DWT_MODE_EVAL: domain d's
+ *     running_mean / running_var instead),   r_d = (sigma2_d + eps)^-1/2,
+ *     y_n = gamma sum_d w_nd r_d (x_n - mu_d) + beta = gamma (a_n x_n + b_n) + beta,  a_n = sum_d w_nd r_d,
+ *     b_n = -sum_d w_nd r_d mu_d   (gamma = beta = NULL: no affine).
+ * weights are used as given (no softmax, normalisation or sign check).  With one-hot weights every domain's output and
+ * buffers are those of F.batch_norm on its subset of the batch.
+ * Edge rules, per (domain, channel) unless said otherwise:
+ *   - s_d == 0 exactly: the domain is skipped -- no share in any output, buffers untouched, no status, dweights[:, d] = 0;
+ *   - s_d < 0 or NaN, mu_d or sigma2_d not finite, or sigma2_d + eps <= 0: r_d = NaN, DWT_STATUS_NOT_PD, that domain's EMA
+ *     skipped for that channel;
+ *   - every sum over images or domains skips a weight that is exactly 0 instead of multiplying by it: an image with
+ *     weight 0 on a bad domain stays finite, and so does its dx;
+ *   - an (image, channel) whose a_n is not positive and finite or whose b_n is not finite gets a_n = NaN, b_n = 0 (NaN
+ *     output and dx there) and sets DWT_STATUS_NOT_PD;
+ *   - 0 < M s_d <= 1 (the unbiased variance is undefined): the buffers stay untouched, no status; the output still uses
+ *     the biased sigma2_d.
+ * DWT_MODE_TRAIN with update_running: running_mean_d = (1-momentum) running_mean_d + momentum mu_d and running_var_d =
+ * (1-momentum) running_var_d + momentum sigma2_d M s_d / (M s_d - 1), F.batch_norm's convention.  DWT_MODE_EVAL reads the
+ * buffers and writes nothing; s_d still comes from the weights (the zero-mass rule).
+ * dwt_bn_latent_bwd is the exact gradient of the forward (in eval mu_d and sigma2_d are constants).  With g = gamma dout,
+ * G_n = sum_pixels g, H_n = sum_pixels g (x - m_n), A_d = sum_n w_nd G_n, B_d = sum_n w_nd [H_n + G_n (m_n - mu_d)]:
+ *     dx = a_n g - sum_d (w_nd / (M s_d)) [r_d A_d + r_d^3 B_d (x - mu_d)]                               (eval: a_n g)
+ *     dweights_nd = sum_c { r_d [H_n + G_n (m_n - mu_d)]
+ *                           - (1/s_d) [r_d A_d (m_n - mu_d) + r_d^3 B_d (v_n + (m_n - mu_d)^2 - sigma2_d) / 2] }  (eval: first term)
+ *     dgamma = sum dout zhat, dbeta = sum dout (from the sums of dout, so gamma = 0 is fine).
+ *   x, y, dout, dx  [N, C, HW] (or channels-last [N, HW, C] with DWT_LAYOUT_NHWC), fp32 or bf16 (DWT_DTYPE_BF16);
+ *                   fp32 16-byte, bf16 8-byte aligned (else DWT_E_INVALID)
+ *   n_domains       D, 1..DWT_MAX_LATENT_DOMAINS (else DWT_E_INVALID)
+ *   mode            DWT_MODE_TRAIN / DWT_MODE_EVAL | DWT_LAYOUT_NHWC | DWT_DTYPE_BF16 (any other bit: DWT_E_INVALID)
+ *   running_mean, running_var [D, C] (contiguous): read in eval, updated in train with update_running (else unused, may be
+ *                   NULL)
+ *   weights [N, D]  fp32, device
+ *   gamma, beta     [C] or both NULL;  dgamma, dbeta [C] or both NULL (written, never accumulated; they need gamma)
+ *   save_stats      (4 N + 3 D) C floats, 16-byte aligned, written by fwd and read by bwd: [N][C] m_n (eval: the centre
+ *                   -b_n / a_n, 0 for a bad image), [N][C] v_n (train), [N][C] a_n, [N][C] b_n, then [D][C] mu_d,
+ *                   [D][C] sigma2_d, [D][C] r_d (0 for a skipped domain)
+ *   dweights [N, D] written (never accumulated) by bwd; NULL skips it
+ *   eps             bwd: unused (r_d is saved); kept so both calls take the forward's arguments
+ * Statistics are per-(image, channel) sums about the row's first pixel; the domain moments are taken from them in fp64
+ * about image 0's mean, and every reduction runs in a fixed order (no float atomics): reruns are bit-identical, dweights,
+ * dgamma and dbeta included.  Apart from the statistics pass and the backward reduction nothing reads x again: 12 B per
+ * element forward, 20 B backward in fp32 (eval forward: 8 B).  bf16 loads widen to fp32 and stores round to nearest-even
+ * on the fp32 plan of the shape: every bf16 output is the fp32 call's output on the widened input, rounded.
+ * Geometry: any C >= 1 and HW >= 1 with N*C*HW < 2^31; channels-last needs C % 4 == 0 and NCHW bf16 HW % 4 == 0.  Anything
+ * else is DWT_E_UNSUPPORTED with a text naming latent-domain batch norm.
+ * Workspace: dwt_bn_latent_workspace_bytes(N, C, HW, n_domains) bytes, 256-byte aligned, zero-filled once (it may be the
+ * same buffer as the other entry points'; the status word is shared).  It returns 0 for a call the entry points refuse for
+ * its geometry or n_domains.  Neither call syncs the host; both may be captured into a CUDA graph.
+ * Profile families ldbn_stats, ldbn_fwd_finalize, ldbn_apply, ldbn_bwd_reduce, ldbn_bwd_finalize, ldbn_bwd_apply
+ * (_nhwc, _bf16 on the bandwidth passes).
+ */
+DWT_API size_t dwt_bn_latent_workspace_bytes(int64_t N, int64_t C, int64_t HW, int n_domains);
+DWT_API int dwt_bn_latent_fwd(const float *x, float *y, int64_t N, int64_t C, int64_t HW, int n_domains, int mode, float eps,
+                   float momentum, int update_running, float *running_mean, float *running_var, const float *weights,
+                   const float *gamma, const float *beta, float *save_stats, void *workspace, size_t workspace_bytes,
+                   dwt_stream_t stream);
+DWT_API int dwt_bn_latent_bwd(const float *x, const float *dout, float *dx, int64_t N, int64_t C, int64_t HW, int n_domains,
+                   int mode, float eps, const float *weights, const float *gamma, const float *save_stats, float *dweights,
+                   float *dgamma, float *dbeta, void *workspace, size_t workspace_bytes, dwt_stream_t stream);
 
 /*
  * Domain batch norm (F.batch_norm semantics): biased batch variance normalises,
