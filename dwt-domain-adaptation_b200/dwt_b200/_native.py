@@ -106,6 +106,16 @@ _SIGNATURES = {
                                              ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float,
                                              _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_void_p,
                                              ctypes.c_size_t, ctypes.c_void_p]),
+    "dwt_latent_small_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int64, ctypes.c_int64, ctypes.c_int64, ctypes.c_int,
+                                                           ctypes.c_int]),
+    "dwt_whiten_latent_small_fwd": (ctypes.c_int, [_c_float_p, _c_float_p, ctypes.c_int64, ctypes.c_int64, ctypes.c_int64,
+                                                   ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float,
+                                                   ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
+                                                   _c_float_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]),
+    "dwt_whiten_latent_small_bwd": (ctypes.c_int, [_c_float_p, _c_float_p, _c_float_p, ctypes.c_int64, ctypes.c_int64,
+                                                   ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float,
+                                                   _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, ctypes.c_void_p,
+                                                   ctypes.c_size_t, ctypes.c_void_p]),
     "dwt_bn_latent_workspace_bytes": (ctypes.c_size_t, [ctypes.c_int64, ctypes.c_int64, ctypes.c_int64, ctypes.c_int]),
     "dwt_bn_latent_fwd": (ctypes.c_int, [_c_float_p, _c_float_p, ctypes.c_int64, ctypes.c_int64, ctypes.c_int64, ctypes.c_int,
                                          ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_int, _c_float_p, _c_float_p,

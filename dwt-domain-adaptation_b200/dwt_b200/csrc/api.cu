@@ -1187,6 +1187,102 @@ dwt::Geom ldbn_prof_geom(const dwt::LdbnGeom& g) {
   return gm;
 }
 
+// ---- latent-domain whitening at group sizes 1, 2, 4 (dwt_whiten_latent_small_*) -----------------------------------------
+// Forward: lds_stats -> lds_fwd_finalize (per-image moments, per-domain W_k + EMA, per-image A_n, m~_n) -> lds_apply;
+// backward: lds_bwd_reduce about the images' own means -> lds_bwd_finalize (+ the dweights sum when it is given) ->
+// lds_bwd_apply (norm_ldbn.cu, on latent-domain batch norm's segments).  Scratch behind the common head: the segment
+// partials, the pilot shifts, the per-image fp64 moments, the backward's per-image sums, per-domain P_k | mubar_k and
+// <P_k, Sigma_k>, the apply coefficients and the dweights shares.
+struct LdsWork { float *part, *pilot, *red, *pd, *pc, *coef, *dw; double* im; size_t bytes; };
+
+LdsWork carve_lds(void* base, const dwt::LdbnGeom& g, int GS, int K) {
+  const size_t NG = (size_t)g.N * (g.C / GS), KG = (size_t)K * (g.C / GS);
+  size_t off = kOffScratch;
+  char* b = static_cast<char*>(base);
+  auto take = [&](size_t bytes) { size_t o = off; off = align_up(off + bytes, 256); return b + o; };
+  LdsWork w;
+  w.part = reinterpret_cast<float*>(take(sizeof(float) * NG * g.S * dwt::lds_partial_floats(GS)));
+  w.pilot = reinterpret_cast<float*>(take(sizeof(float) * (size_t)g.N * g.C));
+  w.im = reinterpret_cast<double*>(take(sizeof(double) * NG * (GS + GS * (GS + 1) / 2)));
+  w.red = reinterpret_cast<float*>(take(sizeof(float) * NG * (GS + GS * GS)));
+  w.pd = reinterpret_cast<float*>(take(sizeof(float) * KG * (GS * GS + GS)));
+  w.pc = reinterpret_cast<float*>(take(sizeof(float) * KG));
+  w.coef = reinterpret_cast<float*>(take(sizeof(float) * NG * dwt::lds_coef_floats(GS)));
+  w.dw = reinterpret_cast<float*>(take(sizeof(float) * NG * dwt::kLdsMaxDomains));
+  w.bytes = off;
+  return w;
+}
+
+// n_domains, mode bits and geometry (no device call); fills the plan
+int lds_geom(dwt::LdbnGeom& g, int64_t N, int64_t C, int64_t HW, int GS, int K, int mode) {
+  if (K < 1 || K > DWT_MAX_LATENT_DOMAINS)
+    return fail(DWT_E_INVALID, "n_domains %d outside [1,%d] (latent-domain whitening)", K, DWT_MAX_LATENT_DOMAINS);
+  if (mode & ~(DWT_MODE_EVAL | DWT_LAYOUT_NHWC | DWT_DTYPE_BF16))
+    return fail(DWT_E_INVALID, "bad mode %#x (DWT_MODE_TRAIN or DWT_MODE_EVAL | DWT_LAYOUT_NHWC | DWT_DTYPE_BF16)", mode);
+  if (N <= 0 || C <= 0 || HW <= 0) return fail(DWT_E_INVALID, "empty tensor (N=%lld C=%lld HW=%lld)", (long long)N,
+                                               (long long)C, (long long)HW);
+  const bool nhwc = (mode & DWT_LAYOUT_NHWC) != 0, bf16 = (mode & DWT_DTYPE_BF16) != 0;
+  if ((GS != 1 && GS != 2 && GS != 4) || C % GS != 0)
+    return fail(DWT_E_UNSUPPORTED, "latent-domain whitening at group sizes 1, 2, 4 needs group_size 1, 2 or 4 dividing C "
+                "(C=%lld gs=%d)", (long long)C, GS);
+  if ((double)N * (double)C * (double)HW >= 2147483648.0)
+    return fail(DWT_E_UNSUPPORTED, "latent-domain whitening at group sizes 1, 2, 4 needs N*C*HW < 2^31 (N=%lld C=%lld "
+                "HW=%lld)", (long long)N, (long long)C, (long long)HW);
+  if (nhwc && C % 4 != 0)
+    return fail(DWT_E_UNSUPPORTED, "latent-domain whitening at group sizes 1, 2, 4 runs channels-last at C %% 4 == 0 only "
+                "(C=%lld)", (long long)C);
+  if (bf16 && !nhwc && HW % 4 != 0)
+    return fail(DWT_E_UNSUPPORTED, "latent-domain whitening at group sizes 1, 2, 4 runs NCHW bf16 at HW %% 4 == 0 only "
+                "(HW=%lld)", (long long)HW);
+  g = dwt::lds_plan((int)N, (int)C, (int)HW, GS, K, nhwc, bf16);
+  return DWT_OK;
+}
+
+// The checks both directions make, in order: geometry, pointers, alignment, workspace.  act: the activation tensors.
+int lds_validate(dwt::LdbnGeom& g, LdsWork& w, int64_t N, int64_t C, int64_t HW, int GS, int K, int mode,
+                 const void* const (&act)[3], const float* weights, const float* save_mean, const float* save_w,
+                 const float* save_stats, void* ws, size_t ws_bytes) {
+  if (int rc = lds_geom(g, N, C, HW, GS, K, mode)) return rc;
+  if (!act[0] || !act[1] || !act[2] || !weights || !save_mean || !save_w || !save_stats || !ws)
+    return fail(DWT_E_INVALID, "null pointer argument");
+  const uintptr_t bits = (uintptr_t)act[0] | (uintptr_t)act[1] | (uintptr_t)act[2];
+  if (bits % (g.bf16 ? 8 : 16) != 0)
+    return fail(DWT_E_INVALID, "activation tensors must be %d-byte aligned (latent-domain whitening)", g.bf16 ? 8 : 16);
+  if (((uintptr_t)weights | (uintptr_t)save_w | (uintptr_t)save_stats) % 16 != 0 || (uintptr_t)save_mean % 4 != 0)
+    return fail(DWT_E_INVALID, "weights, save_w and save_stats must be 16-byte and save_mean 4-byte aligned "
+                "(latent-domain whitening)");
+  w = carve_lds(ws, g, GS, K);
+  if (w.bytes > ws_bytes) return fail(DWT_E_WORKSPACE, "workspace too small: need %zu bytes, got %zu", w.bytes, ws_bytes);
+  if ((uintptr_t)ws % 256 != 0) return fail(DWT_E_WORKSPACE, "workspace must be 256-byte aligned");
+  return DWT_OK;
+}
+
+dwt::LdsFin make_lds_fin(const dwt::LdbnGeom& g, int GS, int K, int mode, float eps, const float* weights,
+                         const float* save_mean, const float* save_w, const float* save_stats, void* ws) {
+  dwt::LdsFin f{};
+  f.N = g.N; f.C = g.C; f.GS = GS; f.G = g.C / GS; f.K = K; f.S = g.S; f.M = (double)g.HW;
+  f.a = 1.f - eps; f.b = eps; f.train = (mode & DWT_MODE_EVAL) == 0; f.weights = weights;
+  f.save_mean = const_cast<float*>(save_mean); f.save_w = const_cast<float*>(save_w);
+  f.save_stats = const_cast<float*>(save_stats);
+  f.status = static_cast<int*>(ws);
+  return f;
+}
+
+// Profile family of a launch: [pass][channels-last * 2 + bf16]
+const char* const kLdsName[6][4] = {
+    {"lds_stats", "lds_stats_bf16", "lds_stats_nhwc", "lds_stats_nhwc_bf16"},
+    {"lds_fwd_finalize", "lds_fwd_finalize", "lds_fwd_finalize", "lds_fwd_finalize"},
+    {"lds_apply", "lds_apply_bf16", "lds_apply_nhwc", "lds_apply_nhwc_bf16"},
+    {"lds_bwd_reduce", "lds_bwd_reduce_bf16", "lds_bwd_reduce_nhwc", "lds_bwd_reduce_nhwc_bf16"},
+    {"lds_bwd_finalize", "lds_bwd_finalize", "lds_bwd_finalize", "lds_bwd_finalize"},
+    {"lds_bwd_apply", "lds_bwd_apply_bf16", "lds_bwd_apply_nhwc", "lds_bwd_apply_nhwc_bf16"}};
+
+dwt::Geom lds_prof_geom(const dwt::LdbnGeom& g, int GS, int K) {
+  dwt::Geom gm{};
+  gm.N = g.N; gm.C = g.C; gm.HW = g.HW; gm.GS = GS; gm.G = g.C / GS; gm.D = K;
+  return gm;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1344,6 +1440,92 @@ int dwt_bn_latent_bwd(const float* x, const float* dout, float* dx, int64_t N, i
     dwt::ldbn_bwd_apply(x, dout, dx, g, w.c0, w.c1, w.c2, centre, st);
   }
   return check_launch("latent-domain batch norm backward apply kernel");
+}
+
+size_t dwt_latent_small_workspace_bytes(int64_t N, int64_t C, int64_t HW, int group_size, int n_domains) {
+  char saved[sizeof(g_err)];
+  memcpy(saved, g_err, sizeof(g_err));
+  size_t bytes = 0;
+  dwt::LdbnGeom g;
+  // the larger of the two layouts' plans (channels-last only where it runs)
+  for (int mode : {0, DWT_LAYOUT_NHWC})
+    if (lds_geom(g, N, C, HW, group_size, n_domains, mode) == DWT_OK) {
+      const size_t b = carve_lds(nullptr, g, group_size, n_domains).bytes;
+      if (b > bytes) bytes = b;
+    }
+  memcpy(g_err, saved, sizeof(g_err));
+  return bytes;
+}
+
+int dwt_whiten_latent_small_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, int group_size, int n_domains,
+                                int mode, float eps, float momentum, int update_running, float* running_mean,
+                                float* running_cov, const float* weights, float* save_mean, float* save_w,
+                                float* save_stats, void* workspace, size_t workspace_bytes, dwt_stream_t stream) {
+  dwt::LdbnGeom g;
+  LdsWork w;
+  const void* const act[3] = {x, x, y};
+  if (int rc = lds_validate(g, w, N, C, HW, group_size, n_domains, mode, act, weights, save_mean, save_w, save_stats,
+                            workspace, workspace_bytes))
+    return rc;
+  const bool train = (mode & DWT_MODE_EVAL) == 0;
+  if ((!train || update_running) && (!running_mean || !running_cov))
+    return fail(DWT_E_INVALID, "running buffer is null (eval, or train with update_running)");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int GS = group_size;
+  dwt::LdsFin f = make_lds_fin(g, GS, n_domains, mode, eps, weights, save_mean, save_w, save_stats, workspace);
+  f.momentum = momentum; f.update_running = train && update_running; f.rmean = running_mean; f.rcov = running_cov;
+  const dwt::Geom pg = lds_prof_geom(g, GS, n_domains);
+  const int k = 2 * g.nhwc + g.bf16;
+  const double E = (g.bf16 ? 2.0 : 4.0) * (double)N * (double)C * (double)HW;
+  {
+    Launch l(kLdsName[0][k], &pg, E, st);
+    dwt::lds_stats(x, g, GS, w.part, w.pilot, st);
+  }
+  if (int rc = check_launch("latent-domain whitening statistics kernel")) return rc;
+  {
+    Launch l(kLdsName[1][k], &pg, 0.0, st);
+    dwt::lds_fwd_finalize(f, w.part, w.pilot, w.im, st);
+  }
+  if (int rc = check_launch("latent-domain whitening finalize kernel")) return rc;
+  {
+    Launch l(kLdsName[2][k], &pg, 2.0 * E, st);
+    dwt::lds_apply(x, y, g, GS, save_mean, save_w, st);
+  }
+  return check_launch("latent-domain whitening apply kernel");
+}
+
+int dwt_whiten_latent_small_bwd(const float* x, const float* dout, float* dx, int64_t N, int64_t C, int64_t HW,
+                                int group_size, int n_domains, int mode, float eps, const float* weights,
+                                const float* save_mean, const float* save_w, const float* save_stats, float* dweights,
+                                void* workspace, size_t workspace_bytes, dwt_stream_t stream) {
+  dwt::LdbnGeom g;
+  LdsWork w;
+  const void* const act[3] = {x, dout, dx};
+  if (int rc = lds_validate(g, w, N, C, HW, group_size, n_domains, mode, act, weights, save_mean, save_w, save_stats,
+                            workspace, workspace_bytes))
+    return rc;
+  if ((uintptr_t)dweights % 4 != 0) return fail(DWT_E_INVALID, "dweights must be 4-byte aligned (latent-domain whitening)");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int GS = group_size;
+  const dwt::LdsFin f = make_lds_fin(g, GS, n_domains, mode, eps, weights, save_mean, save_w, save_stats, workspace);
+  const dwt::Geom pg = lds_prof_geom(g, GS, n_domains);
+  const int k = 2 * g.nhwc + g.bf16;
+  const double E = (g.bf16 ? 2.0 : 4.0) * (double)N * (double)C * (double)HW;
+  {
+    Launch l(kLdsName[3][k], &pg, 2.0 * E, st);
+    dwt::lds_bwd_reduce(x, dout, g, GS, save_stats, w.part, st);
+  }
+  if (int rc = check_launch("latent-domain whitening backward reduction kernel")) return rc;
+  {
+    Launch l(kLdsName[4][k], &pg, 0.0, st);
+    dwt::lds_bwd_finalize(f, w.part, w.red, w.pd, w.pc, w.coef, w.dw, dweights, st);
+  }
+  if (int rc = check_launch("latent-domain whitening backward finalize kernel")) return rc;
+  {
+    Launch l(kLdsName[5][k], &pg, 3.0 * E, st);
+    dwt::lds_bwd_apply(x, dout, dx, g, GS, w.coef, st);
+  }
+  return check_launch("latent-domain whitening backward apply kernel");
 }
 
 const char* dwt_last_error(void) { return g_err; }

@@ -221,6 +221,48 @@ void ldbn_bwd_finalize(const LdbnFin& f, const float* pa, const float* pb, float
 void ldbn_bwd_apply(const void* x, const void* dy, void* dx, const LdbnGeom& g, const float* ca, const float* cp,
                     const float* cq, const float* centre, cudaStream_t st);
 
+// latent-domain whitening at group sizes 1, 2, 4 (norm_ldbn.cu; dwt_whiten_latent_small_*) on latent-domain batch
+// norm's segments: NCHW a warp per (image, group, segment) reads the group's gs channel rows, planned by ldbn_plan over
+// N x C/gs rows; channels-last ldbn_plan's CTAs, a thread's 4 channels being 4/gs whole groups.  Partials
+// [N][S][G][lds_partial_floats]: forward the gs sums and the gs(gs+1)/2 lower cross-products about the pilot (each row's
+// first pixel), backward g_n = sum dy and R_n = sum dy (x - m_n)^T about the image's own mean.  save_stats and the
+// save layout are dwt_whiten_latent_*'s.
+struct LdsFin {
+  int N, C, G, GS, K, S;
+  double M;                   // HW
+  float a, b;                 // S = a Sigma + b I (1 - eps, eps)
+  float momentum;
+  int train, update_running;
+  const float* weights;       // [N][K]
+  float* rmean;               // [K][C]
+  float* rcov;                // [K][G][gs*gs]
+  float* save_mean;           // [N][C]  m~_n
+  float* save_w;              // [N][G][gs*gs]  A_n
+  float* save_stats;
+  int* status;
+};
+constexpr int kLdsMaxDomains = 8;   // dweights shares per (image, group)
+static_assert(DWT_MAX_LATENT_DOMAINS <= kLdsMaxDomains, "latent-domain whitening: raise kLdsMaxDomains with the header limit");
+LdbnGeom lds_plan(int N, int C, int HW, int GS, int K, bool nhwc, bool bf16);
+// floats per (image, segment, group) partial: the larger of the forward's and the backward's
+int lds_partial_floats(int GS);
+// floats per (image, group) of the backward apply's coefficients: A_n (lower) | B_n | c_n | m_n
+int lds_coef_floats(int GS);
+// forward: statistics -> finalize (per-image moments into save_stats and im [N][G][gs + gs(gs+1)/2] fp64, then per
+// (domain, group) moments, W_k and EMA, then per (image, group) A_n, m~_n) -> apply y = A_n (x - m~_n)
+void lds_stats(const void* x, const LdbnGeom& g, int GS, float* part, float* pilot, cudaStream_t st);
+void lds_fwd_finalize(const LdsFin& f, const float* part, const float* pilot, double* im, cudaStream_t st);
+void lds_apply(const void* x, void* y, const LdbnGeom& g, int GS, const float* save_mean, const float* save_w,
+               cudaStream_t st);
+// backward: reduction about the saved image means -> finalize (red [N][G][gs + gs^2], pd [K][G][gs^2 + gs] P_k | mubar_k,
+// pc [K][G] <P_k, Sigma_k>, coef [N][G][lds_coef_floats], dwpart [N][G][kLdsMaxDomains]; dweights null: no dwpart)
+// -> apply dx = A_n^T dy + B_n (x - m_n) + c_n
+void lds_bwd_reduce(const void* x, const void* dy, const LdbnGeom& g, int GS, const float* save_stats, float* part,
+                    cudaStream_t st);
+void lds_bwd_finalize(const LdsFin& f, const float* part, float* red, float* pd, float* pc, float* coef, float* dwpart,
+                      float* dweights, cudaStream_t st);
+void lds_bwd_apply(const void* x, const void* dy, void* dx, const LdbnGeom& g, int GS, const float* coef, cudaStream_t st);
+
 // channels-last max-pool (pool.cu); bf16: x, y, dy, dx are bf16 (compared and summed in fp32, stored rounded)
 void maxpool_fwd_launch(const void* x, void* y, bool bf16, uint8_t* idx, int N, int H, int W, int C, int OH, int OW, int k, int s, int p,
                         cudaStream_t st);

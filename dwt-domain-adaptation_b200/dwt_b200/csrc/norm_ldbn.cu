@@ -12,6 +12,11 @@
 //
 // Finalize kernels: a CTA per 32 channels, lane = channel, warp w takes images w, w + 8, ...; the eight warps' sums are
 // added in warp order through shared memory (block_sum).
+//
+// Latent-domain whitening at group sizes 1, 2, 4 (dwt_whiten_latent_small_*, the lds_* kernels below) runs on the same
+// plan and passes, a group of GS channels in place of one channel.
+#include <type_traits>
+
 #include "norm_launch.h"
 
 namespace dwt {
@@ -494,6 +499,765 @@ __global__ void __launch_bounds__(kThreads) ldbn_apply_nhwc(const T* __restrict_
   }
 }
 
+// ------------------------------------------------------------------------------------------------------------------------
+// Latent-domain whitening at group sizes 1, 2, 4 (dwt_whiten_latent_small_*): the same four bandwidth passes on the same
+// segments, a group of GS channels in place of one channel.  The reductions keep per group the GS sums and the
+// GS(GS+1)/2 lower cross-products about the pilot (forward), or g_n = sum dy and the full R_n = sum dy (x - m_n)^T
+// (backward); the apply passes hold their group's coefficients in registers for a whole segment.  The finalize
+// kernels give every (image, group) its own thread and every (domain, group) its own warp (a domain's 14 forward and 20
+// backward fp64 sums at GS 4 do not fit LDBN's per-lane layout, and one thread walking every image is latency-bound);
+// all sums run in a fixed order, the domain moments in fp64 about image 0's mean.
+// ------------------------------------------------------------------------------------------------------------------------
+template <int GS> struct LdsDim {
+  static constexpr int T = GS * (GS + 1) / 2;            // lower triangle
+  static constexpr int NF = GS + T;                      // forward partial: sums | lower cross-products
+  static constexpr int NB = GS + GS * GS;                // backward partial: g | R row-major
+  static constexpr int REC = GS * GS + GS;               // a save_stats record: (cov, mean)
+  static constexpr int NCF = T + GS;                     // forward apply: A lower | -A m~
+  static constexpr int NCB = T + GS * GS + 2 * GS;       // backward apply: A lower | B | c | m
+  static constexpr int PER4 = 4 / GS;                    // whole groups in a float4 of channels
+};
+
+// NCHW: four float4 loads of x in flight per lane and iteration, as ldbn_reduce_nchw's unrolled loop
+template <int GS> constexpr int kLdsVecUnroll = 4 / GS;
+
+__device__ __forceinline__ float lane4(const float4& v, int e) { return e == 0 ? v.x : e == 1 ? v.y : e == 2 ? v.z : v.w; }
+
+// one pixel of one group into its partials at a[o..]: forward d = x - K, the sums of d_i, then d_i d_j (j <= i) row by
+// row; backward d = x - K (K: the image mean), the sums of dy_i, then dy_i d_j row-major
+template <int GS, bool BWD, int NA>
+__device__ __forceinline__ void lds_acc(float (&a)[NA], int o, const float (&x)[GS], const float (&dy)[GS],
+                                        const float (&K)[GS]) {
+  float d[GS];
+#pragma unroll
+  for (int i = 0; i < GS; ++i) d[i] = x[i] - K[i];
+#pragma unroll
+  for (int i = 0; i < GS; ++i) {
+    if (BWD) {
+      a[o + i] += dy[i];
+#pragma unroll
+      for (int j = 0; j < GS; ++j) a[o + GS + i * GS + j] = fmaf(dy[i], d[j], a[o + GS + i * GS + j]);
+    } else {
+      a[o + i] += d[i];
+#pragma unroll
+      for (int j = 0; j <= i; ++j) a[o + GS + i * (i + 1) / 2 + j] = fmaf(d[i], d[j], a[o + GS + i * (i + 1) / 2 + j]);
+    }
+  }
+}
+
+// a group's apply coefficients into cf[o..]: forward A_n's lower triangle and bp = -A_n m~_n; backward the finalize's
+// A_n lower | B_n | c_n | m_n.  gi = n G + group.
+template <int GS, bool BWD, int NC>
+__device__ __forceinline__ void lds_load(float (&cf)[NC], int o, size_t gi, const float* save_mean, const float* save_w,
+                                         const float* coef) {
+  using Dm = LdsDim<GS>;
+  if (BWD) {
+#pragma unroll
+    for (int k = 0; k < Dm::NCB; ++k) cf[o + k] = __ldg(coef + gi * Dm::NCB + k);
+  } else {
+#pragma unroll
+    for (int i = 0; i < GS; ++i) {
+      float b = 0.f;
+#pragma unroll
+      for (int j = 0; j <= i; ++j) {
+        const float w = __ldg(save_w + gi * GS * GS + i * GS + j);
+        b = fmaf(-w, __ldg(save_mean + gi * GS + j), b);
+        cf[o + i * (i + 1) / 2 + j] = w;
+      }
+      cf[o + Dm::T + i] = b;
+    }
+  }
+}
+
+// forward y_i = bp_i + sum_{j<=i} A_ij x_j;  backward dx_i = c_i + sum_j B_ij (x_j - m_j) + sum_{j>=i} A_ji dy_j
+template <int GS, bool BWD, int NC>
+__device__ __forceinline__ void lds_map(const float (&cf)[NC], int o, const float (&x)[GS], const float (&dy)[GS],
+                                        float (&out)[GS]) {
+  constexpr int T = LdsDim<GS>::T;
+#pragma unroll
+  for (int i = 0; i < GS; ++i) {
+    float acc;
+    if (BWD) {
+      acc = cf[o + T + GS * GS + i];
+#pragma unroll
+      for (int j = 0; j < GS; ++j) acc = fmaf(cf[o + T + i * GS + j], x[j] - cf[o + T + GS * GS + GS + j], acc);
+#pragma unroll
+      for (int j = i; j < GS; ++j) acc = fmaf(cf[o + j * (j + 1) / 2 + i], dy[j], acc);
+    } else {
+      acc = cf[o + T + i];
+#pragma unroll
+      for (int j = 0; j <= i; ++j) acc = fmaf(cf[o + i * (i + 1) / 2 + j], x[j], acc);
+    }
+    out[i] = acc;
+  }
+}
+
+// NCHW reduction: a warp per (image, group, segment) over the group's GS rows.  VEC: HW % 4 == 0.  stats: save_stats
+// (backward: the image means are the centre).
+template <int GS, bool BWD, bool VEC, class T>
+__global__ void __launch_bounds__(kThreads, 1) lds_reduce_nchw(const T* __restrict__ x, const T* __restrict__ dy, LdbnGeom g,
+                                                            const float* __restrict__ stats, float* __restrict__ part,
+                                                            float* __restrict__ pilot) {
+  using Dm = LdsDim<GS>;
+  constexpr int NA = BWD ? Dm::NB : Dm::NF;
+  const long long wid = ((long long)blockIdx.x * kThreads + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  const int G = g.C / GS;
+  const long long rows = (long long)g.N * G;
+  if (wid >= rows * g.S) return;
+  const long long row = wid / g.S;                       // n G + group
+  const int s = (int)(wid - row * g.S);
+  const size_t base = (size_t)row * GS * g.HW;
+  float K[GS];
+#pragma unroll
+  for (int i = 0; i < GS; ++i) K[i] = BWD ? stats[row * Dm::REC + GS * GS + i] : ld1(x + base + (size_t)i * g.HW);
+  const int p0 = s * g.P, p1 = min(p0 + g.P, g.HW);
+  float a[NA];
+#pragma unroll
+  for (int k = 0; k < NA; ++k) a[k] = 0.f;
+  float xv[GS], dv[GS];
+  if (VEC) {
+#pragma unroll kLdsVecUnroll<GS>
+    for (int p = p0 + 4 * lane; p < p1; p += 128) {
+      float4 v[GS], d[GS];
+#pragma unroll
+      for (int i = 0; i < GS; ++i) {
+        v[i] = ld4(x + base + (size_t)i * g.HW + p);
+        d[i] = BWD ? ld4(dy + base + (size_t)i * g.HW + p) : float4{};
+      }
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+#pragma unroll
+        for (int i = 0; i < GS; ++i) { xv[i] = lane4(v[i], e); dv[i] = lane4(d[i], e); }
+        lds_acc<GS, BWD>(a, 0, xv, dv, K);
+      }
+    }
+  } else {
+#pragma unroll 4
+    for (int p = p0 + lane; p < p1; p += 32) {
+#pragma unroll
+      for (int i = 0; i < GS; ++i) {
+        xv[i] = ld1(x + base + (size_t)i * g.HW + p);
+        dv[i] = BWD ? ld1(dy + base + (size_t)i * g.HW + p) : 0.f;
+      }
+      lds_acc<GS, BWD>(a, 0, xv, dv, K);
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < NA; ++k) a[k] = warp_sum(a[k]);
+  if (lane == 0) {
+    const long long n = row / G;
+    float* o = part + (((size_t)n * g.S + s) * G + (size_t)(row - n * G)) * NA;
+#pragma unroll
+    for (int k = 0; k < NA; ++k) o[k] = a[k];
+    if (!BWD && s == 0) {
+#pragma unroll
+      for (int i = 0; i < GS; ++i) pilot[row * GS + i] = K[i];
+    }
+  }
+}
+
+// channels-last reduction: ldbn_reduce_nhwc's CTA (slab, segment, image); a thread's 4 channels are 4/GS groups, the
+// pixel rows added in order through shared memory
+template <int GS, bool BWD, class T>
+__global__ void __launch_bounds__(kThreads, 1) lds_reduce_nhwc(const T* __restrict__ x, const T* __restrict__ dy, LdbnGeom g,
+                                                            const float* __restrict__ stats, float* __restrict__ part,
+                                                            float* __restrict__ pilot) {
+  using Dm = LdsDim<GS>;
+  constexpr int NA = BWD ? Dm::NB : Dm::NF, NV = Dm::PER4 * NA;
+  __shared__ float sm[NV * kThreads];
+  const int slabs = (g.C / 4 + g.qc - 1) / g.qc;
+  int b = blockIdx.x;
+  const int slab = b % slabs; b /= slabs;
+  const int s = b % g.S;
+  const int n = b / g.S;
+  const int q = threadIdx.x % g.qc, r = threadIdx.x / g.qc;
+  const int c4 = slab * g.qc + q;
+  const int G = g.C / GS;
+  const bool on = r < g.pr && c4 < g.C / 4;
+  float a[NV];
+#pragma unroll
+  for (int k = 0; k < NV; ++k) a[k] = 0.f;
+  if (on) {
+    const size_t img = (size_t)n * g.HW * g.C + 4 * c4;
+    float K[4];
+    if (BWD) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int ch = 4 * c4 + j;
+        K[j] = stats[((size_t)n * G + ch / GS) * Dm::REC + GS * GS + ch % GS];
+      }
+    } else {
+      const float4 k = ld4(x + img);
+      K[0] = k.x; K[1] = k.y; K[2] = k.z; K[3] = k.w;
+    }
+    const int p0 = s * g.P, p1 = min(p0 + g.P, g.HW);
+#pragma unroll 4
+    for (int p = p0 + r; p < p1; p += g.pr) {
+      const float4 v = ld4(x + img + (size_t)p * g.C);
+      const float4 d = BWD ? ld4(dy + img + (size_t)p * g.C) : float4{};
+#pragma unroll
+      for (int t = 0; t < Dm::PER4; ++t) {
+        float xv[GS], dv[GS], kv[GS];
+#pragma unroll
+        for (int i = 0; i < GS; ++i) { xv[i] = lane4(v, t * GS + i); dv[i] = lane4(d, t * GS + i); kv[i] = K[t * GS + i]; }
+        lds_acc<GS, BWD>(a, t * NA, xv, dv, kv);
+      }
+    }
+    if (!BWD && s == 0 && r == 0)
+      *reinterpret_cast<float4*>(pilot + (size_t)n * g.C + 4 * c4) = make_float4(K[0], K[1], K[2], K[3]);
+  }
+#pragma unroll
+  for (int k = 0; k < NV; ++k) sm[k * kThreads + threadIdx.x] = a[k];
+  __syncthreads();
+  if (on && r == 0) {
+    for (int rr = 1; rr < g.pr; ++rr)
+#pragma unroll
+      for (int k = 0; k < NV; ++k) a[k] += sm[k * kThreads + rr * g.qc + q];
+    float* o = part + (((size_t)n * g.S + s) * G + 4 * c4 / GS) * NA;
+#pragma unroll
+    for (int k = 0; k < NV; ++k) o[k] = a[k];
+  }
+}
+
+// NCHW apply: the reduction's warps, the group's coefficients held for the segment
+template <int GS, bool BWD, bool VEC, class T>
+__global__ void __launch_bounds__(kThreads, 1) lds_apply_nchw(const T* __restrict__ x, const T* __restrict__ dy,
+                                                           T* __restrict__ out, LdbnGeom g, const float* __restrict__ save_mean,
+                                                           const float* __restrict__ save_w, const float* __restrict__ coef) {
+  using Dm = LdsDim<GS>;
+  constexpr int NC = BWD ? Dm::NCB : Dm::NCF;
+  const long long wid = ((long long)blockIdx.x * kThreads + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  const long long rows = (long long)g.N * (g.C / GS);
+  if (wid >= rows * g.S) return;
+  const long long row = wid / g.S;
+  const int s = (int)(wid - row * g.S);
+  const size_t base = (size_t)row * GS * g.HW;
+  float cf[NC];
+  lds_load<GS, BWD>(cf, 0, (size_t)row, save_mean, save_w, coef);
+  const int p0 = s * g.P, p1 = min(p0 + g.P, g.HW);
+  float xv[GS], dv[GS], ov[GS];
+  if (VEC) {
+#pragma unroll kLdsVecUnroll<GS>
+    for (int p = p0 + 4 * lane; p < p1; p += 128) {
+      float4 v[GS], d[GS];
+      float o4[GS][4];
+#pragma unroll
+      for (int i = 0; i < GS; ++i) {
+        v[i] = ld4(x + base + (size_t)i * g.HW + p);
+        d[i] = BWD ? ld4(dy + base + (size_t)i * g.HW + p) : float4{};
+      }
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+#pragma unroll
+        for (int i = 0; i < GS; ++i) { xv[i] = lane4(v[i], e); dv[i] = lane4(d[i], e); }
+        lds_map<GS, BWD>(cf, 0, xv, dv, ov);
+#pragma unroll
+        for (int i = 0; i < GS; ++i) o4[i][e] = ov[i];
+      }
+#pragma unroll
+      for (int i = 0; i < GS; ++i)
+        st4(out + base + (size_t)i * g.HW + p, make_float4(o4[i][0], o4[i][1], o4[i][2], o4[i][3]));
+    }
+  } else {
+#pragma unroll 4
+    for (int p = p0 + lane; p < p1; p += 32) {
+#pragma unroll
+      for (int i = 0; i < GS; ++i) {
+        xv[i] = ld1(x + base + (size_t)i * g.HW + p);
+        dv[i] = BWD ? ld1(dy + base + (size_t)i * g.HW + p) : 0.f;
+      }
+      lds_map<GS, BWD>(cf, 0, xv, dv, ov);
+#pragma unroll
+      for (int i = 0; i < GS; ++i) st1(out + base + (size_t)i * g.HW + p, ov[i]);
+    }
+  }
+}
+
+// channels-last apply: the reduction's CTAs, a thread's 4/GS groups' coefficients held for the segment
+template <int GS, bool BWD, class T>
+__global__ void __launch_bounds__(kThreads, 1) lds_apply_nhwc(const T* __restrict__ x, const T* __restrict__ dy,
+                                                           T* __restrict__ out, LdbnGeom g, const float* __restrict__ save_mean,
+                                                           const float* __restrict__ save_w, const float* __restrict__ coef) {
+  using Dm = LdsDim<GS>;
+  constexpr int NC = BWD ? Dm::NCB : Dm::NCF;
+  const int slabs = (g.C / 4 + g.qc - 1) / g.qc;
+  int b = blockIdx.x;
+  const int slab = b % slabs; b /= slabs;
+  const int s = b % g.S;
+  const int n = b / g.S;
+  const int q = threadIdx.x % g.qc, r = threadIdx.x / g.qc;
+  const int c4 = slab * g.qc + q;
+  if (r >= g.pr || c4 >= g.C / 4) return;
+  float cf[Dm::PER4 * NC];
+#pragma unroll
+  for (int t = 0; t < Dm::PER4; ++t)
+    lds_load<GS, BWD>(cf, t * NC, (size_t)n * (g.C / GS) + 4 * c4 / GS + t, save_mean, save_w, coef);
+  const size_t img = (size_t)n * g.HW * g.C + 4 * c4;
+  const int p0 = s * g.P, p1 = min(p0 + g.P, g.HW);
+#pragma unroll 4
+  for (int p = p0 + r; p < p1; p += g.pr) {
+    const float4 v = ld4(x + img + (size_t)p * g.C);
+    const float4 d = BWD ? ld4(dy + img + (size_t)p * g.C) : float4{};
+    float o[4];
+#pragma unroll
+    for (int t = 0; t < Dm::PER4; ++t) {
+      float xv[GS], dv[GS], ov[GS];
+#pragma unroll
+      for (int i = 0; i < GS; ++i) { xv[i] = lane4(v, t * GS + i); dv[i] = lane4(d, t * GS + i); }
+      lds_map<GS, BWD>(cf, t * NC, xv, dv, ov);
+#pragma unroll
+      for (int i = 0; i < GS; ++i) o[t * GS + i] = ov[i];
+    }
+    st4(out + img + (size_t)p * g.C, make_float4(o[0], o[1], o[2], o[3]));
+  }
+}
+
+// save_stats of dwt_whiten_latent_*: [N][G] records (C_n, m_n), [K][G] records (Sigma_k, mu_k), [K][G][GS*GS] W_k, [K] s_k
+template <int GS> struct LdsLayout {
+  float* base;
+  int N, G, K;
+  __device__ LdsLayout(const LdsFin& f) : base(f.save_stats), N(f.N), G(f.G), K(f.K) {}
+  __device__ float* img(size_t gi) const { return base + gi * LdsDim<GS>::REC; }
+  __device__ float* dom(int k, int g) const { return base + ((size_t)(N + k) * G + g) * LdsDim<GS>::REC; }
+  __device__ float* w(int k, int g) const { return base + ((size_t)(N + K) * G * LdsDim<GS>::REC) + ((size_t)k * G + g) * GS * GS; }
+  __device__ float* mass() const { return base + (size_t)(N + K) * G * LdsDim<GS>::REC + (size_t)K * G * GS * GS; }
+};
+
+// per (image, group): the segment partials added in order (fp64) into the image's mean and biased covariance about the
+// pilot; save_stats' image record and im (fp64: m | C lower)
+template <int GS>
+__global__ void __launch_bounds__(kThreads) lds_fwd_image(const LdsFin f, const float* __restrict__ part,
+                                                          const float* __restrict__ pilot, double* __restrict__ im) {
+  using Dm = LdsDim<GS>;
+  const int gi = blockIdx.x * kThreads + threadIdx.x;
+  if (gi >= f.N * f.G) return;
+  const int n = gi / f.G, grp = gi - n * f.G;
+  double s1[GS], s2[Dm::T];
+#pragma unroll
+  for (int i = 0; i < GS; ++i) s1[i] = 0.0;
+#pragma unroll
+  for (int t = 0; t < Dm::T; ++t) s2[t] = 0.0;
+  for (int j = 0; j < f.S; ++j) {
+    const float* p = part + (((size_t)n * f.S + j) * f.G + grp) * Dm::NF;
+#pragma unroll
+    for (int i = 0; i < GS; ++i) s1[i] += p[i];
+#pragma unroll
+    for (int t = 0; t < Dm::T; ++t) s2[t] += p[GS + t];
+  }
+  const LdsLayout<GS> L(f);
+  float* rec = L.img(gi);
+  double* o = im + (size_t)gi * Dm::NF;
+  double dm[GS];
+#pragma unroll
+  for (int i = 0; i < GS; ++i) {
+    dm[i] = s1[i] / f.M;
+    const double m = (double)pilot[(size_t)gi * GS + i] + dm[i];
+    o[i] = m;
+    rec[GS * GS + i] = (float)m;
+  }
+#pragma unroll
+  for (int i = 0; i < GS; ++i)
+#pragma unroll
+    for (int j = 0; j <= i; ++j) {
+      const double c = s2[i * (i + 1) / 2 + j] / f.M - dm[i] * dm[j];
+      o[GS + i * (i + 1) / 2 + j] = c;
+      rec[i * GS + j] = (float)c;
+      rec[j * GS + i] = (float)c;
+    }
+}
+
+// the sum of v over the warp by a fixed butterfly: every lane ends with the same, rerun-identical value
+__device__ __forceinline__ double warp_sum_d(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+// a warp per (domain, group): s_k (fp64, lane l takes images l, l + 32, ..., zero weights skipped, the lanes added by
+// warp_sum_d); train: mu_k, Sigma_k by the law of total covariance about image 0's mean, eval: the running buffers; then
+// lane 0: S_k = a Sigma_k + b I = L L^T, W_k = L^-1 (fp32) and the EMA.  s_k == 0: skipped (no W_k, no status, no EMA);
+// s_k < 0 or NaN, non-finite statistics or S_k not positive definite: W_k = NaN, DWT_STATUS_NOT_PD, no EMA.
+template <int GS>
+__global__ void __launch_bounds__(kThreads) lds_fwd_domain(const LdsFin f, const double* __restrict__ im) {
+  using Dm = LdsDim<GS>;
+  const int idx = (blockIdx.x * kThreads + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (idx >= f.K * f.G) return;
+  const int k = idx / f.G, grp = idx - k * f.G;
+  const LdsLayout<GS> L(f);
+  double ref[GS], a1[GS], a2[Dm::T], s = 0.0;
+#pragma unroll
+  for (int i = 0; i < GS; ++i) { ref[i] = im[(size_t)grp * Dm::NF + i]; a1[i] = 0.0; }
+#pragma unroll
+  for (int t = 0; t < Dm::T; ++t) a2[t] = 0.0;
+  for (int n = lane; n < f.N; n += 32) {
+    const float w = __ldg(f.weights + (size_t)n * f.K + k);
+    if (w == 0.f) continue;
+    s += (double)w;
+    if (!f.train) continue;
+    const double* r = im + ((size_t)n * f.G + grp) * Dm::NF;
+    const double dw = (double)w;
+    double e[GS];
+#pragma unroll
+    for (int i = 0; i < GS; ++i) { e[i] = r[i] - ref[i]; a1[i] += dw * e[i]; }
+#pragma unroll
+    for (int i = 0; i < GS; ++i)
+#pragma unroll
+      for (int j = 0; j <= i; ++j) a2[i * (i + 1) / 2 + j] += dw * (r[GS + i * (i + 1) / 2 + j] + e[i] * e[j]);
+  }
+  s = warp_sum_d(s);
+#pragma unroll
+  for (int i = 0; i < GS; ++i) a1[i] = warp_sum_d(a1[i]);
+#pragma unroll
+  for (int t = 0; t < Dm::T; ++t) a2[t] = warp_sum_d(a2[t]);
+  if (lane != 0) return;
+  const float sf = (float)s;
+  if (grp == 0) L.mass()[k] = sf;
+  float mu[GS], sig[GS][GS];
+  if (f.train) {
+    const double inv = s != 0.0 ? 1.0 / s : 0.0;
+    double mi[GS];
+#pragma unroll
+    for (int i = 0; i < GS; ++i) { mi[i] = a1[i] * inv; mu[i] = s != 0.0 ? (float)(ref[i] + mi[i]) : 0.f; }
+#pragma unroll
+    for (int i = 0; i < GS; ++i)
+#pragma unroll
+      for (int j = 0; j <= i; ++j) {
+        const float v = s != 0.0 ? (float)(a2[i * (i + 1) / 2 + j] * inv - mi[i] * mi[j]) : 0.f;
+        sig[i][j] = v; sig[j][i] = v;
+      }
+  } else {
+#pragma unroll
+    for (int i = 0; i < GS; ++i) {
+      mu[i] = f.rmean[(size_t)k * f.C + grp * GS + i];
+#pragma unroll
+      for (int j = 0; j < GS; ++j) sig[i][j] = f.rcov[((size_t)k * f.G + grp) * GS * GS + i * GS + j];
+    }
+  }
+  float* dr = L.dom(k, grp);
+#pragma unroll
+  for (int i = 0; i < GS; ++i) {
+    dr[GS * GS + i] = mu[i];
+#pragma unroll
+    for (int j = 0; j < GS; ++j) dr[i * GS + j] = sig[i][j];
+  }
+  if (sf == 0.f) return;
+  bool bad = !(sf > 0.f);
+  float Lm[GS][GS], W[GS][GS];
+#pragma unroll
+  for (int i = 0; i < GS; ++i) {
+    bad = bad || !isfinite(mu[i]);
+#pragma unroll
+    for (int j = 0; j < GS; ++j) {
+      Lm[i][j] = f.a * sig[i][j] + (i == j ? f.b : 0.f);
+      bad = bad || !isfinite(Lm[i][j]);
+      W[i][j] = 0.f;
+    }
+  }
+#pragma unroll
+  for (int c = 0; c < GS; ++c) {
+    bad = bad || !(Lm[c][c] > 0.f);
+    Lm[c][c] = sqrtf(Lm[c][c]);
+    const float inv = 1.f / Lm[c][c];
+#pragma unroll
+    for (int i = c + 1; i < GS; ++i) Lm[i][c] *= inv;
+#pragma unroll
+    for (int i = c + 1; i < GS; ++i)
+#pragma unroll
+      for (int j = c + 1; j <= i; ++j) Lm[i][j] -= Lm[i][c] * Lm[j][c];
+  }
+#pragma unroll
+  for (int j = 0; j < GS; ++j) {
+    W[j][j] = 1.f / Lm[j][j];
+#pragma unroll
+    for (int i = j + 1; i < GS; ++i) {
+      float acc = 0.f;
+#pragma unroll
+      for (int c = j; c < i; ++c) acc = fmaf(Lm[i][c], W[c][j], acc);
+      W[i][j] = -acc / Lm[i][i];
+    }
+  }
+  float* wr = L.w(k, grp);
+#pragma unroll
+  for (int i = 0; i < GS; ++i)
+#pragma unroll
+    for (int j = 0; j < GS; ++j) wr[i * GS + j] = bad ? __int_as_float(0x7fc00000) : W[i][j];
+  if (bad) { atomicOr(f.status, DWT_STATUS_NOT_PD); return; }
+  if (!f.train || !f.update_running) return;
+  const float m = f.momentum, km = 1.f - f.momentum;    // dwt_whiten_fwd's EMA on the unshrunk, biased moments
+  float* rc = f.rcov + ((size_t)k * f.G + grp) * GS * GS;
+  float* rm = f.rmean + (size_t)k * f.C + grp * GS;
+#pragma unroll
+  for (int i = 0; i < GS; ++i) {
+    rm[i] = fmaf(km, rm[i], __fmul_rn(m, mu[i]));
+#pragma unroll
+    for (int j = 0; j < GS; ++j) rc[i * GS + j] = m * sig[i][j] + km * rc[i * GS + j];
+  }
+}
+
+// per (image, group): A_n = sum_k w_nk W_k and b_n = sum_k w_nk W_k mu_k over the domains in order (skipping w_nk == 0
+// and s_k == 0), A_n m~_n = b_n by forward substitution.  A diagonal entry that is not positive and finite, or a
+// non-finite A_n or m~_n: A_n = NaN, m~_n = 0, DWT_STATUS_NOT_PD.
+template <int GS>
+__global__ void __launch_bounds__(kThreads) lds_fwd_mix(const LdsFin f) {
+  const int gi = blockIdx.x * kThreads + threadIdx.x;
+  if (gi >= f.N * f.G) return;
+  const int n = gi / f.G, grp = gi - n * f.G;
+  const LdsLayout<GS> L(f);
+  float A[GS][GS], b[GS];
+#pragma unroll
+  for (int i = 0; i < GS; ++i) {
+    b[i] = 0.f;
+#pragma unroll
+    for (int j = 0; j < GS; ++j) A[i][j] = 0.f;
+  }
+  for (int k = 0; k < f.K; ++k) {
+    const float w = __ldg(f.weights + (size_t)n * f.K + k);
+    if (w == 0.f || L.mass()[k] == 0.f) continue;
+    const float* Wk = L.w(k, grp);
+    const float* mk = L.dom(k, grp) + GS * GS;
+#pragma unroll
+    for (int i = 0; i < GS; ++i) {
+      float v = 0.f;
+#pragma unroll
+      for (int j = 0; j <= i; ++j) {
+        const float wij = Wk[i * GS + j];
+        A[i][j] = fmaf(w, wij, A[i][j]);
+        v = fmaf(wij, mk[j], v);
+      }
+      b[i] = fmaf(w, v, b[i]);
+    }
+  }
+  bool bad = false;
+  float z[GS];
+#pragma unroll
+  for (int i = 0; i < GS; ++i) {
+    float r = b[i];
+#pragma unroll
+    for (int j = 0; j < i; ++j) {
+      r = fmaf(-A[i][j], z[j], r);
+      bad = bad || !isfinite(A[i][j]);
+    }
+    bad = bad || !(A[i][i] > 0.f && A[i][i] < INFINITY);
+    z[i] = r / A[i][i];
+    bad = bad || !isfinite(z[i]);
+  }
+  float* sw = f.save_w + (size_t)gi * GS * GS;
+  float* sm = f.save_mean + (size_t)gi * GS;
+#pragma unroll
+  for (int i = 0; i < GS; ++i) {
+    sm[i] = bad ? 0.f : z[i];
+#pragma unroll
+    for (int j = 0; j < GS; ++j) sw[i * GS + j] = bad ? __int_as_float(0x7fc00000) : (j <= i ? A[i][j] : 0.f);
+  }
+  if (bad) atomicOr(f.status, DWT_STATUS_NOT_PD);
+}
+
+// per (image, group): the backward segment partials added in order (fp64) into red = g_n | R_n
+template <int GS>
+__global__ void __launch_bounds__(kThreads) lds_bwd_image(const LdsFin f, const float* __restrict__ part,
+                                                          float* __restrict__ red) {
+  using Dm = LdsDim<GS>;
+  const int gi = blockIdx.x * kThreads + threadIdx.x;
+  if (gi >= f.N * f.G) return;
+  const int n = gi / f.G, grp = gi - n * f.G;
+  double acc[Dm::NB];
+#pragma unroll
+  for (int k = 0; k < Dm::NB; ++k) acc[k] = 0.0;
+  for (int j = 0; j < f.S; ++j) {
+    const float* p = part + (((size_t)n * f.S + j) * f.G + grp) * Dm::NB;
+#pragma unroll
+    for (int k = 0; k < Dm::NB; ++k) acc[k] += p[k];
+  }
+#pragma unroll
+  for (int k = 0; k < Dm::NB; ++k) red[(size_t)gi * Dm::NB + k] = (float)acc[k];
+}
+
+// a warp per (domain, group), train, s_k != 0: Wbar_k = sum_n w_nk [R_n + g_n (m_n - mu_k)^T] and sum_n w_nk g_n (fp64,
+// lane l takes images l, l + 32, ..., zero weights skipped, the lanes added by warp_sum_d); then lane 0: the Cholesky
+// backward P_k = a sym(W^T Phi(-Wbar W^T) W) and mubar_k = -W_k^T sum_n w_nk g_n into pd, <P_k, Sigma_k> into pc
+template <int GS>
+__global__ void __launch_bounds__(kThreads) lds_bwd_domain(const LdsFin f, const float* __restrict__ red,
+                                                           float* __restrict__ pd, float* __restrict__ pc) {
+  using Dm = LdsDim<GS>;
+  const int idx = (blockIdx.x * kThreads + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (idx >= f.K * f.G) return;
+  const int k = idx / f.G, grp = idx - k * f.G;
+  const LdsLayout<GS> L(f);
+  if (L.mass()[k] == 0.f) return;
+  const float* dr = L.dom(k, grp);
+  double wb[GS][GS], gs[GS];
+#pragma unroll
+  for (int i = 0; i < GS; ++i) {
+    gs[i] = 0.0;
+#pragma unroll
+    for (int j = 0; j < GS; ++j) wb[i][j] = 0.0;
+  }
+  for (int n = lane; n < f.N; n += 32) {
+    const float w = __ldg(f.weights + (size_t)n * f.K + k);
+    if (w == 0.f) continue;
+    const size_t gi = (size_t)n * f.G + grp;
+    const float* r = red + gi * Dm::NB;
+    const float* mn = L.img(gi) + GS * GS;
+    const double dw = (double)w;
+#pragma unroll
+    for (int i = 0; i < GS; ++i) {
+      const double gi_ = r[i];
+      gs[i] += dw * gi_;
+#pragma unroll
+      for (int j = 0; j < GS; ++j)
+        wb[i][j] += dw * ((double)r[GS + i * GS + j] + gi_ * ((double)mn[j] - (double)dr[GS * GS + j]));
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < GS; ++i) {
+    gs[i] = warp_sum_d(gs[i]);
+#pragma unroll
+    for (int j = 0; j < GS; ++j) wb[i][j] = warp_sum_d(wb[i][j]);
+  }
+  if (lane != 0) return;
+  float W[GS][GS], P1[GS][GS], T[GS][GS], S[GS][GS];
+  const float* Wk = L.w(k, grp);
+#pragma unroll
+  for (int i = 0; i < GS; ++i)
+#pragma unroll
+    for (int j = 0; j < GS; ++j) W[i][j] = j <= i ? Wk[i * GS + j] : 0.f;
+#pragma unroll
+  for (int i = 0; i < GS; ++i)
+#pragma unroll
+    for (int j = 0; j < GS; ++j) {
+      float q = 0.f;
+      if (j <= i) {
+#pragma unroll
+        for (int l = 0; l <= j; ++l) q = fmaf((float)wb[i][l], W[j][l], q);
+        q *= i == j ? -0.5f : -1.f;
+      }
+      P1[i][j] = q;
+    }
+#pragma unroll
+  for (int i = 0; i < GS; ++i)
+#pragma unroll
+    for (int j = 0; j < GS; ++j) {
+      float t = 0.f;
+#pragma unroll
+      for (int l = (i > j ? i : j); l < GS; ++l) t = fmaf(W[l][i], P1[l][j], t);
+      T[i][j] = t;
+    }
+#pragma unroll
+  for (int i = 0; i < GS; ++i)
+#pragma unroll
+    for (int j = 0; j < GS; ++j) {
+      float t = 0.f;
+#pragma unroll
+      for (int l = j; l < GS; ++l) t = fmaf(T[i][l], W[l][j], t);
+      S[i][j] = t;
+    }
+  float* o = pd + (size_t)idx * Dm::REC;
+  const float h = 0.5f * f.a;
+  float c = 0.f;
+#pragma unroll
+  for (int i = 0; i < GS; ++i)
+#pragma unroll
+    for (int j = 0; j < GS; ++j) {
+      const float p = h * (S[i][j] + S[j][i]);
+      o[i * GS + j] = p;
+      c = fmaf(p, dr[i * GS + j], c);
+    }
+#pragma unroll
+  for (int i = 0; i < GS; ++i) {
+    float v = 0.f;
+#pragma unroll
+    for (int j = i; j < GS; ++j) v = fmaf(W[j][i], (float)gs[j], v);
+    o[GS * GS + i] = -v;
+  }
+  pc[idx] = c;
+}
+
+// per (image, group), the domains in order (skipping s_k == 0; the terms of dx also skip w_nk == 0, dweights does not),
+// with u_k = m_n - mu_k:  coef = A_n (lower) | B_n = train (2/M) sum_k (w_nk/s_k) P_k |
+// c_n = train (1/M) sum_k (w_nk/s_k) [mubar_k + 2 P_k u_k] | m_n, and
+// dwpart[k] = <W_k, R_n + g_n u_k^T> + train [<mubar_k, u_k> + <P_k, C_n + u_k u_k^T> - <P_k, Sigma_k>] / s_k
+template <int GS>
+__global__ void __launch_bounds__(kThreads) lds_bwd_coef(const LdsFin f, const float* __restrict__ red,
+                                                         const float* __restrict__ pd, const float* __restrict__ pc,
+                                                         float* __restrict__ coef, float* __restrict__ dwpart) {
+  using Dm = LdsDim<GS>;
+  const int gi = blockIdx.x * kThreads + threadIdx.x;
+  if (gi >= f.N * f.G) return;
+  const int n = gi / f.G, grp = gi - n * f.G;
+  const LdsLayout<GS> L(f);
+  const float* rec = L.img(gi);
+  const float* r = red + (size_t)gi * Dm::NB;
+  float m[GS], B[GS][GS], kv[GS];
+#pragma unroll
+  for (int i = 0; i < GS; ++i) {
+    m[i] = rec[GS * GS + i];
+    kv[i] = 0.f;
+#pragma unroll
+    for (int j = 0; j < GS; ++j) B[i][j] = 0.f;
+  }
+  for (int k = 0; k < f.K; ++k) {
+    const float sk = L.mass()[k];
+    float dw = 0.f;
+    if (sk != 0.f) {
+      const float rs = 1.f / sk, w = __ldg(f.weights + (size_t)n * f.K + k);
+      const float* dr = L.dom(k, grp);
+      const float* Wk = L.w(k, grp);
+      float u[GS];
+#pragma unroll
+      for (int i = 0; i < GS; ++i) u[i] = m[i] - dr[GS * GS + i];
+#pragma unroll
+      for (int i = 0; i < GS; ++i)
+#pragma unroll
+        for (int j = 0; j <= i; ++j) dw = fmaf(Wk[i * GS + j], fmaf(r[i], u[j], r[GS + i * GS + j]), dw);
+      if (f.train) {
+        const float* P = pd + ((size_t)k * f.G + grp) * Dm::REC;
+        const float wr = w * rs;
+        float t = -pc[(size_t)k * f.G + grp];
+#pragma unroll
+        for (int i = 0; i < GS; ++i) {
+          float pu = 0.f;
+#pragma unroll
+          for (int j = 0; j < GS; ++j) {
+            const float p = P[i * GS + j];
+            pu = fmaf(p, u[j], pu);
+            t = fmaf(p, fmaf(u[i], u[j], rec[i * GS + j]), t);
+            if (w != 0.f) B[i][j] = fmaf(wr, p, B[i][j]);
+          }
+          t = fmaf(P[GS * GS + i], u[i], t);
+          if (w != 0.f) kv[i] = fmaf(wr, fmaf(2.f, pu, P[GS * GS + i]), kv[i]);
+        }
+        dw = fmaf(rs, t, dw);
+      }
+    }
+    if (dwpart) dwpart[(size_t)gi * kLdsMaxDomains + k] = dw;
+  }
+  float* cf = coef + (size_t)gi * Dm::NCB;
+  const float* A = f.save_w + (size_t)gi * GS * GS;
+  const float invM = (float)(1.0 / f.M);
+#pragma unroll
+  for (int i = 0; i < GS; ++i) {
+#pragma unroll
+    for (int j = 0; j <= i; ++j) cf[i * (i + 1) / 2 + j] = A[i * GS + j];
+#pragma unroll
+    for (int j = 0; j < GS; ++j) cf[Dm::T + i * GS + j] = 2.f * invM * B[i][j];
+    cf[Dm::T + GS * GS + i] = kv[i] * invM;
+    cf[Dm::T + GS * GS + GS + i] = m[i];
+  }
+}
+
+// dweights[n][k] = the groups' shares in order (fp64)
+__global__ void __launch_bounds__(kThreads) lds_dw(const float* __restrict__ dwpart, int N, int G, int K,
+                                                   float* __restrict__ dweights) {
+  const int i = blockIdx.x * kThreads + threadIdx.x;
+  if (i >= N * K) return;
+  const int n = i / K, k = i - n * K;
+  double t = 0.0;
+  for (int g = 0; g < G; ++g) t += dwpart[((size_t)n * G + g) * kLdsMaxDomains + k];
+  dweights[i] = (float)t;
+}
+
 int sms() {
   static int n = 0;
   if (n == 0) {
@@ -612,6 +1376,111 @@ void ldbn_bwd_apply(const void* x, const void* dy, void* dx, const LdbnGeom& g, 
                     const float* cq, const float* centre, cudaStream_t st) {
   if (g.bf16) apply<true, __nv_bfloat16>(x, dy, dx, g, ca, cp, cq, centre, st);
   else apply<true, float>(x, dy, dx, g, ca, cp, cq, centre, st);
+}
+
+namespace {
+
+// grid of the bandwidth passes: NCHW a warp per (image, group, segment), channels-last a CTA per (slab, segment, image)
+unsigned lds_blocks(const LdbnGeom& g, int GS) {
+  if (g.nhwc) return (unsigned)((size_t)((g.C / 4 + g.qc - 1) / g.qc) * g.S * g.N);
+  const size_t warps = (size_t)g.N * (g.C / GS) * g.S;
+  return (unsigned)((warps + kWarps - 1) / kWarps);
+}
+
+// PASS 0: forward statistics, 1: forward apply, 2: backward reduction, 3: backward apply.  NCHW bf16 runs at HW % 4 == 0.
+template <int GS, int PASS, class T>
+void lds_launch(const void* x, const void* dy, void* out, const LdbnGeom& g, const float* p0, const float* p1,
+                const float* p2, float* part, float* pilot, cudaStream_t st) {
+  constexpr bool BWD = PASS >= 2, APPLY = PASS == 1 || PASS == 3;
+  const T* xt = static_cast<const T*>(x);
+  const T* dt = static_cast<const T*>(dy);
+  T* ot = static_cast<T*>(out);
+  const unsigned blocks = lds_blocks(g, GS);
+  if (g.nhwc) {
+    if constexpr (APPLY) lds_apply_nhwc<GS, BWD, T><<<blocks, kThreads, 0, st>>>(xt, dt, ot, g, p0, p1, p2);
+    else lds_reduce_nhwc<GS, BWD, T><<<blocks, kThreads, 0, st>>>(xt, dt, g, p0, part, pilot);
+    return;
+  }
+  if (g.HW % 4 == 0) {
+    if constexpr (APPLY) lds_apply_nchw<GS, BWD, true, T><<<blocks, kThreads, 0, st>>>(xt, dt, ot, g, p0, p1, p2);
+    else lds_reduce_nchw<GS, BWD, true, T><<<blocks, kThreads, 0, st>>>(xt, dt, g, p0, part, pilot);
+  } else if constexpr (std::is_same<T, float>::value) {
+    if constexpr (APPLY) lds_apply_nchw<GS, BWD, false, T><<<blocks, kThreads, 0, st>>>(xt, dt, ot, g, p0, p1, p2);
+    else lds_reduce_nchw<GS, BWD, false, T><<<blocks, kThreads, 0, st>>>(xt, dt, g, p0, part, pilot);
+  }
+}
+
+template <int PASS>
+void lds_pass(const void* x, const void* dy, void* out, const LdbnGeom& g, int GS, const float* p0, const float* p1,
+              const float* p2, float* part, float* pilot, cudaStream_t st) {
+#define DWT_LDS_GS(G_)                                                                                                   \
+  if (GS == G_) {                                                                                                        \
+    if (g.bf16) lds_launch<G_, PASS, __nv_bfloat16>(x, dy, out, g, p0, p1, p2, part, pilot, st);                         \
+    else lds_launch<G_, PASS, float>(x, dy, out, g, p0, p1, p2, part, pilot, st);                                        \
+  }
+  DWT_LDS_GS(1) else DWT_LDS_GS(2) else DWT_LDS_GS(4)
+#undef DWT_LDS_GS
+}
+
+unsigned lds_grid(int work) { return (unsigned)((work + kThreads - 1) / kThreads); }
+
+template <int GS>
+void lds_fwd_fin(const LdsFin& f, const float* part, const float* pilot, double* im, cudaStream_t st) {
+  lds_fwd_image<GS><<<lds_grid(f.N * f.G), kThreads, 0, st>>>(f, part, pilot, im);
+  lds_fwd_domain<GS><<<lds_grid(32 * f.K * f.G), kThreads, 0, st>>>(f, im);
+  lds_fwd_mix<GS><<<lds_grid(f.N * f.G), kThreads, 0, st>>>(f);
+}
+
+template <int GS>
+void lds_bwd_fin(const LdsFin& f, const float* part, float* red, float* pd, float* pc, float* coef, float* dwpart,
+                 float* dweights, cudaStream_t st) {
+  lds_bwd_image<GS><<<lds_grid(f.N * f.G), kThreads, 0, st>>>(f, part, red);
+  if (f.train) lds_bwd_domain<GS><<<lds_grid(32 * f.K * f.G), kThreads, 0, st>>>(f, red, pd, pc);
+  lds_bwd_coef<GS><<<lds_grid(f.N * f.G), kThreads, 0, st>>>(f, red, pd, pc, coef, dweights ? dwpart : nullptr);
+  if (dweights) lds_dw<<<lds_grid(f.N * f.K), kThreads, 0, st>>>(dwpart, f.N, f.G, f.K, dweights);
+}
+
+}  // namespace
+
+LdbnGeom lds_plan(int N, int C, int HW, int GS, int K, bool nhwc, bool bf16) {
+  LdbnGeom g = ldbn_plan(N, nhwc ? C : C / GS, HW, K, nhwc, bf16);
+  g.C = C;
+  return g;
+}
+
+int lds_partial_floats(int GS) { return GS + GS * GS; }   // the backward's g | R; the forward's GS + GS(GS+1)/2 fits
+
+int lds_coef_floats(int GS) { return GS * (GS + 1) / 2 + GS * GS + 2 * GS; }
+
+void lds_stats(const void* x, const LdbnGeom& g, int GS, float* part, float* pilot, cudaStream_t st) {
+  lds_pass<0>(x, nullptr, nullptr, g, GS, nullptr, nullptr, nullptr, part, pilot, st);
+}
+
+void lds_fwd_finalize(const LdsFin& f, const float* part, const float* pilot, double* im, cudaStream_t st) {
+  if (f.GS == 1) lds_fwd_fin<1>(f, part, pilot, im, st);
+  else if (f.GS == 2) lds_fwd_fin<2>(f, part, pilot, im, st);
+  else lds_fwd_fin<4>(f, part, pilot, im, st);
+}
+
+void lds_apply(const void* x, void* y, const LdbnGeom& g, int GS, const float* save_mean, const float* save_w,
+               cudaStream_t st) {
+  lds_pass<1>(x, nullptr, y, g, GS, save_mean, save_w, nullptr, nullptr, nullptr, st);
+}
+
+void lds_bwd_reduce(const void* x, const void* dy, const LdbnGeom& g, int GS, const float* save_stats, float* part,
+                    cudaStream_t st) {
+  lds_pass<2>(x, dy, nullptr, g, GS, save_stats, nullptr, nullptr, part, nullptr, st);
+}
+
+void lds_bwd_finalize(const LdsFin& f, const float* part, float* red, float* pd, float* pc, float* coef, float* dwpart,
+                      float* dweights, cudaStream_t st) {
+  if (f.GS == 1) lds_bwd_fin<1>(f, part, red, pd, pc, coef, dwpart, dweights, st);
+  else if (f.GS == 2) lds_bwd_fin<2>(f, part, red, pd, pc, coef, dwpart, dweights, st);
+  else lds_bwd_fin<4>(f, part, red, pd, pc, coef, dwpart, dweights, st);
+}
+
+void lds_bwd_apply(const void* x, const void* dy, void* dx, const LdbnGeom& g, int GS, const float* coef, cudaStream_t st) {
+  lds_pass<3>(x, dy, dx, g, GS, nullptr, nullptr, coef, nullptr, nullptr, st);
 }
 
 }  // namespace dwt

@@ -609,16 +609,20 @@ class _LatentFunction(torch.autograd.Function):
     n_domains latent domains under its row of weights [N, n_domains] (float32, on the device), per group of group_size
     channels, in the Cholesky basis.  The gradient of weights is returned.  Running buffers: (mean [D, C], second moment
     [D, C/gs, gs, gs]), one row per domain.  x is float32 or bfloat16, NCHW-contiguous or (4-D) channels-last; it goes to
-    the kernels in its own layout and dtype."""
+    the kernels in its own layout and dtype.  small: group sizes up to 4 on dwt_whiten_latent_small_* (x prepared by
+    latent_domain_whiten, fmt its layout), else the tensor-core entry points."""
 
     @staticmethod
-    def forward(ctx, x, weights, group_size, mode, eps, momentum, update_running, running):
+    def forward(ctx, x, weights, group_size, mode, eps, momentum, update_running, running, small=False, fmt=None):
         dev = nv.require_cuda(x, bf16=True)
         rm_t, rv_t = running
         nv.require_cuda(weights, rm_t, rv_t)
         lib = nv.lib()
         gs = group_size
-        x, fmt = _tma_ready(x)
+        if not small:
+            x, fmt = _tma_ready(x)
+        ws_bytes, fwd = ((lib.dwt_latent_small_workspace_bytes, lib.dwt_whiten_latent_small_fwd) if small
+                         else (lib.dwt_latent_workspace_bytes, lib.dwt_whiten_latent_fwd))
         n, c, hw = x.shape[0], x.shape[1], math.prod(x.shape[2:])
         k = weights.shape[1]
         w_c = _aligned(weights)
@@ -633,36 +637,36 @@ class _LatentFunction(torch.autograd.Function):
         save_mean = torch.empty(n, c, dtype=torch.float32, device=dev)
         save_w = torch.empty(n, g, gs, gs, dtype=torch.float32, device=dev)
         save_stats = torch.empty((n + k) * g * rec + k * g * gs * gs + k, dtype=torch.float32, device=dev)
-        ws = nv.grow_workspace(dev, lib.dwt_latent_workspace_bytes(n, c, hw, gs, k))
+        ws = nv.grow_workspace(dev, ws_bytes(n, c, hw, gs, k))
         rm, rv = (nv.ptr(rm_t), nv.ptr(rv_t)) if need_running else (None, None)
         with torch.cuda.device(dev):
-            rc = lib.dwt_whiten_latent_fwd(nv.ptr(x), nv.ptr(y), n, c, hw, gs, k, flags, eps, momentum, int(update_running),
-                                           rm, rv, nv.ptr(w_c), nv.ptr(save_mean), nv.ptr(save_w), nv.ptr(save_stats),
-                                           nv.ptr(ws), ws.numel(), nv.stream_ptr(dev))
+            rc = fwd(nv.ptr(x), nv.ptr(y), n, c, hw, gs, k, flags, eps, momentum, int(update_running), rm, rv, nv.ptr(w_c),
+                     nv.ptr(save_mean), nv.ptr(save_w), nv.ptr(save_stats), nv.ptr(ws), ws.numel(), nv.stream_ptr(dev))
         nv.check(rc)
         nv.poll_status(dev)
         if update_running and mode == nv.MODE_TRAIN:
             _bump_versions([running])
         ctx.save_for_backward(x, w_c, save_mean, save_w, save_stats)
-        ctx.cfg = (gs, flags, eps, n, c, hw, k, fmt)
+        ctx.cfg = (gs, flags, eps, n, c, hw, k, fmt, small)
         return y
 
     @staticmethod
     def backward(ctx, dout):
         lib = nv.lib()
         x, w_c, save_mean, save_w, save_stats = ctx.saved_tensors
-        gs, flags, eps, n, c, hw, k, fmt = ctx.cfg
+        gs, flags, eps, n, c, hw, k, fmt, small = ctx.cfg
+        ws_bytes, bwd = ((lib.dwt_latent_small_workspace_bytes, lib.dwt_whiten_latent_small_bwd) if small
+                         else (lib.dwt_latent_workspace_bytes, lib.dwt_whiten_latent_bwd))
         dout, _ = _prepare_dout(ctx, dout, x, fmt, 16)
         dev = nv.require_cuda(dout, bf16=True)
         dx = torch.empty_like(x)
         dw = torch.empty(n, k, dtype=torch.float32, device=dev) if ctx.needs_input_grad[1] else None
-        ws = nv.grow_workspace(dev, lib.dwt_latent_workspace_bytes(n, c, hw, gs, k))
+        ws = nv.grow_workspace(dev, ws_bytes(n, c, hw, gs, k))
         with torch.cuda.device(dev):
-            rc = lib.dwt_whiten_latent_bwd(nv.ptr(x), nv.ptr(dout), nv.ptr(dx), n, c, hw, gs, k, flags, eps, nv.ptr(w_c),
-                                           nv.ptr(save_mean), nv.ptr(save_w), nv.ptr(save_stats), nv.ptr(dw), nv.ptr(ws),
-                                           ws.numel(), nv.stream_ptr(dev))
+            rc = bwd(nv.ptr(x), nv.ptr(dout), nv.ptr(dx), n, c, hw, gs, k, flags, eps, nv.ptr(w_c), nv.ptr(save_mean),
+                     nv.ptr(save_w), nv.ptr(save_stats), nv.ptr(dw), nv.ptr(ws), ws.numel(), nv.stream_ptr(dev))
         nv.check(rc)
-        return dx, dw, None, None, None, None, None, None
+        return dx, dw, None, None, None, None, None, None, None, None
 
 
 def latent_domain_whiten(x, weights, *, group_size, training_stats, eps, momentum, update_running, running):
@@ -675,10 +679,13 @@ def latent_domain_whiten(x, weights, *, group_size, training_stats, eps, momentu
     A domain whose weights sum to exactly 0 is skipped (its weights get gradient 0).  running = (mean [D, C], second
     moment [D, C/gs, gs, gs]): read when training_stats is False; updated with (mu_d, Sigma_d) by momentum when
     training_stats and update_running.  weights gets its gradient.
-    The tensor-core kernels only (group sizes 8, 16, 32, 64, H*W >= 256, D <= 8; dwt_b200.h): a call they cannot take
-    raises NativeError with the library's reason and is never sent to another kernel family.  A bfloat16 NCHW x whose H*W
-    is not a multiple of 8 (the bf16 kernels' TMA rows) runs the same kernels in float32 on an upcast copy, the result in
-    bfloat16."""
+    Group sizes up to 4 run the register-resident kernels (dwt_whiten_latent_small_*; group sizes 1, 2, 4, any H*W):
+    a channels-last x whose C is not a multiple of 4 runs as an NCHW copy, and a bfloat16 NCHW x whose H*W is not a
+    multiple of 4 runs the float32 kernels on an upcast copy, the result in bfloat16.  Larger group sizes run the
+    tensor-core kernels (group sizes 8, 16, 32, 64, H*W >= 256; dwt_whiten_latent_*): a bfloat16 NCHW x whose H*W is not
+    a multiple of 8 (the bf16 kernels' TMA rows) runs them in float32 on an upcast copy, the result in bfloat16.  D <= 8
+    either way; a call the kernels cannot take raises NativeError with the library's reason and is never sent to another
+    kernel family."""
     if x.dim() < 3:
         raise ValueError(f"latent-domain whitening expects [N, C, *] input (got {x.dim()}D input)")
     if weights.dim() != 2 or weights.shape[0] != x.shape[0]:
@@ -691,7 +698,17 @@ def latent_domain_whiten(x, weights, *, group_size, training_stats, eps, momentu
     nv.require_cuda(x, bf16=True)
     mode = nv.MODE_TRAIN if training_stats else nv.MODE_EVAL
     args = (int(group_size), mode, float(eps), float(momentum), bool(update_running), tuple(running))
-    return _apply_per_image(_LatentFunction, x, weights.float(), *args)
+    if int(group_size) > 4:
+        return _apply_per_image(_LatentFunction, x, weights.float(), *args)
+    # latent-domain batch norm's preparation: the same four bandwidth passes take the same layouts
+    fmt = torch.channels_last if _channels_last(x) and x.shape[1] % 4 == 0 else torch.contiguous_format
+    xk = x
+    if x.dtype == torch.bfloat16 and fmt == torch.contiguous_format and math.prod(x.shape[2:]) % 4:
+        xk = x.float()
+    xk = xk.contiguous(memory_format=fmt)
+    if xk.data_ptr() % (8 if xk.dtype == torch.bfloat16 else 16):
+        xk = xk.clone(memory_format=fmt)
+    return _LatentFunction.apply(xk, weights.float(), *args, True, fmt).to(x.dtype)
 
 
 class _LatentBatchNormFunction(torch.autograd.Function):

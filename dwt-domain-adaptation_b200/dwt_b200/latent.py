@@ -1,5 +1,5 @@
 """Latent-domain whitening: whitening by the statistics of latent domains under per-image soft domain weights, on the
-tensor-core whitening kernels.
+register-resident kernels at group sizes 1, 2, 4 and the tensor-core whitening kernels at 8 to 64.
 
 ``LatentDomainWTransform2d`` is the whitening form of the mDA layer of Mancini et al., "Boosting Domain Adaptation by
 Discovering Latent Domains" (CVPR 2018).  ``WTransform2d`` and ``DomainTripleNorm`` need every domain as a contiguous,
@@ -15,9 +15,10 @@ their gradient.  A domain whose weights sum to exactly 0 is skipped: it adds to 
 Buffers hold one row per domain: ``running_mean`` [D, C] and ``running_variance`` [D, C/gs, gs, gs], initialised as
 ``WTransform2d``'s (zero mean, an all-ones matrix per group) and updated by its convention, so one-hot weights keep the
 buffers a ``WTransform2d`` per domain would.  ``group_size`` clamping, modes (train, eval, ``track_running_stats=False``)
-and error texts are ``WTransform2d``'s.  There is no affine; the caller adds it.  Group sizes 8, 16, 32, 64 with
-H*W >= 256, 1 <= D <= 8, float32 or bfloat16, NCHW or channels-last (dwt_whiten_latent_*, include/dwt_b200.h); anything
-else raises ``NativeError``.
+and error texts are ``WTransform2d``'s.  There is no affine; the caller adds it.  1 <= D <= 8, float32 or bfloat16,
+NCHW or channels-last.  Group sizes 1, 2, 4 take any H*W (dwt_whiten_latent_small_*: ResNet-50-DWT's stem and layer1
+sites and the digits LeNet's sites at group size 4; the clamping gives 1 or 2 on narrow layers); group sizes 8, 16, 32,
+64 need H*W >= 256 (dwt_whiten_latent_*, include/dwt_b200.h).  Anything else raises ``NativeError``.
 """
 from __future__ import annotations
 

@@ -24,6 +24,7 @@
  *   dwt_whiten_switch_fwd/bwd  switchable whitening: a learned mix of batch and per-image statistics (not in the reference)
  *   dwt_whiten_latent_fwd/bwd  latent-domain whitening: statistics of up to 8 domains under per-image soft weights (not in
  *                    the reference)
+ *   dwt_whiten_latent_small_fwd/bwd  the same at group sizes 1, 2, 4 and any H*W (not in the reference)
  *   dwt_bn_latent_fwd/bwd  latent-domain batch norm: batch norm by the statistics of up to 8 domains under per-image soft
  *                    weights (the mDA layer; not in the reference)
  *   dwt_bn_fwd/bwd   _BatchNorm.forward             utils/batch_norm.py:54-69
@@ -419,6 +420,41 @@ DWT_API int dwt_whiten_latent_fwd(const float *x, float *y, int64_t N, int64_t C
                    const float *weights, float *save_mean, float *save_w, float *save_stats,
                    void *workspace, size_t workspace_bytes, dwt_stream_t stream);
 DWT_API int dwt_whiten_latent_bwd(const float *x, const float *dout, float *dx, int64_t N, int64_t C, int64_t HW,
+                   int group_size, int n_domains, int mode, float eps, const float *weights, const float *save_mean,
+                   const float *save_w, const float *save_stats, float *dweights, void *workspace, size_t workspace_bytes,
+                   dwt_stream_t stream);
+
+/*
+ * Latent-domain whitening at group sizes 1, 2, 4 (the whitening sites of ResNet-50-DWT and the digits LeNet): the
+ * function, edge rules, EMA, backward, dweights and every argument and save layout of dwt_whiten_latent_fwd / _bwd
+ * above, so a caller changes only which symbols it calls.  What differs is the geometry and the kernels:
+ *   group_size 1, 2 or 4 dividing C, any HW >= 1, 1..DWT_MAX_LATENT_DOMAINS domains, N*C*HW < 2^31; channels-last needs
+ *   C % 4 == 0 and NCHW bf16 HW % 4 == 0.  Anything else is DWT_E_UNSUPPORTED with a text naming latent-domain whitening
+ *   at group sizes 1, 2, 4.
+ *   x, y, dout, dx fp32 16-byte, bf16 8-byte aligned; weights, save_w and save_stats 16-byte, save_mean and dweights
+ *   4-byte aligned (else DWT_E_INVALID).
+ * The kernels are latent-domain batch norm's four bandwidth passes on its segments, a group of gs channels in place of one
+ * channel: per (image, segment, group) the gs sums and gs(gs+1)/2 cross-products about each row's first pixel (forward)
+ * or g_n and R_n about the image's own mean (backward), then y = A_n (x - m~_n) and dx = A_n^T dout + B_n (x - m_n) + c_n
+ * with the per-image coefficients in registers.  The finalize kernels give every (image, group) a thread and every
+ * (domain, group) a warp; the domain moments are taken in fp64 about image 0's mean (lane l adds images l, l + 32, ...
+ * in order, then the lanes by a fixed butterfly) and every reduction runs in a fixed order (no float atomics): reruns
+ * are bit-identical, dweights included.  The statistics pass also runs in eval
+ * (the backward's centre is the image's own mean): 12 B per element forward, 20 B backward in fp32.  bf16 loads widen to
+ * fp32 and stores round to nearest-even on the fp32 plan of the shape: every bf16 output is the fp32 call's output on the
+ * widened input, rounded.  Neither call syncs the host; both may be captured into a CUDA graph.
+ * Workspace: dwt_latent_small_workspace_bytes(N, C, HW, group_size, n_domains) bytes, 256-byte aligned, zero-filled once
+ * (it may be the same buffer as the other entry points'; the status word is shared).  It returns 0 for a call the entry
+ * points refuse for its geometry or n_domains.
+ * Profile families lds_stats, lds_fwd_finalize, lds_apply, lds_bwd_reduce, lds_bwd_finalize, lds_bwd_apply (_nhwc, _bf16
+ * on the bandwidth passes).
+ */
+DWT_API size_t dwt_latent_small_workspace_bytes(int64_t N, int64_t C, int64_t HW, int group_size, int n_domains);
+DWT_API int dwt_whiten_latent_small_fwd(const float *x, float *y, int64_t N, int64_t C, int64_t HW, int group_size,
+                   int n_domains, int mode, float eps, float momentum, int update_running, float *running_mean,
+                   float *running_cov, const float *weights, float *save_mean, float *save_w, float *save_stats,
+                   void *workspace, size_t workspace_bytes, dwt_stream_t stream);
+DWT_API int dwt_whiten_latent_small_bwd(const float *x, const float *dout, float *dx, int64_t N, int64_t C, int64_t HW,
                    int group_size, int n_domains, int mode, float eps, const float *weights, const float *save_mean,
                    const float *save_w, const float *save_stats, float *dweights, void *workspace, size_t workspace_bytes,
                    dwt_stream_t stream);
