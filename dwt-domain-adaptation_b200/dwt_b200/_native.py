@@ -125,6 +125,16 @@ _SIGNATURES = {
                                          ctypes.c_int, ctypes.c_int, ctypes.c_float, _c_float_p, _c_float_p, _c_float_p,
                                          _c_float_p, _c_float_p, _c_float_p, ctypes.c_void_p, ctypes.c_size_t,
                                          ctypes.c_void_p]),
+    "dwt_latent_site_fwd": (ctypes.c_int, [ctypes.c_int, _c_float_p, _c_float_p, ctypes.c_int64, ctypes.c_int64,
+                                           ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float,
+                                           ctypes.c_float, ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
+                                           _c_float_p, _c_float_p, ctypes.c_void_p, ctypes.c_int, _c_float_p, _c_float_p,
+                                           _c_float_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]),
+    "dwt_latent_site_bwd": (ctypes.c_int, [ctypes.c_int, _c_float_p, _c_float_p, _c_float_p, ctypes.c_int64, ctypes.c_int64,
+                                           ctypes.c_int64, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_float,
+                                           _c_float_p, _c_float_p, _c_float_p, ctypes.c_void_p, _c_float_p, ctypes.c_int,
+                                           _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p, _c_float_p,
+                                           ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]),
     "dwt_bn_fwd": (ctypes.c_int, [_c_float_p, _c_float_p, ctypes.c_int64, ctypes.c_int64, ctypes.c_int64,
                                   ctypes.c_int, ctypes.c_int, ctypes.c_float, ctypes.c_float, ctypes.c_int,
                                   ctypes.POINTER(ctypes.c_void_p), ctypes.POINTER(ctypes.c_void_p), _c_float_p,

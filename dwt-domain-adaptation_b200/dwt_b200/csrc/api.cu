@@ -1283,6 +1283,217 @@ dwt::Geom lds_prof_geom(const dwt::LdbnGeom& g, int GS, int K) {
   return gm;
 }
 
+// dwt_bn_latent_fwd, and dwt_latent_site_fwd with a site epilogue epi (checked by the caller)
+int ldbn_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, int n_domains, int mode, float eps, float momentum,
+             int update_running, float* running_mean, float* running_var, const float* weights, const float* gamma,
+             const float* beta, float* save_stats, void* workspace, size_t workspace_bytes, dwt_stream_t stream, int epi,
+             const void* residual, uint8_t* relu_mask) {
+  dwt::LdbnGeom g;
+  LdbnWork w;
+  const void* const act[3] = {x, x, y};
+  if (int rc = ldbn_validate(g, w, N, C, HW, n_domains, mode, act, weights, save_stats, gamma, beta, workspace,
+                             workspace_bytes))
+    return rc;
+  const bool train = (mode & DWT_MODE_EVAL) == 0;
+  if ((!train || update_running) && (!running_mean || !running_var))
+    return fail(DWT_E_INVALID, "running buffer is null (eval, or train with update_running)");
+  cudaStream_t st = (cudaStream_t)stream;
+  dwt::LdbnFin f = make_ldbn_fin(g, mode, eps, weights, gamma, beta, save_stats, workspace);
+  f.momentum = momentum; f.update_running = train && update_running; f.rmean = running_mean; f.rvar = running_var;
+  const dwt::Geom pg = ldbn_prof_geom(g);
+  const int k = 2 * g.nhwc + g.bf16;
+  const double E = (g.bf16 ? 2.0 : 4.0) * (double)N * (double)C * (double)HW;
+  if (train) {
+    Launch l(kLdbnName[0][k], &pg, E, st);
+    dwt::ldbn_stats(x, g, w.pa, w.pb, w.pilot, st);
+  }
+  if (int rc = check_launch("latent-domain batch norm statistics kernel")) return rc;
+  {
+    Launch l(kLdbnName[1][k], &pg, 0.0, st);
+    dwt::ldbn_fwd_finalize(f, w.pa, w.pb, w.pilot, w.c0, w.c1, st);
+  }
+  if (int rc = check_launch("latent-domain batch norm finalize kernel")) return rc;
+  {
+    const bool res = (epi & DWT_EPI_RESIDUAL) != 0;
+    Launch l(kLdbnName[2][k], &pg, (res ? 3.0 : 2.0) * E + (relu_mask ? E / (g.bf16 ? 8.0 : 16.0) : 0.0), st);
+    if (epi & (DWT_EPI_RELU | DWT_EPI_RESIDUAL)) {
+      const float* save_a = save_stats + (size_t)2 * N * C;
+      const dwt::LdEpi ep{gamma, beta, save_a, save_a + (size_t)N * C, residual, relu_mask, nullptr};
+      dwt::ldbn_site_apply(x, y, g, w.c0, w.c1, epi, ep, st);
+    } else {
+      dwt::ldbn_apply(x, y, g, w.c0, w.c1, st);
+    }
+  }
+  return check_launch("latent-domain batch norm apply kernel");
+}
+
+// dwt_bn_latent_bwd, and dwt_latent_site_bwd with a site epilogue epi (checked by the caller)
+int ldbn_bwd(const float* x, const float* dout, float* dx, int64_t N, int64_t C, int64_t HW, int n_domains, int mode,
+             float eps, const float* weights, const float* gamma, const float* save_stats, float* dweights, float* dgamma,
+             float* dbeta, void* workspace, size_t workspace_bytes, dwt_stream_t stream, int epi, const float* beta,
+             const uint8_t* relu_mask, float* dresidual) {
+  dwt::LdbnGeom g;
+  LdbnWork w;
+  const void* const act[3] = {x, dout, dx};
+  if (int rc = ldbn_validate(g, w, N, C, HW, n_domains, mode, act, weights, save_stats, dgamma, dbeta, workspace,
+                             workspace_bytes))
+    return rc;
+  if (dgamma && !gamma) return fail(DWT_E_INVALID, "dgamma / dbeta given without gamma (latent-domain batch norm)");
+  if ((uintptr_t)dweights % 4 != 0) return fail(DWT_E_INVALID, "dweights must be 4-byte aligned (latent-domain batch norm)");
+  cudaStream_t st = (cudaStream_t)stream;
+  dwt::LdbnFin f = make_ldbn_fin(g, mode, eps, weights, gamma, nullptr, save_stats, workspace);
+  f.dgamma = dgamma; f.dbeta = dbeta;
+  const dwt::Geom pg = ldbn_prof_geom(g);
+  const int k = 2 * g.nhwc + g.bf16;
+  const double E = (g.bf16 ? 2.0 : 4.0) * (double)N * (double)C * (double)HW;
+  const float* centre = save_stats;                           // [N][C] first in save_stats
+  const float* save_a = save_stats + (size_t)2 * N * C;
+  const dwt::LdEpi ep{gamma, beta, save_a, save_a + (size_t)N * C, nullptr, const_cast<uint8_t*>(relu_mask), dresidual};
+  {
+    const bool mk = (epi & DWT_EPI_RESIDUAL) != 0;
+    Launch l(kLdbnName[3][k], &pg, (mk ? 3.0 : 2.0) * E + (mk ? E / (g.bf16 ? 8.0 : 16.0) : 0.0), st);
+    if (epi & DWT_EPI_RELU) dwt::ldbn_site_bwd_reduce(x, dout, g, centre, w.pa, w.pb, epi, ep, st);
+    else dwt::ldbn_bwd_reduce(x, dout, g, centre, w.pa, w.pb, st);
+  }
+  if (int rc = check_launch("latent-domain batch norm backward reduction kernel")) return rc;
+  {
+    Launch l(kLdbnName[4][k], &pg, 0.0, st);
+    dwt::ldbn_bwd_finalize(f, w.pa, w.pb, w.c0, w.c1, w.c2, w.dw, dweights, st);
+  }
+  if (int rc = check_launch("latent-domain batch norm backward finalize kernel")) return rc;
+  {
+    Launch l(kLdbnName[5][k], &pg, 3.0 * E, st);
+    // a residual's apply reads the masked gradient its reduction wrote
+    const void* dz = (epi & DWT_EPI_RESIDUAL) ? static_cast<const void*>(dresidual) : dout;
+    dwt::ldbn_site_bwd_apply(x, dz, dx, g, w.c0, w.c1, w.c2, centre, epi, ep, st);
+  }
+  return check_launch("latent-domain batch norm backward apply kernel");
+}
+
+// dwt_whiten_latent_small_fwd, and dwt_latent_site_fwd with a site epilogue epi (checked by the caller)
+int lds_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, int group_size, int n_domains, int mode, float eps,
+            float momentum, int update_running, float* running_mean, float* running_cov, const float* weights,
+            float* save_mean, float* save_w, float* save_stats, void* workspace, size_t workspace_bytes,
+            dwt_stream_t stream, int epi, const float* gamma, const float* beta, const void* residual,
+            uint8_t* relu_mask) {
+  dwt::LdbnGeom g;
+  LdsWork w;
+  const void* const act[3] = {x, x, y};
+  if (int rc = lds_validate(g, w, N, C, HW, group_size, n_domains, mode, act, weights, save_mean, save_w, save_stats,
+                            workspace, workspace_bytes))
+    return rc;
+  const bool train = (mode & DWT_MODE_EVAL) == 0;
+  if ((!train || update_running) && (!running_mean || !running_cov))
+    return fail(DWT_E_INVALID, "running buffer is null (eval, or train with update_running)");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int GS = group_size;
+  dwt::LdsFin f = make_lds_fin(g, GS, n_domains, mode, eps, weights, save_mean, save_w, save_stats, workspace);
+  f.momentum = momentum; f.update_running = train && update_running; f.rmean = running_mean; f.rcov = running_cov;
+  const dwt::Geom pg = lds_prof_geom(g, GS, n_domains);
+  const int k = 2 * g.nhwc + g.bf16;
+  const double E = (g.bf16 ? 2.0 : 4.0) * (double)N * (double)C * (double)HW;
+  {
+    Launch l(kLdsName[0][k], &pg, E, st);
+    dwt::lds_stats(x, g, GS, w.part, w.pilot, st);
+  }
+  if (int rc = check_launch("latent-domain whitening statistics kernel")) return rc;
+  {
+    Launch l(kLdsName[1][k], &pg, 0.0, st);
+    dwt::lds_fwd_finalize(f, w.part, w.pilot, w.im, st);
+  }
+  if (int rc = check_launch("latent-domain whitening finalize kernel")) return rc;
+  {
+    const bool res = (epi & DWT_EPI_RESIDUAL) != 0;
+    Launch l(kLdsName[2][k], &pg, (res ? 3.0 : 2.0) * E + (relu_mask ? E / (g.bf16 ? 8.0 : 16.0) : 0.0), st);
+    if (epi) {
+      const dwt::LdEpi ep{gamma, beta, save_mean, save_w, residual, relu_mask, nullptr};
+      dwt::lds_site_apply(x, y, g, GS, epi, ep, st);
+    } else {
+      dwt::lds_apply(x, y, g, GS, save_mean, save_w, st);
+    }
+  }
+  return check_launch("latent-domain whitening apply kernel");
+}
+
+// dwt_whiten_latent_small_bwd, and dwt_latent_site_bwd with a site epilogue epi (checked by the caller)
+int lds_bwd(const float* x, const float* dout, float* dx, int64_t N, int64_t C, int64_t HW, int group_size, int n_domains,
+            int mode, float eps, const float* weights, const float* save_mean, const float* save_w, const float* save_stats,
+            float* dweights, void* workspace, size_t workspace_bytes, dwt_stream_t stream, int epi, const float* gamma,
+            const float* beta, const uint8_t* relu_mask, float* dresidual, float* dgamma, float* dbeta) {
+  dwt::LdbnGeom g;
+  LdsWork w;
+  const void* const act[3] = {x, dout, dx};
+  if (int rc = lds_validate(g, w, N, C, HW, group_size, n_domains, mode, act, weights, save_mean, save_w, save_stats,
+                            workspace, workspace_bytes))
+    return rc;
+  if ((uintptr_t)dweights % 4 != 0) return fail(DWT_E_INVALID, "dweights must be 4-byte aligned (latent-domain whitening)");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int GS = group_size;
+  const dwt::LdsFin f = make_lds_fin(g, GS, n_domains, mode, eps, weights, save_mean, save_w, save_stats, workspace);
+  const dwt::Geom pg = lds_prof_geom(g, GS, n_domains);
+  const dwt::LdEpi ep{gamma, beta, save_mean, save_w, nullptr, const_cast<uint8_t*>(relu_mask), dresidual};
+  const int k = 2 * g.nhwc + g.bf16;
+  const double E = (g.bf16 ? 2.0 : 4.0) * (double)N * (double)C * (double)HW;
+  {
+    const bool mk = (epi & DWT_EPI_RESIDUAL) != 0;
+    Launch l(kLdsName[3][k], &pg, (mk ? 3.0 : 2.0) * E + (mk ? E / (g.bf16 ? 8.0 : 16.0) : 0.0), st);
+    if (epi) dwt::lds_site_bwd_reduce(x, dout, g, GS, save_stats, w.part, epi, ep, st);
+    else dwt::lds_bwd_reduce(x, dout, g, GS, save_stats, w.part, st);
+  }
+  if (int rc = check_launch("latent-domain whitening backward reduction kernel")) return rc;
+  {
+    Launch l(kLdsName[4][k], &pg, 0.0, st);
+    // a site's per-image dgamma / dbeta shares reuse the forward's per-image moments (w.im, free in the backward)
+    if (epi) dwt::lds_site_bwd_finalize(f, w.part, w.red, w.pd, w.pc, w.coef, w.dw, dweights, gamma,
+                                        reinterpret_cast<float*>(w.im), dgamma, dbeta, st);
+    else dwt::lds_bwd_finalize(f, w.part, w.red, w.pd, w.pc, w.coef, w.dw, dweights, st);
+  }
+  if (int rc = check_launch("latent-domain whitening backward finalize kernel")) return rc;
+  {
+    Launch l(kLdsName[5][k], &pg, 3.0 * E, st);
+    // a residual's apply reads the masked gradient its reduction wrote
+    const void* dz = (epi & DWT_EPI_RESIDUAL) ? static_cast<const void*>(dresidual) : dout;
+    if (epi) dwt::lds_site_bwd_apply(x, dz, dx, g, GS, w.coef, epi, ep, st);
+    else dwt::lds_bwd_apply(x, dout, dx, g, GS, w.coef, st);
+  }
+  return check_launch("latent-domain whitening backward apply kernel");
+}
+
+
+// ---- latent-domain sites (dwt_latent_site_*) ----------------------------------------------------------------------------
+// The checks of a site call the layer's own entry points do not make: kind and group size, the epilogue bits and the
+// pointers they need.  The drivers above check the rest.  bwd: dresidual / relu_mask of the backward.
+int site_check(int kind, int GS, int mode, int epi, const float* gamma, const float* beta, const void* residual,
+               const void* relu_mask, const void* dresidual, bool bwd, bool bf16_bytes) {
+  if (kind != DWT_KIND_BN && kind != DWT_KIND_WHITEN)
+    return fail(DWT_E_INVALID, "kind %d is neither DWT_KIND_BN nor DWT_KIND_WHITEN (latent-domain site)", kind);
+  if (kind == DWT_KIND_BN && GS != 1)
+    return fail(DWT_E_INVALID, "a batch-norm latent-domain site takes group_size 1 (got %d)", GS);
+  if (kind == DWT_KIND_WHITEN && GS != 1 && GS != 2 && GS != 4)
+    return fail(DWT_E_UNSUPPORTED, "a whitening latent-domain site runs at group sizes 1, 2, 4 only (got %d)", GS);
+  if (epi & ~(DWT_EPI_AFFINE | DWT_EPI_RELU | DWT_EPI_RESIDUAL))
+    return fail(DWT_E_INVALID, "bad epilogue %#x (latent-domain site)", epi);
+  if ((epi & DWT_EPI_RELU) && !(epi & DWT_EPI_AFFINE))
+    return fail(DWT_E_INVALID, "a latent-domain site's RELU epilogue needs AFFINE");
+  if ((epi & DWT_EPI_RESIDUAL) && !(epi & DWT_EPI_RELU))
+    return fail(DWT_E_INVALID, "a latent-domain site's RESIDUAL epilogue needs AFFINE|RELU");
+  if (!(epi & DWT_EPI_AFFINE) != (!gamma || !beta) || !gamma != !beta)
+    return fail(DWT_E_INVALID, "a latent-domain site takes gamma and beta exactly with the AFFINE epilogue");
+  if (((uintptr_t)gamma | (uintptr_t)beta) % 4 != 0)
+    return fail(DWT_E_INVALID, "gamma and beta must be 4-byte aligned (latent-domain site)");
+  const bool nhwc = (mode & DWT_LAYOUT_NHWC) != 0, res = (epi & DWT_EPI_RESIDUAL) != 0;
+  if (res && bwd && !nhwc)
+    return fail(DWT_E_INVALID, "an NCHW latent-domain site's residual backward is the AFFINE one on dz = dout * (out > 0)");
+  if (!relu_mask != !(res && nhwc))
+    return fail(DWT_E_INVALID, "a latent-domain site takes a ReLU byte map exactly with the channels-last RESIDUAL epilogue");
+  const void* t = bwd ? dresidual : residual;
+  if (!t != !res)
+    return fail(DWT_E_INVALID, "a latent-domain site takes %s exactly with the RESIDUAL epilogue", bwd ? "dresidual" : "residual");
+  if ((uintptr_t)t % (bf16_bytes ? 8 : 16) != 0)
+    return fail(DWT_E_INVALID, "%s must be %d-byte aligned (latent-domain site)", bwd ? "dresidual" : "residual",
+                bf16_bytes ? 8 : 16);
+  return DWT_OK;
+}
 }  // namespace
 
 extern "C" {
@@ -1375,71 +1586,15 @@ int dwt_bn_latent_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW
                       float momentum, int update_running, float* running_mean, float* running_var, const float* weights,
                       const float* gamma, const float* beta, float* save_stats, void* workspace, size_t workspace_bytes,
                       dwt_stream_t stream) {
-  dwt::LdbnGeom g;
-  LdbnWork w;
-  const void* const act[3] = {x, x, y};
-  if (int rc = ldbn_validate(g, w, N, C, HW, n_domains, mode, act, weights, save_stats, gamma, beta, workspace,
-                             workspace_bytes))
-    return rc;
-  const bool train = (mode & DWT_MODE_EVAL) == 0;
-  if ((!train || update_running) && (!running_mean || !running_var))
-    return fail(DWT_E_INVALID, "running buffer is null (eval, or train with update_running)");
-  cudaStream_t st = (cudaStream_t)stream;
-  dwt::LdbnFin f = make_ldbn_fin(g, mode, eps, weights, gamma, beta, save_stats, workspace);
-  f.momentum = momentum; f.update_running = train && update_running; f.rmean = running_mean; f.rvar = running_var;
-  const dwt::Geom pg = ldbn_prof_geom(g);
-  const int k = 2 * g.nhwc + g.bf16;
-  const double E = (g.bf16 ? 2.0 : 4.0) * (double)N * (double)C * (double)HW;
-  if (train) {
-    Launch l(kLdbnName[0][k], &pg, E, st);
-    dwt::ldbn_stats(x, g, w.pa, w.pb, w.pilot, st);
-  }
-  if (int rc = check_launch("latent-domain batch norm statistics kernel")) return rc;
-  {
-    Launch l(kLdbnName[1][k], &pg, 0.0, st);
-    dwt::ldbn_fwd_finalize(f, w.pa, w.pb, w.pilot, w.c0, w.c1, st);
-  }
-  if (int rc = check_launch("latent-domain batch norm finalize kernel")) return rc;
-  {
-    Launch l(kLdbnName[2][k], &pg, 2.0 * E, st);
-    dwt::ldbn_apply(x, y, g, w.c0, w.c1, st);
-  }
-  return check_launch("latent-domain batch norm apply kernel");
+  return ldbn_fwd(x, y, N, C, HW, n_domains, mode, eps, momentum, update_running, running_mean, running_var, weights, gamma,
+                  beta, save_stats, workspace, workspace_bytes, stream, 0, nullptr, nullptr);
 }
 
 int dwt_bn_latent_bwd(const float* x, const float* dout, float* dx, int64_t N, int64_t C, int64_t HW, int n_domains, int mode,
                       float eps, const float* weights, const float* gamma, const float* save_stats, float* dweights,
                       float* dgamma, float* dbeta, void* workspace, size_t workspace_bytes, dwt_stream_t stream) {
-  dwt::LdbnGeom g;
-  LdbnWork w;
-  const void* const act[3] = {x, dout, dx};
-  if (int rc = ldbn_validate(g, w, N, C, HW, n_domains, mode, act, weights, save_stats, dgamma, dbeta, workspace,
-                             workspace_bytes))
-    return rc;
-  if (dgamma && !gamma) return fail(DWT_E_INVALID, "dgamma / dbeta given without gamma (latent-domain batch norm)");
-  if ((uintptr_t)dweights % 4 != 0) return fail(DWT_E_INVALID, "dweights must be 4-byte aligned (latent-domain batch norm)");
-  cudaStream_t st = (cudaStream_t)stream;
-  dwt::LdbnFin f = make_ldbn_fin(g, mode, eps, weights, gamma, nullptr, save_stats, workspace);
-  f.dgamma = dgamma; f.dbeta = dbeta;
-  const dwt::Geom pg = ldbn_prof_geom(g);
-  const int k = 2 * g.nhwc + g.bf16;
-  const double E = (g.bf16 ? 2.0 : 4.0) * (double)N * (double)C * (double)HW;
-  const float* centre = save_stats;                           // [N][C] first in save_stats
-  {
-    Launch l(kLdbnName[3][k], &pg, 2.0 * E, st);
-    dwt::ldbn_bwd_reduce(x, dout, g, centre, w.pa, w.pb, st);
-  }
-  if (int rc = check_launch("latent-domain batch norm backward reduction kernel")) return rc;
-  {
-    Launch l(kLdbnName[4][k], &pg, 0.0, st);
-    dwt::ldbn_bwd_finalize(f, w.pa, w.pb, w.c0, w.c1, w.c2, w.dw, dweights, st);
-  }
-  if (int rc = check_launch("latent-domain batch norm backward finalize kernel")) return rc;
-  {
-    Launch l(kLdbnName[5][k], &pg, 3.0 * E, st);
-    dwt::ldbn_bwd_apply(x, dout, dx, g, w.c0, w.c1, w.c2, centre, st);
-  }
-  return check_launch("latent-domain batch norm backward apply kernel");
+  return ldbn_bwd(x, dout, dx, N, C, HW, n_domains, mode, eps, weights, gamma, save_stats, dweights, dgamma, dbeta, workspace,
+                  workspace_bytes, stream, 0, nullptr, nullptr, nullptr);
 }
 
 size_t dwt_latent_small_workspace_bytes(int64_t N, int64_t C, int64_t HW, int group_size, int n_domains) {
@@ -1461,71 +1616,61 @@ int dwt_whiten_latent_small_fwd(const float* x, float* y, int64_t N, int64_t C, 
                                 int mode, float eps, float momentum, int update_running, float* running_mean,
                                 float* running_cov, const float* weights, float* save_mean, float* save_w,
                                 float* save_stats, void* workspace, size_t workspace_bytes, dwt_stream_t stream) {
-  dwt::LdbnGeom g;
-  LdsWork w;
-  const void* const act[3] = {x, x, y};
-  if (int rc = lds_validate(g, w, N, C, HW, group_size, n_domains, mode, act, weights, save_mean, save_w, save_stats,
-                            workspace, workspace_bytes))
-    return rc;
-  const bool train = (mode & DWT_MODE_EVAL) == 0;
-  if ((!train || update_running) && (!running_mean || !running_cov))
-    return fail(DWT_E_INVALID, "running buffer is null (eval, or train with update_running)");
-  cudaStream_t st = (cudaStream_t)stream;
-  const int GS = group_size;
-  dwt::LdsFin f = make_lds_fin(g, GS, n_domains, mode, eps, weights, save_mean, save_w, save_stats, workspace);
-  f.momentum = momentum; f.update_running = train && update_running; f.rmean = running_mean; f.rcov = running_cov;
-  const dwt::Geom pg = lds_prof_geom(g, GS, n_domains);
-  const int k = 2 * g.nhwc + g.bf16;
-  const double E = (g.bf16 ? 2.0 : 4.0) * (double)N * (double)C * (double)HW;
-  {
-    Launch l(kLdsName[0][k], &pg, E, st);
-    dwt::lds_stats(x, g, GS, w.part, w.pilot, st);
-  }
-  if (int rc = check_launch("latent-domain whitening statistics kernel")) return rc;
-  {
-    Launch l(kLdsName[1][k], &pg, 0.0, st);
-    dwt::lds_fwd_finalize(f, w.part, w.pilot, w.im, st);
-  }
-  if (int rc = check_launch("latent-domain whitening finalize kernel")) return rc;
-  {
-    Launch l(kLdsName[2][k], &pg, 2.0 * E, st);
-    dwt::lds_apply(x, y, g, GS, save_mean, save_w, st);
-  }
-  return check_launch("latent-domain whitening apply kernel");
+  return lds_fwd(x, y, N, C, HW, group_size, n_domains, mode, eps, momentum, update_running, running_mean, running_cov,
+                 weights, save_mean, save_w, save_stats, workspace, workspace_bytes, stream, 0, nullptr, nullptr, nullptr,
+                 nullptr);
 }
 
 int dwt_whiten_latent_small_bwd(const float* x, const float* dout, float* dx, int64_t N, int64_t C, int64_t HW,
                                 int group_size, int n_domains, int mode, float eps, const float* weights,
                                 const float* save_mean, const float* save_w, const float* save_stats, float* dweights,
                                 void* workspace, size_t workspace_bytes, dwt_stream_t stream) {
-  dwt::LdbnGeom g;
-  LdsWork w;
-  const void* const act[3] = {x, dout, dx};
-  if (int rc = lds_validate(g, w, N, C, HW, group_size, n_domains, mode, act, weights, save_mean, save_w, save_stats,
-                            workspace, workspace_bytes))
+  return lds_bwd(x, dout, dx, N, C, HW, group_size, n_domains, mode, eps, weights, save_mean, save_w, save_stats, dweights,
+                 workspace, workspace_bytes, stream, 0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
+}
+
+// a refusal of the layer's own checks or launches, passed through a site call: its text also names the site
+static int site_rc(int rc) {
+  if (rc != DWT_OK) {
+    const size_t n = strlen(g_err);
+    snprintf(g_err + n, sizeof(g_err) - n, " [latent-domain site]");
+  }
+  return rc;
+}
+
+int dwt_latent_site_fwd(int kind, const float* x, float* y, int64_t N, int64_t C, int64_t HW, int group_size, int n_domains,
+                        int mode, float eps, float momentum, int update_running, float* running_mean,
+                        float* running_second, const float* weights, const float* gamma, const float* beta,
+                        const float* residual, uint8_t* relu_mask, int epilogue, float* save_mean, float* save_w,
+                        float* save_stats, void* workspace, size_t workspace_bytes, dwt_stream_t stream) {
+  if (int rc = site_check(kind, group_size, mode, epilogue, gamma, beta, residual, relu_mask, nullptr, false,
+                          (mode & DWT_DTYPE_BF16) != 0))
     return rc;
-  if ((uintptr_t)dweights % 4 != 0) return fail(DWT_E_INVALID, "dweights must be 4-byte aligned (latent-domain whitening)");
-  cudaStream_t st = (cudaStream_t)stream;
-  const int GS = group_size;
-  const dwt::LdsFin f = make_lds_fin(g, GS, n_domains, mode, eps, weights, save_mean, save_w, save_stats, workspace);
-  const dwt::Geom pg = lds_prof_geom(g, GS, n_domains);
-  const int k = 2 * g.nhwc + g.bf16;
-  const double E = (g.bf16 ? 2.0 : 4.0) * (double)N * (double)C * (double)HW;
-  {
-    Launch l(kLdsName[3][k], &pg, 2.0 * E, st);
-    dwt::lds_bwd_reduce(x, dout, g, GS, save_stats, w.part, st);
-  }
-  if (int rc = check_launch("latent-domain whitening backward reduction kernel")) return rc;
-  {
-    Launch l(kLdsName[4][k], &pg, 0.0, st);
-    dwt::lds_bwd_finalize(f, w.part, w.red, w.pd, w.pc, w.coef, w.dw, dweights, st);
-  }
-  if (int rc = check_launch("latent-domain whitening backward finalize kernel")) return rc;
-  {
-    Launch l(kLdsName[5][k], &pg, 3.0 * E, st);
-    dwt::lds_bwd_apply(x, dout, dx, g, GS, w.coef, st);
-  }
-  return check_launch("latent-domain whitening backward apply kernel");
+  if (kind == DWT_KIND_BN)
+    return site_rc(ldbn_fwd(x, y, N, C, HW, n_domains, mode, eps, momentum, update_running, running_mean, running_second, weights,
+                    gamma, beta, save_stats, workspace, workspace_bytes, stream, epilogue, residual, relu_mask));
+  return site_rc(lds_fwd(x, y, N, C, HW, group_size, n_domains, mode, eps, momentum, update_running, running_mean, running_second,
+                 weights, save_mean, save_w, save_stats, workspace, workspace_bytes, stream, epilogue, gamma, beta, residual,
+                 relu_mask));
+}
+
+int dwt_latent_site_bwd(int kind, const float* x, const float* dout, float* dx, int64_t N, int64_t C, int64_t HW,
+                        int group_size, int n_domains, int mode, float eps, const float* weights, const float* gamma,
+                        const float* beta, const uint8_t* relu_mask, float* dresidual, int epilogue, const float* save_mean,
+                        const float* save_w, const float* save_stats, float* dweights, float* dgamma, float* dbeta,
+                        void* workspace, size_t workspace_bytes, dwt_stream_t stream) {
+  if (int rc = site_check(kind, group_size, mode, epilogue, gamma, beta, nullptr, relu_mask, dresidual, true,
+                          (mode & DWT_DTYPE_BF16) != 0))
+    return rc;
+  if (!dgamma != !dbeta || (dgamma && !gamma))
+    return fail(DWT_E_INVALID, "dgamma and dbeta go together and need the AFFINE epilogue (latent-domain site)");
+  if (((uintptr_t)dgamma | (uintptr_t)dbeta) % 4 != 0)
+    return fail(DWT_E_INVALID, "dgamma and dbeta must be 4-byte aligned (latent-domain site)");
+  if (kind == DWT_KIND_BN)
+    return site_rc(ldbn_bwd(x, dout, dx, N, C, HW, n_domains, mode, eps, weights, gamma, save_stats, dweights, dgamma, dbeta,
+                    workspace, workspace_bytes, stream, epilogue, beta, relu_mask, dresidual));
+  return site_rc(lds_bwd(x, dout, dx, N, C, HW, group_size, n_domains, mode, eps, weights, save_mean, save_w, save_stats, dweights,
+                 workspace, workspace_bytes, stream, epilogue, gamma, beta, relu_mask, dresidual, dgamma, dbeta));
 }
 
 const char* dwt_last_error(void) { return g_err; }

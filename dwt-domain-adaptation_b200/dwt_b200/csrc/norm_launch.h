@@ -204,6 +204,20 @@ struct LdbnFin {
   float* dbeta;
   int* status;
 };
+// The site epilogue of the latent-domain bandwidth passes (dwt_latent_site_*): out = relu(gamma zhat + beta [+ residual])
+// with DWT_EPI_* bits.  A ReLU without a residual is recomputed by the backward passes from x with the forward's
+// coefficients; a channels-last residual leaves the forward's byte map (one byte per float4, the four out > 0 bits), which
+// the backward reduction reads to write the masked gradient dz.  An NCHW residual's backward is the AFFINE one on dz.
+struct LdEpi {
+  const float* gamma;         // [C]
+  const float* beta;
+  const float* p0;            // batch norm: save_stats' a_n [N][C]; whitening: save_mean (m~_n)
+  const float* p1;            // batch norm: save_stats' b_n [N][C]; whitening: save_w (A_n)
+  const void* res;            // forward RESIDUAL: x's shape, layout and dtype
+  uint8_t* mask;              // channels-last RESIDUAL: forward writes, backward reduction reads
+  void* dz;                   // backward reduction, channels-last RESIDUAL: dout * mask, x's dtype
+};
+
 LdbnGeom ldbn_plan(int N, int C, int HW, int D, bool nhwc, bool bf16);
 int ldbn_finalize_ctas(int C);
 // scratch floats of a call: two partial arrays of `part`, four [N][C] arrays of `nc` (pilot and the apply coefficients),
@@ -220,6 +234,13 @@ void ldbn_bwd_finalize(const LdbnFin& f, const float* pa, const float* pb, float
                        float* dweights, cudaStream_t st);
 void ldbn_bwd_apply(const void* x, const void* dy, void* dx, const LdbnGeom& g, const float* ca, const float* cp,
                     const float* cq, const float* centre, cudaStream_t st);
+// the bandwidth passes under a site epilogue epi != 0 (AFFINE is in the coefficients; ep.p0 / p1 = a_n / b_n)
+void ldbn_site_apply(const void* x, void* y, const LdbnGeom& g, const float* alpha, const float* shift, int epi,
+                     const LdEpi& ep, cudaStream_t st);
+void ldbn_site_bwd_reduce(const void* x, const void* dy, const LdbnGeom& g, const float* centre, float* pa, float* pb,
+                          int epi, const LdEpi& ep, cudaStream_t st);
+void ldbn_site_bwd_apply(const void* x, const void* dy, void* dx, const LdbnGeom& g, const float* ca, const float* cp,
+                         const float* cq, const float* centre, int epi, const LdEpi& ep, cudaStream_t st);
 
 // latent-domain whitening at group sizes 1, 2, 4 (norm_ldbn.cu; dwt_whiten_latent_small_*) on latent-domain batch
 // norm's segments: NCHW a warp per (image, group, segment) reads the group's gs channel rows, planned by ldbn_plan over
@@ -262,6 +283,17 @@ void lds_bwd_reduce(const void* x, const void* dy, const LdbnGeom& g, int GS, co
 void lds_bwd_finalize(const LdsFin& f, const float* part, float* red, float* pd, float* pc, float* coef, float* dwpart,
                       float* dweights, cudaStream_t st);
 void lds_bwd_apply(const void* x, const void* dy, void* dx, const LdbnGeom& g, int GS, const float* coef, cudaStream_t st);
+// the passes under a site epilogue epi with AFFINE (ep.p0 / p1 = save_mean / save_w): diag(gamma) folds into A_n's rows
+// and beta into the bias; the backward's reductions take dz, the finalize scales g_n, R_n by gamma and writes dgamma /
+// dbeta (per-image shares in pgb [2][N][C], then added over the images in order), the apply maps gamma dz.
+void lds_site_apply(const void* x, void* y, const LdbnGeom& g, int GS, int epi, const LdEpi& ep, cudaStream_t st);
+void lds_site_bwd_reduce(const void* x, const void* dy, const LdbnGeom& g, int GS, const float* save_stats, float* part,
+                         int epi, const LdEpi& ep, cudaStream_t st);
+void lds_site_bwd_finalize(const LdsFin& f, const float* part, float* red, float* pd, float* pc, float* coef,
+                           float* dwpart, float* dweights, const float* gamma, float* pgb, float* dgamma, float* dbeta,
+                           cudaStream_t st);
+void lds_site_bwd_apply(const void* x, const void* dy, void* dx, const LdbnGeom& g, int GS, const float* coef, int epi,
+                        const LdEpi& ep, cudaStream_t st);
 
 // channels-last max-pool (pool.cu); bf16: x, y, dy, dx are bf16 (compared and summed in fp32, stored rounded)
 void maxpool_fwd_launch(const void* x, void* y, bool bf16, uint8_t* idx, int N, int H, int W, int C, int OH, int OW, int k, int s, int p,

@@ -43,12 +43,41 @@ __device__ __forceinline__ void acc4(Acc& s, const float4& x, const float4& dy, 
 __device__ __forceinline__ void st1(float* p, float v) { *p = v; }
 __device__ __forceinline__ void st1(__nv_bfloat16* p, float v) { *p = __float2bfloat16_rn(v); }
 
+// Site epilogue E (DWT_EPI_* bits; 0: the plain layer).  RC: the backward recomputes the ReLU mask from x (a ReLU
+// without a residual); MK: the channels-last residual's byte map.
+template <int E> constexpr bool kEpiRc = (E & DWT_EPI_RELU) && !(E & DWT_EPI_RESIDUAL);
+template <int E> constexpr bool kEpiMk = (E & DWT_EPI_RESIDUAL) != 0;
+
+// ReLU as torch.relu and its gradient as threshold_backward: a NaN pre-activation stays NaN and passes its gradient,
+// so a bad image's NaN (the layers' edge rules) survives the site
+__device__ __forceinline__ bool relu_pass(float z) { return !(z <= 0.f); }
+
+// the forward's output of a site: z (+ r), bit k of bits = relu_pass(that), then the ReLU
+template <int E>
+__device__ __forceinline__ float site_out(float z, float r, unsigned& bits, int k) {
+  if (E & DWT_EPI_RESIDUAL) {
+    z += r;
+    bits |= (relu_pass(z) ? 1u : 0u) << k;
+  }
+  return (E & DWT_EPI_RELU) ? (z != z ? z : fmaxf(z, 0.f)) : z;
+}
+
+// batch norm: the forward's apply coefficients of (image, channel) o, channel c -- alpha = gamma a_n, shift = gamma b_n +
+// beta, the finalize's arithmetic, so a recomputed pre-activation is the forward's bit for bit
+__device__ __forceinline__ float2 ldbn_fwd_coef(const LdEpi& ep, size_t o, int c) {
+  const float gam = __ldg(ep.gamma + c);
+  return make_float2(gam * __ldg(ep.p0 + o), fmaf(gam, __ldg(ep.p1 + o), __ldg(ep.beta + c)));
+}
+__device__ __forceinline__ float relu_dy(float x, float dy, float2 k) { return relu_pass(fmaf(k.x, x, k.y)) ? dy : 0.f; }
+__device__ __forceinline__ float bit_dy(unsigned bits, int k, float dy) { return (bits >> k) & 1u ? dy : 0.f; }
+
 // NCHW reduction: a warp per (row, segment).  VEC: HW % 4 == 0, segments of whole float4s.
-template <bool BWD, bool VEC, class T>
+template <bool BWD, bool VEC, class T, int E = 0>
 __global__ void __launch_bounds__(kThreads) ldbn_reduce_nchw(const T* __restrict__ x, const T* __restrict__ dy,
                                                              LdbnGeom g, const float* __restrict__ centre,
                                                              float* __restrict__ pa, float* __restrict__ pb,
-                                                             float* __restrict__ pilot) {
+                                                             float* __restrict__ pilot, LdEpi ep) {
+  static_assert(!kEpiMk<E>, "an NCHW residual's backward runs on dz without the epilogue");
   const long long wid = ((long long)blockIdx.x * kThreads + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   const long long rows = (long long)g.N * g.C;
@@ -59,7 +88,23 @@ __global__ void __launch_bounds__(kThreads) ldbn_reduce_nchw(const T* __restrict
   const float K = BWD ? centre[row] : ld1(x + base);
   const int p0 = s * g.P, p1 = min(p0 + g.P, g.HW);
   Acc a{0.f, 0.f};
-  if (VEC) {
+  if constexpr (kEpiRc<E>) {
+    const float2 k = ldbn_fwd_coef(ep, (size_t)row, (int)(row % g.C));
+    if (VEC) {
+#pragma unroll 4
+      for (int p = p0 + 4 * lane; p < p1; p += 128) {
+        const float4 v = ld4(x + base + p), d = ld4(dy + base + p);
+        acc4<BWD>(a, v, make_float4(relu_dy(v.x, d.x, k), relu_dy(v.y, d.y, k), relu_dy(v.z, d.z, k),
+                                    relu_dy(v.w, d.w, k)), K);
+      }
+    } else {
+#pragma unroll 4
+      for (int p = p0 + lane; p < p1; p += 32) {
+        const float v = ld1(x + base + p);
+        acc1<BWD>(a, v, relu_dy(v, ld1(dy + base + p), k), K);
+      }
+    }
+  } else if (VEC) {
 #pragma unroll 4
     for (int p = p0 + 4 * lane; p < p1; p += 128)
       acc4<BWD>(a, ld4(x + base + p), BWD ? ld4(dy + base + p) : float4{}, K);
@@ -79,12 +124,12 @@ __global__ void __launch_bounds__(kThreads) ldbn_reduce_nchw(const T* __restrict
 }
 
 // channels-last reduction: CTA (slab, segment, image) of g.qc float4 columns x g.pr pixel rows; the rows are added in
-// order through shared memory
-template <bool BWD, class T>
+// order through shared memory.  MK: dy masked by the byte map, written to ep.dz.
+template <bool BWD, class T, int E = 0>
 __global__ void __launch_bounds__(kThreads) ldbn_reduce_nhwc(const T* __restrict__ x, const T* __restrict__ dy,
                                                              LdbnGeom g, const float* __restrict__ centre,
                                                              float* __restrict__ pa, float* __restrict__ pb,
-                                                             float* __restrict__ pilot) {
+                                                             float* __restrict__ pilot, LdEpi ep) {
   __shared__ float4 sa[kThreads], sb[kThreads];
   const int slabs = (g.C / 4 + g.qc - 1) / g.qc;
   int b = blockIdx.x;
@@ -100,12 +145,36 @@ __global__ void __launch_bounds__(kThreads) ldbn_reduce_nhwc(const T* __restrict
     const float4 K = BWD ? *reinterpret_cast<const float4*>(centre + (size_t)n * g.C + 4 * c4) : ld4(x + img);
     Acc ax{0.f, 0.f}, ay{0.f, 0.f}, az{0.f, 0.f}, aw{0.f, 0.f};
     const int p0 = s * g.P, p1 = min(p0 + g.P, g.HW);
+    if constexpr (kEpiRc<E> || kEpiMk<E>) {
+      float2 k[4];
+      if constexpr (kEpiRc<E>) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) k[j] = ldbn_fwd_coef(ep, (size_t)n * g.C + 4 * c4 + j, 4 * c4 + j);
+      }
+      const unsigned C4 = (unsigned)g.C / 4;
+#pragma unroll 4
+      for (int p = p0 + r; p < p1; p += g.pr) {
+        const float4 v = ld4(x + img + (size_t)p * g.C);
+        float4 d = ld4(dy + img + (size_t)p * g.C);
+        if constexpr (kEpiMk<E>) {
+          const unsigned bits = __ldg(ep.mask + ((size_t)n * g.HW + p) * C4 + c4);
+          d = make_float4(bit_dy(bits, 0, d.x), bit_dy(bits, 1, d.y), bit_dy(bits, 2, d.z), bit_dy(bits, 3, d.w));
+          st4(static_cast<T*>(ep.dz) + img + (size_t)p * g.C, d);
+        } else {
+          d = make_float4(relu_dy(v.x, d.x, k[0]), relu_dy(v.y, d.y, k[1]), relu_dy(v.z, d.z, k[2]),
+                          relu_dy(v.w, d.w, k[3]));
+        }
+        acc1<BWD>(ax, v.x, d.x, K.x); acc1<BWD>(ay, v.y, d.y, K.y);
+        acc1<BWD>(az, v.z, d.z, K.z); acc1<BWD>(aw, v.w, d.w, K.w);
+      }
+    } else {
 #pragma unroll 4
     for (int p = p0 + r; p < p1; p += g.pr) {
       const float4 v = ld4(x + img + (size_t)p * g.C);
       const float4 d = BWD ? ld4(dy + img + (size_t)p * g.C) : float4{};
       acc1<BWD>(ax, v.x, d.x, K.x); acc1<BWD>(ay, v.y, d.y, K.y);
       acc1<BWD>(az, v.z, d.z, K.z); acc1<BWD>(aw, v.w, d.w, K.w);
+    }
     }
     va = make_float4(ax.a, ay.a, az.a, aw.a);
     vb = make_float4(ax.b, ay.b, az.b, aw.b);
@@ -462,15 +531,46 @@ __device__ __forceinline__ float apply1(float x, float dy, int i, const float* c
   return fmaf(__ldg(ca + i), x, __ldg(cb + i));
 }
 
-// NCHW: VEC -- a thread per 4 pixels of a row (HW % 4 == 0); else a thread per element
-template <bool BWD, bool VEC, class T>
+// NCHW: VEC -- a thread per 4 pixels of a row (HW % 4 == 0); else a thread per element.  E: forward the site's residual
+// and ReLU on the output, backward (RC) dy masked by the recomputed pre-activation.
+template <bool BWD, bool VEC, class T, int E = 0>
 __global__ void __launch_bounds__(kThreads) ldbn_apply_nchw(const T* __restrict__ x, const T* __restrict__ dy,
                                                             T* __restrict__ out, LdbnGeom g, const float* __restrict__ ca,
                                                             const float* __restrict__ cb, const float* __restrict__ cq,
-                                                            const float* __restrict__ K) {
+                                                            const float* __restrict__ K, LdEpi ep) {
+  static_assert(!BWD || !kEpiMk<E>, "a residual's backward apply reads dz without the epilogue");
   const unsigned total = (unsigned)((size_t)g.N * g.C * g.HW / (VEC ? 4 : 1));
   for (unsigned e = blockIdx.x * kThreads + threadIdx.x; e < total; e += gridDim.x * kThreads) {
-    if (VEC) {
+    if constexpr (E != 0) {
+      const T* res = static_cast<const T*>(ep.res);
+      unsigned bits = 0;
+      if (VEC) {
+        const unsigned i = 4 * e, row = i / (unsigned)g.HW;
+        const float4 v = ld4(x + i);
+        float4 d = BWD ? ld4(dy + i) : float4{};
+        if constexpr (BWD) {
+          const float2 k = ldbn_fwd_coef(ep, row, (int)(row % (unsigned)g.C));
+          d = make_float4(relu_dy(v.x, d.x, k), relu_dy(v.y, d.y, k), relu_dy(v.z, d.z, k), relu_dy(v.w, d.w, k));
+          st4(out + i, make_float4(apply1<true>(v.x, d.x, row, ca, cb, cq, K), apply1<true>(v.y, d.y, row, ca, cb, cq, K),
+                                   apply1<true>(v.z, d.z, row, ca, cb, cq, K), apply1<true>(v.w, d.w, row, ca, cb, cq, K)));
+        } else {
+          const float4 rv = kEpiMk<E> ? ld4(res + i) : float4{};
+          st4(out + i, make_float4(site_out<E>(apply1<false>(v.x, 0.f, row, ca, cb, cq, K), rv.x, bits, 0),
+                                   site_out<E>(apply1<false>(v.y, 0.f, row, ca, cb, cq, K), rv.y, bits, 1),
+                                   site_out<E>(apply1<false>(v.z, 0.f, row, ca, cb, cq, K), rv.z, bits, 2),
+                                   site_out<E>(apply1<false>(v.w, 0.f, row, ca, cb, cq, K), rv.w, bits, 3)));
+        }
+      } else {
+        const unsigned row = e / (unsigned)g.HW;
+        const float v = ld1(x + e);
+        if constexpr (BWD) {
+          const float d = relu_dy(v, ld1(dy + e), ldbn_fwd_coef(ep, row, (int)(row % (unsigned)g.C)));
+          st1(out + e, apply1<true>(v, d, row, ca, cb, cq, K));
+        } else {
+          st1(out + e, site_out<E>(apply1<false>(v, 0.f, row, ca, cb, cq, K), kEpiMk<E> ? ld1(res + e) : 0.f, bits, 0));
+        }
+      }
+    } else if (VEC) {
       const unsigned i = 4 * e, row = i / (unsigned)g.HW;
       const float4 v = ld4(x + i), d = BWD ? ld4(dy + i) : float4{};
       st4(out + i, make_float4(apply1<BWD>(v.x, d.x, row, ca, cb, cq, K), apply1<BWD>(v.y, d.y, row, ca, cb, cq, K),
@@ -482,16 +582,39 @@ __global__ void __launch_bounds__(kThreads) ldbn_apply_nchw(const T* __restrict_
   }
 }
 
-// channels-last: a thread per 4 channels of a pixel
-template <bool BWD, class T>
+// channels-last: a thread per 4 channels of a pixel.  E as ldbn_apply_nchw; a residual's forward writes the byte map.
+template <bool BWD, class T, int E = 0>
 __global__ void __launch_bounds__(kThreads) ldbn_apply_nhwc(const T* __restrict__ x, const T* __restrict__ dy,
                                                             T* __restrict__ out, LdbnGeom g, const float* __restrict__ ca,
                                                             const float* __restrict__ cb, const float* __restrict__ cq,
-                                                            const float* __restrict__ K) {
+                                                            const float* __restrict__ K, LdEpi ep) {
+  static_assert(!BWD || !kEpiMk<E>, "a residual's backward apply reads dz without the epilogue");
   const unsigned C4 = (unsigned)g.C / 4, per_img = (unsigned)g.HW * C4;
   const unsigned total = (unsigned)g.N * per_img;
   for (unsigned e = blockIdx.x * kThreads + threadIdx.x; e < total; e += gridDim.x * kThreads) {
     const unsigned n = e / per_img, c = 4 * (e % C4), o = n * (unsigned)g.C + c;
+    if constexpr (E != 0) {
+      const float4 v = ld4(x + 4 * (size_t)e);
+      if constexpr (BWD) {
+        float4 d = ld4(dy + 4 * (size_t)e);
+        d = make_float4(relu_dy(v.x, d.x, ldbn_fwd_coef(ep, o, c)), relu_dy(v.y, d.y, ldbn_fwd_coef(ep, o + 1, c + 1)),
+                        relu_dy(v.z, d.z, ldbn_fwd_coef(ep, o + 2, c + 2)),
+                        relu_dy(v.w, d.w, ldbn_fwd_coef(ep, o + 3, c + 3)));
+        st4(out + 4 * (size_t)e, make_float4(apply1<true>(v.x, d.x, o, ca, cb, cq, K),
+                                             apply1<true>(v.y, d.y, o + 1, ca, cb, cq, K),
+                                             apply1<true>(v.z, d.z, o + 2, ca, cb, cq, K),
+                                             apply1<true>(v.w, d.w, o + 3, ca, cb, cq, K)));
+      } else {
+        const float4 rv = kEpiMk<E> ? ld4(static_cast<const T*>(ep.res) + 4 * (size_t)e) : float4{};
+        unsigned bits = 0;
+        st4(out + 4 * (size_t)e, make_float4(site_out<E>(apply1<false>(v.x, 0.f, o, ca, cb, cq, K), rv.x, bits, 0),
+                                             site_out<E>(apply1<false>(v.y, 0.f, o + 1, ca, cb, cq, K), rv.y, bits, 1),
+                                             site_out<E>(apply1<false>(v.z, 0.f, o + 2, ca, cb, cq, K), rv.z, bits, 2),
+                                             site_out<E>(apply1<false>(v.w, 0.f, o + 3, ca, cb, cq, K), rv.w, bits, 3)));
+        if constexpr (kEpiMk<E>) ep.mask[e] = (uint8_t)bits;
+      }
+      continue;
+    }
     const float4 v = ld4(x + 4 * (size_t)e), d = BWD ? ld4(dy + 4 * (size_t)e) : float4{};
     st4(out + 4 * (size_t)e, make_float4(apply1<BWD>(v.x, d.x, o, ca, cb, cq, K), apply1<BWD>(v.y, d.y, o + 1, ca, cb, cq, K),
                                          apply1<BWD>(v.z, d.z, o + 2, ca, cb, cq, K),
@@ -569,6 +692,21 @@ __device__ __forceinline__ void lds_load(float (&cf)[NC], int o, size_t gi, cons
   }
 }
 
+// a site's forward coefficients: lds_load's with diag(gamma) folded into A_n's rows and beta into the bias (c0: the
+// group's first channel).  The forward apply and both backward passes load them here, so a recomputed pre-activation
+// is the forward's bit for bit.
+template <int GS, int NC>
+__device__ __forceinline__ void lds_site_load(float (&cf)[NC], int o, size_t gi, int c0, const LdEpi& ep) {
+  lds_load<GS, false>(cf, o, gi, ep.p0, ep.p1, nullptr);
+#pragma unroll
+  for (int i = 0; i < GS; ++i) {
+    const float gam = __ldg(ep.gamma + c0 + i);
+#pragma unroll
+    for (int j = 0; j <= i; ++j) cf[o + i * (i + 1) / 2 + j] *= gam;
+    cf[o + LdsDim<GS>::T + i] = fmaf(gam, cf[o + LdsDim<GS>::T + i], __ldg(ep.beta + c0 + i));
+  }
+}
+
 // forward y_i = bp_i + sum_{j<=i} A_ij x_j;  backward dx_i = c_i + sum_j B_ij (x_j - m_j) + sum_{j>=i} A_ji dy_j
 template <int GS, bool BWD, int NC>
 __device__ __forceinline__ void lds_map(const float (&cf)[NC], int o, const float (&x)[GS], const float (&dy)[GS],
@@ -592,12 +730,22 @@ __device__ __forceinline__ void lds_map(const float (&cf)[NC], int o, const floa
   }
 }
 
+// a site's ReLU mask recomputed on one pixel of a group: dy_i = 0 where the forward's pre-activation is <= 0
+template <int GS, int NC>
+__device__ __forceinline__ void lds_relu_dy(const float (&fc)[NC], int o, const float (&x)[GS], float (&dy)[GS]) {
+  float z[GS];
+  lds_map<GS, false>(fc, o, x, dy, z);
+#pragma unroll
+  for (int i = 0; i < GS; ++i) dy[i] = relu_pass(z[i]) ? dy[i] : 0.f;
+}
+
 // NCHW reduction: a warp per (image, group, segment) over the group's GS rows.  VEC: HW % 4 == 0.  stats: save_stats
-// (backward: the image means are the centre).
-template <int GS, bool BWD, bool VEC, class T>
+// (backward: the image means are the centre).  E (backward): RC masks dy by the recomputed pre-activation.
+template <int GS, bool BWD, bool VEC, class T, int E = 0>
 __global__ void __launch_bounds__(kThreads, 1) lds_reduce_nchw(const T* __restrict__ x, const T* __restrict__ dy, LdbnGeom g,
                                                             const float* __restrict__ stats, float* __restrict__ part,
-                                                            float* __restrict__ pilot) {
+                                                            float* __restrict__ pilot, LdEpi ep) {
+  static_assert(!kEpiMk<E>, "an NCHW residual's backward runs on dz without the epilogue");
   using Dm = LdsDim<GS>;
   constexpr int NA = BWD ? Dm::NB : Dm::NF;
   const long long wid = ((long long)blockIdx.x * kThreads + threadIdx.x) >> 5;
@@ -615,6 +763,8 @@ __global__ void __launch_bounds__(kThreads, 1) lds_reduce_nchw(const T* __restri
   float a[NA];
 #pragma unroll
   for (int k = 0; k < NA; ++k) a[k] = 0.f;
+  float fc[kEpiRc<E> ? Dm::NCF : 1];
+  if constexpr (kEpiRc<E>) lds_site_load<GS>(fc, 0, (size_t)row, (int)(row % G) * GS, ep);
   float xv[GS], dv[GS];
   if (VEC) {
 #pragma unroll kLdsVecUnroll<GS>
@@ -629,6 +779,7 @@ __global__ void __launch_bounds__(kThreads, 1) lds_reduce_nchw(const T* __restri
       for (int e = 0; e < 4; ++e) {
 #pragma unroll
         for (int i = 0; i < GS; ++i) { xv[i] = lane4(v[i], e); dv[i] = lane4(d[i], e); }
+        if constexpr (kEpiRc<E>) lds_relu_dy<GS>(fc, 0, xv, dv);
         lds_acc<GS, BWD>(a, 0, xv, dv, K);
       }
     }
@@ -640,6 +791,7 @@ __global__ void __launch_bounds__(kThreads, 1) lds_reduce_nchw(const T* __restri
         xv[i] = ld1(x + base + (size_t)i * g.HW + p);
         dv[i] = BWD ? ld1(dy + base + (size_t)i * g.HW + p) : 0.f;
       }
+      if constexpr (kEpiRc<E>) lds_relu_dy<GS>(fc, 0, xv, dv);
       lds_acc<GS, BWD>(a, 0, xv, dv, K);
     }
   }
@@ -658,11 +810,12 @@ __global__ void __launch_bounds__(kThreads, 1) lds_reduce_nchw(const T* __restri
 }
 
 // channels-last reduction: ldbn_reduce_nhwc's CTA (slab, segment, image); a thread's 4 channels are 4/GS groups, the
-// pixel rows added in order through shared memory
-template <int GS, bool BWD, class T>
+// pixel rows added in order through shared memory.  E (backward): RC as lds_reduce_nchw; MK masks dy by the byte map and
+// writes it to ep.dz.
+template <int GS, bool BWD, class T, int E = 0>
 __global__ void __launch_bounds__(kThreads, 1) lds_reduce_nhwc(const T* __restrict__ x, const T* __restrict__ dy, LdbnGeom g,
                                                             const float* __restrict__ stats, float* __restrict__ part,
-                                                            float* __restrict__ pilot) {
+                                                            float* __restrict__ pilot, LdEpi ep) {
   using Dm = LdsDim<GS>;
   constexpr int NA = BWD ? Dm::NB : Dm::NF, NV = Dm::PER4 * NA;
   __shared__ float sm[NV * kThreads];
@@ -692,15 +845,27 @@ __global__ void __launch_bounds__(kThreads, 1) lds_reduce_nhwc(const T* __restri
       K[0] = k.x; K[1] = k.y; K[2] = k.z; K[3] = k.w;
     }
     const int p0 = s * g.P, p1 = min(p0 + g.P, g.HW);
+    float fc[kEpiRc<E> ? Dm::PER4 * Dm::NCF : 1];
+    if constexpr (kEpiRc<E>) {
+#pragma unroll
+      for (int t = 0; t < Dm::PER4; ++t)
+        lds_site_load<GS>(fc, t * Dm::NCF, (size_t)n * G + 4 * c4 / GS + t, 4 * c4 + t * GS, ep);
+    }
 #pragma unroll 4
     for (int p = p0 + r; p < p1; p += g.pr) {
       const float4 v = ld4(x + img + (size_t)p * g.C);
-      const float4 d = BWD ? ld4(dy + img + (size_t)p * g.C) : float4{};
+      float4 d = BWD ? ld4(dy + img + (size_t)p * g.C) : float4{};
+      if constexpr (kEpiMk<E>) {
+        const unsigned bits = __ldg(ep.mask + ((size_t)n * g.HW + p) * (g.C / 4) + c4);
+        d = make_float4(bit_dy(bits, 0, d.x), bit_dy(bits, 1, d.y), bit_dy(bits, 2, d.z), bit_dy(bits, 3, d.w));
+        st4(static_cast<T*>(ep.dz) + img + (size_t)p * g.C, d);
+      }
 #pragma unroll
       for (int t = 0; t < Dm::PER4; ++t) {
         float xv[GS], dv[GS], kv[GS];
 #pragma unroll
         for (int i = 0; i < GS; ++i) { xv[i] = lane4(v, t * GS + i); dv[i] = lane4(d, t * GS + i); kv[i] = K[t * GS + i]; }
+        if constexpr (kEpiRc<E>) lds_relu_dy<GS>(fc, t * Dm::NCF, xv, dv);
         lds_acc<GS, BWD>(a, t * NA, xv, dv, kv);
       }
     }
@@ -720,11 +885,31 @@ __global__ void __launch_bounds__(kThreads, 1) lds_reduce_nhwc(const T* __restri
   }
 }
 
-// NCHW apply: the reduction's warps, the group's coefficients held for the segment
-template <int GS, bool BWD, bool VEC, class T>
+// A site pixel of one group in the apply passes.  Forward: the folded map, the residual r and the ReLU (bit t GS + i of
+// bits: out > 0).  Backward: dy masked by the recomputed pre-activation (RC), times gamma, through the backward map.
+template <int GS, bool BWD, int E, int NC, int NF>
+__device__ __forceinline__ void lds_site_px(const float (&cf)[NC], const float (&fc)[NF], int o, int of, const float (&gam)[4],
+                                            int t, const float (&x)[GS], float (&dy)[GS], const float* r, float (&out)[GS],
+                                            unsigned& bits) {
+  if constexpr (BWD) {
+    if constexpr (kEpiRc<E>) lds_relu_dy<GS>(fc, of, x, dy);
+#pragma unroll
+    for (int i = 0; i < GS; ++i) dy[i] *= gam[t * GS + i];
+    lds_map<GS, true>(cf, o, x, dy, out);
+  } else {
+    lds_map<GS, false>(cf, o, x, dy, out);
+#pragma unroll
+    for (int i = 0; i < GS; ++i) out[i] = site_out<E>(out[i], r[i], bits, t * GS + i);
+  }
+}
+
+// NCHW apply: the reduction's warps, the group's coefficients held for the segment.  E: a site (lds_site_px; an NCHW
+// residual's forward reads it, no byte map).
+template <int GS, bool BWD, bool VEC, class T, int E = 0>
 __global__ void __launch_bounds__(kThreads, 1) lds_apply_nchw(const T* __restrict__ x, const T* __restrict__ dy,
                                                            T* __restrict__ out, LdbnGeom g, const float* __restrict__ save_mean,
-                                                           const float* __restrict__ save_w, const float* __restrict__ coef) {
+                                                           const float* __restrict__ save_w, const float* __restrict__ coef,
+                                                           LdEpi ep) {
   using Dm = LdsDim<GS>;
   constexpr int NC = BWD ? Dm::NCB : Dm::NCF;
   const long long wid = ((long long)blockIdx.x * kThreads + threadIdx.x) >> 5;
@@ -735,51 +920,110 @@ __global__ void __launch_bounds__(kThreads, 1) lds_apply_nchw(const T* __restric
   const int s = (int)(wid - row * g.S);
   const size_t base = (size_t)row * GS * g.HW;
   float cf[NC];
-  lds_load<GS, BWD>(cf, 0, (size_t)row, save_mean, save_w, coef);
-  const int p0 = s * g.P, p1 = min(p0 + g.P, g.HW);
-  float xv[GS], dv[GS], ov[GS];
-  if (VEC) {
+  if constexpr (E != 0) {
+    static_assert((E & DWT_EPI_AFFINE) && !(BWD && kEpiMk<E>), "a site has AFFINE; a residual's backward reads dz");
+    const int c0 = (int)(row % (g.C / GS)) * GS;
+    float fc[BWD && kEpiRc<E> ? Dm::NCF : 1], gam[4] = {1.f, 1.f, 1.f, 1.f};
+    if constexpr (BWD) {
+      lds_load<GS, true>(cf, 0, (size_t)row, save_mean, save_w, coef);
+      if constexpr (kEpiRc<E>) lds_site_load<GS>(fc, 0, (size_t)row, c0, ep);
+#pragma unroll
+      for (int i = 0; i < GS; ++i) gam[i] = __ldg(ep.gamma + c0 + i);
+    } else {
+      lds_site_load<GS>(cf, 0, (size_t)row, c0, ep);
+    }
+    const T* res = static_cast<const T*>(ep.res);
+    const int p0 = s * g.P, p1 = min(p0 + g.P, g.HW);
+    float xv[GS], dv[GS], rv[GS], ov[GS];
+    unsigned bits = 0;
+#pragma unroll
+    for (int i = 0; i < GS; ++i) rv[i] = 0.f;
+    if (VEC) {
 #pragma unroll kLdsVecUnroll<GS>
-    for (int p = p0 + 4 * lane; p < p1; p += 128) {
-      float4 v[GS], d[GS];
-      float o4[GS][4];
+      for (int p = p0 + 4 * lane; p < p1; p += 128) {
+        float4 v[GS], d[GS], r4[GS];
+        float o4[GS][4];
 #pragma unroll
-      for (int i = 0; i < GS; ++i) {
-        v[i] = ld4(x + base + (size_t)i * g.HW + p);
-        d[i] = BWD ? ld4(dy + base + (size_t)i * g.HW + p) : float4{};
+        for (int i = 0; i < GS; ++i) {
+          v[i] = ld4(x + base + (size_t)i * g.HW + p);
+          d[i] = BWD ? ld4(dy + base + (size_t)i * g.HW + p) : float4{};
+          r4[i] = (!BWD && kEpiMk<E>) ? ld4(res + base + (size_t)i * g.HW + p) : float4{};
+        }
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+#pragma unroll
+          for (int i = 0; i < GS; ++i) { xv[i] = lane4(v[i], e); dv[i] = lane4(d[i], e); rv[i] = lane4(r4[i], e); }
+          lds_site_px<GS, BWD, E>(cf, fc, 0, 0, gam, 0, xv, dv, rv, ov, bits);
+#pragma unroll
+          for (int i = 0; i < GS; ++i) o4[i][e] = ov[i];
+        }
+#pragma unroll
+        for (int i = 0; i < GS; ++i)
+          st4(out + base + (size_t)i * g.HW + p, make_float4(o4[i][0], o4[i][1], o4[i][2], o4[i][3]));
       }
+    } else {
+#pragma unroll 4
+      for (int p = p0 + lane; p < p1; p += 32) {
 #pragma unroll
-      for (int e = 0; e < 4; ++e) {
+        for (int i = 0; i < GS; ++i) {
+          xv[i] = ld1(x + base + (size_t)i * g.HW + p);
+          dv[i] = BWD ? ld1(dy + base + (size_t)i * g.HW + p) : 0.f;
+          if (!BWD && kEpiMk<E>) rv[i] = ld1(res + base + (size_t)i * g.HW + p);
+        }
+        lds_site_px<GS, BWD, E>(cf, fc, 0, 0, gam, 0, xv, dv, rv, ov, bits);
 #pragma unroll
-        for (int i = 0; i < GS; ++i) { xv[i] = lane4(v[i], e); dv[i] = lane4(d[i], e); }
-        lds_map<GS, BWD>(cf, 0, xv, dv, ov);
-#pragma unroll
-        for (int i = 0; i < GS; ++i) o4[i][e] = ov[i];
+        for (int i = 0; i < GS; ++i) st1(out + base + (size_t)i * g.HW + p, ov[i]);
       }
-#pragma unroll
-      for (int i = 0; i < GS; ++i)
-        st4(out + base + (size_t)i * g.HW + p, make_float4(o4[i][0], o4[i][1], o4[i][2], o4[i][3]));
     }
   } else {
-#pragma unroll 4
-    for (int p = p0 + lane; p < p1; p += 32) {
-#pragma unroll
-      for (int i = 0; i < GS; ++i) {
-        xv[i] = ld1(x + base + (size_t)i * g.HW + p);
-        dv[i] = BWD ? ld1(dy + base + (size_t)i * g.HW + p) : 0.f;
+    lds_load<GS, BWD>(cf, 0, (size_t)row, save_mean, save_w, coef);
+    const int p0 = s * g.P, p1 = min(p0 + g.P, g.HW);
+    float xv[GS], dv[GS], ov[GS];
+    if (VEC) {
+  #pragma unroll kLdsVecUnroll<GS>
+      for (int p = p0 + 4 * lane; p < p1; p += 128) {
+        float4 v[GS], d[GS];
+        float o4[GS][4];
+  #pragma unroll
+        for (int i = 0; i < GS; ++i) {
+          v[i] = ld4(x + base + (size_t)i * g.HW + p);
+          d[i] = BWD ? ld4(dy + base + (size_t)i * g.HW + p) : float4{};
+        }
+  #pragma unroll
+        for (int e = 0; e < 4; ++e) {
+  #pragma unroll
+          for (int i = 0; i < GS; ++i) { xv[i] = lane4(v[i], e); dv[i] = lane4(d[i], e); }
+          lds_map<GS, BWD>(cf, 0, xv, dv, ov);
+  #pragma unroll
+          for (int i = 0; i < GS; ++i) o4[i][e] = ov[i];
+        }
+  #pragma unroll
+        for (int i = 0; i < GS; ++i)
+          st4(out + base + (size_t)i * g.HW + p, make_float4(o4[i][0], o4[i][1], o4[i][2], o4[i][3]));
       }
-      lds_map<GS, BWD>(cf, 0, xv, dv, ov);
-#pragma unroll
-      for (int i = 0; i < GS; ++i) st1(out + base + (size_t)i * g.HW + p, ov[i]);
+    } else {
+  #pragma unroll 4
+      for (int p = p0 + lane; p < p1; p += 32) {
+  #pragma unroll
+        for (int i = 0; i < GS; ++i) {
+          xv[i] = ld1(x + base + (size_t)i * g.HW + p);
+          dv[i] = BWD ? ld1(dy + base + (size_t)i * g.HW + p) : 0.f;
+        }
+        lds_map<GS, BWD>(cf, 0, xv, dv, ov);
+  #pragma unroll
+        for (int i = 0; i < GS; ++i) st1(out + base + (size_t)i * g.HW + p, ov[i]);
+      }
     }
   }
 }
 
-// channels-last apply: the reduction's CTAs, a thread's 4/GS groups' coefficients held for the segment
-template <int GS, bool BWD, class T>
+// channels-last apply: the reduction's CTAs, a thread's 4/GS groups' coefficients held for the segment.  E: a site
+// (lds_site_px); a residual's forward writes the byte map.
+template <int GS, bool BWD, class T, int E = 0>
 __global__ void __launch_bounds__(kThreads, 1) lds_apply_nhwc(const T* __restrict__ x, const T* __restrict__ dy,
                                                            T* __restrict__ out, LdbnGeom g, const float* __restrict__ save_mean,
-                                                           const float* __restrict__ save_w, const float* __restrict__ coef) {
+                                                           const float* __restrict__ save_w, const float* __restrict__ coef,
+                                                           LdEpi ep) {
   using Dm = LdsDim<GS>;
   constexpr int NC = BWD ? Dm::NCB : Dm::NCF;
   const int slabs = (g.C / 4 + g.qc - 1) / g.qc;
@@ -791,26 +1035,67 @@ __global__ void __launch_bounds__(kThreads, 1) lds_apply_nhwc(const T* __restric
   const int c4 = slab * g.qc + q;
   if (r >= g.pr || c4 >= g.C / 4) return;
   float cf[Dm::PER4 * NC];
-#pragma unroll
-  for (int t = 0; t < Dm::PER4; ++t)
-    lds_load<GS, BWD>(cf, t * NC, (size_t)n * (g.C / GS) + 4 * c4 / GS + t, save_mean, save_w, coef);
-  const size_t img = (size_t)n * g.HW * g.C + 4 * c4;
-  const int p0 = s * g.P, p1 = min(p0 + g.P, g.HW);
-#pragma unroll 4
-  for (int p = p0 + r; p < p1; p += g.pr) {
-    const float4 v = ld4(x + img + (size_t)p * g.C);
-    const float4 d = BWD ? ld4(dy + img + (size_t)p * g.C) : float4{};
-    float o[4];
+  if constexpr (E != 0) {
+    static_assert((E & DWT_EPI_AFFINE) && !(BWD && kEpiMk<E>), "a site has AFFINE; a residual's backward reads dz");
+    float fc[BWD && kEpiRc<E> ? Dm::PER4 * Dm::NCF : 1], gam[4];
 #pragma unroll
     for (int t = 0; t < Dm::PER4; ++t) {
-      float xv[GS], dv[GS], ov[GS];
-#pragma unroll
-      for (int i = 0; i < GS; ++i) { xv[i] = lane4(v, t * GS + i); dv[i] = lane4(d, t * GS + i); }
-      lds_map<GS, BWD>(cf, t * NC, xv, dv, ov);
-#pragma unroll
-      for (int i = 0; i < GS; ++i) o[t * GS + i] = ov[i];
+      const size_t gi = (size_t)n * (g.C / GS) + 4 * c4 / GS + t;
+      if constexpr (BWD) {
+        lds_load<GS, true>(cf, t * NC, gi, save_mean, save_w, coef);
+        if constexpr (kEpiRc<E>) lds_site_load<GS>(fc, t * Dm::NCF, gi, 4 * c4 + t * GS, ep);
+      } else {
+        lds_site_load<GS>(cf, t * NC, gi, 4 * c4 + t * GS, ep);
+      }
     }
-    st4(out + img + (size_t)p * g.C, make_float4(o[0], o[1], o[2], o[3]));
+#pragma unroll
+    for (int j = 0; j < 4; ++j) gam[j] = BWD ? __ldg(ep.gamma + 4 * c4 + j) : 1.f;
+    const size_t img = (size_t)n * g.HW * g.C + 4 * c4;
+    const int p0 = s * g.P, p1 = min(p0 + g.P, g.HW);
+#pragma unroll 4
+    for (int p = p0 + r; p < p1; p += g.pr) {
+      const size_t at = img + (size_t)p * g.C;
+      const float4 v = ld4(x + at);
+      const float4 d = BWD ? ld4(dy + at) : float4{};
+      const float4 rr = (!BWD && kEpiMk<E>) ? ld4(static_cast<const T*>(ep.res) + at) : float4{};
+      float o[4];
+      unsigned bits = 0;
+#pragma unroll
+      for (int t = 0; t < Dm::PER4; ++t) {
+        float xv[GS], dv[GS], rv[GS], ov[GS];
+#pragma unroll
+        for (int i = 0; i < GS; ++i) {
+          xv[i] = lane4(v, t * GS + i); dv[i] = lane4(d, t * GS + i); rv[i] = lane4(rr, t * GS + i);
+        }
+        lds_site_px<GS, BWD, E>(cf, fc, t * NC, t * Dm::NCF, gam, t, xv, dv, rv, ov, bits);
+#pragma unroll
+        for (int i = 0; i < GS; ++i) o[t * GS + i] = ov[i];
+      }
+      st4(out + at, make_float4(o[0], o[1], o[2], o[3]));
+      if constexpr (!BWD && kEpiMk<E>) ep.mask[at / 4] = (uint8_t)bits;
+    }
+  } else {
+  #pragma unroll
+    for (int t = 0; t < Dm::PER4; ++t)
+      lds_load<GS, BWD>(cf, t * NC, (size_t)n * (g.C / GS) + 4 * c4 / GS + t, save_mean, save_w, coef);
+    const size_t img = (size_t)n * g.HW * g.C + 4 * c4;
+    const int p0 = s * g.P, p1 = min(p0 + g.P, g.HW);
+  #pragma unroll 4
+    for (int p = p0 + r; p < p1; p += g.pr) {
+      const float4 v = ld4(x + img + (size_t)p * g.C);
+      const float4 d = BWD ? ld4(dy + img + (size_t)p * g.C) : float4{};
+      float o[4];
+  #pragma unroll
+      for (int t = 0; t < Dm::PER4; ++t) {
+        float xv[GS], dv[GS], ov[GS];
+  #pragma unroll
+        for (int i = 0; i < GS; ++i) { xv[i] = lane4(v, t * GS + i); dv[i] = lane4(d, t * GS + i); }
+        lds_map<GS, BWD>(cf, t * NC, xv, dv, ov);
+  #pragma unroll
+        for (int i = 0; i < GS; ++i) o[t * GS + i] = ov[i];
+      }
+      st4(out + img + (size_t)p * g.C, make_float4(o[0], o[1], o[2], o[3]));
+    }
   }
 }
 
@@ -1054,10 +1339,15 @@ __global__ void __launch_bounds__(kThreads) lds_fwd_mix(const LdsFin f) {
   if (bad) atomicOr(f.status, DWT_STATUS_NOT_PD);
 }
 
-// per (image, group): the backward segment partials added in order (fp64) into red = g_n | R_n
-template <int GS>
+// per (image, group): the backward segment partials added in order (fp64) into red = g_n | R_n.  AFF (a site): the
+// partials are those of dz, the gradient of gamma zhat + beta; with zhat = A_n (x - m~_n) the image's shares
+//   dgamma_i = sum_{j<=i} A_ij Rz_ij + [A_n (m_n - m~_n)]_i gz_i,   dbeta_i = gz_i
+// go to pgb ([2][N][C]), and red gets the sums of the whitened value's gradient gamma dz: g_n = gamma gz, R_n's rows
+// scaled by gamma.
+template <int GS, bool AFF = false>
 __global__ void __launch_bounds__(kThreads) lds_bwd_image(const LdsFin f, const float* __restrict__ part,
-                                                          float* __restrict__ red) {
+                                                          float* __restrict__ red, const float* __restrict__ gamma,
+                                                          float* __restrict__ pgb) {
   using Dm = LdsDim<GS>;
   const int gi = blockIdx.x * kThreads + threadIdx.x;
   if (gi >= f.N * f.G) return;
@@ -1070,8 +1360,44 @@ __global__ void __launch_bounds__(kThreads) lds_bwd_image(const LdsFin f, const 
 #pragma unroll
     for (int k = 0; k < Dm::NB; ++k) acc[k] += p[k];
   }
+  if constexpr (AFF) {
+    const float* A = f.save_w + (size_t)gi * GS * GS;
+    const float* mt = f.save_mean + (size_t)gi * GS;
+    const float* m = f.save_stats + (size_t)gi * Dm::REC + GS * GS;
+#pragma unroll
+    for (int i = 0; i < GS; ++i) {
+      double dg = 0.0, off = 0.0;
+#pragma unroll
+      for (int j = 0; j <= i; ++j) {
+        const double a = A[i * GS + j];
+        dg += a * acc[GS + i * GS + j];
+        off += a * ((double)m[j] - (double)mt[j]);
+      }
+      const int c = grp * GS + i;
+      pgb[(size_t)n * f.C + c] = (float)(dg + off * acc[i]);
+      pgb[((size_t)f.N + n) * f.C + c] = (float)acc[i];
+      const double gam = gamma[c];
+      acc[i] *= gam;
+#pragma unroll
+      for (int j = 0; j < GS; ++j) acc[GS + i * GS + j] *= gam;
+    }
+  }
 #pragma unroll
   for (int k = 0; k < Dm::NB; ++k) red[(size_t)gi * Dm::NB + k] = (float)acc[k];
+}
+
+// a site's dgamma[c], dbeta[c]: the images' shares in order (fp64)
+__global__ void __launch_bounds__(kThreads) lds_site_dgb(const float* __restrict__ pgb, int N, int C,
+                                                         float* __restrict__ dgamma, float* __restrict__ dbeta) {
+  const int c = blockIdx.x * kThreads + threadIdx.x;
+  if (c >= C) return;
+  double tg = 0.0, tb = 0.0;
+  for (int n = 0; n < N; ++n) {
+    tg += pgb[(size_t)n * C + c];
+    tb += pgb[((size_t)N + n) * C + c];
+  }
+  dgamma[c] = (float)tg;
+  dbeta[c] = (float)tb;
 }
 
 // a warp per (domain, group), train, s_k != 0: Wbar_k = sum_n w_nk [R_n + g_n (m_n - mu_k)^T] and sum_n w_nk g_n (fp64,
@@ -1274,33 +1600,45 @@ int ew_blocks(size_t work) {
   return (int)(want < cap ? (want < 1 ? 1 : want) : cap);
 }
 
-template <bool BWD, class T>
+template <bool BWD, class T, int E = 0>
 void reduce(const void* x, const void* dy, const LdbnGeom& g, const float* centre, float* pa, float* pb, float* pilot,
-            cudaStream_t st) {
+            cudaStream_t st, const LdEpi& ep = LdEpi{}) {
   const T* xt = static_cast<const T*>(x);
   const T* dt = static_cast<const T*>(dy);
   if (g.nhwc) {
     const int slabs = (g.C / 4 + g.qc - 1) / g.qc;
-    ldbn_reduce_nhwc<BWD, T><<<(unsigned)((size_t)slabs * g.S * g.N), kThreads, 0, st>>>(xt, dt, g, centre, pa, pb, pilot);
-  } else {
+    ldbn_reduce_nhwc<BWD, T, E><<<(unsigned)((size_t)slabs * g.S * g.N), kThreads, 0, st>>>(xt, dt, g, centre, pa, pb,
+                                                                                             pilot, ep);
+  } else if constexpr (!kEpiMk<E>) {
     const size_t warps = (size_t)g.N * g.C * g.S;
     const unsigned blocks = (unsigned)((warps + kWarps - 1) / kWarps);
-    if (g.HW % 4 == 0) ldbn_reduce_nchw<BWD, true, T><<<blocks, kThreads, 0, st>>>(xt, dt, g, centre, pa, pb, pilot);
-    else ldbn_reduce_nchw<BWD, false, T><<<blocks, kThreads, 0, st>>>(xt, dt, g, centre, pa, pb, pilot);
+    if (g.HW % 4 == 0) ldbn_reduce_nchw<BWD, true, T, E><<<blocks, kThreads, 0, st>>>(xt, dt, g, centre, pa, pb, pilot, ep);
+    else ldbn_reduce_nchw<BWD, false, T, E><<<blocks, kThreads, 0, st>>>(xt, dt, g, centre, pa, pb, pilot, ep);
   }
 }
 
-template <bool BWD, class T>
+template <bool BWD, class T, int E = 0>
 void apply(const void* x, const void* dy, void* out, const LdbnGeom& g, const float* ca, const float* cb, const float* cq,
-           const float* K, cudaStream_t st) {
+           const float* K, cudaStream_t st, const LdEpi& ep = LdEpi{}) {
   const T* xt = static_cast<const T*>(x);
   const T* dt = static_cast<const T*>(dy);
   T* ot = static_cast<T*>(out);
   const size_t n = (size_t)g.N * g.C * g.HW;
-  if (g.nhwc) ldbn_apply_nhwc<BWD, T><<<ew_blocks(n / 4), kThreads, 0, st>>>(xt, dt, ot, g, ca, cb, cq, K);
-  else if (g.HW % 4 == 0) ldbn_apply_nchw<BWD, true, T><<<ew_blocks(n / 4), kThreads, 0, st>>>(xt, dt, ot, g, ca, cb, cq, K);
-  else ldbn_apply_nchw<BWD, false, T><<<ew_blocks(n), kThreads, 0, st>>>(xt, dt, ot, g, ca, cb, cq, K);
+  if (g.nhwc) ldbn_apply_nhwc<BWD, T, E><<<ew_blocks(n / 4), kThreads, 0, st>>>(xt, dt, ot, g, ca, cb, cq, K, ep);
+  else if (g.HW % 4 == 0)
+    ldbn_apply_nchw<BWD, true, T, E><<<ew_blocks(n / 4), kThreads, 0, st>>>(xt, dt, ot, g, ca, cb, cq, K, ep);
+  else ldbn_apply_nchw<BWD, false, T, E><<<ew_blocks(n), kThreads, 0, st>>>(xt, dt, ot, g, ca, cb, cq, K, ep);
 }
+
+// a site's epilogue bits -> the kernels' E: forward RELU or RELU|RESIDUAL; backward RELU (recomputed mask) or
+// RELU|RESIDUAL (channels-last byte map, reduction only); AFFINE alone (in the coefficients) runs the plain kernels
+#define DWT_LD_SITE(EPI, ...)                                                                                          \
+  do {                                                                                                                 \
+    const int e_ = (EPI) & (DWT_EPI_RELU | DWT_EPI_RESIDUAL);                                                          \
+    if (e_ == (DWT_EPI_RELU | DWT_EPI_RESIDUAL)) { constexpr int E = DWT_EPI_RELU | DWT_EPI_RESIDUAL; __VA_ARGS__; }   \
+    else if (e_ == DWT_EPI_RELU) { constexpr int E = DWT_EPI_RELU; __VA_ARGS__; }                                      \
+    else { constexpr int E = 0; __VA_ARGS__; }                                                                         \
+  } while (0)
 
 }  // namespace
 
@@ -1378,6 +1716,30 @@ void ldbn_bwd_apply(const void* x, const void* dy, void* dx, const LdbnGeom& g, 
   else apply<true, float>(x, dy, dx, g, ca, cp, cq, centre, st);
 }
 
+void ldbn_site_apply(const void* x, void* y, const LdbnGeom& g, const float* alpha, const float* shift, int epi,
+                     const LdEpi& ep, cudaStream_t st) {
+  DWT_LD_SITE(epi, {
+    if (g.bf16) apply<false, __nv_bfloat16, E>(x, nullptr, y, g, alpha, shift, nullptr, nullptr, st, ep);
+    else apply<false, float, E>(x, nullptr, y, g, alpha, shift, nullptr, nullptr, st, ep);
+  });
+}
+
+void ldbn_site_bwd_reduce(const void* x, const void* dy, const LdbnGeom& g, const float* centre, float* pa, float* pb,
+                          int epi, const LdEpi& ep, cudaStream_t st) {
+  DWT_LD_SITE(epi, {
+    if (g.bf16) reduce<true, __nv_bfloat16, E>(x, dy, g, centre, pa, pb, nullptr, st, ep);
+    else reduce<true, float, E>(x, dy, g, centre, pa, pb, nullptr, st, ep);
+  });
+}
+
+// the residual's backward apply reads dz: the plain kernels
+void ldbn_site_bwd_apply(const void* x, const void* dy, void* dx, const LdbnGeom& g, const float* ca, const float* cp,
+                         const float* cq, const float* centre, int epi, const LdEpi& ep, cudaStream_t st) {
+  if ((epi & (DWT_EPI_RELU | DWT_EPI_RESIDUAL)) != DWT_EPI_RELU) return ldbn_bwd_apply(x, dy, dx, g, ca, cp, cq, centre, st);
+  if (g.bf16) apply<true, __nv_bfloat16, DWT_EPI_RELU>(x, dy, dx, g, ca, cp, cq, centre, st, ep);
+  else apply<true, float, DWT_EPI_RELU>(x, dy, dx, g, ca, cp, cq, centre, st, ep);
+}
+
 namespace {
 
 // grid of the bandwidth passes: NCHW a warp per (image, group, segment), channels-last a CTA per (slab, segment, image)
@@ -1388,38 +1750,54 @@ unsigned lds_blocks(const LdbnGeom& g, int GS) {
 }
 
 // PASS 0: forward statistics, 1: forward apply, 2: backward reduction, 3: backward apply.  NCHW bf16 runs at HW % 4 == 0.
-template <int GS, int PASS, class T>
+// E: a site's epilogue (lds_site_*).
+template <int GS, int PASS, class T, int E = 0>
 void lds_launch(const void* x, const void* dy, void* out, const LdbnGeom& g, const float* p0, const float* p1,
-                const float* p2, float* part, float* pilot, cudaStream_t st) {
+                const float* p2, float* part, float* pilot, cudaStream_t st, const LdEpi& ep = LdEpi{}) {
   constexpr bool BWD = PASS >= 2, APPLY = PASS == 1 || PASS == 3;
   const T* xt = static_cast<const T*>(x);
   const T* dt = static_cast<const T*>(dy);
   T* ot = static_cast<T*>(out);
   const unsigned blocks = lds_blocks(g, GS);
   if (g.nhwc) {
-    if constexpr (APPLY) lds_apply_nhwc<GS, BWD, T><<<blocks, kThreads, 0, st>>>(xt, dt, ot, g, p0, p1, p2);
-    else lds_reduce_nhwc<GS, BWD, T><<<blocks, kThreads, 0, st>>>(xt, dt, g, p0, part, pilot);
+    if constexpr (APPLY) lds_apply_nhwc<GS, BWD, T, E><<<blocks, kThreads, 0, st>>>(xt, dt, ot, g, p0, p1, p2, ep);
+    else lds_reduce_nhwc<GS, BWD, T, E><<<blocks, kThreads, 0, st>>>(xt, dt, g, p0, part, pilot, ep);
     return;
   }
-  if (g.HW % 4 == 0) {
-    if constexpr (APPLY) lds_apply_nchw<GS, BWD, true, T><<<blocks, kThreads, 0, st>>>(xt, dt, ot, g, p0, p1, p2);
-    else lds_reduce_nchw<GS, BWD, true, T><<<blocks, kThreads, 0, st>>>(xt, dt, g, p0, part, pilot);
+  if constexpr (!APPLY && kEpiMk<E>) return;
+  else if (g.HW % 4 == 0) {
+    if constexpr (APPLY) lds_apply_nchw<GS, BWD, true, T, E><<<blocks, kThreads, 0, st>>>(xt, dt, ot, g, p0, p1, p2, ep);
+    else lds_reduce_nchw<GS, BWD, true, T, E><<<blocks, kThreads, 0, st>>>(xt, dt, g, p0, part, pilot, ep);
   } else if constexpr (std::is_same<T, float>::value) {
-    if constexpr (APPLY) lds_apply_nchw<GS, BWD, false, T><<<blocks, kThreads, 0, st>>>(xt, dt, ot, g, p0, p1, p2);
-    else lds_reduce_nchw<GS, BWD, false, T><<<blocks, kThreads, 0, st>>>(xt, dt, g, p0, part, pilot);
+    if constexpr (APPLY) lds_apply_nchw<GS, BWD, false, T, E><<<blocks, kThreads, 0, st>>>(xt, dt, ot, g, p0, p1, p2, ep);
+    else lds_reduce_nchw<GS, BWD, false, T, E><<<blocks, kThreads, 0, st>>>(xt, dt, g, p0, part, pilot, ep);
   }
 }
 
-template <int PASS>
+template <int PASS, int E = 0>
 void lds_pass(const void* x, const void* dy, void* out, const LdbnGeom& g, int GS, const float* p0, const float* p1,
-              const float* p2, float* part, float* pilot, cudaStream_t st) {
+              const float* p2, float* part, float* pilot, cudaStream_t st, const LdEpi& ep = LdEpi{}) {
 #define DWT_LDS_GS(G_)                                                                                                   \
   if (GS == G_) {                                                                                                        \
-    if (g.bf16) lds_launch<G_, PASS, __nv_bfloat16>(x, dy, out, g, p0, p1, p2, part, pilot, st);                         \
-    else lds_launch<G_, PASS, float>(x, dy, out, g, p0, p1, p2, part, pilot, st);                                        \
+    if (g.bf16) lds_launch<G_, PASS, __nv_bfloat16, E>(x, dy, out, g, p0, p1, p2, part, pilot, st, ep);                  \
+    else lds_launch<G_, PASS, float, E>(x, dy, out, g, p0, p1, p2, part, pilot, st, ep);                                 \
   }
   DWT_LDS_GS(1) else DWT_LDS_GS(2) else DWT_LDS_GS(4)
 #undef DWT_LDS_GS
+}
+
+// a site pass: the epilogue bits as that pass's kernels take them -- the backward reduction without a ReLU and the
+// backward apply of a residual (which reads dz) need only gamma, the reduction none of it
+template <int PASS>
+void lds_site_pass(const void* x, const void* dy, void* out, const LdbnGeom& g, int GS, const float* p0, const float* p1,
+                   const float* p2, float* part, int epi, const LdEpi& ep, cudaStream_t st) {
+  constexpr int A = DWT_EPI_AFFINE, AR = A | DWT_EPI_RELU, ARR = AR | DWT_EPI_RESIDUAL;
+  if (PASS == 2 && !(epi & DWT_EPI_RELU)) epi = 0;
+  if (PASS == 3 && (epi & DWT_EPI_RESIDUAL)) epi = A;
+  if (epi == ARR) { if constexpr (PASS != 3) lds_pass<PASS, ARR>(x, dy, out, g, GS, p0, p1, p2, part, nullptr, st, ep); }
+  else if (epi == AR) lds_pass<PASS, AR>(x, dy, out, g, GS, p0, p1, p2, part, nullptr, st, ep);
+  else if (epi == A) { if constexpr (PASS != 2) lds_pass<PASS, A>(x, dy, out, g, GS, p0, p1, p2, part, nullptr, st, ep); }
+  else lds_pass<PASS>(x, dy, out, g, GS, p0, p1, p2, part, nullptr, st);
 }
 
 unsigned lds_grid(int work) { return (unsigned)((work + kThreads - 1) / kThreads); }
@@ -1434,10 +1812,21 @@ void lds_fwd_fin(const LdsFin& f, const float* part, const float* pilot, double*
 template <int GS>
 void lds_bwd_fin(const LdsFin& f, const float* part, float* red, float* pd, float* pc, float* coef, float* dwpart,
                  float* dweights, cudaStream_t st) {
-  lds_bwd_image<GS><<<lds_grid(f.N * f.G), kThreads, 0, st>>>(f, part, red);
+  lds_bwd_image<GS><<<lds_grid(f.N * f.G), kThreads, 0, st>>>(f, part, red, nullptr, nullptr);
   if (f.train) lds_bwd_domain<GS><<<lds_grid(32 * f.K * f.G), kThreads, 0, st>>>(f, red, pd, pc);
   lds_bwd_coef<GS><<<lds_grid(f.N * f.G), kThreads, 0, st>>>(f, red, pd, pc, coef, dweights ? dwpart : nullptr);
   if (dweights) lds_dw<<<lds_grid(f.N * f.K), kThreads, 0, st>>>(dwpart, f.N, f.G, f.K, dweights);
+}
+
+// a site's backward finalize: lds_bwd_fin with gamma folded into the per-image sums, then dgamma / dbeta
+template <int GS>
+void lds_site_bwd_fin(const LdsFin& f, const float* part, float* red, float* pd, float* pc, float* coef, float* dwpart,
+                      float* dweights, const float* gamma, float* pgb, float* dgamma, float* dbeta, cudaStream_t st) {
+  lds_bwd_image<GS, true><<<lds_grid(f.N * f.G), kThreads, 0, st>>>(f, part, red, gamma, pgb);
+  if (f.train) lds_bwd_domain<GS><<<lds_grid(32 * f.K * f.G), kThreads, 0, st>>>(f, red, pd, pc);
+  lds_bwd_coef<GS><<<lds_grid(f.N * f.G), kThreads, 0, st>>>(f, red, pd, pc, coef, dweights ? dwpart : nullptr);
+  if (dweights) lds_dw<<<lds_grid(f.N * f.K), kThreads, 0, st>>>(dwpart, f.N, f.G, f.K, dweights);
+  if (dgamma) lds_site_dgb<<<lds_grid(f.C), kThreads, 0, st>>>(pgb, f.N, f.C, dgamma, dbeta);
 }
 
 }  // namespace
@@ -1481,6 +1870,28 @@ void lds_bwd_finalize(const LdsFin& f, const float* part, float* red, float* pd,
 
 void lds_bwd_apply(const void* x, const void* dy, void* dx, const LdbnGeom& g, int GS, const float* coef, cudaStream_t st) {
   lds_pass<3>(x, dy, dx, g, GS, nullptr, nullptr, coef, nullptr, nullptr, st);
+}
+
+void lds_site_apply(const void* x, void* y, const LdbnGeom& g, int GS, int epi, const LdEpi& ep, cudaStream_t st) {
+  lds_site_pass<1>(x, nullptr, y, g, GS, ep.p0, ep.p1, nullptr, nullptr, epi, ep, st);
+}
+
+void lds_site_bwd_reduce(const void* x, const void* dy, const LdbnGeom& g, int GS, const float* save_stats, float* part,
+                         int epi, const LdEpi& ep, cudaStream_t st) {
+  lds_site_pass<2>(x, dy, nullptr, g, GS, save_stats, nullptr, nullptr, part, epi, ep, st);
+}
+
+void lds_site_bwd_finalize(const LdsFin& f, const float* part, float* red, float* pd, float* pc, float* coef,
+                           float* dwpart, float* dweights, const float* gamma, float* pgb, float* dgamma, float* dbeta,
+                           cudaStream_t st) {
+  if (f.GS == 1) lds_site_bwd_fin<1>(f, part, red, pd, pc, coef, dwpart, dweights, gamma, pgb, dgamma, dbeta, st);
+  else if (f.GS == 2) lds_site_bwd_fin<2>(f, part, red, pd, pc, coef, dwpart, dweights, gamma, pgb, dgamma, dbeta, st);
+  else lds_site_bwd_fin<4>(f, part, red, pd, pc, coef, dwpart, dweights, gamma, pgb, dgamma, dbeta, st);
+}
+
+void lds_site_bwd_apply(const void* x, const void* dy, void* dx, const LdbnGeom& g, int GS, const float* coef, int epi,
+                        const LdEpi& ep, cudaStream_t st) {
+  lds_site_pass<3>(x, dy, dx, g, GS, nullptr, nullptr, coef, nullptr, epi, ep, st);
 }
 
 }  // namespace dwt

@@ -377,7 +377,7 @@ def tail_pair(x, xd, gamma, beta, gamma_d, beta_d, *, kind, group_size, n_domain
 
 class _ForkForSum(torch.autograd.Function):
     """a, b = fork(y): two aliases of y whose gradients are NOT summed by autograd.  y must be the output of a
-    _NormFunction or _TailPairFunction node (the producer): backward hands the first gradient on as y's gradient and parks the second on the
+    _NormFunction, _TailPairFunction or _LatentSiteFunction node (the producer): backward hands the first gradient on as y's gradient and parks the second on the
     producer's node, whose backward passes it to the kernels as the second addend (dwt_whiten_bwd's dout2).  If y gets
     other gradients as well, autograd adds them to the first one as usual -- the parked addend is independent of that."""
 
@@ -403,7 +403,8 @@ def fork_for_sum(y):
     (a, b), two aliases of y.  Falls back to (y, y) when y was not produced by one of this package's norm sites or no
     gradient is being recorded; results are identical either way."""
     fn = getattr(y, "grad_fn", None)
-    if not torch.is_grad_enabled() or fn is None or not isinstance(fn, (_NormFunction._backward_cls, _TailPairFunction._backward_cls)):
+    if not torch.is_grad_enabled() or fn is None or not isinstance(fn, (_NormFunction._backward_cls, _TailPairFunction._backward_cls,
+                                                                        _LatentSiteFunction._backward_cls)):
         return y, y
     return _ForkForSum.apply(y)
 
@@ -669,7 +670,8 @@ class _LatentFunction(torch.autograd.Function):
         return dx, dw, None, None, None, None, None, None, None, None
 
 
-def latent_domain_whiten(x, weights, *, group_size, training_stats, eps, momentum, update_running, running):
+def latent_domain_whiten(x, weights, *, group_size, training_stats, eps, momentum, update_running, running, weight=None,
+                         bias=None, relu=False, residual=None):
     """Latent-domain whitening of x [N, C, *] under per-image domain weights [N, D] (used as given: no softmax, no value
     checks; cast to float32).  Per group of group_size channels, with each image's own mean and (biased) covariance
     m_n, C_n and s_d = sum_n w_nd:
@@ -695,19 +697,23 @@ def latent_domain_whiten(x, weights, *, group_size, training_stats, eps, momentu
         raise TypeError(f"latent-domain whitening expects floating-point weights (got {weights.dtype})")
     if weights.device != x.device:
         raise ValueError(f"latent-domain whitening expects weights on x's device {x.device} (got {weights.device})")
+    site = _site_args("latent-domain whitening", x, weight, bias, relu, residual)
     nv.require_cuda(x, bf16=True)
     mode = nv.MODE_TRAIN if training_stats else nv.MODE_EVAL
     args = (int(group_size), mode, float(eps), float(momentum), bool(update_running), tuple(running))
     if int(group_size) > 4:
-        return _apply_per_image(_LatentFunction, x, weights.float(), *args)
+        y = _apply_per_image(_LatentFunction, x, weights.float(), *args)
+        if not site:
+            return y
+        # no fused epilogue on the tensor-core kernels: the site as tensor ops (DomainTripleNorm's rule there)
+        shape = (1, -1) + (1,) * (x.dim() - 2)
+        y = y * weight.view(shape) + bias.view(shape)
+        return torch.relu(y + residual if residual is not None else y) if relu else y
+    if site:
+        return _LatentSiteFunction.apply(*_bandwidth_ready(x, residual), weights.float(), weight, bias, nv.KIND_WHITEN,
+                                         *args, bool(relu)).to(x.dtype)
     # latent-domain batch norm's preparation: the same four bandwidth passes take the same layouts
-    fmt = torch.channels_last if _channels_last(x) and x.shape[1] % 4 == 0 else torch.contiguous_format
-    xk = x
-    if x.dtype == torch.bfloat16 and fmt == torch.contiguous_format and math.prod(x.shape[2:]) % 4:
-        xk = x.float()
-    xk = xk.contiguous(memory_format=fmt)
-    if xk.data_ptr() % (8 if xk.dtype == torch.bfloat16 else 16):
-        xk = xk.clone(memory_format=fmt)
+    xk, fmt = _bandwidth_ready(x)[:2]
     return _LatentFunction.apply(xk, weights.float(), *args, True, fmt).to(x.dtype)
 
 
@@ -774,7 +780,8 @@ class _LatentBatchNormFunction(torch.autograd.Function):
         return dx, dw, dgamma, dbeta, None, None, None, None, None, None
 
 
-def latent_domain_batch_norm(x, weights, weight, bias, *, training_stats, eps, momentum, update_running, running):
+def latent_domain_batch_norm(x, weights, weight, bias, *, training_stats, eps, momentum, update_running, running,
+                             relu=False, residual=None):
     """Latent-domain batch norm of x [N, C, *] under per-image domain weights [N, D] (used as given: no softmax, no value
     checks; cast to float32).  Per channel, with each image's own mean and (biased) variance m_n, v_n and s_d = sum_n w_nd:
         mu_d = sum_n w_nd m_n / s_d,  sigma2_d = sum_n w_nd [v_n + (m_n - mu_d)^2] / s_d  (training_stats=False: the
@@ -784,7 +791,9 @@ def latent_domain_batch_norm(x, weights, weight, bias, *, training_stats, eps, m
     by momentum when training_stats and update_running.  x, weights, weight and bias get their gradients.
     The latent-domain batch-norm kernels (dwt_bn_latent_*; dwt_b200.h) take every shape.  A channels-last x whose C is not
     a multiple of 4 runs as an NCHW copy; a bfloat16 NCHW x whose H*W is not a multiple of 4 runs the float32 kernels on
-    an upcast copy, the result in bfloat16."""
+    an upcast copy, the result in bfloat16.
+    relu, residual (x's shape; needs relu and weight / bias): the norm site relu(y [+ residual]) in the same kernels
+    (dwt_latent_site_*: ReLU and residual in registers, the ReLU mask recomputed or saved as one byte per 4 values)."""
     if x.dim() < 2:
         raise ValueError(f"latent-domain batch norm expects [N, C, *] input (got {x.dim()}D input)")
     if weights.dim() != 2 or weights.shape[0] != x.shape[0]:
@@ -796,18 +805,148 @@ def latent_domain_batch_norm(x, weights, weight, bias, *, training_stats, eps, m
         raise ValueError(f"latent-domain batch norm expects weights on x's device {x.device} (got {weights.device})")
     if (weight is None) != (bias is None):
         raise ValueError("latent-domain batch norm takes weight and bias together, or neither")
+    site = _site_args("latent-domain batch norm", x, weight, bias, relu, residual, needs_affine=False)
     nv.require_cuda(x, bf16=True)
     mode = nv.MODE_TRAIN if training_stats else nv.MODE_EVAL
     args = (mode, float(eps), float(momentum), bool(update_running), tuple(running))
+    if site:
+        return _LatentSiteFunction.apply(*_bandwidth_ready(x, residual), weights.float(), weight, bias, nv.KIND_BN, 1,
+                                         *args, bool(relu)).to(x.dtype)
+    xk, fmt = _bandwidth_ready(x)[:2]
+    y = _LatentBatchNormFunction.apply(xk, weights.float(), weight, bias, fmt, *args)
+    return y.to(x.dtype)
+
+
+def _bandwidth_ready(x, residual=None):
+    """-> (x, memory format, residual) as the latent-domain bandwidth passes take them: channels-last when x is and C % 4
+    == 0, else NCHW-contiguous; a bfloat16 NCHW x whose H*W is not a multiple of 4 upcast to float32; data_ptr() 16-byte
+    (bf16: 8-byte) aligned.  The residual gets x's dtype and layout."""
     fmt = torch.channels_last if _channels_last(x) and x.shape[1] % 4 == 0 else torch.contiguous_format
     xk = x
     if x.dtype == torch.bfloat16 and fmt == torch.contiguous_format and math.prod(x.shape[2:]) % 4:
         xk = x.float()
-    xk = xk.contiguous(memory_format=fmt)
-    if xk.data_ptr() % (8 if xk.dtype == torch.bfloat16 else 16):
-        xk = xk.clone(memory_format=fmt)
-    y = _LatentBatchNormFunction.apply(xk, weights.float(), weight, bias, fmt, *args)
-    return y.to(x.dtype)
+    align = 8 if xk.dtype == torch.bfloat16 else 16
+    out = []
+    for t in (xk, residual):
+        if t is not None:
+            t = t.to(xk.dtype).contiguous(memory_format=fmt)
+            if t.data_ptr() % align:
+                t = t.clone(memory_format=fmt)
+        out.append(t)
+    return out[0], fmt, out[1]
+
+
+def _site_args(what, x, weight, bias, relu, residual, needs_affine=True):
+    """Check a latent-domain layer's site arguments; True when the call has a site epilogue (weight / bias, relu or
+    residual; needs_affine=False: relu or residual, batch norm's affine being its own)."""
+    if (weight is None) != (bias is None):
+        raise ValueError(f"{what} takes weight and bias together, or neither")
+    if (relu or residual is not None) and weight is None:
+        raise ValueError(f"{what}: a fused ReLU or residual needs weight and bias")
+    if residual is not None:
+        if not relu:
+            raise ValueError(f"{what}: a fused residual needs relu=True (the site is relu(weight * y + bias + residual))")
+        if residual.shape != x.shape or residual.device != x.device:
+            raise ValueError(f"{what}: the residual must be shaped like x and on its device (got {list(residual.shape)})")
+    return bool(relu) or residual is not None or (needs_affine and weight is not None)
+
+
+class _LatentSiteFunction(torch.autograd.Function):
+    """A latent-domain site (dwt_latent_site_fwd / _bwd): out = relu(gamma * zhat + beta [+ residual]) with zhat the
+    latent-domain batch norm (kind nv.KIND_BN) or small-group whitening (nv.KIND_WHITEN, group sizes 1, 2, 4) of x under
+    weights.  x and the residual as _bandwidth_ready leaves them.  Gradients of x, weights, gamma, beta and the residual.
+    A channels-last residual saves the kernels' ReLU byte map; an NCHW one saves the output and forms dz = dout * (out >
+    0) with one ATen pass (_NormFunction's rule)."""
+
+    @staticmethod
+    def forward(ctx, x, fmt, residual, weights, gamma, beta, kind, group_size, mode, eps, momentum, update_running,
+                running, relu):
+        dev = nv.require_cuda(x, residual, bf16=True)
+        rm_t, rv_t = running
+        nv.require_cuda(weights, gamma, beta, rm_t, rv_t)
+        lib = nv.lib()
+        gs = group_size
+        n, c, hw = x.shape[0], x.shape[1], math.prod(x.shape[2:])
+        k = weights.shape[1]
+        w_c = _aligned(weights)
+        need_running = (mode == nv.MODE_EVAL) or update_running
+        if need_running:
+            _check_param("running mean", rm_t, k * c)
+            _check_param("running second moment", rv_t, k * c * gs)
+        _check_param("gamma / weight", gamma, c)
+        _check_param("beta / bias", beta, c)
+        gamma_c, beta_c = gamma.detach().reshape(-1).contiguous(), beta.detach().reshape(-1).contiguous()
+        nhwc = fmt == torch.channels_last
+        epi = nv.EPI_AFFINE | (nv.EPI_RELU if relu else 0) | (nv.EPI_RESIDUAL if residual is not None else 0)
+        flags = mode | (nv.LAYOUT_NHWC if nhwc else 0) | (nv.DTYPE_BF16 if x.dtype == torch.bfloat16 else 0)
+        y = torch.empty_like(x)
+        mask = torch.empty(x.numel() // 4, dtype=torch.uint8, device=dev) if (residual is not None and nhwc) else None
+        if kind == nv.KIND_BN:
+            save_mean = save_w = None
+            save = torch.empty((4 * n + 3 * k) * c, dtype=torch.float32, device=dev)
+            ws_bytes = lib.dwt_bn_latent_workspace_bytes(n, c, hw, k)
+        else:
+            g = c // gs
+            save_mean = torch.empty(n, c, dtype=torch.float32, device=dev)
+            save_w = torch.empty(n, g, gs, gs, dtype=torch.float32, device=dev)
+            save = torch.empty((n + k) * g * (gs * gs + gs) + k * g * gs * gs + k, dtype=torch.float32, device=dev)
+            ws_bytes = lib.dwt_latent_small_workspace_bytes(n, c, hw, gs, k)
+        ws = nv.grow_workspace(dev, ws_bytes)
+        rm, rv = (nv.ptr(rm_t), nv.ptr(rv_t)) if need_running else (None, None)
+        with torch.cuda.device(dev):
+            rc = lib.dwt_latent_site_fwd(kind, nv.ptr(x), nv.ptr(y), n, c, hw, gs, k, flags, eps, momentum,
+                                         int(update_running), rm, rv, nv.ptr(w_c), nv.ptr(gamma_c), nv.ptr(beta_c),
+                                         nv.ptr(residual), nv.ptr(mask), epi, nv.ptr(save_mean), nv.ptr(save_w),
+                                         nv.ptr(save), nv.ptr(ws), ws.numel(), nv.stream_ptr(dev))
+        nv.check(rc)
+        nv.poll_status(dev)
+        if update_running and mode == nv.MODE_TRAIN:
+            _bump_versions([running])
+        ctx.residual_mode = None
+        extra = None
+        if mask is not None:
+            ctx.residual_mode, extra = "mask", mask
+        elif residual is not None:
+            ctx.residual_mode, extra, epi = "aten", y, nv.EPI_AFFINE
+        ctx.save_for_backward(x, w_c, gamma_c, beta_c, save_mean, save_w, save, extra)
+        ctx.cfg = (kind, gs, flags, eps, epi, n, c, hw, k, fmt, gamma.shape, beta.shape)
+        return y
+
+    @staticmethod
+    def backward(ctx, dout):
+        lib = nv.lib()
+        x, w_c, gamma_c, beta_c, save_mean, save_w, save, extra = ctx.saved_tensors
+        kind, gs, flags, eps, epi, n, c, hw, k, fmt, gshape, bshape = ctx.cfg
+        if ctx.residual_mode == "aten":
+            dout2 = ctx.__dict__.pop("_dwt_extra_grad", None)
+            if dout2 is not None:
+                dout = dout + dout2
+            dout = torch.ops.aten.threshold_backward(dout, extra, 0)
+        dout, _ = _prepare_dout(ctx, dout, x, fmt, 8 if x.dtype == torch.bfloat16 else 16)
+        dev = nv.require_cuda(dout, bf16=True)
+        dx = torch.empty_like(x)
+        dw = torch.empty(n, k, dtype=torch.float32, device=dev) if ctx.needs_input_grad[3] else None
+        want_affine = ctx.needs_input_grad[4] or ctx.needs_input_grad[5]
+        dgamma = torch.empty(c, dtype=torch.float32, device=dev) if want_affine else None
+        dbeta = torch.empty(c, dtype=torch.float32, device=dev) if want_affine else None
+        mask = d_res = None
+        if ctx.residual_mode == "mask":
+            mask, d_res = extra, torch.empty_like(x)     # dz, written even when the residual needs no gradient
+        elif ctx.residual_mode == "aten":
+            d_res = dout
+        ws_bytes = (lib.dwt_bn_latent_workspace_bytes(n, c, hw, k) if kind == nv.KIND_BN
+                    else lib.dwt_latent_small_workspace_bytes(n, c, hw, gs, k))
+        ws = nv.grow_workspace(dev, ws_bytes)
+        with torch.cuda.device(dev):
+            rc = lib.dwt_latent_site_bwd(kind, nv.ptr(x), nv.ptr(dout), nv.ptr(dx), n, c, hw, gs, k, flags, eps,
+                                         nv.ptr(w_c), nv.ptr(gamma_c), nv.ptr(beta_c), nv.ptr(mask),
+                                         nv.ptr(d_res) if mask is not None else None, epi, nv.ptr(save_mean),
+                                         nv.ptr(save_w), nv.ptr(save), nv.ptr(dw), nv.ptr(dgamma), nv.ptr(dbeta),
+                                         nv.ptr(ws), ws.numel(), nv.stream_ptr(dev))
+        nv.check(rc)
+        if want_affine:
+            dgamma, dbeta = dgamma.view(gshape), dbeta.view(bshape)
+        return (dx, None, d_res if ctx.needs_input_grad[2] else None, dw, dgamma, dbeta) + (None,) * 8
 
 
 class _MecFunction(torch.autograd.Function):

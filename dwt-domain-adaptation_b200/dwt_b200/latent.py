@@ -46,7 +46,9 @@ class LatentDomainWTransform2d(nn.Module):
     def extra_repr(self):
         return f"{self.num_features}, group_size={self.group_size}, num_domains={self.num_domains}, eps={self.eps}"
 
-    def forward(self, x, weights):
+    def forward(self, x, weights, *, gamma=None, beta=None, relu=False, residual=None):
+        """gamma / beta ([C] each, together), relu, residual: the site relu(gamma * self(x) + beta [+ residual]); at group
+        sizes up to 4 in the same kernels (functional.latent_domain_whiten)."""
         rank = x.dim()
         if rank != 4:
             raise ValueError(_MSG_RANK.format(rank))
@@ -60,4 +62,5 @@ class LatentDomainWTransform2d(nn.Module):
         # WTransform2d's modes: train updates the buffers even under no_grad; eval whitens with them
         return F.latent_domain_whiten(x, weights, group_size=self.group_size, training_stats=self.training or not tracking,
                                       eps=self.eps, momentum=self.momentum, update_running=self.training and tracking,
-                                      running=(self.running_mean, self.running_variance))
+                                      running=(self.running_mean, self.running_variance), weight=gamma, bias=beta,
+                                      relu=relu, residual=residual)

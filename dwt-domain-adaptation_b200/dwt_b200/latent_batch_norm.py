@@ -52,7 +52,10 @@ class _LatentDomainBatchNorm(nn.Module):
         return (f"{self.num_features}, num_domains={self.num_domains}, eps={self.eps}, momentum={self.momentum}, "
                 f"affine={self.affine}, track_running_stats={self.track_running_stats}")
 
-    def forward(self, x, weights):
+    def forward(self, x, weights, *, relu=False, residual=None):
+        """relu / residual: the site relu(self(x) [+ residual]) in the same kernels (needs affine=True)."""
+        if (relu or residual is not None) and self.weight is None:
+            raise ValueError("a fused ReLU or residual needs the layer's affine parameters (affine=True)")
         if x.dim() not in self._ranks:
             raise ValueError("expected {} input (got {}D input)".format(self._rank_text, x.dim()))
         if x.shape[1] != self.num_features:
@@ -70,7 +73,8 @@ class _LatentDomainBatchNorm(nn.Module):
                 tuple(x.shape)))
         return F.latent_domain_batch_norm(x, weights, self.weight, self.bias, training_stats=batch_stats, eps=self.eps,
                                           momentum=factor, update_running=self.training and tracking,
-                                          running=(self.running_mean, self.running_var) if tracking else (None, None))
+                                          running=(self.running_mean, self.running_var) if tracking else (None, None),
+                                          relu=relu, residual=residual)
 
 
 class LatentDomainBatchNorm1d(_LatentDomainBatchNorm):

@@ -21,6 +21,9 @@ package ``dwt_b200`` by default, the CPU oracle port in CPU tests:
     "modules"  reference composition: split/3 -> 3 modules -> cat -> *gamma+beta -> relu
                (resnet50_dwt_mec_officehome.py:220-222,335-337)
     "fused"    one DomainTripleNorm call per site (needs layers.DomainTripleNorm)
+
+``domains="latent"`` builds the same network on latent-domain sites instead (ResNet50Latent): every site one latent
+layer of ``num_domains`` domains under per-image weights plus the site's gamma/beta, ``model(x, weights)``.
 """
 from __future__ import annotations
 
@@ -33,6 +36,7 @@ EXPANSION = 4
 
 
 _REPLICATED = [False]          # set by collect_stats(): one copy of the batch stands for all three branches
+_LATENT_WEIGHTS = [None]       # set inside ResNet50Latent.forward: the [N, K] domain weights every latent site uses
 _BATCHED_COUNTERS = [False]    # set inside ResNet50DWT.forward (fused sites): the model has bumped every BN step counter itself
 
 
@@ -268,15 +272,24 @@ class ResNet50DWT(_SiteOwner):
 
 
 def build_resnet50_dwt(state_dict, layers, site_mode="modules", num_classes=65, channels_last=False, stem_pad=0,
-                       stem_nchw=False, stem_s2d=False, group_size=4):
+                       stem_nchw=False, stem_s2d=False, group_size=4, domains="triple", num_domains=3):
     """state_dict uses the reference checkpoint's key names *without* the 7-char
     ``module.`` prefix (resnet50_dwt_mec_officehome.py:370-376).  channels_last=True converts the
     convolution weights to torch.channels_last so that, fed channels-last images, every activation
     stays NHWC (no cuDNN NCHW<->NHWC copies); results are identical, only strides change.
     group_size is the reference ResNet's option (resnet50_dwt_mec_officehome.py:266): the stem site's whitening group
-    size (the layers keep 4, as the reference's _make_layer does)."""
-    model = ResNet50DWT(layers, state_dict, num_classes=num_classes, group_size=group_size, site_mode=site_mode,
-                        stem_pad=stem_pad, stem_nchw=stem_nchw and channels_last, stem_s2d=stem_s2d)
+    size (the layers keep 4, as the reference's _make_layer does).
+    domains="latent": ResNet50Latent with num_domains latent domains (the stem and stem-stage options do not apply)."""
+    if domains == "latent":
+        model = ResNet50Latent(layers, state_dict, num_domains, num_classes=num_classes, group_size=group_size,
+                               site_mode=site_mode)
+    elif domains == "triple":
+        model = ResNet50DWT(layers, state_dict, num_classes=num_classes, group_size=group_size, site_mode=site_mode,
+                            stem_pad=stem_pad, stem_nchw=stem_nchw and channels_last, stem_s2d=stem_s2d)
+    else:
+        raise ValueError("domains must be 'triple' or 'latent'")
+    if domains == "latent":      # the sites took their buffers and gamma / beta at construction: convolutions and fc here
+        state_dict = {k: v for k, v in state_dict.items() if "conv" in k or "downsample.0" in k or k.startswith("fc_out")}
     model.load_state_dict(state_dict, strict=False)
     if channels_last and hasattr(layers, "MaxPool2d"):
         model.maxpool = layers.MaxPool2d(3, stride=2, padding=1)    # the library's channels-last kernel pair (no state)
@@ -284,9 +297,126 @@ def build_resnet50_dwt(state_dict, layers, site_mode="modules", num_classes=65, 
         # only the convolution weights: Module.to(memory_format=...) would also re-stride the [1,C,1,1]
         # running-mean buffers into fresh tensors and silently break the aliasing of the three domain branches
         for m in model.modules():
-            if isinstance(m, nn.Conv2d) and not (model.stem_nchw and m is model.conv1):
+            if isinstance(m, nn.Conv2d) and not (getattr(model, "stem_nchw", False) and m is model.conv1):
                 m.weight.data = m.weight.data.contiguous(memory_format=torch.channels_last)
     return model
+
+
+# --------------------------------------------------------------------------------------------------------------------
+# Latent-domain sites (domains="latent")
+# --------------------------------------------------------------------------------------------------------------------
+class LatentSite(nn.Module):
+    """One norm site on latent domains: ``norm`` is layers.LatentDomainWTransform2d (whitening sites; ``gamma`` /
+    ``beta`` [C] are the site's) or layers.LatentDomainBatchNorm2d (its own weight / bias are the site's gamma / beta).
+    Each of the num_domains running-buffer pairs starts from the checkpoint's site buffers."""
+
+    def __init__(self, layers, key, planes, whiten, group_size, num_domains, stats, site_mode):
+        super().__init__()
+        self.whiten, self.site_mode = whiten, site_mode
+        k = num_domains
+        if whiten:
+            self.norm = layers.LatentDomainWTransform2d(planes, group_size, k)
+            rm, rv = stats[key + ".wh.running_mean"], stats[key + ".wh.running_variance"]
+            self.norm.running_mean.copy_(rm.reshape(1, planes).expand(k, planes))
+            self.norm.running_variance.copy_(rv.reshape((1,) + tuple(self.norm.running_variance.shape[1:]))
+                                             .expand_as(self.norm.running_variance))
+            self.gamma = nn.Parameter(stats[key + ".gamma"].reshape(planes).clone())
+            self.beta = nn.Parameter(stats[key + ".beta"].reshape(planes).clone())
+        else:
+            self.norm = layers.LatentDomainBatchNorm2d(planes, k)
+            self.norm.running_mean.copy_(stats[key + ".running_mean"].reshape(1, planes).expand(k, planes))
+            self.norm.running_var.copy_(stats[key + ".running_var"].reshape(1, planes).expand(k, planes))
+            with torch.no_grad():
+                self.norm.weight.copy_(stats[key + ".weight"].reshape(planes))
+                self.norm.bias.copy_(stats[key + ".bias"].reshape(planes))
+
+    def forward(self, x, relu, residual=None):
+        w = _LATENT_WEIGHTS[0]
+        if self.site_mode == "fused":       # gamma / beta, ReLU and the residual inside the latent kernels
+            if self.whiten:
+                return self.norm(x, w, gamma=self.gamma, beta=self.beta, relu=relu, residual=residual)
+            return self.norm(x, w, relu=relu, residual=residual)
+        # "modules": the layer, then gamma / beta (whitening; batch norm's are its own), the add and the ReLU as ATen ops
+        out = self.norm(x, w)
+        if self.whiten:
+            out = out * self.gamma.view(1, -1, 1, 1) + self.beta.view(1, -1, 1, 1)
+        if residual is not None:
+            out = out + residual
+        return torch.relu(out) if relu else out
+
+
+class LatentBottleneck(nn.Module):
+    """Bottleneck on latent sites: bn1 / bn2 / bn3 (and downsample_bn) are LatentSites.  A downsampling block runs two
+    calls: the downsample site (affine only), then site 3 with it as the residual."""
+
+    def __init__(self, layers, inplanes, planes, layer, sub_layer, stats, num_domains, stride, downsample, site_mode):
+        super().__init__()
+        whiten = layer == 1
+        key = f"layer{layer}.{sub_layer}"
+        site = lambda k, c: LatentSite(layers, k, c, whiten, 4, num_domains, stats, site_mode)   # noqa: E731
+        self.conv1 = nn.Conv2d(inplanes, planes, 1, bias=False)
+        self.bn1 = site(key + ".bn1", planes)
+        self.conv2 = nn.Conv2d(planes, planes, 3, stride=stride, padding=1, bias=False)
+        self.bn2 = site(key + ".bn2", planes)
+        self.conv3 = nn.Conv2d(planes, planes * EXPANSION, 1, bias=False)
+        self.bn3 = site(key + ".bn3", planes * EXPANSION)
+        self.downsample = downsample
+        if downsample is not None:
+            self.downsample_bn = site(f"layer{layer}.0.downsample_bn", planes * EXPANSION)
+        # fused: the block input's two gradients (conv1 and the identity) are summed before the producing site's
+        # backward call (layers.fork_for_sum) instead of by an autograd add
+        object.__setattr__(self, "_fork", getattr(layers, "fork_for_sum", None) if site_mode == "fused" else None)
+
+    def forward(self, x):
+        xa, xb = self._fork(x) if (self._fork is not None and self.training) else (x, x)
+        out = self.bn1(self.conv1(xa), relu=True)
+        out = self.bn2(self.conv2(out), relu=True)
+        identity = xb if self.downsample is None else self.downsample_bn(self.downsample(xb), relu=False)
+        return self.bn3(self.conv3(out), relu=True, residual=identity)
+
+
+class ResNet50Latent(nn.Module):
+    """ResNet-50-DWT's topology on latent-domain sites: the stem whitens with group_size, layer1 with 4, layers 2-4 use
+    latent-domain batch norm.  Convolution and fc names are ResNet50DWT's, so the same checkpoint loads; forward(x,
+    weights) with weights [N, num_domains] reaching every site.  Eval mode normalises by each site's running buffers,
+    mixed by the given weights."""
+
+    def __init__(self, layers, state_dict, num_domains, num_classes=65, group_size=4, site_mode="modules"):
+        super().__init__()
+        if site_mode not in ("modules", "fused"):
+            raise ValueError("site_mode must be 'modules' or 'fused'")
+        stats = {k: v for k, v in state_dict.items() if "bn" in k or "downsample" in k}
+        self.site_mode, self.num_domains = site_mode, num_domains
+        self.conv1 = nn.Conv2d(3, 64, 7, stride=2, padding=3, bias=False)
+        self.bn1 = LatentSite(layers, "bn1", 64, True, group_size, num_domains, stats, site_mode)
+        self.maxpool = nn.MaxPool2d(3, stride=2, padding=1)
+        inplanes = 64
+        for li, (planes, blocks, stride) in enumerate(_STAGES, start=1):
+            seq = []
+            for b in range(blocks):
+                down = None
+                if b == 0 and (stride != 1 or inplanes != planes * EXPANSION):
+                    down = nn.Sequential(nn.Conv2d(inplanes, planes * EXPANSION, 1, stride=stride, bias=False))
+                seq.append(LatentBottleneck(layers, inplanes, planes, li, b, stats, num_domains,
+                                            stride if b == 0 else 1, down, site_mode))
+                inplanes = planes * EXPANSION
+            setattr(self, f"layer{li}", nn.Sequential(*seq))
+        self.avgpool = nn.AdaptiveAvgPool2d((1, 1))
+        self.fc_out = nn.Linear(512 * EXPANSION, num_classes)
+        for m in self.modules():
+            if isinstance(m, nn.Conv2d):
+                nn.init.kaiming_normal_(m.weight, mode="fan_out", nonlinearity="relu")
+
+    def forward(self, x, weights):
+        if weights.dim() != 2 or tuple(weights.shape) != (x.shape[0], self.num_domains):
+            raise ValueError(f"expected weights of shape [{x.shape[0]}, {self.num_domains}] (got {list(weights.shape)})")
+        _LATENT_WEIGHTS[0] = weights
+        try:
+            x = self.maxpool(self.bn1(self.conv1(x), relu=True))
+            x = self.layer4(self.layer3(self.layer2(self.layer1(x))))
+        finally:
+            _LATENT_WEIGHTS[0] = None
+        return self.fc_out(torch.flatten(self.avgpool(x), 1))
 
 
 def collect_stats(model, batches, passes=1, replicated=True):

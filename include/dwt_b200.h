@@ -524,6 +524,50 @@ DWT_API int dwt_bn_latent_bwd(const float *x, const float *dout, float *dx, int6
                    float *dgamma, float *dbeta, void *workspace, size_t workspace_bytes, dwt_stream_t stream);
 
 /*
+ * Latent-domain sites: a latent-domain layer with the norm site of ResNet-50-DWT fused behind it,
+ *     out = relu(gamma (.) zhat + beta [+ residual]),
+ * zhat being the output of dwt_bn_latent_fwd (kind DWT_KIND_BN, group_size 1) or dwt_whiten_latent_small_fwd (kind
+ * DWT_KIND_WHITEN, group sizes 1, 2, 4) without gamma / beta.  Everything but the epilogue -- the function, edge rules, EMA,
+ * modes, layouts, dtypes, geometry, alignment, workspace (dwt_bn_latent_workspace_bytes / dwt_latent_small_workspace_bytes)
+ * and save layouts -- is that entry point's: batch norm reads and writes save_stats only (save_mean, save_w unused, may be
+ * NULL), whitening save_mean, save_w and save_stats.  running_second is batch norm's running_var or whitening's
+ * running_cov.  With epilogue 0 (and gamma = beta = NULL) both calls are those entry points.
+ *   epilogue    DWT_EPI_* bits as in dwt_whiten_fwd: AFFINE (gamma, beta [C] required, and only with it), RELU (needs
+ *               AFFINE), RESIDUAL (needs AFFINE|RELU; forward: residual of x's shape, layout and dtype)
+ *   relu_mask   channels-last RESIDUAL only (else NULL): one byte per float4 of the output in memory order [N*HW*C/4],
+ *               bit k = !(pre-activation <= 0); written by fwd, read by bwd
+ * The ReLU is torch.relu's and its gradient threshold_backward's: a NaN pre-activation (a bad image or domain of the edge
+ * rules) stays NaN and passes its gradient, so the layer's edge rules hold under every epilogue.
+ *   dresidual   bwd, channels-last RESIDUAL only (else NULL): receives dz = dout * (out > 0), the gradient of the identity
+ *               branch; the backward apply reads it back instead of dout
+ *   dgamma, dbeta  bwd: [C], written (never accumulated), or both NULL; need AFFINE
+ * The forward folds gamma, beta into the apply's coefficients (batch norm: alpha = gamma a_n, shift = gamma b_n + beta;
+ * whitening: diag(gamma) A_n and gamma (-A_n m~_n) + beta) and adds the residual and takes the ReLU in registers.  A ReLU
+ * without a residual is recomputed by both backward passes from x with the forward's coefficients and FMA order, so its
+ * mask is the forward's bit for bit (batch norm's backward therefore takes beta too).  An NCHW residual has no byte map: its
+ * backward is the AFFINE call on dz = dout * (out > 0), which the caller forms (RESIDUAL in an NCHW backward:
+ * DWT_E_INVALID).  Whitening's backward runs on gamma dz, and dgamma_i = sum_n [sum_{j<=i} (A_n)_ij Rz_n,ij + (A_n (m_n -
+ * m~_n))_i gz_n,i], dbeta_i = sum_n gz_n,i from the per-(image, group) sums gz_n = sum dz, Rz_n = sum dz (x - m_n)^T the
+ * backward reduction already takes (no further pass over x).  Reductions keep their fixed order: reruns are bit-identical;
+ * bf16 outputs (residual widened too) are the fp32 call's on the widened inputs, rounded once.
+ * Refusals: kind not DWT_KIND_BN / DWT_KIND_WHITEN, batch norm at group_size != 1, a bad epilogue combination, gamma / beta
+ * / residual / dresidual / relu_mask outside the epilogue that uses them, misaligned gamma, beta (4 bytes), residual or
+ * dresidual (x's rule): DWT_E_INVALID; whitening at group_size 8 and above: DWT_E_UNSUPPORTED; then every refusal of the
+ * layer's own entry points, whose texts (naming the layer) the pair ends with " [latent-domain site]".
+ * Profile families: those of the layer's entry points (ldbn_*, lds_*), the residual and byte map counted in the bytes.
+ */
+DWT_API int dwt_latent_site_fwd(int kind, const float *x, float *y, int64_t N, int64_t C, int64_t HW, int group_size,
+                   int n_domains, int mode, float eps, float momentum, int update_running, float *running_mean,
+                   float *running_second, const float *weights, const float *gamma, const float *beta,
+                   const float *residual, uint8_t *relu_mask, int epilogue, float *save_mean, float *save_w,
+                   float *save_stats, void *workspace, size_t workspace_bytes, dwt_stream_t stream);
+DWT_API int dwt_latent_site_bwd(int kind, const float *x, const float *dout, float *dx, int64_t N, int64_t C, int64_t HW,
+                   int group_size, int n_domains, int mode, float eps, const float *weights, const float *gamma,
+                   const float *beta, const uint8_t *relu_mask, float *dresidual, int epilogue, const float *save_mean,
+                   const float *save_w, const float *save_stats, float *dweights, float *dgamma, float *dbeta,
+                   void *workspace, size_t workspace_bytes, dwt_stream_t stream);
+
+/*
  * Domain batch norm (F.batch_norm semantics): biased batch variance normalises,
  * the UNBIASED one goes into running_var with weight `factor` (momentum, or
  * 1/num_batches_tracked for the cumulative average, batch_norm.py:59-64).
