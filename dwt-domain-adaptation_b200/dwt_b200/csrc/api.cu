@@ -957,6 +957,21 @@ size_t image_workspace_bytes(int64_t N, int64_t C, int64_t HW, int GS, const Mix
   return rc ? 0 : carve_image(nullptr, gm, m).w.bytes;
 }
 
+// The workspace of the latent-domain bandwidth layers: the larger of the two layouts' plans, each bytes(mode) (0 where
+// the layout does not run), leaving the last error text alone
+template <class Bytes>
+size_t larger_layout_workspace_bytes(Bytes bytes) {
+  char saved[sizeof(g_err)];
+  memcpy(saved, g_err, sizeof(g_err));
+  size_t most = 0;
+  for (int mode : {0, DWT_LAYOUT_NHWC}) {
+    const size_t b = bytes(mode);
+    if (b > most) most = b;
+  }
+  memcpy(g_err, saved, sizeof(g_err));
+  return most;
+}
+
 // Profile family of a launch: [MixKind][pass][channels-last * 2 + bf16]
 enum ImagePass { I_STATS, I_FWD_FINALIZE, I_APPLY, I_BWD_REDUCE, I_BWD_FINALIZE, I_BWD_APPLY };
 const char* const kImageName[3][6][4] = {
@@ -1300,6 +1315,8 @@ int ldbn_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, int n_d
   cudaStream_t st = (cudaStream_t)stream;
   dwt::LdbnFin f = make_ldbn_fin(g, mode, eps, weights, gamma, beta, save_stats, workspace);
   f.momentum = momentum; f.update_running = train && update_running; f.rmean = running_mean; f.rvar = running_var;
+  const float* save_a = save_stats + (size_t)2 * N * C;
+  const dwt::LdEpi ep{gamma, beta, save_a, save_a + (size_t)N * C, residual, relu_mask, nullptr};
   const dwt::Geom pg = ldbn_prof_geom(g);
   const int k = 2 * g.nhwc + g.bf16;
   const double E = (g.bf16 ? 2.0 : 4.0) * (double)N * (double)C * (double)HW;
@@ -1316,13 +1333,7 @@ int ldbn_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, int n_d
   {
     const bool res = (epi & DWT_EPI_RESIDUAL) != 0;
     Launch l(kLdbnName[2][k], &pg, (res ? 3.0 : 2.0) * E + (relu_mask ? E / (g.bf16 ? 8.0 : 16.0) : 0.0), st);
-    if (epi & (DWT_EPI_RELU | DWT_EPI_RESIDUAL)) {
-      const float* save_a = save_stats + (size_t)2 * N * C;
-      const dwt::LdEpi ep{gamma, beta, save_a, save_a + (size_t)N * C, residual, relu_mask, nullptr};
-      dwt::ldbn_site_apply(x, y, g, w.c0, w.c1, epi, ep, st);
-    } else {
-      dwt::ldbn_apply(x, y, g, w.c0, w.c1, st);
-    }
+    dwt::ldbn_apply(x, y, g, w.c0, w.c1, epi, ep, st);
   }
   return check_launch("latent-domain batch norm apply kernel");
 }
@@ -1352,8 +1363,7 @@ int ldbn_bwd(const float* x, const float* dout, float* dx, int64_t N, int64_t C,
   {
     const bool mk = (epi & DWT_EPI_RESIDUAL) != 0;
     Launch l(kLdbnName[3][k], &pg, (mk ? 3.0 : 2.0) * E + (mk ? E / (g.bf16 ? 8.0 : 16.0) : 0.0), st);
-    if (epi & DWT_EPI_RELU) dwt::ldbn_site_bwd_reduce(x, dout, g, centre, w.pa, w.pb, epi, ep, st);
-    else dwt::ldbn_bwd_reduce(x, dout, g, centre, w.pa, w.pb, st);
+    dwt::ldbn_bwd_reduce(x, dout, g, centre, w.pa, w.pb, epi, ep, st);
   }
   if (int rc = check_launch("latent-domain batch norm backward reduction kernel")) return rc;
   {
@@ -1365,7 +1375,7 @@ int ldbn_bwd(const float* x, const float* dout, float* dx, int64_t N, int64_t C,
     Launch l(kLdbnName[5][k], &pg, 3.0 * E, st);
     // a residual's apply reads the masked gradient its reduction wrote
     const void* dz = (epi & DWT_EPI_RESIDUAL) ? static_cast<const void*>(dresidual) : dout;
-    dwt::ldbn_site_bwd_apply(x, dz, dx, g, w.c0, w.c1, w.c2, centre, epi, ep, st);
+    dwt::ldbn_bwd_apply(x, dz, dx, g, w.c0, w.c1, w.c2, centre, epi, ep, st);
   }
   return check_launch("latent-domain batch norm backward apply kernel");
 }
@@ -1389,6 +1399,7 @@ int lds_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, int grou
   const int GS = group_size;
   dwt::LdsFin f = make_lds_fin(g, GS, n_domains, mode, eps, weights, save_mean, save_w, save_stats, workspace);
   f.momentum = momentum; f.update_running = train && update_running; f.rmean = running_mean; f.rcov = running_cov;
+  const dwt::LdEpi ep{gamma, beta, save_mean, save_w, residual, relu_mask, nullptr};
   const dwt::Geom pg = lds_prof_geom(g, GS, n_domains);
   const int k = 2 * g.nhwc + g.bf16;
   const double E = (g.bf16 ? 2.0 : 4.0) * (double)N * (double)C * (double)HW;
@@ -1405,12 +1416,7 @@ int lds_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, int grou
   {
     const bool res = (epi & DWT_EPI_RESIDUAL) != 0;
     Launch l(kLdsName[2][k], &pg, (res ? 3.0 : 2.0) * E + (relu_mask ? E / (g.bf16 ? 8.0 : 16.0) : 0.0), st);
-    if (epi) {
-      const dwt::LdEpi ep{gamma, beta, save_mean, save_w, residual, relu_mask, nullptr};
-      dwt::lds_site_apply(x, y, g, GS, epi, ep, st);
-    } else {
-      dwt::lds_apply(x, y, g, GS, save_mean, save_w, st);
-    }
+    dwt::lds_apply(x, y, g, GS, epi, ep, st);
   }
   return check_launch("latent-domain whitening apply kernel");
 }
@@ -1437,24 +1443,21 @@ int lds_bwd(const float* x, const float* dout, float* dx, int64_t N, int64_t C, 
   {
     const bool mk = (epi & DWT_EPI_RESIDUAL) != 0;
     Launch l(kLdsName[3][k], &pg, (mk ? 3.0 : 2.0) * E + (mk ? E / (g.bf16 ? 8.0 : 16.0) : 0.0), st);
-    if (epi) dwt::lds_site_bwd_reduce(x, dout, g, GS, save_stats, w.part, epi, ep, st);
-    else dwt::lds_bwd_reduce(x, dout, g, GS, save_stats, w.part, st);
+    dwt::lds_bwd_reduce(x, dout, g, GS, save_stats, w.part, epi, ep, st);
   }
   if (int rc = check_launch("latent-domain whitening backward reduction kernel")) return rc;
   {
     Launch l(kLdsName[4][k], &pg, 0.0, st);
     // a site's per-image dgamma / dbeta shares reuse the forward's per-image moments (w.im, free in the backward)
-    if (epi) dwt::lds_site_bwd_finalize(f, w.part, w.red, w.pd, w.pc, w.coef, w.dw, dweights, gamma,
-                                        reinterpret_cast<float*>(w.im), dgamma, dbeta, st);
-    else dwt::lds_bwd_finalize(f, w.part, w.red, w.pd, w.pc, w.coef, w.dw, dweights, st);
+    dwt::lds_bwd_finalize(f, w.part, w.red, w.pd, w.pc, w.coef, w.dw, dweights, gamma, reinterpret_cast<float*>(w.im),
+                          dgamma, dbeta, st);
   }
   if (int rc = check_launch("latent-domain whitening backward finalize kernel")) return rc;
   {
     Launch l(kLdsName[5][k], &pg, 3.0 * E, st);
     // a residual's apply reads the masked gradient its reduction wrote
     const void* dz = (epi & DWT_EPI_RESIDUAL) ? static_cast<const void*>(dresidual) : dout;
-    if (epi) dwt::lds_site_bwd_apply(x, dz, dx, g, GS, w.coef, epi, ep, st);
-    else dwt::lds_bwd_apply(x, dout, dx, g, GS, w.coef, st);
+    dwt::lds_bwd_apply(x, dz, dx, g, GS, w.coef, epi, ep, st);
   }
   return check_launch("latent-domain whitening backward apply kernel");
 }
@@ -1568,18 +1571,10 @@ int dwt_whiten_latent_bwd(const float* x, const float* dout, float* dx, int64_t 
 }
 
 size_t dwt_bn_latent_workspace_bytes(int64_t N, int64_t C, int64_t HW, int n_domains) {
-  char saved[sizeof(g_err)];
-  memcpy(saved, g_err, sizeof(g_err));
-  size_t bytes = 0;
-  dwt::LdbnGeom g;
-  // the larger of the two layouts' plans (channels-last only where it runs)
-  for (int mode : {0, DWT_LAYOUT_NHWC})
-    if (ldbn_geom(g, N, C, HW, n_domains, mode) == DWT_OK) {
-      const size_t b = carve_ldbn(nullptr, g).bytes;
-      if (b > bytes) bytes = b;
-    }
-  memcpy(g_err, saved, sizeof(g_err));
-  return bytes;
+  return larger_layout_workspace_bytes([&](int mode) -> size_t {
+    dwt::LdbnGeom g;
+    return ldbn_geom(g, N, C, HW, n_domains, mode) == DWT_OK ? carve_ldbn(nullptr, g).bytes : 0;
+  });
 }
 
 int dwt_bn_latent_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, int n_domains, int mode, float eps,
@@ -1598,18 +1593,11 @@ int dwt_bn_latent_bwd(const float* x, const float* dout, float* dx, int64_t N, i
 }
 
 size_t dwt_latent_small_workspace_bytes(int64_t N, int64_t C, int64_t HW, int group_size, int n_domains) {
-  char saved[sizeof(g_err)];
-  memcpy(saved, g_err, sizeof(g_err));
-  size_t bytes = 0;
-  dwt::LdbnGeom g;
-  // the larger of the two layouts' plans (channels-last only where it runs)
-  for (int mode : {0, DWT_LAYOUT_NHWC})
-    if (lds_geom(g, N, C, HW, group_size, n_domains, mode) == DWT_OK) {
-      const size_t b = carve_lds(nullptr, g, group_size, n_domains).bytes;
-      if (b > bytes) bytes = b;
-    }
-  memcpy(g_err, saved, sizeof(g_err));
-  return bytes;
+  return larger_layout_workspace_bytes([&](int mode) -> size_t {
+    dwt::LdbnGeom g;
+    return lds_geom(g, N, C, HW, group_size, n_domains, mode) == DWT_OK ? carve_lds(nullptr, g, group_size, n_domains).bytes
+                                                                        : 0;
+  });
 }
 
 int dwt_whiten_latent_small_fwd(const float* x, float* y, int64_t N, int64_t C, int64_t HW, int group_size, int n_domains,

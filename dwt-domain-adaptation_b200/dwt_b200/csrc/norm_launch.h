@@ -205,7 +205,7 @@ struct LdbnFin {
   int* status;
 };
 // The site epilogue of the latent-domain bandwidth passes (dwt_latent_site_*): out = relu(gamma zhat + beta [+ residual])
-// with DWT_EPI_* bits.  A ReLU without a residual is recomputed by the backward passes from x with the forward's
+// with DWT_EPI_* bits; epi 0 is the layer.  A ReLU without a residual is recomputed by the backward passes from x with the forward's
 // coefficients; a channels-last residual leaves the forward's byte map (one byte per float4, the four out > 0 bits), which
 // the backward reduction reads to write the masked gradient dz.  An NCHW residual's backward is the AFFINE one on dz.
 struct LdEpi {
@@ -226,21 +226,16 @@ size_t ldbn_scratch_floats(const LdbnGeom& g, size_t* part, size_t* nc, size_t* 
 void ldbn_stats(const void* x, const LdbnGeom& g, float* pa, float* pb, float* pilot, cudaStream_t st);
 void ldbn_fwd_finalize(const LdbnFin& f, const float* pa, const float* pb, const float* pilot, float* alpha, float* shift,
                        cudaStream_t st);
-void ldbn_apply(const void* x, void* y, const LdbnGeom& g, const float* alpha, const float* shift, cudaStream_t st);
-void ldbn_bwd_reduce(const void* x, const void* dy, const LdbnGeom& g, const float* centre, float* pa, float* pb,
-                     cudaStream_t st);
+// the bandwidth passes below take the epilogue epi (AFFINE is in the coefficients; ep.p0 / p1 = a_n / b_n)
+void ldbn_apply(const void* x, void* y, const LdbnGeom& g, const float* alpha, const float* shift, int epi,
+                const LdEpi& ep, cudaStream_t st);
+void ldbn_bwd_reduce(const void* x, const void* dy, const LdbnGeom& g, const float* centre, float* pa, float* pb, int epi,
+                     const LdEpi& ep, cudaStream_t st);
 // dweights null: no dwpart, no ldbn_dw launch
 void ldbn_bwd_finalize(const LdbnFin& f, const float* pa, const float* pb, float* ca, float* cp, float* cq, float* dwpart,
                        float* dweights, cudaStream_t st);
 void ldbn_bwd_apply(const void* x, const void* dy, void* dx, const LdbnGeom& g, const float* ca, const float* cp,
-                    const float* cq, const float* centre, cudaStream_t st);
-// the bandwidth passes under a site epilogue epi != 0 (AFFINE is in the coefficients; ep.p0 / p1 = a_n / b_n)
-void ldbn_site_apply(const void* x, void* y, const LdbnGeom& g, const float* alpha, const float* shift, int epi,
-                     const LdEpi& ep, cudaStream_t st);
-void ldbn_site_bwd_reduce(const void* x, const void* dy, const LdbnGeom& g, const float* centre, float* pa, float* pb,
-                          int epi, const LdEpi& ep, cudaStream_t st);
-void ldbn_site_bwd_apply(const void* x, const void* dy, void* dx, const LdbnGeom& g, const float* ca, const float* cp,
-                         const float* cq, const float* centre, int epi, const LdEpi& ep, cudaStream_t st);
+                    const float* cq, const float* centre, int epi, const LdEpi& ep, cudaStream_t st);
 
 // latent-domain whitening at group sizes 1, 2, 4 (norm_ldbn.cu; dwt_whiten_latent_small_*) on latent-domain batch
 // norm's segments: NCHW a warp per (image, group, segment) reads the group's gs channel rows, planned by ldbn_plan over
@@ -269,31 +264,24 @@ LdbnGeom lds_plan(int N, int C, int HW, int GS, int K, bool nhwc, bool bf16);
 int lds_partial_floats(int GS);
 // floats per (image, group) of the backward apply's coefficients: A_n (lower) | B_n | c_n | m_n
 int lds_coef_floats(int GS);
+// The bandwidth passes take the epilogue epi (ep.p0 / p1 = save_mean / save_w).  Under AFFINE diag(gamma) folds into
+// A_n's rows and beta into the bias; the backward's reductions take dz, the finalize scales g_n, R_n by gamma and writes
+// dgamma / dbeta (per-image shares in pgb [2][N][C], then added over the images in order), the apply maps gamma dz.
 // forward: statistics -> finalize (per-image moments into save_stats and im [N][G][gs + gs(gs+1)/2] fp64, then per
 // (domain, group) moments, W_k and EMA, then per (image, group) A_n, m~_n) -> apply y = A_n (x - m~_n)
 void lds_stats(const void* x, const LdbnGeom& g, int GS, float* part, float* pilot, cudaStream_t st);
 void lds_fwd_finalize(const LdsFin& f, const float* part, const float* pilot, double* im, cudaStream_t st);
-void lds_apply(const void* x, void* y, const LdbnGeom& g, int GS, const float* save_mean, const float* save_w,
-               cudaStream_t st);
+void lds_apply(const void* x, void* y, const LdbnGeom& g, int GS, int epi, const LdEpi& ep, cudaStream_t st);
 // backward: reduction about the saved image means -> finalize (red [N][G][gs + gs^2], pd [K][G][gs^2 + gs] P_k | mubar_k,
-// pc [K][G] <P_k, Sigma_k>, coef [N][G][lds_coef_floats], dwpart [N][G][kLdsMaxDomains]; dweights null: no dwpart)
-// -> apply dx = A_n^T dy + B_n (x - m_n) + c_n
-void lds_bwd_reduce(const void* x, const void* dy, const LdbnGeom& g, int GS, const float* save_stats, float* part,
-                    cudaStream_t st);
+// pc [K][G] <P_k, Sigma_k>, coef [N][G][lds_coef_floats], dwpart [N][G][kLdsMaxDomains]; dweights null: no dwpart;
+// gamma null: no AFFINE, pgb, dgamma and dbeta unused; dgamma null: no dgamma / dbeta) -> apply dx = A_n^T dy +
+// B_n (x - m_n) + c_n
+void lds_bwd_reduce(const void* x, const void* dy, const LdbnGeom& g, int GS, const float* save_stats, float* part, int epi,
+                    const LdEpi& ep, cudaStream_t st);
 void lds_bwd_finalize(const LdsFin& f, const float* part, float* red, float* pd, float* pc, float* coef, float* dwpart,
-                      float* dweights, cudaStream_t st);
-void lds_bwd_apply(const void* x, const void* dy, void* dx, const LdbnGeom& g, int GS, const float* coef, cudaStream_t st);
-// the passes under a site epilogue epi with AFFINE (ep.p0 / p1 = save_mean / save_w): diag(gamma) folds into A_n's rows
-// and beta into the bias; the backward's reductions take dz, the finalize scales g_n, R_n by gamma and writes dgamma /
-// dbeta (per-image shares in pgb [2][N][C], then added over the images in order), the apply maps gamma dz.
-void lds_site_apply(const void* x, void* y, const LdbnGeom& g, int GS, int epi, const LdEpi& ep, cudaStream_t st);
-void lds_site_bwd_reduce(const void* x, const void* dy, const LdbnGeom& g, int GS, const float* save_stats, float* part,
-                         int epi, const LdEpi& ep, cudaStream_t st);
-void lds_site_bwd_finalize(const LdsFin& f, const float* part, float* red, float* pd, float* pc, float* coef,
-                           float* dwpart, float* dweights, const float* gamma, float* pgb, float* dgamma, float* dbeta,
-                           cudaStream_t st);
-void lds_site_bwd_apply(const void* x, const void* dy, void* dx, const LdbnGeom& g, int GS, const float* coef, int epi,
-                        const LdEpi& ep, cudaStream_t st);
+                      float* dweights, const float* gamma, float* pgb, float* dgamma, float* dbeta, cudaStream_t st);
+void lds_bwd_apply(const void* x, const void* dy, void* dx, const LdbnGeom& g, int GS, const float* coef, int epi,
+                   const LdEpi& ep, cudaStream_t st);
 
 // channels-last max-pool (pool.cu); bf16: x, y, dy, dx are bf16 (compared and summed in fp32, stored rounded)
 void maxpool_fwd_launch(const void* x, void* y, bool bf16, uint8_t* idx, int N, int H, int W, int C, int OH, int OW, int k, int s, int p,

@@ -1631,7 +1631,7 @@ void apply(const void* x, const void* dy, void* out, const LdbnGeom& g, const fl
 }
 
 // a site's epilogue bits -> the kernels' E: forward RELU or RELU|RESIDUAL; backward RELU (recomputed mask) or
-// RELU|RESIDUAL (channels-last byte map, reduction only); AFFINE alone (in the coefficients) runs the plain kernels
+// RELU|RESIDUAL (channels-last byte map, reduction only); AFFINE alone (in the coefficients) or none runs the plain kernels
 #define DWT_LD_SITE(EPI, ...)                                                                                          \
   do {                                                                                                                 \
     const int e_ = (EPI) & (DWT_EPI_RELU | DWT_EPI_RESIDUAL);                                                          \
@@ -1689,15 +1689,20 @@ void ldbn_fwd_finalize(const LdbnFin& f, const float* pa, const float* pb, const
   ldbn_fwd_finalize<<<ldbn_finalize_ctas(f.C), kThreads, 0, st>>>(f, pa, pb, pilot, alpha, shift);
 }
 
-void ldbn_apply(const void* x, void* y, const LdbnGeom& g, const float* alpha, const float* shift, cudaStream_t st) {
-  if (g.bf16) apply<false, __nv_bfloat16>(x, nullptr, y, g, alpha, shift, nullptr, nullptr, st);
-  else apply<false, float>(x, nullptr, y, g, alpha, shift, nullptr, nullptr, st);
+void ldbn_apply(const void* x, void* y, const LdbnGeom& g, const float* alpha, const float* shift, int epi,
+                const LdEpi& ep, cudaStream_t st) {
+  DWT_LD_SITE(epi, {
+    if (g.bf16) apply<false, __nv_bfloat16, E>(x, nullptr, y, g, alpha, shift, nullptr, nullptr, st, ep);
+    else apply<false, float, E>(x, nullptr, y, g, alpha, shift, nullptr, nullptr, st, ep);
+  });
 }
 
-void ldbn_bwd_reduce(const void* x, const void* dy, const LdbnGeom& g, const float* centre, float* pa, float* pb,
-                     cudaStream_t st) {
-  if (g.bf16) reduce<true, __nv_bfloat16>(x, dy, g, centre, pa, pb, nullptr, st);
-  else reduce<true, float>(x, dy, g, centre, pa, pb, nullptr, st);
+void ldbn_bwd_reduce(const void* x, const void* dy, const LdbnGeom& g, const float* centre, float* pa, float* pb, int epi,
+                     const LdEpi& ep, cudaStream_t st) {
+  DWT_LD_SITE(epi, {
+    if (g.bf16) reduce<true, __nv_bfloat16, E>(x, dy, g, centre, pa, pb, nullptr, st, ep);
+    else reduce<true, float, E>(x, dy, g, centre, pa, pb, nullptr, st, ep);
+  });
 }
 
 void ldbn_bwd_finalize(const LdbnFin& f, const float* pa, const float* pb, float* ca, float* cp, float* cq, float* dwpart,
@@ -1710,34 +1715,17 @@ void ldbn_bwd_finalize(const LdbnFin& f, const float* pa, const float* pb, float
   }
 }
 
+// only a ReLU without a residual recomputes its mask here; the residual's backward apply reads dz: the plain kernels
 void ldbn_bwd_apply(const void* x, const void* dy, void* dx, const LdbnGeom& g, const float* ca, const float* cp,
-                    const float* cq, const float* centre, cudaStream_t st) {
-  if (g.bf16) apply<true, __nv_bfloat16>(x, dy, dx, g, ca, cp, cq, centre, st);
-  else apply<true, float>(x, dy, dx, g, ca, cp, cq, centre, st);
-}
-
-void ldbn_site_apply(const void* x, void* y, const LdbnGeom& g, const float* alpha, const float* shift, int epi,
-                     const LdEpi& ep, cudaStream_t st) {
-  DWT_LD_SITE(epi, {
-    if (g.bf16) apply<false, __nv_bfloat16, E>(x, nullptr, y, g, alpha, shift, nullptr, nullptr, st, ep);
-    else apply<false, float, E>(x, nullptr, y, g, alpha, shift, nullptr, nullptr, st, ep);
-  });
-}
-
-void ldbn_site_bwd_reduce(const void* x, const void* dy, const LdbnGeom& g, const float* centre, float* pa, float* pb,
-                          int epi, const LdEpi& ep, cudaStream_t st) {
-  DWT_LD_SITE(epi, {
-    if (g.bf16) reduce<true, __nv_bfloat16, E>(x, dy, g, centre, pa, pb, nullptr, st, ep);
-    else reduce<true, float, E>(x, dy, g, centre, pa, pb, nullptr, st, ep);
-  });
-}
-
-// the residual's backward apply reads dz: the plain kernels
-void ldbn_site_bwd_apply(const void* x, const void* dy, void* dx, const LdbnGeom& g, const float* ca, const float* cp,
-                         const float* cq, const float* centre, int epi, const LdEpi& ep, cudaStream_t st) {
-  if ((epi & (DWT_EPI_RELU | DWT_EPI_RESIDUAL)) != DWT_EPI_RELU) return ldbn_bwd_apply(x, dy, dx, g, ca, cp, cq, centre, st);
-  if (g.bf16) apply<true, __nv_bfloat16, DWT_EPI_RELU>(x, dy, dx, g, ca, cp, cq, centre, st, ep);
-  else apply<true, float, DWT_EPI_RELU>(x, dy, dx, g, ca, cp, cq, centre, st, ep);
+                    const float* cq, const float* centre, int epi, const LdEpi& ep, cudaStream_t st) {
+  if ((epi & (DWT_EPI_RELU | DWT_EPI_RESIDUAL)) == DWT_EPI_RELU) {
+    if (g.bf16) apply<true, __nv_bfloat16, DWT_EPI_RELU>(x, dy, dx, g, ca, cp, cq, centre, st, ep);
+    else apply<true, float, DWT_EPI_RELU>(x, dy, dx, g, ca, cp, cq, centre, st, ep);
+  } else if (g.bf16) {
+    apply<true, __nv_bfloat16>(x, dy, dx, g, ca, cp, cq, centre, st);
+  } else {
+    apply<true, float>(x, dy, dx, g, ca, cp, cq, centre, st);
+  }
 }
 
 namespace {
@@ -1750,7 +1738,7 @@ unsigned lds_blocks(const LdbnGeom& g, int GS) {
 }
 
 // PASS 0: forward statistics, 1: forward apply, 2: backward reduction, 3: backward apply.  NCHW bf16 runs at HW % 4 == 0.
-// E: a site's epilogue (lds_site_*).
+// E: the kernels' epilogue (lds_site_pass).
 template <int GS, int PASS, class T, int E = 0>
 void lds_launch(const void* x, const void* dy, void* out, const LdbnGeom& g, const float* p0, const float* p1,
                 const float* p2, float* part, float* pilot, cudaStream_t st, const LdEpi& ep = LdEpi{}) {
@@ -1786,8 +1774,8 @@ void lds_pass(const void* x, const void* dy, void* out, const LdbnGeom& g, int G
 #undef DWT_LDS_GS
 }
 
-// a site pass: the epilogue bits as that pass's kernels take them -- the backward reduction without a ReLU and the
-// backward apply of a residual (which reads dz) need only gamma, the reduction none of it
+// a pass under the epilogue bits epi (0: the layer) as that pass's kernels take them -- the backward reduction without
+// a ReLU and the backward apply of a residual (which reads dz) need only gamma, the reduction none of it
 template <int PASS>
 void lds_site_pass(const void* x, const void* dy, void* out, const LdbnGeom& g, int GS, const float* p0, const float* p1,
                    const float* p2, float* part, int epi, const LdEpi& ep, cudaStream_t st) {
@@ -1809,20 +1797,12 @@ void lds_fwd_fin(const LdsFin& f, const float* part, const float* pilot, double*
   lds_fwd_mix<GS><<<lds_grid(f.N * f.G), kThreads, 0, st>>>(f);
 }
 
+// gamma (a site's AFFINE) folds into the per-image sums; dgamma / dbeta when asked
 template <int GS>
 void lds_bwd_fin(const LdsFin& f, const float* part, float* red, float* pd, float* pc, float* coef, float* dwpart,
-                 float* dweights, cudaStream_t st) {
-  lds_bwd_image<GS><<<lds_grid(f.N * f.G), kThreads, 0, st>>>(f, part, red, nullptr, nullptr);
-  if (f.train) lds_bwd_domain<GS><<<lds_grid(32 * f.K * f.G), kThreads, 0, st>>>(f, red, pd, pc);
-  lds_bwd_coef<GS><<<lds_grid(f.N * f.G), kThreads, 0, st>>>(f, red, pd, pc, coef, dweights ? dwpart : nullptr);
-  if (dweights) lds_dw<<<lds_grid(f.N * f.K), kThreads, 0, st>>>(dwpart, f.N, f.G, f.K, dweights);
-}
-
-// a site's backward finalize: lds_bwd_fin with gamma folded into the per-image sums, then dgamma / dbeta
-template <int GS>
-void lds_site_bwd_fin(const LdsFin& f, const float* part, float* red, float* pd, float* pc, float* coef, float* dwpart,
-                      float* dweights, const float* gamma, float* pgb, float* dgamma, float* dbeta, cudaStream_t st) {
-  lds_bwd_image<GS, true><<<lds_grid(f.N * f.G), kThreads, 0, st>>>(f, part, red, gamma, pgb);
+                 float* dweights, const float* gamma, float* pgb, float* dgamma, float* dbeta, cudaStream_t st) {
+  if (gamma) lds_bwd_image<GS, true><<<lds_grid(f.N * f.G), kThreads, 0, st>>>(f, part, red, gamma, pgb);
+  else lds_bwd_image<GS><<<lds_grid(f.N * f.G), kThreads, 0, st>>>(f, part, red, nullptr, nullptr);
   if (f.train) lds_bwd_domain<GS><<<lds_grid(32 * f.K * f.G), kThreads, 0, st>>>(f, red, pd, pc);
   lds_bwd_coef<GS><<<lds_grid(f.N * f.G), kThreads, 0, st>>>(f, red, pd, pc, coef, dweights ? dwpart : nullptr);
   if (dweights) lds_dw<<<lds_grid(f.N * f.K), kThreads, 0, st>>>(dwpart, f.N, f.G, f.K, dweights);
@@ -1851,46 +1831,24 @@ void lds_fwd_finalize(const LdsFin& f, const float* part, const float* pilot, do
   else lds_fwd_fin<4>(f, part, pilot, im, st);
 }
 
-void lds_apply(const void* x, void* y, const LdbnGeom& g, int GS, const float* save_mean, const float* save_w,
-               cudaStream_t st) {
-  lds_pass<1>(x, nullptr, y, g, GS, save_mean, save_w, nullptr, nullptr, nullptr, st);
-}
-
-void lds_bwd_reduce(const void* x, const void* dy, const LdbnGeom& g, int GS, const float* save_stats, float* part,
-                    cudaStream_t st) {
-  lds_pass<2>(x, dy, nullptr, g, GS, save_stats, nullptr, nullptr, part, nullptr, st);
-}
-
-void lds_bwd_finalize(const LdsFin& f, const float* part, float* red, float* pd, float* pc, float* coef, float* dwpart,
-                      float* dweights, cudaStream_t st) {
-  if (f.GS == 1) lds_bwd_fin<1>(f, part, red, pd, pc, coef, dwpart, dweights, st);
-  else if (f.GS == 2) lds_bwd_fin<2>(f, part, red, pd, pc, coef, dwpart, dweights, st);
-  else lds_bwd_fin<4>(f, part, red, pd, pc, coef, dwpart, dweights, st);
-}
-
-void lds_bwd_apply(const void* x, const void* dy, void* dx, const LdbnGeom& g, int GS, const float* coef, cudaStream_t st) {
-  lds_pass<3>(x, dy, dx, g, GS, nullptr, nullptr, coef, nullptr, nullptr, st);
-}
-
-void lds_site_apply(const void* x, void* y, const LdbnGeom& g, int GS, int epi, const LdEpi& ep, cudaStream_t st) {
+void lds_apply(const void* x, void* y, const LdbnGeom& g, int GS, int epi, const LdEpi& ep, cudaStream_t st) {
   lds_site_pass<1>(x, nullptr, y, g, GS, ep.p0, ep.p1, nullptr, nullptr, epi, ep, st);
 }
 
-void lds_site_bwd_reduce(const void* x, const void* dy, const LdbnGeom& g, int GS, const float* save_stats, float* part,
-                         int epi, const LdEpi& ep, cudaStream_t st) {
+void lds_bwd_reduce(const void* x, const void* dy, const LdbnGeom& g, int GS, const float* save_stats, float* part, int epi,
+                    const LdEpi& ep, cudaStream_t st) {
   lds_site_pass<2>(x, dy, nullptr, g, GS, save_stats, nullptr, nullptr, part, epi, ep, st);
 }
 
-void lds_site_bwd_finalize(const LdsFin& f, const float* part, float* red, float* pd, float* pc, float* coef,
-                           float* dwpart, float* dweights, const float* gamma, float* pgb, float* dgamma, float* dbeta,
-                           cudaStream_t st) {
-  if (f.GS == 1) lds_site_bwd_fin<1>(f, part, red, pd, pc, coef, dwpart, dweights, gamma, pgb, dgamma, dbeta, st);
-  else if (f.GS == 2) lds_site_bwd_fin<2>(f, part, red, pd, pc, coef, dwpart, dweights, gamma, pgb, dgamma, dbeta, st);
-  else lds_site_bwd_fin<4>(f, part, red, pd, pc, coef, dwpart, dweights, gamma, pgb, dgamma, dbeta, st);
+void lds_bwd_finalize(const LdsFin& f, const float* part, float* red, float* pd, float* pc, float* coef, float* dwpart,
+                      float* dweights, const float* gamma, float* pgb, float* dgamma, float* dbeta, cudaStream_t st) {
+  if (f.GS == 1) lds_bwd_fin<1>(f, part, red, pd, pc, coef, dwpart, dweights, gamma, pgb, dgamma, dbeta, st);
+  else if (f.GS == 2) lds_bwd_fin<2>(f, part, red, pd, pc, coef, dwpart, dweights, gamma, pgb, dgamma, dbeta, st);
+  else lds_bwd_fin<4>(f, part, red, pd, pc, coef, dwpart, dweights, gamma, pgb, dgamma, dbeta, st);
 }
 
-void lds_site_bwd_apply(const void* x, const void* dy, void* dx, const LdbnGeom& g, int GS, const float* coef, int epi,
-                        const LdEpi& ep, cudaStream_t st) {
+void lds_bwd_apply(const void* x, const void* dy, void* dx, const LdbnGeom& g, int GS, const float* coef, int epi,
+                   const LdEpi& ep, cudaStream_t st) {
   lds_site_pass<3>(x, dy, dx, g, GS, nullptr, nullptr, coef, nullptr, epi, ep, st);
 }
 

@@ -377,7 +377,7 @@ def tail_pair(x, xd, gamma, beta, gamma_d, beta_d, *, kind, group_size, n_domain
 
 class _ForkForSum(torch.autograd.Function):
     """a, b = fork(y): two aliases of y whose gradients are NOT summed by autograd.  y must be the output of a
-    _NormFunction, _TailPairFunction or _LatentSiteFunction node (the producer): backward hands the first gradient on as y's gradient and parks the second on the
+    _NormFunction, _TailPairFunction or _LatentBandwidthFunction node (the producer): backward hands the first gradient on as y's gradient and parks the second on the
     producer's node, whose backward passes it to the kernels as the second addend (dwt_whiten_bwd's dout2).  If y gets
     other gradients as well, autograd adds them to the first one as usual -- the parked addend is independent of that."""
 
@@ -404,7 +404,7 @@ def fork_for_sum(y):
     gradient is being recorded; results are identical either way."""
     fn = getattr(y, "grad_fn", None)
     if not torch.is_grad_enabled() or fn is None or not isinstance(fn, (_NormFunction._backward_cls, _TailPairFunction._backward_cls,
-                                                                        _LatentSiteFunction._backward_cls)):
+                                                                        _LatentBandwidthFunction._backward_cls)):
         return y, y
     return _ForkForSum.apply(y)
 
@@ -610,20 +610,16 @@ class _LatentFunction(torch.autograd.Function):
     n_domains latent domains under its row of weights [N, n_domains] (float32, on the device), per group of group_size
     channels, in the Cholesky basis.  The gradient of weights is returned.  Running buffers: (mean [D, C], second moment
     [D, C/gs, gs, gs]), one row per domain.  x is float32 or bfloat16, NCHW-contiguous or (4-D) channels-last; it goes to
-    the kernels in its own layout and dtype.  small: group sizes up to 4 on dwt_whiten_latent_small_* (x prepared by
-    latent_domain_whiten, fmt its layout), else the tensor-core entry points."""
+    the kernels in its own layout and dtype."""
 
     @staticmethod
-    def forward(ctx, x, weights, group_size, mode, eps, momentum, update_running, running, small=False, fmt=None):
+    def forward(ctx, x, weights, group_size, mode, eps, momentum, update_running, running):
         dev = nv.require_cuda(x, bf16=True)
         rm_t, rv_t = running
         nv.require_cuda(weights, rm_t, rv_t)
         lib = nv.lib()
         gs = group_size
-        if not small:
-            x, fmt = _tma_ready(x)
-        ws_bytes, fwd = ((lib.dwt_latent_small_workspace_bytes, lib.dwt_whiten_latent_small_fwd) if small
-                         else (lib.dwt_latent_workspace_bytes, lib.dwt_whiten_latent_fwd))
+        x, fmt = _tma_ready(x)
         n, c, hw = x.shape[0], x.shape[1], math.prod(x.shape[2:])
         k = weights.shape[1]
         w_c = _aligned(weights)
@@ -638,36 +634,36 @@ class _LatentFunction(torch.autograd.Function):
         save_mean = torch.empty(n, c, dtype=torch.float32, device=dev)
         save_w = torch.empty(n, g, gs, gs, dtype=torch.float32, device=dev)
         save_stats = torch.empty((n + k) * g * rec + k * g * gs * gs + k, dtype=torch.float32, device=dev)
-        ws = nv.grow_workspace(dev, ws_bytes(n, c, hw, gs, k))
+        ws = nv.grow_workspace(dev, lib.dwt_latent_workspace_bytes(n, c, hw, gs, k))
         rm, rv = (nv.ptr(rm_t), nv.ptr(rv_t)) if need_running else (None, None)
         with torch.cuda.device(dev):
-            rc = fwd(nv.ptr(x), nv.ptr(y), n, c, hw, gs, k, flags, eps, momentum, int(update_running), rm, rv, nv.ptr(w_c),
-                     nv.ptr(save_mean), nv.ptr(save_w), nv.ptr(save_stats), nv.ptr(ws), ws.numel(), nv.stream_ptr(dev))
+            rc = lib.dwt_whiten_latent_fwd(nv.ptr(x), nv.ptr(y), n, c, hw, gs, k, flags, eps, momentum, int(update_running),
+                                           rm, rv, nv.ptr(w_c), nv.ptr(save_mean), nv.ptr(save_w), nv.ptr(save_stats),
+                                           nv.ptr(ws), ws.numel(), nv.stream_ptr(dev))
         nv.check(rc)
         nv.poll_status(dev)
         if update_running and mode == nv.MODE_TRAIN:
             _bump_versions([running])
         ctx.save_for_backward(x, w_c, save_mean, save_w, save_stats)
-        ctx.cfg = (gs, flags, eps, n, c, hw, k, fmt, small)
+        ctx.cfg = (gs, flags, eps, n, c, hw, k, fmt)
         return y
 
     @staticmethod
     def backward(ctx, dout):
         lib = nv.lib()
         x, w_c, save_mean, save_w, save_stats = ctx.saved_tensors
-        gs, flags, eps, n, c, hw, k, fmt, small = ctx.cfg
-        ws_bytes, bwd = ((lib.dwt_latent_small_workspace_bytes, lib.dwt_whiten_latent_small_bwd) if small
-                         else (lib.dwt_latent_workspace_bytes, lib.dwt_whiten_latent_bwd))
+        gs, flags, eps, n, c, hw, k, fmt = ctx.cfg
         dout, _ = _prepare_dout(ctx, dout, x, fmt, 16)
         dev = nv.require_cuda(dout, bf16=True)
         dx = torch.empty_like(x)
         dw = torch.empty(n, k, dtype=torch.float32, device=dev) if ctx.needs_input_grad[1] else None
-        ws = nv.grow_workspace(dev, ws_bytes(n, c, hw, gs, k))
+        ws = nv.grow_workspace(dev, lib.dwt_latent_workspace_bytes(n, c, hw, gs, k))
         with torch.cuda.device(dev):
-            rc = bwd(nv.ptr(x), nv.ptr(dout), nv.ptr(dx), n, c, hw, gs, k, flags, eps, nv.ptr(w_c), nv.ptr(save_mean),
-                     nv.ptr(save_w), nv.ptr(save_stats), nv.ptr(dw), nv.ptr(ws), ws.numel(), nv.stream_ptr(dev))
+            rc = lib.dwt_whiten_latent_bwd(nv.ptr(x), nv.ptr(dout), nv.ptr(dx), n, c, hw, gs, k, flags, eps, nv.ptr(w_c),
+                                           nv.ptr(save_mean), nv.ptr(save_w), nv.ptr(save_stats), nv.ptr(dw), nv.ptr(ws),
+                                           ws.numel(), nv.stream_ptr(dev))
         nv.check(rc)
-        return dx, dw, None, None, None, None, None, None, None, None
+        return dx, dw, None, None, None, None, None, None
 
 
 def latent_domain_whiten(x, weights, *, group_size, training_stats, eps, momentum, update_running, running, weight=None,
@@ -688,96 +684,24 @@ def latent_domain_whiten(x, weights, *, group_size, training_stats, eps, momentu
     a multiple of 8 (the bf16 kernels' TMA rows) runs them in float32 on an upcast copy, the result in bfloat16.  D <= 8
     either way; a call the kernels cannot take raises NativeError with the library's reason and is never sent to another
     kernel family."""
+    what = "latent-domain whitening"
     if x.dim() < 3:
-        raise ValueError(f"latent-domain whitening expects [N, C, *] input (got {x.dim()}D input)")
-    if weights.dim() != 2 or weights.shape[0] != x.shape[0]:
-        raise ValueError(f"latent-domain whitening expects weights of shape [N, n_domains] with N = {x.shape[0]} "
-                         f"(got {list(weights.shape)})")
-    if not weights.is_floating_point():
-        raise TypeError(f"latent-domain whitening expects floating-point weights (got {weights.dtype})")
-    if weights.device != x.device:
-        raise ValueError(f"latent-domain whitening expects weights on x's device {x.device} (got {weights.device})")
-    site = _site_args("latent-domain whitening", x, weight, bias, relu, residual)
+        raise ValueError(f"{what} expects [N, C, *] input (got {x.dim()}D input)")
+    _check_weights(what, x, weights)
+    _check_site(what, x, weight, bias, relu, residual)
     nv.require_cuda(x, bf16=True)
     mode = nv.MODE_TRAIN if training_stats else nv.MODE_EVAL
     args = (int(group_size), mode, float(eps), float(momentum), bool(update_running), tuple(running))
     if int(group_size) > 4:
         y = _apply_per_image(_LatentFunction, x, weights.float(), *args)
-        if not site:
+        if weight is None:
             return y
         # no fused epilogue on the tensor-core kernels: the site as tensor ops (DomainTripleNorm's rule there)
         shape = (1, -1) + (1,) * (x.dim() - 2)
         y = y * weight.view(shape) + bias.view(shape)
         return torch.relu(y + residual if residual is not None else y) if relu else y
-    if site:
-        return _LatentSiteFunction.apply(*_bandwidth_ready(x, residual), weights.float(), weight, bias, nv.KIND_WHITEN,
-                                         *args, bool(relu)).to(x.dtype)
-    # latent-domain batch norm's preparation: the same four bandwidth passes take the same layouts
-    xk, fmt = _bandwidth_ready(x)[:2]
-    return _LatentFunction.apply(xk, weights.float(), *args, True, fmt).to(x.dtype)
-
-
-class _LatentBatchNormFunction(torch.autograd.Function):
-    """Latent-domain batch norm (dwt_bn_latent_fwd / _bwd) of x [N, C, *] under weights [N, n_domains] (float32, on the
-    device).  x is float32 or bfloat16, NCHW-contiguous or channels-last as latent_domain_batch_norm routes it; gamma /
-    beta are [C]-sized or both None; running = (mean [D, C], var [D, C]).  Gradients of x, weights (when it needs one),
-    gamma and beta."""
-
-    @staticmethod
-    def forward(ctx, x, weights, gamma, beta, fmt, mode, eps, momentum, update_running, running):
-        dev = nv.require_cuda(x, bf16=True)
-        rm_t, rv_t = running
-        nv.require_cuda(weights, gamma, beta, rm_t, rv_t)
-        lib = nv.lib()
-        n, c, hw = x.shape[0], x.shape[1], math.prod(x.shape[2:])
-        k = weights.shape[1]
-        w_c = weights.detach().contiguous()
-        need_running = (mode == nv.MODE_EVAL) or update_running
-        if need_running:
-            _check_param("running mean", rm_t, k * c)
-            _check_param("running var", rv_t, k * c)
-        _check_param("gamma / weight", gamma, c)
-        _check_param("beta / bias", beta, c)
-        gamma_c = None if gamma is None else gamma.detach().reshape(-1).contiguous()
-        beta_c = None if beta is None else beta.detach().reshape(-1).contiguous()
-        flags = mode | (nv.LAYOUT_NHWC if fmt == torch.channels_last else 0) | (nv.DTYPE_BF16 if x.dtype == torch.bfloat16 else 0)
-        y = torch.empty_like(x)
-        save = torch.empty((4 * n + 3 * k) * c, dtype=torch.float32, device=dev)
-        ws = nv.grow_workspace(dev, lib.dwt_bn_latent_workspace_bytes(n, c, hw, k))
-        rm, rv = (nv.ptr(rm_t), nv.ptr(rv_t)) if need_running else (None, None)
-        with torch.cuda.device(dev):
-            rc = lib.dwt_bn_latent_fwd(nv.ptr(x), nv.ptr(y), n, c, hw, k, flags, eps, momentum, int(update_running), rm, rv,
-                                       nv.ptr(w_c), nv.ptr(gamma_c), nv.ptr(beta_c), nv.ptr(save), nv.ptr(ws), ws.numel(),
-                                       nv.stream_ptr(dev))
-        nv.check(rc)
-        nv.poll_status(dev)
-        if update_running and mode == nv.MODE_TRAIN:
-            _bump_versions([running])
-        ctx.save_for_backward(x, w_c, gamma_c, save)
-        ctx.cfg = (flags, eps, n, c, hw, k, fmt, None if gamma is None else (gamma.shape, beta.shape))
-        return y
-
-    @staticmethod
-    def backward(ctx, dout):
-        lib = nv.lib()
-        x, w_c, gamma_c, save = ctx.saved_tensors
-        flags, eps, n, c, hw, k, fmt, shapes = ctx.cfg
-        dout, _ = _prepare_dout(ctx, dout, x, fmt, 8 if x.dtype == torch.bfloat16 else 16)
-        dev = nv.require_cuda(dout, bf16=True)
-        dx = torch.empty_like(x)
-        dw = torch.empty(n, k, dtype=torch.float32, device=dev) if ctx.needs_input_grad[1] else None
-        want_affine = gamma_c is not None and (ctx.needs_input_grad[2] or ctx.needs_input_grad[3])
-        dgamma = torch.empty(c, dtype=torch.float32, device=dev) if want_affine else None
-        dbeta = torch.empty(c, dtype=torch.float32, device=dev) if want_affine else None
-        ws = nv.grow_workspace(dev, lib.dwt_bn_latent_workspace_bytes(n, c, hw, k))
-        with torch.cuda.device(dev):
-            rc = lib.dwt_bn_latent_bwd(nv.ptr(x), nv.ptr(dout), nv.ptr(dx), n, c, hw, k, flags, eps, nv.ptr(w_c),
-                                       nv.ptr(gamma_c), nv.ptr(save), nv.ptr(dw), nv.ptr(dgamma), nv.ptr(dbeta), nv.ptr(ws),
-                                       ws.numel(), nv.stream_ptr(dev))
-        nv.check(rc)
-        if want_affine:
-            dgamma, dbeta = dgamma.view(shapes[0]), dbeta.view(shapes[1])
-        return dx, dw, dgamma, dbeta, None, None, None, None, None, None
+    return _LatentBandwidthFunction.apply(*_bandwidth_ready(x, residual), weights.float(), weight, bias, nv.KIND_WHITEN,
+                                          *args, bool(relu)).to(x.dtype)
 
 
 def latent_domain_batch_norm(x, weights, weight, bias, *, training_stats, eps, momentum, update_running, running,
@@ -794,27 +718,16 @@ def latent_domain_batch_norm(x, weights, weight, bias, *, training_stats, eps, m
     an upcast copy, the result in bfloat16.
     relu, residual (x's shape; needs relu and weight / bias): the norm site relu(y [+ residual]) in the same kernels
     (dwt_latent_site_*: ReLU and residual in registers, the ReLU mask recomputed or saved as one byte per 4 values)."""
+    what = "latent-domain batch norm"
     if x.dim() < 2:
-        raise ValueError(f"latent-domain batch norm expects [N, C, *] input (got {x.dim()}D input)")
-    if weights.dim() != 2 or weights.shape[0] != x.shape[0]:
-        raise ValueError(f"latent-domain batch norm expects weights of shape [N, n_domains] with N = {x.shape[0]} "
-                         f"(got {list(weights.shape)})")
-    if not weights.is_floating_point():
-        raise TypeError(f"latent-domain batch norm expects floating-point weights (got {weights.dtype})")
-    if weights.device != x.device:
-        raise ValueError(f"latent-domain batch norm expects weights on x's device {x.device} (got {weights.device})")
-    if (weight is None) != (bias is None):
-        raise ValueError("latent-domain batch norm takes weight and bias together, or neither")
-    site = _site_args("latent-domain batch norm", x, weight, bias, relu, residual, needs_affine=False)
+        raise ValueError(f"{what} expects [N, C, *] input (got {x.dim()}D input)")
+    _check_weights(what, x, weights)
+    _check_site(what, x, weight, bias, relu, residual)
     nv.require_cuda(x, bf16=True)
     mode = nv.MODE_TRAIN if training_stats else nv.MODE_EVAL
     args = (mode, float(eps), float(momentum), bool(update_running), tuple(running))
-    if site:
-        return _LatentSiteFunction.apply(*_bandwidth_ready(x, residual), weights.float(), weight, bias, nv.KIND_BN, 1,
-                                         *args, bool(relu)).to(x.dtype)
-    xk, fmt = _bandwidth_ready(x)[:2]
-    y = _LatentBatchNormFunction.apply(xk, weights.float(), weight, bias, fmt, *args)
-    return y.to(x.dtype)
+    return _LatentBandwidthFunction.apply(*_bandwidth_ready(x, residual), weights.float(), weight, bias, nv.KIND_BN, 1,
+                                          *args, bool(relu)).to(x.dtype)
 
 
 def _bandwidth_ready(x, residual=None):
@@ -836,9 +749,19 @@ def _bandwidth_ready(x, residual=None):
     return out[0], fmt, out[1]
 
 
-def _site_args(what, x, weight, bias, relu, residual, needs_affine=True):
-    """Check a latent-domain layer's site arguments; True when the call has a site epilogue (weight / bias, relu or
-    residual; needs_affine=False: relu or residual, batch norm's affine being its own)."""
+def _check_weights(what, x, weights):
+    """A latent-domain layer's per-image domain weights: [N, n_domains], floating point, on x's device."""
+    if weights.dim() != 2 or weights.shape[0] != x.shape[0]:
+        raise ValueError(f"{what} expects weights of shape [N, n_domains] with N = {x.shape[0]} "
+                         f"(got {list(weights.shape)})")
+    if not weights.is_floating_point():
+        raise TypeError(f"{what} expects floating-point weights (got {weights.dtype})")
+    if weights.device != x.device:
+        raise ValueError(f"{what} expects weights on x's device {x.device} (got {weights.device})")
+
+
+def _check_site(what, x, weight, bias, relu, residual):
+    """A latent-domain layer's site arguments: weight / bias together, relu and the residual only with them."""
     if (weight is None) != (bias is None):
         raise ValueError(f"{what} takes weight and bias together, or neither")
     if (relu or residual is not None) and weight is None:
@@ -848,13 +771,14 @@ def _site_args(what, x, weight, bias, relu, residual, needs_affine=True):
             raise ValueError(f"{what}: a fused residual needs relu=True (the site is relu(weight * y + bias + residual))")
         if residual.shape != x.shape or residual.device != x.device:
             raise ValueError(f"{what}: the residual must be shaped like x and on its device (got {list(residual.shape)})")
-    return bool(relu) or residual is not None or (needs_affine and weight is not None)
 
 
-class _LatentSiteFunction(torch.autograd.Function):
-    """A latent-domain site (dwt_latent_site_fwd / _bwd): out = relu(gamma * zhat + beta [+ residual]) with zhat the
-    latent-domain batch norm (kind nv.KIND_BN) or small-group whitening (nv.KIND_WHITEN, group sizes 1, 2, 4) of x under
-    weights.  x and the residual as _bandwidth_ready leaves them.  Gradients of x, weights, gamma, beta and the residual.
+class _LatentBandwidthFunction(torch.autograd.Function):
+    """Latent-domain batch norm (kind nv.KIND_BN) or small-group whitening (nv.KIND_WHITEN, group sizes 1, 2, 4) of x
+    under weights on the bandwidth kernels (dwt_latent_site_fwd / _bwd), with the site out = relu(gamma * zhat + beta
+    [+ residual]) in the same kernels.  gamma / beta are [C]-sized or both None (no epilogue: the layer alone); relu and
+    the residual need them.  x and the residual as _bandwidth_ready leaves them.  Running buffers: (mean [D, C], var
+    [D, C] or second moment [D, C/gs, gs, gs]).  Gradients of x, weights, gamma, beta and the residual.
     A channels-last residual saves the kernels' ReLU byte map; an NCHW one saves the output and forms dz = dout * (out >
     0) with one ATen pass (_NormFunction's rule)."""
 
@@ -872,12 +796,14 @@ class _LatentSiteFunction(torch.autograd.Function):
         need_running = (mode == nv.MODE_EVAL) or update_running
         if need_running:
             _check_param("running mean", rm_t, k * c)
-            _check_param("running second moment", rv_t, k * c * gs)
+            _check_param("running var" if kind == nv.KIND_BN else "running second moment", rv_t, k * c * gs)
         _check_param("gamma / weight", gamma, c)
         _check_param("beta / bias", beta, c)
-        gamma_c, beta_c = gamma.detach().reshape(-1).contiguous(), beta.detach().reshape(-1).contiguous()
+        gamma_c, beta_c = ((None, None) if gamma is None
+                           else (gamma.detach().reshape(-1).contiguous(), beta.detach().reshape(-1).contiguous()))
         nhwc = fmt == torch.channels_last
-        epi = nv.EPI_AFFINE | (nv.EPI_RELU if relu else 0) | (nv.EPI_RESIDUAL if residual is not None else 0)
+        epi = ((nv.EPI_AFFINE if gamma is not None else 0) | (nv.EPI_RELU if relu else 0)
+               | (nv.EPI_RESIDUAL if residual is not None else 0))
         flags = mode | (nv.LAYOUT_NHWC if nhwc else 0) | (nv.DTYPE_BF16 if x.dtype == torch.bfloat16 else 0)
         y = torch.empty_like(x)
         mask = torch.empty(x.numel() // 4, dtype=torch.uint8, device=dev) if (residual is not None and nhwc) else None
@@ -909,14 +835,14 @@ class _LatentSiteFunction(torch.autograd.Function):
         elif residual is not None:
             ctx.residual_mode, extra, epi = "aten", y, nv.EPI_AFFINE
         ctx.save_for_backward(x, w_c, gamma_c, beta_c, save_mean, save_w, save, extra)
-        ctx.cfg = (kind, gs, flags, eps, epi, n, c, hw, k, fmt, gamma.shape, beta.shape)
+        ctx.cfg = (kind, gs, flags, eps, epi, n, c, hw, k, fmt, None if gamma is None else (gamma.shape, beta.shape))
         return y
 
     @staticmethod
     def backward(ctx, dout):
         lib = nv.lib()
         x, w_c, gamma_c, beta_c, save_mean, save_w, save, extra = ctx.saved_tensors
-        kind, gs, flags, eps, epi, n, c, hw, k, fmt, gshape, bshape = ctx.cfg
+        kind, gs, flags, eps, epi, n, c, hw, k, fmt, shapes = ctx.cfg
         if ctx.residual_mode == "aten":
             dout2 = ctx.__dict__.pop("_dwt_extra_grad", None)
             if dout2 is not None:
@@ -945,7 +871,7 @@ class _LatentSiteFunction(torch.autograd.Function):
                                          nv.ptr(ws), ws.numel(), nv.stream_ptr(dev))
         nv.check(rc)
         if want_affine:
-            dgamma, dbeta = dgamma.view(gshape), dbeta.view(bshape)
+            dgamma, dbeta = dgamma.view(shapes[0]), dbeta.view(shapes[1])
         return (dx, None, d_res if ctx.needs_input_grad[2] else None, dw, dgamma, dbeta) + (None,) * 8
 
 
