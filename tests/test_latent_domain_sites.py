@@ -331,7 +331,10 @@ def test_model_sites_against_float64(dev, worst, kind, shape, gs, epi, layout):
 @pytest.mark.parametrize("kind, shape, gs, layout", [
     ("bn", (16, 64, 28, 28), 1, "nchw"), ("bn", (16, 64, 28, 28), 1, "cl"), ("bn", (13, 6, 5, 5), 1, "nchw"),
     ("bn", (64, 100), 1, "nchw"), ("whiten", (16, 64, 28, 28), 1, "cl"), ("whiten", (16, 64, 28, 28), 2, "nchw"),
-    ("whiten", (16, 64, 28, 28), 4, "cl"), ("whiten", (13, 8, 5, 5), 4, "nchw"), ("whiten", (13, 6, 5, 5), 2, "nchw")])
+    ("whiten", (16, 64, 28, 28), 4, "cl"), ("whiten", (13, 8, 5, 5), 4, "nchw"), ("whiten", (13, 6, 5, 5), 2, "nchw"),
+    # channels-last widths off the power-of-two slabs: C/4 = 3 and 25 (qc does not divide 256), 65 (a 1-column last slab)
+    ("bn", (8, 12, 14, 14), 1, "cl"), ("bn", (8, 100, 7, 7), 1, "cl"), ("bn", (4, 260, 7, 7), 1, "cl"),
+    ("whiten", (8, 12, 14, 14), 1, "cl"), ("whiten", (8, 100, 7, 7), 2, "cl"), ("whiten", (4, 260, 7, 7), 1, "cl")])
 def test_modes_and_edges_against_float64(dev, worst, kind, shape, gs, layout, epi, d, mode):
     if len(shape) == 2 and epi not in ("none", "relu"):
         pytest.skip("[N, C]: batch norm with ReLU")

@@ -315,8 +315,8 @@ def test_model_sites_against_float64(dev, worst, shape, gs, d, layout):
 @pytest.mark.parametrize("shape, gs", [
     ((1, 64, 56, 56), 4), ((32, 4, 28, 28), 4), ((64, 64, 1, 1), 4), ((64, 64, 1, 1), 1), ((64, 64, 7, 7), 4),
     ((64, 8, 7, 7), 2), ((16, 16, 5, 5), 4),
-    ((2, 8, 257, 1), 4),                                     # NCHW: one pixel past one 256-pixel segment
-    ((2, 4, 1025, 1), 4),                                    # channels-last: one pixel past one 1024-pixel segment
+    ((2, 8, 257, 1), 4),                                     # NCHW: one pixel past 256, two segments of 132 + 125
+    ((2, 4, 1025, 1), 4),                                    # channels-last: one pixel past 1024, segments of 513 + 512
 ])
 def test_edges_against_float64(dev, worst, shape, gs, layout):
     x, dy = images(shape, dev, gs, seed=7), grad(shape, dev)
